@@ -113,9 +113,16 @@ int main(int argc, char** argv) {
         }
         rc = ksh_reconcile(ctx, &pods[i], KS_SCORE_LEFTOVER, &node, body, sizeof(body));
         if (rc < 0) return die("ksh_reconcile", rc);
-        if (rc == KSH_RECONCILE_NO_NODE_FOUND)
+        if (rc == KSH_RECONCILE_NO_NODE_FOUND) {
             printf("%s: ReconcileError::NoNodeFound\n", pods[i].name);
-        else if (node < 0)
+            /* why: the FailedScheduling message `kubectl describe pod` would show */
+            ks_pod_reasons why;
+            char msg[256];
+            int64_t msg_off = -1;
+            rc = ksh_explain_pods(ctx, &pods[i], 1, &why, msg, sizeof(msg), &msg_off);
+            if (rc) return die("ksh_explain_pods", rc);
+            if (msg_off >= 0) printf("%s: %s\n", pods[i].name, msg + msg_off);
+        } else if (node < 0)
             printf("%s: already bound, skipped\n", pods[i].name);
         else
             printf("%s: POST /api/v1/namespaces/%s/pods/%s/binding %s\n", pods[i].name, pods[i].ns, pods[i].name, body);

@@ -140,6 +140,25 @@ impl Gpu {
             e => Err(e),
         }
     }
+
+    /// Why a pod did not schedule: the per-check rejection counts and, when no node is feasible, the FailedScheduling
+    /// message (`0/5 nodes are available: 2 Insufficient cpu, ...`) that `kubectl describe pod` would show.
+    pub fn explain(&self, pod: &corev1::Pod) -> (ks_pod_reasons, Option<String>) {
+        let v = PodView::new(pod);
+        let mut r = ks_pod_reasons::default();
+        let mut buf = vec![0u8; 512];
+        let mut off: i64 = -1;
+        let rc = unsafe { ksh_explain_pods(self.ctx, &v.obj, 1, &mut r, buf.as_mut_ptr() as *mut c_char, buf.len(), &mut off) };
+        if rc != KS_OK {
+            panic!("ksh_explain_pods failed ({}): {}", rc, last_error());
+        }
+        let msg = if off < 0 {
+            None
+        } else {
+            Some(unsafe { CStr::from_ptr(buf.as_ptr().add(off as usize) as *const c_char) }.to_string_lossy().into_owned())
+        };
+        (r, msg)
+    }
 }
 
 impl Drop for Gpu {

@@ -92,6 +92,14 @@ pub struct ks_bindings {
     pub bindings_ready_event: *mut c_void, // optional cudaEvent_t
     pub exchange: *const ks_exchange,      // optional fused all-gather over NVLink
 }
+#[repr(C)]
+#[derive(Clone, Copy, Default, Debug)]
+pub struct ks_pod_reasons {
+    pub insufficient_cpu: u32,
+    pub insufficient_memory: u32,
+    pub not_enough_resources: u32,
+    pub node_selector_mismatch: u32,
+}
 pub enum ks_snapshot {}
 pub enum ks_stream {}
 pub enum ksh_context {}
@@ -113,6 +121,7 @@ extern "C" {
     pub fn ks_select(s: *mut ks_snapshot, pods: *const ks_pods, policy: c_int, flags: u32, out: *mut ks_bindings, stream: *mut c_void) -> c_int;
     pub fn ks_select_sampling(s: *mut ks_snapshot, pods: *const ks_pods, attempts: u32, seed: u64, first_pod_index: u64,
                               node_idx: *mut i32, attempts_used: *mut u32, draw_node: *mut i32, draw_code: *mut u8) -> c_int;
+    pub fn ks_explain(s: *mut ks_snapshot, pods: *const ks_pods, out: *mut ks_pod_reasons, out_space: i32, stream: *mut c_void) -> c_int;
     pub fn ks_snapshot_commit_claims(s: *mut ks_snapshot, n: u64, node: *const i32, cpu: *const i64, mem: *const i64, accepted: *mut u8) -> c_int;
     pub fn ks_stream_bind(s: *mut ks_snapshot, pods: *const ks_pods, policy: c_int, node_idx: *mut i32, score: *mut i64, rounds: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
@@ -149,4 +158,7 @@ extern "C" {
                          binding_json: *mut c_char, cap: usize) -> c_int;
     pub fn ksh_reconcile_batch(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, policy: c_int, status: *mut i32,
                                node_idx: *mut i32, json: *mut c_char, cap: usize, json_off: *mut i64, rounds: *mut u32) -> c_int;
+    pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,
+                            messages: *mut c_char, cap: usize, msg_off: *mut i64) -> c_int;
+    pub fn ksh_format_unschedulable(n_nodes: u32, r: *const ks_pod_reasons, buf: *mut c_char, cap: usize) -> c_int;
 }

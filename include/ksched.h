@@ -227,6 +227,22 @@ void ks_stream_close(ks_stream* q); /* stops the dispatcher; unpolled results ar
 int ks_select_sampling(ks_snapshot* s, const ks_pods* pods, uint32_t attempts, uint64_t seed, uint64_t first_pod_index,
                        int32_t* out_node_idx, uint32_t* out_attempts, int32_t* out_draw_node, uint8_t* out_draw_code);
 
+/* ---- why a pod has no node: per-pod rejection counts (the batched form of the log line at src/main.rs:62) ----
+ * For pod p, over the snapshot's N real nodes only (padding never counts):
+ *   insufficient_cpu       nodes with req_cpu > free_cpu                   (half of can_pod_fit, src/predicates.rs:42)
+ *   insufficient_memory    nodes with req_mem > free_mem                   (the other half)
+ *   not_enough_resources   nodes failing either: cell code KS_CELL_NOT_ENOUGH_RESOURCES (fit is checked first, :68-70)
+ *   node_selector_mismatch nodes the pod fits whose labels miss a selector pair: KS_CELL_NODE_SELECTOR_MISMATCH (:72-74)
+ * so not_enough_resources + node_selector_mismatch + feasible_cnt == N (feasible_cnt as ks_select reports it) and
+ * max(cpu, mem) <= not_enough_resources <= cpu + mem.  Precedence is the reference's (fit first); upstream
+ * kube-scheduler runs NodeAffinity before NodeResourcesFit and would count a node failing both as a selector miss. */
+typedef struct ks_pod_reasons {
+    uint32_t insufficient_cpu, insufficient_memory, not_enough_resources, node_selector_mismatch;
+} ks_pod_reasons;
+/* out[pods->n] in out_space (KS_MEM_HOST / KS_MEM_DEVICE); pods in pods->mem_space.  Returns after completion when
+ * out or the pods are in host memory, after enqueue on cuda_stream (NULL = library stream) when both are on the device. */
+int ks_explain(ks_snapshot* s, const ks_pods* pods, ks_pod_reasons* out, int32_t out_space, void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -122,6 +122,22 @@ int ksh_reconcile(ksh_context* ctx, const ks_pod_obj* pod, int policy, int32_t* 
 int ksh_reconcile_batch(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, int policy, int32_t* out_status,
                         int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off, uint32_t* out_rounds);
 
+/* Why pods do not schedule: ks_explain (ksched.h) over pod objects, packed as ksh_select_nodes packs them (a selector
+ * pair that no node carries counts as a selector mismatch on every node).  out[n_pods] receives the counts.  For each
+ * pod with no feasible node, a FailedScheduling message (ksh_format_unschedulable) is written into messages (cap bytes),
+ * back to back and NUL-terminated like ksh_reconcile_batch's bodies; out_msg_off[i] = its offset, or -1 (the pod has a
+ * feasible node, or the buffer was full).  messages / out_msg_off may be NULL. */
+int ksh_explain_pods(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, ks_pod_reasons* out, char* messages,
+                     size_t cap, int64_t* out_msg_off);
+/* Upstream kube-scheduler's message for a pod no node accepts, e.g.
+ *   "0/5 nodes are available: 2 Insufficient cpu, 3 node(s) didn't match Pod's node affinity/selector."
+ * "0/<n_nodes> nodes are available: " then the non-zero terms of insufficient_cpu ("<a> Insufficient cpu"),
+ * insufficient_memory ("<b> Insufficient memory") and node_selector_mismatch ("<c> node(s) didn't match Pod's node
+ * affinity/selector"), joined by ", ", ended by "."; with no term (n_nodes = 0) "0/<n_nodes> nodes are available.".
+ * Pure CPU.  Like snprintf: writes at most cap bytes including the NUL and returns the full length (>= cap means
+ * truncated); KS_ERR_INVALID when r is NULL, or buf is NULL with cap > 0. */
+int ksh_format_unschedulable(uint32_t n_nodes, const ks_pod_reasons* r, char* buf, size_t cap);
+
 #ifdef __cplusplus
 }
 #endif

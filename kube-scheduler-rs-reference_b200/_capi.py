@@ -49,6 +49,11 @@ class ks_bindings(C.Structure):
                 ("mask_space", C.c_int32), ("bindings_ready_event", C.c_void_p), ("exchange", C.POINTER(ks_exchange))]
 
 
+class ks_pod_reasons(C.Structure):
+    _fields_ = [("insufficient_cpu", C.c_uint32), ("insufficient_memory", C.c_uint32),
+                ("not_enough_resources", C.c_uint32), ("node_selector_mismatch", C.c_uint32)]
+
+
 def _proto(name, restype, *argtypes):
     fn = getattr(lib, name)
     fn.restype = restype
@@ -95,6 +100,8 @@ _proto("ks_measure_write_bandwidth", C.c_int, C.c_int, C.c_void_p, C.c_uint64, C
 _proto("ks_device_read", C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64)
 _proto("ks_select_sampling", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p,
        C.c_void_p, C.c_void_p, C.c_void_p)
+if hasattr(lib, "ks_explain"):  # a library built from the host layer and a device stand-in has no ks_explain
+    _proto("ks_explain", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_int32, C.c_void_p)
 KS_REFERENCE_ATTEMPTS = 5
 _SAMPLING_MULT = 0xD1B54A32D192ED03
 

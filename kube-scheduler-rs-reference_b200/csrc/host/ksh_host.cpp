@@ -18,6 +18,10 @@
 #include "../../../include/ksched_host.h"
 
 extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not part of the public ABI)
+// ks_explain is defined by the CUDA core in the same library.  The reference is weak so that this file still links
+// with device stand-ins that only provide the older ks_* entries (tests/native); ksh_explain_pods then reports
+// KS_ERR_NO_DEVICE.
+#pragma weak ks_explain
 
 namespace {
 
@@ -1294,6 +1298,61 @@ int ksh_reconcile_batch(ksh_context* c, const ks_pod_obj* pods, uint64_t n, int 
                 used += body.size() + 1;
             }
         }
+    }
+    return KS_OK;
+}
+KSH_CATCH
+
+int ksh_format_unschedulable(uint32_t n_nodes, const ks_pod_reasons* r, char* buf, size_t cap) try {
+    if (!r || (!buf && cap)) return fail(KS_ERR_INVALID, "NULL argument");
+    // upstream's order: the reason strings sorted lexicographically
+    const struct {
+        uint32_t count;
+        const char* text;
+    } terms[3] = {{r->insufficient_cpu, "Insufficient cpu"},
+                  {r->insufficient_memory, "Insufficient memory"},
+                  {r->node_selector_mismatch, "node(s) didn't match Pod's node affinity/selector"}};
+    std::string s = "0/" + std::to_string(n_nodes) + " nodes are available";
+    const char* sep = ": ";
+    for (const auto& t : terms) {
+        if (!t.count) continue;
+        s += sep;
+        s += std::to_string(t.count) + " " + t.text;
+        sep = ", ";
+    }
+    s += ".";
+    if (cap) std::snprintf(buf, cap, "%s", s.c_str());
+    return (int)s.size();
+}
+KSH_CATCH
+
+int ksh_explain_pods(ksh_context* c, const ks_pod_obj* pods, uint64_t n, ks_pod_reasons* out, char* messages, size_t cap,
+                     int64_t* out_msg_off) try {
+    if (!c || (n && (!pods || !out))) return fail(KS_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    if (out_msg_off)
+        for (uint64_t i = 0; i < n; i++) out_msg_off[i] = -1;
+    if (n == 0) return KS_OK;
+    std::vector<int64_t> rc_, rm_;
+    std::vector<uint64_t> sel;
+    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel);
+    if (rc) return rc;
+    if (!ks_explain) return fail(KS_ERR_NO_DEVICE, "this library has no ks_explain");
+    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
+    rc = ks_explain(c->snap, &kp, out, KS_MEM_HOST, nullptr);
+    if (rc) return rc;
+    if (!messages || !out_msg_off) return KS_OK;
+    const uint32_t N = c->N; // what pack_and_upload just gave the snapshot
+    size_t used = 0;
+    char msg[256]; // the longest message (three 10-digit counts) is under 200 bytes
+    for (uint64_t i = 0; i < n; i++) {
+        if ((uint64_t)out[i].not_enough_resources + out[i].node_selector_mismatch < N) continue; // a node is feasible
+        const int len = ksh_format_unschedulable(N, &out[i], msg, sizeof(msg));
+        if (used + (size_t)len + 1 > cap) continue; // -1 = did not fit
+        std::memcpy(messages + used, msg, (size_t)len + 1);
+        out_msg_off[i] = (int64_t)used;
+        used += (size_t)len + 1;
     }
     return KS_OK;
 }

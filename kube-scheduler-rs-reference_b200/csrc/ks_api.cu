@@ -73,6 +73,7 @@ struct ks_snapshot {
     DevBuf alloc_cpu, alloc_mem, free_cpu, free_mem, prio, labels, flag;
     DevBuf st_rc, st_rm, st_sel, st_idx, st_score, st_cnt, st_mask, st_codes, st_bnode, st_bcpu, st_bmem;
     DevBuf part_key, part_idx, part_cnt, st_samp, xflag;
+    DevBuf st_reasons; // ks_explain with host-space output
     DevBuf sb_pkey, sb_pidx, sb_pend; // device-side streaming loop (k_stream_batch)
     void* h_stream = nullptr;                 // pinned staging of one streaming micro-batch (inputs and results)
     int sms = 0, coop = 0;
@@ -179,7 +180,7 @@ void ks_snapshot_destroy(ks_snapshot* s) {
                       &s->flag,      &s->st_rc,     &s->st_rm,    &s->st_sel,   &s->st_idx,   &s->st_score,
                       &s->st_cnt,    &s->st_mask,   &s->st_codes, &s->st_bnode, &s->st_bcpu,  &s->st_bmem,
                       &s->part_key,  &s->part_idx,  &s->part_cnt, &s->st_samp,  &s->xflag,
-                      &s->sb_pkey,   &s->sb_pidx,   &s->sb_pend};
+                      &s->sb_pkey,   &s->sb_pidx,   &s->sb_pend,  &s->st_reasons};
     if (s->h_stream) cudaFreeHost(s->h_stream);
     for (DevBuf* b : bufs) b->release();
     bitpar_release(s->bp);
@@ -875,6 +876,36 @@ int ks_select_sampling(ks_snapshot* s, const ks_pods* pods, uint32_t attempts, u
     if (out_draw_node) CU_TRY(cudaMemcpyAsync(out_draw_node, base + off_dn, draws * 4, cudaMemcpyDeviceToHost, s->stream));
     if (out_draw_code) CU_TRY(cudaMemcpyAsync(out_draw_code, base + off_dc, draws, cudaMemcpyDeviceToHost, s->stream));
     CU_TRY(cudaStreamSynchronize(s->stream));
+    return KS_OK;
+}
+
+int ks_explain(ks_snapshot* s, const ks_pods* pods, ks_pod_reasons* out, int32_t out_space, void* cuda_stream) {
+    static_assert(sizeof(ks_pod_reasons) == 16, "ks_pod_reasons is four uint32");
+    int rc = check_pods(s, pods);
+    if (rc) return rc;
+    if (out_space != KS_MEM_HOST && out_space != KS_MEM_DEVICE) return fail(KS_ERR_INVALID, "bad out_space");
+    const uint64_t P = pods->n;
+    if (P && !out) return fail(KS_ERR_INVALID, "out is NULL");
+    if (P == 0) return KS_OK;
+    std::lock_guard<std::mutex> lk(s->mu);
+    CU_TRY(cudaSetDevice(s->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
+    uint32_t* d_out = reinterpret_cast<uint32_t*>(out);
+    if (out_space == KS_MEM_HOST) {
+        CU_TRY(s->st_reasons.ensure(P * sizeof(ks_pod_reasons)));
+        d_out = s->st_reasons.as<uint32_t>();
+    }
+    if (s->N == 0) {
+        CU_TRY(cudaMemsetAsync(d_out, 0, P * sizeof(ks_pod_reasons), st));
+    } else {
+        PodView pv;
+        rc = stage_pods(s, pods, st, &pv);
+        if (rc) return rc;
+        CU_TRY(launch_explain_counts(node_table(s), pv, d_out, s->sms, st));
+    }
+    if (out_space == KS_MEM_HOST)
+        CU_TRY(cudaMemcpyAsync(out, d_out, P * sizeof(ks_pod_reasons), cudaMemcpyDeviceToHost, st));
+    if (out_space == KS_MEM_HOST || pods->mem_space == KS_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
     return KS_OK;
 }
 

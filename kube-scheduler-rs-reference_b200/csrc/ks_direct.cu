@@ -508,4 +508,152 @@ cudaError_t launch_select_direct(const SelectLaunch& L, const PartialView& part,
     }
 }
 
+// ------------------------------------------------------------------------------------------------ K2e
+// Per-pod rejection counts (ks_explain): K2d's tile staging and pod-per-warp layout, three ballots per 32 nodes
+// instead of one.  Counts of one CTA row are warp-uniform; with gridDim.y > 1 the node chunks add into a zeroed
+// output, and integer adds make the result independent of their order.
+template <int W>
+__global__ void __launch_bounds__(DIRECT_THREADS)
+    k_explain_counts(NodeTable nt, PodView pv, uint32_t* __restrict__ out, uint32_t tiles_per_chunk) {
+    constexpr int PW = PodsPerWarp<W>::v;
+    constexpr uint32_t STAGE_BYTES = (2u + W) * TILE_N * 8u;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    __shared__ __align__(8) uint64_t full_bar[2];
+
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t n_tiles_total = nt.Npad / TILE_N;
+    const uint32_t tile_begin = blockIdx.y * tiles_per_chunk;
+    const uint32_t tile_end = min(tile_begin + tiles_per_chunk, n_tiles_total);
+
+    if (threadIdx.x == 0) {
+        mbar_init(&full_bar[0], 1);
+        mbar_init(&full_bar[1], 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    auto issue_tile = [&](uint32_t tile, uint32_t stage) {
+        unsigned char* dst = smem_raw + (size_t)stage * STAGE_BYTES;
+        uint64_t* bar = &full_bar[stage];
+        mbar_arrive_expect_tx(bar, STAGE_BYTES);
+        const size_t off = (size_t)tile * TILE_N;
+        tma_bulk_g2s(dst, nt.free_cpu + off, TILE_N * 8, bar);
+        tma_bulk_g2s(dst + TILE_N * 8, nt.free_mem + off, TILE_N * 8, bar);
+#pragma unroll
+        for (int w = 0; w < W; w++)
+            tma_bulk_g2s(dst + (2 + w) * TILE_N * 8, nt.labels + (size_t)w * nt.Npad + off, TILE_N * 8, bar);
+    };
+
+    if (threadIdx.x == 0 && tile_begin < tile_end) issue_tile(tile_begin, 0);
+
+    const uint32_t p0 = (blockIdx.x * (DIRECT_THREADS / 32) + warp) * PW;
+    int64_t rc[PW], rm[PW];
+    uint64_t sel[PW][W];
+    uint32_t n_cpu[PW], n_mem[PW], n_res[PW], n_sel[PW];
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        uint32_t p = min(p0 + i, pv.P - 1);
+        rc[i] = __ldg(pv.req_cpu + p);
+        rm[i] = __ldg(pv.req_mem + p);
+#pragma unroll
+        for (int w = 0; w < W; w++) sel[i][w] = __ldg(pv.sel + (uint64_t)p * W + w);
+        n_cpu[i] = n_mem[i] = n_res[i] = n_sel[i] = 0;
+    }
+
+    for (uint32_t tile = tile_begin; tile < tile_end; tile++) {
+        const uint32_t it = tile - tile_begin, stage = it & 1;
+        if (threadIdx.x == 0 && tile + 1 < tile_end) issue_tile(tile + 1, stage ^ 1);
+        mbar_wait(&full_bar[stage], (it >> 1) & 1);
+
+        const unsigned char* base = smem_raw + (size_t)stage * STAGE_BYTES;
+        const int64_t* s_fc = reinterpret_cast<const int64_t*>(base);
+        const int64_t* s_fm = s_fc + TILE_N;
+        const uint64_t* s_lab = reinterpret_cast<const uint64_t*>(s_fm + TILE_N);
+
+#pragma unroll 2
+        for (uint32_t g = 0; g < 32; g++) {
+            const uint32_t ln = g * 32 + lane;
+            const int64_t fc = s_fc[ln], fm = s_fm[ln];
+            uint64_t lab[W];
+#pragma unroll
+            for (int w = 0; w < W; w++) lab[w] = s_lab[w * TILE_N + ln];
+            const bool real = tile * TILE_N + ln < nt.N; // padding sentinels never count
+#pragma unroll
+            for (int i = 0; i < PW; i++) {
+                const bool cpu_fail = real && rc[i] > fc; // predicates.rs:42, each half
+                const bool mem_fail = real && rm[i] > fm;
+                uint64_t miss = 0;
+#pragma unroll
+                for (int w = 0; w < W; w++) miss |= sel[i][w] & ~lab[w];
+                const bool sel_fail = real && !cpu_fail && !mem_fail && miss != 0; // fit first, :68-74
+                const uint32_t bc = __ballot_sync(0xffffffffu, cpu_fail);
+                const uint32_t bm = __ballot_sync(0xffffffffu, mem_fail);
+                const uint32_t bs = __ballot_sync(0xffffffffu, sel_fail);
+                n_cpu[i] += __popc(bc);
+                n_mem[i] += __popc(bm);
+                n_res[i] += __popc(bc | bm);
+                n_sel[i] += __popc(bs);
+            }
+        }
+        __syncthreads(); // everyone is done with `stage` before it is refilled two iterations later
+    }
+
+    if (lane == 0) { // the counts are warp-uniform
+#pragma unroll
+        for (int i = 0; i < PW; i++) {
+            if (p0 + i >= pv.P) continue;
+            uint32_t* o = out + (uint64_t)(p0 + i) * 4;
+            if (gridDim.y == 1) {
+                o[0] = n_cpu[i];
+                o[1] = n_mem[i];
+                o[2] = n_res[i];
+                o[3] = n_sel[i];
+            } else {
+                atomicAdd(o + 0, n_cpu[i]);
+                atomicAdd(o + 1, n_mem[i]);
+                atomicAdd(o + 2, n_res[i]);
+                atomicAdd(o + 3, n_sel[i]);
+            }
+        }
+    }
+}
+
+template <int W>
+static cudaError_t launch_explain_w(const NodeTable& nt, const PodView& pv, uint32_t* out, int sms, cudaStream_t st) {
+    constexpr uint32_t SMEM = 2u * (2u + W) * TILE_N * 8u;
+    static bool prepared = false; // opt-in shared memory size, once per label width
+    if (!prepared) {
+        cudaError_t e = cudaFuncSetAttribute(k_explain_counts<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
+        if (e != cudaSuccess) return e;
+        prepared = true;
+    }
+    // node chunks across gridDim.y when the pods alone give fewer than two CTAs per SM (same rule as ks_select)
+    const uint32_t pods_per_cta = (DIRECT_THREADS / 32) * PodsPerWarp<W>::v;
+    const uint32_t n_tiles = nt.Npad / TILE_N;
+    const uint32_t pod_ctas = (pv.P + pods_per_cta - 1) / pods_per_cta;
+    const uint32_t want_ctas = 2u * (uint32_t)sms;
+    uint32_t n_chunks = 1;
+    if (pod_ctas < want_ctas) n_chunks = std::min<uint32_t>(n_tiles, (want_ctas + pod_ctas - 1) / pod_ctas);
+    const uint32_t tiles_per_chunk = (n_tiles + n_chunks - 1) / n_chunks;
+    n_chunks = (n_tiles + tiles_per_chunk - 1) / tiles_per_chunk;
+    if (n_chunks > 1) {
+        cudaError_t e = cudaMemsetAsync(out, 0, (size_t)pv.P * 16, st);
+        if (e != cudaSuccess) return e;
+    }
+    k_explain_counts<W><<<dim3(pod_ctas, n_chunks), DIRECT_THREADS, SMEM, st>>>(nt, pv, out, tiles_per_chunk);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_explain_counts(const NodeTable& nt, const PodView& pv, uint32_t* out, int sms, cudaStream_t st) {
+    if (pv.P == 0 || nt.Npad == 0) return cudaSuccess;
+    switch (nt.W) {
+        case 1: return launch_explain_w<1>(nt, pv, out, sms, st);
+        case 2: return launch_explain_w<2>(nt, pv, out, sms, st);
+        case 4: return launch_explain_w<4>(nt, pv, out, sms, st);
+        case 8: return launch_explain_w<8>(nt, pv, out, sms, st);
+        default: return cudaErrorInvalidValue;
+    }
+}
+
 } // namespace ks

@@ -21,6 +21,8 @@ uint32_t direct_pods_per_cta(uint32_t W);
 cudaError_t prepare_select_direct(uint32_t W);
 cudaError_t launch_select_direct(const SelectLaunch& L, const PartialView& part, uint32_t n_chunks,
                                  uint32_t tiles_per_chunk);
+// per-pod rejection counts (ks_explain): out = uint32 [P][4] in ks_pod_reasons order, device memory
+cudaError_t launch_explain_counts(const NodeTable& nt, const PodView& pv, uint32_t* out, int sms, cudaStream_t st);
 
 } // namespace ks
 

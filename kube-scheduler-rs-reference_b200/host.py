@@ -34,6 +34,8 @@ for _name, _res, _args in [
     ("ksh_select_node_for_pod", C.c_int, [_vp, _vp, C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64, _vp, _vp, _vp, _vp]),
     ("ksh_reconcile_batch", C.c_int, [_vp, _vp, C.c_uint64, C.c_int, _vp, _vp, _vp, C.c_size_t, _vp, C.POINTER(C.c_uint32)]),
     ("ksh_reconcile", C.c_int, [_vp, _vp, C.c_int, C.POINTER(C.c_int32), C.c_char_p, C.c_size_t]),
+    ("ksh_explain_pods", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, C.c_size_t, _vp]),
+    ("ksh_format_unschedulable", C.c_int, [C.c_uint32, C.POINTER(capi.ks_pod_reasons), _vp, C.c_size_t]),
 ]:
     _f = getattr(lib, _name)
     _f.restype = _res
@@ -67,6 +69,16 @@ def total_pod_resources(pods, i=0):
 
 def is_pod_bound(pods, i=0):
     return bool(lib.ksh_is_pod_bound(_addr(pods, i)))
+
+
+def format_unschedulable(n_nodes, reasons, cap=256):
+    """FailedScheduling message for one pod's counts (4 ints in ks_pod_reasons order): (full length, text in cap bytes)."""
+    r = capi.ks_pod_reasons(*[int(x) for x in reasons])
+    buf = C.create_string_buffer(max(cap, 1))
+    n = lib.ksh_format_unschedulable(int(n_nodes), C.byref(r), C.addressof(buf) if cap else None, int(cap))
+    if n < 0:
+        raise KsError(n, "ksh_format_unschedulable")
+    return n, buf.value.decode()
 
 
 class Context:
@@ -192,6 +204,18 @@ class Context:
         if rc != capi.KS_OK:
             raise KsError(rc, "ksh_select_node_for_pod")
         return idx, used, dn, dc
+
+    def explain_pods(self, pods, n, first=0, msg_cap=None):
+        """Why pods do not schedule: (reasons uint32 [n, 4], messages[n]) where messages[i] is the FailedScheduling
+        message of a pod with no feasible node (str) or None."""
+        out = np.empty((n, 4), np.uint32)
+        off = np.empty(n, np.int64)
+        cap = int(msg_cap if msg_cap is not None else 256 * max(n, 1))
+        buf = C.create_string_buffer(max(cap, 1))
+        rc = lib.ksh_explain_pods(self._h, _addr(pods, first), n, out.ctypes.data, C.addressof(buf), cap, off.ctypes.data)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ksh_explain_pods")
+        return out, [None if o < 0 else C.string_at(C.addressof(buf) + int(o)).decode() for o in off]
 
     def reconcile(self, pods, i, policy=capi.KS_SCORE_LEFTOVER):
         node = C.c_int32(-1)

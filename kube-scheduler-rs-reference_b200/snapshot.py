@@ -195,6 +195,24 @@ class Snapshot:
             raise KsError(rc, "ks_select_sampling")
         return idx, used, dn, dc
 
+    def explain(self, req_cpu, req_mem, sel):
+        """Per-pod rejection counts (ks_explain) over host (numpy) pods: uint32 [P, 4] with columns insufficient_cpu,
+        insufficient_memory, not_enough_resources, node_selector_mismatch."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        out = np.empty((int(pods.n), 4), np.uint32)
+        rc = lib.ks_explain(self._h, C.byref(pods), _ptr(out), capi.KS_MEM_HOST, None)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ks_explain")
+        return out
+
+    def explain_raw(self, n_pods, req_cpu, req_mem, sel, pods_space, out, out_space, stream=None):
+        """Pointer-level ks_explain (torch tensors / raw addresses); out holds n_pods x 16 bytes.  The caller keeps the
+        buffers alive; with device pods and output the call returns after enqueue on `stream`."""
+        pods = ks_pods(int(n_pods), _ptr(req_cpu), _ptr(req_mem), _ptr(sel), int(pods_space))
+        rc = lib.ks_explain(self._h, C.byref(pods), _ptr(out), int(out_space), C.c_void_p(stream) if stream else None)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ks_explain")
+
     def last_timings(self):
         ms = (C.c_float * 3)()
         rc = lib.ks_last_timings(self._h, ms)
