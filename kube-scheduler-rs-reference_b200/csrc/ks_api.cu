@@ -164,6 +164,7 @@ int ks_snapshot_create(int device, ks_snapshot** out) {
     if (e == cudaSuccess) e = s->flag.ensure(sizeof(int));
     if (e == cudaSuccess) e = s->xflag.ensure(sizeof(int));
     if (e == cudaSuccess) e = cudaMemset(s->xflag.p, 0, sizeof(int));
+    if (e == cudaSuccess) e = prepare_direct();
     if (e != cudaSuccess) {
         ks_snapshot_destroy(s);
         return fail(KS_ERR_CUDA, "snapshot init failed: %s", cudaGetErrorString(e));
@@ -539,28 +540,21 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
         else if (!(flags & KS_SELECT_FORCE_DIRECT))
             use_bitpar = may_bitpar && bitpar_profitable(s->bp, L.pv.P);
         // everything that allocates happens before the (possibly captured) launch sequence
-        uint32_t n_chunks = 1, tiles_per_chunk = 0;
+        DirectGrid grid{};
         PartialView part{nullptr, nullptr, nullptr};
         if (use_bitpar) {
             cudaError_t e = bitpar_prepare(s->bp, L.pv.P);
             if (e != cudaSuccess) return fail(KS_ERR_CUDA, "bit-parallel prepare failed: %s", cudaGetErrorString(e));
         } else {
-            const uint32_t n_tiles = s->Npad / TILE_N;
-            const uint32_t pod_ctas = (L.pv.P + direct_pods_per_cta(s->W) - 1) / direct_pods_per_cta(s->W);
-            const uint32_t want_ctas = 2u * (uint32_t)s->sms; // at least two CTAs per SM
-            if (pod_ctas < want_ctas) n_chunks = std::min<uint32_t>(n_tiles, (want_ctas + pod_ctas - 1) / pod_ctas);
-            tiles_per_chunk = (n_tiles + n_chunks - 1) / n_chunks;
-            n_chunks = (n_tiles + tiles_per_chunk - 1) / tiles_per_chunk;
-            if (n_chunks > 1) {
-                CU_TRY(s->part_key.ensure((size_t)n_chunks * P * 8));
-                CU_TRY(s->part_idx.ensure((size_t)n_chunks * P * 4));
-                CU_TRY(s->part_cnt.ensure((size_t)n_chunks * P * 4));
+            grid = direct_grid(s->W, L.pv.P, s->Npad, s->sms);
+            if (grid.n_chunks > 1) {
+                CU_TRY(s->part_key.ensure((size_t)grid.n_chunks * P * 8));
+                CU_TRY(s->part_idx.ensure((size_t)grid.n_chunks * P * 4));
+                CU_TRY(s->part_cnt.ensure((size_t)grid.n_chunks * P * 4));
                 part.key = s->part_key.as<int64_t>();
                 part.idx = s->part_idx.as<int32_t>();
                 part.cnt = s->part_cnt.as<uint32_t>();
             }
-            cudaError_t e = prepare_select_direct(s->W);
-            if (e != cudaSuccess) return fail(KS_ERR_CUDA, "direct prepare failed: %s", cudaGetErrorString(e));
         }
         s->last_path = use_bitpar ? "bitpar" : "direct";
         // Host-space batches on the bit-parallel path are pipelined in two pod chunks: the second chunk is copied in
@@ -620,7 +614,7 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
                 if (e != cudaSuccess) return fail(KS_ERR_CUDA, "bit-parallel select failed: %s", cudaGetErrorString(e));
             } else {
                 if (timing) CU_TRY(cudaEventRecord(s->ev[1], st));
-                cudaError_t e = launch_select_direct(L, part, n_chunks, tiles_per_chunk);
+                cudaError_t e = launch_select_direct(L, part, grid);
                 if (e != cudaSuccess) return fail(KS_ERR_CUDA, "direct select failed: %s", cudaGetErrorString(e));
                 if (timing) CU_TRY(cudaEventRecord(s->ev[2], st));
                 if (xc) CU_TRY(launch_exchange_push(po, ov.node_idx, ov.score, (uint32_t)P, st));
@@ -918,8 +912,7 @@ int ks_stream_bind(ks_snapshot* s, const ks_pods* pods, int policy, int32_t* out
     const uint64_t n = pods->n;
     const uint32_t W = s->W;
     if (policy != KS_SCORE_LEFTOVER && policy != KS_SCORE_LEAST_ALLOCATED) return fail(KS_ERR_INVALID, "bad policy");
-    static const bool host_loop = getenv("KS_STREAM_HOST_LOOP") != nullptr; // A/B switch: the round-1 host-driven loop
-    if (n > 0 && n <= STREAM_BATCH_MAX && s->N > 0 && s->coop && !host_loop) {
+    if (n > 0 && n <= STREAM_BATCH_MAX && s->N > 0 && s->coop) {
         // device-side loop: one H2D, ONE cooperative launch that runs every round, one D2H
         std::lock_guard<std::mutex> lk(s->mu);
         CU_TRY(cudaSetDevice(s->device));
@@ -977,7 +970,7 @@ int ks_stream_bind(ks_snapshot* s, const ks_pods* pods, int policy, int32_t* out
         s->last_path = "stream_batch";
         return KS_OK;
     }
-    try { // host-driven loop (large batches, A/B): its vectors must not throw across the ABI
+    try { // host-driven loop (large batches, no cooperative launch): its vectors must not throw across the ABI
         std::vector<uint64_t> pending(n);
         for (uint64_t i = 0; i < n; i++) {
             pending[i] = i;

@@ -65,10 +65,7 @@ __device__ __forceinline__ bool key_less(int64_t av, uint32_t ai, int64_t bv, ui
 // KS_SCORE_LEAST_ALLOCATED bound: the score of node n for a pod that requests nothing.  For requests >= 0 the score of
 // every feasible (pod, n) cell is <= least_alloc_bound(n) (same truncating divisions, monotone in the numerators).
 __device__ __forceinline__ int64_t least_alloc_bound(const NodeTable& nt, uint32_t n) {
-    const int64_t fc = nt.free_cpu[n], fm = nt.free_mem[n], ac = nt.alloc_cpu[n], am = nt.alloc_mem[n];
-    const int64_t pc = ac > 0 ? (fc * 100) / ac : 0;
-    const int64_t pm = am > 0 ? (fm * 100) / am : 0;
-    return (pc + pm) / 2;
+    return least_alloc_int(nt.free_cpu[n], nt.free_mem[n], nt.alloc_cpu[n], nt.alloc_mem[n], 0, 0);
 }
 // prio[0..Npad) = leftover priority, prio[Npad..Npad+N) = least-allocated bound (k_node_bound, once per build)
 __device__ __forceinline__ int64_t order_value(const NodeTable& nt, const int64_t* __restrict__ prio, int k, uint32_t n) {
@@ -883,7 +880,7 @@ __device__ __forceinline__ void write_binding(const OutView& ov, const PodView& 
     int64_t score = 0;
     if (slot >= 0) {
         best = __ldg(ord_idx + slot);
-        score = __ldg(ord_prio + slot) - (int64_t)(((uint64_t)__ldg(pv.req_cpu + p) << 22) + (uint64_t)__ldg(pv.req_mem + p));
+        score = leftover_score(__ldg(ord_prio + slot), __ldg(pv.req_cpu + p), __ldg(pv.req_mem + p));
     }
     if (ov.node_idx) ov.node_idx[p] = best;
     if (ov.score) ov.score[p] = score;
@@ -1596,13 +1593,7 @@ cudaError_t bitpar_read_trace(const BitparIndex& ix, unsigned long long out_ns[B
 
 cudaError_t bitpar_select(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before_mask, cudaEvent_t after_mask) {
     if (!ix.valid) return cudaErrorNotSupported;
-    switch (ix.W) {
-        case 1: return select_w<1>(ix, L, before_mask, after_mask);
-        case 2: return select_w<2>(ix, L, before_mask, after_mask);
-        case 4: return select_w<4>(ix, L, before_mask, after_mask);
-        case 8: return select_w<8>(ix, L, before_mask, after_mask);
-        default: return cudaErrorInvalidValue;
-    }
+    return with_label_width(ix.W, [&](auto w) { return select_w<decltype(w)::value>(ix, L, before_mask, after_mask); });
 }
 
 } // namespace ks

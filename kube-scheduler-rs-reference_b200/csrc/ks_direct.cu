@@ -1,9 +1,11 @@
 // ks_direct.cu — per-cell ("direct") kernels for sm_90a.
 //   K0  k_node_free_reduce     free = alloc - sum(bound)            /root/reference/src/predicates.rs:27-38
 //   K1  k_check_cells          2-bit reason code per cell           /root/reference/src/predicates.rs:63-77
-//   K2d k_select_direct        fused feasible mask + count + argmax score, node tiles staged through
-//                              shared memory by TMA bulk copies (cp.async.bulk + mbarrier), one lane per
-//                              node, warp ballot packs 32 cells into one mask word, warp-shuffle argmax.
+//   K2d k_select_direct        fused feasible mask + count + argmax score, warp ballot packs 32 cells into
+//                              one mask word, warp-shuffle argmax
+//   K2e k_explain_counts       per-pod rejection counts (ks_explain)
+// K2d and K2e share one node-tile scan (scan_node_tiles): tiles staged through shared memory by TMA bulk
+// copies (cp.async.bulk + mbarrier), one lane per node, several pods per warp in registers.
 // The per-cell kernel is the generic path (any score policy, any P); ks_bitpar.cu holds the bit-parallel
 // fast path that the headline configuration uses.
 #include "ks_internal.cuh"
@@ -56,7 +58,7 @@ __global__ void k_node_prio(const int64_t* __restrict__ free_cpu, const int64_t*
         prio[n] = INT64_MIN + 1;
         return;
     }
-    prio[n] = fc * ((int64_t)1 << 22) + fm;
+    prio[n] = leftover_key(fc, fm); // no overflow inside the range checked above: the same bits as fc * 2^22 + fm
 }
 
 cudaError_t launch_node_prio(const int64_t* free_cpu, const int64_t* free_mem, int64_t* prio, uint32_t N,
@@ -222,31 +224,57 @@ cudaError_t launch_select_sampling(const NodeTable& nt, const PodView& pv, uint3
     return cudaGetLastError();
 }
 
-// ------------------------------------------------------------------------------------------------ K2 direct
-template <int W>
-struct PodsPerWarp {
-    static constexpr int v = W <= 2 ? 8 : (W == 4 ? 4 : 2);
-};
+// ------------------------------------------------------------------------------------------------ K2d / K2e
+__host__ __device__ constexpr uint32_t pods_per_warp(uint32_t W) { return W <= 2 ? 8u : (W == 4 ? 4u : 2u); }
 
-template <int W, int POLICY>
-struct DirectCfg {
-    static constexpr int NARR = 2 + W + (POLICY == KS_SCORE_LEAST_ALLOCATED ? 2 : 0);
-    static constexpr uint32_t STAGE_BYTES = (uint32_t)NARR * TILE_N * 8u;
-    static constexpr uint32_t SMEM_BYTES = 2u * STAGE_BYTES;
-};
+// Shared memory of one stage of the node-tile scan: free_cpu, free_mem, the W label words and, when the body scores
+// LeastAllocated, alloc_cpu and alloc_mem, TILE_N nodes each.  Two stages double-buffer the tiles.
+template <int W, bool ALLOC>
+__host__ __device__ constexpr uint32_t tile_stage_bytes() {
+    return (2u + W + (ALLOC ? 2u : 0u)) * TILE_N * 8u;
+}
+template <int W, bool ALLOC>
+__host__ __device__ constexpr uint32_t tile_smem_bytes() {
+    return 2u * tile_stage_bytes<W, ALLOC>();
+}
 
-template <int W, int POLICY, bool EMIT_MASK>
-__global__ void __launch_bounds__(DIRECT_THREADS)
-    k_select_direct(NodeTable nt, PodView pv, OutView ov, PartialView part, uint32_t tiles_per_chunk) {
-    constexpr int PW = PodsPerWarp<W>::v;
-    using Cfg = DirectCfg<W, POLICY>;
+// The first of this warp's PW pods.
+template <int PW>
+__device__ __forceinline__ uint32_t warp_first_pod() {
+    return (blockIdx.x * (DIRECT_THREADS / 32) + (threadIdx.x >> 5)) * PW;
+}
+
+// This warp's pods p0.. into warp-uniform registers.  Slots past P repeat the last pod (their results are never
+// written).
+template <int W, int PW>
+__device__ __forceinline__ void load_warp_pods(const PodView& pv, uint32_t p0, int64_t (&rc)[PW], int64_t (&rm)[PW],
+                                               uint64_t (&sel)[PW][W]) {
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        const uint32_t p = min(p0 + i, pv.P - 1);
+        rc[i] = __ldg(pv.req_cpu + p);
+        rm[i] = __ldg(pv.req_mem + p);
+#pragma unroll
+        for (int w = 0; w < W; w++) sel[i][w] = __ldg(pv.sel + (uint64_t)p * W + w);
+    }
+}
+
+// The node scan of K2d and K2e over this CTA's chunk of tiles, [blockIdx.y * tiles_per_chunk, +tiles_per_chunk).  One
+// thread stages each tile through shared memory with bulk copies, one tile ahead of the warps.  The warp's first pod p0
+// and its pods' registers rc/rm/sel are loaded while the first tile is in flight.  Each lane takes one node of every
+// group of 32 and the whole warp calls cell(g, node, real, fc, fm, lab, ac, am), so the body may ballot; real is false
+// for padding nodes, and ac/am are 0 unless ALLOC.  After a tile's 32 groups every thread calls tile_done(tile).
+template <int W, bool ALLOC, int PW, class Cell, class TileDone>
+__device__ __forceinline__ void scan_node_tiles(const NodeTable& nt, uint32_t tiles_per_chunk, const PodView& pv, uint32_t& p0,
+                                                int64_t (&rc)[PW], int64_t (&rm)[PW], uint64_t (&sel)[PW][W], Cell&& cell,
+                                                TileDone&& tile_done) {
+    constexpr uint32_t STAGE_BYTES = tile_stage_bytes<W, ALLOC>();
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ __align__(8) uint64_t full_bar[2];
 
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t n_tiles_total = nt.Npad / TILE_N;
+    const uint32_t lane = threadIdx.x & 31;
     const uint32_t tile_begin = blockIdx.y * tiles_per_chunk;
-    const uint32_t tile_end = min(tile_begin + tiles_per_chunk, n_tiles_total);
+    const uint32_t tile_end = min(tile_begin + tiles_per_chunk, nt.Npad / TILE_N);
 
     if (threadIdx.x == 0) {
         mbar_init(&full_bar[0], 1);
@@ -256,51 +284,32 @@ __global__ void __launch_bounds__(DIRECT_THREADS)
     __syncthreads();
 
     auto issue_tile = [&](uint32_t tile, uint32_t stage) {
-        // one elected thread arms the barrier with the byte count, then issues one bulk copy per SoA column
-        unsigned char* dst = smem_raw + (size_t)stage * Cfg::STAGE_BYTES;
+        // arm the barrier with the byte count, then issue one bulk copy per SoA column
+        unsigned char* dst = smem_raw + (size_t)stage * STAGE_BYTES;
         uint64_t* bar = &full_bar[stage];
-        mbar_arrive_expect_tx(bar, Cfg::STAGE_BYTES);
+        mbar_arrive_expect_tx(bar, STAGE_BYTES);
         const size_t off = (size_t)tile * TILE_N;
         tma_bulk_g2s(dst, nt.free_cpu + off, TILE_N * 8, bar);
         tma_bulk_g2s(dst + TILE_N * 8, nt.free_mem + off, TILE_N * 8, bar);
 #pragma unroll
         for (int w = 0; w < W; w++)
             tma_bulk_g2s(dst + (2 + w) * TILE_N * 8, nt.labels + (size_t)w * nt.Npad + off, TILE_N * 8, bar);
-        if (POLICY == KS_SCORE_LEAST_ALLOCATED) {
+        if (ALLOC) {
             tma_bulk_g2s(dst + (2 + W) * TILE_N * 8, nt.alloc_cpu + off, TILE_N * 8, bar);
             tma_bulk_g2s(dst + (3 + W) * TILE_N * 8, nt.alloc_mem + off, TILE_N * 8, bar);
         }
     };
 
     if (threadIdx.x == 0 && tile_begin < tile_end) issue_tile(tile_begin, 0);
-
-    // this warp's pods (uniform registers)
-    const uint32_t p0 = (blockIdx.x * (DIRECT_THREADS / 32) + warp) * PW;
-    int64_t rc[PW], rm[PW];
-    uint64_t sel[PW][W];
-    int64_t best[PW];
-    int32_t bidx[PW];
-    uint32_t cnt[PW];
-    uint32_t acc[PW];
-#pragma unroll
-    for (int i = 0; i < PW; i++) {
-        uint32_t p = min(p0 + i, pv.P - 1);
-        rc[i] = __ldg(pv.req_cpu + p);
-        rm[i] = __ldg(pv.req_mem + p);
-#pragma unroll
-        for (int w = 0; w < W; w++) sel[i][w] = __ldg(pv.sel + (uint64_t)p * W + w);
-        best[i] = INT64_MIN;
-        bidx[i] = -1;
-        cnt[i] = 0;
-        acc[i] = 0;
-    }
+    p0 = warp_first_pod<PW>();
+    load_warp_pods(pv, p0, rc, rm, sel);
 
     for (uint32_t tile = tile_begin; tile < tile_end; tile++) {
         const uint32_t it = tile - tile_begin, stage = it & 1;
         if (threadIdx.x == 0 && tile + 1 < tile_end) issue_tile(tile + 1, stage ^ 1);
         mbar_wait(&full_bar[stage], (it >> 1) & 1);
 
-        const unsigned char* base = smem_raw + (size_t)stage * Cfg::STAGE_BYTES;
+        const unsigned char* base = smem_raw + (size_t)stage * STAGE_BYTES;
         const int64_t* s_fc = reinterpret_cast<const int64_t*>(base);
         const int64_t* s_fm = s_fc + TILE_N;
         const uint64_t* s_lab = reinterpret_cast<const uint64_t*>(s_fm + TILE_N);
@@ -314,15 +323,39 @@ __global__ void __launch_bounds__(DIRECT_THREADS)
             uint64_t lab[W];
 #pragma unroll
             for (int w = 0; w < W; w++) lab[w] = s_lab[w * TILE_N + ln];
-            const int32_t node = (int32_t)(tile * TILE_N + ln);
-            const bool real = (uint32_t)node < nt.N; // padding sentinels are never feasible
-            int64_t key_n = 0, ac = 0, am = 0;
-            if (POLICY == KS_SCORE_LEFTOVER) {
-                key_n = (int64_t)(((uint64_t)fc << 22) + (uint64_t)fm); // node priority; pod part is constant
-            } else {
-                ac = s_ac[ln];
-                am = s_am[ln];
-            }
+            const uint32_t node = tile * TILE_N + ln;
+            cell(g, node, node < nt.N, fc, fm, lab, ALLOC ? s_ac[ln] : 0, ALLOC ? s_am[ln] : 0);
+        }
+        tile_done(tile);
+        __syncthreads(); // everyone is done with `stage` before it is refilled two iterations later
+    }
+}
+
+template <int W, int POLICY, bool EMIT_MASK>
+__global__ void __launch_bounds__(DIRECT_THREADS)
+    k_select_direct(NodeTable nt, PodView pv, OutView ov, PartialView part, uint32_t tiles_per_chunk) {
+    constexpr int PW = pods_per_warp(W);
+    constexpr bool LA = POLICY == KS_SCORE_LEAST_ALLOCATED;
+    const uint32_t lane = threadIdx.x & 31;
+    int64_t rc[PW], rm[PW];
+    uint64_t sel[PW][W];
+    uint32_t p0;
+    int64_t best[PW];
+    int32_t bidx[PW];
+    uint32_t cnt[PW];
+    uint32_t acc[PW];
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        best[i] = INT64_MIN;
+        bidx[i] = -1;
+        cnt[i] = 0;
+        acc[i] = 0;
+    }
+
+    scan_node_tiles<W, LA>(
+        nt, tiles_per_chunk, pv, p0, rc, rm, sel,
+        [&](uint32_t g, uint32_t node, bool real, int64_t fc, int64_t fm, const uint64_t(&lab)[W], int64_t ac, int64_t am) {
+            const int64_t key_n = LA ? 0 : leftover_key(fc, fm); // LEFTOVER: node priority; the pod part is constant
 #pragma unroll
             for (int i = 0; i < PW; i++) {
                 const bool fit = (rc[i] <= fc) & (rm[i] <= fm);
@@ -333,56 +366,34 @@ __global__ void __launch_bounds__(DIRECT_THREADS)
                 const uint32_t b = __ballot_sync(0xffffffffu, ok);
                 cnt[i] += __popc(b);
                 if (EMIT_MASK) acc[i] = (lane == g) ? b : acc[i];
-                if (POLICY == KS_SCORE_LEFTOVER) {
-                    if (ok && key_n > best[i]) {
-                        best[i] = key_n;
-                        bidx[i] = node;
-                    }
-                } else {
-                    if (ok) {
-                        int64_t pc = ac > 0 ? ((fc - rc[i]) * 100) / ac : 0;
-                        int64_t pm = am > 0 ? ((fm - rm[i]) * 100) / am : 0;
-                        int64_t s = (pc + pm) / 2;
-                        if (s > best[i]) {
-                            best[i] = s;
-                            bidx[i] = node;
-                        }
+                if (ok) {
+                    const int64_t key = LA ? least_alloc_int(fc, fm, ac, am, rc[i], rm[i]) : key_n;
+                    if (key > best[i]) {
+                        best[i] = key;
+                        bidx[i] = (int32_t)node;
                     }
                 }
             }
-        }
-        if (EMIT_MASK) {
+        },
+        [&](uint32_t tile) {
+            if (!EMIT_MASK) return;
             const uint32_t word = tile * 32 + lane; // 32 words per 1024-node tile
             if (word < ov.mask_valid_words) {
 #pragma unroll
                 for (int i = 0; i < PW; i++)
                     if (p0 + i < pv.P) ov.mask[(uint64_t)(p0 + i) * ov.mask_row_words + word] = acc[i];
             }
-        }
-        __syncthreads(); // everyone is done with `stage` before it is refilled two iterations later
-    }
+        });
 
-    // warp argmax: larger key wins, ties -> lower node index
 #pragma unroll
     for (int i = 0; i < PW; i++) {
         int64_t k = best[i];
         int32_t ix = bidx[i];
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) {
-            int64_t ok_ = __shfl_xor_sync(0xffffffffu, k, off);
-            int32_t oi = __shfl_xor_sync(0xffffffffu, ix, off);
-            bool take = (oi >= 0) && (ix < 0 || ok_ > k || (ok_ == k && oi < ix));
-            if (take) {
-                k = ok_;
-                ix = oi;
-            }
-        }
+        warp_argmax(k, ix);
         if (lane == 0 && p0 + i < pv.P) {
             const uint32_t p = p0 + i;
             if (gridDim.y == 1) {
-                int64_t s = 0;
-                if (ix >= 0)
-                    s = (POLICY == KS_SCORE_LEFTOVER) ? k - (int64_t)(((uint64_t)rc[i] << 22) + (uint64_t)rm[i]) : k;
+                const int64_t s = ix < 0 ? 0 : (LA ? k : leftover_score(k, rc[i], rm[i]));
                 if (ov.node_idx) ov.node_idx[p] = ix;
                 if (ov.score) ov.score[p] = s;
                 if (ov.cnt) ov.cnt[p] = cnt[i];
@@ -396,7 +407,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS)
     }
 }
 
-// combine partials of node chunks: ascending chunk order + strict '>' keeps the lowest node index on ties
+// combine the partials of the node chunks, in ascending chunk order
 template <int POLICY>
 __global__ void k_select_combine(PodView pv, OutView ov, PartialView part, uint32_t n_chunks) {
     uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
@@ -407,177 +418,30 @@ __global__ void k_select_combine(PodView pv, OutView ov, PartialView part, uint3
     for (uint32_t ch = 0; ch < n_chunks; ch++) {
         const uint64_t o = (uint64_t)ch * pv.P + p;
         c += part.cnt[o];
-        int32_t oi = part.idx[o];
-        int64_t ok_ = part.key[o];
-        if (oi >= 0 && (ix < 0 || ok_ > k)) {
-            k = ok_;
-            ix = oi;
-        }
+        merge_partial(k, ix, part.key[o], part.idx[o]);
     }
-    int64_t s = 0;
-    if (ix >= 0)
-        s = (POLICY == KS_SCORE_LEFTOVER)
-                ? k - (int64_t)(((uint64_t)pv.req_cpu[p] << 22) + (uint64_t)pv.req_mem[p])
-                : k;
+    const int64_t s = ix < 0 ? 0 : (POLICY == KS_SCORE_LEFTOVER ? leftover_score(k, pv.req_cpu[p], pv.req_mem[p]) : k);
     if (ov.node_idx) ov.node_idx[p] = ix;
     if (ov.score) ov.score[p] = s;
     if (ov.cnt) ov.cnt[p] = c;
 }
 
-template <int W, int POLICY, bool EMIT>
-static cudaError_t launch_direct_t(const SelectLaunch& L, const PartialView& part, uint32_t n_chunks,
-                                   uint32_t tiles_per_chunk) {
-    using Cfg = DirectCfg<W, POLICY>;
-    constexpr int PW = PodsPerWarp<W>::v;
-    auto kern = k_select_direct<W, POLICY, EMIT>;
-    cudaError_t e;
-    const uint32_t pods_per_cta = (DIRECT_THREADS / 32) * PW;
-    dim3 grid((L.pv.P + pods_per_cta - 1) / pods_per_cta, n_chunks);
-    kern<<<grid, DIRECT_THREADS, Cfg::SMEM_BYTES, L.stream>>>(L.nt, L.pv, L.ov, part, tiles_per_chunk);
-    g_launches++;
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    if (n_chunks > 1) {
-        k_select_combine<POLICY><<<(L.pv.P + 255) / 256, 256, 0, L.stream>>>(L.pv, L.ov, part, n_chunks);
-        g_launches++;
-        e = cudaGetLastError();
-    }
-    return e;
-}
-
-template <int W>
-static cudaError_t launch_direct_w(const SelectLaunch& L, const PartialView& part, uint32_t n_chunks,
-                                   uint32_t tiles_per_chunk) {
-    const bool emit = L.ov.mask != nullptr;
-    if (L.policy == KS_SCORE_LEFTOVER)
-        return emit ? launch_direct_t<W, KS_SCORE_LEFTOVER, true>(L, part, n_chunks, tiles_per_chunk)
-                    : launch_direct_t<W, KS_SCORE_LEFTOVER, false>(L, part, n_chunks, tiles_per_chunk);
-    return emit ? launch_direct_t<W, KS_SCORE_LEAST_ALLOCATED, true>(L, part, n_chunks, tiles_per_chunk)
-                : launch_direct_t<W, KS_SCORE_LEAST_ALLOCATED, false>(L, part, n_chunks, tiles_per_chunk);
-}
-
-template <int W>
-static cudaError_t prepare_w() {
-    cudaError_t e;
-#define KS_SET(P_, M_)                                                                                            \
-    if ((e = cudaFuncSetAttribute(k_select_direct<W, P_, M_>, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
-                                  (int)DirectCfg<W, P_>::SMEM_BYTES)) != cudaSuccess)                             \
-        return e;
-    KS_SET(KS_SCORE_LEFTOVER, true)
-    KS_SET(KS_SCORE_LEFTOVER, false)
-    KS_SET(KS_SCORE_LEAST_ALLOCATED, true)
-    KS_SET(KS_SCORE_LEAST_ALLOCATED, false)
-#undef KS_SET
-    return cudaSuccess;
-}
-
-// opt-in shared memory sizes, once per label width (must not run inside a stream capture)
-cudaError_t prepare_select_direct(uint32_t W) {
-    static bool done[9] = {false, false, false, false, false, false, false, false, false};
-    if (W > 8) return cudaErrorInvalidValue;
-    if (done[W]) return cudaSuccess;
-    cudaError_t e = cudaErrorInvalidValue;
-    switch (W) {
-        case 1: e = prepare_w<1>(); break;
-        case 2: e = prepare_w<2>(); break;
-        case 4: e = prepare_w<4>(); break;
-        case 8: e = prepare_w<8>(); break;
-        default: break;
-    }
-    if (e == cudaSuccess) done[W] = true;
-    return e;
-}
-
-uint32_t direct_pods_per_cta(uint32_t W) {
-    switch (W) {
-        case 1: return (DIRECT_THREADS / 32) * PodsPerWarp<1>::v;
-        case 2: return (DIRECT_THREADS / 32) * PodsPerWarp<2>::v;
-        case 4: return (DIRECT_THREADS / 32) * PodsPerWarp<4>::v;
-        default: return (DIRECT_THREADS / 32) * PodsPerWarp<8>::v;
-    }
-}
-
-cudaError_t launch_select_direct(const SelectLaunch& L, const PartialView& part, uint32_t n_chunks,
-                                 uint32_t tiles_per_chunk) {
-    switch (L.nt.W) {
-        case 1: return launch_direct_w<1>(L, part, n_chunks, tiles_per_chunk);
-        case 2: return launch_direct_w<2>(L, part, n_chunks, tiles_per_chunk);
-        case 4: return launch_direct_w<4>(L, part, n_chunks, tiles_per_chunk);
-        case 8: return launch_direct_w<8>(L, part, n_chunks, tiles_per_chunk);
-        default: return cudaErrorInvalidValue;
-    }
-}
-
-// ------------------------------------------------------------------------------------------------ K2e
-// Per-pod rejection counts (ks_explain): K2d's tile staging and pod-per-warp layout, three ballots per 32 nodes
-// instead of one.  Counts of one CTA row are warp-uniform; with gridDim.y > 1 the node chunks add into a zeroed
-// output, and integer adds make the result independent of their order.
+// Per-pod rejection counts (ks_explain): three ballots per 32 nodes.  Counts of one CTA row are warp-uniform; with
+// gridDim.y > 1 the node chunks add into a zeroed output, and integer adds make the result independent of their order.
 template <int W>
 __global__ void __launch_bounds__(DIRECT_THREADS)
     k_explain_counts(NodeTable nt, PodView pv, uint32_t* __restrict__ out, uint32_t tiles_per_chunk) {
-    constexpr int PW = PodsPerWarp<W>::v;
-    constexpr uint32_t STAGE_BYTES = (2u + W) * TILE_N * 8u;
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[2];
-
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t n_tiles_total = nt.Npad / TILE_N;
-    const uint32_t tile_begin = blockIdx.y * tiles_per_chunk;
-    const uint32_t tile_end = min(tile_begin + tiles_per_chunk, n_tiles_total);
-
-    if (threadIdx.x == 0) {
-        mbar_init(&full_bar[0], 1);
-        mbar_init(&full_bar[1], 1);
-        fence_mbar_init();
-    }
-    __syncthreads();
-
-    auto issue_tile = [&](uint32_t tile, uint32_t stage) {
-        unsigned char* dst = smem_raw + (size_t)stage * STAGE_BYTES;
-        uint64_t* bar = &full_bar[stage];
-        mbar_arrive_expect_tx(bar, STAGE_BYTES);
-        const size_t off = (size_t)tile * TILE_N;
-        tma_bulk_g2s(dst, nt.free_cpu + off, TILE_N * 8, bar);
-        tma_bulk_g2s(dst + TILE_N * 8, nt.free_mem + off, TILE_N * 8, bar);
-#pragma unroll
-        for (int w = 0; w < W; w++)
-            tma_bulk_g2s(dst + (2 + w) * TILE_N * 8, nt.labels + (size_t)w * nt.Npad + off, TILE_N * 8, bar);
-    };
-
-    if (threadIdx.x == 0 && tile_begin < tile_end) issue_tile(tile_begin, 0);
-
-    const uint32_t p0 = (blockIdx.x * (DIRECT_THREADS / 32) + warp) * PW;
+    constexpr int PW = pods_per_warp(W);
     int64_t rc[PW], rm[PW];
     uint64_t sel[PW][W];
+    uint32_t p0;
     uint32_t n_cpu[PW], n_mem[PW], n_res[PW], n_sel[PW];
 #pragma unroll
-    for (int i = 0; i < PW; i++) {
-        uint32_t p = min(p0 + i, pv.P - 1);
-        rc[i] = __ldg(pv.req_cpu + p);
-        rm[i] = __ldg(pv.req_mem + p);
-#pragma unroll
-        for (int w = 0; w < W; w++) sel[i][w] = __ldg(pv.sel + (uint64_t)p * W + w);
-        n_cpu[i] = n_mem[i] = n_res[i] = n_sel[i] = 0;
-    }
+    for (int i = 0; i < PW; i++) n_cpu[i] = n_mem[i] = n_res[i] = n_sel[i] = 0;
 
-    for (uint32_t tile = tile_begin; tile < tile_end; tile++) {
-        const uint32_t it = tile - tile_begin, stage = it & 1;
-        if (threadIdx.x == 0 && tile + 1 < tile_end) issue_tile(tile + 1, stage ^ 1);
-        mbar_wait(&full_bar[stage], (it >> 1) & 1);
-
-        const unsigned char* base = smem_raw + (size_t)stage * STAGE_BYTES;
-        const int64_t* s_fc = reinterpret_cast<const int64_t*>(base);
-        const int64_t* s_fm = s_fc + TILE_N;
-        const uint64_t* s_lab = reinterpret_cast<const uint64_t*>(s_fm + TILE_N);
-
-#pragma unroll 2
-        for (uint32_t g = 0; g < 32; g++) {
-            const uint32_t ln = g * 32 + lane;
-            const int64_t fc = s_fc[ln], fm = s_fm[ln];
-            uint64_t lab[W];
-#pragma unroll
-            for (int w = 0; w < W; w++) lab[w] = s_lab[w * TILE_N + ln];
-            const bool real = tile * TILE_N + ln < nt.N; // padding sentinels never count
+    scan_node_tiles<W, false>(
+        nt, tiles_per_chunk, pv, p0, rc, rm, sel,
+        [&](uint32_t, uint32_t, bool real, int64_t fc, int64_t fm, const uint64_t(&lab)[W], int64_t, int64_t) {
 #pragma unroll
             for (int i = 0; i < PW; i++) {
                 const bool cpu_fail = real && rc[i] > fc; // predicates.rs:42, each half
@@ -594,11 +458,10 @@ __global__ void __launch_bounds__(DIRECT_THREADS)
                 n_res[i] += __popc(bc | bm);
                 n_sel[i] += __popc(bs);
             }
-        }
-        __syncthreads(); // everyone is done with `stage` before it is refilled two iterations later
-    }
+        },
+        [](uint32_t) {});
 
-    if (lane == 0) { // the counts are warp-uniform
+    if ((threadIdx.x & 31) == 0) { // the counts are warp-uniform
 #pragma unroll
         for (int i = 0; i < PW; i++) {
             if (p0 + i >= pv.P) continue;
@@ -618,42 +481,79 @@ __global__ void __launch_bounds__(DIRECT_THREADS)
     }
 }
 
-template <int W>
-static cudaError_t launch_explain_w(const NodeTable& nt, const PodView& pv, uint32_t* out, int sms, cudaStream_t st) {
-    constexpr uint32_t SMEM = 2u * (2u + W) * TILE_N * 8u;
-    static bool prepared = false; // opt-in shared memory size, once per label width
-    if (!prepared) {
-        cudaError_t e = cudaFuncSetAttribute(k_explain_counts<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
-        if (e != cudaSuccess) return e;
-        prepared = true;
-    }
-    // node chunks across gridDim.y when the pods alone give fewer than two CTAs per SM (same rule as ks_select)
-    const uint32_t pods_per_cta = (DIRECT_THREADS / 32) * PodsPerWarp<W>::v;
-    const uint32_t n_tiles = nt.Npad / TILE_N;
-    const uint32_t pod_ctas = (pv.P + pods_per_cta - 1) / pods_per_cta;
+// node chunks across gridDim.y when the pods alone give fewer than two CTAs per SM
+DirectGrid direct_grid(uint32_t W, uint32_t P, uint32_t Npad, int sms) {
+    const uint32_t pods_per_cta = (DIRECT_THREADS / 32) * pods_per_warp(W);
+    const uint32_t n_tiles = Npad / TILE_N;
     const uint32_t want_ctas = 2u * (uint32_t)sms;
-    uint32_t n_chunks = 1;
-    if (pod_ctas < want_ctas) n_chunks = std::min<uint32_t>(n_tiles, (want_ctas + pod_ctas - 1) / pod_ctas);
-    const uint32_t tiles_per_chunk = (n_tiles + n_chunks - 1) / n_chunks;
-    n_chunks = (n_tiles + tiles_per_chunk - 1) / tiles_per_chunk;
-    if (n_chunks > 1) {
-        cudaError_t e = cudaMemsetAsync(out, 0, (size_t)pv.P * 16, st);
-        if (e != cudaSuccess) return e;
-    }
-    k_explain_counts<W><<<dim3(pod_ctas, n_chunks), DIRECT_THREADS, SMEM, st>>>(nt, pv, out, tiles_per_chunk);
+    DirectGrid g;
+    g.pod_ctas = (P + pods_per_cta - 1) / pods_per_cta;
+    g.n_chunks = 1;
+    if (g.pod_ctas < want_ctas) g.n_chunks = std::min<uint32_t>(n_tiles, (want_ctas + g.pod_ctas - 1) / g.pod_ctas);
+    g.tiles_per_chunk = (n_tiles + g.n_chunks - 1) / g.n_chunks;
+    g.n_chunks = (n_tiles + g.tiles_per_chunk - 1) / g.tiles_per_chunk;
+    return g;
+}
+
+// opt-in shared memory sizes of every K2d / K2e kernel on the current device (must not run inside a stream capture)
+cudaError_t prepare_direct() {
+    cudaError_t e = cudaSuccess;
+    auto opt_in = [&e](auto kern, uint32_t bytes) {
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    };
+    for (uint32_t W : {1u, 2u, 4u, 8u})
+        with_label_width(W, [&](auto w) {
+            constexpr int W_ = decltype(w)::value;
+            constexpr int LO = KS_SCORE_LEFTOVER, LA = KS_SCORE_LEAST_ALLOCATED;
+            opt_in(k_select_direct<W_, LO, true>, tile_smem_bytes<W_, false>());
+            opt_in(k_select_direct<W_, LO, false>, tile_smem_bytes<W_, false>());
+            opt_in(k_select_direct<W_, LA, true>, tile_smem_bytes<W_, true>());
+            opt_in(k_select_direct<W_, LA, false>, tile_smem_bytes<W_, true>());
+            opt_in(k_explain_counts<W_>, tile_smem_bytes<W_, false>());
+            return e;
+        });
+    return e;
+}
+
+template <int W, int POLICY, bool EMIT>
+static cudaError_t launch_direct_t(const SelectLaunch& L, const PartialView& part, const DirectGrid& g) {
+    constexpr uint32_t SMEM = tile_smem_bytes<W, POLICY == KS_SCORE_LEAST_ALLOCATED>();
+    k_select_direct<W, POLICY, EMIT><<<dim3(g.pod_ctas, g.n_chunks), DIRECT_THREADS, SMEM, L.stream>>>(
+        L.nt, L.pv, L.ov, part, g.tiles_per_chunk);
+    g_launches++;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess || g.n_chunks == 1) return e;
+    k_select_combine<POLICY><<<(L.pv.P + 255) / 256, 256, 0, L.stream>>>(L.pv, L.ov, part, g.n_chunks);
     g_launches++;
     return cudaGetLastError();
 }
 
+cudaError_t launch_select_direct(const SelectLaunch& L, const PartialView& part, const DirectGrid& g) {
+    return with_label_width(L.nt.W, [&](auto w) {
+        constexpr int W = decltype(w)::value;
+        const bool emit = L.ov.mask != nullptr;
+        if (L.policy == KS_SCORE_LEFTOVER)
+            return emit ? launch_direct_t<W, KS_SCORE_LEFTOVER, true>(L, part, g)
+                        : launch_direct_t<W, KS_SCORE_LEFTOVER, false>(L, part, g);
+        return emit ? launch_direct_t<W, KS_SCORE_LEAST_ALLOCATED, true>(L, part, g)
+                    : launch_direct_t<W, KS_SCORE_LEAST_ALLOCATED, false>(L, part, g);
+    });
+}
+
 cudaError_t launch_explain_counts(const NodeTable& nt, const PodView& pv, uint32_t* out, int sms, cudaStream_t st) {
     if (pv.P == 0 || nt.Npad == 0) return cudaSuccess;
-    switch (nt.W) {
-        case 1: return launch_explain_w<1>(nt, pv, out, sms, st);
-        case 2: return launch_explain_w<2>(nt, pv, out, sms, st);
-        case 4: return launch_explain_w<4>(nt, pv, out, sms, st);
-        case 8: return launch_explain_w<8>(nt, pv, out, sms, st);
-        default: return cudaErrorInvalidValue;
-    }
+    return with_label_width(nt.W, [&](auto w) {
+        constexpr int W = decltype(w)::value;
+        const DirectGrid g = direct_grid(W, pv.P, nt.Npad, sms);
+        if (g.n_chunks > 1) {
+            const cudaError_t e = cudaMemsetAsync(out, 0, (size_t)pv.P * 16, st);
+            if (e != cudaSuccess) return e;
+        }
+        k_explain_counts<W><<<dim3(g.pod_ctas, g.n_chunks), DIRECT_THREADS, tile_smem_bytes<W, false>(), st>>>(
+            nt, pv, out, g.tiles_per_chunk);
+        g_launches++;
+        return cudaGetLastError();
+    });
 }
 
 } // namespace ks

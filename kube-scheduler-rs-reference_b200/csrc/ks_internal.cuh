@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include <atomic>
+#include <type_traits>
 
 #include "../../include/ksched.h"
 
@@ -93,6 +94,56 @@ struct PartialView {
 };
 
 extern std::atomic<uint64_t> g_launches;
+
+// ---- scores and the tie rule: one definition for every argmax path ----
+// KS_SCORE_LEFTOVER: score = (free_cpu - rc) * 2^22 + (free_mem - rm) = node key - pod key.  The node key alone orders
+// the nodes for a fixed pod; the range limits of ksched.h keep both keys and their difference inside int64.
+__device__ __forceinline__ int64_t leftover_key(int64_t cpu, int64_t mem) {
+    return (int64_t)(((uint64_t)cpu << 22) + (uint64_t)mem);
+}
+__device__ __forceinline__ int64_t leftover_score(int64_t node_key, int64_t rc, int64_t rm) {
+    return node_key - leftover_key(rc, rm);
+}
+// KS_SCORE_LEAST_ALLOCATED in exact integer arithmetic: the mean of the truncated percentages left free after placement
+__device__ __forceinline__ int64_t least_alloc_int(int64_t fc, int64_t fm, int64_t ac, int64_t am, int64_t rc, int64_t rm) {
+    const int64_t pc = ac > 0 ? ((fc - rc) * 100) / ac : 0;
+    const int64_t pm = am > 0 ? ((fm - rm) * 100) / am : 0;
+    return (pc + pm) / 2;
+}
+// Warp argmax over (key, idx) with idx < 0 for "no candidate": larger key wins, ties go to the lower node index.
+// Every lane ends with the result.
+__device__ __forceinline__ void warp_argmax(int64_t& key, int32_t& idx) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        const int64_t ok = __shfl_xor_sync(0xffffffffu, key, off);
+        const int32_t oi = __shfl_xor_sync(0xffffffffu, idx, off);
+        const bool take = oi >= 0 && (idx < 0 || ok > key || (ok == key && oi < idx));
+        if (take) {
+            key = ok;
+            idx = oi;
+        }
+    }
+}
+// Ordered merge of partial results over disjoint node ranges: fed in ascending range order, the strict '>' keeps the
+// lower node index on ties.
+__device__ __forceinline__ void merge_partial(int64_t& key, int32_t& idx, int64_t ok, int32_t oi) {
+    if (oi >= 0 && (idx < 0 || ok > key)) {
+        key = ok;
+        idx = oi;
+    }
+}
+
+// Label-width dispatch: calls f(std::integral_constant<int, W>{}) for W in {1, 2, 4, 8}; any other W is invalid.
+template <class F>
+cudaError_t with_label_width(uint32_t W, F&& f) {
+    switch (W) {
+        case 1: return f(std::integral_constant<int, 1>{});
+        case 2: return f(std::integral_constant<int, 2>{});
+        case 4: return f(std::integral_constant<int, 4>{});
+        case 8: return f(std::integral_constant<int, 8>{});
+        default: return cudaErrorInvalidValue;
+    }
+}
 
 // ---- PTX helpers: mbarrier + 1-D TMA bulk copy (cp.async.bulk -> SASS UBLKCP) ----
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {

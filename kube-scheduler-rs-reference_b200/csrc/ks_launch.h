@@ -17,10 +17,14 @@ cudaError_t launch_select_sampling(const NodeTable& nt, const PodView& pv, uint3
 cudaError_t launch_exchange_push(const PeerOut& po, const int32_t* node_idx, const int64_t* score, uint32_t P, cudaStream_t st);
 cudaError_t launch_exchange_wait(const PeerOut& po, int* error_flag, cudaStream_t st);
 cudaError_t launch_fill256(void* dst, uint64_t bytes, uint32_t v, int sms, cudaStream_t st);
-uint32_t direct_pods_per_cta(uint32_t W);
-cudaError_t prepare_select_direct(uint32_t W);
-cudaError_t launch_select_direct(const SelectLaunch& L, const PartialView& part, uint32_t n_chunks,
-                                 uint32_t tiles_per_chunk);
+// launch geometry of the per-cell kernels (K2d, K2e) for P > 0 pods and Npad > 0 nodes: CTAs over the pods times node
+// chunks over gridDim.y; n_chunks > 1 needs partial buffers of n_chunks * P entries (K2d)
+struct DirectGrid {
+    uint32_t pod_ctas, n_chunks, tiles_per_chunk;
+};
+DirectGrid direct_grid(uint32_t W, uint32_t P, uint32_t Npad, int sms);
+cudaError_t prepare_direct(); // once per snapshot, outside any stream capture
+cudaError_t launch_select_direct(const SelectLaunch& L, const PartialView& part, const DirectGrid& g);
 // per-pod rejection counts (ks_explain): out = uint32 [P][4] in ks_pod_reasons order, device memory
 cudaError_t launch_explain_counts(const NodeTable& nt, const PodView& pv, uint32_t* out, int sms, cudaStream_t st);
 

@@ -11,29 +11,30 @@ namespace ks {
 
 constexpr int STREAM_MAX = 4096; // claims per launch (one CTA sorts them in shared memory)
 
-// One CTA.  (1) bitonic sort of (node, arrival) keys in shared memory; (2) one thread per node segment walks
-// its claimants in arrival order: accept iff the request still fits, then decrement free[] (single writer
-// per node: no atomics, deterministic).
-__global__ void __launch_bounds__(1024)
-    k_stream_resolve(int64_t* __restrict__ free_cpu, int64_t* __restrict__ free_mem, const int32_t* __restrict__ claim_node,
-                     const int64_t* __restrict__ req_cpu, const int64_t* __restrict__ req_mem, uint32_t n, uint32_t N,
-                     uint8_t* __restrict__ accepted) {
-    __shared__ unsigned long long key[STREAM_MAX];
+// The capacity commit of a batch of n claims, by one CTA of THREADS threads: (1) bitonic sort of (node, arrival) keys
+// in key[] (room for n rounded up to a power of two); (2) one thread per node segment walks its claimants in arrival
+// order: accept iff the request still fits, then decrement free[] (single writer per node: no atomics,
+// deterministic).  node_of(i) is claim i's node or -1 for none, request(i, rc, rm) reads its request and
+// accept(i, ok) records the verdict; a claim without a node is rejected without a walk.  free[] is read through L2
+// (__ldcg): inside the cooperative kernel other CTAs read it and this CTA wrote it in earlier rounds.
+template <uint32_t THREADS, class NodeOf, class Request, class Accept>
+__device__ __forceinline__ void commit_claims(unsigned long long* key, uint32_t n, int64_t* free_cpu, int64_t* free_mem,
+                                              NodeOf&& node_of, Request&& request, Accept&& accept) {
     uint32_t m = 1;
     while (m < n) m <<= 1;
-    for (uint32_t i = threadIdx.x; i < m; i += blockDim.x) {
+    for (uint32_t i = threadIdx.x; i < m; i += THREADS) {
         unsigned long long k = ~0ull; // padding and "no claim" sort last
         if (i < n) {
-            const int32_t nd = claim_node[i];
-            if (nd >= 0 && (uint32_t)nd < N) k = ((unsigned long long)(uint32_t)nd << 32) | i;
-            else accepted[i] = 0;
+            const int32_t nd = node_of(i);
+            if (nd >= 0) k = ((unsigned long long)(uint32_t)nd << 32) | i;
+            else accept(i, false);
         }
         key[i] = k;
     }
     __syncthreads();
     for (uint32_t size = 2; size <= m; size <<= 1) {
         for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
-            for (uint32_t i = threadIdx.x; i < m / 2; i += blockDim.x) {
+            for (uint32_t i = threadIdx.x; i < m / 2; i += THREADS) {
                 const uint32_t lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
                 const bool up = (lo & size) == 0;
                 const unsigned long long a = key[lo], b = key[hi];
@@ -45,17 +46,18 @@ __global__ void __launch_bounds__(1024)
             __syncthreads();
         }
     }
-    for (uint32_t i = threadIdx.x; i < m; i += blockDim.x) {
+    for (uint32_t i = threadIdx.x; i < m; i += THREADS) {
         const unsigned long long k = key[i];
         if (k == ~0ull) continue;
         const uint32_t node = (uint32_t)(k >> 32);
         if (i > 0 && (uint32_t)(key[i - 1] >> 32) == node) continue; // not a segment head
-        int64_t fc = free_cpu[node], fm = free_mem[node];
-        for (uint32_t j = i; j < m && (uint32_t)(key[j] >> 32) == node && key[j] != ~0ull; j++) {
+        int64_t fc = __ldcg(free_cpu + node), fm = __ldcg(free_mem + node);
+        for (uint32_t j = i; j < m && key[j] != ~0ull && (uint32_t)(key[j] >> 32) == node; j++) {
             const uint32_t c = (uint32_t)key[j];
-            const int64_t rc = req_cpu[c], rm = req_mem[c];
+            int64_t rc, rm;
+            request(c, rc, rm);
             const bool ok = rc <= fc && rm <= fm; // predicates.rs:42 against what is left
-            accepted[c] = ok;
+            accept(c, ok);
             if (ok) { // util.rs:31-36
                 fc -= rc;
                 fm -= rm;
@@ -64,6 +66,24 @@ __global__ void __launch_bounds__(1024)
         free_cpu[node] = fc;
         free_mem[node] = fm;
     }
+}
+
+__global__ void __launch_bounds__(1024)
+    k_stream_resolve(int64_t* __restrict__ free_cpu, int64_t* __restrict__ free_mem, const int32_t* __restrict__ claim_node,
+                     const int64_t* __restrict__ req_cpu, const int64_t* __restrict__ req_mem, uint32_t n, uint32_t N,
+                     uint8_t* __restrict__ accepted) {
+    __shared__ unsigned long long key[STREAM_MAX];
+    commit_claims<1024>(
+        key, n, free_cpu, free_mem,
+        [&](uint32_t i) {
+            const int32_t nd = claim_node[i];
+            return nd >= 0 && (uint32_t)nd < N ? nd : -1;
+        },
+        [&](uint32_t c, int64_t& rc, int64_t& rm) {
+            rc = req_cpu[c];
+            rm = req_mem[c];
+        },
+        [&](uint32_t c, bool ok) { accepted[c] = ok; });
 }
 
 cudaError_t launch_stream_resolve(int64_t* free_cpu, int64_t* free_mem, const int32_t* claim_node, const int64_t* req_cpu,
@@ -83,18 +103,14 @@ uint32_t stream_max_claims() { return STREAM_MAX; }
 //   A  every CTA scans its slice of the node table for every pending pod (one warp per pod, lanes over nodes):
 //      feasible (predicates.rs:42,45-61) -> policy key -> warp argmax (ties -> lowest node index) -> partial[pod][cta]
 //   B  CTA 0 reduces the partials to one claim per pod, resolves the claims per node in arrival order against what
-//      is left (same walk as k_stream_resolve), commits the accepted requests to free[], writes the bindings and
-//      compacts the losers (order preserved) into the next round's pending list
-// separated by grid-wide barriers.  Batches of up to STREAM_BATCH_MAX pods.
+//      is left (commit_claims, as k_stream_resolve), writes the bindings and compacts the losers (order preserved)
+//      into the next round's pending list
+// separated by grid-wide barriers.  Batches of up to STREAM_BATCH_MAX pods.  The pods' requests, selectors and the
+// node table are read-only here (__ldg); free[] changes between rounds and is read through L2 (__ldcg).
 constexpr uint32_t SB_THREADS = 256;
 
 template <int W>
-__global__ void __launch_bounds__(SB_THREADS)
-    k_stream_batch(uint32_t N, uint32_t Npad, const int64_t* __restrict__ alloc_cpu, const int64_t* __restrict__ alloc_mem,
-                   const uint64_t* __restrict__ labels, int64_t* free_cpu, int64_t* free_mem, int policy, uint32_t m,
-                   const int64_t* __restrict__ req_cpu, const int64_t* __restrict__ req_mem, const uint64_t* __restrict__ sel,
-                   int64_t* pkey, int32_t* pidx, uint32_t* pend, uint32_t* ctl, int32_t* out_idx, int64_t* out_score,
-                   uint32_t max_rounds) {
+__global__ void __launch_bounds__(SB_THREADS) k_stream_batch(const StreamBatchArgs a) {
     cg::grid_group grid = cg::this_grid();
     __shared__ unsigned long long s_key[STREAM_BATCH_MAX];
     __shared__ int64_t s_ckey[STREAM_BATCH_MAX];
@@ -102,67 +118,53 @@ __global__ void __launch_bounds__(SB_THREADS)
     __shared__ uint8_t s_acc[STREAM_BATCH_MAX];
     __shared__ uint32_t s_scan[SB_THREADS];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, G = gridDim.x;
-    const uint32_t chunk = (N + G - 1) / G, n0 = min(N, blockIdx.x * chunk), n1 = min(N, n0 + chunk);
+    const uint32_t chunk = (a.N + G - 1) / G, n0 = min(a.N, blockIdx.x * chunk), n1 = min(a.N, n0 + chunk);
     if (blockIdx.x == 0) {
-        for (uint32_t i = tid; i < m; i += SB_THREADS) {
-            pend[i] = i;
-            out_idx[i] = -1; // NoNodeFound until bound (src/main.rs:116-118)
-            out_score[i] = 0;
+        for (uint32_t i = tid; i < a.m; i += SB_THREADS) {
+            a.pend[i] = i;
+            a.out_idx[i] = -1; // NoNodeFound until bound (src/main.rs:116-118)
+            a.out_score[i] = 0;
         }
         if (tid == 0) {
-            ctl[0] = m;
-            ctl[1] = 0;
+            a.ctl[0] = a.m;
+            a.ctl[1] = 0;
         }
         __threadfence();
     }
     grid.sync();
     uint32_t cur = 0;
     for (uint32_t round = 0;; round++) {
-        const uint32_t cnt = *reinterpret_cast<volatile uint32_t*>(ctl);
-        if (cnt == 0 || round > max_rounds) break; // grid-uniform
-        const uint32_t* pl = pend + cur * STREAM_BATCH_MAX;
+        const uint32_t cnt = *reinterpret_cast<volatile uint32_t*>(a.ctl);
+        if (cnt == 0 || round > a.max_rounds) break; // grid-uniform
+        const uint32_t* pl = a.pend + cur * STREAM_BATCH_MAX;
         // ---- A: partial argmax over this CTA's node slice ----
         for (uint32_t k = warp; k < cnt; k += SB_THREADS / 32) {
             const uint32_t p = __ldcg(pl + k);
-            const int64_t rc = req_cpu[p], rm = req_mem[p];
+            const int64_t rc = __ldg(a.req_cpu + p), rm = __ldg(a.req_mem + p);
             uint64_t sw[W];
 #pragma unroll
-            for (int w = 0; w < W; w++) sw[w] = sel[(size_t)p * W + w];
+            for (int w = 0; w < W; w++) sw[w] = __ldg(a.sel + (size_t)p * W + w);
             int64_t best = INT64_MIN;
             int32_t bidx = -1;
             for (uint32_t n = n0 + lane; n < n1; n += 32) {
-                const int64_t fc = __ldcg(free_cpu + n), fm = __ldcg(free_mem + n); // free[] changes between rounds
+                const int64_t fc = __ldcg(a.free_cpu + n), fm = __ldcg(a.free_mem + n);
                 uint64_t miss = 0;
 #pragma unroll
-                for (int w = 0; w < W; w++) miss |= sw[w] & ~labels[(size_t)w * Npad + n];
+                for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
                 if (rc <= fc && rm <= fm && miss == 0) {
-                    int64_t key;
-                    if (policy == KS_SCORE_LEFTOVER) {
-                        key = (int64_t)(((uint64_t)fc << 22) + (uint64_t)fm);
-                    } else {
-                        const int64_t ac = alloc_cpu[n], am = alloc_mem[n];
-                        const int64_t pc = ac > 0 ? ((fc - rc) * 100) / ac : 0;
-                        const int64_t pm = am > 0 ? ((fm - rm) * 100) / am : 0;
-                        key = (pc + pm) / 2;
-                    }
+                    const int64_t key = a.policy == KS_SCORE_LEFTOVER
+                                            ? leftover_key(fc, fm)
+                                            : least_alloc_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm);
                     if (key > best) { // ascending n per lane: strict '>' keeps the lowest index
                         best = key;
                         bidx = (int32_t)n;
                     }
                 }
             }
-#pragma unroll
-            for (int off = 16; off > 0; off >>= 1) {
-                const int64_t ok_ = __shfl_xor_sync(0xffffffffu, best, off);
-                const int32_t oi = __shfl_xor_sync(0xffffffffu, bidx, off);
-                if (oi >= 0 && (bidx < 0 || ok_ > best || (ok_ == best && oi < bidx))) {
-                    best = ok_;
-                    bidx = oi;
-                }
-            }
+            warp_argmax(best, bidx);
             if (lane == 0) {
-                pkey[(size_t)k * G + blockIdx.x] = best;
-                pidx[(size_t)k * G + blockIdx.x] = bidx;
+                a.pkey[(size_t)k * G + blockIdx.x] = best;
+                a.pidx[(size_t)k * G + blockIdx.x] = bidx;
             }
         }
         __threadfence();
@@ -172,77 +174,27 @@ __global__ void __launch_bounds__(SB_THREADS)
             for (uint32_t k = warp; k < cnt; k += SB_THREADS / 32) {
                 int64_t best = INT64_MIN;
                 int32_t bidx = -1;
-                for (uint32_t c = lane; c < G; c += 32) { // ascending CTA = ascending node range
-                    const int64_t ok_ = __ldcg(pkey + (size_t)k * G + c);
-                    const int32_t oi = __ldcg(pidx + (size_t)k * G + c);
-                    if (oi >= 0 && (bidx < 0 || ok_ > best)) {
-                        best = ok_;
-                        bidx = oi;
-                    }
-                }
-#pragma unroll
-                for (int off = 16; off > 0; off >>= 1) {
-                    const int64_t ok_ = __shfl_xor_sync(0xffffffffu, best, off);
-                    const int32_t oi = __shfl_xor_sync(0xffffffffu, bidx, off);
-                    if (oi >= 0 && (bidx < 0 || ok_ > best || (ok_ == best && oi < bidx))) {
-                        best = ok_;
-                        bidx = oi;
-                    }
-                }
+                for (uint32_t c = lane; c < G; c += 32) // ascending CTA = ascending node range
+                    merge_partial(best, bidx, __ldcg(a.pkey + (size_t)k * G + c), __ldcg(a.pidx + (size_t)k * G + c));
+                warp_argmax(best, bidx);
                 if (lane == 0) {
                     s_claim[k] = bidx;
                     s_ckey[k] = best;
                 }
             }
             __syncthreads();
-            // claims per node in arrival (batch) order: sort (node, k), one thread per node segment walks it
-            uint32_t m2 = 1;
-            while (m2 < cnt) m2 <<= 1;
-            for (uint32_t i = tid; i < m2; i += SB_THREADS) {
-                unsigned long long key = ~0ull;
-                if (i < cnt) {
-                    s_acc[i] = 0;
-                    if (s_claim[i] >= 0) key = ((unsigned long long)(uint32_t)s_claim[i] << 32) | i;
-                }
-                s_key[i] = key;
-            }
-            __syncthreads();
-            for (uint32_t size = 2; size <= m2; size <<= 1)
-                for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
-                    for (uint32_t i = tid; i < m2 / 2; i += SB_THREADS) {
-                        const uint32_t lo = 2 * i - (i & (stride - 1)), hi = lo + stride;
-                        const bool up = (lo & size) == 0;
-                        const unsigned long long a = s_key[lo], b = s_key[hi];
-                        if ((a > b) == up) {
-                            s_key[lo] = b;
-                            s_key[hi] = a;
-                        }
-                    }
-                    __syncthreads();
-                }
-            for (uint32_t i = tid; i < m2; i += SB_THREADS) {
-                const unsigned long long key = s_key[i];
-                if (key == ~0ull) continue;
-                const uint32_t node = (uint32_t)(key >> 32);
-                if (i > 0 && (uint32_t)(s_key[i - 1] >> 32) == node) continue; // not a segment head
-                int64_t fc = __ldcg(free_cpu + node), fm = __ldcg(free_mem + node);
-                for (uint32_t j = i; j < m2 && s_key[j] != ~0ull && (uint32_t)(s_key[j] >> 32) == node; j++) {
-                    const uint32_t k = (uint32_t)s_key[j];
+            // claims per node in arrival (batch) order
+            commit_claims<SB_THREADS>(
+                s_key, cnt, a.free_cpu, a.free_mem, [&](uint32_t k) { return s_claim[k]; },
+                [&](uint32_t k, int64_t& rc, int64_t& rm) {
                     const uint32_t p = __ldcg(pl + k);
-                    const int64_t rc = req_cpu[p], rm = req_mem[p];
-                    const bool ok = rc <= fc && rm <= fm; // predicates.rs:42 against what is left
-                    s_acc[k] = ok;
-                    if (ok) { // util.rs:31-36
-                        fc -= rc;
-                        fm -= rm;
-                    }
-                }
-                free_cpu[node] = fc;
-                free_mem[node] = fm;
-            }
+                    rc = __ldg(a.req_cpu + p);
+                    rm = __ldg(a.req_mem + p);
+                },
+                [&](uint32_t k, bool ok) { s_acc[k] = ok; });
             __syncthreads();
             // bindings of the winners; losers keep their order in the next pending list
-            uint32_t* nl = pend + (cur ^ 1u) * STREAM_BATCH_MAX;
+            uint32_t* nl = a.pend + (cur ^ 1u) * STREAM_BATCH_MAX;
             constexpr uint32_t PER = STREAM_BATCH_MAX / SB_THREADS;
             uint32_t loser[PER], n_loser = 0;
 #pragma unroll
@@ -252,10 +204,10 @@ __global__ void __launch_bounds__(SB_THREADS)
                 if (k < cnt && s_claim[k] >= 0) {
                     const uint32_t p = __ldcg(pl + k);
                     if (s_acc[k]) {
-                        out_idx[p] = s_claim[k];
-                        out_score[p] = policy == KS_SCORE_LEFTOVER
-                                           ? s_ckey[k] - (int64_t)(((uint64_t)req_cpu[p] << 22) + (uint64_t)req_mem[p])
-                                           : s_ckey[k];
+                        a.out_idx[p] = s_claim[k];
+                        a.out_score[p] = a.policy == KS_SCORE_LEFTOVER
+                                             ? leftover_score(s_ckey[k], __ldg(a.req_cpu + p), __ldg(a.req_mem + p))
+                                             : s_ckey[k];
                     } else {
                         loser[e] = 1;
                         n_loser++;
@@ -275,8 +227,8 @@ __global__ void __launch_bounds__(SB_THREADS)
             for (uint32_t e = 0; e < PER; e++)
                 if (loser[e]) nl[pos++] = __ldcg(pl + tid * PER + e);
             if (tid == SB_THREADS - 1) {
-                ctl[0] = s_scan[tid];
-                ctl[1] = round + 1;
+                a.ctl[0] = s_scan[tid];
+                a.ctl[1] = round + 1;
             }
             __threadfence();
         }
@@ -285,24 +237,15 @@ __global__ void __launch_bounds__(SB_THREADS)
     }
 }
 
-template <int W>
-static cudaError_t launch_stream_batch_w(const StreamBatchArgs& a, cudaStream_t st) {
-    StreamBatchArgs b = a;
-    void* args[] = {&b.N,   &b.Npad, &b.alloc_cpu, &b.alloc_mem, &b.labels, &b.free_cpu, &b.free_mem, &b.policy,    &b.m,         &b.req_cpu,
-                    &b.req_mem, &b.sel,  &b.pkey,      &b.pidx,      &b.pend,   &b.ctl,      &b.out_idx,  &b.out_score, &b.max_rounds};
-    cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(k_stream_batch<W>), dim3(a.grid), dim3(SB_THREADS), args, 0, st);
-    if (e == cudaSuccess) g_launches++;
-    return e;
-}
-
 cudaError_t launch_stream_batch(const StreamBatchArgs& a, uint32_t W, cudaStream_t st) {
-    switch (W) {
-        case 1: return launch_stream_batch_w<1>(a, st);
-        case 2: return launch_stream_batch_w<2>(a, st);
-        case 4: return launch_stream_batch_w<4>(a, st);
-        case 8: return launch_stream_batch_w<8>(a, st);
-        default: return cudaErrorInvalidValue;
-    }
+    return with_label_width(W, [&](auto w) {
+        StreamBatchArgs b = a;
+        void* args[] = {&b};
+        const cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(k_stream_batch<decltype(w)::value>),
+                                                          dim3(a.grid), dim3(SB_THREADS), args, 0, st);
+        if (e == cudaSuccess) g_launches++;
+        return e;
+    });
 }
 
 } // namespace ks
