@@ -127,6 +127,25 @@ impl Gpu {
         Some(unsafe { CStr::from_ptr(ksh_context_node_name(self.ctx, idx as u32)) }.to_string_lossy().into_owned())
     }
 
+    /// Up to `k` (1..=KS_TOPK_MAX) feasible nodes for the pod, best first: (node name, score) under the leftover score.
+    /// The first is what `select_node_for_pod` picks; the rest are the fall-backs to try when its Binding POST fails.
+    /// Nothing is charged: report the bind that succeeded with `ksh_context_pod_bound`.  Err = the library's status.
+    pub fn rank_nodes(&self, pod: &corev1::Pod, k: u32) -> Result<Vec<(String, i64)>, i32> {
+        let v = PodView::new(pod);
+        let mut idx = vec![-1i32; k as usize];
+        let mut score = vec![0i64; k as usize];
+        let rc = unsafe {
+            ksh_rank_nodes(self.ctx, &v.obj, 1, KS_SCORE_LEFTOVER, k, idx.as_mut_ptr(), score.as_mut_ptr(), ptr::null_mut())
+        };
+        if rc != KS_OK {
+            return Err(rc);
+        }
+        Ok(idx.iter().zip(score.iter()).take_while(|(i, _)| **i >= 0).map(|(i, s)| {
+            let name = unsafe { CStr::from_ptr(ksh_context_node_name(self.ctx, *i as u32)) }.to_string_lossy().into_owned();
+            (name, *s)
+        }).collect())
+    }
+
     /// src/main.rs:79-103 up to (not including) the POST: Ok(Some(body)) = bind, Ok(None) = already bound,
     /// Err(1) = NoNodeFound, Err(2) = CreateBindingObjectFailed.  A failed POST needs no rollback call: the requeued
     /// pod comes back through reconcile(), which releases the earlier charge before it selects again.

@@ -26,6 +26,7 @@ pub const KSH_RECONCILE_NO_NODE_FOUND: c_int = 1; // ReconcileError::NoNodeFound
 pub const KSH_RECONCILE_BINDING_OBJECT_FAILED: c_int = 2; // ReconcileError::CreateBindingObjectFailed
 pub const KS_REFERENCE_ATTEMPTS: u32 = 5; // ATTEMPTS, src/main.rs:49
 pub const KS_MAX_PEERS: usize = 15;
+pub const KS_TOPK_MAX: u32 = 32; // largest k of ks_select_topk / ksh_rank_nodes
 
 #[repr(C)]
 pub struct ks_kv {
@@ -122,6 +123,8 @@ extern "C" {
     pub fn ks_select_sampling(s: *mut ks_snapshot, pods: *const ks_pods, attempts: u32, seed: u64, first_pod_index: u64,
                               node_idx: *mut i32, attempts_used: *mut u32, draw_node: *mut i32, draw_code: *mut u8) -> c_int;
     pub fn ks_explain(s: *mut ks_snapshot, pods: *const ks_pods, out: *mut ks_pod_reasons, out_space: i32, stream: *mut c_void) -> c_int;
+    pub fn ks_select_topk(s: *mut ks_snapshot, pods: *const ks_pods, policy: c_int, k: u32, node_idx: *mut i32, score: *mut i64,
+                          feasible_cnt: *mut u32, out_space: i32, stream: *mut c_void) -> c_int;
     pub fn ks_snapshot_commit_claims(s: *mut ks_snapshot, n: u64, node: *const i32, cpu: *const i64, mem: *const i64, accepted: *mut u8) -> c_int;
     pub fn ks_stream_bind(s: *mut ks_snapshot, pods: *const ks_pods, policy: c_int, node_idx: *mut i32, score: *mut i64, rounds: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
@@ -151,6 +154,8 @@ extern "C" {
     pub fn ksh_check_node_validity(ctx: *mut ksh_context, pod: *const ks_pod_obj, node_idx: u32) -> c_int;
     pub fn ksh_select_nodes(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, policy: c_int,
                             node_idx: *mut i32, score: *mut i64, cnt: *mut u32) -> c_int;
+    pub fn ksh_rank_nodes(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, policy: c_int, k: u32,
+                          node_idx: *mut i32, score: *mut i64, cnt: *mut u32) -> c_int;
     pub fn ksh_select_node_for_pod(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, attempts: u32, seed: u64,
                                    first_pod_index: u64, node_idx: *mut i32, attempts_used: *mut u32,
                                    draw_node: *mut i32, draw_code: *mut u8) -> c_int;

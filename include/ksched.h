@@ -243,6 +243,23 @@ typedef struct ks_pod_reasons {
  * out or the pods are in host memory, after enqueue on cuda_stream (NULL = library stream) when both are on the device. */
 int ks_explain(ks_snapshot* s, const ks_pods* pods, ks_pod_reasons* out, int32_t out_space, void* cuda_stream);
 
+/* ---- ranked candidates: the k best feasible nodes per pod (fall-backs after a failed Binding POST, extender
+ * "prioritize" replies, "why node X and not node Y") ----
+ * For pod p and 1 <= k <= KS_TOPK_MAX, row p holds the min(k, feasible_cnt[p]) feasible nodes with the highest score
+ * under `policy`, score descending, ties to the lower node index: the total order ks_select uses, so entry 0 of every
+ * row is ks_select's node_idx / score for that pod and policy (on either kernel path) and out_feasible_cnt is its
+ * feasible_cnt.  Slots past the feasible count hold node -1 and score 0.  Scores are the values ks_select reports
+ * (LEFTOVER: (free_cpu-req_cpu)*2^22 + (free_mem-req_mem); LEAST_ALLOCATED: the integer-floor formula above).  Padding
+ * nodes never appear, and nothing is charged: the snapshot is not changed.
+ * KS_ERR_RANGE when k = 0 or k > KS_TOPK_MAX; KS_ERR_INVALID for a bad policy or out_space, or a NULL out_node_idx with
+ * pods->n > 0.  pods->n = 0 does nothing; an empty snapshot gives every row -1 / 0 and count 0. */
+#define KS_TOPK_MAX 32u
+/* out_node_idx[P*k] (row-major, required), out_score[P*k] and out_feasible_cnt[P] (may be NULL), all in out_space;
+ * pods in pods->mem_space.  Returns after completion when outputs or pods are on the host, after enqueue on
+ * cuda_stream (NULL = library stream) when both are on the device - the same rule as ks_explain. */
+int ks_select_topk(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t k, int32_t* out_node_idx,
+                   int64_t* out_score, uint32_t* out_feasible_cnt, int32_t out_space, void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif

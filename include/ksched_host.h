@@ -96,6 +96,13 @@ int ksh_check_node_validity(ksh_context* ctx, const ks_pod_obj* pod, uint32_t no
  * (24 + 8W bytes per pod) until it is destroyed, so that repeated calls do not fault in fresh pages. */
 int ksh_select_nodes(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, int policy, int32_t* out_node_idx,
                      int64_t* out_score, uint32_t* out_feasible_cnt);
+/* Ranked alternatives: ks_select_topk (ksched.h) over pod objects, packed as ksh_select_nodes packs them.  Row p of
+ * out_node_idx[n_pods*k] lists pod p's k best feasible nodes (-1 past the feasible count), entry 0 being what
+ * ksh_select_nodes picks; map indices to names with ksh_context_node_name.  Nothing is charged: after a Binding POST
+ * for one of them succeeds, report it with ksh_context_pod_bound.  out_score[n_pods*k] / out_feasible_cnt[n_pods] may
+ * be NULL.  KS_ERR_NO_DEVICE on a packing-only context. */
+int ksh_rank_nodes(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, int policy, uint32_t k,
+                   int32_t* out_node_idx, int64_t* out_score, uint32_t* out_feasible_cnt);
 
 /* select_node_for_pod with the reference's OWN policy (src/main.rs:49-71): <= attempts seeded random draws per pod,
  * first valid draw wins, -1 = None.  Arguments as ks_select_sampling (ksched.h); pass KS_REFERENCE_ATTEMPTS for the

@@ -102,6 +102,11 @@ _proto("ks_select_sampling", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_uint32
        C.c_void_p, C.c_void_p, C.c_void_p)
 if hasattr(lib, "ks_explain"):  # a library built from the host layer and a device stand-in has no ks_explain
     _proto("ks_explain", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_int32, C.c_void_p)
+if hasattr(lib, "ks_select_topk"):  # the same for ks_select_topk
+    _proto("ks_select_topk", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_int, C.c_uint32, C.c_void_p, C.c_void_p,
+           C.c_void_p, C.c_int32, C.c_void_p)
+KS_TOPK_MAX = 32
+KS_ERR_INVALID, KS_ERR_RANGE = -1, -5
 KS_REFERENCE_ATTEMPTS = 5
 _SAMPLING_MULT = 0xD1B54A32D192ED03
 

@@ -18,10 +18,11 @@
 #include "../../../include/ksched_host.h"
 
 extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not part of the public ABI)
-// ks_explain is defined by the CUDA core in the same library.  The reference is weak so that this file still links
-// with device stand-ins that only provide the older ks_* entries (tests/native); ksh_explain_pods then reports
-// KS_ERR_NO_DEVICE.
+// ks_explain and ks_select_topk are defined by the CUDA core in the same library.  The references are weak so that this
+// file still links with device stand-ins that only provide the older ks_* entries (tests/native); ksh_explain_pods and
+// ksh_rank_nodes then report KS_ERR_NO_DEVICE.
 #pragma weak ks_explain
+#pragma weak ks_select_topk
 
 namespace {
 
@@ -1159,6 +1160,24 @@ int ksh_select_nodes(ksh_context* c, const ks_pod_obj* pods, uint64_t n, int pol
     ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     ks_bindings kb{out_node_idx, out_score, out_cnt, KS_MEM_HOST, nullptr, 0, KS_MEM_HOST, nullptr, nullptr};
     return ks_select(c->snap, &kp, policy, KS_SELECT_AUTO, &kb, nullptr);
+}
+KSH_CATCH
+
+int ksh_rank_nodes(ksh_context* c, const ks_pod_obj* pods, uint64_t n, int policy, uint32_t k, int32_t* out_node_idx,
+                   int64_t* out_score, uint32_t* out_cnt) try {
+    if (!c || (n && !pods)) return fail(KS_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    if (k == 0 || k > KS_TOPK_MAX) return fail(KS_ERR_RANGE, "k must be in [1, " + std::to_string(KS_TOPK_MAX) + "]");
+    if (n == 0) return KS_OK;
+    if (!out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
+    std::vector<int64_t>&rc_ = c->pk_cpu, &rm_ = c->pk_mem; // the same packed batch buffers as ksh_select_nodes
+    std::vector<uint64_t>& sel = c->pk_sel;
+    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel);
+    if (rc) return rc;
+    if (!ks_select_topk) return fail(KS_ERR_NO_DEVICE, "this library has no ks_select_topk");
+    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
+    return ks_select_topk(c->snap, &kp, policy, k, out_node_idx, out_score, out_cnt, KS_MEM_HOST, nullptr);
 }
 KSH_CATCH
 

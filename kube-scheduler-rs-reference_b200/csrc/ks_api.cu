@@ -74,6 +74,7 @@ struct ks_snapshot {
     DevBuf st_rc, st_rm, st_sel, st_idx, st_score, st_cnt, st_mask, st_codes, st_bnode, st_bcpu, st_bmem;
     DevBuf part_key, part_idx, part_cnt, st_samp, xflag;
     DevBuf st_reasons; // ks_explain with host-space output
+    DevBuf st_topk, part_topk; // ks_select_topk: host-space outputs, node-chunk partials
     DevBuf sb_pkey, sb_pidx, sb_pend; // device-side streaming loop (k_stream_batch)
     void* h_stream = nullptr;                 // pinned staging of one streaming micro-batch (inputs and results)
     int sms = 0, coop = 0;
@@ -181,7 +182,8 @@ void ks_snapshot_destroy(ks_snapshot* s) {
                       &s->flag,      &s->st_rc,     &s->st_rm,    &s->st_sel,   &s->st_idx,   &s->st_score,
                       &s->st_cnt,    &s->st_mask,   &s->st_codes, &s->st_bnode, &s->st_bcpu,  &s->st_bmem,
                       &s->part_key,  &s->part_idx,  &s->part_cnt, &s->st_samp,  &s->xflag,
-                      &s->sb_pkey,   &s->sb_pidx,   &s->sb_pend,  &s->st_reasons};
+                      &s->sb_pkey,   &s->sb_pidx,   &s->sb_pend,  &s->st_reasons, &s->st_topk,
+                      &s->part_topk};
     if (s->h_stream) cudaFreeHost(s->h_stream);
     for (DevBuf* b : bufs) b->release();
     bitpar_release(s->bp);
@@ -899,6 +901,57 @@ int ks_explain(ks_snapshot* s, const ks_pods* pods, ks_pod_reasons* out, int32_t
     }
     if (out_space == KS_MEM_HOST)
         CU_TRY(cudaMemcpyAsync(out, d_out, P * sizeof(ks_pod_reasons), cudaMemcpyDeviceToHost, st));
+    if (out_space == KS_MEM_HOST || pods->mem_space == KS_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
+    return KS_OK;
+}
+
+int ks_select_topk(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t k, int32_t* out_node_idx,
+                   int64_t* out_score, uint32_t* out_feasible_cnt, int32_t out_space, void* cuda_stream) {
+    int rc = check_pods(s, pods);
+    if (rc) return rc;
+    if (k == 0 || k > KS_TOPK_MAX) return fail(KS_ERR_RANGE, "k must be in [1, %u] (got %u)", KS_TOPK_MAX, k);
+    if (policy != KS_SCORE_LEFTOVER && policy != KS_SCORE_LEAST_ALLOCATED) return fail(KS_ERR_INVALID, "bad policy");
+    if (out_space != KS_MEM_HOST && out_space != KS_MEM_DEVICE) return fail(KS_ERR_INVALID, "bad out_space");
+    const uint64_t P = pods->n;
+    if (P && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
+    if (P == 0) return KS_OK;
+    std::lock_guard<std::mutex> lk(s->mu);
+    CU_TRY(cudaSetDevice(s->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
+    const uint64_t cells = P * k;
+    OutView ov{out_node_idx, out_score, out_feasible_cnt, nullptr, 0, 0};
+    if (out_space == KS_MEM_HOST) { // one staging block: score [P*k] | node_idx [P*k] | feasible_cnt [P]
+        CU_TRY(s->st_topk.ensure(cells * 12 + P * 4));
+        uint8_t* b = s->st_topk.as<uint8_t>();
+        ov.score = out_score ? reinterpret_cast<int64_t*>(b) : nullptr;
+        ov.node_idx = reinterpret_cast<int32_t*>(b + cells * 8);
+        ov.cnt = out_feasible_cnt ? reinterpret_cast<uint32_t*>(b + cells * 12) : nullptr;
+    }
+    if (s->N == 0) { // no node: every slot is empty
+        CU_TRY(cudaMemsetAsync(ov.node_idx, 0xff, cells * 4, st));
+        if (ov.score) CU_TRY(cudaMemsetAsync(ov.score, 0, cells * 8, st));
+        if (ov.cnt) CU_TRY(cudaMemsetAsync(ov.cnt, 0, P * 4, st));
+    } else {
+        PodView pv;
+        rc = stage_pods(s, pods, st, &pv);
+        if (rc) return rc;
+        const DirectGrid g = direct_grid(s->W, pv.P, s->Npad, s->sms);
+        PartialView part{nullptr, nullptr, nullptr};
+        if (g.n_chunks > 1) { // keys [chunks*P*k] | indices [chunks*P*k] | counts [chunks*P]
+            const uint64_t rows = (uint64_t)g.n_chunks * P;
+            CU_TRY(s->part_topk.ensure(rows * k * 12 + rows * 4));
+            uint8_t* b = s->part_topk.as<uint8_t>();
+            part.key = reinterpret_cast<int64_t*>(b);
+            part.idx = reinterpret_cast<int32_t*>(b + rows * k * 8);
+            part.cnt = reinterpret_cast<uint32_t*>(b + rows * k * 12);
+        }
+        CU_TRY(launch_select_topk(node_table(s), pv, policy, k, ov, part, g, st));
+    }
+    if (out_space == KS_MEM_HOST) {
+        CU_TRY(cudaMemcpyAsync(out_node_idx, ov.node_idx, cells * 4, cudaMemcpyDeviceToHost, st));
+        if (out_score) CU_TRY(cudaMemcpyAsync(out_score, ov.score, cells * 8, cudaMemcpyDeviceToHost, st));
+        if (out_feasible_cnt) CU_TRY(cudaMemcpyAsync(out_feasible_cnt, ov.cnt, P * 4, cudaMemcpyDeviceToHost, st));
+    }
     if (out_space == KS_MEM_HOST || pods->mem_space == KS_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
     return KS_OK;
 }

@@ -4,7 +4,8 @@
 //   K2d k_select_direct        fused feasible mask + count + argmax score, warp ballot packs 32 cells into
 //                              one mask word, warp-shuffle argmax
 //   K2e k_explain_counts       per-pod rejection counts (ks_explain)
-// K2d and K2e share one node-tile scan (scan_node_tiles): tiles staged through shared memory by TMA bulk
+//   K2k k_select_topk          per-pod ranked list of the k best feasible nodes (ks_select_topk), held across the warp
+// K2d, K2e and K2k share one node-tile scan (scan_node_tiles): tiles staged through shared memory by TMA bulk
 // copies (cp.async.bulk + mbarrier), one lane per node, several pods per warp in registers.
 // The per-cell kernel is the generic path (any score policy, any P); ks_bitpar.cu holds the bit-parallel
 // fast path that the headline configuration uses.
@@ -481,6 +482,113 @@ __global__ void __launch_bounds__(DIRECT_THREADS)
     }
 }
 
+// Ranked candidates (ks_select_topk): per pod the k best feasible nodes, held across the warp (warp_topk_insert), plus
+// the feasible count.  A feasible cell that ranks above the list's k-th entry (the threshold, warp-uniform) is a
+// candidate.  Each group of 32 nodes takes one ballot of candidates and inserts them in ascending lane order, which is
+// ascending node order; after each insertion the threshold is re-read and the candidates it now excludes are dropped.
+// With gridDim.y > 1 each node chunk writes its list and count to partials [chunk][P][k], merged by k_topk_combine.
+template <int W, int POLICY>
+// One CTA per SM: eight lists per warp at W <= 2 need more than 128 registers, and ptxas spills when held to that.
+__global__ void __launch_bounds__(DIRECT_THREADS, 1)
+    k_select_topk(NodeTable nt, PodView pv, OutView ov, PartialView part, uint32_t k, uint32_t tiles_per_chunk) {
+    constexpr int PW = pods_per_warp(W);
+    constexpr bool LA = POLICY == KS_SCORE_LEAST_ALLOCATED;
+    const uint32_t lane = threadIdx.x & 31;
+    int64_t rc[PW], rm[PW];
+    uint64_t sel[PW][W];
+    uint32_t p0;
+    int64_t lkey[PW], tkey[PW]; // this lane's list entry; the k-th entry of the list
+    int32_t lidx[PW], tidx[PW];
+    uint32_t cnt[PW];
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        lkey[i] = tkey[i] = 0;
+        lidx[i] = tidx[i] = -1;
+        cnt[i] = 0;
+    }
+
+    scan_node_tiles<W, LA>(
+        nt, tiles_per_chunk, pv, p0, rc, rm, sel,
+        [&](uint32_t, uint32_t node, bool real, int64_t fc, int64_t fm, const uint64_t(&lab)[W], int64_t ac, int64_t am) {
+            const int64_t key_n = LA ? 0 : leftover_key(fc, fm); // LEFTOVER: node priority; the pod part is constant
+#pragma unroll
+            for (int i = 0; i < PW; i++) {
+                const bool fit = (rc[i] <= fc) & (rm[i] <= fm);
+                uint64_t miss = 0;
+#pragma unroll
+                for (int w = 0; w < W; w++) miss |= sel[i][w] & ~lab[w];
+                const bool ok = fit && (miss == 0) && real;
+                cnt[i] += __popc(__ballot_sync(0xffffffffu, ok));
+                const int64_t key = LA ? (ok ? least_alloc_int(fc, fm, ac, am, rc[i], rm[i]) : 0) : key_n;
+                uint32_t cand = __ballot_sync(0xffffffffu, ok && topk_beats(key, (int32_t)node, tkey[i], tidx[i]));
+                while (cand) { // warp-uniform
+                    const int src = __ffs(cand) - 1;
+                    cand &= cand - 1;
+                    const int64_t ck = __shfl_sync(0xffffffffu, key, src);
+                    const int32_t ci = (int32_t)(node - lane + src);
+                    warp_topk_insert(lkey[i], lidx[i], ck, ci, k);
+                    tkey[i] = __shfl_sync(0xffffffffu, lkey[i], k - 1);
+                    tidx[i] = __shfl_sync(0xffffffffu, lidx[i], k - 1);
+                    cand &= __ballot_sync(0xffffffffu, topk_beats(key, (int32_t)node, tkey[i], tidx[i]));
+                }
+            }
+        },
+        [](uint32_t) {});
+
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        const uint32_t p = p0 + i;
+        if (p >= pv.P) continue; // warp-uniform
+        if (gridDim.y == 1) {
+            const uint64_t o = (uint64_t)p * k + lane;
+            if (lane < k) {
+                ov.node_idx[o] = lidx[i];
+                if (ov.score) ov.score[o] = lidx[i] < 0 ? 0 : (LA ? lkey[i] : leftover_score(lkey[i], rc[i], rm[i]));
+            }
+            if (lane == 0 && ov.cnt) ov.cnt[p] = cnt[i];
+        } else {
+            const uint64_t row = (uint64_t)blockIdx.y * pv.P + p;
+            if (lane < k) {
+                part.key[row * k + lane] = lkey[i];
+                part.idx[row * k + lane] = lidx[i];
+            }
+            if (lane == 0) part.cnt[row] = cnt[i];
+        }
+    }
+}
+
+// Merge the chunk lists of k_select_topk, one warp per pod, in ascending chunk order; keys become scores.
+template <int POLICY>
+__global__ void __launch_bounds__(256) k_topk_combine(PodView pv, OutView ov, PartialView part, uint32_t n_chunks, uint32_t k) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (p >= pv.P) return; // warp-uniform
+    int64_t key = 0, tkey = 0;
+    int32_t idx = -1, tidx = -1;
+    uint32_t c = 0;
+    for (uint32_t ch = 0; ch < n_chunks; ch++) {
+        const uint64_t row = (uint64_t)ch * pv.P + p;
+        c += part.cnt[row];
+        const int64_t pk = lane < k ? part.key[row * k + lane] : 0;
+        const int32_t pi = lane < k ? part.idx[row * k + lane] : -1;
+        for (uint32_t j = 0; j < k; j++) {
+            const int64_t ck = __shfl_sync(0xffffffffu, pk, j);
+            const int32_t ci = __shfl_sync(0xffffffffu, pi, j);
+            if (!topk_beats(ck, ci, tkey, tidx)) break; // the chunk's list is ranked: nothing after j gets in either
+            warp_topk_insert(key, idx, ck, ci, k);
+            tkey = __shfl_sync(0xffffffffu, key, k - 1);
+            tidx = __shfl_sync(0xffffffffu, idx, k - 1);
+        }
+    }
+    const uint64_t o = (uint64_t)p * k + lane;
+    if (lane < k) {
+        ov.node_idx[o] = idx;
+        if (ov.score)
+            ov.score[o] = idx < 0 ? 0 : (POLICY == KS_SCORE_LEFTOVER ? leftover_score(key, pv.req_cpu[p], pv.req_mem[p]) : key);
+    }
+    if (lane == 0 && ov.cnt) ov.cnt[p] = c;
+}
+
 // node chunks across gridDim.y when the pods alone give fewer than two CTAs per SM
 DirectGrid direct_grid(uint32_t W, uint32_t P, uint32_t Npad, int sms) {
     const uint32_t pods_per_cta = (DIRECT_THREADS / 32) * pods_per_warp(W);
@@ -510,6 +618,8 @@ cudaError_t prepare_direct() {
             opt_in(k_select_direct<W_, LA, true>, tile_smem_bytes<W_, true>());
             opt_in(k_select_direct<W_, LA, false>, tile_smem_bytes<W_, true>());
             opt_in(k_explain_counts<W_>, tile_smem_bytes<W_, false>());
+            opt_in(k_select_topk<W_, LO>, tile_smem_bytes<W_, false>());
+            opt_in(k_select_topk<W_, LA>, tile_smem_bytes<W_, true>());
             return e;
         });
     return e;
@@ -553,6 +663,29 @@ cudaError_t launch_explain_counts(const NodeTable& nt, const PodView& pv, uint32
             nt, pv, out, g.tiles_per_chunk);
         g_launches++;
         return cudaGetLastError();
+    });
+}
+
+template <int W, int POLICY>
+static cudaError_t launch_topk_t(const NodeTable& nt, const PodView& pv, uint32_t k, const OutView& ov,
+                                 const PartialView& part, const DirectGrid& g, cudaStream_t st) {
+    constexpr uint32_t SMEM = tile_smem_bytes<W, POLICY == KS_SCORE_LEAST_ALLOCATED>();
+    k_select_topk<W, POLICY><<<dim3(g.pod_ctas, g.n_chunks), DIRECT_THREADS, SMEM, st>>>(nt, pv, ov, part, k,
+                                                                                          g.tiles_per_chunk);
+    g_launches++;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess || g.n_chunks == 1) return e;
+    k_topk_combine<POLICY><<<(pv.P + 7) / 8, 256, 0, st>>>(pv, ov, part, g.n_chunks, k);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_select_topk(const NodeTable& nt, const PodView& pv, int policy, uint32_t k, const OutView& ov,
+                               const PartialView& part, const DirectGrid& g, cudaStream_t st) {
+    return with_label_width(nt.W, [&](auto w) {
+        constexpr int W = decltype(w)::value;
+        return policy == KS_SCORE_LEFTOVER ? launch_topk_t<W, KS_SCORE_LEFTOVER>(nt, pv, k, ov, part, g, st)
+                                           : launch_topk_t<W, KS_SCORE_LEAST_ALLOCATED>(nt, pv, k, ov, part, g, st);
     });
 }
 

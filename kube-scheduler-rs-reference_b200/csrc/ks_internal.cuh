@@ -132,6 +132,24 @@ __device__ __forceinline__ void merge_partial(int64_t& key, int32_t& idx, int64_
         idx = oi;
     }
 }
+// The same total order as a predicate: entry a ranks above entry b when a is an entry (ai >= 0) and b is empty, or a has
+// the larger key, or the same key and the lower node index.
+__device__ __forceinline__ bool topk_beats(int64_t ak, int32_t ai, int64_t bk, int32_t bi) {
+    return ai >= 0 && (bi < 0 || ak > bk || (ak == bk && ai < bi));
+}
+// A ranked list held across the warp (ks_select_topk): lane j holds the j-th best (key, idx) for j < k, empty slots
+// (idx = -1) come last and lanes >= k stay empty.  Inserts the warp-uniform candidate (ck, ci) at its rank, shifting the
+// entries below it down one lane; a candidate that ranks k-th or lower changes nothing.  Called by the whole warp.
+__device__ __forceinline__ void warp_topk_insert(int64_t& key, int32_t& idx, int64_t ck, int32_t ci, uint32_t k) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t pos = __popc(__ballot_sync(0xffffffffu, topk_beats(key, idx, ck, ci)));
+    const int64_t uk = __shfl_up_sync(0xffffffffu, key, 1);
+    const int32_t ui = __shfl_up_sync(0xffffffffu, idx, 1);
+    if (lane < k && lane >= pos) {
+        key = lane == pos ? ck : uk;
+        idx = lane == pos ? ci : ui;
+    }
+}
 
 // Label-width dispatch: calls f(std::integral_constant<int, W>{}) for W in {1, 2, 4, 8}; any other W is invalid.
 template <class F>

@@ -27,6 +27,10 @@ cudaError_t prepare_direct(); // once per snapshot, outside any stream capture
 cudaError_t launch_select_direct(const SelectLaunch& L, const PartialView& part, const DirectGrid& g);
 // per-pod rejection counts (ks_explain): out = uint32 [P][4] in ks_pod_reasons order, device memory
 cudaError_t launch_explain_counts(const NodeTable& nt, const PodView& pv, uint32_t* out, int sms, cudaStream_t st);
+// ranked candidates (ks_select_topk): ov.node_idx / score = [P][k], ov.cnt = [P] (score and cnt may be null), device
+// memory; with g.n_chunks > 1, part holds g.n_chunks * P * k keys and indices and g.n_chunks * P counts
+cudaError_t launch_select_topk(const NodeTable& nt, const PodView& pv, int policy, uint32_t k, const OutView& ov,
+                               const PartialView& part, const DirectGrid& g, cudaStream_t st);
 
 } // namespace ks
 

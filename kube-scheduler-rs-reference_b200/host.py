@@ -31,6 +31,7 @@ for _name, _res, _args in [
     ("ksh_pack_pods", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, _vp, C.c_uint32]),
     ("ksh_check_node_validity", C.c_int, [_vp, _vp, C.c_uint32]),
     ("ksh_select_nodes", C.c_int, [_vp, _vp, C.c_uint64, C.c_int, _vp, _vp, _vp]),
+    ("ksh_rank_nodes", C.c_int, [_vp, _vp, C.c_uint64, C.c_int, C.c_uint32, _vp, _vp, _vp]),
     ("ksh_select_node_for_pod", C.c_int, [_vp, _vp, C.c_uint64, C.c_uint32, C.c_uint64, C.c_uint64, _vp, _vp, _vp, _vp]),
     ("ksh_reconcile_batch", C.c_int, [_vp, _vp, C.c_uint64, C.c_int, _vp, _vp, _vp, C.c_size_t, _vp, C.POINTER(C.c_uint32)]),
     ("ksh_reconcile", C.c_int, [_vp, _vp, C.c_int, C.POINTER(C.c_int32), C.c_char_p, C.c_size_t]),
@@ -191,6 +192,18 @@ class Context:
                                   cnt.ctypes.data)
         if rc != capi.KS_OK:
             raise KsError(rc, "ksh_select_nodes")
+        return idx, score, cnt
+
+    def rank_nodes(self, pods, n, k, policy=capi.KS_SCORE_LEFTOVER, first=0):
+        """Ranked alternatives (ksh_rank_nodes): (node_idx int32 [n, k], score int64 [n, k], feasible_cnt uint32 [n]);
+        entry 0 of a row is select_nodes()'s pick, -1 fills the slots past the feasible count.  Charges nothing."""
+        idx = np.empty((n, int(k)), np.int32)
+        score = np.empty((n, int(k)), np.int64)
+        cnt = np.empty(n, np.uint32)
+        rc = lib.ksh_rank_nodes(self._h, _addr(pods, first), n, int(policy), int(k), idx.ctypes.data, score.ctypes.data,
+                                cnt.ctypes.data)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ksh_rank_nodes")
         return idx, score, cnt
 
     def select_node_for_pod(self, pods, n, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first=0):

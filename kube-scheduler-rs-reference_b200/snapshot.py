@@ -213,6 +213,31 @@ class Snapshot:
         if rc != capi.KS_OK:
             raise KsError(rc, "ks_explain")
 
+    def select_topk(self, req_cpu, req_mem, sel, k, policy=capi.KS_SCORE_LEFTOVER):
+        """The k best feasible nodes per pod (ks_select_topk) over host (numpy) pods: node_idx int32 [P, k] (-1 past the
+        feasible count), score int64 [P, k] (0 there), feasible_cnt uint32 [P].  Entry 0 of a row is select()'s pick."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        p = int(pods.n)
+        idx = np.empty((p, int(k)), np.int32)
+        score = np.empty((p, int(k)), np.int64)
+        cnt = np.empty(p, np.uint32)
+        rc = lib.ks_select_topk(self._h, C.byref(pods), int(policy), int(k), _ptr(idx), _ptr(score), _ptr(cnt),
+                                capi.KS_MEM_HOST, None)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ks_select_topk")
+        return idx, score, cnt
+
+    def select_topk_raw(self, n_pods, req_cpu, req_mem, sel, pods_space, k, node_idx, score, cnt, out_space,
+                        policy=capi.KS_SCORE_LEFTOVER, stream=None):
+        """Pointer-level ks_select_topk (torch tensors / raw addresses); node_idx / score hold n_pods x k entries, cnt
+        n_pods (score and cnt may be None).  The caller keeps the buffers alive; with device pods and outputs the call
+        returns after enqueue on `stream`."""
+        pods = ks_pods(int(n_pods), _ptr(req_cpu), _ptr(req_mem), _ptr(sel), int(pods_space))
+        rc = lib.ks_select_topk(self._h, C.byref(pods), int(policy), int(k), _ptr(node_idx), _ptr(score), _ptr(cnt),
+                                int(out_space), C.c_void_p(stream) if stream else None)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ks_select_topk")
+
     def last_timings(self):
         ms = (C.c_float * 3)()
         rc = lib.ks_last_timings(self._h, ms)
