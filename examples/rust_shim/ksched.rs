@@ -178,6 +178,36 @@ impl Gpu {
         };
         (r, msg)
     }
+
+    /// Priority preemption for a pod no node accepts (upstream's PostFilter without PodDisruptionBudgets): the node
+    /// name and the "namespace/name" keys of the lower-priority pods to evict there, in visit order; None = no plan.
+    /// `priority` is the pod's spec.priority; bound pods' priorities come from `ksh_context_set_pod_priorities`.
+    /// Nothing is charged: DELETE the victims, report each with `ksh_context_pod_deleted`, requeue the pod.
+    pub fn preempt(&self, pod: &corev1::Pod, priority: i32, max_victims: u32) -> Result<Option<(String, Vec<String>)>, i32> {
+        let v = PodView::new(pod);
+        let mut row = ks_preemption::default();
+        let mut buf = vec![0u8; 256 * max_victims as usize];
+        let mut off: i64 = -1;
+        let rc = unsafe {
+            ksh_preempt_pods(self.ctx, &v.obj, 1, &priority, max_victims, &mut row, buf.as_mut_ptr() as *mut c_char,
+                             buf.len(), &mut off)
+        };
+        if rc != KS_OK {
+            return Err(rc);
+        }
+        if row.node_idx < 0 || off < 0 {
+            return Ok(None);
+        }
+        let node = unsafe { CStr::from_ptr(ksh_context_node_name(self.ctx, row.node_idx as u32)) }.to_string_lossy().into_owned();
+        let mut keys = Vec::with_capacity(row.n_victims as usize);
+        let mut at = off as usize;
+        for _ in 0..row.n_victims {
+            let k = unsafe { CStr::from_ptr(buf.as_ptr().add(at) as *const c_char) };
+            at += k.to_bytes().len() + 1;
+            keys.push(k.to_string_lossy().into_owned());
+        }
+        Ok(Some((node, keys)))
+    }
 }
 
 impl Drop for Gpu {

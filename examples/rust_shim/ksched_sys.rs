@@ -27,6 +27,7 @@ pub const KSH_RECONCILE_BINDING_OBJECT_FAILED: c_int = 2; // ReconcileError::Cre
 pub const KS_REFERENCE_ATTEMPTS: u32 = 5; // ATTEMPTS, src/main.rs:49
 pub const KS_MAX_PEERS: usize = 15;
 pub const KS_TOPK_MAX: u32 = 32; // largest k of ks_select_topk / ksh_rank_nodes
+pub const KS_PREEMPT_MAX_VICTIMS: u32 = 128; // largest max_victims of ks_preempt / ksh_preempt_pods
 
 #[repr(C)]
 pub struct ks_kv {
@@ -101,6 +102,25 @@ pub struct ks_pod_reasons {
     pub not_enough_resources: u32,
     pub node_selector_mismatch: u32,
 }
+#[repr(C)]
+pub struct ks_bound_pods {
+    pub n: u64,
+    pub node_idx: *const i32,
+    pub req_cpu: *const i64,
+    pub req_mem: *const i64,
+    pub priority: *const i32,
+}
+#[repr(C)]
+#[derive(Clone, Copy, Default, Debug)]
+pub struct ks_preemption {
+    pub node_idx: i32,
+    pub n_victims: u32,
+    pub candidates: u32,
+    pub feasible_cnt: u32,
+    pub max_victim_priority: i32,
+    pub reserved: u32,
+    pub victim_priority_sum: i64,
+}
 pub enum ks_snapshot {}
 pub enum ks_stream {}
 pub enum ksh_context {}
@@ -125,6 +145,9 @@ extern "C" {
     pub fn ks_explain(s: *mut ks_snapshot, pods: *const ks_pods, out: *mut ks_pod_reasons, out_space: i32, stream: *mut c_void) -> c_int;
     pub fn ks_select_topk(s: *mut ks_snapshot, pods: *const ks_pods, policy: c_int, k: u32, node_idx: *mut i32, score: *mut i64,
                           feasible_cnt: *mut u32, out_space: i32, stream: *mut c_void) -> c_int;
+    pub fn ks_preempt(s: *mut ks_snapshot, pods: *const ks_pods, pod_priority: *const i32, bound: *const ks_bound_pods,
+                      max_victims: u32, out: *mut ks_preemption, out_victims: *mut i32, out_space: i32,
+                      stream: *mut c_void) -> c_int;
     pub fn ks_snapshot_commit_claims(s: *mut ks_snapshot, n: u64, node: *const i32, cpu: *const i64, mem: *const i64, accepted: *mut u8) -> c_int;
     pub fn ks_stream_bind(s: *mut ks_snapshot, pods: *const ks_pods, policy: c_int, node_idx: *mut i32, score: *mut i64, rounds: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
@@ -156,6 +179,9 @@ extern "C" {
                             node_idx: *mut i32, score: *mut i64, cnt: *mut u32) -> c_int;
     pub fn ksh_rank_nodes(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, policy: c_int, k: u32,
                           node_idx: *mut i32, score: *mut i64, cnt: *mut u32) -> c_int;
+    pub fn ksh_context_set_pod_priorities(ctx: *mut ksh_context, pods: *const ks_pod_obj, priority: *const i32, n: u64) -> c_int;
+    pub fn ksh_preempt_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, pod_priority: *const i32, max_victims: u32,
+                            out: *mut ks_preemption, victims: *mut c_char, cap: usize, out_victim_off: *mut i64) -> c_int;
     pub fn ksh_select_node_for_pod(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, attempts: u32, seed: u64,
                                    first_pod_index: u64, node_idx: *mut i32, attempts_used: *mut u32,
                                    draw_node: *mut i32, draw_code: *mut u8) -> c_int;

@@ -260,6 +260,51 @@ int ks_explain(ks_snapshot* s, const ks_pods* pods, ks_pod_reasons* out, int32_t
 int ks_select_topk(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t k, int32_t* out_node_idx,
                    int64_t* out_score, uint32_t* out_feasible_cnt, int32_t out_space, void* cuda_stream);
 
+/* ---- priority preemption: for a pod no node accepts, the node and the lower-priority pods to evict (upstream
+ * kube-scheduler's PostFilter / DefaultPreemption without PodDisruptionBudgets; spec extension, DESIGN.md 5d) ----
+ * Pending pod p has priority pi_p; bound pod b (its bound index b = its position in `bound`) sits on node b.node with
+ * request req_b and priority pi_b.  `bound` must be the list that produced the snapshot's free[] (ks_snapshot_set_bound
+ * plus later apply_bind / accepted commits).  For p and real node n:
+ *   1. n is eligible only if p fails there on resources alone: !fit(p, n) and the selector matches;
+ *   2. L = {b on n : pi_b < pi_p} (strictly lower); empty L: not a candidate;
+ *   3. avail = free[n] + sum of req_b over L; unless req_p <= avail (both resources, non-strict): not a candidate;
+ *   4. reprieve: visit L by priority descending, ties to the lower bound index (the older pod); b is reprieved when p
+ *      still fits avail - req_b (then avail -= req_b), else it is a victim; victims are listed in visit order;
+ *   5. more than max_victims victims: not a candidate;
+ *   6. among the candidates the plan takes the node with, in order, the lowest highest-victim priority, the lowest
+ *      sum of (pi_b + 2^31) over the victims, the fewest victims, the lowest node index;
+ *   7. a pod with feasible_cnt > 0 (as ks_select reports it) gets no plan: node -1, no victims, 0 candidates.
+ * Nothing is charged and the snapshot is not changed: evict the victims, report them (ks_snapshot_set_bound with the
+ * shorter list, or ksh_context_pod_deleted), and the pod schedules on its next pass. */
+#define KS_PREEMPT_MAX_VICTIMS 128u
+typedef struct ks_bound_pods { /* host memory; the list that produced the snapshot's free[] */
+    uint64_t n;
+    const int32_t* node_idx;
+    const int64_t* req_cpu;
+    const int64_t* req_mem;
+    const int32_t* priority;
+} ks_bound_pods;
+typedef struct ks_preemption { /* 32 bytes per pod */
+    int32_t node_idx;              /* -1 = no plan */
+    uint32_t n_victims;
+    uint32_t candidates;           /* nodes where eviction within max_victims makes room (0 when feasible_cnt > 0) */
+    uint32_t feasible_cnt;         /* as ks_select reports it */
+    int32_t max_victim_priority;   /* INT32_MIN without a plan */
+    uint32_t reserved;             /* 0 */
+    int64_t victim_priority_sum;   /* sum of (priority + 2^31) over the victims; 0 without a plan */
+} ks_preemption;
+/* out[pods->n] and out_victims[pods->n * max_victims] (bound indices in visit order, -1 past n_victims; may be NULL)
+ * in out_space; pod_priority[pods->n] in pods->mem_space.  `bound` is checked as ks_snapshot_set_bound checks it (node
+ * range, per-pod request limits) plus one range rule: for every node, the sum of |req_cpu| and the sum of |req_mem|
+ * over its bound pods must each be <= 2^62, which keeps free[n] plus any subset of them inside int64 (KS_ERR_RANGE).
+ * KS_ERR_RANGE when max_victims is 0 or above KS_PREEMPT_MAX_VICTIMS, or bound->n >= 2^32; KS_ERR_INVALID for a bad
+ * out_space, a NULL bound array, or a NULL pod_priority / out with pods->n > 0.  pods->n = 0 does nothing; an empty
+ * snapshot gives every pod no plan.  Returns after completion when pods or outputs are on the host, after enqueue on
+ * cuda_stream (NULL = library stream) when both are on the device - the rule of ks_explain. */
+#define KS_PREEMPT_MAX_ABS_SUM ((int64_t)1 << 62)
+int ks_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* pod_priority, const ks_bound_pods* bound,
+               uint32_t max_victims, ks_preemption* out, int32_t* out_victims, int32_t out_space, void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -145,6 +145,24 @@ int ksh_explain_pods(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, 
  * truncated); KS_ERR_INVALID when r is NULL, or buf is NULL with cap > 0. */
 int ksh_format_unschedulable(uint32_t n_nodes, const ks_pod_reasons* r, char* buf, size_t cap);
 
+/* Priority preemption over pod objects (ks_preempt, ksched.h).
+ * ksh_context_set_pod_priorities records spec.priority for bound pods known by namespace/name; unknown pods are ignored
+ * (KS_OK), as with the other events.  A bound pod's priority is 0 until it is set, follows its pod through pod events
+ * (a repeated ksh_context_pod_bound for the same pod keeps it: spec.priority is immutable), and is reset to 0 by
+ * ksh_context_set_nodes / ksh_context_set_cluster_pods, which rebuild the bound list, and for pods that
+ * ksh_reconcile / ksh_reconcile_batch bind.  Bound pods without namespace and name cannot be named for eviction, so they
+ * are passed as priority INT32_MAX and are never victims.
+ * ksh_preempt_pods packs pods as ksh_select_nodes does and passes the context's bound pods as the ks_bound_pods list;
+ * pod_priority[n_pods] is each pending pod's priority.  out[n_pods] receives the plans (node index: map it with
+ * ksh_context_node_name).  For each pod with a plan, its victims' "namespace/name" keys are written into victims (cap
+ * bytes) back to back, each NUL-terminated, in visit order; out_victim_off[i] = offset of pod i's first key, or -1 (no
+ * plan, or the buffer was full).  victims / out_victim_off may be NULL.  Nothing is charged: DELETE the victims, report
+ * each with ksh_context_pod_deleted, and requeue the pod.  KS_ERR_RANGE for max_victims outside
+ * [1, KS_PREEMPT_MAX_VICTIMS]; KS_ERR_NO_DEVICE on a packing-only context. */
+int ksh_context_set_pod_priorities(ksh_context* ctx, const ks_pod_obj* pods, const int32_t* priority, uint64_t n_pods);
+int ksh_preempt_pods(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, const int32_t* pod_priority,
+                     uint32_t max_victims, ks_preemption* out, char* victims, size_t cap, int64_t* out_victim_off);
+
 #ifdef __cplusplus
 }
 #endif

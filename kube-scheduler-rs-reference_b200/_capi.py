@@ -3,6 +3,8 @@ import ctypes as C
 import os
 import re
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libksched.so")
 INCLUDE_DIR = os.path.join(os.path.dirname(_HERE), "include")
@@ -106,6 +108,28 @@ if hasattr(lib, "ks_select_topk"):  # the same for ks_select_topk
     _proto("ks_select_topk", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_int, C.c_uint32, C.c_void_p, C.c_void_p,
            C.c_void_p, C.c_int32, C.c_void_p)
 KS_TOPK_MAX = 32
+
+
+class ks_bound_pods(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("node_idx", C.c_void_p), ("req_cpu", C.c_void_p), ("req_mem", C.c_void_p),
+                ("priority", C.c_void_p)]
+
+
+class ks_preemption(C.Structure):
+    _fields_ = [("node_idx", C.c_int32), ("n_victims", C.c_uint32), ("candidates", C.c_uint32),
+                ("feasible_cnt", C.c_uint32), ("max_victim_priority", C.c_int32), ("reserved", C.c_uint32),
+                ("victim_priority_sum", C.c_int64)]
+
+
+# ks_preemption as a numpy record, for whole batches of rows
+PREEMPTION_DTYPE = np.dtype([("node_idx", np.int32), ("n_victims", np.uint32), ("candidates", np.uint32),
+                             ("feasible_cnt", np.uint32), ("max_victim_priority", np.int32), ("reserved", np.uint32),
+                             ("victim_priority_sum", np.int64)])
+if hasattr(lib, "ks_preempt"):  # the same for ks_preempt
+    _proto("ks_preempt", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.POINTER(ks_bound_pods), C.c_uint32,
+           C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p)
+KS_PREEMPT_MAX_VICTIMS = 128
+KS_PREEMPT_MAX_ABS_SUM = 1 << 62
 KS_ERR_INVALID, KS_ERR_RANGE = -1, -5
 KS_REFERENCE_ATTEMPTS = 5
 _SAMPLING_MULT = 0xD1B54A32D192ED03

@@ -18,11 +18,12 @@
 #include "../../../include/ksched_host.h"
 
 extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not part of the public ABI)
-// ks_explain and ks_select_topk are defined by the CUDA core in the same library.  The references are weak so that this
-// file still links with device stand-ins that only provide the older ks_* entries (tests/native); ksh_explain_pods and
-// ksh_rank_nodes then report KS_ERR_NO_DEVICE.
+// ks_explain, ks_select_topk and ks_preempt are defined by the CUDA core in the same library.  The references are weak so
+// that this file still links with device stand-ins that only provide the older ks_* entries (tests/native);
+// ksh_explain_pods, ksh_rank_nodes and ksh_preempt_pods then report KS_ERR_NO_DEVICE.
 #pragma weak ks_explain
 #pragma weak ks_select_topk
+#pragma weak ks_preempt
 
 namespace {
 
@@ -258,6 +259,7 @@ struct ksh_context {
     std::vector<uint64_t> bhash;  // hash of "ns/name"; 0 with blen 0 = anonymous pod, not tracked
     std::vector<uint64_t> boff;   // key bytes in bkeys
     std::vector<uint32_t> blen;
+    std::vector<int32_t> bprio;   // spec.priority (ksh_context_set_pod_priorities), 0 until set
     std::vector<char> bkeys;
     PosTable btab;
     uint64_t live_pairs = 0;     // pairs carried by at least one node
@@ -584,10 +586,13 @@ static void bound_erase(ksh_context* c, size_t pos);
 static void bound_push(ksh_context* c, const ks_pod_obj* pod, uint64_t h, size_t lns, size_t lname, int32_t node, int64_t cpu,
                        int64_t mem) {
     const bool tracked = lns + lname > 0; // a pod without namespace and name cannot be addressed by later events
+    int32_t prio = 0;
     if (tracked) {
         const int64_t old = btab_find_slot(c, h, pod, lns, lname);
         if (old >= 0) {
-            bound_erase(c, slot_low(c->btab.slots[(size_t)old]) - 2);
+            const size_t old_pos = slot_low(c->btab.slots[(size_t)old]) - 2;
+            prio = c->bprio[old_pos]; // the same pod: spec.priority is immutable
+            bound_erase(c, old_pos);
             c->dirty = true;
         }
     }
@@ -595,6 +600,7 @@ static void bound_push(ksh_context* c, const ks_pod_obj* pod, uint64_t h, size_t
     c->bnode.push_back(node);
     c->bcpu.push_back(cpu);
     c->bmem.push_back(mem);
+    c->bprio.push_back(prio);
     c->bhash.push_back(tracked ? h : 0);
     c->boff.push_back(c->bkeys.size());
     c->blen.push_back(tracked ? (uint32_t)(lns + 1 + lname) : 0);
@@ -647,6 +653,7 @@ static void bound_erase(ksh_context* c, size_t pos) { // swap-remove
         c->bhash[pos] = c->bhash[last];
         c->boff[pos] = c->boff[last];
         c->blen[pos] = c->blen[last];
+        c->bprio[pos] = c->bprio[last];
     }
     c->bnode.pop_back();
     c->bcpu.pop_back();
@@ -654,6 +661,7 @@ static void bound_erase(ksh_context* c, size_t pos) { // swap-remove
     c->bhash.pop_back();
     c->boff.pop_back();
     c->blen.pop_back();
+    c->bprio.pop_back();
     if (c->bnode.empty()) c->bkeys.clear(); // otherwise erased keys wait for gc_bound_keys
 }
 
@@ -664,6 +672,7 @@ static void bound_clear(ksh_context* c) {
     c->bhash.clear();
     c->boff.clear();
     c->blen.clear();
+    c->bprio.clear();
     c->bkeys.clear();
     c->btab.clear();
     c->live_key_bytes = 0;
@@ -1019,11 +1028,7 @@ int ksh_context_pod_bound(ksh_context* c, const ks_pod_obj* pod) try {
     if (rc) return fail(rc, err);
     size_t lns, lname;
     const uint64_t h = pod_key_hash(pod, &lns, &lname);
-    if (lns + lname > 0) {
-        const int64_t slot = btab_find_slot(c, h, pod, lns, lname);
-        if (slot >= 0) bound_erase(c, slot_low(c->btab.slots[(size_t)slot]) - 2); // update of a pod already known
-    }
-    bound_push(c, pod, h, lns, lname, node, cpu, mem);
+    bound_push(c, pod, h, lns, lname, node, cpu, mem); // an update of a pod already known replaces its row
     gc_bound_keys(c);
     c->dirty = true;
     return KS_OK;
@@ -1097,6 +1102,7 @@ int ksh_context_set_cluster_pods(ksh_context* c, const ks_pod_obj* pods, uint64_
     c->bhash.reserve(kept);
     c->boff.reserve(kept);
     c->blen.reserve(kept);
+    c->bprio.reserve(kept);
     c->bkeys.reserve(key_bytes);
     btab_rebuild(c, kept); // sized once for the whole list
     for (uint64_t p = 0; p < n; p++)
@@ -1372,6 +1378,63 @@ int ksh_explain_pods(ksh_context* c, const ks_pod_obj* pods, uint64_t n, ks_pod_
         std::memcpy(messages + used, msg, (size_t)len + 1);
         out_msg_off[i] = (int64_t)used;
         used += (size_t)len + 1;
+    }
+    return KS_OK;
+}
+KSH_CATCH
+
+int ksh_context_set_pod_priorities(ksh_context* c, const ks_pod_obj* pods, const int32_t* priority, uint64_t n) try {
+    if (!c || (n && (!pods || !priority))) return fail(KS_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    for (uint64_t i = 0; i < n; i++) {
+        size_t lns, lname;
+        const uint64_t h = pod_key_hash(&pods[i], &lns, &lname);
+        if (lns + lname == 0) continue;
+        const int64_t slot = btab_find_slot(c, h, &pods[i], lns, lname);
+        if (slot >= 0) c->bprio[slot_low(c->btab.slots[(size_t)slot]) - 2] = priority[i];
+    }
+    return KS_OK; // the device keeps no priorities: nothing to re-upload
+}
+KSH_CATCH
+
+int ksh_preempt_pods(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* pod_priority, uint32_t max_victims,
+                     ks_preemption* out, char* victims, size_t cap, int64_t* out_victim_off) try {
+    if (!c || (n && (!pods || !pod_priority || !out))) return fail(KS_ERR_INVALID, "NULL argument");
+    if (max_victims == 0 || max_victims > KS_PREEMPT_MAX_VICTIMS)
+        return fail(KS_ERR_RANGE, "max_victims must be in [1, " + std::to_string(KS_PREEMPT_MAX_VICTIMS) + "]");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    if (out_victim_off)
+        for (uint64_t i = 0; i < n; i++) out_victim_off[i] = -1;
+    if (n == 0) return KS_OK;
+    std::vector<int64_t>&rc_ = c->pk_cpu, &rm_ = c->pk_mem; // the same packed batch buffers as ksh_select_nodes
+    std::vector<uint64_t>& sel = c->pk_sel;
+    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel); // after this the device's free[] comes from the bound rows below
+    if (rc) return rc;
+    if (!ks_preempt) return fail(KS_ERR_NO_DEVICE, "this library has no ks_preempt");
+    const size_t B = c->bnode.size();
+    std::vector<int32_t> prio(B);
+    for (size_t b = 0; b < B; b++) prio[b] = c->blen[b] ? c->bprio[b] : INT32_MAX; // anonymous: cannot be evicted
+    std::vector<int32_t> vic((size_t)n * max_victims);
+    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
+    ks_bound_pods kb{B, c->bnode.data(), c->bcpu.data(), c->bmem.data(), prio.data()};
+    rc = ks_preempt(c->snap, &kp, pod_priority, &kb, max_victims, out, vic.data(), KS_MEM_HOST, nullptr);
+    if (rc) return rc;
+    if (!victims || !out_victim_off) return KS_OK;
+    size_t used = 0;
+    for (uint64_t i = 0; i < n; i++) {
+        if (out[i].node_idx < 0) continue;
+        const int32_t* v = &vic[(size_t)i * max_victims];
+        size_t need = 0;
+        for (uint32_t j = 0; j < out[i].n_victims; j++) need += c->blen[(size_t)v[j]] + 1;
+        if (used + need > cap) continue; // -1 = did not fit
+        out_victim_off[i] = (int64_t)used;
+        for (uint32_t j = 0; j < out[i].n_victims; j++) { // "namespace/name", NUL-terminated, in visit order
+            const size_t b = (size_t)v[j];
+            std::memcpy(victims + used, c->bkeys.data() + c->boff[b], c->blen[b]);
+            used += c->blen[b];
+            victims[used++] = '\0';
+        }
     }
     return KS_OK;
 }

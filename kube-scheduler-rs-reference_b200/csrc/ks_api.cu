@@ -75,6 +75,7 @@ struct ks_snapshot {
     DevBuf part_key, part_idx, part_cnt, st_samp, xflag;
     DevBuf st_reasons; // ks_explain with host-space output
     DevBuf st_topk, part_topk; // ks_select_topk: host-space outputs, node-chunk partials
+    DevBuf st_pre, vx_pre, part_pre; // ks_preempt: host-space outputs and priorities, victim index, node-chunk partials
     DevBuf sb_pkey, sb_pidx, sb_pend; // device-side streaming loop (k_stream_batch)
     void* h_stream = nullptr;                 // pinned staging of one streaming micro-batch (inputs and results)
     int sms = 0, coop = 0;
@@ -183,7 +184,7 @@ void ks_snapshot_destroy(ks_snapshot* s) {
                       &s->st_cnt,    &s->st_mask,   &s->st_codes, &s->st_bnode, &s->st_bcpu,  &s->st_bmem,
                       &s->part_key,  &s->part_idx,  &s->part_cnt, &s->st_samp,  &s->xflag,
                       &s->sb_pkey,   &s->sb_pidx,   &s->sb_pend,  &s->st_reasons, &s->st_topk,
-                      &s->part_topk};
+                      &s->part_topk, &s->st_pre,     &s->vx_pre,   &s->part_pre};
     if (s->h_stream) cudaFreeHost(s->h_stream);
     for (DevBuf* b : bufs) b->release();
     bitpar_release(s->bp);
@@ -951,6 +952,104 @@ int ks_select_topk(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t k, 
         CU_TRY(cudaMemcpyAsync(out_node_idx, ov.node_idx, cells * 4, cudaMemcpyDeviceToHost, st));
         if (out_score) CU_TRY(cudaMemcpyAsync(out_score, ov.score, cells * 8, cudaMemcpyDeviceToHost, st));
         if (out_feasible_cnt) CU_TRY(cudaMemcpyAsync(out_feasible_cnt, ov.cnt, P * 4, cudaMemcpyDeviceToHost, st));
+    }
+    if (out_space == KS_MEM_HOST || pods->mem_space == KS_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
+    return KS_OK;
+}
+
+// the bound list of ks_preempt against the snapshot's nodes: set_bound's checks plus the per-node sums of |request|
+static int check_preempt_bound(const ks_snapshot* s, const ks_bound_pods* bound) {
+    const uint64_t B = bound->n;
+    std::vector<uint64_t> abs_sum;
+    try {
+        abs_sum.assign((size_t)s->N * 2, 0);
+    } catch (...) {
+        return fail(KS_ERR_NOMEM, "out of host memory checking %llu bound pods", (unsigned long long)B);
+    }
+    const uint64_t LIMIT = (uint64_t)KS_PREEMPT_MAX_ABS_SUM;
+    for (uint64_t b = 0; b < B; b++) {
+        const int32_t n = bound->node_idx[b];
+        const int64_t c = bound->req_cpu[b], m = bound->req_mem[b];
+        if (n < 0 || (uint32_t)n >= s->N)
+            return fail(KS_ERR_INVALID, "bound pod %llu: node index %d out of range", (unsigned long long)b, n);
+        if (c > KS_MAX_CPU_MILLI || c < -KS_MAX_CPU_MILLI || m > KS_MAX_MEM_BYTES || m < -KS_MAX_MEM_BYTES)
+            return fail(KS_ERR_RANGE, "bound pod %llu request out of range", (unsigned long long)b);
+        uint64_t* a = &abs_sum[(size_t)n * 2];
+        a[0] += (uint64_t)(c < 0 ? -c : c); // each term <= 2^55: no wrap before the sum passes the limit
+        a[1] += (uint64_t)(m < 0 ? -m : m);
+        if (a[0] > LIMIT || a[1] > LIMIT)
+            return fail(KS_ERR_RANGE, "node %d: the bound pods' requests sum above 2^62 in absolute value", n);
+    }
+    return KS_OK;
+}
+
+int ks_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* pod_priority, const ks_bound_pods* bound,
+               uint32_t max_victims, ks_preemption* out, int32_t* out_victims, int32_t out_space, void* cuda_stream) {
+    static_assert(sizeof(ks_preemption) == 32, "ks_preemption is 32 bytes");
+    int rc = check_pods(s, pods);
+    if (rc) return rc;
+    if (max_victims == 0 || max_victims > KS_PREEMPT_MAX_VICTIMS)
+        return fail(KS_ERR_RANGE, "max_victims must be in [1, %u] (got %u)", KS_PREEMPT_MAX_VICTIMS, max_victims);
+    if (out_space != KS_MEM_HOST && out_space != KS_MEM_DEVICE) return fail(KS_ERR_INVALID, "bad out_space");
+    const uint64_t P = pods->n;
+    if (P && (!pod_priority || !out)) return fail(KS_ERR_INVALID, "pod_priority or out is NULL");
+    if (!bound) return fail(KS_ERR_INVALID, "bound is NULL");
+    const uint64_t B = bound->n;
+    if (B && (!bound->node_idx || !bound->req_cpu || !bound->req_mem || !bound->priority))
+        return fail(KS_ERR_INVALID, "NULL bound array");
+    if (B > 0xffffffffull) return fail(KS_ERR_RANGE, "too many bound pods in one call");
+    if (P == 0) return KS_OK;
+    std::lock_guard<std::mutex> lk(s->mu);
+    rc = check_preempt_bound(s, bound);
+    if (rc) return rc;
+    CU_TRY(cudaSetDevice(s->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
+    const uint64_t n_vic = out_victims ? P * max_victims : 0;
+    ks_preemption* d_out = out;
+    int32_t* d_vic = out_victims;
+    const int32_t* d_prio = pod_priority;
+    // one staging block: rows [P] | victims [P * max_victims] (host-space outputs) | priorities [P] (host-space pods)
+    const size_t o_vic = P * sizeof(ks_preemption), o_prio = o_vic + n_vic * 4;
+    CU_TRY(s->st_pre.ensure(o_prio + P * 4));
+    uint8_t* stg = s->st_pre.as<uint8_t>();
+    if (out_space == KS_MEM_HOST) {
+        d_out = reinterpret_cast<ks_preemption*>(stg);
+        d_vic = out_victims ? reinterpret_cast<int32_t*>(stg + o_vic) : nullptr;
+    }
+    PodView pv{nullptr, nullptr, nullptr, (uint32_t)P};
+    VictimIndex vx{};
+    PreemptPartials part{};
+    DirectGrid g{};
+    if (s->N) {
+        rc = stage_pods(s, pods, st, &pv);
+        if (rc) return rc;
+        if (pods->mem_space == KS_MEM_HOST) {
+            CU_TRY(cudaMemcpyAsync(stg + o_prio, pod_priority, P * 4, cudaMemcpyHostToDevice, st));
+            d_prio = reinterpret_cast<const int32_t*>(stg + o_prio);
+        }
+        // the victim index: upload the bound list, sort it by (node, priority), prefix sums per node
+        CU_TRY(s->vx_pre.ensure(victim_index_bytes(B, s->N)));
+        if (B) {
+            const BoundUpload up = victim_index_inputs(s->vx_pre.p, B, s->N);
+            CU_TRY(cudaMemcpyAsync(up.node, bound->node_idx, B * 4, cudaMemcpyHostToDevice, st));
+            CU_TRY(cudaMemcpyAsync(up.cpu, bound->req_cpu, B * 8, cudaMemcpyHostToDevice, st));
+            CU_TRY(cudaMemcpyAsync(up.mem, bound->req_mem, B * 8, cudaMemcpyHostToDevice, st));
+            CU_TRY(cudaMemcpyAsync(up.prio, bound->priority, B * 4, cudaMemcpyHostToDevice, st));
+        }
+        CU_TRY(build_victim_index(s->vx_pre.p, B, s->N, &vx, st));
+        g = direct_grid(s->W, pv.P, s->Npad, s->sms);
+        const uint64_t rows = (uint64_t)g.n_chunks * P; // hi [rows] | lo [rows] | candidates [rows] | feasible [rows]
+        CU_TRY(s->part_pre.ensure(rows * 24));
+        uint8_t* b = s->part_pre.as<uint8_t>();
+        part.hi = reinterpret_cast<uint64_t*>(b);
+        part.lo = reinterpret_cast<uint64_t*>(b + rows * 8);
+        part.cand = reinterpret_cast<uint32_t*>(b + rows * 16);
+        part.cnt = reinterpret_cast<uint32_t*>(b + rows * 20);
+    }
+    CU_TRY(launch_preempt(node_table(s), pv, d_prio, vx, max_victims, part, g, d_out, d_vic, st));
+    if (out_space == KS_MEM_HOST) {
+        CU_TRY(cudaMemcpyAsync(out, d_out, P * sizeof(ks_preemption), cudaMemcpyDeviceToHost, st));
+        if (out_victims) CU_TRY(cudaMemcpyAsync(out_victims, d_vic, n_vic * 4, cudaMemcpyDeviceToHost, st));
     }
     if (out_space == KS_MEM_HOST || pods->mem_space == KS_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
     return KS_OK;

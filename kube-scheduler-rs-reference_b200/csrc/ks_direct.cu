@@ -5,7 +5,9 @@
 //                              one mask word, warp-shuffle argmax
 //   K2e k_explain_counts       per-pod rejection counts (ks_explain)
 //   K2k k_select_topk          per-pod ranked list of the k best feasible nodes (ks_select_topk), held across the warp
-// K2d, K2e and K2k share one node-tile scan (scan_node_tiles): tiles staged through shared memory by TMA bulk
+//   K2p k_preempt_scan         per-pod best preemption candidate (ks_preempt) over a per-call victim index;
+//       k_preempt_emit         chunk merge, victim list and ks_preemption row
+// K2d, K2e, K2k and K2p share one node-tile scan (scan_node_tiles): tiles staged through shared memory by TMA bulk
 // copies (cp.async.bulk + mbarrier), one lane per node, several pods per warp in registers.
 // The per-cell kernel is the generic path (any score policy, any P); ks_bitpar.cu holds the bit-parallel
 // fast path that the headline configuration uses.
@@ -589,6 +591,407 @@ __global__ void __launch_bounds__(256) k_topk_combine(PodView pv, OutView ov, Pa
     if (lane == 0 && ov.cnt) ov.cnt[p] = c;
 }
 
+// ------------------------------------------------------------------------------------------------ K2p (ks_preempt)
+// Steps 2-5 of ks_preempt (include/ksched.h) for one pod (priority pi, request rc/rm) on one node (free fc/fm, sorted
+// segment [s0, s1) of the victim index): the lower set is the segment's prefix below pi (binary search), the room check
+// reads its prefix sums, and the reprieve walk goes backwards from the prefix's end - priority descending, ties to the
+// lower bound index.  Returns whether the node is a candidate, with the victims' highest priority, priority sum (each
+// pi_b + 2^31) and count; when out is not null the victims' bound indices go to out[0..count).  The range rule of
+// ks_preempt keeps every sum below inside int64.
+__device__ __forceinline__ bool preempt_walk(const VictimIndex& vx, uint32_t s0, uint32_t s1, int32_t pi, int64_t rc,
+                                             int64_t rm, int64_t fc, int64_t fm, uint32_t max_victims, int32_t& vmax,
+                                             int64_t& vsum, uint32_t& vcnt, int32_t* out) {
+    uint32_t lo = s0, hi = s1;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (__ldg(vx.prio + mid) < pi) lo = mid + 1;
+        else hi = mid;
+    }
+    if (lo == s0) return false; // no pod of lower priority
+    int64_t ac = fc + __ldg(vx.pre_cpu + lo - 1), am = fm + __ldg(vx.pre_mem + lo - 1);
+    if (rc > ac || rm > am) return false; // evicting the whole lower set is not enough
+    vmax = INT32_MIN;
+    vsum = 0;
+    vcnt = 0;
+    for (uint32_t j = lo; j-- > s0;) {
+        const int64_t bc = __ldg(vx.cpu + j), bm = __ldg(vx.mem + j);
+        if (rc <= ac - bc && rm <= am - bm) { // still fits without evicting b: reprieved
+            ac -= bc;
+            am -= bm;
+            continue;
+        }
+        if (vcnt == max_victims) return false;
+        const int32_t bp = __ldg(vx.prio + j);
+        if (vcnt == 0) vmax = bp; // visited in descending priority: the first victim has the highest
+        if (out) out[vcnt] = (int32_t)__ldg(vx.idx + j);
+        vsum += (int64_t)bp + 2147483648ll;
+        vcnt++;
+    }
+    return true; // at least one victim: with none, the pod would fit free[] and the node would not be eligible
+}
+
+// Candidate scan (ks_preempt): per pod the feasible count (as K2d counts it), the number of candidate nodes and the
+// best candidate's key (preempt_key).  A cell goes to preempt_walk only when it fails on resources, its selector matches
+// and the node holds a pod of lower priority (min_prio, one coalesced load per node); the walk reads the node's segment
+// from L2.  Results go to partials [blockIdx.y][P], merged by k_preempt_emit.
+template <int W>
+__global__ void __launch_bounds__(DIRECT_THREADS)
+    k_preempt_scan(NodeTable nt, PodView pv, const int32_t* __restrict__ pod_prio, VictimIndex vx, uint32_t max_victims,
+                   PreemptPartials part, uint32_t tiles_per_chunk) {
+    constexpr int PW = pods_per_warp(W);
+    int64_t rc[PW], rm[PW];
+    uint64_t sel[PW][W];
+    uint32_t p0;
+    int32_t pi[PW];
+    uint64_t bhi[PW], blo[PW];
+    uint32_t cnt[PW], ncand[PW];
+    const uint32_t q0 = warp_first_pod<PW>(); // the p0 scan_node_tiles sets
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        pi[i] = __ldg(pod_prio + min(q0 + i, pv.P - 1));
+        bhi[i] = blo[i] = PREEMPT_NONE;
+        cnt[i] = ncand[i] = 0;
+    }
+
+    scan_node_tiles<W, false>(
+        nt, tiles_per_chunk, pv, p0, rc, rm, sel,
+        [&](uint32_t, uint32_t node, bool real, int64_t fc, int64_t fm, const uint64_t(&lab)[W], int64_t, int64_t) {
+            const int32_t mp = real ? __ldg(vx.min_prio + node) : INT32_MAX; // padding: never a candidate
+#pragma unroll
+            for (int i = 0; i < PW; i++) {
+                const bool fit = (rc[i] <= fc) & (rm[i] <= fm);
+                uint64_t miss = 0;
+#pragma unroll
+                for (int w = 0; w < W; w++) miss |= sel[i][w] & ~lab[w];
+                cnt[i] += __popc(__ballot_sync(0xffffffffu, fit && (miss == 0) && real));
+                if (!fit && miss == 0 && mp < pi[i]) {
+                    int32_t vmax;
+                    int64_t vsum;
+                    uint32_t vcnt;
+                    if (preempt_walk(vx, __ldg(vx.off + node), __ldg(vx.off + node + 1), pi[i], rc[i], rm[i], fc, fm,
+                                     max_victims, vmax, vsum, vcnt, nullptr)) {
+                        uint64_t h, l;
+                        preempt_key(vmax, vsum, vcnt, node, h, l);
+                        ncand[i]++;
+                        if (preempt_less(h, l, bhi[i], blo[i])) {
+                            bhi[i] = h;
+                            blo[i] = l;
+                        }
+                    }
+                }
+            }
+        },
+        [](uint32_t) {});
+
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        uint64_t h = bhi[i], l = blo[i];
+        warp_preempt_min(h, l);
+        const uint32_t c = __reduce_add_sync(0xffffffffu, ncand[i]);
+        const uint32_t p = p0 + i;
+        if ((threadIdx.x & 31) == 0 && p < pv.P) {
+            const uint64_t o = (uint64_t)blockIdx.y * pv.P + p;
+            part.hi[o] = h;
+            part.lo[o] = l;
+            part.cand[o] = c;
+            part.cnt[o] = cnt[i];
+        }
+    }
+}
+
+// One thread per pod: merge the node chunks in ascending order, apply "already fits => no plan", walk the chosen node
+// once more to list the victims, and write the ks_preemption row.  n_chunks = 0 (no node) gives every pod no plan.
+__global__ void __launch_bounds__(256)
+    k_preempt_emit(NodeTable nt, PodView pv, const int32_t* __restrict__ pod_prio, VictimIndex vx, uint32_t max_victims,
+                   PreemptPartials part, uint32_t n_chunks, ks_preemption* __restrict__ out, int32_t* __restrict__ victims) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= pv.P) return;
+    uint64_t hi = PREEMPT_NONE, lo = PREEMPT_NONE;
+    uint32_t cand = 0, cnt = 0;
+    for (uint32_t ch = 0; ch < n_chunks; ch++) {
+        const uint64_t o = (uint64_t)ch * pv.P + p;
+        cnt += part.cnt[o];
+        cand += part.cand[o];
+        if (preempt_less(part.hi[o], part.lo[o], hi, lo)) {
+            hi = part.hi[o];
+            lo = part.lo[o];
+        }
+    }
+    ks_preemption r;
+    r.node_idx = -1;
+    r.n_victims = 0;
+    r.candidates = cnt ? 0u : cand;
+    r.feasible_cnt = cnt;
+    r.max_victim_priority = INT32_MIN;
+    r.reserved = 0;
+    r.victim_priority_sum = 0;
+    int32_t* v = victims ? victims + (uint64_t)p * max_victims : nullptr;
+    if (cnt == 0 && hi != PREEMPT_NONE) {
+        const uint32_t node = (uint32_t)(lo & 0xffffffffffffull);
+        int32_t vmax;
+        int64_t vsum;
+        uint32_t vcnt;
+        if (preempt_walk(vx, vx.off[node], vx.off[node + 1], pod_prio[p], pv.req_cpu[p], pv.req_mem[p],
+                         nt.free_cpu[node], nt.free_mem[node], max_victims, vmax, vsum, vcnt, v)) {
+            r.node_idx = (int32_t)node;
+            r.n_victims = vcnt;
+            r.max_victim_priority = vmax;
+            r.victim_priority_sum = vsum;
+        }
+    }
+    if (v)
+        for (uint32_t j = r.n_victims; j < max_victims; j++) v[j] = -1;
+    out[p] = r;
+}
+
+// ---- the victim index, built per call: a stable LSD radix sort of (node << 32 | priority + 2^31) keys over the bound
+// list fed in descending bound index, then segment offsets, prefix sums and per-node minimum priorities.
+constexpr uint32_t RADIX_TILE = 2048; // keys per CTA of a radix pass (256 threads x 8 rounds)
+
+__global__ void __launch_bounds__(256)
+    k_victim_keys(const int32_t* __restrict__ bnode, const int32_t* __restrict__ bprio, uint64_t* __restrict__ key,
+                  uint32_t* __restrict__ val, uint64_t B) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < B; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t b = B - 1 - i; // reversed: the stable sort leaves ties in descending bound index
+        key[i] = ((uint64_t)(uint32_t)bnode[b] << 32) | ((uint32_t)bprio[b] ^ 0x80000000u);
+        val[i] = (uint32_t)b;
+    }
+}
+
+// per CTA tile: counts of each 8-bit digit, stored digit-major (hist[d * nblk + tile]) so that one exclusive scan over
+// the whole array gives every (digit, tile) its first output position
+__global__ void __launch_bounds__(256)
+    k_radix_hist(const uint64_t* __restrict__ key, uint64_t B, uint32_t shift, uint32_t* __restrict__ hist, uint32_t nblk) {
+    __shared__ uint32_t h[256];
+    h[threadIdx.x] = 0;
+    __syncthreads();
+    const uint64_t base = (uint64_t)blockIdx.x * RADIX_TILE;
+    for (uint32_t j = threadIdx.x; j < RADIX_TILE; j += 256)
+        if (base + j < B) atomicAdd(&h[(uint32_t)(key[base + j] >> shift) & 255u], 1u);
+    __syncthreads();
+    hist[(uint64_t)threadIdx.x * nblk + blockIdx.x] = h[threadIdx.x];
+}
+
+// one CTA: exclusive scan of n counts in place (each thread scans a contiguous run, then the run totals are scanned)
+__global__ void __launch_bounds__(1024) k_radix_scan(uint32_t* __restrict__ a, uint32_t n) {
+    __shared__ uint32_t tot[1024];
+    const uint32_t per = (n + 1023) / 1024, b = threadIdx.x * per, e = min(b + per, n);
+    uint32_t s = 0;
+    for (uint32_t i = b; i < e; i++) s += a[i];
+    tot[threadIdx.x] = s;
+    __syncthreads();
+    for (uint32_t off = 1; off < 1024; off <<= 1) { // Hillis-Steele over the run totals
+        const uint32_t v = threadIdx.x >= off ? tot[threadIdx.x - off] : 0;
+        __syncthreads();
+        tot[threadIdx.x] += v;
+        __syncthreads();
+    }
+    uint32_t run = tot[threadIdx.x] - s;
+    for (uint32_t i = b; i < e; i++) {
+        const uint32_t x = a[i];
+        a[i] = run;
+        run += x;
+    }
+}
+
+// Stable scatter of one radix pass.  A CTA takes its tile in rounds of 256 keys in order; within a round, warps hold
+// consecutive keys and peers of a digit are ranked by lane (match_any), so every key lands after all earlier keys of its
+// digit: the pass is stable.
+__global__ void __launch_bounds__(256)
+    k_radix_scatter(const uint64_t* __restrict__ kin, const uint32_t* __restrict__ vin, uint64_t* __restrict__ kout,
+                    uint32_t* __restrict__ vout, uint64_t B, uint32_t shift, const uint32_t* __restrict__ hist,
+                    uint32_t nblk) {
+    __shared__ uint32_t base[256];
+    __shared__ uint32_t wcnt[8][256];
+    const uint32_t t = threadIdx.x, lane = t & 31, w = t >> 5;
+    base[t] = hist[(uint64_t)t * nblk + blockIdx.x];
+#pragma unroll
+    for (int q = 0; q < 8; q++) wcnt[q][t] = 0;
+    __syncthreads();
+    const uint64_t tile = (uint64_t)blockIdx.x * RADIX_TILE;
+    for (uint32_t r = 0; r < RADIX_TILE / 256; r++) {
+        const uint64_t i = tile + r * 256 + t;
+        const bool valid = i < B;
+        const uint64_t k = valid ? kin[i] : 0;
+        const uint32_t v = valid ? vin[i] : 0;
+        const uint32_t d = (uint32_t)(k >> shift) & 255u;
+        const uint32_t peers = __match_any_sync(0xffffffffu, valid ? d : 256u);
+        const uint32_t rank = __popc(peers & ((1u << lane) - 1u));
+        if (valid && rank == 0) wcnt[w][d] = __popc(peers);
+        __syncthreads();
+        if (valid) {
+            uint32_t pos = base[d] + rank;
+            for (uint32_t q = 0; q < w; q++) pos += wcnt[q][d];
+            kout[pos] = k;
+            vout[pos] = v;
+        }
+        __syncthreads();
+        uint32_t add = 0;
+#pragma unroll
+        for (int q = 0; q < 8; q++) {
+            add += wcnt[q][t];
+            wcnt[q][t] = 0;
+        }
+        base[t] += add;
+        __syncthreads();
+    }
+}
+
+// sorted arrays: priority (from the key), requests gathered by bound index
+__global__ void __launch_bounds__(256)
+    k_victim_gather(const uint64_t* __restrict__ key, const uint32_t* __restrict__ val, const int64_t* __restrict__ bcpu,
+                    const int64_t* __restrict__ bmem, int32_t* __restrict__ prio, int64_t* __restrict__ cpu,
+                    int64_t* __restrict__ mem, uint64_t B) {
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < B; j += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t b = val[j];
+        prio[j] = (int32_t)((uint32_t)key[j] ^ 0x80000000u);
+        cpu[j] = bcpu[b];
+        mem[j] = bmem[b];
+    }
+}
+
+// off[n] = first sorted position of node n (n = N gives B): a binary search over the sorted keys
+__global__ void __launch_bounds__(256)
+    k_victim_offsets(const uint64_t* __restrict__ key, uint64_t B, uint32_t N, uint32_t* __restrict__ off) {
+    const uint32_t n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n > N) return;
+    const uint64_t want = (uint64_t)n << 32;
+    uint64_t lo = 0, hi = B;
+    while (lo < hi) {
+        const uint64_t mid = (lo + hi) >> 1;
+        if (key[mid] < want) lo = mid + 1;
+        else hi = mid;
+    }
+    off[n] = (uint32_t)lo;
+}
+
+// one warp per node: inclusive prefix sums of the segment's requests, 32 at a time, and its lowest priority
+__global__ void __launch_bounds__(256)
+    k_victim_prefix(const uint32_t* __restrict__ off, const int32_t* __restrict__ prio, const int64_t* __restrict__ cpu,
+                    const int64_t* __restrict__ mem, int64_t* __restrict__ pre_cpu, int64_t* __restrict__ pre_mem,
+                    int32_t* __restrict__ min_prio, uint32_t N) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (n >= N) return; // warp-uniform
+    const uint32_t s0 = off[n], s1 = off[n + 1];
+    int64_t carry_c = 0, carry_m = 0;
+    for (uint32_t j0 = s0; j0 < s1; j0 += 32) {
+        const uint32_t j = j0 + lane;
+        int64_t c = j < s1 ? cpu[j] : 0, m = j < s1 ? mem[j] : 0;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const int64_t uc = __shfl_up_sync(0xffffffffu, c, d), um = __shfl_up_sync(0xffffffffu, m, d);
+            if (lane >= (uint32_t)d) {
+                c += uc;
+                m += um;
+            }
+        }
+        if (j < s1) {
+            pre_cpu[j] = carry_c + c;
+            pre_mem[j] = carry_m + m;
+        }
+        carry_c += __shfl_sync(0xffffffffu, c, 31);
+        carry_m += __shfl_sync(0xffffffffu, m, 31);
+    }
+    if (lane == 0) min_prio[n] = s1 > s0 ? prio[s0] : INT32_MAX;
+}
+
+// scratch layout: the upload, two key/value buffers of the sort, the digit counts, then the index itself
+struct VictimLayout {
+    size_t node, cpu, mem, prio, key[2], val[2], hist, s_prio, s_cpu, s_mem, pre_cpu, pre_mem, off, min_prio, total;
+    uint32_t nblk;
+};
+static VictimLayout victim_layout(uint64_t B, uint32_t N) {
+    VictimLayout L;
+    size_t o = 0;
+    auto take = [&o](size_t bytes) {
+        const size_t at = o;
+        o += (bytes + 255) & ~(size_t)255;
+        return at;
+    };
+    L.nblk = (uint32_t)((B + RADIX_TILE - 1) / RADIX_TILE);
+    L.node = take(B * 4);
+    L.cpu = take(B * 8);
+    L.mem = take(B * 8);
+    L.prio = take(B * 4);
+    L.key[0] = take(B * 8);
+    L.key[1] = take(B * 8);
+    L.val[0] = take(B * 4);
+    L.val[1] = take(B * 4);
+    L.hist = take((size_t)256 * L.nblk * 4);
+    L.s_prio = take(B * 4);
+    L.s_cpu = take(B * 8);
+    L.s_mem = take(B * 8);
+    L.pre_cpu = take(B * 8);
+    L.pre_mem = take(B * 8);
+    L.off = take(((size_t)N + 1) * 4);
+    L.min_prio = take((size_t)N * 4);
+    L.total = o;
+    return L;
+}
+
+size_t victim_index_bytes(uint64_t B, uint32_t N) { return victim_layout(B, N).total; }
+
+BoundUpload victim_index_inputs(void* scratch, uint64_t B, uint32_t N) {
+    const VictimLayout L = victim_layout(B, N);
+    unsigned char* s = static_cast<unsigned char*>(scratch);
+    return BoundUpload{reinterpret_cast<int32_t*>(s + L.node), reinterpret_cast<int64_t*>(s + L.cpu),
+                       reinterpret_cast<int64_t*>(s + L.mem), reinterpret_cast<int32_t*>(s + L.prio)};
+}
+
+cudaError_t build_victim_index(void* scratch, uint64_t B, uint32_t N, VictimIndex* vx, cudaStream_t st) {
+    const VictimLayout L = victim_layout(B, N);
+    unsigned char* s = static_cast<unsigned char*>(scratch);
+    auto at = [s](size_t o) { return static_cast<void*>(s + o); };
+    uint64_t* key[2] = {static_cast<uint64_t*>(at(L.key[0])), static_cast<uint64_t*>(at(L.key[1]))};
+    uint32_t* val[2] = {static_cast<uint32_t*>(at(L.val[0])), static_cast<uint32_t*>(at(L.val[1]))};
+    int cur = 0;
+    const uint32_t grid_b = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(4096, (B + 255) / 256));
+    cudaError_t e;
+    if (B) {
+        k_victim_keys<<<grid_b, 256, 0, st>>>(static_cast<const int32_t*>(at(L.node)), static_cast<const int32_t*>(at(L.prio)),
+                                              key[0], val[0], B);
+        g_launches++;
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        // priority bits [0, 32), then as many node bits as N needs
+        const uint32_t node_bits = N > 1 ? 32u - (uint32_t)__builtin_clz(N - 1) : 0u;
+        for (uint32_t shift = 0; shift < 32 + node_bits; shift += 8) {
+            uint32_t* hist = static_cast<uint32_t*>(at(L.hist));
+            k_radix_hist<<<L.nblk, 256, 0, st>>>(key[cur], B, shift, hist, L.nblk);
+            k_radix_scan<<<1, 1024, 0, st>>>(hist, 256 * L.nblk);
+            k_radix_scatter<<<L.nblk, 256, 0, st>>>(key[cur], val[cur], key[cur ^ 1], val[cur ^ 1], B, shift, hist, L.nblk);
+            g_launches += 3;
+            if ((e = cudaGetLastError()) != cudaSuccess) return e;
+            cur ^= 1;
+        }
+        k_victim_gather<<<grid_b, 256, 0, st>>>(key[cur], val[cur], static_cast<const int64_t*>(at(L.cpu)),
+                                                static_cast<const int64_t*>(at(L.mem)), static_cast<int32_t*>(at(L.s_prio)),
+                                                static_cast<int64_t*>(at(L.s_cpu)), static_cast<int64_t*>(at(L.s_mem)), B);
+        g_launches++;
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+    k_victim_offsets<<<(N + 1 + 255) / 256, 256, 0, st>>>(key[cur], B, N, static_cast<uint32_t*>(at(L.off)));
+    g_launches++;
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if (N) {
+        k_victim_prefix<<<(N + 7) / 8, 256, 0, st>>>(
+            static_cast<const uint32_t*>(at(L.off)), static_cast<const int32_t*>(at(L.s_prio)),
+            static_cast<const int64_t*>(at(L.s_cpu)), static_cast<const int64_t*>(at(L.s_mem)),
+            static_cast<int64_t*>(at(L.pre_cpu)), static_cast<int64_t*>(at(L.pre_mem)), static_cast<int32_t*>(at(L.min_prio)), N);
+        g_launches++;
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+    vx->off = static_cast<const uint32_t*>(at(L.off));
+    vx->min_prio = static_cast<const int32_t*>(at(L.min_prio));
+    vx->prio = static_cast<const int32_t*>(at(L.s_prio));
+    vx->cpu = static_cast<const int64_t*>(at(L.s_cpu));
+    vx->mem = static_cast<const int64_t*>(at(L.s_mem));
+    vx->pre_cpu = static_cast<const int64_t*>(at(L.pre_cpu));
+    vx->pre_mem = static_cast<const int64_t*>(at(L.pre_mem));
+    vx->idx = val[cur];
+    return cudaSuccess;
+}
+
 // node chunks across gridDim.y when the pods alone give fewer than two CTAs per SM
 DirectGrid direct_grid(uint32_t W, uint32_t P, uint32_t Npad, int sms) {
     const uint32_t pods_per_cta = (DIRECT_THREADS / 32) * pods_per_warp(W);
@@ -620,6 +1023,7 @@ cudaError_t prepare_direct() {
             opt_in(k_explain_counts<W_>, tile_smem_bytes<W_, false>());
             opt_in(k_select_topk<W_, LO>, tile_smem_bytes<W_, false>());
             opt_in(k_select_topk<W_, LA>, tile_smem_bytes<W_, true>());
+            opt_in(k_preempt_scan<W_>, tile_smem_bytes<W_, false>());
             return e;
         });
     return e;
@@ -687,6 +1091,27 @@ cudaError_t launch_select_topk(const NodeTable& nt, const PodView& pv, int polic
         return policy == KS_SCORE_LEFTOVER ? launch_topk_t<W, KS_SCORE_LEFTOVER>(nt, pv, k, ov, part, g, st)
                                            : launch_topk_t<W, KS_SCORE_LEAST_ALLOCATED>(nt, pv, k, ov, part, g, st);
     });
+}
+
+cudaError_t launch_preempt(const NodeTable& nt, const PodView& pv, const int32_t* pod_prio, const VictimIndex& vx,
+                           uint32_t max_victims, const PreemptPartials& part, const DirectGrid& g, ks_preemption* out,
+                           int32_t* victims, cudaStream_t st) {
+    if (pv.P == 0) return cudaSuccess;
+    uint32_t n_chunks = 0;
+    if (nt.N > 0) {
+        const cudaError_t e = with_label_width(nt.W, [&](auto w) {
+            constexpr int W = decltype(w)::value;
+            k_preempt_scan<W><<<dim3(g.pod_ctas, g.n_chunks), DIRECT_THREADS, tile_smem_bytes<W, false>(), st>>>(
+                nt, pv, pod_prio, vx, max_victims, part, g.tiles_per_chunk);
+            g_launches++;
+            return cudaGetLastError();
+        });
+        if (e != cudaSuccess) return e;
+        n_chunks = g.n_chunks;
+    }
+    k_preempt_emit<<<(pv.P + 255) / 256, 256, 0, st>>>(nt, pv, pod_prio, vx, max_victims, part, n_chunks, out, victims);
+    g_launches++;
+    return cudaGetLastError();
 }
 
 } // namespace ks

@@ -150,6 +150,31 @@ __device__ __forceinline__ void warp_topk_insert(int64_t& key, int32_t& idx, int
         idx = lane == pos ? ci : ui;
     }
 }
+// Priority preemption (ks_preempt): a candidate node as one 128-bit key (hi, lo) whose unsigned order is the plan's node
+// order - the victims' highest priority, then their priority sum, then their count, then the node index, lowest first.
+// hi = (max priority + 2^31) << 32 | sum >> 8 and lo = (sum & 255) << 56 | count << 48 | node, which is exact because
+// the sum of at most 128 values below 2^32 stays below 2^39.  "No candidate" is (~0, ~0), above every key.
+constexpr uint64_t PREEMPT_NONE = ~0ull;
+__device__ __forceinline__ void preempt_key(int32_t vmax, int64_t vsum, uint32_t vcnt, uint32_t node, uint64_t& hi,
+                                            uint64_t& lo) {
+    hi = ((uint64_t)((uint32_t)vmax ^ 0x80000000u) << 32) | ((uint64_t)vsum >> 8);
+    lo = ((uint64_t)vsum << 56) | ((uint64_t)vcnt << 48) | node;
+}
+__device__ __forceinline__ bool preempt_less(uint64_t ahi, uint64_t alo, uint64_t bhi, uint64_t blo) {
+    return ahi < bhi || (ahi == bhi && alo < blo);
+}
+// Warp minimum of the keys above; every lane ends with the result.
+__device__ __forceinline__ void warp_preempt_min(uint64_t& hi, uint64_t& lo) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        const uint64_t oh = __shfl_xor_sync(0xffffffffu, hi, off);
+        const uint64_t ol = __shfl_xor_sync(0xffffffffu, lo, off);
+        if (preempt_less(oh, ol, hi, lo)) {
+            hi = oh;
+            lo = ol;
+        }
+    }
+}
 
 // Label-width dispatch: calls f(std::integral_constant<int, W>{}) for W in {1, 2, 4, 8}; any other W is invalid.
 template <class F>

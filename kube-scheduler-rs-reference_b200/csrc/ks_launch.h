@@ -32,6 +32,40 @@ cudaError_t launch_explain_counts(const NodeTable& nt, const PodView& pv, uint32
 cudaError_t launch_select_topk(const NodeTable& nt, const PodView& pv, int policy, uint32_t k, const OutView& ov,
                                const PartialView& part, const DirectGrid& g, cudaStream_t st);
 
+// priority preemption (ks_preempt).  The victim index: the bound list sorted by (node, priority ascending), ties by
+// descending bound index, so that walking a node's segment backwards visits priority descending, ties to the lower
+// bound index.  Device memory, B bound pods, N nodes.
+struct VictimIndex {
+    const uint32_t* off;     // [N+1]: node n's segment is [off[n], off[n+1])
+    const int32_t* min_prio; // [N]: lowest priority on node n, INT32_MAX when it has no pod
+    const int32_t* prio;     // [B] sorted
+    const int64_t* cpu;      // [B] requests, sorted
+    const int64_t* mem;
+    const int64_t* pre_cpu;  // [B] inclusive prefix sums of the requests within each segment
+    const int64_t* pre_mem;
+    const uint32_t* idx;     // [B] bound index
+};
+struct BoundUpload { // where the host list is copied before build_victim_index
+    int32_t* node;
+    int64_t* cpu;
+    int64_t* mem;
+    int32_t* prio;
+};
+size_t victim_index_bytes(uint64_t B, uint32_t N); // one scratch block holds the upload, the sort and the index
+BoundUpload victim_index_inputs(void* scratch, uint64_t B, uint32_t N);
+cudaError_t build_victim_index(void* scratch, uint64_t B, uint32_t N, VictimIndex* vx, cudaStream_t st);
+// per-(node chunk, pod) results of the scan, [n_chunks][P]
+struct PreemptPartials {
+    uint64_t* hi; // best candidate key (preempt_key), PREEMPT_NONE when none
+    uint64_t* lo;
+    uint32_t* cand; // candidate nodes
+    uint32_t* cnt;  // feasible nodes
+};
+// out[P] and victims[P * max_victims] (may be null), device memory.  With nt.N == 0 only the rows are written (no plan).
+cudaError_t launch_preempt(const NodeTable& nt, const PodView& pv, const int32_t* pod_prio, const VictimIndex& vx,
+                           uint32_t max_victims, const PreemptPartials& part, const DirectGrid& g, ks_preemption* out,
+                           int32_t* victims, cudaStream_t st);
+
 } // namespace ks
 
 namespace ks {

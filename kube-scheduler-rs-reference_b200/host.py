@@ -37,6 +37,8 @@ for _name, _res, _args in [
     ("ksh_reconcile", C.c_int, [_vp, _vp, C.c_int, C.POINTER(C.c_int32), C.c_char_p, C.c_size_t]),
     ("ksh_explain_pods", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, C.c_size_t, _vp]),
     ("ksh_format_unschedulable", C.c_int, [C.c_uint32, C.POINTER(capi.ks_pod_reasons), _vp, C.c_size_t]),
+    ("ksh_context_set_pod_priorities", C.c_int, [_vp, _vp, _vp, C.c_uint64]),
+    ("ksh_preempt_pods", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, _vp, C.c_size_t, _vp]),
 ]:
     _f = getattr(lib, _name)
     _f.restype = _res
@@ -229,6 +231,37 @@ class Context:
         if rc != capi.KS_OK:
             raise KsError(rc, "ksh_explain_pods")
         return out, [None if o < 0 else C.string_at(C.addressof(buf) + int(o)).decode() for o in off]
+
+    def set_pod_priorities(self, pods, priority, n, first=0):
+        """spec.priority of bound pods known by namespace/name (others are ignored)."""
+        priority = np.ascontiguousarray(priority, np.int32)
+        rc = lib.ksh_context_set_pod_priorities(self._h, _addr(pods, first), priority.ctypes.data, n)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ksh_context_set_pod_priorities")
+
+    def preempt_pods(self, pods, n, priority, max_victims, first=0, victims_cap=None):
+        """Priority preemption (ksh_preempt_pods): (rows PREEMPTION_DTYPE [n], victims[n]) where victims[i] is the list
+        of "namespace/name" keys to evict for pod i, in visit order, or None (no plan, or the buffer was full)."""
+        priority = np.ascontiguousarray(priority, np.int32)
+        rows = np.empty(n, capi.PREEMPTION_DTYPE)
+        off = np.empty(n, np.int64)
+        cap = int(victims_cap if victims_cap is not None else 64 * int(max_victims) * max(n, 1))
+        buf = C.create_string_buffer(max(cap, 1))
+        rc = lib.ksh_preempt_pods(self._h, _addr(pods, first), n, priority.ctypes.data, int(max_victims), rows.ctypes.data,
+                                  C.addressof(buf), cap, off.ctypes.data)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ksh_preempt_pods")
+        victims = []
+        for i, o in enumerate(off):
+            if o < 0:
+                victims.append(None)
+                continue
+            keys, at = [], C.addressof(buf) + int(o)
+            for _ in range(int(rows["n_victims"][i])):
+                keys.append(C.string_at(at).decode())
+                at += len(keys[-1].encode()) + 1
+            victims.append(keys)
+        return rows, victims
 
     def reconcile(self, pods, i, policy=capi.KS_SCORE_LEFTOVER):
         node = C.c_int32(-1)

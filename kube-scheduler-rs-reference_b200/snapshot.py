@@ -8,7 +8,7 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _capi as capi
-from ._capi import KsError, ks_bindings, ks_pods, lib
+from ._capi import KsError, ks_bindings, ks_bound_pods, ks_pods, lib
 
 
 def _ptr(a):
@@ -237,6 +237,39 @@ class Snapshot:
                                 int(out_space), C.c_void_p(stream) if stream else None)
         if rc != capi.KS_OK:
             raise KsError(rc, "ks_select_topk")
+
+    @staticmethod
+    def _bound(node_idx, req_cpu, req_mem, priority):
+        arrs = (_c(node_idx, np.int32), _c(req_cpu, np.int64), _c(req_mem, np.int64), _c(priority, np.int32))
+        return ks_bound_pods(arrs[0].shape[0], *[_ptr(a) for a in arrs]), arrs
+
+    def preempt(self, req_cpu, req_mem, sel, priority, bound_node, bound_cpu, bound_mem, bound_priority, max_victims):
+        """Priority preemption (ks_preempt) over host (numpy) pods.  The bound list (node, requests, priority) must be
+        the one that produced free[].  Returns (rows, victims): rows = PREEMPTION_DTYPE records [P] (node_idx -1 = no
+        plan), victims = int32 [P, max_victims] bound indices in visit order, -1 past n_victims."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        priority = _c(priority, np.int32)
+        bound, keep_b = self._bound(bound_node, bound_cpu, bound_mem, bound_priority)
+        p = int(pods.n)
+        rows = np.empty(p, capi.PREEMPTION_DTYPE)
+        victims = np.empty((p, int(max_victims)), np.int32)
+        rc = lib.ks_preempt(self._h, C.byref(pods), _ptr(priority), C.byref(bound), int(max_victims), _ptr(rows),
+                            _ptr(victims), capi.KS_MEM_HOST, None)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ks_preempt")
+        return rows, victims
+
+    def preempt_raw(self, n_pods, req_cpu, req_mem, sel, pods_space, priority, bound, max_victims, out, victims,
+                    out_space, stream=None):
+        """Pointer-level ks_preempt (torch tensors / raw addresses): priority in pods_space; bound = (node, cpu, mem,
+        priority) host arrays; out holds n_pods x 32 bytes, victims n_pods x max_victims int32 (may be None).  With device
+        pods and outputs the call returns after enqueue on `stream`."""
+        pods = ks_pods(int(n_pods), _ptr(req_cpu), _ptr(req_mem), _ptr(sel), int(pods_space))
+        b, keep_b = self._bound(*bound)
+        rc = lib.ks_preempt(self._h, C.byref(pods), _ptr(priority), C.byref(b), int(max_victims), _ptr(out),
+                            _ptr(victims), int(out_space), C.c_void_p(stream) if stream else None)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ks_preempt")
 
     def last_timings(self):
         ms = (C.c_float * 3)()
