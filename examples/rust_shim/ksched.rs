@@ -208,6 +208,49 @@ impl Gpu {
         }
         Ok(Some((node, keys)))
     }
+
+    /// Pod groups, all or nothing (upstream coscheduling's PodGroup `minMember`): `groups` holds each group's pods
+    /// and min_member, in order.  Per pod: Ok(Some(body)) = bind, Ok(None) = already bound (counts toward its group),
+    /// Err(1) = NoNodeFound in a group that committed, Err(2) = CreateBindingObjectFailed, Err(4) = the group rolled
+    /// back (nothing charged).  Outer Err = the library's status (bad offsets or sizes, no device).
+    pub fn reconcile_gangs(&self, groups: &[(&[corev1::Pod], u32)]) -> Result<Vec<Result<Option<String>, i32>>, i32> {
+        let views: Vec<PodView> = groups.iter().flat_map(|(pods, _)| pods.iter().map(PodView::new)).collect();
+        // ks_pod_obj is plain pointers into `views`, which outlive the call
+        let objs: Vec<ks_pod_obj> = views.iter().map(|v| unsafe { ptr::read(&v.obj) }).collect();
+        let mut offset = vec![0u64];
+        for (pods, _) in groups {
+            offset.push(offset.last().unwrap() + pods.len() as u64);
+        }
+        let min_member: Vec<u32> = groups.iter().map(|(_, m)| *m).collect();
+        let n = objs.len();
+        let (mut status, mut idx, mut off) = (vec![0i32; n], vec![-1i32; n], vec![-1i64; n]);
+        // room for every body: {"apiVersion":"v1","kind":"Binding","metadata":<ObjectMeta JSON>,"target":{"name":"<node>"}}
+        // with the longest node name JSON-escaped at worst 6 bytes per character, and the NUL
+        let longest_node = (0..unsafe { ksh_context_num_nodes(self.ctx) })
+            .map(|k| unsafe { CStr::from_ptr(ksh_context_node_name(self.ctx, k)) }.to_bytes().len())
+            .max()
+            .unwrap_or(0);
+        let cap: usize = views.iter()
+            .map(|v| unsafe { CStr::from_ptr(v.obj.metadata_json) }.to_bytes().len() + 6 * longest_node + 128)
+            .sum();
+        let mut buf = vec![0u8; cap.max(1)];
+        let rc = unsafe {
+            ksh_reconcile_gangs(self.ctx, objs.as_ptr(), n as u64, offset.as_ptr(), groups.len() as u64, min_member.as_ptr(),
+                                KS_SCORE_LEFTOVER, status.as_mut_ptr(), idx.as_mut_ptr(), ptr::null_mut(),
+                                buf.as_mut_ptr() as *mut c_char, buf.len(), off.as_mut_ptr())
+        };
+        if rc != KS_OK {
+            return Err(rc);
+        }
+        Ok((0..n).map(|i| match status[i] {
+            KSH_RECONCILE_OK if idx[i] < 0 => Ok(None), // already running
+            // bound and charged: the buffer holds every body, so a missing one is a broken invariant, not a skip
+            KSH_RECONCILE_OK if off[i] < 0 => panic!("ksh_reconcile_gangs bound pod {} but returned no Binding body", i),
+            KSH_RECONCILE_OK => Ok(Some(unsafe { CStr::from_ptr(buf.as_ptr().add(off[i] as usize) as *const c_char) }
+                .to_string_lossy().into_owned())),
+            e => Err(e),
+        }).collect())
+    }
 }
 
 impl Drop for Gpu {

@@ -24,10 +24,12 @@ pub const KS_CELL_NODE_SELECTOR_MISMATCH: c_int = 2; // InvalidNodeReason::NodeS
 pub const KSH_RECONCILE_OK: c_int = 0;
 pub const KSH_RECONCILE_NO_NODE_FOUND: c_int = 1; // ReconcileError::NoNodeFound (src/error.rs)
 pub const KSH_RECONCILE_BINDING_OBJECT_FAILED: c_int = 2; // ReconcileError::CreateBindingObjectFailed
+pub const KSH_RECONCILE_GANG_UNSATISFIED: c_int = 4; // ksh_reconcile_gangs: the pod's group rolled back
 pub const KS_REFERENCE_ATTEMPTS: u32 = 5; // ATTEMPTS, src/main.rs:49
 pub const KS_MAX_PEERS: usize = 15;
 pub const KS_TOPK_MAX: u32 = 32; // largest k of ks_select_topk / ksh_rank_nodes
 pub const KS_PREEMPT_MAX_VICTIMS: u32 = 128; // largest max_victims of ks_preempt / ksh_preempt_pods
+pub const KS_GANG_MAX_SIZE: u32 = 1024; // most pods in one group of ks_gang_bind / ksh_reconcile_gangs
 
 #[repr(C)]
 pub struct ks_kv {
@@ -121,6 +123,12 @@ pub struct ks_preemption {
     pub reserved: u32,
     pub victim_priority_sum: i64,
 }
+#[repr(C)]
+pub struct ks_gangs {
+    pub n: u64,
+    pub offset: *const u64,
+    pub min_member: *const u32,
+}
 pub enum ks_snapshot {}
 pub enum ks_stream {}
 pub enum ksh_context {}
@@ -150,6 +158,8 @@ extern "C" {
                       stream: *mut c_void) -> c_int;
     pub fn ks_snapshot_commit_claims(s: *mut ks_snapshot, n: u64, node: *const i32, cpu: *const i64, mem: *const i64, accepted: *mut u8) -> c_int;
     pub fn ks_stream_bind(s: *mut ks_snapshot, pods: *const ks_pods, policy: c_int, node_idx: *mut i32, score: *mut i64, rounds: *mut u32) -> c_int;
+    pub fn ks_gang_bind(s: *mut ks_snapshot, pods: *const ks_pods, gangs: *const ks_gangs, policy: c_int, node_idx: *mut i32,
+                        score: *mut i64, placed: *mut u32, rounds: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -172,6 +182,7 @@ extern "C" {
     pub fn ksh_context_pod_bound(ctx: *mut ksh_context, pod: *const ks_pod_obj) -> c_int;
     pub fn ksh_context_pod_deleted(ctx: *mut ksh_context, pod: *const ks_pod_obj) -> c_int;
     pub fn ksh_context_node_name(ctx: *const ksh_context, node_idx: u32) -> *const c_char;
+    pub fn ksh_context_num_nodes(ctx: *const ksh_context) -> u32;
     pub fn ksh_total_pod_resources(pod: *const ks_pod_obj, cpu: *mut i64, mem: *mut i64) -> c_int;
     pub fn ksh_is_pod_bound(pod: *const ks_pod_obj) -> c_int;
     pub fn ksh_check_node_validity(ctx: *mut ksh_context, pod: *const ks_pod_obj, node_idx: u32) -> c_int;
@@ -189,6 +200,9 @@ extern "C" {
                          binding_json: *mut c_char, cap: usize) -> c_int;
     pub fn ksh_reconcile_batch(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, policy: c_int, status: *mut i32,
                                node_idx: *mut i32, json: *mut c_char, cap: usize, json_off: *mut i64, rounds: *mut u32) -> c_int;
+    pub fn ksh_reconcile_gangs(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group_offset: *const u64, n_groups: u64,
+                               min_member: *const u32, policy: c_int, status: *mut i32, node_idx: *mut i32, placed: *mut u32,
+                               json: *mut c_char, cap: usize, json_off: *mut i64) -> c_int;
     pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,
                             messages: *mut c_char, cap: usize, msg_off: *mut i64) -> c_int;
     pub fn ksh_format_unschedulable(n_nodes: u32, r: *const ks_pod_reasons, buf: *mut c_char, cap: usize) -> c_int;

@@ -192,6 +192,37 @@ int ks_snapshot_commit_claims(ks_snapshot* s, uint64_t n_claims, const int32_t* 
 int ks_stream_bind(ks_snapshot* s, const ks_pods* pods /* host space */, int policy, int32_t* out_node_idx,
                    int64_t* out_score, uint32_t* out_rounds);
 
+/* ---- pod groups, all-or-nothing (gang scheduling; upstream's coscheduling PodGroup minMember; spec extension,
+ * DESIGN.md 5e) ----
+ * Pods arrive in array order and are cut into groups: group g is the pods [offset[g], offset[g+1]), 1 to
+ * KS_GANG_MAX_SIZE of them, with 0 <= min_member[g] <= its size.  Groups run in order, each against free[] as the
+ * earlier groups left it:
+ *   1. the ks_stream_bind micro-batch loop runs over the group's pods, unchanged: every round selects against the
+ *      current free[] under `policy`, claims are accepted per node in arrival order while they fit, losers retry; the
+ *      loop ends when no pod is pending (or after size + 2 rounds, which never binds);  placed[g] = pods it bound;
+ *   2. placed[g] >= min_member[g]: the group commits; its placed pods keep their nodes and scores and stay charged,
+ *      the others get -1 / 0 (NoNodeFound);
+ *   3. otherwise it rolls back: every pod of the group gets -1 / 0 and free[] is restored bit for bit to its value
+ *      before the group, so the next group sees exactly what this one saw.
+ * So one group with min_member 0 is ks_stream_bind (same bindings, scores and final free[]), and singleton groups
+ * give every pod the binds of all earlier pods (the reference's sequential reconcile, with the argmax).  Placement
+ * inside a group is the stream loop's greedy, not a bin-packing search: a group can fail where another assignment
+ * would have fitted (upstream coscheduling does not search either).
+ * One H2D copy, one cooperative launch that walks every group on the device, one D2H copy.  Host-space pods and
+ * outputs: out_node_idx[pods->n] (required when pods->n > 0), out_score[pods->n], out_placed[n] (before any
+ * rollback) and out_rounds[n] may be NULL.  Checked before any device work: KS_ERR_INVALID for a NULL gangs or group
+ * array, offset[0] != 0, decreasing offsets, offset[n] != pods->n, a bad policy or device-space pods;
+ * KS_ERR_RANGE for a group of 0 or more than KS_GANG_MAX_SIZE pods or min_member above its size.  free[] changes, as
+ * with ks_stream_bind.  An empty snapshot places nothing: every group with min_member >= 1 rolls back. */
+#define KS_GANG_MAX_SIZE 1024u
+typedef struct ks_gangs { /* host memory */
+    uint64_t n;                  /* groups */
+    const uint64_t* offset;      /* [n+1] */
+    const uint32_t* min_member;  /* [n] */
+} ks_gangs;
+int ks_gang_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const ks_gangs* gangs, int policy,
+                 int32_t* out_node_idx, int64_t* out_score, uint32_t* out_placed, uint32_t* out_rounds);
+
 /* ---- asynchronous streaming surface = the reference's Controller queue (src/main.rs:73, :141-148) ----
  * The reference runs reconcile() for many pods concurrently from a work queue.  ks_stream is that queue in front of
  * one snapshot: ks_stream_submit appends pending (unbound) pods and returns at once; a dispatcher thread owned by the

@@ -36,6 +36,7 @@ extern "C" {
 #define KSH_RECONCILE_BINDING_OBJECT_FAILED 2 /* ReconcileError::CreateBindingObjectFailed (src/main.rs:111-114);
                                                  also a pod without namespace (reference: unwrap panic, :80) */
 #define KSH_RECONCILE_BINDING_FAILED 3       /* ReconcileError::CreateBindingFailed: transport, caller side (:105-108) */
+#define KSH_RECONCILE_GANG_UNSATISFIED 4     /* ksh_reconcile_gangs: the pod's group could not place min_member pods */
 
 /* Kubernetes quantity strings, exact: cpu -> millicores, memory -> bytes.
  * KS_ERR_PARSE (malformed), KS_ERR_INEXACT (finer than 1m / 1 byte), KS_ERR_RANGE. */
@@ -128,6 +129,22 @@ int ksh_reconcile(ksh_context* ctx, const ks_pod_obj* pod, int policy, int32_t* 
  * out_json_off / out_rounds may be NULL. */
 int ksh_reconcile_batch(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, int policy, int32_t* out_status,
                         int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off, uint32_t* out_rounds);
+
+/* reconcile() for pod groups, all or nothing (ks_gang_bind, ksched.h; upstream coscheduling's PodGroup minMember).  Group
+ * g is pods [group_offset[g], group_offset[g+1]), 1..KS_GANG_MAX_SIZE of them, min_member[g] <= its size; groups run in
+ * order.  Pods are filtered as ksh_reconcile_batch filters them: already bound pods are skipped (KSH_RECONCILE_OK, node
+ * -1) but count toward their group's min_member, as running members do upstream; pods without namespace/name get
+ * KSH_RECONCILE_BINDING_OBJECT_FAILED and do not count.  The rest of each group goes to the device with
+ * max(0, min_member - bound members).  A group that commits binds as ksh_reconcile_batch does (charged to the snapshot
+ * and the bound list at priority 0, Binding bodies in json / out_json_off, KSH_RECONCILE_NO_NODE_FOUND for its unplaced
+ * pods); a group that rolls back - or has fewer schedulable members than it still needs - binds nothing, and those
+ * pods get KSH_RECONCILE_GANG_UNSATISFIED.  As in ksh_reconcile_batch, every unbound pod with a namespace and name first
+ * loses any charge this context made earlier for it (it came back unbound), whatever its group's outcome.  out_placed[n_groups] (may be NULL) = pods the device placed before any
+ * rollback.  Offsets and sizes are checked first: KS_ERR_INVALID (offsets) / KS_ERR_RANGE (sizes, min_member);
+ * KS_ERR_NO_DEVICE on a packing-only context. */
+int ksh_reconcile_gangs(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, const uint64_t* group_offset,
+                        uint64_t n_groups, const uint32_t* min_member, int policy, int32_t* out_status,
+                        int32_t* out_node_idx, uint32_t* out_placed, char* json, size_t cap, int64_t* out_json_off);
 
 /* Why pods do not schedule: ks_explain (ksched.h) over pod objects, packed as ksh_select_nodes packs them (a selector
  * pair that no node carries counts as a selector mismatch on every node).  out[n_pods] receives the counts.  For each

@@ -129,6 +129,16 @@ if hasattr(lib, "ks_preempt"):  # the same for ks_preempt
     _proto("ks_preempt", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.POINTER(ks_bound_pods), C.c_uint32,
            C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p)
 KS_PREEMPT_MAX_VICTIMS = 128
+
+
+class ks_gangs(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("offset", C.c_void_p), ("min_member", C.c_void_p)]
+
+
+if hasattr(lib, "ks_gang_bind"):  # the same for ks_gang_bind
+    _proto("ks_gang_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.POINTER(ks_gangs), C.c_int, C.c_void_p,
+           C.c_void_p, C.c_void_p, C.c_void_p)
+KS_GANG_MAX_SIZE = 1024
 KS_PREEMPT_MAX_ABS_SUM = 1 << 62
 KS_ERR_INVALID, KS_ERR_RANGE = -1, -5
 KS_REFERENCE_ATTEMPTS = 5

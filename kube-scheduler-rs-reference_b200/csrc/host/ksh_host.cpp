@@ -18,12 +18,13 @@
 #include "../../../include/ksched_host.h"
 
 extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not part of the public ABI)
-// ks_explain, ks_select_topk and ks_preempt are defined by the CUDA core in the same library.  The references are weak so
-// that this file still links with device stand-ins that only provide the older ks_* entries (tests/native);
-// ksh_explain_pods, ksh_rank_nodes and ksh_preempt_pods then report KS_ERR_NO_DEVICE.
+// ks_explain, ks_select_topk, ks_preempt and ks_gang_bind are defined by the CUDA core in the same library.  The
+// references are weak so that this file still links with device stand-ins that only provide the older ks_* entries
+// (tests/native); ksh_explain_pods, ksh_rank_nodes, ksh_preempt_pods and ksh_reconcile_gangs then report KS_ERR_NO_DEVICE.
 #pragma weak ks_explain
 #pragma weak ks_select_topk
 #pragma weak ks_preempt
+#pragma weak ks_gang_bind
 
 namespace {
 
@@ -1321,6 +1322,103 @@ int ksh_reconcile_batch(ksh_context* c, const ks_pod_obj* pods, uint64_t n, int 
                 std::memcpy(json + used, body.c_str(), body.size() + 1);
                 out_json_off[i] = (int64_t)used;
                 used += body.size() + 1;
+            }
+        }
+    }
+    return KS_OK;
+}
+KSH_CATCH
+
+// reconcile() for pod groups: ksh_reconcile_batch's filtering, then ks_gang_bind over the pods that go to the device,
+// one sub-group per group; already bound members count toward min_member
+int ksh_reconcile_gangs(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const uint64_t* group_offset, uint64_t n_groups,
+                        const uint32_t* min_member, int policy, int32_t* out_status, int32_t* out_node_idx,
+                        uint32_t* out_placed, char* json, size_t cap, int64_t* out_json_off) try {
+    if (!c || !group_offset || (n && (!pods || !out_status || !out_node_idx)) || (n_groups && !min_member))
+        return fail(KS_ERR_INVALID, "NULL argument");
+    if (group_offset[0] != 0) return fail(KS_ERR_INVALID, "group_offset[0] must be 0");
+    for (uint64_t g = 0; g < n_groups; g++) {
+        if (group_offset[g + 1] < group_offset[g]) return fail(KS_ERR_INVALID, "group offsets decrease");
+        const uint64_t size = group_offset[g + 1] - group_offset[g];
+        if (size == 0 || size > KS_GANG_MAX_SIZE)
+            return fail(KS_ERR_RANGE, "a group has " + std::to_string(size) + " pods (1.." + std::to_string(KS_GANG_MAX_SIZE) + ")");
+        if (min_member[g] > size) return fail(KS_ERR_RANGE, "min_member above the group's size");
+    }
+    if (group_offset[n_groups] != n) return fail(KS_ERR_INVALID, "group_offset[n_groups] must be n_pods");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    if (!ks_gang_bind) return fail(KS_ERR_NO_DEVICE, "this library has no ks_gang_bind");
+    std::vector<uint64_t> todo, sub_off{0}, sub_group; // the pods that go to the device; sub-group k is group sub_group[k]
+    std::vector<uint32_t> sub_min;
+    std::vector<ks_pod_obj> sub;
+    if (out_placed)
+        for (uint64_t g = 0; g < n_groups; g++) out_placed[g] = 0;
+    for (uint64_t g = 0; g < n_groups; g++) {
+        uint32_t bound = 0;
+        const size_t first = todo.size();
+        for (uint64_t i = group_offset[g]; i < group_offset[g + 1]; i++) {
+            out_node_idx[i] = -1;
+            if (out_json_off) out_json_off[i] = -1;
+            if (ksh_is_pod_bound(&pods[i])) {
+                out_status[i] = KSH_RECONCILE_OK; // src/main.rs:74-76; a running member of the group
+                bound++;
+            } else if (!pods[i].ns || !pods[i].name) {
+                out_status[i] = KSH_RECONCILE_BINDING_OBJECT_FAILED; // reference: unwrap panic, src/main.rs:80
+            } else {
+                out_status[i] = KSH_RECONCILE_NO_NODE_FOUND; // until bound below (src/main.rs:116-118)
+                release_earlier_binding(c, &pods[i]); // it came back unbound: whatever its group does, drop the old charge
+                todo.push_back(i);
+            }
+        }
+        const uint32_t need = min_member[g] > bound ? min_member[g] - bound : 0;
+        if (todo.size() == first) continue;
+        if (need > todo.size() - first) { // too few schedulable members: the group cannot commit, nothing is tried
+            for (size_t k = first; k < todo.size(); k++) out_status[todo[k]] = KSH_RECONCILE_GANG_UNSATISFIED;
+            todo.resize(first);
+            continue;
+        }
+        for (size_t k = first; k < todo.size(); k++) sub.push_back(pods[todo[k]]);
+        sub_off.push_back(todo.size());
+        sub_group.push_back(g);
+        sub_min.push_back(need);
+    }
+    if (todo.empty()) return KS_OK;
+    std::vector<int64_t> rc_, rm_;
+    std::vector<uint64_t> sel;
+    int rc = pack_and_upload(c, sub.data(), sub.size(), rc_, rm_, sel);
+    if (rc) return rc;
+    std::vector<int32_t> idx(sub.size(), -1);
+    std::vector<uint32_t> placed(sub_group.size());
+    ks_pods kp{sub.size(), rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
+    ks_gangs kg{sub_group.size(), sub_off.data(), sub_min.data()};
+    rc = ks_gang_bind(c->snap, &kp, &kg, policy, idx.data(), nullptr, placed.data(), nullptr); // commits on the device
+    if (rc) {
+        c->dirty = true; // the device may carry part of the call: the host list is the truth
+        return rc;
+    }
+    size_t used = 0;
+    for (size_t k = 0; k < sub_group.size(); k++) {
+        if (out_placed) out_placed[sub_group[k]] = placed[k];
+        const bool commit = placed[k] >= sub_min[k];
+        for (uint64_t j = sub_off[k]; j < sub_off[k + 1]; j++) {
+            const uint64_t i = todo[j];
+            if (!commit) {
+                out_status[i] = KSH_RECONCILE_GANG_UNSATISFIED;
+                continue;
+            }
+            if (idx[j] < 0) continue; // NoNodeFound
+            size_t lns, lname;
+            const uint64_t h = pod_key_hash(&pods[i], &lns, &lname);
+            bound_push(c, &pods[i], h, lns, lname, idx[j], rc_[j], rm_[j]);
+            out_status[i] = KSH_RECONCILE_OK;
+            out_node_idx[i] = idx[j];
+            if (json && out_json_off) {
+                const std::string body = binding_body(c, &pods[i], (uint32_t)idx[j]);
+                if (used + body.size() + 1 <= cap) { // bodies back to back, each NUL-terminated; -1 = did not fit
+                    std::memcpy(json + used, body.c_str(), body.size() + 1);
+                    out_json_off[i] = (int64_t)used;
+                    used += body.size() + 1;
+                }
             }
         }
     }

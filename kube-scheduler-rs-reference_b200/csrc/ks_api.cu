@@ -78,6 +78,9 @@ struct ks_snapshot {
     DevBuf st_pre, vx_pre, part_pre; // ks_preempt: host-space outputs and priorities, victim index, node-chunk partials
     DevBuf sb_pkey, sb_pidx, sb_pend; // device-side streaming loop (k_stream_batch)
     void* h_stream = nullptr;                 // pinned staging of one streaming micro-batch (inputs and results)
+    DevBuf gb_in, gb_out;                     // ks_gang_bind: pods and groups in, results out
+    void* h_gang = nullptr;                   // pinned staging of both (grown on demand)
+    size_t h_gang_cap = 0;
     int sms = 0, coop = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     // host-space calls are pipelined in pod chunks: chunk c+1 is copied in on copy_stream while chunk c computes
@@ -184,8 +187,9 @@ void ks_snapshot_destroy(ks_snapshot* s) {
                       &s->st_cnt,    &s->st_mask,   &s->st_codes, &s->st_bnode, &s->st_bcpu,  &s->st_bmem,
                       &s->part_key,  &s->part_idx,  &s->part_cnt, &s->st_samp,  &s->xflag,
                       &s->sb_pkey,   &s->sb_pidx,   &s->sb_pend,  &s->st_reasons, &s->st_topk,
-                      &s->part_topk, &s->st_pre,     &s->vx_pre,   &s->part_pre};
+                      &s->part_topk, &s->st_pre,     &s->vx_pre,   &s->part_pre, &s->gb_in,      &s->gb_out};
     if (s->h_stream) cudaFreeHost(s->h_stream);
+    if (s->h_gang) cudaFreeHost(s->h_gang);
     for (DevBuf* b : bufs) b->release();
     bitpar_release(s->bp);
     if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
@@ -1172,6 +1176,107 @@ int ks_stream_bind(ks_snapshot* s, const ks_pods* pods, int policy, int32_t* out
     } catch (...) {
         return fail(KS_ERR_NOMEM, "out of host memory in ks_stream_bind");
     }
+}
+
+int ks_gang_bind(ks_snapshot* s, const ks_pods* pods, const ks_gangs* gangs, int policy, int32_t* out_node_idx,
+                 int64_t* out_score, uint32_t* out_placed, uint32_t* out_rounds) {
+    int rc = check_pods(s, pods);
+    if (rc) return rc;
+    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_gang_bind takes host-space pods");
+    if (!gangs || !gangs->offset || (gangs->n && !gangs->min_member)) return fail(KS_ERR_INVALID, "NULL group array");
+    if (pods->n && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
+    if (policy != KS_SCORE_LEFTOVER && policy != KS_SCORE_LEAST_ALLOCATED) return fail(KS_ERR_INVALID, "bad policy");
+    const uint64_t P = pods->n, G = gangs->n;
+    const uint64_t* off = gangs->offset;
+    if (off[0] != 0) return fail(KS_ERR_INVALID, "offset[0] must be 0");
+    for (uint64_t g = 0; g < G; g++) {
+        if (off[g + 1] < off[g]) return fail(KS_ERR_INVALID, "offsets decrease at group %llu", (unsigned long long)g);
+        const uint64_t size = off[g + 1] - off[g];
+        if (size == 0 || size > KS_GANG_MAX_SIZE)
+            return fail(KS_ERR_RANGE, "group %llu has %llu pods (1..%u)", (unsigned long long)g, (unsigned long long)size,
+                        KS_GANG_MAX_SIZE);
+        if (gangs->min_member[g] > size)
+            return fail(KS_ERR_RANGE, "group %llu: min_member %u above its %llu pods", (unsigned long long)g,
+                        gangs->min_member[g], (unsigned long long)size);
+    }
+    if (off[G] != P) return fail(KS_ERR_INVALID, "offset[n] must be pods->n");
+    if (G == 0) return KS_OK;
+    const uint32_t W = s->W;
+    std::lock_guard<std::mutex> lk(s->mu);
+    CU_TRY(cudaSetDevice(s->device));
+    if (!s->coop) return fail(KS_ERR_CUDA, "device %d has no cooperative launch", s->device);
+    // one pinned block each way: in = [rc P | rm P | sel P*W | offset G+1 | min_member G],
+    // out = [score P | idx P | ctl 2G | placed G]
+    const size_t o_rm = P * 8, o_sel = 2 * P * 8, o_off = o_sel + P * 8 * W, o_min = o_off + (G + 1) * 4,
+                 in_bytes = o_min + G * 4;
+    const size_t o_idx = P * 8, o_ctl = o_idx + P * 4, o_placed = o_ctl + 2 * G * 4, out_bytes = o_placed + G * 4;
+    const size_t h_out_at = (in_bytes + 7) & ~(size_t)7, h_bytes = h_out_at + out_bytes; // out block 8-byte aligned
+    if (s->h_gang_cap < h_bytes) {
+        if (s->h_gang) cudaFreeHost(s->h_gang);
+        s->h_gang = nullptr;
+        s->h_gang_cap = 0;
+        const size_t want = h_bytes + h_bytes / 8 + 256;
+        CU_TRY(cudaHostAlloc(&s->h_gang, want, cudaHostAllocDefault));
+        s->h_gang_cap = want;
+    }
+    uint8_t* h_in = static_cast<uint8_t*>(s->h_gang);
+    uint8_t* h_out = h_in + h_out_at;
+    memcpy(h_in, pods->req_cpu, P * 8);
+    memcpy(h_in + o_rm, pods->req_mem, P * 8);
+    memcpy(h_in + o_sel, pods->sel, P * 8 * W);
+    uint32_t* h_off = reinterpret_cast<uint32_t*>(h_in + o_off);
+    for (uint64_t g = 0; g <= G; g++) h_off[g] = (uint32_t)off[g];
+    memcpy(h_in + o_min, gangs->min_member, G * 4);
+    CU_TRY(s->gb_in.ensure(in_bytes));
+    CU_TRY(s->gb_out.ensure(out_bytes));
+    CU_TRY(s->sb_pkey.ensure((size_t)STREAM_BATCH_MAX * s->sms * 8));
+    CU_TRY(s->sb_pidx.ensure((size_t)STREAM_BATCH_MAX * s->sms * 4));
+    CU_TRY(s->sb_pend.ensure(2 * STREAM_BATCH_MAX * 4));
+    cudaStream_t st = s->stream;
+    uint8_t* d_in = s->gb_in.as<uint8_t>();
+    uint8_t* d_out = s->gb_out.as<uint8_t>();
+    CU_TRY(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, st));
+    StreamBatchArgs a;
+    a.N = s->N;
+    a.Npad = s->Npad;
+    a.alloc_cpu = s->alloc_cpu.as<int64_t>();
+    a.alloc_mem = s->alloc_mem.as<int64_t>();
+    a.labels = s->labels.as<uint64_t>();
+    a.free_cpu = s->free_cpu.as<int64_t>();
+    a.free_mem = s->free_mem.as<int64_t>();
+    a.policy = policy;
+    a.m = (uint32_t)P;
+    a.req_cpu = reinterpret_cast<const int64_t*>(d_in);
+    a.req_mem = reinterpret_cast<const int64_t*>(d_in + o_rm);
+    a.sel = reinterpret_cast<const uint64_t*>(d_in + o_sel);
+    a.pkey = s->sb_pkey.as<int64_t>();
+    a.pidx = s->sb_pidx.as<int32_t>();
+    a.pend = s->sb_pend.as<uint32_t>();
+    a.ctl = nullptr; // per group: ga.ctl
+    a.out_idx = reinterpret_cast<int32_t*>(d_out + o_idx);
+    a.out_score = reinterpret_cast<int64_t*>(d_out);
+    a.max_rounds = 0; // per group
+    a.grid = std::max(1u, std::min<uint32_t>((uint32_t)s->sms, (s->N + 127u) / 128u));
+    GangArgs ga;
+    ga.n = (uint32_t)G;
+    ga.offset = reinterpret_cast<const uint32_t*>(d_in + o_off);
+    ga.min_member = reinterpret_cast<const uint32_t*>(d_in + o_min);
+    ga.ctl = reinterpret_cast<uint32_t*>(d_out + o_ctl);
+    ga.placed = reinterpret_cast<uint32_t*>(d_out + o_placed);
+    s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
+    s->version++;
+    cudaError_t e = launch_gang_batch(a, ga, W, st);
+    if (e != cudaSuccess) return fail(KS_ERR_CUDA, "k_gang_batch launch failed: %s", cudaGetErrorString(e));
+    CU_TRY(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    memcpy(out_node_idx, h_out + o_idx, P * 4);
+    if (out_score) memcpy(out_score, h_out, P * 8);
+    const uint32_t* ctl = reinterpret_cast<const uint32_t*>(h_out + o_ctl);
+    if (out_rounds)
+        for (uint64_t g = 0; g < G; g++) out_rounds[g] = ctl[2 * g + 1];
+    if (out_placed) memcpy(out_placed, h_out + o_placed, G * 4);
+    s->last_path = "gang_batch";
+    return KS_OK;
 }
 
 // ---------------------------------------------------------------------------------------------- async streaming

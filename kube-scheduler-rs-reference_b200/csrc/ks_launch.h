@@ -94,4 +94,13 @@ struct StreamBatchArgs {
     uint32_t grid;
 };
 cudaError_t launch_stream_batch(const StreamBatchArgs& a, uint32_t W, cudaStream_t st);
+// pod groups (k_gang_batch, ks_stream.cu): a.m = all pods, a.max_rounds unused (each group runs up to size + 1 rounds)
+struct GangArgs {
+    uint32_t n;                 // groups
+    const uint32_t* offset;     // [n+1]: group g = pods [offset[g], offset[g+1]), 1..STREAM_BATCH_MAX of them
+    const uint32_t* min_member; // [n]
+    uint32_t* ctl;              // [2n]: per group pending count, rounds
+    uint32_t* placed;           // [n]: pods the round loop bound (before any rollback)
+};
+cudaError_t launch_gang_batch(const StreamBatchArgs& a, const GangArgs& g, uint32_t W, cudaStream_t st);
 } // namespace ks

@@ -107,7 +107,115 @@ uint32_t stream_max_claims() { return STREAM_MAX; }
 //      into the next round's pending list
 // separated by grid-wide barriers.  Batches of up to STREAM_BATCH_MAX pods.  The pods' requests, selectors and the
 // node table are read-only here (__ldg); free[] changes between rounds and is read through L2 (__ldcg).
+// Phases A and B are the two functions below; k_gang_batch runs the same rounds once per pod group.
 constexpr uint32_t SB_THREADS = 256;
+
+// Phase A of one round, every CTA: for the cnt pending pods of pl (indices into a's pod arrays), the best feasible
+// node of this CTA's slice [n0, n1) into a.pkey / a.pidx [pod][cta]
+template <int W>
+__device__ __forceinline__ void stream_round_scan(const StreamBatchArgs& a, const uint32_t* pl, uint32_t cnt, uint32_t n0,
+                                                  uint32_t n1, uint32_t G, uint32_t lane, uint32_t warp) {
+    for (uint32_t k = warp; k < cnt; k += SB_THREADS / 32) {
+        const uint32_t p = __ldcg(pl + k);
+        const int64_t rc = __ldg(a.req_cpu + p), rm = __ldg(a.req_mem + p);
+        uint64_t sw[W];
+#pragma unroll
+        for (int w = 0; w < W; w++) sw[w] = __ldg(a.sel + (size_t)p * W + w);
+        int64_t best = INT64_MIN;
+        int32_t bidx = -1;
+        for (uint32_t n = n0 + lane; n < n1; n += 32) {
+            const int64_t fc = __ldcg(a.free_cpu + n), fm = __ldcg(a.free_mem + n);
+            uint64_t miss = 0;
+#pragma unroll
+            for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
+            if (rc <= fc && rm <= fm && miss == 0) {
+                const int64_t key = a.policy == KS_SCORE_LEFTOVER
+                                        ? leftover_key(fc, fm)
+                                        : least_alloc_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm);
+                if (key > best) { // ascending n per lane: strict '>' keeps the lowest index
+                    best = key;
+                    bidx = (int32_t)n;
+                }
+            }
+        }
+        warp_argmax(best, bidx);
+        if (lane == 0) {
+            a.pkey[(size_t)k * G + blockIdx.x] = best;
+            a.pidx[(size_t)k * G + blockIdx.x] = bidx;
+        }
+    }
+}
+
+// Phase B of one round, CTA 0 only: reduce the partials to one claim per pod, commit the claims, write the winners'
+// bindings into a.out_idx / a.out_score, compact the losers into the other pending list (a.pend half cur ^ 1) and
+// publish (losers, round + 1) in a.ctl
+template <int W>
+__device__ __forceinline__ void stream_round_commit(const StreamBatchArgs& a, const uint32_t* pl, uint32_t cur,
+                                                    uint32_t cnt, uint32_t round, uint32_t G, uint32_t tid,
+                                                    uint32_t lane, uint32_t warp, unsigned long long* s_key,
+                                                    int64_t* s_ckey, int32_t* s_claim, uint8_t* s_acc,
+                                                    uint32_t* s_scan) {
+    for (uint32_t k = warp; k < cnt; k += SB_THREADS / 32) {
+        int64_t best = INT64_MIN;
+        int32_t bidx = -1;
+        for (uint32_t c = lane; c < G; c += 32) // ascending CTA = ascending node range
+            merge_partial(best, bidx, __ldcg(a.pkey + (size_t)k * G + c), __ldcg(a.pidx + (size_t)k * G + c));
+        warp_argmax(best, bidx);
+        if (lane == 0) {
+            s_claim[k] = bidx;
+            s_ckey[k] = best;
+        }
+    }
+    __syncthreads();
+    // claims per node in arrival (batch) order
+    commit_claims<SB_THREADS>(
+        s_key, cnt, a.free_cpu, a.free_mem, [&](uint32_t k) { return s_claim[k]; },
+        [&](uint32_t k, int64_t& rc, int64_t& rm) {
+            const uint32_t p = __ldcg(pl + k);
+            rc = __ldg(a.req_cpu + p);
+            rm = __ldg(a.req_mem + p);
+        },
+        [&](uint32_t k, bool ok) { s_acc[k] = ok; });
+    __syncthreads();
+    // bindings of the winners; losers keep their order in the next pending list
+    uint32_t* nl = a.pend + (cur ^ 1u) * STREAM_BATCH_MAX;
+    constexpr uint32_t PER = STREAM_BATCH_MAX / SB_THREADS;
+    uint32_t loser[PER], n_loser = 0;
+#pragma unroll
+    for (uint32_t e = 0; e < PER; e++) {
+        const uint32_t k = tid * PER + e;
+        loser[e] = 0;
+        if (k < cnt && s_claim[k] >= 0) {
+            const uint32_t p = __ldcg(pl + k);
+            if (s_acc[k]) {
+                a.out_idx[p] = s_claim[k];
+                a.out_score[p] = a.policy == KS_SCORE_LEFTOVER
+                                     ? leftover_score(s_ckey[k], __ldg(a.req_cpu + p), __ldg(a.req_mem + p))
+                                     : s_ckey[k];
+            } else {
+                loser[e] = 1;
+                n_loser++;
+            }
+        }
+    }
+    s_scan[tid] = n_loser;
+    __syncthreads();
+    for (uint32_t off = 1; off < SB_THREADS; off <<= 1) { // inclusive scan (Hillis-Steele, 256 entries)
+        const uint32_t v = tid >= off ? s_scan[tid - off] : 0;
+        __syncthreads();
+        s_scan[tid] += v;
+        __syncthreads();
+    }
+    uint32_t pos = s_scan[tid] - n_loser;
+#pragma unroll
+    for (uint32_t e = 0; e < PER; e++)
+        if (loser[e]) nl[pos++] = __ldcg(pl + tid * PER + e);
+    if (tid == SB_THREADS - 1) {
+        a.ctl[0] = s_scan[tid];
+        a.ctl[1] = round + 1;
+    }
+    __threadfence();
+}
 
 template <int W>
 __global__ void __launch_bounds__(SB_THREADS) k_stream_batch(const StreamBatchArgs a) {
@@ -137,104 +245,106 @@ __global__ void __launch_bounds__(SB_THREADS) k_stream_batch(const StreamBatchAr
         const uint32_t cnt = *reinterpret_cast<volatile uint32_t*>(a.ctl);
         if (cnt == 0 || round > a.max_rounds) break; // grid-uniform
         const uint32_t* pl = a.pend + cur * STREAM_BATCH_MAX;
-        // ---- A: partial argmax over this CTA's node slice ----
-        for (uint32_t k = warp; k < cnt; k += SB_THREADS / 32) {
-            const uint32_t p = __ldcg(pl + k);
-            const int64_t rc = __ldg(a.req_cpu + p), rm = __ldg(a.req_mem + p);
-            uint64_t sw[W];
-#pragma unroll
-            for (int w = 0; w < W; w++) sw[w] = __ldg(a.sel + (size_t)p * W + w);
-            int64_t best = INT64_MIN;
-            int32_t bidx = -1;
-            for (uint32_t n = n0 + lane; n < n1; n += 32) {
-                const int64_t fc = __ldcg(a.free_cpu + n), fm = __ldcg(a.free_mem + n);
-                uint64_t miss = 0;
-#pragma unroll
-                for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
-                if (rc <= fc && rm <= fm && miss == 0) {
-                    const int64_t key = a.policy == KS_SCORE_LEFTOVER
-                                            ? leftover_key(fc, fm)
-                                            : least_alloc_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm);
-                    if (key > best) { // ascending n per lane: strict '>' keeps the lowest index
-                        best = key;
-                        bidx = (int32_t)n;
-                    }
-                }
-            }
-            warp_argmax(best, bidx);
-            if (lane == 0) {
-                a.pkey[(size_t)k * G + blockIdx.x] = best;
-                a.pidx[(size_t)k * G + blockIdx.x] = bidx;
-            }
-        }
+        stream_round_scan<W>(a, pl, cnt, n0, n1, G, lane, warp);
         __threadfence();
         grid.sync();
-        // ---- B: CTA 0 reduces, resolves, commits, compacts ----
-        if (blockIdx.x == 0) {
-            for (uint32_t k = warp; k < cnt; k += SB_THREADS / 32) {
-                int64_t best = INT64_MIN;
-                int32_t bidx = -1;
-                for (uint32_t c = lane; c < G; c += 32) // ascending CTA = ascending node range
-                    merge_partial(best, bidx, __ldcg(a.pkey + (size_t)k * G + c), __ldcg(a.pidx + (size_t)k * G + c));
-                warp_argmax(best, bidx);
-                if (lane == 0) {
-                    s_claim[k] = bidx;
-                    s_ckey[k] = best;
-                }
-            }
-            __syncthreads();
-            // claims per node in arrival (batch) order
-            commit_claims<SB_THREADS>(
-                s_key, cnt, a.free_cpu, a.free_mem, [&](uint32_t k) { return s_claim[k]; },
-                [&](uint32_t k, int64_t& rc, int64_t& rm) {
-                    const uint32_t p = __ldcg(pl + k);
-                    rc = __ldg(a.req_cpu + p);
-                    rm = __ldg(a.req_mem + p);
-                },
-                [&](uint32_t k, bool ok) { s_acc[k] = ok; });
-            __syncthreads();
-            // bindings of the winners; losers keep their order in the next pending list
-            uint32_t* nl = a.pend + (cur ^ 1u) * STREAM_BATCH_MAX;
-            constexpr uint32_t PER = STREAM_BATCH_MAX / SB_THREADS;
-            uint32_t loser[PER], n_loser = 0;
-#pragma unroll
-            for (uint32_t e = 0; e < PER; e++) {
-                const uint32_t k = tid * PER + e;
-                loser[e] = 0;
-                if (k < cnt && s_claim[k] >= 0) {
-                    const uint32_t p = __ldcg(pl + k);
-                    if (s_acc[k]) {
-                        a.out_idx[p] = s_claim[k];
-                        a.out_score[p] = a.policy == KS_SCORE_LEFTOVER
-                                             ? leftover_score(s_ckey[k], __ldg(a.req_cpu + p), __ldg(a.req_mem + p))
-                                             : s_ckey[k];
-                    } else {
-                        loser[e] = 1;
-                        n_loser++;
-                    }
-                }
-            }
-            s_scan[tid] = n_loser;
-            __syncthreads();
-            for (uint32_t off = 1; off < SB_THREADS; off <<= 1) { // inclusive scan (Hillis-Steele, 256 entries)
-                const uint32_t v = tid >= off ? s_scan[tid - off] : 0;
-                __syncthreads();
-                s_scan[tid] += v;
-                __syncthreads();
-            }
-            uint32_t pos = s_scan[tid] - n_loser;
-#pragma unroll
-            for (uint32_t e = 0; e < PER; e++)
-                if (loser[e]) nl[pos++] = __ldcg(pl + tid * PER + e);
-            if (tid == SB_THREADS - 1) {
-                a.ctl[0] = s_scan[tid];
-                a.ctl[1] = round + 1;
-            }
-            __threadfence();
-        }
+        if (blockIdx.x == 0)
+            stream_round_commit<W>(a, pl, cur, cnt, round, G, tid, lane, warp, s_key, s_ckey, s_claim, s_acc, s_scan);
         grid.sync();
         cur ^= 1u;
     }
+}
+
+// ------------------------------------------------------------------------------------------------ pod groups
+// k_gang_batch: ks_gang_bind in ONE cooperative launch.  The groups run in order; group g is the pods
+// [offset[g], offset[g+1]) of a's arrays, and its rounds are k_stream_batch's (phases A and B above) on a view of a
+// shifted to the group, with the group's own control words ctl[2g..2g+1] (so no CTA can still be reading them when the
+// next group starts).  After the last round CTA 0 counts the placed pods; if there are fewer than min_member[g] it
+// rolls the group back: every placed pod's request is added back to free[] with 64-bit integer atomics (two's-complement
+// sums do not depend on their order, so free[] returns bit for bit to its value before the group) and its binding
+// becomes -1 / 0.  Then one grid barrier, and the next group sees the state the previous one left.
+// a group's pods fill one pending list and the per-claim shared arrays, all STREAM_BATCH_MAX entries long
+static_assert(KS_GANG_MAX_SIZE <= STREAM_BATCH_MAX, "a pod group must fit one cooperative micro-batch");
+
+template <int W>
+__global__ void __launch_bounds__(SB_THREADS, 1) k_gang_batch(const StreamBatchArgs a, const GangArgs ga) {
+    cg::grid_group grid = cg::this_grid();
+    __shared__ unsigned long long s_key[STREAM_BATCH_MAX];
+    __shared__ int64_t s_ckey[STREAM_BATCH_MAX];
+    __shared__ int32_t s_claim[STREAM_BATCH_MAX];
+    __shared__ uint8_t s_acc[STREAM_BATCH_MAX];
+    __shared__ uint32_t s_scan[SB_THREADS];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, G = gridDim.x;
+    const uint32_t chunk = (a.N + G - 1) / G, n0 = min(a.N, blockIdx.x * chunk), n1 = min(a.N, n0 + chunk);
+    for (uint32_t i = blockIdx.x * SB_THREADS + tid; i < a.m; i += G * SB_THREADS) {
+        a.out_idx[i] = -1; // NoNodeFound until bound (src/main.rs:116-118)
+        a.out_score[i] = 0;
+    }
+    for (uint32_t g = blockIdx.x * SB_THREADS + tid; g < ga.n; g += G * SB_THREADS) {
+        ga.ctl[2 * g] = __ldg(ga.offset + g + 1) - __ldg(ga.offset + g);
+        ga.ctl[2 * g + 1] = 0;
+    }
+    if (blockIdx.x == 0 && ga.n)
+        for (uint32_t i = tid; i < __ldg(ga.offset + 1); i += SB_THREADS) a.pend[i] = i;
+    __threadfence();
+    grid.sync();
+    for (uint32_t g = 0; g < ga.n; g++) {
+        const uint32_t base = __ldg(ga.offset + g), size = __ldg(ga.offset + g + 1) - base;
+        StreamBatchArgs b = a; // the group's view: its pods, its bindings, its control words
+        b.req_cpu = a.req_cpu + base;
+        b.req_mem = a.req_mem + base;
+        b.sel = a.sel + (size_t)base * W;
+        b.out_idx = a.out_idx + base;
+        b.out_score = a.out_score + base;
+        b.ctl = ga.ctl + 2 * g;
+        b.m = size;
+        b.max_rounds = size + 1;
+        uint32_t cur = 0;
+        for (uint32_t round = 0;; round++) {
+            const uint32_t cnt = *reinterpret_cast<volatile uint32_t*>(b.ctl);
+            if (cnt == 0 || round > b.max_rounds) break; // grid-uniform
+            const uint32_t* pl = b.pend + cur * STREAM_BATCH_MAX;
+            stream_round_scan<W>(b, pl, cnt, n0, n1, G, lane, warp);
+            __threadfence();
+            grid.sync();
+            if (blockIdx.x == 0)
+                stream_round_commit<W>(b, pl, cur, cnt, round, G, tid, lane, warp, s_key, s_ckey, s_claim, s_acc, s_scan);
+            grid.sync();
+            cur ^= 1u;
+        }
+        if (blockIdx.x == 0) {
+            uint32_t placed = 0;
+            for (uint32_t i0 = 0; i0 < size; i0 += SB_THREADS)
+                placed += __syncthreads_count(i0 + tid < size && __ldcg(b.out_idx + i0 + tid) >= 0);
+            if (placed < __ldg(ga.min_member + g)) { // roll back (placed is CTA-uniform)
+                for (uint32_t i = tid; i < size; i += SB_THREADS) {
+                    const int32_t nd = __ldcg(b.out_idx + i);
+                    if (nd < 0) continue;
+                    atomicAdd(reinterpret_cast<unsigned long long*>(a.free_cpu + nd), (unsigned long long)__ldg(b.req_cpu + i));
+                    atomicAdd(reinterpret_cast<unsigned long long*>(a.free_mem + nd), (unsigned long long)__ldg(b.req_mem + i));
+                    b.out_idx[i] = -1;
+                    b.out_score[i] = 0;
+                }
+            }
+            if (tid == 0) ga.placed[g] = placed;
+            if (g + 1 < ga.n) // the next group starts from the pending list 0..size-1
+                for (uint32_t i = tid; i < __ldg(ga.offset + g + 2) - __ldg(ga.offset + g + 1); i += SB_THREADS) a.pend[i] = i;
+            __threadfence();
+        }
+        grid.sync();
+    }
+}
+
+cudaError_t launch_gang_batch(const StreamBatchArgs& a, const GangArgs& g, uint32_t W, cudaStream_t st) {
+    return with_label_width(W, [&](auto w) {
+        StreamBatchArgs b = a;
+        GangArgs h = g;
+        void* args[] = {&b, &h};
+        const cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(k_gang_batch<decltype(w)::value>),
+                                                          dim3(a.grid), dim3(SB_THREADS), args, 0, st);
+        if (e == cudaSuccess) g_launches++;
+        return e;
+    });
 }
 
 cudaError_t launch_stream_batch(const StreamBatchArgs& a, uint32_t W, cudaStream_t st) {

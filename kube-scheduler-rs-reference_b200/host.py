@@ -39,6 +39,8 @@ for _name, _res, _args in [
     ("ksh_format_unschedulable", C.c_int, [C.c_uint32, C.POINTER(capi.ks_pod_reasons), _vp, C.c_size_t]),
     ("ksh_context_set_pod_priorities", C.c_int, [_vp, _vp, _vp, C.c_uint64]),
     ("ksh_preempt_pods", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, _vp, C.c_size_t, _vp]),
+    ("ksh_reconcile_gangs", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint64, _vp, C.c_int, _vp, _vp, _vp, _vp,
+                                      C.c_size_t, _vp]),
 ]:
     _f = getattr(lib, _name)
     _f.restype = _res
@@ -46,6 +48,7 @@ for _name, _res, _args in [
 
 KSH_DEVICE_NONE = -1  # packing-only context: objects -> SoA arrays on the host, no predicate is ever evaluated
 KSH_RECONCILE_OK, KSH_RECONCILE_NO_NODE_FOUND, KSH_RECONCILE_BINDING_OBJECT_FAILED = 0, 1, 2
+KSH_RECONCILE_GANG_UNSATISFIED = 4
 
 
 def _addr(arr, i=0):
@@ -285,3 +288,26 @@ class Context:
             raise KsError(rc, "ksh_reconcile_batch")
         bodies = [None if o < 0 else C.string_at(C.addressof(buf) + int(o)).decode() for o in off]
         return status, node, bodies, rounds.value
+
+    def reconcile_gangs(self, pods, n, offset, min_member, policy=capi.KS_SCORE_LEFTOVER, json_cap=None):
+        """reconcile() over pod groups, all or nothing (ksh_reconcile_gangs): group g is pods [offset[g], offset[g+1]).
+        Returns (status[n], node_idx[n], bodies[n] (str | None), placed[G])."""
+        offset = np.ascontiguousarray(offset, np.uint64).reshape(-1)
+        min_member = np.ascontiguousarray(min_member, np.uint32).reshape(-1)
+        g = offset.shape[0] - 1
+        if g < 0 or min_member.shape[0] != g:
+            raise ValueError(f"need len(offset) >= 1 and len(min_member) == len(offset) - 1 "
+                             f"(got {offset.shape[0]} and {min_member.shape[0]})")
+        status = np.empty(n, np.int32)
+        node = np.empty(n, np.int32)
+        off = np.empty(n, np.int64)
+        placed = np.empty(g, np.uint32)
+        cap = int(json_cap if json_cap is not None else 512 * max(n, 1))
+        buf = C.create_string_buffer(max(cap, 1))
+        rc = lib.ksh_reconcile_gangs(self._h, C.addressof(pods), n, offset.ctypes.data, g, min_member.ctypes.data,
+                                     int(policy), status.ctypes.data, node.ctypes.data, placed.ctypes.data,
+                                     C.addressof(buf), cap, off.ctypes.data)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ksh_reconcile_gangs")
+        bodies = [None if o < 0 else C.string_at(C.addressof(buf) + int(o)).decode() for o in off]
+        return status, node, bodies, placed

@@ -181,6 +181,28 @@ class Snapshot:
             raise KsError(rc, "ks_stream_bind")
         return idx, score, rounds.value
 
+    def gang_bind(self, req_cpu, req_mem, sel, offset, min_member, policy=capi.KS_SCORE_LEFTOVER):
+        """Pod groups, all or nothing (ks_gang_bind): group g is pods [offset[g], offset[g+1]) and commits only if at
+        least min_member[g] of them are placed.  Returns (node_idx[P], score[P], placed[G], rounds[G])."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        offset = _c(offset, np.uint64).reshape(-1)
+        min_member = _c(min_member, np.uint32).reshape(-1)
+        g = offset.shape[0] - 1
+        if g < 0 or min_member.shape[0] != g:
+            raise ValueError(f"need len(offset) >= 1 and len(min_member) == len(offset) - 1 "
+                             f"(got {offset.shape[0]} and {min_member.shape[0]})")
+        gangs = capi.ks_gangs(g, _ptr(offset), _ptr(min_member))
+        p = int(pods.n)
+        idx = np.empty(p, np.int32)
+        score = np.empty(p, np.int64)
+        placed = np.empty(g, np.uint32)
+        rounds = np.empty(g, np.uint32)
+        rc = lib.ks_gang_bind(self._h, C.byref(pods), C.byref(gangs), int(policy), _ptr(idx), _ptr(score),
+                              _ptr(placed), _ptr(rounds))
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ks_gang_bind")
+        return idx, score, placed, rounds
+
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
         """The reference's own policy (src/main.rs:49-71), seeded: (node_idx, attempts_used, draw_node, draw_code)."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
