@@ -59,7 +59,13 @@ extern "C" {
 #define KS_SELECT_TIMING 4u        /* record CUDA events around each kernel; read with ks_last_timings */
 #define KS_SELECT_NO_GRAPH 8u      /* all-device calls are replayed from a cached CUDA graph; this disables it */
 
-/* value limits enforced on inputs so that scores and sums stay inside int64 */
+/* value limits that keep scores and sums inside int64.  Every node's free value stays within +-KS_MAX_CPU_MILLI /
+ * +-KS_MAX_MEM_BYTES: allocatable and bound pods are checked by set_nodes / set_bound, a bind by apply_bind (against
+ * the node's free after it), and every call that commits requests against free[] (ks_snapshot_commit_claims,
+ * ks_stream_bind, ks_gang_bind, ks_stream_submit) takes requests in [0, limit] only, so an accepted request leaves its
+ * node's free in [0, free]; anything else is KS_ERR_RANGE before any change.  Pending pods of the calls that change
+ * nothing (ks_select, ks_explain, ks_select_topk, ks_preempt, ks_check_cell(s), ks_select_sampling) are NOT checked:
+ * device-space pods could not be without an extra pass.  Outside +-limit their scores are undefined. */
 #define KS_MAX_CPU_MILLI ((int64_t)1 << 36)
 #define KS_MAX_MEM_BYTES ((int64_t)1 << 55)
 #define KS_MAX_LABEL_WORDS 8u
@@ -130,7 +136,9 @@ int ks_snapshot_set_nodes(ks_snapshot* s, uint32_t n_nodes, uint32_t label_words
 /* K0: free[n] = alloc[n] - sum over bound pods on n (src/predicates.rs:27-38).  host arrays. */
 int ks_snapshot_set_bound(ks_snapshot* s, uint64_t n_bound, const int32_t* node_idx, const int64_t* req_cpu,
                           const int64_t* req_mem);
-/* incremental: one more pod bound to node_idx (what the next LIST would show after src/main.rs:103) */
+/* incremental: one more pod bound to node_idx (what the next LIST would show after src/main.rs:103).  A negated
+ * request releases it.  KS_ERR_RANGE, and free[] unchanged, for a request outside +-limit or a bind that would leave
+ * the node's free outside +-limit. */
 int ks_snapshot_apply_bind(ks_snapshot* s, int32_t node_idx, int64_t req_cpu, int64_t req_mem);
 int ks_snapshot_get_free(ks_snapshot* s, int64_t* free_cpu, int64_t* free_mem); /* D2H, [n_nodes] each */
 uint32_t ks_snapshot_num_nodes(const ks_snapshot* s);
@@ -186,7 +194,9 @@ int ks_last_trace(ks_snapshot* s, uint64_t out_ns[16]);
  *   order ends with the same free[] (multi-GPU streaming: all-gather the claims, commit everywhere).
  * ks_stream_bind: the full micro-batch loop on one GPU — select (per-cell kernel, any policy) for the pending
  *   pods, commit, re-select the losers against the updated free[], until every pod is bound or has no feasible
- *   node.  out_node_idx[i] = bound node or -1 (= ReconcileError::NoNodeFound, src/main.rs:116-118). */
+ *   node.  out_node_idx[i] = bound node or -1 (= ReconcileError::NoNodeFound, src/main.rs:116-118).
+ * Both take requests in [0, KS_MAX_CPU_MILLI] / [0, KS_MAX_MEM_BYTES] only (every claim, every pod; -1 claims too):
+ * KS_ERR_RANGE before any device work otherwise. */
 int ks_snapshot_commit_claims(ks_snapshot* s, uint64_t n_claims, const int32_t* claim_node, const int64_t* req_cpu,
                               const int64_t* req_mem, uint8_t* out_accepted);
 int ks_stream_bind(ks_snapshot* s, const ks_pods* pods /* host space */, int policy, int32_t* out_node_idx,
@@ -212,7 +222,8 @@ int ks_stream_bind(ks_snapshot* s, const ks_pods* pods /* host space */, int pol
  * outputs: out_node_idx[pods->n] (required when pods->n > 0), out_score[pods->n], out_placed[n] (before any
  * rollback) and out_rounds[n] may be NULL.  Checked before any device work: KS_ERR_INVALID for a NULL gangs or group
  * array, offset[0] != 0, decreasing offsets, offset[n] != pods->n, a bad policy or device-space pods;
- * KS_ERR_RANGE for a group of 0 or more than KS_GANG_MAX_SIZE pods or min_member above its size.  free[] changes, as
+ * KS_ERR_RANGE for a group of 0 or more than KS_GANG_MAX_SIZE pods, min_member above its size or a request outside
+ * [0, limit] (as ks_stream_bind).  free[] changes, as
  * with ks_stream_bind.  An empty snapshot places nothing: every group with min_member >= 1 rolls back. */
 #define KS_GANG_MAX_SIZE 1024u
 typedef struct ks_gangs { /* host memory */
@@ -231,7 +242,8 @@ int ks_gang_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const ks_
  * finished pods without blocking.  Results carry the caller's ticket; node -1 = ReconcileError::NoNodeFound
  * (src/main.rs:116-118).  Pods with spec.nodeName set must be filtered out before submission (src/main.rs:74-76).
  * While a stream is open its snapshot must not be mutated by other calls (same rule as the reference's node store
- * being written only by its reflector). */
+ * being written only by its reflector).  ks_stream_submit checks the requests as ks_stream_bind does: one outside
+ * [0, limit] refuses the whole submit with KS_ERR_RANGE and queues none of its pods. */
 typedef struct ks_stream ks_stream;
 int ks_stream_open(ks_snapshot* s, int policy, uint32_t max_batch, ks_stream** out);
 int ks_stream_submit(ks_stream* q, uint64_t n, const int64_t* req_cpu, const int64_t* req_mem, const uint64_t* sel /* [n*W] */,

@@ -125,6 +125,17 @@ static int check_range_and_prio(ks_snapshot* s, cudaStream_t st) {
     return KS_OK;
 }
 
+// Requests that are committed against free[] (claims, stream and gang pods) must lie in [0, limit]: an accepted claim
+// then leaves its node's free in [0, free], so free[] stays inside the limits by construction.  Checked on the host
+// before any device work.  (A negative request would always fit and raise free[]; API validation rejects them upstream.)
+static int check_commit_requests(uint64_t n, const int64_t* req_cpu, const int64_t* req_mem) {
+    for (uint64_t i = 0; i < n; i++)
+        if (req_cpu[i] < 0 || req_cpu[i] > KS_MAX_CPU_MILLI || req_mem[i] < 0 || req_mem[i] > KS_MAX_MEM_BYTES)
+            return fail(KS_ERR_RANGE, "pod %llu: request (%lld millicores, %lld bytes) outside [0, 2^36] / [0, 2^55]",
+                        (unsigned long long)i, (long long)req_cpu[i], (long long)req_mem[i]);
+    return KS_OK;
+}
+
 extern "C" {
 
 // internal hook for the host layer (host/ksh_host.cpp); not declared in include/
@@ -305,6 +316,16 @@ int ks_snapshot_apply_bind(ks_snapshot* s, int32_t node_idx, int64_t req_cpu, in
         return fail(KS_ERR_RANGE, "request out of range");
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
+    // free[] stays inside the limits: refuse a bind that would take the node's free outside them, before anything
+    // changes (both values are inside them, so the differences cannot overflow)
+    int64_t f[2];
+    CU_TRY(cudaMemcpyAsync(&f[0], s->free_cpu.as<int64_t>() + node_idx, 8, cudaMemcpyDeviceToHost, s->stream));
+    CU_TRY(cudaMemcpyAsync(&f[1], s->free_mem.as<int64_t>() + node_idx, 8, cudaMemcpyDeviceToHost, s->stream));
+    CU_TRY(cudaStreamSynchronize(s->stream));
+    const int64_t nc = f[0] - req_cpu, nm = f[1] - req_mem;
+    if (nc > KS_MAX_CPU_MILLI || nc < -KS_MAX_CPU_MILLI || nm > KS_MAX_MEM_BYTES || nm < -KS_MAX_MEM_BYTES)
+        return fail(KS_ERR_RANGE, "node %d: the bind would leave free at %lld millicores / %lld bytes, outside +-2^36 / +-2^55",
+                    node_idx, (long long)nc, (long long)nm);
     s->derived_dirty = true;
     s->version++;
     CU_TRY(s->st_bnode.ensure(4));
@@ -819,6 +840,8 @@ int ks_snapshot_commit_claims(ks_snapshot* s, uint64_t n, const int32_t* claim_n
     if (!s) return fail(KS_ERR_INVALID, "snapshot is NULL");
     if (n && (!claim_node || !req_cpu || !req_mem || !out_accepted)) return fail(KS_ERR_INVALID, "NULL claim array");
     if (n == 0) return KS_OK;
+    int rc = check_commit_requests(n, req_cpu, req_mem);
+    if (rc) return rc;
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
     s->derived_dirty = true;
@@ -1068,6 +1091,8 @@ int ks_stream_bind(ks_snapshot* s, const ks_pods* pods, int policy, int32_t* out
     const uint64_t n = pods->n;
     const uint32_t W = s->W;
     if (policy != KS_SCORE_LEFTOVER && policy != KS_SCORE_LEAST_ALLOCATED) return fail(KS_ERR_INVALID, "bad policy");
+    rc = check_commit_requests(n, pods->req_cpu, pods->req_mem);
+    if (rc) return rc;
     if (n > 0 && n <= STREAM_BATCH_MAX && s->N > 0 && s->coop) {
         // device-side loop: one H2D, ONE cooperative launch that runs every round, one D2H
         std::lock_guard<std::mutex> lk(s->mu);
@@ -1201,6 +1226,8 @@ int ks_gang_bind(ks_snapshot* s, const ks_pods* pods, const ks_gangs* gangs, int
     }
     if (off[G] != P) return fail(KS_ERR_INVALID, "offset[n] must be pods->n");
     if (G == 0) return KS_OK;
+    rc = check_commit_requests(P, pods->req_cpu, pods->req_mem);
+    if (rc) return rc;
     const uint32_t W = s->W;
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
@@ -1388,6 +1415,9 @@ int ks_stream_submit(ks_stream* q, uint64_t n, const int64_t* req_cpu, const int
                      const uint64_t* tickets) {
     if (!q || (n && (!req_cpu || !req_mem || !sel || !tickets))) return fail(KS_ERR_INVALID, "NULL argument");
     if (n == 0) return KS_OK;
+    // checked here, so that one bad pod fails its own submit and not the dispatcher batch it would have joined
+    const int rc = check_commit_requests(n, req_cpu, req_mem);
+    if (rc) return rc;
     try {
         std::lock_guard<std::mutex> lk(q->mu);
         for (uint64_t i = 0; i < n; i++) {

@@ -78,9 +78,12 @@ __global__ void __launch_bounds__(256) k_node_bound(NodeTable nt, int64_t* __res
     const uint32_t n = blockIdx.x * blockDim.x + threadIdx.x;
     if (n >= nt.N) return;
     bound[n] = least_alloc_bound(nt, n);
-    long long* amax = reinterpret_cast<long long*>(live + KS_MAX_LABEL_WORDS); // [2]: max allocatable cpu, memory
-    if (nt.alloc_cpu[n] > __ldcg(amax)) atomicMax(amax, (long long)nt.alloc_cpu[n]);
-    if (nt.alloc_mem[n] > __ldcg(amax + 1)) atomicMax(amax + 1, (long long)nt.alloc_mem[n]);
+    // [2]: max allocatable cpu, memory.  A node with allocatable <= 0 scores 0 for that resource whatever the request,
+    // its bound too, so it gives k_least_alloc's per-pod slack nothing: it counts as INT64_MAX, which makes that term 0.
+    long long* amax = reinterpret_cast<long long*>(live + KS_MAX_LABEL_WORDS);
+    const long long ac = nt.alloc_cpu[n] > 0 ? nt.alloc_cpu[n] : INT64_MAX, am = nt.alloc_mem[n] > 0 ? nt.alloc_mem[n] : INT64_MAX;
+    if (ac > __ldcg(amax)) atomicMax(amax, ac);
+    if (am > __ldcg(amax + 1)) atomicMax(amax + 1, am);
     for (uint32_t w = 0; w < nt.W; w++) {
         const unsigned long long v = nt.labels[(size_t)w * nt.Npad + n];
         if (v & ~__ldcg(live + w)) atomicOr(live + w, v);
@@ -1086,7 +1089,8 @@ __global__ void __launch_bounds__(256)
         const bool rc_exact = rc > -(1ll << 24) && rc < (1ll << 24); // (float)rc is rc
         const bool bounded = rc >= 0 && rm >= 0; // else the bound does not hold: no early exit
         // per-pod slack: floor((f-r)*100/a) <= floor(f*100/a) - floor(r*100/a) and a <= a_max, so every feasible cell
-        // scores <= bound(n) - D with D = (rc*100/ac_max + rm*100/am_max) / 2
+        // scores <= bound(n) - D with D = (rc*100/ac_max + rm*100/am_max) / 2 (a_max = INT64_MAX, no slack, when some
+        // node has a <= 0: its term is 0 in score and bound alike)
         const int64_t D = bounded ? ((amax.x > 0 ? (rc * 100) / amax.x : 0) + (amax.y > 0 ? (rm * 100) / amax.y : 0)) / 2 : 0;
         int64_t best = INT64_MIN;
         int32_t bidx = -1;
