@@ -2,15 +2,16 @@
 //
 //   per snapshot   k_node_bound, k_node_splitters/_bucket/_scatter/_rank  sample sort: global position of every node in
 //                                   free_cpu / free_mem / leftover-priority / least-allocated-bound order
-//                  k_build_cbtile   per column block (8 tiles of 256 nodes, node-index order): octet-interleaved prefix
-//                                   tables + label-pair columns, staged in shared memory by the mask kernel
+//                  k_build_cbtile   per column block (8 tiles of 256 nodes, node-index order): prefix tables + label-pair
+//                                   columns, 256-byte lines in tile order, staged in shared memory by the mask kernel
 //                  k_build_ranks    rank tables: tile-local rank of every possible threshold (read through L1/L2)
 //                  k_build_tile     flat indexes in priority order / bound order for the argmax kernels
 //   per call       k_pod_ranks      request -> global rank threshold (splitters in smem + short global search) and the mask
 //                                   kernel's 16-byte pod record, in pod order
 //                  k_mask_rows      persistent, 1 CTA per SM; table blob staged by TMA bulk copies (cp.async.bulk + mbarrier);
-//                                   8 lanes = the 8 tiles of one pod: rank load -> 2 table rows (+ label columns) -> AND ->
-//                                   32 bytes per lane (two 128-bit stores); counts by shuffle + one RED per pod and column block
+//                                   8 lanes = the 256 bytes of one pod: rank load -> 2 table granules per resource (+ label
+//                                   columns) -> AND -> two 128-bit stores per lane, each instruction one whole 128-byte line
+//                                   per pod; counts by shuffle + one RED per pod and column block
 //                  k_first_fit_head/_tail  argmax KS_SCORE_LEFTOVER = first feasible node in priority order (early exit)
 //                  k_least_alloc    argmax KS_SCORE_LEAST_ALLOCATED: bound-ordered scan, exact scores, early exit
 // Semantics per cell are exactly predicates.rs:42 / :45-61 (see include/ksched.h); only the evaluation
@@ -393,9 +394,9 @@ __global__ void __launch_bounds__(288)
                 }
                 w[j] = acc;
             }
-            uint8_t* line = B + (r ? lay.off_tabM : lay.off_tabC) + (size_t)s * RW_LINE + t * 16;
+            uint8_t* line = B + (r ? lay.off_tabM : lay.off_tabC) + (size_t)s * RW_LINE + t * 32;
             *reinterpret_cast<uint4*>(line) = make_uint4(w[0], w[1], w[2], w[3]);
-            *reinterpret_cast<uint4*>(line + 128) = make_uint4(w[4], w[5], w[6], w[7]);
+            *reinterpret_cast<uint4*>(line + 16) = make_uint4(w[4], w[5], w[6], w[7]);
         }
     }
     // label-pair columns
@@ -408,17 +409,18 @@ __global__ void __launch_bounds__(288)
             for (int b = 0; b < 32; b++) acc |= (uint32_t)((s_lab[w_][j * 32 + b] >> sh) & 1ull) << b;
             w[j] = acc;
         }
-        uint8_t* line = B + lay.off_pairs + (size_t)bit * RW_LINE + t * 16;
+        uint8_t* line = B + lay.off_pairs + (size_t)bit * RW_LINE + t * 32;
         *reinterpret_cast<uint4*>(line) = make_uint4(w[0], w[1], w[2], w[3]);
-        *reinterpret_cast<uint4*>(line + 128) = make_uint4(w[4], w[5], w[6], w[7]);
+        *reinterpret_cast<uint4*>(line + 16) = make_uint4(w[4], w[5], w[6], w[7]);
     }
 }
 
-// rank tables: rank[cb][g][resource][t] = number of nodes of tile (cb, t) at sorted positions < g in that
-// resource's order, for every threshold g in [0, N].  One thread = one threshold of one column block: 8 binary searches per resource over the tile's
-// sorted positions (shared memory), one 16-byte store per resource.
+// rank tables: the number of nodes of tile (cb, t) at sorted positions < g in a resource's order, for every threshold g in
+// [0, N], as rank[cb][g][resource][j] u32 = tile j (low half) | tile j + 4 (high half), j < 4: the two tiles whose mask
+// granules one lane of k_mask_rows writes.  One thread = one threshold of one column block: 8 binary searches per resource
+// over the tiles' sorted positions (shared memory), one 16-byte store per resource.
 __global__ void __launch_bounds__(256)
-    k_build_ranks(const uint32_t* __restrict__ tile_sorted, RowsLayout lay, uint16_t* __restrict__ rank) {
+    k_build_ranks(const uint32_t* __restrict__ tile_sorted, RowsLayout lay, uint32_t* __restrict__ rank) {
     __shared__ uint32_t s_pos[2][RW_TILES][BP_TILE];
     const uint32_t cb = blockIdx.y, n_tiles_pad = lay.ncb * RW_TILES;
     for (uint32_t i = threadIdx.x; i < 2 * RW_TILES * BP_TILE; i += blockDim.x) {
@@ -441,9 +443,9 @@ __global__ void __launch_bounds__(256)
             if (a[lo] < g) lo++; // lo <= 255 here
             out[tt] = lo;
         }
-        uint16_t* dst = rank + (((size_t)cb * lay.n_thr + g) * 2 + r) * RW_TILES; // [cb][g][resource][tile]
-        *reinterpret_cast<uint4*>(dst) = make_uint4(out[0] | (out[1] << 16), out[2] | (out[3] << 16),
-                                                   out[4] | (out[5] << 16), out[6] | (out[7] << 16));
+        uint32_t* dst = rank + (((size_t)cb * lay.n_thr + g) * 2 + r) * (RW_TILES / 2); // [cb][g][resource][tile pair]
+        *reinterpret_cast<uint4*>(dst) = make_uint4(out[0] | (out[4] << 16), out[1] | (out[5] << 16),
+                                                   out[2] | (out[6] << 16), out[3] | (out[7] << 16));
     }
 }
 
@@ -562,13 +564,15 @@ __global__ void __launch_bounds__(RANK_THREADS, 1)
 
 // ------------------------------------------------------------------------------------------------ rows kernel
 // k_mask_rows: the round-2 mask / count kernel ("rows" format, ks_bitpar.h).
-//   * lane = (pod slot, tile): 8 lanes per pod = the 8 tiles of the column block = 256 contiguous bytes of the
-//     pod's mask row per pair of 128-bit stores; a warp iteration covers 8 consecutive pods (two per thread, two
-//     independent dependency chains);
-//   * the tile-local rank of the pod's thresholds comes from the rank tables (one 16-bit load per resource from
-//     L1/L2; the 8 lanes of a pod read 16 contiguous bytes) - no base/membership lookup, no POPC for ranks;
-//   * table rows and label-pair columns are octet-interleaved: the 8 lanes of a shared-memory phase read granule t
-//     of their own 256-byte line -> conflict-free for any ranks, plain (unswapped) stores;
+//   * lane = (pod slot, t): 8 lanes per pod = 256 contiguous bytes of the pod's mask row; lane t stores granule t
+//     (half of tile t/2) and granule 8 + t (half of tile 4 + t/2), so each of the two 128-bit store instructions
+//     writes one whole 128-byte line per pod (on the H100, stores that leave every sector half-written run at half
+//     the rate: BASELINE.md); a warp iteration covers 8 consecutive pods (two per thread, two independent chains);
+//   * the tile-local ranks of the pod's thresholds come from the rank tables (one 32-bit load per resource from
+//     L1/L2 = the ranks of the lane's two tiles; the 8 lanes of a pod read 16 contiguous bytes) - no
+//     base/membership lookup, no POPC for ranks;
+//   * table rows and label-pair columns are 256-byte lines in tile order: the 8 lanes of a shared-memory phase read
+//     offsets 16 t (mod 128) of their own rows -> conflict-free for any ranks;
 //   * work = (column block, pod group) items handed out dynamically: one atomic cursor per column block, warps claim
 //     RW_CLAIM groups at a time, a CTA whose block is exhausted re-stages the blob of the block with the most work left
 //     (all SMs busy whatever ncb is, and SMs that stream faster simply claim more);
@@ -578,9 +582,14 @@ __device__ __forceinline__ uint4 lds128(uint32_t a) { // pure: scheduled freely;
     asm("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
     return v;
 }
-__device__ __forceinline__ uint32_t ldg_u16_keep(const uint16_t* p, uint64_t pol) { // L2 evict-last: the rank tables are re-read
+__device__ __forceinline__ uint32_t ldg_u32_keep(const uint32_t* p, uint64_t pol) { // L2 evict-last: the rank tables are re-read
     uint32_t v;
-    asm("ld.global.nc.L2::cache_hint.u16 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+    asm("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ uint4 ldg128_keep(const uint4* p, uint64_t pol) { // L2 evict-last: pod records, read once per column block
+    uint4 v;
+    asm("ld.global.nc.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(pol));
     return v;
 }
 template <class T>
@@ -595,7 +604,7 @@ __device__ __forceinline__ uint4 and4(uint4 a, uint4 b, uint4 c) {
 struct RowsParams { // kernel parameters stay in the constant bank: the loop reads them from there on demand
     const uint8_t* blob;
     RowsLayout lay;
-    const uint16_t* rank;            // [cb][threshold g][resource][tile] u16: 32 bytes per (cb, g)
+    const uint32_t* rank;            // [cb][threshold g][resource][j] = tile j | tile j + 4 << 16: 32 bytes per (cb, g)
     const uint4* rec_s;              // sorted pod records, padded to a multiple of 8
     const unsigned long long* sel_s; // the pods' selector words, pod order (generic path only)
     uint32_t n_groups;               // groups of 8 pods
@@ -607,14 +616,18 @@ struct RowsParams { // kernel parameters stay in the constant bank: the loop rea
 constexpr uint32_t RW_CLAIM = 4;     // pod groups per claim (one atomicAdd per warp and ~4 x 2 KB x 8 of mask)
 constexpr uint32_t RW_HOP_MIN = 256; // a partly claimed column block is worth moving to while it has this many groups left
 
-// one (pod, tile) item: 256 cells -> mask words a (0..3), b (4..7); returns the number of feasible cells.
+// one lane's share of a (pod, column block) item: granules t (tile t/2) and 8 + t (tile 4 + t/2) of the pod's 256 bytes ->
+// mask words a, b (128 cells); returns the number of feasible cells among them.
 // a_tab = shared-window address of granule t of line 0 of tabC; tabM and the pair columns sit at constant offsets.
+// rC, rM = tile-local ranks of the two tiles (low half: tile t/2, high half: tile 4 + t/2).
 template <int W, bool PSMEM>
 __device__ __forceinline__ uint32_t rows_item(const RowsParams& prm, uint32_t a_tab, uint32_t cb, uint32_t t, uint32_t* mask_col,
-                                              uint32_t rC, uint32_t rM, uint32_t pid, uint32_t sel, uint32_t q, uint64_t pol_st) {
-    const uint32_t aC = a_tab + rC * RW_LINE, aM = a_tab + rM * RW_LINE;
-    const uint4 c0 = lds128(aC), c1 = lds128(aC + 128);
-    const uint4 m0 = lds128(aM + RW_TAB_BYTES), m1 = lds128(aM + RW_TAB_BYTES + 128);
+                                              bool st_hi, uint32_t rC, uint32_t rM, uint32_t pid, uint32_t sel, uint32_t q,
+                                              uint64_t pol_st) {
+    const uint32_t aC = a_tab + (rC & 0xFFFFu) * RW_LINE, aM = a_tab + RW_TAB_BYTES + (rM & 0xFFFFu) * RW_LINE;
+    const uint32_t aC1 = a_tab + 128 + (rC >> 16) * RW_LINE, aM1 = a_tab + RW_TAB_BYTES + 128 + (rM >> 16) * RW_LINE;
+    const uint4 c0 = lds128(aC), c1 = lds128(aC1);
+    const uint4 m0 = lds128(aM), m1 = lds128(aM1);
     uint4 a, b;
     auto column = [&](uint32_t bit, uint4& q0, uint4& q1) { // node column of one required pair (predicates.rs:48-53)
         if (PSMEM) {
@@ -664,15 +677,17 @@ __device__ __forceinline__ uint32_t rows_item(const RowsParams& prm, uint32_t a_
         }
     }
     if (mask_col != nullptr && pid != RW_PID_NONE) {
-        uint32_t* dst = mask_col + (size_t)pid * prm.row_words; // 32-byte aligned
+        uint32_t* dst = mask_col + (size_t)pid * prm.row_words; // granule t of the pod's 256-byte block
         // the mask is write-once streaming data: first in line for eviction from L2.  sm_90 stores at most 128 bits
-        // per instruction, so the 32 bytes go out as two 16-byte stores that fill the same sector pair.
+        // per instruction; the 8 lanes of a pod store granules 0..7, then 8..15, so each instruction writes one whole
+        // 128-byte line per pod.
         asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(dst), "r"(a.x), "r"(a.y), "r"(a.z),
                      "r"(a.w), "l"(pol_st)
                      : "memory");
-        asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(dst + 4), "r"(b.x), "r"(b.y),
-                     "r"(b.z), "r"(b.w), "l"(pol_st)
-                     : "memory");
+        if (st_hi)
+            asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(dst + 32), "r"(b.x), "r"(b.y),
+                         "r"(b.z), "r"(b.w), "l"(pol_st)
+                         : "memory");
     }
     return __popc(a.x) + __popc(a.y) + __popc(a.z) + __popc(a.w) + __popc(b.x) + __popc(b.y) + __popc(b.z) + __popc(b.w);
 }
@@ -685,7 +700,7 @@ __global__ void __launch_bounds__(BP_THREADS, 1) k_mask_rows(const __grid_consta
     __shared__ __align__(8) uint64_t bar;
     __shared__ unsigned long long s_key;
     const uint32_t tid = threadIdx.x, t = tid & 7, ps = (tid >> 3) & 3;
-    uint64_t pol_st, pol_ld; // L2 policies: mask stores evict-first, rank-table loads evict-last
+    uint64_t pol_st, pol_ld; // L2 policies: mask stores evict-first, rank-table and pod-record loads evict-last
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_st));
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_ld));
     if (tid == 0) {
@@ -709,8 +724,8 @@ __global__ void __launch_bounds__(BP_THREADS, 1) k_mask_rows(const __grid_consta
     // loads are unconditional (group index clamped into the list)
     auto fetch_rec = [&](uint32_t j, uint4& ra, uint4& rb) {
         const uint4* rp = rec_t + (size_t)min(j, last_grp) * 8u;
-        ra = __ldg(rp);
-        rb = __ldg(rp + 1);
+        ra = ldg128_keep(rp, pol_ld);
+        rb = ldg128_keep(rp + 1, pol_ld);
     };
     uint32_t cb = (uint32_t)((uint64_t)blockIdx.x * ncb / gridDim.x);
     for (;;) { // one iteration per column block this CTA works on
@@ -728,13 +743,13 @@ __global__ void __launch_bounds__(BP_THREADS, 1) k_mask_rows(const __grid_consta
         };
         uint32_t base = __shfl_sync(0xffffffffu, claim(), 0);
         uint32_t next_raw = claim();
-        // rank entry of (g, resource r, tile t): rk_t[g * 16 + r * 8]
-        const uint16_t* rk_t = opaque_ptr(prm.rank + (size_t)cb * prm.lay.n_thr * (2 * RW_TILES) + t);
+        // rank entry of (g, resource r, tiles t/2 and 4 + t/2): rk_t[g * 8 + r * 4]
+        const uint32_t* rk_t = opaque_ptr(prm.rank + (size_t)cb * prm.lay.n_thr * RW_TILES + (t >> 1));
         auto fetch_ranks = [&](const uint4& ra, const uint4& rb, uint32_t& rCa, uint32_t& rMa, uint32_t& rCb, uint32_t& rMb) {
-            rCa = ldg_u16_keep(rk_t + (size_t)ra.x * 16u, pol_ld);
-            rMa = ldg_u16_keep(rk_t + (size_t)ra.y * 16u + 8, pol_ld);
-            rCb = ldg_u16_keep(rk_t + (size_t)rb.x * 16u, pol_ld);
-            rMb = ldg_u16_keep(rk_t + (size_t)rb.y * 16u + 8, pol_ld);
+            rCa = ldg_u32_keep(rk_t + (size_t)ra.x * 8u, pol_ld);
+            rMa = ldg_u32_keep(rk_t + (size_t)ra.y * 8u + 4, pol_ld);
+            rCb = ldg_u32_keep(rk_t + (size_t)rb.x * 8u, pol_ld);
+            rMb = ldg_u32_keep(rk_t + (size_t)rb.y * 8u + 4, pol_ld);
         };
         // records of iteration k+1 are in flight while k computes (its ranks are loaded at the top of k; a deeper pipeline
         // - records two ahead, ranks one ahead - has not been tried on the H100)
@@ -746,12 +761,15 @@ __global__ void __launch_bounds__(BP_THREADS, 1) k_mask_rows(const __grid_consta
         uint32_t tok; // every shared-memory load below depends on a value produced after the wait
         asm volatile("mov.u32 %0, 0;" : "=r"(tok)::"memory");
         const uint32_t a_tab = smem_u32(smem) + t * 16u + tok;
-        const uint32_t tile = cb * RW_TILES + t;
         // a tile is written when it holds nodes, or when the caller's row pitch has room for it (a pitch that is a multiple
         // of 256 bytes - ks_mask_row_bytes_aligned - lets the 8 lanes of a pod always store one whole, 256-byte-aligned
-        // block, and no store straddles a 256-byte boundary); padding tiles hold zeros
-        uint32_t* mask_col = (prm.mask != nullptr && (tile < prm.lay.n_tiles || (tile + 1u) * 8u <= prm.row_words))
-                                 ? opaque_ptr(prm.mask + (size_t)tile * 8u)
+        // block: two whole 128-byte lines); padding tiles hold zeros.  This lane writes half of tile t/2 and half of
+        // tile 4 + t/2; the condition falls with the tile index, so st_hi implies that the low granule is written too.
+        auto written = [&](uint32_t tile) { return tile < prm.lay.n_tiles || (tile + 1u) * 8u <= prm.row_words; };
+        const uint32_t tile_lo = cb * RW_TILES + (t >> 1);
+        const bool st_hi = written(tile_lo + 4);
+        uint32_t* mask_col = (prm.mask != nullptr && written(tile_lo))
+                                 ? opaque_ptr(prm.mask + (size_t)cb * (RW_LINE / 4) + t * 4u)
                                  : nullptr;
 
         while (base < n_slots) { // warp-uniform: one claim of up to RW_CLAIM pod groups
@@ -767,8 +785,8 @@ __global__ void __launch_bounds__(BP_THREADS, 1) k_mask_rows(const __grid_consta
                     jn = next;
                 }
                 fetch_rec(jn, nA, nB);
-                const uint32_t cA = rows_item<W, PSMEM>(prm, a_tab, cb, t, mask_col, rCa, rMa, pidA, selA, j * 8u + 2u * ps, pol_st);
-                const uint32_t cB = rows_item<W, PSMEM>(prm, a_tab, cb, t, mask_col, rCb, rMb, pidB, selB, j * 8u + 2u * ps + 1u, pol_st);
+                const uint32_t cA = rows_item<W, PSMEM>(prm, a_tab, cb, t, mask_col, st_hi, rCa, rMa, pidA, selA, j * 8u + 2u * ps, pol_st);
+                const uint32_t cB = rows_item<W, PSMEM>(prm, a_tab, cb, t, mask_col, st_hi, rCb, rMb, pidB, selB, j * 8u + 2u * ps + 1u, pol_st);
                 if (prm.cnt != nullptr) { // the 8 lanes of a pod are adjacent; both pods' counts ride in one register
                     uint32_t c = cA | (cB << 16);
                     c += __shfl_xor_sync(0xffffffffu, c, 1);
@@ -1368,7 +1386,7 @@ cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cu
             if ((e = regrow(ix.blobR, need + need / 8)) != cudaSuccess) return e;
             ix.cap_blobR = need + need / 8;
         }
-        const size_t need_rank = (size_t)lr.ncb * lr.n_thr * 2 * RW_TILES;
+        const size_t need_rank = (size_t)lr.ncb * lr.n_thr * 2 * (RW_TILES / 2); // u32 tile pairs
         if (need_rank > ix.cap_rank) {
             const size_t cap = need_rank + need_rank / 8;
             if ((e = regrow(ix.rank, cap)) != cudaSuccess) return e;

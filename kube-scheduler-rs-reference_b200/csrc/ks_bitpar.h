@@ -7,9 +7,9 @@
 //   base[bucket][tile] + popc(member[bucket][tile] & lowmask)
 // (bucket = 64 consecutive global positions).  Label selectors are ANDs of per-(key,value) node columns.
 // Round 2 ("rows" kernel, the default): the tile-local rank of every possible threshold is tabulated once per
-// snapshot ([column block][threshold][tile] u16, read through L1/L2), the prefix tables are octet-interleaved
-// (row r of the 8 tiles of a column block = one 256-byte line, conflict-free whatever the ranks are), and one pod
-// takes 8 lanes = 8 tiles = 256 contiguous bytes of its mask row: ~50 instructions per 256 cells.
+// snapshot ([column block][threshold][tile pair] u32, read through L1/L2), row r of the 8 tiles of a column block is
+// one 256-byte line in tile order, and one pod takes 8 lanes = 256 contiguous bytes of its mask row, lane t granules
+// t and 8 + t (each store instruction writes one whole 128-byte line per pod): ~50 instructions per 256 cells.
 // KS_SCORE_LEFTOVER is separable (node part - pod part), so argmax-score is the first
 // feasible node in a static priority order: a short early-exit scan per pod (k_first_fit).
 #pragma once
@@ -34,8 +34,9 @@ struct BitparLayout { // byte offsets inside one column-block blob
 
 // "rows" format: column block = 8 tiles (2048 nodes).  One blob per column block:
 //   tabC [257 rows][256 B], tabM [257 rows][256 B], pairs [64*W bits][256 B]
-// and every 256-byte line is [half 0 of tiles 0..7 | half 1 of tiles 0..7] (16 B each): lane t of an 8-lane
-// shared-memory phase reads granule t of its own row -> 8 distinct bank groups for any ranks.
+// and every 256-byte line is [tile 0 | tile 1 | ... | tile 7] (32 B each) = 16 granules of 16 B.  Lane t of an 8-lane
+// shared-memory phase reads granule t (tile t/2) of the row of its tile's rank, then granule 8 + t (tile 4 + t/2) of
+// another row: offsets 16 t modulo 128 -> 8 distinct bank groups for any ranks.
 constexpr uint32_t RW_TILES = 8;                            // tiles per column block
 constexpr uint32_t RW_LINE = 256;                           // bytes per table row / pair column of a column block
 constexpr uint32_t RW_TAB_BYTES = (uint32_t)BP_ROWS * RW_LINE; // 65792
@@ -74,7 +75,8 @@ struct BitparIndex {
     unsigned long long* live = nullptr; // [KS_MAX_LABEL_WORDS] label bits carried by at least one node
     uint4* rec_s = nullptr;        // rows kernel: {threshold_cpu, threshold_mem, pod index, selector columns} per sorted pod
     uint8_t* blobR = nullptr;      // rows kernel: lay_r.ncb column-block blobs
-    uint16_t* rank = nullptr;      // rows kernel: [cb][threshold g][resource][tile] = nodes of the tile at sorted positions < g
+    uint32_t* rank = nullptr;      // rows kernel: [cb][threshold g][resource][j] = nodes of tile j (low 16 bits) and tile j + 4
+                                   // (high 16 bits) at sorted positions < g
     uint32_t* tile_sorted = nullptr; // build scratch: per tile, its nodes' global positions in ascending order
     size_t cap_blobR = 0, cap_rank = 0, cap_tsorted = 0, cap_cursor = 0;
     RowsLayout lay_r{};
