@@ -251,6 +251,41 @@ impl Gpu {
             e => Err(e),
         }).collect())
     }
+
+    /// Node drain / scale-down check (cluster-autoscaler's removal simulation): `candidates` holds each node's name and
+    /// the pods to move off it (its bound pods, after the caller's PodDisruptionBudget / DaemonSet / local-storage
+    /// filtering).  Each candidate is evaluated on its own against the current cluster; nothing is charged.  Per
+    /// candidate: Some(destination node names, one per pod) when every pod finds a place, None when it cannot be
+    /// drained.  `exclude_candidates`: no listed node takes pods from another (several nodes removed together).
+    pub fn drain_nodes(&self, candidates: &[(&str, &[corev1::Pod])], exclude_candidates: bool)
+                       -> Result<Vec<Option<Vec<String>>>, i32> {
+        let names: Vec<CString> = candidates.iter().map(|(n, _)| CString::new(*n).expect("NUL in a node name")).collect();
+        let name_ptrs: Vec<*const c_char> = names.iter().map(|n| n.as_ptr()).collect();
+        let views: Vec<PodView> = candidates.iter().flat_map(|(_, pods)| pods.iter().map(PodView::new)).collect();
+        let objs: Vec<ks_pod_obj> = views.iter().map(|v| unsafe { ptr::read(&v.obj) }).collect();
+        let mut offset = vec![0u64];
+        for (_, pods) in candidates {
+            offset.push(offset.last().unwrap() + pods.len() as u64);
+        }
+        let mut placed = vec![0u32; candidates.len()];
+        let mut idx = vec![-1i32; objs.len()];
+        let flags = if exclude_candidates { KS_DRAIN_EXCLUDE_CANDIDATES } else { 0 };
+        let rc = unsafe {
+            ksh_drain_nodes(self.ctx, name_ptrs.as_ptr(), candidates.len() as u64, objs.as_ptr(), offset.as_ptr(),
+                            KS_SCORE_LEFTOVER, flags, placed.as_mut_ptr(), idx.as_mut_ptr())
+        };
+        if rc != KS_OK {
+            return Err(rc);
+        }
+        Ok((0..candidates.len()).map(|d| {
+            let (a, b) = (offset[d] as usize, offset[d + 1] as usize);
+            if placed[d] as usize != b - a {
+                return None;
+            }
+            Some(idx[a..b].iter().map(|&n| unsafe { CStr::from_ptr(ksh_context_node_name(self.ctx, n as u32)) }
+                .to_string_lossy().into_owned()).collect())
+        }).collect())
+    }
 }
 
 impl Drop for Gpu {

@@ -30,6 +30,8 @@ pub const KS_MAX_PEERS: usize = 15;
 pub const KS_TOPK_MAX: u32 = 32; // largest k of ks_select_topk / ksh_rank_nodes
 pub const KS_PREEMPT_MAX_VICTIMS: u32 = 128; // largest max_victims of ks_preempt / ksh_preempt_pods
 pub const KS_GANG_MAX_SIZE: u32 = 1024; // most pods in one group of ks_gang_bind / ksh_reconcile_gangs
+pub const KS_DRAIN_MAX_PODS: u32 = 1024; // most pods of one candidate of ks_drain_check / ksh_drain_nodes
+pub const KS_DRAIN_EXCLUDE_CANDIDATES: u32 = 1; // no candidate's node is a destination of any candidate
 
 #[repr(C)]
 pub struct ks_kv {
@@ -129,6 +131,12 @@ pub struct ks_gangs {
     pub offset: *const u64,
     pub min_member: *const u32,
 }
+#[repr(C)]
+pub struct ks_drain_candidates {
+    pub n: u64,
+    pub node_idx: *const i32,
+    pub offset: *const u64,
+}
 pub enum ks_snapshot {}
 pub enum ks_stream {}
 pub enum ksh_context {}
@@ -160,6 +168,8 @@ extern "C" {
     pub fn ks_stream_bind(s: *mut ks_snapshot, pods: *const ks_pods, policy: c_int, node_idx: *mut i32, score: *mut i64, rounds: *mut u32) -> c_int;
     pub fn ks_gang_bind(s: *mut ks_snapshot, pods: *const ks_pods, gangs: *const ks_gangs, policy: c_int, node_idx: *mut i32,
                         score: *mut i64, placed: *mut u32, rounds: *mut u32) -> c_int;
+    pub fn ks_drain_check(s: *mut ks_snapshot, pods: *const ks_pods, cand: *const ks_drain_candidates, policy: c_int,
+                          flags: u32, placed: *mut u32, node_idx: *mut i32, score: *mut i64) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -203,6 +213,8 @@ extern "C" {
     pub fn ksh_reconcile_gangs(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group_offset: *const u64, n_groups: u64,
                                min_member: *const u32, policy: c_int, status: *mut i32, node_idx: *mut i32, placed: *mut u32,
                                json: *mut c_char, cap: usize, json_off: *mut i64) -> c_int;
+    pub fn ksh_drain_nodes(ctx: *mut ksh_context, node_names: *const *const c_char, n: u64, pods: *const ks_pod_obj,
+                           pod_offset: *const u64, policy: c_int, flags: u32, placed: *mut u32, node_idx: *mut i32) -> c_int;
     pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,
                             messages: *mut c_char, cap: usize, msg_off: *mut i64) -> c_int;
     pub fn ksh_format_unschedulable(n_nodes: u32, r: *const ks_pod_reasons, buf: *mut c_char, cap: usize) -> c_int;

@@ -349,6 +349,44 @@ typedef struct ks_preemption { /* 32 bytes per pod */
 int ks_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* pod_priority, const ks_bound_pods* bound,
                uint32_t max_victims, ks_preemption* out, int32_t* out_victims, int32_t out_space, void* cuda_stream);
 
+/* ---- drain simulation: if a node were removed, where would its pods go (cluster-autoscaler's scale-down simulation,
+ * Karpenter consolidation, the descheduler; spec extension, DESIGN.md 5f) ----
+ * Candidate d is node node_idx[d] (duplicates allowed) and owns pods [offset[d], offset[d+1]) of `pods`, in the caller's
+ * order, 0 to KS_DRAIN_MAX_PODS of them (normally the pods bound to that node).  Each candidate is evaluated on its own
+ * against the snapshot's current free[]:
+ *   1. destinations: every real node except node_idx[d]; with KS_DRAIN_EXCLUDE_CANDIDATES also no node that appears
+ *      anywhere in node_idx (cluster-autoscaler's rule when several nodes are checked for removal together);
+ *   2. placement: start from a private copy f of free[]; visit the candidate's pods in array order; each takes the argmax
+ *      under `policy` over the destinations where it fits f and its selector matches, ties to the lower node index
+ *      (ks_select's order and score), and its request is subtracted from f at that node, so later pods of the same
+ *      candidate see the earlier moves (other candidates never do);
+ *   3. the first pod with no destination stops the candidate: it and every later pod of the candidate get node -1 and
+ *      score 0.  out_placed[d] = pods placed before the stop; the candidate is drainable iff that is its pod count (a
+ *      candidate without pods is drainable);
+ *   4. nothing is charged: free[], the bit-parallel index and the snapshot are unchanged.
+ * Upstream places each pod on the first node its filters accept (with a hinting heuristic); here the destination is the
+ * library's own argmax.  Filtering pods before the simulation (PodDisruptionBudgets, DaemonSet and mirror pods, local
+ * storage, safe-to-evict) is the caller's job, and so is removing several nodes in sequence: commit one candidate's
+ * moves and call again.
+ * Host-space pods and outputs: out_placed[n] (required when n > 0), out_node_idx[pods->n] (required when pods->n > 0),
+ * out_score[pods->n] (may be NULL).  Checked before any device work: KS_ERR_INVALID for a NULL cand or array, offset[0]
+ * != 0, decreasing offsets, offset[n] != pods->n, a candidate node outside [0, N) (so an empty snapshot takes no
+ * candidate), unknown flags, a bad policy or device-space pods; KS_ERR_RANGE for a candidate with more than
+ * KS_DRAIN_MAX_PODS pods or a request outside [0, limit] (as ks_stream_bind: f stays inside [0, free]).  n = 0 does
+ * nothing.  A pod whose selector needs a pair no node carries fits nowhere: its candidate stops there.
+ * One H2D copy, one round of two kernels per pod position (round r places pod r of every candidate still running), one
+ * D2H copy; the rounds are enqueued back to back. */
+#define KS_DRAIN_MAX_PODS 1024u
+#define KS_DRAIN_EXCLUDE_CANDIDATES 1u
+typedef struct ks_drain_candidates { /* host memory */
+    uint64_t n;                /* candidates */
+    const int32_t* node_idx;   /* [n] */
+    const uint64_t* offset;    /* [n+1], offset[0] = 0, offset[n] = pods->n */
+} ks_drain_candidates;
+int ks_drain_check(ks_snapshot* s, const ks_pods* pods /* host space */, const ks_drain_candidates* cand, int policy,
+                   uint32_t flags, uint32_t* out_placed /* [n], required */, int32_t* out_node_idx /* [pods->n] */,
+                   int64_t* out_score /* [pods->n], may be NULL */);
+
 #ifdef __cplusplus
 }
 #endif

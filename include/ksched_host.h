@@ -180,6 +180,16 @@ int ksh_context_set_pod_priorities(ksh_context* ctx, const ks_pod_obj* pods, con
 int ksh_preempt_pods(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, const int32_t* pod_priority,
                      uint32_t max_victims, ks_preemption* out, char* victims, size_t cap, int64_t* out_victim_off);
 
+/* Node drain and scale-down checks over objects (ks_drain_check, ksched.h): candidate d is the node named node_names[d]
+ * and owns pods [pod_offset[d], pod_offset[d+1]) (normally the pods bound to it, already filtered by the caller for
+ * PodDisruptionBudgets, DaemonSet and mirror pods, local storage), packed as ksh_select_nodes packs them.  Every pod
+ * must have spec.nodeName equal to its candidate's name and every name must be in the store; either failure is
+ * KS_ERR_INVALID before anything else, and ks_last_error() names the offender.  out_placed[n] and out_node_idx[
+ * pod_offset[n]] as ks_drain_check gives them (destinations map to names with ksh_context_node_name); candidate d is
+ * drainable iff out_placed[d] is its pod count.  Nothing is charged.  KS_ERR_NO_DEVICE on a packing-only context. */
+int ksh_drain_nodes(ksh_context* ctx, const char* const* node_names, uint64_t n, const ks_pod_obj* pods,
+                    const uint64_t* pod_offset, int policy, uint32_t flags, uint32_t* out_placed, int32_t* out_node_idx);
+
 #ifdef __cplusplus
 }
 #endif

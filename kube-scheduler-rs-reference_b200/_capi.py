@@ -139,6 +139,17 @@ if hasattr(lib, "ks_gang_bind"):  # the same for ks_gang_bind
     _proto("ks_gang_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.POINTER(ks_gangs), C.c_int, C.c_void_p,
            C.c_void_p, C.c_void_p, C.c_void_p)
 KS_GANG_MAX_SIZE = 1024
+
+
+class ks_drain_candidates(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("node_idx", C.c_void_p), ("offset", C.c_void_p)]
+
+
+if hasattr(lib, "ks_drain_check"):  # the same for ks_drain_check
+    _proto("ks_drain_check", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.POINTER(ks_drain_candidates), C.c_int,
+           C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p)
+KS_DRAIN_MAX_PODS = 1024
+KS_DRAIN_EXCLUDE_CANDIDATES = 1
 KS_PREEMPT_MAX_ABS_SUM = 1 << 62
 KS_ERR_INVALID, KS_ERR_RANGE = -1, -5
 KS_REFERENCE_ATTEMPTS = 5

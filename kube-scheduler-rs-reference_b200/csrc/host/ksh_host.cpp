@@ -18,13 +18,15 @@
 #include "../../../include/ksched_host.h"
 
 extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not part of the public ABI)
-// ks_explain, ks_select_topk, ks_preempt and ks_gang_bind are defined by the CUDA core in the same library.  The
-// references are weak so that this file still links with device stand-ins that only provide the older ks_* entries
-// (tests/native); ksh_explain_pods, ksh_rank_nodes, ksh_preempt_pods and ksh_reconcile_gangs then report KS_ERR_NO_DEVICE.
+// ks_explain, ks_select_topk, ks_preempt, ks_gang_bind and ks_drain_check are defined by the CUDA core in the same
+// library.  The references are weak so that this file still links with device stand-ins that only provide the older ks_*
+// entries (tests/native); ksh_explain_pods, ksh_rank_nodes, ksh_preempt_pods, ksh_reconcile_gangs and ksh_drain_nodes
+// then report KS_ERR_NO_DEVICE.
 #pragma weak ks_explain
 #pragma weak ks_select_topk
 #pragma weak ks_preempt
 #pragma weak ks_gang_bind
+#pragma weak ks_drain_check
 
 namespace {
 
@@ -1535,6 +1537,39 @@ int ksh_preempt_pods(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const i
         }
     }
     return KS_OK;
+}
+KSH_CATCH
+
+int ksh_drain_nodes(ksh_context* c, const char* const* node_names, uint64_t n, const ks_pod_obj* pods,
+                    const uint64_t* pod_offset, int policy, uint32_t flags, uint32_t* out_placed, int32_t* out_node_idx) try {
+    if (!c || !pod_offset || (n && (!node_names || !out_placed))) return fail(KS_ERR_INVALID, "NULL argument");
+    if (pod_offset[0] != 0) return fail(KS_ERR_INVALID, "pod_offset[0] must be 0");
+    for (uint64_t d = 0; d < n; d++)
+        if (pod_offset[d + 1] < pod_offset[d]) return fail(KS_ERR_INVALID, "pod offsets decrease");
+    const uint64_t P = pod_offset[n];
+    if (P && (!pods || !out_node_idx)) return fail(KS_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    std::vector<int32_t> node(n);
+    for (uint64_t d = 0; d < n; d++) { // mis-grouped input is refused before anything is packed
+        const char* name = node_names[d];
+        if (!name) return fail(KS_ERR_INVALID, "candidate " + std::to_string(d) + ": node name is NULL");
+        node[d] = node_index_of(c, name);
+        if (node[d] < 0) return fail(KS_ERR_INVALID, "candidate " + std::to_string(d) + ": node \"" + name + "\" is not in the store");
+        for (uint64_t i = pod_offset[d]; i < pod_offset[d + 1]; i++)
+            if (!ksh_is_pod_bound(&pods[i]) || std::strcmp(pods[i].node_name, name) != 0)
+                return fail(KS_ERR_INVALID, "pod " + std::to_string(i) + " (" + nz(pods[i].ns) + "/" + nz(pods[i].name) +
+                                                ") has spec.nodeName \"" + (ksh_is_pod_bound(&pods[i]) ? pods[i].node_name : "") +
+                                                "\", not its candidate's node \"" + name + "\"");
+    }
+    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    if (!ks_drain_check) return fail(KS_ERR_NO_DEVICE, "this library has no ks_drain_check");
+    std::vector<int64_t>&rc_ = c->pk_cpu, &rm_ = c->pk_mem; // the same packed batch buffers as ksh_select_nodes
+    std::vector<uint64_t>& sel = c->pk_sel;
+    int rc = pack_and_upload(c, pods, P, rc_, rm_, sel);
+    if (rc) return rc;
+    ks_pods kp{P, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
+    ks_drain_candidates kc{n, node.data(), pod_offset};
+    return ks_drain_check(c->snap, &kp, &kc, policy, flags, out_placed, out_node_idx, nullptr);
 }
 KSH_CATCH
 

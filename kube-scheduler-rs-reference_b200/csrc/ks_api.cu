@@ -81,6 +81,9 @@ struct ks_snapshot {
     DevBuf gb_in, gb_out;                     // ks_gang_bind: pods and groups in, results out
     void* h_gang = nullptr;                   // pinned staging of both (grown on demand)
     size_t h_gang_cap = 0;
+    DevBuf dr_in, dr_work, dr_out;            // ks_drain_check: pods and candidates in, overlays and partials, results out
+    void* h_drain = nullptr;                  // pinned staging of the input and result blocks (grown on demand)
+    size_t h_drain_cap = 0;
     int sms = 0, coop = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     // host-space calls are pipelined in pod chunks: chunk c+1 is copied in on copy_stream while chunk c computes
@@ -198,9 +201,11 @@ void ks_snapshot_destroy(ks_snapshot* s) {
                       &s->st_cnt,    &s->st_mask,   &s->st_codes, &s->st_bnode, &s->st_bcpu,  &s->st_bmem,
                       &s->part_key,  &s->part_idx,  &s->part_cnt, &s->st_samp,  &s->xflag,
                       &s->sb_pkey,   &s->sb_pidx,   &s->sb_pend,  &s->st_reasons, &s->st_topk,
-                      &s->part_topk, &s->st_pre,     &s->vx_pre,   &s->part_pre, &s->gb_in,      &s->gb_out};
+                      &s->part_topk, &s->st_pre,     &s->vx_pre,   &s->part_pre, &s->gb_in,      &s->gb_out,
+                      &s->dr_in,     &s->dr_work,   &s->dr_out};
     if (s->h_stream) cudaFreeHost(s->h_stream);
     if (s->h_gang) cudaFreeHost(s->h_gang);
+    if (s->h_drain) cudaFreeHost(s->h_drain);
     for (DevBuf* b : bufs) b->release();
     bitpar_release(s->bp);
     if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
@@ -1303,6 +1308,141 @@ int ks_gang_bind(ks_snapshot* s, const ks_pods* pods, const ks_gangs* gangs, int
         for (uint64_t g = 0; g < G; g++) out_rounds[g] = ctl[2 * g + 1];
     if (out_placed) memcpy(out_placed, h_out + o_placed, G * 4);
     s->last_path = "gang_batch";
+    return KS_OK;
+}
+
+int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidates* cand, int policy, uint32_t flags,
+                   uint32_t* out_placed, int32_t* out_node_idx, int64_t* out_score) {
+    int rc = check_pods(s, pods);
+    if (rc) return rc;
+    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_drain_check takes host-space pods");
+    if (!cand || !cand->offset || (cand->n && (!cand->node_idx || !out_placed)))
+        return fail(KS_ERR_INVALID, "NULL candidate array or out_placed");
+    if (pods->n && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
+    if (policy != KS_SCORE_LEFTOVER && policy != KS_SCORE_LEAST_ALLOCATED) return fail(KS_ERR_INVALID, "bad policy");
+    if (flags & ~KS_DRAIN_EXCLUDE_CANDIDATES) return fail(KS_ERR_INVALID, "unknown flags 0x%x", flags);
+    const uint64_t P = pods->n, D = cand->n;
+    const uint64_t* off = cand->offset;
+    if (D > 0x7fffffffull) return fail(KS_ERR_RANGE, "too many candidates in one call");
+    if (off[0] != 0) return fail(KS_ERR_INVALID, "offset[0] must be 0");
+    uint32_t rounds = 0;
+    for (uint64_t d = 0; d < D; d++) {
+        if (off[d + 1] < off[d]) return fail(KS_ERR_INVALID, "offsets decrease at candidate %llu", (unsigned long long)d);
+        const uint64_t size = off[d + 1] - off[d];
+        if (size > KS_DRAIN_MAX_PODS)
+            return fail(KS_ERR_RANGE, "candidate %llu has %llu pods (at most %u)", (unsigned long long)d,
+                        (unsigned long long)size, KS_DRAIN_MAX_PODS);
+        if (cand->node_idx[d] < 0 || (uint32_t)cand->node_idx[d] >= s->N)
+            return fail(KS_ERR_INVALID, "candidate %llu: node index %d out of range", (unsigned long long)d,
+                        cand->node_idx[d]);
+        rounds = std::max(rounds, (uint32_t)size);
+    }
+    if (off[D] != P) return fail(KS_ERR_INVALID, "offset[n] must be pods->n");
+    if (D == 0) return KS_OK;
+    rc = check_commit_requests(P, pods->req_cpu, pods->req_mem);
+    if (rc) return rc;
+    const uint32_t W = s->W;
+    std::vector<uint32_t> order, per_round; // candidates by pod count descending; candidates still running in round r
+    try {
+        order.resize(D);
+        per_round.assign(rounds, 0);
+    } catch (...) {
+        return fail(KS_ERR_NOMEM, "out of host memory ordering %llu candidates", (unsigned long long)D);
+    }
+    for (uint32_t d = 0; d < D; d++) order[d] = d;
+    std::stable_sort(order.begin(), order.end(), [off](uint32_t a, uint32_t b) {
+        return off[a + 1] - off[a] > off[b + 1] - off[b];
+    });
+    for (uint64_t d = 0; d < D; d++)
+        for (uint64_t r = 0; r < off[d + 1] - off[d]; r++) per_round[r]++;
+    std::lock_guard<std::mutex> lk(s->mu);
+    CU_TRY(cudaSetDevice(s->device));
+    // one pinned block each way: in = [rc P | rm P | sel P*W (pods in round order) | cand_node D | pod_base D | cand_id D |
+    // excluded-node bits Npad/32 (with the flag)], out = [score P | idx P | placed D]
+    const bool excl = flags & KS_DRAIN_EXCLUDE_CANDIDATES;
+    const size_t o_rm = P * 8, o_sel = 2 * P * 8, o_node = o_sel + P * 8 * W, o_base = o_node + D * 4, o_id = o_base + D * 4,
+                 o_excl = o_id + D * 4, in_bytes = o_excl + (excl ? (size_t)s->Npad / 8 : 0);
+    const size_t o_idx = P * 8, o_placed = o_idx + P * 4, out_bytes = o_placed + D * 4;
+    const size_t h_out_at = (in_bytes + 7) & ~(size_t)7, h_bytes = h_out_at + out_bytes; // out block 8-byte aligned
+    if (s->h_drain_cap < h_bytes) {
+        if (s->h_drain) cudaFreeHost(s->h_drain);
+        s->h_drain = nullptr;
+        s->h_drain_cap = 0;
+        const size_t want = h_bytes + h_bytes / 8 + 256;
+        CU_TRY(cudaHostAlloc(&s->h_drain, want, cudaHostAllocDefault));
+        s->h_drain_cap = want;
+    }
+    uint8_t* h_in = static_cast<uint8_t*>(s->h_drain);
+    uint8_t* h_out = h_in + h_out_at;
+    int64_t* h_rc = reinterpret_cast<int64_t*>(h_in);
+    int64_t* h_rm = reinterpret_cast<int64_t*>(h_in + o_rm);
+    uint64_t* h_sel = reinterpret_cast<uint64_t*>(h_in + o_sel);
+    int32_t* h_node = reinterpret_cast<int32_t*>(h_in + o_node);
+    uint32_t* h_base = reinterpret_cast<uint32_t*>(h_in + o_base);
+    uint32_t* h_id = reinterpret_cast<uint32_t*>(h_in + o_id);
+    for (uint64_t j = 0; j < D; j++) {
+        h_node[j] = cand->node_idx[order[j]];
+        h_base[j] = (uint32_t)off[order[j]];
+        h_id[j] = order[j];
+    }
+    for (uint64_t r = 0, at = 0; r < rounds; at += per_round[r], r++) // round r: pod r of the first per_round[r] candidates
+        for (uint64_t j = 0; j < per_round[r]; j++) {
+            const uint64_t p = off[order[j]] + r;
+            h_rc[at + j] = pods->req_cpu[p];
+            h_rm[at + j] = pods->req_mem[p];
+            memcpy(h_sel + (at + j) * W, pods->sel + p * W, 8 * W);
+        }
+    if (excl) {
+        uint32_t* h_excl = reinterpret_cast<uint32_t*>(h_in + o_excl);
+        memset(h_excl, 0, (size_t)s->Npad / 8);
+        for (uint64_t d = 0; d < D; d++) h_excl[cand->node_idx[d] >> 5] |= 1u << (cand->node_idx[d] & 31);
+    }
+    // node-chunk partials: the largest round needs the most
+    uint64_t part_rows = 0;
+    for (uint32_t r = 0; r < rounds; r++)
+        part_rows = std::max<uint64_t>(part_rows, (uint64_t)direct_grid(W, per_round[r], s->Npad, s->sms).n_chunks * per_round[r]);
+    // work = [ov_fc P | ov_fm P | part keys | ov_node P | part indices | ov_cnt D | failed D]
+    const size_t w_fm = P * 8, w_key = 2 * P * 8, w_node = w_key + part_rows * 8, w_idx = w_node + P * 4,
+                 w_cnt = w_idx + part_rows * 4, w_failed = w_cnt + D * 4, work_bytes = w_failed + D * 4;
+    CU_TRY(s->dr_in.ensure(in_bytes));
+    CU_TRY(s->dr_work.ensure(work_bytes));
+    CU_TRY(s->dr_out.ensure(out_bytes));
+    cudaStream_t st = s->stream;
+    uint8_t* d_in = s->dr_in.as<uint8_t>();
+    uint8_t* d_work = s->dr_work.as<uint8_t>();
+    uint8_t* d_out = s->dr_out.as<uint8_t>();
+    CU_TRY(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, st));
+    CU_TRY(cudaMemsetAsync(d_out, 0, out_bytes, st));
+    CU_TRY(cudaMemsetAsync(d_out + o_idx, 0xff, P * 4, st));
+    CU_TRY(cudaMemsetAsync(d_work + w_cnt, 0, D * 8, st));
+    DrainArgs da;
+    da.cand_node = reinterpret_cast<const int32_t*>(d_in + o_node);
+    da.pod_base = reinterpret_cast<const uint32_t*>(d_in + o_base);
+    da.cand_id = reinterpret_cast<const uint32_t*>(d_in + o_id);
+    da.excl = excl ? reinterpret_cast<const uint32_t*>(d_in + o_excl) : nullptr;
+    da.ov_cnt = reinterpret_cast<uint32_t*>(d_work + w_cnt);
+    da.failed = reinterpret_cast<uint32_t*>(d_work + w_failed);
+    da.ov_node = reinterpret_cast<int32_t*>(d_work + w_node);
+    da.ov_fc = reinterpret_cast<int64_t*>(d_work);
+    da.ov_fm = reinterpret_cast<int64_t*>(d_work + w_fm);
+    da.out_idx = reinterpret_cast<int32_t*>(d_out + o_idx);
+    da.out_score = reinterpret_cast<int64_t*>(d_out);
+    da.placed = reinterpret_cast<uint32_t*>(d_out + o_placed);
+    const PartialView part{reinterpret_cast<int64_t*>(d_work + w_key), reinterpret_cast<int32_t*>(d_work + w_idx), nullptr};
+    const NodeTable nt = node_table(s);
+    for (uint64_t r = 0, at = 0; r < rounds; at += per_round[r], r++) {
+        const PodView pv{reinterpret_cast<const int64_t*>(d_in) + at, reinterpret_cast<const int64_t*>(d_in + o_rm) + at,
+                         reinterpret_cast<const uint64_t*>(d_in + o_sel) + at * W, per_round[r]};
+        const DirectGrid g = direct_grid(W, per_round[r], s->Npad, s->sms);
+        cudaError_t e = launch_drain_round(nt, pv, da, policy, (uint32_t)r, part, g, st);
+        if (e != cudaSuccess) return fail(KS_ERR_CUDA, "drain round %llu launch failed: %s", (unsigned long long)r, cudaGetErrorString(e));
+    }
+    CU_TRY(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    if (P) memcpy(out_node_idx, h_out + o_idx, P * 4);
+    if (out_score && P) memcpy(out_score, h_out, P * 8);
+    memcpy(out_placed, h_out + o_placed, D * 4);
+    s->last_path = "drain";
     return KS_OK;
 }
 

@@ -744,6 +744,193 @@ __global__ void __launch_bounds__(256)
     out[p] = r;
 }
 
+// ------------------------------------------------------------------------------------------------ K2r (ks_drain_check)
+// Round r places pod r of every candidate still running (DrainArgs, ks_launch.h).  A candidate's private free f differs
+// from free[] only on its overlay nodes, and its own node (plus, with KS_DRAIN_EXCLUDE_CANDIDATES, every candidate's node)
+// is no destination.  So the scan reads free[] as K2d does but skips those nodes, through one skip word per (pod, 32
+// nodes) built from the node-sorted overlay with a cursor at the start of each tile: the cost is in overlay entries, not
+// cells.  The commit step then scores the overlay nodes against f, merges them with the scan's best and records the move.
+
+// Bit (node & 31) of lane (node - tb) / 32's word: nodes tb .. tb + TILE_N - 1 that pod slot p may not take.  xw is this
+// lane's word of the excluded-node column; cur is the pod's overlay cursor, advanced past the entries below the tile's
+// end.  A failed candidate skips every node.  Called by the whole warp.
+__device__ __forceinline__ uint32_t drain_skip_word(const DrainArgs& da, uint32_t p, uint32_t tb, uint32_t xw,
+                                                    uint32_t& cur) {
+    if (da.failed[p]) return ~0u;
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t w = xw;
+    const uint32_t cn = (uint32_t)da.cand_node[p];
+    if (cn - tb < (uint32_t)TILE_N && lane == (cn - tb) >> 5) w |= 1u << (cn & 31);
+    const uint32_t n = da.ov_cnt[p], base = da.pod_base[p];
+    while (cur < n) { // warp-uniform: 32 entries per step; the list is sorted, so the entries before the end are a prefix
+        const uint32_t k = cur + lane;
+        const uint32_t v = k < n ? (uint32_t)da.ov_node[base + k] : 0xffffffffu;
+        const uint32_t in = __ballot_sync(0xffffffffu, v < tb + TILE_N);
+        for (uint32_t b = in; b; b &= b - 1) {
+            const uint32_t nn = __shfl_sync(0xffffffffu, v, __ffs(b) - 1);
+            if (nn >= tb && lane == (nn - tb) >> 5) w |= 1u << (nn & 31);
+        }
+        cur += __popc(in);
+        if (in != 0xffffffffu) break;
+    }
+    return w;
+}
+
+template <int W, int POLICY>
+// One CTA per SM, as k_select_topk: the skip words and cursors on top of K2d's registers make ptxas spill when held to 128.
+__global__ void __launch_bounds__(DIRECT_THREADS, 1)
+    k_drain_scan(NodeTable nt, PodView pv, DrainArgs da, PartialView part, uint32_t tiles_per_chunk) {
+    constexpr int PW = pods_per_warp(W);
+    constexpr bool LA = POLICY == KS_SCORE_LEAST_ALLOCATED;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t q0 = warp_first_pod<PW>(); // the p0 scan_node_tiles sets
+    bool dead = true; // every pod of this warp failed earlier (or there is none)
+#pragma unroll
+    for (int i = 0; i < PW; i++)
+        if (q0 + i < pv.P && !da.failed[q0 + i]) dead = false;
+    if (__syncthreads_and(dead)) return; // the whole CTA: nothing to scan
+    int64_t rc[PW], rm[PW];
+    uint64_t sel[PW][W];
+    uint32_t p0;
+    int64_t best[PW];
+    int32_t bidx[PW];
+    uint32_t skip[PW], cur[PW];
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        best[i] = INT64_MIN;
+        bidx[i] = -1;
+        skip[i] = 0;
+        cur[i] = 0;
+    }
+
+    scan_node_tiles<W, LA>(
+        nt, tiles_per_chunk, pv, p0, rc, rm, sel,
+        [&](uint32_t g, uint32_t node, bool real, int64_t fc, int64_t fm, const uint64_t(&lab)[W], int64_t ac, int64_t am) {
+            if (g == 0) { // first group of a tile: this tile's skip words
+                const uint32_t tb = node - lane;
+                const uint32_t xw = da.excl ? __ldg(da.excl + tb / 32 + lane) : 0u;
+#pragma unroll
+                for (int i = 0; i < PW; i++) skip[i] = drain_skip_word(da, min(p0 + i, pv.P - 1), tb, xw, cur[i]);
+            }
+            const int64_t key_n = LA ? 0 : leftover_key(fc, fm);
+#pragma unroll
+            for (int i = 0; i < PW; i++) {
+                const bool fit = (rc[i] <= fc) & (rm[i] <= fm);
+                uint64_t miss = 0;
+#pragma unroll
+                for (int w = 0; w < W; w++) miss |= sel[i][w] & ~lab[w];
+                const bool off = (__shfl_sync(0xffffffffu, skip[i], g) >> lane) & 1u;
+                if (fit && miss == 0 && real && !off) {
+                    const int64_t key = LA ? least_alloc_int(fc, fm, ac, am, rc[i], rm[i]) : key_n;
+                    if (key > best[i]) {
+                        best[i] = key;
+                        bidx[i] = (int32_t)node;
+                    }
+                }
+            }
+        },
+        [](uint32_t) {});
+
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        int64_t k = best[i];
+        int32_t ix = bidx[i];
+        warp_argmax(k, ix);
+        if (lane == 0 && p0 + i < pv.P) {
+            const uint64_t o = (uint64_t)blockIdx.y * pv.P + p0 + i;
+            part.key[o] = k;
+            part.idx[o] = ix;
+        }
+    }
+}
+
+// One warp per running candidate: the scan's best (chunks merged), the overlay nodes scored against f, the better of the
+// two in ks_select's order.  No destination: the candidate fails.  Else the pod's node and score are written, placed
+// becomes r + 1, and the move is charged to the overlay - to the node's entry, or a new entry inserted in node order.
+template <int W, int POLICY>
+__global__ void __launch_bounds__(256)
+    k_drain_commit(NodeTable nt, PodView pv, DrainArgs da, PartialView part, uint32_t n_chunks, uint32_t r) {
+    constexpr bool LA = POLICY == KS_SCORE_LEAST_ALLOCATED;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (p >= pv.P || da.failed[p]) return; // warp-uniform
+    const int64_t rc = pv.req_cpu[p], rm = pv.req_mem[p];
+    uint64_t sel[W];
+#pragma unroll
+    for (int w = 0; w < W; w++) sel[w] = pv.sel[(uint64_t)p * W + w];
+    int64_t key = INT64_MIN;
+    int32_t idx = -1;
+    for (uint32_t ch = lane; ch < n_chunks; ch += 32) { // each lane's chunks in ascending order
+        const uint64_t o = (uint64_t)ch * pv.P + p;
+        merge_partial(key, idx, part.key[o], part.idx[o]);
+    }
+    const uint32_t n = da.ov_cnt[p], base = da.pod_base[p];
+    for (uint32_t k = lane; k < n; k += 32) {
+        const int32_t node = da.ov_node[base + k];
+        const int64_t fc = da.ov_fc[base + k], fm = da.ov_fm[base + k];
+        uint64_t miss = 0;
+#pragma unroll
+        for (int w = 0; w < W; w++) miss |= sel[w] & ~nt.labels[(uint64_t)w * nt.Npad + node];
+        if (rc <= fc && rm <= fm && miss == 0) {
+            const int64_t kk = LA ? least_alloc_int(fc, fm, nt.alloc_cpu[node], nt.alloc_mem[node], rc, rm) : leftover_key(fc, fm);
+            if (topk_beats(kk, node, key, idx)) {
+                key = kk;
+                idx = node;
+            }
+        }
+    }
+    warp_argmax(key, idx);
+    if (idx < 0) {
+        if (lane == 0) da.failed[p] = 1;
+        return;
+    }
+    const uint32_t pod = da.pod_base[p] + r;
+    if (lane == 0) {
+        da.out_idx[pod] = idx;
+        da.out_score[pod] = LA ? key : leftover_score(key, rc, rm);
+        da.placed[da.cand_id[p]] = r + 1;
+    }
+    uint32_t pos = 0; // entries below idx
+    bool found = false;
+    for (uint32_t k0 = 0; k0 < n; k0 += 32) {
+        const uint32_t k = k0 + lane;
+        const int32_t v = k < n ? da.ov_node[base + k] : INT32_MAX;
+        pos += __popc(__ballot_sync(0xffffffffu, v < idx));
+        found |= __any_sync(0xffffffffu, v == idx);
+    }
+    if (found) {
+        if (lane == 0) {
+            da.ov_fc[base + pos] -= rc;
+            da.ov_fm[base + pos] -= rm;
+        }
+        return;
+    }
+    for (uint32_t top = n; top > pos; top = top > pos + 32 ? top - 32 : pos) { // shift [pos, n) up one, top chunk first
+        const int64_t k = (int64_t)top - 1 - lane;
+        const bool mv = k >= (int64_t)pos;
+        int32_t vn = 0;
+        int64_t vc = 0, vm = 0;
+        if (mv) {
+            vn = da.ov_node[base + k];
+            vc = da.ov_fc[base + k];
+            vm = da.ov_fm[base + k];
+        }
+        __syncwarp();
+        if (mv) {
+            da.ov_node[base + k + 1] = vn;
+            da.ov_fc[base + k + 1] = vc;
+            da.ov_fm[base + k + 1] = vm;
+        }
+        __syncwarp();
+    }
+    if (lane == 0) {
+        da.ov_node[base + pos] = idx;
+        da.ov_fc[base + pos] = nt.free_cpu[idx] - rc;
+        da.ov_fm[base + pos] = nt.free_mem[idx] - rm;
+        da.ov_cnt[p] = n + 1;
+    }
+}
+
 // ---- the victim index, built per call: a stable LSD radix sort of (node << 32 | priority + 2^31) keys over the bound
 // list fed in descending bound index, then segment offsets, prefix sums and per-node minimum priorities.
 constexpr uint32_t RADIX_TILE = 2048; // keys per CTA of a radix pass (256 threads x 8 rounds)
@@ -1024,6 +1211,8 @@ cudaError_t prepare_direct() {
             opt_in(k_select_topk<W_, LO>, tile_smem_bytes<W_, false>());
             opt_in(k_select_topk<W_, LA>, tile_smem_bytes<W_, true>());
             opt_in(k_preempt_scan<W_>, tile_smem_bytes<W_, false>());
+            opt_in(k_drain_scan<W_, LO>, tile_smem_bytes<W_, false>());
+            opt_in(k_drain_scan<W_, LA>, tile_smem_bytes<W_, true>());
             return e;
         });
     return e;
@@ -1112,6 +1301,26 @@ cudaError_t launch_preempt(const NodeTable& nt, const PodView& pv, const int32_t
     k_preempt_emit<<<(pv.P + 255) / 256, 256, 0, st>>>(nt, pv, pod_prio, vx, max_victims, part, n_chunks, out, victims);
     g_launches++;
     return cudaGetLastError();
+}
+
+template <int W, int POLICY>
+static cudaError_t launch_drain_t(const NodeTable& nt, const PodView& pv, const DrainArgs& da, uint32_t r,
+                                  const PartialView& part, const DirectGrid& g, cudaStream_t st) {
+    constexpr uint32_t SMEM = tile_smem_bytes<W, POLICY == KS_SCORE_LEAST_ALLOCATED>();
+    k_drain_scan<W, POLICY><<<dim3(g.pod_ctas, g.n_chunks), DIRECT_THREADS, SMEM, st>>>(nt, pv, da, part, g.tiles_per_chunk);
+    k_drain_commit<W, POLICY><<<(pv.P + 7) / 8, 256, 0, st>>>(nt, pv, da, part, g.n_chunks, r);
+    g_launches += 2;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_drain_round(const NodeTable& nt, const PodView& pv, const DrainArgs& da, int policy, uint32_t r,
+                               const PartialView& part, const DirectGrid& g, cudaStream_t st) {
+    if (pv.P == 0) return cudaSuccess;
+    return with_label_width(nt.W, [&](auto w) {
+        constexpr int W = decltype(w)::value;
+        return policy == KS_SCORE_LEFTOVER ? launch_drain_t<W, KS_SCORE_LEFTOVER>(nt, pv, da, r, part, g, st)
+                                           : launch_drain_t<W, KS_SCORE_LEAST_ALLOCATED>(nt, pv, da, r, part, g, st);
+    });
 }
 
 } // namespace ks

@@ -66,6 +66,29 @@ cudaError_t launch_preempt(const NodeTable& nt, const PodView& pv, const int32_t
                            uint32_t max_victims, const PreemptPartials& part, const DirectGrid& g, ks_preemption* out,
                            int32_t* victims, cudaStream_t st);
 
+// drain simulation (ks_drain_check).  Candidates are in the host's round order (pod count descending), so the pods of
+// round r - pod r of every candidate that has one - are the first R_r candidates; slot j of every round is candidate j.
+// Each candidate's moves are an overlay sorted by node, (node, f_cpu, f_mem) with f its private free, kept in
+// [pod_base[j], pod_base[j] + ov_cnt[j]) of the overlay arrays.  Device memory.
+struct DrainArgs {
+    const int32_t* cand_node; // [D] the candidate's own node
+    const uint32_t* pod_base; // [D] its first pod in the caller's order (and its overlay's base)
+    const uint32_t* cand_id;  // [D] its index in the caller's order
+    const uint32_t* excl;     // [Npad / 32] bits of the nodes that are no destination of any candidate, or null
+    uint32_t* ov_cnt;         // [D] overlay entries, zeroed before round 0
+    uint32_t* failed;         // [D] 1 once a pod of the candidate found no destination, zeroed before round 0
+    int32_t* ov_node;         // [P]
+    int64_t* ov_fc;           // [P]
+    int64_t* ov_fm;           // [P]
+    int32_t* out_idx;         // [P] caller's order, -1 before the call
+    int64_t* out_score;       // [P] caller's order, 0 before the call
+    uint32_t* placed;         // [D] caller's order, 0 before the call
+};
+// one round: the node scan for pod r of the pv.P running candidates, then their commit.  part holds g.n_chunks * pv.P
+// keys and indices.
+cudaError_t launch_drain_round(const NodeTable& nt, const PodView& pv, const DrainArgs& da, int policy, uint32_t r,
+                               const PartialView& part, const DirectGrid& g, cudaStream_t st);
+
 } // namespace ks
 
 namespace ks {

@@ -41,6 +41,7 @@ for _name, _res, _args in [
     ("ksh_preempt_pods", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, _vp, C.c_size_t, _vp]),
     ("ksh_reconcile_gangs", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint64, _vp, C.c_int, _vp, _vp, _vp, _vp,
                                       C.c_size_t, _vp]),
+    ("ksh_drain_nodes", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, C.c_int, C.c_uint32, _vp, _vp]),
 ]:
     _f = getattr(lib, _name)
     _f.restype = _res
@@ -311,3 +312,20 @@ class Context:
             raise KsError(rc, "ksh_reconcile_gangs")
         bodies = [None if o < 0 else C.string_at(C.addressof(buf) + int(o)).decode() for o in off]
         return status, node, bodies, placed
+
+    def drain_nodes(self, node_names, pods, pod_offset, policy=capi.KS_SCORE_LEFTOVER, flags=0):
+        """Drain simulation over objects (ksh_drain_nodes): candidate d is the node named node_names[d] with pods
+        [pod_offset[d], pod_offset[d+1]), each bound to that node.  Returns (placed[D], node_idx[P])."""
+        pod_offset = np.ascontiguousarray(pod_offset, np.uint64).reshape(-1)
+        d = len(node_names)
+        if pod_offset.shape[0] != d + 1:
+            raise ValueError(f"need len(pod_offset) == len(node_names) + 1 (got {pod_offset.shape[0]} and {d})")
+        names = (C.c_char_p * max(d, 1))(*[n.encode() if isinstance(n, str) else n for n in node_names])
+        p = int(pod_offset[-1])
+        placed = np.empty(d, np.uint32)
+        node = np.empty(p, np.int32)
+        rc = lib.ksh_drain_nodes(self._h, C.addressof(names), d, C.addressof(pods) if pods is not None else None,
+                                 pod_offset.ctypes.data, int(policy), int(flags), placed.ctypes.data, node.ctypes.data)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ksh_drain_nodes")
+        return placed, node

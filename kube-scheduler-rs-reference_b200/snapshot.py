@@ -203,6 +203,27 @@ class Snapshot:
             raise KsError(rc, "ks_gang_bind")
         return idx, score, placed, rounds
 
+    def drain_check(self, req_cpu, req_mem, sel, node_idx, offset, policy=capi.KS_SCORE_LEFTOVER, flags=0):
+        """Drain simulation (ks_drain_check): candidate d is node node_idx[d] with pods [offset[d], offset[d+1]); each
+        candidate's pods are placed in order on the other nodes, against a private copy of free[].  Nothing is charged.
+        Returns (placed[D], node_idx[P], score[P]); candidate d is drainable iff placed[d] is its pod count."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        node_idx = _c(node_idx, np.int32).reshape(-1)
+        offset = _c(offset, np.uint64).reshape(-1)
+        d = node_idx.shape[0]
+        if offset.shape[0] != d + 1:
+            raise ValueError(f"need len(offset) == len(node_idx) + 1 (got {offset.shape[0]} and {d})")
+        cand = capi.ks_drain_candidates(d, _ptr(node_idx), _ptr(offset))
+        p = int(pods.n)
+        placed = np.empty(d, np.uint32)
+        idx = np.empty(p, np.int32)
+        score = np.empty(p, np.int64)
+        rc = lib.ks_drain_check(self._h, C.byref(pods), C.byref(cand), int(policy), int(flags), _ptr(placed), _ptr(idx),
+                                _ptr(score))
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ks_drain_check")
+        return placed, idx, score
+
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
         """The reference's own policy (src/main.rs:49-71), seeded: (node_idx, attempts_used, draw_node, draw_code)."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
