@@ -75,6 +75,38 @@ impl PodView {
     }
 }
 
+/// Owns the CStrings a `ks_node_obj` view points into (per call, as `PodView`).
+pub struct NodeView {
+    _strings: Vec<CString>,
+    _kvs: Vec<Vec<ks_kv>>,
+    pub obj: ks_node_obj,
+}
+
+impl NodeView {
+    pub fn new(node: &corev1::Node) -> NodeView {
+        let mut strings = Vec::new();
+        let mut kvs: Vec<Vec<ks_kv>> = Vec::new();
+        let name = node.metadata.name.as_deref().map(|s| cs(&mut strings, s)).unwrap_or(ptr::null());
+        let (mut has_labels, mut n_labels, mut labels) = (0, 0u32, ptr::null());
+        if let Some(l) = &node.metadata.labels {
+            let v: Vec<ks_kv> = l.iter().map(|(k, val)| ks_kv { key: cs(&mut strings, k), val: cs(&mut strings, val) }).collect();
+            kvs.push(v);
+            let v = kvs.last().unwrap();
+            (has_labels, n_labels, labels) = (1, v.len() as u32, v.as_ptr());
+        }
+        let (mut has_alloc, mut n_alloc, mut alloc) = (0, 0u32, ptr::null());
+        if let Some(a) = node.status.as_ref().and_then(|s| s.allocatable.as_ref()) {
+            let v: Vec<ks_kv> = a.iter().map(|(k, q)| ks_kv { key: cs(&mut strings, k), val: cs(&mut strings, &q.0) }).collect();
+            kvs.push(v);
+            let v = kvs.last().unwrap();
+            (has_alloc, n_alloc, alloc) = (1, v.len() as u32, v.as_ptr());
+        }
+        let obj = ks_node_obj { name, has_labels, n_labels, labels, has_allocatable: has_alloc, n_allocatable: n_alloc,
+                                allocatable: alloc };
+        NodeView { _strings: strings, _kvs: kvs, obj }
+    }
+}
+
 /// Replaces Context.node_store + the per-cell LIST (src/util.rs:12-15, src/predicates.rs:21-38).
 pub struct Gpu {
     ctx: *mut ksh_context,
@@ -285,6 +317,86 @@ impl Gpu {
             Some(idx[a..b].iter().map(|&n| unsafe { CStr::from_ptr(ksh_context_node_name(self.ctx, n as u32)) }
                 .to_string_lossy().into_owned()).collect())
         }).collect())
+    }
+}
+
+/// One node template of a node group for `Gpu::scaleup_estimate_packed`: allocatable, capacity of an empty node (allocatable
+/// minus its DaemonSet and system pods), label words in the call's own bit layout, and the nodes the group may add.
+pub struct NodeTemplate {
+    pub alloc_cpu: i64,
+    pub alloc_mem: i64,
+    pub free_cpu: i64,
+    pub free_mem: i64,
+    pub labels: Vec<u64>,
+    pub max_nodes: u32,
+}
+
+impl Gpu {
+    /// Node-group scale-up estimate (cluster-autoscaler's binpacking estimator) over objects: each template is a Node
+    /// object standing for one new node of a group (labels it would carry, instance type included; allocatable) with
+    /// the nodes the group may still add; `daemonsets` are the pods that would run on every such node, each with
+    /// spec.nodeName set to its template's name; `pending` are the pods no node accepts.  Each template is packed on its
+    /// own by first fit in decreasing-size order; nothing is charged.  Returns the per-template rows, the best template
+    /// (most pods placed, then utilization, then fewest nodes) and, per (template, pending pod), the new node's ordinal
+    /// or -1.  Err = the library's status (KS_ERR_NO_DEVICE on a packing-only context).
+    pub fn scaleup_estimate(&self, templates: &[(corev1::Node, u32)], daemonsets: &[corev1::Pod], pending: &[corev1::Pod])
+                            -> Result<(Vec<ks_scaleup_option>, Option<usize>, Vec<i32>), i32> {
+        let tv: Vec<NodeView> = templates.iter().map(|(n, _)| NodeView::new(n)).collect();
+        let tobj: Vec<ks_node_obj> = tv.iter().map(|v| unsafe { ptr::read(&v.obj) }).collect();
+        let max_nodes: Vec<u32> = templates.iter().map(|(_, m)| *m).collect();
+        let dv: Vec<PodView> = daemonsets.iter().map(PodView::new).collect();
+        let dobj: Vec<ks_pod_obj> = dv.iter().map(|v| unsafe { ptr::read(&v.obj) }).collect();
+        let pv: Vec<PodView> = pending.iter().map(PodView::new).collect();
+        let pobj: Vec<ks_pod_obj> = pv.iter().map(|v| unsafe { ptr::read(&v.obj) }).collect();
+        let mut rows = vec![ks_scaleup_option::default(); templates.len()];
+        let mut best = -1i32;
+        let mut node = vec![-1i32; templates.len() * pending.len()];
+        let rc = unsafe {
+            ksh_scaleup_estimate(self.ctx, tobj.as_ptr(), tobj.len() as u64, max_nodes.as_ptr(), dobj.as_ptr(),
+                                 dobj.len() as u64, pobj.as_ptr(), pobj.len() as u64, rows.as_mut_ptr(), &mut best,
+                                 node.as_mut_ptr(), ptr::null_mut())
+        };
+        if rc != KS_OK {
+            return Err(rc);
+        }
+        Ok((rows, if best < 0 { None } else { Some(best as usize) }, node))
+    }
+
+    /// The same over packed pods, for callers with their own label bit layout: `req` holds each pending pod's (cpu
+    /// millicores, memory bytes) and `sel` its `label_words` selector words, in the templates' bit layout.  Panics when
+    /// `sel` or a template's `labels` does not hold `label_words` words per entry.
+    pub fn scaleup_estimate_packed(&self, req: &[(i64, i64)], sel: &[u64], label_words: u32, templates: &[NodeTemplate])
+                                   -> Result<(Vec<ks_scaleup_option>, Option<usize>, Vec<i32>), i32> {
+        let w = label_words as usize;
+        assert_eq!(sel.len(), req.len() * w, "sel must hold label_words words per pod");
+        assert!(templates.iter().all(|t| t.labels.len() == w), "each template's labels must hold label_words words");
+        let snap = unsafe { ksh_context_snapshot(self.ctx) };
+        if snap.is_null() {
+            return Err(KS_ERR_NO_DEVICE);
+        }
+        let cpu: Vec<i64> = req.iter().map(|r| r.0).collect();
+        let mem: Vec<i64> = req.iter().map(|r| r.1).collect();
+        let ac: Vec<i64> = templates.iter().map(|t| t.alloc_cpu).collect();
+        let am: Vec<i64> = templates.iter().map(|t| t.alloc_mem).collect();
+        let fc: Vec<i64> = templates.iter().map(|t| t.free_cpu).collect();
+        let fm: Vec<i64> = templates.iter().map(|t| t.free_mem).collect();
+        let labels: Vec<u64> = templates.iter().flat_map(|t| t.labels.iter().copied()).collect();
+        let max_nodes: Vec<u32> = templates.iter().map(|t| t.max_nodes).collect();
+        let pods = ks_pods { n: req.len() as u64, req_cpu: cpu.as_ptr(), req_mem: mem.as_ptr(), sel: sel.as_ptr(),
+                             mem_space: KS_MEM_HOST };
+        let t = ks_node_templates { n: templates.len() as u64, label_words, alloc_cpu: ac.as_ptr(), alloc_mem: am.as_ptr(),
+                                    free_cpu: fc.as_ptr(), free_mem: fm.as_ptr(), labels: labels.as_ptr(),
+                                    max_nodes: max_nodes.as_ptr() };
+        let mut rows = vec![ks_scaleup_option::default(); templates.len()];
+        let mut best = -1i32;
+        let mut node = vec![-1i32; templates.len() * req.len()];
+        let rc = unsafe {
+            ks_scaleup_estimate(snap, &pods, &t, rows.as_mut_ptr(), &mut best, node.as_mut_ptr(), ptr::null_mut())
+        };
+        if rc != KS_OK {
+            return Err(rc);
+        }
+        Ok((rows, if best < 0 { None } else { Some(best as usize) }, node))
     }
 }
 

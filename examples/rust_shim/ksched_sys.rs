@@ -18,6 +18,7 @@ pub const KS_SCORE_LEFTOVER: c_int = 0;
 pub const KS_SCORE_LEAST_ALLOCATED: c_int = 1;
 pub const KS_MEM_HOST: i32 = 0;
 pub const KS_MEM_DEVICE: i32 = 1;
+pub const KS_ERR_NO_DEVICE: c_int = -8; // packing-only context or no CUDA device
 pub const KS_CELL_OK: c_int = 0;
 pub const KS_CELL_NOT_ENOUGH_RESOURCES: c_int = 1; // InvalidNodeReason::NotEnoughResources  (src/predicates.rs:16)
 pub const KS_CELL_NODE_SELECTOR_MISMATCH: c_int = 2; // InvalidNodeReason::NodeSelectorMismatch (src/predicates.rs:17)
@@ -32,6 +33,9 @@ pub const KS_PREEMPT_MAX_VICTIMS: u32 = 128; // largest max_victims of ks_preemp
 pub const KS_GANG_MAX_SIZE: u32 = 1024; // most pods in one group of ks_gang_bind / ksh_reconcile_gangs
 pub const KS_DRAIN_MAX_PODS: u32 = 1024; // most pods of one candidate of ks_drain_check / ksh_drain_nodes
 pub const KS_DRAIN_EXCLUDE_CANDIDATES: u32 = 1; // no candidate's node is a destination of any candidate
+pub const KS_SCALEUP_MAX_NODES: u32 = 1024; // most new nodes of one template of ks_scaleup_estimate
+pub const KS_SCALEUP_MAX_PODS: u32 = 65536; // most pods of one ks_scaleup_estimate call
+pub const KS_SCALEUP_MAX_TEMPLATES: u32 = 4096; // most templates of one ks_scaleup_estimate call
 
 #[repr(C)]
 pub struct ks_kv {
@@ -137,6 +141,27 @@ pub struct ks_drain_candidates {
     pub node_idx: *const i32,
     pub offset: *const u64,
 }
+#[repr(C)]
+pub struct ks_node_templates {
+    pub n: u64,
+    pub label_words: u32,
+    pub alloc_cpu: *const i64,
+    pub alloc_mem: *const i64,
+    pub free_cpu: *const i64,
+    pub free_mem: *const i64,
+    pub labels: *const u64,
+    pub max_nodes: *const u32,
+}
+#[repr(C)]
+#[derive(Clone, Copy, Default, Debug)]
+pub struct ks_scaleup_option {
+    pub nodes: u32,
+    pub placed: u32,
+    pub eligible: u32,
+    pub utilization: i32,
+    pub used_cpu: i64,
+    pub used_mem: i64,
+}
 pub enum ks_snapshot {}
 pub enum ks_stream {}
 pub enum ksh_context {}
@@ -170,6 +195,9 @@ extern "C" {
                         score: *mut i64, placed: *mut u32, rounds: *mut u32) -> c_int;
     pub fn ks_drain_check(s: *mut ks_snapshot, pods: *const ks_pods, cand: *const ks_drain_candidates, policy: c_int,
                           flags: u32, placed: *mut u32, node_idx: *mut i32, score: *mut i64) -> c_int;
+    pub fn ks_scaleup_estimate(s: *mut ks_snapshot, pods: *const ks_pods, t: *const ks_node_templates,
+                               out: *mut ks_scaleup_option, best: *mut i32, node: *mut i32,
+                               reasons: *mut ks_pod_reasons) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -213,6 +241,11 @@ extern "C" {
     pub fn ksh_reconcile_gangs(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group_offset: *const u64, n_groups: u64,
                                min_member: *const u32, policy: c_int, status: *mut i32, node_idx: *mut i32, placed: *mut u32,
                                json: *mut c_char, cap: usize, json_off: *mut i64) -> c_int;
+    pub fn ksh_context_snapshot(ctx: *mut ksh_context) -> *mut ks_snapshot; // borrowed, until the next mutation
+    pub fn ksh_scaleup_estimate(ctx: *mut ksh_context, templates: *const ks_node_obj, n_templates: u64, max_nodes: *const u32,
+                                overhead_pods: *const ks_pod_obj, n_overhead: u64, pods: *const ks_pod_obj, n_pods: u64,
+                                out: *mut ks_scaleup_option, best: *mut i32, node: *mut i32,
+                                reasons: *mut ks_pod_reasons) -> c_int;
     pub fn ksh_drain_nodes(ctx: *mut ksh_context, node_names: *const *const c_char, n: u64, pods: *const ks_pod_obj,
                            pod_offset: *const u64, policy: c_int, flags: u32, placed: *mut u32, node_idx: *mut i32) -> c_int;
     pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,

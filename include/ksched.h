@@ -387,6 +387,66 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods /* host space */, const k
                    uint32_t flags, uint32_t* out_placed /* [n], required */, int32_t* out_node_idx /* [pods->n] */,
                    int64_t* out_score /* [pods->n], may be NULL */);
 
+/* ---- scale-up estimate: for pods no node accepts, how many new nodes of each node template would place them
+ * (cluster-autoscaler's binpacking estimator, Karpenter's instance-type sizing; spec extension, DESIGN.md 5g) ----
+ * Template t is one new, empty node of a node group: allocatable A = (alloc_cpu[t], alloc_mem[t]), capacity
+ * F = (free_cpu[t], free_mem[t]) of an empty node (allocatable minus its DaemonSet and system pods), label words
+ * labels[t * label_words ...] and max_nodes[t], the nodes the group may still add.  Each template is evaluated on its
+ * own; it reads neither the snapshot's node table nor the other templates of the call:
+ *   1. eligible: pod p is eligible for t iff its cell code against an empty node of t is KS_CELL_OK (req <= F on both
+ *      resources, and (sel & ~labels) == 0 on every word);
+ *   2. order: eligible pods by req_cpu/A_c + req_mem/A_m descending (the requests as fractions of the allocatable),
+ *      then by lower pod index; compared exactly on the integer key req_cpu*A_m + req_mem*A_c (up to 72 bits);
+ *   3. first fit: the open-node list starts empty; each pod, in that order, goes to the lowest-ordinal open node whose
+ *      remaining capacity holds it on both resources (non-strict).  If none does and fewer than max_nodes[t] are open,
+ *      a new node with remaining F is opened and takes the pod.  Otherwise the pod is not placed and the walk goes on
+ *      (a later, smaller pod may still fit).  Placing a pod subtracts its request from its node's remaining capacity;
+ *   4. out[t]: nodes opened, pods placed, pods eligible, used_cpu / used_mem = the sum of the placed requests, and
+ *      utilization = (used_cpu*100/(nodes*A_c) + used_mem*100/(nodes*A_m))/2 in truncating int64 division (0 when
+ *      nodes = 0), in the style of KS_SCORE_LEAST_ALLOCATED;
+ *   5. *out_best: the template with the most pods placed, then the highest utilization, then the fewest nodes, then the
+ *      lowest index; -1 when no template places a pod.  Other expanders (least-waste, priority, ...) are the caller's
+ *      choice: the rows carry what they need;
+ *   6. out_node[t * pods->n + p] (may be NULL): the ordinal of the new node of t that p lands on, or -1;
+ *      out_reasons[p] (may be NULL): ks_explain's counts with the templates as the nodes, so not_enough_resources +
+ *      node_selector_mismatch + (templates p is eligible for) = n - why a pod triggers no scale-up;
+ *   7. nothing is charged: free[], the bit-parallel index and the snapshot are unchanged.
+ * The label words belong to the call, not to the snapshot's dictionary (a template normally carries pairs no existing
+ * node carries yet, such as its instance type); label_words may differ from the snapshot's.  Splitting the templates
+ * of one call over several calls gives the same rows; only the best has to be picked again.
+ * Checked on the host before any device work: KS_ERR_INVALID for a NULL argument or array, device-space pods, or
+ * label_words outside {1, 2, 4, 8}; KS_ERR_RANGE for pods->n > KS_SCALEUP_MAX_PODS, n > KS_SCALEUP_MAX_TEMPLATES, an
+ * allocatable outside [1, limit >> 10] (cpu <= 2^26 m, memory <= 2^45 B), a capacity outside [-(limit >> 10), A],
+ * max_nodes > KS_SCALEUP_MAX_NODES, or a request outside [0, limit] (as ks_stream_bind).  These keep every sum of a
+ * template (at most 1024 nodes of 2^45 B) and the utilization products inside int64.  n = 0 or pods->n = 0 needs no
+ * device work: rows and reasons are zero and *out_best = -1.
+ * Host-space pods and outputs.  One H2D copy, two kernels (the per-pod reasons only when out_reasons is set), one D2H
+ * copy; the best template is picked on the host.  With out_node the snapshot's pinned staging block and its device
+ * result block each grow to n * pods->n * 4 bytes (1 GiB each at 4096 templates x 65536 pods) and are kept for reuse
+ * until ks_snapshot_destroy; callers near the limits who want that memory back can split the templates over calls or
+ * use a snapshot of their own for the estimate. */
+#define KS_SCALEUP_MAX_NODES 1024u
+#define KS_SCALEUP_MAX_PODS 65536u
+#define KS_SCALEUP_MAX_TEMPLATES 4096u
+typedef struct ks_node_templates { /* host memory */
+    uint64_t n;                  /* templates */
+    uint32_t label_words;        /* pods->sel is [pods->n * label_words] for this call */
+    const int64_t* alloc_cpu;    /* [n] */
+    const int64_t* alloc_mem;    /* [n] */
+    const int64_t* free_cpu;     /* [n] */
+    const int64_t* free_mem;     /* [n] */
+    const uint64_t* labels;      /* [n * label_words] */
+    const uint32_t* max_nodes;   /* [n] */
+} ks_node_templates;
+typedef struct ks_scaleup_option { /* 32 bytes per template */
+    uint32_t nodes, placed, eligible;
+    int32_t utilization;
+    int64_t used_cpu, used_mem;
+} ks_scaleup_option;
+int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods /* host space */, const ks_node_templates* t,
+                        ks_scaleup_option* out /* [n], required */, int32_t* out_best /* required */,
+                        int32_t* out_node /* [n * pods->n] or NULL */, ks_pod_reasons* out_reasons /* [pods->n] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -190,6 +190,24 @@ int ksh_preempt_pods(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, 
 int ksh_drain_nodes(ksh_context* ctx, const char* const* node_names, uint64_t n, const ks_pod_obj* pods,
                     const uint64_t* pod_offset, int policy, uint32_t flags, uint32_t* out_placed, int32_t* out_node_idx);
 
+/* Node-group scale-up estimate over objects (ks_scaleup_estimate, ksched.h): template t is the Node object templates[t]
+ * (one new node of a group; its labels are those a new node would carry, instance type included) with max_nodes[t].
+ * Allocatable is parsed as ksh_context_set_nodes parses it (a missing cpu or memory key is KS_ERR_MISSING; a template
+ * without allocatable has allocatable 0, which ks_scaleup_estimate refuses with KS_ERR_RANGE).  Each overhead pod (a
+ * DaemonSet pod) has spec.nodeName equal to a template's name and its total_pod_resources is charged to that template,
+ * so capacity = allocatable - the sum, as upstream builds a template's NodeInfo.  The pending pods are packed against a
+ * call-local dictionary: one bit per (key, value) pair that some pending pod's selector names and some template
+ * carries, in the order the pods name them; every other selector pair maps to the never-set bit (more than 511 such
+ * pairs is KS_ERR_RANGE).  KS_ERR_INVALID before any device work for a NULL argument or name, duplicate template
+ * names, an overhead pod without spec.nodeName or naming an unknown template, or a pending pod with spec.nodeName set;
+ * ks_last_error() names the offender.  A malformed quantity fails with its parse status first as well.  The context's
+ * node store, dictionary, bound list and snapshot are not changed.  Outputs as ks_scaleup_estimate gives them
+ * (out[n_templates] required when n_templates > 0, out_best required, out_node[n_templates * n_pods] and
+ * out_reasons[n_pods] may be NULL).  KS_ERR_NO_DEVICE on a packing-only context. */
+int ksh_scaleup_estimate(ksh_context* ctx, const ks_node_obj* templates, uint64_t n_templates, const uint32_t* max_nodes,
+                         const ks_pod_obj* overhead_pods, uint64_t n_overhead, const ks_pod_obj* pods, uint64_t n_pods,
+                         ks_scaleup_option* out, int32_t* out_best, int32_t* out_node, ks_pod_reasons* out_reasons);
+
 #ifdef __cplusplus
 }
 #endif

@@ -150,6 +150,27 @@ if hasattr(lib, "ks_drain_check"):  # the same for ks_drain_check
            C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p)
 KS_DRAIN_MAX_PODS = 1024
 KS_DRAIN_EXCLUDE_CANDIDATES = 1
+
+
+class ks_node_templates(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("label_words", C.c_uint32), ("alloc_cpu", C.c_void_p), ("alloc_mem", C.c_void_p),
+                ("free_cpu", C.c_void_p), ("free_mem", C.c_void_p), ("labels", C.c_void_p), ("max_nodes", C.c_void_p)]
+
+
+class ks_scaleup_option(C.Structure):
+    _fields_ = [("nodes", C.c_uint32), ("placed", C.c_uint32), ("eligible", C.c_uint32), ("utilization", C.c_int32),
+                ("used_cpu", C.c_int64), ("used_mem", C.c_int64)]
+
+
+# the same row as a numpy record
+SCALEUP_OPTION_DTYPE = np.dtype([("nodes", np.uint32), ("placed", np.uint32), ("eligible", np.uint32),
+                                 ("utilization", np.int32), ("used_cpu", np.int64), ("used_mem", np.int64)])
+if hasattr(lib, "ks_scaleup_estimate"):  # the same for ks_scaleup_estimate
+    _proto("ks_scaleup_estimate", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.POINTER(ks_node_templates), C.c_void_p,
+           C.c_void_p, C.c_void_p, C.c_void_p)
+KS_SCALEUP_MAX_NODES = 1024
+KS_SCALEUP_MAX_PODS = 65536
+KS_SCALEUP_MAX_TEMPLATES = 4096
 KS_PREEMPT_MAX_ABS_SUM = 1 << 62
 KS_ERR_INVALID, KS_ERR_RANGE = -1, -5
 KS_REFERENCE_ATTEMPTS = 5

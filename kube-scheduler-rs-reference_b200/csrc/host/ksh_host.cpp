@@ -13,20 +13,22 @@
 #include <cstdlib>
 #include <mutex>
 #include <thread>
+#include <unordered_map>
 #include <vector>
 
 #include "../../../include/ksched_host.h"
 
 extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not part of the public ABI)
-// ks_explain, ks_select_topk, ks_preempt, ks_gang_bind and ks_drain_check are defined by the CUDA core in the same
-// library.  The references are weak so that this file still links with device stand-ins that only provide the older ks_*
-// entries (tests/native); ksh_explain_pods, ksh_rank_nodes, ksh_preempt_pods, ksh_reconcile_gangs and ksh_drain_nodes
-// then report KS_ERR_NO_DEVICE.
+// ks_explain, ks_select_topk, ks_preempt, ks_gang_bind, ks_drain_check and ks_scaleup_estimate are defined by the CUDA
+// core in the same library.  The references are weak so that this file still links with device stand-ins that only
+// provide the older ks_* entries (tests/native); ksh_explain_pods, ksh_rank_nodes, ksh_preempt_pods, ksh_reconcile_gangs,
+// ksh_drain_nodes and ksh_scaleup_estimate then report KS_ERR_NO_DEVICE.
 #pragma weak ks_explain
 #pragma weak ks_select_topk
 #pragma weak ks_preempt
 #pragma weak ks_gang_bind
 #pragma weak ks_drain_check
+#pragma weak ks_scaleup_estimate
 
 namespace {
 
@@ -1570,6 +1572,94 @@ int ksh_drain_nodes(ksh_context* c, const char* const* node_names, uint64_t n, c
     ks_pods kp{P, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     ks_drain_candidates kc{n, node.data(), pod_offset};
     return ks_drain_check(c->snap, &kp, &kc, policy, flags, out_placed, out_node_idx, nullptr);
+}
+KSH_CATCH
+
+int ksh_scaleup_estimate(ksh_context* c, const ks_node_obj* templates, uint64_t n_templates, const uint32_t* max_nodes,
+                         const ks_pod_obj* overhead_pods, uint64_t n_overhead, const ks_pod_obj* pods, uint64_t n_pods,
+                         ks_scaleup_option* out, int32_t* out_best, int32_t* out_node, ks_pod_reasons* out_reasons) try {
+    if (!c || !out_best || (n_templates && (!templates || !max_nodes || !out)) || (n_overhead && !overhead_pods) ||
+        (n_pods && !pods))
+        return fail(KS_ERR_INVALID, "NULL argument");
+    if (n_pods > KS_SCALEUP_MAX_PODS || n_templates > KS_SCALEUP_MAX_TEMPLATES)
+        return fail(KS_ERR_RANGE, "more than " + std::to_string(KS_SCALEUP_MAX_PODS) + " pods or " +
+                                      std::to_string(KS_SCALEUP_MAX_TEMPLATES) + " templates");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    // templates: names, allocatable as ksh_context_set_nodes parses it; capacity = allocatable minus the overhead pods
+    std::unordered_map<std::string, uint32_t> index;
+    std::vector<int64_t> ac(n_templates), am(n_templates), fc(n_templates), fm(n_templates);
+    for (uint64_t t = 0; t < n_templates; t++) {
+        if (!templates[t].name) return fail(KS_ERR_INVALID, "template " + std::to_string(t) + ": name is NULL");
+        if (!index.emplace(templates[t].name, (uint32_t)t).second)
+            return fail(KS_ERR_INVALID, "template " + std::to_string(t) + ": duplicate name \"" + templates[t].name + "\"");
+        std::string err;
+        const int rc = parse_node_allocatable(templates[t], &ac[t], &am[t], &err);
+        if (rc) return fail(rc, "template " + std::to_string(t) + ": " + err);
+        fc[t] = ac[t];
+        fm[t] = am[t];
+    }
+    for (uint64_t i = 0; i < n_overhead; i++) { // DaemonSet pods, charged to the template spec.nodeName names
+        const ks_pod_obj& pod = overhead_pods[i];
+        const std::string who = "overhead pod " + std::to_string(i) + " (" + nz(pod.ns) + "/" + nz(pod.name) + ")";
+        if (!ksh_is_pod_bound(&pod)) return fail(KS_ERR_INVALID, who + " has no spec.nodeName naming its template");
+        const auto it = index.find(pod.node_name);
+        if (it == index.end()) return fail(KS_ERR_INVALID, who + " names unknown template \"" + pod.node_name + "\"");
+        int64_t cpu, mem;
+        std::string err;
+        const int rc = total_pod_resources(&pod, &cpu, &mem, &err);
+        if (rc) return fail(rc, who + ": " + err);
+        if (__builtin_sub_overflow(fc[it->second], cpu, &fc[it->second]) ||
+            __builtin_sub_overflow(fm[it->second], mem, &fm[it->second]))
+            return fail(KS_ERR_RANGE, who + ": capacity of its template overflows");
+    }
+    // pending pods: unbound, requests as ksh_select_nodes packs them
+    std::vector<int64_t> rc_(n_pods), rm_(n_pods);
+    for (uint64_t p = 0; p < n_pods; p++) {
+        const std::string who = "pod " + std::to_string(p) + " (" + nz(pods[p].ns) + "/" + nz(pods[p].name) + ")";
+        if (ksh_is_pod_bound(&pods[p]))
+            return fail(KS_ERR_INVALID, who + " has spec.nodeName \"" + pods[p].node_name + "\": not a pending pod");
+        std::string err;
+        const int rc = total_pod_resources(&pods[p], &rc_[p], &rm_[p], &err);
+        if (rc) return fail(rc, who + ": " + err);
+    }
+    // call-local dictionary: a bit for every pair that some pending pod names and some template carries, in the order
+    // the pods name them; every other selector pair takes the never-set bit (the last bit of the last word)
+    std::unordered_map<std::string, int32_t> carried; // "key\0value" -> bit, -1 until a pod names it
+    for (uint64_t t = 0; t < n_templates; t++)
+        if (templates[t].has_labels)
+            for (uint32_t i = 0; i < templates[t].n_labels; i++)
+                carried.emplace(std::string(nz(templates[t].labels[i].key)) + '\0' + nz(templates[t].labels[i].val), -1);
+    uint32_t bits = 0;
+    for (uint64_t p = 0; p < n_pods; p++) {
+        if (!(pods[p].has_spec && pods[p].has_node_selector)) continue;
+        for (uint32_t i = 0; i < pods[p].n_selector; i++) {
+            const auto it = carried.find(std::string(nz(pods[p].selector[i].key)) + '\0' + nz(pods[p].selector[i].val));
+            if (it != carried.end() && it->second < 0) it->second = (int32_t)bits++;
+        }
+    }
+    if (bits > 64 * KS_MAX_LABEL_WORDS - 1)
+        return fail(KS_ERR_RANGE, "more than 511 distinct (key,value) pairs named by pending pods and carried by templates");
+    const uint32_t W = words_for_bits(bits), never = 64 * W - 1;
+    std::vector<uint64_t> lab(n_templates * W, 0), sel(n_pods * W, 0);
+    for (uint64_t t = 0; t < n_templates; t++)
+        if (templates[t].has_labels)
+            for (uint32_t i = 0; i < templates[t].n_labels; i++) {
+                const int32_t b = carried[std::string(nz(templates[t].labels[i].key)) + '\0' + nz(templates[t].labels[i].val)];
+                if (b >= 0) lab[t * W + b / 64] |= 1ull << (b % 64);
+            }
+    for (uint64_t p = 0; p < n_pods; p++) {
+        if (!(pods[p].has_spec && pods[p].has_node_selector)) continue;
+        for (uint32_t i = 0; i < pods[p].n_selector; i++) {
+            const auto it = carried.find(std::string(nz(pods[p].selector[i].key)) + '\0' + nz(pods[p].selector[i].val));
+            const uint32_t b = it != carried.end() ? (uint32_t)it->second : never;
+            sel[p * W + b / 64] |= 1ull << (b % 64);
+        }
+    }
+    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    if (!ks_scaleup_estimate) return fail(KS_ERR_NO_DEVICE, "this library has no ks_scaleup_estimate");
+    ks_pods kp{n_pods, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
+    ks_node_templates kt{n_templates, W, ac.data(), am.data(), fc.data(), fm.data(), lab.data(), max_nodes};
+    return ks_scaleup_estimate(c->snap, &kp, &kt, out, out_best, out_node, out_reasons);
 }
 KSH_CATCH
 

@@ -84,6 +84,9 @@ struct ks_snapshot {
     DevBuf dr_in, dr_work, dr_out;            // ks_drain_check: pods and candidates in, overlays and partials, results out
     void* h_drain = nullptr;                  // pinned staging of the input and result blocks (grown on demand)
     size_t h_drain_cap = 0;
+    DevBuf su_in, su_work, su_out;            // ks_scaleup_estimate: pods and templates in, sort scratch, results out
+    void* h_scaleup = nullptr;                // pinned staging of the input and result blocks (grown on demand)
+    size_t h_scaleup_cap = 0;
     int sms = 0, coop = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     // host-space calls are pipelined in pod chunks: chunk c+1 is copied in on copy_stream while chunk c computes
@@ -202,10 +205,11 @@ void ks_snapshot_destroy(ks_snapshot* s) {
                       &s->part_key,  &s->part_idx,  &s->part_cnt, &s->st_samp,  &s->xflag,
                       &s->sb_pkey,   &s->sb_pidx,   &s->sb_pend,  &s->st_reasons, &s->st_topk,
                       &s->part_topk, &s->st_pre,     &s->vx_pre,   &s->part_pre, &s->gb_in,      &s->gb_out,
-                      &s->dr_in,     &s->dr_work,   &s->dr_out};
+                      &s->dr_in,     &s->dr_work,   &s->dr_out,   &s->su_in,    &s->su_work,  &s->su_out};
     if (s->h_stream) cudaFreeHost(s->h_stream);
     if (s->h_gang) cudaFreeHost(s->h_gang);
     if (s->h_drain) cudaFreeHost(s->h_drain);
+    if (s->h_scaleup) cudaFreeHost(s->h_scaleup);
     for (DevBuf* b : bufs) b->release();
     bitpar_release(s->bp);
     if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
@@ -1443,6 +1447,119 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidate
     if (out_score && P) memcpy(out_score, h_out, P * 8);
     memcpy(out_placed, h_out + o_placed, D * 4);
     s->last_path = "drain";
+    return KS_OK;
+}
+
+int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const ks_node_templates* t, ks_scaleup_option* out,
+                        int32_t* out_best, int32_t* out_node, ks_pod_reasons* out_reasons) {
+    int rc = check_pods(s, pods);
+    if (rc) return rc;
+    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_scaleup_estimate takes host-space pods");
+    if (!t || !out_best) return fail(KS_ERR_INVALID, "NULL templates or out_best");
+    const uint64_t P = pods->n, T = t->n;
+    const uint32_t W = t->label_words;
+    if (W != 1 && W != 2 && W != 4 && W != 8) return fail(KS_ERR_INVALID, "label_words must be 1, 2, 4 or 8 (got %u)", W);
+    if (T && (!out || !t->alloc_cpu || !t->alloc_mem || !t->free_cpu || !t->free_mem || !t->labels || !t->max_nodes))
+        return fail(KS_ERR_INVALID, "NULL template array or out");
+    if (P > KS_SCALEUP_MAX_PODS) return fail(KS_ERR_RANGE, "%llu pods (at most %u)", (unsigned long long)P, KS_SCALEUP_MAX_PODS);
+    if (T > KS_SCALEUP_MAX_TEMPLATES)
+        return fail(KS_ERR_RANGE, "%llu templates (at most %u)", (unsigned long long)T, KS_SCALEUP_MAX_TEMPLATES);
+    const int64_t lc = KS_MAX_CPU_MILLI >> 10, lm = KS_MAX_MEM_BYTES >> 10;
+    for (uint64_t i = 0; i < T; i++) {
+        const int64_t ac = t->alloc_cpu[i], am = t->alloc_mem[i], fc = t->free_cpu[i], fm = t->free_mem[i];
+        if (ac < 1 || ac > lc || am < 1 || am > lm)
+            return fail(KS_ERR_RANGE, "template %llu: allocatable (%lld millicores, %lld bytes) outside [1, 2^26] / [1, 2^45]",
+                        (unsigned long long)i, (long long)ac, (long long)am);
+        if (fc < -lc || fc > ac || fm < -lm || fm > am)
+            return fail(KS_ERR_RANGE, "template %llu: capacity (%lld millicores, %lld bytes) outside [-2^26, allocatable] / "
+                        "[-2^45, allocatable]", (unsigned long long)i, (long long)fc, (long long)fm);
+        if (t->max_nodes[i] > KS_SCALEUP_MAX_NODES)
+            return fail(KS_ERR_RANGE, "template %llu: max_nodes %u (at most %u)", (unsigned long long)i, t->max_nodes[i],
+                        KS_SCALEUP_MAX_NODES);
+    }
+    rc = check_commit_requests(P, pods->req_cpu, pods->req_mem);
+    if (rc) return rc;
+    *out_best = -1;
+    if (T == 0 || P == 0) { // nothing to pack: every row and reason count is zero
+        if (T) memset(out, 0, T * sizeof(ks_scaleup_option));
+        if (out_reasons && P) memset(out_reasons, 0, P * sizeof(ks_pod_reasons));
+        return KS_OK;
+    }
+    std::lock_guard<std::mutex> lk(s->mu);
+    CU_TRY(cudaSetDevice(s->device));
+    // one pinned block each way: in = [rc P | rm P | alloc_cpu T | alloc_mem T | free_cpu T | free_mem T | sel P*W |
+    // labels T*W | max_nodes T], out = [rows T | reasons P (when asked) | node T*P (when asked)]
+    const size_t o_rm = P * 8, o_ac = 2 * P * 8, o_am = o_ac + T * 8, o_fc = o_am + T * 8, o_fm = o_fc + T * 8,
+                 o_sel = o_fm + T * 8, o_lab = o_sel + P * 8 * W, o_max = o_lab + T * 8 * W, in_bytes = o_max + T * 4;
+    const size_t o_why = T * sizeof(ks_scaleup_option), o_node = o_why + (out_reasons ? P * sizeof(ks_pod_reasons) : 0),
+                 out_bytes = o_node + (out_node ? T * P * 4 : 0);
+    const size_t h_out_at = (in_bytes + 15) & ~(size_t)15, h_bytes = h_out_at + out_bytes; // out block 16-byte aligned
+    if (s->h_scaleup_cap < h_bytes) {
+        if (s->h_scaleup) cudaFreeHost(s->h_scaleup);
+        s->h_scaleup = nullptr;
+        s->h_scaleup_cap = 0;
+        const size_t want = h_bytes + h_bytes / 8 + 256;
+        CU_TRY(cudaHostAlloc(&s->h_scaleup, want, cudaHostAllocDefault));
+        s->h_scaleup_cap = want;
+    }
+    uint8_t* h_in = static_cast<uint8_t*>(s->h_scaleup);
+    uint8_t* h_out = h_in + h_out_at;
+    memcpy(h_in, pods->req_cpu, P * 8);
+    memcpy(h_in + o_rm, pods->req_mem, P * 8);
+    memcpy(h_in + o_ac, t->alloc_cpu, T * 8);
+    memcpy(h_in + o_am, t->alloc_mem, T * 8);
+    memcpy(h_in + o_fc, t->free_cpu, T * 8);
+    memcpy(h_in + o_fm, t->free_mem, T * 8);
+    memcpy(h_in + o_sel, pods->sel, P * 8 * W);
+    memcpy(h_in + o_lab, t->labels, T * 8 * W);
+    memcpy(h_in + o_max, t->max_nodes, T * 4);
+    const uint32_t slots = scaleup_slots((uint32_t)T, s->sms);
+    CU_TRY(s->su_in.ensure(in_bytes));
+    CU_TRY(s->su_work.ensure((size_t)slots * 2 * P * 4));
+    CU_TRY(s->su_out.ensure(out_bytes));
+    cudaStream_t st = s->stream;
+    uint8_t* d_in = s->su_in.as<uint8_t>();
+    uint8_t* d_out = s->su_out.as<uint8_t>();
+    CU_TRY(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, st));
+    if (out_node) CU_TRY(cudaMemsetAsync(d_out + o_node, 0xff, T * P * 4, st));
+    const PodView pv{reinterpret_cast<const int64_t*>(d_in), reinterpret_cast<const int64_t*>(d_in + o_rm),
+                     reinterpret_cast<const uint64_t*>(d_in + o_sel), (uint32_t)P};
+    ScaleupArgs a;
+    a.T = (uint32_t)T;
+    a.alloc_cpu = reinterpret_cast<const int64_t*>(d_in + o_ac);
+    a.alloc_mem = reinterpret_cast<const int64_t*>(d_in + o_am);
+    a.free_cpu = reinterpret_cast<const int64_t*>(d_in + o_fc);
+    a.free_mem = reinterpret_cast<const int64_t*>(d_in + o_fm);
+    a.labels = reinterpret_cast<const uint64_t*>(d_in + o_lab);
+    a.max_nodes = reinterpret_cast<const uint32_t*>(d_in + o_max);
+    a.rows = reinterpret_cast<ks_scaleup_option*>(d_out);
+    a.out_node = out_node ? reinterpret_cast<int32_t*>(d_out + o_node) : nullptr;
+    a.reasons = out_reasons ? reinterpret_cast<uint32_t*>(d_out + o_why) : nullptr;
+    a.scratch = s->su_work.as<uint32_t>();
+    a.slots = slots;
+    cudaError_t e = launch_scaleup(pv, W, a, st);
+    if (e != cudaSuccess) return fail(KS_ERR_CUDA, "scale-up launch failed: %s", cudaGetErrorString(e));
+    CU_TRY(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    memcpy(out, h_out, T * sizeof(ks_scaleup_option));
+    if (out_reasons) memcpy(out_reasons, h_out + o_why, P * sizeof(ks_pod_reasons));
+    if (out_node) memcpy(out_node, h_out + o_node, T * P * 4);
+    // the best template: most pods placed, then the highest utilization, then the fewest nodes, then the lowest index
+    int32_t best = -1;
+    for (uint32_t i = 0; i < T; i++) {
+        const ks_scaleup_option& r = out[i];
+        if (r.placed == 0) continue;
+        if (best < 0) {
+            best = (int32_t)i;
+            continue;
+        }
+        const ks_scaleup_option& b = out[best];
+        if (r.placed > b.placed || (r.placed == b.placed && (r.utilization > b.utilization ||
+                                                            (r.utilization == b.utilization && r.nodes < b.nodes))))
+            best = (int32_t)i;
+    }
+    *out_best = best;
+    s->last_path = "scaleup";
     return KS_OK;
 }
 

@@ -89,6 +89,23 @@ struct DrainArgs {
 cudaError_t launch_drain_round(const NodeTable& nt, const PodView& pv, const DrainArgs& da, int policy, uint32_t r,
                                const PartialView& part, const DirectGrid& g, cudaStream_t st);
 
+// scale-up estimate (ks_scaleup_estimate, ks_scaleup.cu).  T templates, each packed on its own by one CTA of
+// k_scaleup_pack; the grid holds `slots` CTAs, CTA b takes templates b, b + slots, ... and sorts in its own scratch
+// slot of 2 * pv.P entries.  Device memory.
+struct ScaleupArgs {
+    uint32_t T;
+    const int64_t *alloc_cpu, *alloc_mem, *free_cpu, *free_mem; // [T]
+    const uint64_t* labels;                                      // [T * W], row-major like the pods' selectors
+    const uint32_t* max_nodes;                                   // [T]
+    ks_scaleup_option* rows;                                     // [T]
+    int32_t* out_node;                                           // [T * P], -1 before the call, or null
+    uint32_t* reasons;                                           // [P][4] in ks_pod_reasons order, or null
+    uint32_t* scratch;                                           // [slots * 2 * P]
+    uint32_t slots;
+};
+uint32_t scaleup_slots(uint32_t T, int sms);
+cudaError_t launch_scaleup(const PodView& pv, uint32_t W, const ScaleupArgs& a, cudaStream_t st);
+
 } // namespace ks
 
 namespace ks {

@@ -1,0 +1,263 @@
+// ks_scaleup.cu — scale-up estimate (ks_scaleup_estimate, include/ksched.h; DESIGN.md 5g), sm_90a.
+// Templates are independent, so each one is a CTA of k_scaleup_pack: it compacts its eligible pods in pod order, sorts
+// them by the order key with a stable LSD radix sort in its own scratch slot, and then one warp walks them through the
+// first-fit packing with the open nodes' remaining capacity in shared memory.  k_scaleup_reasons counts the per-pod
+// rejection reasons over the templates without atomics, one thread per pod.
+#include "ks_launch.h"
+
+namespace ks {
+
+constexpr int SU_THREADS = 256; // 8 warps; the radix pass gives each thread one of the 256 digits
+constexpr int SU_WARPS = SU_THREADS / 32;
+constexpr int SU_CHUNK = 256; // templates staged in shared memory per step of k_scaleup_reasons
+static_assert(SU_THREADS == 256, "one thread per radix digit");
+
+// The order key of a pod for a template: req_cpu * A_m + req_mem * A_c.  Requests lie in [0, 2^36] / [0, 2^55] and
+// allocatables in [1, 2^26] / [1, 2^45] (checked on the host), so the key fits 128 bits; for an eligible pod (req <= F
+// <= A) it is below 2^73.
+__device__ __forceinline__ unsigned __int128 su_key(int64_t rc, int64_t rm, int64_t ac, int64_t am) {
+    return (unsigned __int128)(uint64_t)rc * (uint64_t)am + (unsigned __int128)(uint64_t)rm * (uint64_t)ac;
+}
+
+// Digit of the pod's key at `shift`, inverted so that an ascending stable sort orders the keys descending and keeps
+// equal keys in pod order.
+__device__ __forceinline__ uint32_t su_digit(const PodView& pv, uint32_t p, int64_t ac, int64_t am, uint32_t shift) {
+    const unsigned __int128 k = su_key(__ldg(pv.req_cpu + p), __ldg(pv.req_mem + p), ac, am);
+    return 255u - ((uint32_t)(k >> shift) & 255u);
+}
+
+struct SuShared {
+    int64_t rem_cpu[KS_SCALEUP_MAX_NODES]; // remaining capacity of the open nodes, by ordinal
+    int64_t rem_mem[KS_SCALEUP_MAX_NODES];
+    uint32_t hist[SU_WARPS][256]; // radix pass: per-warp digit counts, then per-warp digit cursors
+    uint32_t wsum[SU_WARPS];
+};
+
+// Exclusive block-wide prefix sum of v; all threads get the total.  Called by the whole CTA.
+__device__ __forceinline__ uint32_t su_block_scan(uint32_t v, uint32_t* wsum, uint32_t& total) {
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t x = v;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const uint32_t y = __shfl_up_sync(0xffffffffu, x, off);
+        if (lane >= (uint32_t)off) x += y;
+    }
+    if (lane == 31) wsum[warp] = x;
+    __syncthreads();
+    uint32_t before = 0, all = 0;
+#pragma unroll
+    for (int w = 0; w < SU_WARPS; w++) {
+        const uint32_t c = wsum[w];
+        before += (uint32_t)w < warp ? c : 0u;
+        all += c;
+    }
+    __syncthreads(); // wsum may be reused
+    total = all;
+    return before + x - v;
+}
+
+// One stable pass of the LSD radix sort, src[0, n) -> dst[0, n), on the 8-bit digit at `shift`.  Warp w owns a
+// contiguous range of src, so the per-(digit, warp) cursors in that order give every element its stable position;
+// inside a warp, equal digits are ranked by lane.  Called by the whole CTA.
+__device__ void su_radix_pass(const PodView& pv, const uint32_t* src, uint32_t* dst, uint32_t n, uint32_t shift,
+                              int64_t ac, int64_t am, SuShared& s) {
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t per = ((n + SU_WARPS - 1) / SU_WARPS + 31) & ~31u;
+    const uint32_t lo = min(n, warp * per), hi = min(n, lo + per);
+    for (uint32_t i = threadIdx.x; i < SU_WARPS * 256; i += SU_THREADS) (&s.hist[0][0])[i] = 0;
+    __syncthreads();
+    for (uint32_t i = lo + lane; i < hi; i += 32) atomicAdd(&s.hist[warp][su_digit(pv, src[i], ac, am, shift)], 1u);
+    __syncthreads();
+    { // thread d: the cursors of digit d, warps in order
+        const uint32_t d = threadIdx.x;
+        uint32_t c[SU_WARPS], sum = 0;
+#pragma unroll
+        for (int w = 0; w < SU_WARPS; w++) {
+            c[w] = s.hist[w][d];
+            sum += c[w];
+        }
+        uint32_t total;
+        uint32_t base = su_block_scan(sum, s.wsum, total);
+#pragma unroll
+        for (int w = 0; w < SU_WARPS; w++) {
+            s.hist[w][d] = base;
+            base += c[w];
+        }
+    }
+    __syncthreads();
+    const uint32_t lt = (1u << lane) - 1u;
+    for (uint32_t i0 = lo; i0 < hi; i0 += 32) { // warp-uniform bounds
+        const uint32_t i = i0 + lane;
+        const bool valid = i < hi;
+        const uint32_t p = valid ? src[i] : 0u;
+        const uint32_t d = valid ? su_digit(pv, p, ac, am, shift) : 0xffffffffu;
+        const uint32_t peers = __match_any_sync(0xffffffffu, d);
+        const uint32_t rank = __popc(peers & lt);
+        const uint32_t pos = valid ? s.hist[warp][d] + rank : 0u;
+        __syncwarp();
+        if (valid && rank == 0) s.hist[warp][d] += __popc(peers);
+        __syncwarp();
+        if (valid) dst[pos] = p;
+    }
+    __syncthreads(); // dst is complete for the next pass
+}
+
+template <int W>
+__global__ void __launch_bounds__(SU_THREADS) k_scaleup_pack(PodView pv, ScaleupArgs a) {
+    __shared__ SuShared s;
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t P = pv.P;
+    uint32_t* const buf0 = a.scratch + (uint64_t)blockIdx.x * 2 * P;
+    uint32_t* const buf1 = buf0 + P;
+    for (uint32_t t = blockIdx.x; t < a.T; t += gridDim.x) {
+        __syncthreads(); // the previous template's walk is done with the scratch slot and the open nodes
+        const int64_t ac = a.alloc_cpu[t], am = a.alloc_mem[t], fc = a.free_cpu[t], fm = a.free_mem[t];
+        uint64_t lab[W];
+#pragma unroll
+        for (int w = 0; w < W; w++) lab[w] = a.labels[(uint64_t)t * W + w];
+        // 1. eligible pods, compacted in pod order
+        uint32_t E = 0;
+        for (uint32_t b = 0; b < P; b += SU_THREADS) {
+            const uint32_t p = b + threadIdx.x;
+            bool ok = false;
+            if (p < P) {
+                ok = (pv.req_cpu[p] <= fc) & (pv.req_mem[p] <= fm);
+                uint64_t miss = 0;
+#pragma unroll
+                for (int w = 0; w < W; w++) miss |= pv.sel[(uint64_t)p * W + w] & ~lab[w];
+                ok &= miss == 0;
+            }
+            uint32_t total;
+            const uint32_t pre = su_block_scan(ok ? 1u : 0u, s.wsum, total);
+            if (ok) buf0[E + pre] = p;
+            E += total;
+        }
+        __syncthreads();
+        // 2. stable sort by the key, descending, over the digits the largest possible key has (fc, fm >= 0 when E > 0)
+        uint32_t* src = buf0;
+        uint32_t* dst = buf1;
+        if (E > 1) {
+            const unsigned __int128 kmax = su_key(fc, fm, ac, am);
+            const uint64_t hi = (uint64_t)(kmax >> 64), lo = (uint64_t)kmax;
+            const uint32_t bits = hi ? 128u - __clzll(hi) : lo ? 64u - __clzll(lo) : 0u;
+            for (uint32_t shift = 0; shift < bits; shift += 8) {
+                su_radix_pass(pv, src, dst, E, shift, ac, am, s);
+                uint32_t* x = src;
+                src = dst;
+                dst = x;
+            }
+        }
+        // 3. first fit, one warp: 32 pods prefetched per step, the open nodes scanned 32 ordinals per ballot
+        if (warp != 0) continue;
+        const uint32_t maxn = a.max_nodes[t];
+        uint32_t nodes = 0, placed = 0;
+        int64_t used_cpu = 0, used_mem = 0;
+        for (uint32_t b = 0; b < E; b += 32) {
+            const uint32_t k = b + lane;
+            const uint32_t kp = k < E ? src[k] : 0u;
+            const int64_t kc = k < E ? pv.req_cpu[kp] : 0, km = k < E ? pv.req_mem[kp] : 0;
+            const uint32_t cnt = min(32u, E - b);
+            for (uint32_t j = 0; j < cnt; j++) {
+                const uint32_t p = __shfl_sync(0xffffffffu, kp, j);
+                const int64_t c = __shfl_sync(0xffffffffu, kc, j), m = __shfl_sync(0xffffffffu, km, j);
+                int32_t node = -1;
+                for (uint32_t o0 = 0; o0 < nodes; o0 += 32) {
+                    const uint32_t o = o0 + lane;
+                    const uint32_t fit = __ballot_sync(0xffffffffu, o < nodes && c <= s.rem_cpu[o] && m <= s.rem_mem[o]);
+                    if (fit) {
+                        node = (int32_t)(o0 + __ffs(fit) - 1);
+                        break;
+                    }
+                }
+                if (node < 0 && nodes < maxn) {
+                    node = (int32_t)nodes++;
+                    if (lane == 0) {
+                        s.rem_cpu[node] = fc;
+                        s.rem_mem[node] = fm;
+                    }
+                }
+                if (node >= 0) {
+                    if (lane == 0) {
+                        s.rem_cpu[node] -= c;
+                        s.rem_mem[node] -= m;
+                        if (a.out_node) a.out_node[(uint64_t)t * P + p] = node;
+                    }
+                    placed++;
+                    used_cpu += c;
+                    used_mem += m;
+                }
+                __syncwarp(); // lane 0's update is seen by the next pod's scan
+            }
+        }
+        if (lane == 0) {
+            ks_scaleup_option r;
+            r.nodes = nodes;
+            r.placed = placed;
+            r.eligible = E;
+            r.utilization = 0;
+            if (nodes) {
+                const int64_t pc = used_cpu * 100 / ((int64_t)nodes * ac), pm = used_mem * 100 / ((int64_t)nodes * am);
+                r.utilization = (int32_t)((pc + pm) / 2);
+            }
+            r.used_cpu = used_cpu;
+            r.used_mem = used_mem;
+            a.rows[t] = r;
+        }
+    }
+}
+
+// One thread per pod: ks_explain's four counts over the templates (capacity F as the free values), staged SU_CHUNK
+// templates at a time.
+template <int W>
+__global__ void __launch_bounds__(SU_THREADS) k_scaleup_reasons(PodView pv, ScaleupArgs a) {
+    __shared__ int64_t s_fc[SU_CHUNK], s_fm[SU_CHUNK];
+    __shared__ uint64_t s_lab[W][SU_CHUNK];
+    const uint32_t p = blockIdx.x * SU_THREADS + threadIdx.x;
+    const bool live = p < pv.P;
+    const int64_t rc = live ? pv.req_cpu[p] : 0, rm = live ? pv.req_mem[p] : 0;
+    uint64_t sel[W];
+#pragma unroll
+    for (int w = 0; w < W; w++) sel[w] = live ? pv.sel[(uint64_t)p * W + w] : 0;
+    uint32_t cpu = 0, mem = 0, nores = 0, nosel = 0;
+    for (uint32_t t0 = 0; t0 < a.T; t0 += SU_CHUNK) {
+        const uint32_t n = min((uint32_t)SU_CHUNK, a.T - t0);
+        __syncthreads();
+        if (threadIdx.x < n) {
+            const uint32_t t = t0 + threadIdx.x;
+            s_fc[threadIdx.x] = a.free_cpu[t];
+            s_fm[threadIdx.x] = a.free_mem[t];
+#pragma unroll
+            for (int w = 0; w < W; w++) s_lab[w][threadIdx.x] = a.labels[(uint64_t)t * W + w];
+        }
+        __syncthreads();
+        for (uint32_t j = 0; j < n; j++) {
+            const bool fc = rc > s_fc[j], fm = rm > s_fm[j];
+            uint64_t miss = 0;
+#pragma unroll
+            for (int w = 0; w < W; w++) miss |= sel[w] & ~s_lab[w][j];
+            cpu += fc;
+            mem += fm;
+            nores += fc | fm;
+            nosel += !(fc | fm) && miss != 0;
+        }
+    }
+    if (live) reinterpret_cast<uint4*>(a.reasons)[p] = make_uint4(cpu, mem, nores, nosel);
+}
+
+uint32_t scaleup_slots(uint32_t T, int sms) { return std::min<uint32_t>(T, 4u * (uint32_t)std::max(sms, 1)); }
+
+cudaError_t launch_scaleup(const PodView& pv, uint32_t W, const ScaleupArgs& a, cudaStream_t st) {
+    if (a.T == 0 || pv.P == 0) return cudaSuccess;
+    return with_label_width(W, [&](auto w) {
+        constexpr int W_ = decltype(w)::value;
+        k_scaleup_pack<W_><<<a.slots, SU_THREADS, 0, st>>>(pv, a);
+        g_launches++;
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess || !a.reasons) return e;
+        k_scaleup_reasons<W_><<<(pv.P + SU_THREADS - 1) / SU_THREADS, SU_THREADS, 0, st>>>(pv, a);
+        g_launches++;
+        return cudaGetLastError();
+    });
+}
+
+} // namespace ks

@@ -42,6 +42,7 @@ for _name, _res, _args in [
     ("ksh_reconcile_gangs", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint64, _vp, C.c_int, _vp, _vp, _vp, _vp,
                                       C.c_size_t, _vp]),
     ("ksh_drain_nodes", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, C.c_int, C.c_uint32, _vp, _vp]),
+    ("ksh_scaleup_estimate", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, C.c_uint64, _vp, C.c_uint64, _vp, _vp, _vp, _vp]),
 ]:
     _f = getattr(lib, _name)
     _f.restype = _res
@@ -329,3 +330,27 @@ class Context:
         if rc != capi.KS_OK:
             raise KsError(rc, "ksh_drain_nodes")
         return placed, node
+
+    def scaleup_estimate(self, templates, n_templates, max_nodes, pods, n_pods, overhead_pods=None, n_overhead=0,
+                         want_nodes=True, want_reasons=True):
+        """Node-group scale-up estimate over objects (ksh_scaleup_estimate): templates are Node objects, overhead_pods
+        the DaemonSet pods charged to the template their spec.nodeName names, pods the pending pods.  Nothing is
+        charged and the context is not changed.  Returns (rows, best, node, reasons) as Snapshot.scaleup_estimate."""
+        max_nodes = np.ascontiguousarray(max_nodes, np.uint32).reshape(-1)
+        if max_nodes.shape[0] != n_templates:
+            raise ValueError(f"need {n_templates} max_nodes entries (got {max_nodes.shape[0]})")
+        rows = np.zeros(n_templates, capi.SCALEUP_OPTION_DTYPE)
+        best = C.c_int32(-1)
+        node = np.empty((n_templates, n_pods), np.int32) if want_nodes else None
+        why = np.empty((n_pods, 4), np.uint32) if want_reasons else None
+
+        def ptr(a):
+            return None if a is None else a.ctypes.data
+
+        def obj(a):
+            return C.addressof(a) if a is not None else None
+        rc = lib.ksh_scaleup_estimate(self._h, obj(templates), n_templates, ptr(max_nodes), obj(overhead_pods),
+                                      n_overhead, obj(pods), n_pods, ptr(rows), C.addressof(best), ptr(node), ptr(why))
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ksh_scaleup_estimate")
+        return rows, best.value, node, why

@@ -224,6 +224,42 @@ class Snapshot:
             raise KsError(rc, "ks_drain_check")
         return placed, idx, score
 
+    def scaleup_estimate(self, req_cpu, req_mem, sel, alloc_cpu, alloc_mem, free_cpu, free_mem, labels, max_nodes,
+                         want_nodes=True, want_reasons=True):
+        """Scale-up estimate (ks_scaleup_estimate): for every node template, how many new nodes would place which of
+        the pods, by first fit in decreasing-size order.  labels is [T, label_words] (the call's own label bits, not the
+        snapshot's) and sel [P, label_words].  Nothing is charged.  Returns (rows, best, node, reasons): rows a
+        capi.SCALEUP_OPTION_DTYPE record array [T], best the picked template or -1, node int32 [T, P] (the new node's
+        ordinal, -1 = not placed; None unless want_nodes), reasons uint32 [P, 4] in ks_explain's columns over the
+        templates (None unless want_reasons)."""
+        req_cpu, req_mem = _c(req_cpu, np.int64).reshape(-1), _c(req_mem, np.int64).reshape(-1)
+        alloc_cpu, alloc_mem = _c(alloc_cpu, np.int64).reshape(-1), _c(alloc_mem, np.int64).reshape(-1)
+        free_cpu, free_mem = _c(free_cpu, np.int64).reshape(-1), _c(free_mem, np.int64).reshape(-1)
+        max_nodes = _c(max_nodes, np.uint32).reshape(-1)
+        t, p = alloc_cpu.shape[0], req_cpu.shape[0]
+        labels = _c(labels, np.uint64).reshape(t, -1) if t else None
+        sel = _c(sel, np.uint64).reshape(p, -1) if p else None
+        w = labels.shape[1] if t else sel.shape[1] if p else 1
+        if p and sel.shape[1] != w:
+            raise ValueError(f"sel has {sel.shape[1]} words per pod, labels {w}")
+        for name, a in (("alloc_mem", alloc_mem), ("free_cpu", free_cpu), ("free_mem", free_mem), ("max_nodes", max_nodes)):
+            if a.shape[0] != t:
+                raise ValueError(f"{name} has {a.shape[0]} entries, alloc_cpu {t}")
+        if req_mem.shape[0] != p:
+            raise ValueError(f"req_mem has {req_mem.shape[0]} entries, req_cpu {p}")
+        pods = ks_pods(p, _ptr(req_cpu), _ptr(req_mem), _ptr(sel), capi.KS_MEM_HOST)
+        tmpl = capi.ks_node_templates(t, w, _ptr(alloc_cpu), _ptr(alloc_mem), _ptr(free_cpu), _ptr(free_mem),
+                                      _ptr(labels), _ptr(max_nodes))
+        rows = np.zeros(t, capi.SCALEUP_OPTION_DTYPE)
+        best = C.c_int32(-1)
+        node = np.empty((t, p), np.int32) if want_nodes else None
+        why = np.empty((p, 4), np.uint32) if want_reasons else None
+        rc = lib.ks_scaleup_estimate(self._h, C.byref(pods), C.byref(tmpl), _ptr(rows), C.addressof(best), _ptr(node),
+                                     _ptr(why))
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ks_scaleup_estimate")
+        return rows, best.value, node, why
+
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
         """The reference's own policy (src/main.rs:49-71), seeded: (node_idx, attempts_used, draw_node, draw_code)."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
