@@ -41,30 +41,37 @@ static int fail(int code, const char* fmt, ...) {
 // larger call, ks_check_cells / ks_select_sampling scratch, ...).
 static std::atomic<uint64_t> g_devbuf_epoch{0};
 
-struct DevBuf {
+// Grow-only buffer in device (DevBuf) or pinned host (HostBuf) memory: ensure() reallocates, dropping the contents, when a
+// call needs more than it holds.  Freed by its destructor, which must run with the owner's device current.
+template <bool Pinned>
+struct Buf {
     void* p = nullptr;
     size_t cap = 0;
+    Buf() = default;
+    Buf(const Buf&) = delete;
+    Buf& operator=(const Buf&) = delete;
+    ~Buf() { release(); }
+    void release() {
+        if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
+        p = nullptr;
+        cap = 0;
+    }
     cudaError_t ensure(size_t bytes) {
         if (bytes <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        g_devbuf_epoch++;
+        release();
+        if (!Pinned) g_devbuf_epoch++; // a pinned block leaves the epoch alone: no captured graph points into one
         size_t want = bytes + bytes / 8 + 256;
-        cudaError_t e = cudaMalloc(&p, want);
+        cudaError_t e = Pinned ? cudaHostAlloc(&p, want, cudaHostAllocDefault) : cudaMalloc(&p, want);
         if (e == cudaSuccess) cap = want;
         return e;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
     }
     template <class T>
     T* as() {
         return static_cast<T*>(p);
     }
 };
+using DevBuf = Buf<false>;
+using HostBuf = Buf<true>;
 
 struct ks_snapshot {
     int device = 0;
@@ -76,17 +83,13 @@ struct ks_snapshot {
     DevBuf st_reasons; // ks_explain with host-space output
     DevBuf st_topk, part_topk; // ks_select_topk: host-space outputs, node-chunk partials
     DevBuf st_pre, vx_pre, part_pre; // ks_preempt: host-space outputs and priorities, victim index, node-chunk partials
-    DevBuf sb_pkey, sb_pidx, sb_pend; // device-side streaming loop (k_stream_batch)
-    void* h_stream = nullptr;                 // pinned staging of one streaming micro-batch (inputs and results)
-    DevBuf gb_in, gb_out;                     // ks_gang_bind: pods and groups in, results out
-    void* h_gang = nullptr;                   // pinned staging of both (grown on demand)
-    size_t h_gang_cap = 0;
-    DevBuf dr_in, dr_work, dr_out;            // ks_drain_check: pods and candidates in, overlays and partials, results out
-    void* h_drain = nullptr;                  // pinned staging of the input and result blocks (grown on demand)
-    size_t h_drain_cap = 0;
-    DevBuf su_in, su_work, su_out;            // ks_scaleup_estimate: pods and templates in, sort scratch, results out
-    void* h_scaleup = nullptr;                // pinned staging of the input and result blocks (grown on demand)
-    size_t h_scaleup_cap = 0;
+    DevBuf sb_pkey, sb_pidx, sb_pend; // device-side streaming loop (k_stream_batch, k_gang_batch)
+    // Staging of the host-staged calls (ks_stream_bind's device loop, ks_gang_bind, ks_drain_check,
+    // ks_scaleup_estimate): a pinned block with the inputs at 0 and the results after them (stage_blocks), the device
+    // copies of both, and device work space.  One set serves all four because each of them holds mu from its first
+    // staging write to its final stream synchronise, so no two are ever live; the snapshot keeps the largest.
+    HostBuf h_stage;
+    DevBuf d_in, d_work, d_out;
     int sms = 0, coop = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     // host-space calls are pipelined in pod chunks: chunk c+1 is copied in on copy_stream while chunk c computes
@@ -139,6 +142,40 @@ static int check_commit_requests(uint64_t n, const int64_t* req_cpu, const int64
         if (req_cpu[i] < 0 || req_cpu[i] > KS_MAX_CPU_MILLI || req_mem[i] < 0 || req_mem[i] > KS_MAX_MEM_BYTES)
             return fail(KS_ERR_RANGE, "pod %llu: request (%lld millicores, %lld bytes) outside [0, 2^36] / [0, 2^55]",
                         (unsigned long long)i, (long long)req_cpu[i], (long long)req_mem[i]);
+    return KS_OK;
+}
+
+// The shared staging set for one host-staged call: d_in and d_out hold in_bytes and out_bytes, and the pinned block holds
+// the inputs at 0 and the results at the next multiple of 16 after them (*h_out).
+static int stage_blocks(ks_snapshot* s, size_t in_bytes, size_t out_bytes, uint8_t** h_out) {
+    BlockLayout h;
+    h.take<uint8_t>(in_bytes);
+    const size_t out_at = h.take<uint8_t>(out_bytes, 16);
+    CU_TRY(s->h_stage.ensure(h.size));
+    CU_TRY(s->d_in.ensure(in_bytes));
+    CU_TRY(s->d_out.ensure(out_bytes));
+    *h_out = at<uint8_t>(s->h_stage.p, out_at);
+    return KS_OK;
+}
+
+// What k_stream_batch and k_gang_batch take from the snapshot: the node table, the policy, the sb_* scratch and the
+// grid.  The caller sets the pods, the outputs, ctl and max_rounds.
+static int stream_batch_args(ks_snapshot* s, int policy, StreamBatchArgs* a) {
+    CU_TRY(s->sb_pkey.ensure((size_t)STREAM_BATCH_MAX * s->sms * 8));
+    CU_TRY(s->sb_pidx.ensure((size_t)STREAM_BATCH_MAX * s->sms * 4));
+    CU_TRY(s->sb_pend.ensure(2 * STREAM_BATCH_MAX * 4));
+    a->N = s->N;
+    a->Npad = s->Npad;
+    a->alloc_cpu = s->alloc_cpu.as<int64_t>();
+    a->alloc_mem = s->alloc_mem.as<int64_t>();
+    a->labels = s->labels.as<uint64_t>();
+    a->free_cpu = s->free_cpu.as<int64_t>();
+    a->free_mem = s->free_mem.as<int64_t>();
+    a->policy = policy;
+    a->pkey = s->sb_pkey.as<int64_t>();
+    a->pidx = s->sb_pidx.as<int32_t>();
+    a->pend = s->sb_pend.as<uint32_t>();
+    a->grid = std::max(1u, std::min<uint32_t>((uint32_t)s->sms, (s->N + 127u) / 128u));
     return KS_OK;
 }
 
@@ -199,18 +236,6 @@ void ks_snapshot_destroy(ks_snapshot* s) {
     if (!s) return;
     cudaSetDevice(s->device);
     if (s->stream) cudaStreamSynchronize(s->stream);
-    DevBuf* bufs[] = {&s->alloc_cpu, &s->alloc_mem, &s->free_cpu, &s->free_mem, &s->prio,     &s->labels,
-                      &s->flag,      &s->st_rc,     &s->st_rm,    &s->st_sel,   &s->st_idx,   &s->st_score,
-                      &s->st_cnt,    &s->st_mask,   &s->st_codes, &s->st_bnode, &s->st_bcpu,  &s->st_bmem,
-                      &s->part_key,  &s->part_idx,  &s->part_cnt, &s->st_samp,  &s->xflag,
-                      &s->sb_pkey,   &s->sb_pidx,   &s->sb_pend,  &s->st_reasons, &s->st_topk,
-                      &s->part_topk, &s->st_pre,     &s->vx_pre,   &s->part_pre, &s->gb_in,      &s->gb_out,
-                      &s->dr_in,     &s->dr_work,   &s->dr_out,   &s->su_in,    &s->su_work,  &s->su_out};
-    if (s->h_stream) cudaFreeHost(s->h_stream);
-    if (s->h_gang) cudaFreeHost(s->h_gang);
-    if (s->h_drain) cudaFreeHost(s->h_drain);
-    if (s->h_scaleup) cudaFreeHost(s->h_scaleup);
-    for (DevBuf* b : bufs) b->release();
     bitpar_release(s->bp);
     if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
     for (int i = 0; i < 4; i++)
@@ -220,7 +245,7 @@ void ks_snapshot_destroy(ks_snapshot* s) {
     if (s->ev_cfork) cudaEventDestroy(s->ev_cfork);
     if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
     if (s->stream) cudaStreamDestroy(s->stream);
-    delete s;
+    delete s; // frees the buffers: the device is set and the stream synchronised
 }
 
 uint32_t ks_snapshot_num_nodes(const ks_snapshot* s) { return s ? s->N : 0; }
@@ -897,14 +922,15 @@ int ks_select_sampling(ks_snapshot* s, const ks_pods* pods, uint32_t attempts, u
     rc = stage_pods(s, pods, s->stream, &pv);
     if (rc) return rc;
     // one scratch buffer: node_idx[P] | attempts[P] | draw_node[P*attempts] | draw_code[P*attempts]
-    const size_t off_att = P * 4, off_dn = off_att + P * 4, off_dc = off_dn + draws * 4;
-    CU_TRY(s->st_samp.ensure(off_dc + draws));
+    BlockLayout L;
+    const size_t off_idx = L.take<int32_t>(P), off_att = L.take<uint32_t>(P), off_dn = L.take<int32_t>(draws),
+                 off_dc = L.take<uint8_t>(draws);
+    CU_TRY(s->st_samp.ensure(L.size));
     uint8_t* base = s->st_samp.as<uint8_t>();
-    CU_TRY(launch_select_sampling(node_table(s), pv, attempts, seed, first_pod_index, reinterpret_cast<int32_t*>(base),
-                                  reinterpret_cast<uint32_t*>(base + off_att),
-                                  out_draw_node ? reinterpret_cast<int32_t*>(base + off_dn) : nullptr,
+    CU_TRY(launch_select_sampling(node_table(s), pv, attempts, seed, first_pod_index, at<int32_t>(base, off_idx),
+                                  at<uint32_t>(base, off_att), out_draw_node ? at<int32_t>(base, off_dn) : nullptr,
                                   out_draw_code ? base + off_dc : nullptr, s->stream));
-    CU_TRY(cudaMemcpyAsync(out_node_idx, base, P * 4, cudaMemcpyDeviceToHost, s->stream));
+    CU_TRY(cudaMemcpyAsync(out_node_idx, base + off_idx, P * 4, cudaMemcpyDeviceToHost, s->stream));
     if (out_attempts) CU_TRY(cudaMemcpyAsync(out_attempts, base + off_att, P * 4, cudaMemcpyDeviceToHost, s->stream));
     if (out_draw_node) CU_TRY(cudaMemcpyAsync(out_draw_node, base + off_dn, draws * 4, cudaMemcpyDeviceToHost, s->stream));
     if (out_draw_code) CU_TRY(cudaMemcpyAsync(out_draw_code, base + off_dc, draws, cudaMemcpyDeviceToHost, s->stream));
@@ -958,11 +984,13 @@ int ks_select_topk(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t k, 
     const uint64_t cells = P * k;
     OutView ov{out_node_idx, out_score, out_feasible_cnt, nullptr, 0, 0};
     if (out_space == KS_MEM_HOST) { // one staging block: score [P*k] | node_idx [P*k] | feasible_cnt [P]
-        CU_TRY(s->st_topk.ensure(cells * 12 + P * 4));
-        uint8_t* b = s->st_topk.as<uint8_t>();
-        ov.score = out_score ? reinterpret_cast<int64_t*>(b) : nullptr;
-        ov.node_idx = reinterpret_cast<int32_t*>(b + cells * 8);
-        ov.cnt = out_feasible_cnt ? reinterpret_cast<uint32_t*>(b + cells * 12) : nullptr;
+        BlockLayout L;
+        const size_t o_score = L.take<int64_t>(cells), o_idx = L.take<int32_t>(cells), o_cnt = L.take<uint32_t>(P);
+        CU_TRY(s->st_topk.ensure(L.size));
+        void* b = s->st_topk.p;
+        ov.score = out_score ? at<int64_t>(b, o_score) : nullptr;
+        ov.node_idx = at<int32_t>(b, o_idx);
+        ov.cnt = out_feasible_cnt ? at<uint32_t>(b, o_cnt) : nullptr;
     }
     if (s->N == 0) { // no node: every slot is empty
         CU_TRY(cudaMemsetAsync(ov.node_idx, 0xff, cells * 4, st));
@@ -976,11 +1004,13 @@ int ks_select_topk(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t k, 
         PartialView part{nullptr, nullptr, nullptr};
         if (g.n_chunks > 1) { // keys [chunks*P*k] | indices [chunks*P*k] | counts [chunks*P]
             const uint64_t rows = (uint64_t)g.n_chunks * P;
-            CU_TRY(s->part_topk.ensure(rows * k * 12 + rows * 4));
-            uint8_t* b = s->part_topk.as<uint8_t>();
-            part.key = reinterpret_cast<int64_t*>(b);
-            part.idx = reinterpret_cast<int32_t*>(b + rows * k * 8);
-            part.cnt = reinterpret_cast<uint32_t*>(b + rows * k * 12);
+            BlockLayout L;
+            const size_t o_key = L.take<int64_t>(rows * k), o_idx = L.take<int32_t>(rows * k), o_cnt = L.take<uint32_t>(rows);
+            CU_TRY(s->part_topk.ensure(L.size));
+            void* b = s->part_topk.p;
+            part.key = at<int64_t>(b, o_key);
+            part.idx = at<int32_t>(b, o_idx);
+            part.cnt = at<uint32_t>(b, o_cnt);
         }
         CU_TRY(launch_select_topk(node_table(s), pv, policy, k, ov, part, g, st));
     }
@@ -1045,12 +1075,13 @@ int ks_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* pod_priority,
     int32_t* d_vic = out_victims;
     const int32_t* d_prio = pod_priority;
     // one staging block: rows [P] | victims [P * max_victims] (host-space outputs) | priorities [P] (host-space pods)
-    const size_t o_vic = P * sizeof(ks_preemption), o_prio = o_vic + n_vic * 4;
-    CU_TRY(s->st_pre.ensure(o_prio + P * 4));
-    uint8_t* stg = s->st_pre.as<uint8_t>();
+    BlockLayout L;
+    const size_t o_rows = L.take<ks_preemption>(P), o_vic = L.take<int32_t>(n_vic), o_prio = L.take<int32_t>(P);
+    CU_TRY(s->st_pre.ensure(L.size));
+    void* stg = s->st_pre.p;
     if (out_space == KS_MEM_HOST) {
-        d_out = reinterpret_cast<ks_preemption*>(stg);
-        d_vic = out_victims ? reinterpret_cast<int32_t*>(stg + o_vic) : nullptr;
+        d_out = at<ks_preemption>(stg, o_rows);
+        d_vic = out_victims ? at<int32_t>(stg, o_vic) : nullptr;
     }
     PodView pv{nullptr, nullptr, nullptr, (uint32_t)P};
     VictimIndex vx{};
@@ -1060,8 +1091,8 @@ int ks_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* pod_priority,
         rc = stage_pods(s, pods, st, &pv);
         if (rc) return rc;
         if (pods->mem_space == KS_MEM_HOST) {
-            CU_TRY(cudaMemcpyAsync(stg + o_prio, pod_priority, P * 4, cudaMemcpyHostToDevice, st));
-            d_prio = reinterpret_cast<const int32_t*>(stg + o_prio);
+            CU_TRY(cudaMemcpyAsync(at<int32_t>(stg, o_prio), pod_priority, P * 4, cudaMemcpyHostToDevice, st));
+            d_prio = at<int32_t>(stg, o_prio);
         }
         // the victim index: upload the bound list, sort it by (node, priority), prefix sums per node
         CU_TRY(s->vx_pre.ensure(victim_index_bytes(B, s->N)));
@@ -1075,12 +1106,15 @@ int ks_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* pod_priority,
         CU_TRY(build_victim_index(s->vx_pre.p, B, s->N, &vx, st));
         g = direct_grid(s->W, pv.P, s->Npad, s->sms);
         const uint64_t rows = (uint64_t)g.n_chunks * P; // hi [rows] | lo [rows] | candidates [rows] | feasible [rows]
-        CU_TRY(s->part_pre.ensure(rows * 24));
-        uint8_t* b = s->part_pre.as<uint8_t>();
-        part.hi = reinterpret_cast<uint64_t*>(b);
-        part.lo = reinterpret_cast<uint64_t*>(b + rows * 8);
-        part.cand = reinterpret_cast<uint32_t*>(b + rows * 16);
-        part.cnt = reinterpret_cast<uint32_t*>(b + rows * 20);
+        BlockLayout PL;
+        const size_t o_hi = PL.take<uint64_t>(rows), o_lo = PL.take<uint64_t>(rows), o_cand = PL.take<uint32_t>(rows),
+                     o_cnt = PL.take<uint32_t>(rows);
+        CU_TRY(s->part_pre.ensure(PL.size));
+        void* b = s->part_pre.p;
+        part.hi = at<uint64_t>(b, o_hi);
+        part.lo = at<uint64_t>(b, o_lo);
+        part.cand = at<uint32_t>(b, o_cand);
+        part.cnt = at<uint32_t>(b, o_cnt);
     }
     CU_TRY(launch_preempt(node_table(s), pv, d_prio, vx, max_victims, part, g, d_out, d_vic, st));
     if (out_space == KS_MEM_HOST) {
@@ -1103,60 +1137,46 @@ int ks_stream_bind(ks_snapshot* s, const ks_pods* pods, int policy, int32_t* out
     rc = check_commit_requests(n, pods->req_cpu, pods->req_mem);
     if (rc) return rc;
     if (n > 0 && n <= STREAM_BATCH_MAX && s->N > 0 && s->coop) {
-        // device-side loop: one H2D, ONE cooperative launch that runs every round, one D2H
+        // device-side loop: the inputs [rc | rm | sel] and the results [score | idx | ctl] each travel as one block, so
+        // the micro-batch costs ONE H2D copy, ONE cooperative launch that runs every round and ONE D2H copy
         std::lock_guard<std::mutex> lk(s->mu);
         CU_TRY(cudaSetDevice(s->device));
-        // one pinned staging block: inputs [rc | rm | sel] and results [score | idx | ctl] are contiguous, so the whole
-        // micro-batch costs ONE H2D copy, ONE cooperative launch and ONE D2H copy
-        const size_t in_bytes = n * (16 + 8 * (size_t)W), o_score = 0, o_idx = n * 8, o_ctl = o_idx + ((n * 4 + 7) & ~(size_t)7),
-                     out_bytes = o_ctl + 8;
-        const size_t h_cap = (size_t)STREAM_BATCH_MAX * (16 + 8 * KS_MAX_LABEL_WORDS) + (size_t)STREAM_BATCH_MAX * 12 + 64;
-        if (!s->h_stream) CU_TRY(cudaHostAlloc(&s->h_stream, h_cap, cudaHostAllocDefault));
-        uint8_t* h_in = static_cast<uint8_t*>(s->h_stream);
-        uint8_t* h_out = h_in + (size_t)STREAM_BATCH_MAX * (16 + 8 * KS_MAX_LABEL_WORDS);
-        memcpy(h_in, pods->req_cpu, n * 8);
-        memcpy(h_in + n * 8, pods->req_mem, n * 8);
-        memcpy(h_in + n * 16, pods->sel, n * 8 * W);
-        const uint32_t grid = std::max(1u, std::min<uint32_t>((uint32_t)s->sms, (s->N + 127u) / 128u));
-        CU_TRY(s->st_rc.ensure((size_t)STREAM_BATCH_MAX * (16 + 8 * KS_MAX_LABEL_WORDS))); // device copy of the input block
-        CU_TRY(s->st_score.ensure((size_t)STREAM_BATCH_MAX * 12 + 64));                      // device copy of the result block
-        CU_TRY(s->sb_pkey.ensure((size_t)STREAM_BATCH_MAX * s->sms * 8));
-        CU_TRY(s->sb_pidx.ensure((size_t)STREAM_BATCH_MAX * s->sms * 4));
-        CU_TRY(s->sb_pend.ensure(2 * STREAM_BATCH_MAX * 4));
-        cudaStream_t st = s->stream;
-        uint8_t* d_in = s->st_rc.as<uint8_t>();
-        uint8_t* d_out = s->st_score.as<uint8_t>();
-        CU_TRY(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, st));
+        BlockLayout in, out;
+        const size_t i_rc = in.take<int64_t>(n), i_rm = in.take<int64_t>(n), i_sel = in.take<uint64_t>(n * W);
+        const size_t o_score = out.take<int64_t>(n), o_idx = out.take<int32_t>(n), o_ctl = out.take<uint32_t>(2);
+        // sized for STREAM_BATCH_MAX pods on first use, so a stream of growing micro-batches never reallocates
+        uint8_t* h_out = nullptr;
+        rc = stage_blocks(s, (size_t)STREAM_BATCH_MAX * (16 + 8 * KS_MAX_LABEL_WORDS), (size_t)STREAM_BATCH_MAX * 12 + 8,
+                          &h_out);
+        if (!rc) rc = stage_blocks(s, in.size, out.size, &h_out);
         StreamBatchArgs a;
-        a.N = s->N;
-        a.Npad = s->Npad;
-        a.alloc_cpu = s->alloc_cpu.as<int64_t>();
-        a.alloc_mem = s->alloc_mem.as<int64_t>();
-        a.labels = s->labels.as<uint64_t>();
-        a.free_cpu = s->free_cpu.as<int64_t>();
-        a.free_mem = s->free_mem.as<int64_t>();
-        a.policy = policy;
+        if (!rc) rc = stream_batch_args(s, policy, &a);
+        if (rc) return rc;
+        uint8_t* h_in = s->h_stage.as<uint8_t>();
+        memcpy(h_in + i_rc, pods->req_cpu, n * 8);
+        memcpy(h_in + i_rm, pods->req_mem, n * 8);
+        memcpy(h_in + i_sel, pods->sel, n * 8 * W);
+        cudaStream_t st = s->stream;
+        uint8_t* d_in = s->d_in.as<uint8_t>();
+        uint8_t* d_out = s->d_out.as<uint8_t>();
+        CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
         a.m = (uint32_t)n;
-        a.req_cpu = reinterpret_cast<const int64_t*>(d_in);
-        a.req_mem = reinterpret_cast<const int64_t*>(d_in + n * 8);
-        a.sel = reinterpret_cast<const uint64_t*>(d_in + n * 16);
-        a.pkey = s->sb_pkey.as<int64_t>();
-        a.pidx = s->sb_pidx.as<int32_t>();
-        a.pend = s->sb_pend.as<uint32_t>();
-        a.ctl = reinterpret_cast<uint32_t*>(d_out + o_ctl);
-        a.out_idx = reinterpret_cast<int32_t*>(d_out + o_idx);
-        a.out_score = reinterpret_cast<int64_t*>(d_out + o_score);
+        a.req_cpu = at<int64_t>(d_in, i_rc);
+        a.req_mem = at<int64_t>(d_in, i_rm);
+        a.sel = at<uint64_t>(d_in, i_sel);
+        a.ctl = at<uint32_t>(d_out, o_ctl);
+        a.out_idx = at<int32_t>(d_out, o_idx);
+        a.out_score = at<int64_t>(d_out, o_score);
         a.max_rounds = (uint32_t)n + 1;
-        a.grid = grid;
         s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
         s->version++;
         cudaError_t e = launch_stream_batch(a, W, st);
         if (e != cudaSuccess) return fail(KS_ERR_CUDA, "k_stream_batch launch failed: %s", cudaGetErrorString(e));
-        CU_TRY(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(h_out, d_out, out.size, cudaMemcpyDeviceToHost, st));
         CU_TRY(cudaStreamSynchronize(st));
         memcpy(out_node_idx, h_out + o_idx, n * 4);
         if (out_score) memcpy(out_score, h_out + o_score, n * 8);
-        if (out_rounds) *out_rounds = reinterpret_cast<const uint32_t*>(h_out + o_ctl)[1];
+        if (out_rounds) *out_rounds = at<uint32_t>(h_out, o_ctl)[1];
         s->last_path = "stream_batch";
         return KS_OK;
     }
@@ -1241,73 +1261,51 @@ int ks_gang_bind(ks_snapshot* s, const ks_pods* pods, const ks_gangs* gangs, int
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
     if (!s->coop) return fail(KS_ERR_CUDA, "device %d has no cooperative launch", s->device);
-    // one pinned block each way: in = [rc P | rm P | sel P*W | offset G+1 | min_member G],
-    // out = [score P | idx P | ctl 2G | placed G]
-    const size_t o_rm = P * 8, o_sel = 2 * P * 8, o_off = o_sel + P * 8 * W, o_min = o_off + (G + 1) * 4,
-                 in_bytes = o_min + G * 4;
-    const size_t o_idx = P * 8, o_ctl = o_idx + P * 4, o_placed = o_ctl + 2 * G * 4, out_bytes = o_placed + G * 4;
-    const size_t h_out_at = (in_bytes + 7) & ~(size_t)7, h_bytes = h_out_at + out_bytes; // out block 8-byte aligned
-    if (s->h_gang_cap < h_bytes) {
-        if (s->h_gang) cudaFreeHost(s->h_gang);
-        s->h_gang = nullptr;
-        s->h_gang_cap = 0;
-        const size_t want = h_bytes + h_bytes / 8 + 256;
-        CU_TRY(cudaHostAlloc(&s->h_gang, want, cudaHostAllocDefault));
-        s->h_gang_cap = want;
-    }
-    uint8_t* h_in = static_cast<uint8_t*>(s->h_gang);
-    uint8_t* h_out = h_in + h_out_at;
-    memcpy(h_in, pods->req_cpu, P * 8);
-    memcpy(h_in + o_rm, pods->req_mem, P * 8);
-    memcpy(h_in + o_sel, pods->sel, P * 8 * W);
-    uint32_t* h_off = reinterpret_cast<uint32_t*>(h_in + o_off);
-    for (uint64_t g = 0; g <= G; g++) h_off[g] = (uint32_t)off[g];
-    memcpy(h_in + o_min, gangs->min_member, G * 4);
-    CU_TRY(s->gb_in.ensure(in_bytes));
-    CU_TRY(s->gb_out.ensure(out_bytes));
-    CU_TRY(s->sb_pkey.ensure((size_t)STREAM_BATCH_MAX * s->sms * 8));
-    CU_TRY(s->sb_pidx.ensure((size_t)STREAM_BATCH_MAX * s->sms * 4));
-    CU_TRY(s->sb_pend.ensure(2 * STREAM_BATCH_MAX * 4));
-    cudaStream_t st = s->stream;
-    uint8_t* d_in = s->gb_in.as<uint8_t>();
-    uint8_t* d_out = s->gb_out.as<uint8_t>();
-    CU_TRY(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, st));
+    // one block each way: in = [rc P | rm P | sel P*W | offset G+1 | min_member G], out = [score P | idx P | ctl 2G | placed G]
+    BlockLayout in, out;
+    const size_t i_rc = in.take<int64_t>(P), i_rm = in.take<int64_t>(P), i_sel = in.take<uint64_t>(P * W),
+                 i_off = in.take<uint32_t>(G + 1), i_min = in.take<uint32_t>(G);
+    const size_t o_score = out.take<int64_t>(P), o_idx = out.take<int32_t>(P), o_ctl = out.take<uint32_t>(2 * G),
+                 o_placed = out.take<uint32_t>(G);
+    uint8_t* h_out = nullptr;
+    rc = stage_blocks(s, in.size, out.size, &h_out);
     StreamBatchArgs a;
-    a.N = s->N;
-    a.Npad = s->Npad;
-    a.alloc_cpu = s->alloc_cpu.as<int64_t>();
-    a.alloc_mem = s->alloc_mem.as<int64_t>();
-    a.labels = s->labels.as<uint64_t>();
-    a.free_cpu = s->free_cpu.as<int64_t>();
-    a.free_mem = s->free_mem.as<int64_t>();
-    a.policy = policy;
+    if (!rc) rc = stream_batch_args(s, policy, &a);
+    if (rc) return rc;
+    uint8_t* h_in = s->h_stage.as<uint8_t>();
+    memcpy(h_in + i_rc, pods->req_cpu, P * 8);
+    memcpy(h_in + i_rm, pods->req_mem, P * 8);
+    memcpy(h_in + i_sel, pods->sel, P * 8 * W);
+    uint32_t* h_off = at<uint32_t>(h_in, i_off);
+    for (uint64_t g = 0; g <= G; g++) h_off[g] = (uint32_t)off[g];
+    memcpy(h_in + i_min, gangs->min_member, G * 4);
+    cudaStream_t st = s->stream;
+    uint8_t* d_in = s->d_in.as<uint8_t>();
+    uint8_t* d_out = s->d_out.as<uint8_t>();
+    CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
     a.m = (uint32_t)P;
-    a.req_cpu = reinterpret_cast<const int64_t*>(d_in);
-    a.req_mem = reinterpret_cast<const int64_t*>(d_in + o_rm);
-    a.sel = reinterpret_cast<const uint64_t*>(d_in + o_sel);
-    a.pkey = s->sb_pkey.as<int64_t>();
-    a.pidx = s->sb_pidx.as<int32_t>();
-    a.pend = s->sb_pend.as<uint32_t>();
+    a.req_cpu = at<int64_t>(d_in, i_rc);
+    a.req_mem = at<int64_t>(d_in, i_rm);
+    a.sel = at<uint64_t>(d_in, i_sel);
     a.ctl = nullptr; // per group: ga.ctl
-    a.out_idx = reinterpret_cast<int32_t*>(d_out + o_idx);
-    a.out_score = reinterpret_cast<int64_t*>(d_out);
+    a.out_idx = at<int32_t>(d_out, o_idx);
+    a.out_score = at<int64_t>(d_out, o_score);
     a.max_rounds = 0; // per group
-    a.grid = std::max(1u, std::min<uint32_t>((uint32_t)s->sms, (s->N + 127u) / 128u));
     GangArgs ga;
     ga.n = (uint32_t)G;
-    ga.offset = reinterpret_cast<const uint32_t*>(d_in + o_off);
-    ga.min_member = reinterpret_cast<const uint32_t*>(d_in + o_min);
-    ga.ctl = reinterpret_cast<uint32_t*>(d_out + o_ctl);
-    ga.placed = reinterpret_cast<uint32_t*>(d_out + o_placed);
+    ga.offset = at<uint32_t>(d_in, i_off);
+    ga.min_member = at<uint32_t>(d_in, i_min);
+    ga.ctl = at<uint32_t>(d_out, o_ctl);
+    ga.placed = at<uint32_t>(d_out, o_placed);
     s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
     s->version++;
     cudaError_t e = launch_gang_batch(a, ga, W, st);
     if (e != cudaSuccess) return fail(KS_ERR_CUDA, "k_gang_batch launch failed: %s", cudaGetErrorString(e));
-    CU_TRY(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(h_out, d_out, out.size, cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));
     memcpy(out_node_idx, h_out + o_idx, P * 4);
-    if (out_score) memcpy(out_score, h_out, P * 8);
-    const uint32_t* ctl = reinterpret_cast<const uint32_t*>(h_out + o_ctl);
+    if (out_score) memcpy(out_score, h_out + o_score, P * 8);
+    const uint32_t* ctl = at<uint32_t>(h_out, o_ctl);
     if (out_rounds)
         for (uint64_t g = 0; g < G; g++) out_rounds[g] = ctl[2 * g + 1];
     if (out_placed) memcpy(out_placed, h_out + o_placed, G * 4);
@@ -1361,90 +1359,84 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidate
         for (uint64_t r = 0; r < off[d + 1] - off[d]; r++) per_round[r]++;
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
-    // one pinned block each way: in = [rc P | rm P | sel P*W (pods in round order) | cand_node D | pod_base D | cand_id D |
+    // one block each way: in = [rc P | rm P | sel P*W (pods in round order) | cand_node D | pod_base D | cand_id D |
     // excluded-node bits Npad/32 (with the flag)], out = [score P | idx P | placed D]
     const bool excl = flags & KS_DRAIN_EXCLUDE_CANDIDATES;
-    const size_t o_rm = P * 8, o_sel = 2 * P * 8, o_node = o_sel + P * 8 * W, o_base = o_node + D * 4, o_id = o_base + D * 4,
-                 o_excl = o_id + D * 4, in_bytes = o_excl + (excl ? (size_t)s->Npad / 8 : 0);
-    const size_t o_idx = P * 8, o_placed = o_idx + P * 4, out_bytes = o_placed + D * 4;
-    const size_t h_out_at = (in_bytes + 7) & ~(size_t)7, h_bytes = h_out_at + out_bytes; // out block 8-byte aligned
-    if (s->h_drain_cap < h_bytes) {
-        if (s->h_drain) cudaFreeHost(s->h_drain);
-        s->h_drain = nullptr;
-        s->h_drain_cap = 0;
-        const size_t want = h_bytes + h_bytes / 8 + 256;
-        CU_TRY(cudaHostAlloc(&s->h_drain, want, cudaHostAllocDefault));
-        s->h_drain_cap = want;
-    }
-    uint8_t* h_in = static_cast<uint8_t*>(s->h_drain);
-    uint8_t* h_out = h_in + h_out_at;
-    int64_t* h_rc = reinterpret_cast<int64_t*>(h_in);
-    int64_t* h_rm = reinterpret_cast<int64_t*>(h_in + o_rm);
-    uint64_t* h_sel = reinterpret_cast<uint64_t*>(h_in + o_sel);
-    int32_t* h_node = reinterpret_cast<int32_t*>(h_in + o_node);
-    uint32_t* h_base = reinterpret_cast<uint32_t*>(h_in + o_base);
-    uint32_t* h_id = reinterpret_cast<uint32_t*>(h_in + o_id);
+    BlockLayout in, out;
+    const size_t i_rc = in.take<int64_t>(P), i_rm = in.take<int64_t>(P), i_sel = in.take<uint64_t>(P * W),
+                 i_node = in.take<int32_t>(D), i_base = in.take<uint32_t>(D), i_id = in.take<uint32_t>(D),
+                 i_excl = in.take<uint32_t>(excl ? s->Npad / 32 : 0);
+    const size_t o_score = out.take<int64_t>(P), o_idx = out.take<int32_t>(P), o_placed = out.take<uint32_t>(D);
+    // node-chunk partials: the largest round needs the most
+    uint64_t part_rows = 0;
+    for (uint32_t r = 0; r < rounds; r++)
+        part_rows = std::max<uint64_t>(part_rows, (uint64_t)direct_grid(W, per_round[r], s->Npad, s->sms).n_chunks * per_round[r]);
+    // work = [ov_fc P | ov_fm P | part keys | ov_node P | part indices | ov_cnt D, failed D (one array: zeroed together)]
+    BlockLayout work;
+    const size_t w_fc = work.take<int64_t>(P), w_fm = work.take<int64_t>(P), w_key = work.take<int64_t>(part_rows),
+                 w_node = work.take<int32_t>(P), w_idx = work.take<int32_t>(part_rows), w_cnt = work.take<uint32_t>(2 * D);
+    uint8_t* h_out = nullptr;
+    rc = stage_blocks(s, in.size, out.size, &h_out);
+    if (rc) return rc;
+    CU_TRY(s->d_work.ensure(work.size));
+    uint8_t* h_in = s->h_stage.as<uint8_t>();
+    int64_t* h_rc = at<int64_t>(h_in, i_rc);
+    int64_t* h_rm = at<int64_t>(h_in, i_rm);
+    uint64_t* h_sel = at<uint64_t>(h_in, i_sel);
+    int32_t* h_node = at<int32_t>(h_in, i_node);
+    uint32_t* h_base = at<uint32_t>(h_in, i_base);
+    uint32_t* h_id = at<uint32_t>(h_in, i_id);
     for (uint64_t j = 0; j < D; j++) {
         h_node[j] = cand->node_idx[order[j]];
         h_base[j] = (uint32_t)off[order[j]];
         h_id[j] = order[j];
     }
-    for (uint64_t r = 0, at = 0; r < rounds; at += per_round[r], r++) // round r: pod r of the first per_round[r] candidates
+    for (uint64_t r = 0, r0 = 0; r < rounds; r0 += per_round[r], r++) // round r: pod r of the first per_round[r] candidates
         for (uint64_t j = 0; j < per_round[r]; j++) {
             const uint64_t p = off[order[j]] + r;
-            h_rc[at + j] = pods->req_cpu[p];
-            h_rm[at + j] = pods->req_mem[p];
-            memcpy(h_sel + (at + j) * W, pods->sel + p * W, 8 * W);
+            h_rc[r0 + j] = pods->req_cpu[p];
+            h_rm[r0 + j] = pods->req_mem[p];
+            memcpy(h_sel + (r0 + j) * W, pods->sel + p * W, 8 * W);
         }
     if (excl) {
-        uint32_t* h_excl = reinterpret_cast<uint32_t*>(h_in + o_excl);
+        uint32_t* h_excl = at<uint32_t>(h_in, i_excl);
         memset(h_excl, 0, (size_t)s->Npad / 8);
         for (uint64_t d = 0; d < D; d++) h_excl[cand->node_idx[d] >> 5] |= 1u << (cand->node_idx[d] & 31);
     }
-    // node-chunk partials: the largest round needs the most
-    uint64_t part_rows = 0;
-    for (uint32_t r = 0; r < rounds; r++)
-        part_rows = std::max<uint64_t>(part_rows, (uint64_t)direct_grid(W, per_round[r], s->Npad, s->sms).n_chunks * per_round[r]);
-    // work = [ov_fc P | ov_fm P | part keys | ov_node P | part indices | ov_cnt D | failed D]
-    const size_t w_fm = P * 8, w_key = 2 * P * 8, w_node = w_key + part_rows * 8, w_idx = w_node + P * 4,
-                 w_cnt = w_idx + part_rows * 4, w_failed = w_cnt + D * 4, work_bytes = w_failed + D * 4;
-    CU_TRY(s->dr_in.ensure(in_bytes));
-    CU_TRY(s->dr_work.ensure(work_bytes));
-    CU_TRY(s->dr_out.ensure(out_bytes));
     cudaStream_t st = s->stream;
-    uint8_t* d_in = s->dr_in.as<uint8_t>();
-    uint8_t* d_work = s->dr_work.as<uint8_t>();
-    uint8_t* d_out = s->dr_out.as<uint8_t>();
-    CU_TRY(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, st));
-    CU_TRY(cudaMemsetAsync(d_out, 0, out_bytes, st));
+    uint8_t* d_in = s->d_in.as<uint8_t>();
+    uint8_t* d_work = s->d_work.as<uint8_t>();
+    uint8_t* d_out = s->d_out.as<uint8_t>();
+    CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
+    CU_TRY(cudaMemsetAsync(d_out, 0, out.size, st));
     CU_TRY(cudaMemsetAsync(d_out + o_idx, 0xff, P * 4, st));
     CU_TRY(cudaMemsetAsync(d_work + w_cnt, 0, D * 8, st));
     DrainArgs da;
-    da.cand_node = reinterpret_cast<const int32_t*>(d_in + o_node);
-    da.pod_base = reinterpret_cast<const uint32_t*>(d_in + o_base);
-    da.cand_id = reinterpret_cast<const uint32_t*>(d_in + o_id);
-    da.excl = excl ? reinterpret_cast<const uint32_t*>(d_in + o_excl) : nullptr;
-    da.ov_cnt = reinterpret_cast<uint32_t*>(d_work + w_cnt);
-    da.failed = reinterpret_cast<uint32_t*>(d_work + w_failed);
-    da.ov_node = reinterpret_cast<int32_t*>(d_work + w_node);
-    da.ov_fc = reinterpret_cast<int64_t*>(d_work);
-    da.ov_fm = reinterpret_cast<int64_t*>(d_work + w_fm);
-    da.out_idx = reinterpret_cast<int32_t*>(d_out + o_idx);
-    da.out_score = reinterpret_cast<int64_t*>(d_out);
-    da.placed = reinterpret_cast<uint32_t*>(d_out + o_placed);
-    const PartialView part{reinterpret_cast<int64_t*>(d_work + w_key), reinterpret_cast<int32_t*>(d_work + w_idx), nullptr};
+    da.cand_node = at<int32_t>(d_in, i_node);
+    da.pod_base = at<uint32_t>(d_in, i_base);
+    da.cand_id = at<uint32_t>(d_in, i_id);
+    da.excl = excl ? at<uint32_t>(d_in, i_excl) : nullptr;
+    da.ov_cnt = at<uint32_t>(d_work, w_cnt);
+    da.failed = da.ov_cnt + D;
+    da.ov_node = at<int32_t>(d_work, w_node);
+    da.ov_fc = at<int64_t>(d_work, w_fc);
+    da.ov_fm = at<int64_t>(d_work, w_fm);
+    da.out_idx = at<int32_t>(d_out, o_idx);
+    da.out_score = at<int64_t>(d_out, o_score);
+    da.placed = at<uint32_t>(d_out, o_placed);
+    const PartialView part{at<int64_t>(d_work, w_key), at<int32_t>(d_work, w_idx), nullptr};
     const NodeTable nt = node_table(s);
-    for (uint64_t r = 0, at = 0; r < rounds; at += per_round[r], r++) {
-        const PodView pv{reinterpret_cast<const int64_t*>(d_in) + at, reinterpret_cast<const int64_t*>(d_in + o_rm) + at,
-                         reinterpret_cast<const uint64_t*>(d_in + o_sel) + at * W, per_round[r]};
+    for (uint64_t r = 0, r0 = 0; r < rounds; r0 += per_round[r], r++) {
+        const PodView pv{at<int64_t>(d_in, i_rc) + r0, at<int64_t>(d_in, i_rm) + r0, at<uint64_t>(d_in, i_sel) + r0 * W,
+                         per_round[r]};
         const DirectGrid g = direct_grid(W, per_round[r], s->Npad, s->sms);
         cudaError_t e = launch_drain_round(nt, pv, da, policy, (uint32_t)r, part, g, st);
         if (e != cudaSuccess) return fail(KS_ERR_CUDA, "drain round %llu launch failed: %s", (unsigned long long)r, cudaGetErrorString(e));
     }
-    CU_TRY(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(h_out, d_out, out.size, cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));
     if (P) memcpy(out_node_idx, h_out + o_idx, P * 4);
-    if (out_score && P) memcpy(out_score, h_out, P * 8);
+    if (out_score && P) memcpy(out_score, h_out + o_score, P * 8);
     memcpy(out_placed, h_out + o_placed, D * 4);
     s->last_path = "drain";
     return KS_OK;
@@ -1487,61 +1479,54 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const ks_node_templ
     }
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
-    // one pinned block each way: in = [rc P | rm P | alloc_cpu T | alloc_mem T | free_cpu T | free_mem T | sel P*W |
-    // labels T*W | max_nodes T], out = [rows T | reasons P (when asked) | node T*P (when asked)]
-    const size_t o_rm = P * 8, o_ac = 2 * P * 8, o_am = o_ac + T * 8, o_fc = o_am + T * 8, o_fm = o_fc + T * 8,
-                 o_sel = o_fm + T * 8, o_lab = o_sel + P * 8 * W, o_max = o_lab + T * 8 * W, in_bytes = o_max + T * 4;
-    const size_t o_why = T * sizeof(ks_scaleup_option), o_node = o_why + (out_reasons ? P * sizeof(ks_pod_reasons) : 0),
-                 out_bytes = o_node + (out_node ? T * P * 4 : 0);
-    const size_t h_out_at = (in_bytes + 15) & ~(size_t)15, h_bytes = h_out_at + out_bytes; // out block 16-byte aligned
-    if (s->h_scaleup_cap < h_bytes) {
-        if (s->h_scaleup) cudaFreeHost(s->h_scaleup);
-        s->h_scaleup = nullptr;
-        s->h_scaleup_cap = 0;
-        const size_t want = h_bytes + h_bytes / 8 + 256;
-        CU_TRY(cudaHostAlloc(&s->h_scaleup, want, cudaHostAllocDefault));
-        s->h_scaleup_cap = want;
-    }
-    uint8_t* h_in = static_cast<uint8_t*>(s->h_scaleup);
-    uint8_t* h_out = h_in + h_out_at;
-    memcpy(h_in, pods->req_cpu, P * 8);
-    memcpy(h_in + o_rm, pods->req_mem, P * 8);
-    memcpy(h_in + o_ac, t->alloc_cpu, T * 8);
-    memcpy(h_in + o_am, t->alloc_mem, T * 8);
-    memcpy(h_in + o_fc, t->free_cpu, T * 8);
-    memcpy(h_in + o_fm, t->free_mem, T * 8);
-    memcpy(h_in + o_sel, pods->sel, P * 8 * W);
-    memcpy(h_in + o_lab, t->labels, T * 8 * W);
-    memcpy(h_in + o_max, t->max_nodes, T * 4);
+    // one block each way: in = [rc P | rm P | alloc_cpu T | alloc_mem T | free_cpu T | free_mem T | sel P*W | labels T*W |
+    // max_nodes T], results = [rows T | reasons P (when asked) | node T*P (when asked)]
+    BlockLayout in, res;
+    const size_t i_rc = in.take<int64_t>(P), i_rm = in.take<int64_t>(P), i_ac = in.take<int64_t>(T),
+                 i_am = in.take<int64_t>(T), i_fc = in.take<int64_t>(T), i_fm = in.take<int64_t>(T),
+                 i_sel = in.take<uint64_t>(P * W), i_lab = in.take<uint64_t>(T * W), i_max = in.take<uint32_t>(T);
+    const size_t o_rows = res.take<ks_scaleup_option>(T),
+                 o_why = res.take<ks_pod_reasons>(out_reasons ? P : 0, 16), // k_scaleup_reasons stores uint4
+                 o_node = res.take<int32_t>(out_node ? T * P : 0);
+    uint8_t* h_out = nullptr;
+    rc = stage_blocks(s, in.size, res.size, &h_out);
+    if (rc) return rc;
     const uint32_t slots = scaleup_slots((uint32_t)T, s->sms);
-    CU_TRY(s->su_in.ensure(in_bytes));
-    CU_TRY(s->su_work.ensure((size_t)slots * 2 * P * 4));
-    CU_TRY(s->su_out.ensure(out_bytes));
+    CU_TRY(s->d_work.ensure((size_t)slots * 2 * P * 4));
+    uint8_t* h_in = s->h_stage.as<uint8_t>();
+    memcpy(h_in + i_rc, pods->req_cpu, P * 8);
+    memcpy(h_in + i_rm, pods->req_mem, P * 8);
+    memcpy(h_in + i_ac, t->alloc_cpu, T * 8);
+    memcpy(h_in + i_am, t->alloc_mem, T * 8);
+    memcpy(h_in + i_fc, t->free_cpu, T * 8);
+    memcpy(h_in + i_fm, t->free_mem, T * 8);
+    memcpy(h_in + i_sel, pods->sel, P * 8 * W);
+    memcpy(h_in + i_lab, t->labels, T * 8 * W);
+    memcpy(h_in + i_max, t->max_nodes, T * 4);
     cudaStream_t st = s->stream;
-    uint8_t* d_in = s->su_in.as<uint8_t>();
-    uint8_t* d_out = s->su_out.as<uint8_t>();
-    CU_TRY(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, st));
+    uint8_t* d_in = s->d_in.as<uint8_t>();
+    uint8_t* d_out = s->d_out.as<uint8_t>();
+    CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
     if (out_node) CU_TRY(cudaMemsetAsync(d_out + o_node, 0xff, T * P * 4, st));
-    const PodView pv{reinterpret_cast<const int64_t*>(d_in), reinterpret_cast<const int64_t*>(d_in + o_rm),
-                     reinterpret_cast<const uint64_t*>(d_in + o_sel), (uint32_t)P};
+    const PodView pv{at<int64_t>(d_in, i_rc), at<int64_t>(d_in, i_rm), at<uint64_t>(d_in, i_sel), (uint32_t)P};
     ScaleupArgs a;
     a.T = (uint32_t)T;
-    a.alloc_cpu = reinterpret_cast<const int64_t*>(d_in + o_ac);
-    a.alloc_mem = reinterpret_cast<const int64_t*>(d_in + o_am);
-    a.free_cpu = reinterpret_cast<const int64_t*>(d_in + o_fc);
-    a.free_mem = reinterpret_cast<const int64_t*>(d_in + o_fm);
-    a.labels = reinterpret_cast<const uint64_t*>(d_in + o_lab);
-    a.max_nodes = reinterpret_cast<const uint32_t*>(d_in + o_max);
-    a.rows = reinterpret_cast<ks_scaleup_option*>(d_out);
-    a.out_node = out_node ? reinterpret_cast<int32_t*>(d_out + o_node) : nullptr;
-    a.reasons = out_reasons ? reinterpret_cast<uint32_t*>(d_out + o_why) : nullptr;
-    a.scratch = s->su_work.as<uint32_t>();
+    a.alloc_cpu = at<int64_t>(d_in, i_ac);
+    a.alloc_mem = at<int64_t>(d_in, i_am);
+    a.free_cpu = at<int64_t>(d_in, i_fc);
+    a.free_mem = at<int64_t>(d_in, i_fm);
+    a.labels = at<uint64_t>(d_in, i_lab);
+    a.max_nodes = at<uint32_t>(d_in, i_max);
+    a.rows = at<ks_scaleup_option>(d_out, o_rows);
+    a.out_node = out_node ? at<int32_t>(d_out, o_node) : nullptr;
+    a.reasons = out_reasons ? at<uint32_t>(d_out, o_why) : nullptr;
+    a.scratch = s->d_work.as<uint32_t>();
     a.slots = slots;
     cudaError_t e = launch_scaleup(pv, W, a, st);
     if (e != cudaSuccess) return fail(KS_ERR_CUDA, "scale-up launch failed: %s", cudaGetErrorString(e));
-    CU_TRY(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(h_out, d_out, res.size, cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));
-    memcpy(out, h_out, T * sizeof(ks_scaleup_option));
+    memcpy(out, h_out + o_rows, T * sizeof(ks_scaleup_option));
     if (out_reasons) memcpy(out_reasons, h_out + o_why, P * sizeof(ks_pod_reasons));
     if (out_node) memcpy(out_node, h_out + o_node, T * P * 4);
     // the best template: most pods placed, then the highest utilization, then the fewest nodes, then the lowest index

@@ -1090,30 +1090,25 @@ struct VictimLayout {
 };
 static VictimLayout victim_layout(uint64_t B, uint32_t N) {
     VictimLayout L;
-    size_t o = 0;
-    auto take = [&o](size_t bytes) {
-        const size_t at = o;
-        o += (bytes + 255) & ~(size_t)255;
-        return at;
-    };
+    BlockLayout b; // every array 256-byte aligned
     L.nblk = (uint32_t)((B + RADIX_TILE - 1) / RADIX_TILE);
-    L.node = take(B * 4);
-    L.cpu = take(B * 8);
-    L.mem = take(B * 8);
-    L.prio = take(B * 4);
-    L.key[0] = take(B * 8);
-    L.key[1] = take(B * 8);
-    L.val[0] = take(B * 4);
-    L.val[1] = take(B * 4);
-    L.hist = take((size_t)256 * L.nblk * 4);
-    L.s_prio = take(B * 4);
-    L.s_cpu = take(B * 8);
-    L.s_mem = take(B * 8);
-    L.pre_cpu = take(B * 8);
-    L.pre_mem = take(B * 8);
-    L.off = take(((size_t)N + 1) * 4);
-    L.min_prio = take((size_t)N * 4);
-    L.total = o;
+    L.node = b.take<int32_t>(B, 256);
+    L.cpu = b.take<int64_t>(B, 256);
+    L.mem = b.take<int64_t>(B, 256);
+    L.prio = b.take<int32_t>(B, 256);
+    L.key[0] = b.take<uint64_t>(B, 256);
+    L.key[1] = b.take<uint64_t>(B, 256);
+    L.val[0] = b.take<uint32_t>(B, 256);
+    L.val[1] = b.take<uint32_t>(B, 256);
+    L.hist = b.take<uint32_t>((size_t)256 * L.nblk, 256);
+    L.s_prio = b.take<int32_t>(B, 256);
+    L.s_cpu = b.take<int64_t>(B, 256);
+    L.s_mem = b.take<int64_t>(B, 256);
+    L.pre_cpu = b.take<int64_t>(B, 256);
+    L.pre_mem = b.take<int64_t>(B, 256);
+    L.off = b.take<uint32_t>((size_t)N + 1, 256);
+    L.min_prio = b.take<int32_t>(N, 256);
+    L.total = b.size;
     return L;
 }
 
@@ -1121,29 +1116,26 @@ size_t victim_index_bytes(uint64_t B, uint32_t N) { return victim_layout(B, N).t
 
 BoundUpload victim_index_inputs(void* scratch, uint64_t B, uint32_t N) {
     const VictimLayout L = victim_layout(B, N);
-    unsigned char* s = static_cast<unsigned char*>(scratch);
-    return BoundUpload{reinterpret_cast<int32_t*>(s + L.node), reinterpret_cast<int64_t*>(s + L.cpu),
-                       reinterpret_cast<int64_t*>(s + L.mem), reinterpret_cast<int32_t*>(s + L.prio)};
+    return BoundUpload{at<int32_t>(scratch, L.node), at<int64_t>(scratch, L.cpu), at<int64_t>(scratch, L.mem),
+                       at<int32_t>(scratch, L.prio)};
 }
 
 cudaError_t build_victim_index(void* scratch, uint64_t B, uint32_t N, VictimIndex* vx, cudaStream_t st) {
     const VictimLayout L = victim_layout(B, N);
-    unsigned char* s = static_cast<unsigned char*>(scratch);
-    auto at = [s](size_t o) { return static_cast<void*>(s + o); };
-    uint64_t* key[2] = {static_cast<uint64_t*>(at(L.key[0])), static_cast<uint64_t*>(at(L.key[1]))};
-    uint32_t* val[2] = {static_cast<uint32_t*>(at(L.val[0])), static_cast<uint32_t*>(at(L.val[1]))};
+    void* s = scratch;
+    uint64_t* key[2] = {at<uint64_t>(s, L.key[0]), at<uint64_t>(s, L.key[1])};
+    uint32_t* val[2] = {at<uint32_t>(s, L.val[0]), at<uint32_t>(s, L.val[1])};
     int cur = 0;
     const uint32_t grid_b = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(4096, (B + 255) / 256));
     cudaError_t e;
     if (B) {
-        k_victim_keys<<<grid_b, 256, 0, st>>>(static_cast<const int32_t*>(at(L.node)), static_cast<const int32_t*>(at(L.prio)),
-                                              key[0], val[0], B);
+        k_victim_keys<<<grid_b, 256, 0, st>>>(at<int32_t>(s, L.node), at<int32_t>(s, L.prio), key[0], val[0], B);
         g_launches++;
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
         // priority bits [0, 32), then as many node bits as N needs
         const uint32_t node_bits = N > 1 ? 32u - (uint32_t)__builtin_clz(N - 1) : 0u;
         for (uint32_t shift = 0; shift < 32 + node_bits; shift += 8) {
-            uint32_t* hist = static_cast<uint32_t*>(at(L.hist));
+            uint32_t* hist = at<uint32_t>(s, L.hist);
             k_radix_hist<<<L.nblk, 256, 0, st>>>(key[cur], B, shift, hist, L.nblk);
             k_radix_scan<<<1, 1024, 0, st>>>(hist, 256 * L.nblk);
             k_radix_scatter<<<L.nblk, 256, 0, st>>>(key[cur], val[cur], key[cur ^ 1], val[cur ^ 1], B, shift, hist, L.nblk);
@@ -1151,30 +1143,30 @@ cudaError_t build_victim_index(void* scratch, uint64_t B, uint32_t N, VictimInde
             if ((e = cudaGetLastError()) != cudaSuccess) return e;
             cur ^= 1;
         }
-        k_victim_gather<<<grid_b, 256, 0, st>>>(key[cur], val[cur], static_cast<const int64_t*>(at(L.cpu)),
-                                                static_cast<const int64_t*>(at(L.mem)), static_cast<int32_t*>(at(L.s_prio)),
-                                                static_cast<int64_t*>(at(L.s_cpu)), static_cast<int64_t*>(at(L.s_mem)), B);
+        k_victim_gather<<<grid_b, 256, 0, st>>>(key[cur], val[cur], at<int64_t>(s, L.cpu), at<int64_t>(s, L.mem),
+                                                at<int32_t>(s, L.s_prio), at<int64_t>(s, L.s_cpu),
+                                                at<int64_t>(s, L.s_mem), B);
         g_launches++;
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
-    k_victim_offsets<<<(N + 1 + 255) / 256, 256, 0, st>>>(key[cur], B, N, static_cast<uint32_t*>(at(L.off)));
+    k_victim_offsets<<<(N + 1 + 255) / 256, 256, 0, st>>>(key[cur], B, N, at<uint32_t>(s, L.off));
     g_launches++;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     if (N) {
-        k_victim_prefix<<<(N + 7) / 8, 256, 0, st>>>(
-            static_cast<const uint32_t*>(at(L.off)), static_cast<const int32_t*>(at(L.s_prio)),
-            static_cast<const int64_t*>(at(L.s_cpu)), static_cast<const int64_t*>(at(L.s_mem)),
-            static_cast<int64_t*>(at(L.pre_cpu)), static_cast<int64_t*>(at(L.pre_mem)), static_cast<int32_t*>(at(L.min_prio)), N);
+        k_victim_prefix<<<(N + 7) / 8, 256, 0, st>>>(at<uint32_t>(s, L.off), at<int32_t>(s, L.s_prio),
+                                                     at<int64_t>(s, L.s_cpu), at<int64_t>(s, L.s_mem),
+                                                     at<int64_t>(s, L.pre_cpu), at<int64_t>(s, L.pre_mem),
+                                                     at<int32_t>(s, L.min_prio), N);
         g_launches++;
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
-    vx->off = static_cast<const uint32_t*>(at(L.off));
-    vx->min_prio = static_cast<const int32_t*>(at(L.min_prio));
-    vx->prio = static_cast<const int32_t*>(at(L.s_prio));
-    vx->cpu = static_cast<const int64_t*>(at(L.s_cpu));
-    vx->mem = static_cast<const int64_t*>(at(L.s_mem));
-    vx->pre_cpu = static_cast<const int64_t*>(at(L.pre_cpu));
-    vx->pre_mem = static_cast<const int64_t*>(at(L.pre_mem));
+    vx->off = at<uint32_t>(s, L.off);
+    vx->min_prio = at<int32_t>(s, L.min_prio);
+    vx->prio = at<int32_t>(s, L.s_prio);
+    vx->cpu = at<int64_t>(s, L.s_cpu);
+    vx->mem = at<int64_t>(s, L.s_mem);
+    vx->pre_cpu = at<int64_t>(s, L.pre_cpu);
+    vx->pre_mem = at<int64_t>(s, L.pre_mem);
     vx->idx = val[cur];
     return cudaSuccess;
 }

@@ -230,6 +230,22 @@ __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gmem_sr
 }
 
 // ---- launch-side plumbing shared by the API and the kernel files ----
+// Arrays packed into one allocation in call order: take<T>(n) places n Ts at the next multiple of `align` and returns
+// their byte offset; size is the bytes used so far.
+struct BlockLayout {
+    size_t size = 0;
+    template <class T>
+    size_t take(size_t n, size_t align = alignof(T)) {
+        const size_t off = (size + align - 1) / align * align;
+        size = off + n * sizeof(T);
+        return off;
+    }
+};
+template <class T>
+T* at(void* base, size_t off) {
+    return reinterpret_cast<T*>(static_cast<unsigned char*>(base) + off);
+}
+
 struct SelectLaunch {
     NodeTable nt;
     PodView pv;
