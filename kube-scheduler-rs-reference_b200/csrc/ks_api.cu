@@ -36,46 +36,9 @@ static int fail(int code, const char* fmt, ...) {
                         __LINE__);                                                                     \
     } while (0)
 
-// Every reallocation of a device buffer bumps this counter; it is part of the CUDA-graph cache key of ks_select, so a
-// cached graph is never replayed after one of the buffers its nodes point to has moved (staging buffers grown by a
-// larger call, ks_check_cells / ks_select_sampling scratch, ...).
-static std::atomic<uint64_t> g_devbuf_epoch{0};
-
-// Grow-only buffer in device (DevBuf) or pinned host (HostBuf) memory: ensure() reallocates, dropping the contents, when a
-// call needs more than it holds.  Freed by its destructor, which must run with the owner's device current.
-template <bool Pinned>
-struct Buf {
-    void* p = nullptr;
-    size_t cap = 0;
-    Buf() = default;
-    Buf(const Buf&) = delete;
-    Buf& operator=(const Buf&) = delete;
-    ~Buf() { release(); }
-    void release() {
-        if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-    cudaError_t ensure(size_t bytes) {
-        if (bytes <= cap) return cudaSuccess;
-        release();
-        if (!Pinned) g_devbuf_epoch++; // a pinned block leaves the epoch alone: no captured graph points into one
-        size_t want = bytes + bytes / 8 + 256;
-        cudaError_t e = Pinned ? cudaHostAlloc(&p, want, cudaHostAllocDefault) : cudaMalloc(&p, want);
-        if (e == cudaSuccess) cap = want;
-        return e;
-    }
-    template <class T>
-    T* as() {
-        return static_cast<T*>(p);
-    }
-};
-using DevBuf = Buf<false>;
-using HostBuf = Buf<true>;
-
 struct ks_snapshot {
     int device = 0;
-    cudaStream_t stream = nullptr;
+    Stream stream;
     uint32_t N = 0, Npad = 0, W = 1;
     DevBuf alloc_cpu, alloc_mem, free_cpu, free_mem, prio, labels, flag;
     DevBuf st_rc, st_rm, st_sel, st_idx, st_score, st_cnt, st_mask, st_codes, st_bnode, st_bcpu, st_bmem;
@@ -91,16 +54,16 @@ struct ks_snapshot {
     HostBuf h_stage;
     DevBuf d_in, d_work, d_out;
     int sms = 0, coop = 0;
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    Event ev[4];
     // host-space calls are pipelined in pod chunks: chunk c+1 is copied in on copy_stream while chunk c computes
-    cudaStream_t copy_stream = nullptr;
-    cudaEvent_t ev_cfork = nullptr, ev_in[4] = {nullptr, nullptr, nullptr, nullptr};
+    Stream copy_stream;
+    Event ev_cfork, ev_in[4];
     bool timing_valid = false;
     bool derived_dirty = true; // prio + bit-parallel index must be rebuilt before the next select
     const char* last_path = "none";
     BitparIndex bp;
     // CUDA-graph replay of the launch sequence of an all-device ks_select (same arguments, same snapshot state)
-    cudaGraphExec_t graph_exec = nullptr;
+    GraphExec graph_exec;
     uint64_t graph_key[16] = {0};
     bool graph_valid = false;
     uint64_t graph_launches = 0; // kernels inside the cached graph
@@ -215,11 +178,11 @@ int ks_snapshot_create(int device, ks_snapshot** out) {
     s->device = device;
     s->sms = prop.multiProcessorCount;
     s->coop = prop.cooperativeLaunch;
-    cudaError_t e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
-    for (int i = 0; i < 4 && e == cudaSuccess; i++) e = cudaEventCreate(&s->ev[i]);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s->copy_stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev_cfork, cudaEventDisableTiming);
-    for (int i = 0; i < 4 && e == cudaSuccess; i++) e = cudaEventCreateWithFlags(&s->ev_in[i], cudaEventDisableTiming);
+    cudaError_t e = cudaStreamCreateWithFlags(&s->stream.h, cudaStreamNonBlocking);
+    for (int i = 0; i < 4 && e == cudaSuccess; i++) e = cudaEventCreate(&s->ev[i].h);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s->copy_stream.h, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev_cfork.h, cudaEventDisableTiming);
+    for (int i = 0; i < 4 && e == cudaSuccess; i++) e = cudaEventCreateWithFlags(&s->ev_in[i].h, cudaEventDisableTiming);
     if (e == cudaSuccess) e = s->flag.ensure(sizeof(int));
     if (e == cudaSuccess) e = s->xflag.ensure(sizeof(int));
     if (e == cudaSuccess) e = cudaMemset(s->xflag.p, 0, sizeof(int));
@@ -236,16 +199,7 @@ void ks_snapshot_destroy(ks_snapshot* s) {
     if (!s) return;
     cudaSetDevice(s->device);
     if (s->stream) cudaStreamSynchronize(s->stream);
-    bitpar_release(s->bp);
-    if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
-    for (int i = 0; i < 4; i++)
-        if (s->ev[i]) cudaEventDestroy(s->ev[i]);
-    for (int i = 0; i < 4; i++)
-        if (s->ev_in[i]) cudaEventDestroy(s->ev_in[i]);
-    if (s->ev_cfork) cudaEventDestroy(s->ev_cfork);
-    if (s->copy_stream) cudaStreamDestroy(s->copy_stream);
-    if (s->stream) cudaStreamDestroy(s->stream);
-    delete s; // frees the buffers: the device is set and the stream synchronised
+    delete s; // frees the buffers and destroys the handles: the device is set and the stream synchronised
 }
 
 uint32_t ks_snapshot_num_nodes(const ks_snapshot* s) { return s ? s->N : 0; }
@@ -672,7 +626,7 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
             L.host_score = out_host ? out->score : nullptr;
             L.ready_event = out_host ? nullptr : (cudaEvent_t)out->bindings_ready_event;
             if (use_bitpar) {
-                cudaError_t e = bitpar_select(s->bp, L, timing ? s->ev[1] : nullptr, timing ? s->ev[2] : nullptr);
+                cudaError_t e = bitpar_select(s->bp, L, timing ? s->ev[1].h : nullptr, timing ? s->ev[2].h : nullptr);
                 if (e != cudaSuccess) return fail(KS_ERR_CUDA, "bit-parallel select failed: %s", cudaGetErrorString(e));
             } else {
                 if (timing) CU_TRY(cudaEventRecord(s->ev[1], st));
@@ -708,7 +662,7 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
                                   (uint64_t)policy | ((uint64_t)pods->mem_space << 8) | ((uint64_t)out->mem_space << 9) |
                                       ((uint64_t)out->mask_space << 10),
                                   (uint64_t)flags ^ ((uint64_t)out->bindings_ready_event << 8) ^ ((uint64_t)(xc ? xc->local_state : nullptr) << 20), (uint64_t)st, s->version, (uint64_t)use_bitpar,
-                                  g_devbuf_epoch.load(), s->bp.epoch};
+                                  g_devbuf_epoch.load()};
         const bool key_hit = s->graph_valid && memcmp(key, s->graph_key, sizeof(key)) == 0;
         bool graph_ok = !timing && !(flags & KS_SELECT_NO_GRAPH);
         if (graph_ok && !key_hit) {
@@ -720,23 +674,18 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
         }
         if (graph_ok) {
             if (!key_hit) {
-                if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
-                s->graph_exec = nullptr;
+                s->graph_exec.reset();
                 s->graph_valid = false;
                 CU_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
                 const uint64_t launches_before = g_launches.load();
                 const int erc = enqueue();
                 s->graph_launches = g_launches.load() - launches_before; // captured, not executed yet
                 g_launches -= s->graph_launches;
-                cudaGraph_t graph = nullptr;
-                cudaError_t e = cudaStreamEndCapture(st, &graph);
-                if (erc) {
-                    if (graph) cudaGraphDestroy(graph);
-                    return erc;
-                }
+                Graph graph;
+                cudaError_t e = cudaStreamEndCapture(st, &graph.h);
+                if (erc) return erc;
                 if (e != cudaSuccess) return fail(KS_ERR_CUDA, "stream capture failed: %s", cudaGetErrorString(e));
-                e = cudaGraphInstantiate(&s->graph_exec, graph, 0);
-                cudaGraphDestroy(graph);
+                e = cudaGraphInstantiate(&s->graph_exec.h, graph, 0);
                 if (e != cudaSuccess) return fail(KS_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
                 memcpy(s->graph_key, key, sizeof(key));
                 s->graph_valid = true;
@@ -835,9 +784,9 @@ int ks_measure_write_bandwidth(int device, void* dev_buf, uint64_t bytes, int it
     CU_TRY(cudaSetDevice(device));
     int sms = 0;
     CU_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-    cudaEvent_t e0, e1;
-    CU_TRY(cudaEventCreate(&e0));
-    CU_TRY(cudaEventCreate(&e1));
+    Event e0, e1;
+    CU_TRY(cudaEventCreate(&e0.h));
+    CU_TRY(cudaEventCreate(&e1.h));
     float best = 1e30f;
     for (int it = 0; it < std::max(2, iters); it++) { // first pass untimed
         CU_TRY(cudaEventRecord(e0, nullptr));
@@ -848,8 +797,6 @@ int ks_measure_write_bandwidth(int device, void* dev_buf, uint64_t bytes, int it
         CU_TRY(cudaEventElapsedTime(&ms, e0, e1));
         if (it > 0) best = std::min(best, ms);
     }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
     *out_gbs = (double)(bytes / 32 * 32) / (best * 1e-3) / 1e9;
     return KS_OK;
 }

@@ -1293,31 +1293,11 @@ static bool make_layout_flat(uint32_t N, uint32_t W, BitparLayout* lay) {
     return lay->nt > 0 && fill_offsets(lay, W);
 }
 
-static std::atomic<uint64_t> g_regrow_epoch{0}; // any reallocation invalidates cached CUDA graphs (BitparIndex::epoch)
-template <class T>
-static cudaError_t regrow(T*& p, size_t count) {
-    if (p) cudaFree(p);
-    p = nullptr;
-    g_regrow_epoch++;
-    return cudaMalloc(reinterpret_cast<void**>(&p), count * sizeof(T));
-}
-
-void bitpar_release(BitparIndex& ix) {
-    void* ptrs[] = {ix.sortedC, ix.sortedM, ix.gposC, ix.gposM, ix.ord_prio,
-                    ix.ord_idx, ix.splC,  ix.splM,  ix.blobP,    ix.pod_ranks, ix.tail_list,
-                    ix.rk_hist, ix.rk_spl_v, ix.rk_spl_i, ix.rk_bkt, ix.rk_loc, ix.rk_perm, ix.rec_s,
-                    ix.blobR,   ix.rank,   ix.tile_sorted, ix.ordL_s0, ix.ordL_idx, ix.evalL, ix.hintL, ix.blobL, ix.live, ix.cursor};
-    for (void* p : ptrs)
-        if (p) cudaFree(p);
-    if (ix.trace) {
+BitparIndex::~BitparIndex() {
+    if (trace.p) {
         unsigned long long* none = nullptr;
         cudaMemcpyToSymbol(c_trace, &none, sizeof(none));
-        cudaFree(ix.trace);
     }
-    if (ix.aux) cudaStreamDestroy(ix.aux);
-    if (ix.ev_fork) cudaEventDestroy(ix.ev_fork);
-    if (ix.ev_join) cudaEventDestroy(ix.ev_join);
-    ix = BitparIndex();
 }
 
 cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cudaStream_t st) {
@@ -1328,101 +1308,85 @@ cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cu
     const uint32_t Nord = ((nt.N + BP_TILE - 1) / BP_TILE) * BP_TILE;
     ix.Nord = Nord;
     cudaError_t e;
-    if (Nord > ix.cap_nodes) {
-        const size_t cap = Nord + Nord / 8 + BP_TILE;
-        if ((e = regrow(ix.sortedC, cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.sortedM, cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.gposC, cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.gposM, cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.ord_prio, cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.ord_idx, cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.splC, RANK_SPLITTERS)) != cudaSuccess) return e;
-        if ((e = regrow(ix.splM, RANK_SPLITTERS)) != cudaSuccess) return e;
-        if ((e = regrow(ix.rk_bkt, N_ORDERS * cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.rk_loc, N_ORDERS * cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.rk_perm, N_ORDERS * cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.ordL_s0, cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.ordL_idx, cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.evalL, cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.hintL, cap)) != cudaSuccess) return e;
-        ix.cap_nodes = cap;
-    }
+    for (DevBuf* b : {&ix.sortedC, &ix.sortedM, &ix.ord_prio, &ix.ordL_s0})
+        if ((e = b->ensure((size_t)Nord * sizeof(int64_t))) != cudaSuccess) return e;
+    for (DevBuf* b : {&ix.gposC, &ix.gposM, &ix.ord_idx, &ix.ordL_idx})
+        if ((e = b->ensure((size_t)Nord * sizeof(uint32_t))) != cudaSuccess) return e;
+    if ((e = ix.evalL.ensure((size_t)Nord * sizeof(NodeEval))) != cudaSuccess) return e;
+    if ((e = ix.hintL.ensure((size_t)Nord * sizeof(float4))) != cudaSuccess) return e;
+    for (DevBuf* b : {&ix.splC, &ix.splM})
+        if ((e = b->ensure(RANK_SPLITTERS * sizeof(int64_t))) != cudaSuccess) return e;
+    // [order][node], strided by N
+    if ((e = ix.rk_bkt.ensure((size_t)N_ORDERS * nt.N * sizeof(uint8_t))) != cudaSuccess) return e;
+    for (DevBuf* b : {&ix.rk_loc, &ix.rk_perm})
+        if ((e = b->ensure((size_t)N_ORDERS * nt.N * sizeof(uint32_t))) != cudaSuccess) return e;
+    if ((e = ix.rk_hist.ensure(N_ORDERS * RANK_BUCKETS * sizeof(uint32_t))) != cudaSuccess) return e;
+    if ((e = ix.rk_spl_v.ensure(N_ORDERS * RANK_BUCKETS * sizeof(int64_t))) != cudaSuccess) return e;
+    if ((e = ix.rk_spl_i.ensure(N_ORDERS * RANK_BUCKETS * sizeof(uint32_t))) != cudaSuccess) return e;
     uint32_t stride = 1;
     while ((nt.N + stride - 1) / stride > (uint32_t)RANK_SPLITTERS) stride <<= 1;
     ix.spl_stride = stride;
     ix.n_spl = (nt.N + stride - 1) / stride;
-    if (!ix.rk_hist) {
-        if ((e = regrow(ix.rk_hist, N_ORDERS * RANK_BUCKETS)) != cudaSuccess) return e;
-        if ((e = regrow(ix.rk_spl_v, N_ORDERS * RANK_BUCKETS)) != cudaSuccess) return e;
-        if ((e = regrow(ix.rk_spl_i, N_ORDERS * RANK_BUCKETS)) != cudaSuccess) return e;
-    }
-    if (!ix.live) {
-        if ((e = regrow(ix.live, KS_MAX_LABEL_WORDS + 2)) != cudaSuccess) return e; // + max allocatable cpu, memory
-    }
-    if ((e = cudaMemsetAsync(ix.live, 0, (KS_MAX_LABEL_WORDS + 2) * 8, st)) != cudaSuccess) return e;
-    k_node_bound<<<(nt.N + 255) / 256, 256, 0, st>>>(nt, prio + nt.Npad, ix.live);
+    const size_t live_bytes = (KS_MAX_LABEL_WORDS + 2) * sizeof(unsigned long long); // + max allocatable cpu, memory
+    if ((e = ix.live.ensure(live_bytes)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(ix.live.p, 0, live_bytes, st)) != cudaSuccess) return e;
+    k_node_bound<<<(nt.N + 255) / 256, 256, 0, st>>>(nt, prio + nt.Npad, ix.live.as<unsigned long long>());
     g_launches++;
-    k_node_splitters<<<N_ORDERS, RANK_SAMPLES, 0, st>>>(nt, prio, ix.rk_spl_v, ix.rk_spl_i, ix.rk_hist);
-    k_node_bucket<<<(nt.N + 255) / 256, 256, 0, st>>>(nt, prio, ix.rk_spl_v, ix.rk_spl_i, ix.rk_hist, ix.rk_bkt, ix.rk_loc);
-    k_node_scatter<<<(nt.N + 255) / 256, 256, 0, st>>>(nt.N, ix.rk_hist, ix.rk_bkt, ix.rk_loc, ix.rk_perm);
-    k_node_rank<<<(Nord + 255) / 256, 256, 0, st>>>(nt, prio, ix.rk_hist, ix.rk_bkt, ix.rk_perm, ix.sortedC, ix.sortedM,
-                                                    ix.gposC, ix.gposM, ix.ord_prio, ix.ord_idx, Nord, ix.splC, ix.splM,
-                                                    stride, ix.ordL_s0, ix.ordL_idx);
+    k_node_splitters<<<N_ORDERS, RANK_SAMPLES, 0, st>>>(nt, prio, ix.rk_spl_v.as<int64_t>(), ix.rk_spl_i.as<uint32_t>(),
+                                                        ix.rk_hist.as<uint32_t>());
+    k_node_bucket<<<(nt.N + 255) / 256, 256, 0, st>>>(nt, prio, ix.rk_spl_v.as<int64_t>(), ix.rk_spl_i.as<uint32_t>(),
+                                                      ix.rk_hist.as<uint32_t>(), ix.rk_bkt.as<uint8_t>(),
+                                                      ix.rk_loc.as<uint32_t>());
+    k_node_scatter<<<(nt.N + 255) / 256, 256, 0, st>>>(nt.N, ix.rk_hist.as<uint32_t>(), ix.rk_bkt.as<uint8_t>(),
+                                                       ix.rk_loc.as<uint32_t>(), ix.rk_perm.as<uint32_t>());
+    k_node_rank<<<(Nord + 255) / 256, 256, 0, st>>>(
+        nt, prio, ix.rk_hist.as<uint32_t>(), ix.rk_bkt.as<uint8_t>(), ix.rk_perm.as<uint32_t>(), ix.sortedC.as<int64_t>(),
+        ix.sortedM.as<int64_t>(), ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(), ix.ord_prio.as<int64_t>(),
+        ix.ord_idx.as<int32_t>(), Nord, ix.splC.as<int64_t>(), ix.splM.as<int64_t>(), stride, ix.ordL_s0.as<int64_t>(),
+        ix.ordL_idx.as<int32_t>());
     g_launches += 4;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     BitparLayout lay{}, layP{};
     if (!make_layout_flat(nt.N, nt.W, &layP)) return cudaSuccess; // direct path only
-    if (layP.blob_bytes > ix.cap_blobP) {
-        const size_t cap = (size_t)layP.blob_bytes + layP.blob_bytes / 8;
-        if ((e = regrow(ix.blobP, cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.blobL, cap)) != cudaSuccess) return e;
-        ix.cap_blobP = cap;
-    }
+    for (DevBuf* b : {&ix.blobP, &ix.blobL})
+        if ((e = b->ensure(layP.blob_bytes)) != cudaSuccess) return e;
     {
         RowsLayout lr{};
         if (!make_layout_rows(nt.N, nt.W, &lr)) return cudaSuccess; // direct path only
         const size_t need = (size_t)lr.ncb * lr.cb_stride;
-        if (need > ix.cap_blobR) {
-            if ((e = regrow(ix.blobR, need + need / 8)) != cudaSuccess) return e;
-            ix.cap_blobR = need + need / 8;
-        }
+        if ((e = ix.blobR.ensure(need)) != cudaSuccess) return e;
         const size_t need_rank = (size_t)lr.ncb * lr.n_thr * 2 * (RW_TILES / 2); // u32 tile pairs
-        if (need_rank > ix.cap_rank) {
-            const size_t cap = need_rank + need_rank / 8;
-            if ((e = regrow(ix.rank, cap)) != cudaSuccess) return e;
-            ix.cap_rank = cap;
-        }
-        if (lr.ncb > ix.cap_cursor) { // one work cursor per column block (k_mask_rows)
-            if ((e = regrow(ix.cursor, ((size_t)lr.ncb + 64) * RW_CURSOR_STRIDE)) != cudaSuccess) return e;
-            ix.cap_cursor = (size_t)lr.ncb + 64;
-        }
+        if ((e = ix.rank.ensure(need_rank * sizeof(uint32_t))) != cudaSuccess) return e;
+        // one work cursor per column block (k_mask_rows)
+        if ((e = ix.cursor.ensure((size_t)lr.ncb * RW_CURSOR_STRIDE * sizeof(uint32_t))) != cudaSuccess) return e;
         const size_t need_ts = 2ull * lr.ncb * RW_TILES * BP_TILE;
-        if (need_ts > ix.cap_tsorted) {
-            if ((e = regrow(ix.tile_sorted, need_ts + need_ts / 8)) != cudaSuccess) return e;
-            ix.cap_tsorted = need_ts + need_ts / 8;
-        }
-        k_build_cbtile<<<lr.ncb * RW_TILES, 288, 0, st>>>(nt, ix.gposC, ix.gposM, ix.blobR, lr, ix.tile_sorted);
+        if ((e = ix.tile_sorted.ensure(need_ts * sizeof(uint32_t))) != cudaSuccess) return e;
+        k_build_cbtile<<<lr.ncb * RW_TILES, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(),
+                                                          ix.blobR.as<uint8_t>(), lr, ix.tile_sorted.as<uint32_t>());
         g_launches++;
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        k_build_ranks<<<dim3((lr.n_thr + 255) / 256, lr.ncb), 256, 0, st>>>(ix.tile_sorted, lr, ix.rank);
+        k_build_ranks<<<dim3((lr.n_thr + 255) / 256, lr.ncb), 256, 0, st>>>(ix.tile_sorted.as<uint32_t>(), lr,
+                                                                             ix.rank.as<uint32_t>());
         g_launches++;
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
         ix.lay_r = lr;
         lay.nt = RW_TILES; // bitpar_profitable: (pod, tile) items
         lay.ncb = lr.ncb;
     }
-    k_build_tile<<<layP.nt, 288, 0, st>>>(nt, ix.gposC, ix.gposM, ix.ord_idx, ix.blobP, layP);
+    k_build_tile<<<layP.nt, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(), ix.ord_idx.as<int32_t>(),
+                                          ix.blobP.as<uint8_t>(), layP);
     g_launches++;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     // KS_SCORE_LEAST_ALLOCATED: the same flat index in descending order of the score bound + per-slot evaluation rows
-    k_build_tile<<<layP.nt, 288, 0, st>>>(nt, ix.gposC, ix.gposM, ix.ordL_idx, ix.blobL, layP);
-    k_build_eval<<<(Nord + 255) / 256, 256, 0, st>>>(nt, ix.ordL_idx, Nord, ix.evalL, ix.hintL);
+    k_build_tile<<<layP.nt, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(), ix.ordL_idx.as<int32_t>(),
+                                          ix.blobL.as<uint8_t>(), layP);
+    k_build_eval<<<(Nord + 255) / 256, 256, 0, st>>>(nt, ix.ordL_idx.as<int32_t>(), Nord, ix.evalL.as<NodeEval>(),
+                                                     ix.hintL.as<float4>());
     g_launches += 2;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     ix.lay = lay;
     ix.layP = layP;
     ix.valid = true;
-    ix.epoch = g_regrow_epoch.load();
     return cudaSuccess;
 }
 
@@ -1451,9 +1415,9 @@ cudaError_t bitpar_prepare(BitparIndex& ix, uint32_t P) {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&ix.sms, cudaDevAttrMultiProcessorCount, dev);
-        if ((e = cudaStreamCreateWithFlags(&ix.aux, cudaStreamNonBlocking)) != cudaSuccess) return e;
-        if ((e = cudaEventCreateWithFlags(&ix.ev_fork, cudaEventDisableTiming)) != cudaSuccess) return e;
-        if ((e = cudaEventCreateWithFlags(&ix.ev_join, cudaEventDisableTiming)) != cudaSuccess) return e;
+        if ((e = cudaStreamCreateWithFlags(&ix.aux.h, cudaStreamNonBlocking)) != cudaSuccess) return e;
+        if ((e = cudaEventCreateWithFlags(&ix.ev_fork.h, cudaEventDisableTiming)) != cudaSuccess) return e;
+        if ((e = cudaEventCreateWithFlags(&ix.ev_join.h, cudaEventDisableTiming)) != cudaSuccess) return e;
         if ((e = set_smem_attr<1>()) != cudaSuccess) return e;
         if ((e = set_smem_attr<2>()) != cudaSuccess) return e;
         if ((e = set_smem_attr<4>()) != cudaSuccess) return e;
@@ -1463,19 +1427,14 @@ cudaError_t bitpar_prepare(BitparIndex& ix, uint32_t P) {
             return e;
         const char* tr = getenv("KS_TRACE");
         if (tr && tr[0] == '1') { // one trace buffer per device: the most recently prepared index owns the stamps
-            if ((e = cudaMalloc(&ix.trace, BP_TRACE_WORDS * sizeof(unsigned long long))) != cudaSuccess) return e;
-            if ((e = cudaMemset(ix.trace, 0, BP_TRACE_WORDS * sizeof(unsigned long long))) != cudaSuccess) return e;
-            if ((e = cudaMemcpyToSymbol(c_trace, &ix.trace, sizeof(ix.trace))) != cudaSuccess) return e;
+            if ((e = ix.trace.ensure(BP_TRACE_WORDS * sizeof(unsigned long long))) != cudaSuccess) return e;
+            if ((e = cudaMemset(ix.trace.p, 0, BP_TRACE_WORDS * sizeof(unsigned long long))) != cudaSuccess) return e;
+            if ((e = cudaMemcpyToSymbol(c_trace, &ix.trace.p, sizeof(ix.trace.p))) != cudaSuccess) return e;
         }
     }
-    if (P > ix.cap_pods) {
-        const size_t cap = (size_t)P + P / 8 + 64;
-        if ((e = regrow(ix.pod_ranks, cap)) != cudaSuccess) return e;
-        if ((e = regrow(ix.tail_list, cap + 1)) != cudaSuccess) return e; // [cap] = the list length counter
-        if ((e = regrow(ix.rec_s, cap + 8)) != cudaSuccess) return e;
-        ix.cap_pods = cap;
-    }
-    ix.epoch = g_regrow_epoch.load();
+    if ((e = ix.pod_ranks.ensure((size_t)P * sizeof(uint2))) != cudaSuccess) return e;
+    if ((e = ix.tail_list.ensure(((size_t)P + 1) * sizeof(uint32_t))) != cudaSuccess) return e;
+    if ((e = ix.rec_s.ensure((((size_t)P + 7) & ~(size_t)7) * sizeof(uint4))) != cudaSuccess) return e;
     return cudaSuccess;
 }
 
@@ -1487,8 +1446,8 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
     if ((e = bitpar_prepare(ix, P)) != cudaSuccess) return e; // no-op when the caller prepared already
     const bool need_mask_pass = L.ov.mask || L.ov.cnt;
     const int sms = ix.sms;
-    if (ix.trace)
-        if ((e = cudaMemsetAsync(ix.trace, 0, BP_TRACE_WORDS * sizeof(unsigned long long), L.stream)) != cudaSuccess) return e;
+    if (ix.trace.p)
+        if ((e = cudaMemsetAsync(ix.trace.p, 0, BP_TRACE_WORDS * sizeof(unsigned long long), L.stream)) != cudaSuccess) return e;
     // one 1024-thread CTA per SM (splitters in dynamic shared memory); two pods per thread and pass once P > #SMs * 1024
     const uint32_t rank_grid = (uint32_t)std::min<uint64_t>((uint64_t)sms, ((uint64_t)P + RANK_THREADS - 1) / RANK_THREADS);
     const size_t rank_smem = (size_t)ix.n_spl * 2 * sizeof(int64_t);
@@ -1515,9 +1474,11 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
     const uint64_t F = (uint64_t)n_groups * ix.lay_r.ncb;
     const uint32_t warps = (uint32_t)threads / 32;
     const uint32_t mask_grid = (uint32_t)std::min<uint64_t>((uint64_t)mask_sms, (F + warps - 1) / warps);
-    k_pod_ranks<<<rank_grid, RANK_THREADS, rank_smem, L.stream>>>(L.pv, ix.sortedC, ix.sortedM, ix.N, ix.splC, ix.splM, ix.n_spl, ix.spl_stride,
-                                                 ix.pod_ranks, (need_mask_pass && ix.lay.ncb > 1) ? L.ov.cnt : nullptr, ix.W,
-                                                 need_mask_pass ? ix.rec_s : nullptr, ix.cursor, need_mask_pass ? ix.lay_r.ncb : 0u);
+    k_pod_ranks<<<rank_grid, RANK_THREADS, rank_smem, L.stream>>>(L.pv, ix.sortedC.as<int64_t>(), ix.sortedM.as<int64_t>(), ix.N,
+                                                 ix.splC.as<int64_t>(), ix.splM.as<int64_t>(), ix.n_spl, ix.spl_stride,
+                                                 ix.pod_ranks.as<uint2>(), (need_mask_pass && ix.lay.ncb > 1) ? L.ov.cnt : nullptr, ix.W,
+                                                 need_mask_pass ? ix.rec_s.as<uint4>() : nullptr, ix.cursor.as<uint32_t>(),
+                                                 need_mask_pass ? ix.lay_r.ncb : 0u);
     g_launches++;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     // argmax scan (needs only the pod ranks) on an auxiliary stream, forked here.  In timing mode it is enqueued on the main
@@ -1527,24 +1488,29 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
         if ((e = cudaStreamWaitEvent(ix.aux, ix.ev_fork, 0)) != cudaSuccess) return e;
     }
     auto enqueue_bind = [&](cudaStream_t bs) -> cudaError_t {
-        uint32_t* tail_count = ix.tail_list + ix.cap_pods;
+        uint32_t* tail_list = ix.tail_list.as<uint32_t>();
+        uint32_t* tail_count = tail_list + P; // the list holds at most P pods
         if ((e = cudaMemsetAsync(tail_count, 0, sizeof(uint32_t), bs)) != cudaSuccess) return e;
         if (L.policy == KS_SCORE_LEAST_ALLOCATED) {
             const uint32_t wpc = at / 32; // one warp per pod
             const uint32_t grid = (uint32_t)std::min<uint64_t>((uint64_t)sms * (2048 / at), ((uint64_t)P + wpc - 1) / wpc);
-            k_least_alloc<W><<<grid, at, 0, bs>>>(ix.blobL, ix.layP, ix.evalL, ix.hintL, ix.ordL_s0, ix.ordL_idx, L.pv, ix.pod_ranks, L.ov, L.po, ix.live,
-                                                  ix.N);
+            k_least_alloc<W><<<grid, at, 0, bs>>>(ix.blobL.as<uint8_t>(), ix.layP, ix.evalL.as<NodeEval>(), ix.hintL.as<float4>(),
+                                                  ix.ordL_s0.as<int64_t>(), ix.ordL_idx.as<int32_t>(), L.pv, ix.pod_ranks.as<uint2>(),
+                                                  L.ov, L.po, ix.live.as<unsigned long long>(), ix.N);
             g_launches++;
             if ((e = cudaGetLastError()) != cudaSuccess) return e;
         } else {
             const bool has_tail = ix.layP.nt > FF_HEAD_TILES;
-            k_first_fit_head<W><<<(P + at - 1) / at, at, 0, bs>>>(ix.blobP, ix.layP, ix.ord_idx, ix.ord_prio, L.pv, ix.pod_ranks, L.ov,
-                                                                 ix.tail_list, tail_count, L.po, !has_tail, ix.live, ix.N);
+            k_first_fit_head<W><<<(P + at - 1) / at, at, 0, bs>>>(ix.blobP.as<uint8_t>(), ix.layP, ix.ord_idx.as<int32_t>(),
+                                                                 ix.ord_prio.as<int64_t>(), L.pv, ix.pod_ranks.as<uint2>(), L.ov,
+                                                                 tail_list, tail_count, L.po, !has_tail,
+                                                                 ix.live.as<unsigned long long>(), ix.N);
             g_launches++;
             if ((e = cudaGetLastError()) != cudaSuccess) return e;
             if (has_tail) {
-                k_first_fit_tail<W><<<sms * (512 / at), at, 0, bs>>>(ix.blobP, ix.layP, ix.ord_idx, ix.ord_prio, L.pv, ix.pod_ranks, L.ov,
-                                                             ix.tail_list, tail_count, L.po);
+                k_first_fit_tail<W><<<sms * (512 / at), at, 0, bs>>>(ix.blobP.as<uint8_t>(), ix.layP, ix.ord_idx.as<int32_t>(),
+                                                                     ix.ord_prio.as<int64_t>(), L.pv, ix.pod_ranks.as<uint2>(),
+                                                                     L.ov, tail_list, tail_count, L.po);
                 g_launches++;
                 if ((e = cudaGetLastError()) != cudaSuccess) return e;
             }
@@ -1574,16 +1540,16 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
         if (before_mask)
             if ((e = cudaEventRecord(before_mask, L.stream)) != cudaSuccess) return e;
         RowsParams prm;
-        prm.blob = ix.blobR;
+        prm.blob = ix.blobR.as<uint8_t>();
         prm.lay = ix.lay_r;
-        prm.rank = ix.rank;
-        prm.rec_s = ix.rec_s;
+        prm.rank = ix.rank.as<uint32_t>();
+        prm.rec_s = ix.rec_s.as<uint4>();
         prm.sel_s = reinterpret_cast<const unsigned long long*>(L.pv.sel); // pod order: the caller's selector words
         prm.n_groups = n_groups;
         prm.mask = L.ov.mask;
         prm.row_words = (uint32_t)L.ov.mask_row_words;
         prm.cnt = L.ov.cnt;
-        prm.cursor = ix.cursor;
+        prm.cursor = ix.cursor.as<uint32_t>();
         void (*kern)(RowsParams) = threads == 896 ? k_mask_rows<W, W <= 4, 896> : k_mask_rows<W, W <= 4, 960>;
         kern<<<mask_grid, threads, ix.lay_r.smem_bytes, L.stream>>>(prm);
         g_launches++;
@@ -1605,10 +1571,10 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
 }
 
 cudaError_t bitpar_read_trace(const BitparIndex& ix, unsigned long long out_ns[BP_TRACE_WORDS]) {
-    if (!ix.trace) return cudaErrorNotSupported;
+    if (!ix.trace.p) return cudaErrorNotSupported;
     cudaError_t e = cudaDeviceSynchronize();
     if (e != cudaSuccess) return e;
-    if ((e = cudaMemcpy(out_ns, ix.trace, BP_TRACE_WORDS * sizeof(unsigned long long), cudaMemcpyDeviceToHost)) != cudaSuccess) return e;
+    if ((e = cudaMemcpy(out_ns, ix.trace.p, BP_TRACE_WORDS * sizeof(unsigned long long), cudaMemcpyDeviceToHost)) != cudaSuccess) return e;
     if (out_ns[TR_MASK_FIRST_CTA_END_INV]) out_ns[TR_MASK_FIRST_CTA_END_INV] = ~out_ns[TR_MASK_FIRST_CTA_END_INV];
     return cudaSuccess;
 }

@@ -51,51 +51,48 @@ struct RowsLayout {
     uint32_t n_thr;      // thresholds per column block in the rank tables: N + 1
 };
 
-struct NodeEval;
-
+// The index of one snapshot.  Device arrays (element type in brackets) are grow-only buffers, read through .as<T>().
+// Owned by the snapshot and freed with it, with the snapshot's device current.
 struct BitparIndex {
-    // per-snapshot index (device)
-    int64_t* sortedC = nullptr;  // [N] free_cpu ascending
-    int64_t* sortedM = nullptr;  // [N] free_mem ascending
-    uint32_t* gposC = nullptr;   // [N] position of node n in sortedC (ties by node index)
-    uint32_t* gposM = nullptr;
-    int64_t* ord_prio = nullptr; // nodes in descending priority order (ties by node index), padded to a tile
-    int32_t* ord_idx = nullptr;
-    int64_t* splC = nullptr;     // every `spl_stride`-th element of sortedC / sortedM (<= RANK_SPLITTERS = 8192 splitters)
-    int64_t* splM = nullptr;
-    uint8_t* blobP = nullptr;    // one blob of layP.blob_bytes: priority order (tile k = priority ranks 256k..),
-                                 // read through L1/L2 by k_first_fit_bp
-    uint2* pod_ranks = nullptr;  // per-call scratch [P]
-    uint32_t* tail_list = nullptr; // per-call scratch [cap_pods + 1]: pods left for k_first_fit_tail, then the count
-    int64_t* ordL_s0 = nullptr;    // KS_SCORE_LEAST_ALLOCATED: score bound of every node in descending order (ties by index)
-    int32_t* ordL_idx = nullptr;
-    struct NodeEval* evalL = nullptr; // per slot of that order: what the exact score needs
-    float4* hintL = nullptr;          // per slot of that order: single-precision score model (pre-filter of k_least_alloc)
-    uint8_t* blobL = nullptr;      // flat index (layP) in that order
-    unsigned long long* live = nullptr; // [KS_MAX_LABEL_WORDS] label bits carried by at least one node
-    uint4* rec_s = nullptr;        // rows kernel: {threshold_cpu, threshold_mem, pod index, selector columns} per sorted pod
-    uint8_t* blobR = nullptr;      // rows kernel: lay_r.ncb column-block blobs
-    uint32_t* rank = nullptr;      // rows kernel: [cb][threshold g][resource][j] = nodes of tile j (low 16 bits) and tile j + 4
-                                   // (high 16 bits) at sorted positions < g
-    uint32_t* tile_sorted = nullptr; // build scratch: per tile, its nodes' global positions in ascending order
-    size_t cap_blobR = 0, cap_rank = 0, cap_tsorted = 0, cap_cursor = 0;
+    DevBuf sortedC;   // [int64 N] free_cpu ascending
+    DevBuf sortedM;   // [int64 N] free_mem ascending
+    DevBuf gposC;     // [uint32 N] position of node n in sortedC (ties by node index)
+    DevBuf gposM;
+    DevBuf ord_prio;  // [int64 Nord] nodes in descending priority order (ties by node index), padded to a tile
+    DevBuf ord_idx;   // [int32 Nord]
+    DevBuf splC;      // [int64] every `spl_stride`-th element of sortedC / sortedM (<= RANK_SPLITTERS = 8192 splitters)
+    DevBuf splM;
+    DevBuf blobP;     // one blob of layP.blob_bytes: priority order (tile k = priority ranks 256k..),
+                      // read through L1/L2 by k_first_fit_head / _tail
+    DevBuf pod_ranks; // [uint2 P] per-call scratch
+    DevBuf tail_list; // [uint32 P + 1] per-call scratch: pods left for k_first_fit_tail, then the count at word P
+    DevBuf ordL_s0;   // [int64 Nord] KS_SCORE_LEAST_ALLOCATED: score bound of every node in descending order (ties by index)
+    DevBuf ordL_idx;  // [int32 Nord]
+    DevBuf evalL;     // [NodeEval Nord] per slot of that order: what the exact score needs
+    DevBuf hintL;     // [float4 Nord] per slot of that order: single-precision score model (pre-filter of k_least_alloc)
+    DevBuf blobL;     // flat index (layP) in that order
+    DevBuf live;      // [uint64 KS_MAX_LABEL_WORDS + 2] label bits carried by at least one node, max allocatable cpu, memory
+    DevBuf rec_s;     // [uint4] rows kernel: {threshold_cpu, threshold_mem, pod index, selector columns} per pod, P rounded up to 8
+    DevBuf blobR;     // rows kernel: lay_r.ncb column-block blobs
+    DevBuf rank;      // [uint32] rows kernel: [cb][threshold g][resource][j] = nodes of tile j (low 16 bits) and tile j + 4
+                      // (high 16 bits) at sorted positions < g
+    DevBuf tile_sorted; // [uint32] build scratch: per tile, its nodes' global positions in ascending order
     RowsLayout lay_r{};
-    uint64_t epoch = 0;            // bumped whenever a device buffer of the index is reallocated (CUDA-graph cache key)
-    uint32_t* rk_hist = nullptr;   // node sample sort scratch: [3][256] bucket counts, splitters, per-node bucket / slot, lists
-    int64_t* rk_spl_v = nullptr;
-    uint32_t* rk_spl_i = nullptr;
-    uint8_t* rk_bkt = nullptr;
-    uint32_t* rk_loc = nullptr;
-    uint32_t* rk_perm = nullptr;
-    size_t cap_nodes = 0, cap_blobP = 0, cap_pods = 0;
+    DevBuf rk_hist;   // [uint32] node sample sort scratch: per order 256 bucket counts, splitters, per-node bucket / slot, lists
+    DevBuf rk_spl_v;
+    DevBuf rk_spl_i;
+    DevBuf rk_bkt;
+    DevBuf rk_loc;
+    DevBuf rk_perm;
     uint32_t N = 0, Nord = 0, W = 0, spl_stride = 1, n_spl = 0;
     BitparLayout lay{}, layP{};
     bool valid = false;
     int sms = 0;
-    cudaStream_t aux = nullptr; // the argmax kernels run here, overlapped with k_mask_rows
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-    uint32_t* cursor = nullptr; // [ncb] work cursors of the mask kernel (k_mask_rows), zeroed by k_pod_ranks
-    unsigned long long* trace = nullptr; // KS_TRACE=1: per-kernel %globaltimer stamps of the last select (ks_last_trace)
+    Stream aux; // the argmax kernels run here, overlapped with k_mask_rows
+    Event ev_fork, ev_join;
+    DevBuf cursor; // [uint32 ncb * RW_CURSOR_STRIDE] work cursors of the mask kernel (k_mask_rows), zeroed by k_pod_ranks
+    DevBuf trace;  // KS_TRACE=1: per-kernel %globaltimer stamps of the last select (ks_last_trace)
+    ~BitparIndex(); // detaches the kernels from a trace buffer this index owns
 };
 constexpr int BP_TRACE_WORDS = 16;
 
@@ -103,7 +100,6 @@ cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cu
 bool bitpar_profitable(const BitparIndex& ix, uint32_t P);
 cudaError_t bitpar_prepare(BitparIndex& ix, uint32_t P);
 cudaError_t bitpar_select(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before_mask, cudaEvent_t after_mask);
-void bitpar_release(BitparIndex& ix);
 // slots of ks_last_trace (include/ksched.h); cudaErrorNotSupported unless the index was created under KS_TRACE=1
 cudaError_t bitpar_read_trace(const BitparIndex& ix, unsigned long long out_ns[BP_TRACE_WORDS]);
 

@@ -19,6 +19,7 @@
 namespace ks {
 
 std::atomic<uint64_t> g_launches{0};
+std::atomic<uint64_t> g_devbuf_epoch{0};
 
 // ------------------------------------------------------------------------------------------------ K0
 __global__ void k_node_free_reduce(int64_t* __restrict__ free_cpu, int64_t* __restrict__ free_mem,

@@ -94,6 +94,10 @@ struct PartialView {
 };
 
 extern std::atomic<uint64_t> g_launches;
+// Every reallocation of a device buffer bumps this counter; it is part of the CUDA-graph cache key of ks_select, so a
+// cached graph is never replayed after one of the buffers its nodes point to has moved (staging buffers grown by a
+// larger call, ks_check_cells / ks_select_sampling scratch, the bit-parallel index, ...).
+extern std::atomic<uint64_t> g_devbuf_epoch;
 
 // ---- scores and the tie rule: one definition for every argmax path ----
 // KS_SCORE_LEFTOVER: score = (free_cpu - rc) * 2^22 + (free_mem - rm) = node key - pod key.  The node key alone orders
@@ -245,6 +249,58 @@ template <class T>
 T* at(void* base, size_t off) {
     return reinterpret_cast<T*>(static_cast<unsigned char*>(base) + off);
 }
+
+// Grow-only buffer in device (DevBuf) or pinned host (HostBuf) memory: ensure() reallocates, dropping the contents, when a
+// call needs more than it holds.  Freed by its destructor, which must run with the owner's device current.
+template <bool Pinned>
+struct Buf {
+    void* p = nullptr;
+    size_t cap = 0;
+    Buf() = default;
+    Buf(const Buf&) = delete;
+    Buf& operator=(const Buf&) = delete;
+    ~Buf() { release(); }
+    void release() {
+        if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
+        p = nullptr;
+        cap = 0;
+    }
+    cudaError_t ensure(size_t bytes) {
+        if (bytes <= cap) return cudaSuccess;
+        release();
+        if (!Pinned) g_devbuf_epoch++; // a pinned block leaves the epoch alone: no captured graph points into one
+        size_t want = bytes + bytes / 8 + 256;
+        cudaError_t e = Pinned ? cudaHostAlloc(&p, want, cudaHostAllocDefault) : cudaMalloc(&p, want);
+        if (e == cudaSuccess) cap = want;
+        return e;
+    }
+    template <class T>
+    T* as() const {
+        return static_cast<T*>(p);
+    }
+};
+using DevBuf = Buf<false>;
+using HostBuf = Buf<true>;
+
+// Owner of one CUDA stream, event, graph or graph exec: Destroy runs when the owner goes (with its device current) or
+// when reset() replaces the handle.  Created in place through &h; reads as the plain handle.
+template <class H, cudaError_t (*Destroy)(H)>
+struct Handle {
+    H h = nullptr;
+    Handle() = default;
+    Handle(const Handle&) = delete;
+    Handle& operator=(const Handle&) = delete;
+    ~Handle() { reset(); }
+    void reset() {
+        if (h) Destroy(h);
+        h = nullptr;
+    }
+    operator H() const { return h; }
+};
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+using Graph = Handle<cudaGraph_t, cudaGraphDestroy>;
+using GraphExec = Handle<cudaGraphExec_t, cudaGraphExecDestroy>;
 
 struct SelectLaunch {
     NodeTable nt;

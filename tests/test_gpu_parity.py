@@ -430,6 +430,7 @@ def test_graph_replay_tracks_snapshot_changes(ks, orc):
         snap.set_nodes(ac, am, lab)
         snap.set_bound(bn, bc, bm)
         mask = torch.zeros((cl.P, row), dtype=torch.uint8, device=dev)
+        big = 2 * cl.P  # doubled per pass, so that every pass grows the index's per-call pod scratch
         for space in (ks.KS_MEM_DEVICE, ks.KS_MEM_HOST):
             t, idx, score, cnt = buffers(space)
             st = torch.cuda.Stream()
@@ -462,6 +463,23 @@ def test_graph_replay_tracks_snapshot_changes(ks, orc):
             assert all(np.array_equal(a, b) for a, b in zip(g, o3[:3]))
             t[0].copy_(torch.from_numpy(rc))
             torch.cuda.synchronize()
+            # an uncached device-space select of more pods moves only the index's pod scratch (pod ranks, tail list,
+            # mask records): the cached graph points into the old buffers and must not be replayed
+            reps = big // cl.P
+            tb = [torch.from_numpy(np.ascontiguousarray(np.concatenate([a] * reps).view(np.int64))).to(dev)
+                  for a in (rc, rm, sel)]
+            ib = torch.empty(big, dtype=torch.int32, device=dev)
+            sb = torch.empty(big, dtype=torch.int64, device=dev)
+            cb = torch.empty(big, dtype=torch.int32, device=dev)
+            snap.select_raw(big, tb[0], tb[1], tb[2], ks.KS_MEM_DEVICE, ib, sb, cb, ks.KS_MEM_DEVICE,
+                            flags=ks.KS_SELECT_FORCE_BITPAR | ks.KS_SELECT_NO_GRAPH, stream=st.cuda_stream)
+            st.synchronize()
+            assert snap.last_path() == "bitpar"
+            gb = ib.cpu().numpy(), sb.cpu().numpy(), cb.cpu().numpy().view(np.uint32)
+            assert all(np.array_equal(a, np.tile(b, reps)) for a, b in zip(gb, o2[:3]))
+            big *= 2
+            g = run()
+            assert all(np.array_equal(a, b) for a, b in zip(g, o2[:3]))
 
 
 def test_bindings_ready_event_orders_a_side_stream(ks, orc):
