@@ -423,8 +423,9 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods /* host space */, const k
  * Host-space pods and outputs.  One H2D copy, two kernels (the per-pod reasons only when out_reasons is set), one D2H
  * copy; the best template is picked on the host.  With out_node the snapshot's pinned staging block and its device
  * result block each grow to n * pods->n * 4 bytes (1 GiB each at 4096 templates x 65536 pods) and are kept for reuse
- * until ks_snapshot_destroy.  ks_gang_bind, ks_drain_check and ks_stream_bind stage through the same blocks, so the
- * snapshot holds the largest any of these calls needed, not their sum.  Callers near the limits who want that memory
+ * until ks_snapshot_destroy.  ks_gang_bind, ks_drain_check and ks_stream_bind stage through the same blocks, and every
+ * call that returns only after its host-space results are back stages through the same device blocks, so the snapshot
+ * holds the largest any of these calls needed, not their sum.  Callers near the limits who want that memory
  * back can split the templates over calls or use a snapshot of their own for the estimate. */
 #define KS_SCALEUP_MAX_NODES 1024u
 #define KS_SCALEUP_MAX_PODS 65536u

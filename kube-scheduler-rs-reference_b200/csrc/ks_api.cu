@@ -40,19 +40,17 @@ struct ks_snapshot {
     int device = 0;
     Stream stream;
     uint32_t N = 0, Npad = 0, W = 1;
-    DevBuf alloc_cpu, alloc_mem, free_cpu, free_mem, prio, labels, flag;
-    DevBuf st_rc, st_rm, st_sel, st_idx, st_score, st_cnt, st_mask, st_codes, st_bnode, st_bcpu, st_bmem;
-    DevBuf part_key, part_idx, part_cnt, st_samp, xflag;
-    DevBuf st_reasons; // ks_explain with host-space output
-    DevBuf st_topk, part_topk; // ks_select_topk: host-space outputs, node-chunk partials
-    DevBuf st_pre, vx_pre, part_pre; // ks_preempt: host-space outputs and priorities, victim index, node-chunk partials
-    DevBuf sb_pkey, sb_pidx, sb_pend; // device-side streaming loop (k_stream_batch, k_gang_batch)
-    // Staging of the host-staged calls (ks_stream_bind's device loop, ks_gang_bind, ks_drain_check,
-    // ks_scaleup_estimate): a pinned block with the inputs at 0 and the results after them (stage_blocks), the device
-    // copies of both, and device work space.  One set serves all four because each of them holds mu from its first
-    // staging write to its final stream synchronise, so no two are ever live; the snapshot keeps the largest.
+    DevBuf alloc_cpu, alloc_mem, free_cpu, free_mem, prio, labels, flag, xflag;
+    // Staging shared by every call that holds mu until its final stream synchronise: no two are ever live, and the
+    // snapshot keeps the largest any of them needed.  d_in: host-space pods (stage_pods), bound and claim lists
+    // (stage_claims) and the host-staged calls' inputs; d_out: every host-space result, a host-space mask at 0; d_work:
+    // stream/gang, drain and scale-up scratch; h_stage: the host-staged calls' pinned block (stage_blocks).  A call
+    // ensures each buffer once, for its whole layout, before it takes a pointer: a growing ensure frees those taken.
     HostBuf h_stage;
     DevBuf d_in, d_work, d_out;
+    // Per call kind: an all-device select, top-k or preempt returns after enqueue and its kernels keep using these (as
+    // they do the node table, flag, xflag and bp), so sharing one would let calls on two caller streams race.
+    DevBuf part_sel, part_topk, part_pre, vx_pre; // node-chunk partials of select, top-k, preempt; preempt's victim index
     int sms = 0, coop = 0;
     Event ev[4];
     // host-space calls are pipelined in pod chunks: chunk c+1 is copied in on copy_stream while chunk c computes
@@ -97,6 +95,14 @@ static int check_range_and_prio(ks_snapshot* s, cudaStream_t st) {
     return KS_OK;
 }
 
+static bool valid_policy(int policy) { return policy == KS_SCORE_LEFTOVER || policy == KS_SCORE_LEAST_ALLOCATED; }
+static bool valid_space(int32_t space) { return space == KS_MEM_HOST || space == KS_MEM_DEVICE; }
+static bool valid_label_words(uint32_t W) { return W == 1 || W == 2 || W == 4 || W == 8; }
+// inside +-2^36 millicores / +-2^55 bytes, the range that keeps every score inside int64
+static bool within_limits(int64_t cpu, int64_t mem) {
+    return cpu >= -KS_MAX_CPU_MILLI && cpu <= KS_MAX_CPU_MILLI && mem >= -KS_MAX_MEM_BYTES && mem <= KS_MAX_MEM_BYTES;
+}
+
 // Requests that are committed against free[] (claims, stream and gang pods) must lie in [0, limit]: an accepted claim
 // then leaves its node's free in [0, free], so free[] stays inside the limits by construction.  Checked on the host
 // before any device work.  (A negative request would always fit and raise free[]; API validation rejects them upstream.)
@@ -121,12 +127,15 @@ static int stage_blocks(ks_snapshot* s, size_t in_bytes, size_t out_bytes, uint8
     return KS_OK;
 }
 
-// What k_stream_batch and k_gang_batch take from the snapshot: the node table, the policy, the sb_* scratch and the
-// grid.  The caller sets the pods, the outputs, ctl and max_rounds.
+// What k_stream_batch and k_gang_batch take from the snapshot: the node table, the policy, the grid and their scratch in
+// d_work, [pkey | pidx | pend] (the kernels rebuild the pending list on every call: nothing in it persists).  The caller
+// sets the pods, the outputs, ctl and max_rounds.
 static int stream_batch_args(ks_snapshot* s, int policy, StreamBatchArgs* a) {
-    CU_TRY(s->sb_pkey.ensure((size_t)STREAM_BATCH_MAX * s->sms * 8));
-    CU_TRY(s->sb_pidx.ensure((size_t)STREAM_BATCH_MAX * s->sms * 4));
-    CU_TRY(s->sb_pend.ensure(2 * STREAM_BATCH_MAX * 4));
+    BlockLayout w;
+    const size_t o_key = w.take<int64_t>((size_t)STREAM_BATCH_MAX * s->sms),
+                 o_idx = w.take<int32_t>((size_t)STREAM_BATCH_MAX * s->sms, 256),
+                 o_pend = w.take<uint32_t>(2 * STREAM_BATCH_MAX, 256);
+    CU_TRY(s->d_work.ensure(w.size));
     a->N = s->N;
     a->Npad = s->Npad;
     a->alloc_cpu = s->alloc_cpu.as<int64_t>();
@@ -135,10 +144,29 @@ static int stream_batch_args(ks_snapshot* s, int policy, StreamBatchArgs* a) {
     a->free_cpu = s->free_cpu.as<int64_t>();
     a->free_mem = s->free_mem.as<int64_t>();
     a->policy = policy;
-    a->pkey = s->sb_pkey.as<int64_t>();
-    a->pidx = s->sb_pidx.as<int32_t>();
-    a->pend = s->sb_pend.as<uint32_t>();
+    a->pkey = at<int64_t>(s->d_work.p, o_key);
+    a->pidx = at<int32_t>(s->d_work.p, o_idx);
+    a->pend = at<uint32_t>(s->d_work.p, o_pend);
     a->grid = std::max(1u, std::min<uint32_t>((uint32_t)s->sms, (s->N + 127u) / 128u));
+    return KS_OK;
+}
+
+// The host bound or claim list of set_bound, apply_bind and commit_claims, copied to d_in on the snapshot's stream as
+// [node | cpu | mem], each array at a multiple of 256 bytes.
+struct Claims {
+    const int32_t* node;
+    const int64_t* cpu;
+    const int64_t* mem;
+};
+static int stage_claims(ks_snapshot* s, uint64_t n, const int32_t* node, const int64_t* cpu, const int64_t* mem, Claims* c) {
+    BlockLayout L;
+    const size_t o_node = L.take<int32_t>(n), o_cpu = L.take<int64_t>(n, 256), o_mem = L.take<int64_t>(n, 256);
+    CU_TRY(s->d_in.ensure(L.size));
+    void* b = s->d_in.p;
+    CU_TRY(cudaMemcpyAsync(at<int32_t>(b, o_node), node, n * 4, cudaMemcpyHostToDevice, s->stream));
+    CU_TRY(cudaMemcpyAsync(at<int64_t>(b, o_cpu), cpu, n * 8, cudaMemcpyHostToDevice, s->stream));
+    CU_TRY(cudaMemcpyAsync(at<int64_t>(b, o_mem), mem, n * 8, cudaMemcpyHostToDevice, s->stream));
+    *c = Claims{at<int32_t>(b, o_node), at<int64_t>(b, o_cpu), at<int64_t>(b, o_mem)};
     return KS_OK;
 }
 
@@ -208,15 +236,13 @@ uint32_t ks_snapshot_label_words(const ks_snapshot* s) { return s ? s->W : 0; }
 int ks_snapshot_set_nodes(ks_snapshot* s, uint32_t n_nodes, uint32_t label_words, const int64_t* alloc_cpu,
                           const int64_t* alloc_mem, const uint64_t* labels) {
     if (!s) return fail(KS_ERR_INVALID, "snapshot is NULL");
-    if (label_words != 1 && label_words != 2 && label_words != 4 && label_words != 8)
+    if (!valid_label_words(label_words))
         return fail(KS_ERR_INVALID, "label_words must be 1, 2, 4 or 8 (got %u)", label_words);
     if (n_nodes && (!alloc_cpu || !alloc_mem || !labels)) return fail(KS_ERR_INVALID, "NULL node array");
     if (n_nodes > (1u << 30)) return fail(KS_ERR_RANGE, "n_nodes too large");
-    for (uint32_t n = 0; n < n_nodes; n++) {
-        if (alloc_cpu[n] > KS_MAX_CPU_MILLI || alloc_cpu[n] < -KS_MAX_CPU_MILLI || alloc_mem[n] > KS_MAX_MEM_BYTES ||
-            alloc_mem[n] < -KS_MAX_MEM_BYTES)
+    for (uint32_t n = 0; n < n_nodes; n++)
+        if (!within_limits(alloc_cpu[n], alloc_mem[n]))
             return fail(KS_ERR_RANGE, "node %u allocatable outside +-2^36 millicores / +-2^55 bytes", n);
-    }
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
     const uint32_t Npad = ((n_nodes + TILE_N - 1) / TILE_N) * TILE_N;
@@ -273,8 +299,7 @@ int ks_snapshot_set_bound(ks_snapshot* s, uint64_t n_bound, const int32_t* node_
         if (node_idx[b] < 0 || (uint32_t)node_idx[b] >= s->N)
             return fail(KS_ERR_INVALID, "bound pod %llu: node index %d out of range", (unsigned long long)b,
                         node_idx[b]);
-        if (req_cpu[b] > KS_MAX_CPU_MILLI || req_cpu[b] < -KS_MAX_CPU_MILLI || req_mem[b] > KS_MAX_MEM_BYTES ||
-            req_mem[b] < -KS_MAX_MEM_BYTES)
+        if (!within_limits(req_cpu[b], req_mem[b]))
             return fail(KS_ERR_RANGE, "bound pod %llu request out of range", (unsigned long long)b);
     }
     std::lock_guard<std::mutex> lk(s->mu);
@@ -285,14 +310,11 @@ int ks_snapshot_set_bound(ks_snapshot* s, uint64_t n_bound, const int32_t* node_
     int rc = reset_free_to_alloc(s);
     if (rc) return rc;
     if (n_bound) {
-        CU_TRY(s->st_bnode.ensure(n_bound * 4));
-        CU_TRY(s->st_bcpu.ensure(n_bound * 8));
-        CU_TRY(s->st_bmem.ensure(n_bound * 8));
-        CU_TRY(cudaMemcpyAsync(s->st_bnode.p, node_idx, n_bound * 4, cudaMemcpyHostToDevice, s->stream));
-        CU_TRY(cudaMemcpyAsync(s->st_bcpu.p, req_cpu, n_bound * 8, cudaMemcpyHostToDevice, s->stream));
-        CU_TRY(cudaMemcpyAsync(s->st_bmem.p, req_mem, n_bound * 8, cudaMemcpyHostToDevice, s->stream));
-        CU_TRY(launch_free_reduce(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), s->st_bnode.as<int32_t>(),
-                                  s->st_bcpu.as<int64_t>(), s->st_bmem.as<int64_t>(), n_bound, s->stream));
+        Claims c;
+        rc = stage_claims(s, n_bound, node_idx, req_cpu, req_mem, &c);
+        if (rc) return rc;
+        CU_TRY(launch_free_reduce(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), c.node, c.cpu, c.mem, n_bound,
+                                  s->stream));
     }
     return check_range_and_prio(s, s->stream);
 }
@@ -300,8 +322,7 @@ int ks_snapshot_set_bound(ks_snapshot* s, uint64_t n_bound, const int32_t* node_
 int ks_snapshot_apply_bind(ks_snapshot* s, int32_t node_idx, int64_t req_cpu, int64_t req_mem) {
     if (!s) return fail(KS_ERR_INVALID, "snapshot is NULL");
     if (node_idx < 0 || (uint32_t)node_idx >= s->N) return fail(KS_ERR_INVALID, "node index %d out of range", node_idx);
-    if (req_cpu > KS_MAX_CPU_MILLI || req_cpu < -KS_MAX_CPU_MILLI || req_mem > KS_MAX_MEM_BYTES || req_mem < -KS_MAX_MEM_BYTES)
-        return fail(KS_ERR_RANGE, "request out of range");
+    if (!within_limits(req_cpu, req_mem)) return fail(KS_ERR_RANGE, "request out of range");
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
     // free[] stays inside the limits: refuse a bind that would take the node's free outside them, before anything
@@ -311,19 +332,15 @@ int ks_snapshot_apply_bind(ks_snapshot* s, int32_t node_idx, int64_t req_cpu, in
     CU_TRY(cudaMemcpyAsync(&f[1], s->free_mem.as<int64_t>() + node_idx, 8, cudaMemcpyDeviceToHost, s->stream));
     CU_TRY(cudaStreamSynchronize(s->stream));
     const int64_t nc = f[0] - req_cpu, nm = f[1] - req_mem;
-    if (nc > KS_MAX_CPU_MILLI || nc < -KS_MAX_CPU_MILLI || nm > KS_MAX_MEM_BYTES || nm < -KS_MAX_MEM_BYTES)
+    if (!within_limits(nc, nm))
         return fail(KS_ERR_RANGE, "node %d: the bind would leave free at %lld millicores / %lld bytes, outside +-2^36 / +-2^55",
                     node_idx, (long long)nc, (long long)nm);
     s->derived_dirty = true;
     s->version++;
-    CU_TRY(s->st_bnode.ensure(4));
-    CU_TRY(s->st_bcpu.ensure(8));
-    CU_TRY(s->st_bmem.ensure(8));
-    CU_TRY(cudaMemcpyAsync(s->st_bnode.p, &node_idx, 4, cudaMemcpyHostToDevice, s->stream));
-    CU_TRY(cudaMemcpyAsync(s->st_bcpu.p, &req_cpu, 8, cudaMemcpyHostToDevice, s->stream));
-    CU_TRY(cudaMemcpyAsync(s->st_bmem.p, &req_mem, 8, cudaMemcpyHostToDevice, s->stream));
-    CU_TRY(launch_free_reduce(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), s->st_bnode.as<int32_t>(),
-                              s->st_bcpu.as<int64_t>(), s->st_bmem.as<int64_t>(), 1, s->stream));
+    Claims c;
+    const int rc = stage_claims(s, 1, &node_idx, &req_cpu, &req_mem, &c);
+    if (rc) return rc;
+    CU_TRY(launch_free_reduce(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), c.node, c.cpu, c.mem, 1, s->stream));
     CU_TRY(cudaStreamSynchronize(s->stream));
     return KS_OK;
 }
@@ -351,12 +368,14 @@ static int refresh_derived(ks_snapshot* s, cudaStream_t st) {
     return KS_OK;
 }
 
-static int copy_pods_in(ks_snapshot* s, const ks_pods* pods, cudaStream_t st) {
+// host-space pods [c0, c1) to their staging in d_in (pv, from stage_pods)
+static int copy_pods_in(const ks_pods* pods, const PodView& pv, uint32_t W, uint64_t c0, uint64_t c1, cudaStream_t st) {
     if (pods->mem_space == KS_MEM_DEVICE) return KS_OK;
-    const uint64_t P = pods->n;
-    CU_TRY(cudaMemcpyAsync(s->st_rc.p, pods->req_cpu, P * 8, cudaMemcpyHostToDevice, st));
-    CU_TRY(cudaMemcpyAsync(s->st_rm.p, pods->req_mem, P * 8, cudaMemcpyHostToDevice, st));
-    CU_TRY(cudaMemcpyAsync(s->st_sel.p, pods->sel, P * 8 * s->W, cudaMemcpyHostToDevice, st));
+    const uint64_t m = c1 - c0;
+    CU_TRY(cudaMemcpyAsync(const_cast<int64_t*>(pv.req_cpu) + c0, pods->req_cpu + c0, m * 8, cudaMemcpyHostToDevice, st));
+    CU_TRY(cudaMemcpyAsync(const_cast<int64_t*>(pv.req_mem) + c0, pods->req_mem + c0, m * 8, cudaMemcpyHostToDevice, st));
+    CU_TRY(cudaMemcpyAsync(const_cast<uint64_t*>(pv.sel) + c0 * W, pods->sel + c0 * W, m * 8 * W, cudaMemcpyHostToDevice,
+                           st));
     return KS_OK;
 }
 
@@ -370,7 +389,9 @@ static bool is_pinned_host(const void* p) {
     return a.type == cudaMemoryTypeHost;
 }
 
-// passing st == nullptr only prepares (allocates staging, fills *pv); the copies are enqueued by copy_pods_in
+// Host-space pods are staged in d_in as [rc | rm | sel], each array at a multiple of 256 bytes; device-space pods are
+// read in place.  Passing st == nullptr only prepares (allocates staging, fills *pv); the copies are enqueued by
+// copy_pods_in.
 static int stage_pods(ks_snapshot* s, const ks_pods* pods, cudaStream_t st, PodView* pv) {
     const uint64_t P = pods->n;
     pv->P = (uint32_t)P;
@@ -380,14 +401,14 @@ static int stage_pods(ks_snapshot* s, const ks_pods* pods, cudaStream_t st, PodV
         pv->sel = pods->sel;
         return KS_OK;
     }
-    CU_TRY(s->st_rc.ensure(P * 8));
-    CU_TRY(s->st_rm.ensure(P * 8));
-    CU_TRY(s->st_sel.ensure(P * 8 * s->W));
-    pv->req_cpu = s->st_rc.as<int64_t>();
-    pv->req_mem = s->st_rm.as<int64_t>();
-    pv->sel = s->st_sel.as<uint64_t>();
+    BlockLayout L;
+    const size_t o_rc = L.take<int64_t>(P), o_rm = L.take<int64_t>(P, 256), o_sel = L.take<uint64_t>(P * s->W, 256);
+    CU_TRY(s->d_in.ensure(L.size));
+    pv->req_cpu = at<int64_t>(s->d_in.p, o_rc);
+    pv->req_mem = at<int64_t>(s->d_in.p, o_rm);
+    pv->sel = at<uint64_t>(s->d_in.p, o_sel);
     if (st == nullptr) return KS_OK; // prepare only: the caller enqueues the copies itself (copy_pods_in)
-    return copy_pods_in(s, pods, st);
+    return copy_pods_in(pods, *pv, s->W, 0, P, st);
 }
 
 static int check_pods(const ks_snapshot* s, const ks_pods* pods) {
@@ -395,8 +416,7 @@ static int check_pods(const ks_snapshot* s, const ks_pods* pods) {
     if (!pods) return fail(KS_ERR_INVALID, "pods is NULL");
     if (pods->n > 0xfffffff0ull) return fail(KS_ERR_RANGE, "too many pods in one call");
     if (pods->n && (!pods->req_cpu || !pods->req_mem || !pods->sel)) return fail(KS_ERR_INVALID, "NULL pod array");
-    if (pods->mem_space != KS_MEM_HOST && pods->mem_space != KS_MEM_DEVICE)
-        return fail(KS_ERR_INVALID, "bad pods.mem_space");
+    if (!valid_space(pods->mem_space)) return fail(KS_ERR_INVALID, "bad pods.mem_space");
     return KS_OK;
 }
 
@@ -412,9 +432,9 @@ int ks_check_cells(ks_snapshot* s, const ks_pods* pods, uint8_t* out_codes) {
     PodView pv;
     rc = stage_pods(s, pods, s->stream, &pv);
     if (rc) return rc;
-    CU_TRY(s->st_codes.ensure(cells));
-    CU_TRY(launch_check_cells(node_table(s), pv, s->st_codes.as<uint8_t>(), 0, s->N, s->stream));
-    CU_TRY(cudaMemcpyAsync(out_codes, s->st_codes.p, cells, cudaMemcpyDeviceToHost, s->stream));
+    CU_TRY(s->d_out.ensure(cells));
+    CU_TRY(launch_check_cells(node_table(s), pv, s->d_out.as<uint8_t>(), 0, s->N, s->stream));
+    CU_TRY(cudaMemcpyAsync(out_codes, s->d_out.p, cells, cudaMemcpyDeviceToHost, s->stream));
     CU_TRY(cudaStreamSynchronize(s->stream));
     return KS_OK;
 }
@@ -433,19 +453,29 @@ int ks_check_cell(ks_snapshot* s, int64_t req_cpu, int64_t req_mem, const uint64
     PodView pv;
     int rc = stage_pods(s, &pods, s->stream, &pv);
     if (rc) return rc;
-    CU_TRY(s->st_codes.ensure(16));
-    CU_TRY(launch_check_cells(node_table(s), pv, s->st_codes.as<uint8_t>(), node_idx, 1, s->stream));
+    CU_TRY(s->d_out.ensure(16));
+    CU_TRY(launch_check_cells(node_table(s), pv, s->d_out.as<uint8_t>(), node_idx, 1, s->stream));
     uint8_t code = 0xff;
-    CU_TRY(cudaMemcpyAsync(&code, s->st_codes.p, 1, cudaMemcpyDeviceToHost, s->stream));
+    CU_TRY(cudaMemcpyAsync(&code, s->d_out.p, 1, cudaMemcpyDeviceToHost, s->stream));
     CU_TRY(cudaStreamSynchronize(s->stream));
     return (int)code;
+}
+
+// ks_select's bindings of ov's first m pods back to the host.  Each host pointer is already offset to the same pods, and
+// null when absent or already served by the launcher.
+static int copy_bindings_back(const OutView& ov, int32_t* node_idx, int64_t* score, uint32_t* cnt, uint64_t m,
+                              cudaStream_t st) {
+    if (node_idx) CU_TRY(cudaMemcpyAsync(node_idx, ov.node_idx, m * 4, cudaMemcpyDeviceToHost, st));
+    if (score) CU_TRY(cudaMemcpyAsync(score, ov.score, m * 8, cudaMemcpyDeviceToHost, st));
+    if (cnt) CU_TRY(cudaMemcpyAsync(cnt, ov.cnt, m * 4, cudaMemcpyDeviceToHost, st));
+    return KS_OK;
 }
 
 int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, ks_bindings* out, void* cuda_stream) {
     int rc = check_pods(s, pods);
     if (rc) return rc;
     if (!out) return fail(KS_ERR_INVALID, "out is NULL");
-    if (policy != KS_SCORE_LEFTOVER && policy != KS_SCORE_LEAST_ALLOCATED) return fail(KS_ERR_INVALID, "bad policy");
+    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
     if ((flags & KS_SELECT_FORCE_BITPAR) && (flags & KS_SELECT_FORCE_DIRECT)) return fail(KS_ERR_INVALID, "bad flags");
     const uint64_t P = pods->n;
     if (out->mask) {
@@ -509,23 +539,21 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
     ov.mask = reinterpret_cast<uint32_t*>(out->mask);
     ov.mask_row_words = out->mask_row_bytes / 4;
     ov.mask_valid_words = (uint32_t)(ks_mask_row_bytes(s->N) / 4);
-    if (out_host) {
-        if (out->node_idx) {
-            CU_TRY(s->st_idx.ensure(P * 4));
-            ov.node_idx = s->st_idx.as<int32_t>();
-        }
-        if (out->score) {
-            CU_TRY(s->st_score.ensure(P * 8));
-            ov.score = s->st_score.as<int64_t>();
-        }
-        if (out->feasible_cnt) {
-            CU_TRY(s->st_cnt.ensure(P * 4));
-            ov.cnt = s->st_cnt.as<uint32_t>();
-        }
-    }
-    if (mask_host) {
-        CU_TRY(s->st_mask.ensure(P * out->mask_row_bytes));
-        ov.mask = s->st_mask.as<uint32_t>();
+    // the host destinations of the bindings; null when absent or device-space
+    int32_t* h_idx = out_host ? out->node_idx : nullptr;
+    int64_t* h_score = out_host ? out->score : nullptr;
+    uint32_t* h_cnt = out_host ? out->feasible_cnt : nullptr;
+    if (out_host || mask_host) { // staged in d_out: [mask | node_idx | score | cnt], each at a multiple of 256 bytes
+        BlockLayout D;
+        const size_t o_mask = D.take<uint8_t>(mask_host ? P * out->mask_row_bytes : 0),
+                     o_idx = D.take<int32_t>(h_idx ? P : 0, 256), o_score = D.take<int64_t>(h_score ? P : 0, 256),
+                     o_cnt = D.take<uint32_t>(h_cnt ? P : 0, 256);
+        CU_TRY(s->d_out.ensure(D.size));
+        void* b = s->d_out.p;
+        if (mask_host) ov.mask = at<uint32_t>(b, o_mask);
+        if (h_idx) ov.node_idx = at<int32_t>(b, o_idx);
+        if (h_score) ov.score = at<int64_t>(b, o_score);
+        if (h_cnt) ov.cnt = at<uint32_t>(b, o_cnt);
     }
 
     if (s->N == 0) { // empty node store: every pod gets None (src/main.rs:56,70)
@@ -536,11 +564,8 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
             CU_TRY(launch_exchange_push(po, ov.node_idx, ov.score, (uint32_t)P, st));
             CU_TRY(launch_exchange_wait(po, s->xflag.as<int>(), st));
         }
-        if (out_host) {
-            if (out->node_idx) CU_TRY(cudaMemcpyAsync(out->node_idx, ov.node_idx, P * 4, cudaMemcpyDeviceToHost, st));
-            if (out->score) CU_TRY(cudaMemcpyAsync(out->score, ov.score, P * 8, cudaMemcpyDeviceToHost, st));
-            if (out->feasible_cnt) CU_TRY(cudaMemcpyAsync(out->feasible_cnt, ov.cnt, P * 4, cudaMemcpyDeviceToHost, st));
-        }
+        rc = copy_bindings_back(ov, h_idx, h_score, h_cnt, P, st);
+        if (rc) return rc;
         s->last_path = "empty";
     } else {
         SelectLaunch L;
@@ -563,13 +588,14 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
             if (e != cudaSuccess) return fail(KS_ERR_CUDA, "bit-parallel prepare failed: %s", cudaGetErrorString(e));
         } else {
             grid = direct_grid(s->W, L.pv.P, s->Npad, s->sms);
-            if (grid.n_chunks > 1) {
-                CU_TRY(s->part_key.ensure((size_t)grid.n_chunks * P * 8));
-                CU_TRY(s->part_idx.ensure((size_t)grid.n_chunks * P * 4));
-                CU_TRY(s->part_cnt.ensure((size_t)grid.n_chunks * P * 4));
-                part.key = s->part_key.as<int64_t>();
-                part.idx = s->part_idx.as<int32_t>();
-                part.cnt = s->part_cnt.as<uint32_t>();
+            if (grid.n_chunks > 1) { // keys | indices | counts, each [chunks*P] at a multiple of 256 bytes
+                const uint64_t rows = (uint64_t)grid.n_chunks * P;
+                BlockLayout PL;
+                const size_t o_key = PL.take<int64_t>(rows), o_idx = PL.take<int32_t>(rows, 256),
+                             o_cnt = PL.take<uint32_t>(rows, 256);
+                CU_TRY(s->part_sel.ensure(PL.size));
+                void* b = s->part_sel.p;
+                part = PartialView{at<int64_t>(b, o_key), at<int32_t>(b, o_idx), at<uint32_t>(b, o_cnt)};
             }
         }
         s->last_path = use_bitpar ? "bitpar" : "direct";
@@ -583,19 +609,14 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
                                     : 1u;
         auto enqueue = [&]() -> int {
             if (n_pipe == 1) {
-                int crc = copy_pods_in(s, pods, st);
+                int crc = copy_pods_in(pods, L.pv, s->W, 0, P, st);
                 if (crc) return crc;
             } else {
                 CU_TRY(cudaEventRecord(s->ev_cfork, st));
                 CU_TRY(cudaStreamWaitEvent(s->copy_stream, s->ev_cfork, 0));
                 for (uint32_t c = 0; c < n_pipe; c++) {
-                    const uint64_t c0 = P * c / n_pipe, c1 = P * (c + 1) / n_pipe, m = c1 - c0;
-                    CU_TRY(cudaMemcpyAsync(s->st_rc.as<int64_t>() + c0, pods->req_cpu + c0, m * 8, cudaMemcpyHostToDevice,
-                                           s->copy_stream));
-                    CU_TRY(cudaMemcpyAsync(s->st_rm.as<int64_t>() + c0, pods->req_mem + c0, m * 8, cudaMemcpyHostToDevice,
-                                           s->copy_stream));
-                    CU_TRY(cudaMemcpyAsync(s->st_sel.as<uint64_t>() + c0 * s->W, pods->sel + c0 * s->W, m * 8 * s->W,
-                                           cudaMemcpyHostToDevice, s->copy_stream));
+                    int crc = copy_pods_in(pods, L.pv, s->W, P * c / n_pipe, P * (c + 1) / n_pipe, s->copy_stream);
+                    if (crc) return crc;
                     CU_TRY(cudaEventRecord(s->ev_in[c], s->copy_stream));
                 }
                 for (uint32_t c = 0; c < n_pipe; c++) {
@@ -610,20 +631,17 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
                     if (Lc.ov.score) Lc.ov.score += c0;
                     if (Lc.ov.cnt) Lc.ov.cnt += c0;
                     if (Lc.ov.mask) Lc.ov.mask += c0 * Lc.ov.mask_row_words;
-                    Lc.host_node_idx = out->node_idx ? out->node_idx + c0 : nullptr;
-                    Lc.host_score = out->score ? out->score + c0 : nullptr;
+                    Lc.host_node_idx = h_idx ? h_idx + c0 : nullptr;
+                    Lc.host_score = h_score ? h_score + c0 : nullptr;
                     cudaError_t e = bitpar_select(s->bp, Lc, nullptr, nullptr);
                     if (e != cudaSuccess) return fail(KS_ERR_CUDA, "bit-parallel select failed: %s", cudaGetErrorString(e));
-                    if (Lc.host_node_idx)
-                        CU_TRY(cudaMemcpyAsync(Lc.host_node_idx, Lc.ov.node_idx, m * 4, cudaMemcpyDeviceToHost, st));
-                    if (Lc.host_score) CU_TRY(cudaMemcpyAsync(Lc.host_score, Lc.ov.score, m * 8, cudaMemcpyDeviceToHost, st));
-                    if (out->feasible_cnt)
-                        CU_TRY(cudaMemcpyAsync(out->feasible_cnt + c0, Lc.ov.cnt, m * 4, cudaMemcpyDeviceToHost, st));
+                    int crc = copy_bindings_back(Lc.ov, Lc.host_node_idx, Lc.host_score, h_cnt ? h_cnt + c0 : nullptr, m, st);
+                    if (crc) return crc;
                 }
                 return KS_OK;
             }
-            L.host_node_idx = out_host ? out->node_idx : nullptr; // served early by the launcher when it can
-            L.host_score = out_host ? out->score : nullptr;
+            L.host_node_idx = h_idx; // served early by the launcher when it can
+            L.host_score = h_score;
             L.ready_event = out_host ? nullptr : (cudaEvent_t)out->bindings_ready_event;
             if (use_bitpar) {
                 cudaError_t e = bitpar_select(s->bp, L, timing ? s->ev[1].h : nullptr, timing ? s->ev[2].h : nullptr);
@@ -638,12 +656,8 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
             // fused all-gather: this rank's bindings went out from the argmax kernels (bit-parallel path) or the push
             // kernel; the call's stream work ends when every other rank's bindings have arrived here
             if (xc) CU_TRY(launch_exchange_wait(po, s->xflag.as<int>(), st));
-            if (out_host) {
-                if (L.host_node_idx) CU_TRY(cudaMemcpyAsync(out->node_idx, ov.node_idx, P * 4, cudaMemcpyDeviceToHost, st));
-                if (L.host_score) CU_TRY(cudaMemcpyAsync(out->score, ov.score, P * 8, cudaMemcpyDeviceToHost, st));
-                if (out->feasible_cnt)
-                    CU_TRY(cudaMemcpyAsync(out->feasible_cnt, ov.cnt, P * 4, cudaMemcpyDeviceToHost, st));
-            }
+            int crc = copy_bindings_back(ov, L.host_node_idx, L.host_score, h_cnt, P, st);
+            if (crc) return crc;
             if (mask_host)
                 CU_TRY(cudaMemcpyAsync(out->mask, ov.mask, P * out->mask_row_bytes, cudaMemcpyDeviceToHost, st));
             if (L.ready_event) { // not served earlier (per-cell path): the bindings are final here
@@ -828,21 +842,18 @@ int ks_snapshot_commit_claims(ks_snapshot* s, uint64_t n, const int32_t* claim_n
     s->derived_dirty = true;
     s->version++;
     const uint32_t chunk = stream_max_claims();
-    CU_TRY(s->st_bnode.ensure(n * 4));
-    CU_TRY(s->st_bcpu.ensure(n * 8));
-    CU_TRY(s->st_bmem.ensure(n * 8));
-    CU_TRY(s->st_codes.ensure(n));
-    CU_TRY(cudaMemcpyAsync(s->st_bnode.p, claim_node, n * 4, cudaMemcpyHostToDevice, s->stream));
-    CU_TRY(cudaMemcpyAsync(s->st_bcpu.p, req_cpu, n * 8, cudaMemcpyHostToDevice, s->stream));
-    CU_TRY(cudaMemcpyAsync(s->st_bmem.p, req_mem, n * 8, cudaMemcpyHostToDevice, s->stream));
+    CU_TRY(s->d_out.ensure(n));
+    Claims c;
+    rc = stage_claims(s, n, claim_node, req_cpu, req_mem, &c);
+    if (rc) return rc;
+    uint8_t* codes = s->d_out.as<uint8_t>();
     // chunks run in arrival order on one stream: per-node arrival order is preserved across chunks
     for (uint64_t off = 0; off < n; off += chunk) {
         const uint32_t m = (uint32_t)std::min<uint64_t>(chunk, n - off);
-        CU_TRY(launch_stream_resolve(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), s->st_bnode.as<int32_t>() + off,
-                                     s->st_bcpu.as<int64_t>() + off, s->st_bmem.as<int64_t>() + off, m, s->N,
-                                     s->st_codes.as<uint8_t>() + off, s->stream));
+        CU_TRY(launch_stream_resolve(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), c.node + off, c.cpu + off,
+                                     c.mem + off, m, s->N, codes + off, s->stream));
     }
-    CU_TRY(cudaMemcpyAsync(out_accepted, s->st_codes.p, n, cudaMemcpyDeviceToHost, s->stream));
+    CU_TRY(cudaMemcpyAsync(out_accepted, codes, n, cudaMemcpyDeviceToHost, s->stream));
     CU_TRY(cudaStreamSynchronize(s->stream));
     return KS_OK;
 }
@@ -868,12 +879,12 @@ int ks_select_sampling(ks_snapshot* s, const ks_pods* pods, uint32_t attempts, u
     PodView pv;
     rc = stage_pods(s, pods, s->stream, &pv);
     if (rc) return rc;
-    // one scratch buffer: node_idx[P] | attempts[P] | draw_node[P*attempts] | draw_code[P*attempts]
+    // one block in d_out: node_idx[P] | attempts[P] | draw_node[P*attempts] | draw_code[P*attempts]
     BlockLayout L;
     const size_t off_idx = L.take<int32_t>(P), off_att = L.take<uint32_t>(P), off_dn = L.take<int32_t>(draws),
                  off_dc = L.take<uint8_t>(draws);
-    CU_TRY(s->st_samp.ensure(L.size));
-    uint8_t* base = s->st_samp.as<uint8_t>();
+    CU_TRY(s->d_out.ensure(L.size));
+    uint8_t* base = s->d_out.as<uint8_t>();
     CU_TRY(launch_select_sampling(node_table(s), pv, attempts, seed, first_pod_index, at<int32_t>(base, off_idx),
                                   at<uint32_t>(base, off_att), out_draw_node ? at<int32_t>(base, off_dn) : nullptr,
                                   out_draw_code ? base + off_dc : nullptr, s->stream));
@@ -889,7 +900,7 @@ int ks_explain(ks_snapshot* s, const ks_pods* pods, ks_pod_reasons* out, int32_t
     static_assert(sizeof(ks_pod_reasons) == 16, "ks_pod_reasons is four uint32");
     int rc = check_pods(s, pods);
     if (rc) return rc;
-    if (out_space != KS_MEM_HOST && out_space != KS_MEM_DEVICE) return fail(KS_ERR_INVALID, "bad out_space");
+    if (!valid_space(out_space)) return fail(KS_ERR_INVALID, "bad out_space");
     const uint64_t P = pods->n;
     if (P && !out) return fail(KS_ERR_INVALID, "out is NULL");
     if (P == 0) return KS_OK;
@@ -898,8 +909,8 @@ int ks_explain(ks_snapshot* s, const ks_pods* pods, ks_pod_reasons* out, int32_t
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
     uint32_t* d_out = reinterpret_cast<uint32_t*>(out);
     if (out_space == KS_MEM_HOST) {
-        CU_TRY(s->st_reasons.ensure(P * sizeof(ks_pod_reasons)));
-        d_out = s->st_reasons.as<uint32_t>();
+        CU_TRY(s->d_out.ensure(P * sizeof(ks_pod_reasons)));
+        d_out = s->d_out.as<uint32_t>();
     }
     if (s->N == 0) {
         CU_TRY(cudaMemsetAsync(d_out, 0, P * sizeof(ks_pod_reasons), st));
@@ -920,8 +931,8 @@ int ks_select_topk(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t k, 
     int rc = check_pods(s, pods);
     if (rc) return rc;
     if (k == 0 || k > KS_TOPK_MAX) return fail(KS_ERR_RANGE, "k must be in [1, %u] (got %u)", KS_TOPK_MAX, k);
-    if (policy != KS_SCORE_LEFTOVER && policy != KS_SCORE_LEAST_ALLOCATED) return fail(KS_ERR_INVALID, "bad policy");
-    if (out_space != KS_MEM_HOST && out_space != KS_MEM_DEVICE) return fail(KS_ERR_INVALID, "bad out_space");
+    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    if (!valid_space(out_space)) return fail(KS_ERR_INVALID, "bad out_space");
     const uint64_t P = pods->n;
     if (P && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
     if (P == 0) return KS_OK;
@@ -930,11 +941,11 @@ int ks_select_topk(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t k, 
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
     const uint64_t cells = P * k;
     OutView ov{out_node_idx, out_score, out_feasible_cnt, nullptr, 0, 0};
-    if (out_space == KS_MEM_HOST) { // one staging block: score [P*k] | node_idx [P*k] | feasible_cnt [P]
+    if (out_space == KS_MEM_HOST) { // one block in d_out: score [P*k] | node_idx [P*k] | feasible_cnt [P]
         BlockLayout L;
         const size_t o_score = L.take<int64_t>(cells), o_idx = L.take<int32_t>(cells), o_cnt = L.take<uint32_t>(P);
-        CU_TRY(s->st_topk.ensure(L.size));
-        void* b = s->st_topk.p;
+        CU_TRY(s->d_out.ensure(L.size));
+        void* b = s->d_out.p;
         ov.score = out_score ? at<int64_t>(b, o_score) : nullptr;
         ov.node_idx = at<int32_t>(b, o_idx);
         ov.cnt = out_feasible_cnt ? at<uint32_t>(b, o_cnt) : nullptr;
@@ -985,8 +996,7 @@ static int check_preempt_bound(const ks_snapshot* s, const ks_bound_pods* bound)
         const int64_t c = bound->req_cpu[b], m = bound->req_mem[b];
         if (n < 0 || (uint32_t)n >= s->N)
             return fail(KS_ERR_INVALID, "bound pod %llu: node index %d out of range", (unsigned long long)b, n);
-        if (c > KS_MAX_CPU_MILLI || c < -KS_MAX_CPU_MILLI || m > KS_MAX_MEM_BYTES || m < -KS_MAX_MEM_BYTES)
-            return fail(KS_ERR_RANGE, "bound pod %llu request out of range", (unsigned long long)b);
+        if (!within_limits(c, m)) return fail(KS_ERR_RANGE, "bound pod %llu request out of range", (unsigned long long)b);
         uint64_t* a = &abs_sum[(size_t)n * 2];
         a[0] += (uint64_t)(c < 0 ? -c : c); // each term <= 2^55: no wrap before the sum passes the limit
         a[1] += (uint64_t)(m < 0 ? -m : m);
@@ -1003,7 +1013,7 @@ int ks_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* pod_priority,
     if (rc) return rc;
     if (max_victims == 0 || max_victims > KS_PREEMPT_MAX_VICTIMS)
         return fail(KS_ERR_RANGE, "max_victims must be in [1, %u] (got %u)", KS_PREEMPT_MAX_VICTIMS, max_victims);
-    if (out_space != KS_MEM_HOST && out_space != KS_MEM_DEVICE) return fail(KS_ERR_INVALID, "bad out_space");
+    if (!valid_space(out_space)) return fail(KS_ERR_INVALID, "bad out_space");
     const uint64_t P = pods->n;
     if (P && (!pod_priority || !out)) return fail(KS_ERR_INVALID, "pod_priority or out is NULL");
     if (!bound) return fail(KS_ERR_INVALID, "bound is NULL");
@@ -1021,11 +1031,12 @@ int ks_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* pod_priority,
     ks_preemption* d_out = out;
     int32_t* d_vic = out_victims;
     const int32_t* d_prio = pod_priority;
-    // one staging block: rows [P] | victims [P * max_victims] (host-space outputs) | priorities [P] (host-space pods)
+    // one block in d_out when outputs or pods are host-space: rows [P] | victims [P * max_victims] (host-space outputs) |
+    // priorities [P] (host-space pods)
     BlockLayout L;
     const size_t o_rows = L.take<ks_preemption>(P), o_vic = L.take<int32_t>(n_vic), o_prio = L.take<int32_t>(P);
-    CU_TRY(s->st_pre.ensure(L.size));
-    void* stg = s->st_pre.p;
+    if (out_space == KS_MEM_HOST || pods->mem_space == KS_MEM_HOST) CU_TRY(s->d_out.ensure(L.size));
+    void* stg = s->d_out.p;
     if (out_space == KS_MEM_HOST) {
         d_out = at<ks_preemption>(stg, o_rows);
         d_vic = out_victims ? at<int32_t>(stg, o_vic) : nullptr;
@@ -1080,7 +1091,7 @@ int ks_stream_bind(ks_snapshot* s, const ks_pods* pods, int policy, int32_t* out
     if (pods->n && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
     const uint64_t n = pods->n;
     const uint32_t W = s->W;
-    if (policy != KS_SCORE_LEFTOVER && policy != KS_SCORE_LEAST_ALLOCATED) return fail(KS_ERR_INVALID, "bad policy");
+    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
     rc = check_commit_requests(n, pods->req_cpu, pods->req_mem);
     if (rc) return rc;
     if (n > 0 && n <= STREAM_BATCH_MAX && s->N > 0 && s->coop) {
@@ -1186,7 +1197,7 @@ int ks_gang_bind(ks_snapshot* s, const ks_pods* pods, const ks_gangs* gangs, int
     if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_gang_bind takes host-space pods");
     if (!gangs || !gangs->offset || (gangs->n && !gangs->min_member)) return fail(KS_ERR_INVALID, "NULL group array");
     if (pods->n && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
-    if (policy != KS_SCORE_LEFTOVER && policy != KS_SCORE_LEAST_ALLOCATED) return fail(KS_ERR_INVALID, "bad policy");
+    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
     const uint64_t P = pods->n, G = gangs->n;
     const uint64_t* off = gangs->offset;
     if (off[0] != 0) return fail(KS_ERR_INVALID, "offset[0] must be 0");
@@ -1268,7 +1279,7 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidate
     if (!cand || !cand->offset || (cand->n && (!cand->node_idx || !out_placed)))
         return fail(KS_ERR_INVALID, "NULL candidate array or out_placed");
     if (pods->n && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
-    if (policy != KS_SCORE_LEFTOVER && policy != KS_SCORE_LEAST_ALLOCATED) return fail(KS_ERR_INVALID, "bad policy");
+    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
     if (flags & ~KS_DRAIN_EXCLUDE_CANDIDATES) return fail(KS_ERR_INVALID, "unknown flags 0x%x", flags);
     const uint64_t P = pods->n, D = cand->n;
     const uint64_t* off = cand->offset;
@@ -1397,7 +1408,7 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const ks_node_templ
     if (!t || !out_best) return fail(KS_ERR_INVALID, "NULL templates or out_best");
     const uint64_t P = pods->n, T = t->n;
     const uint32_t W = t->label_words;
-    if (W != 1 && W != 2 && W != 4 && W != 8) return fail(KS_ERR_INVALID, "label_words must be 1, 2, 4 or 8 (got %u)", W);
+    if (!valid_label_words(W)) return fail(KS_ERR_INVALID, "label_words must be 1, 2, 4 or 8 (got %u)", W);
     if (T && (!out || !t->alloc_cpu || !t->alloc_mem || !t->free_cpu || !t->free_mem || !t->labels || !t->max_nodes))
         return fail(KS_ERR_INVALID, "NULL template array or out");
     if (P > KS_SCALEUP_MAX_PODS) return fail(KS_ERR_RANGE, "%llu pods (at most %u)", (unsigned long long)P, KS_SCALEUP_MAX_PODS);
@@ -1583,7 +1594,7 @@ static void stream_worker(ks_stream* q) {
 
 int ks_stream_open(ks_snapshot* s, int policy, uint32_t max_batch, ks_stream** out) {
     if (!s || !out) return fail(KS_ERR_INVALID, "NULL argument");
-    if (policy != KS_SCORE_LEFTOVER && policy != KS_SCORE_LEAST_ALLOCATED) return fail(KS_ERR_INVALID, "bad policy");
+    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
     ks_stream* q = new (std::nothrow) ks_stream();
     if (!q) return fail(KS_ERR_NOMEM, "out of host memory");
     q->snap = s;

@@ -1,8 +1,12 @@
-"""The staging block shared by the host-staged calls (-m gpu): ks_scaleup_estimate, ks_gang_bind, ks_drain_check and
-ks_stream_bind's device loop stage through one pinned block and one device in/work/out set per snapshot.  One snapshot
-runs a sequence of those calls that grows and shrinks the block, so each call finds contents a larger call of another
-kind left behind.  Every result, and free[] after the committing calls, must equal the same call on a fresh snapshot;
-cached-graph device-space selects, a select_topk and a preempt in between keep returning what they return alone."""
+"""The staging set shared by every call that synchronises before it returns (-m gpu): the host-staged calls
+(ks_scaleup_estimate, ks_gang_bind, ks_drain_check, ks_stream_bind's device loop) and the host-space pods and results of
+select, explain, top-k, preempt, check_cells, sampling, commit_claims and apply_bind stage through one device
+in/work/out set per snapshot.  One snapshot runs a sequence of those calls that grows and shrinks the set, so each call
+finds contents a larger call of another kind left behind.  Every result, and free[] after the committing calls, must
+equal the same call on a fresh snapshot; cached-graph selects in between, with device-space buffers and with pinned host
+pods, outputs and mask (a graph that points into the shared set), keep returning the oracle's bindings."""
+from dataclasses import astuple
+
 import numpy as np
 import pytest
 
@@ -48,13 +52,17 @@ def test_shared_staging_across_call_kinds(ks, orc, cluster):
     ac, am, lab, bn, bc, bm, rc, rm, sel = cluster
     rng = np.random.default_rng(0x57A6)
     fc, fm = orc.free_reduce(ac, am, bn, bc, bm)
-    Q = 3000  # pods of the device-space select
-    o_idx, o_score, o_cnt = orc.run_packed(fc, fm, ac, am, lab, rc[:Q], rm[:Q], sel[:Q], want_mask=False)[:3]
+    Q = 3000  # pods of the cached-graph selects
+    o_idx, o_score, o_cnt, o_mask = orc.run_packed(fc, fm, ac, am, lab, rc[:Q], rm[:Q], sel[:Q])[:4]
     dev = torch.device("cuda:0")
     t = [torch.from_numpy(np.ascontiguousarray(x[:Q]).view(np.int64)).to(dev) for x in (rc, rm, sel)]
     idx = torch.empty(Q, dtype=torch.int32, device=dev)
     score = torch.empty(Q, dtype=torch.int64, device=dev)
     cnt = torch.empty(Q, dtype=torch.int32, device=dev)
+    row = ks.capi.mask_row_bytes(N)
+    h_pods = [x.cpu().pin_memory() for x in t]
+    h_idx, h_score, h_cnt = (torch.empty(Q, dtype=d).pin_memory() for d in (torch.int32, torch.int64, torch.int32))
+    h_mask = torch.empty((Q, row), dtype=torch.uint8).pin_memory()
     bprio = rng.integers(-100, 100, len(bn)).astype(np.int32)
     pprio = rng.integers(-100, 200, P).astype(np.int32)
 
@@ -84,6 +92,16 @@ def test_shared_staging_across_call_kinds(ks, orc, cluster):
                 assert np.array_equal(idx.cpu().numpy(), o_idx), (what, rep)
                 assert np.array_equal(score.cpu().numpy(), o_score), (what, rep)
                 assert np.array_equal(cnt.cpu().numpy().view(np.uint32), o_cnt), (what, rep)
+            for rep in range(2):  # the same select from pinned host memory: its graph points into d_in / d_out
+                for b in (h_idx, h_cnt):
+                    b.fill_(-7)
+                h_mask.fill_(0x5A)
+                snap.select_raw(Q, *h_pods, ks.KS_MEM_HOST, h_idx, h_score, h_cnt, ks.KS_MEM_HOST, mask=h_mask,
+                                mask_row_bytes=row, mask_space=ks.KS_MEM_HOST)
+                assert np.array_equal(h_idx.numpy(), o_idx), (what, "host", rep)
+                assert np.array_equal(h_score.numpy(), o_score), (what, "host", rep)
+                assert np.array_equal(h_cnt.numpy().view(np.uint32), o_cnt), (what, "host", rep)
+                assert np.array_equal(h_mask.numpy(), o_mask), (what, "host mask", rep)
 
         big = _templates(rng, 256)
         run("scaleup T=256 P=4096 with out_node", lambda s: s.scaleup_estimate(rc[:4096], rm[:4096], sel[:4096], *big))
@@ -104,3 +122,10 @@ def test_shared_staging_across_call_kinds(ks, orc, cluster):
         node, doff, pick = _candidates(rng, 900, 16)
         assert len(pick) > first
         run("drain D=900 policy 1", lambda s: s.drain_check(rc[pick], rm[pick], sel[pick], node, doff, 1))
+        run("select with mask, all pods", lambda s: astuple(s.select(rc, rm, sel, want_mask=True)))
+        run("explain", lambda s: s.explain(rc, rm, sel))
+        # P x N bytes of codes: d_out grows past every earlier step (scale-up's out_node took 256 x 4096 x 4)
+        run("check_cells", lambda s: s.check_cells(rc, rm, sel))
+        run("select_sampling", lambda s: s.select_sampling(rc[:1000], rm[:1000], sel[:1000], seed=7))
+        run("commit_claims", lambda s: s.commit_claims(o_idx, rc[:Q], rm[:Q]), commits=True)
+        run("apply_bind", lambda s: s.apply_bind(int(o_idx[o_idx >= 0][0]), 100, 1 << 20), commits=True)
