@@ -2,10 +2,11 @@
 //
 //   per snapshot   k_node_bound, k_node_splitters/_bucket/_scatter/_rank  sample sort: global position of every node in
 //                                   free_cpu / free_mem / leftover-priority / least-allocated-bound order
-//                  k_build_cbtile   per column block (8 tiles of 256 nodes, node-index order): prefix tables + label-pair
-//                                   columns, 256-byte lines in tile order, staged in shared memory by the mask kernel
+//                  k_build_tiles    one tile of 256 nodes of an index in the column-block format (8 tiles per block):
+//                                   prefix tables + label-pair columns, 256-byte lines in tile order; three indexes:
+//                                   node order (staged in shared memory by the mask kernel), priority order and bound
+//                                   order (read through L1/L2 by the argmax kernels, with their bucket arrays)
 //                  k_build_ranks    rank tables: tile-local rank of every possible threshold (read through L1/L2)
-//                  k_build_tile     flat indexes in priority order / bound order for the argmax kernels
 //   per call       k_pod_ranks      request -> global rank threshold (splitters in smem + short global search) and the mask
 //                                   kernel's 16-byte pod record, in pod order
 //                  k_mask_rows      persistent, 1 CTA per SM; table blob staged by TMA bulk copies (cp.async.bulk + mbarrier);
@@ -236,28 +237,22 @@ __global__ void __launch_bounds__(256)
     }
 }
 
-static uint32_t pair_stride(uint32_t nt) { return nt * 32u; }
-
-// Prefix tables are interleaved by QUADS of tiles: row r of tiles 4k..4k+3 forms one 128-byte line
-//   [tile 4k row r | tile 4k+1 row r | tile 4k+2 row r | tile 4k+3 row r]
-// so the four tiles that the 8 lanes of a shared-memory phase work on always sit in four different pairs of 16-byte
-// bank groups, whatever their (unrelated) ranks are.  Byte offset of (tile, row) inside a table area:
-__host__ __device__ __forceinline__ uint32_t table_row_offset(uint32_t tile, uint32_t row) {
-    return (tile >> 2) * (uint32_t)(BP_ROWS * 128) + row * 128u + (tile & 3u) * 32u;
-}
-__host__ __device__ __forceinline__ uint32_t table_area_bytes(uint32_t nt) { return ((nt + 3u) / 4u) * (uint32_t)(BP_ROWS * 128); }
-
-// One CTA builds the index of one 256-slot tile.  slot_node maps slot -> node (nullptr = identity, i.e. the
-// node-index order used for the mask; ord_idx = priority order used for the argmax).
+// One CTA builds tile k of an index in the column-block format (ks_bitpar.h): its prefix rows and label-pair columns, at
+// 32 * (k % 8) of the 256-byte lines of column block k / 8.  slot_node maps the index's slots to nodes (nullptr = node
+// order).  Optional outputs: tile_sorted (node order, for k_build_ranks) gets the tile's global positions in ascending
+// order; bk (the ordered indexes, for the argmax kernels) gets the tile's column of the bucket arrays, which have no
+// columns for the padding tiles.
 __global__ void __launch_bounds__(288)
-    k_build_tile(NodeTable nt, const uint32_t* __restrict__ gposC, const uint32_t* __restrict__ gposM,
-                 const int32_t* __restrict__ slot_node, uint8_t* __restrict__ blob, BitparLayout lay) {
+    k_build_tiles(NodeTable nt, const uint32_t* __restrict__ gposC, const uint32_t* __restrict__ gposM,
+                  const int32_t* __restrict__ slot_node, uint8_t* __restrict__ blob, RowsLayout lay,
+                  uint32_t* __restrict__ tile_sorted, TileBuckets bk) {
     __shared__ uint32_t s_g[2][BP_TILE];
     __shared__ uint16_t s_lr[2][BP_TILE];
     __shared__ uint8_t s_valid[BP_TILE];
     __shared__ uint64_t s_lab[KS_MAX_LABEL_WORDS][BP_TILE];
-    const uint32_t tile_g = blockIdx.x, cb = tile_g / lay.nt, t = tile_g % lay.nt, s = threadIdx.x;
-    uint8_t* B = blob + (size_t)cb * lay.blob_bytes;
+    const uint32_t tile_g = blockIdx.x, cb = tile_g / RW_TILES, t = tile_g % RW_TILES, s = threadIdx.x;
+    const uint32_t n_tiles_pad = lay.ncb * RW_TILES;
+    uint8_t* B = blob + (size_t)cb * lay.cb_stride;
     if (s < BP_TILE) {
         const uint32_t slot = tile_g * BP_TILE + s;
         const bool v = slot < nt.N;
@@ -274,110 +269,13 @@ __global__ void __launch_bounds__(288)
             uint32_t c = 0;
             for (int k = 0; k < BP_TILE; k++) c += s_g[r][k] < g;
             s_lr[r][s] = (uint16_t)c;
-        }
-    }
-    __syncthreads();
-    // prefix tables: row r = slots of the tile whose tile-local rank is >= r  (i.e. free >= threshold)
-    if (s < BP_ROWS) {
-        for (int r = 0; r < 2; r++) {
-            uint32_t w[8];
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                uint32_t acc = 0;
-                for (int b = 0; b < 32; b++) {
-                    const int k = j * 32 + b;
-                    acc |= (uint32_t)(s_valid[k] && s_lr[r][k] >= s) << b;
-                }
-                w[j] = acc;
-            }
-            uint4* tab = reinterpret_cast<uint4*>(B + (r ? lay.off_tabM : lay.off_tabC) + table_row_offset(t, s));
-            tab[0] = make_uint4(w[0], w[1], w[2], w[3]);
-            tab[1] = make_uint4(w[4], w[5], w[6], w[7]);
-        }
-    }
-    // bucket membership + base counts, layout [bucket][tile]
-    unsigned long long* membC = reinterpret_cast<unsigned long long*>(B + lay.off_membC);
-    unsigned long long* membM = reinterpret_cast<unsigned long long*>(B + lay.off_membM);
-    uint16_t* baseC = reinterpret_cast<uint16_t*>(B + lay.off_baseC);
-    uint16_t* baseM = reinterpret_cast<uint16_t*>(B + lay.off_baseM);
-    for (uint32_t hi = s; hi < lay.nb; hi += blockDim.x) {
-        membC[(size_t)hi * lay.nt + t] = 0ull;
-        membM[(size_t)hi * lay.nt + t] = 0ull;
-    }
-    __syncthreads();
-    if (s < BP_TILE && s_valid[s]) {
-        atomicOr(&membC[(size_t)(s_g[0][s] >> 6) * lay.nt + t], 1ull << (s_g[0][s] & 63));
-        atomicOr(&membM[(size_t)(s_g[1][s] >> 6) * lay.nt + t], 1ull << (s_g[1][s] & 63));
-    }
-    __threadfence();
-    __syncthreads();
-    const uint32_t warp = s >> 5, lane = s & 31;
-    if (warp < 2) {
-        const unsigned long long* memb = warp ? membM : membC;
-        uint16_t* base = warp ? baseM : baseC;
-        uint32_t running = 0;
-        for (uint32_t h0 = 0; h0 < lay.nb; h0 += 32) {
-            const uint32_t hi = h0 + lane;
-            const uint32_t c = hi < lay.nb ? __popcll(__ldcg(&memb[(size_t)hi * lay.nt + t])) : 0;
-            uint32_t inc = c;
-#pragma unroll
-            for (int off = 1; off < 32; off <<= 1) {
-                const uint32_t o = __shfl_up_sync(0xffffffffu, inc, off);
-                if (lane >= (uint32_t)off) inc += o;
-            }
-            if (hi < lay.nb) base[(size_t)hi * lay.nt + t] = (uint16_t)(running + inc - c);
-            running += __shfl_sync(0xffffffffu, inc, 31);
-        }
-    }
-    // label-pair columns, layout [bit][tile][8 words]
-    uint8_t* pairs = B + lay.off_pairs;
-    for (uint32_t bit = s; bit < 64u * nt.W; bit += blockDim.x) {
-        const uint32_t w_ = bit >> 6, sh = bit & 63;
-        uint32_t w[8];
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-            uint32_t acc = 0;
-            for (int b = 0; b < 32; b++) acc |= (uint32_t)((s_lab[w_][j * 32 + b] >> sh) & 1ull) << b;
-            w[j] = acc;
-        }
-        uint4* dst = reinterpret_cast<uint4*>(pairs + (size_t)bit * lay.pstride + (size_t)t * 32);
-        dst[0] = make_uint4(w[0], w[1], w[2], w[3]);
-        dst[1] = make_uint4(w[4], w[5], w[6], w[7]);
-    }
-}
-
-// ---- "rows" format (ks_bitpar.h): one CTA builds one 256-slot tile of a column block, node-index order ----
-// Also leaves the tile's global positions in ascending order (tile_sorted) for k_build_ranks.
-__global__ void __launch_bounds__(288)
-    k_build_cbtile(NodeTable nt, const uint32_t* __restrict__ gposC, const uint32_t* __restrict__ gposM,
-                   uint8_t* __restrict__ blob, RowsLayout lay, uint32_t* __restrict__ tile_sorted) {
-    __shared__ uint32_t s_g[2][BP_TILE];
-    __shared__ uint16_t s_lr[2][BP_TILE];
-    __shared__ uint8_t s_valid[BP_TILE];
-    __shared__ uint64_t s_lab[KS_MAX_LABEL_WORDS][BP_TILE];
-    const uint32_t tile_g = blockIdx.x, cb = tile_g / RW_TILES, t = tile_g % RW_TILES, s = threadIdx.x;
-    const uint32_t n_tiles_pad = lay.ncb * RW_TILES;
-    uint8_t* B = blob + (size_t)cb * lay.cb_stride;
-    if (s < BP_TILE) {
-        const uint32_t n = tile_g * BP_TILE + s;
-        const bool v = n < nt.N;
-        s_valid[s] = v;
-        s_g[0][s] = v ? gposC[n] : 0xFFFFFFFFu;
-        s_g[1][s] = v ? gposM[n] : 0xFFFFFFFFu;
-        for (uint32_t w = 0; w < nt.W; w++) s_lab[w][s] = v ? nt.labels[(size_t)w * nt.Npad + n] : 0ull;
-    }
-    __syncthreads();
-    if (s < BP_TILE) {
-        for (int r = 0; r < 2; r++) {
-            const uint32_t g = s_g[r][s];
-            uint32_t c = 0;
-            for (int k = 0; k < BP_TILE; k++) c += s_g[r][k] < g;
-            s_lr[r][s] = (uint16_t)c;
             // positions are distinct, so the valid slots fill tile_sorted[0..count) exactly; the rest is +inf
-            uint32_t* ts = tile_sorted + ((size_t)r * n_tiles_pad + tile_g) * BP_TILE;
-            if (s_valid[s]) ts[c] = g;
-            const uint32_t count = nt.N > tile_g * BP_TILE ? min((uint32_t)BP_TILE, nt.N - tile_g * BP_TILE) : 0u;
-            if (s >= count) ts[s] = 0xFFFFFFFFu;
+            if (tile_sorted) {
+                uint32_t* ts = tile_sorted + ((size_t)r * n_tiles_pad + tile_g) * BP_TILE;
+                if (s_valid[s]) ts[c] = g;
+                const uint32_t count = nt.N > tile_g * BP_TILE ? min((uint32_t)BP_TILE, nt.N - tile_g * BP_TILE) : 0u;
+                if (s >= count) ts[s] = 0xFFFFFFFFu;
+            }
         }
     }
     __syncthreads();
@@ -397,6 +295,39 @@ __global__ void __launch_bounds__(288)
             uint8_t* line = B + (r ? lay.off_tabM : lay.off_tabC) + (size_t)s * RW_LINE + t * 32;
             *reinterpret_cast<uint4*>(line) = make_uint4(w[0], w[1], w[2], w[3]);
             *reinterpret_cast<uint4*>(line + 16) = make_uint4(w[4], w[5], w[6], w[7]);
+        }
+    }
+    // bucket membership + base counts of this tile's column
+    if (bk.base[0] && tile_g < lay.n_tiles) {
+        const uint32_t nb = (nt.N >> 6) + 1;
+        for (uint32_t hi = s; hi < nb; hi += blockDim.x) {
+            bk.memb[0][(size_t)hi * lay.n_tiles + tile_g] = 0ull;
+            bk.memb[1][(size_t)hi * lay.n_tiles + tile_g] = 0ull;
+        }
+        __syncthreads();
+        if (s < BP_TILE && s_valid[s]) {
+            atomicOr(&bk.memb[0][(size_t)(s_g[0][s] >> 6) * lay.n_tiles + tile_g], 1ull << (s_g[0][s] & 63));
+            atomicOr(&bk.memb[1][(size_t)(s_g[1][s] >> 6) * lay.n_tiles + tile_g], 1ull << (s_g[1][s] & 63));
+        }
+        __threadfence();
+        __syncthreads();
+        const uint32_t warp = s >> 5, lane = s & 31;
+        if (warp < 2) {
+            const unsigned long long* memb = warp ? bk.memb[1] : bk.memb[0];
+            uint16_t* base = warp ? bk.base[1] : bk.base[0];
+            uint32_t running = 0;
+            for (uint32_t h0 = 0; h0 < nb; h0 += 32) {
+                const uint32_t hi = h0 + lane;
+                const uint32_t c = hi < nb ? __popcll(__ldcg(&memb[(size_t)hi * lay.n_tiles + tile_g])) : 0;
+                uint32_t inc = c;
+#pragma unroll
+                for (int off = 1; off < 32; off <<= 1) {
+                    const uint32_t o = __shfl_up_sync(0xffffffffu, inc, off);
+                    if (lane >= (uint32_t)off) inc += o;
+                }
+                if (hi < nb) base[(size_t)hi * lay.n_tiles + tile_g] = (uint16_t)(running + inc - c);
+                running += __shfl_sync(0xffffffffu, inc, 31);
+            }
         }
     }
     // label-pair columns
@@ -849,36 +780,44 @@ struct PodThreshold {
     unsigned long long lowC, lowM;
 };
 
-__device__ __forceinline__ PodThreshold pod_threshold(const uint8_t* __restrict__ blobP, const BitparLayout& lay, uint2 r) {
+// tile-local ranks through the bucket arrays of the index's order (TileBuckets, ks_bitpar.h)
+__device__ __forceinline__ PodThreshold pod_threshold(const TileBuckets& bk, const RowsLayout& lay, uint2 r) {
     PodThreshold t;
-    t.baseC = reinterpret_cast<const uint16_t*>(blobP + lay.off_baseC) + (size_t)(r.x >> 6) * lay.nt;
-    t.baseM = reinterpret_cast<const uint16_t*>(blobP + lay.off_baseM) + (size_t)(r.y >> 6) * lay.nt;
-    t.membC = reinterpret_cast<const unsigned long long*>(blobP + lay.off_membC) + (size_t)(r.x >> 6) * lay.nt;
-    t.membM = reinterpret_cast<const unsigned long long*>(blobP + lay.off_membM) + (size_t)(r.y >> 6) * lay.nt;
+    t.baseC = bk.base[0] + (size_t)(r.x >> 6) * lay.n_tiles;
+    t.baseM = bk.base[1] + (size_t)(r.y >> 6) * lay.n_tiles;
+    t.membC = bk.memb[0] + (size_t)(r.x >> 6) * lay.n_tiles;
+    t.membM = bk.memb[1] + (size_t)(r.y >> 6) * lay.n_tiles;
     t.lowC = (1ull << (r.x & 63)) - 1ull;
     t.lowM = (1ull << (r.y & 63)) - 1ull;
     return t;
 }
 
+// the pod's tile-local ranks (cpu, memory) in tile k
+__device__ __forceinline__ uint2 tile_ranks(const PodThreshold& t, uint32_t k) {
+    return make_uint2(__ldg(t.baseC + k) + __popcll(__ldg(t.membC + k) & t.lowC),
+                      __ldg(t.baseM + k) + __popcll(__ldg(t.membM + k) & t.lowM));
+}
+
+// feasibility mask of tile k of a column-block index for one pod, from its tile-local ranks
 template <int W>
-__device__ __forceinline__ void ptile_mask(const uint8_t* __restrict__ blobP, const BitparLayout& lay, const PodThreshold& t,
+__device__ __forceinline__ void ptile_mask(const uint8_t* __restrict__ blob, const RowsLayout& lay, uint2 rank,
                                            const unsigned long long (&sel)[W], uint32_t k, uint32_t (&m)[8]) {
-    const uint32_t rankC = __ldg(t.baseC + k) + __popcll(__ldg(t.membC + k) & t.lowC);
-    const uint32_t rankM = __ldg(t.baseM + k) + __popcll(__ldg(t.membM + k) & t.lowM);
-    const uint4* tc = reinterpret_cast<const uint4*>(blobP + lay.off_tabC + table_row_offset(k, rankC));
-    const uint4* tm = reinterpret_cast<const uint4*>(blobP + lay.off_tabM + table_row_offset(k, rankM));
+    const uint8_t* cbp = blob + (size_t)(k / RW_TILES) * lay.cb_stride; // the tile's column block
+    const uint32_t t32 = (k % RW_TILES) * 32;                          // the tile's bytes in every line of it
+    const uint4* tc = reinterpret_cast<const uint4*>(cbp + (lay.off_tabC + rank.x * RW_LINE + t32));
+    const uint4* tm = reinterpret_cast<const uint4*>(cbp + (lay.off_tabM + rank.y * RW_LINE + t32));
     const uint4 c0 = __ldg(tc), c1 = __ldg(tc + 1);
     const uint4 m0 = __ldg(tm), m1 = __ldg(tm + 1);
     m[0] = c0.x & m0.x; m[1] = c0.y & m0.y; m[2] = c0.z & m0.z; m[3] = c0.w & m0.w;
     m[4] = c1.x & m1.x; m[5] = c1.y & m1.y; m[6] = c1.z & m1.z; m[7] = c1.w & m1.w;
-    const uint8_t* pairs = blobP + lay.off_pairs;
+    const uint8_t* pairs = cbp + (lay.off_pairs + t32);
 #pragma unroll
     for (int w = 0; w < W; w++) {
         unsigned long long bits = sel[w];
         while (bits) {
             const uint32_t bit = w * 64 + __ffsll((long long)bits) - 1;
             bits &= bits - 1;
-            const uint4* col = reinterpret_cast<const uint4*>(pairs + (size_t)bit * lay.pstride + (size_t)k * 32);
+            const uint4* col = reinterpret_cast<const uint4*>(pairs + (size_t)bit * RW_LINE);
             const uint4 q0 = __ldg(col);
             const uint4 q1 = __ldg(col + 1);
             m[0] &= q0.x; m[1] &= q0.y; m[2] &= q0.z; m[3] &= q0.w;
@@ -915,7 +854,7 @@ constexpr uint32_t FF_HEAD_TILES = 2;
 
 template <int W>
 __global__ void __launch_bounds__(256)
-    k_first_fit_head(const uint8_t* __restrict__ blobP, BitparLayout lay, const int32_t* __restrict__ ord_idx,
+    k_first_fit_head(const uint8_t* __restrict__ blobP, TileBuckets bk, RowsLayout lay, const int32_t* __restrict__ ord_idx,
                      const int64_t* __restrict__ ord_prio, PodView pv, const uint2* __restrict__ rk, OutView ov,
                      uint32_t* __restrict__ tail_list, uint32_t* __restrict__ tail_count, PeerOut po, bool last_kernel,
                      const unsigned long long* __restrict__ live, uint32_t N) {
@@ -924,7 +863,7 @@ __global__ void __launch_bounds__(256)
     if (threadIdx.x == 0) trace_start(TR_ARGMAX1_START);
     if (p < pv.P) {
         const uint2 r = __ldg(rk + p);
-        const PodThreshold t = pod_threshold(blobP, lay, r);
+        const PodThreshold t = pod_threshold(bk, lay, r);
         unsigned long long sel[W];
         bool dead = r.x >= N || r.y >= N; // the request exceeds every node's free cpu / memory
 #pragma unroll
@@ -936,14 +875,17 @@ __global__ void __launch_bounds__(256)
             write_binding(ov, pv, po, p, -1, ord_idx, ord_prio);
         } else {
         uint32_t m0[8], m1[8];
-        ptile_mask<W>(blobP, lay, t, sel, 0, m0);
-        ptile_mask<W>(blobP, lay, t, sel, min(1u, lay.nt - 1), m1);
+        const uint32_t k1 = min(1u, lay.n_tiles - 1);
+        // both tiles' bucket words first: their table rows are then requested together, one load round after them
+        const uint2 r0 = tile_ranks(t, 0), r1 = tile_ranks(t, k1);
+        ptile_mask<W>(blobP, lay, r0, sel, 0, m0);
+        ptile_mask<W>(blobP, lay, r1, sel, k1, m1);
         int slot = first_bit_256(m0);
-        if (slot < 0 && lay.nt > 1) {
+        if (slot < 0 && lay.n_tiles > 1) {
             const int s1 = first_bit_256(m1);
             if (s1 >= 0) slot = BP_TILE + s1;
         }
-        if (slot >= 0 || lay.nt <= FF_HEAD_TILES) write_binding(ov, pv, po, p, slot, ord_idx, ord_prio);
+        if (slot >= 0 || lay.n_tiles <= FF_HEAD_TILES) write_binding(ov, pv, po, p, slot, ord_idx, ord_prio);
         else tail_list[atomicAdd(tail_count, 1u)] = p; // order of the list does not affect any result
         }
     }
@@ -956,7 +898,7 @@ __global__ void __launch_bounds__(256)
 
 template <int W>
 __global__ void __launch_bounds__(256)
-    k_first_fit_tail(const uint8_t* __restrict__ blobP, BitparLayout lay, const int32_t* __restrict__ ord_idx,
+    k_first_fit_tail(const uint8_t* __restrict__ blobP, TileBuckets bk, RowsLayout lay, const int32_t* __restrict__ ord_idx,
                      const int64_t* __restrict__ ord_prio, PodView pv, const uint2* __restrict__ rk, OutView ov,
                      const uint32_t* __restrict__ tail_list, const uint32_t* __restrict__ tail_count, PeerOut po) {
     const uint32_t lane = threadIdx.x & 31;
@@ -966,17 +908,17 @@ __global__ void __launch_bounds__(256)
     if (threadIdx.x == 0) trace_start(TR_ARGMAX2_START);
     for (uint32_t i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < n; i += warps) {
         const uint32_t p = tail_list[i];
-        const PodThreshold t = pod_threshold(blobP, lay, __ldg(rk + p));
+        const PodThreshold t = pod_threshold(bk, lay, __ldg(rk + p));
         unsigned long long sel[W];
 #pragma unroll
         for (int w = 0; w < W; w++) sel[w] = __ldg(pv.sel + (size_t)p * W + w);
         int slot = -1;
-        for (uint32_t k0 = FF_HEAD_TILES; k0 < lay.nt; k0 += 32) {
+        for (uint32_t k0 = FF_HEAD_TILES; k0 < lay.n_tiles; k0 += 32) {
             const uint32_t k = k0 + lane;
             int s = -1;
-            if (k < lay.nt) {
+            if (k < lay.n_tiles) {
                 uint32_t m[8];
-                ptile_mask<W>(blobP, lay, t, sel, k, m);
+                ptile_mask<W>(blobP, lay, tile_ranks(t, k), sel, k, m);
                 s = first_bit_256(m);
             }
             const uint32_t b = __ballot_sync(0xffffffffu, s >= 0);
@@ -1081,7 +1023,7 @@ constexpr uint32_t LA_FIRST_WINDOW = 8;  // tiles of the first window (then 32 p
 
 template <int W>
 __global__ void __launch_bounds__(256)
-    k_least_alloc(const uint8_t* __restrict__ blobL, BitparLayout lay, const NodeEval* __restrict__ ev,
+    k_least_alloc(const uint8_t* __restrict__ blobL, TileBuckets bk, RowsLayout lay, const NodeEval* __restrict__ ev,
                   const float4* __restrict__ hint, const int64_t* __restrict__ ordL_s0, const int32_t* __restrict__ ordL_idx, PodView pv,
                   const uint2* __restrict__ rk, OutView ov, PeerOut po, const unsigned long long* __restrict__ live, uint32_t N) {
     const longlong2 amax = *reinterpret_cast<const longlong2*>(live + KS_MAX_LABEL_WORDS); // max allocatable cpu / memory
@@ -1094,7 +1036,7 @@ __global__ void __launch_bounds__(256)
     if (threadIdx.x == 0) trace_start(TR_ARGMAX1_START);
     for (uint32_t p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); p < pv.P; p += warps) {
         const uint2 r = __ldg(rk + p);
-        const PodThreshold t = pod_threshold(blobL, lay, r);
+        const PodThreshold t = pod_threshold(bk, lay, r);
         unsigned long long sel[W];
         bool dead = r.x >= N || r.y >= N; // the request exceeds every node's free cpu / memory
 #pragma unroll
@@ -1121,14 +1063,14 @@ __global__ void __launch_bounds__(256)
         // there whenever it would have fired in front of an empty tile before it.
         uint32_t k0 = 0, win = LA_FIRST_WINDOW;
         bool done = dead;
-        while (!done && k0 < lay.nt) {
+        while (!done && k0 < lay.n_tiles) {
             if (k0 > 0 && bounded && bidx >= 0 && best > __ldg(ordL_s0 + (size_t)k0 * BP_TILE) - D) break; // warp-uniform
             {
                 uint32_t m[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
                 int64_t top = INT64_MIN;
                 const uint32_t kt = k0 + lane;
-                if (lane < win && kt < lay.nt) {
-                    ptile_mask<W>(blobL, lay, t, sel, kt, m);
+                if (lane < win && kt < lay.n_tiles) {
+                    ptile_mask<W>(blobL, lay, tile_ranks(t, kt), sel, kt, m);
                     top = __ldg(ordL_s0 + (size_t)kt * BP_TILE);
                 }
                 s_mask[wid][lane][0] = make_uint4(m[0], m[1], m[2], m[3]);
@@ -1235,39 +1177,8 @@ __global__ void __launch_bounds__(256)
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-static uint32_t round16(uint32_t x) { return (x + 15u) & ~15u; }
-
-static uint64_t per_tile_bytes(uint32_t nb, uint32_t W) {
-    return (uint64_t)nb * 20 + 2ull * BP_TABLE_BYTES + 64ull * W * 32 + 64ull * W * 16; // last term: pair-column skew
-    // (tables are allocated per quad of tiles: make_layout_smem re-checks the exact blob size)
-}
-
-static bool fill_offsets(BitparLayout* lay, uint32_t W) {
-    const uint64_t nb = lay->nb, nt = lay->nt;
-    if (per_tile_bytes(lay->nb, W) * nt + 1024 > 0xF0000000ull) return false;
-    uint32_t off = 0;
-    lay->off_baseC = off;
-    off += round16((uint32_t)(nb * nt * 2));
-    lay->off_baseM = off;
-    off += round16((uint32_t)(nb * nt * 2));
-    lay->off_membC = off;
-    off += round16((uint32_t)(nb * nt * 8));
-    lay->off_membM = off;
-    off += round16((uint32_t)(nb * nt * 8));
-    off = (off + 127u) & ~127u; // table lines are 128 bytes
-    lay->off_tabC = off;
-    off += table_area_bytes((uint32_t)nt);
-    lay->off_tabM = off;
-    off += table_area_bytes((uint32_t)nt);
-    lay->off_pairs = off;
-    lay->pstride = pair_stride((uint32_t)nt);
-    off += 64u * W * lay->pstride;
-    lay->blob_bytes = (off + 127u) & ~127u;
-    return true;
-}
-
-// "rows" format (ks_bitpar.h): column blocks of RW_TILES tiles; the pair columns are staged with the tables when
-// everything fits in shared memory (W <= 4), else they are read through L1/L2
+// The column-block format (ks_bitpar.h) of all three indexes: column blocks of RW_TILES tiles; the mask kernel stages the
+// pair columns with the tables when everything fits in shared memory (W <= 4), else it reads them through L1/L2
 static bool make_layout_rows(uint32_t N, uint32_t W, RowsLayout* lay) {
     const uint32_t n_tiles = (N + BP_TILE - 1) / BP_TILE;
     if (n_tiles == 0) return false;
@@ -1281,16 +1192,24 @@ static bool make_layout_rows(uint32_t N, uint32_t W, RowsLayout* lay) {
     lay->pairs_smem = lay->cb_stride <= (uint32_t)BP_SMEM_MAX - 1024u ? 1u : 0u;
     lay->smem_bytes = lay->pairs_smem ? lay->cb_stride : 2 * RW_TAB_BYTES;
     lay->n_thr = N + 1;
-    // rank tables: 2 x ncb x (N+1) x 16 B; beyond 4 GB the per-cell kernel serves the snapshot
+    // rank tables: 2 x ncb x (N+1) x 16 B; beyond 4 GB (N >= 2^19) the per-cell kernel serves the snapshot.  The largest
+    // index this admits (N = 2^19 - 1, W = 8) has 64 MB blobs and 320 MB of bucket arrays per order.
     return (uint64_t)lay->ncb * lay->n_thr * RW_TILES * 2ull * 2ull <= (4ull << 30);
 }
 
-// flat layout for the priority-ordered index (global memory, all tiles in one blob)
-static bool make_layout_flat(uint32_t N, uint32_t W, BitparLayout* lay) {
-    lay->nb = (N >> 6) + 1;
-    lay->ncb = 1;
-    lay->nt = (N + BP_TILE - 1) / BP_TILE;
-    return lay->nt > 0 && fill_offsets(lay, W);
+// The bucket arrays of an ordered index in one block (TileBuckets): base [resource][bucket][tile] u16, then memb
+// [resource][bucket][tile] u64, rows of n_tiles entries (no argmax kernel reads a padding tile).  Returns the block's
+// size; given the block, also sets *bk to the arrays in it.
+static size_t tile_buckets(void* block, uint32_t N, const RowsLayout& lay, TileBuckets* bk) {
+    const size_t n = ((size_t)(N >> 6) + 1) * lay.n_tiles;
+    BlockLayout L;
+    const size_t o_base = L.take<uint16_t>(2 * n), o_memb = L.take<unsigned long long>(2 * n);
+    if (block)
+        for (int r = 0; r < 2; r++) {
+            bk->base[r] = at<uint16_t>(block, o_base) + r * n;
+            bk->memb[r] = at<unsigned long long>(block, o_memb) + r * n;
+        }
+    return L.size;
 }
 
 BitparIndex::~BitparIndex() {
@@ -1346,46 +1265,43 @@ cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cu
         ix.ordL_idx.as<int32_t>());
     g_launches += 4;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    BitparLayout lay{}, layP{};
-    if (!make_layout_flat(nt.N, nt.W, &layP)) return cudaSuccess; // direct path only
-    for (DevBuf* b : {&ix.blobP, &ix.blobL})
-        if ((e = b->ensure(layP.blob_bytes)) != cudaSuccess) return e;
-    {
-        RowsLayout lr{};
-        if (!make_layout_rows(nt.N, nt.W, &lr)) return cudaSuccess; // direct path only
-        const size_t need = (size_t)lr.ncb * lr.cb_stride;
-        if ((e = ix.blobR.ensure(need)) != cudaSuccess) return e;
-        const size_t need_rank = (size_t)lr.ncb * lr.n_thr * 2 * (RW_TILES / 2); // u32 tile pairs
-        if ((e = ix.rank.ensure(need_rank * sizeof(uint32_t))) != cudaSuccess) return e;
-        // one work cursor per column block (k_mask_rows)
-        if ((e = ix.cursor.ensure((size_t)lr.ncb * RW_CURSOR_STRIDE * sizeof(uint32_t))) != cudaSuccess) return e;
-        const size_t need_ts = 2ull * lr.ncb * RW_TILES * BP_TILE;
-        if ((e = ix.tile_sorted.ensure(need_ts * sizeof(uint32_t))) != cudaSuccess) return e;
-        k_build_cbtile<<<lr.ncb * RW_TILES, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(),
-                                                          ix.blobR.as<uint8_t>(), lr, ix.tile_sorted.as<uint32_t>());
-        g_launches++;
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        k_build_ranks<<<dim3((lr.n_thr + 255) / 256, lr.ncb), 256, 0, st>>>(ix.tile_sorted.as<uint32_t>(), lr,
-                                                                             ix.rank.as<uint32_t>());
-        g_launches++;
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        ix.lay_r = lr;
-        lay.nt = RW_TILES; // bitpar_profitable: (pod, tile) items
-        lay.ncb = lr.ncb;
-    }
-    k_build_tile<<<layP.nt, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(), ix.ord_idx.as<int32_t>(),
-                                          ix.blobP.as<uint8_t>(), layP);
+    RowsLayout lay{};
+    if (!make_layout_rows(nt.N, nt.W, &lay)) return cudaSuccess; // direct path only
+    for (DevBuf* b : {&ix.blobR, &ix.blobP, &ix.blobL})
+        if ((e = b->ensure((size_t)lay.ncb * lay.cb_stride)) != cudaSuccess) return e;
+    const size_t bucket_bytes = tile_buckets(nullptr, nt.N, lay, nullptr);
+    for (DevBuf* b : {&ix.bucketsP, &ix.bucketsL})
+        if ((e = b->ensure(bucket_bytes)) != cudaSuccess) return e;
+    const size_t need_rank = (size_t)lay.ncb * lay.n_thr * 2 * (RW_TILES / 2); // u32 tile pairs
+    if ((e = ix.rank.ensure(need_rank * sizeof(uint32_t))) != cudaSuccess) return e;
+    // one work cursor per column block (k_mask_rows)
+    if ((e = ix.cursor.ensure((size_t)lay.ncb * RW_CURSOR_STRIDE * sizeof(uint32_t))) != cudaSuccess) return e;
+    const size_t need_ts = 2ull * lay.ncb * RW_TILES * BP_TILE;
+    if ((e = ix.tile_sorted.ensure(need_ts * sizeof(uint32_t))) != cudaSuccess) return e;
+    const uint32_t tiles = lay.ncb * RW_TILES;
+    k_build_tiles<<<tiles, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(), nullptr, ix.blobR.as<uint8_t>(),
+                                         lay, ix.tile_sorted.as<uint32_t>(), TileBuckets{});
     g_launches++;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    // KS_SCORE_LEAST_ALLOCATED: the same flat index in descending order of the score bound + per-slot evaluation rows
-    k_build_tile<<<layP.nt, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(), ix.ordL_idx.as<int32_t>(),
-                                          ix.blobL.as<uint8_t>(), layP);
+    k_build_ranks<<<dim3((lay.n_thr + 255) / 256, lay.ncb), 256, 0, st>>>(ix.tile_sorted.as<uint32_t>(), lay,
+                                                                           ix.rank.as<uint32_t>());
+    g_launches++;
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    TileBuckets bk;
+    tile_buckets(ix.bucketsP.p, nt.N, lay, &bk);
+    k_build_tiles<<<tiles, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(), ix.ord_idx.as<int32_t>(),
+                                         ix.blobP.as<uint8_t>(), lay, nullptr, bk);
+    g_launches++;
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    // KS_SCORE_LEAST_ALLOCATED: the same index in descending order of the score bound + per-slot evaluation rows
+    tile_buckets(ix.bucketsL.p, nt.N, lay, &bk);
+    k_build_tiles<<<tiles, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(), ix.ordL_idx.as<int32_t>(),
+                                         ix.blobL.as<uint8_t>(), lay, nullptr, bk);
     k_build_eval<<<(Nord + 255) / 256, 256, 0, st>>>(nt, ix.ordL_idx.as<int32_t>(), Nord, ix.evalL.as<NodeEval>(),
                                                      ix.hintL.as<float4>());
     g_launches += 2;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ix.lay = lay;
-    ix.layP = layP;
+    ix.lay_r = lay;
     ix.valid = true;
     return cudaSuccess;
 }
@@ -1393,7 +1309,7 @@ cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cu
 bool bitpar_profitable(const BitparIndex& ix, uint32_t P) {
     // below ~16M cells the per-call rank pass and blob staging outweigh the per-cell kernel;
     // the mask kernel indexes (pod, tile) items with 32 bits
-    return ix.valid && (uint64_t)P * ix.N >= (1ull << 24) && (uint64_t)P * ix.lay.nt < (1ull << 31);
+    return ix.valid && (uint64_t)P * ix.N >= (1ull << 24) && (uint64_t)P * RW_TILES < (1ull << 31);
 }
 
 template <int W, int THREADS>
@@ -1442,7 +1358,7 @@ template <int W>
 static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before_mask, cudaEvent_t after_mask) {
     cudaError_t e;
     const uint32_t P = L.pv.P;
-    if ((uint64_t)P * ix.lay.nt >= (1ull << 31)) return cudaErrorInvalidValue;
+    if ((uint64_t)P * RW_TILES >= (1ull << 31)) return cudaErrorInvalidValue;
     if ((e = bitpar_prepare(ix, P)) != cudaSuccess) return e; // no-op when the caller prepared already
     const bool need_mask_pass = L.ov.mask || L.ov.cnt;
     const int sms = ix.sms;
@@ -1476,7 +1392,7 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
     const uint32_t mask_grid = (uint32_t)std::min<uint64_t>((uint64_t)mask_sms, (F + warps - 1) / warps);
     k_pod_ranks<<<rank_grid, RANK_THREADS, rank_smem, L.stream>>>(L.pv, ix.sortedC.as<int64_t>(), ix.sortedM.as<int64_t>(), ix.N,
                                                  ix.splC.as<int64_t>(), ix.splM.as<int64_t>(), ix.n_spl, ix.spl_stride,
-                                                 ix.pod_ranks.as<uint2>(), (need_mask_pass && ix.lay.ncb > 1) ? L.ov.cnt : nullptr, ix.W,
+                                                 ix.pod_ranks.as<uint2>(), (need_mask_pass && ix.lay_r.ncb > 1) ? L.ov.cnt : nullptr, ix.W,
                                                  need_mask_pass ? ix.rec_s.as<uint4>() : nullptr, ix.cursor.as<uint32_t>(),
                                                  need_mask_pass ? ix.lay_r.ncb : 0u);
     g_launches++;
@@ -1491,24 +1407,27 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
         uint32_t* tail_list = ix.tail_list.as<uint32_t>();
         uint32_t* tail_count = tail_list + P; // the list holds at most P pods
         if ((e = cudaMemsetAsync(tail_count, 0, sizeof(uint32_t), bs)) != cudaSuccess) return e;
-        if (L.policy == KS_SCORE_LEAST_ALLOCATED) {
+        const bool least_alloc = L.policy == KS_SCORE_LEAST_ALLOCATED;
+        TileBuckets bk;
+        tile_buckets(least_alloc ? ix.bucketsL.p : ix.bucketsP.p, ix.N, ix.lay_r, &bk);
+        if (least_alloc) {
             const uint32_t wpc = at / 32; // one warp per pod
             const uint32_t grid = (uint32_t)std::min<uint64_t>((uint64_t)sms * (2048 / at), ((uint64_t)P + wpc - 1) / wpc);
-            k_least_alloc<W><<<grid, at, 0, bs>>>(ix.blobL.as<uint8_t>(), ix.layP, ix.evalL.as<NodeEval>(), ix.hintL.as<float4>(),
+            k_least_alloc<W><<<grid, at, 0, bs>>>(ix.blobL.as<uint8_t>(), bk, ix.lay_r, ix.evalL.as<NodeEval>(), ix.hintL.as<float4>(),
                                                   ix.ordL_s0.as<int64_t>(), ix.ordL_idx.as<int32_t>(), L.pv, ix.pod_ranks.as<uint2>(),
                                                   L.ov, L.po, ix.live.as<unsigned long long>(), ix.N);
             g_launches++;
             if ((e = cudaGetLastError()) != cudaSuccess) return e;
         } else {
-            const bool has_tail = ix.layP.nt > FF_HEAD_TILES;
-            k_first_fit_head<W><<<(P + at - 1) / at, at, 0, bs>>>(ix.blobP.as<uint8_t>(), ix.layP, ix.ord_idx.as<int32_t>(),
+            const bool has_tail = ix.lay_r.n_tiles > FF_HEAD_TILES;
+            k_first_fit_head<W><<<(P + at - 1) / at, at, 0, bs>>>(ix.blobP.as<uint8_t>(), bk, ix.lay_r, ix.ord_idx.as<int32_t>(),
                                                                  ix.ord_prio.as<int64_t>(), L.pv, ix.pod_ranks.as<uint2>(), L.ov,
                                                                  tail_list, tail_count, L.po, !has_tail,
                                                                  ix.live.as<unsigned long long>(), ix.N);
             g_launches++;
             if ((e = cudaGetLastError()) != cudaSuccess) return e;
             if (has_tail) {
-                k_first_fit_tail<W><<<sms * (512 / at), at, 0, bs>>>(ix.blobP.as<uint8_t>(), ix.layP, ix.ord_idx.as<int32_t>(),
+                k_first_fit_tail<W><<<sms * (512 / at), at, 0, bs>>>(ix.blobP.as<uint8_t>(), bk, ix.lay_r, ix.ord_idx.as<int32_t>(),
                                                                      ix.ord_prio.as<int64_t>(), L.pv, ix.pod_ranks.as<uint2>(),
                                                                      L.ov, tail_list, tail_count, L.po);
                 g_launches++;

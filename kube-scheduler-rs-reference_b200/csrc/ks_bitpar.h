@@ -6,12 +6,14 @@
 // prefix table indexed by the tile-local rank of the threshold, and the tile-local rank is
 //   base[bucket][tile] + popc(member[bucket][tile] & lowmask)
 // (bucket = 64 consecutive global positions).  Label selectors are ANDs of per-(key,value) node columns.
-// Round 2 ("rows" kernel, the default): the tile-local rank of every possible threshold is tabulated once per
-// snapshot ([column block][threshold][tile pair] u32, read through L1/L2), row r of the 8 tiles of a column block is
-// one 256-byte line in tile order, and one pod takes 8 lanes = 256 contiguous bytes of its mask row, lane t granules
-// t and 8 + t (each store instruction writes one whole 128-byte line per pod): ~50 instructions per 256 cells.
-// KS_SCORE_LEFTOVER is separable (node part - pod part), so argmax-score is the first
-// feasible node in a static priority order: a short early-exit scan per pod (k_first_fit).
+// Three tile indexes are built per snapshot, all in the column-block format below: node order for the mask kernel
+// (k_mask_rows), descending priority order for the LEFTOVER argmax and descending score-bound order for the
+// LeastAllocated argmax.  The mask kernel takes tile-local ranks from rank tables that hold the rank of every possible
+// threshold ([column block][threshold][tile pair] u32, read through L1/L2); one pod takes 8 lanes = 256 contiguous bytes
+// of its mask row, lane t granules t and 8 + t (each store instruction writes one whole 128-byte line per pod): ~50
+// instructions per 256 cells.  The argmax kernels derive the rank with the base + popc formula from the bucket arrays of
+// their order.  KS_SCORE_LEFTOVER is separable (node part - pod part), so argmax-score is the first feasible node in a
+// static priority order: a short early-exit scan per pod (k_first_fit).
 #pragma once
 #include "ks_internal.cuh"
 
@@ -19,29 +21,21 @@ namespace ks {
 
 constexpr int BP_TILE = 256;          // nodes per tile = 8 mask words = one 32-byte row
 constexpr int BP_ROWS = BP_TILE + 1;  // prefix-table rows per tile and resource (local rank 0..256)
-constexpr int BP_TABLE_BYTES = BP_ROWS * 32;
 constexpr int BP_THREADS = 1024;
 constexpr int BP_SMEM_MAX = 232448;   // 227 KB opt-in limit per CTA
 
-struct BitparLayout { // byte offsets inside one column-block blob
-    uint32_t nt;       // tiles per column block
-    uint32_t nb;       // buckets of 64 global positions: (N >> 6) + 1
-    uint32_t ncb;      // column blocks
-    uint32_t off_baseC, off_membC, off_baseM, off_membM, off_tabC, off_tabM, off_pairs;
-    uint32_t pstride;  // bytes between two label-pair columns
-    uint32_t blob_bytes;
-};
-
-// "rows" format: column block = 8 tiles (2048 nodes).  One blob per column block:
+// Column-block format: column block = 8 tiles (2048 slots of the index's order); tile k is position k % 8 of column
+// block k / 8.  One blob per column block:
 //   tabC [257 rows][256 B], tabM [257 rows][256 B], pairs [64*W bits][256 B]
 // and every 256-byte line is [tile 0 | tile 1 | ... | tile 7] (32 B each) = 16 granules of 16 B.  Lane t of an 8-lane
 // shared-memory phase reads granule t (tile t/2) of the row of its tile's rank, then granule 8 + t (tile 4 + t/2) of
-// another row: offsets 16 t modulo 128 -> 8 distinct bank groups for any ranks.
+// another row: offsets 16 t modulo 128 -> 8 distinct bank groups for any ranks.  Tiles past the last node are built too,
+// with all-zero rows and columns.
 constexpr uint32_t RW_TILES = 8;                            // tiles per column block
 constexpr uint32_t RW_LINE = 256;                           // bytes per table row / pair column of a column block
 constexpr uint32_t RW_TAB_BYTES = (uint32_t)BP_ROWS * RW_LINE; // 65792
 
-struct RowsLayout {
+struct RowsLayout { // of all three indexes (make_layout_rows)
     uint32_t ncb;        // column blocks
     uint32_t n_tiles;    // ceil(N / 256)
     uint32_t off_tabC, off_tabM, off_pairs; // byte offsets inside a column-block blob
@@ -49,6 +43,15 @@ struct RowsLayout {
     uint32_t cb_stride;  // bytes between two column-block blobs in global memory
     uint32_t pairs_smem; // 1 = the pair columns are staged with the tables, 0 = read through L1/L2 (W = 8)
     uint32_t n_thr;      // thresholds per column block in the rank tables: N + 1
+};
+
+// The bucket arrays of one ordered index, [resource][bucket][tile] (resource 0 = cpu, 1 = memory), with (N >> 6) + 1
+// buckets of 64 global positions and n_tiles tiles (none for the padding tiles).  The tile-local rank of threshold g in
+// tile k is
+//   base[r][g >> 6][k] + popc(memb[r][g >> 6][k] & ((1 << (g & 63)) - 1)).
+struct TileBuckets {
+    uint16_t* base[2];
+    unsigned long long* memb[2];
 };
 
 // The index of one snapshot.  Device arrays (element type in brackets) are grow-only buffers, read through .as<T>().
@@ -62,22 +65,24 @@ struct BitparIndex {
     DevBuf ord_idx;   // [int32 Nord]
     DevBuf splC;      // [int64] every `spl_stride`-th element of sortedC / sortedM (<= RANK_SPLITTERS = 8192 splitters)
     DevBuf splM;
-    DevBuf blobP;     // one blob of layP.blob_bytes: priority order (tile k = priority ranks 256k..),
-                      // read through L1/L2 by k_first_fit_head / _tail
+    DevBuf blobP;     // lay_r.ncb column-block blobs in priority order (tile k = priority ranks 256k..), read through
+                      // L1/L2 by k_first_fit_head / _tail
+    DevBuf bucketsP;  // TileBuckets of blobP (tile_buckets)
     DevBuf pod_ranks; // [uint2 P] per-call scratch
     DevBuf tail_list; // [uint32 P + 1] per-call scratch: pods left for k_first_fit_tail, then the count at word P
     DevBuf ordL_s0;   // [int64 Nord] KS_SCORE_LEAST_ALLOCATED: score bound of every node in descending order (ties by index)
     DevBuf ordL_idx;  // [int32 Nord]
     DevBuf evalL;     // [NodeEval Nord] per slot of that order: what the exact score needs
     DevBuf hintL;     // [float4 Nord] per slot of that order: single-precision score model (pre-filter of k_least_alloc)
-    DevBuf blobL;     // flat index (layP) in that order
+    DevBuf blobL;     // lay_r.ncb column-block blobs in that order, read through L1/L2 by k_least_alloc
+    DevBuf bucketsL;  // TileBuckets of blobL
     DevBuf live;      // [uint64 KS_MAX_LABEL_WORDS + 2] label bits carried by at least one node, max allocatable cpu, memory
     DevBuf rec_s;     // [uint4] rows kernel: {threshold_cpu, threshold_mem, pod index, selector columns} per pod, P rounded up to 8
-    DevBuf blobR;     // rows kernel: lay_r.ncb column-block blobs
+    DevBuf blobR;     // rows kernel: lay_r.ncb column-block blobs in node order
     DevBuf rank;      // [uint32] rows kernel: [cb][threshold g][resource][j] = nodes of tile j (low 16 bits) and tile j + 4
                       // (high 16 bits) at sorted positions < g
     DevBuf tile_sorted; // [uint32] build scratch: per tile, its nodes' global positions in ascending order
-    RowsLayout lay_r{};
+    RowsLayout lay_r{}; // the layout of blobR, blobP and blobL
     DevBuf rk_hist;   // [uint32] node sample sort scratch: per order 256 bucket counts, splitters, per-node bucket / slot, lists
     DevBuf rk_spl_v;
     DevBuf rk_spl_i;
@@ -85,7 +90,6 @@ struct BitparIndex {
     DevBuf rk_loc;
     DevBuf rk_perm;
     uint32_t N = 0, Nord = 0, W = 0, spl_stride = 1, n_spl = 0;
-    BitparLayout lay{}, layP{};
     bool valid = false;
     int sms = 0;
     Stream aux; // the argmax kernels run here, overlapped with k_mask_rows

@@ -102,7 +102,9 @@ def test_random_clusters_leftover(ks, orc, path, P, N, keys):
 
 @pytest.mark.parametrize("path", list(PATHS))
 @pytest.mark.parametrize("P,N,keys", [(5, 31, 8), (257, 1025, 8), (500, 3000, 8), (64, 2500, 32), (3, 20000, 8), (4000, 9000, 8),
-                                      (300, 150_000, 8)])
+                                      (300, 150_000, 8),
+                                      (300, 2049, 16),  # one tile past a column block: the last block holds one real tile
+                                      (40, 1300, 64)])  # W = 8: k_least_alloc<8> reads the bound-order pair columns through L1/L2
 def test_random_clusters_least_allocated(ks, orc, path, P, N, keys):
     """KS_SCORE_LEAST_ALLOCATED (not separable): the per-cell kernel and the bit-parallel path (bound-ordered scan with
     early exit, k_least_alloc) against the oracle - node, score, count and mask."""
