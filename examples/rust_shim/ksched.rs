@@ -400,6 +400,37 @@ impl Gpu {
     }
 }
 
+impl Gpu {
+    /// Replica placement (a Deployment, ReplicaSet or Job scaled out; kubernetes-sigs/cluster-capacity): for each
+    /// (pod, replicas) pair, where that many copies of the pod would land placed one after another by the library's
+    /// argmax, with the earlier copies bound, and the row with the cluster's capacity for the pod.  Nothing is charged.
+    /// Returns per pair the row and the node names of the placed copies in placement order (shorter than the request
+    /// when the capacity is).  Err = the library's status (KS_ERR_NO_DEVICE on a packing-only context).
+    pub fn place_replicas(&self, specs: &[(corev1::Pod, u32)], policy: i32)
+                          -> Result<Vec<(ks_replica_plan, Vec<String>)>, i32> {
+        let pv: Vec<PodView> = specs.iter().map(|(p, _)| PodView::new(p)).collect();
+        let pobj: Vec<ks_pod_obj> = pv.iter().map(|v| unsafe { ptr::read(&v.obj) }).collect();
+        let replicas: Vec<u32> = specs.iter().map(|(_, r)| *r).collect();
+        let total: usize = replicas.iter().map(|&r| r as usize).sum();
+        let mut rows = vec![ks_replica_plan::default(); specs.len()];
+        let mut node = vec![-1i32; total];
+        let rc = unsafe {
+            ksh_place_replicas(self.ctx, pobj.as_ptr(), pobj.len() as u64, replicas.as_ptr(), policy, rows.as_mut_ptr(),
+                               node.as_mut_ptr(), ptr::null_mut())
+        };
+        if rc != KS_OK {
+            return Err(rc);
+        }
+        let mut at = 0usize;
+        Ok(rows.into_iter().zip(replicas).map(|(row, r)| {
+            let names = node[at..at + row.placed as usize].iter().map(|&n| unsafe {
+                CStr::from_ptr(ksh_context_node_name(self.ctx, n as u32)) }.to_string_lossy().into_owned()).collect();
+            at += r as usize;
+            (row, names)
+        }).collect())
+    }
+}
+
 impl Drop for Gpu {
     fn drop(&mut self) {
         unsafe { ksh_context_destroy(self.ctx) }

@@ -36,6 +36,9 @@ pub const KS_DRAIN_EXCLUDE_CANDIDATES: u32 = 1; // no candidate's node is a dest
 pub const KS_SCALEUP_MAX_NODES: u32 = 1024; // most new nodes of one template of ks_scaleup_estimate
 pub const KS_SCALEUP_MAX_PODS: u32 = 65536; // most pods of one ks_scaleup_estimate call
 pub const KS_SCALEUP_MAX_TEMPLATES: u32 = 4096; // most templates of one ks_scaleup_estimate call
+pub const KS_REPLICAS_MAX_SPECS: u32 = 4096; // most specs of one ks_place_replicas call
+pub const KS_REPLICAS_MAX: u32 = 65536; // most copies of one spec
+pub const KS_REPLICAS_MAX_TOTAL: u32 = 1 << 24; // most copies of one ks_place_replicas call
 
 #[repr(C)]
 pub struct ks_kv {
@@ -162,6 +165,16 @@ pub struct ks_scaleup_option {
     pub used_cpu: i64,
     pub used_mem: i64,
 }
+#[repr(C)]
+#[derive(Clone, Copy, Default, Debug)]
+pub struct ks_replica_plan {
+    pub capacity: u64,
+    pub placed: u32,
+    pub nodes: u32,
+    pub feasible_cnt: u32,
+    pub max_per_node: u32,
+    pub last_score: i64,
+}
 pub enum ks_snapshot {}
 pub enum ks_stream {}
 pub enum ksh_context {}
@@ -198,6 +211,8 @@ extern "C" {
     pub fn ks_scaleup_estimate(s: *mut ks_snapshot, pods: *const ks_pods, t: *const ks_node_templates,
                                out: *mut ks_scaleup_option, best: *mut i32, node: *mut i32,
                                reasons: *mut ks_pod_reasons) -> c_int;
+    pub fn ks_place_replicas(s: *mut ks_snapshot, specs: *const ks_pods, replicas: *const u32, policy: c_int,
+                             out: *mut ks_replica_plan, node: *mut i32, score: *mut i64) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -246,6 +261,8 @@ extern "C" {
                                 overhead_pods: *const ks_pod_obj, n_overhead: u64, pods: *const ks_pod_obj, n_pods: u64,
                                 out: *mut ks_scaleup_option, best: *mut i32, node: *mut i32,
                                 reasons: *mut ks_pod_reasons) -> c_int;
+    pub fn ksh_place_replicas(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, replicas: *const u32, policy: c_int,
+                              out: *mut ks_replica_plan, node: *mut i32, score: *mut i64) -> c_int;
     pub fn ksh_drain_nodes(ctx: *mut ksh_context, node_names: *const *const c_char, n: u64, pods: *const ks_pod_obj,
                            pod_offset: *const u64, policy: c_int, flags: u32, placed: *mut u32, node_idx: *mut i32) -> c_int;
     pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,

@@ -449,6 +449,51 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods /* host space */, co
                         ks_scaleup_option* out /* [n], required */, int32_t* out_best /* required */,
                         int32_t* out_node /* [n * pods->n] or NULL */, ks_pod_reasons* out_reasons /* [pods->n] or NULL */);
 
+/* ---- replica placement: where R copies of one pod spec land one after another, and how many copies the cluster holds
+ * (a Deployment, ReplicaSet or Job scaled out; kubernetes-sigs/cluster-capacity; spec extension, DESIGN.md 5h) ----
+ * Spec t is row t of `specs` with replicas[t] copies requested.  Each spec is evaluated on its own against the
+ * snapshot's current free[]; nothing is charged.  s_n(j) is the score ks_select reports for the spec on node n with j
+ * earlier copies bound there (free minus j * request), under `policy`:
+ *   1. c_n, the copies node n takes on its own: 0 unless copy 0's cell code is KS_CELL_OK, else the largest c with
+ *      c * req_cpu <= free_cpu and c * req_mem <= free_mem (unbounded when both requests are 0);
+ *   2. placement: copy r goes to the node with the highest s_n(j) among the nodes with j < c_n copies placed so far, ties
+ *      to the lower node index: ks_select run once per copy with the earlier copies bound.  placed = min(replicas[t],
+ *      sum of c_n).  Requests are >= 0, so every s_n(j) is non-increasing in j and the plan is the first `placed' of all
+ *      (node, copy) pairs ordered by score descending, node ascending, copy ascending;
+ *   3. out[t]: capacity = sum of c_n (saturating: UINT64_MAX also means unbounded), placed, nodes = distinct nodes among
+ *      the placed copies, feasible_cnt = nodes with c_n >= 1 (ks_select's feasible_cnt), max_per_node = most copies on one
+ *      node, last_score = score of copy placed - 1 (0 when nothing is placed);
+ *   4. out_node[off_t + r] / out_score[off_t + r], off_t = replicas[0] + ... + replicas[t-1]: node and score of copy r in
+ *      placement order; -1 / 0 past `placed'.  Either may be NULL; with both NULL no copy is ordered (the capacity query).
+ * To bind one spec's plan, pass its out_node slice to ks_snapshot_commit_claims with the spec's request: every claim is
+ * accepted, by construction, and free[] ends as after ks_gang_bind with one singleton group per copy.
+ * Checked on the host before any device work: KS_ERR_INVALID for a NULL argument or array, out NULL with specs->n > 0,
+ * device-space specs or a bad policy; KS_ERR_RANGE for specs->n > KS_REPLICAS_MAX_SPECS, a replicas[t] above
+ * KS_REPLICAS_MAX, a sum of replicas above KS_REPLICAS_MAX_TOTAL or a request outside [0, limit] (as ks_stream_bind: the
+ * scores are then monotone and stay inside int64).  replicas[t] = 0 fills the row and places nothing; specs->n = 0 does
+ * nothing; an empty snapshot gives capacity 0 and every copy -1.
+ * Host-space specs and outputs.  One H2D copy, a fixed sequence of kernels enqueued back to back whose number does not
+ * depend on the replicas (a scan, thirteen threshold-search passes of two kernels, the tie split and, with a copy list, one
+ * sorting CTA per spec), one D2H copy.  Staging: the snapshot's pinned block and its device input and result blocks hold
+ * the specs and n * 32 bytes of rows, plus 12 bytes per requested copy with a copy list (up to 192 MiB at
+ * KS_REPLICAS_MAX_TOTAL); its device scratch block holds the search state, plus 20 bytes per requested copy with a copy
+ * list (up to 320 MiB).  Like every staging block these grow to the largest call and are kept until
+ * ks_snapshot_destroy; ks_gang_bind, ks_drain_check, ks_stream_bind and ks_scaleup_estimate share them. */
+#define KS_REPLICAS_MAX_SPECS 4096u
+#define KS_REPLICAS_MAX 65536u
+#define KS_REPLICAS_MAX_TOTAL (1u << 24)
+typedef struct ks_replica_plan { /* 32 bytes per spec */
+    uint64_t capacity;           /* sum of c_n, saturating; UINT64_MAX also = unbounded */
+    uint32_t placed;
+    uint32_t nodes;              /* distinct nodes among the placed copies */
+    uint32_t feasible_cnt;       /* nodes with c_n >= 1 = ks_select's feasible_cnt */
+    uint32_t max_per_node;       /* most copies placed on one node */
+    int64_t last_score;          /* score of copy placed-1; 0 when placed = 0 */
+} ks_replica_plan;
+int ks_place_replicas(ks_snapshot* s, const ks_pods* specs /* host space */, const uint32_t* replicas /* [specs->n] */,
+                      int policy, ks_replica_plan* out /* [specs->n] */, int32_t* out_node /* [sum replicas] or NULL */,
+                      int64_t* out_score /* [sum replicas] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

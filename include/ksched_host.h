@@ -208,6 +208,14 @@ int ksh_scaleup_estimate(ksh_context* ctx, const ks_node_obj* templates, uint64_
                          const ks_pod_obj* overhead_pods, uint64_t n_overhead, const ks_pod_obj* pods, uint64_t n_pods,
                          ks_scaleup_option* out, int32_t* out_best, int32_t* out_node, ks_pod_reasons* out_reasons);
 
+/* Replica placement over objects (ks_place_replicas, ksched.h): spec t is pods[t] with replicas[t] copies, packed as
+ * ksh_select_nodes packs them (a selector pair no node carries maps to the never-set bit, so that spec's capacity is 0).
+ * Nothing is charged: the bound list, the store and free[] are unchanged.  Outputs as ks_place_replicas gives them
+ * (out[n] required when n > 0; out_node and out_score [sum of replicas] may be NULL; node indices map to names with
+ * ksh_context_node_name).  KS_ERR_NO_DEVICE on a packing-only context. */
+int ksh_place_replicas(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n, const uint32_t* replicas, int policy,
+                       ks_replica_plan* out, int32_t* out_node, int64_t* out_score);
+
 #ifdef __cplusplus
 }
 #endif

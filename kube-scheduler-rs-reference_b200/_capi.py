@@ -171,6 +171,22 @@ if hasattr(lib, "ks_scaleup_estimate"):  # the same for ks_scaleup_estimate
 KS_SCALEUP_MAX_NODES = 1024
 KS_SCALEUP_MAX_PODS = 65536
 KS_SCALEUP_MAX_TEMPLATES = 4096
+
+
+class ks_replica_plan(C.Structure):
+    _fields_ = [("capacity", C.c_uint64), ("placed", C.c_uint32), ("nodes", C.c_uint32), ("feasible_cnt", C.c_uint32),
+                ("max_per_node", C.c_uint32), ("last_score", C.c_int64)]
+
+
+# the same row as a numpy record
+REPLICA_PLAN_DTYPE = np.dtype([("capacity", np.uint64), ("placed", np.uint32), ("nodes", np.uint32),
+                               ("feasible_cnt", np.uint32), ("max_per_node", np.uint32), ("last_score", np.int64)])
+if hasattr(lib, "ks_place_replicas"):  # the same for ks_place_replicas
+    _proto("ks_place_replicas", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+           C.c_void_p)
+KS_REPLICAS_MAX_SPECS = 4096
+KS_REPLICAS_MAX = 65536
+KS_REPLICAS_MAX_TOTAL = 1 << 24
 KS_PREEMPT_MAX_ABS_SUM = 1 << 62
 KS_ERR_INVALID, KS_ERR_RANGE = -1, -5
 KS_REFERENCE_ATTEMPTS = 5

@@ -22,13 +22,14 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 // ks_explain, ks_select_topk, ks_preempt, ks_gang_bind, ks_drain_check and ks_scaleup_estimate are defined by the CUDA
 // core in the same library.  The references are weak so that this file still links with device stand-ins that only
 // provide the older ks_* entries (tests/native); ksh_explain_pods, ksh_rank_nodes, ksh_preempt_pods, ksh_reconcile_gangs,
-// ksh_drain_nodes and ksh_scaleup_estimate then report KS_ERR_NO_DEVICE.
+// ksh_drain_nodes, ksh_scaleup_estimate and ksh_place_replicas then report KS_ERR_NO_DEVICE.
 #pragma weak ks_explain
 #pragma weak ks_select_topk
 #pragma weak ks_preempt
 #pragma weak ks_gang_bind
 #pragma weak ks_drain_check
 #pragma weak ks_scaleup_estimate
+#pragma weak ks_place_replicas
 
 namespace {
 
@@ -1572,6 +1573,22 @@ int ksh_drain_nodes(ksh_context* c, const char* const* node_names, uint64_t n, c
     ks_pods kp{P, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     ks_drain_candidates kc{n, node.data(), pod_offset};
     return ks_drain_check(c->snap, &kp, &kc, policy, flags, out_placed, out_node_idx, nullptr);
+}
+KSH_CATCH
+
+int ksh_place_replicas(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const uint32_t* replicas, int policy,
+                       ks_replica_plan* out, int32_t* out_node, int64_t* out_score) try {
+    if (!c || (n && (!pods || !replicas || !out))) return fail(KS_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    if (!ks_place_replicas) return fail(KS_ERR_NO_DEVICE, "this library has no ks_place_replicas");
+    if (n == 0) return KS_OK;
+    std::vector<int64_t>&rc_ = c->pk_cpu, &rm_ = c->pk_mem; // the same packed batch buffers as ksh_select_nodes
+    std::vector<uint64_t>& sel = c->pk_sel;
+    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel);
+    if (rc) return rc;
+    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
+    return ks_place_replicas(c->snap, &kp, replicas, policy, out, out_node, out_score);
 }
 KSH_CATCH
 

@@ -1506,6 +1506,96 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const ks_node_templ
     return KS_OK;
 }
 
+int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* replicas, int policy, ks_replica_plan* out,
+                      int32_t* out_node, int64_t* out_score) {
+    int rc = check_pods(s, specs);
+    if (rc) return rc;
+    if (specs->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_place_replicas takes host-space specs");
+    const uint64_t T = specs->n;
+    if (T && (!replicas || !out)) return fail(KS_ERR_INVALID, "NULL replicas or out");
+    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    if (T > KS_REPLICAS_MAX_SPECS) return fail(KS_ERR_RANGE, "%llu specs (at most %u)", (unsigned long long)T, KS_REPLICAS_MAX_SPECS);
+    uint64_t total = 0;
+    for (uint64_t t = 0; t < T; t++) {
+        if (replicas[t] > KS_REPLICAS_MAX)
+            return fail(KS_ERR_RANGE, "spec %llu: %u replicas (at most %u)", (unsigned long long)t, replicas[t], KS_REPLICAS_MAX);
+        total += replicas[t];
+    }
+    if (total > KS_REPLICAS_MAX_TOTAL)
+        return fail(KS_ERR_RANGE, "%llu replicas in one call (at most %u)", (unsigned long long)total, KS_REPLICAS_MAX_TOTAL);
+    rc = check_commit_requests(T, specs->req_cpu, specs->req_mem);
+    if (rc) return rc;
+    if (T == 0) return KS_OK;
+    const bool copies = out_node || out_score;
+    if (s->N == 0) { // no node: nothing fits, every copy is -1
+        memset(out, 0, T * sizeof(ks_replica_plan));
+        if (out_node) memset(out_node, 0xff, total * 4);
+        if (out_score) memset(out_score, 0, total * 8);
+        return KS_OK;
+    }
+    const uint32_t W = s->W;
+    std::lock_guard<std::mutex> lk(s->mu);
+    CU_TRY(cudaSetDevice(s->device));
+    uint32_t n_chunks, chunk_len;
+    replica_chunks(s->N, (uint32_t)T, s->sms, &n_chunks, &chunk_len);
+    const uint64_t C = copies ? total : 0;
+    // in = [rc T | rm T | sel T*W | replicas T | offset T], results = [rows T | score C | node C],
+    // work = [search state T | chunk partials T*n_chunks | copy scores C | copy nodes C | sort indices 2C]
+    BlockLayout in, res, work;
+    const size_t i_rc = in.take<int64_t>(T), i_rm = in.take<int64_t>(T), i_sel = in.take<uint64_t>(T * W),
+                 i_rep = in.take<uint32_t>(T), i_off = in.take<uint64_t>(T);
+    const size_t o_rows = res.take<ks_replica_plan>(T), o_score = res.take<int64_t>(C), o_node = res.take<int32_t>(C);
+    const size_t w_spec = work.take<uint8_t>(replica_spec_bytes((uint32_t)T), 16),
+                 w_chunk = work.take<uint8_t>(replica_chunk_bytes((uint32_t)T, n_chunks), 16),
+                 w_score = work.take<int64_t>(C), w_node = work.take<int32_t>(C), w_sort = work.take<uint32_t>(2 * C);
+    uint8_t* h_out = nullptr;
+    rc = stage_blocks(s, in.size, res.size, &h_out);
+    if (rc) return rc;
+    CU_TRY(s->d_work.ensure(work.size));
+    uint8_t* h_in = s->h_stage.as<uint8_t>();
+    memcpy(h_in + i_rc, specs->req_cpu, T * 8);
+    memcpy(h_in + i_rm, specs->req_mem, T * 8);
+    memcpy(h_in + i_sel, specs->sel, T * 8 * W);
+    memcpy(h_in + i_rep, replicas, T * 4);
+    uint64_t* h_off = at<uint64_t>(h_in, i_off);
+    for (uint64_t t = 0, o = 0; t < T; o += replicas[t], t++) h_off[t] = o;
+    cudaStream_t st = s->stream;
+    uint8_t* d_in = s->d_in.as<uint8_t>();
+    uint8_t* d_out = s->d_out.as<uint8_t>();
+    uint8_t* d_work = s->d_work.as<uint8_t>();
+    CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
+    if (copies) { // copies past `placed' stay -1 / 0
+        CU_TRY(cudaMemsetAsync(d_out + o_score, 0, C * 8, st));
+        CU_TRY(cudaMemsetAsync(d_out + o_node, 0xff, C * 4, st));
+    }
+    ReplicaArgs a;
+    a.T = (uint32_t)T;
+    a.req_cpu = at<int64_t>(d_in, i_rc);
+    a.req_mem = at<int64_t>(d_in, i_rm);
+    a.sel = at<uint64_t>(d_in, i_sel);
+    a.replicas = at<uint32_t>(d_in, i_rep);
+    a.offset = at<uint64_t>(d_in, i_off);
+    a.rows = at<ks_replica_plan>(d_out, o_rows);
+    a.out_node = copies ? at<int32_t>(d_out, o_node) : nullptr;
+    a.out_score = copies ? at<int64_t>(d_out, o_score) : nullptr;
+    a.spec = at<RepSpec>(d_work, w_spec);
+    a.chunk = at<RepChunk>(d_work, w_chunk);
+    a.copy_node = copies ? at<int32_t>(d_work, w_node) : nullptr;
+    a.copy_score = copies ? at<int64_t>(d_work, w_score) : nullptr;
+    a.sort_buf = copies ? at<uint32_t>(d_work, w_sort) : nullptr;
+    a.n_chunks = n_chunks;
+    a.chunk_len = chunk_len;
+    cudaError_t e = launch_replicas(node_table(s), policy, a, st);
+    if (e != cudaSuccess) return fail(KS_ERR_CUDA, "replica placement launch failed: %s", cudaGetErrorString(e));
+    CU_TRY(cudaMemcpyAsync(h_out, d_out, res.size, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    memcpy(out, h_out + o_rows, T * sizeof(ks_replica_plan));
+    if (out_node) memcpy(out_node, h_out + o_node, C * 4);
+    if (out_score) memcpy(out_score, h_out + o_score, C * 8);
+    s->last_path = "replicas";
+    return KS_OK;
+}
+
 // ---------------------------------------------------------------------------------------------- async streaming
 struct StreamItem {
     uint64_t ticket;

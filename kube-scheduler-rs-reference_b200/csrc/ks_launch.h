@@ -106,6 +106,32 @@ struct ScaleupArgs {
 uint32_t scaleup_slots(uint32_t T, int sms);
 cudaError_t launch_scaleup(const PodView& pv, uint32_t W, const ScaleupArgs& a, cudaStream_t st);
 
+// replica placement (ks_place_replicas, ks_replicas.cu).  T specs, each evaluated on its own over the node table by a
+// grid of (node chunk, spec) CTAs: a scan, a fixed number of threshold-search passes, the tie split and, with the copy
+// list, one CTA per spec that sorts its copies.  Device memory.
+struct RepSpec;  // per-spec search state (ks_replicas.cu)
+struct RepChunk; // per-(spec, node chunk) partial sums
+struct ReplicaArgs {
+    uint32_t T;
+    const int64_t *req_cpu, *req_mem; // [T]
+    const uint64_t* sel;              // [T * W], row-major
+    const uint32_t* replicas;         // [T]
+    const uint64_t* offset;           // [T]: first copy of spec t in the copy list
+    ks_replica_plan* rows;            // [T]
+    int32_t* out_node;                // [sum of replicas], -1 before the call, or null (no copy list)
+    int64_t* out_score;               // [sum of replicas], 0 before the call; set exactly when out_node is
+    RepSpec* spec;                    // [T]
+    RepChunk* chunk;                  // [T * n_chunks]
+    int32_t* copy_node;               // [sum of replicas] copies in node-then-copy order, with out_node
+    int64_t* copy_score;
+    uint32_t* sort_buf;               // [2 * sum of replicas], with out_node
+    uint32_t n_chunks, chunk_len;     // node chunks per spec and nodes per chunk (a multiple of 256)
+};
+size_t replica_spec_bytes(uint32_t T);
+size_t replica_chunk_bytes(uint32_t T, uint32_t n_chunks);
+void replica_chunks(uint32_t N, uint32_t T, int sms, uint32_t* n_chunks, uint32_t* chunk_len);
+cudaError_t launch_replicas(const NodeTable& nt, int policy, const ReplicaArgs& a, cudaStream_t st);
+
 } // namespace ks
 
 namespace ks {

@@ -1,16 +1,16 @@
 // ks_scaleup.cu — scale-up estimate (ks_scaleup_estimate, include/ksched.h; DESIGN.md 5g), sm_90a.
 // Templates are independent, so each one is a CTA of k_scaleup_pack: it compacts its eligible pods in pod order, sorts
-// them by the order key with a stable LSD radix sort in its own scratch slot, and then one warp walks them through the
-// first-fit packing with the open nodes' remaining capacity in shared memory.  k_scaleup_reasons counts the per-pod
-// rejection reasons over the templates without atomics, one thread per pod.
+// them by the order key with ks_sort.cuh's stable LSD radix sort in its own scratch slot, and then one warp walks them
+// through the first-fit packing with the open nodes' remaining capacity in shared memory.  k_scaleup_reasons counts the
+// per-pod rejection reasons over the templates without atomics, one thread per pod.
 #include "ks_launch.h"
+#include "ks_sort.cuh"
 
 namespace ks {
 
 constexpr int SU_THREADS = 256; // 8 warps; the radix pass gives each thread one of the 256 digits
-constexpr int SU_WARPS = SU_THREADS / 32;
 constexpr int SU_CHUNK = 256; // templates staged in shared memory per step of k_scaleup_reasons
-static_assert(SU_THREADS == 256, "one thread per radix digit");
+static_assert(SU_THREADS == SORT_THREADS, "one thread per radix digit");
 
 // The order key of a pod for a template: req_cpu * A_m + req_mem * A_c.  Requests lie in [0, 2^36] / [0, 2^55] and
 // allocatables in [1, 2^26] / [1, 2^45] (checked on the host), so the key fits 128 bits; for an eligible pod (req <= F
@@ -29,78 +29,8 @@ __device__ __forceinline__ uint32_t su_digit(const PodView& pv, uint32_t p, int6
 struct SuShared {
     int64_t rem_cpu[KS_SCALEUP_MAX_NODES]; // remaining capacity of the open nodes, by ordinal
     int64_t rem_mem[KS_SCALEUP_MAX_NODES];
-    uint32_t hist[SU_WARPS][256]; // radix pass: per-warp digit counts, then per-warp digit cursors
-    uint32_t wsum[SU_WARPS];
+    SortShared sort; // the radix passes and the block scan
 };
-
-// Exclusive block-wide prefix sum of v; all threads get the total.  Called by the whole CTA.
-__device__ __forceinline__ uint32_t su_block_scan(uint32_t v, uint32_t* wsum, uint32_t& total) {
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t x = v;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-        const uint32_t y = __shfl_up_sync(0xffffffffu, x, off);
-        if (lane >= (uint32_t)off) x += y;
-    }
-    if (lane == 31) wsum[warp] = x;
-    __syncthreads();
-    uint32_t before = 0, all = 0;
-#pragma unroll
-    for (int w = 0; w < SU_WARPS; w++) {
-        const uint32_t c = wsum[w];
-        before += (uint32_t)w < warp ? c : 0u;
-        all += c;
-    }
-    __syncthreads(); // wsum may be reused
-    total = all;
-    return before + x - v;
-}
-
-// One stable pass of the LSD radix sort, src[0, n) -> dst[0, n), on the 8-bit digit at `shift`.  Warp w owns a
-// contiguous range of src, so the per-(digit, warp) cursors in that order give every element its stable position;
-// inside a warp, equal digits are ranked by lane.  Called by the whole CTA.
-__device__ void su_radix_pass(const PodView& pv, const uint32_t* src, uint32_t* dst, uint32_t n, uint32_t shift,
-                              int64_t ac, int64_t am, SuShared& s) {
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t per = ((n + SU_WARPS - 1) / SU_WARPS + 31) & ~31u;
-    const uint32_t lo = min(n, warp * per), hi = min(n, lo + per);
-    for (uint32_t i = threadIdx.x; i < SU_WARPS * 256; i += SU_THREADS) (&s.hist[0][0])[i] = 0;
-    __syncthreads();
-    for (uint32_t i = lo + lane; i < hi; i += 32) atomicAdd(&s.hist[warp][su_digit(pv, src[i], ac, am, shift)], 1u);
-    __syncthreads();
-    { // thread d: the cursors of digit d, warps in order
-        const uint32_t d = threadIdx.x;
-        uint32_t c[SU_WARPS], sum = 0;
-#pragma unroll
-        for (int w = 0; w < SU_WARPS; w++) {
-            c[w] = s.hist[w][d];
-            sum += c[w];
-        }
-        uint32_t total;
-        uint32_t base = su_block_scan(sum, s.wsum, total);
-#pragma unroll
-        for (int w = 0; w < SU_WARPS; w++) {
-            s.hist[w][d] = base;
-            base += c[w];
-        }
-    }
-    __syncthreads();
-    const uint32_t lt = (1u << lane) - 1u;
-    for (uint32_t i0 = lo; i0 < hi; i0 += 32) { // warp-uniform bounds
-        const uint32_t i = i0 + lane;
-        const bool valid = i < hi;
-        const uint32_t p = valid ? src[i] : 0u;
-        const uint32_t d = valid ? su_digit(pv, p, ac, am, shift) : 0xffffffffu;
-        const uint32_t peers = __match_any_sync(0xffffffffu, d);
-        const uint32_t rank = __popc(peers & lt);
-        const uint32_t pos = valid ? s.hist[warp][d] + rank : 0u;
-        __syncwarp();
-        if (valid && rank == 0) s.hist[warp][d] += __popc(peers);
-        __syncwarp();
-        if (valid) dst[pos] = p;
-    }
-    __syncthreads(); // dst is complete for the next pass
-}
 
 template <int W>
 __global__ void __launch_bounds__(SU_THREADS) k_scaleup_pack(PodView pv, ScaleupArgs a) {
@@ -128,7 +58,7 @@ __global__ void __launch_bounds__(SU_THREADS) k_scaleup_pack(PodView pv, Scaleup
                 ok &= miss == 0;
             }
             uint32_t total;
-            const uint32_t pre = su_block_scan(ok ? 1u : 0u, s.wsum, total);
+            const uint32_t pre = cta_block_scan(ok ? 1u : 0u, s.sort.wsum, total);
             if (ok) buf0[E + pre] = p;
             E += total;
         }
@@ -141,7 +71,7 @@ __global__ void __launch_bounds__(SU_THREADS) k_scaleup_pack(PodView pv, Scaleup
             const uint64_t hi = (uint64_t)(kmax >> 64), lo = (uint64_t)kmax;
             const uint32_t bits = hi ? 128u - __clzll(hi) : lo ? 64u - __clzll(lo) : 0u;
             for (uint32_t shift = 0; shift < bits; shift += 8) {
-                su_radix_pass(pv, src, dst, E, shift, ac, am, s);
+                cta_radix_pass(src, dst, E, [&](uint32_t p) { return su_digit(pv, p, ac, am, shift); }, s.sort);
                 uint32_t* x = src;
                 src = dst;
                 dst = x;

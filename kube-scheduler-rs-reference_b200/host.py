@@ -43,6 +43,7 @@ for _name, _res, _args in [
                                       C.c_size_t, _vp]),
     ("ksh_drain_nodes", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, C.c_int, C.c_uint32, _vp, _vp]),
     ("ksh_scaleup_estimate", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, C.c_uint64, _vp, C.c_uint64, _vp, _vp, _vp, _vp]),
+    ("ksh_place_replicas", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_int, _vp, _vp, _vp]),
 ]:
     _f = getattr(lib, _name)
     _f.restype = _res
@@ -190,6 +191,26 @@ class Context:
         if rc < 0:
             raise KsError(rc, "ksh_check_node_validity")
         return rc
+
+    def place_replicas(self, pods, n, replicas, policy=capi.KS_SCORE_LEFTOVER, want_nodes=True, first=0):
+        """Replica placement over objects (ksh_place_replicas): pod t asks for replicas[t] copies of itself.  Charges
+        nothing.  Returns (rows, node, score, offset) as Snapshot.place_replicas; node indices name nodes through
+        node_name()."""
+        replicas = np.ascontiguousarray(replicas, np.uint32).reshape(-1)
+        if replicas.shape[0] != n:
+            raise ValueError(f"replicas has {replicas.shape[0]} entries, pods {n}")
+        offset = np.zeros(n + 1, np.uint64)
+        np.cumsum(replicas, dtype=np.uint64, out=offset[1:])
+        rows = np.zeros(n, capi.REPLICA_PLAN_DTYPE)
+        total = int(offset[-1]) if want_nodes and int(offset[-1]) <= capi.KS_REPLICAS_MAX_TOTAL else 0
+        node = np.empty(total, np.int32) if want_nodes else None
+        score = np.empty(total, np.int64) if want_nodes else None
+        rc = lib.ksh_place_replicas(self._h, _addr(pods, first), n, replicas.ctypes.data, int(policy), rows.ctypes.data,
+                                    None if node is None else node.ctypes.data,
+                                    None if score is None else score.ctypes.data)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ksh_place_replicas")
+        return rows, node, score, offset
 
     def select_nodes(self, pods, n, policy=capi.KS_SCORE_LEFTOVER, first=0):
         idx = np.empty(n, np.int32)

@@ -260,6 +260,32 @@ class Snapshot:
             raise KsError(rc, "ks_scaleup_estimate")
         return rows, best.value, node, why
 
+    def place_replicas(self, req_cpu, req_mem, sel, replicas, policy=capi.KS_SCORE_LEFTOVER, want_nodes=True):
+        """Replica placement (ks_place_replicas): spec t (a row of req_cpu / req_mem / sel) asks for replicas[t] copies,
+        placed one at a time by ks_select's argmax with the earlier copies bound.  Nothing is charged.  Returns (rows,
+        node, score, offset): rows a capi.REPLICA_PLAN_DTYPE record array [T]; node int32 / score int64 [sum replicas],
+        spec t's copies in placement order at [offset[t], offset[t+1]) (-1 / 0 past rows['placed'][t]; both None
+        unless want_nodes); offset uint64 [T + 1]."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        t = int(pods.n)
+        replicas = np.asarray(replicas).reshape(-1)
+        if replicas.shape[0] != t:
+            raise ValueError(f"replicas has {replicas.shape[0]} entries, specs {t}")
+        if t and (replicas.min() < 0 or replicas.max() > 0xFFFFFFFF):
+            raise ValueError("replicas must lie in [0, 2^32)")
+        replicas = _c(replicas, np.uint32)
+        offset = np.zeros(t + 1, np.uint64)
+        np.cumsum(replicas, dtype=np.uint64, out=offset[1:])
+        rows = np.zeros(t, capi.REPLICA_PLAN_DTYPE)
+        total = int(offset[-1]) if want_nodes and int(offset[-1]) <= capi.KS_REPLICAS_MAX_TOTAL else 0
+        node = np.empty(total, np.int32) if want_nodes else None
+        score = np.empty(total, np.int64) if want_nodes else None
+        rc = lib.ks_place_replicas(self._h, C.byref(pods), _ptr(replicas), int(policy), _ptr(rows), _ptr(node),
+                                   _ptr(score))
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ks_place_replicas")
+        return rows, node, score, offset
+
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
         """The reference's own policy (src/main.rs:49-71), seeded: (node_idx, attempts_used, draw_node, draw_code)."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
