@@ -47,6 +47,17 @@ extern "C" {
 /* score policies (spec extension — the reference has no score; DESIGN.md "Score") */
 #define KS_SCORE_LEFTOVER 0        /* (free_cpu-req_cpu)*2^22 + (free_mem-req_mem); separable => static node order */
 #define KS_SCORE_LEAST_ALLOCATED 1 /* ((free_cpu-req_cpu)*100/alloc_cpu + (free_mem-req_mem)*100/alloc_mem)/2, floor */
+/* 2 is reserved and rejected as a policy. */
+/* KS_SCORE_MOST_ALLOCATED: bin-packing, upstream NodeResourcesFit's MostAllocated strategy with weights 1 and 1.  Per
+ * resource, with allocatable A, free f and request q:
+ *   term(f, A, q) = A > 0 ? clamp(A - (f - q), 0, A) * 100 / A : 0     (int64, truncating division of a value >= 0)
+ *   score         = (term(free_cpu, alloc_cpu, req_cpu) + term(free_mem, alloc_mem, req_mem)) / 2,   in [0, 100]
+ * A - (f - q) is upstream's `requested` (the bound pods' requests plus this pod's); upstream clamps it to A, and the
+ * lower clamp covers free > allocatable, which negative bound requests or releases can leave here.  Like
+ * KS_SCORE_LEAST_ALLOCATED, pods without requests are scored as requesting 0: upstream's non-zero defaults (100m CPU,
+ * 200 MB memory) are not added.  Every call that takes a policy takes this one, and ks_select runs it on both kernel
+ * paths; its bit-parallel order is built on the first call that needs it after each snapshot change. */
+#define KS_SCORE_MOST_ALLOCATED 3
 
 /* where caller-owned buffers live */
 #define KS_MEM_HOST 0
@@ -55,7 +66,7 @@ extern "C" {
 /* ks_select flags */
 #define KS_SELECT_AUTO 0u
 #define KS_SELECT_FORCE_DIRECT 1u  /* per-cell kernel (any policy) */
-#define KS_SELECT_FORCE_BITPAR 2u  /* bit-parallel kernel (KS_SCORE_LEFTOVER only) */
+#define KS_SELECT_FORCE_BITPAR 2u  /* bit-parallel kernel (any policy) */
 #define KS_SELECT_TIMING 4u        /* record CUDA events around each kernel; read with ks_last_timings */
 #define KS_SELECT_NO_GRAPH 8u      /* all-device calls are replayed from a cached CUDA graph; this disables it */
 
@@ -293,7 +304,8 @@ int ks_explain(ks_snapshot* s, const ks_pods* pods, ks_pod_reasons* out, int32_t
  * under `policy`, score descending, ties to the lower node index: the total order ks_select uses, so entry 0 of every
  * row is ks_select's node_idx / score for that pod and policy (on either kernel path) and out_feasible_cnt is its
  * feasible_cnt.  Slots past the feasible count hold node -1 and score 0.  Scores are the values ks_select reports
- * (LEFTOVER: (free_cpu-req_cpu)*2^22 + (free_mem-req_mem); LEAST_ALLOCATED: the integer-floor formula above).  Padding
+ * (LEFTOVER: (free_cpu-req_cpu)*2^22 + (free_mem-req_mem); LEAST_ALLOCATED, MOST_ALLOCATED: the integer-floor formulas
+ * above).  Padding
  * nodes never appear, and nothing is charged: the snapshot is not changed.
  * KS_ERR_RANGE when k = 0 or k > KS_TOPK_MAX; KS_ERR_INVALID for a bad policy or out_space, or a NULL out_node_idx with
  * pods->n > 0.  pods->n = 0 does nothing; an empty snapshot gives every row -1 / 0 and count 0. */
@@ -458,8 +470,11 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods /* host space */, co
  *      c * req_cpu <= free_cpu and c * req_mem <= free_mem (unbounded when both requests are 0);
  *   2. placement: copy r goes to the node with the highest s_n(j) among the nodes with j < c_n copies placed so far, ties
  *      to the lower node index: ks_select run once per copy with the earlier copies bound.  placed = min(replicas[t],
- *      sum of c_n).  Requests are >= 0, so every s_n(j) is non-increasing in j and the plan is the first `placed' of all
- *      (node, copy) pairs ordered by score descending, node ascending, copy ascending;
+ *      sum of c_n).  Requests are >= 0, so under LEFTOVER and LEAST_ALLOCATED every s_n(j) is non-increasing in j and
+ *      the plan is the first `placed' of all (node, copy) pairs ordered by score descending, node ascending, copy
+ *      ascending.  Under MOST_ALLOCATED every s_n(j) is non-decreasing in j: the node being filled never loses to a node
+ *      not yet touched, so the plan fills the nodes one after another in order of s_n(0) descending, node ascending,
+ *      each with up to c_n copies, and the copies of one node are contiguous in placement order;
  *   3. out[t]: capacity = sum of c_n (saturating: UINT64_MAX also means unbounded), placed, nodes = distinct nodes among
  *      the placed copies, feasible_cnt = nodes with c_n >= 1 (ks_select's feasible_cnt), max_per_node = most copies on one
  *      node, last_score = score of copy placed - 1 (0 when nothing is placed);

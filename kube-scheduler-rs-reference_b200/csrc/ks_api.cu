@@ -95,7 +95,9 @@ static int check_range_and_prio(ks_snapshot* s, cudaStream_t st) {
     return KS_OK;
 }
 
-static bool valid_policy(int policy) { return policy == KS_SCORE_LEFTOVER || policy == KS_SCORE_LEAST_ALLOCATED; }
+static bool valid_policy(int policy) {
+    return policy == KS_SCORE_LEFTOVER || policy == KS_SCORE_LEAST_ALLOCATED || policy == KS_SCORE_MOST_ALLOCATED;
+}
 static bool valid_space(int32_t space) { return space == KS_MEM_HOST || space == KS_MEM_DEVICE; }
 static bool valid_label_words(uint32_t W) { return W == 1 || W == 2 || W == 4 || W == 8; }
 // inside +-2^36 millicores / +-2^55 bytes, the range that keeps every score inside int64
@@ -585,6 +587,7 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
         PartialView part{nullptr, nullptr, nullptr};
         if (use_bitpar) {
             cudaError_t e = bitpar_prepare(s->bp, L.pv.P);
+            if (e == cudaSuccess && policy == KS_SCORE_MOST_ALLOCATED) e = bitpar_prepare_most(s->bp, L.nt, st);
             if (e != cudaSuccess) return fail(KS_ERR_CUDA, "bit-parallel prepare failed: %s", cudaGetErrorString(e));
         } else {
             grid = direct_grid(s->W, L.pv.P, s->Npad, s->sms);

@@ -15,9 +15,11 @@
 //                                   per pod; counts by shuffle + one RED per pod and column block
 //                  k_first_fit_head/_tail  argmax KS_SCORE_LEFTOVER = first feasible node in priority order (early exit)
 //                  k_least_alloc    argmax KS_SCORE_LEAST_ALLOCATED: bound-ordered scan, exact scores, early exit
+//                  k_most_alloc     argmax KS_SCORE_MOST_ALLOCATED: the same scan over its own order (built lazily)
 // Semantics per cell are exactly predicates.rs:42 / :45-61 (see include/ksched.h); only the evaluation
 // order differs, and every output is compared bit-for-bit with the oracle in tests/.
 #include "ks_bitpar.h"
+#include "ks_sort.cuh"
 
 #include <algorithm>
 #include <cstdlib>
@@ -1176,6 +1178,159 @@ __global__ void __launch_bounds__(256)
     exchange_signal(po);
 }
 
+// ---- argmax of KS_SCORE_MOST_ALLOCATED: k_least_alloc's bound-ordered scan over an order of its own ----
+// b(n) = term(f_c, A_c, 0) + term(f_m, A_m, 0) in [0, 200] (most_alloc_term, ks_internal.cuh).  For q >= 0,
+// clamp(x + q) <= clamp(x) + q and floor((y + q) * 100 / A) <= floor(y * 100 / A) + ceil(q * 100 / A), and a term is at
+// most 100, so every feasible cell of a pod with requests q >= 0 scores <= floor((b(n) + D) / 2) with
+// D = min(100, ceil(q_c * 100 / m_c)) + min(100, ceil(q_m * 100 / m_m)), m the smallest positive allocatable (a node with
+// A <= 0 has a term of 0 in score and bound alike).  Nodes are visited in descending b(n), ties by node index; the scan
+// stops once that bound of everything left is strictly below the best exact score.  A negative request voids the bound.
+// Built only when a MOST_ALLOCATED call needs it: one CTA sorts the nodes stably on 200 - b(n) (one 8-bit radix pass of
+// ks_sort.cuh), then k_build_tiles and k_build_eval fill the tile index and the evaluation rows in that order.
+__global__ void __launch_bounds__(SORT_THREADS)
+    k_most_order(NodeTable nt, uint32_t Nord, uint32_t* __restrict__ buf, int32_t* __restrict__ ord_idx,
+                 int64_t* __restrict__ ord_b, long long* __restrict__ amin) {
+    __shared__ SortShared s;
+    __shared__ long long s_min[2];
+    const uint32_t N = nt.N;
+    if (threadIdx.x == 0) s_min[0] = s_min[1] = LLONG_MAX;
+    __syncthreads();
+    long long mc = LLONG_MAX, mm = LLONG_MAX;
+    for (uint32_t i = threadIdx.x; i < N; i += SORT_THREADS) {
+        buf[i] = i;
+        const long long ac = nt.alloc_cpu[i], am = nt.alloc_mem[i];
+        if (ac > 0) mc = min(mc, ac);
+        if (am > 0) mm = min(mm, am);
+    }
+    atomicMin(&s_min[0], mc);
+    atomicMin(&s_min[1], mm);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        amin[0] = s_min[0];
+        amin[1] = s_min[1];
+    }
+    auto b = [&](uint32_t n) {
+        return most_alloc_term(nt.free_cpu[n], nt.alloc_cpu[n], 0) + most_alloc_term(nt.free_mem[n], nt.alloc_mem[n], 0);
+    };
+    cta_radix_pass(buf, buf + N, N, [&](uint32_t n) { return (uint32_t)(200 - b(n)); }, s);
+    for (uint32_t k = threadIdx.x; k < Nord; k += SORT_THREADS) {
+        const int32_t n = k < N ? (int32_t)buf[N + k] : -1;
+        ord_idx[k] = n;
+        ord_b[k] = n >= 0 ? b((uint32_t)n) : -1; // padding: below every bound, never feasible
+    }
+}
+
+// min(100, ceil(q * 100 / m)) for q >= 0, m > 0 (m may be LLONG_MAX: no node has a positive allocatable)
+__device__ __forceinline__ int64_t most_alloc_slack(int64_t q, long long m) {
+    const int64_t x = q * 100;
+    const int64_t c = (int64_t)(x / m) + (x % m != 0 ? 1 : 0);
+    return c < 100 ? c : 100;
+}
+
+template <int W>
+__global__ void __launch_bounds__(256)
+    k_most_alloc(const uint8_t* __restrict__ blobM, TileBuckets bk, RowsLayout lay, const NodeEval* __restrict__ ev,
+                 const int64_t* __restrict__ ordM_b, const long long* __restrict__ amin, PodView pv,
+                 const uint2* __restrict__ rk, OutView ov, PeerOut po, const unsigned long long* __restrict__ live, uint32_t N) {
+    __shared__ uint4 s_mask[LA_MAX_WARPS][32][2]; // per warp: the feasibility masks of the current window of tiles
+    __shared__ int64_t s_top[LA_MAX_WARPS][32];   //           and the bound of the first slot of each of them
+    const uint32_t lane = threadIdx.x & 31, wq = lane & 7, quarter = lane >> 3, wid = threadIdx.x >> 5;
+    const uint32_t warps = gridDim.x * (blockDim.x >> 5);
+    const long long mc = __ldg(amin), mm = __ldg(amin + 1);
+    uint32_t ne = 0;
+    if (blockIdx.x == 0 && threadIdx.x == 0) exchange_stamp(po, 0);
+    if (threadIdx.x == 0) trace_start(TR_ARGMAX1_START);
+    for (uint32_t p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); p < pv.P; p += warps) {
+        const uint2 r = __ldg(rk + p);
+        const PodThreshold t = pod_threshold(bk, lay, r);
+        unsigned long long sel[W];
+        bool dead = r.x >= N || r.y >= N; // the request exceeds every node's free cpu / memory
+#pragma unroll
+        for (int w = 0; w < W; w++) {
+            sel[w] = __ldg(pv.sel + (size_t)p * W + w);
+            dead |= (sel[w] & ~__ldg(live + w)) != 0; // a required pair that no node carries
+        }
+        const int64_t rc = __ldg(pv.req_cpu + p), rm = __ldg(pv.req_mem + p);
+        const bool bounded = rc >= 0 && rm >= 0; // else the bound does not hold: no early exit
+        const int64_t D = bounded ? most_alloc_slack(rc, mc) + most_alloc_slack(rm, mm) : 0;
+        int64_t best = INT64_MIN;
+        int32_t bidx = -1;
+        // windows of tiles as in k_least_alloc: phase A derives a window's feasibility masks (lane j: tile k0 + j), phase
+        // B scores the tiles with a feasible slot in bound order; the early exit is tested in front of each of them
+        uint32_t k0 = 0, win = LA_FIRST_WINDOW;
+        bool done = dead;
+        while (!done && k0 < lay.n_tiles) {
+            if (k0 > 0 && bounded && bidx >= 0 && best > (__ldg(ordM_b + (size_t)k0 * BP_TILE) + D) / 2) break; // warp-uniform
+            {
+                uint32_t m[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+                int64_t top = INT64_MIN;
+                const uint32_t kt = k0 + lane;
+                if (lane < win && kt < lay.n_tiles) {
+                    ptile_mask<W>(blobM, lay, tile_ranks(t, kt), sel, kt, m);
+                    top = __ldg(ordM_b + (size_t)kt * BP_TILE);
+                }
+                s_mask[wid][lane][0] = make_uint4(m[0], m[1], m[2], m[3]);
+                s_mask[wid][lane][1] = make_uint4(m[4], m[5], m[6], m[7]);
+                s_top[wid][lane] = top;
+                ne = __ballot_sync(0xffffffffu, (m[0] | m[1] | m[2] | m[3] | m[4] | m[5] | m[6] | m[7]) != 0u);
+            }
+            __syncwarp();
+            while (ne) {
+                const uint32_t j = __ffs(ne) - 1;
+                ne &= ne - 1;
+                const uint32_t k = k0 + j;
+                if (bounded && bidx >= 0 && best > (s_top[wid][j] + D) / 2) { // warp-uniform: nothing left can win or tie
+                    done = true;
+                    break;
+                }
+                // this lane's share of the tile's feasible slots: word wq, bit positions congruent to `quarter` mod 4
+                const uint32_t bits = reinterpret_cast<const uint32_t*>(&s_mask[wid][j][0])[wq] & (0x11111111u << quarter);
+                bool changed = false;
+#pragma unroll
+                for (int i = 0; i < 8; i++) {
+                    const uint32_t b = quarter + 4u * i;
+                    if (!((bits >> b) & 1u)) continue;
+                    const NodeEval e = ev[(size_t)k * BP_TILE + wq * 32 + b];
+                    const int64_t sc = most_alloc_int(e.fc, e.fm, e.ac, e.am, rc, rm);
+                    if (sc > best || (sc == best && e.idx < bidx)) {
+                        best = sc;
+                        bidx = e.idx;
+                        changed = true;
+                    }
+                }
+                if (__any_sync(0xffffffffu, changed)) {
+#pragma unroll
+                    for (int off = 16; off > 0; off >>= 1) { // every lane ends with the tile-merged best
+                        const int64_t os = __shfl_xor_sync(0xffffffffu, best, off);
+                        const int32_t oi = __shfl_xor_sync(0xffffffffu, bidx, off);
+                        if (oi >= 0 && (bidx < 0 || os > best || (os == best && oi < bidx))) {
+                            best = os;
+                            bidx = oi;
+                        }
+                    }
+                }
+            }
+            __syncwarp(); // the next window overwrites this warp's slice of s_mask / s_top
+            k0 += win;
+            win = 32;
+        }
+        if (lane == 0) {
+            const int64_t score = bidx >= 0 ? best : 0;
+            if (ov.node_idx) ov.node_idx[p] = bidx;
+            if (ov.score) ov.score[p] = score;
+            for (uint32_t q = 0; q < po.n; q++) {
+                po.idx[q][p] = bidx;
+                po.score[q][p] = score;
+            }
+        }
+    }
+    if (c_trace) {
+        __syncthreads();
+        if (threadIdx.x == 0) trace_end(TR_ARGMAX1_END);
+    }
+    exchange_signal(po);
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 // The column-block format (ks_bitpar.h) of all three indexes: column blocks of RW_TILES tiles; the mask kernel stages the
 // pair columns with the tables when everything fits in shared memory (W <= 4), else it reads them through L1/L2
@@ -1221,6 +1376,7 @@ BitparIndex::~BitparIndex() {
 
 cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cudaStream_t st) {
     ix.valid = false;
+    ix.validM = false; // the MOST_ALLOCATED order follows on the next call that needs it (bitpar_prepare_most)
     ix.N = nt.N;
     ix.W = nt.W;
     if (nt.N == 0) return cudaSuccess;
@@ -1303,6 +1459,34 @@ cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cu
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     ix.lay_r = lay;
     ix.valid = true;
+    return cudaSuccess;
+}
+
+cudaError_t bitpar_prepare_most(BitparIndex& ix, const NodeTable& nt, cudaStream_t st) {
+    if (!ix.valid) return cudaErrorNotSupported;
+    if (ix.validM) return cudaSuccess;
+    cudaError_t e;
+    const uint32_t Nord = ix.Nord;
+    if ((e = ix.ordM_b.ensure((size_t)Nord * sizeof(int64_t))) != cudaSuccess) return e;
+    if ((e = ix.ordM_idx.ensure((size_t)Nord * sizeof(int32_t))) != cudaSuccess) return e;
+    if ((e = ix.evalM.ensure((size_t)Nord * sizeof(NodeEval))) != cudaSuccess) return e;
+    if ((e = ix.hintM.ensure((size_t)Nord * sizeof(float4))) != cudaSuccess) return e;
+    if ((e = ix.sortM.ensure(2ull * nt.N * sizeof(uint32_t) + 2 * sizeof(long long))) != cudaSuccess) return e;
+    if ((e = ix.blobM.ensure((size_t)ix.lay_r.ncb * ix.lay_r.cb_stride)) != cudaSuccess) return e;
+    if ((e = ix.bucketsM.ensure(tile_buckets(nullptr, nt.N, ix.lay_r, nullptr))) != cudaSuccess) return e;
+    long long* amin = reinterpret_cast<long long*>(ix.sortM.as<uint32_t>() + 2ull * nt.N);
+    k_most_order<<<1, SORT_THREADS, 0, st>>>(nt, Nord, ix.sortM.as<uint32_t>(), ix.ordM_idx.as<int32_t>(),
+                                             ix.ordM_b.as<int64_t>(), amin);
+    TileBuckets bk;
+    tile_buckets(ix.bucketsM.p, nt.N, ix.lay_r, &bk);
+    k_build_tiles<<<ix.lay_r.ncb * RW_TILES, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(),
+                                                          ix.ordM_idx.as<int32_t>(), ix.blobM.as<uint8_t>(), ix.lay_r,
+                                                          nullptr, bk);
+    k_build_eval<<<(Nord + 255) / 256, 256, 0, st>>>(nt, ix.ordM_idx.as<int32_t>(), Nord, ix.evalM.as<NodeEval>(),
+                                                     ix.hintM.as<float4>());
+    g_launches += 3;
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    ix.validM = true;
     return cudaSuccess;
 }
 
@@ -1409,8 +1593,19 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
         if ((e = cudaMemsetAsync(tail_count, 0, sizeof(uint32_t), bs)) != cudaSuccess) return e;
         const bool least_alloc = L.policy == KS_SCORE_LEAST_ALLOCATED;
         TileBuckets bk;
-        tile_buckets(least_alloc ? ix.bucketsL.p : ix.bucketsP.p, ix.N, ix.lay_r, &bk);
-        if (least_alloc) {
+        if (L.policy == KS_SCORE_MOST_ALLOCATED) {
+            if (!ix.validM) return cudaErrorNotSupported; // bitpar_prepare_most runs first
+            tile_buckets(ix.bucketsM.p, ix.N, ix.lay_r, &bk);
+            const uint32_t wpc = at / 32; // one warp per pod
+            const uint32_t grid = (uint32_t)std::min<uint64_t>((uint64_t)sms * (2048 / at), ((uint64_t)P + wpc - 1) / wpc);
+            const long long* amin = reinterpret_cast<const long long*>(ix.sortM.as<uint32_t>() + 2ull * ix.N);
+            k_most_alloc<W><<<grid, at, 0, bs>>>(ix.blobM.as<uint8_t>(), bk, ix.lay_r, ix.evalM.as<NodeEval>(),
+                                                 ix.ordM_b.as<int64_t>(), amin, L.pv, ix.pod_ranks.as<uint2>(), L.ov, L.po,
+                                                 ix.live.as<unsigned long long>(), ix.N);
+            g_launches++;
+            if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        } else if (least_alloc) {
+            tile_buckets(ix.bucketsL.p, ix.N, ix.lay_r, &bk);
             const uint32_t wpc = at / 32; // one warp per pod
             const uint32_t grid = (uint32_t)std::min<uint64_t>((uint64_t)sms * (2048 / at), ((uint64_t)P + wpc - 1) / wpc);
             k_least_alloc<W><<<grid, at, 0, bs>>>(ix.blobL.as<uint8_t>(), bk, ix.lay_r, ix.evalL.as<NodeEval>(), ix.hintL.as<float4>(),
@@ -1419,6 +1614,7 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
             g_launches++;
             if ((e = cudaGetLastError()) != cudaSuccess) return e;
         } else {
+            tile_buckets(ix.bucketsP.p, ix.N, ix.lay_r, &bk);
             const bool has_tail = ix.lay_r.n_tiles > FF_HEAD_TILES;
             k_first_fit_head<W><<<(P + at - 1) / at, at, 0, bs>>>(ix.blobP.as<uint8_t>(), bk, ix.lay_r, ix.ord_idx.as<int32_t>(),
                                                                  ix.ord_prio.as<int64_t>(), L.pv, ix.pod_ranks.as<uint2>(), L.ov,

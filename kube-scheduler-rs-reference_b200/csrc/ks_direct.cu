@@ -339,7 +339,7 @@ template <int W, int POLICY, bool EMIT_MASK>
 __global__ void __launch_bounds__(DIRECT_THREADS)
     k_select_direct(NodeTable nt, PodView pv, OutView ov, PartialView part, uint32_t tiles_per_chunk) {
     constexpr int PW = pods_per_warp(W);
-    constexpr bool LA = POLICY == KS_SCORE_LEAST_ALLOCATED;
+    constexpr bool ALLOC = POLICY != KS_SCORE_LEFTOVER; // scored from the allocatables
     const uint32_t lane = threadIdx.x & 31;
     int64_t rc[PW], rm[PW];
     uint64_t sel[PW][W];
@@ -356,10 +356,10 @@ __global__ void __launch_bounds__(DIRECT_THREADS)
         acc[i] = 0;
     }
 
-    scan_node_tiles<W, LA>(
+    scan_node_tiles<W, ALLOC>(
         nt, tiles_per_chunk, pv, p0, rc, rm, sel,
         [&](uint32_t g, uint32_t node, bool real, int64_t fc, int64_t fm, const uint64_t(&lab)[W], int64_t ac, int64_t am) {
-            const int64_t key_n = LA ? 0 : leftover_key(fc, fm); // LEFTOVER: node priority; the pod part is constant
+            const int64_t key_n = ALLOC ? 0 : leftover_key(fc, fm); // LEFTOVER: node priority; the pod part is constant
 #pragma unroll
             for (int i = 0; i < PW; i++) {
                 const bool fit = (rc[i] <= fc) & (rm[i] <= fm);
@@ -371,7 +371,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS)
                 cnt[i] += __popc(b);
                 if (EMIT_MASK) acc[i] = (lane == g) ? b : acc[i];
                 if (ok) {
-                    const int64_t key = LA ? least_alloc_int(fc, fm, ac, am, rc[i], rm[i]) : key_n;
+                    const int64_t key = ALLOC ? alloc_score<POLICY>(fc, fm, ac, am, rc[i], rm[i]) : key_n;
                     if (key > best[i]) {
                         best[i] = key;
                         bidx[i] = (int32_t)node;
@@ -397,7 +397,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS)
         if (lane == 0 && p0 + i < pv.P) {
             const uint32_t p = p0 + i;
             if (gridDim.y == 1) {
-                const int64_t s = ix < 0 ? 0 : (LA ? k : leftover_score(k, rc[i], rm[i]));
+                const int64_t s = ix < 0 ? 0 : (ALLOC ? k : leftover_score(k, rc[i], rm[i]));
                 if (ov.node_idx) ov.node_idx[p] = ix;
                 if (ov.score) ov.score[p] = s;
                 if (ov.cnt) ov.cnt[p] = cnt[i];
@@ -495,7 +495,7 @@ template <int W, int POLICY>
 __global__ void __launch_bounds__(DIRECT_THREADS, 1)
     k_select_topk(NodeTable nt, PodView pv, OutView ov, PartialView part, uint32_t k, uint32_t tiles_per_chunk) {
     constexpr int PW = pods_per_warp(W);
-    constexpr bool LA = POLICY == KS_SCORE_LEAST_ALLOCATED;
+    constexpr bool ALLOC = POLICY != KS_SCORE_LEFTOVER; // scored from the allocatables
     const uint32_t lane = threadIdx.x & 31;
     int64_t rc[PW], rm[PW];
     uint64_t sel[PW][W];
@@ -510,10 +510,10 @@ __global__ void __launch_bounds__(DIRECT_THREADS, 1)
         cnt[i] = 0;
     }
 
-    scan_node_tiles<W, LA>(
+    scan_node_tiles<W, ALLOC>(
         nt, tiles_per_chunk, pv, p0, rc, rm, sel,
         [&](uint32_t, uint32_t node, bool real, int64_t fc, int64_t fm, const uint64_t(&lab)[W], int64_t ac, int64_t am) {
-            const int64_t key_n = LA ? 0 : leftover_key(fc, fm); // LEFTOVER: node priority; the pod part is constant
+            const int64_t key_n = ALLOC ? 0 : leftover_key(fc, fm); // LEFTOVER: node priority; the pod part is constant
 #pragma unroll
             for (int i = 0; i < PW; i++) {
                 const bool fit = (rc[i] <= fc) & (rm[i] <= fm);
@@ -522,7 +522,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS, 1)
                 for (int w = 0; w < W; w++) miss |= sel[i][w] & ~lab[w];
                 const bool ok = fit && (miss == 0) && real;
                 cnt[i] += __popc(__ballot_sync(0xffffffffu, ok));
-                const int64_t key = LA ? (ok ? least_alloc_int(fc, fm, ac, am, rc[i], rm[i]) : 0) : key_n;
+                const int64_t key = ALLOC ? (ok ? alloc_score<POLICY>(fc, fm, ac, am, rc[i], rm[i]) : 0) : key_n;
                 uint32_t cand = __ballot_sync(0xffffffffu, ok && topk_beats(key, (int32_t)node, tkey[i], tidx[i]));
                 while (cand) { // warp-uniform
                     const int src = __ffs(cand) - 1;
@@ -546,7 +546,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS, 1)
             const uint64_t o = (uint64_t)p * k + lane;
             if (lane < k) {
                 ov.node_idx[o] = lidx[i];
-                if (ov.score) ov.score[o] = lidx[i] < 0 ? 0 : (LA ? lkey[i] : leftover_score(lkey[i], rc[i], rm[i]));
+                if (ov.score) ov.score[o] = lidx[i] < 0 ? 0 : (ALLOC ? lkey[i] : leftover_score(lkey[i], rc[i], rm[i]));
             }
             if (lane == 0 && ov.cnt) ov.cnt[p] = cnt[i];
         } else {
@@ -782,7 +782,7 @@ template <int W, int POLICY>
 __global__ void __launch_bounds__(DIRECT_THREADS, 1)
     k_drain_scan(NodeTable nt, PodView pv, DrainArgs da, PartialView part, uint32_t tiles_per_chunk) {
     constexpr int PW = pods_per_warp(W);
-    constexpr bool LA = POLICY == KS_SCORE_LEAST_ALLOCATED;
+    constexpr bool ALLOC = POLICY != KS_SCORE_LEFTOVER; // scored from the allocatables
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t q0 = warp_first_pod<PW>(); // the p0 scan_node_tiles sets
     bool dead = true; // every pod of this warp failed earlier (or there is none)
@@ -804,7 +804,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS, 1)
         cur[i] = 0;
     }
 
-    scan_node_tiles<W, LA>(
+    scan_node_tiles<W, ALLOC>(
         nt, tiles_per_chunk, pv, p0, rc, rm, sel,
         [&](uint32_t g, uint32_t node, bool real, int64_t fc, int64_t fm, const uint64_t(&lab)[W], int64_t ac, int64_t am) {
             if (g == 0) { // first group of a tile: this tile's skip words
@@ -813,7 +813,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS, 1)
 #pragma unroll
                 for (int i = 0; i < PW; i++) skip[i] = drain_skip_word(da, min(p0 + i, pv.P - 1), tb, xw, cur[i]);
             }
-            const int64_t key_n = LA ? 0 : leftover_key(fc, fm);
+            const int64_t key_n = ALLOC ? 0 : leftover_key(fc, fm);
 #pragma unroll
             for (int i = 0; i < PW; i++) {
                 const bool fit = (rc[i] <= fc) & (rm[i] <= fm);
@@ -822,7 +822,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS, 1)
                 for (int w = 0; w < W; w++) miss |= sel[i][w] & ~lab[w];
                 const bool off = (__shfl_sync(0xffffffffu, skip[i], g) >> lane) & 1u;
                 if (fit && miss == 0 && real && !off) {
-                    const int64_t key = LA ? least_alloc_int(fc, fm, ac, am, rc[i], rm[i]) : key_n;
+                    const int64_t key = ALLOC ? alloc_score<POLICY>(fc, fm, ac, am, rc[i], rm[i]) : key_n;
                     if (key > best[i]) {
                         best[i] = key;
                         bidx[i] = (int32_t)node;
@@ -851,7 +851,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS, 1)
 template <int W, int POLICY>
 __global__ void __launch_bounds__(256)
     k_drain_commit(NodeTable nt, PodView pv, DrainArgs da, PartialView part, uint32_t n_chunks, uint32_t r) {
-    constexpr bool LA = POLICY == KS_SCORE_LEAST_ALLOCATED;
+    constexpr bool ALLOC = POLICY != KS_SCORE_LEFTOVER; // scored from the allocatables
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (p >= pv.P || da.failed[p]) return; // warp-uniform
@@ -873,7 +873,7 @@ __global__ void __launch_bounds__(256)
 #pragma unroll
         for (int w = 0; w < W; w++) miss |= sel[w] & ~nt.labels[(uint64_t)w * nt.Npad + node];
         if (rc <= fc && rm <= fm && miss == 0) {
-            const int64_t kk = LA ? least_alloc_int(fc, fm, nt.alloc_cpu[node], nt.alloc_mem[node], rc, rm) : leftover_key(fc, fm);
+            const int64_t kk = ALLOC ? alloc_score<POLICY>(fc, fm, nt.alloc_cpu[node], nt.alloc_mem[node], rc, rm) : leftover_key(fc, fm);
             if (topk_beats(kk, node, key, idx)) {
                 key = kk;
                 idx = node;
@@ -888,7 +888,7 @@ __global__ void __launch_bounds__(256)
     const uint32_t pod = da.pod_base[p] + r;
     if (lane == 0) {
         da.out_idx[pod] = idx;
-        da.out_score[pod] = LA ? key : leftover_score(key, rc, rm);
+        da.out_score[pod] = ALLOC ? key : leftover_score(key, rc, rm);
         da.placed[da.cand_id[p]] = r + 1;
     }
     uint32_t pos = 0; // entries below idx
@@ -1195,17 +1195,21 @@ cudaError_t prepare_direct() {
     for (uint32_t W : {1u, 2u, 4u, 8u})
         with_label_width(W, [&](auto w) {
             constexpr int W_ = decltype(w)::value;
-            constexpr int LO = KS_SCORE_LEFTOVER, LA = KS_SCORE_LEAST_ALLOCATED;
+            constexpr int LO = KS_SCORE_LEFTOVER, LA = KS_SCORE_LEAST_ALLOCATED, MA = KS_SCORE_MOST_ALLOCATED;
             opt_in(k_select_direct<W_, LO, true>, tile_smem_bytes<W_, false>());
             opt_in(k_select_direct<W_, LO, false>, tile_smem_bytes<W_, false>());
             opt_in(k_select_direct<W_, LA, true>, tile_smem_bytes<W_, true>());
             opt_in(k_select_direct<W_, LA, false>, tile_smem_bytes<W_, true>());
+            opt_in(k_select_direct<W_, MA, true>, tile_smem_bytes<W_, true>());
+            opt_in(k_select_direct<W_, MA, false>, tile_smem_bytes<W_, true>());
             opt_in(k_explain_counts<W_>, tile_smem_bytes<W_, false>());
             opt_in(k_select_topk<W_, LO>, tile_smem_bytes<W_, false>());
             opt_in(k_select_topk<W_, LA>, tile_smem_bytes<W_, true>());
+            opt_in(k_select_topk<W_, MA>, tile_smem_bytes<W_, true>());
             opt_in(k_preempt_scan<W_>, tile_smem_bytes<W_, false>());
             opt_in(k_drain_scan<W_, LO>, tile_smem_bytes<W_, false>());
             opt_in(k_drain_scan<W_, LA>, tile_smem_bytes<W_, true>());
+            opt_in(k_drain_scan<W_, MA>, tile_smem_bytes<W_, true>());
             return e;
         });
     return e;
@@ -1213,7 +1217,7 @@ cudaError_t prepare_direct() {
 
 template <int W, int POLICY, bool EMIT>
 static cudaError_t launch_direct_t(const SelectLaunch& L, const PartialView& part, const DirectGrid& g) {
-    constexpr uint32_t SMEM = tile_smem_bytes<W, POLICY == KS_SCORE_LEAST_ALLOCATED>();
+    constexpr uint32_t SMEM = tile_smem_bytes<W, POLICY != KS_SCORE_LEFTOVER>();
     k_select_direct<W, POLICY, EMIT><<<dim3(g.pod_ctas, g.n_chunks), DIRECT_THREADS, SMEM, L.stream>>>(
         L.nt, L.pv, L.ov, part, g.tiles_per_chunk);
     g_launches++;
@@ -1231,6 +1235,9 @@ cudaError_t launch_select_direct(const SelectLaunch& L, const PartialView& part,
         if (L.policy == KS_SCORE_LEFTOVER)
             return emit ? launch_direct_t<W, KS_SCORE_LEFTOVER, true>(L, part, g)
                         : launch_direct_t<W, KS_SCORE_LEFTOVER, false>(L, part, g);
+        if (L.policy == KS_SCORE_MOST_ALLOCATED)
+            return emit ? launch_direct_t<W, KS_SCORE_MOST_ALLOCATED, true>(L, part, g)
+                        : launch_direct_t<W, KS_SCORE_MOST_ALLOCATED, false>(L, part, g);
         return emit ? launch_direct_t<W, KS_SCORE_LEAST_ALLOCATED, true>(L, part, g)
                     : launch_direct_t<W, KS_SCORE_LEAST_ALLOCATED, false>(L, part, g);
     });
@@ -1255,7 +1262,7 @@ cudaError_t launch_explain_counts(const NodeTable& nt, const PodView& pv, uint32
 template <int W, int POLICY>
 static cudaError_t launch_topk_t(const NodeTable& nt, const PodView& pv, uint32_t k, const OutView& ov,
                                  const PartialView& part, const DirectGrid& g, cudaStream_t st) {
-    constexpr uint32_t SMEM = tile_smem_bytes<W, POLICY == KS_SCORE_LEAST_ALLOCATED>();
+    constexpr uint32_t SMEM = tile_smem_bytes<W, POLICY != KS_SCORE_LEFTOVER>();
     k_select_topk<W, POLICY><<<dim3(g.pod_ctas, g.n_chunks), DIRECT_THREADS, SMEM, st>>>(nt, pv, ov, part, k,
                                                                                           g.tiles_per_chunk);
     g_launches++;
@@ -1270,6 +1277,7 @@ cudaError_t launch_select_topk(const NodeTable& nt, const PodView& pv, int polic
                                const PartialView& part, const DirectGrid& g, cudaStream_t st) {
     return with_label_width(nt.W, [&](auto w) {
         constexpr int W = decltype(w)::value;
+        if (policy == KS_SCORE_MOST_ALLOCATED) return launch_topk_t<W, KS_SCORE_MOST_ALLOCATED>(nt, pv, k, ov, part, g, st);
         return policy == KS_SCORE_LEFTOVER ? launch_topk_t<W, KS_SCORE_LEFTOVER>(nt, pv, k, ov, part, g, st)
                                            : launch_topk_t<W, KS_SCORE_LEAST_ALLOCATED>(nt, pv, k, ov, part, g, st);
     });
@@ -1299,7 +1307,7 @@ cudaError_t launch_preempt(const NodeTable& nt, const PodView& pv, const int32_t
 template <int W, int POLICY>
 static cudaError_t launch_drain_t(const NodeTable& nt, const PodView& pv, const DrainArgs& da, uint32_t r,
                                   const PartialView& part, const DirectGrid& g, cudaStream_t st) {
-    constexpr uint32_t SMEM = tile_smem_bytes<W, POLICY == KS_SCORE_LEAST_ALLOCATED>();
+    constexpr uint32_t SMEM = tile_smem_bytes<W, POLICY != KS_SCORE_LEFTOVER>();
     k_drain_scan<W, POLICY><<<dim3(g.pod_ctas, g.n_chunks), DIRECT_THREADS, SMEM, st>>>(nt, pv, da, part, g.tiles_per_chunk);
     k_drain_commit<W, POLICY><<<(pv.P + 7) / 8, 256, 0, st>>>(nt, pv, da, part, g.n_chunks, r);
     g_launches += 2;
@@ -1311,6 +1319,7 @@ cudaError_t launch_drain_round(const NodeTable& nt, const PodView& pv, const Dra
     if (pv.P == 0) return cudaSuccess;
     return with_label_width(nt.W, [&](auto w) {
         constexpr int W = decltype(w)::value;
+        if (policy == KS_SCORE_MOST_ALLOCATED) return launch_drain_t<W, KS_SCORE_MOST_ALLOCATED>(nt, pv, da, r, part, g, st);
         return policy == KS_SCORE_LEFTOVER ? launch_drain_t<W, KS_SCORE_LEFTOVER>(nt, pv, da, r, part, g, st)
                                            : launch_drain_t<W, KS_SCORE_LEAST_ALLOCATED>(nt, pv, da, r, part, g, st);
     });

@@ -88,7 +88,7 @@ __device__ __forceinline__ void exchange_signal(const PeerOut& po) {
 
 // Per-(chunk,pod) partial results when the node dimension is split across CTAs (small P).
 struct PartialView {
-    int64_t* key;  // best policy key (LEFTOVER: node priority; LEAST_ALLOCATED: score)
+    int64_t* key;  // best policy key (LEFTOVER: node priority; LEAST_ALLOCATED, MOST_ALLOCATED: score)
     int32_t* idx;
     uint32_t* cnt;
 };
@@ -113,6 +113,23 @@ __device__ __forceinline__ int64_t least_alloc_int(int64_t fc, int64_t fm, int64
     const int64_t pc = ac > 0 ? ((fc - rc) * 100) / ac : 0;
     const int64_t pm = am > 0 ? ((fm - rm) * 100) / am : 0;
     return (pc + pm) / 2;
+}
+// KS_SCORE_MOST_ALLOCATED in exact integer arithmetic: the mean of the truncated percentages requested after placement,
+// requested = A - (f - q) clamped to [0, A].  Inside the limits of ksched.h every intermediate fits int64 (A - (f - q)
+// is below 2^57 in magnitude and the clamped product below 100 * 2^55), and the score lies in [0, 100].
+__device__ __forceinline__ int64_t most_alloc_term(int64_t f, int64_t a, int64_t q) {
+    if (a <= 0) return 0;
+    const int64_t u = a - (f - q);
+    return (u < 0 ? 0 : u > a ? a : u) * 100 / a;
+}
+__device__ __forceinline__ int64_t most_alloc_int(int64_t fc, int64_t fm, int64_t ac, int64_t am, int64_t rc, int64_t rm) {
+    return (most_alloc_term(fc, ac, rc) + most_alloc_term(fm, am, rm)) / 2;
+}
+// The score of a policy that reads the allocatables, chosen at compile time: MOST_ALLOCATED, else LEAST_ALLOCATED
+template <int POLICY>
+__device__ __forceinline__ int64_t alloc_score(int64_t fc, int64_t fm, int64_t ac, int64_t am, int64_t rc, int64_t rm) {
+    return POLICY == KS_SCORE_MOST_ALLOCATED ? most_alloc_int(fc, fm, ac, am, rc, rm)
+                                             : least_alloc_int(fc, fm, ac, am, rc, rm);
 }
 // Warp argmax over (key, idx) with idx < 0 for "no candidate": larger key wins, ties go to the lower node index.
 // Every lane ends with the result.

@@ -11,6 +11,10 @@
 //                 copies go to the lowest nodes (chunk prefixes here, the prefix inside a chunk in k_rep_emit);
 //   k_rep_emit    count_n, the row's node count and maximum and, with the copy list, every copy in node-then-copy order;
 //   k_rep_order   one CTA per spec: the stable radix sort of ks_sort.cuh on top - score, which is placement order.
+// Under MOST_ALLOCATED s_n(j) is non-decreasing in j instead, and placement fills whole nodes in order of s_n(0) descending,
+// node ascending (include/ksched.h).  The same kernels compute that plan with G_n(S) = s_n(0) >= S ? k_n : 0: S* is the
+// s_n(0) of the last node that takes copies, the nodes above it take all k_n, the tie split fills the nodes at S* in node
+// order, and k_rep_order_most sorts on top - s_n(0) of each copy's node, which keeps a node's copies together.
 #include "ks_launch.h"
 #include "ks_sort.cuh"
 
@@ -55,7 +59,7 @@ void replica_chunks(uint32_t N, uint32_t T, int sms, uint32_t* n_chunks, uint32_
     *n_chunks = (tiles + per - 1) / per;
 }
 
-// One node as a spec sees it: free values, allocatable (LEAST_ALLOCATED) and k_n.
+// One node as a spec sees it: free values, allocatable (LEAST_ALLOCATED, MOST_ALLOCATED) and k_n.
 struct RepNode {
     int64_t fc, fm, ac, am;
     uint32_t k;
@@ -83,7 +87,7 @@ __device__ __forceinline__ void rep_node(const NodeTable& nt, uint32_t n, int64_
                                          uint32_t R, RepNode& v, uint64_t& c) {
     c = rep_copies<W>(nt, n, rc, rm, sel, v);
     v.k = (uint32_t)min(c, (uint64_t)R);
-    if (POL == KS_SCORE_LEAST_ALLOCATED && v.k) {
+    if (POL != KS_SCORE_LEFTOVER && v.k) {
         v.ac = nt.alloc_cpu[n];
         v.am = nt.alloc_mem[n];
     } else {
@@ -96,11 +100,12 @@ template <int POL>
 __device__ __forceinline__ int64_t rep_score(const RepNode& v, int64_t rc, int64_t rm, uint32_t j) {
     const int64_t c = v.fc - (int64_t)j * rc, m = v.fm - (int64_t)j * rm;
     if (POL == KS_SCORE_LEFTOVER) return leftover_score(leftover_key(c, m), rc, rm);
-    return least_alloc_int(c, m, v.ac, v.am, rc, rm);
+    return alloc_score<POL>(c, m, v.ac, v.am, rc, rm);
 }
 
 // G_n(S) = #{j < k : s_n(j) >= S}.  LEFTOVER: s_n(j) = key_n - (j + 1) * d, a closed form.  LEAST_ALLOCATED: a binary
-// search over j, after the bounds s0 = s_n(0) and sl = s_n(k - 1).
+// search over j, after the bounds s0 = s_n(0) and sl = s_n(k - 1).  MOST_ALLOCATED: not that count but the copies a
+// node filled in s_n(0) order holds, s0 >= S ? k : 0.
 template <int POL>
 __device__ __forceinline__ uint32_t rep_at(const RepNode& v, int64_t rc, int64_t rm, int64_t s0, int64_t sl, int64_t S) {
     if (v.k == 0) return 0;
@@ -110,6 +115,7 @@ __device__ __forceinline__ uint32_t rep_at(const RepNode& v, int64_t rc, int64_t
         return d == 0 ? v.k : (uint32_t)min((uint64_t)v.k, (uint64_t)x / (uint64_t)d);
     }
     if (S > s0) return 0;
+    if (POL == KS_SCORE_MOST_ALLOCATED) return v.k;
     if (S <= sl) return v.k;
     uint32_t a = 1, b = v.k - 1; // s(a - 1) >= S > s(b)
     while (a < b) {
@@ -168,7 +174,7 @@ __global__ void __launch_bounds__(REP_THREADS) k_rep_scan(NodeTable nt, ReplicaA
         sumk += v.k;
         if (v.k) {
             hi = max(hi, rep_score<POL>(v, x.rc, x.rm, 0));
-            lo = min(lo, rep_score<POL>(v, x.rc, x.rm, v.k - 1));
+            lo = min(lo, rep_score<POL>(v, x.rc, x.rm, POL == KS_SCORE_MOST_ALLOCATED ? 0 : v.k - 1));
         }
     }
     cap = rep_reduce(cap, sat_add, red);
@@ -245,9 +251,9 @@ __global__ void __launch_bounds__(REP_THREADS) k_rep_count(NodeTable nt, Replica
         if (n < x.n1) {
             uint64_t cn;
             rep_node<W, POL>(nt, n, x.rc, x.rm, x.sel, x.R, v, cn);
-            if (POL == KS_SCORE_LEAST_ALLOCATED && v.k) {
+            if (POL != KS_SCORE_LEFTOVER && v.k) {
                 s0 = rep_score<POL>(v, x.rc, x.rm, 0);
-                sl = rep_score<POL>(v, x.rc, x.rm, v.k - 1);
+                sl = POL == KS_SCORE_MOST_ALLOCATED ? s0 : rep_score<POL>(v, x.rc, x.rm, v.k - 1); // MOST: rep_at reads s0 only
             }
         }
         for (uint32_t live = __ballot_sync(0xffffffffu, v.k != 0); live; live &= live - 1) {
@@ -307,7 +313,8 @@ __global__ void __launch_bounds__(REP_THREADS) k_rep_tally(NodeTable nt, Replica
             uint64_t cn;
             rep_node<W, POL>(nt, n, x.rc, x.rm, x.sel, x.R, v, cn);
             if (!v.k) continue;
-            const int64_t s0 = rep_score<POL>(v, x.rc, x.rm, 0), sl = rep_score<POL>(v, x.rc, x.rm, v.k - 1);
+            const int64_t s0 = rep_score<POL>(v, x.rc, x.rm, 0);
+            const int64_t sl = POL == KS_SCORE_MOST_ALLOCATED ? s0 : rep_score<POL>(v, x.rc, x.rm, v.k - 1);
             const uint32_t above = rep_at<POL>(v, x.rc, x.rm, s0, sl, S + 1);
             sa += above;
             se += rep_at<POL>(v, x.rc, x.rm, s0, sl, S) - above;
@@ -368,7 +375,8 @@ __global__ void __launch_bounds__(REP_THREADS) k_rep_emit(NodeTable nt, ReplicaA
             uint64_t cn;
             rep_node<W, POL>(nt, n, x.rc, x.rm, x.sel, x.R, v, cn);
             if (v.k) {
-                const int64_t s0 = rep_score<POL>(v, x.rc, x.rm, 0), sl = rep_score<POL>(v, x.rc, x.rm, v.k - 1);
+                const int64_t s0 = rep_score<POL>(v, x.rc, x.rm, 0);
+            const int64_t sl = POL == KS_SCORE_MOST_ALLOCATED ? s0 : rep_score<POL>(v, x.rc, x.rm, v.k - 1);
                 above = rep_at<POL>(v, x.rc, x.rm, s0, sl, S + 1);
                 e = rep_at<POL>(v, x.rc, x.rm, s0, sl, S) - above;
             }
@@ -376,6 +384,9 @@ __global__ void __launch_bounds__(REP_THREADS) k_rep_emit(NodeTable nt, ReplicaA
         uint32_t e_tot, c_tot;
         const uint64_t pre = e_run + cta_block_scan(e, wsum, e_tot);
         const uint32_t cnt = above + (K > pre ? (uint32_t)min((uint64_t)e, K - pre) : 0u);
+        // MOST_ALLOCATED: the last copy placed is the last one of the node at S* whose tied copies reach K
+        if (POL == KS_SCORE_MOST_ALLOCATED && e && pre < K && K <= pre + e)
+            a.rows[t].last_score = rep_score<POL>(v, x.rc, x.rm, cnt - 1);
         const uint64_t base = off + c_run + cta_block_scan(cnt, wsum, c_tot);
         e_run += e_tot;
         c_run += c_tot;
@@ -407,9 +418,10 @@ __global__ void __launch_bounds__(REP_THREADS) k_rep_emit(NodeTable nt, ReplicaA
     }
 }
 
-// One CTA per spec: the copies, laid out node then copy, sorted stably by top - score (ascending) are in placement
-// order; only the digits of top - S* are sorted.
-__global__ void __launch_bounds__(REP_THREADS) k_rep_order(ReplicaArgs a) {
+// One CTA per spec: the copies, laid out node then copy, sorted stably by key(top, scores, t, nodes, i) (ascending; top - the
+// copy's score, or top - s_n(0) of its node) are in placement order; only the digits of top - S* are sorted.
+template <class Key>
+__device__ __forceinline__ void rep_order(const ReplicaArgs& a, Key key) {
     __shared__ SortShared s;
     for (uint32_t t = blockIdx.x; t < a.T; t += gridDim.x) {
         const RepSpec& sp = a.spec[t];
@@ -425,7 +437,7 @@ __global__ void __launch_bounds__(REP_THREADS) k_rep_order(ReplicaArgs a) {
         const uint64_t span = (uint64_t)(top - sp.lo);
         const uint32_t bits = span ? 64u - __clzll((long long)span) : 0u;
         for (uint32_t shift = 0; shift < bits; shift += 8) {
-            cta_radix_pass(src, dst, M, [&](uint32_t i) { return (uint32_t)((uint64_t)(top - sc[i]) >> shift) & 255u; }, s);
+            cta_radix_pass(src, dst, M, [&](uint32_t i) { return (uint32_t)(key(top, sc, t, nd, i) >> shift) & 255u; }, s);
             uint32_t* y = src;
             src = dst;
             dst = y;
@@ -437,6 +449,17 @@ __global__ void __launch_bounds__(REP_THREADS) k_rep_order(ReplicaArgs a) {
         }
         __syncthreads(); // the shared sort state is reused by the next spec
     }
+}
+__global__ void __launch_bounds__(REP_THREADS) k_rep_order(ReplicaArgs a) {
+    rep_order(a, [](int64_t top, const int64_t* sc, uint32_t, const int32_t*, uint32_t i) { return (uint64_t)(top - sc[i]); });
+}
+// MOST_ALLOCATED: the key is top - s_n(0) of the copy's node
+__global__ void __launch_bounds__(REP_THREADS) k_rep_order_most(NodeTable nt, ReplicaArgs a) {
+    rep_order(a, [&](int64_t top, const int64_t*, uint32_t t, const int32_t* nd, uint32_t i) {
+        const int32_t n = nd[i];
+        return (uint64_t)(top - most_alloc_int(nt.free_cpu[n], nt.free_mem[n], nt.alloc_cpu[n], nt.alloc_mem[n],
+                                               a.req_cpu[t], a.req_mem[t]));
+    });
 }
 
 template <int W, int POL>
@@ -454,7 +477,8 @@ static cudaError_t rep_sequence(const NodeTable& nt, const ReplicaArgs& a, cudaS
     k_rep_emit<W, POL><<<grid, REP_THREADS, 0, st>>>(nt, a);
     g_launches += 5 + 2 * REP_PASSES;
     if (a.out_node) {
-        k_rep_order<<<a.T, REP_THREADS, 0, st>>>(a);
+        if (POL == KS_SCORE_MOST_ALLOCATED) k_rep_order_most<<<a.T, REP_THREADS, 0, st>>>(nt, a);
+        else k_rep_order<<<a.T, REP_THREADS, 0, st>>>(a);
         g_launches++;
     }
     return cudaGetLastError();
@@ -464,6 +488,7 @@ cudaError_t launch_replicas(const NodeTable& nt, int policy, const ReplicaArgs& 
     if (a.T == 0 || nt.N == 0) return cudaSuccess;
     return with_label_width(nt.W, [&](auto w) {
         constexpr int W_ = decltype(w)::value;
+        if (policy == KS_SCORE_MOST_ALLOCATED) return rep_sequence<W_, KS_SCORE_MOST_ALLOCATED>(nt, a, st);
         return policy == KS_SCORE_LEFTOVER ? rep_sequence<W_, KS_SCORE_LEFTOVER>(nt, a, st)
                                            : rep_sequence<W_, KS_SCORE_LEAST_ALLOCATED>(nt, a, st);
     });

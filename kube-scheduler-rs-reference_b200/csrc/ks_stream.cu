@@ -129,9 +129,11 @@ __device__ __forceinline__ void stream_round_scan(const StreamBatchArgs& a, cons
 #pragma unroll
             for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
             if (rc <= fc && rm <= fm && miss == 0) {
-                const int64_t key = a.policy == KS_SCORE_LEFTOVER
-                                        ? leftover_key(fc, fm)
-                                        : least_alloc_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm);
+                const int64_t key =
+                    a.policy == KS_SCORE_LEFTOVER ? leftover_key(fc, fm)
+                    : a.policy == KS_SCORE_MOST_ALLOCATED
+                        ? most_alloc_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm)
+                        : least_alloc_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm);
                 if (key > best) { // ascending n per lane: strict '>' keeps the lowest index
                     best = key;
                     bidx = (int32_t)n;
