@@ -406,7 +406,8 @@ impl Gpu {
     /// argmax, with the earlier copies bound, and the row with the cluster's capacity for the pod.  Nothing is charged.
     /// Returns per pair the row and the node names of the placed copies in placement order (shorter than the request
     /// when the capacity is).  Err = the library's status (KS_ERR_NO_DEVICE on a packing-only context).  `policy`:
-    /// KS_SCORE_LEFTOVER, KS_SCORE_LEAST_ALLOCATED or KS_SCORE_MOST_ALLOCATED (bin-packing: fills busy nodes first).
+    /// KS_SCORE_LEFTOVER, KS_SCORE_LEAST_ALLOCATED, KS_SCORE_MOST_ALLOCATED (bin-packing: fills busy nodes first) or
+    /// KS_SCORE_LEAST_BALANCED (the default scheduler's choice; its copies are placed one at a time).
     pub fn place_replicas(&self, specs: &[(corev1::Pod, u32)], policy: i32)
                           -> Result<Vec<(ks_replica_plan, Vec<String>)>, i32> {
         let pv: Vec<PodView> = specs.iter().map(|(p, _)| PodView::new(p)).collect();

@@ -18,6 +18,8 @@ pub const KS_SCORE_LEFTOVER: c_int = 0;
 pub const KS_SCORE_LEAST_ALLOCATED: c_int = 1;
 /// Bin-packing (upstream MostAllocated); 2 is reserved and rejected.
 pub const KS_SCORE_MOST_ALLOCATED: c_int = 3;
+/// Upstream's default profile: LeastAllocated + BalancedAllocation, in [0, 200].
+pub const KS_SCORE_LEAST_BALANCED: c_int = 4;
 pub const KS_MEM_HOST: i32 = 0;
 pub const KS_MEM_DEVICE: i32 = 1;
 pub const KS_ERR_NO_DEVICE: c_int = -8; // packing-only context or no CUDA device

@@ -58,6 +58,22 @@ extern "C" {
  * 200 MB memory) are not added.  Every call that takes a policy takes this one, and ks_select runs it on both kernel
  * paths; its bit-parallel order is built on the first call that needs it after each snapshot change. */
 #define KS_SCORE_MOST_ALLOCATED 3
+/* KS_SCORE_LEAST_BALANCED: upstream's default resource scoring, NodeResourcesFit (LeastAllocated) plus
+ * NodeResourcesBalancedAllocation, each with weight 1, for cpu and memory.  With allocatable A, free f and request q:
+ *   least    = the KS_SCORE_LEAST_ALLOCATED score, in [0, 100] on feasible cells
+ *   u_r      = clamp(A_r - (f_r - q_r), 0, A_r)                            (int64, as KS_SCORE_MOST_ALLOCATED)
+ *   x_r      = (double)u_r / (double)A_r for each resource with A_r > 0 (each operand rounded to nearest even, then
+ *              one IEEE division; a resource with A_r <= 0 is skipped)
+ *   std      = |x_cpu - x_mem| / 2 when both resources are kept, else 0
+ *   balanced = (int64) trunc((1 - std) * 100), each operation one IEEE double operation rounded to nearest, in [0, 100]
+ *   score    = least + balanced,   in [0, 200]
+ * Every kernel path computes `balanced' with the same correctly rounded operations (no FMA contraction, no reciprocal),
+ * so every call returns the same score bit for bit.  Departures from upstream: its non-zero request defaults are not
+ * added, u has a lower clamp (free > allocatable), and ties go to the lowest node index instead of a random one.  Every
+ * call that takes a policy takes this one.  ks_select runs it on both kernel paths, and KS_SELECT_AUTO chooses between
+ * them by the same P * N >= 2^24 rule as for the other policies; its bit-parallel order is built on the first call that
+ * needs it after each snapshot change.  ks_place_replicas places its copies one at a time (see there). */
+#define KS_SCORE_LEAST_BALANCED 4
 
 /* where caller-owned buffers live */
 #define KS_MEM_HOST 0
@@ -474,7 +490,8 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods /* host space */, co
  *      the plan is the first `placed' of all (node, copy) pairs ordered by score descending, node ascending, copy
  *      ascending.  Under MOST_ALLOCATED every s_n(j) is non-decreasing in j: the node being filled never loses to a node
  *      not yet touched, so the plan fills the nodes one after another in order of s_n(0) descending, node ascending,
- *      each with up to c_n copies, and the copies of one node are contiguous in placement order;
+ *      each with up to c_n copies, and the copies of one node are contiguous in placement order.  Under LEAST_BALANCED
+ *      s_n(j) can rise or fall with j: the copies are placed one at a time, exactly as defined;
  *   3. out[t]: capacity = sum of c_n (saturating: UINT64_MAX also means unbounded), placed, nodes = distinct nodes among
  *      the placed copies, feasible_cnt = nodes with c_n >= 1 (ks_select's feasible_cnt), max_per_node = most copies on one
  *      node, last_score = score of copy placed - 1 (0 when nothing is placed);
@@ -493,7 +510,11 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods /* host space */, co
  * the specs and n * 32 bytes of rows, plus 12 bytes per requested copy with a copy list (up to 192 MiB at
  * KS_REPLICAS_MAX_TOTAL); its device scratch block holds the search state, plus 20 bytes per requested copy with a copy
  * list (up to 320 MiB).  Like every staging block these grow to the largest call and are kept until
- * ks_snapshot_destroy; ks_gang_bind, ks_drain_check, ks_stream_bind and ks_scaleup_estimate share them. */
+ * ks_snapshot_destroy; ks_gang_bind, ks_drain_check, ks_stream_bind and ks_scaleup_estimate share them.
+ * KS_SCORE_LEAST_BALANCED: the scan, then one CTA per spec (specs strided over at most 2 per SM) places that spec's copies
+ * one after another, so the time grows with the copies of the largest spec (about 4 us per copy on an H100, DESIGN.md
+ * 5j) and no fixed number of passes holds.  Its device scratch block also holds 12 bytes per node for each of those
+ * CTAs, as many CTAs as fit in 64 MiB (at least one). */
 #define KS_REPLICAS_MAX_SPECS 4096u
 #define KS_REPLICAS_MAX 65536u
 #define KS_REPLICAS_MAX_TOTAL (1u << 24)

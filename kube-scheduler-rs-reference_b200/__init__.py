@@ -8,6 +8,7 @@ missing libksched.so raises at import time.
 """
 from ._capi import (  # noqa: F401
     KS_OK, KS_MEM_HOST, KS_MEM_DEVICE, KS_SCORE_LEFTOVER, KS_SCORE_LEAST_ALLOCATED, KS_SCORE_MOST_ALLOCATED,
+    KS_SCORE_LEAST_BALANCED,
     KS_SELECT_AUTO, KS_SELECT_FORCE_DIRECT, KS_SELECT_FORCE_BITPAR, KS_SELECT_TIMING, KS_SELECT_NO_GRAPH,
     KS_CELL_OK, KS_CELL_NOT_ENOUGH_RESOURCES, KS_CELL_NODE_SELECTOR_MISMATCH,
     KsError, lib, LIB_PATH, declared_symbols, mask_row_bytes, mask_row_bytes_aligned, device_count, launch_count,

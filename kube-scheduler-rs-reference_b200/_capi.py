@@ -20,6 +20,7 @@ KS_OK = 0
 KS_MEM_HOST, KS_MEM_DEVICE = 0, 1
 KS_SCORE_LEFTOVER, KS_SCORE_LEAST_ALLOCATED = 0, 1
 KS_SCORE_MOST_ALLOCATED = 3  # bin-packing; 2 is reserved and rejected
+KS_SCORE_LEAST_BALANCED = 4  # upstream's default profile: LeastAllocated + BalancedAllocation
 KS_SELECT_AUTO, KS_SELECT_FORCE_DIRECT, KS_SELECT_FORCE_BITPAR, KS_SELECT_TIMING, KS_SELECT_NO_GRAPH = 0, 1, 2, 4, 8
 KS_CELL_OK, KS_CELL_NOT_ENOUGH_RESOURCES, KS_CELL_NODE_SELECTOR_MISMATCH = 0, 1, 2
 KS_ERR_NO_DEVICE = -8

@@ -96,7 +96,8 @@ static int check_range_and_prio(ks_snapshot* s, cudaStream_t st) {
 }
 
 static bool valid_policy(int policy) {
-    return policy == KS_SCORE_LEFTOVER || policy == KS_SCORE_LEAST_ALLOCATED || policy == KS_SCORE_MOST_ALLOCATED;
+    return policy == KS_SCORE_LEFTOVER || policy == KS_SCORE_LEAST_ALLOCATED || policy == KS_SCORE_MOST_ALLOCATED ||
+           policy == KS_SCORE_LEAST_BALANCED;
 }
 static bool valid_space(int32_t space) { return space == KS_MEM_HOST || space == KS_MEM_DEVICE; }
 static bool valid_label_words(uint32_t W) { return W == 1 || W == 2 || W == 4 || W == 8; }
@@ -587,7 +588,7 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
         PartialView part{nullptr, nullptr, nullptr};
         if (use_bitpar) {
             cudaError_t e = bitpar_prepare(s->bp, L.pv.P);
-            if (e == cudaSuccess && policy == KS_SCORE_MOST_ALLOCATED) e = bitpar_prepare_most(s->bp, L.nt, st);
+            if (e == cudaSuccess) e = bitpar_prepare_order(s->bp, L.nt, policy, st);
             if (e != cudaSuccess) return fail(KS_ERR_CUDA, "bit-parallel prepare failed: %s", cudaGetErrorString(e));
         } else {
             grid = direct_grid(s->W, L.pv.P, s->Npad, s->sms);
@@ -1543,7 +1544,10 @@ int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* repl
     replica_chunks(s->N, (uint32_t)T, s->sms, &n_chunks, &chunk_len);
     const uint64_t C = copies ? total : 0;
     // in = [rc T | rm T | sel T*W | replicas T | offset T], results = [rows T | score C | node C],
-    // work = [search state T | chunk partials T*n_chunks | copy scores C | copy nodes C | sort indices 2C]
+    // work = [search state T | chunk partials T*n_chunks | copy scores C | copy nodes C | sort indices 2C], and under
+    // KS_SCORE_LEAST_BALANCED [scores | copies placed] per node and k_rep_seq CTA
+    uint32_t seq_ctas = 0, seq_block = 0;
+    if (policy == KS_SCORE_LEAST_BALANCED) replica_seq_grid(s->N, (uint32_t)T, s->sms, &seq_ctas, &seq_block);
     BlockLayout in, res, work;
     const size_t i_rc = in.take<int64_t>(T), i_rm = in.take<int64_t>(T), i_sel = in.take<uint64_t>(T * W),
                  i_rep = in.take<uint32_t>(T), i_off = in.take<uint64_t>(T);
@@ -1551,6 +1555,8 @@ int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* repl
     const size_t w_spec = work.take<uint8_t>(replica_spec_bytes((uint32_t)T), 16),
                  w_chunk = work.take<uint8_t>(replica_chunk_bytes((uint32_t)T, n_chunks), 16),
                  w_score = work.take<int64_t>(C), w_node = work.take<int32_t>(C), w_sort = work.take<uint32_t>(2 * C);
+    const size_t w_seq_score = work.take<int64_t>((uint64_t)seq_ctas * s->N),
+                 w_seq_placed = work.take<uint32_t>((uint64_t)seq_ctas * s->N);
     uint8_t* h_out = nullptr;
     rc = stage_blocks(s, in.size, res.size, &h_out);
     if (rc) return rc;
@@ -1588,7 +1594,12 @@ int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* repl
     a.sort_buf = copies ? at<uint32_t>(d_work, w_sort) : nullptr;
     a.n_chunks = n_chunks;
     a.chunk_len = chunk_len;
-    cudaError_t e = launch_replicas(node_table(s), policy, a, st);
+    ReplicaSeqArgs q;
+    q.score = seq_ctas ? at<int64_t>(d_work, w_seq_score) : nullptr;
+    q.placed = seq_ctas ? at<uint32_t>(d_work, w_seq_placed) : nullptr;
+    q.ctas = seq_ctas;
+    q.block = seq_block;
+    cudaError_t e = launch_replicas(node_table(s), policy, a, q, st);
     if (e != cudaSuccess) return fail(KS_ERR_CUDA, "replica placement launch failed: %s", cudaGetErrorString(e));
     CU_TRY(cudaMemcpyAsync(h_out, d_out, res.size, cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaStreamSynchronize(st));

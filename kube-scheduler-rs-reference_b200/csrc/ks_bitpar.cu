@@ -16,6 +16,7 @@
 //                  k_first_fit_head/_tail  argmax KS_SCORE_LEFTOVER = first feasible node in priority order (early exit)
 //                  k_least_alloc    argmax KS_SCORE_LEAST_ALLOCATED: bound-ordered scan, exact scores, early exit
 //                  k_most_alloc     argmax KS_SCORE_MOST_ALLOCATED: the same scan over its own order (built lazily)
+//                  k_least_balanced argmax KS_SCORE_LEAST_BALANCED: the same scan over another order (built lazily)
 // Semantics per cell are exactly predicates.rs:42 / :45-61 (see include/ksched.h); only the evaluation
 // order differs, and every output is compared bit-for-bit with the oracle in tests/.
 #include "ks_bitpar.h"
@@ -1187,9 +1188,12 @@ __global__ void __launch_bounds__(256)
 // stops once that bound of everything left is strictly below the best exact score.  A negative request voids the bound.
 // Built only when a MOST_ALLOCATED call needs it: one CTA sorts the nodes stably on 200 - b(n) (one 8-bit radix pass of
 // ks_sort.cuh), then k_build_tiles and k_build_eval fill the tile index and the evaluation rows in that order.
-__global__ void __launch_bounds__(SORT_THREADS)
-    k_most_order(NodeTable nt, uint32_t Nord, uint32_t* __restrict__ buf, int32_t* __restrict__ ord_idx,
-                 int64_t* __restrict__ ord_b, long long* __restrict__ amin) {
+// bound_order is that CTA for any order: `key' is the node's 8-bit sort digit (ascending = bound descending) and `val'
+// the bound stored for it.
+template <class Key, class Val>
+__device__ __forceinline__ void bound_order(const NodeTable& nt, uint32_t Nord, uint32_t* __restrict__ buf,
+                                            int32_t* __restrict__ ord_idx, int64_t* __restrict__ ord_b,
+                                            long long* __restrict__ amin, Key key, Val val) {
     __shared__ SortShared s;
     __shared__ long long s_min[2];
     const uint32_t N = nt.N;
@@ -1209,15 +1213,55 @@ __global__ void __launch_bounds__(SORT_THREADS)
         amin[0] = s_min[0];
         amin[1] = s_min[1];
     }
-    auto b = [&](uint32_t n) {
-        return most_alloc_term(nt.free_cpu[n], nt.alloc_cpu[n], 0) + most_alloc_term(nt.free_mem[n], nt.alloc_mem[n], 0);
-    };
-    cta_radix_pass(buf, buf + N, N, [&](uint32_t n) { return (uint32_t)(200 - b(n)); }, s);
+    cta_radix_pass(buf, buf + N, N, key, s);
     for (uint32_t k = threadIdx.x; k < Nord; k += SORT_THREADS) {
         const int32_t n = k < N ? (int32_t)buf[N + k] : -1;
         ord_idx[k] = n;
-        ord_b[k] = n >= 0 ? b((uint32_t)n) : -1; // padding: below every bound, never feasible
+        ord_b[k] = n >= 0 ? val((uint32_t)n) : -1; // padding: below every bound, never feasible
     }
+}
+__global__ void __launch_bounds__(SORT_THREADS)
+    k_most_order(NodeTable nt, uint32_t Nord, uint32_t* __restrict__ buf, int32_t* __restrict__ ord_idx,
+                 int64_t* __restrict__ ord_b, long long* __restrict__ amin) {
+    auto b = [&](uint32_t n) {
+        return most_alloc_term(nt.free_cpu[n], nt.alloc_cpu[n], 0) + most_alloc_term(nt.free_mem[n], nt.alloc_mem[n], 0);
+    };
+    bound_order(nt, Nord, buf, ord_idx, ord_b, amin, [&](uint32_t n) { return (uint32_t)(200 - b(n)); }, b);
+}
+
+// ---- argmax of KS_SCORE_LEAST_BALANCED: the same scan over an order of its own (DESIGN.md 5j has the proof) ----
+// b(n) = least_alloc_bound(n) + bal(n), bal(n) an integer upper bound of the balanced term at q = 0:
+//   P_r = most_alloc_term(f_r, A_r, 0) = floor(100 * x_r(0)), so |x_c(0) - x_m(0)| > (|P_c - P_m| - 1) / 100 and
+//   bal(n) = 100 - floor(max(0, |P_c - P_m| - 1) / 2) >= 100 - 50 * |x_c(0) - x_m(0)|   (100 when some A_r <= 0).
+// For q >= 0 each share rises by at most min(1, q_r / m_r) <= C / 100, C = max_r min(100, ceil(q_r * 100 / m_r)), so the
+// gap falls by at most C / 100 and the real-valued balanced term by at most C / 2; the double evaluation of balanced_int
+// lies within 2^-43 of the real value, so trunc() of it is <= bal(n) + E with E = ceil(C / 2).  LEAST_ALLOCATED's
+// per-pod slack D (k_least_alloc) bounds the other term: every feasible cell scores <= b(n) - D + E.  b(n) lies in
+// [0, 200] unless free exceeds the allocatable or is negative: such nodes sort first with the bound LB_UNBOUNDED (no
+// early exit while one is left), or last with the bound 0 (they are infeasible for q >= 0); either way the stored bound
+// is >= b(n) and descending, which is all the early exit needs.
+constexpr int64_t LB_UNBOUNDED = 1ll << 62; // above every b(n) inside the limits of ksched.h, and below 2^63 - any D
+__device__ __forceinline__ int64_t balanced_bound(int64_t fc, int64_t fm, int64_t ac, int64_t am) {
+    if (ac <= 0 || am <= 0) return 100;
+    const int64_t d = llabs(most_alloc_term(fc, ac, 0) - most_alloc_term(fm, am, 0));
+    return 100 - (d > 0 ? (d - 1) / 2 : 0);
+}
+__device__ __forceinline__ int64_t least_balanced_bound(const NodeTable& nt, uint32_t n) {
+    return least_alloc_bound(nt, n) + balanced_bound(nt.free_cpu[n], nt.free_mem[n], nt.alloc_cpu[n], nt.alloc_mem[n]);
+}
+__global__ void __launch_bounds__(SORT_THREADS)
+    k_balanced_order(NodeTable nt, uint32_t Nord, uint32_t* __restrict__ buf, int32_t* __restrict__ ord_idx,
+                     int64_t* __restrict__ ord_b, long long* __restrict__ amin) {
+    bound_order(
+        nt, Nord, buf, ord_idx, ord_b, amin,
+        [&](uint32_t n) { // 0: above 200; 1..201: 200 down to 0
+            const int64_t b = least_balanced_bound(nt, n);
+            return b > 200 ? 0u : (uint32_t)(201 - (b > 0 ? b : 0));
+        },
+        [&](uint32_t n) {
+            const int64_t b = least_balanced_bound(nt, n);
+            return b > 200 ? LB_UNBOUNDED : (b > 0 ? b : 0);
+        });
 }
 
 // min(100, ceil(q * 100 / m)) for q >= 0, m > 0 (m may be LLONG_MAX: no node has a positive allocatable)
@@ -1227,11 +1271,20 @@ __device__ __forceinline__ int64_t most_alloc_slack(int64_t q, long long m) {
     return c < 100 ? c : 100;
 }
 
-template <int W>
-__global__ void __launch_bounds__(256)
-    k_most_alloc(const uint8_t* __restrict__ blobM, TileBuckets bk, RowsLayout lay, const NodeEval* __restrict__ ev,
-                 const int64_t* __restrict__ ordM_b, const long long* __restrict__ amin, PodView pv,
-                 const uint2* __restrict__ rk, OutView ov, PeerOut po, const unsigned long long* __restrict__ live, uint32_t N) {
+// The highest score a cell in a slot with bound `top' can have: MOST_ALLOCATED (b + D) / 2, LEAST_BALANCED b - D
+template <bool MOST>
+__device__ __forceinline__ int64_t limit(int64_t top, int64_t D) { return MOST ? (top + D) / 2 : top - D; }
+
+// The walk of k_most_alloc and k_least_balanced: k_least_alloc's windows over an order of their own, exact scores
+// (alloc_score), and the early exit of each policy in front of every tile with a feasible slot.
+template <int W, int POLICY>
+__device__ __forceinline__ void bound_walk(const uint8_t* __restrict__ blob, const TileBuckets& bk, const RowsLayout& lay,
+                                           const NodeEval* __restrict__ ev, const int64_t* __restrict__ ord_b,
+                                           const long long* __restrict__ amin, const PodView& pv,
+                                           const uint2* __restrict__ rk, const OutView& ov, const PeerOut& po,
+                                           const unsigned long long* __restrict__ live, uint32_t N) {
+    static_assert(POLICY == KS_SCORE_MOST_ALLOCATED || POLICY == KS_SCORE_LEAST_BALANCED, "a bound-ordered policy");
+    constexpr bool MOST = POLICY == KS_SCORE_MOST_ALLOCATED;
     __shared__ uint4 s_mask[LA_MAX_WARPS][32][2]; // per warp: the feasibility masks of the current window of tiles
     __shared__ int64_t s_top[LA_MAX_WARPS][32];   //           and the bound of the first slot of each of them
     const uint32_t lane = threadIdx.x & 31, wq = lane & 7, quarter = lane >> 3, wid = threadIdx.x >> 5;
@@ -1252,7 +1305,17 @@ __global__ void __launch_bounds__(256)
         }
         const int64_t rc = __ldg(pv.req_cpu + p), rm = __ldg(pv.req_mem + p);
         const bool bounded = rc >= 0 && rm >= 0; // else the bound does not hold: no early exit
-        const int64_t D = bounded ? most_alloc_slack(rc, mc) + most_alloc_slack(rm, mm) : 0;
+        // MOST_ALLOCATED: every feasible cell scores <= (b + D) / 2.  LEAST_BALANCED: <= b - D, D = LEAST_ALLOCATED's slack
+        // (k_least_alloc) minus E
+        int64_t D = 0;
+        if (MOST) {
+            D = bounded ? most_alloc_slack(rc, mc) + most_alloc_slack(rm, mm) : 0;
+        } else if (bounded) {
+            const longlong2 amax = *reinterpret_cast<const longlong2*>(live + KS_MAX_LABEL_WORDS);
+            const int64_t dl = ((amax.x > 0 ? (rc * 100) / amax.x : 0) + (amax.y > 0 ? (rm * 100) / amax.y : 0)) / 2;
+            const int64_t sc = most_alloc_slack(rc, mc), sm = most_alloc_slack(rm, mm);
+            D = dl - ((sc > sm ? sc : sm) + 1) / 2;
+        }
         int64_t best = INT64_MIN;
         int32_t bidx = -1;
         // windows of tiles as in k_least_alloc: phase A derives a window's feasibility masks (lane j: tile k0 + j), phase
@@ -1260,14 +1323,15 @@ __global__ void __launch_bounds__(256)
         uint32_t k0 = 0, win = LA_FIRST_WINDOW;
         bool done = dead;
         while (!done && k0 < lay.n_tiles) {
-            if (k0 > 0 && bounded && bidx >= 0 && best > (__ldg(ordM_b + (size_t)k0 * BP_TILE) + D) / 2) break; // warp-uniform
+            if (k0 > 0 && bounded && bidx >= 0 && best > limit<MOST>(__ldg(ord_b + (size_t)k0 * BP_TILE), D))
+                break; // warp-uniform
             {
                 uint32_t m[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
                 int64_t top = INT64_MIN;
                 const uint32_t kt = k0 + lane;
                 if (lane < win && kt < lay.n_tiles) {
-                    ptile_mask<W>(blobM, lay, tile_ranks(t, kt), sel, kt, m);
-                    top = __ldg(ordM_b + (size_t)kt * BP_TILE);
+                    ptile_mask<W>(blob, lay, tile_ranks(t, kt), sel, kt, m);
+                    top = __ldg(ord_b + (size_t)kt * BP_TILE);
                 }
                 s_mask[wid][lane][0] = make_uint4(m[0], m[1], m[2], m[3]);
                 s_mask[wid][lane][1] = make_uint4(m[4], m[5], m[6], m[7]);
@@ -1279,7 +1343,7 @@ __global__ void __launch_bounds__(256)
                 const uint32_t j = __ffs(ne) - 1;
                 ne &= ne - 1;
                 const uint32_t k = k0 + j;
-                if (bounded && bidx >= 0 && best > (s_top[wid][j] + D) / 2) { // warp-uniform: nothing left can win or tie
+                if (bounded && bidx >= 0 && best > limit<MOST>(s_top[wid][j], D)) { // warp-uniform: nothing left can win or tie
                     done = true;
                     break;
                 }
@@ -1291,7 +1355,7 @@ __global__ void __launch_bounds__(256)
                     const uint32_t b = quarter + 4u * i;
                     if (!((bits >> b) & 1u)) continue;
                     const NodeEval e = ev[(size_t)k * BP_TILE + wq * 32 + b];
-                    const int64_t sc = most_alloc_int(e.fc, e.fm, e.ac, e.am, rc, rm);
+                    const int64_t sc = alloc_score<POLICY>(e.fc, e.fm, e.ac, e.am, rc, rm);
                     if (sc > best || (sc == best && e.idx < bidx)) {
                         best = sc;
                         bidx = e.idx;
@@ -1329,6 +1393,22 @@ __global__ void __launch_bounds__(256)
         if (threadIdx.x == 0) trace_end(TR_ARGMAX1_END);
     }
     exchange_signal(po);
+}
+
+template <int W>
+__global__ void __launch_bounds__(256)
+    k_most_alloc(const uint8_t* __restrict__ blobM, TileBuckets bk, RowsLayout lay, const NodeEval* __restrict__ ev,
+                 const int64_t* __restrict__ ordM_b, const long long* __restrict__ amin, PodView pv,
+                 const uint2* __restrict__ rk, OutView ov, PeerOut po, const unsigned long long* __restrict__ live, uint32_t N) {
+    bound_walk<W, KS_SCORE_MOST_ALLOCATED>(blobM, bk, lay, ev, ordM_b, amin, pv, rk, ov, po, live, N);
+}
+template <int W>
+__global__ void __launch_bounds__(256)
+    k_least_balanced(const uint8_t* __restrict__ blobB, TileBuckets bk, RowsLayout lay, const NodeEval* __restrict__ ev,
+                     const int64_t* __restrict__ ordB_b, const long long* __restrict__ amin, PodView pv,
+                     const uint2* __restrict__ rk, OutView ov, PeerOut po, const unsigned long long* __restrict__ live,
+                     uint32_t N) {
+    bound_walk<W, KS_SCORE_LEAST_BALANCED>(blobB, bk, lay, ev, ordB_b, amin, pv, rk, ov, po, live, N);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -1376,7 +1456,7 @@ BitparIndex::~BitparIndex() {
 
 cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cudaStream_t st) {
     ix.valid = false;
-    ix.validM = false; // the MOST_ALLOCATED order follows on the next call that needs it (bitpar_prepare_most)
+    ix.ordM.valid = ix.ordB.valid = false; // these orders follow on the next call that needs them (bitpar_prepare_order)
     ix.N = nt.N;
     ix.W = nt.W;
     if (nt.N == 0) return cudaSuccess;
@@ -1462,31 +1542,35 @@ cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cu
     return cudaSuccess;
 }
 
-cudaError_t bitpar_prepare_most(BitparIndex& ix, const NodeTable& nt, cudaStream_t st) {
+cudaError_t bitpar_prepare_order(BitparIndex& ix, const NodeTable& nt, int policy, cudaStream_t st) {
+    if (policy != KS_SCORE_MOST_ALLOCATED && policy != KS_SCORE_LEAST_BALANCED) return cudaSuccess;
     if (!ix.valid) return cudaErrorNotSupported;
-    if (ix.validM) return cudaSuccess;
+    BoundOrder& o = policy == KS_SCORE_MOST_ALLOCATED ? ix.ordM : ix.ordB;
+    if (o.valid) return cudaSuccess;
     cudaError_t e;
     const uint32_t Nord = ix.Nord;
-    if ((e = ix.ordM_b.ensure((size_t)Nord * sizeof(int64_t))) != cudaSuccess) return e;
-    if ((e = ix.ordM_idx.ensure((size_t)Nord * sizeof(int32_t))) != cudaSuccess) return e;
-    if ((e = ix.evalM.ensure((size_t)Nord * sizeof(NodeEval))) != cudaSuccess) return e;
-    if ((e = ix.hintM.ensure((size_t)Nord * sizeof(float4))) != cudaSuccess) return e;
-    if ((e = ix.sortM.ensure(2ull * nt.N * sizeof(uint32_t) + 2 * sizeof(long long))) != cudaSuccess) return e;
-    if ((e = ix.blobM.ensure((size_t)ix.lay_r.ncb * ix.lay_r.cb_stride)) != cudaSuccess) return e;
-    if ((e = ix.bucketsM.ensure(tile_buckets(nullptr, nt.N, ix.lay_r, nullptr))) != cudaSuccess) return e;
-    long long* amin = reinterpret_cast<long long*>(ix.sortM.as<uint32_t>() + 2ull * nt.N);
-    k_most_order<<<1, SORT_THREADS, 0, st>>>(nt, Nord, ix.sortM.as<uint32_t>(), ix.ordM_idx.as<int32_t>(),
-                                             ix.ordM_b.as<int64_t>(), amin);
+    if ((e = o.b.ensure((size_t)Nord * sizeof(int64_t))) != cudaSuccess) return e;
+    if ((e = o.idx.ensure((size_t)Nord * sizeof(int32_t))) != cudaSuccess) return e;
+    if ((e = o.eval.ensure((size_t)Nord * sizeof(NodeEval))) != cudaSuccess) return e;
+    if ((e = o.hint.ensure((size_t)Nord * sizeof(float4))) != cudaSuccess) return e;
+    if ((e = o.sort.ensure(2ull * nt.N * sizeof(uint32_t) + 2 * sizeof(long long))) != cudaSuccess) return e;
+    if ((e = o.blob.ensure((size_t)ix.lay_r.ncb * ix.lay_r.cb_stride)) != cudaSuccess) return e;
+    if ((e = o.buckets.ensure(tile_buckets(nullptr, nt.N, ix.lay_r, nullptr))) != cudaSuccess) return e;
+    long long* amin = reinterpret_cast<long long*>(o.sort.as<uint32_t>() + 2ull * nt.N);
+    if (policy == KS_SCORE_MOST_ALLOCATED)
+        k_most_order<<<1, SORT_THREADS, 0, st>>>(nt, Nord, o.sort.as<uint32_t>(), o.idx.as<int32_t>(), o.b.as<int64_t>(), amin);
+    else
+        k_balanced_order<<<1, SORT_THREADS, 0, st>>>(nt, Nord, o.sort.as<uint32_t>(), o.idx.as<int32_t>(), o.b.as<int64_t>(),
+                                                     amin);
     TileBuckets bk;
-    tile_buckets(ix.bucketsM.p, nt.N, ix.lay_r, &bk);
+    tile_buckets(o.buckets.p, nt.N, ix.lay_r, &bk);
     k_build_tiles<<<ix.lay_r.ncb * RW_TILES, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(),
-                                                          ix.ordM_idx.as<int32_t>(), ix.blobM.as<uint8_t>(), ix.lay_r,
-                                                          nullptr, bk);
-    k_build_eval<<<(Nord + 255) / 256, 256, 0, st>>>(nt, ix.ordM_idx.as<int32_t>(), Nord, ix.evalM.as<NodeEval>(),
-                                                     ix.hintM.as<float4>());
+                                                          o.idx.as<int32_t>(), o.blob.as<uint8_t>(), ix.lay_r, nullptr, bk);
+    k_build_eval<<<(Nord + 255) / 256, 256, 0, st>>>(nt, o.idx.as<int32_t>(), Nord, o.eval.as<NodeEval>(),
+                                                     o.hint.as<float4>());
     g_launches += 3;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    ix.validM = true;
+    o.valid = true;
     return cudaSuccess;
 }
 
@@ -1593,15 +1677,21 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
         if ((e = cudaMemsetAsync(tail_count, 0, sizeof(uint32_t), bs)) != cudaSuccess) return e;
         const bool least_alloc = L.policy == KS_SCORE_LEAST_ALLOCATED;
         TileBuckets bk;
-        if (L.policy == KS_SCORE_MOST_ALLOCATED) {
-            if (!ix.validM) return cudaErrorNotSupported; // bitpar_prepare_most runs first
-            tile_buckets(ix.bucketsM.p, ix.N, ix.lay_r, &bk);
+        if (L.policy == KS_SCORE_MOST_ALLOCATED || L.policy == KS_SCORE_LEAST_BALANCED) {
+            const BoundOrder& o = L.policy == KS_SCORE_MOST_ALLOCATED ? ix.ordM : ix.ordB;
+            if (!o.valid) return cudaErrorNotSupported; // bitpar_prepare_order runs first
+            tile_buckets(o.buckets.p, ix.N, ix.lay_r, &bk);
             const uint32_t wpc = at / 32; // one warp per pod
             const uint32_t grid = (uint32_t)std::min<uint64_t>((uint64_t)sms * (2048 / at), ((uint64_t)P + wpc - 1) / wpc);
-            const long long* amin = reinterpret_cast<const long long*>(ix.sortM.as<uint32_t>() + 2ull * ix.N);
-            k_most_alloc<W><<<grid, at, 0, bs>>>(ix.blobM.as<uint8_t>(), bk, ix.lay_r, ix.evalM.as<NodeEval>(),
-                                                 ix.ordM_b.as<int64_t>(), amin, L.pv, ix.pod_ranks.as<uint2>(), L.ov, L.po,
-                                                 ix.live.as<unsigned long long>(), ix.N);
+            const long long* amin = reinterpret_cast<const long long*>(o.sort.as<uint32_t>() + 2ull * ix.N);
+            if (L.policy == KS_SCORE_MOST_ALLOCATED)
+                k_most_alloc<W><<<grid, at, 0, bs>>>(o.blob.as<uint8_t>(), bk, ix.lay_r, o.eval.as<NodeEval>(),
+                                                     o.b.as<int64_t>(), amin, L.pv, ix.pod_ranks.as<uint2>(), L.ov, L.po,
+                                                     ix.live.as<unsigned long long>(), ix.N);
+            else
+                k_least_balanced<W><<<grid, at, 0, bs>>>(o.blob.as<uint8_t>(), bk, ix.lay_r, o.eval.as<NodeEval>(),
+                                                         o.b.as<int64_t>(), amin, L.pv, ix.pod_ranks.as<uint2>(), L.ov,
+                                                         L.po, ix.live.as<unsigned long long>(), ix.N);
             g_launches++;
             if ((e = cudaGetLastError()) != cudaSuccess) return e;
         } else if (least_alloc) {

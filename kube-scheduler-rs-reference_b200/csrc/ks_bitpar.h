@@ -54,6 +54,19 @@ struct TileBuckets {
     unsigned long long* memb[2];
 };
 
+// The node order of a bound-ordered argmax that is built on the first call that needs it after each bitpar_build
+// (bitpar_prepare_order): every node's score bound, the tile index and evaluation rows in descending bound order.
+struct BoundOrder {
+    DevBuf b;       // [int64 Nord] bound of every node in descending order (ties by index), -1 for padding
+    DevBuf idx;     // [int32 Nord]
+    DevBuf eval;    // [NodeEval Nord] per slot of that order
+    DevBuf hint;    // [float4 Nord] written by k_build_eval, not read by the bound-ordered walks
+    DevBuf blob;    // lay_r.ncb column-block blobs in that order, read through L1/L2 by the walk
+    DevBuf buckets; // TileBuckets of blob
+    DevBuf sort;    // [uint32 2N] sort scratch, then [int64 2] smallest positive allocatable cpu / memory (8-aligned)
+    bool valid = false; // matches the current index
+};
+
 // The index of one snapshot.  Device arrays (element type in brackets) are grow-only buffers, read through .as<T>().
 // Owned by the snapshot and freed with it, with the snapshot's device current.
 struct BitparIndex {
@@ -76,14 +89,8 @@ struct BitparIndex {
     DevBuf hintL;     // [float4 Nord] per slot of that order: single-precision score model (pre-filter of k_least_alloc)
     DevBuf blobL;     // lay_r.ncb column-block blobs in that order, read through L1/L2 by k_least_alloc
     DevBuf bucketsL;  // TileBuckets of blobL
-    DevBuf ordM_b;    // [int64 Nord] KS_SCORE_MOST_ALLOCATED (built lazily, validM): bound b(n) of every node in descending
-                      // order (ties by index), -1 for padding
-    DevBuf ordM_idx;  // [int32 Nord]
-    DevBuf evalM;     // [NodeEval Nord] per slot of that order
-    DevBuf hintM;     // [float4 Nord] written by k_build_eval, not read by k_most_alloc
-    DevBuf blobM;     // lay_r.ncb column-block blobs in that order, read through L1/L2 by k_most_alloc
-    DevBuf bucketsM;  // TileBuckets of blobM
-    DevBuf sortM;     // [uint32 2N] sort scratch, then [int64 2] smallest positive allocatable cpu / memory (8-aligned)
+    BoundOrder ordM;  // KS_SCORE_MOST_ALLOCATED (k_most_alloc), built lazily
+    BoundOrder ordB;  // KS_SCORE_LEAST_BALANCED (k_least_balanced), built lazily
     DevBuf live;      // [uint64 KS_MAX_LABEL_WORDS + 2] label bits carried by at least one node, max allocatable cpu, memory
     DevBuf rec_s;     // [uint4] rows kernel: {threshold_cpu, threshold_mem, pod index, selector columns} per pod, P rounded up to 8
     DevBuf blobR;     // rows kernel: lay_r.ncb column-block blobs in node order
@@ -99,7 +106,6 @@ struct BitparIndex {
     DevBuf rk_perm;
     uint32_t N = 0, Nord = 0, W = 0, spl_stride = 1, n_spl = 0;
     bool valid = false;
-    bool validM = false; // the MOST_ALLOCATED order above matches the current index
     int sms = 0;
     Stream aux; // the argmax kernels run here, overlapped with k_mask_rows
     Event ev_fork, ev_join;
@@ -112,9 +118,10 @@ constexpr int BP_TRACE_WORDS = 16;
 cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cudaStream_t st);
 bool bitpar_profitable(const BitparIndex& ix, uint32_t P);
 cudaError_t bitpar_prepare(BitparIndex& ix, uint32_t P);
-// KS_SCORE_MOST_ALLOCATED's order, tile index and evaluation rows: built on the first call after each bitpar_build that
-// needs them (enqueued on st; must run before a stream-captured bitpar_select), a no-op after that
-cudaError_t bitpar_prepare_most(BitparIndex& ix, const NodeTable& nt, cudaStream_t st);
+// The order of `policy' (KS_SCORE_MOST_ALLOCATED, KS_SCORE_LEAST_BALANCED; a no-op for the others): built on the first
+// call after each bitpar_build that needs it (enqueued on st; must run before a stream-captured bitpar_select), a no-op
+// after that
+cudaError_t bitpar_prepare_order(BitparIndex& ix, const NodeTable& nt, int policy, cudaStream_t st);
 cudaError_t bitpar_select(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before_mask, cudaEvent_t after_mask);
 // slots of ks_last_trace (include/ksched.h); cudaErrorNotSupported unless the index was created under KS_TRACE=1
 cudaError_t bitpar_read_trace(const BitparIndex& ix, unsigned long long out_ns[BP_TRACE_WORDS]);

@@ -1195,21 +1195,26 @@ cudaError_t prepare_direct() {
     for (uint32_t W : {1u, 2u, 4u, 8u})
         with_label_width(W, [&](auto w) {
             constexpr int W_ = decltype(w)::value;
-            constexpr int LO = KS_SCORE_LEFTOVER, LA = KS_SCORE_LEAST_ALLOCATED, MA = KS_SCORE_MOST_ALLOCATED;
+            constexpr int LO = KS_SCORE_LEFTOVER, LA = KS_SCORE_LEAST_ALLOCATED, MA = KS_SCORE_MOST_ALLOCATED,
+                          LB = KS_SCORE_LEAST_BALANCED;
             opt_in(k_select_direct<W_, LO, true>, tile_smem_bytes<W_, false>());
             opt_in(k_select_direct<W_, LO, false>, tile_smem_bytes<W_, false>());
             opt_in(k_select_direct<W_, LA, true>, tile_smem_bytes<W_, true>());
             opt_in(k_select_direct<W_, LA, false>, tile_smem_bytes<W_, true>());
             opt_in(k_select_direct<W_, MA, true>, tile_smem_bytes<W_, true>());
             opt_in(k_select_direct<W_, MA, false>, tile_smem_bytes<W_, true>());
+            opt_in(k_select_direct<W_, LB, true>, tile_smem_bytes<W_, true>());
+            opt_in(k_select_direct<W_, LB, false>, tile_smem_bytes<W_, true>());
             opt_in(k_explain_counts<W_>, tile_smem_bytes<W_, false>());
             opt_in(k_select_topk<W_, LO>, tile_smem_bytes<W_, false>());
             opt_in(k_select_topk<W_, LA>, tile_smem_bytes<W_, true>());
             opt_in(k_select_topk<W_, MA>, tile_smem_bytes<W_, true>());
+            opt_in(k_select_topk<W_, LB>, tile_smem_bytes<W_, true>());
             opt_in(k_preempt_scan<W_>, tile_smem_bytes<W_, false>());
             opt_in(k_drain_scan<W_, LO>, tile_smem_bytes<W_, false>());
             opt_in(k_drain_scan<W_, LA>, tile_smem_bytes<W_, true>());
             opt_in(k_drain_scan<W_, MA>, tile_smem_bytes<W_, true>());
+            opt_in(k_drain_scan<W_, LB>, tile_smem_bytes<W_, true>());
             return e;
         });
     return e;
@@ -1238,6 +1243,9 @@ cudaError_t launch_select_direct(const SelectLaunch& L, const PartialView& part,
         if (L.policy == KS_SCORE_MOST_ALLOCATED)
             return emit ? launch_direct_t<W, KS_SCORE_MOST_ALLOCATED, true>(L, part, g)
                         : launch_direct_t<W, KS_SCORE_MOST_ALLOCATED, false>(L, part, g);
+        if (L.policy == KS_SCORE_LEAST_BALANCED)
+            return emit ? launch_direct_t<W, KS_SCORE_LEAST_BALANCED, true>(L, part, g)
+                        : launch_direct_t<W, KS_SCORE_LEAST_BALANCED, false>(L, part, g);
         return emit ? launch_direct_t<W, KS_SCORE_LEAST_ALLOCATED, true>(L, part, g)
                     : launch_direct_t<W, KS_SCORE_LEAST_ALLOCATED, false>(L, part, g);
     });
@@ -1278,6 +1286,7 @@ cudaError_t launch_select_topk(const NodeTable& nt, const PodView& pv, int polic
     return with_label_width(nt.W, [&](auto w) {
         constexpr int W = decltype(w)::value;
         if (policy == KS_SCORE_MOST_ALLOCATED) return launch_topk_t<W, KS_SCORE_MOST_ALLOCATED>(nt, pv, k, ov, part, g, st);
+        if (policy == KS_SCORE_LEAST_BALANCED) return launch_topk_t<W, KS_SCORE_LEAST_BALANCED>(nt, pv, k, ov, part, g, st);
         return policy == KS_SCORE_LEFTOVER ? launch_topk_t<W, KS_SCORE_LEFTOVER>(nt, pv, k, ov, part, g, st)
                                            : launch_topk_t<W, KS_SCORE_LEAST_ALLOCATED>(nt, pv, k, ov, part, g, st);
     });
@@ -1320,6 +1329,7 @@ cudaError_t launch_drain_round(const NodeTable& nt, const PodView& pv, const Dra
     return with_label_width(nt.W, [&](auto w) {
         constexpr int W = decltype(w)::value;
         if (policy == KS_SCORE_MOST_ALLOCATED) return launch_drain_t<W, KS_SCORE_MOST_ALLOCATED>(nt, pv, da, r, part, g, st);
+        if (policy == KS_SCORE_LEAST_BALANCED) return launch_drain_t<W, KS_SCORE_LEAST_BALANCED>(nt, pv, da, r, part, g, st);
         return policy == KS_SCORE_LEFTOVER ? launch_drain_t<W, KS_SCORE_LEFTOVER>(nt, pv, da, r, part, g, st)
                                            : launch_drain_t<W, KS_SCORE_LEAST_ALLOCATED>(nt, pv, da, r, part, g, st);
     });

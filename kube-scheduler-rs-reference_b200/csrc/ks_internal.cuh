@@ -125,11 +125,30 @@ __device__ __forceinline__ int64_t most_alloc_term(int64_t f, int64_t a, int64_t
 __device__ __forceinline__ int64_t most_alloc_int(int64_t fc, int64_t fm, int64_t ac, int64_t am, int64_t rc, int64_t rm) {
     return (most_alloc_term(fc, ac, rc) + most_alloc_term(fm, am, rm)) / 2;
 }
-// The score of a policy that reads the allocatables, chosen at compile time: MOST_ALLOCATED, else LEAST_ALLOCATED
+// The balanced term of KS_SCORE_LEAST_BALANCED (upstream NodeResourcesBalancedAllocation, include/ksched.h): the shares
+// x_r = u_r / A_r requested after placement, u_r clamped as in most_alloc_term, and trunc((1 - |x_c - x_m| / 2) * 100).
+// Every step is one correctly rounded double operation spelled as an intrinsic, so no flag can contract it to an FMA or
+// turn the division into a reciprocal: every kernel, and the restatement in the tests, gets the same bits.  In [0, 100].
+__device__ __forceinline__ int64_t balanced_int(int64_t fc, int64_t fm, int64_t ac, int64_t am, int64_t rc, int64_t rm) {
+    if (ac <= 0 || am <= 0) return 100; // a resource is skipped: std = 0
+    int64_t uc = ac - (fc - rc), um = am - (fm - rm);
+    uc = uc < 0 ? 0 : uc > ac ? ac : uc;
+    um = um < 0 ? 0 : um > am ? am : um;
+    const double xc = __ddiv_rn(__ll2double_rn(uc), __ll2double_rn(ac));
+    const double xm = __ddiv_rn(__ll2double_rn(um), __ll2double_rn(am));
+    const double sd = __ddiv_rn(fabs(__dsub_rn(xc, xm)), 2.0);
+    return __double2ll_rz(__dmul_rn(__dsub_rn(1.0, sd), 100.0));
+}
+__device__ __forceinline__ int64_t least_balanced_int(int64_t fc, int64_t fm, int64_t ac, int64_t am, int64_t rc, int64_t rm) {
+    return least_alloc_int(fc, fm, ac, am, rc, rm) + balanced_int(fc, fm, ac, am, rc, rm);
+}
+// The score of a policy that reads the allocatables, chosen at compile time: MOST_ALLOCATED, LEAST_BALANCED, else
+// LEAST_ALLOCATED
 template <int POLICY>
 __device__ __forceinline__ int64_t alloc_score(int64_t fc, int64_t fm, int64_t ac, int64_t am, int64_t rc, int64_t rm) {
-    return POLICY == KS_SCORE_MOST_ALLOCATED ? most_alloc_int(fc, fm, ac, am, rc, rm)
-                                             : least_alloc_int(fc, fm, ac, am, rc, rm);
+    return POLICY == KS_SCORE_MOST_ALLOCATED   ? most_alloc_int(fc, fm, ac, am, rc, rm)
+           : POLICY == KS_SCORE_LEAST_BALANCED ? least_balanced_int(fc, fm, ac, am, rc, rm)
+                                               : least_alloc_int(fc, fm, ac, am, rc, rm);
 }
 // Warp argmax over (key, idx) with idx < 0 for "no candidate": larger key wins, ties go to the lower node index.
 // Every lane ends with the result.

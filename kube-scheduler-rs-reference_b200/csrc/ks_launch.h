@@ -127,10 +127,20 @@ struct ReplicaArgs {
     uint32_t* sort_buf;               // [2 * sum of replicas], with out_node
     uint32_t n_chunks, chunk_len;     // node chunks per spec and nodes per chunk (a multiple of 256)
 };
+// KS_SCORE_LEAST_BALANCED places the copies one at a time (k_rep_seq): per CTA, device scratch for every node
+struct ReplicaSeqArgs {
+    int64_t* score;        // [ctas * N] current score of every node, INT64_MIN when it takes no further copy
+    uint32_t* placed;      // [ctas * N] copies placed on every node
+    uint32_t ctas, block;  // the grid, and nodes per block maximum
+};
 size_t replica_spec_bytes(uint32_t T);
 size_t replica_chunk_bytes(uint32_t T, uint32_t n_chunks);
 void replica_chunks(uint32_t N, uint32_t T, int sms, uint32_t* n_chunks, uint32_t* chunk_len);
-cudaError_t launch_replicas(const NodeTable& nt, int policy, const ReplicaArgs& a, cudaStream_t st);
+// KS_SCORE_LEAST_BALANCED's sequential placement: its CTAs (12 bytes of scratch per node each, 64 MiB in all or one
+// CTA's worth) and the nodes per block maximum
+void replica_seq_grid(uint32_t N, uint32_t T, int sms, uint32_t* ctas, uint32_t* block);
+cudaError_t launch_replicas(const NodeTable& nt, int policy, const ReplicaArgs& a, const ReplicaSeqArgs& q,
+                            cudaStream_t st);
 
 } // namespace ks
 

@@ -15,6 +15,8 @@
 // node ascending (include/ksched.h).  The same kernels compute that plan with G_n(S) = s_n(0) >= S ? k_n : 0: S* is the
 // s_n(0) of the last node that takes copies, the nodes above it take all k_n, the tie split fills the nodes at S* in node
 // order, and k_rep_order_most sorts on top - s_n(0) of each copy's node, which keeps a node's copies together.
+// Under LEAST_BALANCED s_n(j) can rise or fall with j, and neither shortcut holds: after k_rep_scan and k_rep_init,
+// k_rep_seq places the copies one at a time, one CTA per spec (specs strided over a grid sized to a scratch budget).
 #include "ks_launch.h"
 #include "ks_sort.cuh"
 
@@ -46,6 +48,20 @@ struct RepChunk {
     int64_t hi, lo;       // max s_n(0), min s_n(k_n - 1) over the chunk's nodes with k_n >= 1
     uint32_t feas, pad;
 };
+
+// k_rep_seq: a CTA keeps the current score of every node (int64, INT64_MIN once it holds no further copy) and its copies
+// placed so far (uint32) in device scratch, and the maximum of every block of `block' nodes, with its node, in shared
+// memory.  block = 1024 nodes up to REP_SEQ_BLOCKS * 1024 nodes, larger beyond.
+constexpr uint32_t REP_SEQ_BLOCKS = 2048;
+constexpr uint64_t REP_SEQ_BUDGET = 64ull << 20; // scratch of all k_rep_seq CTAs of a call (at least one CTA's)
+constexpr uint32_t REP_SEQ_NODE_BYTES = 12;
+
+void replica_seq_grid(uint32_t N, uint32_t T, int sms, uint32_t* ctas, uint32_t* block) {
+    const uint64_t fit = std::max<uint64_t>(1, REP_SEQ_BUDGET / ((uint64_t)std::max(N, 1u) * REP_SEQ_NODE_BYTES));
+    *ctas = (uint32_t)std::min<uint64_t>(std::min<uint64_t>(fit, std::max(T, 1u)), 2ull * (uint64_t)std::max(sms, 1));
+    const uint32_t per = 1024u * REP_SEQ_BLOCKS;
+    *block = 1024u * std::max(1u, (N + per - 1) / per);
+}
 
 size_t replica_spec_bytes(uint32_t T) { return (size_t)T * sizeof(RepSpec); }
 size_t replica_chunk_bytes(uint32_t T, uint32_t n_chunks) { return (size_t)T * n_chunks * sizeof(RepChunk); }
@@ -172,7 +188,7 @@ __global__ void __launch_bounds__(REP_THREADS) k_rep_scan(NodeTable nt, ReplicaA
         feas++;
         cap = sat_add(cap, cn);
         sumk += v.k;
-        if (v.k) {
+        if (v.k && POL != KS_SCORE_LEAST_BALANCED) { // k_rep_seq needs no bracket
             hi = max(hi, rep_score<POL>(v, x.rc, x.rm, 0));
             lo = min(lo, rep_score<POL>(v, x.rc, x.rm, POL == KS_SCORE_MOST_ALLOCATED ? 0 : v.k - 1));
         }
@@ -462,6 +478,108 @@ __global__ void __launch_bounds__(REP_THREADS) k_rep_order_most(NodeTable nt, Re
     });
 }
 
+// LEAST_BALANCED: one CTA per spec places its `need' copies one at a time, exactly as step 2 of ks_place_replicas
+// defines them.  The whole CTA fills the node scores and the block maxima; then warp 0 alone runs the copies (no CTA
+// barrier per copy): the argmax over the block maxima (ties to the lower block, and inside a block to the lower node),
+// the copy written at its place, the node advanced to its next copy or retired, and its block's maximum rescanned.
+template <int W>
+__global__ void __launch_bounds__(REP_THREADS) k_rep_seq(NodeTable nt, ReplicaArgs a, ReplicaSeqArgs q) {
+    constexpr int POL = KS_SCORE_LEAST_BALANCED;
+    __shared__ int64_t s_best[REP_SEQ_BLOCKS];
+    __shared__ int32_t s_node[REP_SEQ_BLOCKS];
+    const uint32_t N = nt.N, B = q.block, nb = (N + B - 1) / B;
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int64_t* score = q.score + (uint64_t)blockIdx.x * N;
+    uint32_t* placed = q.placed + (uint64_t)blockIdx.x * N;
+    // the best node of block b, every lane of the calling warp ends with it
+    auto block_max = [&](uint32_t b, int64_t& key, int32_t& idx) {
+        key = INT64_MIN;
+        idx = -1;
+        const uint32_t n1 = min(N, (b + 1) * B);
+        for (uint32_t n = b * B + lane; n < n1; n += 32) { // ascending n per lane: strict '>' keeps the lowest index
+            const int64_t v = score[n];
+            if (v > key) {
+                key = v;
+                idx = (int32_t)n;
+            }
+        }
+        warp_argmax(key, idx);
+    };
+    for (uint32_t t = blockIdx.x; t < a.T; t += gridDim.x) {
+        const uint64_t need = a.spec[t].need;
+        if (!need) continue; // block-uniform; k_rep_init wrote the row
+        const int64_t rc = a.req_cpu[t], rm = a.req_mem[t];
+        uint64_t sel[W];
+#pragma unroll
+        for (int w = 0; w < W; w++) sel[w] = a.sel[(uint64_t)t * W + w];
+        const uint32_t R = a.replicas[t];
+        for (uint32_t n = threadIdx.x; n < N; n += REP_THREADS) {
+            RepNode v;
+            uint64_t cn;
+            rep_node<W, POL>(nt, n, rc, rm, sel, R, v, cn);
+            score[n] = v.k ? rep_score<POL>(v, rc, rm, 0) : INT64_MIN;
+            placed[n] = 0;
+        }
+        __syncthreads();
+        for (uint32_t b = warp; b < nb; b += REP_WARPS) {
+            int64_t key;
+            int32_t idx;
+            block_max(b, key, idx);
+            if (lane == 0) {
+                s_best[b] = key;
+                s_node[b] = idx;
+            }
+        }
+        __syncthreads();
+        if (warp == 0) {
+            const uint64_t off = a.offset[t];
+            uint32_t nodes = 0, most = 0;
+            int64_t last = 0;
+            for (uint64_t r = 0; r < need; r++) {
+                int64_t key = INT64_MIN;
+                int32_t bb = -1;
+                for (uint32_t b = lane; b < nb; b += 32) // ascending b per lane: strict '>' keeps the lowest block
+                    if (s_node[b] >= 0 && s_best[b] > key) {
+                        key = s_best[b];
+                        bb = (int32_t)b;
+                    }
+                warp_argmax(key, bb); // blocks are node ranges in order: the lower block holds the lower node
+                const int32_t n = s_node[bb];
+                if (lane == 0) {
+                    if (a.out_node) {
+                        a.out_node[off + r] = n;
+                        a.out_score[off + r] = key;
+                    }
+                    const uint32_t j = placed[n] + 1; // copies on n with this one
+                    placed[n] = j;
+                    nodes += j == 1;
+                    most = max(most, j);
+                    last = key;
+                    RepNode v;
+                    uint64_t cn;
+                    rep_node<W, POL>(nt, (uint32_t)n, rc, rm, sel, R, v, cn);
+                    score[n] = j < v.k ? rep_score<POL>(v, rc, rm, j) : INT64_MIN;
+                }
+                __syncwarp(); // lane 0's stores to score[] are seen by the rescan
+                int64_t k2;
+                int32_t i2;
+                block_max((uint32_t)bb, k2, i2);
+                if (lane == 0) {
+                    s_best[bb] = k2;
+                    s_node[bb] = i2;
+                }
+                __syncwarp();
+            }
+            if (lane == 0) {
+                a.rows[t].nodes = nodes;
+                a.rows[t].max_per_node = most;
+                a.rows[t].last_score = last;
+            }
+        }
+        __syncthreads(); // the scratch and the block maxima are reused by the next spec
+    }
+}
+
 template <int W, int POL>
 static cudaError_t rep_sequence(const NodeTable& nt, const ReplicaArgs& a, cudaStream_t st) {
     const dim3 grid(a.n_chunks, a.T);
@@ -484,11 +602,24 @@ static cudaError_t rep_sequence(const NodeTable& nt, const ReplicaArgs& a, cudaS
     return cudaGetLastError();
 }
 
-cudaError_t launch_replicas(const NodeTable& nt, int policy, const ReplicaArgs& a, cudaStream_t st) {
+// LEAST_BALANCED: the scan and the rows, then the copies one at a time
+template <int W>
+static cudaError_t rep_one_by_one(const NodeTable& nt, const ReplicaArgs& a, const ReplicaSeqArgs& q, cudaStream_t st) {
+    constexpr int POL = KS_SCORE_LEAST_BALANCED;
+    k_rep_scan<W, POL><<<dim3(a.n_chunks, a.T), REP_THREADS, 0, st>>>(nt, a);
+    k_rep_init<<<(a.T + 127) / 128, 128, 0, st>>>(a);
+    k_rep_seq<W><<<q.ctas, REP_THREADS, 0, st>>>(nt, a, q);
+    g_launches += 3;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_replicas(const NodeTable& nt, int policy, const ReplicaArgs& a, const ReplicaSeqArgs& q,
+                            cudaStream_t st) {
     if (a.T == 0 || nt.N == 0) return cudaSuccess;
     return with_label_width(nt.W, [&](auto w) {
         constexpr int W_ = decltype(w)::value;
         if (policy == KS_SCORE_MOST_ALLOCATED) return rep_sequence<W_, KS_SCORE_MOST_ALLOCATED>(nt, a, st);
+        if (policy == KS_SCORE_LEAST_BALANCED) return rep_one_by_one<W_>(nt, a, q, st);
         return policy == KS_SCORE_LEFTOVER ? rep_sequence<W_, KS_SCORE_LEFTOVER>(nt, a, st)
                                            : rep_sequence<W_, KS_SCORE_LEAST_ALLOCATED>(nt, a, st);
     });

@@ -133,6 +133,8 @@ __device__ __forceinline__ void stream_round_scan(const StreamBatchArgs& a, cons
                     a.policy == KS_SCORE_LEFTOVER ? leftover_key(fc, fm)
                     : a.policy == KS_SCORE_MOST_ALLOCATED
                         ? most_alloc_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm)
+                    : a.policy == KS_SCORE_LEAST_BALANCED
+                        ? least_balanced_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm)
                         : least_alloc_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm);
                 if (key > best) { // ascending n per lane: strict '>' keeps the lowest index
                     best = key;

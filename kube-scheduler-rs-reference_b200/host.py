@@ -92,8 +92,8 @@ def format_unschedulable(n_nodes, reasons, cap=256):
 
 class Context:
     """ksh_context = the reference's Context{client, node_store} for this path (src/util.rs:12-15).  Every method that
-    takes a policy passes it through to the packed call: KS_SCORE_LEFTOVER, KS_SCORE_LEAST_ALLOCATED or
-    KS_SCORE_MOST_ALLOCATED (bin-packing)."""
+    takes a policy passes it through to the packed call: KS_SCORE_LEFTOVER, KS_SCORE_LEAST_ALLOCATED,
+    KS_SCORE_MOST_ALLOCATED (bin-packing) or KS_SCORE_LEAST_BALANCED (upstream's default profile)."""
 
     def __init__(self, device=0):
         h = _vp()

@@ -128,8 +128,9 @@ class Snapshot:
 
     def select(self, req_cpu, req_mem, sel, policy=capi.KS_SCORE_LEFTOVER, flags=capi.KS_SELECT_AUTO, want_mask=False):
         """Batched select_node_for_pod over host (numpy) pods; returns host results.  policy: KS_SCORE_LEFTOVER,
-        KS_SCORE_LEAST_ALLOCATED or KS_SCORE_MOST_ALLOCATED (bin-packing), on either kernel path.  Every method here
-        that takes a policy takes these three."""
+        KS_SCORE_LEAST_ALLOCATED, KS_SCORE_MOST_ALLOCATED (bin-packing) or KS_SCORE_LEAST_BALANCED (upstream's default
+        profile: LeastAllocated + BalancedAllocation), on either kernel path.  Every method here that takes a policy
+        takes these four."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
         p = int(pods.n)
         idx = np.empty(p, np.int32)

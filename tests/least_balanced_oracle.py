@@ -1,0 +1,245 @@
+"""CPU restatement of KS_SCORE_LEAST_BALANCED (include/ksched.h) for the tests.
+
+The oracle library scores LEFTOVER and LEAST_ALLOCATED only, so this module adds upstream's default resource scoring on
+top of it, as most_allocated_oracle does for bin-packing: which cells are feasible (and the mask and counts) still come
+from orc_run_packed's cell codes, and the scores from the definition below.  `Oracle(orc)` has orc's run_packed /
+stream_bind_packed / commit_claims / free_reduce and accepts policy 4, so the existing restatements (gang_oracle,
+drain_oracle, replicas_oracle.sequential_packed) run under it unchanged.  `heap_packed` is the replica plan placed one
+copy at a time with a heap instead of one full select per copy.
+
+The balanced term is defined in IEEE double arithmetic: each operand is converted with float() (round to nearest even,
+as CUDA's __ll2double_rn) before one true division, and every later step is one rounded double operation.  Python's
+`u / A` on two ints rounds the exact quotient once instead, which differs above 2^53: the helpers below never use it."""
+import heapq
+
+import numpy as np
+
+from replicas_oracle import PLAN_DTYPE, _row, _specs, node_copies
+
+LEAST_BALANCED = 4
+
+
+def least(fc, fm, ac, am, rc, rm):
+    """KS_SCORE_LEAST_ALLOCATED on Python ints: truncating divisions, as the C expression."""
+    def t(f, q, a):
+        if a <= 0:
+            return 0
+        x = (f - q) * 100
+        return abs(x) // a * (1 if x >= 0 else -1)
+    s = t(int(fc), int(rc), int(ac)) + t(int(fm), int(rm), int(am))
+    return abs(s) // 2 * (1 if s >= 0 else -1)
+
+
+def balanced(fc, fm, ac, am, rc, rm):
+    """The balanced term on Python ints and floats, one rounded double operation per step."""
+    fc, fm, ac, am, rc, rm = (int(v) for v in (fc, fm, ac, am, rc, rm))
+    if ac <= 0 or am <= 0:
+        return 100
+    uc = min(max(ac - (fc - rc), 0), ac)
+    um = min(max(am - (fm - rm), 0), am)
+    xc = float(uc) / float(ac)
+    xm = float(um) / float(am)
+    sd = abs(xc - xm) / 2.0
+    return int((1.0 - sd) * 100.0)  # int() truncates toward zero; the value is >= 50
+
+
+def score(fc, fm, ac, am, rc, rm):
+    return least(fc, fm, ac, am, rc, rm) + balanced(fc, fm, ac, am, rc, rm)
+
+
+def scores(fc, fm, ac, am, rc, rm):
+    """The same on int64 arrays (broadcasting).  numpy's int64 -> float64 cast rounds to nearest even and its float64
+    operations are single IEEE operations, so this is bit for bit the scalar form; inside the limits of ksched.h nothing
+    overflows."""
+    fc, fm, ac, am, rc, rm = np.broadcast_arrays(*(np.asarray(v, np.int64) for v in (fc, fm, ac, am, rc, rm)))
+
+    def pct(f, q, a):  # truncating (f - q) * 100 / a, 0 for a <= 0
+        pos = a > 0
+        x = (f - q) * 100
+        d = np.where(pos, a, 1)
+        return np.where(pos, np.sign(x) * (np.abs(x) // d), 0)
+
+    s = pct(fc, rc, ac) + pct(fm, rm, am)
+    lst = np.sign(s) * (np.abs(s) // 2)
+    both = (ac > 0) & (am > 0)
+    a_c, a_m = np.where(ac > 0, ac, 1), np.where(am > 0, am, 1)
+    uc = np.clip(ac - (fc - rc), 0, np.maximum(ac, 0))
+    um = np.clip(am - (fm - rm), 0, np.maximum(am, 0))
+    with np.errstate(all="ignore"):
+        xc = uc.astype(np.float64) / a_c.astype(np.float64)
+        xm = um.astype(np.float64) / a_m.astype(np.float64)
+        sd = np.abs(xc - xm) / 2.0
+        bal = ((1.0 - sd) * 100.0).astype(np.int64)  # truncation toward zero
+    return lst + np.where(both, bal, 100)
+
+
+# ---- the bit-parallel walk's bound (ks_bitpar.cu, DESIGN.md 5j), restated for the bound tests ----
+def most_term(f, a, q):
+    return 0 if a <= 0 else min(max(a - (f - q), 0), a) * 100 // a
+
+
+def node_bound(fc, fm, ac, am):
+    """b(n) = least_alloc_bound(n) + bal(n), unclamped."""
+    b = least(fc, fm, ac, am, 0, 0)
+    if ac <= 0 or am <= 0:
+        return b + 100
+    d = abs(most_term(fc, ac, 0) - most_term(fm, am, 0))
+    return b + 100 - (max(d - 1, 0) // 2)
+
+
+def slack(q, m):
+    """min(100, ceil(q * 100 / m)) for q >= 0, m > 0."""
+    x = q * 100
+    return min(100, x // m + (1 if x % m else 0))
+
+
+def pod_slack(rc, rm, amax_c, amax_m, amin_c, amin_m):
+    """D - E: every feasible cell of the pod scores <= b(n) - (D - E).  amax = max allocatable (INT64_MAX when some node
+    has none), amin = smallest positive allocatable (INT64_MAX when none)."""
+    dl = ((rc * 100) // amax_c + (rm * 100) // amax_m) // 2
+    e = (max(slack(rc, amin_c), slack(rm, amin_m)) + 1) // 2
+    return dl - e
+
+
+class Oracle:
+    """orc with policy 4 added to run_packed and stream_bind_packed."""
+
+    def __init__(self, orc):
+        self.orc = orc
+
+    def __getattr__(self, name):
+        return getattr(self.orc, name)
+
+    def run_packed(self, free_cpu, free_mem, alloc_cpu, alloc_mem, labels, req_cpu, req_mem, sel, policy=0,
+                   want_mask=True, want_codes=False, nthreads=0):
+        if policy != LEAST_BALANCED:
+            return self.orc.run_packed(free_cpu, free_mem, alloc_cpu, alloc_mem, labels, req_cpu, req_mem, sel, policy,
+                                       want_mask, want_codes, nthreads)
+        _, _, cnt, mask, codes = self.orc.run_packed(free_cpu, free_mem, alloc_cpu, alloc_mem, labels, req_cpu, req_mem,
+                                                     sel, 0, want_mask, True, nthreads)
+        fc, fm = np.asarray(free_cpu, np.int64), np.asarray(free_mem, np.int64)
+        ac, am = np.asarray(alloc_cpu, np.int64), np.asarray(alloc_mem, np.int64)
+        rc, rm = np.asarray(req_cpu, np.int64), np.asarray(req_mem, np.int64)
+        P = rc.shape[0]
+        idx = np.full(P, -1, np.int32)
+        sc = np.zeros(P, np.int64)
+        INF = np.iinfo(np.int64).min
+        for p0 in range(0, P, 512):  # bounded memory for large P
+            p1 = min(P, p0 + 512)
+            if not fc.shape[0]:
+                break
+            s = scores(fc[None, :], fm[None, :], ac[None, :], am[None, :], rc[p0:p1, None], rm[p0:p1, None])
+            s = np.where(codes[p0:p1] == 0, s, INF)
+            best = s.argmax(axis=1)  # first maximum: ties to the lowest node index
+            bs = s[np.arange(p1 - p0), best]
+            ok = bs != INF
+            idx[p0:p1][ok] = best[ok]
+            sc[p0:p1][ok] = bs[ok]
+        return idx, sc, cnt, mask, codes if want_codes else None
+
+    def stream_bind_packed(self, free_cpu, free_mem, alloc_cpu, alloc_mem, labels, req_cpu, req_mem, sel, policy=0):
+        """orc_stream_bind_packed's round loop: select the pending pods, commit the claims per node in arrival order,
+        losers retry; in place on free_cpu / free_mem."""
+        if policy != LEAST_BALANCED:
+            return self.orc.stream_bind_packed(free_cpu, free_mem, alloc_cpu, alloc_mem, labels, req_cpu, req_mem, sel,
+                                               policy)
+        P = len(req_cpu)
+        rc, rm = np.asarray(req_cpu, np.int64), np.asarray(req_mem, np.int64)
+        sel = np.ascontiguousarray(sel, np.uint64).reshape(P, -1)
+        idx = np.full(P, -1, np.int32)
+        sc = np.zeros(P, np.int64)
+        pending = np.arange(P)
+        rounds = 0
+        while len(pending) and rounds <= P + 1:
+            i, s = self.run_packed(free_cpu, free_mem, alloc_cpu, alloc_mem, labels, rc[pending], rm[pending],
+                                   sel[pending], policy, want_mask=False)[:2]
+            acc = self.orc.commit_claims(free_cpu, free_mem, i, rc[pending], rm[pending])
+            won = (i >= 0) & (acc != 0)
+            idx[pending[won]], sc[pending[won]] = i[won], s[won]
+            pending = pending[(i >= 0) & (acc == 0)]
+            rounds += 1
+        return idx, sc, rounds
+
+
+def topk_packed(oracle, free_cpu, free_mem, alloc_cpu, alloc_mem, labels, req_cpu, req_mem, sel, k):
+    """ks_select_topk's rows under policy 4: feasible nodes by score descending, node ascending."""
+    from topk_oracle import _ranked
+    fc, fm = np.asarray(free_cpu, np.int64), np.asarray(free_mem, np.int64)
+    ac, am = np.asarray(alloc_cpu, np.int64), np.asarray(alloc_mem, np.int64)
+    rc, rm = np.asarray(req_cpu, np.int64), np.asarray(req_mem, np.int64)
+    codes = oracle.orc.run_packed(fc, fm, ac, am, labels, rc, rm, sel, 0, want_mask=False, want_codes=True)[4]
+    rows = []
+    for p in range(len(rc)):
+        n = np.nonzero(codes[p] == 0)[0]
+        rows.append((n, scores(fc[n], fm[n], ac[n], am[n], rc[p], rm[p])))
+    return _ranked(rows, k)
+
+
+def heap_packed(free_cpu, free_mem, alloc_cpu, alloc_mem, labels, req_cpu, req_mem, sel, replicas):
+    """Replica placement under policy 4, one copy at a time: a heap of (-s_n(j), n) over the nodes that hold another
+    copy; the popped node takes the copy and goes back with s_n(j + 1) while j + 1 < min(c_n, R).  Ties pop the lower
+    node index, as the argmax.  Returns (rows, node, score, offset) as replicas_oracle.merge_packed does."""
+    fc, fm = np.asarray(free_cpu, np.int64), np.asarray(free_mem, np.int64)
+    ac, am = np.asarray(alloc_cpu, np.int64), np.asarray(alloc_mem, np.int64)
+    N, T = fc.shape[0], len(req_cpu)
+    labels, sel = _specs(labels, sel, N, T)
+    offset = np.zeros(T + 1, np.uint64)
+    np.cumsum(np.asarray(replicas, np.uint64), out=offset[1:])
+    rows = np.zeros(T, PLAN_DTYPE)
+    node = np.full(int(offset[-1]), -1, np.int32)
+    sc = np.zeros(int(offset[-1]), np.int64)
+    for t in range(T):
+        rc, rm, R, o = int(req_cpu[t]), int(req_mem[t]), int(replicas[t]), int(offset[t])
+        c, cap = node_copies(fc, fm, labels, rc, rm, sel[t])
+        feas = np.nonzero(c != 0)[0]
+        k = np.where(c < 0, R, np.minimum(c, R))
+        s0 = scores(fc[feas], fm[feas], ac[feas], am[feas], rc, rm)
+        heap = [(-int(s), int(n)) for s, n in zip(s0, feas) if k[n] > 0]
+        heapq.heapify(heap)
+        placed = np.zeros(N, np.int64)
+        r = 0
+        while r < R and heap:
+            s, n = heapq.heappop(heap)
+            node[o + r], sc[o + r] = n, -s
+            r += 1
+            j = placed[n] = placed[n] + 1
+            if j < k[n]:
+                heapq.heappush(heap, (-score(fc[n] - j * rc, fm[n] - j * rm, ac[n], am[n], rc, rm), n))
+        rows[t] = _row(cap, len(feas), node[o:o + r], int(sc[o + r - 1]) if r else 0)
+    return rows, node, sc, offset
+
+
+# ---- cells whose (1 - std) * 100 lies within a few ulps of an integer ----
+def _chain(uc, ac, um, am, fma=False, recip=False):
+    from fractions import Fraction
+    if recip:
+        xc, xm = float(uc) * (1.0 / float(ac)), float(um) * (1.0 / float(am))
+    else:
+        xc, xm = float(uc) / float(ac), float(um) / float(am)
+    sd = abs(xc - xm) / 2.0
+    v = float(Fraction(100) - Fraction(100) * Fraction(sd)) if fma else (1.0 - sd) * 100.0
+    return int(v)
+
+
+def hazard_cells(seed, n):
+    """Cells (fc, fm, ac, am, rc, rm) whose exact shares differ by 2k/100, so the exact (1 - std) * 100 is the integer
+    100 - k and the double evaluation lands a few ulps to either side.  Kept: the cells where contracting the last two
+    steps to an FMA or dividing by a reciprocal would change the truncated result, and as many where neither would.
+    Returns the arrays and the number of distinguishing cells."""
+    rng = np.random.default_rng(seed)
+    hit, calm = [], []
+    while len(hit) < n // 2 or len(calm) < n - n // 2:
+        ac, am = 50 * int(rng.integers(1, 1 << 29)), 50 * int(rng.integers(1, 1 << 49))
+        i = int(rng.integers(0, 51))
+        k = int(rng.integers(0, i + 1))
+        uc, um = ac // 50 * i, am // 50 * (i - k)
+        if rng.random() < 0.5:  # the larger share on either resource
+            uc, um = ac // 50 * (i - k), am // 50 * i
+        fc, fm = ac - uc, am - um  # u = A - (f - q) with q = 0: free = A - u
+        q_c = int(rng.integers(0, 1 << 20)) if rng.random() < 0.3 else 0
+        fc += q_c  # the same u with a request: f - q unchanged
+        b = _chain(uc, ac, um, am)
+        distinct = b != _chain(uc, ac, um, am, fma=True) or b != _chain(uc, ac, um, am, recip=True)
+        (hit if distinct else calm).append((fc, fm, ac, am, q_c, 0))
+    cells = hit[:n // 2] + calm[:n - n // 2]
+    return tuple(np.array(c, np.int64) for c in zip(*cells)), len(hit[:n // 2])
