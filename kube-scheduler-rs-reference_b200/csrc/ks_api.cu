@@ -95,10 +95,6 @@ static int check_range_and_prio(ks_snapshot* s, cudaStream_t st) {
     return KS_OK;
 }
 
-static bool valid_policy(int policy) {
-    return policy == KS_SCORE_LEFTOVER || policy == KS_SCORE_LEAST_ALLOCATED || policy == KS_SCORE_MOST_ALLOCATED ||
-           policy == KS_SCORE_LEAST_BALANCED;
-}
 static bool valid_space(int32_t space) { return space == KS_MEM_HOST || space == KS_MEM_DEVICE; }
 static bool valid_label_words(uint32_t W) { return W == 1 || W == 2 || W == 4 || W == 8; }
 // inside +-2^36 millicores / +-2^55 bytes, the range that keeps every score inside int64
@@ -478,7 +474,7 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
     int rc = check_pods(s, pods);
     if (rc) return rc;
     if (!out) return fail(KS_ERR_INVALID, "out is NULL");
-    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
     if ((flags & KS_SELECT_FORCE_BITPAR) && (flags & KS_SELECT_FORCE_DIRECT)) return fail(KS_ERR_INVALID, "bad flags");
     const uint64_t P = pods->n;
     if (out->mask) {
@@ -935,7 +931,7 @@ int ks_select_topk(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t k, 
     int rc = check_pods(s, pods);
     if (rc) return rc;
     if (k == 0 || k > KS_TOPK_MAX) return fail(KS_ERR_RANGE, "k must be in [1, %u] (got %u)", KS_TOPK_MAX, k);
-    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
     if (!valid_space(out_space)) return fail(KS_ERR_INVALID, "bad out_space");
     const uint64_t P = pods->n;
     if (P && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
@@ -1095,7 +1091,7 @@ int ks_stream_bind(ks_snapshot* s, const ks_pods* pods, int policy, int32_t* out
     if (pods->n && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
     const uint64_t n = pods->n;
     const uint32_t W = s->W;
-    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
     rc = check_commit_requests(n, pods->req_cpu, pods->req_mem);
     if (rc) return rc;
     if (n > 0 && n <= STREAM_BATCH_MAX && s->N > 0 && s->coop) {
@@ -1201,7 +1197,7 @@ int ks_gang_bind(ks_snapshot* s, const ks_pods* pods, const ks_gangs* gangs, int
     if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_gang_bind takes host-space pods");
     if (!gangs || !gangs->offset || (gangs->n && !gangs->min_member)) return fail(KS_ERR_INVALID, "NULL group array");
     if (pods->n && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
-    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
     const uint64_t P = pods->n, G = gangs->n;
     const uint64_t* off = gangs->offset;
     if (off[0] != 0) return fail(KS_ERR_INVALID, "offset[0] must be 0");
@@ -1283,7 +1279,7 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidate
     if (!cand || !cand->offset || (cand->n && (!cand->node_idx || !out_placed)))
         return fail(KS_ERR_INVALID, "NULL candidate array or out_placed");
     if (pods->n && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
-    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
     if (flags & ~KS_DRAIN_EXCLUDE_CANDIDATES) return fail(KS_ERR_INVALID, "unknown flags 0x%x", flags);
     const uint64_t P = pods->n, D = cand->n;
     const uint64_t* off = cand->offset;
@@ -1517,7 +1513,7 @@ int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* repl
     if (specs->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_place_replicas takes host-space specs");
     const uint64_t T = specs->n;
     if (T && (!replicas || !out)) return fail(KS_ERR_INVALID, "NULL replicas or out");
-    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
     if (T > KS_REPLICAS_MAX_SPECS) return fail(KS_ERR_RANGE, "%llu specs (at most %u)", (unsigned long long)T, KS_REPLICAS_MAX_SPECS);
     uint64_t total = 0;
     for (uint64_t t = 0; t < T; t++) {
@@ -1698,7 +1694,7 @@ static void stream_worker(ks_stream* q) {
 
 int ks_stream_open(ks_snapshot* s, int policy, uint32_t max_batch, ks_stream** out) {
     if (!s || !out) return fail(KS_ERR_INVALID, "NULL argument");
-    if (!valid_policy(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
     ks_stream* q = new (std::nothrow) ks_stream();
     if (!q) return fail(KS_ERR_NOMEM, "out of host memory");
     q->snap = s;

@@ -963,6 +963,7 @@ struct NodeEval { // one row per slot of the bound order
 // t < 2^24).  Memory is in bytes and does not fit: z = free_mem * 100 / alloc_mem and w = 100 / alloc_mem (both 0 for
 // alloc_mem <= 0) give the real-valued quotient z - r * w with a relative error of a few 2^-24; its floor is known
 // whenever no integer lies within the error bound (the kernel uses 2e-6 * (|z| + |r * w|) + 1e-3, > 8 x the worst case).
+// k_build_eval writes the rows of one bound order, and this view too unless hint is null (only k_least_alloc reads it).
 __global__ void __launch_bounds__(256)
     k_build_eval(NodeTable nt, const int32_t* __restrict__ ordL_idx, uint32_t Nord, NodeEval* __restrict__ ev,
                  float4* __restrict__ hint) {
@@ -984,6 +985,7 @@ __global__ void __launch_bounds__(256)
     e.inv_ac = e.ac > 0 ? 1.0 / (double)e.ac : 0.0;
     e.inv_am = e.am > 0 ? 1.0 / (double)e.am : 0.0;
     ev[s] = e;
+    if (!hint) return;
     const float qnan = __int_as_float(0x7fc00000);
     const bool fc_exact = e.fc > -(1ll << 24) && e.fc < (1ll << 24);
     const double Sm = e.am > 0 ? (double)e.fm * 100.0 * e.inv_am : 0.0;
@@ -1456,6 +1458,7 @@ BitparIndex::~BitparIndex() {
 
 cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cudaStream_t st) {
     ix.valid = false;
+    ix.ordL.valid = false;
     ix.ordM.valid = ix.ordB.valid = false; // these orders follow on the next call that needs them (bitpar_prepare_order)
     ix.N = nt.N;
     ix.W = nt.W;
@@ -1463,11 +1466,11 @@ cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cu
     const uint32_t Nord = ((nt.N + BP_TILE - 1) / BP_TILE) * BP_TILE;
     ix.Nord = Nord;
     cudaError_t e;
-    for (DevBuf* b : {&ix.sortedC, &ix.sortedM, &ix.ord_prio, &ix.ordL_s0})
+    for (DevBuf* b : {&ix.sortedC, &ix.sortedM, &ix.ord_prio, &ix.ordL.b})
         if ((e = b->ensure((size_t)Nord * sizeof(int64_t))) != cudaSuccess) return e;
-    for (DevBuf* b : {&ix.gposC, &ix.gposM, &ix.ord_idx, &ix.ordL_idx})
+    for (DevBuf* b : {&ix.gposC, &ix.gposM, &ix.ord_idx, &ix.ordL.idx})
         if ((e = b->ensure((size_t)Nord * sizeof(uint32_t))) != cudaSuccess) return e;
-    if ((e = ix.evalL.ensure((size_t)Nord * sizeof(NodeEval))) != cudaSuccess) return e;
+    if ((e = ix.ordL.eval.ensure((size_t)Nord * sizeof(NodeEval))) != cudaSuccess) return e;
     if ((e = ix.hintL.ensure((size_t)Nord * sizeof(float4))) != cudaSuccess) return e;
     for (DevBuf* b : {&ix.splC, &ix.splM})
         if ((e = b->ensure(RANK_SPLITTERS * sizeof(int64_t))) != cudaSuccess) return e;
@@ -1497,16 +1500,16 @@ cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cu
     k_node_rank<<<(Nord + 255) / 256, 256, 0, st>>>(
         nt, prio, ix.rk_hist.as<uint32_t>(), ix.rk_bkt.as<uint8_t>(), ix.rk_perm.as<uint32_t>(), ix.sortedC.as<int64_t>(),
         ix.sortedM.as<int64_t>(), ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(), ix.ord_prio.as<int64_t>(),
-        ix.ord_idx.as<int32_t>(), Nord, ix.splC.as<int64_t>(), ix.splM.as<int64_t>(), stride, ix.ordL_s0.as<int64_t>(),
-        ix.ordL_idx.as<int32_t>());
+        ix.ord_idx.as<int32_t>(), Nord, ix.splC.as<int64_t>(), ix.splM.as<int64_t>(), stride, ix.ordL.b.as<int64_t>(),
+        ix.ordL.idx.as<int32_t>());
     g_launches += 4;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     RowsLayout lay{};
     if (!make_layout_rows(nt.N, nt.W, &lay)) return cudaSuccess; // direct path only
-    for (DevBuf* b : {&ix.blobR, &ix.blobP, &ix.blobL})
+    for (DevBuf* b : {&ix.blobR, &ix.blobP, &ix.ordL.blob})
         if ((e = b->ensure((size_t)lay.ncb * lay.cb_stride)) != cudaSuccess) return e;
     const size_t bucket_bytes = tile_buckets(nullptr, nt.N, lay, nullptr);
-    for (DevBuf* b : {&ix.bucketsP, &ix.bucketsL})
+    for (DevBuf* b : {&ix.bucketsP, &ix.ordL.buckets})
         if ((e = b->ensure(bucket_bytes)) != cudaSuccess) return e;
     const size_t need_rank = (size_t)lay.ncb * lay.n_thr * 2 * (RW_TILES / 2); // u32 tile pairs
     if ((e = ix.rank.ensure(need_rank * sizeof(uint32_t))) != cudaSuccess) return e;
@@ -1530,29 +1533,33 @@ cudaError_t bitpar_build(BitparIndex& ix, const NodeTable& nt, int64_t* prio, cu
     g_launches++;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     // KS_SCORE_LEAST_ALLOCATED: the same index in descending order of the score bound + per-slot evaluation rows
-    tile_buckets(ix.bucketsL.p, nt.N, lay, &bk);
-    k_build_tiles<<<tiles, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(), ix.ordL_idx.as<int32_t>(),
-                                         ix.blobL.as<uint8_t>(), lay, nullptr, bk);
-    k_build_eval<<<(Nord + 255) / 256, 256, 0, st>>>(nt, ix.ordL_idx.as<int32_t>(), Nord, ix.evalL.as<NodeEval>(),
+    tile_buckets(ix.ordL.buckets.p, nt.N, lay, &bk);
+    k_build_tiles<<<tiles, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(), ix.ordL.idx.as<int32_t>(),
+                                         ix.ordL.blob.as<uint8_t>(), lay, nullptr, bk);
+    k_build_eval<<<(Nord + 255) / 256, 256, 0, st>>>(nt, ix.ordL.idx.as<int32_t>(), Nord, ix.ordL.eval.as<NodeEval>(),
                                                      ix.hintL.as<float4>());
     g_launches += 2;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     ix.lay_r = lay;
-    ix.valid = true;
+    ix.ordL.valid = ix.valid = true;
     return cudaSuccess;
+}
+
+// The order of a bound-ordered policy: KS_SCORE_LEAST_ALLOCATED, KS_SCORE_MOST_ALLOCATED or KS_SCORE_LEAST_BALANCED
+static BoundOrder& bound_order(BitparIndex& ix, int policy) {
+    return policy == KS_SCORE_LEAST_ALLOCATED ? ix.ordL : policy == KS_SCORE_MOST_ALLOCATED ? ix.ordM : ix.ordB;
 }
 
 cudaError_t bitpar_prepare_order(BitparIndex& ix, const NodeTable& nt, int policy, cudaStream_t st) {
     if (policy != KS_SCORE_MOST_ALLOCATED && policy != KS_SCORE_LEAST_BALANCED) return cudaSuccess;
     if (!ix.valid) return cudaErrorNotSupported;
-    BoundOrder& o = policy == KS_SCORE_MOST_ALLOCATED ? ix.ordM : ix.ordB;
+    BoundOrder& o = bound_order(ix, policy);
     if (o.valid) return cudaSuccess;
     cudaError_t e;
     const uint32_t Nord = ix.Nord;
     if ((e = o.b.ensure((size_t)Nord * sizeof(int64_t))) != cudaSuccess) return e;
     if ((e = o.idx.ensure((size_t)Nord * sizeof(int32_t))) != cudaSuccess) return e;
     if ((e = o.eval.ensure((size_t)Nord * sizeof(NodeEval))) != cudaSuccess) return e;
-    if ((e = o.hint.ensure((size_t)Nord * sizeof(float4))) != cudaSuccess) return e;
     if ((e = o.sort.ensure(2ull * nt.N * sizeof(uint32_t) + 2 * sizeof(long long))) != cudaSuccess) return e;
     if ((e = o.blob.ensure((size_t)ix.lay_r.ncb * ix.lay_r.cb_stride)) != cudaSuccess) return e;
     if ((e = o.buckets.ensure(tile_buckets(nullptr, nt.N, ix.lay_r, nullptr))) != cudaSuccess) return e;
@@ -1566,8 +1573,7 @@ cudaError_t bitpar_prepare_order(BitparIndex& ix, const NodeTable& nt, int polic
     tile_buckets(o.buckets.p, nt.N, ix.lay_r, &bk);
     k_build_tiles<<<ix.lay_r.ncb * RW_TILES, 288, 0, st>>>(nt, ix.gposC.as<uint32_t>(), ix.gposM.as<uint32_t>(),
                                                           o.idx.as<int32_t>(), o.blob.as<uint8_t>(), ix.lay_r, nullptr, bk);
-    k_build_eval<<<(Nord + 255) / 256, 256, 0, st>>>(nt, o.idx.as<int32_t>(), Nord, o.eval.as<NodeEval>(),
-                                                     o.hint.as<float4>());
+    k_build_eval<<<(Nord + 255) / 256, 256, 0, st>>>(nt, o.idx.as<int32_t>(), Nord, o.eval.as<NodeEval>(), nullptr);
     g_launches += 3;
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     o.valid = true;
@@ -1675,32 +1681,29 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
         uint32_t* tail_list = ix.tail_list.as<uint32_t>();
         uint32_t* tail_count = tail_list + P; // the list holds at most P pods
         if ((e = cudaMemsetAsync(tail_count, 0, sizeof(uint32_t), bs)) != cudaSuccess) return e;
-        const bool least_alloc = L.policy == KS_SCORE_LEAST_ALLOCATED;
         TileBuckets bk;
-        if (L.policy == KS_SCORE_MOST_ALLOCATED || L.policy == KS_SCORE_LEAST_BALANCED) {
-            const BoundOrder& o = L.policy == KS_SCORE_MOST_ALLOCATED ? ix.ordM : ix.ordB;
+        if (L.policy != KS_SCORE_LEFTOVER) {
+            const BoundOrder& o = bound_order(ix, L.policy);
             if (!o.valid) return cudaErrorNotSupported; // bitpar_prepare_order runs first
             tile_buckets(o.buckets.p, ix.N, ix.lay_r, &bk);
             const uint32_t wpc = at / 32; // one warp per pod
             const uint32_t grid = (uint32_t)std::min<uint64_t>((uint64_t)sms * (2048 / at), ((uint64_t)P + wpc - 1) / wpc);
-            const long long* amin = reinterpret_cast<const long long*>(o.sort.as<uint32_t>() + 2ull * ix.N);
-            if (L.policy == KS_SCORE_MOST_ALLOCATED)
-                k_most_alloc<W><<<grid, at, 0, bs>>>(o.blob.as<uint8_t>(), bk, ix.lay_r, o.eval.as<NodeEval>(),
-                                                     o.b.as<int64_t>(), amin, L.pv, ix.pod_ranks.as<uint2>(), L.ov, L.po,
-                                                     ix.live.as<unsigned long long>(), ix.N);
-            else
-                k_least_balanced<W><<<grid, at, 0, bs>>>(o.blob.as<uint8_t>(), bk, ix.lay_r, o.eval.as<NodeEval>(),
+            if (L.policy == KS_SCORE_LEAST_ALLOCATED) {
+                k_least_alloc<W><<<grid, at, 0, bs>>>(o.blob.as<uint8_t>(), bk, ix.lay_r, o.eval.as<NodeEval>(),
+                                                      ix.hintL.as<float4>(), o.b.as<int64_t>(), o.idx.as<int32_t>(), L.pv,
+                                                      ix.pod_ranks.as<uint2>(), L.ov, L.po,
+                                                      ix.live.as<unsigned long long>(), ix.N);
+            } else {
+                const long long* amin = reinterpret_cast<const long long*>(o.sort.as<uint32_t>() + 2ull * ix.N);
+                if (L.policy == KS_SCORE_MOST_ALLOCATED)
+                    k_most_alloc<W><<<grid, at, 0, bs>>>(o.blob.as<uint8_t>(), bk, ix.lay_r, o.eval.as<NodeEval>(),
                                                          o.b.as<int64_t>(), amin, L.pv, ix.pod_ranks.as<uint2>(), L.ov,
                                                          L.po, ix.live.as<unsigned long long>(), ix.N);
-            g_launches++;
-            if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        } else if (least_alloc) {
-            tile_buckets(ix.bucketsL.p, ix.N, ix.lay_r, &bk);
-            const uint32_t wpc = at / 32; // one warp per pod
-            const uint32_t grid = (uint32_t)std::min<uint64_t>((uint64_t)sms * (2048 / at), ((uint64_t)P + wpc - 1) / wpc);
-            k_least_alloc<W><<<grid, at, 0, bs>>>(ix.blobL.as<uint8_t>(), bk, ix.lay_r, ix.evalL.as<NodeEval>(), ix.hintL.as<float4>(),
-                                                  ix.ordL_s0.as<int64_t>(), ix.ordL_idx.as<int32_t>(), L.pv, ix.pod_ranks.as<uint2>(),
-                                                  L.ov, L.po, ix.live.as<unsigned long long>(), ix.N);
+                else
+                    k_least_balanced<W><<<grid, at, 0, bs>>>(o.blob.as<uint8_t>(), bk, ix.lay_r, o.eval.as<NodeEval>(),
+                                                             o.b.as<int64_t>(), amin, L.pv, ix.pod_ranks.as<uint2>(),
+                                                             L.ov, L.po, ix.live.as<unsigned long long>(), ix.N);
+            }
             g_launches++;
             if ((e = cudaGetLastError()) != cudaSuccess) return e;
         } else {

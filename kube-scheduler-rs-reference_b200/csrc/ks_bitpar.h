@@ -54,16 +54,18 @@ struct TileBuckets {
     unsigned long long* memb[2];
 };
 
-// The node order of a bound-ordered argmax that is built on the first call that needs it after each bitpar_build
-// (bitpar_prepare_order): every node's score bound, the tile index and evaluation rows in descending bound order.
+// The node order of a bound-ordered argmax (k_least_alloc, k_most_alloc, k_least_balanced): every node's score bound,
+// the tile index and evaluation rows in descending bound order.  LEAST_ALLOCATED's is built by bitpar_build, the others
+// on the first call that needs them after each bitpar_build (bitpar_prepare_order).
 struct BoundOrder {
-    DevBuf b;       // [int64 Nord] bound of every node in descending order (ties by index), -1 for padding
+    DevBuf b;       // [int64 Nord] bound of every node in descending order (ties by index); padding: INT64_MIN for
+                    // LEAST_ALLOCATED, -1 for the others
     DevBuf idx;     // [int32 Nord]
-    DevBuf eval;    // [NodeEval Nord] per slot of that order
-    DevBuf hint;    // [float4 Nord] written by k_build_eval, not read by the bound-ordered walks
+    DevBuf eval;    // [NodeEval Nord] per slot of that order: what the exact score needs
     DevBuf blob;    // lay_r.ncb column-block blobs in that order, read through L1/L2 by the walk
     DevBuf buckets; // TileBuckets of blob
-    DevBuf sort;    // [uint32 2N] sort scratch, then [int64 2] smallest positive allocatable cpu / memory (8-aligned)
+    DevBuf sort;    // [uint32 2N] sort scratch, then [int64 2] smallest positive allocatable cpu / memory (8-aligned);
+                    // not allocated for LEAST_ALLOCATED, whose order k_node_rank writes
     bool valid = false; // matches the current index
 };
 
@@ -83,12 +85,8 @@ struct BitparIndex {
     DevBuf bucketsP;  // TileBuckets of blobP (tile_buckets)
     DevBuf pod_ranks; // [uint2 P] per-call scratch
     DevBuf tail_list; // [uint32 P + 1] per-call scratch: pods left for k_first_fit_tail, then the count at word P
-    DevBuf ordL_s0;   // [int64 Nord] KS_SCORE_LEAST_ALLOCATED: score bound of every node in descending order (ties by index)
-    DevBuf ordL_idx;  // [int32 Nord]
-    DevBuf evalL;     // [NodeEval Nord] per slot of that order: what the exact score needs
-    DevBuf hintL;     // [float4 Nord] per slot of that order: single-precision score model (pre-filter of k_least_alloc)
-    DevBuf blobL;     // lay_r.ncb column-block blobs in that order, read through L1/L2 by k_least_alloc
-    DevBuf bucketsL;  // TileBuckets of blobL
+    BoundOrder ordL;  // KS_SCORE_LEAST_ALLOCATED (k_least_alloc)
+    DevBuf hintL;     // [float4 Nord] per slot of ordL: single-precision score model (pre-filter of k_least_alloc)
     BoundOrder ordM;  // KS_SCORE_MOST_ALLOCATED (k_most_alloc), built lazily
     BoundOrder ordB;  // KS_SCORE_LEAST_BALANCED (k_least_balanced), built lazily
     DevBuf live;      // [uint64 KS_MAX_LABEL_WORDS + 2] label bits carried by at least one node, max allocatable cpu, memory
@@ -97,7 +95,7 @@ struct BitparIndex {
     DevBuf rank;      // [uint32] rows kernel: [cb][threshold g][resource][j] = nodes of tile j (low 16 bits) and tile j + 4
                       // (high 16 bits) at sorted positions < g
     DevBuf tile_sorted; // [uint32] build scratch: per tile, its nodes' global positions in ascending order
-    RowsLayout lay_r{}; // the layout of blobR, blobP and blobL
+    RowsLayout lay_r{}; // the layout of blobR, blobP and every BoundOrder's blob
     DevBuf rk_hist;   // [uint32] node sample sort scratch: per order 256 bucket counts, splitters, per-node bucket / slot, lists
     DevBuf rk_spl_v;
     DevBuf rk_spl_i;

@@ -397,7 +397,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS)
         if (lane == 0 && p0 + i < pv.P) {
             const uint32_t p = p0 + i;
             if (gridDim.y == 1) {
-                const int64_t s = ix < 0 ? 0 : (ALLOC ? k : leftover_score(k, rc[i], rm[i]));
+                const int64_t s = ix < 0 ? 0 : key_score<POLICY>(k, rc[i], rm[i]);
                 if (ov.node_idx) ov.node_idx[p] = ix;
                 if (ov.score) ov.score[p] = s;
                 if (ov.cnt) ov.cnt[p] = cnt[i];
@@ -424,7 +424,7 @@ __global__ void k_select_combine(PodView pv, OutView ov, PartialView part, uint3
         c += part.cnt[o];
         merge_partial(k, ix, part.key[o], part.idx[o]);
     }
-    const int64_t s = ix < 0 ? 0 : (POLICY == KS_SCORE_LEFTOVER ? leftover_score(k, pv.req_cpu[p], pv.req_mem[p]) : k);
+    const int64_t s = ix < 0 ? 0 : key_score<POLICY>(k, pv.req_cpu[p], pv.req_mem[p]);
     if (ov.node_idx) ov.node_idx[p] = ix;
     if (ov.score) ov.score[p] = s;
     if (ov.cnt) ov.cnt[p] = c;
@@ -546,7 +546,7 @@ __global__ void __launch_bounds__(DIRECT_THREADS, 1)
             const uint64_t o = (uint64_t)p * k + lane;
             if (lane < k) {
                 ov.node_idx[o] = lidx[i];
-                if (ov.score) ov.score[o] = lidx[i] < 0 ? 0 : (ALLOC ? lkey[i] : leftover_score(lkey[i], rc[i], rm[i]));
+                if (ov.score) ov.score[o] = lidx[i] < 0 ? 0 : key_score<POLICY>(lkey[i], rc[i], rm[i]);
             }
             if (lane == 0 && ov.cnt) ov.cnt[p] = cnt[i];
         } else {
@@ -587,7 +587,7 @@ __global__ void __launch_bounds__(256) k_topk_combine(PodView pv, OutView ov, Pa
     if (lane < k) {
         ov.node_idx[o] = idx;
         if (ov.score)
-            ov.score[o] = idx < 0 ? 0 : (POLICY == KS_SCORE_LEFTOVER ? leftover_score(key, pv.req_cpu[p], pv.req_mem[p]) : key);
+            ov.score[o] = idx < 0 ? 0 : key_score<POLICY>(key, pv.req_cpu[p], pv.req_mem[p]);
     }
     if (lane == 0 && ov.cnt) ov.cnt[p] = c;
 }
@@ -1195,26 +1195,18 @@ cudaError_t prepare_direct() {
     for (uint32_t W : {1u, 2u, 4u, 8u})
         with_label_width(W, [&](auto w) {
             constexpr int W_ = decltype(w)::value;
-            constexpr int LO = KS_SCORE_LEFTOVER, LA = KS_SCORE_LEAST_ALLOCATED, MA = KS_SCORE_MOST_ALLOCATED,
-                          LB = KS_SCORE_LEAST_BALANCED;
-            opt_in(k_select_direct<W_, LO, true>, tile_smem_bytes<W_, false>());
-            opt_in(k_select_direct<W_, LO, false>, tile_smem_bytes<W_, false>());
-            opt_in(k_select_direct<W_, LA, true>, tile_smem_bytes<W_, true>());
-            opt_in(k_select_direct<W_, LA, false>, tile_smem_bytes<W_, true>());
-            opt_in(k_select_direct<W_, MA, true>, tile_smem_bytes<W_, true>());
-            opt_in(k_select_direct<W_, MA, false>, tile_smem_bytes<W_, true>());
-            opt_in(k_select_direct<W_, LB, true>, tile_smem_bytes<W_, true>());
-            opt_in(k_select_direct<W_, LB, false>, tile_smem_bytes<W_, true>());
             opt_in(k_explain_counts<W_>, tile_smem_bytes<W_, false>());
-            opt_in(k_select_topk<W_, LO>, tile_smem_bytes<W_, false>());
-            opt_in(k_select_topk<W_, LA>, tile_smem_bytes<W_, true>());
-            opt_in(k_select_topk<W_, MA>, tile_smem_bytes<W_, true>());
-            opt_in(k_select_topk<W_, LB>, tile_smem_bytes<W_, true>());
             opt_in(k_preempt_scan<W_>, tile_smem_bytes<W_, false>());
-            opt_in(k_drain_scan<W_, LO>, tile_smem_bytes<W_, false>());
-            opt_in(k_drain_scan<W_, LA>, tile_smem_bytes<W_, true>());
-            opt_in(k_drain_scan<W_, MA>, tile_smem_bytes<W_, true>());
-            opt_in(k_drain_scan<W_, LB>, tile_smem_bytes<W_, true>());
+            for (int policy : {KS_SCORE_LEFTOVER, KS_SCORE_LEAST_ALLOCATED, KS_SCORE_MOST_ALLOCATED, KS_SCORE_LEAST_BALANCED})
+                with_policy(policy, [&](auto pol) {
+                    constexpr int POL = decltype(pol)::value;
+                    constexpr uint32_t SMEM = tile_smem_bytes<W_, POL != KS_SCORE_LEFTOVER>();
+                    opt_in(k_select_direct<W_, POL, true>, SMEM);
+                    opt_in(k_select_direct<W_, POL, false>, SMEM);
+                    opt_in(k_select_topk<W_, POL>, SMEM);
+                    opt_in(k_drain_scan<W_, POL>, SMEM);
+                    return e;
+                });
             return e;
         });
     return e;
@@ -1236,18 +1228,10 @@ static cudaError_t launch_direct_t(const SelectLaunch& L, const PartialView& par
 cudaError_t launch_select_direct(const SelectLaunch& L, const PartialView& part, const DirectGrid& g) {
     return with_label_width(L.nt.W, [&](auto w) {
         constexpr int W = decltype(w)::value;
-        const bool emit = L.ov.mask != nullptr;
-        if (L.policy == KS_SCORE_LEFTOVER)
-            return emit ? launch_direct_t<W, KS_SCORE_LEFTOVER, true>(L, part, g)
-                        : launch_direct_t<W, KS_SCORE_LEFTOVER, false>(L, part, g);
-        if (L.policy == KS_SCORE_MOST_ALLOCATED)
-            return emit ? launch_direct_t<W, KS_SCORE_MOST_ALLOCATED, true>(L, part, g)
-                        : launch_direct_t<W, KS_SCORE_MOST_ALLOCATED, false>(L, part, g);
-        if (L.policy == KS_SCORE_LEAST_BALANCED)
-            return emit ? launch_direct_t<W, KS_SCORE_LEAST_BALANCED, true>(L, part, g)
-                        : launch_direct_t<W, KS_SCORE_LEAST_BALANCED, false>(L, part, g);
-        return emit ? launch_direct_t<W, KS_SCORE_LEAST_ALLOCATED, true>(L, part, g)
-                    : launch_direct_t<W, KS_SCORE_LEAST_ALLOCATED, false>(L, part, g);
+        return with_policy(L.policy, [&](auto pol) {
+            constexpr int POL = decltype(pol)::value;
+            return L.ov.mask ? launch_direct_t<W, POL, true>(L, part, g) : launch_direct_t<W, POL, false>(L, part, g);
+        });
     });
 }
 
@@ -1285,10 +1269,9 @@ cudaError_t launch_select_topk(const NodeTable& nt, const PodView& pv, int polic
                                const PartialView& part, const DirectGrid& g, cudaStream_t st) {
     return with_label_width(nt.W, [&](auto w) {
         constexpr int W = decltype(w)::value;
-        if (policy == KS_SCORE_MOST_ALLOCATED) return launch_topk_t<W, KS_SCORE_MOST_ALLOCATED>(nt, pv, k, ov, part, g, st);
-        if (policy == KS_SCORE_LEAST_BALANCED) return launch_topk_t<W, KS_SCORE_LEAST_BALANCED>(nt, pv, k, ov, part, g, st);
-        return policy == KS_SCORE_LEFTOVER ? launch_topk_t<W, KS_SCORE_LEFTOVER>(nt, pv, k, ov, part, g, st)
-                                           : launch_topk_t<W, KS_SCORE_LEAST_ALLOCATED>(nt, pv, k, ov, part, g, st);
+        return with_policy(policy, [&](auto pol) {
+            return launch_topk_t<W, decltype(pol)::value>(nt, pv, k, ov, part, g, st);
+        });
     });
 }
 
@@ -1328,10 +1311,9 @@ cudaError_t launch_drain_round(const NodeTable& nt, const PodView& pv, const Dra
     if (pv.P == 0) return cudaSuccess;
     return with_label_width(nt.W, [&](auto w) {
         constexpr int W = decltype(w)::value;
-        if (policy == KS_SCORE_MOST_ALLOCATED) return launch_drain_t<W, KS_SCORE_MOST_ALLOCATED>(nt, pv, da, r, part, g, st);
-        if (policy == KS_SCORE_LEAST_BALANCED) return launch_drain_t<W, KS_SCORE_LEAST_BALANCED>(nt, pv, da, r, part, g, st);
-        return policy == KS_SCORE_LEFTOVER ? launch_drain_t<W, KS_SCORE_LEFTOVER>(nt, pv, da, r, part, g, st)
-                                           : launch_drain_t<W, KS_SCORE_LEAST_ALLOCATED>(nt, pv, da, r, part, g, st);
+        return with_policy(policy, [&](auto pol) {
+            return launch_drain_t<W, decltype(pol)::value>(nt, pv, da, r, part, g, st);
+        });
     });
 }
 

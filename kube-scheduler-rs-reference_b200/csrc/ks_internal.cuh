@@ -150,6 +150,29 @@ __device__ __forceinline__ int64_t alloc_score(int64_t fc, int64_t fm, int64_t a
            : POLICY == KS_SCORE_LEAST_BALANCED ? least_balanced_int(fc, fm, ac, am, rc, rm)
                                                : least_alloc_int(fc, fm, ac, am, rc, rm);
 }
+// The same chain with the policy chosen at run time, for the kernels that take it as an argument (k_stream_batch,
+// k_gang_batch: one instantiation per label width).  LEFTOVER gives the node key; node n's allocatables are read only by
+// the policies that score them.  The array pointers come by reference, so the kernel argument itself is read inside the
+// branch that uses it, as in the chain written out in place: the kernels' code stays the same.
+__device__ __forceinline__ int64_t alloc_score_rt(int policy, int64_t fc, int64_t fm, const int64_t* const& alloc_cpu,
+                                                  const int64_t* const& alloc_mem, uint32_t n, int64_t rc, int64_t rm) {
+    return policy == KS_SCORE_LEFTOVER ? leftover_key(fc, fm)
+           : policy == KS_SCORE_MOST_ALLOCATED
+               ? most_alloc_int(fc, fm, __ldg(alloc_cpu + n), __ldg(alloc_mem + n), rc, rm)
+           : policy == KS_SCORE_LEAST_BALANCED
+               ? least_balanced_int(fc, fm, __ldg(alloc_cpu + n), __ldg(alloc_mem + n), rc, rm)
+               : least_alloc_int(fc, fm, __ldg(alloc_cpu + n), __ldg(alloc_mem + n), rc, rm);
+}
+// The score of a winning key: LEFTOVER's key is the node part only, every other policy's key is its score
+template <int POLICY>
+__device__ __forceinline__ int64_t key_score(int64_t key, int64_t rc, int64_t rm) {
+    return POLICY == KS_SCORE_LEFTOVER ? leftover_score(key, rc, rm) : key;
+}
+// ... and with the policy chosen at run time, pod p's request read only for LEFTOVER
+__device__ __forceinline__ int64_t key_score_rt(int policy, int64_t key, const int64_t* const& req_cpu,
+                                                const int64_t* const& req_mem, uint32_t p) {
+    return policy == KS_SCORE_LEFTOVER ? leftover_score(key, __ldg(req_cpu + p), __ldg(req_mem + p)) : key;
+}
 // Warp argmax over (key, idx) with idx < 0 for "no candidate": larger key wins, ties go to the lower node index.
 // Every lane ends with the result.
 __device__ __forceinline__ void warp_argmax(int64_t& key, int32_t& idx) {
@@ -225,6 +248,24 @@ cudaError_t with_label_width(uint32_t W, F&& f) {
         case 4: return f(std::integral_constant<int, 4>{});
         case 8: return f(std::integral_constant<int, 8>{});
         default: return cudaErrorInvalidValue;
+    }
+}
+
+// The score policies (include/ksched.h).  A new policy is added here, in with_policy, in alloc_score / alloc_score_rt,
+// in prepare_direct's list and in the tests' restatement (DESIGN.md 5j); every launcher reaches it through with_policy.
+inline bool policy_valid(int policy) {
+    return policy == KS_SCORE_LEFTOVER || policy == KS_SCORE_LEAST_ALLOCATED || policy == KS_SCORE_MOST_ALLOCATED ||
+           policy == KS_SCORE_LEAST_BALANCED;
+}
+// Policy dispatch: calls f(std::integral_constant<int, POLICY>{}) for a valid policy; any other value is invalid.
+template <class F>
+cudaError_t with_policy(int policy, F&& f) {
+    if (!policy_valid(policy)) return cudaErrorInvalidValue;
+    switch (policy) {
+        case KS_SCORE_LEFTOVER: return f(std::integral_constant<int, KS_SCORE_LEFTOVER>{});
+        case KS_SCORE_LEAST_ALLOCATED: return f(std::integral_constant<int, KS_SCORE_LEAST_ALLOCATED>{});
+        case KS_SCORE_MOST_ALLOCATED: return f(std::integral_constant<int, KS_SCORE_MOST_ALLOCATED>{});
+        default: return f(std::integral_constant<int, KS_SCORE_LEAST_BALANCED>{});
     }
 }
 

@@ -115,8 +115,7 @@ __device__ __forceinline__ void rep_node(const NodeTable& nt, uint32_t n, int64_
 template <int POL>
 __device__ __forceinline__ int64_t rep_score(const RepNode& v, int64_t rc, int64_t rm, uint32_t j) {
     const int64_t c = v.fc - (int64_t)j * rc, m = v.fm - (int64_t)j * rm;
-    if (POL == KS_SCORE_LEFTOVER) return leftover_score(leftover_key(c, m), rc, rm);
-    return alloc_score<POL>(c, m, v.ac, v.am, rc, rm);
+    return key_score<POL>(POL == KS_SCORE_LEFTOVER ? leftover_key(c, m) : alloc_score<POL>(c, m, v.ac, v.am, rc, rm), rc, rm);
 }
 
 // G_n(S) = #{j < k : s_n(j) >= S}.  LEFTOVER: s_n(j) = key_n - (j + 1) * d, a closed form.  LEAST_ALLOCATED: a binary
@@ -618,10 +617,12 @@ cudaError_t launch_replicas(const NodeTable& nt, int policy, const ReplicaArgs& 
     if (a.T == 0 || nt.N == 0) return cudaSuccess;
     return with_label_width(nt.W, [&](auto w) {
         constexpr int W_ = decltype(w)::value;
-        if (policy == KS_SCORE_MOST_ALLOCATED) return rep_sequence<W_, KS_SCORE_MOST_ALLOCATED>(nt, a, st);
-        if (policy == KS_SCORE_LEAST_BALANCED) return rep_one_by_one<W_>(nt, a, q, st);
-        return policy == KS_SCORE_LEFTOVER ? rep_sequence<W_, KS_SCORE_LEFTOVER>(nt, a, st)
-                                           : rep_sequence<W_, KS_SCORE_LEAST_ALLOCATED>(nt, a, st);
+        return with_policy(policy, [&](auto pol) {
+            constexpr int POL = decltype(pol)::value;
+            // copy scores can rise and fall under LEAST_BALANCED: no threshold search, the copies go one at a time
+            if constexpr (POL == KS_SCORE_LEAST_BALANCED) return rep_one_by_one<W_>(nt, a, q, st);
+            else return rep_sequence<W_, POL>(nt, a, st);
+        });
     });
 }
 

@@ -129,13 +129,7 @@ __device__ __forceinline__ void stream_round_scan(const StreamBatchArgs& a, cons
 #pragma unroll
             for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
             if (rc <= fc && rm <= fm && miss == 0) {
-                const int64_t key =
-                    a.policy == KS_SCORE_LEFTOVER ? leftover_key(fc, fm)
-                    : a.policy == KS_SCORE_MOST_ALLOCATED
-                        ? most_alloc_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm)
-                    : a.policy == KS_SCORE_LEAST_BALANCED
-                        ? least_balanced_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm)
-                        : least_alloc_int(fc, fm, __ldg(a.alloc_cpu + n), __ldg(a.alloc_mem + n), rc, rm);
+                const int64_t key = alloc_score_rt(a.policy, fc, fm, a.alloc_cpu, a.alloc_mem, n, rc, rm);
                 if (key > best) { // ascending n per lane: strict '>' keeps the lowest index
                     best = key;
                     bidx = (int32_t)n;
@@ -193,9 +187,7 @@ __device__ __forceinline__ void stream_round_commit(const StreamBatchArgs& a, co
             const uint32_t p = __ldcg(pl + k);
             if (s_acc[k]) {
                 a.out_idx[p] = s_claim[k];
-                a.out_score[p] = a.policy == KS_SCORE_LEFTOVER
-                                     ? leftover_score(s_ckey[k], __ldg(a.req_cpu + p), __ldg(a.req_mem + p))
-                                     : s_ckey[k];
+                a.out_score[p] = key_score_rt(a.policy, s_ckey[k], a.req_cpu, a.req_mem, p);
             } else {
                 loser[e] = 1;
                 n_loser++;

@@ -1,26 +1,30 @@
 """KS_SCORE_LEAST_BALANCED (upstream's default resource scoring), CPU part: the numpy restatement against the Python
 definition on random and edge cells, near 2^53-2^55 and on cells where (1 - std) * 100 lies within a few ulps of an
-integer; the early-exit bound of the bit-parallel walk on a million (pod, node) pairs; the restatement's select and the
-one-copy-at-a-time replica heap against the oracle's cell codes and one full select per copy; the hand-derived GV-1
-values of tests/golden/gv1_least_balanced.json; the constant's mirrors; and KS_ERR_NO_DEVICE from every object-level
-call that takes a policy on a packing-only context (policies 2 and 5 are refused on the GPU, test_least_balanced_gpu)."""
-import os
-import re
+integer; the early-exit bound of the bit-parallel walk on a million (pod, node) pairs; the one-copy-at-a-time replica
+heap against one full select per copy; and, under policy 4, the tests of tests/policy_suite.py (select, round loop,
+GV-1, constant mirrors, packing-only context; policies 2 and 5 are refused on the GPU, test_least_balanced_gpu)."""
 from fractions import Fraction
 
 import numpy as np
 import pytest
 
-from helpers import load_golden
-from least_balanced_oracle import (LEAST_BALANCED, Oracle, _chain, balanced, hazard_cells, heap_packed, least,
-                                   node_bound, pod_slack, score, scores, topk_packed)
+from policy_oracle import (LEAST_BALANCED, Oracle, _chain, balanced, hazard_cells, heap_packed, least, node_bound,
+                           pod_slack)
+from policy_oracle import balanced_score as score
+from policy_oracle import balanced_scores as scores
+from policy_suite import *  # noqa: F401,F403 - the shared tests, run under the policy fixture below
+from policy_suite import check_packing_only_context
 from replicas_oracle import sequential_packed
 from test_replicas import random_cluster
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIM_C, LIM_M = 1 << 36, 1 << 55
 LB = LEAST_BALANCED
 I64_MAX = (1 << 63) - 1
+
+
+@pytest.fixture(scope="module")
+def policy():
+    return LEAST_BALANCED
 
 
 def test_definition_by_hand():
@@ -157,37 +161,6 @@ def test_walk_bound_holds_on_a_million_pairs(family):
     assert np.median((lim - s)[feas & (stored[None, :] <= 200)]) <= 60
 
 
-def _cluster(rng, N, P, W=1):
-    ac = rng.choice([0, 1000, 2000, 4000, 96000], N).astype(np.int64)
-    am = rng.choice([0, 1 << 30, 1 << 33, 3 << 32], N).astype(np.int64)
-    fc = (ac * rng.integers(-1, 9, N) // 8).astype(np.int64)
-    fm = (am * rng.integers(-1, 9, N) // 8).astype(np.int64)
-    lab = rng.integers(0, 8, (N, W)).astype(np.uint64)
-    rc = rng.choice([0, 250, 500, 1000], P).astype(np.int64)
-    rm = rng.choice([0, 1 << 28, 1 << 30], P).astype(np.int64)
-    sel = np.where(rng.random((P, W)) < 0.3, rng.integers(1, 4, (P, W)), 0).astype(np.uint64)
-    return fc, fm, ac, am, lab, rc, rm, sel
-
-
-def test_select_restatement_is_the_argmax_of_the_definition(orc):
-    o = Oracle(orc)
-    rng = np.random.default_rng(0xA5)
-    for it in range(60):
-        fc, fm, ac, am, lab, rc, rm, sel = _cluster(rng, int(rng.integers(1, 40)), int(rng.integers(1, 30)))
-        idx, sc, cnt, mask, codes = o.run_packed(fc, fm, ac, am, lab, rc, rm, sel, LB, want_codes=True)
-        lo = orc.run_packed(fc, fm, ac, am, lab, rc, rm, sel, 0)
-        assert np.array_equal(cnt, lo[2]) and np.array_equal(mask, lo[3])  # the mask and counts do not depend on it
-        for p in range(len(rc)):
-            cand = [(score(fc[n], fm[n], ac[n], am[n], rc[p], rm[p]), -n) for n in range(len(fc)) if codes[p, n] == 0]
-            if not cand:
-                assert idx[p] == -1 and sc[p] == 0
-            else:
-                s, n = max(cand)
-                assert (idx[p], sc[p]) == (-n, s), (it, p)
-        top = topk_packed(o, fc, fm, ac, am, lab, rc, rm, sel, 5)
-        assert np.array_equal(top[0][:, 0], idx) and np.array_equal(top[1][:, 0], sc) and np.array_equal(top[2], cnt)
-
-
 def test_copy_scores_are_not_monotone():
     """Why ks_place_replicas places these copies one at a time: s_n(j) rises and falls with j."""
     ac, am, fc, fm, rc, rm = 8000, 16 << 30, 8000, 4 << 30, 1000, 0
@@ -209,74 +182,6 @@ def test_heap_plan_equals_one_copy_at_a_time(orc):
     assert cases > 1000
 
 
-def _gv1(ks, orc):
-    g = load_golden("gv1.json")
-    arena = ks.objects.ObjectArena()
-    with ks.host.Context(ks.host.KSH_DEVICE_NONE) as ctx:
-        ctx.set_nodes(arena.nodes(g["nodes"]), len(g["nodes"]))
-        ctx.set_cluster_pods(arena.pods(g["bound_pods"]), len(g["bound_pods"]))
-        ac, am, lab, bn, bc, bm = ctx.export_packed()
-        rc, rm, sel = ctx.pack_pods(arena.pods(g["pods"]), len(g["pods"]))
-    fc, fm = orc.free_reduce(ac, am, bn, bc, bm)
-    assert fc.tolist() == g["expected_free_cpu_milli"] and fm.tolist() == g["expected_free_mem_bytes"]
-    return [p["name"] for p in g["pods"]], (fc, fm, ac, am, lab), rc, rm, sel
-
-
-def test_gv1_golden(ks, orc):
-    o = Oracle(orc)
-    want = load_golden("gv1_least_balanced.json")
-    names, cl, rc, rm, sel = _gv1(ks, orc)
-    fc, fm, ac, am, lab = cl
-    for pod, w in want["select"].items():
-        p = names.index(pod)
-        idx, sc = o.run_packed(*cl, rc[p:p + 1], rm[p:p + 1], sel[p:p + 1], LB, want_mask=False)[:2]
-        assert (int(idx[0]), int(sc[0])) == (w["node"], w["score"])
-        for n, (l, b) in enumerate(zip(w["least"], w["balanced"])):
-            if l is not None:
-                assert least(fc[n], fm[n], ac[n], am[n], rc[p], rm[p]) == l
-                assert balanced(fc[n], fm[n], ac[n], am[n], rc[p], rm[p]) == b
-    k = want["topk"]["k"]
-    for pod in ("p0", "p1"):
-        p = names.index(pod)
-        top = topk_packed(o, *cl, rc[p:p + 1], rm[p:p + 1], sel[p:p + 1], k)
-        assert top[0][0].tolist() == want["topk"][pod]["node"] and top[1][0].tolist() == want["topk"][pod]["score"]
-    w = want["replicas"]
-    p = names.index(w["spec"])
-    R = np.array([w["replicas"]], np.uint32)
-    rows, node, sc, _ = heap_packed(*cl, rc[p:p + 1], rm[p:p + 1], sel[p:p + 1], R)
-    seq = sequential_packed(o, *cl, rc[p:p + 1], rm[p:p + 1], sel[p:p + 1], R, LB)
-    assert all(np.array_equal(a, b) for a, b in zip((rows, node, sc), seq))
-    assert {f: int(rows[f][0]) for f in w["row"]} == w["row"]
-    assert node.tolist() == w["node"] and sc.tolist() == w["score"]
-
-
-def test_policy_constant_mirrors(ks):
-    hdr = open(os.path.join(ROOT, "include", "ksched.h")).read()
-    assert int(re.search(r"#define KS_SCORE_LEAST_BALANCED (\d+)", hdr).group(1)) == 4
-    assert ks.KS_SCORE_LEAST_BALANCED == ks.capi.KS_SCORE_LEAST_BALANCED == 4
-    rs = open(os.path.join(ROOT, "examples", "rust_shim", "ksched_sys.rs")).read()
-    assert re.search(r"pub const KS_SCORE_LEAST_BALANCED: c_int = 4;", rs)
-    assert "KS_SCORE_LEAST_BALANCED" in open(os.path.join(ROOT, "examples", "rust_shim", "ksched.rs")).read()
-    assert not re.search(r"#define KS_SCORE_\w+ (2|5)\b", hdr)  # 2 stays reserved, nothing above 4
-
-
-def test_packing_only_context_is_no_device_under_policy_4(ks):
+def test_packing_only_context_is_no_device_under_policy_4(ks, policy):
     """Every object-level call that takes a policy passes 4 through and, without a snapshot, is KS_ERR_NO_DEVICE."""
-    g = load_golden("gv1.json")
-    arena = ks.objects.ObjectArena()
-    pods = arena.pods(g["pods"][:3])
-    on_n2 = arena.pods(g["bound_pods"][1:3])
-    with ks.host.Context(ks.host.KSH_DEVICE_NONE) as ctx:
-        ctx.set_nodes(arena.nodes(g["nodes"]), len(g["nodes"]))
-        calls = [
-            lambda pol: ctx.select_nodes(pods, 3, policy=pol),
-            lambda pol: ctx.rank_nodes(pods, 3, 4, policy=pol),
-            lambda pol: ctx.reconcile_batch(pods, 3, policy=pol),
-            lambda pol: ctx.reconcile_gangs(pods, 3, [0, 2, 3], [1, 1], policy=pol),
-            lambda pol: ctx.drain_nodes(["n2"], on_n2, [0, 2], policy=pol),
-            lambda pol: ctx.place_replicas(pods, 3, [3, 1, 2], policy=pol),
-        ]
-        for i, call in enumerate(calls):
-            with pytest.raises(ks.KsError) as e:
-                call(LB)
-            assert e.value.code == ks.capi.KS_ERR_NO_DEVICE, i
+    check_packing_only_context(ks, policy)
