@@ -431,6 +431,63 @@ impl Gpu {
             (row, names)
         }).collect())
     }
+
+    /// Replica placement under one topology spread constraint (`topologySpreadConstraints` with `whenUnsatisfiable:
+    /// DoNotSchedule`): as `place_replicas`, but the copies spread over the values of `topology_key` (e.g.
+    /// "topology.kubernetes.io/zone" or "kubernetes.io/hostname") within `max_skew` of the least-loaded eligible
+    /// domain; `existing[t]` names the nodes of the bound pods that match spec t's constraint selector.  Returns per
+    /// spec the row (`blocked_domain` indexes the returned domain values) and the node names of the placed copies, and
+    /// the domain values.  Nothing is charged.
+    pub fn place_replicas_spread(&self, specs: &[(corev1::Pod, u32, u32)], topology_key: &str, existing: &[Vec<String>],
+                                 policy: i32) -> Result<(Vec<(ks_spread_plan, Vec<String>)>, Vec<String>), i32> {
+        let key = CString::new(topology_key).map_err(|_| KS_ERR_INVALID)?;
+        let n_nodes = unsafe { ksh_context_num_nodes(self.ctx) } as usize;
+        let mut dom = vec![-1i32; n_nodes.max(1)];
+        let mut d = 0u32;
+        let mut names = vec![0 as c_char; 64 * n_nodes.max(1)];
+        let mut off = vec![-1i64; n_nodes.max(1)];
+        let rc = unsafe {
+            ksh_context_topology_domains(self.ctx, key.as_ptr(), dom.as_mut_ptr(), &mut d, names.as_mut_ptr(), names.len(),
+                                         off.as_mut_ptr())
+        };
+        if rc != KS_OK {
+            return Err(rc);
+        }
+        let values: Vec<String> = off[..d as usize].iter().map(|&o| if o < 0 { String::new() } else {
+            unsafe { CStr::from_ptr(names.as_ptr().add(o as usize)) }.to_string_lossy().into_owned() }).collect();
+        let pv: Vec<PodView> = specs.iter().map(|(p, _, _)| PodView::new(p)).collect();
+        let pobj: Vec<ks_pod_obj> = pv.iter().map(|v| unsafe { ptr::read(&v.obj) }).collect();
+        let replicas: Vec<u32> = specs.iter().map(|s| s.1).collect();
+        let skew: Vec<u32> = specs.iter().map(|s| s.2).collect();
+        let mut ex: Vec<CString> = Vec::new();
+        let mut ex_off = vec![0u64; specs.len() + 1];
+        for t in 0..specs.len() {
+            for name in existing.get(t).map(|v| v.as_slice()).unwrap_or(&[]) {
+                ex.push(CString::new(name.as_str()).map_err(|_| KS_ERR_INVALID)?);
+            }
+            ex_off[t + 1] = ex.len() as u64;
+        }
+        let ex_ptr: Vec<*const c_char> = ex.iter().map(|s| s.as_ptr()).collect();
+        let total: usize = replicas.iter().map(|&r| r as usize).sum();
+        let mut rows = vec![ks_spread_plan::default(); specs.len()];
+        let mut node = vec![-1i32; total];
+        let rc = unsafe {
+            ksh_place_replicas_spread(self.ctx, pobj.as_ptr(), pobj.len() as u64, replicas.as_ptr(), key.as_ptr(),
+                                      skew.as_ptr(), ptr::null(), ex_ptr.as_ptr(), ex_off.as_ptr(), policy,
+                                      rows.as_mut_ptr(), node.as_mut_ptr(), ptr::null_mut(), ptr::null_mut())
+        };
+        if rc != KS_OK {
+            return Err(rc);
+        }
+        let mut at = 0usize;
+        let plans = rows.into_iter().zip(replicas).map(|(row, r)| {
+            let names = node[at..at + row.placed as usize].iter().map(|&n| unsafe {
+                CStr::from_ptr(ksh_context_node_name(self.ctx, n as u32)) }.to_string_lossy().into_owned()).collect();
+            at += r as usize;
+            (row, names)
+        }).collect();
+        Ok((plans, values))
+    }
 }
 
 impl Drop for Gpu {

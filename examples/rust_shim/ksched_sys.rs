@@ -22,6 +22,7 @@ pub const KS_SCORE_MOST_ALLOCATED: c_int = 3;
 pub const KS_SCORE_LEAST_BALANCED: c_int = 4;
 pub const KS_MEM_HOST: i32 = 0;
 pub const KS_MEM_DEVICE: i32 = 1;
+pub const KS_ERR_INVALID: c_int = -1; // a NULL or malformed argument
 pub const KS_ERR_NO_DEVICE: c_int = -8; // packing-only context or no CUDA device
 pub const KS_CELL_OK: c_int = 0;
 pub const KS_CELL_NOT_ENOUGH_RESOURCES: c_int = 1; // InvalidNodeReason::NotEnoughResources  (src/predicates.rs:16)
@@ -43,6 +44,9 @@ pub const KS_SCALEUP_MAX_TEMPLATES: u32 = 4096; // most templates of one ks_scal
 pub const KS_REPLICAS_MAX_SPECS: u32 = 4096; // most specs of one ks_place_replicas call
 pub const KS_REPLICAS_MAX: u32 = 65536; // most copies of one spec
 pub const KS_REPLICAS_MAX_TOTAL: u32 = 1 << 24; // most copies of one ks_place_replicas call
+pub const KS_SPREAD_MAX_DOMAINS: u32 = 1 << 20; // most topology domains of one ks_place_replicas_spread call
+pub const KS_SPREAD_MAX_EXISTING: u32 = 1 << 24; // most existing pods counted in one domain
+pub const KS_SPREAD_MAX_COUNTS: u64 = 1 << 26; // most specs x domains of existing or output counts
 
 #[repr(C)]
 pub struct ks_kv {
@@ -179,6 +183,25 @@ pub struct ks_replica_plan {
     pub max_per_node: u32,
     pub last_score: i64,
 }
+#[repr(C)]
+pub struct ks_spread {
+    pub n_domains: u32,
+    pub node_domain: *const i32,
+    pub max_skew: *const u32,
+    pub min_domains: *const u32,
+    pub existing: *const u32,
+}
+#[repr(C)]
+#[derive(Clone, Copy, Default, Debug)]
+pub struct ks_spread_plan {
+    pub placed: u32,
+    pub nodes: u32,
+    pub max_per_node: u32,
+    pub eligible_domains: u32,
+    pub min_count: u32,
+    pub blocked_domain: i32,
+    pub last_score: i64,
+}
 pub enum ks_snapshot {}
 pub enum ks_stream {}
 pub enum ksh_context {}
@@ -217,6 +240,9 @@ extern "C" {
                                reasons: *mut ks_pod_reasons) -> c_int;
     pub fn ks_place_replicas(s: *mut ks_snapshot, specs: *const ks_pods, replicas: *const u32, policy: c_int,
                              out: *mut ks_replica_plan, node: *mut i32, score: *mut i64) -> c_int;
+    pub fn ks_place_replicas_spread(s: *mut ks_snapshot, specs: *const ks_pods, replicas: *const u32, spread: *const ks_spread,
+                                    policy: c_int, out: *mut ks_spread_plan, node: *mut i32, score: *mut i64,
+                                    domain_count: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -267,6 +293,13 @@ extern "C" {
                                 reasons: *mut ks_pod_reasons) -> c_int;
     pub fn ksh_place_replicas(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, replicas: *const u32, policy: c_int,
                               out: *mut ks_replica_plan, node: *mut i32, score: *mut i64) -> c_int;
+    pub fn ksh_context_topology_domains(ctx: *const ksh_context, key: *const c_char, node_domain: *mut i32,
+                                        n_domains: *mut u32, names: *mut c_char, cap: usize, name_off: *mut i64) -> c_int;
+    pub fn ksh_place_replicas_spread(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, replicas: *const u32,
+                                     topology_key: *const c_char, max_skew: *const u32, min_domains: *const u32,
+                                     existing_node_names: *const *const c_char, existing_offset: *const u64, policy: c_int,
+                                     out: *mut ks_spread_plan, node: *mut i32, score: *mut i64,
+                                     domain_count: *mut u32) -> c_int;
     pub fn ksh_drain_nodes(ctx: *mut ksh_context, node_names: *const *const c_char, n: u64, pods: *const ks_pod_obj,
                            pod_offset: *const u64, policy: c_int, flags: u32, placed: *mut u32, node_idx: *mut i32) -> c_int;
     pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,

@@ -530,6 +530,69 @@ int ks_place_replicas(ks_snapshot* s, const ks_pods* specs /* host space */, con
                       int policy, ks_replica_plan* out /* [specs->n] */, int32_t* out_node /* [sum replicas] or NULL */,
                       int64_t* out_score /* [sum replicas] or NULL */);
 
+/* ---- topology spread for replica placement: where R copies of a pod spec land under a zone or hostname maxSkew, and
+ * how many fit (upstream PodTopologySpread, whenUnsatisfiable: DoNotSchedule; spec extension, DESIGN.md 5k) ----
+ * One constraint per spec whose label selector matches the spec's own pods (the copies count themselves), with
+ * nodeAffinityPolicy: Honor, nodeTaintsPolicy: Ignore and minDomains.  Domains are dense ids 0..D-1 of one topology key;
+ * node_domain[n] = -1 means node n lacks the key.  For spec t:
+ *   1. node n is eligible when node_domain[n] >= 0 and the spec's selector matches it ((sel & ~labels) == 0 on every
+ *      word); resource fit plays no part.  E_t = the domains that hold an eligible node;
+ *   2. cnt[d] starts at existing[t * D + d], the pods already bound in domain d that match the constraint's selector
+ *      (existing NULL: zeros);
+ *   3. m = min of cnt[d] over E_t, or 0 when |E_t| < min_domains[t] (upstream's minDomains rule).  E_t empty: nothing
+ *      is placed;
+ *   4. copy r goes to the node with the highest s_n(j_n) among the eligible nodes with j_n < c_n (j_n = copies already
+ *      on n; c_n and s_n(j) exactly as ks_place_replicas defines them) and cnt[d(n)] + 1 - m <= max_skew[t]; ties to
+ *      the lower node index.  Then j_n, cnt[d(n)] and m are updated.  The first copy with no candidate stops the spec
+ *      (nothing changes after a stop, so no later copy could be placed): the rest get node -1 and score 0;
+ *   5. out[t]: placed, nodes, max_per_node and last_score as in ks_replica_plan; eligible_domains = |E_t|; min_count = m
+ *      after the last copy; blocked_domain = the lowest domain of E_t that the skew rule still admits but whose eligible
+ *      nodes hold no further copy, -1 when every copy was placed or no such domain exists (E_t empty, or minDomains held
+ *      m at 0 and every domain is at max_skew).  When m is a true minimum, every domain at m is then full, so this is
+ *      the domain that blocks the scale-out;
+ *   6. out_node / out_score as in ks_place_replicas (per-spec offset = prefix sum of replicas), out_domain_count[t * D +
+ *      d] = the final cnt[d].  Each may be NULL;
+ *   7. nothing is charged; committing a spec's out_node slice with ks_snapshot_commit_claims accepts every claim.
+ * If every node has a domain and max_skew >= replicas + max(existing), or all nodes share one domain, the plan is
+ * ks_place_replicas' plan.  With node_domain[n] = n (kubernetes.io/hostname), max_skew 1 and no existing pods, the copies
+ * go to distinct nodes in order of copy 0's score until every node with room holds one.
+ * Limits and checks as ks_place_replicas (specs, replicas per spec and in total, requests in [0, limit]; every policy),
+ * plus, on the host before any device work: KS_ERR_INVALID for a NULL spread, node_domain or max_skew, or a node_domain
+ * entry outside [-1, D); KS_ERR_RANGE for D = 0 or D > KS_SPREAD_MAX_DOMAINS, a max_skew of 0, an existing entry above
+ * KS_SPREAD_MAX_EXISTING, or T * D > KS_SPREAD_MAX_COUNTS when existing or out_domain_count is given.  An empty
+ * snapshot gives every row zeros with blocked_domain = -1, every copy -1, and counts = existing.
+ * Host-space arguments and outputs.  One H2D copy; one kernel orders the nodes by domain (a stable sort, once per call);
+ * then one CTA per spec (specs strided over at most 2 per SM) places that spec's copies one after another, so the time
+ * grows with the copies of the largest spec, as KS_SCORE_LEAST_BALANCED's ks_place_replicas; one D2H copy.  Staging: the
+ * snapshot's pinned block and its device input and result blocks hold the specs, 4 bytes per node, 4 * T * D bytes of
+ * existing counts when given, n * 32 bytes of rows, 12 bytes per requested copy with a copy list and 4 * T * D bytes of
+ * counts when asked; its device scratch block holds 16 bytes per node for the order, and per CTA 12 bytes per node,
+ * 20 bytes per domain and 12 bytes per 1024-node block, as many CTAs as fit in 64 MiB (at least one).  The blocks are
+ * shared with the other staged calls and grow to the largest. */
+#define KS_SPREAD_MAX_DOMAINS (1u << 20)
+#define KS_SPREAD_MAX_EXISTING (1u << 24)
+#define KS_SPREAD_MAX_COUNTS (1ull << 26)
+typedef struct ks_spread {          /* host memory */
+    uint32_t n_domains;             /* D >= 1 */
+    const int32_t* node_domain;     /* [N], each in [-1, D) */
+    const uint32_t* max_skew;       /* [T], >= 1 */
+    const uint32_t* min_domains;    /* [T] or NULL (= no minDomains) */
+    const uint32_t* existing;       /* [T * D] or NULL (= 0) */
+} ks_spread;
+typedef struct ks_spread_plan {     /* 32 bytes per spec */
+    uint32_t placed;
+    uint32_t nodes;                 /* distinct nodes among the placed copies */
+    uint32_t max_per_node;          /* most copies placed on one node */
+    uint32_t eligible_domains;      /* |E_t| */
+    uint32_t min_count;             /* m after the last copy */
+    int32_t blocked_domain;         /* see 5 above; -1 = none */
+    int64_t last_score;             /* score of copy placed-1; 0 when placed = 0 */
+} ks_spread_plan;
+int ks_place_replicas_spread(ks_snapshot* s, const ks_pods* specs /* host space */, const uint32_t* replicas /* [n] */,
+                             const ks_spread* spread, int policy, ks_spread_plan* out /* [specs->n] */,
+                             int32_t* out_node /* [sum replicas] or NULL */, int64_t* out_score /* [sum replicas] or NULL */,
+                             uint32_t* out_domain_count /* [specs->n * D] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

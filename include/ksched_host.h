@@ -216,6 +216,30 @@ int ksh_scaleup_estimate(ksh_context* ctx, const ks_node_obj* templates, uint64_
 int ksh_place_replicas(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n, const uint32_t* replicas, int policy,
                        ks_replica_plan* out, int32_t* out_node, int64_t* out_score);
 
+/* The domains of one topology key (e.g. "topology.kubernetes.io/zone", "kubernetes.io/hostname") over the node store:
+ * nodes whose labels carry `key' get dense ids 0..D-1, numbered by the value's first appearance in node-index order;
+ * every other node gets -1.  out_node_domain[N] (N = ksh_context_num_nodes) and *out_n_domains receive them.  The
+ * values are written into names (cap bytes) back to back, NUL-terminated like ksh_reconcile_batch's bodies;
+ * out_name_off[d] = offset of domain d's value, or -1 (the buffer was full); D <= N, so N entries always suffice.
+ * names / out_name_off may be NULL.  Pure host work: works on a packing-only context.  Node upserts and removals
+ * renumber the domains of later calls. */
+int ksh_context_topology_domains(const ksh_context* ctx, const char* key, int32_t* out_node_domain,
+                                 uint32_t* out_n_domains, char* names, size_t cap, int64_t* out_name_off);
+
+/* Replica placement under one topology spread constraint over objects (ks_place_replicas_spread, ksched.h): spec t is
+ * pods[t] with replicas[t] copies, packed as ksh_place_replicas packs them, spread over the domains of topology_key as
+ * ksh_context_topology_domains numbers them, with max_skew[t] and min_domains[t] (min_domains may be NULL).  The nodes
+ * of the bound pods that match spec t's constraint selector are existing_node_names[existing_offset[t] ..
+ * existing_offset[t+1]) (ks_pod_obj carries no pod labels, so the caller filters the pods); a name not in the store,
+ * or a node without the key, is not counted.  existing_offset [n + 1] may be NULL (no existing pods).  Nothing is
+ * charged.  Outputs as ks_place_replicas_spread gives them (out[n] required when n > 0; out_node, out_score [sum of
+ * replicas] and out_domain_count [n * D] may be NULL).  With no node carrying the key, every row is empty and
+ * out_domain_count is not written.  KS_ERR_NO_DEVICE on a packing-only context. */
+int ksh_place_replicas_spread(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n, const uint32_t* replicas,
+                              const char* topology_key, const uint32_t* max_skew, const uint32_t* min_domains,
+                              const char* const* existing_node_names, const uint64_t* existing_offset, int policy,
+                              ks_spread_plan* out, int32_t* out_node, int64_t* out_score, uint32_t* out_domain_count);
+
 #ifdef __cplusplus
 }
 #endif

@@ -189,6 +189,29 @@ if hasattr(lib, "ks_place_replicas"):  # the same for ks_place_replicas
 KS_REPLICAS_MAX_SPECS = 4096
 KS_REPLICAS_MAX = 65536
 KS_REPLICAS_MAX_TOTAL = 1 << 24
+
+
+class ks_spread(C.Structure):
+    _fields_ = [("n_domains", C.c_uint32), ("node_domain", C.c_void_p), ("max_skew", C.c_void_p),
+                ("min_domains", C.c_void_p), ("existing", C.c_void_p)]
+
+
+class ks_spread_plan(C.Structure):
+    _fields_ = [("placed", C.c_uint32), ("nodes", C.c_uint32), ("max_per_node", C.c_uint32),
+                ("eligible_domains", C.c_uint32), ("min_count", C.c_uint32), ("blocked_domain", C.c_int32),
+                ("last_score", C.c_int64)]
+
+
+# the same row as a numpy record
+SPREAD_PLAN_DTYPE = np.dtype([("placed", np.uint32), ("nodes", np.uint32), ("max_per_node", np.uint32),
+                              ("eligible_domains", np.uint32), ("min_count", np.uint32), ("blocked_domain", np.int32),
+                              ("last_score", np.int64)])
+if hasattr(lib, "ks_place_replicas_spread"):  # the same for ks_place_replicas_spread
+    _proto("ks_place_replicas_spread", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.POINTER(ks_spread),
+           C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p)
+KS_SPREAD_MAX_DOMAINS = 1 << 20
+KS_SPREAD_MAX_EXISTING = 1 << 24
+KS_SPREAD_MAX_COUNTS = 1 << 26
 KS_PREEMPT_MAX_ABS_SUM = 1 << 62
 KS_ERR_INVALID, KS_ERR_RANGE = -1, -5
 KS_REFERENCE_ATTEMPTS = 5

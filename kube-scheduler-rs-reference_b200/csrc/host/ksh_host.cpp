@@ -22,7 +22,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 // ks_explain, ks_select_topk, ks_preempt, ks_gang_bind, ks_drain_check and ks_scaleup_estimate are defined by the CUDA
 // core in the same library.  The references are weak so that this file still links with device stand-ins that only
 // provide the older ks_* entries (tests/native); ksh_explain_pods, ksh_rank_nodes, ksh_preempt_pods, ksh_reconcile_gangs,
-// ksh_drain_nodes, ksh_scaleup_estimate and ksh_place_replicas then report KS_ERR_NO_DEVICE.
+// ksh_drain_nodes, ksh_scaleup_estimate, ksh_place_replicas and ksh_place_replicas_spread then report KS_ERR_NO_DEVICE.
 #pragma weak ks_explain
 #pragma weak ks_select_topk
 #pragma weak ks_preempt
@@ -30,6 +30,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 #pragma weak ks_drain_check
 #pragma weak ks_scaleup_estimate
 #pragma weak ks_place_replicas
+#pragma weak ks_place_replicas_spread
 
 namespace {
 
@@ -1589,6 +1590,85 @@ int ksh_place_replicas(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const
     if (rc) return rc;
     ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     return ks_place_replicas(c->snap, &kp, replicas, policy, out, out_node, out_score);
+}
+KSH_CATCH
+
+// Dense domain ids of one topology key in order of first appearance over the node indices; -1 for a node without it.
+// values[d] = the pair id of domain d.
+static uint32_t topology_domains(const ksh_context* c, const char* key, int32_t* dom, std::vector<uint32_t>* values) {
+    std::unordered_map<uint32_t, int32_t> of_pair; // pair id -> domain
+    for (uint32_t n = 0; n < c->N; n++) {
+        dom[n] = -1;
+        for (uint32_t pid : c->node_pids[n]) {
+            if (std::strcmp(c->pairs.str(pid), key) != 0) continue; // "key\0value": the key part ends at the NUL
+            auto it = of_pair.emplace(pid, (int32_t)of_pair.size()).first;
+            if (it->second == (int32_t)values->size()) values->push_back(pid);
+            dom[n] = it->second;
+            break; // a node carries a key once
+        }
+    }
+    return (uint32_t)values->size();
+}
+
+int ksh_context_topology_domains(const ksh_context* c, const char* key, int32_t* out_node_domain, uint32_t* out_n_domains,
+                                 char* names, size_t cap, int64_t* out_name_off) try {
+    if (!c || !key || !out_n_domains || (c->N && !out_node_domain)) return fail(KS_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    std::vector<uint32_t> values;
+    const uint32_t D = topology_domains(c, key, out_node_domain, &values);
+    *out_n_domains = D;
+    if (!names || !out_name_off) return KS_OK;
+    size_t used = 0;
+    for (uint32_t d = 0; d < D; d++) {
+        const char* k = c->pairs.str(values[d]);
+        const char* v = k + std::strlen(k) + 1;
+        const size_t len = std::strlen(v);
+        out_name_off[d] = -1;
+        if (used + len + 1 > cap) continue; // -1 = did not fit
+        std::memcpy(names + used, v, len + 1);
+        out_name_off[d] = (int64_t)used;
+        used += len + 1;
+    }
+    return KS_OK;
+}
+KSH_CATCH
+
+int ksh_place_replicas_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const uint32_t* replicas,
+                              const char* topology_key, const uint32_t* max_skew, const uint32_t* min_domains,
+                              const char* const* existing_node_names, const uint64_t* existing_offset, int policy,
+                              ks_spread_plan* out, int32_t* out_node, int64_t* out_score, uint32_t* out_domain_count) try {
+    if (!c || !topology_key || (n && (!pods || !replicas || !max_skew || !out))) return fail(KS_ERR_INVALID, "NULL argument");
+    if (existing_offset && existing_offset[n] && !existing_node_names) return fail(KS_ERR_INVALID, "NULL existing_node_names");
+    if (existing_offset)
+        for (uint64_t t = 0; t < n; t++)
+            if (existing_offset[t + 1] < existing_offset[t]) return fail(KS_ERR_INVALID, "existing offsets decrease");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    if (!ks_place_replicas_spread) return fail(KS_ERR_NO_DEVICE, "this library has no ks_place_replicas_spread");
+    if (n == 0) return KS_OK;
+    std::vector<int64_t>&rc_ = c->pk_cpu, &rm_ = c->pk_mem; // the same packed batch buffers as ksh_select_nodes
+    std::vector<uint64_t>& sel = c->pk_sel;
+    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel);
+    if (rc) return rc;
+    std::vector<int32_t> dom(c->N);
+    std::vector<uint32_t> values;
+    const uint32_t D = topology_domains(c, topology_key, dom.data(), &values);
+    // no node carries the key: no domain is eligible, and a single empty domain gives exactly that
+    const uint32_t Dc = std::max(D, 1u);
+    std::vector<uint32_t> existing;
+    if (existing_offset) {
+        if (n * Dc > KS_SPREAD_MAX_COUNTS) return fail(KS_ERR_RANGE, "too many specs x domains of existing counts (at most 2^26)");
+        existing.assign(n * Dc, 0);
+        for (uint64_t t = 0; t < n; t++)
+            for (uint64_t i = existing_offset[t]; i < existing_offset[t + 1]; i++) {
+                const int32_t idx = existing_node_names[i] ? node_index_of(c, existing_node_names[i]) : -1;
+                if (idx >= 0 && dom[idx] >= 0) existing[t * Dc + (uint32_t)dom[idx]]++; // unknown or keyless: not counted
+            }
+    }
+    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
+    ks_spread sp{Dc, dom.data(), max_skew, min_domains, existing_offset ? existing.data() : nullptr};
+    return ks_place_replicas_spread(c->snap, &kp, replicas, &sp, policy, out, out_node, out_score,
+                                    D ? out_domain_count : nullptr);
 }
 KSH_CATCH
 

@@ -1606,6 +1606,135 @@ int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* repl
     return KS_OK;
 }
 
+int ks_place_replicas_spread(ks_snapshot* s, const ks_pods* specs, const uint32_t* replicas, const ks_spread* spread,
+                             int policy, ks_spread_plan* out, int32_t* out_node, int64_t* out_score,
+                             uint32_t* out_domain_count) {
+    int rc = check_pods(s, specs);
+    if (rc) return rc;
+    if (specs->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_place_replicas_spread takes host-space specs");
+    const uint64_t T = specs->n;
+    if (T && (!replicas || !out)) return fail(KS_ERR_INVALID, "NULL replicas or out");
+    if (!spread || !spread->node_domain || !spread->max_skew) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
+    if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    const uint32_t D = spread->n_domains, N = s->N;
+    if (D == 0 || D > KS_SPREAD_MAX_DOMAINS) return fail(KS_ERR_RANGE, "%u domains (1 to %u)", D, KS_SPREAD_MAX_DOMAINS);
+    for (uint32_t n = 0; n < N; n++)
+        if (spread->node_domain[n] < -1 || spread->node_domain[n] >= (int64_t)D)
+            return fail(KS_ERR_INVALID, "node %u: domain %d outside [-1, %u)", n, spread->node_domain[n], D);
+    if (T > KS_REPLICAS_MAX_SPECS) return fail(KS_ERR_RANGE, "%llu specs (at most %u)", (unsigned long long)T, KS_REPLICAS_MAX_SPECS);
+    uint64_t total = 0;
+    for (uint64_t t = 0; t < T; t++) {
+        if (replicas[t] > KS_REPLICAS_MAX)
+            return fail(KS_ERR_RANGE, "spec %llu: %u replicas (at most %u)", (unsigned long long)t, replicas[t], KS_REPLICAS_MAX);
+        if (spread->max_skew[t] == 0) return fail(KS_ERR_RANGE, "spec %llu: max_skew 0 (at least 1)", (unsigned long long)t);
+        total += replicas[t];
+    }
+    if (total > KS_REPLICAS_MAX_TOTAL)
+        return fail(KS_ERR_RANGE, "%llu replicas in one call (at most %u)", (unsigned long long)total, KS_REPLICAS_MAX_TOTAL);
+    const uint64_t TD = T * D;
+    if ((spread->existing || out_domain_count) && TD > KS_SPREAD_MAX_COUNTS)
+        return fail(KS_ERR_RANGE, "%llu specs x %u domains of counts (at most 2^26)", (unsigned long long)T, D);
+    if (spread->existing)
+        for (uint64_t i = 0; i < TD; i++)
+            if (spread->existing[i] > KS_SPREAD_MAX_EXISTING)
+                return fail(KS_ERR_RANGE, "spec %llu, domain %llu: %u existing pods (at most 2^24)",
+                            (unsigned long long)(i / D), (unsigned long long)(i % D), spread->existing[i]);
+    rc = check_commit_requests(T, specs->req_cpu, specs->req_mem);
+    if (rc) return rc;
+    if (T == 0) return KS_OK;
+    const bool copies = out_node || out_score;
+    if (N == 0) { // no node: no eligible domain, every copy is -1
+        for (uint64_t t = 0; t < T; t++) out[t] = ks_spread_plan{0, 0, 0, 0, 0, -1, 0};
+        if (out_node) memset(out_node, 0xff, total * 4);
+        if (out_score) memset(out_score, 0, total * 8);
+        if (out_domain_count) {
+            if (spread->existing) memcpy(out_domain_count, spread->existing, TD * 4);
+            else memset(out_domain_count, 0, TD * 4);
+        }
+        return KS_OK;
+    }
+    const uint32_t W = s->W;
+    std::lock_guard<std::mutex> lk(s->mu);
+    CU_TRY(cudaSetDevice(s->device));
+    const uint64_t C = copies ? total : 0, E = spread->existing ? TD : 0, K = out_domain_count ? TD : 0;
+    uint32_t ctas;
+    uint64_t seq_bytes;
+    spread_seq_grid(N, D, (uint32_t)T, s->sms, &ctas, &seq_bytes);
+    // in = [rc T | rm T | sel T*W | replicas T | offset T | max_skew T | min_domains T | node_domain N | existing T*D],
+    // results = [rows T | score C | node C | counts T*D], work = [sort 2N | perm N | pos N | dstart D+1 | k_spread_seq]
+    BlockLayout in, res, work;
+    const size_t i_rc = in.take<int64_t>(T), i_rm = in.take<int64_t>(T), i_sel = in.take<uint64_t>(T * W),
+                 i_rep = in.take<uint32_t>(T), i_off = in.take<uint64_t>(T), i_skew = in.take<uint32_t>(T),
+                 i_mind = in.take<uint32_t>(spread->min_domains ? T : 0), i_dom = in.take<int32_t>(N),
+                 i_ex = in.take<uint32_t>(E);
+    const size_t o_rows = res.take<ks_spread_plan>(T), o_score = res.take<int64_t>(C), o_node = res.take<int32_t>(C),
+                 o_cnt = res.take<uint32_t>(K);
+    const size_t w_sort = work.take<uint32_t>(2ull * N), w_perm = work.take<uint32_t>(N), w_pos = work.take<uint32_t>(N),
+                 w_dstart = work.take<uint32_t>((uint64_t)D + 1), w_seq = work.take<uint8_t>(seq_bytes, 16);
+    uint8_t* h_out = nullptr;
+    rc = stage_blocks(s, in.size, res.size, &h_out);
+    if (rc) return rc;
+    CU_TRY(s->d_work.ensure(work.size));
+    uint8_t* h_in = s->h_stage.as<uint8_t>();
+    memcpy(h_in + i_rc, specs->req_cpu, T * 8);
+    memcpy(h_in + i_rm, specs->req_mem, T * 8);
+    memcpy(h_in + i_sel, specs->sel, T * 8 * W);
+    memcpy(h_in + i_rep, replicas, T * 4);
+    uint64_t* h_off = at<uint64_t>(h_in, i_off);
+    for (uint64_t t = 0, o = 0; t < T; o += replicas[t], t++) h_off[t] = o;
+    memcpy(h_in + i_skew, spread->max_skew, T * 4);
+    if (spread->min_domains) memcpy(h_in + i_mind, spread->min_domains, T * 4);
+    memcpy(h_in + i_dom, spread->node_domain, (size_t)N * 4);
+    if (E) memcpy(h_in + i_ex, spread->existing, E * 4);
+    cudaStream_t st = s->stream;
+    uint8_t* d_in = s->d_in.as<uint8_t>();
+    uint8_t* d_out = s->d_out.as<uint8_t>();
+    uint8_t* d_work = s->d_work.as<uint8_t>();
+    CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
+    if (copies) { // copies past `placed' stay -1 / 0
+        CU_TRY(cudaMemsetAsync(d_out + o_score, 0, C * 8, st));
+        CU_TRY(cudaMemsetAsync(d_out + o_node, 0xff, C * 4, st));
+    }
+    ReplicaArgs a{};
+    a.T = (uint32_t)T;
+    a.req_cpu = at<int64_t>(d_in, i_rc);
+    a.req_mem = at<int64_t>(d_in, i_rm);
+    a.sel = at<uint64_t>(d_in, i_sel);
+    a.replicas = at<uint32_t>(d_in, i_rep);
+    a.offset = at<uint64_t>(d_in, i_off);
+    a.out_node = copies ? at<int32_t>(d_out, o_node) : nullptr;
+    a.out_score = copies ? at<int64_t>(d_out, o_score) : nullptr;
+    SpreadOrder o;
+    o.node_domain = at<int32_t>(d_in, i_dom);
+    o.sort_buf = at<uint32_t>(d_work, w_sort);
+    o.perm = at<uint32_t>(d_work, w_perm);
+    o.pos = at<uint32_t>(d_work, w_pos);
+    o.dstart = at<uint32_t>(d_work, w_dstart);
+    SpreadArgs q;
+    q.D = D;
+    q.node_domain = o.node_domain;
+    q.perm = o.perm;
+    q.pos = o.pos;
+    q.dstart = o.dstart;
+    q.max_skew = at<uint32_t>(d_in, i_skew);
+    q.min_domains = spread->min_domains ? at<uint32_t>(d_in, i_mind) : nullptr;
+    q.existing = E ? at<uint32_t>(d_in, i_ex) : nullptr;
+    q.rows = at<ks_spread_plan>(d_out, o_rows);
+    q.out_count = K ? at<uint32_t>(d_out, o_cnt) : nullptr;
+    q.scratch = at<unsigned char>(d_work, w_seq);
+    q.ctas = ctas;
+    cudaError_t e = launch_spread(node_table(s), policy, a, o, q, st);
+    if (e != cudaSuccess) return fail(KS_ERR_CUDA, "spread placement launch failed: %s", cudaGetErrorString(e));
+    CU_TRY(cudaMemcpyAsync(h_out, d_out, res.size, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaStreamSynchronize(st));
+    memcpy(out, h_out + o_rows, T * sizeof(ks_spread_plan));
+    if (out_node) memcpy(out_node, h_out + o_node, C * 4);
+    if (out_score) memcpy(out_score, h_out + o_score, C * 8);
+    if (K) memcpy(out_domain_count, h_out + o_cnt, K * 4);
+    s->last_path = "spread";
+    return KS_OK;
+}
+
 // ---------------------------------------------------------------------------------------------- async streaming
 struct StreamItem {
     uint64_t ticket;

@@ -142,6 +142,33 @@ void replica_seq_grid(uint32_t N, uint32_t T, int sms, uint32_t* ctas, uint32_t*
 cudaError_t launch_replicas(const NodeTable& nt, int policy, const ReplicaArgs& a, const ReplicaSeqArgs& q,
                             cudaStream_t st);
 
+// topology spread for replica placement (ks_place_replicas_spread, ks_spread.cu).  The specs come as ReplicaArgs' T,
+// requests, selectors, replicas, offsets and copy list (its rows and search state are not used).  Device memory.
+struct SpreadOrder {              // k_spread_order's input and outputs, once per call
+    const int32_t* node_domain;   // [N]
+    uint32_t* sort_buf;           // [2N]
+    uint32_t* perm;               // [N]: nodes with a domain by (domain, node), the rest after dstart[D]
+    uint32_t* pos;                // [N]: node -> position in perm
+    uint32_t* dstart;             // [D + 1]: domain d's nodes are perm[dstart[d] .. dstart[d + 1])
+};
+struct SpreadArgs {
+    uint32_t D;
+    const int32_t* node_domain;   // [N]
+    const uint32_t *perm, *pos, *dstart;
+    const uint32_t* max_skew;     // [T]
+    const uint32_t* min_domains;  // [T] or null
+    const uint32_t* existing;     // [T * D] or null
+    ks_spread_plan* rows;         // [T]
+    uint32_t* out_count;          // [T * D] or null
+    unsigned char* scratch;       // [bytes of spread_seq_grid]
+    uint32_t ctas;
+};
+// k_spread_seq's CTAs - as many as fit in 64 MiB (at least one, at most one per spec and two per SM) - and the bytes of
+// their scratch: per CTA 12 per node, 20 per domain and 12 per block slot
+void spread_seq_grid(uint32_t N, uint32_t D, uint32_t T, int sms, uint32_t* ctas, uint64_t* bytes);
+cudaError_t launch_spread(const NodeTable& nt, int policy, const ReplicaArgs& a, const SpreadOrder& o,
+                          const SpreadArgs& q, cudaStream_t st);
+
 } // namespace ks
 
 namespace ks {

@@ -18,12 +18,11 @@
 // Under LEAST_BALANCED s_n(j) can rise or fall with j, and neither shortcut holds: after k_rep_scan and k_rep_init,
 // k_rep_seq places the copies one at a time, one CTA per spec (specs strided over a grid sized to a scratch budget).
 #include "ks_launch.h"
+#include "ks_replicas.cuh"
 #include "ks_sort.cuh"
 
 namespace ks {
 
-constexpr int REP_THREADS = 256;
-constexpr int REP_WARPS = REP_THREADS / 32;
 constexpr int REP_PROBES = 32; // thresholds per search pass, one per lane
 // The score of a placed copy lies in [0, 2^61): free after the copy is >= 0 and free <= 2^36 m / 2^55 B, so LEFTOVER's
 // score is at most 2^58 + 2^55, and LEAST_ALLOCATED's at most (100 * 2^36 + 100 * 2^55) / 2 < 2^61 (an allocatable of
@@ -75,49 +74,6 @@ void replica_chunks(uint32_t N, uint32_t T, int sms, uint32_t* n_chunks, uint32_
     *n_chunks = (tiles + per - 1) / per;
 }
 
-// One node as a spec sees it: free values, allocatable (LEAST_ALLOCATED, MOST_ALLOCATED) and k_n.
-struct RepNode {
-    int64_t fc, fm, ac, am;
-    uint32_t k;
-};
-
-// c_n: 0 unless copy 0's cell is KS_CELL_OK, else the copies the node's free holds (UINT64_MAX when both requests are 0).
-// fc >= rc >= 0 and fm >= rm >= 0 when it is not 0, so the divisions are exact integer floors.
-template <int W>
-__device__ __forceinline__ uint64_t rep_copies(const NodeTable& nt, uint32_t n, int64_t rc, int64_t rm,
-                                               const uint64_t (&sel)[W], RepNode& v) {
-    v.fc = nt.free_cpu[n];
-    v.fm = nt.free_mem[n];
-    uint64_t miss = 0;
-#pragma unroll
-    for (int w = 0; w < W; w++) miss |= sel[w] & ~nt.labels[(uint64_t)w * nt.Npad + n];
-    if (rc > v.fc || rm > v.fm || miss) return 0;
-    uint64_t c = ~0ull;
-    if (rc > 0) c = (uint64_t)(v.fc / rc);
-    if (rm > 0) c = min(c, (uint64_t)(v.fm / rm));
-    return c;
-}
-
-template <int W, int POL>
-__device__ __forceinline__ void rep_node(const NodeTable& nt, uint32_t n, int64_t rc, int64_t rm, const uint64_t (&sel)[W],
-                                         uint32_t R, RepNode& v, uint64_t& c) {
-    c = rep_copies<W>(nt, n, rc, rm, sel, v);
-    v.k = (uint32_t)min(c, (uint64_t)R);
-    if (POL != KS_SCORE_LEFTOVER && v.k) {
-        v.ac = nt.alloc_cpu[n];
-        v.am = nt.alloc_mem[n];
-    } else {
-        v.ac = v.am = 0;
-    }
-}
-
-// s_n(j): ks_select's score with j copies bound (j < c_n)
-template <int POL>
-__device__ __forceinline__ int64_t rep_score(const RepNode& v, int64_t rc, int64_t rm, uint32_t j) {
-    const int64_t c = v.fc - (int64_t)j * rc, m = v.fm - (int64_t)j * rm;
-    return key_score<POL>(POL == KS_SCORE_LEFTOVER ? leftover_key(c, m) : alloc_score<POL>(c, m, v.ac, v.am, rc, rm), rc, rm);
-}
-
 // G_n(S) = #{j < k : s_n(j) >= S}.  LEFTOVER: s_n(j) = key_n - (j + 1) * d, a closed form.  LEAST_ALLOCATED: a binary
 // search over j, after the bounds s0 = s_n(0) and sl = s_n(k - 1).  MOST_ALLOCATED: not that count but the copies a
 // node filled in s_n(0) order holds, s0 >= S ? k : 0.
@@ -141,18 +97,6 @@ __device__ __forceinline__ uint32_t rep_at(const RepNode& v, int64_t rc, int64_t
     return a;
 }
 
-template <class T, class Op>
-__device__ __forceinline__ T rep_reduce(T x, Op op, T* sh /* [REP_WARPS] */) {
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) x = op(x, __shfl_xor_sync(0xffffffffu, x, off));
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = x;
-    __syncthreads();
-    T r = sh[0];
-#pragma unroll
-    for (int w = 1; w < REP_WARPS; w++) r = op(r, sh[w]);
-    __syncthreads(); // sh may be reused
-    return r;
-}
 __device__ __forceinline__ uint64_t sat_add(uint64_t a, uint64_t b) { return a + b < a ? ~0ull : a + b; }
 
 // What every (chunk, spec) kernel reads of its spec

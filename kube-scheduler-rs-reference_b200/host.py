@@ -44,6 +44,9 @@ for _name, _res, _args in [
     ("ksh_drain_nodes", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, C.c_int, C.c_uint32, _vp, _vp]),
     ("ksh_scaleup_estimate", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, C.c_uint64, _vp, C.c_uint64, _vp, _vp, _vp, _vp]),
     ("ksh_place_replicas", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_int, _vp, _vp, _vp]),
+    ("ksh_context_topology_domains", C.c_int, [_vp, C.c_char_p, _vp, C.POINTER(C.c_uint32), _vp, C.c_size_t, _vp]),
+    ("ksh_place_replicas_spread", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_char_p, _vp, _vp, _vp, _vp, C.c_int, _vp,
+                                            _vp, _vp, _vp]),
 ]:
     _f = getattr(lib, _name)
     _f.restype = _res
@@ -213,6 +216,65 @@ class Context:
         if rc != capi.KS_OK:
             raise KsError(rc, "ksh_place_replicas")
         return rows, node, score, offset
+
+    def topology_domains(self, key):
+        """(node_domain int32 [N], values): dense domain ids of the topology key `key' over the node store, numbered by
+        each value's first appearance in node order (-1 = the node lacks the key), and values[d] = domain d's value."""
+        n = self.n_nodes
+        dom = np.empty(n, np.int32)
+        d = C.c_uint32()
+        # every value is at most a label value's length; grow once if some did not fit
+        cap = 64 * max(n, 1)
+        while True:
+            buf = C.create_string_buffer(cap)
+            off = np.empty(max(n, 1), np.int64)
+            rc = lib.ksh_context_topology_domains(self._h, key.encode(), dom.ctypes.data, C.byref(d), buf, cap,
+                                                  off.ctypes.data)
+            if rc != capi.KS_OK:
+                raise KsError(rc, "ksh_context_topology_domains")
+            if (off[:d.value] >= 0).all():
+                break
+            cap *= 4
+        raw = buf.raw
+        values = [raw[o:raw.index(b"\0", o)].decode() for o in off[:d.value].tolist()]
+        return dom, values
+
+    def place_replicas_spread(self, pods, n, replicas, topology_key, max_skew, min_domains=None, existing_nodes=None,
+                              policy=capi.KS_SCORE_LEFTOVER, want_nodes=True, first=0):
+        """Replica placement under one topology spread constraint over objects (ksh_place_replicas_spread): pod t asks
+        for replicas[t] copies of itself, spread over the domains of topology_key with max_skew[t] (and min_domains[t]).
+        existing_nodes[t] lists the node names of the bound pods that match spec t's constraint selector (None: none).
+        Charges nothing.  Returns (rows, node, score, offset, counts) as Snapshot.place_replicas_spread, with the
+        domains numbered as topology_domains(topology_key) numbers them (counts None when no node has the key)."""
+        replicas = np.ascontiguousarray(replicas, np.uint32).reshape(-1)
+        max_skew = np.ascontiguousarray(max_skew, np.uint32).reshape(-1)
+        if replicas.shape[0] != n or max_skew.shape[0] != n:
+            raise ValueError(f"replicas / max_skew have {replicas.shape[0]} / {max_skew.shape[0]} entries, pods {n}")
+        mind = None if min_domains is None else np.ascontiguousarray(min_domains, np.uint32).reshape(-1)
+        names, ex_off = None, None
+        if existing_nodes is not None:
+            flat = [s.encode() for lst in existing_nodes for s in lst]
+            names = (C.c_char_p * max(len(flat), 1))(*flat)
+            ex_off = np.zeros(n + 1, np.uint64)
+            np.cumsum([len(lst) for lst in existing_nodes], out=ex_off[1:])
+        D = len(self.topology_domains(topology_key)[1])
+        offset = np.zeros(n + 1, np.uint64)
+        np.cumsum(replicas, dtype=np.uint64, out=offset[1:])
+        rows = np.zeros(n, capi.SPREAD_PLAN_DTYPE)
+        total = int(offset[-1]) if want_nodes and int(offset[-1]) <= capi.KS_REPLICAS_MAX_TOTAL else 0
+        node = np.empty(total, np.int32) if want_nodes else None
+        score = np.empty(total, np.int64) if want_nodes else None
+        counts = np.empty((n, D), np.uint32) if D and n * D <= capi.KS_SPREAD_MAX_COUNTS else None
+        rc = lib.ksh_place_replicas_spread(self._h, _addr(pods, first), n, replicas.ctypes.data, topology_key.encode(),
+                                           max_skew.ctypes.data, None if mind is None else mind.ctypes.data,
+                                           None if names is None else C.cast(names, _vp),
+                                           None if ex_off is None else ex_off.ctypes.data, int(policy), rows.ctypes.data,
+                                           None if node is None else node.ctypes.data,
+                                           None if score is None else score.ctypes.data,
+                                           None if counts is None else counts.ctypes.data)
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ksh_place_replicas_spread")
+        return rows, node, score, offset, counts
 
     def select_nodes(self, pods, n, policy=capi.KS_SCORE_LEFTOVER, first=0):
         idx = np.empty(n, np.int32)

@@ -289,6 +289,50 @@ class Snapshot:
             raise KsError(rc, "ks_place_replicas")
         return rows, node, score, offset
 
+    def place_replicas_spread(self, req_cpu, req_mem, sel, replicas, node_domain, n_domains, max_skew, min_domains=None,
+                              existing=None, policy=capi.KS_SCORE_LEFTOVER, want_nodes=True, want_counts=True):
+        """Replica placement under one topology spread constraint (ks_place_replicas_spread, whenUnsatisfiable:
+        DoNotSchedule): as place_replicas, but copy r may only go to a node whose domain (node_domain[n] in
+        [0, n_domains), -1 = no topology key) keeps the domain's count within max_skew[t] of the minimum over the
+        eligible domains.  min_domains [T] and existing [T, n_domains] (matching pods already bound per domain) may be
+        None.  Nothing is charged.  Returns (rows, node, score, offset, counts): rows a capi.SPREAD_PLAN_DTYPE record
+        array [T]; node / score / offset as place_replicas (node and score None unless want_nodes); counts uint32
+        [T, n_domains], the final count per domain (None unless want_counts)."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        t = int(pods.n)
+        replicas = np.asarray(replicas).reshape(-1)
+        if replicas.shape[0] != t:
+            raise ValueError(f"replicas has {replicas.shape[0]} entries, specs {t}")
+        if t and (replicas.min() < 0 or replicas.max() > 0xFFFFFFFF):
+            raise ValueError("replicas must lie in [0, 2^32)")
+        replicas = _c(replicas, np.uint32)
+        node_domain = _c(node_domain, np.int32).reshape(-1)
+        max_skew = _c(max_skew, np.uint32).reshape(-1)
+        if max_skew.shape[0] != t:
+            raise ValueError(f"max_skew has {max_skew.shape[0]} entries, specs {t}")
+        if min_domains is not None:
+            min_domains = _c(min_domains, np.uint32).reshape(-1)
+            if min_domains.shape[0] != t:
+                raise ValueError(f"min_domains has {min_domains.shape[0]} entries, specs {t}")
+        d = int(n_domains)
+        if existing is not None:
+            existing = _c(existing, np.uint32).reshape(-1)
+            if existing.shape[0] != t * d:
+                raise ValueError(f"existing has {existing.shape[0]} entries, specs x domains {t * d}")
+        spread = capi.ks_spread(d, _ptr(node_domain), _ptr(max_skew), _ptr(min_domains), _ptr(existing))
+        offset = np.zeros(t + 1, np.uint64)
+        np.cumsum(replicas, dtype=np.uint64, out=offset[1:])
+        rows = np.zeros(t, capi.SPREAD_PLAN_DTYPE)
+        total = int(offset[-1]) if want_nodes and int(offset[-1]) <= capi.KS_REPLICAS_MAX_TOTAL else 0
+        node = np.empty(total, np.int32) if want_nodes else None
+        score = np.empty(total, np.int64) if want_nodes else None
+        counts = np.empty((t, d), np.uint32) if want_counts and 0 < t * d <= capi.KS_SPREAD_MAX_COUNTS else None
+        rc = lib.ks_place_replicas_spread(self._h, C.byref(pods), _ptr(replicas), C.byref(spread), int(policy),
+                                          _ptr(rows), _ptr(node), _ptr(score), _ptr(counts))
+        if rc != capi.KS_OK:
+            raise KsError(rc, "ks_place_replicas_spread")
+        return rows, node, score, offset, counts
+
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
         """The reference's own policy (src/main.rs:49-71), seeded: (node_idx, attempts_used, draw_node, draw_code)."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
