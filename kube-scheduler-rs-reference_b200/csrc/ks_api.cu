@@ -1,6 +1,7 @@
 // ks_api.cu — implementation of the C ABI declared in include/ksched.h (snapshot handle, staging,
 // path selection).  Plain CUDA runtime; no torch, no oracle, no CPU fallback: every entry point that
 // computes returns KS_ERR_NO_DEVICE / KS_ERR_CUDA when no H100 (sm_90) is present.
+#include <cassert>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -44,8 +45,8 @@ struct ks_snapshot {
     // Staging shared by every call that holds mu until its final stream synchronise: no two are ever live, and the
     // snapshot keeps the largest any of them needed.  d_in: host-space pods (stage_pods), bound and claim lists
     // (stage_claims) and the host-staged calls' inputs; d_out: every host-space result, a host-space mask at 0; d_work:
-    // stream/gang, drain and scale-up scratch; h_stage: the host-staged calls' pinned block (stage_blocks).  A call
-    // ensures each buffer once, for its whole layout, before it takes a pointer: a growing ensure frees those taken.
+    // stream/gang, drain, scale-up and replica scratch; h_stage: the host-staged calls' pinned block (HostStaged).  A
+    // call ensures each buffer once, for its whole layout, before it takes a pointer: a growing ensure frees those taken.
     HostBuf h_stage;
     DevBuf d_in, d_work, d_out;
     // Per call kind: an all-device select, top-k or preempt returns after enqueue and its kernels keep using these (as
@@ -113,41 +114,118 @@ static int check_commit_requests(uint64_t n, const int64_t* req_cpu, const int64
     return KS_OK;
 }
 
-// The shared staging set for one host-staged call: d_in and d_out hold in_bytes and out_bytes, and the pinned block holds
-// the inputs at 0 and the results at the next multiple of 16 after them (*h_out).
-static int stage_blocks(ks_snapshot* s, size_t in_bytes, size_t out_bytes, uint8_t** h_out) {
-    BlockLayout h;
-    h.take<uint8_t>(in_bytes);
-    const size_t out_at = h.take<uint8_t>(out_bytes, 16);
-    CU_TRY(s->h_stage.ensure(h.size));
-    CU_TRY(s->d_in.ensure(in_bytes));
-    CU_TRY(s->d_out.ensure(out_bytes));
-    *h_out = at<uint8_t>(s->h_stage.p, out_at);
-    return KS_OK;
+// ---- host-staged calls: ks_stream_bind's device loop, ks_gang_bind, ks_drain_check, ks_scaleup_estimate,
+// ks_place_replicas and ks_place_replicas_spread ----
+// Such a call gathers its host inputs into the snapshot's pinned block, makes one H2D copy to d_in, launches, makes one
+// D2H copy from d_out and copies its results out before it returns.  Its HostStaged plan declares every array it stages
+// once, with its type and count: in() an input, gathered from src or, with src NULL, filled by the caller through
+// host(); out() a result, copied to dst when dst is set and n > 0; work() device scratch in d_work.  The handle a
+// declaration returns is the only way to the array afterwards, so its offset, size and type are written once.  The
+// pinned block holds the inputs at 0 and the results at the next multiple of 16 after them.
+template <class T>
+struct Staged { int block; size_t off; uint64_t n; }; // block: HostStaged::IN, OUT or WORK
+
+class HostStaged {
+  public:
+    enum { IN, OUT, WORK };
+    template <class T>
+    Staged<T> in(const T* src, uint64_t n, size_t align = alignof(T)) { return add<T>(IN, const_cast<T*>(src), n, align); }
+    template <class T>
+    Staged<T> out(T* dst, uint64_t n, size_t align = alignof(T)) { return add<T>(OUT, dst, n, align); }
+    template <class T>
+    Staged<T> work(uint64_t n, size_t align = alignof(T)) { return add<T>(WORK, nullptr, n, align); }
+    // With the snapshot locked and every array declared: ensures h_stage, d_in, d_out and d_work once, for the whole plan
+    // and at least min_in / min_out bytes of inputs / results, then gathers the inputs that have a source.  A growing
+    // ensure frees what the buffer held, so no pointer is handed out before this.
+    cudaError_t reserve(ks_snapshot* s, size_t min_in = 0, size_t min_out = 0) {
+        const size_t in = std::max(layout_[IN].size, min_in), out = std::max(layout_[OUT].size, min_out);
+        cudaError_t e = s->h_stage.ensure((in + 15) / 16 * 16 + out);
+        if (e == cudaSuccess) e = s->d_in.ensure(in);
+        if (e == cudaSuccess) e = s->d_out.ensure(out);
+        if (e == cudaSuccess) e = s->d_work.ensure(layout_[WORK].size);
+        if (e != cudaSuccess) return e;
+        dev_[IN] = s->d_in.p;
+        dev_[OUT] = s->d_out.p;
+        dev_[WORK] = s->d_work.p;
+        host_[IN] = s->h_stage.p;
+        host_[OUT] = at<unsigned char>(s->h_stage.p, (layout_[IN].size + 15) / 16 * 16);
+        reserved_ = true;
+        copy(IN);
+        return cudaSuccess;
+    }
+    template <class T>
+    T* dev(Staged<T> a) const {
+        assert(reserved_);
+        return at<T>(dev_[a.block], a.off);
+    }
+    // the pinned copy of an input or result: inputs before upload(), results after finish()
+    template <class T>
+    T* host(Staged<T> a) const {
+        assert(reserved_ && a.block != WORK);
+        return at<T>(host_[a.block], a.off);
+    }
+    cudaError_t upload(cudaStream_t st) const { // the one H2D copy
+        return cudaMemcpyAsync(dev_[IN], host_[IN], layout_[IN].size, cudaMemcpyHostToDevice, st);
+    }
+    cudaError_t finish(cudaStream_t st) const { // the one D2H copy, a synchronise, then each result to its dst
+        cudaError_t e = cudaMemcpyAsync(host_[OUT], dev_[OUT], layout_[OUT].size, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e == cudaSuccess) copy(OUT);
+        return e;
+    }
+
+  private:
+    struct Copy { int block; size_t off; void* p; size_t bytes; }; // p: an input's src or a result's dst
+    template <class T>
+    Staged<T> add(int block, T* p, uint64_t n, size_t align) {
+        const size_t off = layout_[block].take<T>(n, align);
+        if (p && n) {
+            assert(n_copies_ < MAX_COPIES);
+            copies_[n_copies_++] = Copy{block, off, p, n * sizeof(T)};
+        }
+        return Staged<T>{block, off, n};
+    }
+    void copy(int block) const { // gathers the inputs into the pinned block, or scatters the results from it
+        for (int i = 0; i < n_copies_; i++) {
+            const Copy& c = copies_[i];
+            if (c.block == IN && block == IN) memcpy(at<unsigned char>(host_[IN], c.off), c.p, c.bytes);
+            if (c.block == OUT && block == OUT) memcpy(c.p, at<unsigned char>(host_[OUT], c.off), c.bytes);
+        }
+    }
+    static constexpr int MAX_COPIES = 16;
+    BlockLayout layout_[3];
+    void* dev_[3] = {};
+    void* host_[2] = {};
+    Copy copies_[MAX_COPIES];
+    int n_copies_ = 0;
+    bool reserved_ = false;
+};
+
+// The scratch of k_stream_batch and k_gang_batch in d_work, [pkey | pidx | pend] (the kernels rebuild the pending list on
+// every call: nothing in it persists), declared on the caller's plan.
+struct StreamBatchScratch { Staged<int64_t> key; Staged<int32_t> idx; Staged<uint32_t> pend; };
+static StreamBatchScratch stream_batch_scratch(HostStaged& h, int sms) {
+    return {h.work<int64_t>((size_t)STREAM_BATCH_MAX * sms), h.work<int32_t>((size_t)STREAM_BATCH_MAX * sms, 256),
+            h.work<uint32_t>(2 * STREAM_BATCH_MAX, 256)};
 }
 
-// What k_stream_batch and k_gang_batch take from the snapshot: the node table, the policy, the grid and their scratch in
-// d_work, [pkey | pidx | pend] (the kernels rebuild the pending list on every call: nothing in it persists).  The caller
-// sets the pods, the outputs, ctl and max_rounds.
-static int stream_batch_args(ks_snapshot* s, int policy, StreamBatchArgs* a) {
-    BlockLayout w;
-    const size_t o_key = w.take<int64_t>((size_t)STREAM_BATCH_MAX * s->sms),
-                 o_idx = w.take<int32_t>((size_t)STREAM_BATCH_MAX * s->sms, 256),
-                 o_pend = w.take<uint32_t>(2 * STREAM_BATCH_MAX, 256);
-    CU_TRY(s->d_work.ensure(w.size));
-    a->N = s->N;
-    a->Npad = s->Npad;
-    a->alloc_cpu = s->alloc_cpu.as<int64_t>();
-    a->alloc_mem = s->alloc_mem.as<int64_t>();
-    a->labels = s->labels.as<uint64_t>();
-    a->free_cpu = s->free_cpu.as<int64_t>();
-    a->free_mem = s->free_mem.as<int64_t>();
-    a->policy = policy;
-    a->pkey = at<int64_t>(s->d_work.p, o_key);
-    a->pidx = at<int32_t>(s->d_work.p, o_idx);
-    a->pend = at<uint32_t>(s->d_work.p, o_pend);
-    a->grid = std::max(1u, std::min<uint32_t>((uint32_t)s->sms, (s->N + 127u) / 128u));
-    return KS_OK;
+// What k_stream_batch and k_gang_batch take from the snapshot: the node table, the policy, the grid and the scratch, after
+// reserve().  The caller sets the pods, the outputs, ctl and max_rounds.
+static StreamBatchArgs stream_batch_args(const ks_snapshot* s, int policy, const HostStaged& h, const StreamBatchScratch& w) {
+    StreamBatchArgs a;
+    a.N = s->N;
+    a.Npad = s->Npad;
+    a.alloc_cpu = s->alloc_cpu.as<int64_t>();
+    a.alloc_mem = s->alloc_mem.as<int64_t>();
+    a.labels = s->labels.as<uint64_t>();
+    a.free_cpu = s->free_cpu.as<int64_t>();
+    a.free_mem = s->free_mem.as<int64_t>();
+    a.policy = policy;
+    a.pkey = h.dev(w.key);
+    a.pidx = h.dev(w.idx);
+    a.pend = h.dev(w.pend);
+    a.grid = std::max(1u, std::min<uint32_t>((uint32_t)s->sms, (s->N + 127u) / 128u));
+    return a;
 }
 
 // The host bound or claim list of set_bound, apply_bind and commit_claims, copied to d_in on the snapshot's stream as
@@ -1099,42 +1177,32 @@ int ks_stream_bind(ks_snapshot* s, const ks_pods* pods, int policy, int32_t* out
         // the micro-batch costs ONE H2D copy, ONE cooperative launch that runs every round and ONE D2H copy
         std::lock_guard<std::mutex> lk(s->mu);
         CU_TRY(cudaSetDevice(s->device));
-        BlockLayout in, out;
-        const size_t i_rc = in.take<int64_t>(n), i_rm = in.take<int64_t>(n), i_sel = in.take<uint64_t>(n * W);
-        const size_t o_score = out.take<int64_t>(n), o_idx = out.take<int32_t>(n), o_ctl = out.take<uint32_t>(2);
+        HostStaged h;
+        const auto cpu = h.in(pods->req_cpu, n), mem = h.in(pods->req_mem, n);
+        const auto sel = h.in(pods->sel, n * W);
+        const auto score = h.out(out_score, n);
+        const auto idx = h.out(out_node_idx, n);
+        const auto ctl = h.out<uint32_t>(nullptr, 2);
+        const StreamBatchScratch w = stream_batch_scratch(h, s->sms);
         // sized for STREAM_BATCH_MAX pods on first use, so a stream of growing micro-batches never reallocates
-        uint8_t* h_out = nullptr;
-        rc = stage_blocks(s, (size_t)STREAM_BATCH_MAX * (16 + 8 * KS_MAX_LABEL_WORDS), (size_t)STREAM_BATCH_MAX * 12 + 8,
-                          &h_out);
-        if (!rc) rc = stage_blocks(s, in.size, out.size, &h_out);
-        StreamBatchArgs a;
-        if (!rc) rc = stream_batch_args(s, policy, &a);
-        if (rc) return rc;
-        uint8_t* h_in = s->h_stage.as<uint8_t>();
-        memcpy(h_in + i_rc, pods->req_cpu, n * 8);
-        memcpy(h_in + i_rm, pods->req_mem, n * 8);
-        memcpy(h_in + i_sel, pods->sel, n * 8 * W);
+        CU_TRY(h.reserve(s, (size_t)STREAM_BATCH_MAX * (16 + 8 * KS_MAX_LABEL_WORDS), (size_t)STREAM_BATCH_MAX * 12 + 8));
         cudaStream_t st = s->stream;
-        uint8_t* d_in = s->d_in.as<uint8_t>();
-        uint8_t* d_out = s->d_out.as<uint8_t>();
-        CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
+        CU_TRY(h.upload(st));
+        StreamBatchArgs a = stream_batch_args(s, policy, h, w);
         a.m = (uint32_t)n;
-        a.req_cpu = at<int64_t>(d_in, i_rc);
-        a.req_mem = at<int64_t>(d_in, i_rm);
-        a.sel = at<uint64_t>(d_in, i_sel);
-        a.ctl = at<uint32_t>(d_out, o_ctl);
-        a.out_idx = at<int32_t>(d_out, o_idx);
-        a.out_score = at<int64_t>(d_out, o_score);
+        a.req_cpu = h.dev(cpu);
+        a.req_mem = h.dev(mem);
+        a.sel = h.dev(sel);
+        a.ctl = h.dev(ctl);
+        a.out_idx = h.dev(idx);
+        a.out_score = h.dev(score);
         a.max_rounds = (uint32_t)n + 1;
         s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
         s->version++;
         cudaError_t e = launch_stream_batch(a, W, st);
         if (e != cudaSuccess) return fail(KS_ERR_CUDA, "k_stream_batch launch failed: %s", cudaGetErrorString(e));
-        CU_TRY(cudaMemcpyAsync(h_out, d_out, out.size, cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaStreamSynchronize(st));
-        memcpy(out_node_idx, h_out + o_idx, n * 4);
-        if (out_score) memcpy(out_score, h_out + o_score, n * 8);
-        if (out_rounds) *out_rounds = at<uint32_t>(h_out, o_ctl)[1];
+        CU_TRY(h.finish(st));
+        if (out_rounds) *out_rounds = h.host(ctl)[1];
         s->last_path = "stream_batch";
         return KS_OK;
     }
@@ -1219,54 +1287,42 @@ int ks_gang_bind(ks_snapshot* s, const ks_pods* pods, const ks_gangs* gangs, int
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
     if (!s->coop) return fail(KS_ERR_CUDA, "device %d has no cooperative launch", s->device);
-    // one block each way: in = [rc P | rm P | sel P*W | offset G+1 | min_member G], out = [score P | idx P | ctl 2G | placed G]
-    BlockLayout in, out;
-    const size_t i_rc = in.take<int64_t>(P), i_rm = in.take<int64_t>(P), i_sel = in.take<uint64_t>(P * W),
-                 i_off = in.take<uint32_t>(G + 1), i_min = in.take<uint32_t>(G);
-    const size_t o_score = out.take<int64_t>(P), o_idx = out.take<int32_t>(P), o_ctl = out.take<uint32_t>(2 * G),
-                 o_placed = out.take<uint32_t>(G);
-    uint8_t* h_out = nullptr;
-    rc = stage_blocks(s, in.size, out.size, &h_out);
-    StreamBatchArgs a;
-    if (!rc) rc = stream_batch_args(s, policy, &a);
-    if (rc) return rc;
-    uint8_t* h_in = s->h_stage.as<uint8_t>();
-    memcpy(h_in + i_rc, pods->req_cpu, P * 8);
-    memcpy(h_in + i_rm, pods->req_mem, P * 8);
-    memcpy(h_in + i_sel, pods->sel, P * 8 * W);
-    uint32_t* h_off = at<uint32_t>(h_in, i_off);
-    for (uint64_t g = 0; g <= G; g++) h_off[g] = (uint32_t)off[g];
-    memcpy(h_in + i_min, gangs->min_member, G * 4);
+    HostStaged h;
+    const auto cpu = h.in(pods->req_cpu, P), mem = h.in(pods->req_mem, P);
+    const auto sel = h.in(pods->sel, P * W);
+    const auto offset = h.in<uint32_t>(nullptr, G + 1);
+    const auto min_member = h.in(gangs->min_member, G);
+    const auto score = h.out(out_score, P);
+    const auto idx = h.out(out_node_idx, P);
+    const auto ctl = h.out<uint32_t>(nullptr, 2 * G);
+    const auto placed = h.out(out_placed, G);
+    const StreamBatchScratch w = stream_batch_scratch(h, s->sms);
+    CU_TRY(h.reserve(s));
+    for (uint64_t g = 0; g <= G; g++) h.host(offset)[g] = (uint32_t)off[g];
     cudaStream_t st = s->stream;
-    uint8_t* d_in = s->d_in.as<uint8_t>();
-    uint8_t* d_out = s->d_out.as<uint8_t>();
-    CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
+    CU_TRY(h.upload(st));
+    StreamBatchArgs a = stream_batch_args(s, policy, h, w);
     a.m = (uint32_t)P;
-    a.req_cpu = at<int64_t>(d_in, i_rc);
-    a.req_mem = at<int64_t>(d_in, i_rm);
-    a.sel = at<uint64_t>(d_in, i_sel);
+    a.req_cpu = h.dev(cpu);
+    a.req_mem = h.dev(mem);
+    a.sel = h.dev(sel);
     a.ctl = nullptr; // per group: ga.ctl
-    a.out_idx = at<int32_t>(d_out, o_idx);
-    a.out_score = at<int64_t>(d_out, o_score);
+    a.out_idx = h.dev(idx);
+    a.out_score = h.dev(score);
     a.max_rounds = 0; // per group
     GangArgs ga;
     ga.n = (uint32_t)G;
-    ga.offset = at<uint32_t>(d_in, i_off);
-    ga.min_member = at<uint32_t>(d_in, i_min);
-    ga.ctl = at<uint32_t>(d_out, o_ctl);
-    ga.placed = at<uint32_t>(d_out, o_placed);
+    ga.offset = h.dev(offset);
+    ga.min_member = h.dev(min_member);
+    ga.ctl = h.dev(ctl);
+    ga.placed = h.dev(placed);
     s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
     s->version++;
     cudaError_t e = launch_gang_batch(a, ga, W, st);
     if (e != cudaSuccess) return fail(KS_ERR_CUDA, "k_gang_batch launch failed: %s", cudaGetErrorString(e));
-    CU_TRY(cudaMemcpyAsync(h_out, d_out, out.size, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    memcpy(out_node_idx, h_out + o_idx, P * 4);
-    if (out_score) memcpy(out_score, h_out + o_score, P * 8);
-    const uint32_t* ctl = at<uint32_t>(h_out, o_ctl);
+    CU_TRY(h.finish(st));
     if (out_rounds)
-        for (uint64_t g = 0; g < G; g++) out_rounds[g] = ctl[2 * g + 1];
-    if (out_placed) memcpy(out_placed, h_out + o_placed, G * 4);
+        for (uint64_t g = 0; g < G; g++) out_rounds[g] = h.host(ctl)[2 * g + 1];
     s->last_path = "gang_batch";
     return KS_OK;
 }
@@ -1317,33 +1373,29 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidate
         for (uint64_t r = 0; r < off[d + 1] - off[d]; r++) per_round[r]++;
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
-    // one block each way: in = [rc P | rm P | sel P*W (pods in round order) | cand_node D | pod_base D | cand_id D |
-    // excluded-node bits Npad/32 (with the flag)], out = [score P | idx P | placed D]
+    // pods in round order, then the candidates in round order
     const bool excl = flags & KS_DRAIN_EXCLUDE_CANDIDATES;
-    BlockLayout in, out;
-    const size_t i_rc = in.take<int64_t>(P), i_rm = in.take<int64_t>(P), i_sel = in.take<uint64_t>(P * W),
-                 i_node = in.take<int32_t>(D), i_base = in.take<uint32_t>(D), i_id = in.take<uint32_t>(D),
-                 i_excl = in.take<uint32_t>(excl ? s->Npad / 32 : 0);
-    const size_t o_score = out.take<int64_t>(P), o_idx = out.take<int32_t>(P), o_placed = out.take<uint32_t>(D);
+    HostStaged h;
+    const auto cpu = h.in<int64_t>(nullptr, P), mem = h.in<int64_t>(nullptr, P);
+    const auto sel = h.in<uint64_t>(nullptr, P * W);
+    const auto cand_node = h.in<int32_t>(nullptr, D);
+    const auto pod_base = h.in<uint32_t>(nullptr, D), cand_id = h.in<uint32_t>(nullptr, D);
+    const auto excluded = h.in<uint32_t>(nullptr, excl ? s->Npad / 32 : 0); // bits of the candidates' nodes
+    const auto score = h.out(out_score, P);
+    const auto idx = h.out(out_node_idx, P);
+    const auto placed = h.out(out_placed, D);
     // node-chunk partials: the largest round needs the most
     uint64_t part_rows = 0;
     for (uint32_t r = 0; r < rounds; r++)
         part_rows = std::max<uint64_t>(part_rows, (uint64_t)direct_grid(W, per_round[r], s->Npad, s->sms).n_chunks * per_round[r]);
-    // work = [ov_fc P | ov_fm P | part keys | ov_node P | part indices | ov_cnt D, failed D (one array: zeroed together)]
-    BlockLayout work;
-    const size_t w_fc = work.take<int64_t>(P), w_fm = work.take<int64_t>(P), w_key = work.take<int64_t>(part_rows),
-                 w_node = work.take<int32_t>(P), w_idx = work.take<int32_t>(part_rows), w_cnt = work.take<uint32_t>(2 * D);
-    uint8_t* h_out = nullptr;
-    rc = stage_blocks(s, in.size, out.size, &h_out);
-    if (rc) return rc;
-    CU_TRY(s->d_work.ensure(work.size));
-    uint8_t* h_in = s->h_stage.as<uint8_t>();
-    int64_t* h_rc = at<int64_t>(h_in, i_rc);
-    int64_t* h_rm = at<int64_t>(h_in, i_rm);
-    uint64_t* h_sel = at<uint64_t>(h_in, i_sel);
-    int32_t* h_node = at<int32_t>(h_in, i_node);
-    uint32_t* h_base = at<uint32_t>(h_in, i_base);
-    uint32_t* h_id = at<uint32_t>(h_in, i_id);
+    const auto ov_fc = h.work<int64_t>(P), ov_fm = h.work<int64_t>(P), part_key = h.work<int64_t>(part_rows);
+    const auto ov_node = h.work<int32_t>(P), part_idx = h.work<int32_t>(part_rows);
+    const auto ov_cnt = h.work<uint32_t>(2 * D); // ov_cnt D, failed D: one array, zeroed together
+    CU_TRY(h.reserve(s));
+    int64_t *h_rc = h.host(cpu), *h_rm = h.host(mem);
+    uint64_t* h_sel = h.host(sel);
+    int32_t* h_node = h.host(cand_node);
+    uint32_t *h_base = h.host(pod_base), *h_id = h.host(cand_id);
     for (uint64_t j = 0; j < D; j++) {
         h_node[j] = cand->node_idx[order[j]];
         h_base[j] = (uint32_t)off[order[j]];
@@ -1357,45 +1409,38 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidate
             memcpy(h_sel + (r0 + j) * W, pods->sel + p * W, 8 * W);
         }
     if (excl) {
-        uint32_t* h_excl = at<uint32_t>(h_in, i_excl);
-        memset(h_excl, 0, (size_t)s->Npad / 8);
+        uint32_t* h_excl = h.host(excluded);
+        memset(h_excl, 0, excluded.n * 4);
         for (uint64_t d = 0; d < D; d++) h_excl[cand->node_idx[d] >> 5] |= 1u << (cand->node_idx[d] & 31);
     }
     cudaStream_t st = s->stream;
-    uint8_t* d_in = s->d_in.as<uint8_t>();
-    uint8_t* d_work = s->d_work.as<uint8_t>();
-    uint8_t* d_out = s->d_out.as<uint8_t>();
-    CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
-    CU_TRY(cudaMemsetAsync(d_out, 0, out.size, st));
-    CU_TRY(cudaMemsetAsync(d_out + o_idx, 0xff, P * 4, st));
-    CU_TRY(cudaMemsetAsync(d_work + w_cnt, 0, D * 8, st));
+    CU_TRY(h.upload(st));
+    CU_TRY(cudaMemsetAsync(h.dev(score), 0, P * 8, st));
+    CU_TRY(cudaMemsetAsync(h.dev(idx), 0xff, P * 4, st));
+    CU_TRY(cudaMemsetAsync(h.dev(placed), 0, D * 4, st));
+    CU_TRY(cudaMemsetAsync(h.dev(ov_cnt), 0, D * 8, st));
     DrainArgs da;
-    da.cand_node = at<int32_t>(d_in, i_node);
-    da.pod_base = at<uint32_t>(d_in, i_base);
-    da.cand_id = at<uint32_t>(d_in, i_id);
-    da.excl = excl ? at<uint32_t>(d_in, i_excl) : nullptr;
-    da.ov_cnt = at<uint32_t>(d_work, w_cnt);
+    da.cand_node = h.dev(cand_node);
+    da.pod_base = h.dev(pod_base);
+    da.cand_id = h.dev(cand_id);
+    da.excl = excl ? h.dev(excluded) : nullptr;
+    da.ov_cnt = h.dev(ov_cnt);
     da.failed = da.ov_cnt + D;
-    da.ov_node = at<int32_t>(d_work, w_node);
-    da.ov_fc = at<int64_t>(d_work, w_fc);
-    da.ov_fm = at<int64_t>(d_work, w_fm);
-    da.out_idx = at<int32_t>(d_out, o_idx);
-    da.out_score = at<int64_t>(d_out, o_score);
-    da.placed = at<uint32_t>(d_out, o_placed);
-    const PartialView part{at<int64_t>(d_work, w_key), at<int32_t>(d_work, w_idx), nullptr};
+    da.ov_node = h.dev(ov_node);
+    da.ov_fc = h.dev(ov_fc);
+    da.ov_fm = h.dev(ov_fm);
+    da.out_idx = h.dev(idx);
+    da.out_score = h.dev(score);
+    da.placed = h.dev(placed);
+    const PartialView part{h.dev(part_key), h.dev(part_idx), nullptr};
     const NodeTable nt = node_table(s);
     for (uint64_t r = 0, r0 = 0; r < rounds; r0 += per_round[r], r++) {
-        const PodView pv{at<int64_t>(d_in, i_rc) + r0, at<int64_t>(d_in, i_rm) + r0, at<uint64_t>(d_in, i_sel) + r0 * W,
-                         per_round[r]};
+        const PodView pv{h.dev(cpu) + r0, h.dev(mem) + r0, h.dev(sel) + r0 * W, per_round[r]};
         const DirectGrid g = direct_grid(W, per_round[r], s->Npad, s->sms);
         cudaError_t e = launch_drain_round(nt, pv, da, policy, (uint32_t)r, part, g, st);
         if (e != cudaSuccess) return fail(KS_ERR_CUDA, "drain round %llu launch failed: %s", (unsigned long long)r, cudaGetErrorString(e));
     }
-    CU_TRY(cudaMemcpyAsync(h_out, d_out, out.size, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    if (P) memcpy(out_node_idx, h_out + o_idx, P * 4);
-    if (out_score && P) memcpy(out_score, h_out + o_score, P * 8);
-    memcpy(out_placed, h_out + o_placed, D * 4);
+    CU_TRY(h.finish(st));
     s->last_path = "drain";
     return KS_OK;
 }
@@ -1437,56 +1482,37 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const ks_node_templ
     }
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
-    // one block each way: in = [rc P | rm P | alloc_cpu T | alloc_mem T | free_cpu T | free_mem T | sel P*W | labels T*W |
-    // max_nodes T], results = [rows T | reasons P (when asked) | node T*P (when asked)]
-    BlockLayout in, res;
-    const size_t i_rc = in.take<int64_t>(P), i_rm = in.take<int64_t>(P), i_ac = in.take<int64_t>(T),
-                 i_am = in.take<int64_t>(T), i_fc = in.take<int64_t>(T), i_fm = in.take<int64_t>(T),
-                 i_sel = in.take<uint64_t>(P * W), i_lab = in.take<uint64_t>(T * W), i_max = in.take<uint32_t>(T);
-    const size_t o_rows = res.take<ks_scaleup_option>(T),
-                 o_why = res.take<ks_pod_reasons>(out_reasons ? P : 0, 16), // k_scaleup_reasons stores uint4
-                 o_node = res.take<int32_t>(out_node ? T * P : 0);
-    uint8_t* h_out = nullptr;
-    rc = stage_blocks(s, in.size, res.size, &h_out);
-    if (rc) return rc;
+    HostStaged h;
+    const auto cpu = h.in(pods->req_cpu, P), mem = h.in(pods->req_mem, P), alloc_cpu = h.in(t->alloc_cpu, T),
+               alloc_mem = h.in(t->alloc_mem, T), free_cpu = h.in(t->free_cpu, T), free_mem = h.in(t->free_mem, T);
+    const auto sel = h.in(pods->sel, P * W), labels = h.in(t->labels, T * W);
+    const auto max_nodes = h.in(t->max_nodes, T);
+    const auto rows = h.out(out, T);
+    const auto reasons = h.out(out_reasons, out_reasons ? P : 0, 16); // k_scaleup_reasons stores uint4
+    const auto node = h.out(out_node, out_node ? T * P : 0);
     const uint32_t slots = scaleup_slots((uint32_t)T, s->sms);
-    CU_TRY(s->d_work.ensure((size_t)slots * 2 * P * 4));
-    uint8_t* h_in = s->h_stage.as<uint8_t>();
-    memcpy(h_in + i_rc, pods->req_cpu, P * 8);
-    memcpy(h_in + i_rm, pods->req_mem, P * 8);
-    memcpy(h_in + i_ac, t->alloc_cpu, T * 8);
-    memcpy(h_in + i_am, t->alloc_mem, T * 8);
-    memcpy(h_in + i_fc, t->free_cpu, T * 8);
-    memcpy(h_in + i_fm, t->free_mem, T * 8);
-    memcpy(h_in + i_sel, pods->sel, P * 8 * W);
-    memcpy(h_in + i_lab, t->labels, T * 8 * W);
-    memcpy(h_in + i_max, t->max_nodes, T * 4);
+    const auto scratch = h.work<uint32_t>((uint64_t)slots * 2 * P);
+    CU_TRY(h.reserve(s));
     cudaStream_t st = s->stream;
-    uint8_t* d_in = s->d_in.as<uint8_t>();
-    uint8_t* d_out = s->d_out.as<uint8_t>();
-    CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
-    if (out_node) CU_TRY(cudaMemsetAsync(d_out + o_node, 0xff, T * P * 4, st));
-    const PodView pv{at<int64_t>(d_in, i_rc), at<int64_t>(d_in, i_rm), at<uint64_t>(d_in, i_sel), (uint32_t)P};
+    CU_TRY(h.upload(st));
+    if (out_node) CU_TRY(cudaMemsetAsync(h.dev(node), 0xff, T * P * 4, st));
+    const PodView pv{h.dev(cpu), h.dev(mem), h.dev(sel), (uint32_t)P};
     ScaleupArgs a;
     a.T = (uint32_t)T;
-    a.alloc_cpu = at<int64_t>(d_in, i_ac);
-    a.alloc_mem = at<int64_t>(d_in, i_am);
-    a.free_cpu = at<int64_t>(d_in, i_fc);
-    a.free_mem = at<int64_t>(d_in, i_fm);
-    a.labels = at<uint64_t>(d_in, i_lab);
-    a.max_nodes = at<uint32_t>(d_in, i_max);
-    a.rows = at<ks_scaleup_option>(d_out, o_rows);
-    a.out_node = out_node ? at<int32_t>(d_out, o_node) : nullptr;
-    a.reasons = out_reasons ? at<uint32_t>(d_out, o_why) : nullptr;
-    a.scratch = s->d_work.as<uint32_t>();
+    a.alloc_cpu = h.dev(alloc_cpu);
+    a.alloc_mem = h.dev(alloc_mem);
+    a.free_cpu = h.dev(free_cpu);
+    a.free_mem = h.dev(free_mem);
+    a.labels = h.dev(labels);
+    a.max_nodes = h.dev(max_nodes);
+    a.rows = h.dev(rows);
+    a.out_node = out_node ? h.dev(node) : nullptr;
+    a.reasons = out_reasons ? reinterpret_cast<uint32_t*>(h.dev(reasons)) : nullptr;
+    a.scratch = h.dev(scratch);
     a.slots = slots;
     cudaError_t e = launch_scaleup(pv, W, a, st);
     if (e != cudaSuccess) return fail(KS_ERR_CUDA, "scale-up launch failed: %s", cudaGetErrorString(e));
-    CU_TRY(cudaMemcpyAsync(h_out, d_out, res.size, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    memcpy(out, h_out + o_rows, T * sizeof(ks_scaleup_option));
-    if (out_reasons) memcpy(out_reasons, h_out + o_why, P * sizeof(ks_pod_reasons));
-    if (out_node) memcpy(out_node, h_out + o_node, T * P * 4);
+    CU_TRY(h.finish(st));
     // the best template: most pods placed, then the highest utilization, then the fewest nodes, then the lowest index
     int32_t best = -1;
     for (uint32_t i = 0; i < T; i++) {
@@ -1506,25 +1532,35 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const ks_node_templ
     return KS_OK;
 }
 
-int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* replicas, int policy, ks_replica_plan* out,
-                      int32_t* out_node, int64_t* out_score) {
+// The arguments ks_place_replicas and ks_place_replicas_spread share: host-space specs with requests that could be
+// committed, a replica count per spec and the plan rows, a policy, and the limits on specs and copies.  *total = the
+// copies asked for.
+static int check_replica_specs(ks_snapshot* s, const char* call, const ks_pods* specs, const uint32_t* replicas,
+                               const void* out, int policy, uint64_t* total) {
     int rc = check_pods(s, specs);
     if (rc) return rc;
-    if (specs->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_place_replicas takes host-space specs");
+    if (specs->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "%s takes host-space specs", call);
     const uint64_t T = specs->n;
     if (T && (!replicas || !out)) return fail(KS_ERR_INVALID, "NULL replicas or out");
     if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
     if (T > KS_REPLICAS_MAX_SPECS) return fail(KS_ERR_RANGE, "%llu specs (at most %u)", (unsigned long long)T, KS_REPLICAS_MAX_SPECS);
-    uint64_t total = 0;
+    *total = 0;
     for (uint64_t t = 0; t < T; t++) {
         if (replicas[t] > KS_REPLICAS_MAX)
             return fail(KS_ERR_RANGE, "spec %llu: %u replicas (at most %u)", (unsigned long long)t, replicas[t], KS_REPLICAS_MAX);
-        total += replicas[t];
+        *total += replicas[t];
     }
-    if (total > KS_REPLICAS_MAX_TOTAL)
-        return fail(KS_ERR_RANGE, "%llu replicas in one call (at most %u)", (unsigned long long)total, KS_REPLICAS_MAX_TOTAL);
-    rc = check_commit_requests(T, specs->req_cpu, specs->req_mem);
+    if (*total > KS_REPLICAS_MAX_TOTAL)
+        return fail(KS_ERR_RANGE, "%llu replicas in one call (at most %u)", (unsigned long long)*total, KS_REPLICAS_MAX_TOTAL);
+    return check_commit_requests(T, specs->req_cpu, specs->req_mem);
+}
+
+int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* replicas, int policy, ks_replica_plan* out,
+                      int32_t* out_node, int64_t* out_score) {
+    uint64_t total;
+    int rc = check_replica_specs(s, "ks_place_replicas", specs, replicas, out, policy, &total);
     if (rc) return rc;
+    const uint64_t T = specs->n;
     if (T == 0) return KS_OK;
     const bool copies = out_node || out_score;
     if (s->N == 0) { // no node: nothing fits, every copy is -1
@@ -1539,69 +1575,57 @@ int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* repl
     uint32_t n_chunks, chunk_len;
     replica_chunks(s->N, (uint32_t)T, s->sms, &n_chunks, &chunk_len);
     const uint64_t C = copies ? total : 0;
-    // in = [rc T | rm T | sel T*W | replicas T | offset T], results = [rows T | score C | node C],
-    // work = [search state T | chunk partials T*n_chunks | copy scores C | copy nodes C | sort indices 2C], and under
-    // KS_SCORE_LEAST_BALANCED [scores | copies placed] per node and k_rep_seq CTA
     uint32_t seq_ctas = 0, seq_block = 0;
     if (policy == KS_SCORE_LEAST_BALANCED) replica_seq_grid(s->N, (uint32_t)T, s->sms, &seq_ctas, &seq_block);
-    BlockLayout in, res, work;
-    const size_t i_rc = in.take<int64_t>(T), i_rm = in.take<int64_t>(T), i_sel = in.take<uint64_t>(T * W),
-                 i_rep = in.take<uint32_t>(T), i_off = in.take<uint64_t>(T);
-    const size_t o_rows = res.take<ks_replica_plan>(T), o_score = res.take<int64_t>(C), o_node = res.take<int32_t>(C);
-    const size_t w_spec = work.take<uint8_t>(replica_spec_bytes((uint32_t)T), 16),
-                 w_chunk = work.take<uint8_t>(replica_chunk_bytes((uint32_t)T, n_chunks), 16),
-                 w_score = work.take<int64_t>(C), w_node = work.take<int32_t>(C), w_sort = work.take<uint32_t>(2 * C);
-    const size_t w_seq_score = work.take<int64_t>((uint64_t)seq_ctas * s->N),
-                 w_seq_placed = work.take<uint32_t>((uint64_t)seq_ctas * s->N);
-    uint8_t* h_out = nullptr;
-    rc = stage_blocks(s, in.size, res.size, &h_out);
-    if (rc) return rc;
-    CU_TRY(s->d_work.ensure(work.size));
-    uint8_t* h_in = s->h_stage.as<uint8_t>();
-    memcpy(h_in + i_rc, specs->req_cpu, T * 8);
-    memcpy(h_in + i_rm, specs->req_mem, T * 8);
-    memcpy(h_in + i_sel, specs->sel, T * 8 * W);
-    memcpy(h_in + i_rep, replicas, T * 4);
-    uint64_t* h_off = at<uint64_t>(h_in, i_off);
-    for (uint64_t t = 0, o = 0; t < T; o += replicas[t], t++) h_off[t] = o;
+    HostStaged h;
+    const auto cpu = h.in(specs->req_cpu, T), mem = h.in(specs->req_mem, T);
+    const auto sel = h.in(specs->sel, T * W);
+    const auto reps = h.in(replicas, T);
+    const auto offset = h.in<uint64_t>(nullptr, T);
+    const auto rows = h.out(out, T);
+    const auto score = h.out(out_score, C);
+    const auto node = h.out(out_node, C);
+    const auto spec = h.work<unsigned char>(replica_spec_bytes((uint32_t)T), 16);
+    const auto chunk = h.work<unsigned char>(replica_chunk_bytes((uint32_t)T, n_chunks), 16);
+    const auto copy_score = h.work<int64_t>(C);
+    const auto copy_node = h.work<int32_t>(C);
+    const auto sort_buf = h.work<uint32_t>(2 * C);
+    // KS_SCORE_LEAST_BALANCED: [scores | copies placed] per node and k_rep_seq CTA
+    const auto seq_score = h.work<int64_t>((uint64_t)seq_ctas * s->N);
+    const auto seq_placed = h.work<uint32_t>((uint64_t)seq_ctas * s->N);
+    CU_TRY(h.reserve(s));
+    for (uint64_t t = 0, o = 0; t < T; o += replicas[t], t++) h.host(offset)[t] = o;
     cudaStream_t st = s->stream;
-    uint8_t* d_in = s->d_in.as<uint8_t>();
-    uint8_t* d_out = s->d_out.as<uint8_t>();
-    uint8_t* d_work = s->d_work.as<uint8_t>();
-    CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
+    CU_TRY(h.upload(st));
     if (copies) { // copies past `placed' stay -1 / 0
-        CU_TRY(cudaMemsetAsync(d_out + o_score, 0, C * 8, st));
-        CU_TRY(cudaMemsetAsync(d_out + o_node, 0xff, C * 4, st));
+        CU_TRY(cudaMemsetAsync(h.dev(score), 0, C * 8, st));
+        CU_TRY(cudaMemsetAsync(h.dev(node), 0xff, C * 4, st));
     }
     ReplicaArgs a;
     a.T = (uint32_t)T;
-    a.req_cpu = at<int64_t>(d_in, i_rc);
-    a.req_mem = at<int64_t>(d_in, i_rm);
-    a.sel = at<uint64_t>(d_in, i_sel);
-    a.replicas = at<uint32_t>(d_in, i_rep);
-    a.offset = at<uint64_t>(d_in, i_off);
-    a.rows = at<ks_replica_plan>(d_out, o_rows);
-    a.out_node = copies ? at<int32_t>(d_out, o_node) : nullptr;
-    a.out_score = copies ? at<int64_t>(d_out, o_score) : nullptr;
-    a.spec = at<RepSpec>(d_work, w_spec);
-    a.chunk = at<RepChunk>(d_work, w_chunk);
-    a.copy_node = copies ? at<int32_t>(d_work, w_node) : nullptr;
-    a.copy_score = copies ? at<int64_t>(d_work, w_score) : nullptr;
-    a.sort_buf = copies ? at<uint32_t>(d_work, w_sort) : nullptr;
+    a.req_cpu = h.dev(cpu);
+    a.req_mem = h.dev(mem);
+    a.sel = h.dev(sel);
+    a.replicas = h.dev(reps);
+    a.offset = h.dev(offset);
+    a.rows = h.dev(rows);
+    a.out_node = copies ? h.dev(node) : nullptr;
+    a.out_score = copies ? h.dev(score) : nullptr;
+    a.spec = reinterpret_cast<RepSpec*>(h.dev(spec));
+    a.chunk = reinterpret_cast<RepChunk*>(h.dev(chunk));
+    a.copy_node = copies ? h.dev(copy_node) : nullptr;
+    a.copy_score = copies ? h.dev(copy_score) : nullptr;
+    a.sort_buf = copies ? h.dev(sort_buf) : nullptr;
     a.n_chunks = n_chunks;
     a.chunk_len = chunk_len;
     ReplicaSeqArgs q;
-    q.score = seq_ctas ? at<int64_t>(d_work, w_seq_score) : nullptr;
-    q.placed = seq_ctas ? at<uint32_t>(d_work, w_seq_placed) : nullptr;
+    q.score = seq_ctas ? h.dev(seq_score) : nullptr;
+    q.placed = seq_ctas ? h.dev(seq_placed) : nullptr;
     q.ctas = seq_ctas;
     q.block = seq_block;
     cudaError_t e = launch_replicas(node_table(s), policy, a, q, st);
     if (e != cudaSuccess) return fail(KS_ERR_CUDA, "replica placement launch failed: %s", cudaGetErrorString(e));
-    CU_TRY(cudaMemcpyAsync(h_out, d_out, res.size, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    memcpy(out, h_out + o_rows, T * sizeof(ks_replica_plan));
-    if (out_node) memcpy(out_node, h_out + o_node, C * 4);
-    if (out_score) memcpy(out_score, h_out + o_score, C * 8);
+    CU_TRY(h.finish(st));
     s->last_path = "replicas";
     return KS_OK;
 }
@@ -1609,28 +1633,18 @@ int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* repl
 int ks_place_replicas_spread(ks_snapshot* s, const ks_pods* specs, const uint32_t* replicas, const ks_spread* spread,
                              int policy, ks_spread_plan* out, int32_t* out_node, int64_t* out_score,
                              uint32_t* out_domain_count) {
-    int rc = check_pods(s, specs);
+    uint64_t total;
+    int rc = check_replica_specs(s, "ks_place_replicas_spread", specs, replicas, out, policy, &total);
     if (rc) return rc;
-    if (specs->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_place_replicas_spread takes host-space specs");
     const uint64_t T = specs->n;
-    if (T && (!replicas || !out)) return fail(KS_ERR_INVALID, "NULL replicas or out");
     if (!spread || !spread->node_domain || !spread->max_skew) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
-    if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
     const uint32_t D = spread->n_domains, N = s->N;
     if (D == 0 || D > KS_SPREAD_MAX_DOMAINS) return fail(KS_ERR_RANGE, "%u domains (1 to %u)", D, KS_SPREAD_MAX_DOMAINS);
     for (uint32_t n = 0; n < N; n++)
         if (spread->node_domain[n] < -1 || spread->node_domain[n] >= (int64_t)D)
             return fail(KS_ERR_INVALID, "node %u: domain %d outside [-1, %u)", n, spread->node_domain[n], D);
-    if (T > KS_REPLICAS_MAX_SPECS) return fail(KS_ERR_RANGE, "%llu specs (at most %u)", (unsigned long long)T, KS_REPLICAS_MAX_SPECS);
-    uint64_t total = 0;
-    for (uint64_t t = 0; t < T; t++) {
-        if (replicas[t] > KS_REPLICAS_MAX)
-            return fail(KS_ERR_RANGE, "spec %llu: %u replicas (at most %u)", (unsigned long long)t, replicas[t], KS_REPLICAS_MAX);
+    for (uint64_t t = 0; t < T; t++)
         if (spread->max_skew[t] == 0) return fail(KS_ERR_RANGE, "spec %llu: max_skew 0 (at least 1)", (unsigned long long)t);
-        total += replicas[t];
-    }
-    if (total > KS_REPLICAS_MAX_TOTAL)
-        return fail(KS_ERR_RANGE, "%llu replicas in one call (at most %u)", (unsigned long long)total, KS_REPLICAS_MAX_TOTAL);
     const uint64_t TD = T * D;
     if ((spread->existing || out_domain_count) && TD > KS_SPREAD_MAX_COUNTS)
         return fail(KS_ERR_RANGE, "%llu specs x %u domains of counts (at most 2^26)", (unsigned long long)T, D);
@@ -1639,8 +1653,6 @@ int ks_place_replicas_spread(ks_snapshot* s, const ks_pods* specs, const uint32_
             if (spread->existing[i] > KS_SPREAD_MAX_EXISTING)
                 return fail(KS_ERR_RANGE, "spec %llu, domain %llu: %u existing pods (at most 2^24)",
                             (unsigned long long)(i / D), (unsigned long long)(i % D), spread->existing[i]);
-    rc = check_commit_requests(T, specs->req_cpu, specs->req_mem);
-    if (rc) return rc;
     if (T == 0) return KS_OK;
     const bool copies = out_node || out_score;
     if (N == 0) { // no node: no eligible domain, every copy is -1
@@ -1660,77 +1672,61 @@ int ks_place_replicas_spread(ks_snapshot* s, const ks_pods* specs, const uint32_
     uint32_t ctas;
     uint64_t seq_bytes;
     spread_seq_grid(N, D, (uint32_t)T, s->sms, &ctas, &seq_bytes);
-    // in = [rc T | rm T | sel T*W | replicas T | offset T | max_skew T | min_domains T | node_domain N | existing T*D],
-    // results = [rows T | score C | node C | counts T*D], work = [sort 2N | perm N | pos N | dstart D+1 | k_spread_seq]
-    BlockLayout in, res, work;
-    const size_t i_rc = in.take<int64_t>(T), i_rm = in.take<int64_t>(T), i_sel = in.take<uint64_t>(T * W),
-                 i_rep = in.take<uint32_t>(T), i_off = in.take<uint64_t>(T), i_skew = in.take<uint32_t>(T),
-                 i_mind = in.take<uint32_t>(spread->min_domains ? T : 0), i_dom = in.take<int32_t>(N),
-                 i_ex = in.take<uint32_t>(E);
-    const size_t o_rows = res.take<ks_spread_plan>(T), o_score = res.take<int64_t>(C), o_node = res.take<int32_t>(C),
-                 o_cnt = res.take<uint32_t>(K);
-    const size_t w_sort = work.take<uint32_t>(2ull * N), w_perm = work.take<uint32_t>(N), w_pos = work.take<uint32_t>(N),
-                 w_dstart = work.take<uint32_t>((uint64_t)D + 1), w_seq = work.take<uint8_t>(seq_bytes, 16);
-    uint8_t* h_out = nullptr;
-    rc = stage_blocks(s, in.size, res.size, &h_out);
-    if (rc) return rc;
-    CU_TRY(s->d_work.ensure(work.size));
-    uint8_t* h_in = s->h_stage.as<uint8_t>();
-    memcpy(h_in + i_rc, specs->req_cpu, T * 8);
-    memcpy(h_in + i_rm, specs->req_mem, T * 8);
-    memcpy(h_in + i_sel, specs->sel, T * 8 * W);
-    memcpy(h_in + i_rep, replicas, T * 4);
-    uint64_t* h_off = at<uint64_t>(h_in, i_off);
-    for (uint64_t t = 0, o = 0; t < T; o += replicas[t], t++) h_off[t] = o;
-    memcpy(h_in + i_skew, spread->max_skew, T * 4);
-    if (spread->min_domains) memcpy(h_in + i_mind, spread->min_domains, T * 4);
-    memcpy(h_in + i_dom, spread->node_domain, (size_t)N * 4);
-    if (E) memcpy(h_in + i_ex, spread->existing, E * 4);
+    HostStaged h;
+    const auto cpu = h.in(specs->req_cpu, T), mem = h.in(specs->req_mem, T);
+    const auto sel = h.in(specs->sel, T * W);
+    const auto reps = h.in(replicas, T);
+    const auto offset = h.in<uint64_t>(nullptr, T);
+    const auto max_skew = h.in(spread->max_skew, T);
+    const auto min_domains = h.in(spread->min_domains, spread->min_domains ? T : 0);
+    const auto node_domain = h.in(spread->node_domain, N);
+    const auto existing = h.in(spread->existing, E);
+    const auto rows = h.out(out, T);
+    const auto score = h.out(out_score, C);
+    const auto node = h.out(out_node, C);
+    const auto count = h.out(out_domain_count, K);
+    const auto sort_buf = h.work<uint32_t>(2ull * N), perm = h.work<uint32_t>(N), pos = h.work<uint32_t>(N),
+               dstart = h.work<uint32_t>((uint64_t)D + 1);
+    const auto seq = h.work<unsigned char>(seq_bytes, 16); // k_spread_seq's scratch
+    CU_TRY(h.reserve(s));
+    for (uint64_t t = 0, o = 0; t < T; o += replicas[t], t++) h.host(offset)[t] = o;
     cudaStream_t st = s->stream;
-    uint8_t* d_in = s->d_in.as<uint8_t>();
-    uint8_t* d_out = s->d_out.as<uint8_t>();
-    uint8_t* d_work = s->d_work.as<uint8_t>();
-    CU_TRY(cudaMemcpyAsync(d_in, h_in, in.size, cudaMemcpyHostToDevice, st));
+    CU_TRY(h.upload(st));
     if (copies) { // copies past `placed' stay -1 / 0
-        CU_TRY(cudaMemsetAsync(d_out + o_score, 0, C * 8, st));
-        CU_TRY(cudaMemsetAsync(d_out + o_node, 0xff, C * 4, st));
+        CU_TRY(cudaMemsetAsync(h.dev(score), 0, C * 8, st));
+        CU_TRY(cudaMemsetAsync(h.dev(node), 0xff, C * 4, st));
     }
     ReplicaArgs a{};
     a.T = (uint32_t)T;
-    a.req_cpu = at<int64_t>(d_in, i_rc);
-    a.req_mem = at<int64_t>(d_in, i_rm);
-    a.sel = at<uint64_t>(d_in, i_sel);
-    a.replicas = at<uint32_t>(d_in, i_rep);
-    a.offset = at<uint64_t>(d_in, i_off);
-    a.out_node = copies ? at<int32_t>(d_out, o_node) : nullptr;
-    a.out_score = copies ? at<int64_t>(d_out, o_score) : nullptr;
+    a.req_cpu = h.dev(cpu);
+    a.req_mem = h.dev(mem);
+    a.sel = h.dev(sel);
+    a.replicas = h.dev(reps);
+    a.offset = h.dev(offset);
+    a.out_node = copies ? h.dev(node) : nullptr;
+    a.out_score = copies ? h.dev(score) : nullptr;
     SpreadOrder o;
-    o.node_domain = at<int32_t>(d_in, i_dom);
-    o.sort_buf = at<uint32_t>(d_work, w_sort);
-    o.perm = at<uint32_t>(d_work, w_perm);
-    o.pos = at<uint32_t>(d_work, w_pos);
-    o.dstart = at<uint32_t>(d_work, w_dstart);
+    o.node_domain = h.dev(node_domain);
+    o.sort_buf = h.dev(sort_buf);
+    o.perm = h.dev(perm);
+    o.pos = h.dev(pos);
+    o.dstart = h.dev(dstart);
     SpreadArgs q;
     q.D = D;
     q.node_domain = o.node_domain;
     q.perm = o.perm;
     q.pos = o.pos;
     q.dstart = o.dstart;
-    q.max_skew = at<uint32_t>(d_in, i_skew);
-    q.min_domains = spread->min_domains ? at<uint32_t>(d_in, i_mind) : nullptr;
-    q.existing = E ? at<uint32_t>(d_in, i_ex) : nullptr;
-    q.rows = at<ks_spread_plan>(d_out, o_rows);
-    q.out_count = K ? at<uint32_t>(d_out, o_cnt) : nullptr;
-    q.scratch = at<unsigned char>(d_work, w_seq);
+    q.max_skew = h.dev(max_skew);
+    q.min_domains = spread->min_domains ? h.dev(min_domains) : nullptr;
+    q.existing = E ? h.dev(existing) : nullptr;
+    q.rows = h.dev(rows);
+    q.out_count = K ? h.dev(count) : nullptr;
+    q.scratch = h.dev(seq);
     q.ctas = ctas;
     cudaError_t e = launch_spread(node_table(s), policy, a, o, q, st);
     if (e != cudaSuccess) return fail(KS_ERR_CUDA, "spread placement launch failed: %s", cudaGetErrorString(e));
-    CU_TRY(cudaMemcpyAsync(h_out, d_out, res.size, cudaMemcpyDeviceToHost, st));
-    CU_TRY(cudaStreamSynchronize(st));
-    memcpy(out, h_out + o_rows, T * sizeof(ks_spread_plan));
-    if (out_node) memcpy(out_node, h_out + o_node, C * 4);
-    if (out_score) memcpy(out_score, h_out + o_score, C * 8);
-    if (K) memcpy(out_domain_count, h_out + o_cnt, K * 4);
+    CU_TRY(h.finish(st));
     s->last_path = "spread";
     return KS_OK;
 }

@@ -1,7 +1,7 @@
 """The staging set shared by every call that synchronises before it returns (-m gpu): the host-staged calls
-(ks_scaleup_estimate, ks_gang_bind, ks_drain_check, ks_stream_bind's device loop) and the host-space pods and results of
-select, explain, top-k, preempt, check_cells, sampling, commit_claims and apply_bind stage through one device
-in/work/out set per snapshot.  One snapshot runs a sequence of those calls that grows and shrinks the set, so each call
+(ks_scaleup_estimate, ks_gang_bind, ks_drain_check, ks_stream_bind's device loop, ks_place_replicas and
+ks_place_replicas_spread) and the host-space pods and results of select, explain, top-k, preempt, check_cells, sampling,
+commit_claims and apply_bind stage through one device in/work/out set per snapshot.  One snapshot runs a sequence of those calls that grows and shrinks the set, so each call
 finds contents a larger call of another kind left behind.  Every result, and free[] after the committing calls, must
 equal the same call on a fresh snapshot; cached-graph selects in between, with device-space buffers and with pinned host
 pods, outputs and mask (a graph that points into the shared set), keep returning the oracle's bindings."""
@@ -116,9 +116,16 @@ def test_shared_staging_across_call_kinds(ks, orc, cluster):
         run("preempt", lambda s: s.preempt(rc[:400], rm[:400], sel[:400], pprio[:400], bn, bc, bm, bprio, 16))
         run("stream 1 pod", lambda s: s.stream_bind(rc[:1], rm[:1], sel[:1]), commits=True)
         run("stream 1024 pods", lambda s: s.stream_bind(rc[:1024], rm[:1024], sel[:1024]), commits=True)
+        reps = rng.integers(0, 60, 200).astype(np.uint32)
+        run("place_replicas T=200 with copies", lambda s: s.place_replicas(rc[:200], rm[:200], sel[:200], reps, 1))
         small = _templates(rng, 8)
         run("scaleup T=8 P=100 without out_node",
             lambda s: s.scaleup_estimate(rc[:100], rm[:100], sel[:100], *small, want_nodes=False))
+        zone = (np.arange(N) % 4 - 1).astype(np.int32)  # -1 (no key), 0, 1, 2, ...
+        ex = rng.integers(0, 5, (100, 3)).astype(np.uint32)
+        run("place_replicas_spread T=100 with existing counts",
+            lambda s: s.place_replicas_spread(rc[:100], rm[:100], sel[:100], reps[:100], zone, 3, np.full(100, 2),
+                                              existing=ex))
         node, doff, pick = _candidates(rng, 900, 16)
         assert len(pick) > first
         run("drain D=900 policy 1", lambda s: s.drain_check(rc[pick], rm[pick], sel[pick], node, doff, 1))
