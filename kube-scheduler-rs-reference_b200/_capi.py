@@ -33,6 +33,14 @@ class KsError(RuntimeError):
         super().__init__(f"{where} failed with {code}: {msg}")
 
 
+def check(rc, where):
+    """Raise KsError for a negative return code of `where`; otherwise return the code (a count or a cell code for the
+    calls that return one)."""
+    if rc < 0:
+        raise KsError(rc, where)
+    return rc
+
+
 class ks_pods(C.Structure):
     _fields_ = [("n", C.c_uint64), ("req_cpu", C.c_void_p), ("req_mem", C.c_void_p), ("sel", C.c_void_p),
                 ("mem_space", C.c_int32)]
@@ -58,7 +66,11 @@ class ks_pod_reasons(C.Structure):
                 ("not_enough_resources", C.c_uint32), ("node_selector_mismatch", C.c_uint32)]
 
 
-def _proto(name, restype, *argtypes):
+def _proto(name, restype, *argtypes, optional=False):
+    """Declare lib.name.  optional: a library built from the host layer and a device stand-in (tests/native) may lack
+    the entry, which is then left undeclared."""
+    if optional and not hasattr(lib, name):
+        return None
     fn = getattr(lib, name)
     fn.restype = restype
     fn.argtypes = list(argtypes)
@@ -104,11 +116,9 @@ _proto("ks_measure_write_bandwidth", C.c_int, C.c_int, C.c_void_p, C.c_uint64, C
 _proto("ks_device_read", C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64)
 _proto("ks_select_sampling", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p,
        C.c_void_p, C.c_void_p, C.c_void_p)
-if hasattr(lib, "ks_explain"):  # a library built from the host layer and a device stand-in has no ks_explain
-    _proto("ks_explain", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_int32, C.c_void_p)
-if hasattr(lib, "ks_select_topk"):  # the same for ks_select_topk
-    _proto("ks_select_topk", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_int, C.c_uint32, C.c_void_p, C.c_void_p,
-           C.c_void_p, C.c_int32, C.c_void_p)
+_proto("ks_explain", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_int32, C.c_void_p, optional=True)
+_proto("ks_select_topk", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_int, C.c_uint32, C.c_void_p, C.c_void_p,
+       C.c_void_p, C.c_int32, C.c_void_p, optional=True)
 KS_TOPK_MAX = 32
 
 
@@ -123,13 +133,9 @@ class ks_preemption(C.Structure):
                 ("victim_priority_sum", C.c_int64)]
 
 
-# ks_preemption as a numpy record, for whole batches of rows
-PREEMPTION_DTYPE = np.dtype([("node_idx", np.int32), ("n_victims", np.uint32), ("candidates", np.uint32),
-                             ("feasible_cnt", np.uint32), ("max_victim_priority", np.int32), ("reserved", np.uint32),
-                             ("victim_priority_sum", np.int64)])
-if hasattr(lib, "ks_preempt"):  # the same for ks_preempt
-    _proto("ks_preempt", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.POINTER(ks_bound_pods), C.c_uint32,
-           C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p)
+PREEMPTION_DTYPE = np.dtype(ks_preemption)  # the same row as a numpy record, for whole batches of rows
+_proto("ks_preempt", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.POINTER(ks_bound_pods), C.c_uint32,
+       C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, optional=True)
 KS_PREEMPT_MAX_VICTIMS = 128
 
 
@@ -137,9 +143,8 @@ class ks_gangs(C.Structure):
     _fields_ = [("n", C.c_uint64), ("offset", C.c_void_p), ("min_member", C.c_void_p)]
 
 
-if hasattr(lib, "ks_gang_bind"):  # the same for ks_gang_bind
-    _proto("ks_gang_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.POINTER(ks_gangs), C.c_int, C.c_void_p,
-           C.c_void_p, C.c_void_p, C.c_void_p)
+_proto("ks_gang_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.POINTER(ks_gangs), C.c_int, C.c_void_p, C.c_void_p,
+       C.c_void_p, C.c_void_p, optional=True)
 KS_GANG_MAX_SIZE = 1024
 
 
@@ -147,9 +152,8 @@ class ks_drain_candidates(C.Structure):
     _fields_ = [("n", C.c_uint64), ("node_idx", C.c_void_p), ("offset", C.c_void_p)]
 
 
-if hasattr(lib, "ks_drain_check"):  # the same for ks_drain_check
-    _proto("ks_drain_check", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.POINTER(ks_drain_candidates), C.c_int,
-           C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p)
+_proto("ks_drain_check", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.POINTER(ks_drain_candidates), C.c_int, C.c_uint32,
+       C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
 KS_DRAIN_MAX_PODS = 1024
 KS_DRAIN_EXCLUDE_CANDIDATES = 1
 
@@ -164,12 +168,9 @@ class ks_scaleup_option(C.Structure):
                 ("used_cpu", C.c_int64), ("used_mem", C.c_int64)]
 
 
-# the same row as a numpy record
-SCALEUP_OPTION_DTYPE = np.dtype([("nodes", np.uint32), ("placed", np.uint32), ("eligible", np.uint32),
-                                 ("utilization", np.int32), ("used_cpu", np.int64), ("used_mem", np.int64)])
-if hasattr(lib, "ks_scaleup_estimate"):  # the same for ks_scaleup_estimate
-    _proto("ks_scaleup_estimate", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.POINTER(ks_node_templates), C.c_void_p,
-           C.c_void_p, C.c_void_p, C.c_void_p)
+SCALEUP_OPTION_DTYPE = np.dtype(ks_scaleup_option)  # the same row as a numpy record
+_proto("ks_scaleup_estimate", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.POINTER(ks_node_templates), C.c_void_p,
+       C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
 KS_SCALEUP_MAX_NODES = 1024
 KS_SCALEUP_MAX_PODS = 65536
 KS_SCALEUP_MAX_TEMPLATES = 4096
@@ -180,12 +181,9 @@ class ks_replica_plan(C.Structure):
                 ("max_per_node", C.c_uint32), ("last_score", C.c_int64)]
 
 
-# the same row as a numpy record
-REPLICA_PLAN_DTYPE = np.dtype([("capacity", np.uint64), ("placed", np.uint32), ("nodes", np.uint32),
-                               ("feasible_cnt", np.uint32), ("max_per_node", np.uint32), ("last_score", np.int64)])
-if hasattr(lib, "ks_place_replicas"):  # the same for ks_place_replicas
-    _proto("ks_place_replicas", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
-           C.c_void_p)
+REPLICA_PLAN_DTYPE = np.dtype(ks_replica_plan)  # the same row as a numpy record
+_proto("ks_place_replicas", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+       C.c_void_p, optional=True)
 KS_REPLICAS_MAX_SPECS = 4096
 KS_REPLICAS_MAX = 65536
 KS_REPLICAS_MAX_TOTAL = 1 << 24
@@ -202,13 +200,9 @@ class ks_spread_plan(C.Structure):
                 ("last_score", C.c_int64)]
 
 
-# the same row as a numpy record
-SPREAD_PLAN_DTYPE = np.dtype([("placed", np.uint32), ("nodes", np.uint32), ("max_per_node", np.uint32),
-                              ("eligible_domains", np.uint32), ("min_count", np.uint32), ("blocked_domain", np.int32),
-                              ("last_score", np.int64)])
-if hasattr(lib, "ks_place_replicas_spread"):  # the same for ks_place_replicas_spread
-    _proto("ks_place_replicas_spread", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.POINTER(ks_spread),
-           C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p)
+SPREAD_PLAN_DTYPE = np.dtype(ks_spread_plan)  # the same row as a numpy record
+_proto("ks_place_replicas_spread", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.POINTER(ks_spread), C.c_int,
+       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
 KS_SPREAD_MAX_DOMAINS = 1 << 20
 KS_SPREAD_MAX_EXISTING = 1 << 24
 KS_SPREAD_MAX_COUNTS = 1 << 26
@@ -238,9 +232,8 @@ def declared_symbols():
 def measure_write_bandwidth(device, dev_ptr, nbytes, iters=4):
     """GB/s of a store-only fill over a device buffer (its contents are overwritten)."""
     out = C.c_double()
-    rc = lib.ks_measure_write_bandwidth(int(device), C.c_void_p(int(dev_ptr)), int(nbytes), int(iters), C.byref(out))
-    if rc != KS_OK:
-        raise KsError(rc, "ks_measure_write_bandwidth")
+    check(lib.ks_measure_write_bandwidth(int(device), C.c_void_p(int(dev_ptr)), int(nbytes), int(iters), C.byref(out)),
+          "ks_measure_write_bandwidth")
     return float(out.value)
 
 

@@ -276,7 +276,7 @@ struct ksh_context {
     std::vector<int64_t> tmp_cpu, tmp_mem;
     std::vector<uint64_t> tmp_hash;
     std::vector<uint32_t> tmp_len;
-    std::vector<int64_t> pk_cpu, pk_mem; // packed form of the last ksh_select_nodes batch
+    std::vector<int64_t> pk_cpu, pk_mem; // packed form of the last batch a device call packed (pack_batch)
     std::vector<uint64_t> pk_sel;
     bool dirty = true; // device snapshot must be re-uploaded
     // one lock per context: every ksh_* entry that takes a context holds it for the whole call (entries call each other)
@@ -642,6 +642,13 @@ static void bound_push(ksh_context* c, const ks_pod_obj* pod, uint64_t h, size_t
     c->btab.slots[(size_t)free_slot] = btab_word(h, pos);
 }
 
+// bound_push for a pod whose key is not hashed yet
+static void bound_push(ksh_context* c, const ks_pod_obj* pod, int32_t node, int64_t cpu, int64_t mem) {
+    size_t lns, lname;
+    const uint64_t h = pod_key_hash(pod, &lns, &lname);
+    bound_push(c, pod, h, lns, lname, node, cpu, mem);
+}
+
 static void bound_erase(ksh_context* c, size_t pos) { // swap-remove
     const size_t last = c->bnode.size() - 1;
     c->live_key_bytes -= c->blen[pos];
@@ -685,8 +692,11 @@ static void bound_clear(ksh_context* c) {
     c->live_key_bytes = 0;
 }
 
+static const char* const NO_SNAPSHOT =
+    "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host";
+
 static int upload(ksh_context* c) {
-    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    if (!c->snap) return fail(KS_ERR_NO_DEVICE, NO_SNAPSHOT);
     if (!c->dirty) return KS_OK;
     std::vector<uint64_t> lab((size_t)c->N * c->W, 0);
     fill_label_words(c, lab.data());
@@ -808,6 +818,47 @@ static void pack_selectors(const ksh_context* c, const ks_pod_obj* pods, uint64_
         }
     });
 }
+
+// ---- calls that need the device ----
+// Each such call makes this check where it first needs the device: a packing-only context has no snapshot, and a library built
+// with a device stand-in (tests/native) may lack the optional entry.
+template <class F>
+static int device_ready(const ksh_context* c, F* entry, const char* name) {
+    if (!c->snap) return fail(KS_ERR_NO_DEVICE, NO_SNAPSHOT);
+    if (!entry) return fail(KS_ERR_NO_DEVICE, std::string("this library has no ") + name);
+    return KS_OK;
+}
+
+// Packs a batch into the context's pk_* set (kept between calls: fresh pages cost more than the packing), uploads the snapshot,
+// and describes the packed batch in *kp.  *kp stays valid until the next pack; the context lock held for the whole call keeps it so.
+static int pack_batch(ksh_context* c, const ks_pod_obj* pods, uint64_t n, ks_pods* kp) {
+    c->pk_cpu.resize(n);
+    c->pk_mem.resize(n);
+    PackScratch ps;
+    int rc = pack_scan(c, pods, n, c->pk_cpu.data(), c->pk_mem.data(), ps);
+    if (rc) return rc;
+    rc = grow_dictionary(c, ps, pods, n);
+    if (rc) return rc;
+    c->pk_sel.resize((size_t)n * c->W);
+    pack_selectors(c, pods, n, ps, c->pk_sel.data(), c->W);
+    *kp = ks_pods{n, c->pk_cpu.data(), c->pk_mem.data(), c->pk_sel.data(), KS_MEM_HOST};
+    return upload(c);
+}
+
+// A string-list output: entries back to back in buf[0, cap), each NUL-terminated.  An entry that does not fit is skipped (offset -1),
+// and a later, shorter entry may still fit.
+struct StringList {
+    char* buf;
+    size_t cap;
+    size_t used = 0;
+    // s[0, len) holds the entry with its terminating NUL(s); returns its offset, or -1 if it does not fit
+    int64_t append(const char* s, size_t len) {
+        if (used + len > cap) return -1;
+        std::memcpy(buf + used, s, len);
+        used += len;
+        return (int64_t)(used - len);
+    }
+};
 
 extern "C" {
 
@@ -1033,9 +1084,7 @@ int ksh_context_pod_bound(ksh_context* c, const ks_pod_obj* pod) try {
     std::string err;
     const int rc = total_pod_resources(pod, &cpu, &mem, &err);
     if (rc) return fail(rc, err);
-    size_t lns, lname;
-    const uint64_t h = pod_key_hash(pod, &lns, &lname);
-    bound_push(c, pod, h, lns, lname, node, cpu, mem); // an update of a pod already known replaces its row
+    bound_push(c, pod, node, cpu, mem); // an update of a pod already known replaces its row
     gc_bound_keys(c);
     c->dirty = true;
     return KS_OK;
@@ -1134,29 +1183,14 @@ int ksh_pack_pods(ksh_context* c, const ks_pod_obj* pods, uint64_t n, int64_t* r
 }
 KSH_CATCH
 
-static int pack_and_upload(ksh_context* c, const ks_pod_obj* pods, uint64_t n, std::vector<int64_t>& rc_, std::vector<int64_t>& rm_,
-                           std::vector<uint64_t>& sel) {
-    rc_.resize(n);
-    rm_.resize(n);
-    PackScratch ps;
-    int rc = pack_scan(c, pods, n, rc_.data(), rm_.data(), ps);
-    if (rc) return rc;
-    rc = grow_dictionary(c, ps, pods, n);
-    if (rc) return rc;
-    sel.resize((size_t)n * c->W);
-    pack_selectors(c, pods, n, ps, sel.data(), c->W);
-    return upload(c);
-}
-
 int ksh_check_node_validity(ksh_context* c, const ks_pod_obj* pod, uint32_t node_idx) try {
     if (!c || !pod) return fail(KS_ERR_INVALID, "NULL argument");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
     if (node_idx >= c->N) return fail(KS_ERR_INVALID, "node index out of range");
-    std::vector<int64_t> rc_, rm_;
-    std::vector<uint64_t> sel;
-    int rc = pack_and_upload(c, pod, 1, rc_, rm_, sel);
+    ks_pods kp;
+    const int rc = pack_batch(c, pod, 1, &kp);
     if (rc) return rc;
-    return ks_check_cell(c->snap, rc_[0], rm_[0], sel.data(), node_idx);
+    return ks_check_cell(c->snap, kp.req_cpu[0], kp.req_mem[0], kp.sel, node_idx);
 }
 KSH_CATCH
 
@@ -1165,12 +1199,9 @@ int ksh_select_nodes(ksh_context* c, const ks_pod_obj* pods, uint64_t n, int pol
     if (!c || (n && !pods)) return fail(KS_ERR_INVALID, "NULL argument");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
     if (n == 0) return KS_OK;
-    // packed form of the batch: kept in the context between calls (24 bytes per pod; fresh pages cost more than the packing)
-    std::vector<int64_t>&rc_ = c->pk_cpu, &rm_ = c->pk_mem;
-    std::vector<uint64_t>& sel = c->pk_sel;
-    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel);
+    ks_pods kp;
+    const int rc = pack_batch(c, pods, n, &kp);
     if (rc) return rc;
-    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     ks_bindings kb{out_node_idx, out_score, out_cnt, KS_MEM_HOST, nullptr, 0, KS_MEM_HOST, nullptr, nullptr};
     return ks_select(c->snap, &kp, policy, KS_SELECT_AUTO, &kb, nullptr);
 }
@@ -1180,16 +1211,14 @@ int ksh_rank_nodes(ksh_context* c, const ks_pod_obj* pods, uint64_t n, int polic
                    int64_t* out_score, uint32_t* out_cnt) try {
     if (!c || (n && !pods)) return fail(KS_ERR_INVALID, "NULL argument");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    int rc = device_ready(c, ks_select_topk, "ks_select_topk");
+    if (rc) return rc;
     if (k == 0 || k > KS_TOPK_MAX) return fail(KS_ERR_RANGE, "k must be in [1, " + std::to_string(KS_TOPK_MAX) + "]");
     if (n == 0) return KS_OK;
     if (!out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
-    std::vector<int64_t>&rc_ = c->pk_cpu, &rm_ = c->pk_mem; // the same packed batch buffers as ksh_select_nodes
-    std::vector<uint64_t>& sel = c->pk_sel;
-    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel);
+    ks_pods kp;
+    rc = pack_batch(c, pods, n, &kp);
     if (rc) return rc;
-    if (!ks_select_topk) return fail(KS_ERR_NO_DEVICE, "this library has no ks_select_topk");
-    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     return ks_select_topk(c->snap, &kp, policy, k, out_node_idx, out_score, out_cnt, KS_MEM_HOST, nullptr);
 }
 KSH_CATCH
@@ -1200,11 +1229,9 @@ int ksh_select_node_for_pod(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     if (!c || (n && !pods)) return fail(KS_ERR_INVALID, "NULL argument");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
     if (n == 0) return KS_OK;
-    std::vector<int64_t> rc_, rm_;
-    std::vector<uint64_t> sel;
-    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel);
+    ks_pods kp;
+    const int rc = pack_batch(c, pods, n, &kp);
     if (rc) return rc;
-    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     return ks_select_sampling(c->snap, &kp, attempts, seed, first_pod_index, out_node_idx, out_attempts, out_draw_node,
                               out_draw_code);
 }
@@ -1267,16 +1294,35 @@ int ksh_reconcile(ksh_context* c, const ks_pod_obj* pod, int policy, int32_t* no
         c->dirty = true; // the device may or may not carry the bind: re-upload from the host truth next time
         return rc;
     }
-    {
-        size_t lns, lname;
-        const uint64_t h = pod_key_hash(pod, &lns, &lname);
-        bound_push(c, pod, h, lns, lname, idx, cpu, mem);
-    }
+    bound_push(c, pod, idx, cpu, mem);
     *node_idx = idx;
     if (json && cap) std::snprintf(json, cap, "%s", binding_body(c, pod, (uint32_t)idx).c_str());
     return KSH_RECONCILE_OK;
 }
 KSH_CATCH
+
+// reconcile()'s outcome for a pod of a batch before the device: a bound pod is done (src/main.rs:74-76), a pod without namespace
+// or name cannot get a Binding (reference: unwrap panic, src/main.rs:80), and any other goes to the device and stays
+// NO_NODE_FOUND until it binds (src/main.rs:116-118), with an earlier binding of it by this context dropped first.
+static int32_t reconcile_status(ksh_context* c, const ks_pod_obj* pod) {
+    if (ksh_is_pod_bound(pod)) return KSH_RECONCILE_OK;
+    if (!pod->ns || !pod->name) return KSH_RECONCILE_BINDING_OBJECT_FAILED;
+    release_earlier_binding(c, pod);
+    return KSH_RECONCILE_NO_NODE_FOUND;
+}
+
+// The host side of a bind the device committed: the row the next LIST would show, the pod's status and node, and its Binding
+// body in the string list (when body_off is given).
+static void commit_bind(ksh_context* c, const ks_pod_obj* pod, int32_t node, int64_t cpu, int64_t mem, int32_t* status,
+                        int32_t* node_idx, StringList& bodies, int64_t* body_off) {
+    bound_push(c, pod, node, cpu, mem);
+    *status = KSH_RECONCILE_OK;
+    *node_idx = node;
+    if (body_off) {
+        const std::string body = binding_body(c, pod, (uint32_t)node);
+        *body_off = bodies.append(body.c_str(), body.size() + 1);
+    }
+}
 
 // reconcile() for a drained queue: one pack, one micro-batch loop on the device (select -> claims resolved in array order ->
 // losers re-selected against what is left), then the host-side commit of every bind (what the next LIST would show)
@@ -1290,46 +1336,27 @@ int ksh_reconcile_batch(ksh_context* c, const ks_pod_obj* pods, uint64_t n, int 
     for (uint64_t i = 0; i < n; i++) {
         out_node_idx[i] = -1;
         if (out_json_off) out_json_off[i] = -1;
-        if (ksh_is_pod_bound(&pods[i])) {
-            out_status[i] = KSH_RECONCILE_OK; // src/main.rs:74-76
-        } else if (!pods[i].ns || !pods[i].name) {
-            out_status[i] = KSH_RECONCILE_BINDING_OBJECT_FAILED; // reference: unwrap panic, src/main.rs:80
-        } else {
-            out_status[i] = KSH_RECONCILE_NO_NODE_FOUND; // until bound below (src/main.rs:116-118)
-            release_earlier_binding(c, &pods[i]);
-            todo.push_back(i);
-            sub.push_back(pods[i]);
-        }
+        out_status[i] = reconcile_status(c, &pods[i]);
+        if (out_status[i] != KSH_RECONCILE_NO_NODE_FOUND) continue;
+        todo.push_back(i);
+        sub.push_back(pods[i]);
     }
     if (todo.empty()) return KS_OK;
-    std::vector<int64_t> rc_, rm_;
-    std::vector<uint64_t> sel;
-    int rc = pack_and_upload(c, sub.data(), sub.size(), rc_, rm_, sel);
+    ks_pods kp;
+    int rc = pack_batch(c, sub.data(), sub.size(), &kp);
     if (rc) return rc;
     std::vector<int32_t> idx(sub.size(), -1);
-    ks_pods kp{sub.size(), rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     rc = ks_stream_bind(c->snap, &kp, policy, idx.data(), nullptr, out_rounds); // commits capacity on the device
     if (rc) {
         c->dirty = true; // some rounds may have committed claims on the device: the host list is the truth
         return rc;
     }
-    size_t used = 0;
+    StringList bodies{json, cap};
     for (size_t k = 0; k < todo.size(); k++) {
-        if (idx[k] < 0) continue;
         const uint64_t i = todo[k];
-        size_t lns, lname;
-        const uint64_t h = pod_key_hash(&pods[i], &lns, &lname);
-        bound_push(c, &pods[i], h, lns, lname, idx[k], rc_[k], rm_[k]);
-        out_status[i] = KSH_RECONCILE_OK;
-        out_node_idx[i] = idx[k];
-        if (json && out_json_off) {
-            const std::string body = binding_body(c, &pods[i], (uint32_t)idx[k]);
-            if (used + body.size() + 1 <= cap) { // bodies back to back, each NUL-terminated; -1 = did not fit
-                std::memcpy(json + used, body.c_str(), body.size() + 1);
-                out_json_off[i] = (int64_t)used;
-                used += body.size() + 1;
-            }
-        }
+        if (idx[k] >= 0)
+            commit_bind(c, &pods[i], idx[k], kp.req_cpu[k], kp.req_mem[k], &out_status[i], &out_node_idx[i], bodies,
+                        json && out_json_off ? &out_json_off[i] : nullptr);
     }
     return KS_OK;
 }
@@ -1352,29 +1379,22 @@ int ksh_reconcile_gangs(ksh_context* c, const ks_pod_obj* pods, uint64_t n, cons
     }
     if (group_offset[n_groups] != n) return fail(KS_ERR_INVALID, "group_offset[n_groups] must be n_pods");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
-    if (!ks_gang_bind) return fail(KS_ERR_NO_DEVICE, "this library has no ks_gang_bind");
+    int rc = device_ready(c, ks_gang_bind, "ks_gang_bind");
+    if (rc) return rc;
     std::vector<uint64_t> todo, sub_off{0}, sub_group; // the pods that go to the device; sub-group k is group sub_group[k]
     std::vector<uint32_t> sub_min;
     std::vector<ks_pod_obj> sub;
     if (out_placed)
         for (uint64_t g = 0; g < n_groups; g++) out_placed[g] = 0;
     for (uint64_t g = 0; g < n_groups; g++) {
-        uint32_t bound = 0;
+        uint32_t bound = 0; // running members of the group
         const size_t first = todo.size();
         for (uint64_t i = group_offset[g]; i < group_offset[g + 1]; i++) {
             out_node_idx[i] = -1;
             if (out_json_off) out_json_off[i] = -1;
-            if (ksh_is_pod_bound(&pods[i])) {
-                out_status[i] = KSH_RECONCILE_OK; // src/main.rs:74-76; a running member of the group
-                bound++;
-            } else if (!pods[i].ns || !pods[i].name) {
-                out_status[i] = KSH_RECONCILE_BINDING_OBJECT_FAILED; // reference: unwrap panic, src/main.rs:80
-            } else {
-                out_status[i] = KSH_RECONCILE_NO_NODE_FOUND; // until bound below (src/main.rs:116-118)
-                release_earlier_binding(c, &pods[i]); // it came back unbound: whatever its group does, drop the old charge
-                todo.push_back(i);
-            }
+            out_status[i] = reconcile_status(c, &pods[i]); // an earlier binding is dropped whatever the group does
+            if (out_status[i] == KSH_RECONCILE_OK) bound++;
+            if (out_status[i] == KSH_RECONCILE_NO_NODE_FOUND) todo.push_back(i);
         }
         const uint32_t need = min_member[g] > bound ? min_member[g] - bound : 0;
         if (todo.size() == first) continue;
@@ -1389,43 +1409,28 @@ int ksh_reconcile_gangs(ksh_context* c, const ks_pod_obj* pods, uint64_t n, cons
         sub_min.push_back(need);
     }
     if (todo.empty()) return KS_OK;
-    std::vector<int64_t> rc_, rm_;
-    std::vector<uint64_t> sel;
-    int rc = pack_and_upload(c, sub.data(), sub.size(), rc_, rm_, sel);
+    ks_pods kp;
+    rc = pack_batch(c, sub.data(), sub.size(), &kp);
     if (rc) return rc;
     std::vector<int32_t> idx(sub.size(), -1);
     std::vector<uint32_t> placed(sub_group.size());
-    ks_pods kp{sub.size(), rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     ks_gangs kg{sub_group.size(), sub_off.data(), sub_min.data()};
     rc = ks_gang_bind(c->snap, &kp, &kg, policy, idx.data(), nullptr, placed.data(), nullptr); // commits on the device
     if (rc) {
         c->dirty = true; // the device may carry part of the call: the host list is the truth
         return rc;
     }
-    size_t used = 0;
+    StringList bodies{json, cap};
     for (size_t k = 0; k < sub_group.size(); k++) {
         if (out_placed) out_placed[sub_group[k]] = placed[k];
         const bool commit = placed[k] >= sub_min[k];
         for (uint64_t j = sub_off[k]; j < sub_off[k + 1]; j++) {
             const uint64_t i = todo[j];
-            if (!commit) {
+            if (!commit)
                 out_status[i] = KSH_RECONCILE_GANG_UNSATISFIED;
-                continue;
-            }
-            if (idx[j] < 0) continue; // NoNodeFound
-            size_t lns, lname;
-            const uint64_t h = pod_key_hash(&pods[i], &lns, &lname);
-            bound_push(c, &pods[i], h, lns, lname, idx[j], rc_[j], rm_[j]);
-            out_status[i] = KSH_RECONCILE_OK;
-            out_node_idx[i] = idx[j];
-            if (json && out_json_off) {
-                const std::string body = binding_body(c, &pods[i], (uint32_t)idx[j]);
-                if (used + body.size() + 1 <= cap) { // bodies back to back, each NUL-terminated; -1 = did not fit
-                    std::memcpy(json + used, body.c_str(), body.size() + 1);
-                    out_json_off[i] = (int64_t)used;
-                    used += body.size() + 1;
-                }
-            }
+            else if (idx[j] >= 0) // else NoNodeFound
+                commit_bind(c, &pods[i], idx[j], kp.req_cpu[j], kp.req_mem[j], &out_status[i], &out_node_idx[i], bodies,
+                            json && out_json_off ? &out_json_off[i] : nullptr);
         }
     }
     return KS_OK;
@@ -1459,29 +1464,24 @@ int ksh_explain_pods(ksh_context* c, const ks_pod_obj* pods, uint64_t n, ks_pod_
                      int64_t* out_msg_off) try {
     if (!c || (n && (!pods || !out))) return fail(KS_ERR_INVALID, "NULL argument");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    int rc = device_ready(c, ks_explain, "ks_explain");
+    if (rc) return rc;
     if (out_msg_off)
         for (uint64_t i = 0; i < n; i++) out_msg_off[i] = -1;
     if (n == 0) return KS_OK;
-    std::vector<int64_t> rc_, rm_;
-    std::vector<uint64_t> sel;
-    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel);
+    ks_pods kp;
+    rc = pack_batch(c, pods, n, &kp);
     if (rc) return rc;
-    if (!ks_explain) return fail(KS_ERR_NO_DEVICE, "this library has no ks_explain");
-    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     rc = ks_explain(c->snap, &kp, out, KS_MEM_HOST, nullptr);
     if (rc) return rc;
     if (!messages || !out_msg_off) return KS_OK;
-    const uint32_t N = c->N; // what pack_and_upload just gave the snapshot
-    size_t used = 0;
+    const uint32_t N = c->N; // what pack_batch just gave the snapshot
+    StringList list{messages, cap};
     char msg[256]; // the longest message (three 10-digit counts) is under 200 bytes
     for (uint64_t i = 0; i < n; i++) {
         if ((uint64_t)out[i].not_enough_resources + out[i].node_selector_mismatch < N) continue; // a node is feasible
         const int len = ksh_format_unschedulable(N, &out[i], msg, sizeof(msg));
-        if (used + (size_t)len + 1 > cap) continue; // -1 = did not fit
-        std::memcpy(messages + used, msg, (size_t)len + 1);
-        out_msg_off[i] = (int64_t)used;
-        used += (size_t)len + 1;
+        out_msg_off[i] = list.append(msg, (size_t)len + 1);
     }
     return KS_OK;
 }
@@ -1507,38 +1507,33 @@ int ksh_preempt_pods(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const i
     if (max_victims == 0 || max_victims > KS_PREEMPT_MAX_VICTIMS)
         return fail(KS_ERR_RANGE, "max_victims must be in [1, " + std::to_string(KS_PREEMPT_MAX_VICTIMS) + "]");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
+    int rc = device_ready(c, ks_preempt, "ks_preempt");
+    if (rc) return rc;
     if (out_victim_off)
         for (uint64_t i = 0; i < n; i++) out_victim_off[i] = -1;
     if (n == 0) return KS_OK;
-    std::vector<int64_t>&rc_ = c->pk_cpu, &rm_ = c->pk_mem; // the same packed batch buffers as ksh_select_nodes
-    std::vector<uint64_t>& sel = c->pk_sel;
-    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel); // after this the device's free[] comes from the bound rows below
+    ks_pods kp;
+    rc = pack_batch(c, pods, n, &kp); // after this the device's free[] comes from the bound rows below
     if (rc) return rc;
-    if (!ks_preempt) return fail(KS_ERR_NO_DEVICE, "this library has no ks_preempt");
     const size_t B = c->bnode.size();
     std::vector<int32_t> prio(B);
     for (size_t b = 0; b < B; b++) prio[b] = c->blen[b] ? c->bprio[b] : INT32_MAX; // anonymous: cannot be evicted
     std::vector<int32_t> vic((size_t)n * max_victims);
-    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     ks_bound_pods kb{B, c->bnode.data(), c->bcpu.data(), c->bmem.data(), prio.data()};
     rc = ks_preempt(c->snap, &kp, pod_priority, &kb, max_victims, out, vic.data(), KS_MEM_HOST, nullptr);
     if (rc) return rc;
     if (!victims || !out_victim_off) return KS_OK;
-    size_t used = 0;
+    StringList list{victims, cap};
+    std::string keys;
     for (uint64_t i = 0; i < n; i++) {
         if (out[i].node_idx < 0) continue;
-        const int32_t* v = &vic[(size_t)i * max_victims];
-        size_t need = 0;
-        for (uint32_t j = 0; j < out[i].n_victims; j++) need += c->blen[(size_t)v[j]] + 1;
-        if (used + need > cap) continue; // -1 = did not fit
-        out_victim_off[i] = (int64_t)used;
+        keys.clear();
         for (uint32_t j = 0; j < out[i].n_victims; j++) { // "namespace/name", NUL-terminated, in visit order
-            const size_t b = (size_t)v[j];
-            std::memcpy(victims + used, c->bkeys.data() + c->boff[b], c->blen[b]);
-            used += c->blen[b];
-            victims[used++] = '\0';
+            const size_t b = (size_t)vic[(size_t)i * max_victims + j];
+            keys.append(c->bkeys.data() + c->boff[b], c->blen[b]);
+            keys.push_back('\0');
         }
+        out_victim_off[i] = list.append(keys.data(), keys.size());
     }
     return KS_OK;
 }
@@ -1565,13 +1560,11 @@ int ksh_drain_nodes(ksh_context* c, const char* const* node_names, uint64_t n, c
                                                 ") has spec.nodeName \"" + (ksh_is_pod_bound(&pods[i]) ? pods[i].node_name : "") +
                                                 "\", not its candidate's node \"" + name + "\"");
     }
-    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
-    if (!ks_drain_check) return fail(KS_ERR_NO_DEVICE, "this library has no ks_drain_check");
-    std::vector<int64_t>&rc_ = c->pk_cpu, &rm_ = c->pk_mem; // the same packed batch buffers as ksh_select_nodes
-    std::vector<uint64_t>& sel = c->pk_sel;
-    int rc = pack_and_upload(c, pods, P, rc_, rm_, sel);
+    int rc = device_ready(c, ks_drain_check, "ks_drain_check");
     if (rc) return rc;
-    ks_pods kp{P, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
+    ks_pods kp;
+    rc = pack_batch(c, pods, P, &kp);
+    if (rc) return rc;
     ks_drain_candidates kc{n, node.data(), pod_offset};
     return ks_drain_check(c->snap, &kp, &kc, policy, flags, out_placed, out_node_idx, nullptr);
 }
@@ -1581,14 +1574,12 @@ int ksh_place_replicas(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const
                        ks_replica_plan* out, int32_t* out_node, int64_t* out_score) try {
     if (!c || (n && (!pods || !replicas || !out))) return fail(KS_ERR_INVALID, "NULL argument");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
-    if (!ks_place_replicas) return fail(KS_ERR_NO_DEVICE, "this library has no ks_place_replicas");
-    if (n == 0) return KS_OK;
-    std::vector<int64_t>&rc_ = c->pk_cpu, &rm_ = c->pk_mem; // the same packed batch buffers as ksh_select_nodes
-    std::vector<uint64_t>& sel = c->pk_sel;
-    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel);
+    int rc = device_ready(c, ks_place_replicas, "ks_place_replicas");
     if (rc) return rc;
-    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
+    if (n == 0) return KS_OK;
+    ks_pods kp;
+    rc = pack_batch(c, pods, n, &kp);
+    if (rc) return rc;
     return ks_place_replicas(c->snap, &kp, replicas, policy, out, out_node, out_score);
 }
 KSH_CATCH
@@ -1618,16 +1609,11 @@ int ksh_context_topology_domains(const ksh_context* c, const char* key, int32_t*
     const uint32_t D = topology_domains(c, key, out_node_domain, &values);
     *out_n_domains = D;
     if (!names || !out_name_off) return KS_OK;
-    size_t used = 0;
+    StringList list{names, cap};
     for (uint32_t d = 0; d < D; d++) {
         const char* k = c->pairs.str(values[d]);
         const char* v = k + std::strlen(k) + 1;
-        const size_t len = std::strlen(v);
-        out_name_off[d] = -1;
-        if (used + len + 1 > cap) continue; // -1 = did not fit
-        std::memcpy(names + used, v, len + 1);
-        out_name_off[d] = (int64_t)used;
-        used += len + 1;
+        out_name_off[d] = list.append(v, std::strlen(v) + 1);
     }
     return KS_OK;
 }
@@ -1643,12 +1629,11 @@ int ksh_place_replicas_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n
         for (uint64_t t = 0; t < n; t++)
             if (existing_offset[t + 1] < existing_offset[t]) return fail(KS_ERR_INVALID, "existing offsets decrease");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
-    if (!ks_place_replicas_spread) return fail(KS_ERR_NO_DEVICE, "this library has no ks_place_replicas_spread");
+    int rc = device_ready(c, ks_place_replicas_spread, "ks_place_replicas_spread");
+    if (rc) return rc;
     if (n == 0) return KS_OK;
-    std::vector<int64_t>&rc_ = c->pk_cpu, &rm_ = c->pk_mem; // the same packed batch buffers as ksh_select_nodes
-    std::vector<uint64_t>& sel = c->pk_sel;
-    int rc = pack_and_upload(c, pods, n, rc_, rm_, sel);
+    ks_pods kp;
+    rc = pack_batch(c, pods, n, &kp);
     if (rc) return rc;
     std::vector<int32_t> dom(c->N);
     std::vector<uint32_t> values;
@@ -1665,7 +1650,6 @@ int ksh_place_replicas_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n
                 if (idx >= 0 && dom[idx] >= 0) existing[t * Dc + (uint32_t)dom[idx]]++; // unknown or keyless: not counted
             }
     }
-    ks_pods kp{n, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     ks_spread sp{Dc, dom.data(), max_skew, min_domains, existing_offset ? existing.data() : nullptr};
     return ks_place_replicas_spread(c->snap, &kp, replicas, &sp, policy, out, out_node, out_score,
                                     D ? out_domain_count : nullptr);
@@ -1752,8 +1736,8 @@ int ksh_scaleup_estimate(ksh_context* c, const ks_node_obj* templates, uint64_t 
             sel[p * W + b / 64] |= 1ull << (b % 64);
         }
     }
-    if (!c->snap) return fail(KS_ERR_NO_DEVICE, "packing-only context (KSH_DEVICE_NONE): no device snapshot, nothing is computed on the host");
-    if (!ks_scaleup_estimate) return fail(KS_ERR_NO_DEVICE, "this library has no ks_scaleup_estimate");
+    const int rc = device_ready(c, ks_scaleup_estimate, "ks_scaleup_estimate");
+    if (rc) return rc;
     ks_pods kp{n_pods, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
     ks_node_templates kt{n_templates, W, ac.data(), am.data(), fc.data(), fm.data(), lab.data(), max_nodes};
     return ks_scaleup_estimate(c->snap, &kp, &kt, out, out_best, out_node, out_reasons);

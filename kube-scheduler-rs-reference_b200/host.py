@@ -5,8 +5,9 @@ import ctypes as C
 import numpy as np
 
 from . import _capi as capi
-from ._capi import KsError, lib
+from ._capi import _proto, check, lib
 from .objects import ks_node_obj, ks_pod_obj
+from .snapshot import replica_outputs
 
 _vp = C.c_void_p
 for _name, _res, _args in [
@@ -48,9 +49,7 @@ for _name, _res, _args in [
     ("ksh_place_replicas_spread", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_char_p, _vp, _vp, _vp, _vp, C.c_int, _vp,
                                             _vp, _vp, _vp]),
 ]:
-    _f = getattr(lib, _name)
-    _f.restype = _res
-    _f.argtypes = _args
+    _proto(_name, _res, *_args)
 
 KSH_DEVICE_NONE = -1  # packing-only context: objects -> SoA arrays on the host, no predicate is ever evaluated
 KSH_RECONCILE_OK, KSH_RECONCILE_NO_NODE_FOUND, KSH_RECONCILE_BINDING_OBJECT_FAILED = 0, 1, 2
@@ -59,6 +58,23 @@ KSH_RECONCILE_GANG_UNSATISFIED = 4
 
 def _addr(arr, i=0):
     return C.addressof(arr) + i * C.sizeof(arr._type_)
+
+
+def _string_list(buf, off, counts=None):
+    """Decode a string-list output (include/ksched_host.h): entry i starts at byte off[i] of buf (-1 = no entry) and
+    holds counts[i] NUL-terminated strings, or one when counts is None.  Returns per entry a str (a list of str with
+    counts) or None."""
+    out = []
+    for i, o in enumerate(off.tolist()):
+        if o < 0:
+            out.append(None)
+            continue
+        at, strs = C.addressof(buf) + o, []
+        for _ in range(1 if counts is None else int(counts[i])):
+            strs.append(C.string_at(at))
+            at += len(strs[-1]) + 1
+        out.append(strs[0].decode() if counts is None else [k.decode() for k in strs])
+    return out
 
 
 def parse_cpu_millicores(s):
@@ -87,9 +103,8 @@ def format_unschedulable(n_nodes, reasons, cap=256):
     """FailedScheduling message for one pod's counts (4 ints in ks_pod_reasons order): (full length, text in cap bytes)."""
     r = capi.ks_pod_reasons(*[int(x) for x in reasons])
     buf = C.create_string_buffer(max(cap, 1))
-    n = lib.ksh_format_unschedulable(int(n_nodes), C.byref(r), C.addressof(buf) if cap else None, int(cap))
-    if n < 0:
-        raise KsError(n, "ksh_format_unschedulable")
+    n = check(lib.ksh_format_unschedulable(int(n_nodes), C.byref(r), C.addressof(buf) if cap else None, int(cap)),
+              "ksh_format_unschedulable")
     return n, buf.value.decode()
 
 
@@ -100,9 +115,7 @@ class Context:
 
     def __init__(self, device=0):
         h = _vp()
-        rc = lib.ksh_context_create(int(device), C.byref(h))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_context_create")
+        check(lib.ksh_context_create(int(device), C.byref(h)), "ksh_context_create")
         self._h = h
 
     def close(self):
@@ -123,14 +136,10 @@ class Context:
         self.close()
 
     def set_nodes(self, nodes, n):
-        rc = lib.ksh_context_set_nodes(self._h, C.addressof(nodes), n)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_context_set_nodes")
+        check(lib.ksh_context_set_nodes(self._h, C.addressof(nodes), n), "ksh_context_set_nodes")
 
     def set_cluster_pods(self, pods, n):
-        rc = lib.ksh_context_set_cluster_pods(self._h, C.addressof(pods), n)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_context_set_cluster_pods")
+        check(lib.ksh_context_set_cluster_pods(self._h, C.addressof(pods), n), "ksh_context_set_cluster_pods")
 
     @property
     def label_words(self):
@@ -146,25 +155,17 @@ class Context:
 
     def upsert_node(self, nodes, i=0):
         idx = C.c_uint32()
-        rc = lib.ksh_context_upsert_node(self._h, _addr(nodes, i), C.byref(idx))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_context_upsert_node")
+        check(lib.ksh_context_upsert_node(self._h, _addr(nodes, i), C.byref(idx)), "ksh_context_upsert_node")
         return idx.value
 
     def remove_node(self, name):
-        rc = lib.ksh_context_remove_node(self._h, name.encode())
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_context_remove_node")
+        check(lib.ksh_context_remove_node(self._h, name.encode()), "ksh_context_remove_node")
 
     def pod_bound(self, pods, i=0):
-        rc = lib.ksh_context_pod_bound(self._h, _addr(pods, i))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_context_pod_bound")
+        check(lib.ksh_context_pod_bound(self._h, _addr(pods, i)), "ksh_context_pod_bound")
 
     def pod_deleted(self, pods, i=0):
-        rc = lib.ksh_context_pod_deleted(self._h, _addr(pods, i))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_context_pod_deleted")
+        check(lib.ksh_context_pod_deleted(self._h, _addr(pods, i)), "ksh_context_pod_deleted")
 
     def node_name(self, idx):
         n = lib.ksh_context_node_name(self._h, int(idx))
@@ -174,9 +175,8 @@ class Context:
         rc_ = np.empty(n, np.int64)
         rm_ = np.empty(n, np.int64)
         sel = np.zeros((n, 8), np.uint64)
-        w = lib.ksh_pack_pods(self._h, C.addressof(pods), n, rc_.ctypes.data, rm_.ctypes.data, sel.ctypes.data, 8)
-        if w < 0:
-            raise KsError(w, "ksh_pack_pods")
+        w = check(lib.ksh_pack_pods(self._h, C.addressof(pods), n, rc_.ctypes.data, rm_.ctypes.data, sel.ctypes.data,
+                                    8), "ksh_pack_pods")
         return rc_, rm_, np.ascontiguousarray(sel[:, :w])
 
     def export_packed(self):
@@ -185,17 +185,12 @@ class Context:
         ac, am = np.empty(n, np.int64), np.empty(n, np.int64)
         lab = np.zeros((n, w), np.uint64)
         bn, bc, bm = np.empty(b, np.int32), np.empty(b, np.int64), np.empty(b, np.int64)
-        rc = lib.ksh_context_export_packed(self._h, ac.ctypes.data, am.ctypes.data, lab.ctypes.data, bn.ctypes.data,
-                                           bc.ctypes.data, bm.ctypes.data)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_context_export_packed")
+        check(lib.ksh_context_export_packed(self._h, ac.ctypes.data, am.ctypes.data, lab.ctypes.data, bn.ctypes.data,
+                                            bc.ctypes.data, bm.ctypes.data), "ksh_context_export_packed")
         return ac, am, lab, bn, bc, bm
 
     def check_node_validity(self, pods, i, node_idx):
-        rc = lib.ksh_check_node_validity(self._h, _addr(pods, i), int(node_idx))
-        if rc < 0:
-            raise KsError(rc, "ksh_check_node_validity")
-        return rc
+        return check(lib.ksh_check_node_validity(self._h, _addr(pods, i), int(node_idx)), "ksh_check_node_validity")
 
     def place_replicas(self, pods, n, replicas, policy=capi.KS_SCORE_LEFTOVER, want_nodes=True, first=0):
         """Replica placement over objects (ksh_place_replicas): pod t asks for replicas[t] copies of itself.  Charges
@@ -204,17 +199,10 @@ class Context:
         replicas = np.ascontiguousarray(replicas, np.uint32).reshape(-1)
         if replicas.shape[0] != n:
             raise ValueError(f"replicas has {replicas.shape[0]} entries, pods {n}")
-        offset = np.zeros(n + 1, np.uint64)
-        np.cumsum(replicas, dtype=np.uint64, out=offset[1:])
-        rows = np.zeros(n, capi.REPLICA_PLAN_DTYPE)
-        total = int(offset[-1]) if want_nodes and int(offset[-1]) <= capi.KS_REPLICAS_MAX_TOTAL else 0
-        node = np.empty(total, np.int32) if want_nodes else None
-        score = np.empty(total, np.int64) if want_nodes else None
-        rc = lib.ksh_place_replicas(self._h, _addr(pods, first), n, replicas.ctypes.data, int(policy), rows.ctypes.data,
-                                    None if node is None else node.ctypes.data,
-                                    None if score is None else score.ctypes.data)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_place_replicas")
+        offset, rows, node, score = replica_outputs(replicas, capi.REPLICA_PLAN_DTYPE, want_nodes)
+        check(lib.ksh_place_replicas(self._h, _addr(pods, first), n, replicas.ctypes.data, int(policy),
+                                     rows.ctypes.data, None if node is None else node.ctypes.data,
+                                     None if score is None else score.ctypes.data), "ksh_place_replicas")
         return rows, node, score, offset
 
     def topology_domains(self, key):
@@ -228,16 +216,12 @@ class Context:
         while True:
             buf = C.create_string_buffer(cap)
             off = np.empty(max(n, 1), np.int64)
-            rc = lib.ksh_context_topology_domains(self._h, key.encode(), dom.ctypes.data, C.byref(d), buf, cap,
-                                                  off.ctypes.data)
-            if rc != capi.KS_OK:
-                raise KsError(rc, "ksh_context_topology_domains")
+            check(lib.ksh_context_topology_domains(self._h, key.encode(), dom.ctypes.data, C.byref(d), buf, cap,
+                                                   off.ctypes.data), "ksh_context_topology_domains")
             if (off[:d.value] >= 0).all():
                 break
             cap *= 4
-        raw = buf.raw
-        values = [raw[o:raw.index(b"\0", o)].decode() for o in off[:d.value].tolist()]
-        return dom, values
+        return dom, _string_list(buf, off[:d.value])
 
     def place_replicas_spread(self, pods, n, replicas, topology_key, max_skew, min_domains=None, existing_nodes=None,
                               policy=capi.KS_SCORE_LEFTOVER, want_nodes=True, first=0):
@@ -258,32 +242,25 @@ class Context:
             ex_off = np.zeros(n + 1, np.uint64)
             np.cumsum([len(lst) for lst in existing_nodes], out=ex_off[1:])
         D = len(self.topology_domains(topology_key)[1])
-        offset = np.zeros(n + 1, np.uint64)
-        np.cumsum(replicas, dtype=np.uint64, out=offset[1:])
-        rows = np.zeros(n, capi.SPREAD_PLAN_DTYPE)
-        total = int(offset[-1]) if want_nodes and int(offset[-1]) <= capi.KS_REPLICAS_MAX_TOTAL else 0
-        node = np.empty(total, np.int32) if want_nodes else None
-        score = np.empty(total, np.int64) if want_nodes else None
+        offset, rows, node, score = replica_outputs(replicas, capi.SPREAD_PLAN_DTYPE, want_nodes)
         counts = np.empty((n, D), np.uint32) if D and n * D <= capi.KS_SPREAD_MAX_COUNTS else None
-        rc = lib.ksh_place_replicas_spread(self._h, _addr(pods, first), n, replicas.ctypes.data, topology_key.encode(),
-                                           max_skew.ctypes.data, None if mind is None else mind.ctypes.data,
-                                           None if names is None else C.cast(names, _vp),
-                                           None if ex_off is None else ex_off.ctypes.data, int(policy), rows.ctypes.data,
-                                           None if node is None else node.ctypes.data,
-                                           None if score is None else score.ctypes.data,
-                                           None if counts is None else counts.ctypes.data)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_place_replicas_spread")
+        check(lib.ksh_place_replicas_spread(self._h, _addr(pods, first), n, replicas.ctypes.data, topology_key.encode(),
+                                            max_skew.ctypes.data, None if mind is None else mind.ctypes.data,
+                                            None if names is None else C.cast(names, _vp),
+                                            None if ex_off is None else ex_off.ctypes.data, int(policy),
+                                            rows.ctypes.data,
+                                            None if node is None else node.ctypes.data,
+                                            None if score is None else score.ctypes.data,
+                                            None if counts is None else counts.ctypes.data),
+              "ksh_place_replicas_spread")
         return rows, node, score, offset, counts
 
     def select_nodes(self, pods, n, policy=capi.KS_SCORE_LEFTOVER, first=0):
         idx = np.empty(n, np.int32)
         score = np.empty(n, np.int64)
         cnt = np.empty(n, np.uint32)
-        rc = lib.ksh_select_nodes(self._h, _addr(pods, first), n, int(policy), idx.ctypes.data, score.ctypes.data,
-                                  cnt.ctypes.data)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_select_nodes")
+        check(lib.ksh_select_nodes(self._h, _addr(pods, first), n, int(policy), idx.ctypes.data, score.ctypes.data,
+                                   cnt.ctypes.data), "ksh_select_nodes")
         return idx, score, cnt
 
     def rank_nodes(self, pods, n, k, policy=capi.KS_SCORE_LEFTOVER, first=0):
@@ -292,10 +269,8 @@ class Context:
         idx = np.empty((n, int(k)), np.int32)
         score = np.empty((n, int(k)), np.int64)
         cnt = np.empty(n, np.uint32)
-        rc = lib.ksh_rank_nodes(self._h, _addr(pods, first), n, int(policy), int(k), idx.ctypes.data, score.ctypes.data,
-                                cnt.ctypes.data)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_rank_nodes")
+        check(lib.ksh_rank_nodes(self._h, _addr(pods, first), n, int(policy), int(k), idx.ctypes.data,
+                                 score.ctypes.data, cnt.ctypes.data), "ksh_rank_nodes")
         return idx, score, cnt
 
     def select_node_for_pod(self, pods, n, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first=0):
@@ -304,10 +279,9 @@ class Context:
         used = np.empty(n, np.uint32)
         dn = np.empty((n, attempts), np.int32)
         dc = np.empty((n, attempts), np.uint8)
-        rc = lib.ksh_select_node_for_pod(self._h, _addr(pods, first), n, int(attempts), int(seed), int(first),
-                                         idx.ctypes.data, used.ctypes.data, dn.ctypes.data, dc.ctypes.data)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_select_node_for_pod")
+        check(lib.ksh_select_node_for_pod(self._h, _addr(pods, first), n, int(attempts), int(seed), int(first),
+                                          idx.ctypes.data, used.ctypes.data, dn.ctypes.data, dc.ctypes.data),
+              "ksh_select_node_for_pod")
         return idx, used, dn, dc
 
     def explain_pods(self, pods, n, first=0, msg_cap=None):
@@ -317,17 +291,15 @@ class Context:
         off = np.empty(n, np.int64)
         cap = int(msg_cap if msg_cap is not None else 256 * max(n, 1))
         buf = C.create_string_buffer(max(cap, 1))
-        rc = lib.ksh_explain_pods(self._h, _addr(pods, first), n, out.ctypes.data, C.addressof(buf), cap, off.ctypes.data)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_explain_pods")
-        return out, [None if o < 0 else C.string_at(C.addressof(buf) + int(o)).decode() for o in off]
+        check(lib.ksh_explain_pods(self._h, _addr(pods, first), n, out.ctypes.data, C.addressof(buf), cap,
+                                   off.ctypes.data), "ksh_explain_pods")
+        return out, _string_list(buf, off)
 
     def set_pod_priorities(self, pods, priority, n, first=0):
         """spec.priority of bound pods known by namespace/name (others are ignored)."""
         priority = np.ascontiguousarray(priority, np.int32)
-        rc = lib.ksh_context_set_pod_priorities(self._h, _addr(pods, first), priority.ctypes.data, n)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_context_set_pod_priorities")
+        check(lib.ksh_context_set_pod_priorities(self._h, _addr(pods, first), priority.ctypes.data, n),
+              "ksh_context_set_pod_priorities")
 
     def preempt_pods(self, pods, n, priority, max_victims, first=0, victims_cap=None):
         """Priority preemption (ksh_preempt_pods): (rows PREEMPTION_DTYPE [n], victims[n]) where victims[i] is the list
@@ -337,28 +309,15 @@ class Context:
         off = np.empty(n, np.int64)
         cap = int(victims_cap if victims_cap is not None else 64 * int(max_victims) * max(n, 1))
         buf = C.create_string_buffer(max(cap, 1))
-        rc = lib.ksh_preempt_pods(self._h, _addr(pods, first), n, priority.ctypes.data, int(max_victims), rows.ctypes.data,
-                                  C.addressof(buf), cap, off.ctypes.data)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_preempt_pods")
-        victims = []
-        for i, o in enumerate(off):
-            if o < 0:
-                victims.append(None)
-                continue
-            keys, at = [], C.addressof(buf) + int(o)
-            for _ in range(int(rows["n_victims"][i])):
-                keys.append(C.string_at(at).decode())
-                at += len(keys[-1].encode()) + 1
-            victims.append(keys)
-        return rows, victims
+        check(lib.ksh_preempt_pods(self._h, _addr(pods, first), n, priority.ctypes.data, int(max_victims),
+                                   rows.ctypes.data, C.addressof(buf), cap, off.ctypes.data), "ksh_preempt_pods")
+        return rows, _string_list(buf, off, rows["n_victims"])
 
     def reconcile(self, pods, i, policy=capi.KS_SCORE_LEFTOVER):
         node = C.c_int32(-1)
         buf = C.create_string_buffer(1024)
-        rc = lib.ksh_reconcile(self._h, _addr(pods, i), int(policy), C.byref(node), buf, len(buf))
-        if rc < 0:
-            raise KsError(rc, "ksh_reconcile")
+        rc = check(lib.ksh_reconcile(self._h, _addr(pods, i), int(policy), C.byref(node), buf, len(buf)),
+                   "ksh_reconcile")
         return rc, node.value, buf.value.decode()
 
     def reconcile_batch(self, pods, n, policy=capi.KS_SCORE_LEFTOVER, json_cap=None):
@@ -369,11 +328,9 @@ class Context:
         cap = int(json_cap if json_cap is not None else 512 * max(n, 1))
         buf = C.create_string_buffer(cap)
         rounds = C.c_uint32()
-        rc = lib.ksh_reconcile_batch(self._h, C.addressof(pods), n, int(policy), status.ctypes.data, node.ctypes.data,
-                                     C.addressof(buf), cap, off.ctypes.data, C.byref(rounds))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_reconcile_batch")
-        bodies = [None if o < 0 else C.string_at(C.addressof(buf) + int(o)).decode() for o in off]
+        check(lib.ksh_reconcile_batch(self._h, C.addressof(pods), n, int(policy), status.ctypes.data, node.ctypes.data,
+                                      C.addressof(buf), cap, off.ctypes.data, C.byref(rounds)), "ksh_reconcile_batch")
+        bodies = _string_list(buf, off)
         return status, node, bodies, rounds.value
 
     def reconcile_gangs(self, pods, n, offset, min_member, policy=capi.KS_SCORE_LEFTOVER, json_cap=None):
@@ -391,12 +348,10 @@ class Context:
         placed = np.empty(g, np.uint32)
         cap = int(json_cap if json_cap is not None else 512 * max(n, 1))
         buf = C.create_string_buffer(max(cap, 1))
-        rc = lib.ksh_reconcile_gangs(self._h, C.addressof(pods), n, offset.ctypes.data, g, min_member.ctypes.data,
-                                     int(policy), status.ctypes.data, node.ctypes.data, placed.ctypes.data,
-                                     C.addressof(buf), cap, off.ctypes.data)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_reconcile_gangs")
-        bodies = [None if o < 0 else C.string_at(C.addressof(buf) + int(o)).decode() for o in off]
+        check(lib.ksh_reconcile_gangs(self._h, C.addressof(pods), n, offset.ctypes.data, g, min_member.ctypes.data,
+                                      int(policy), status.ctypes.data, node.ctypes.data, placed.ctypes.data,
+                                      C.addressof(buf), cap, off.ctypes.data), "ksh_reconcile_gangs")
+        bodies = _string_list(buf, off)
         return status, node, bodies, placed
 
     def drain_nodes(self, node_names, pods, pod_offset, policy=capi.KS_SCORE_LEFTOVER, flags=0):
@@ -410,10 +365,9 @@ class Context:
         p = int(pod_offset[-1])
         placed = np.empty(d, np.uint32)
         node = np.empty(p, np.int32)
-        rc = lib.ksh_drain_nodes(self._h, C.addressof(names), d, C.addressof(pods) if pods is not None else None,
-                                 pod_offset.ctypes.data, int(policy), int(flags), placed.ctypes.data, node.ctypes.data)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_drain_nodes")
+        check(lib.ksh_drain_nodes(self._h, C.addressof(names), d, C.addressof(pods) if pods is not None else None,
+                                  pod_offset.ctypes.data, int(policy), int(flags), placed.ctypes.data,
+                                  node.ctypes.data), "ksh_drain_nodes")
         return placed, node
 
     def scaleup_estimate(self, templates, n_templates, max_nodes, pods, n_pods, overhead_pods=None, n_overhead=0,
@@ -434,8 +388,7 @@ class Context:
 
         def obj(a):
             return C.addressof(a) if a is not None else None
-        rc = lib.ksh_scaleup_estimate(self._h, obj(templates), n_templates, ptr(max_nodes), obj(overhead_pods),
-                                      n_overhead, obj(pods), n_pods, ptr(rows), C.addressof(best), ptr(node), ptr(why))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ksh_scaleup_estimate")
+        check(lib.ksh_scaleup_estimate(self._h, obj(templates), n_templates, ptr(max_nodes), obj(overhead_pods),
+                                       n_overhead, obj(pods), n_pods, ptr(rows), C.addressof(best), ptr(node),
+                                       ptr(why)), "ksh_scaleup_estimate")
         return rows, best.value, node, why

@@ -80,9 +80,7 @@ class PeerExchange:
         self.bytes = self.off_state + 256
         base = C.c_void_p()
         handle = C.create_string_buffer(64)
-        rc = capi.lib.ks_ipc_alloc(self.device, self.bytes, C.byref(base), handle)
-        if rc != capi.KS_OK:
-            raise capi.KsError(rc, "ks_ipc_alloc")
+        capi.check(capi.lib.ks_ipc_alloc(self.device, self.bytes, C.byref(base), handle), "ks_ipc_alloc")
         self.base = base.value
         handles = [None] * self.world
         dist.all_gather_object(handles, handle.raw, group=group)
@@ -91,9 +89,7 @@ class PeerExchange:
             if r == self.rank:
                 continue
             p = C.c_void_p()
-            rc = capi.lib.ks_ipc_open(self.device, handles[r], C.byref(p))
-            if rc != capi.KS_OK:
-                raise capi.KsError(rc, f"ks_ipc_open(rank {r})")
+            capi.check(capi.lib.ks_ipc_open(self.device, handles[r], C.byref(p)), f"ks_ipc_open(rank {r})")
             self.peer_base[r] = p.value
         d = capi.ks_exchange()
         d.world, d.rank, d.n_peers = self.world, self.rank, self.world - 1
@@ -116,9 +112,8 @@ class PeerExchange:
     def read(self):
         """(node_idx [world, cap] int32, score [world, cap] int64) of everything gathered so far (synchronises)."""
         buf = np.empty(self.world * self.cap * 12, np.uint8)
-        rc = self._capi.lib.ks_device_read(self.device, self.base, buf.ctypes.data, buf.nbytes)
-        if rc != self._capi.KS_OK:
-            raise self._capi.KsError(rc, "ks_device_read")
+        self._capi.check(self._capi.lib.ks_device_read(self.device, self.base, buf.ctypes.data, buf.nbytes),
+                         "ks_device_read")
         score = buf[:self.off_idx].view(np.int64).reshape(self.world, self.cap)
         idx = buf[self.off_idx:self.off_idx + self.world * self.cap * 4].view(np.int32).reshape(self.world, self.cap)
         return idx, score
@@ -128,9 +123,8 @@ class PeerExchange:
         {"argmax1_start", "argmax2_start", "flags_published", "wait_started", "wait_done"}
         (ks_exchange.local_state words 2..11; synchronises)."""
         st = np.zeros(6, np.uint64)
-        rc = self._capi.lib.ks_device_read(self.device, self.base + self.off_state, st.ctypes.data, st.nbytes)
-        if rc != self._capi.KS_OK:
-            raise self._capi.KsError(rc, "ks_device_read")
+        self._capi.check(self._capi.lib.ks_device_read(self.device, self.base + self.off_state, st.ctypes.data,
+                                                       st.nbytes), "ks_device_read")
         names = ("argmax1_start", "flags_published", "wait_started", "wait_done", "argmax2_start")
         return {k: int(st[1 + i]) for i, k in enumerate(names)}
 

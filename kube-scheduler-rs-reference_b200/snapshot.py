@@ -8,7 +8,7 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _capi as capi
-from ._capi import KsError, ks_bindings, ks_bound_pods, ks_pods, lib
+from ._capi import check, ks_bindings, ks_bound_pods, ks_pods, lib
 
 
 def _ptr(a):
@@ -26,6 +26,19 @@ def _c(a, dtype):
     return a
 
 
+def replica_outputs(replicas, row_dtype, want_nodes):
+    """Output arrays of a replica plan for replicas [T] (uint32): (offset uint64 [T + 1], rows row_dtype [T], node
+    int32, score int64).  Spec t's copies go to [offset[t], offset[t+1]) of node / score, which hold no entry when the
+    copies exceed capi.KS_REPLICAS_MAX_TOTAL and are None unless want_nodes."""
+    offset = np.zeros(len(replicas) + 1, np.uint64)
+    np.cumsum(replicas, dtype=np.uint64, out=offset[1:])
+    rows = np.zeros(len(replicas), row_dtype)
+    if not want_nodes:
+        return offset, rows, None, None
+    total = int(offset[-1]) if int(offset[-1]) <= capi.KS_REPLICAS_MAX_TOTAL else 0
+    return offset, rows, np.empty(total, np.int32), np.empty(total, np.int64)
+
+
 @dataclass
 class SelectResult:
     node_idx: np.ndarray
@@ -38,9 +51,7 @@ class SelectResult:
 class Snapshot:
     def __init__(self, device=0):
         h = C.c_void_p()
-        rc = lib.ks_snapshot_create(int(device), C.byref(h))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_snapshot_create")
+        check(lib.ks_snapshot_create(int(device), C.byref(h)), "ks_snapshot_create")
         self._h = h
         self.device = device
 
@@ -76,38 +87,29 @@ class Snapshot:
         n = alloc_cpu.shape[0]
         labels = labels.reshape(n, -1) if n else labels.reshape(0, max(1, labels.shape[-1] if labels.ndim > 1 else 1))
         w = labels.shape[1]
-        rc = lib.ks_snapshot_set_nodes(self._h, n, w, _ptr(alloc_cpu), _ptr(alloc_mem), _ptr(labels))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_snapshot_set_nodes")
+        check(lib.ks_snapshot_set_nodes(self._h, n, w, _ptr(alloc_cpu), _ptr(alloc_mem), _ptr(labels)),
+              "ks_snapshot_set_nodes")
 
     def set_bound(self, node_idx, req_cpu, req_mem):
         node_idx = _c(node_idx, np.int32)
         req_cpu = _c(req_cpu, np.int64)
         req_mem = _c(req_mem, np.int64)
-        rc = lib.ks_snapshot_set_bound(self._h, node_idx.shape[0], _ptr(node_idx), _ptr(req_cpu), _ptr(req_mem))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_snapshot_set_bound")
+        check(lib.ks_snapshot_set_bound(self._h, node_idx.shape[0], _ptr(node_idx), _ptr(req_cpu), _ptr(req_mem)),
+              "ks_snapshot_set_bound")
 
     def apply_bind(self, node_idx, req_cpu, req_mem):
-        rc = lib.ks_snapshot_apply_bind(self._h, int(node_idx), int(req_cpu), int(req_mem))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_snapshot_apply_bind")
+        check(lib.ks_snapshot_apply_bind(self._h, int(node_idx), int(req_cpu), int(req_mem)), "ks_snapshot_apply_bind")
 
     def free(self):
         n = self.n_nodes
         fc = np.empty(n, np.int64)
         fm = np.empty(n, np.int64)
-        rc = lib.ks_snapshot_get_free(self._h, _ptr(fc), _ptr(fm))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_snapshot_get_free")
+        check(lib.ks_snapshot_get_free(self._h, _ptr(fc), _ptr(fm)), "ks_snapshot_get_free")
         return fc, fm
 
     def check_cell(self, req_cpu, req_mem, sel, node_idx):
         sel = _c(sel, np.uint64).reshape(-1)
-        rc = lib.ks_check_cell(self._h, int(req_cpu), int(req_mem), _ptr(sel), int(node_idx))
-        if rc < 0:
-            raise KsError(rc, "ks_check_cell")
-        return rc
+        return check(lib.ks_check_cell(self._h, int(req_cpu), int(req_mem), _ptr(sel), int(node_idx)), "ks_check_cell")
 
     def _pods(self, req_cpu, req_mem, sel):
         req_cpu = _c(req_cpu, np.int64)
@@ -121,9 +123,7 @@ class Snapshot:
     def check_cells(self, req_cpu, req_mem, sel):
         pods, keep = self._pods(req_cpu, req_mem, sel)
         codes = np.empty((pods.n, self.n_nodes), np.uint8)
-        rc = lib.ks_check_cells(self._h, C.byref(pods), _ptr(codes))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_check_cells")
+        check(lib.ks_check_cells(self._h, C.byref(pods), _ptr(codes)), "ks_check_cells")
         return codes
 
     def select(self, req_cpu, req_mem, sel, policy=capi.KS_SCORE_LEFTOVER, flags=capi.KS_SELECT_AUTO, want_mask=False):
@@ -141,9 +141,7 @@ class Snapshot:
         if want_mask:
             mask = np.zeros((p, row), np.uint8)
         out = ks_bindings(_ptr(idx), _ptr(score), _ptr(cnt), capi.KS_MEM_HOST, _ptr(mask), row, capi.KS_MEM_HOST, None, None)
-        rc = lib.ks_select(self._h, C.byref(pods), int(policy), int(flags), C.byref(out), None)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_select")
+        check(lib.ks_select(self._h, C.byref(pods), int(policy), int(flags), C.byref(out), None), "ks_select")
         return SelectResult(idx, score, cnt, mask, self.last_path())
 
     def select_raw(self, n_pods, req_cpu, req_mem, sel, pods_space, node_idx, score, cnt, out_space, mask=None,
@@ -155,10 +153,8 @@ class Snapshot:
         out = ks_bindings(_ptr(node_idx), _ptr(score), _ptr(cnt), int(out_space), _ptr(mask), int(mask_row_bytes),
                           int(mask_space), C.c_void_p(ready_event) if ready_event else None,
                           C.pointer(exchange.desc) if exchange is not None else None)
-        rc = lib.ks_select(self._h, C.byref(pods), int(policy), int(flags), C.byref(out),
-                           C.c_void_p(stream) if stream else None)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_select")
+        check(lib.ks_select(self._h, C.byref(pods), int(policy), int(flags), C.byref(out),
+                            C.c_void_p(stream) if stream else None), "ks_select")
 
     def commit_claims(self, claim_node, req_cpu, req_mem):
         """K3: accept claims per node in arrival order while they fit; decrements free[] on the device."""
@@ -166,10 +162,8 @@ class Snapshot:
         req_cpu = _c(req_cpu, np.int64)
         req_mem = _c(req_mem, np.int64)
         acc = np.zeros(claim_node.shape[0], np.uint8)
-        rc = lib.ks_snapshot_commit_claims(self._h, claim_node.shape[0], _ptr(claim_node), _ptr(req_cpu),
-                                           _ptr(req_mem), _ptr(acc))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_snapshot_commit_claims")
+        check(lib.ks_snapshot_commit_claims(self._h, claim_node.shape[0], _ptr(claim_node), _ptr(req_cpu),
+                                            _ptr(req_mem), _ptr(acc)), "ks_snapshot_commit_claims")
         return acc
 
     def stream_bind(self, req_cpu, req_mem, sel, policy=capi.KS_SCORE_LEFTOVER):
@@ -179,9 +173,8 @@ class Snapshot:
         idx = np.empty(p, np.int32)
         score = np.empty(p, np.int64)
         rounds = C.c_uint32()
-        rc = lib.ks_stream_bind(self._h, C.byref(pods), int(policy), _ptr(idx), _ptr(score), C.byref(rounds))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_stream_bind")
+        check(lib.ks_stream_bind(self._h, C.byref(pods), int(policy), _ptr(idx), _ptr(score), C.byref(rounds)),
+              "ks_stream_bind")
         return idx, score, rounds.value
 
     def gang_bind(self, req_cpu, req_mem, sel, offset, min_member, policy=capi.KS_SCORE_LEFTOVER):
@@ -200,10 +193,8 @@ class Snapshot:
         score = np.empty(p, np.int64)
         placed = np.empty(g, np.uint32)
         rounds = np.empty(g, np.uint32)
-        rc = lib.ks_gang_bind(self._h, C.byref(pods), C.byref(gangs), int(policy), _ptr(idx), _ptr(score),
-                              _ptr(placed), _ptr(rounds))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_gang_bind")
+        check(lib.ks_gang_bind(self._h, C.byref(pods), C.byref(gangs), int(policy), _ptr(idx), _ptr(score),
+                               _ptr(placed), _ptr(rounds)), "ks_gang_bind")
         return idx, score, placed, rounds
 
     def drain_check(self, req_cpu, req_mem, sel, node_idx, offset, policy=capi.KS_SCORE_LEFTOVER, flags=0):
@@ -221,10 +212,8 @@ class Snapshot:
         placed = np.empty(d, np.uint32)
         idx = np.empty(p, np.int32)
         score = np.empty(p, np.int64)
-        rc = lib.ks_drain_check(self._h, C.byref(pods), C.byref(cand), int(policy), int(flags), _ptr(placed), _ptr(idx),
-                                _ptr(score))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_drain_check")
+        check(lib.ks_drain_check(self._h, C.byref(pods), C.byref(cand), int(policy), int(flags), _ptr(placed),
+                                 _ptr(idx), _ptr(score)), "ks_drain_check")
         return placed, idx, score
 
     def scaleup_estimate(self, req_cpu, req_mem, sel, alloc_cpu, alloc_mem, free_cpu, free_mem, labels, max_nodes,
@@ -257,10 +246,8 @@ class Snapshot:
         best = C.c_int32(-1)
         node = np.empty((t, p), np.int32) if want_nodes else None
         why = np.empty((p, 4), np.uint32) if want_reasons else None
-        rc = lib.ks_scaleup_estimate(self._h, C.byref(pods), C.byref(tmpl), _ptr(rows), C.addressof(best), _ptr(node),
-                                     _ptr(why))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_scaleup_estimate")
+        check(lib.ks_scaleup_estimate(self._h, C.byref(pods), C.byref(tmpl), _ptr(rows), C.addressof(best), _ptr(node),
+                                      _ptr(why)), "ks_scaleup_estimate")
         return rows, best.value, node, why
 
     def place_replicas(self, req_cpu, req_mem, sel, replicas, policy=capi.KS_SCORE_LEFTOVER, want_nodes=True):
@@ -277,16 +264,9 @@ class Snapshot:
         if t and (replicas.min() < 0 or replicas.max() > 0xFFFFFFFF):
             raise ValueError("replicas must lie in [0, 2^32)")
         replicas = _c(replicas, np.uint32)
-        offset = np.zeros(t + 1, np.uint64)
-        np.cumsum(replicas, dtype=np.uint64, out=offset[1:])
-        rows = np.zeros(t, capi.REPLICA_PLAN_DTYPE)
-        total = int(offset[-1]) if want_nodes and int(offset[-1]) <= capi.KS_REPLICAS_MAX_TOTAL else 0
-        node = np.empty(total, np.int32) if want_nodes else None
-        score = np.empty(total, np.int64) if want_nodes else None
-        rc = lib.ks_place_replicas(self._h, C.byref(pods), _ptr(replicas), int(policy), _ptr(rows), _ptr(node),
-                                   _ptr(score))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_place_replicas")
+        offset, rows, node, score = replica_outputs(replicas, capi.REPLICA_PLAN_DTYPE, want_nodes)
+        check(lib.ks_place_replicas(self._h, C.byref(pods), _ptr(replicas), int(policy), _ptr(rows), _ptr(node),
+                                    _ptr(score)), "ks_place_replicas")
         return rows, node, score, offset
 
     def place_replicas_spread(self, req_cpu, req_mem, sel, replicas, node_domain, n_domains, max_skew, min_domains=None,
@@ -320,17 +300,11 @@ class Snapshot:
             if existing.shape[0] != t * d:
                 raise ValueError(f"existing has {existing.shape[0]} entries, specs x domains {t * d}")
         spread = capi.ks_spread(d, _ptr(node_domain), _ptr(max_skew), _ptr(min_domains), _ptr(existing))
-        offset = np.zeros(t + 1, np.uint64)
-        np.cumsum(replicas, dtype=np.uint64, out=offset[1:])
-        rows = np.zeros(t, capi.SPREAD_PLAN_DTYPE)
-        total = int(offset[-1]) if want_nodes and int(offset[-1]) <= capi.KS_REPLICAS_MAX_TOTAL else 0
-        node = np.empty(total, np.int32) if want_nodes else None
-        score = np.empty(total, np.int64) if want_nodes else None
+        offset, rows, node, score = replica_outputs(replicas, capi.SPREAD_PLAN_DTYPE, want_nodes)
         counts = np.empty((t, d), np.uint32) if want_counts and 0 < t * d <= capi.KS_SPREAD_MAX_COUNTS else None
-        rc = lib.ks_place_replicas_spread(self._h, C.byref(pods), _ptr(replicas), C.byref(spread), int(policy),
-                                          _ptr(rows), _ptr(node), _ptr(score), _ptr(counts))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_place_replicas_spread")
+        check(lib.ks_place_replicas_spread(self._h, C.byref(pods), _ptr(replicas), C.byref(spread), int(policy),
+                                           _ptr(rows), _ptr(node), _ptr(score), _ptr(counts)),
+              "ks_place_replicas_spread")
         return rows, node, score, offset, counts
 
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
@@ -341,10 +315,8 @@ class Snapshot:
         used = np.empty(p, np.uint32)
         dn = np.empty((p, attempts), np.int32)
         dc = np.empty((p, attempts), np.uint8)
-        rc = lib.ks_select_sampling(self._h, C.byref(pods), int(attempts), int(seed), int(first_pod_index), _ptr(idx),
-                                    _ptr(used), _ptr(dn), _ptr(dc))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_select_sampling")
+        check(lib.ks_select_sampling(self._h, C.byref(pods), int(attempts), int(seed), int(first_pod_index), _ptr(idx),
+                                     _ptr(used), _ptr(dn), _ptr(dc)), "ks_select_sampling")
         return idx, used, dn, dc
 
     def explain(self, req_cpu, req_mem, sel):
@@ -352,18 +324,15 @@ class Snapshot:
         insufficient_memory, not_enough_resources, node_selector_mismatch."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
         out = np.empty((int(pods.n), 4), np.uint32)
-        rc = lib.ks_explain(self._h, C.byref(pods), _ptr(out), capi.KS_MEM_HOST, None)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_explain")
+        check(lib.ks_explain(self._h, C.byref(pods), _ptr(out), capi.KS_MEM_HOST, None), "ks_explain")
         return out
 
     def explain_raw(self, n_pods, req_cpu, req_mem, sel, pods_space, out, out_space, stream=None):
         """Pointer-level ks_explain (torch tensors / raw addresses); out holds n_pods x 16 bytes.  The caller keeps the
         buffers alive; with device pods and output the call returns after enqueue on `stream`."""
         pods = ks_pods(int(n_pods), _ptr(req_cpu), _ptr(req_mem), _ptr(sel), int(pods_space))
-        rc = lib.ks_explain(self._h, C.byref(pods), _ptr(out), int(out_space), C.c_void_p(stream) if stream else None)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_explain")
+        check(lib.ks_explain(self._h, C.byref(pods), _ptr(out), int(out_space), C.c_void_p(stream) if stream else None),
+              "ks_explain")
 
     def select_topk(self, req_cpu, req_mem, sel, k, policy=capi.KS_SCORE_LEFTOVER):
         """The k best feasible nodes per pod (ks_select_topk) over host (numpy) pods: node_idx int32 [P, k] (-1 past the
@@ -373,10 +342,8 @@ class Snapshot:
         idx = np.empty((p, int(k)), np.int32)
         score = np.empty((p, int(k)), np.int64)
         cnt = np.empty(p, np.uint32)
-        rc = lib.ks_select_topk(self._h, C.byref(pods), int(policy), int(k), _ptr(idx), _ptr(score), _ptr(cnt),
-                                capi.KS_MEM_HOST, None)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_select_topk")
+        check(lib.ks_select_topk(self._h, C.byref(pods), int(policy), int(k), _ptr(idx), _ptr(score), _ptr(cnt),
+                                 capi.KS_MEM_HOST, None), "ks_select_topk")
         return idx, score, cnt
 
     def select_topk_raw(self, n_pods, req_cpu, req_mem, sel, pods_space, k, node_idx, score, cnt, out_space,
@@ -385,10 +352,8 @@ class Snapshot:
         n_pods (score and cnt may be None).  The caller keeps the buffers alive; with device pods and outputs the call
         returns after enqueue on `stream`."""
         pods = ks_pods(int(n_pods), _ptr(req_cpu), _ptr(req_mem), _ptr(sel), int(pods_space))
-        rc = lib.ks_select_topk(self._h, C.byref(pods), int(policy), int(k), _ptr(node_idx), _ptr(score), _ptr(cnt),
-                                int(out_space), C.c_void_p(stream) if stream else None)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_select_topk")
+        check(lib.ks_select_topk(self._h, C.byref(pods), int(policy), int(k), _ptr(node_idx), _ptr(score), _ptr(cnt),
+                                 int(out_space), C.c_void_p(stream) if stream else None), "ks_select_topk")
 
     @staticmethod
     def _bound(node_idx, req_cpu, req_mem, priority):
@@ -405,10 +370,8 @@ class Snapshot:
         p = int(pods.n)
         rows = np.empty(p, capi.PREEMPTION_DTYPE)
         victims = np.empty((p, int(max_victims)), np.int32)
-        rc = lib.ks_preempt(self._h, C.byref(pods), _ptr(priority), C.byref(bound), int(max_victims), _ptr(rows),
-                            _ptr(victims), capi.KS_MEM_HOST, None)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_preempt")
+        check(lib.ks_preempt(self._h, C.byref(pods), _ptr(priority), C.byref(bound), int(max_victims), _ptr(rows),
+                             _ptr(victims), capi.KS_MEM_HOST, None), "ks_preempt")
         return rows, victims
 
     def preempt_raw(self, n_pods, req_cpu, req_mem, sel, pods_space, priority, bound, max_victims, out, victims,
@@ -418,16 +381,12 @@ class Snapshot:
         pods and outputs the call returns after enqueue on `stream`."""
         pods = ks_pods(int(n_pods), _ptr(req_cpu), _ptr(req_mem), _ptr(sel), int(pods_space))
         b, keep_b = self._bound(*bound)
-        rc = lib.ks_preempt(self._h, C.byref(pods), _ptr(priority), C.byref(b), int(max_victims), _ptr(out),
-                            _ptr(victims), int(out_space), C.c_void_p(stream) if stream else None)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_preempt")
+        check(lib.ks_preempt(self._h, C.byref(pods), _ptr(priority), C.byref(b), int(max_victims), _ptr(out),
+                             _ptr(victims), int(out_space), C.c_void_p(stream) if stream else None), "ks_preempt")
 
     def last_timings(self):
         ms = (C.c_float * 3)()
-        rc = lib.ks_last_timings(self._h, ms)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_last_timings")
+        check(lib.ks_last_timings(self._h, ms), "ks_last_timings")
         return float(ms[0]), float(ms[1]), float(ms[2])
 
     def last_path(self):
@@ -437,9 +396,7 @@ class Snapshot:
         """Timeline of the last bit-parallel select (ks_last_trace; needs KS_TRACE=1 in the environment): microseconds
         from the start of the pod-rank kernel, {name: (start, end)}; kernels that did not run are left out."""
         ns = (C.c_uint64 * 16)()
-        rc = lib.ks_last_trace(self._h, ns)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_last_trace")
+        check(lib.ks_last_trace(self._h, ns), "ks_last_trace")
         t0 = ns[0]
         out = {}
         for name, a, b in (("pod_ranks", 0, 1), ("argmax1", 2, 3), ("argmax2", 4, 5), ("mask", 6, 7)):
@@ -452,9 +409,7 @@ class Snapshot:
 
     def exchange_check(self):
         """Synchronise and raise if a fused all-gather (ks_exchange) timed out waiting for a peer."""
-        rc = lib.ks_exchange_check(self._h)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_exchange_check")
+        check(lib.ks_exchange_check(self._h), "ks_exchange_check")
 
 
 class Stream:
@@ -462,9 +417,7 @@ class Stream:
 
     def __init__(self, snap, policy=capi.KS_SCORE_LEFTOVER, max_batch=0):
         h = C.c_void_p()
-        rc = lib.ks_stream_open(snap._h, int(policy), int(max_batch), C.byref(h))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_stream_open")
+        check(lib.ks_stream_open(snap._h, int(policy), int(max_batch), C.byref(h)), "ks_stream_open")
         self._h, self._snap = h, snap
         self._cap = 4096
         self._t = np.empty(self._cap, np.uint64)
@@ -474,23 +427,19 @@ class Stream:
     def submit(self, req_cpu, req_mem, sel, tickets):
         req_cpu, req_mem = _c(req_cpu, np.int64), _c(req_mem, np.int64)
         sel, tickets = _c(sel, np.uint64), _c(tickets, np.uint64)
-        rc = lib.ks_stream_submit(self._h, req_cpu.shape[0], _ptr(req_cpu), _ptr(req_mem), _ptr(sel), _ptr(tickets))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_stream_submit")
+        check(lib.ks_stream_submit(self._h, req_cpu.shape[0], _ptr(req_cpu), _ptr(req_mem), _ptr(sel), _ptr(tickets)),
+              "ks_stream_submit")
 
     def poll(self):
         """(tickets, node_idx, score) of the pods finished since the last poll (possibly empty); never blocks."""
         n = C.c_uint64()
-        rc = lib.ks_stream_poll(self._h, self._cap, _ptr(self._t), _ptr(self._i), _ptr(self._s), C.byref(n))
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_stream_poll")
+        check(lib.ks_stream_poll(self._h, self._cap, _ptr(self._t), _ptr(self._i), _ptr(self._s), C.byref(n)),
+              "ks_stream_poll")
         k = int(n.value)
         return self._t[:k].copy(), self._i[:k].copy(), self._s[:k].copy()
 
     def flush(self):
-        rc = lib.ks_stream_flush(self._h)
-        if rc != capi.KS_OK:
-            raise KsError(rc, "ks_stream_flush")
+        check(lib.ks_stream_flush(self._h), "ks_stream_flush")
 
     def stats(self):
         b, r, m = C.c_uint64(), C.c_uint64(), C.c_uint64()

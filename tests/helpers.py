@@ -44,3 +44,14 @@ def pack_by_dictionary(node_label_maps, pod_selector_maps):
             b = pairs.get(kv, absent)
             sel[p, b // 64] |= np.uint64(1) << np.uint64(b % 64)
     return labels, sel
+
+
+def string_list_cases(full, size=lambda s: len(s.encode()) + 1):
+    """The three buffer sizes worth checking for a string-list output (entries back to back, each NUL-terminated, -1 for
+    an entry that does not fit) whose entries, with room for all, are `full` (None = no entry), and what comes back:
+    room for all; no room; room for exactly one shorter entry that follows a longer one, which is skipped."""
+    first = next(i for i, s in enumerate(full) if s is not None)
+    k = next(i for i, s in enumerate(full) if s is not None and i > first and size(s) < size(full[first]))
+    skip = [None] * len(full)
+    skip[k] = full[k]
+    return [(sum(size(s) for s in full if s is not None), list(full)), (0, [None] * len(full)), (size(full[k]), skip)]

@@ -663,7 +663,7 @@ def test_object_level_host_layer_against_a_fake_device(tmp_path):
     assert r.returncode == 0, r.stderr
     env = {k: v for k, v in os.environ.items() if k != "PYTHONPATH"}
     r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider",
-                        "tests/test_host_layer.py", "tests/test_gpu_parity.py::test_reference_sampling_policy_faithful_objects",
+                        "tests/test_host_layer.py", "tests/test_host_calls.py", "tests/test_gpu_parity.py::test_reference_sampling_policy_faithful_objects",
                         "tests/test_gpu_parity.py::test_objects_faithful_oracle_vs_gpu", "tests/test_gpu_parity.py::test_gv1_objects_vs_faithful_oracle"],
                        cwd=str(shadow), capture_output=True, text=True, env=env, timeout=900)
     tail = r.stdout.strip().splitlines()[-1] if r.stdout.strip() else r.stderr
