@@ -8,6 +8,7 @@
 #include <cstdlib>
 #include <condition_variable>
 #include <deque>
+#include <initializer_list>
 #include <mutex>
 #include <thread>
 #include <algorithm>
@@ -43,8 +44,8 @@ struct ks_snapshot {
     uint32_t N = 0, Npad = 0, W = 1;
     DevBuf alloc_cpu, alloc_mem, free_cpu, free_mem, prio, labels, flag, xflag;
     // Staging shared by every call that holds mu until its final stream synchronise: no two are ever live, and the
-    // snapshot keeps the largest any of them needed.  d_in: host-space pods (stage_pods), bound and claim lists
-    // (stage_claims) and the host-staged calls' inputs; d_out: every host-space result, a host-space mask at 0; d_work:
+    // snapshot keeps the largest any of them needed.  d_in: host-space pods and priorities, bound and claim lists
+    // (CallerStaged) and the host-staged calls' inputs; d_out: every host-space result; d_work:
     // stream/gang, drain, scale-up and replica scratch; h_stage: the host-staged calls' pinned block (HostStaged).  A
     // call ensures each buffer once, for its whole layout, before it takes a pointer: a growing ensure frees those taken.
     HostBuf h_stage;
@@ -122,8 +123,10 @@ static int check_commit_requests(uint64_t n, const int64_t* req_cpu, const int64
 // host(); out() a result, copied to dst when dst is set and n > 0; work() device scratch in d_work.  The handle a
 // declaration returns is the only way to the array afterwards, so its offset, size and type are written once.  The
 // pinned block holds the inputs at 0 and the results at the next multiple of 16 after them.
+// block: the plan's IN, OUT, WORK (or CallerStaged::CALLER); n elements.  A CallerStaged array also keeps its row width
+// and the caller's pointer.
 template <class T>
-struct Staged { int block; size_t off; uint64_t n; }; // block: HostStaged::IN, OUT or WORK
+struct Staged { int block; size_t off; uint64_t n; uint64_t width = 1; T* caller = nullptr; };
 
 class HostStaged {
   public:
@@ -228,23 +231,136 @@ static StreamBatchArgs stream_batch_args(const ks_snapshot* s, int policy, const
     return a;
 }
 
-// The host bound or claim list of set_bound, apply_bind and commit_claims, copied to d_in on the snapshot's stream as
-// [node | cpu | mem], each array at a multiple of 256 bytes.
-struct Claims {
-    const int32_t* node;
-    const int64_t* cpu;
-    const int64_t* mem;
+// ---- caller-space calls: ks_select, ks_select_topk, ks_explain, ks_preempt, ks_check_cells / ks_check_cell,
+// ks_select_sampling, and the claim lists of set_bound, apply_bind and commit_claims ----
+// The caller says per array whether it is in host or device memory, and every array is rows of a fixed width, one row
+// per pod or claim.  Such a call declares each array once on a CallerStaged plan: in() an input, out() a result, work()
+// node-chunk partials in the call kind's own buffer.  A host-space array gets a slot at a multiple of 256 bytes, an
+// input in d_in and a result in d_out; a device-space array is used in place; an absent one (NULL) or one with no rows
+// takes no space and no copy.  Unlike HostStaged's one gathered copy, upload() and download() copy each host-space array
+// straight between the caller's memory, which may be pageable, and the device, on the call's stream, so a CUDA graph
+// can capture them.
+namespace { // file-local: none of its members is exported
+class CallerStaged {
+  public:
+    enum { IN, OUT, WORK, CALLER }; // CALLER: used in place (device-space) or absent
+    explicit CallerStaged(DevBuf* part = nullptr) : part_(part) {}
+    template <class T>
+    Staged<T> in(const T* src, uint64_t rows, uint64_t width, bool host) {
+        return add<T>(host ? IN : CALLER, const_cast<T*>(src), rows, width, -1);
+    }
+    // clear() fills a result's bytes with empty
+    template <class T>
+    Staged<T> out(T* dst, uint64_t rows, uint64_t width, bool host, uint8_t empty = 0) {
+        return add<T>(host ? OUT : CALLER, dst, rows, width, empty);
+    }
+    template <class T>
+    Staged<T> work(uint64_t rows, uint64_t width) {
+        assert(part_);
+        return add<T>(WORK, nullptr, rows, width, -1);
+    }
+    // With the snapshot locked and every array declared: ensures d_in, d_out and the partial buffer once, for the whole
+    // plan.  A growing ensure frees what the buffer held, so no pointer is handed out before this.
+    cudaError_t reserve(ks_snapshot* s) {
+        cudaError_t e = s->d_in.ensure(layout_[IN].size);
+        if (e == cudaSuccess) e = s->d_out.ensure(layout_[OUT].size);
+        if (e == cudaSuccess && part_) e = part_->ensure(layout_[WORK].size);
+        if (e != cudaSuccess) return e;
+        base_[IN] = s->d_in.p;
+        base_[OUT] = s->d_out.p;
+        base_[WORK] = part_ ? part_->p : nullptr;
+        reserved_ = true;
+        return cudaSuccess;
+    }
+    // the device array from row on; NULL when absent or empty
+    template <class T>
+    T* dev(Staged<T> a, uint64_t row = 0) const {
+        assert(reserved_);
+        T* p = a.block == CALLER ? a.caller : at<T>(base_[a.block], a.off);
+        return a.n && p ? p + row * a.width : nullptr;
+    }
+    // the caller's host destination of a host-space result from row on; NULL otherwise
+    template <class T>
+    T* host(Staged<T> a, uint64_t row = 0) const {
+        return a.block == OUT && a.n ? a.caller + row * a.width : nullptr;
+    }
+    cudaError_t upload(cudaStream_t st, uint64_t r0, uint64_t r1) const { // rows [r0, r1) of every host-space input
+        for (int i = 0; i < n_arrays_; i++) {
+            const Array& a = arrays_[i];
+            if (a.block != IN || r1 == r0) continue;
+            cudaError_t e = cudaMemcpyAsync(row(a, r0), a.caller + r0 * a.row_bytes, (r1 - r0) * a.row_bytes,
+                                            cudaMemcpyHostToDevice, st);
+            if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    }
+    // rows [r0, r1) of every host-space result, except those whose destination (from r0 on) is in served: a launcher
+    // copied them already
+    cudaError_t download(cudaStream_t st, uint64_t r0, uint64_t r1, std::initializer_list<const void*> served = {}) const {
+        for (int i = 0; i < n_arrays_; i++) {
+            const Array& a = arrays_[i];
+            unsigned char* dst = a.caller + r0 * a.row_bytes;
+            if (a.block != OUT || r1 == r0 || std::find(served.begin(), served.end(), dst) != served.end()) continue;
+            cudaError_t e = cudaMemcpyAsync(dst, row(a, r0), (r1 - r0) * a.row_bytes, cudaMemcpyDeviceToHost, st);
+            if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    }
+    cudaError_t clear(cudaStream_t st) const { // every result filled with its empty byte
+        for (int i = 0; i < n_arrays_; i++) {
+            const Array& a = arrays_[i];
+            if (a.empty < 0) continue;
+            cudaError_t e = cudaMemsetAsync(row(a, 0), a.empty, a.rows * a.row_bytes, st);
+            if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    }
+    bool any_host() const { return any_host_; } // then the call synchronises before it returns
+
+  private:
+    struct Array { int block; size_t off; unsigned char* caller; size_t row_bytes; uint64_t rows; int empty; };
+    template <class T>
+    Staged<T> add(int block, T* p, uint64_t rows, uint64_t width, int empty) {
+        any_host_ |= block == IN || block == OUT;
+        if (block != WORK && (!p || !rows)) return Staged<T>{CALLER, 0, 0, width, nullptr};
+        const size_t off = block == CALLER ? 0 : layout_[block].take<T>(rows * width, 256);
+        if (block != WORK) {
+            assert(n_arrays_ < MAX_ARRAYS);
+            arrays_[n_arrays_++] = Array{block, off, reinterpret_cast<unsigned char*>(p), width * sizeof(T), rows, empty};
+        }
+        return Staged<T>{block, off, rows * width, width, p};
+    }
+    unsigned char* row(const Array& a, uint64_t r) const {
+        return (a.block == CALLER ? a.caller : at<unsigned char>(base_[a.block], a.off)) + r * a.row_bytes;
+    }
+    static constexpr int MAX_ARRAYS = 8;
+    DevBuf* part_;
+    BlockLayout layout_[3];
+    void* base_[3] = {};
+    Array arrays_[MAX_ARRAYS];
+    int n_arrays_ = 0;
+    bool any_host_ = false;
+    bool reserved_ = false;
 };
-static int stage_claims(ks_snapshot* s, uint64_t n, const int32_t* node, const int64_t* cpu, const int64_t* mem, Claims* c) {
-    BlockLayout L;
-    const size_t o_node = L.take<int32_t>(n), o_cpu = L.take<int64_t>(n, 256), o_mem = L.take<int64_t>(n, 256);
-    CU_TRY(s->d_in.ensure(L.size));
-    void* b = s->d_in.p;
-    CU_TRY(cudaMemcpyAsync(at<int32_t>(b, o_node), node, n * 4, cudaMemcpyHostToDevice, s->stream));
-    CU_TRY(cudaMemcpyAsync(at<int64_t>(b, o_cpu), cpu, n * 8, cudaMemcpyHostToDevice, s->stream));
-    CU_TRY(cudaMemcpyAsync(at<int64_t>(b, o_mem), mem, n * 8, cudaMemcpyHostToDevice, s->stream));
-    *c = Claims{at<int32_t>(b, o_node), at<int64_t>(b, o_cpu), at<int64_t>(b, o_mem)};
-    return KS_OK;
+
+// The pods of a caller-space call, [rc | rm | sel]: one row per pod, sel W words wide.
+struct StagedPods {
+    Staged<int64_t> cpu, mem;
+    Staged<uint64_t> sel;
+    PodView view(const CallerStaged& plan, uint64_t r0, uint64_t r1) const {
+        return PodView{plan.dev(cpu, r0), plan.dev(mem, r0), plan.dev(sel, r0), (uint32_t)(r1 - r0)};
+    }
+};
+} // namespace
+static StagedPods declare_pods(CallerStaged& plan, const ks_pods* pods, uint32_t W) {
+    const bool host = pods->mem_space == KS_MEM_HOST;
+    return {plan.in(pods->req_cpu, pods->n, 1, host), plan.in(pods->req_mem, pods->n, 1, host),
+            plan.in(pods->sel, pods->n, W, host)};
+}
+
+// the caller's stream, or the snapshot's when the caller passes none
+static cudaStream_t call_stream(const ks_snapshot* s, void* cuda_stream) {
+    return cuda_stream ? (cudaStream_t)cuda_stream : s->stream.h;
 }
 
 extern "C" {
@@ -387,11 +503,13 @@ int ks_snapshot_set_bound(ks_snapshot* s, uint64_t n_bound, const int32_t* node_
     int rc = reset_free_to_alloc(s);
     if (rc) return rc;
     if (n_bound) {
-        Claims c;
-        rc = stage_claims(s, n_bound, node_idx, req_cpu, req_mem, &c);
-        if (rc) return rc;
-        CU_TRY(launch_free_reduce(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), c.node, c.cpu, c.mem, n_bound,
-                                  s->stream));
+        CallerStaged plan;
+        const auto node = plan.in(node_idx, n_bound, 1, true);
+        const auto cpu = plan.in(req_cpu, n_bound, 1, true), mem = plan.in(req_mem, n_bound, 1, true);
+        CU_TRY(plan.reserve(s));
+        CU_TRY(plan.upload(s->stream, 0, n_bound));
+        CU_TRY(launch_free_reduce(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), plan.dev(node), plan.dev(cpu),
+                                  plan.dev(mem), n_bound, s->stream));
     }
     return check_range_and_prio(s, s->stream);
 }
@@ -414,10 +532,13 @@ int ks_snapshot_apply_bind(ks_snapshot* s, int32_t node_idx, int64_t req_cpu, in
                     node_idx, (long long)nc, (long long)nm);
     s->derived_dirty = true;
     s->version++;
-    Claims c;
-    const int rc = stage_claims(s, 1, &node_idx, &req_cpu, &req_mem, &c);
-    if (rc) return rc;
-    CU_TRY(launch_free_reduce(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), c.node, c.cpu, c.mem, 1, s->stream));
+    CallerStaged plan;
+    const auto node = plan.in(&node_idx, 1, 1, true);
+    const auto cpu = plan.in(&req_cpu, 1, 1, true), mem = plan.in(&req_mem, 1, 1, true);
+    CU_TRY(plan.reserve(s));
+    CU_TRY(plan.upload(s->stream, 0, 1));
+    CU_TRY(launch_free_reduce(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), plan.dev(node), plan.dev(cpu),
+                              plan.dev(mem), 1, s->stream));
     CU_TRY(cudaStreamSynchronize(s->stream));
     return KS_OK;
 }
@@ -445,17 +566,6 @@ static int refresh_derived(ks_snapshot* s, cudaStream_t st) {
     return KS_OK;
 }
 
-// host-space pods [c0, c1) to their staging in d_in (pv, from stage_pods)
-static int copy_pods_in(const ks_pods* pods, const PodView& pv, uint32_t W, uint64_t c0, uint64_t c1, cudaStream_t st) {
-    if (pods->mem_space == KS_MEM_DEVICE) return KS_OK;
-    const uint64_t m = c1 - c0;
-    CU_TRY(cudaMemcpyAsync(const_cast<int64_t*>(pv.req_cpu) + c0, pods->req_cpu + c0, m * 8, cudaMemcpyHostToDevice, st));
-    CU_TRY(cudaMemcpyAsync(const_cast<int64_t*>(pv.req_mem) + c0, pods->req_mem + c0, m * 8, cudaMemcpyHostToDevice, st));
-    CU_TRY(cudaMemcpyAsync(const_cast<uint64_t*>(pv.sel) + c0 * W, pods->sel + c0 * W, m * 8 * W, cudaMemcpyHostToDevice,
-                           st));
-    return KS_OK;
-}
-
 static bool is_pinned_host(const void* p) {
     if (!p) return true;
     cudaPointerAttributes a;
@@ -464,28 +574,6 @@ static bool is_pinned_host(const void* p) {
         return false;
     }
     return a.type == cudaMemoryTypeHost;
-}
-
-// Host-space pods are staged in d_in as [rc | rm | sel], each array at a multiple of 256 bytes; device-space pods are
-// read in place.  Passing st == nullptr only prepares (allocates staging, fills *pv); the copies are enqueued by
-// copy_pods_in.
-static int stage_pods(ks_snapshot* s, const ks_pods* pods, cudaStream_t st, PodView* pv) {
-    const uint64_t P = pods->n;
-    pv->P = (uint32_t)P;
-    if (pods->mem_space == KS_MEM_DEVICE) {
-        pv->req_cpu = pods->req_cpu;
-        pv->req_mem = pods->req_mem;
-        pv->sel = pods->sel;
-        return KS_OK;
-    }
-    BlockLayout L;
-    const size_t o_rc = L.take<int64_t>(P), o_rm = L.take<int64_t>(P, 256), o_sel = L.take<uint64_t>(P * s->W, 256);
-    CU_TRY(s->d_in.ensure(L.size));
-    pv->req_cpu = at<int64_t>(s->d_in.p, o_rc);
-    pv->req_mem = at<int64_t>(s->d_in.p, o_rm);
-    pv->sel = at<uint64_t>(s->d_in.p, o_sel);
-    if (st == nullptr) return KS_OK; // prepare only: the caller enqueues the copies itself (copy_pods_in)
-    return copy_pods_in(pods, *pv, s->W, 0, P, st);
 }
 
 static int check_pods(const ks_snapshot* s, const ks_pods* pods) {
@@ -506,12 +594,13 @@ int ks_check_cells(ks_snapshot* s, const ks_pods* pods, uint8_t* out_codes) {
     if (cells > (1ull << 31)) return fail(KS_ERR_RANGE, "ks_check_cells is for <= 2^31 cells");
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
-    PodView pv;
-    rc = stage_pods(s, pods, s->stream, &pv);
-    if (rc) return rc;
-    CU_TRY(s->d_out.ensure(cells));
-    CU_TRY(launch_check_cells(node_table(s), pv, s->d_out.as<uint8_t>(), 0, s->N, s->stream));
-    CU_TRY(cudaMemcpyAsync(out_codes, s->d_out.p, cells, cudaMemcpyDeviceToHost, s->stream));
+    CallerStaged plan;
+    const StagedPods pd = declare_pods(plan, pods, s->W);
+    const auto codes = plan.out(out_codes, pods->n, s->N, true);
+    CU_TRY(plan.reserve(s));
+    CU_TRY(plan.upload(s->stream, 0, pods->n));
+    CU_TRY(launch_check_cells(node_table(s), pd.view(plan, 0, pods->n), plan.dev(codes), 0, s->N, s->stream));
+    CU_TRY(plan.download(s->stream, 0, pods->n));
     CU_TRY(cudaStreamSynchronize(s->stream));
     return KS_OK;
 }
@@ -521,31 +610,17 @@ int ks_check_cell(ks_snapshot* s, int64_t req_cpu, int64_t req_mem, const uint64
     if (node_idx >= s->N) return fail(KS_ERR_INVALID, "node index %u out of range", node_idx);
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
-    ks_pods pods;
-    pods.n = 1;
-    pods.req_cpu = &req_cpu;
-    pods.req_mem = &req_mem;
-    pods.sel = sel;
-    pods.mem_space = KS_MEM_HOST;
-    PodView pv;
-    int rc = stage_pods(s, &pods, s->stream, &pv);
-    if (rc) return rc;
-    CU_TRY(s->d_out.ensure(16));
-    CU_TRY(launch_check_cells(node_table(s), pv, s->d_out.as<uint8_t>(), node_idx, 1, s->stream));
+    const ks_pods pods{1, &req_cpu, &req_mem, sel, KS_MEM_HOST};
     uint8_t code = 0xff;
-    CU_TRY(cudaMemcpyAsync(&code, s->d_out.p, 1, cudaMemcpyDeviceToHost, s->stream));
+    CallerStaged plan;
+    const StagedPods pd = declare_pods(plan, &pods, s->W);
+    const auto out = plan.out(&code, 1, 1, true);
+    CU_TRY(plan.reserve(s));
+    CU_TRY(plan.upload(s->stream, 0, 1));
+    CU_TRY(launch_check_cells(node_table(s), pd.view(plan, 0, 1), plan.dev(out), node_idx, 1, s->stream));
+    CU_TRY(plan.download(s->stream, 0, 1));
     CU_TRY(cudaStreamSynchronize(s->stream));
     return (int)code;
-}
-
-// ks_select's bindings of ov's first m pods back to the host.  Each host pointer is already offset to the same pods, and
-// null when absent or already served by the launcher.
-static int copy_bindings_back(const OutView& ov, int32_t* node_idx, int64_t* score, uint32_t* cnt, uint64_t m,
-                              cudaStream_t st) {
-    if (node_idx) CU_TRY(cudaMemcpyAsync(node_idx, ov.node_idx, m * 4, cudaMemcpyDeviceToHost, st));
-    if (score) CU_TRY(cudaMemcpyAsync(score, ov.score, m * 8, cudaMemcpyDeviceToHost, st));
-    if (cnt) CU_TRY(cudaMemcpyAsync(cnt, ov.cnt, m * 4, cudaMemcpyDeviceToHost, st));
-    return KS_OK;
 }
 
 int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, ks_bindings* out, void* cuda_stream) {
@@ -576,7 +651,7 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
     if (P == 0 && !xc) return KS_OK;
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
+    const cudaStream_t st = call_stream(s, cuda_stream);
     const bool timing = (flags & KS_SELECT_TIMING) != 0;
     PeerOut po;
     if (xc) {
@@ -609,140 +684,97 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
 
     const bool out_host = out->mem_space == KS_MEM_HOST;
     const bool mask_host = out->mask && out->mask_space == KS_MEM_HOST;
-    OutView ov;
-    ov.node_idx = out->node_idx;
-    ov.score = out->score;
-    ov.cnt = out->feasible_cnt;
-    ov.mask = reinterpret_cast<uint32_t*>(out->mask);
-    ov.mask_row_words = out->mask_row_bytes / 4;
-    ov.mask_valid_words = (uint32_t)(ks_mask_row_bytes(s->N) / 4);
-    // the host destinations of the bindings; null when absent or device-space
-    int32_t* h_idx = out_host ? out->node_idx : nullptr;
-    int64_t* h_score = out_host ? out->score : nullptr;
-    uint32_t* h_cnt = out_host ? out->feasible_cnt : nullptr;
-    if (out_host || mask_host) { // staged in d_out: [mask | node_idx | score | cnt], each at a multiple of 256 bytes
-        BlockLayout D;
-        const size_t o_mask = D.take<uint8_t>(mask_host ? P * out->mask_row_bytes : 0),
-                     o_idx = D.take<int32_t>(h_idx ? P : 0, 256), o_score = D.take<int64_t>(h_score ? P : 0, 256),
-                     o_cnt = D.take<uint32_t>(h_cnt ? P : 0, 256);
-        CU_TRY(s->d_out.ensure(D.size));
-        void* b = s->d_out.p;
-        if (mask_host) ov.mask = at<uint32_t>(b, o_mask);
-        if (h_idx) ov.node_idx = at<int32_t>(b, o_idx);
-        if (h_score) ov.score = at<int64_t>(b, o_score);
-        if (h_cnt) ov.cnt = at<uint32_t>(b, o_cnt);
+    bool use_bitpar = false;
+    DirectGrid grid{};
+    if (s->N) {
+        if (flags & KS_SELECT_FORCE_BITPAR) use_bitpar = true;
+        else if (!(flags & KS_SELECT_FORCE_DIRECT))
+            use_bitpar = may_bitpar && bitpar_profitable(s->bp, (uint32_t)P);
+        if (!use_bitpar) grid = direct_grid(s->W, (uint32_t)P, s->Npad, s->sms);
     }
+    // everything that allocates happens before the (possibly captured) launch sequence; with no node, no mask row is
+    // written
+    CallerStaged plan(&s->part_sel);
+    const StagedPods pd = declare_pods(plan, pods, s->W);
+    const auto idx = plan.out(out->node_idx, P, 1, out_host, 0xff);
+    const auto score = plan.out(out->score, P, 1, out_host);
+    const auto cnt = plan.out(out->feasible_cnt, P, 1, out_host);
+    const auto mask = plan.out(reinterpret_cast<uint32_t*>(out->mask), s->N ? P : 0, out->mask_row_bytes / 4, mask_host);
+    const uint64_t part_rows = grid.n_chunks > 1 ? (uint64_t)grid.n_chunks * P : 0; // keys | indices | counts
+    const auto pkey = plan.work<int64_t>(part_rows, 1);
+    const auto pidx = plan.work<int32_t>(part_rows, 1);
+    const auto pcnt = plan.work<uint32_t>(part_rows, 1);
+    if (use_bitpar) {
+        cudaError_t e = bitpar_prepare(s->bp, (uint32_t)P);
+        if (e == cudaSuccess) e = bitpar_prepare_order(s->bp, node_table(s), policy, st);
+        if (e != cudaSuccess) return fail(KS_ERR_CUDA, "bit-parallel prepare failed: %s", cudaGetErrorString(e));
+    }
+    CU_TRY(plan.reserve(s));
 
     if (s->N == 0) { // empty node store: every pod gets None (src/main.rs:56,70)
-        if (ov.node_idx) CU_TRY(cudaMemsetAsync(ov.node_idx, 0xff, P * 4, st));
-        if (ov.score) CU_TRY(cudaMemsetAsync(ov.score, 0, P * 8, st));
-        if (ov.cnt) CU_TRY(cudaMemsetAsync(ov.cnt, 0, P * 4, st));
+        CU_TRY(plan.clear(st));
         if (xc) {
-            CU_TRY(launch_exchange_push(po, ov.node_idx, ov.score, (uint32_t)P, st));
+            CU_TRY(launch_exchange_push(po, plan.dev(idx), plan.dev(score), (uint32_t)P, st));
             CU_TRY(launch_exchange_wait(po, s->xflag.as<int>(), st));
         }
-        rc = copy_bindings_back(ov, h_idx, h_score, h_cnt, P, st);
-        if (rc) return rc;
+        CU_TRY(plan.download(st, 0, P));
         s->last_path = "empty";
     } else {
         SelectLaunch L;
         L.nt = node_table(s);
-        rc = stage_pods(s, pods, nullptr, &L.pv); // prepare; copies are part of the (possibly captured) sequence
-        if (rc) return rc;
-        L.ov = ov;
         L.policy = policy;
         L.stream = st;
         L.po = po;
-        bool use_bitpar = false;
-        if (flags & KS_SELECT_FORCE_BITPAR) use_bitpar = true;
-        else if (!(flags & KS_SELECT_FORCE_DIRECT))
-            use_bitpar = may_bitpar && bitpar_profitable(s->bp, L.pv.P);
-        // everything that allocates happens before the (possibly captured) launch sequence
-        DirectGrid grid{};
-        PartialView part{nullptr, nullptr, nullptr};
-        if (use_bitpar) {
-            cudaError_t e = bitpar_prepare(s->bp, L.pv.P);
-            if (e == cudaSuccess) e = bitpar_prepare_order(s->bp, L.nt, policy, st);
-            if (e != cudaSuccess) return fail(KS_ERR_CUDA, "bit-parallel prepare failed: %s", cudaGetErrorString(e));
-        } else {
-            grid = direct_grid(s->W, L.pv.P, s->Npad, s->sms);
-            if (grid.n_chunks > 1) { // keys | indices | counts, each [chunks*P] at a multiple of 256 bytes
-                const uint64_t rows = (uint64_t)grid.n_chunks * P;
-                BlockLayout PL;
-                const size_t o_key = PL.take<int64_t>(rows), o_idx = PL.take<int32_t>(rows, 256),
-                             o_cnt = PL.take<uint32_t>(rows, 256);
-                CU_TRY(s->part_sel.ensure(PL.size));
-                void* b = s->part_sel.p;
-                part = PartialView{at<int64_t>(b, o_key), at<int32_t>(b, o_idx), at<uint32_t>(b, o_cnt)};
-            }
-        }
+        L.ready_event = out_host ? nullptr : (cudaEvent_t)out->bindings_ready_event;
+        const PartialView part{plan.dev(pkey), plan.dev(pidx), plan.dev(pcnt)};
         s->last_path = use_bitpar ? "bitpar" : "direct";
         // Host-space batches on the bit-parallel path are pipelined in two pod chunks: the second chunk is copied in
         // on copy_stream while the first computes, and the bindings of a chunk travel back under the next chunk's
         // mask kernel.  (Each chunk is an independent select over its pod range; scratch is reused because a chunk
-        // starts only after the previous chunk's auxiliary-stream work has joined.)
+        // starts only after the previous chunk's auxiliary-stream work has joined.)  A single chunk is copied in on st.
         const uint32_t n_pipe = (use_bitpar && pods->mem_space == KS_MEM_HOST && out_host && !mask_host && !timing &&
                                  P >= 262144) // below that the per-chunk launch overhead outweighs the overlap (measured at 100k pods)
                                     ? 2u
                                     : 1u;
         auto enqueue = [&]() -> int {
-            if (n_pipe == 1) {
-                int crc = copy_pods_in(pods, L.pv, s->W, 0, P, st);
-                if (crc) return crc;
-            } else {
+            if (n_pipe > 1) {
                 CU_TRY(cudaEventRecord(s->ev_cfork, st));
                 CU_TRY(cudaStreamWaitEvent(s->copy_stream, s->ev_cfork, 0));
-                for (uint32_t c = 0; c < n_pipe; c++) {
-                    int crc = copy_pods_in(pods, L.pv, s->W, P * c / n_pipe, P * (c + 1) / n_pipe, s->copy_stream);
-                    if (crc) return crc;
-                    CU_TRY(cudaEventRecord(s->ev_in[c], s->copy_stream));
-                }
-                for (uint32_t c = 0; c < n_pipe; c++) {
-                    const uint64_t c0 = P * c / n_pipe, c1 = P * (c + 1) / n_pipe, m = c1 - c0;
-                    CU_TRY(cudaStreamWaitEvent(st, s->ev_in[c], 0));
-                    SelectLaunch Lc = L;
-                    Lc.pv.req_cpu += c0;
-                    Lc.pv.req_mem += c0;
-                    Lc.pv.sel += c0 * s->W;
-                    Lc.pv.P = (uint32_t)m;
-                    if (Lc.ov.node_idx) Lc.ov.node_idx += c0;
-                    if (Lc.ov.score) Lc.ov.score += c0;
-                    if (Lc.ov.cnt) Lc.ov.cnt += c0;
-                    if (Lc.ov.mask) Lc.ov.mask += c0 * Lc.ov.mask_row_words;
-                    Lc.host_node_idx = h_idx ? h_idx + c0 : nullptr;
-                    Lc.host_score = h_score ? h_score + c0 : nullptr;
-                    cudaError_t e = bitpar_select(s->bp, Lc, nullptr, nullptr);
+            }
+            for (uint32_t c = 0; c < n_pipe; c++) {
+                CU_TRY(plan.upload(n_pipe > 1 ? s->copy_stream.h : st, P * c / n_pipe, P * (c + 1) / n_pipe));
+                if (n_pipe > 1) CU_TRY(cudaEventRecord(s->ev_in[c], s->copy_stream));
+            }
+            for (uint32_t c = 0; c < n_pipe; c++) {
+                const uint64_t c0 = P * c / n_pipe, c1 = P * (c + 1) / n_pipe;
+                if (n_pipe > 1) CU_TRY(cudaStreamWaitEvent(st, s->ev_in[c], 0));
+                SelectLaunch Lc = L;
+                Lc.pv = pd.view(plan, c0, c1);
+                Lc.ov = OutView{plan.dev(idx, c0), plan.dev(score, c0), plan.dev(cnt, c0), plan.dev(mask, c0),
+                                out->mask_row_bytes / 4, (uint32_t)(ks_mask_row_bytes(s->N) / 4)};
+                // served early by the launcher when it can, which then clears them
+                int32_t* const h_idx = Lc.host_node_idx = plan.host(idx, c0);
+                int64_t* const h_score = Lc.host_score = plan.host(score, c0);
+                if (use_bitpar) {
+                    cudaError_t e = bitpar_select(s->bp, Lc, timing ? s->ev[1].h : nullptr, timing ? s->ev[2].h : nullptr);
                     if (e != cudaSuccess) return fail(KS_ERR_CUDA, "bit-parallel select failed: %s", cudaGetErrorString(e));
-                    int crc = copy_bindings_back(Lc.ov, Lc.host_node_idx, Lc.host_score, h_cnt ? h_cnt + c0 : nullptr, m, st);
-                    if (crc) return crc;
+                } else {
+                    if (timing) CU_TRY(cudaEventRecord(s->ev[1], st));
+                    cudaError_t e = launch_select_direct(Lc, part, grid);
+                    if (e != cudaSuccess) return fail(KS_ERR_CUDA, "direct select failed: %s", cudaGetErrorString(e));
+                    if (timing) CU_TRY(cudaEventRecord(s->ev[2], st));
+                    if (xc) CU_TRY(launch_exchange_push(po, Lc.ov.node_idx, Lc.ov.score, Lc.pv.P, st));
                 }
-                return KS_OK;
-            }
-            L.host_node_idx = h_idx; // served early by the launcher when it can
-            L.host_score = h_score;
-            L.ready_event = out_host ? nullptr : (cudaEvent_t)out->bindings_ready_event;
-            if (use_bitpar) {
-                cudaError_t e = bitpar_select(s->bp, L, timing ? s->ev[1].h : nullptr, timing ? s->ev[2].h : nullptr);
-                if (e != cudaSuccess) return fail(KS_ERR_CUDA, "bit-parallel select failed: %s", cudaGetErrorString(e));
-            } else {
-                if (timing) CU_TRY(cudaEventRecord(s->ev[1], st));
-                cudaError_t e = launch_select_direct(L, part, grid);
-                if (e != cudaSuccess) return fail(KS_ERR_CUDA, "direct select failed: %s", cudaGetErrorString(e));
-                if (timing) CU_TRY(cudaEventRecord(s->ev[2], st));
-                if (xc) CU_TRY(launch_exchange_push(po, ov.node_idx, ov.score, (uint32_t)P, st));
-            }
-            // fused all-gather: this rank's bindings went out from the argmax kernels (bit-parallel path) or the push
-            // kernel; the call's stream work ends when every other rank's bindings have arrived here
-            if (xc) CU_TRY(launch_exchange_wait(po, s->xflag.as<int>(), st));
-            int crc = copy_bindings_back(ov, L.host_node_idx, L.host_score, h_cnt, P, st);
-            if (crc) return crc;
-            if (mask_host)
-                CU_TRY(cudaMemcpyAsync(out->mask, ov.mask, P * out->mask_row_bytes, cudaMemcpyDeviceToHost, st));
-            if (L.ready_event) { // not served earlier (per-cell path): the bindings are final here
-                cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-                CU_TRY(cudaStreamIsCapturing(st, &cs));
-                CU_TRY(cudaEventRecordWithFlags(L.ready_event, st, cs == cudaStreamCaptureStatusActive ? cudaEventRecordExternal
-                                                                                                   : cudaEventRecordDefault));
+                // fused all-gather: this rank's bindings went out from the argmax kernels (bit-parallel path) or the push
+                // kernel; the call's stream work ends when every other rank's bindings have arrived here
+                if (xc) CU_TRY(launch_exchange_wait(po, s->xflag.as<int>(), st));
+                CU_TRY(plan.download(st, c0, c1, {Lc.host_node_idx ? nullptr : h_idx, Lc.host_score ? nullptr : h_score}));
+                if (Lc.ready_event) { // not served earlier (per-cell path): the bindings are final here
+                    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+                    CU_TRY(cudaStreamIsCapturing(st, &cs));
+                    CU_TRY(cudaEventRecordWithFlags(Lc.ready_event, st, cs == cudaStreamCaptureStatusActive ? cudaEventRecordExternal
+                                                                                                        : cudaEventRecordDefault));
+                }
             }
             return KS_OK;
         };
@@ -793,7 +825,7 @@ int ks_select(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t flags, k
         CU_TRY(cudaEventRecord(s->ev[3], st));
         s->timing_valid = s->N != 0;
     }
-    if (out_host || mask_host || pods->mem_space == KS_MEM_HOST || timing) CU_TRY(cudaStreamSynchronize(st));
+    if (plan.any_host() || timing) CU_TRY(cudaStreamSynchronize(st));
     return KS_OK;
 }
 
@@ -920,18 +952,19 @@ int ks_snapshot_commit_claims(ks_snapshot* s, uint64_t n, const int32_t* claim_n
     s->derived_dirty = true;
     s->version++;
     const uint32_t chunk = stream_max_claims();
-    CU_TRY(s->d_out.ensure(n));
-    Claims c;
-    rc = stage_claims(s, n, claim_node, req_cpu, req_mem, &c);
-    if (rc) return rc;
-    uint8_t* codes = s->d_out.as<uint8_t>();
+    CallerStaged plan;
+    const auto node = plan.in(claim_node, n, 1, true);
+    const auto cpu = plan.in(req_cpu, n, 1, true), mem = plan.in(req_mem, n, 1, true);
+    const auto codes = plan.out(out_accepted, n, 1, true);
+    CU_TRY(plan.reserve(s));
+    CU_TRY(plan.upload(s->stream, 0, n));
     // chunks run in arrival order on one stream: per-node arrival order is preserved across chunks
     for (uint64_t off = 0; off < n; off += chunk) {
         const uint32_t m = (uint32_t)std::min<uint64_t>(chunk, n - off);
-        CU_TRY(launch_stream_resolve(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), c.node + off, c.cpu + off,
-                                     c.mem + off, m, s->N, codes + off, s->stream));
+        CU_TRY(launch_stream_resolve(s->free_cpu.as<int64_t>(), s->free_mem.as<int64_t>(), plan.dev(node, off),
+                                     plan.dev(cpu, off), plan.dev(mem, off), m, s->N, plan.dev(codes, off), s->stream));
     }
-    CU_TRY(cudaMemcpyAsync(out_accepted, codes, n, cudaMemcpyDeviceToHost, s->stream));
+    CU_TRY(plan.download(s->stream, 0, n));
     CU_TRY(cudaStreamSynchronize(s->stream));
     return KS_OK;
 }
@@ -954,22 +987,17 @@ int ks_select_sampling(ks_snapshot* s, const ks_pods* pods, uint32_t attempts, u
         return KS_OK;
     }
     CU_TRY(cudaSetDevice(s->device));
-    PodView pv;
-    rc = stage_pods(s, pods, s->stream, &pv);
-    if (rc) return rc;
-    // one block in d_out: node_idx[P] | attempts[P] | draw_node[P*attempts] | draw_code[P*attempts]
-    BlockLayout L;
-    const size_t off_idx = L.take<int32_t>(P), off_att = L.take<uint32_t>(P), off_dn = L.take<int32_t>(draws),
-                 off_dc = L.take<uint8_t>(draws);
-    CU_TRY(s->d_out.ensure(L.size));
-    uint8_t* base = s->d_out.as<uint8_t>();
-    CU_TRY(launch_select_sampling(node_table(s), pv, attempts, seed, first_pod_index, at<int32_t>(base, off_idx),
-                                  at<uint32_t>(base, off_att), out_draw_node ? at<int32_t>(base, off_dn) : nullptr,
-                                  out_draw_code ? base + off_dc : nullptr, s->stream));
-    CU_TRY(cudaMemcpyAsync(out_node_idx, base + off_idx, P * 4, cudaMemcpyDeviceToHost, s->stream));
-    if (out_attempts) CU_TRY(cudaMemcpyAsync(out_attempts, base + off_att, P * 4, cudaMemcpyDeviceToHost, s->stream));
-    if (out_draw_node) CU_TRY(cudaMemcpyAsync(out_draw_node, base + off_dn, draws * 4, cudaMemcpyDeviceToHost, s->stream));
-    if (out_draw_code) CU_TRY(cudaMemcpyAsync(out_draw_code, base + off_dc, draws, cudaMemcpyDeviceToHost, s->stream));
+    CallerStaged plan;
+    const StagedPods pd = declare_pods(plan, pods, s->W);
+    const auto idx = plan.out(out_node_idx, P, 1, true);
+    const auto used = plan.out(out_attempts, P, 1, true);
+    const auto dn = plan.out(out_draw_node, P, attempts, true);
+    const auto dc = plan.out(out_draw_code, P, attempts, true);
+    CU_TRY(plan.reserve(s));
+    CU_TRY(plan.upload(s->stream, 0, P));
+    CU_TRY(launch_select_sampling(node_table(s), pd.view(plan, 0, P), attempts, seed, first_pod_index, plan.dev(idx),
+                                  plan.dev(used), plan.dev(dn), plan.dev(dc), s->stream));
+    CU_TRY(plan.download(s->stream, 0, P));
     CU_TRY(cudaStreamSynchronize(s->stream));
     return KS_OK;
 }
@@ -984,23 +1012,19 @@ int ks_explain(ks_snapshot* s, const ks_pods* pods, ks_pod_reasons* out, int32_t
     if (P == 0) return KS_OK;
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
-    uint32_t* d_out = reinterpret_cast<uint32_t*>(out);
-    if (out_space == KS_MEM_HOST) {
-        CU_TRY(s->d_out.ensure(P * sizeof(ks_pod_reasons)));
-        d_out = s->d_out.as<uint32_t>();
-    }
+    const cudaStream_t st = call_stream(s, cuda_stream);
+    CallerStaged plan;
+    const StagedPods pd = declare_pods(plan, pods, s->W);
+    const auto why = plan.out(reinterpret_cast<uint32_t*>(out), P, 4, out_space == KS_MEM_HOST);
+    CU_TRY(plan.reserve(s));
     if (s->N == 0) {
-        CU_TRY(cudaMemsetAsync(d_out, 0, P * sizeof(ks_pod_reasons), st));
+        CU_TRY(plan.clear(st));
     } else {
-        PodView pv;
-        rc = stage_pods(s, pods, st, &pv);
-        if (rc) return rc;
-        CU_TRY(launch_explain_counts(node_table(s), pv, d_out, s->sms, st));
+        CU_TRY(plan.upload(st, 0, P));
+        CU_TRY(launch_explain_counts(node_table(s), pd.view(plan, 0, P), plan.dev(why), s->sms, st));
     }
-    if (out_space == KS_MEM_HOST)
-        CU_TRY(cudaMemcpyAsync(out, d_out, P * sizeof(ks_pod_reasons), cudaMemcpyDeviceToHost, st));
-    if (out_space == KS_MEM_HOST || pods->mem_space == KS_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
+    CU_TRY(plan.download(st, 0, P));
+    if (plan.any_host()) CU_TRY(cudaStreamSynchronize(st));
     return KS_OK;
 }
 
@@ -1016,46 +1040,29 @@ int ks_select_topk(ks_snapshot* s, const ks_pods* pods, int policy, uint32_t k, 
     if (P == 0) return KS_OK;
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
-    const uint64_t cells = P * k;
-    OutView ov{out_node_idx, out_score, out_feasible_cnt, nullptr, 0, 0};
-    if (out_space == KS_MEM_HOST) { // one block in d_out: score [P*k] | node_idx [P*k] | feasible_cnt [P]
-        BlockLayout L;
-        const size_t o_score = L.take<int64_t>(cells), o_idx = L.take<int32_t>(cells), o_cnt = L.take<uint32_t>(P);
-        CU_TRY(s->d_out.ensure(L.size));
-        void* b = s->d_out.p;
-        ov.score = out_score ? at<int64_t>(b, o_score) : nullptr;
-        ov.node_idx = at<int32_t>(b, o_idx);
-        ov.cnt = out_feasible_cnt ? at<uint32_t>(b, o_cnt) : nullptr;
-    }
+    const cudaStream_t st = call_stream(s, cuda_stream);
+    const bool host = out_space == KS_MEM_HOST;
+    const DirectGrid g = s->N ? direct_grid(s->W, (uint32_t)P, s->Npad, s->sms) : DirectGrid{};
+    const uint64_t part_rows = g.n_chunks > 1 ? (uint64_t)g.n_chunks * P : 0; // keys | indices | counts
+    CallerStaged plan(&s->part_topk);
+    const StagedPods pd = declare_pods(plan, pods, s->W);
+    const auto idx = plan.out(out_node_idx, P, k, host, 0xff);
+    const auto score = plan.out(out_score, P, k, host);
+    const auto cnt = plan.out(out_feasible_cnt, P, 1, host);
+    const auto pkey = plan.work<int64_t>(part_rows, k);
+    const auto pidx = plan.work<int32_t>(part_rows, k);
+    const auto pcnt = plan.work<uint32_t>(part_rows, 1);
+    CU_TRY(plan.reserve(s));
     if (s->N == 0) { // no node: every slot is empty
-        CU_TRY(cudaMemsetAsync(ov.node_idx, 0xff, cells * 4, st));
-        if (ov.score) CU_TRY(cudaMemsetAsync(ov.score, 0, cells * 8, st));
-        if (ov.cnt) CU_TRY(cudaMemsetAsync(ov.cnt, 0, P * 4, st));
+        CU_TRY(plan.clear(st));
     } else {
-        PodView pv;
-        rc = stage_pods(s, pods, st, &pv);
-        if (rc) return rc;
-        const DirectGrid g = direct_grid(s->W, pv.P, s->Npad, s->sms);
-        PartialView part{nullptr, nullptr, nullptr};
-        if (g.n_chunks > 1) { // keys [chunks*P*k] | indices [chunks*P*k] | counts [chunks*P]
-            const uint64_t rows = (uint64_t)g.n_chunks * P;
-            BlockLayout L;
-            const size_t o_key = L.take<int64_t>(rows * k), o_idx = L.take<int32_t>(rows * k), o_cnt = L.take<uint32_t>(rows);
-            CU_TRY(s->part_topk.ensure(L.size));
-            void* b = s->part_topk.p;
-            part.key = at<int64_t>(b, o_key);
-            part.idx = at<int32_t>(b, o_idx);
-            part.cnt = at<uint32_t>(b, o_cnt);
-        }
-        CU_TRY(launch_select_topk(node_table(s), pv, policy, k, ov, part, g, st));
+        CU_TRY(plan.upload(st, 0, P));
+        const OutView ov{plan.dev(idx), plan.dev(score), plan.dev(cnt), nullptr, 0, 0};
+        const PartialView part{plan.dev(pkey), plan.dev(pidx), plan.dev(pcnt)};
+        CU_TRY(launch_select_topk(node_table(s), pd.view(plan, 0, P), policy, k, ov, part, g, st));
     }
-    if (out_space == KS_MEM_HOST) {
-        CU_TRY(cudaMemcpyAsync(out_node_idx, ov.node_idx, cells * 4, cudaMemcpyDeviceToHost, st));
-        if (out_score) CU_TRY(cudaMemcpyAsync(out_score, ov.score, cells * 8, cudaMemcpyDeviceToHost, st));
-        if (out_feasible_cnt) CU_TRY(cudaMemcpyAsync(out_feasible_cnt, ov.cnt, P * 4, cudaMemcpyDeviceToHost, st));
-    }
-    if (out_space == KS_MEM_HOST || pods->mem_space == KS_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
+    CU_TRY(plan.download(st, 0, P));
+    if (plan.any_host()) CU_TRY(cudaStreamSynchronize(st));
     return KS_OK;
 }
 
@@ -1104,32 +1111,21 @@ int ks_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* pod_priority,
     rc = check_preempt_bound(s, bound);
     if (rc) return rc;
     CU_TRY(cudaSetDevice(s->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
-    const uint64_t n_vic = out_victims ? P * max_victims : 0;
-    ks_preemption* d_out = out;
-    int32_t* d_vic = out_victims;
-    const int32_t* d_prio = pod_priority;
-    // one block in d_out when outputs or pods are host-space: rows [P] | victims [P * max_victims] (host-space outputs) |
-    // priorities [P] (host-space pods)
-    BlockLayout L;
-    const size_t o_rows = L.take<ks_preemption>(P), o_vic = L.take<int32_t>(n_vic), o_prio = L.take<int32_t>(P);
-    if (out_space == KS_MEM_HOST || pods->mem_space == KS_MEM_HOST) CU_TRY(s->d_out.ensure(L.size));
-    void* stg = s->d_out.p;
-    if (out_space == KS_MEM_HOST) {
-        d_out = at<ks_preemption>(stg, o_rows);
-        d_vic = out_victims ? at<int32_t>(stg, o_vic) : nullptr;
-    }
-    PodView pv{nullptr, nullptr, nullptr, (uint32_t)P};
+    const cudaStream_t st = call_stream(s, cuda_stream);
+    const bool host = out_space == KS_MEM_HOST;
+    const DirectGrid g = s->N ? direct_grid(s->W, (uint32_t)P, s->Npad, s->sms) : DirectGrid{};
+    const uint64_t part_rows = (uint64_t)g.n_chunks * P; // hi | lo | candidates | feasible
+    CallerStaged plan(&s->part_pre);
+    const StagedPods pd = declare_pods(plan, pods, s->W);
+    const auto prio = plan.in(pod_priority, P, 1, pods->mem_space == KS_MEM_HOST);
+    const auto rows = plan.out(out, P, 1, host);
+    const auto vic = plan.out(out_victims, P, max_victims, host);
+    const auto hi = plan.work<uint64_t>(part_rows, 1), lo = plan.work<uint64_t>(part_rows, 1);
+    const auto cand = plan.work<uint32_t>(part_rows, 1), cnt = plan.work<uint32_t>(part_rows, 1);
+    CU_TRY(plan.reserve(s));
     VictimIndex vx{};
-    PreemptPartials part{};
-    DirectGrid g{};
     if (s->N) {
-        rc = stage_pods(s, pods, st, &pv);
-        if (rc) return rc;
-        if (pods->mem_space == KS_MEM_HOST) {
-            CU_TRY(cudaMemcpyAsync(at<int32_t>(stg, o_prio), pod_priority, P * 4, cudaMemcpyHostToDevice, st));
-            d_prio = at<int32_t>(stg, o_prio);
-        }
+        CU_TRY(plan.upload(st, 0, P));
         // the victim index: upload the bound list, sort it by (node, priority), prefix sums per node
         CU_TRY(s->vx_pre.ensure(victim_index_bytes(B, s->N)));
         if (B) {
@@ -1140,24 +1136,12 @@ int ks_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* pod_priority,
             CU_TRY(cudaMemcpyAsync(up.prio, bound->priority, B * 4, cudaMemcpyHostToDevice, st));
         }
         CU_TRY(build_victim_index(s->vx_pre.p, B, s->N, &vx, st));
-        g = direct_grid(s->W, pv.P, s->Npad, s->sms);
-        const uint64_t rows = (uint64_t)g.n_chunks * P; // hi [rows] | lo [rows] | candidates [rows] | feasible [rows]
-        BlockLayout PL;
-        const size_t o_hi = PL.take<uint64_t>(rows), o_lo = PL.take<uint64_t>(rows), o_cand = PL.take<uint32_t>(rows),
-                     o_cnt = PL.take<uint32_t>(rows);
-        CU_TRY(s->part_pre.ensure(PL.size));
-        void* b = s->part_pre.p;
-        part.hi = at<uint64_t>(b, o_hi);
-        part.lo = at<uint64_t>(b, o_lo);
-        part.cand = at<uint32_t>(b, o_cand);
-        part.cnt = at<uint32_t>(b, o_cnt);
     }
-    CU_TRY(launch_preempt(node_table(s), pv, d_prio, vx, max_victims, part, g, d_out, d_vic, st));
-    if (out_space == KS_MEM_HOST) {
-        CU_TRY(cudaMemcpyAsync(out, d_out, P * sizeof(ks_preemption), cudaMemcpyDeviceToHost, st));
-        if (out_victims) CU_TRY(cudaMemcpyAsync(out_victims, d_vic, n_vic * 4, cudaMemcpyDeviceToHost, st));
-    }
-    if (out_space == KS_MEM_HOST || pods->mem_space == KS_MEM_HOST) CU_TRY(cudaStreamSynchronize(st));
+    const PreemptPartials part{plan.dev(hi), plan.dev(lo), plan.dev(cand), plan.dev(cnt)};
+    CU_TRY(launch_preempt(node_table(s), pd.view(plan, 0, P), plan.dev(prio), vx, max_victims, part, g, plan.dev(rows),
+                          plan.dev(vic), st));
+    CU_TRY(plan.download(st, 0, P));
+    if (plan.any_host()) CU_TRY(cudaStreamSynchronize(st));
     return KS_OK;
 }
 
