@@ -47,6 +47,7 @@ pub const KS_REPLICAS_MAX_TOTAL: u32 = 1 << 24; // most copies of one ks_place_r
 pub const KS_SPREAD_MAX_DOMAINS: u32 = 1 << 20; // most topology domains of one ks_place_replicas_spread call
 pub const KS_SPREAD_MAX_EXISTING: u32 = 1 << 24; // most existing pods counted in one domain
 pub const KS_SPREAD_MAX_COUNTS: u64 = 1 << 26; // most specs x domains of existing or output counts
+pub const KS_SPREAD_MAX_KEYS: u32 = 4; // most topology keys of one ks_place_replicas_spread_multi call
 
 #[repr(C)]
 pub struct ks_kv {
@@ -192,6 +193,15 @@ pub struct ks_spread {
     pub existing: *const u32,
 }
 #[repr(C)]
+pub struct ks_spread_multi {
+    pub n_keys: u32,
+    pub n_domains: [u32; KS_SPREAD_MAX_KEYS as usize],
+    pub node_domain: [*const i32; KS_SPREAD_MAX_KEYS as usize],
+    pub max_skew: *const u32,
+    pub min_domains: *const u32,
+    pub existing: *const u32,
+}
+#[repr(C)]
 #[derive(Clone, Copy, Default, Debug)]
 pub struct ks_spread_plan {
     pub placed: u32,
@@ -243,6 +253,9 @@ extern "C" {
     pub fn ks_place_replicas_spread(s: *mut ks_snapshot, specs: *const ks_pods, replicas: *const u32, spread: *const ks_spread,
                                     policy: c_int, out: *mut ks_spread_plan, node: *mut i32, score: *mut i64,
                                     domain_count: *mut u32) -> c_int;
+    pub fn ks_place_replicas_spread_multi(s: *mut ks_snapshot, specs: *const ks_pods, replicas: *const u32,
+                                          spread: *const ks_spread_multi, policy: c_int, out: *mut ks_spread_plan,
+                                          node: *mut i32, score: *mut i64, domain_count: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -300,6 +313,11 @@ extern "C" {
                                      existing_node_names: *const *const c_char, existing_offset: *const u64, policy: c_int,
                                      out: *mut ks_spread_plan, node: *mut i32, score: *mut i64,
                                      domain_count: *mut u32) -> c_int;
+    pub fn ksh_place_replicas_spread_multi(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, replicas: *const u32,
+                                           topology_keys: *const *const c_char, n_keys: u32, max_skew: *const u32,
+                                           min_domains: *const u32, existing_node_names: *const *const c_char,
+                                           existing_offset: *const u64, policy: c_int, out: *mut ks_spread_plan,
+                                           node: *mut i32, score: *mut i64, domain_count: *mut u32) -> c_int;
     pub fn ksh_drain_nodes(ctx: *mut ksh_context, node_names: *const *const c_char, n: u64, pods: *const ks_pod_obj,
                            pod_offset: *const u64, policy: c_int, flags: u32, placed: *mut u32, node_idx: *mut i32) -> c_int;
     pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,

@@ -593,6 +593,55 @@ int ks_place_replicas_spread(ks_snapshot* s, const ks_pods* specs /* host space 
                              int32_t* out_node /* [sum replicas] or NULL */, int64_t* out_score /* [sum replicas] or NULL */,
                              uint32_t* out_domain_count /* [specs->n * D] or NULL */);
 
+/* ---- topology spread over several keys: the same placement when every spec carries one constraint per topology key,
+ * such as topology.kubernetes.io/zone and kubernetes.io/hostname together (upstream: a node must pass every constraint
+ * the pod carries; DESIGN.md 5l) ----
+ * K = n_keys keys, 1 <= K <= KS_SPREAD_MAX_KEYS.  Key k has D_k = n_domains[k] dense domains and its own
+ * node_domain[k][N] (-1 = node lacks the key).  Spec t carries one constraint per key: max_skew[t * K + k] >= 1,
+ * min_domains[t * K + k] and existing counts.  Specs with different key sets go in different calls.  S = sum of D_k,
+ * P_k = D_0 + ... + D_{k-1}.  For spec t:
+ *   1. node n is eligible when node_domain[k][n] >= 0 for every k and the spec's selector matches it (nodes without all
+ *      the keys are neither counted nor chosen); resource fit plays no part.  E_{t,k} = the key-k domains that hold an
+ *      eligible node;
+ *   2. cnt_k[d] starts at existing[t * S + P_k + d] (existing NULL: zeros);
+ *   3. m_k = min of cnt_k over E_{t,k}, or 0 when |E_{t,k}| < min_domains[t * K + k].  No eligible node: nothing is placed;
+ *   4. copy r goes to the eligible node with j_n < c_n and the highest s_n(j_n) such that, for every k,
+ *      cnt_k[d_k(n)] + 1 - m_k <= max_skew[t * K + k]; ties to the lower node index (c_n and s_n(j) as ks_place_replicas
+ *      defines them, every policy).  Then j_n, every cnt_k[d_k(n)] and every m_k are updated.  The first copy with no
+ *      candidate stops the spec; the rest get node -1 and score 0;
+ *   5. out[t * K + k] is a ks_spread_plan: placed, nodes, max_per_node and last_score describe spec t and are the same
+ *      in all K of its rows; eligible_domains = |E_{t,k}|; min_count = m_k after the last copy; blocked_domain = the
+ *      lowest domain of E_{t,k} that key k's own rule still admits and that holds no eligible node with room (j_n < c_n)
+ *      admitted by every other constraint: the lowest domain of key k where capacity and the other keys, not k's own
+ *      rule, stop the copies.  -1 when every copy was placed or no such domain exists;
+ *   6. out_node / out_score as in ks_place_replicas; out_domain_count[t * S + P_k + d] = the final cnt_k[d].  Each may
+ *      be NULL;
+ *   7. nothing is charged; committing a spec's out_node slice with ks_snapshot_commit_claims accepts every claim.
+ * K = 1 is exactly ks_place_replicas_spread (the same rows, copies and counts).
+ * Checks on the host before any device work: those of ks_place_replicas_spread, per key; KS_ERR_INVALID for a NULL
+ * spread, max_skew or node_domain[k] with k < K; KS_ERR_RANGE for K outside [1, KS_SPREAD_MAX_KEYS], or T * S >
+ * KS_SPREAD_MAX_COUNTS when existing or out_domain_count is given.  An empty snapshot gives every row zeros with
+ * blocked_domain = -1, every copy -1, and counts = existing.
+ * Host-space arguments and outputs.  One H2D copy; one kernel orders the nodes by domain, one CTA per key; then one CTA
+ * per spec places its copies one after another, as ks_place_replicas_spread; one D2H copy.  Staging as
+ * ks_place_replicas_spread, with 4 bytes per node and key, 4 * T * S bytes of existing counts and of counts, 32 * T * K
+ * bytes of rows; device scratch 16 bytes per node and key for the orders, and per CTA also 8 bytes per secondary domain
+ * and 4 per 1024-node block slot of the primary. */
+#define KS_SPREAD_MAX_KEYS 4u
+typedef struct ks_spread_multi {                      /* host memory */
+    uint32_t n_keys;                                  /* K */
+    uint32_t n_domains[KS_SPREAD_MAX_KEYS];           /* D_k, k < K */
+    const int32_t* node_domain[KS_SPREAD_MAX_KEYS];   /* [N] each, in [-1, D_k) */
+    const uint32_t* max_skew;                         /* [T * K], each >= 1 */
+    const uint32_t* min_domains;                      /* [T * K] or NULL */
+    const uint32_t* existing;                         /* [T * S] or NULL */
+} ks_spread_multi;
+int ks_place_replicas_spread_multi(ks_snapshot* s, const ks_pods* specs /* host space */,
+                                   const uint32_t* replicas /* [n] */, const ks_spread_multi* spread, int policy,
+                                   ks_spread_plan* out /* [specs->n * K] */, int32_t* out_node /* [sum replicas] or NULL */,
+                                   int64_t* out_score /* [sum replicas] or NULL */,
+                                   uint32_t* out_domain_count /* [specs->n * S] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -240,6 +240,21 @@ int ksh_place_replicas_spread(ksh_context* ctx, const ks_pod_obj* pods, uint64_t
                               const char* const* existing_node_names, const uint64_t* existing_offset, int policy,
                               ks_spread_plan* out, int32_t* out_node, int64_t* out_score, uint32_t* out_domain_count);
 
+/* The same over n_keys topology keys at once (ks_place_replicas_spread_multi, ksched.h), such as
+ * topology.kubernetes.io/zone and kubernetes.io/hostname: key k is topology_keys[k], numbered as
+ * ksh_context_topology_domains numbers it; max_skew [n * K] and min_domains [n * K] (or NULL) per (spec, key).  Spec t's
+ * existing pods under key k are existing_node_names[existing_offset[t * K + k] .. existing_offset[t * K + k + 1])
+ * (existing_offset [n * K + 1] or NULL); a name counts when it is in the store and its node carries every key of the
+ * call.  Outputs as ks_place_replicas_spread_multi gives them (out [n * K], out_domain_count [n * S]).  With a key that
+ * no node carries, every row is empty and out_domain_count is not written.  K = 1 gives exactly what
+ * ksh_place_replicas_spread gives.  KS_ERR_RANGE for n_keys outside [1, KS_SPREAD_MAX_KEYS]; KS_ERR_NO_DEVICE on a
+ * packing-only context. */
+int ksh_place_replicas_spread_multi(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n, const uint32_t* replicas,
+                                    const char* const* topology_keys, uint32_t n_keys, const uint32_t* max_skew,
+                                    const uint32_t* min_domains, const char* const* existing_node_names,
+                                    const uint64_t* existing_offset, int policy, ks_spread_plan* out, int32_t* out_node,
+                                    int64_t* out_score, uint32_t* out_domain_count);
+
 #ifdef __cplusplus
 }
 #endif

@@ -206,6 +206,17 @@ _proto("ks_place_replicas_spread", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_
 KS_SPREAD_MAX_DOMAINS = 1 << 20
 KS_SPREAD_MAX_EXISTING = 1 << 24
 KS_SPREAD_MAX_COUNTS = 1 << 26
+KS_SPREAD_MAX_KEYS = 4
+
+
+class ks_spread_multi(C.Structure):
+    _fields_ = [("n_keys", C.c_uint32), ("n_domains", C.c_uint32 * KS_SPREAD_MAX_KEYS),
+                ("node_domain", C.c_void_p * KS_SPREAD_MAX_KEYS), ("max_skew", C.c_void_p), ("min_domains", C.c_void_p),
+                ("existing", C.c_void_p)]
+
+
+_proto("ks_place_replicas_spread_multi", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p,
+       C.POINTER(ks_spread_multi), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
 KS_PREEMPT_MAX_ABS_SUM = 1 << 62
 KS_ERR_INVALID, KS_ERR_RANGE = -1, -5
 KS_REFERENCE_ATTEMPTS = 5

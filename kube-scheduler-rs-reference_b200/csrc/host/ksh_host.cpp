@@ -22,7 +22,8 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 // ks_explain, ks_select_topk, ks_preempt, ks_gang_bind, ks_drain_check and ks_scaleup_estimate are defined by the CUDA
 // core in the same library.  The references are weak so that this file still links with device stand-ins that only
 // provide the older ks_* entries (tests/native); ksh_explain_pods, ksh_rank_nodes, ksh_preempt_pods, ksh_reconcile_gangs,
-// ksh_drain_nodes, ksh_scaleup_estimate, ksh_place_replicas and ksh_place_replicas_spread then report KS_ERR_NO_DEVICE.
+// ksh_drain_nodes, ksh_scaleup_estimate, ksh_place_replicas and ksh_place_replicas_spread (and _multi) then report
+// KS_ERR_NO_DEVICE.
 #pragma weak ks_explain
 #pragma weak ks_select_topk
 #pragma weak ks_preempt
@@ -31,6 +32,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 #pragma weak ks_scaleup_estimate
 #pragma weak ks_place_replicas
 #pragma weak ks_place_replicas_spread
+#pragma weak ks_place_replicas_spread_multi
 
 namespace {
 
@@ -1619,40 +1621,91 @@ int ksh_context_topology_domains(const ksh_context* c, const char* key, int32_t*
 }
 KSH_CATCH
 
-int ksh_place_replicas_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const uint32_t* replicas,
-                              const char* topology_key, const uint32_t* max_skew, const uint32_t* min_domains,
-                              const char* const* existing_node_names, const uint64_t* existing_offset, int policy,
-                              ks_spread_plan* out, int32_t* out_node, int64_t* out_score, uint32_t* out_domain_count) try {
-    if (!c || !topology_key || (n && (!pods || !replicas || !max_skew || !out))) return fail(KS_ERR_INVALID, "NULL argument");
-    if (existing_offset && existing_offset[n] && !existing_node_names) return fail(KS_ERR_INVALID, "NULL existing_node_names");
+// ksh_place_replicas_spread (multi = false, K = 1) and ksh_place_replicas_spread_multi: existing_offset[t * K + k]
+// indexes spec t's existing pods under key k.  A name counts when it is in the store and its node carries every key.
+static int place_spread_objects(ksh_context* c, bool multi, const ks_pod_obj* pods, uint64_t n, const uint32_t* replicas,
+                                const char* const* keys, uint32_t K, const uint32_t* max_skew, const uint32_t* min_domains,
+                                const char* const* existing_node_names, const uint64_t* existing_offset, int policy,
+                                ks_spread_plan* out, int32_t* out_node, int64_t* out_score, uint32_t* out_domain_count) {
+    if (!c || !keys || (n && (!pods || !replicas || !max_skew || !out))) return fail(KS_ERR_INVALID, "NULL argument");
+    if (K == 0 || K > KS_SPREAD_MAX_KEYS)
+        return fail(KS_ERR_RANGE, std::to_string(K) + " topology keys (1 to " + std::to_string(KS_SPREAD_MAX_KEYS) + ")");
+    for (uint32_t k = 0; k < K; k++)
+        if (!keys[k]) return fail(KS_ERR_INVALID, "NULL argument");
+    const uint64_t nk = n * K;
+    if (existing_offset && existing_offset[nk] && !existing_node_names) return fail(KS_ERR_INVALID, "NULL existing_node_names");
     if (existing_offset)
-        for (uint64_t t = 0; t < n; t++)
-            if (existing_offset[t + 1] < existing_offset[t]) return fail(KS_ERR_INVALID, "existing offsets decrease");
+        for (uint64_t i = 0; i < nk; i++)
+            if (existing_offset[i + 1] < existing_offset[i]) return fail(KS_ERR_INVALID, "existing offsets decrease");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    int rc = device_ready(c, ks_place_replicas_spread, "ks_place_replicas_spread");
+    int rc = multi ? device_ready(c, ks_place_replicas_spread_multi, "ks_place_replicas_spread_multi")
+                   : device_ready(c, ks_place_replicas_spread, "ks_place_replicas_spread");
     if (rc) return rc;
     if (n == 0) return KS_OK;
     ks_pods kp;
     rc = pack_batch(c, pods, n, &kp);
     if (rc) return rc;
-    std::vector<int32_t> dom(c->N);
-    std::vector<uint32_t> values;
-    const uint32_t D = topology_domains(c, topology_key, dom.data(), &values);
-    // no node carries the key: no domain is eligible, and a single empty domain gives exactly that
-    const uint32_t Dc = std::max(D, 1u);
+    std::vector<std::vector<int32_t>> dom(K, std::vector<int32_t>(c->N));
+    uint32_t Dc[KS_SPREAD_MAX_KEYS] = {}, P[KS_SPREAD_MAX_KEYS] = {};
+    uint64_t S = 0;
+    bool keyless = false;
+    for (uint32_t k = 0; k < K; k++) {
+        std::vector<uint32_t> values;
+        const uint32_t D = topology_domains(c, keys[k], dom[k].data(), &values);
+        keyless |= D == 0;
+        // no node carries the key: no domain is eligible, and a single empty domain gives exactly that
+        Dc[k] = std::max(D, 1u);
+        P[k] = (uint32_t)S;
+        S += Dc[k];
+    }
     std::vector<uint32_t> existing;
     if (existing_offset) {
-        if (n * Dc > KS_SPREAD_MAX_COUNTS) return fail(KS_ERR_RANGE, "too many specs x domains of existing counts (at most 2^26)");
-        existing.assign(n * Dc, 0);
+        if (n * S > KS_SPREAD_MAX_COUNTS) return fail(KS_ERR_RANGE, "too many specs x domains of existing counts (at most 2^26)");
+        existing.assign(n * S, 0);
         for (uint64_t t = 0; t < n; t++)
-            for (uint64_t i = existing_offset[t]; i < existing_offset[t + 1]; i++) {
-                const int32_t idx = existing_node_names[i] ? node_index_of(c, existing_node_names[i]) : -1;
-                if (idx >= 0 && dom[idx] >= 0) existing[t * Dc + (uint32_t)dom[idx]]++; // unknown or keyless: not counted
-            }
+            for (uint32_t k = 0; k < K; k++)
+                for (uint64_t i = existing_offset[t * K + k]; i < existing_offset[t * K + k + 1]; i++) {
+                    const int32_t idx = existing_node_names[i] ? node_index_of(c, existing_node_names[i]) : -1;
+                    if (idx < 0) continue; // unknown: not counted
+                    bool all = true;
+                    for (uint32_t k2 = 0; k2 < K; k2++) all &= dom[k2][idx] >= 0;
+                    if (all) existing[t * S + P[k] + (uint32_t)dom[k][idx]]++; // keyless: not counted
+                }
     }
-    ks_spread sp{Dc, dom.data(), max_skew, min_domains, existing_offset ? existing.data() : nullptr};
-    return ks_place_replicas_spread(c->snap, &kp, replicas, &sp, policy, out, out_node, out_score,
-                                    D ? out_domain_count : nullptr);
+    uint32_t* counts = keyless ? nullptr : out_domain_count;
+    if (!multi) {
+        ks_spread sp{Dc[0], dom[0].data(), max_skew, min_domains, existing_offset ? existing.data() : nullptr};
+        return ks_place_replicas_spread(c->snap, &kp, replicas, &sp, policy, out, out_node, out_score, counts);
+    }
+    ks_spread_multi sp{};
+    sp.n_keys = K;
+    for (uint32_t k = 0; k < K; k++) {
+        sp.n_domains[k] = Dc[k];
+        sp.node_domain[k] = dom[k].data();
+    }
+    sp.max_skew = max_skew;
+    sp.min_domains = min_domains;
+    sp.existing = existing_offset ? existing.data() : nullptr;
+    return ks_place_replicas_spread_multi(c->snap, &kp, replicas, &sp, policy, out, out_node, out_score, counts);
+}
+
+int ksh_place_replicas_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const uint32_t* replicas,
+                              const char* topology_key, const uint32_t* max_skew, const uint32_t* min_domains,
+                              const char* const* existing_node_names, const uint64_t* existing_offset, int policy,
+                              ks_spread_plan* out, int32_t* out_node, int64_t* out_score, uint32_t* out_domain_count) try {
+    return place_spread_objects(c, false, pods, n, replicas, topology_key ? &topology_key : nullptr, 1, max_skew,
+                                min_domains, existing_node_names, existing_offset, policy, out, out_node, out_score,
+                                out_domain_count);
+}
+KSH_CATCH
+
+int ksh_place_replicas_spread_multi(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const uint32_t* replicas,
+                                    const char* const* topology_keys, uint32_t n_keys, const uint32_t* max_skew,
+                                    const uint32_t* min_domains, const char* const* existing_node_names,
+                                    const uint64_t* existing_offset, int policy, ks_spread_plan* out, int32_t* out_node,
+                                    int64_t* out_score, uint32_t* out_domain_count) try {
+    return place_spread_objects(c, true, pods, n, replicas, topology_keys, n_keys, max_skew, min_domains,
+                                existing_node_names, existing_offset, policy, out, out_node, out_score, out_domain_count);
 }
 KSH_CATCH
 

@@ -116,7 +116,7 @@ static int check_commit_requests(uint64_t n, const int64_t* req_cpu, const int64
 }
 
 // ---- host-staged calls: ks_stream_bind's device loop, ks_gang_bind, ks_drain_check, ks_scaleup_estimate,
-// ks_place_replicas and ks_place_replicas_spread ----
+// ks_place_replicas and ks_place_replicas_spread (and _multi) ----
 // Such a call gathers its host inputs into the snapshot's pinned block, makes one H2D copy to d_in, launches, makes one
 // D2H copy from d_out and copies its results out before it returns.  Its HostStaged plan declares every array it stages
 // once, with its type and count: in() an input, gathered from src or, with src NULL, filled by the caller through
@@ -1614,33 +1614,45 @@ int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* repl
     return KS_OK;
 }
 
-int ks_place_replicas_spread(ks_snapshot* s, const ks_pods* specs, const uint32_t* replicas, const ks_spread* spread,
-                             int policy, ks_spread_plan* out, int32_t* out_node, int64_t* out_score,
-                             uint32_t* out_domain_count) {
+// ks_place_replicas_spread is the K = 1 case of ks_place_replicas_spread_multi: one argument check, one staging plan
+// and one launcher for both.
+static int place_spread(ks_snapshot* s, const char* call, const ks_pods* specs, const uint32_t* replicas,
+                        const ks_spread_multi* spread, int policy, ks_spread_plan* out, int32_t* out_node,
+                        int64_t* out_score, uint32_t* out_domain_count) {
     uint64_t total;
-    int rc = check_replica_specs(s, "ks_place_replicas_spread", specs, replicas, out, policy, &total);
+    int rc = check_replica_specs(s, call, specs, replicas, out, policy, &total);
     if (rc) return rc;
     const uint64_t T = specs->n;
-    if (!spread || !spread->node_domain || !spread->max_skew) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
-    const uint32_t D = spread->n_domains, N = s->N;
-    if (D == 0 || D > KS_SPREAD_MAX_DOMAINS) return fail(KS_ERR_RANGE, "%u domains (1 to %u)", D, KS_SPREAD_MAX_DOMAINS);
-    for (uint32_t n = 0; n < N; n++)
-        if (spread->node_domain[n] < -1 || spread->node_domain[n] >= (int64_t)D)
-            return fail(KS_ERR_INVALID, "node %u: domain %d outside [-1, %u)", n, spread->node_domain[n], D);
-    for (uint64_t t = 0; t < T; t++)
-        if (spread->max_skew[t] == 0) return fail(KS_ERR_RANGE, "spec %llu: max_skew 0 (at least 1)", (unsigned long long)t);
-    const uint64_t TD = T * D;
+    if (!spread || !spread->max_skew) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
+    const uint32_t NK = spread->n_keys, N = s->N;
+    if (NK == 0 || NK > KS_SPREAD_MAX_KEYS) return fail(KS_ERR_RANGE, "%u topology keys (1 to %u)", NK, KS_SPREAD_MAX_KEYS);
+    uint64_t Stot = 0;
+    for (uint32_t k = 0; k < NK; k++) {
+        if (!spread->node_domain[k]) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
+        const uint32_t D = spread->n_domains[k];
+        if (D == 0 || D > KS_SPREAD_MAX_DOMAINS) return fail(KS_ERR_RANGE, "%u domains (1 to %u)", D, KS_SPREAD_MAX_DOMAINS);
+        for (uint32_t n = 0; n < N; n++)
+            if (spread->node_domain[k][n] < -1 || spread->node_domain[k][n] >= (int64_t)D)
+                return fail(KS_ERR_INVALID, "key %u, node %u: domain %d outside [-1, %u)", k, n, spread->node_domain[k][n], D);
+        Stot += D;
+    }
+    for (uint64_t i = 0; i < T * NK; i++)
+        if (spread->max_skew[i] == 0)
+            return fail(KS_ERR_RANGE, "spec %llu, key %llu: max_skew 0 (at least 1)", (unsigned long long)(i / NK),
+                        (unsigned long long)(i % NK));
+    const uint64_t TD = T * Stot;
     if ((spread->existing || out_domain_count) && TD > KS_SPREAD_MAX_COUNTS)
-        return fail(KS_ERR_RANGE, "%llu specs x %u domains of counts (at most 2^26)", (unsigned long long)T, D);
+        return fail(KS_ERR_RANGE, "%llu specs x %llu domains of counts (at most 2^26)", (unsigned long long)T,
+                    (unsigned long long)Stot);
     if (spread->existing)
         for (uint64_t i = 0; i < TD; i++)
             if (spread->existing[i] > KS_SPREAD_MAX_EXISTING)
-                return fail(KS_ERR_RANGE, "spec %llu, domain %llu: %u existing pods (at most 2^24)",
-                            (unsigned long long)(i / D), (unsigned long long)(i % D), spread->existing[i]);
+                return fail(KS_ERR_RANGE, "spec %llu, count %llu: %u existing pods (at most 2^24)",
+                            (unsigned long long)(i / Stot), (unsigned long long)(i % Stot), spread->existing[i]);
     if (T == 0) return KS_OK;
     const bool copies = out_node || out_score;
     if (N == 0) { // no node: no eligible domain, every copy is -1
-        for (uint64_t t = 0; t < T; t++) out[t] = ks_spread_plan{0, 0, 0, 0, 0, -1, 0};
+        for (uint64_t t = 0; t < T * NK; t++) out[t] = ks_spread_plan{0, 0, 0, 0, 0, -1, 0};
         if (out_node) memset(out_node, 0xff, total * 4);
         if (out_score) memset(out_score, 0, total * 8);
         if (out_domain_count) {
@@ -1649,28 +1661,45 @@ int ks_place_replicas_spread(ks_snapshot* s, const ks_pods* specs, const uint32_
         }
         return KS_OK;
     }
-    const uint32_t W = s->W;
+    // internal key order: the primary (fewest domains, then the lower key) first, the others in the caller's order
+    uint32_t col[KS_SPREAD_MAX_KEYS] = {}, Dk[KS_SPREAD_MAX_KEYS] = {}, P[KS_SPREAD_MAX_KEYS] = {};
+    for (uint32_t k = 0, p = 0; k < NK; p += spread->n_domains[k], k++) {
+        P[k] = p;
+        if (spread->n_domains[k] < spread->n_domains[col[0]]) col[0] = k;
+    }
+    for (uint32_t k = 0, i = 1; k < NK; k++)
+        if (k != col[0]) col[i++] = k;
+    for (uint32_t i = 0; i < NK; i++) Dk[i] = spread->n_domains[col[i]];
+    const uint32_t W = s->W, D = Dk[0];
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
     const uint64_t C = copies ? total : 0, E = spread->existing ? TD : 0, K = out_domain_count ? TD : 0;
+    const uint64_t cta_bytes = spread_cta_bytes_keys(N, Dk, NK);
     uint32_t ctas;
     uint64_t seq_bytes;
-    spread_seq_grid(N, D, (uint32_t)T, s->sms, &ctas, &seq_bytes);
+    spread_seq_grid(cta_bytes, (uint32_t)T, s->sms, &ctas, &seq_bytes);
     HostStaged h;
     const auto cpu = h.in(specs->req_cpu, T), mem = h.in(specs->req_mem, T);
     const auto sel = h.in(specs->sel, T * W);
     const auto reps = h.in(replicas, T);
     const auto offset = h.in<uint64_t>(nullptr, T);
-    const auto max_skew = h.in(spread->max_skew, T);
-    const auto min_domains = h.in(spread->min_domains, spread->min_domains ? T : 0);
-    const auto node_domain = h.in(spread->node_domain, N);
+    const auto max_skew = h.in(spread->max_skew, T * NK);
+    const auto min_domains = h.in(spread->min_domains, spread->min_domains ? T * NK : 0);
+    Staged<int32_t> node_domain[KS_SPREAD_MAX_KEYS];
+    for (uint32_t i = 0; i < NK; i++) node_domain[i] = h.in(spread->node_domain[col[i]], N);
     const auto existing = h.in(spread->existing, E);
-    const auto rows = h.out(out, T);
+    const auto rows = h.out(out, T * NK);
     const auto score = h.out(out_score, C);
     const auto node = h.out(out_node, C);
     const auto count = h.out(out_domain_count, K);
-    const auto sort_buf = h.work<uint32_t>(2ull * N), perm = h.work<uint32_t>(N), pos = h.work<uint32_t>(N),
-               dstart = h.work<uint32_t>((uint64_t)D + 1);
+    Staged<uint32_t> sort_buf[KS_SPREAD_MAX_KEYS], perm[KS_SPREAD_MAX_KEYS], pos[KS_SPREAD_MAX_KEYS],
+        dstart[KS_SPREAD_MAX_KEYS];
+    for (uint32_t i = 0; i < NK; i++) {
+        sort_buf[i] = h.work<uint32_t>(2ull * N);
+        perm[i] = h.work<uint32_t>(N);
+        pos[i] = h.work<uint32_t>(N);
+        dstart[i] = h.work<uint32_t>((uint64_t)Dk[i] + 1);
+    }
     const auto seq = h.work<unsigned char>(seq_bytes, 16); // k_spread_seq's scratch
     CU_TRY(h.reserve(s));
     for (uint64_t t = 0, o = 0; t < T; o += replicas[t], t++) h.host(offset)[t] = o;
@@ -1689,18 +1718,30 @@ int ks_place_replicas_spread(ks_snapshot* s, const ks_pods* specs, const uint32_
     a.offset = h.dev(offset);
     a.out_node = copies ? h.dev(node) : nullptr;
     a.out_score = copies ? h.dev(score) : nullptr;
-    SpreadOrder o;
-    o.node_domain = h.dev(node_domain);
-    o.sort_buf = h.dev(sort_buf);
-    o.perm = h.dev(perm);
-    o.pos = h.dev(pos);
-    o.dstart = h.dev(dstart);
-    SpreadArgs q;
+    SpreadOrders o{};
+    SpreadArgs q{};
+    SpreadKeys mk{};
+    o.K = mk.K = NK;
+    for (uint32_t i = 0; i < NK; i++) {
+        SpreadOrder& k = o.key[i];
+        k.node_domain = h.dev(node_domain[i]);
+        k.sort_buf = h.dev(sort_buf[i]);
+        k.perm = h.dev(perm[i]);
+        k.pos = h.dev(pos[i]);
+        k.dstart = h.dev(dstart[i]);
+        k.D = Dk[i];
+        mk.col[i] = col[i];
+        mk.off[i] = P[col[i]];
+        mk.Dk[i] = Dk[i];
+        mk.dom[i] = k.node_domain;
+        mk.kperm[i] = k.perm;
+        mk.kdstart[i] = k.dstart;
+    }
     q.D = D;
-    q.node_domain = o.node_domain;
-    q.perm = o.perm;
-    q.pos = o.pos;
-    q.dstart = o.dstart;
+    q.node_domain = o.key[0].node_domain;
+    q.perm = o.key[0].perm;
+    q.pos = o.key[0].pos;
+    q.dstart = o.key[0].dstart;
     q.max_skew = h.dev(max_skew);
     q.min_domains = spread->min_domains ? h.dev(min_domains) : nullptr;
     q.existing = E ? h.dev(existing) : nullptr;
@@ -1708,11 +1749,36 @@ int ks_place_replicas_spread(ks_snapshot* s, const ks_pods* specs, const uint32_
     q.out_count = K ? h.dev(count) : nullptr;
     q.scratch = h.dev(seq);
     q.ctas = ctas;
-    cudaError_t e = launch_spread(node_table(s), policy, a, o, q, st);
+    mk.S = (uint32_t)Stot;
+    mk.cta_bytes = cta_bytes;
+    cudaError_t e = launch_spread(node_table(s), policy, a, o, q, mk, st);
     if (e != cudaSuccess) return fail(KS_ERR_CUDA, "spread placement launch failed: %s", cudaGetErrorString(e));
     CU_TRY(h.finish(st));
     s->last_path = "spread";
     return KS_OK;
+}
+
+int ks_place_replicas_spread(ks_snapshot* s, const ks_pods* specs, const uint32_t* replicas, const ks_spread* spread,
+                             int policy, ks_spread_plan* out, int32_t* out_node, int64_t* out_score,
+                             uint32_t* out_domain_count) {
+    ks_spread_multi m{};
+    if (spread) {
+        m.n_keys = 1;
+        m.n_domains[0] = spread->n_domains;
+        m.node_domain[0] = spread->node_domain;
+        m.max_skew = spread->max_skew;
+        m.min_domains = spread->min_domains;
+        m.existing = spread->existing;
+    }
+    return place_spread(s, "ks_place_replicas_spread", specs, replicas, spread ? &m : nullptr, policy, out, out_node,
+                        out_score, out_domain_count);
+}
+
+int ks_place_replicas_spread_multi(ks_snapshot* s, const ks_pods* specs, const uint32_t* replicas,
+                                   const ks_spread_multi* spread, int policy, ks_spread_plan* out, int32_t* out_node,
+                                   int64_t* out_score, uint32_t* out_domain_count) {
+    return place_spread(s, "ks_place_replicas_spread_multi", specs, replicas, spread, policy, out, out_node, out_score,
+                        out_domain_count);
 }
 
 // ---------------------------------------------------------------------------------------------- async streaming

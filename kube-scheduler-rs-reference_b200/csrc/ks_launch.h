@@ -142,32 +142,53 @@ void replica_seq_grid(uint32_t N, uint32_t T, int sms, uint32_t* ctas, uint32_t*
 cudaError_t launch_replicas(const NodeTable& nt, int policy, const ReplicaArgs& a, const ReplicaSeqArgs& q,
                             cudaStream_t st);
 
-// topology spread for replica placement (ks_place_replicas_spread, ks_spread.cu).  The specs come as ReplicaArgs' T,
-// requests, selectors, replicas, offsets and copy list (its rows and search state are not used).  Device memory.
-struct SpreadOrder {              // k_spread_order's input and outputs, once per call
+// topology spread for replica placement (ks_place_replicas_spread and _multi, ks_spread.cu).  The specs come as
+// ReplicaArgs' T, requests, selectors, replicas, offsets and copy list (its rows and search state are not used).  Device
+// memory.  Internal key 0 is the primary, the key with the fewest domains; keys 1 .. K-1 are the secondaries.
+struct SpreadOrder {              // k_spread_order's input and outputs for one key, once per call
     const int32_t* node_domain;   // [N]
     uint32_t* sort_buf;           // [2N]
     uint32_t* perm;               // [N]: nodes with a domain by (domain, node), the rest after dstart[D]
     uint32_t* pos;                // [N]: node -> position in perm
     uint32_t* dstart;             // [D + 1]: domain d's nodes are perm[dstart[d] .. dstart[d + 1])
+    uint32_t D;
+};
+struct SpreadOrders {             // one k_spread_order CTA per key
+    SpreadOrder key[KS_SPREAD_MAX_KEYS];
+    uint32_t K;
 };
 struct SpreadArgs {
-    uint32_t D;
+    uint32_t D;                   // the primary's
     const int32_t* node_domain;   // [N]
     const uint32_t *perm, *pos, *dstart;
-    const uint32_t* max_skew;     // [T]
-    const uint32_t* min_domains;  // [T] or null
-    const uint32_t* existing;     // [T * D] or null
-    ks_spread_plan* rows;         // [T]
-    uint32_t* out_count;          // [T * D] or null
+    const uint32_t* max_skew;     // [T * K]
+    const uint32_t* min_domains;  // [T * K] or null
+    const uint32_t* existing;     // [T * S] or null
+    ks_spread_plan* rows;         // [T * K]
+    uint32_t* out_count;          // [T * S] or null
     unsigned char* scratch;       // [bytes of spread_seq_grid]
     uint32_t ctas;
 };
+// K >= 2 only (the single-key kernel reads none of it, and takes it as a separate parameter so that its own code stays
+// as it was): per internal key i, its column col[i] in the caller's key order (max_skew, min_domains and rows are strided
+// by K), its count offset off[i] = P_col[i] (existing and out_count are strided by S = sum of D_k), its domains Dk[i]
+// and its order (dom[0] = SpreadArgs::node_domain)
+struct SpreadKeys {
+    uint32_t K, S;
+    uint32_t col[KS_SPREAD_MAX_KEYS], off[KS_SPREAD_MAX_KEYS], Dk[KS_SPREAD_MAX_KEYS];
+    const int32_t* dom[KS_SPREAD_MAX_KEYS];
+    const uint32_t* kperm[KS_SPREAD_MAX_KEYS];
+    const uint32_t* kdstart[KS_SPREAD_MAX_KEYS];
+    uint64_t cta_bytes;           // scratch per CTA
+};
+// k_spread_seq's scratch per CTA for the keys' domain counts Dk[0 .. K-1] (Dk[0] the primary's): 12 per node, 20 per
+// primary domain and 12 per block slot, and with K >= 2 also 4 per block slot and 8 per secondary domain
+uint64_t spread_cta_bytes_keys(uint32_t N, const uint32_t* Dk, uint32_t K);
 // k_spread_seq's CTAs - as many as fit in 64 MiB (at least one, at most one per spec and two per SM) - and the bytes of
-// their scratch: per CTA 12 per node, 20 per domain and 12 per block slot
-void spread_seq_grid(uint32_t N, uint32_t D, uint32_t T, int sms, uint32_t* ctas, uint64_t* bytes);
-cudaError_t launch_spread(const NodeTable& nt, int policy, const ReplicaArgs& a, const SpreadOrder& o,
-                          const SpreadArgs& q, cudaStream_t st);
+// their scratch
+void spread_seq_grid(uint64_t cta_bytes, uint32_t T, int sms, uint32_t* ctas, uint64_t* bytes);
+cudaError_t launch_spread(const NodeTable& nt, int policy, const ReplicaArgs& a, const SpreadOrders& o,
+                          const SpreadArgs& q, const SpreadKeys& mk, cudaStream_t st);
 
 } // namespace ks
 

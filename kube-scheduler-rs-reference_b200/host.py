@@ -48,6 +48,8 @@ for _name, _res, _args in [
     ("ksh_context_topology_domains", C.c_int, [_vp, C.c_char_p, _vp, C.POINTER(C.c_uint32), _vp, C.c_size_t, _vp]),
     ("ksh_place_replicas_spread", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_char_p, _vp, _vp, _vp, _vp, C.c_int, _vp,
                                             _vp, _vp, _vp]),
+    ("ksh_place_replicas_spread_multi", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp,
+                                                  C.c_int, _vp, _vp, _vp, _vp]),
 ]:
     _proto(_name, _res, *_args)
 
@@ -253,6 +255,47 @@ class Context:
                                             None if score is None else score.ctypes.data,
                                             None if counts is None else counts.ctypes.data),
               "ksh_place_replicas_spread")
+        return rows, node, score, offset, counts
+
+    def place_replicas_spread_multi(self, pods, n, replicas, topology_keys, max_skew, min_domains=None,
+                                    existing_nodes=None, policy=capi.KS_SCORE_LEFTOVER, want_nodes=True, first=0):
+        """Replica placement under one topology spread constraint per key over objects (ksh_place_replicas_spread_multi):
+        as place_replicas_spread, with topology_keys a list of K keys, max_skew and min_domains [n, K], and
+        existing_nodes[t][k] the node names of the bound pods that match spec t's constraint for key k (None: none).
+        Returns (rows [n, K], node, score, offset, counts) as Snapshot.place_replicas_spread_multi, with each key's
+        domains numbered as topology_domains(key) numbers them (counts None when some key is on no node)."""
+        k = len(topology_keys)
+        replicas = np.ascontiguousarray(replicas, np.uint32).reshape(-1)
+        max_skew = np.ascontiguousarray(max_skew, np.uint32).reshape(-1)
+        if replicas.shape[0] != n or max_skew.shape[0] != n * k:
+            raise ValueError(f"replicas / max_skew have {replicas.shape[0]} / {max_skew.shape[0]} entries, pods {n}, "
+                             f"keys {k}")
+        mind = None if min_domains is None else np.ascontiguousarray(min_domains, np.uint32).reshape(-1)
+        names, ex_off = None, None
+        if existing_nodes is not None:
+            lists = [lst for per_spec in existing_nodes for lst in per_spec]
+            flat = [s.encode() for lst in lists for s in lst]
+            names = (C.c_char_p * max(len(flat), 1))(*flat)
+            ex_off = np.zeros(n * k + 1, np.uint64)
+            np.cumsum([len(lst) for lst in lists], out=ex_off[1:])
+        keys = (C.c_char_p * max(k, 1))(*[key.encode() for key in topology_keys])
+        nd = [len(self.topology_domains(key)[1]) for key in topology_keys]
+        offset, _, node, score = replica_outputs(replicas, capi.SPREAD_PLAN_DTYPE, want_nodes)
+        rows = np.zeros((n, k), capi.SPREAD_PLAN_DTYPE)
+        s = sum(nd)
+        counts = np.empty((n, s), np.uint32) if min(nd, default=0) and n * s <= capi.KS_SPREAD_MAX_COUNTS else None
+        check(lib.ksh_place_replicas_spread_multi(self._h, _addr(pods, first), n, replicas.ctypes.data,
+                                                  C.cast(keys, _vp), k, max_skew.ctypes.data,
+                                                  None if mind is None else mind.ctypes.data,
+                                                  None if names is None else C.cast(names, _vp),
+                                                  None if ex_off is None else ex_off.ctypes.data, int(policy),
+                                                  rows.ctypes.data,
+                                                  None if node is None else node.ctypes.data,
+                                                  None if score is None else score.ctypes.data,
+                                                  None if counts is None else counts.ctypes.data),
+              "ksh_place_replicas_spread_multi")
+        if counts is not None:
+            counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
         return rows, node, score, offset, counts
 
     def select_nodes(self, pods, n, policy=capi.KS_SCORE_LEFTOVER, first=0):

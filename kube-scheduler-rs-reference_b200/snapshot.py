@@ -307,6 +307,52 @@ class Snapshot:
               "ks_place_replicas_spread")
         return rows, node, score, offset, counts
 
+    def place_replicas_spread_multi(self, req_cpu, req_mem, sel, replicas, keys, max_skew, min_domains=None,
+                                    existing=None, policy=capi.KS_SCORE_LEFTOVER, want_nodes=True, want_counts=True):
+        """Replica placement under one topology spread constraint per key, every constraint binding at once
+        (ks_place_replicas_spread_multi): keys is a list of K (node_domain, n_domains) pairs, max_skew and min_domains
+        (None = no minDomains) are [T, K], existing is None or a list of K arrays [T, n_domains_k].  Nothing is charged.
+        Returns (rows, node, score, offset, counts): rows a capi.SPREAD_PLAN_DTYPE record array [T, K]; node / score /
+        offset as place_replicas; counts a list of K arrays uint32 [T, n_domains_k] (None unless want_counts)."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        t = int(pods.n)
+        replicas = np.asarray(replicas).reshape(-1)
+        if replicas.shape[0] != t:
+            raise ValueError(f"replicas has {replicas.shape[0]} entries, specs {t}")
+        if t and (replicas.min() < 0 or replicas.max() > 0xFFFFFFFF):
+            raise ValueError("replicas must lie in [0, 2^32)")
+        replicas = _c(replicas, np.uint32)
+        k = len(keys)
+        if not 1 <= k <= capi.KS_SPREAD_MAX_KEYS:
+            raise ValueError(f"{k} topology keys (1 to {capi.KS_SPREAD_MAX_KEYS})")
+        doms = [_c(d, np.int32).reshape(-1) for d, _ in keys]
+        nd = [int(n) for _, n in keys]
+        max_skew = _c(max_skew, np.uint32).reshape(-1)
+        if max_skew.shape[0] != t * k:
+            raise ValueError(f"max_skew has {max_skew.shape[0]} entries, specs x keys {t * k}")
+        if min_domains is not None:
+            min_domains = _c(min_domains, np.uint32).reshape(-1)
+            if min_domains.shape[0] != t * k:
+                raise ValueError(f"min_domains has {min_domains.shape[0]} entries, specs x keys {t * k}")
+        s = sum(nd)
+        if existing is not None:
+            if len(existing) != k:
+                raise ValueError(f"existing has {len(existing)} blocks, keys {k}")
+            existing = _c(np.concatenate([np.asarray(e, np.uint32).reshape(t, n) for e, n in zip(existing, nd)],
+                                         axis=1), np.uint32).reshape(-1)
+        spread = capi.ks_spread_multi(k, (C.c_uint32 * capi.KS_SPREAD_MAX_KEYS)(*nd),
+                                      (C.c_void_p * capi.KS_SPREAD_MAX_KEYS)(*[_ptr(d) for d in doms]),
+                                      _ptr(max_skew), _ptr(min_domains), _ptr(existing))
+        offset, _, node, score = replica_outputs(replicas, capi.SPREAD_PLAN_DTYPE, want_nodes)
+        rows = np.zeros((t, k), capi.SPREAD_PLAN_DTYPE)
+        counts = np.empty((t, s), np.uint32) if want_counts and 0 < t * s <= capi.KS_SPREAD_MAX_COUNTS else None
+        check(lib.ks_place_replicas_spread_multi(self._h, C.byref(pods), _ptr(replicas), C.byref(spread), int(policy),
+                                                 _ptr(rows), _ptr(node), _ptr(score), _ptr(counts)),
+              "ks_place_replicas_spread_multi")
+        if counts is not None:
+            counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
+        return rows, node, score, offset, counts
+
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
         """The reference's own policy (src/main.rs:49-71), seeded: (node_idx, attempts_used, draw_node, draw_code)."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
