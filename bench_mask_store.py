@@ -3,7 +3,7 @@
 Part 1 compiles examples/mask_store_probe.cu (nvcc, sm_90a, into a temporary directory: the source tree may be read-only)
 and runs its patterns on one 1M x 6400-byte buffer of its own, alternated, several repetitions each: P0 = a plain
 128-bit-store fill, P1 = k_mask_rows' store shape, P2-P5 = P1 with one thing changed (whole-line store order, longer
-column blocks, count atomics, record loads).  Part 2 times k_mask_rows itself on workload c3 through Snapshot.select_raw
+column blocks, count atomics, record loads), P6 = P5 with the records staged in a shared-memory ring by bulk copies.  Part 2 times k_mask_rows itself on workload c3 through Snapshot.select_raw
 with parts of its work switched off (counts NULL, mask NULL, the minimal row pitch), alternated the same way.
 Prints one JSON line with min / median / max per row, the card's name, power limit and SM clock read in the same run."""
 import argparse

@@ -10,8 +10,13 @@
 //   P3  P2 with 512-byte / 1 KB column blocks
 //   P4  P2 + one atomicAdd per pod and column block into a 4 MB count array
 //   P5  P2 + the 16-byte pod record loads of k_mask_rows (16 MB array, once per pod and column block, one group ahead)
+//   P6  P5 with the records staged in shared memory: one thread per CTA claims chunks of CHUNK groups and brings their
+//       records into a two-slot ring by bulk async copies (L2 evict-last, as K2's record loads) a chunk ahead; the warps
+//       take the chunk's groups round robin
 // Output: one JSON line, {"pattern": [GB/s of every repetition, in launch order]}.  Patterns are alternated.
 #include <cuda_runtime.h>
+
+#include "../kube-scheduler-rs-reference_b200/csrc/ks_internal.cuh"
 
 #include <algorithm>
 #include <cstdint>
@@ -53,7 +58,7 @@ struct Probe {
     uint32_t ncb;       // column blocks of BLOCK bytes (the last one may be cut by the pitch)
     uint32_t* cursor;   // [ncb * CURSOR_STRIDE]
     uint32_t* cnt;      // [rows] (P4)
-    const uint4* rec;   // [rows] (P5)
+    const uint4* rec;   // [rows] (P5, P6)
 };
 
 // HALF: P1's store order; else whole lines.  RED: count atomics.  REC: record loads.
@@ -140,6 +145,128 @@ __global__ void __launch_bounds__(1024, 1) k_probe(const __grid_constant__ Probe
     }
 }
 
+// P6: P5's stores and record dependence, with the records staged in a ring of RING slots of C groups (slot x % RING holds
+// the CTA's x-th chunk; thread 0 claims and copies chunk x + 1 when warp 0 starts chunk x).
+constexpr uint32_t RING = 2;
+constexpr uint32_t CHUNK = 32; // 16-32 measured equally fast at the c3 shape, 64 slower (BASELINE.md)
+__global__ void __launch_bounds__(1024, 1) k_probe_ring(const __grid_constant__ Probe pr, uint32_t C) {
+    extern __shared__ __align__(128) uint8_t ring[];
+    __shared__ __align__(8) uint64_t full[RING], empty[RING];
+    __shared__ uint32_t s_base[RING];
+    __shared__ unsigned long long s_key;
+    const uint32_t tid = threadIdx.x, t = tid & 7, ps = (tid >> 3) & 3, lane = tid & 31, warp = tid >> 5;
+    const uint32_t nwarps = blockDim.x >> 5;
+    uint64_t pol, pol_rec;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_rec));
+    if (tid == 0) {
+        for (uint32_t s = 0; s < RING; s++) {
+            ks::mbar_init(&full[s], 1);
+            ks::mbar_init(&empty[s], nwarps);
+        }
+        ks::fence_mbar_init();
+    }
+    const uint32_t n = pr.n_groups, ncb = pr.ncb;
+    uint32_t cb = (uint32_t)((uint64_t)blockIdx.x * ncb / gridDim.x);
+    uint32_t seq = 0, pending = 0; // chunks begun by this CTA; thread 0: the claim for the next chunk
+    bool prod_done = false;
+    for (;;) {
+        __syncthreads();
+        uint32_t* cursor = pr.cursor + (size_t)cb * CURSOR_STRIDE;
+        auto issue = [&](uint32_t x) { // thread 0
+            const uint32_t s = x % RING;
+            ks::mbar_wait(&empty[s], ((x / RING) & 1u) ^ 1u);
+            const uint32_t b = pending;
+            s_base[s] = b;
+            if (b < n) {
+                const uint32_t bytes = min(C, n - b) * 128u;
+                ks::fence_proxy_async();
+                ks::mbar_arrive_expect_tx(&full[s], bytes);
+                ks::tma_bulk_g2s(ring + (size_t)s * C * 128u, pr.rec + (size_t)b * 8u, bytes, &full[s], pol_rec);
+                pending = atomicAdd(cursor, C);
+            } else {
+                ks::mbar_arrive(&full[s]);
+                prod_done = true;
+            }
+        };
+        if (tid == 0) {
+            pending = atomicAdd(cursor, C);
+            prod_done = false;
+            issue(seq);
+        }
+        uint32_t j = seq, i = warp, base = 0, cnt = 0;
+        auto enter = [&]() {
+            if (tid == 0 && !prod_done) issue(j + 1);
+            ks::mbar_wait(&full[j % RING], (j / RING) & 1u);
+            base = s_base[j % RING];
+            cnt = base < n ? min(C, n - base) : 0u;
+        };
+        auto settle = [&]() { // moves (j, i) to this warp's next group; false at the block's end chunk
+            while (i >= cnt && cnt != 0) {
+                __syncwarp();
+                if (lane == 0) ks::mbar_arrive(&empty[j % RING]);
+                i = i >= C ? i - C : 0u;
+                j++;
+                enter();
+            }
+            return cnt != 0;
+        };
+        auto rec = [&](uint32_t q) {
+            return *reinterpret_cast<const uint4*>(ring + ((size_t)(j % RING) * C + i) * 128u + (2u * ps + q) * 16u);
+        };
+        enter();
+        const uint32_t col = cb * 256u;
+        bool more = settle();
+        uint4 nA = more ? rec(0) : make_uint4(0, 0, 0, 0), nB = more ? rec(1) : nA;
+        while (more) {
+            const uint4 rA = nA, rB = nB;
+            const uint32_t g = base + i;
+            i += nwarps;
+            more = settle();
+            if (more) {
+                nA = rec(0);
+                nB = rec(1);
+            }
+#pragma unroll
+            for (int q = 0; q < 2; q++) {
+                const uint32_t pod = g * 8u + 2u * ps + q;
+                const uint4 r = q ? rB : rA;
+                const uint32_t v = pod ^ r.x ^ r.y ^ r.z ^ r.w;
+                uint8_t* row = pr.mask + (size_t)pod * pr.pitch;
+                st_ef(row + col + 16u * t, v, v, v, v, pol);
+                st_ef(row + col + 128u + 16u * t, v, v, v, v, pol);
+            }
+        }
+        __syncwarp();
+        if (lane == 0) ks::mbar_arrive(&empty[j % RING]); // the end chunk
+        seq = j + 1;
+        if (ncb == 1) break;
+        __syncthreads();
+        if (tid == 0) s_key = 0;
+        __syncthreads();
+        for (uint32_t c = tid; c < ncb; c += blockDim.x) {
+            const uint32_t used = *reinterpret_cast<volatile uint32_t*>(pr.cursor + (size_t)c * CURSOR_STRIDE);
+            const uint32_t left = used < n ? n - used : 0u;
+            if (left >= HOP_MIN || (left > 0 && used == 0)) {
+                const uint32_t dist = (c + ncb - cb) % ncb;
+                atomicMax(&s_key, ((unsigned long long)left << 32) | (0xFFFFFFFFu - dist));
+            }
+        }
+        __syncthreads();
+        const unsigned long long key = s_key;
+        if (key == 0) break;
+        cb = (cb + (0xFFFFFFFFu - (uint32_t)key)) % ncb;
+    }
+}
+
+static void launch_ring(Probe pr, int sms, cudaStream_t st) {
+    CK(cudaFuncSetAttribute(k_probe_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_PIN));
+    pr.ncb = (pr.pitch + 255) / 256;
+    CK(cudaMemsetAsync(pr.cursor, 0, (size_t)pr.ncb * CURSOR_STRIDE * 4, st));
+    k_probe_ring<<<sms, THREADS, SMEM_PIN, st>>>(pr, CHUNK);
+    CK(cudaGetLastError());
+}
+
 template <int BLOCK, bool HALF, bool RED, bool REC>
 static void launch(Probe pr, int sms, cudaStream_t st) {
     auto k = k_probe<BLOCK, HALF, RED, REC>;
@@ -188,6 +315,7 @@ int main(int argc, char** argv) {
         {"P3_whole_lines_1KB", [](Probe p, int s, cudaStream_t q) { launch<1024, false, false, false>(p, s, q); }},
         {"P4_whole_lines_red", [](Probe p, int s, cudaStream_t q) { launch<256, false, true, false>(p, s, q); }},
         {"P5_whole_lines_rec", [](Probe p, int s, cudaStream_t q) { launch<256, false, false, true>(p, s, q); }},
+        {"P6_whole_lines_rec_ring", launch_ring},
     };
     const int np = (int)(sizeof(pats) / sizeof(pats[0]));
     cudaEvent_t e0, e1;
@@ -207,13 +335,13 @@ int main(int argc, char** argv) {
             CK(cudaEventElapsedTime(&ms, e0, e1));
             gbs[p].push_back(bytes / (ms * 1e-3) / 1e9);
         }
-    // spot check of the last pattern only (P5, which follows P0 fill): on 3 rows, the first 4 bytes of every 16 no longer
+    // spot check of the last pattern only (P6, which follows P0 fill): on 3 rows, the first 4 bytes of every 16 no longer
     // hold the fill value
     std::vector<uint8_t> h(pitch);
     for (uint32_t row : {0u, rows / 2 + 3, rows - 1}) {
         CK(cudaMemcpy(h.data(), pr.mask + (size_t)row * pitch, pitch, cudaMemcpyDeviceToHost));
         for (uint32_t i = 0; i < pitch; i += 16)
-            if (h[i] == 0x3C && h[i + 1] == 0x3C && h[i + 2] == 0x3C && h[i + 3] == 0x3C) { // P5 writes the row index
+            if (h[i] == 0x3C && h[i + 1] == 0x3C && h[i + 2] == 0x3C && h[i + 3] == 0x3C) { // P6 writes the row index
                 fprintf(stderr, "row %u byte %u not written by the last pattern\n", row, i);
                 return 1;
             }

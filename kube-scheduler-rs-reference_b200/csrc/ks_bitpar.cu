@@ -507,23 +507,28 @@ __global__ void __launch_bounds__(RANK_THREADS, 1)
 //     base/membership lookup, no POPC for ranks;
 //   * table rows and label-pair columns are 256-byte lines in tile order: the 8 lanes of a shared-memory phase read
 //     offsets 16 t (mod 128) of their own rows -> conflict-free for any ranks;
-//   * work = (column block, pod group) items handed out dynamically: one atomic cursor per column block, warps claim
-//     RW_CLAIM groups at a time, a CTA whose block is exhausted re-stages the blob of the block with the most work left
+//   * work = (column block, pod group) items handed out dynamically: one atomic cursor per column block, each CTA claims
+//     chunks of groups, a CTA whose block is exhausted re-stages the blob of the block with the most work left
 //     (all SMs busy whatever ncb is, and SMs that stream faster simply claim more);
-//   * pod records (pod order: no sort) are fetched one iteration ahead.
+//   * pod records (pod order: no sort) arrive in a shared-memory ring by bulk copies a chunk ahead, and every warp loads
+//     the rank entries of its next group before it stores the current one: under a saturated store stream the L2 load
+//     replies queue behind the stores, and record and rank loads issued one group ahead left the stores waiting.
+// k_count_rows: the same items without a mask (feasible counts only), claimed per warp with the records loaded one
+// group ahead.  With no stores to hide them, the ring's chunk edges cost more than they save: at c3 the ring loop took
+// 1.42 ms for the counts alone where this one takes 1.05 ms (H100, BASELINE.md §4).
 __device__ __forceinline__ uint4 lds128(uint32_t a) { // pure: scheduled freely; ordered after the blob wait by the
     uint4 v;                                          // address dependence on the post-wait token
     asm("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
     return v;
 }
-__device__ __forceinline__ uint32_t ldg_u32_keep(const uint32_t* p, uint64_t pol) { // L2 evict-last: the rank tables are re-read
-    uint32_t v;
-    asm("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
-    return v;
-}
 __device__ __forceinline__ uint4 ldg128_keep(const uint4* p, uint64_t pol) { // L2 evict-last: pod records, read once per column block
     uint4 v;
     asm("ld.global.nc.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ uint32_t ldg_u32_keep(const uint32_t* p, uint64_t pol) { // L2 evict-last: the rank tables are re-read
+    uint32_t v;
+    asm("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
     return v;
 }
 template <class T>
@@ -546,8 +551,13 @@ struct RowsParams { // kernel parameters stay in the constant bank: the loop rea
     uint32_t row_words;              // mask row pitch in 32-bit words
     uint32_t* cnt;                   // may be nullptr
     uint32_t* cursor;                // [ncb * RW_CURSOR_STRIDE] next unclaimed pod group of every column block
+    uint32_t chunk;                  // k_mask_rows: pod groups per ring slot, RW_CHUNK_MIN..RW_CHUNK_MAX (rows_chunk)
 };
-constexpr uint32_t RW_CLAIM = 4;     // pod groups per claim (one atomicAdd per warp and ~4 x 2 KB x 8 of mask)
+constexpr uint32_t RW_RING = 2; // record ring slots: a chunk is read while the next one is copied in
+// Groups per chunk, measured at c3 on an H100 (BASELINE.md §4): 16-32 are equally fast, 64 gives back a third of the gain,
+// and at 12 or fewer a chunk is over before the next one has landed.  The ring of 2 x 32 groups is 8 KB beside the blob.
+constexpr uint32_t RW_CHUNK_MIN = 24, RW_CHUNK_MAX = 32;
+constexpr uint32_t RW_CLAIM = 4; // k_count_rows: pod groups per claim (one atomicAdd per warp)
 constexpr uint32_t RW_HOP_MIN = 256; // a partly claimed column block is worth moving to while it has this many groups left
 
 // one lane's share of a (pod, column block) item: granules t (tile t/2) and 8 + t (tile 4 + t/2) of the pod's 256 bytes ->
@@ -630,6 +640,194 @@ __device__ __forceinline__ uint32_t rows_item(const RowsParams& prm, uint32_t a_
 // of the register file to the argmax CTAs that run beside it)
 template <int W, bool PSMEM, int THREADS>
 __global__ void __launch_bounds__(BP_THREADS, 1) k_mask_rows(const __grid_constant__ RowsParams prm) {
+    extern __shared__ __align__(128) uint8_t smem[]; // the column block's blob, then the record ring
+    __shared__ __align__(8) uint64_t bar;
+    __shared__ __align__(8) uint64_t full[RW_RING], empty[RW_RING];
+    __shared__ uint32_t s_base[RW_RING];
+    __shared__ unsigned long long s_key;
+    constexpr uint32_t WARPS = THREADS / 32;
+    const uint32_t tid = threadIdx.x, t = tid & 7, ps = (tid >> 3) & 3, lane = tid & 31, warp = tid >> 5;
+    uint64_t pol_st, pol_ld; // L2 policies: mask stores evict-first, rank-table and pod-record loads evict-last
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_st));
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol_ld));
+    if (tid == 0) {
+        mbar_init(&bar, 1);
+        for (uint32_t s = 0; s < RW_RING; s++) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], WARPS);
+        }
+        fence_mbar_init();
+        trace_start(TR_MASK_START);
+    }
+    __syncthreads();
+    uint32_t phase = 0;
+
+    // Work = (column block, pod group) items.  Every column block has one cursor (zeroed by k_pod_ranks); thread 0 claims
+    // C = prm.chunk consecutive pod groups of the staged column block at a time with one atomicAdd, one chunk ahead of
+    // their use, and brings the chunk's records (C x 128 contiguous bytes) into a ring slot in shared memory by a bulk
+    // copy while the warps work on the chunk before.  The CTA's chunks are numbered across column blocks (slot x % RW_RING
+    // holds chunk x; full[s] completes when its records have landed, empty[s] when every warp is done reading them), and
+    // their groups are dealt to the warps round robin.  A chunk whose base lies past the block's end closes the block.
+    // The CTAs that share a column block therefore finish it together whatever their individual rates (SMs do not all
+    // stream at the same rate), and a CTA whose block is exhausted moves - one barrier, one re-staging of the blob - to
+    // the block with the most unclaimed groups.  CTAs start spread evenly over the column blocks.
+    const uint32_t n_slots = prm.n_groups; // pod groups per column block
+    const uint32_t ncb = prm.lay.ncb;
+    const uint32_t C = prm.chunk;
+    uint8_t* const ring = smem + prm.lay.smem_bytes;
+    uint32_t seq = 0;       // chunks begun by this CTA
+    uint32_t pending = 0;   // thread 0: the claim for the next chunk
+    bool prod_done = false; // thread 0: the block's closing chunk has been issued
+    uint32_t cb = (uint32_t)((uint64_t)blockIdx.x * ncb / gridDim.x);
+    for (;;) { // one iteration per column block this CTA works on
+        __syncthreads(); // all reads of the previous blob are done
+        uint32_t* cursor = prm.cursor + (size_t)cb * RW_CURSOR_STRIDE;
+        auto issue = [&](uint32_t x) { // thread 0: claimed chunk -> ring slot x % RW_RING, once its previous chunk is read
+            const uint32_t s = x % RW_RING;
+            mbar_wait(&empty[s], ((x / RW_RING) & 1u) ^ 1u);
+            const uint32_t b = pending;
+            s_base[s] = b;
+            if (b < n_slots) {
+                const uint32_t bytes = min(C, n_slots - b) * 128u;
+                fence_proxy_async();
+                mbar_arrive_expect_tx(&full[s], bytes);
+                tma_bulk_g2s(ring + (size_t)s * C * 128u, prm.rec_s + (size_t)b * 8u, bytes, &full[s], pol_ld);
+                pending = atomicAdd(cursor, C);
+            } else {
+                mbar_arrive(&full[s]);
+                prod_done = true;
+            }
+        };
+        if (tid == 0) {
+            fence_proxy_async();
+            mbar_arrive_expect_tx(&bar, prm.lay.smem_bytes);
+            const uint8_t* src = prm.blob + (size_t)cb * prm.lay.cb_stride;
+            for (uint32_t off = 0; off < prm.lay.smem_bytes; off += 32768u)
+                tma_bulk_g2s(smem + off, src + off, min(32768u, prm.lay.smem_bytes - off), &bar);
+            pending = atomicAdd(cursor, C);
+            prod_done = false;
+            issue(seq);
+        }
+        // rank entry of (g, resource r, tiles t/2 and 4 + t/2): rk_t[g * 8 + r * 4]
+        const uint32_t* rk_t = opaque_ptr(prm.rank + (size_t)cb * prm.lay.n_thr * RW_TILES + (t >> 1));
+        auto fetch_ranks = [&](const uint4& ra, const uint4& rb, uint32_t& rCa, uint32_t& rMa, uint32_t& rCb, uint32_t& rMb) {
+            rCa = ldg_u32_keep(rk_t + (size_t)ra.x * 8u, pol_ld);
+            rMa = ldg_u32_keep(rk_t + (size_t)ra.y * 8u + 4, pol_ld);
+            rCb = ldg_u32_keep(rk_t + (size_t)rb.x * 8u, pol_ld);
+            rMb = ldg_u32_keep(rk_t + (size_t)rb.y * 8u + 4, pol_ld);
+        };
+        // this warp's next group: index i of chunk j (warp-uniform), whose first group is base and which holds cnt groups
+        uint32_t j = seq, i = warp, base = 0, cnt = 0;
+        auto enter = [&]() {
+            if (tid == 0 && !prod_done) issue(j + 1);
+            mbar_wait(&full[j % RW_RING], (j / RW_RING) & 1u);
+            base = s_base[j % RW_RING];
+            cnt = base < n_slots ? min(C, n_slots - base) : 0u;
+        };
+        auto settle = [&]() { // moves (j, i) on to this warp's next group; false at the block's closing chunk
+            while (i >= cnt && cnt != 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[j % RW_RING]);
+                i = i >= C ? i - C : 0u; // (a chunk cut short by the block's end is followed by the closing chunk)
+                j++;
+                enter();
+            }
+            return cnt != 0;
+        };
+        auto rec = [&](uint32_t q) { // record of pod 2 ps + q of the group
+            return *reinterpret_cast<const uint4*>(ring + ((size_t)(j % RW_RING) * C + i) * 128u + (2u * ps + q) * 16u);
+        };
+        enter();
+        bool more = settle();
+        uint4 nA = make_uint4(0, 0, RW_PID_NONE, 0), nB = nA;
+        uint32_t nCa = 0, nMa = 0, nCb = 0, nMb = 0;
+        if (more) {
+            nA = rec(0);
+            nB = rec(1);
+            fetch_ranks(nA, nB, nCa, nMa, nCb, nMb);
+        }
+
+        mbar_wait(&bar, phase);
+        phase ^= 1;
+        uint32_t tok; // every shared-memory load below depends on a value produced after the wait
+        asm volatile("mov.u32 %0, 0;" : "=r"(tok)::"memory");
+        const uint32_t a_tab = smem_u32(smem) + t * 16u + tok;
+        // a tile is written when it holds nodes, or when the caller's row pitch has room for it (a pitch that is a multiple
+        // of 256 bytes - ks_mask_row_bytes_aligned - lets the 8 lanes of a pod always store one whole, 256-byte-aligned
+        // block: two whole 128-byte lines); padding tiles hold zeros.  This lane writes half of tile t/2 and half of
+        // tile 4 + t/2; the condition falls with the tile index, so st_hi implies that the low granule is written too.
+        auto written = [&](uint32_t tile) { return tile < prm.lay.n_tiles || (tile + 1u) * 8u <= prm.row_words; };
+        const uint32_t tile_lo = cb * RW_TILES + (t >> 1);
+        const bool st_hi = written(tile_lo + 4);
+        uint32_t* mask_col = (prm.mask != nullptr && written(tile_lo))
+                                 ? opaque_ptr(prm.mask + (size_t)cb * (RW_LINE / 4) + t * 4u)
+                                 : nullptr;
+
+        while (more) { // warp-uniform: one pod group; the next group's records and ranks are loaded before its stores
+            const uint32_t pidA = nA.z, selA = nA.w, pidB = nB.z, selB = nB.w;
+            const uint32_t rCa = nCa, rMa = nMa, rCb = nCb, rMb = nMb;
+            const uint32_t g = base + i;
+            i += WARPS;
+            more = settle();
+            if (more) {
+                nA = rec(0);
+                nB = rec(1);
+                fetch_ranks(nA, nB, nCa, nMa, nCb, nMb);
+            }
+            const uint32_t cA = rows_item<W, PSMEM>(prm, a_tab, cb, t, mask_col, st_hi, rCa, rMa, pidA, selA, g * 8u + 2u * ps, pol_st);
+            const uint32_t cB = rows_item<W, PSMEM>(prm, a_tab, cb, t, mask_col, st_hi, rCb, rMb, pidB, selB, g * 8u + 2u * ps + 1u, pol_st);
+            if (prm.cnt != nullptr) { // the 8 lanes of a pod are adjacent; both pods' counts ride in one register
+                uint32_t c = cA | (cB << 16);
+                c += __shfl_xor_sync(0xffffffffu, c, 1);
+                c += __shfl_xor_sync(0xffffffffu, c, 2);
+                c += __shfl_xor_sync(0xffffffffu, c, 4);
+                if (t == 0) {
+                    const uint32_t ca = c & 0xFFFFu, cb_ = c >> 16;
+                    if (ncb == 1) { // single writer, no zero-init needed
+                        if (pidA != RW_PID_NONE) prm.cnt[pidA] = ca;
+                        if (pidB != RW_PID_NONE) prm.cnt[pidB] = cb_;
+                    } else {
+                        if (pidA != RW_PID_NONE && ca) atomicAdd(&prm.cnt[pidA], ca);
+                        if (pidB != RW_PID_NONE && cb_) atomicAdd(&prm.cnt[pidB], cb_);
+                    }
+                }
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[j % RW_RING]); // the closing chunk
+        seq = j + 1;
+
+        // this column block is exhausted (its last groups are being finished by the warps that claimed them, here or in
+        // other CTAs): move to the block with the most unclaimed groups, if any is worth a re-staging
+        if (ncb == 1) break;
+        __syncthreads();
+        if (tid == 0) s_key = 0;
+        __syncthreads();
+        for (uint32_t c = tid; c < ncb; c += THREADS) {
+            const uint32_t used = *reinterpret_cast<volatile uint32_t*>(prm.cursor + (size_t)c * RW_CURSOR_STRIDE);
+            const uint32_t left = used < n_slots ? n_slots - used : 0u;
+            if (left >= RW_HOP_MIN || (left > 0 && used == 0)) { // key: groups left, then nearness to the current block
+                const uint32_t dist = (c + ncb - cb) % ncb;
+                atomicMax(&s_key, ((unsigned long long)left << 32) | (0xFFFFFFFFu - dist));
+            }
+        }
+        __syncthreads();
+        const unsigned long long key = s_key;
+        if (key == 0) break;
+        cb = (cb + (0xFFFFFFFFu - (uint32_t)key)) % ncb;
+    }
+    if (c_trace) {
+        __syncthreads();
+        if (tid == 0) {
+            const unsigned long long now = global_ns();
+            atomicMax(c_trace + TR_MASK_END, now);
+            atomicMax(c_trace + TR_MASK_FIRST_CTA_END_INV, ~now); // = ~(earliest CTA end)
+        }
+    }
+}
+
+template <int W, bool PSMEM, int THREADS>
+__global__ void __launch_bounds__(BP_THREADS, 1) k_count_rows(const __grid_constant__ RowsParams prm) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ __align__(8) uint64_t bar;
     __shared__ unsigned long long s_key;
@@ -1580,6 +1778,13 @@ cudaError_t bitpar_prepare_order(BitparIndex& ix, const NodeTable& nt, int polic
     return cudaSuccess;
 }
 
+// k_mask_rows' pod groups per chunk: about 20 chunks per CTA and column block, so that the CTAs sharing a block finish
+// it close together, within RW_CHUNK_MIN..RW_CHUNK_MAX
+static uint32_t rows_chunk(uint32_t n_groups, uint32_t ncb, uint32_t grid) {
+    const uint32_t ctas_per_cb = std::max(1u, grid / ncb);
+    return std::min(RW_CHUNK_MAX, std::max(RW_CHUNK_MIN, n_groups / (ctas_per_cb * 20u)));
+}
+
 bool bitpar_profitable(const BitparIndex& ix, uint32_t P) {
     // below ~16M cells the per-call rank pass and blob staging outweigh the per-cell kernel;
     // the mask kernel indexes (pod, tile) items with 32 bits
@@ -1588,7 +1793,9 @@ bool bitpar_profitable(const BitparIndex& ix, uint32_t P) {
 
 template <int W, int THREADS>
 static cudaError_t set_smem_attr1() {
-    return cudaFuncSetAttribute(k_mask_rows<W, W <= 4, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, BP_SMEM_MAX - 1024);
+    cudaError_t e = cudaFuncSetAttribute(k_mask_rows<W, W <= 4, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, BP_SMEM_MAX - 1024);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(k_count_rows<W, W <= 4, THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, BP_SMEM_MAX - 1024);
 }
 template <int W>
 static cudaError_t set_smem_attr() {
@@ -1758,8 +1965,14 @@ static cudaError_t select_w(BitparIndex& ix, SelectLaunch& L, cudaEvent_t before
         prm.row_words = (uint32_t)L.ov.mask_row_words;
         prm.cnt = L.ov.cnt;
         prm.cursor = ix.cursor.as<uint32_t>();
+        prm.chunk = rows_chunk(n_groups, ix.lay_r.ncb, mask_grid);
         void (*kern)(RowsParams) = threads == 896 ? k_mask_rows<W, W <= 4, 896> : k_mask_rows<W, W <= 4, 960>;
-        kern<<<mask_grid, threads, ix.lay_r.smem_bytes, L.stream>>>(prm);
+        size_t smem = ix.lay_r.smem_bytes + RW_RING * prm.chunk * 128u;
+        if (prm.mask == nullptr) { // counts only
+            kern = threads == 896 ? k_count_rows<W, W <= 4, 896> : k_count_rows<W, W <= 4, 960>;
+            smem = ix.lay_r.smem_bytes;
+        }
+        kern<<<mask_grid, threads, smem, L.stream>>>(prm);
         g_launches++;
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
         if (after_mask)

@@ -309,6 +309,14 @@ __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gmem_sr
                  "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
+// the same with an L2 cache policy (createpolicy) for the source lines
+__device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar, uint64_t pol) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+            smem_u32(smem_dst)),
+        "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
+        : "memory");
+}
 
 // ---- launch-side plumbing shared by the API and the kernel files ----
 // Arrays packed into one allocation in call order: take<T>(n) places n Ts at the next multiple of `align` and returns
