@@ -31,6 +31,7 @@ pub const KSH_RECONCILE_OK: c_int = 0;
 pub const KSH_RECONCILE_NO_NODE_FOUND: c_int = 1; // ReconcileError::NoNodeFound (src/error.rs)
 pub const KSH_RECONCILE_BINDING_OBJECT_FAILED: c_int = 2; // ReconcileError::CreateBindingObjectFailed
 pub const KSH_RECONCILE_GANG_UNSATISFIED: c_int = 4; // ksh_reconcile_gangs: the pod's group rolled back
+pub const KSH_RECONCILE_SPREAD_UNSATISFIED: c_int = 5; // ksh_reconcile_spread: spread constraints refused every node
 pub const KS_REFERENCE_ATTEMPTS: u32 = 5; // ATTEMPTS, src/main.rs:49
 pub const KS_MAX_PEERS: usize = 15;
 pub const KS_TOPK_MAX: u32 = 32; // largest k of ks_select_topk / ksh_rank_nodes
@@ -48,6 +49,8 @@ pub const KS_SPREAD_MAX_DOMAINS: u32 = 1 << 20; // most topology domains of one 
 pub const KS_SPREAD_MAX_EXISTING: u32 = 1 << 24; // most existing pods counted in one domain
 pub const KS_SPREAD_MAX_COUNTS: u64 = 1 << 26; // most specs x domains of existing or output counts
 pub const KS_SPREAD_MAX_KEYS: u32 = 4; // most topology keys of one ks_place_replicas_spread_multi call
+pub const KS_SPREAD_BIND_MAX_PODS: u32 = 65536; // most pods of one ks_spread_bind call
+pub const KS_SPREAD_BIND_MAX_GROUPS: u32 = 4096; // most groups of one ks_spread_bind call
 
 #[repr(C)]
 pub struct ks_kv {
@@ -256,6 +259,9 @@ extern "C" {
     pub fn ks_place_replicas_spread_multi(s: *mut ks_snapshot, specs: *const ks_pods, replicas: *const u32,
                                           spread: *const ks_spread_multi, policy: c_int, out: *mut ks_spread_plan,
                                           node: *mut i32, score: *mut i64, domain_count: *mut u32) -> c_int;
+    pub fn ks_spread_bind(s: *mut ks_snapshot, pods: *const ks_pods, group: *const i32, n_groups: u32,
+                          spread: *const ks_spread_multi, policy: c_int, node_idx: *mut i32, score: *mut i64,
+                          refused: *mut u32, domain_count: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -318,6 +324,11 @@ extern "C" {
                                            min_domains: *const u32, existing_node_names: *const *const c_char,
                                            existing_offset: *const u64, policy: c_int, out: *mut ks_spread_plan,
                                            node: *mut i32, score: *mut i64, domain_count: *mut u32) -> c_int;
+    pub fn ksh_reconcile_spread(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group: *const i32, n_groups: u32,
+                                topology_keys: *const *const c_char, n_keys: u32, max_skew: *const u32,
+                                min_domains: *const u32, existing_node_names: *const *const c_char,
+                                existing_offset: *const u64, policy: c_int, status: *mut i32, node_idx: *mut i32,
+                                json: *mut c_char, cap: usize, json_off: *mut i64) -> c_int;
     pub fn ksh_drain_nodes(ctx: *mut ksh_context, node_names: *const *const c_char, n: u64, pods: *const ks_pod_obj,
                            pod_offset: *const u64, policy: c_int, flags: u32, placed: *mut u32, node_idx: *mut i32) -> c_int;
     pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,

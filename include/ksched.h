@@ -642,6 +642,57 @@ int ks_place_replicas_spread_multi(ks_snapshot* s, const ks_pods* specs /* host 
                                    int64_t* out_score /* [sum replicas] or NULL */,
                                    uint32_t* out_domain_count /* [specs->n * S] or NULL */);
 
+/* ---- topology spread when binding: a mixed pod queue bound one pod at a time, each pod under its own workload's spread
+ * constraints (upstream kube-scheduler's one scheduling cycle per pod with PodTopologySpread, whenUnsatisfiable:
+ * DoNotSchedule; spec extension, DESIGN.md 5m) ----
+ * K = spread->n_keys keys, 1 <= K <= KS_SPREAD_MAX_KEYS, given as in ks_spread_multi: D_k = n_domains[k],
+ * node_domain[k][N] (-1 = node lacks the key), S = sum of D_k, P_k = D_0 + ... + D_{k-1}.  G = n_groups groups, one per
+ * workload (one constraint set); pod p belongs to group group[p] in [-1, G), -1 = the pod carries no constraint.
+ * Group g has max_skew[g * K + k] per key, 0 = g has no constraint on key k (so zone-only, zone + hostname and
+ * unconstrained workloads share one queue); C_g = the keys with max_skew >= 1.  min_domains[g * K + k] and
+ * existing[g * S + P_k + d] are optional, as in ks_spread_multi with T replaced by G.  Every pod of a group carries the
+ * same selector words (KS_ERR_INVALID otherwise), so eligibility is a property of the group.
+ *   1. group state, once per call, for every k in C_g: a node is eligible for g when it carries every key of C_g and g's
+ *      selector matches it (resource fit plays no part); E_{g,k} = the key-k domains that hold an eligible node;
+ *      cnt_{g,k} starts at existing; m_{g,k} = min of cnt_{g,k} over E_{g,k}, or 0 while |E_{g,k}| < min_domains;
+ *   2. pods run in array order, one at a time, each against the free[] and counts every earlier pod left.  Pod p's
+ *      candidates are the nodes it fits (both resources, non-strict), whose labels its selector matches, and, when
+ *      group[p] = g >= 0, that have for every k in C_g a domain d_k(n) >= 0 with cnt_{g,k}[d_k(n)] + 1 - m_{g,k} <=
+ *      max_skew[g * K + k].  The pod takes the candidate with the highest score under `policy` (ks_select's score against
+ *      the current free[], every policy), ties to the lower node index.  Its request is subtracted from free[n], and for
+ *      each k in C_g cnt_{g,k}[d_k(n)] rises by 1 and m_{g,k} is updated.  A pod with no candidate gets node -1 and score
+ *      0, and nothing changes.  A pod counts only toward its own group (selectors matching other groups' pods are out
+ *      of scope);
+ *   3. out_node_idx[P] (required); out_score[P], out_refused[P] and out_domain_count[G * S] may be NULL.  out_refused[p]
+ *      = the nodes that passed fit and selector at p's turn but that p's constraints refused (a missing key or the skew),
+ *      0 for an unconstrained pod: candidates + refused is the feasible count ks_select would report at that turn.
+ *      out_domain_count = the final cnt_{g,k} for k in C_g, existing (or 0) for the keys g does not constrain.
+ * free[] is charged, as with ks_gang_bind.  Identities:
+ *   (1) every pod in group -1, or every max_skew 0: nodes, scores and the final free[] are those of ks_gang_bind with one
+ *       singleton group per pod and min_member 0, under every policy;
+ *   (2) one group of R pods with identical requests that constrains every key: its nodes and scores are
+ *       ks_place_replicas_spread_multi's copy list for that spec with replicas = R, its counts that call's
+ *       out_domain_count, and the final free[] is free[] after ks_snapshot_commit_claims of that list (K = 1: the same
+ *       against ks_place_replicas_spread).  A pod that fails changes nothing, so every later identical pod of its group
+ *       fails too, which is the plan's stop rule.
+ * Checked on the host before any device work and before free[] changes: requests in [0, limit] (as ks_stream_bind,
+ * KS_ERR_RANGE); the per-key checks of ks_place_replicas_spread_multi (max_skew 0 allowed here); KS_ERR_INVALID for a
+ * group entry outside [-1, G), device-space pods, a bad policy, a NULL spread, group, max_skew (G > 0), node_domain[k] or
+ * out_node_idx (P > 0), or unequal selectors within a group; KS_ERR_RANGE for P > KS_SPREAD_BIND_MAX_PODS,
+ * G > KS_SPREAD_BIND_MAX_GROUPS or G * S > KS_SPREAD_MAX_COUNTS (the counts live on the device whether or not they are
+ * returned).  P = 0 does nothing; an empty snapshot places nothing and returns counts equal to existing.
+ * Host-space arguments and outputs.  One H2D copy; one kernel builds the group state (one CTA per group); one cooperative
+ * launch walks the pods with two grid barriers per pod, as ks_gang_bind's groups; one D2H copy.  Staging: the snapshot's
+ * pinned block and device input and result blocks hold the pods, 4 bytes per pod of groups and of refusals, 4 * K * N
+ * bytes of node domains, the groups' selectors and constraints and 4 * G * S bytes of counts; its device scratch block
+ * holds G * S bytes of eligible-domain flags and 16 bytes per (group, key). */
+#define KS_SPREAD_BIND_MAX_PODS 65536u
+#define KS_SPREAD_BIND_MAX_GROUPS 4096u
+int ks_spread_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const int32_t* group /* [P] */,
+                   uint32_t n_groups, const ks_spread_multi* spread /* max_skew etc. [G * K], existing [G * S] */,
+                   int policy, int32_t* out_node_idx /* [P] */, int64_t* out_score /* [P] or NULL */,
+                   uint32_t* out_refused /* [P] or NULL */, uint32_t* out_domain_count /* [G * S] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

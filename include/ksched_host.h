@@ -37,6 +37,9 @@ extern "C" {
                                                  also a pod without namespace (reference: unwrap panic, :80) */
 #define KSH_RECONCILE_BINDING_FAILED 3       /* ReconcileError::CreateBindingFailed: transport, caller side (:105-108) */
 #define KSH_RECONCILE_GANG_UNSATISFIED 4     /* ksh_reconcile_gangs: the pod's group could not place min_member pods */
+#define KSH_RECONCILE_SPREAD_UNSATISFIED 5   /* ksh_reconcile_spread: a node would take the pod but its spread constraints
+                                                refused every such node (upstream: "didn't match pod topology spread
+                                                constraints") */
 
 /* Kubernetes quantity strings, exact: cpu -> millicores, memory -> bytes.
  * KS_ERR_PARSE (malformed), KS_ERR_INEXACT (finer than 1m / 1 byte), KS_ERR_RANGE. */
@@ -254,6 +257,27 @@ int ksh_place_replicas_spread_multi(ksh_context* ctx, const ks_pod_obj* pods, ui
                                     const uint32_t* min_domains, const char* const* existing_node_names,
                                     const uint64_t* existing_offset, int policy, ks_spread_plan* out, int32_t* out_node,
                                     int64_t* out_score, uint32_t* out_domain_count);
+
+/* reconcile() under topology spread (ks_spread_bind, ksched.h): ksh_reconcile_batch with each workload's spread
+ * constraints.  Pod i belongs to group group[i] in [-1, n_groups) (-1 = no constraint; KS_ERR_INVALID otherwise), and
+ * every pod of a group must carry the same node selector.  Key k is topology_keys[k], numbered as
+ * ksh_context_topology_domains numbers it; max_skew [n_groups * K] (0 = the group does not constrain that key) and
+ * min_domains [n_groups * K] (or NULL) per (group, key).  Group g's existing pods under key k are
+ * existing_node_names[existing_offset[g * K + k] .. existing_offset[g * K + k + 1]) (existing_offset [n_groups * K + 1] or
+ * NULL; ks_pod_obj carries no pod labels, so the caller filters the pods); a name counts when it is in the store and its
+ * node carries key k and every key the group constrains.  Pods are filtered as ksh_reconcile_batch filters them: already
+ * bound pods are skipped (KSH_RECONCILE_OK, node -1) and count only when the caller lists them in existing; pods without
+ * namespace/name get KSH_RECONCILE_BINDING_OBJECT_FAILED.  The rest are bound one at a time in arrival order on the
+ * device, each against the capacity and counts every earlier pod left; binds are charged to the snapshot and the bound
+ * list, with Binding bodies in json / out_json_off, as ksh_reconcile_batch does.  An unbound pod gets
+ * KSH_RECONCILE_SPREAD_UNSATISFIED when some node passed fit and selector but its constraints refused every such node,
+ * else KSH_RECONCILE_NO_NODE_FOUND.  KS_ERR_RANGE for n_keys outside [1, KS_SPREAD_MAX_KEYS]; KS_ERR_NO_DEVICE on a
+ * packing-only context. */
+int ksh_reconcile_spread(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, const int32_t* group,
+                         uint32_t n_groups, const char* const* topology_keys, uint32_t n_keys, const uint32_t* max_skew,
+                         const uint32_t* min_domains, const char* const* existing_node_names,
+                         const uint64_t* existing_offset, int policy, int32_t* out_status, int32_t* out_node_idx,
+                         char* json, size_t cap, int64_t* out_json_off);
 
 #ifdef __cplusplus
 }

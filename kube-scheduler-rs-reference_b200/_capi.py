@@ -217,6 +217,10 @@ class ks_spread_multi(C.Structure):
 
 _proto("ks_place_replicas_spread_multi", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p,
        C.POINTER(ks_spread_multi), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
+_proto("ks_spread_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_uint32, C.POINTER(ks_spread_multi),
+       C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
+KS_SPREAD_BIND_MAX_PODS = 65536
+KS_SPREAD_BIND_MAX_GROUPS = 4096
 KS_PREEMPT_MAX_ABS_SUM = 1 << 62
 KS_ERR_INVALID, KS_ERR_RANGE = -1, -5
 KS_REFERENCE_ATTEMPTS = 5

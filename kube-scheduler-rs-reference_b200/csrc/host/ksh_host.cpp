@@ -33,6 +33,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 #pragma weak ks_place_replicas
 #pragma weak ks_place_replicas_spread
 #pragma weak ks_place_replicas_spread_multi
+#pragma weak ks_spread_bind
 
 namespace {
 
@@ -1706,6 +1707,98 @@ int ksh_place_replicas_spread_multi(ksh_context* c, const ks_pod_obj* pods, uint
                                     int64_t* out_score, uint32_t* out_domain_count) try {
     return place_spread_objects(c, true, pods, n, replicas, topology_keys, n_keys, max_skew, min_domains,
                                 existing_node_names, existing_offset, policy, out, out_node, out_score, out_domain_count);
+}
+KSH_CATCH
+
+// reconcile() under topology spread: ksh_reconcile_batch's filtering, then ks_spread_bind over the pods that go to the
+// device, each in its group.  Group g's existing pods under key k count when their node is in the store and carries key k
+// and every key g constrains.
+int ksh_reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
+                         const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
+                         const uint32_t* min_domains, const char* const* existing_node_names,
+                         const uint64_t* existing_offset, int policy, int32_t* out_status, int32_t* out_node_idx,
+                         char* json, size_t cap, int64_t* out_json_off) try {
+    if (!c || !topology_keys || (n && (!pods || !group || !out_status || !out_node_idx)) || (n_groups && !max_skew))
+        return fail(KS_ERR_INVALID, "NULL argument");
+    if (K == 0 || K > KS_SPREAD_MAX_KEYS)
+        return fail(KS_ERR_RANGE, std::to_string(K) + " topology keys (1 to " + std::to_string(KS_SPREAD_MAX_KEYS) + ")");
+    for (uint32_t k = 0; k < K; k++)
+        if (!topology_keys[k]) return fail(KS_ERR_INVALID, "NULL argument");
+    for (uint64_t i = 0; i < n; i++)
+        if (group[i] < -1 || group[i] >= (int64_t)n_groups)
+            return fail(KS_ERR_INVALID, "pod " + std::to_string(i) + ": group outside [-1, n_groups)");
+    const uint64_t gk = (uint64_t)n_groups * K;
+    if (existing_offset && existing_offset[gk] && !existing_node_names) return fail(KS_ERR_INVALID, "NULL existing_node_names");
+    if (existing_offset)
+        for (uint64_t i = 0; i < gk; i++)
+            if (existing_offset[i + 1] < existing_offset[i]) return fail(KS_ERR_INVALID, "existing offsets decrease");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    int rc = device_ready(c, ks_spread_bind, "ks_spread_bind");
+    if (rc) return rc;
+    std::vector<uint64_t> todo;
+    std::vector<ks_pod_obj> sub; // the pods that go to the device, in arrival order, and their groups
+    std::vector<int32_t> sub_group;
+    for (uint64_t i = 0; i < n; i++) {
+        out_node_idx[i] = -1;
+        if (out_json_off) out_json_off[i] = -1;
+        out_status[i] = reconcile_status(c, &pods[i]);
+        if (out_status[i] != KSH_RECONCILE_NO_NODE_FOUND) continue;
+        todo.push_back(i);
+        sub.push_back(pods[i]);
+        sub_group.push_back(group[i]);
+    }
+    if (todo.empty()) return KS_OK;
+    ks_pods kp;
+    rc = pack_batch(c, sub.data(), sub.size(), &kp);
+    if (rc) return rc;
+    std::vector<std::vector<int32_t>> dom(K, std::vector<int32_t>(c->N));
+    ks_spread_multi sp{};
+    uint32_t P[KS_SPREAD_MAX_KEYS] = {};
+    uint64_t S = 0;
+    for (uint32_t k = 0; k < K; k++) {
+        std::vector<uint32_t> values;
+        // no node carries the key: a single empty domain, so no node is eligible under it
+        sp.n_domains[k] = std::max(topology_domains(c, topology_keys[k], dom[k].data(), &values), 1u);
+        sp.node_domain[k] = dom[k].data();
+        P[k] = (uint32_t)S;
+        S += sp.n_domains[k];
+    }
+    std::vector<uint32_t> existing;
+    if (existing_offset) {
+        if (n_groups * S > KS_SPREAD_MAX_COUNTS) return fail(KS_ERR_RANGE, "too many groups x domains of counts (at most 2^26)");
+        existing.assign(n_groups * S, 0);
+        for (uint64_t g = 0; g < n_groups; g++)
+            for (uint32_t k = 0; k < K; k++)
+                for (uint64_t i = existing_offset[g * K + k]; i < existing_offset[g * K + k + 1]; i++) {
+                    const int32_t idx = existing_node_names[i] ? node_index_of(c, existing_node_names[i]) : -1;
+                    if (idx < 0) continue; // unknown: not counted
+                    bool all = dom[k][idx] >= 0;
+                    for (uint32_t k2 = 0; k2 < K; k2++) all &= max_skew[g * K + k2] == 0 || dom[k2][idx] >= 0;
+                    if (all) existing[g * S + P[k] + (uint32_t)dom[k][idx]]++;
+                }
+    }
+    sp.n_keys = K;
+    sp.max_skew = max_skew;
+    sp.min_domains = min_domains;
+    sp.existing = existing_offset ? existing.data() : nullptr;
+    std::vector<int32_t> idx(sub.size(), -1);
+    std::vector<uint32_t> refused(sub.size(), 0);
+    rc = ks_spread_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, policy, idx.data(), nullptr, refused.data(),
+                        nullptr); // commits capacity on the device
+    if (rc) {
+        c->dirty = true; // the host list is the truth
+        return rc;
+    }
+    StringList bodies{json, cap};
+    for (size_t k = 0; k < todo.size(); k++) {
+        const uint64_t i = todo[k];
+        if (idx[k] >= 0)
+            commit_bind(c, &pods[i], idx[k], kp.req_cpu[k], kp.req_mem[k], &out_status[i], &out_node_idx[i], bodies,
+                        json && out_json_off ? &out_json_off[i] : nullptr);
+        else if (refused[k] > 0)
+            out_status[i] = KSH_RECONCILE_SPREAD_UNSATISFIED;
+    }
+    return KS_OK;
 }
 KSH_CATCH
 

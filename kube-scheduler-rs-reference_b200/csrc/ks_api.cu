@@ -116,7 +116,7 @@ static int check_commit_requests(uint64_t n, const int64_t* req_cpu, const int64
 }
 
 // ---- host-staged calls: ks_stream_bind's device loop, ks_gang_bind, ks_drain_check, ks_scaleup_estimate,
-// ks_place_replicas and ks_place_replicas_spread (and _multi) ----
+// ks_place_replicas, ks_place_replicas_spread (and _multi) and ks_spread_bind ----
 // Such a call gathers its host inputs into the snapshot's pinned block, makes one H2D copy to d_in, launches, makes one
 // D2H copy from d_out and copies its results out before it returns.  Its HostStaged plan declares every array it stages
 // once, with its type and count: in() an input, gathered from src or, with src NULL, filled by the caller through
@@ -1614,6 +1614,24 @@ int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* repl
     return KS_OK;
 }
 
+// The keys of a ks_spread_multi against the snapshot's N nodes: 1 to KS_SPREAD_MAX_KEYS of them, each with a
+// node_domain, 1 to KS_SPREAD_MAX_DOMAINS domains and every node's domain in [-1, D).  *S = the sum of the domains.
+static int check_spread_keys(const ks_snapshot* s, const ks_spread_multi* spread, uint64_t* S) {
+    const uint32_t NK = spread->n_keys, N = s->N;
+    if (NK == 0 || NK > KS_SPREAD_MAX_KEYS) return fail(KS_ERR_RANGE, "%u topology keys (1 to %u)", NK, KS_SPREAD_MAX_KEYS);
+    *S = 0;
+    for (uint32_t k = 0; k < NK; k++) {
+        if (!spread->node_domain[k]) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
+        const uint32_t D = spread->n_domains[k];
+        if (D == 0 || D > KS_SPREAD_MAX_DOMAINS) return fail(KS_ERR_RANGE, "%u domains (1 to %u)", D, KS_SPREAD_MAX_DOMAINS);
+        for (uint32_t n = 0; n < N; n++)
+            if (spread->node_domain[k][n] < -1 || spread->node_domain[k][n] >= (int64_t)D)
+                return fail(KS_ERR_INVALID, "key %u, node %u: domain %d outside [-1, %u)", k, n, spread->node_domain[k][n], D);
+        *S += D;
+    }
+    return KS_OK;
+}
+
 // ks_place_replicas_spread is the K = 1 case of ks_place_replicas_spread_multi: one argument check, one staging plan
 // and one launcher for both.
 static int place_spread(ks_snapshot* s, const char* call, const ks_pods* specs, const uint32_t* replicas,
@@ -1625,17 +1643,9 @@ static int place_spread(ks_snapshot* s, const char* call, const ks_pods* specs, 
     const uint64_t T = specs->n;
     if (!spread || !spread->max_skew) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
     const uint32_t NK = spread->n_keys, N = s->N;
-    if (NK == 0 || NK > KS_SPREAD_MAX_KEYS) return fail(KS_ERR_RANGE, "%u topology keys (1 to %u)", NK, KS_SPREAD_MAX_KEYS);
-    uint64_t Stot = 0;
-    for (uint32_t k = 0; k < NK; k++) {
-        if (!spread->node_domain[k]) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
-        const uint32_t D = spread->n_domains[k];
-        if (D == 0 || D > KS_SPREAD_MAX_DOMAINS) return fail(KS_ERR_RANGE, "%u domains (1 to %u)", D, KS_SPREAD_MAX_DOMAINS);
-        for (uint32_t n = 0; n < N; n++)
-            if (spread->node_domain[k][n] < -1 || spread->node_domain[k][n] >= (int64_t)D)
-                return fail(KS_ERR_INVALID, "key %u, node %u: domain %d outside [-1, %u)", k, n, spread->node_domain[k][n], D);
-        Stot += D;
-    }
+    uint64_t Stot;
+    rc = check_spread_keys(s, spread, &Stot);
+    if (rc) return rc;
     for (uint64_t i = 0; i < T * NK; i++)
         if (spread->max_skew[i] == 0)
             return fail(KS_ERR_RANGE, "spec %llu, key %llu: max_skew 0 (at least 1)", (unsigned long long)(i / NK),
@@ -1779,6 +1789,139 @@ int ks_place_replicas_spread_multi(ks_snapshot* s, const ks_pods* specs, const u
                                    int64_t* out_score, uint32_t* out_domain_count) {
     return place_spread(s, "ks_place_replicas_spread_multi", specs, replicas, spread, policy, out, out_node, out_score,
                         out_domain_count);
+}
+
+int ks_spread_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
+                   const ks_spread_multi* spread, int policy, int32_t* out_node_idx, int64_t* out_score,
+                   uint32_t* out_refused, uint32_t* out_domain_count) {
+    int rc = check_pods(s, pods);
+    if (rc) return rc;
+    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_spread_bind takes host-space pods");
+    if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    const uint64_t P = pods->n, G = n_groups;
+    if (P && (!group || !out_node_idx)) return fail(KS_ERR_INVALID, "NULL group or out_node_idx");
+    if (!spread || (G && !spread->max_skew)) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
+    if (P > KS_SPREAD_BIND_MAX_PODS)
+        return fail(KS_ERR_RANGE, "%llu pods (at most %u)", (unsigned long long)P, KS_SPREAD_BIND_MAX_PODS);
+    if (G > KS_SPREAD_BIND_MAX_GROUPS)
+        return fail(KS_ERR_RANGE, "%llu groups (at most %u)", (unsigned long long)G, KS_SPREAD_BIND_MAX_GROUPS);
+    uint64_t S;
+    rc = check_spread_keys(s, spread, &S);
+    if (rc) return rc;
+    const uint32_t K = spread->n_keys, W = s->W, N = s->N;
+    const uint64_t GS = G * S;
+    if (GS > KS_SPREAD_MAX_COUNTS)
+        return fail(KS_ERR_RANGE, "%llu groups x %llu domains of counts (at most 2^26)", (unsigned long long)G,
+                    (unsigned long long)S);
+    if (spread->existing)
+        for (uint64_t i = 0; i < GS; i++)
+            if (spread->existing[i] > KS_SPREAD_MAX_EXISTING)
+                return fail(KS_ERR_RANGE, "group %llu, count %llu: %u existing pods (at most 2^24)",
+                            (unsigned long long)(i / S), (unsigned long long)(i % S), spread->existing[i]);
+    // every pod of a group carries the group's selector: first[g] = the first pod of group g, or -1
+    std::vector<int64_t> first;
+    try {
+        first.assign(G, -1);
+    } catch (...) {
+        return fail(KS_ERR_NOMEM, "out of host memory in ks_spread_bind");
+    }
+    for (uint64_t p = 0; p < P; p++) {
+        const int32_t g = group[p];
+        if (g < -1 || g >= (int64_t)G)
+            return fail(KS_ERR_INVALID, "pod %llu: group %d outside [-1, %u)", (unsigned long long)p, g, n_groups);
+        if (g < 0) continue;
+        if (first[g] < 0) first[g] = (int64_t)p;
+        else if (memcmp(pods->sel + p * W, pods->sel + first[g] * W, W * 8) != 0)
+            return fail(KS_ERR_INVALID, "pod %llu: selector differs from pod %lld of group %d", (unsigned long long)p,
+                        (long long)first[g], g);
+    }
+    rc = check_commit_requests(P, pods->req_cpu, pods->req_mem);
+    if (rc) return rc;
+    if (P == 0) return KS_OK;
+    if (N == 0) { // no node: nothing is placed, every count is existing
+        memset(out_node_idx, 0xff, P * 4);
+        if (out_score) memset(out_score, 0, P * 8);
+        if (out_refused) memset(out_refused, 0, P * 4);
+        if (out_domain_count) {
+            if (spread->existing) memcpy(out_domain_count, spread->existing, GS * 4);
+            else memset(out_domain_count, 0, GS * 4);
+        }
+        return KS_OK;
+    }
+    std::lock_guard<std::mutex> lk(s->mu);
+    CU_TRY(cudaSetDevice(s->device));
+    if (!s->coop) return fail(KS_ERR_CUDA, "device %d has no cooperative launch", s->device);
+    SpreadBindArgs a{};
+    a.grid = std::max(1u, std::min<uint32_t>((uint32_t)s->sms, (N + 127u) / 128u));
+    a.setup_grid = spread_bind_setup_grid((uint32_t)G, s->sms);
+    HostStaged h;
+    const auto cpu = h.in(pods->req_cpu, P), mem = h.in(pods->req_mem, P);
+    const auto sel = h.in(pods->sel, P * W);
+    const auto grp = h.in(group, P);
+    const auto max_skew = h.in(spread->max_skew, G * K);
+    const auto min_domains = h.in(spread->min_domains, spread->min_domains ? G * K : 0);
+    const auto existing = h.in(spread->existing, spread->existing ? GS : 0);
+    const auto dom = h.in<int32_t>(nullptr, (uint64_t)K * N);  // the K node_domain arrays, gathered below
+    const auto gsel = h.in<uint64_t>(nullptr, G * W);          // each group's selector
+    const auto score = h.out(out_score, P);
+    const auto idx = h.out(out_node_idx, P);
+    const auto refused = h.out(out_refused, P);
+    const auto count = h.out(out_domain_count, GS);           // the counts themselves: device state of the whole call
+    const auto elig = h.work<uint8_t>(GS);
+    const auto gk = h.work<uint32_t>(G * K * 4, 16);
+    const auto pkey = h.work<int64_t>(a.grid);
+    const auto pidx = h.work<int32_t>(a.grid);
+    const auto pref = h.work<uint32_t>(a.grid);
+    CU_TRY(h.reserve(s));
+    for (uint32_t k = 0; k < K; k++) memcpy(h.host(dom) + (size_t)k * N, spread->node_domain[k], (size_t)N * 4);
+    for (uint64_t g = 0; g < G; g++) {
+        uint64_t* row = h.host(gsel) + g * W;
+        if (first[g] >= 0) memcpy(row, pods->sel + first[g] * W, W * 8);
+        else memset(row, 0, W * 8);
+    }
+    cudaStream_t st = s->stream;
+    CU_TRY(h.upload(st));
+    a.N = N;
+    a.Npad = s->Npad;
+    a.P = (uint32_t)P;
+    a.G = (uint32_t)G;
+    a.K = K;
+    a.S = (uint32_t)S;
+    for (uint32_t k = 0, o = 0; k < K; o += spread->n_domains[k], k++) {
+        a.Dk[k] = spread->n_domains[k];
+        a.Pk[k] = o;
+    }
+    a.alloc_cpu = s->alloc_cpu.as<int64_t>();
+    a.alloc_mem = s->alloc_mem.as<int64_t>();
+    a.labels = s->labels.as<uint64_t>();
+    a.free_cpu = s->free_cpu.as<int64_t>();
+    a.free_mem = s->free_mem.as<int64_t>();
+    a.policy = policy;
+    a.req_cpu = h.dev(cpu);
+    a.req_mem = h.dev(mem);
+    a.sel = h.dev(sel);
+    a.group = h.dev(grp);
+    a.gsel = h.dev(gsel);
+    a.dom = h.dev(dom);
+    a.max_skew = h.dev(max_skew);
+    a.min_domains = spread->min_domains ? h.dev(min_domains) : nullptr;
+    a.existing = spread->existing ? h.dev(existing) : nullptr;
+    a.elig = h.dev(elig);
+    a.gk = h.dev(gk);
+    a.cnt = h.dev(count);
+    a.pkey = h.dev(pkey);
+    a.pidx = h.dev(pidx);
+    a.pref = h.dev(pref);
+    a.out_idx = h.dev(idx);
+    a.out_score = h.dev(score);
+    a.out_refused = h.dev(refused);
+    s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
+    s->version++;
+    cudaError_t e = launch_spread_bind(a, W, st);
+    if (e != cudaSuccess) return fail(KS_ERR_CUDA, "spread bind launch failed: %s", cudaGetErrorString(e));
+    CU_TRY(h.finish(st));
+    s->last_path = "spread_bind";
+    return KS_OK;
 }
 
 // ---------------------------------------------------------------------------------------------- async streaming

@@ -227,4 +227,36 @@ struct GangArgs {
     uint32_t* placed;           // [n]: pods the round loop bound (before any rollback)
 };
 cudaError_t launch_gang_batch(const StreamBatchArgs& a, const GangArgs& g, uint32_t W, cudaStream_t st);
+
+// topology spread when binding (ks_spread_bind, ks_spread_bind.cu): k_spread_bind_setup (one CTA per group, grid-strided
+// over setup_grid CTAs; not launched when G = 0), then one cooperative launch of grid CTAs that walks the P pods.
+// Device memory.  Key k's domains are the counts [Pk[k], Pk[k] + Dk[k]) of each group's S.
+struct SpreadBindArgs {
+    uint32_t N, Npad, P, G, K, S;
+    uint32_t Dk[KS_SPREAD_MAX_KEYS], Pk[KS_SPREAD_MAX_KEYS];
+    const int64_t *alloc_cpu, *alloc_mem;
+    const uint64_t* labels;
+    int64_t *free_cpu, *free_mem;   // charged
+    int policy;
+    const int64_t *req_cpu, *req_mem; // [P]
+    const uint64_t* sel;              // [P * W], row-major
+    const int32_t* group;             // [P], each in [-1, G)
+    const uint64_t* gsel;             // [G * W]: each group's selector (the same in all its pods)
+    const int32_t* dom;               // [K * N]: key k's node_domain at k * N
+    const uint32_t* max_skew;         // [G * K], 0 = key not constrained
+    const uint32_t* min_domains;      // [G * K] or null
+    const uint32_t* existing;         // [G * S] or null
+    uint8_t* elig;                    // [G * S] eligible-domain flags
+    uint32_t* gk;                     // [G * K * 4] per (group, key): m, domains at m, |E|, flags
+    uint32_t* cnt;                    // [G * S] counts, final after the call
+    int64_t* pkey;                    // [grid] per-CTA partials
+    int32_t* pidx;
+    uint32_t* pref;
+    int32_t* out_idx;                 // [P]
+    int64_t* out_score;               // [P]
+    uint32_t* out_refused;            // [P]
+    uint32_t grid, setup_grid;
+};
+uint32_t spread_bind_setup_grid(uint32_t G, int sms);
+cudaError_t launch_spread_bind(const SpreadBindArgs& a, uint32_t W, cudaStream_t st);
 } // namespace ks

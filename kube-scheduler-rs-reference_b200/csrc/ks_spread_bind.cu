@@ -1,0 +1,292 @@
+// ks_spread_bind.cu — topology spread when binding (ks_spread_bind, include/ksched.h; DESIGN.md 5m).
+// A mixed pod queue is bound one pod at a time, each pod under its group's spread constraints against the counts and the
+// free[] every earlier pod left, as upstream kube-scheduler runs one scheduling cycle per pod.  Two kernels:
+//   k_spread_bind_setup  one CTA per group (grid-strided): the group's eligible domains per constrained key, its counts
+//                        (existing, or 0), and per key |E|, m, the number of eligible domains at m and the minDomains flag
+//   k_spread_bind_seq    one cooperative launch that walks the pods, shaped like k_gang_batch (ks_stream.cu): every CTA
+//                        owns one slice of the node table; per pod, phase A scans every slice and writes one partial per
+//                        CTA, phase B (CTA 0) merges the partials in CTA order, charges free[], writes the binding and
+//                        raises the counts; the two phases are separated by grid barriers.
+#include "ks_internal.cuh"
+#include "ks_launch.h"
+
+#include <algorithm>
+#include <cooperative_groups.h>
+namespace cg = cooperative_groups;
+
+namespace ks {
+
+constexpr uint32_t SBD_THREADS = 256;
+constexpr uint32_t SBD_WARPS = SBD_THREADS / 32;
+
+// Per (group, key) state words in a.gk: the minimum m, the eligible domains whose count is m, |E| and the flags
+enum : uint32_t { GK_M = 0, GK_AT_M = 1, GK_NE = 2, GK_FLAGS = 3, GK_WORDS = 4 };
+constexpr uint32_t GK_CONSTRAINED = 1u, GK_FORCED = 2u; // max_skew >= 1; minDomains holds m at 0
+
+// CTA-wide sum and minimum of one value per thread; every thread gets the result.  s holds SBD_WARPS words.
+__device__ __forceinline__ uint32_t cta_sum(uint32_t v, uint32_t* s) {
+    v = __reduce_add_sync(0xffffffffu, v);
+    __syncthreads(); // s is free
+    if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = v;
+    __syncthreads();
+    uint32_t r = 0;
+#pragma unroll
+    for (uint32_t w = 0; w < SBD_WARPS; w++) r += s[w];
+    return r;
+}
+__device__ __forceinline__ uint32_t cta_min(uint32_t v, uint32_t* s) {
+    v = __reduce_min_sync(0xffffffffu, v);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = v;
+    __syncthreads();
+    uint32_t r = 0xffffffffu;
+#pragma unroll
+    for (uint32_t w = 0; w < SBD_WARPS; w++) r = min(r, s[w]);
+    return r;
+}
+
+// The keys group g constrains, one bit per key (max_skew >= 1)
+__device__ __forceinline__ uint32_t constrained_keys(const SpreadBindArgs& a, int32_t g) {
+    uint32_t ck = 0;
+    if (g >= 0)
+        for (uint32_t k = 0; k < a.K; k++)
+            if (__ldg(a.max_skew + (size_t)g * a.K + k)) ck |= 1u << k;
+    return ck;
+}
+
+// The eligible domains of key k at count m: the domain count of a (group, key) after its minimum has risen
+__device__ __forceinline__ uint32_t domains_at(const SpreadBindArgs& a, uint32_t g, uint32_t k, uint32_t m, uint32_t* s) {
+    const size_t base = (size_t)g * a.S + a.Pk[k];
+    uint32_t c = 0;
+    for (uint32_t d = threadIdx.x; d < a.Dk[k]; d += SBD_THREADS)
+        c += a.elig[base + d] && __ldcg(a.cnt + base + d) == m;
+    return cta_sum(c, s);
+}
+
+template <int W>
+__global__ void __launch_bounds__(SBD_THREADS) k_spread_bind_setup(const SpreadBindArgs a) {
+    __shared__ uint32_t s_red[SBD_WARPS];
+    const uint32_t tid = threadIdx.x;
+    for (uint32_t g = blockIdx.x; g < a.G; g += gridDim.x) {
+        uint32_t* cnt = a.cnt + (size_t)g * a.S;
+        uint8_t* el = a.elig + (size_t)g * a.S;
+        for (uint32_t i = tid; i < a.S; i += SBD_THREADS) {
+            cnt[i] = a.existing ? __ldg(a.existing + (size_t)g * a.S + i) : 0u;
+            el[i] = 0;
+        }
+        const uint32_t ck = constrained_keys(a, (int32_t)g);
+        __syncthreads();
+        if (ck) { // eligible: the group's selector matches and the node carries every key the group constrains
+            uint64_t sw[W];
+#pragma unroll
+            for (int w = 0; w < W; w++) sw[w] = __ldg(a.gsel + (size_t)g * W + w);
+            for (uint32_t n = tid; n < a.N; n += SBD_THREADS) {
+                uint64_t miss = 0;
+#pragma unroll
+                for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
+                if (miss) continue;
+                int32_t d[KS_SPREAD_MAX_KEYS];
+                bool all = true;
+#pragma unroll
+                for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) {
+                    d[k] = (ck >> k & 1u) ? __ldg(a.dom + (size_t)k * a.N + n) : 0;
+                    all &= d[k] >= 0;
+                }
+                if (!all) continue;
+#pragma unroll
+                for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
+                    if (ck >> k & 1u) el[a.Pk[k] + (uint32_t)d[k]] = 1;
+            }
+        }
+        __syncthreads();
+        for (uint32_t k = 0; k < a.K; k++) {
+            uint32_t* st = a.gk + ((size_t)g * a.K + k) * GK_WORDS;
+            if (!(ck >> k & 1u)) {
+                if (tid < GK_WORDS) st[tid] = 0;
+                continue;
+            }
+            uint32_t ne = 0, mn = 0xffffffffu;
+            for (uint32_t d = tid; d < a.Dk[k]; d += SBD_THREADS)
+                if (el[a.Pk[k] + d]) {
+                    ne++;
+                    mn = min(mn, cnt[a.Pk[k] + d]);
+                }
+            ne = cta_sum(ne, s_red);
+            mn = cta_min(mn, s_red);
+            const uint32_t mind = a.min_domains ? __ldg(a.min_domains + (size_t)g * a.K + k) : 0u;
+            const bool forced = ne < mind; // upstream's minDomains: the global minimum counts as 0
+            const uint32_t m = ne == 0 || forced ? 0u : mn;
+            const uint32_t at = ne == 0 || forced ? 0u : domains_at(a, g, k, m, s_red);
+            if (tid == 0) {
+                st[GK_M] = m;
+                st[GK_AT_M] = at;
+                st[GK_NE] = ne;
+                st[GK_FLAGS] = GK_CONSTRAINED | (forced ? GK_FORCED : 0u);
+            }
+        }
+        __syncthreads(); // el and cnt of this group are final before the CTA's next group
+    }
+}
+
+// Phase A of pod p in this CTA's slice [n0, n1): fit, selector and, for a constrained pod, cnt < m + max_skew on every
+// constrained key; the best candidate by the policy's key (ties to the lower node) and the refused count into the CTA's
+// partial
+template <int W>
+__device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32_t p, uint32_t n0, uint32_t n1,
+                                                 int64_t* s_key, int32_t* s_idx, uint32_t* s_ref) {
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int32_t g = __ldg(a.group + p);
+    const int64_t rc = __ldg(a.req_cpu + p), rm = __ldg(a.req_mem + p);
+    uint64_t sw[W];
+#pragma unroll
+    for (int w = 0; w < W; w++) sw[w] = __ldg(a.sel + (size_t)p * W + w);
+    const uint32_t ck = constrained_keys(a, g);
+    uint64_t lim[KS_SPREAD_MAX_KEYS]; // a domain admits while its count is below m + max_skew
+#pragma unroll
+    for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
+        lim[k] = (ck >> k & 1u) ? (uint64_t)__ldcg(a.gk + ((size_t)g * a.K + k) * GK_WORDS + GK_M) +
+                                      __ldg(a.max_skew + (size_t)g * a.K + k)
+                                : 0;
+    const uint32_t* cnt = a.cnt + (size_t)(g < 0 ? 0 : g) * a.S;
+    int64_t best = INT64_MIN;
+    int32_t bidx = -1;
+    uint32_t refused = 0;
+    for (uint32_t n = n0 + tid; n < n1; n += SBD_THREADS) {
+        const int64_t fc = __ldcg(a.free_cpu + n), fm = __ldcg(a.free_mem + n);
+        uint64_t miss = 0;
+#pragma unroll
+        for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
+        if (!(rc <= fc && rm <= fm && miss == 0)) continue;
+        bool ok = true;
+#pragma unroll
+        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
+            if (ck >> k & 1u) {
+                const int32_t d = __ldg(a.dom + (size_t)k * a.N + n);
+                ok &= d >= 0 && __ldcg(cnt + a.Pk[k] + (uint32_t)max(d, 0)) < lim[k];
+            }
+        if (!ok) {
+            refused++;
+            continue;
+        }
+        const int64_t key = alloc_score_rt(a.policy, fc, fm, a.alloc_cpu, a.alloc_mem, n, rc, rm);
+        if (key > best) { // ascending n per thread: strict '>' keeps the lowest index
+            best = key;
+            bidx = (int32_t)n;
+        }
+    }
+    warp_argmax(best, bidx);
+    refused = __reduce_add_sync(0xffffffffu, refused);
+    if (lane == 0) {
+        s_key[warp] = best;
+        s_idx[warp] = bidx;
+        s_ref[warp] = refused;
+    }
+    __syncthreads();
+    if (warp == 0) {
+        best = lane < SBD_WARPS ? s_key[lane] : INT64_MIN;
+        bidx = lane < SBD_WARPS ? s_idx[lane] : -1;
+        warp_argmax(best, bidx);
+        refused = __reduce_add_sync(0xffffffffu, lane < SBD_WARPS ? s_ref[lane] : 0u);
+        if (lane == 0) {
+            a.pkey[blockIdx.x] = best;
+            a.pidx[blockIdx.x] = bidx;
+            a.pref[blockIdx.x] = refused;
+        }
+    }
+}
+
+// Phase B of pod p, CTA 0 only: merge the partials in CTA order, write the binding, charge free[] and raise the group's
+// counts.  When the last eligible domain at m takes the pod, m rises by exactly one and the domains at the new m are
+// counted over the group's domains of that key (the counts only rise, so at most final m - initial m such passes).
+__device__ __forceinline__ void spread_bind_commit(const SpreadBindArgs& a, uint32_t p, uint32_t* s_rescan,
+                                                   uint32_t* s_red) {
+    const uint32_t tid = threadIdx.x, lane = tid & 31;
+    const int32_t g = __ldg(a.group + p);
+    if (tid < 32) {
+        int64_t best = INT64_MIN;
+        int32_t bidx = -1;
+        uint32_t refused = 0;
+        for (uint32_t c = lane; c < gridDim.x; c += 32) { // ascending CTA = ascending node range
+            merge_partial(best, bidx, __ldcg(a.pkey + c), __ldcg(a.pidx + c));
+            refused += __ldcg(a.pref + c);
+        }
+        warp_argmax(best, bidx);
+        refused = __reduce_add_sync(0xffffffffu, refused);
+        if (lane == 0) {
+            uint32_t rescan = 0;
+            a.out_idx[p] = bidx;
+            a.out_score[p] = bidx >= 0 ? key_score_rt(a.policy, best, a.req_cpu, a.req_mem, p) : 0;
+            a.out_refused[p] = refused;
+            if (bidx >= 0) {
+                a.free_cpu[bidx] = __ldcg(a.free_cpu + bidx) - __ldg(a.req_cpu + p);
+                a.free_mem[bidx] = __ldcg(a.free_mem + bidx) - __ldg(a.req_mem + p);
+                const uint32_t ck = constrained_keys(a, g);
+                for (uint32_t k = 0; k < a.K; k++) {
+                    if (!(ck >> k & 1u)) continue;
+                    const uint32_t d = (uint32_t)__ldg(a.dom + (size_t)k * a.N + bidx);
+                    uint32_t* c = a.cnt + (size_t)g * a.S + a.Pk[k] + d;
+                    const uint32_t before = __ldcg(c);
+                    *c = before + 1;
+                    uint32_t* st = a.gk + ((size_t)g * a.K + k) * GK_WORDS;
+                    if ((__ldcg(st + GK_FLAGS) & GK_FORCED) || before != __ldcg(st + GK_M)) continue;
+                    const uint32_t at = __ldcg(st + GK_AT_M) - 1;
+                    st[GK_AT_M] = at;
+                    if (at == 0) { // the last domain at m took the pod: m + 1, and its domains are counted below
+                        st[GK_M] = before + 1;
+                        rescan |= 1u << k;
+                    }
+                }
+            }
+            *s_rescan = rescan;
+        }
+    }
+    __syncthreads();
+    const uint32_t rescan = *s_rescan;
+    for (uint32_t k = 0; k < a.K; k++) {
+        if (!(rescan >> k & 1u)) continue;
+        uint32_t* st = a.gk + ((size_t)g * a.K + k) * GK_WORDS;
+        const uint32_t at = domains_at(a, (uint32_t)g, k, __ldcg(st + GK_M), s_red);
+        if (tid == 0) st[GK_AT_M] = at;
+    }
+}
+
+template <int W>
+__global__ void __launch_bounds__(SBD_THREADS, 1) k_spread_bind_seq(const SpreadBindArgs a) {
+    cg::grid_group grid = cg::this_grid();
+    __shared__ int64_t s_key[SBD_WARPS];
+    __shared__ int32_t s_idx[SBD_WARPS];
+    __shared__ uint32_t s_ref[SBD_WARPS];
+    __shared__ uint32_t s_rescan;
+    const uint32_t G = gridDim.x;
+    const uint32_t chunk = (a.N + G - 1) / G, n0 = min(a.N, blockIdx.x * chunk), n1 = min(a.N, n0 + chunk);
+    for (uint32_t p = 0; p < a.P; p++) {
+        spread_bind_scan<W>(a, p, n0, n1, s_key, s_idx, s_ref);
+        __threadfence();
+        grid.sync();
+        if (blockIdx.x == 0) spread_bind_commit(a, p, &s_rescan, s_ref);
+        __threadfence();
+        grid.sync();
+    }
+}
+
+uint32_t spread_bind_setup_grid(uint32_t G, int sms) { return std::max(1u, std::min<uint32_t>(G, 4u * (uint32_t)sms)); }
+
+cudaError_t launch_spread_bind(const SpreadBindArgs& a, uint32_t W, cudaStream_t st) {
+    return with_label_width(W, [&](auto w) {
+        constexpr int LW = decltype(w)::value;
+        if (a.G) {
+            k_spread_bind_setup<LW><<<a.setup_grid, SBD_THREADS, 0, st>>>(a);
+            g_launches++;
+            const cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess) return e;
+        }
+        SpreadBindArgs b = a;
+        void* args[] = {&b};
+        const cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(k_spread_bind_seq<LW>),
+                                                          dim3(a.grid), dim3(SBD_THREADS), args, 0, st);
+        if (e == cudaSuccess) g_launches++;
+        return e;
+    });
+}
+
+} // namespace ks

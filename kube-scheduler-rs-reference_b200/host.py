@@ -50,12 +50,15 @@ for _name, _res, _args in [
                                             _vp, _vp, _vp]),
     ("ksh_place_replicas_spread_multi", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp,
                                                   C.c_int, _vp, _vp, _vp, _vp]),
+    ("ksh_reconcile_spread", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp, C.c_int,
+                                       _vp, _vp, _vp, C.c_size_t, _vp]),
 ]:
     _proto(_name, _res, *_args)
 
 KSH_DEVICE_NONE = -1  # packing-only context: objects -> SoA arrays on the host, no predicate is ever evaluated
 KSH_RECONCILE_OK, KSH_RECONCILE_NO_NODE_FOUND, KSH_RECONCILE_BINDING_OBJECT_FAILED = 0, 1, 2
 KSH_RECONCILE_GANG_UNSATISFIED = 4
+KSH_RECONCILE_SPREAD_UNSATISFIED = 5
 
 
 def _addr(arr, i=0):
@@ -396,6 +399,40 @@ class Context:
                                       C.addressof(buf), cap, off.ctypes.data), "ksh_reconcile_gangs")
         bodies = _string_list(buf, off)
         return status, node, bodies, placed
+
+    def reconcile_spread(self, pods, n, group, n_groups, topology_keys, max_skew, min_domains=None, existing_nodes=None,
+                         policy=capi.KS_SCORE_LEFTOVER, json_cap=None):
+        """reconcile() under topology spread (ksh_reconcile_spread): pod i belongs to group group[i] (-1 = none), each
+        group with max_skew and min_domains [n_groups, K] over topology_keys (max_skew 0 = the key is not constrained);
+        existing_nodes[g][k] lists the node names of group g's bound pods for key k (None: none).  Pods are bound one at
+        a time in arrival order.  Returns (status[n], node_idx[n], bodies[n] (str | None))."""
+        k = len(topology_keys)
+        group = np.ascontiguousarray(group, np.int32).reshape(-1)
+        max_skew = np.ascontiguousarray(max_skew, np.uint32).reshape(-1)
+        if group.shape[0] != n or max_skew.shape[0] != n_groups * k:
+            raise ValueError(f"group / max_skew have {group.shape[0]} / {max_skew.shape[0]} entries, pods {n}, groups "
+                             f"{n_groups}, keys {k}")
+        mind = None if min_domains is None else np.ascontiguousarray(min_domains, np.uint32).reshape(-1)
+        names, ex_off = None, None
+        if existing_nodes is not None:
+            lists = [lst for per_group in existing_nodes for lst in per_group]
+            flat = [s.encode() for lst in lists for s in lst]
+            names = (C.c_char_p * max(len(flat), 1))(*flat)
+            ex_off = np.zeros(n_groups * k + 1, np.uint64)
+            np.cumsum([len(lst) for lst in lists], out=ex_off[1:])
+        keys = (C.c_char_p * max(k, 1))(*[key.encode() for key in topology_keys])
+        status = np.empty(n, np.int32)
+        node = np.empty(n, np.int32)
+        off = np.empty(n, np.int64)
+        cap = int(json_cap if json_cap is not None else 512 * max(n, 1))
+        buf = C.create_string_buffer(max(cap, 1))
+        check(lib.ksh_reconcile_spread(self._h, C.addressof(pods) if n else None, n, group.ctypes.data, int(n_groups),
+                                       C.cast(keys, _vp), k, max_skew.ctypes.data,
+                                       None if mind is None else mind.ctypes.data,
+                                       None if names is None else C.cast(names, _vp),
+                                       None if ex_off is None else ex_off.ctypes.data, int(policy), status.ctypes.data,
+                                       node.ctypes.data, C.addressof(buf), cap, off.ctypes.data), "ksh_reconcile_spread")
+        return status, node, _string_list(buf, off)
 
     def drain_nodes(self, node_names, pods, pod_offset, policy=capi.KS_SCORE_LEFTOVER, flags=0):
         """Drain simulation over objects (ksh_drain_nodes): candidate d is the node named node_names[d] with pods

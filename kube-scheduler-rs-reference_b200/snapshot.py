@@ -353,6 +353,48 @@ class Snapshot:
             counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
         return rows, node, score, offset, counts
 
+    def spread_bind(self, req_cpu, req_mem, sel, group, keys, max_skew, min_domains=None, existing=None,
+                    policy=capi.KS_SCORE_LEFTOVER, want_counts=True):
+        """Bind a mixed pod queue one pod at a time under each workload's spread constraints (ks_spread_bind): pod p
+        belongs to group group[p] (-1 = unconstrained); keys is a list of K (node_domain, n_domains) pairs; max_skew
+        [G, K] (0 = the group does not constrain that key), min_domains [G, K] or None, existing None or a list of K
+        arrays [G, n_domains_k].  G = len(max_skew).  Charges free[].  Returns (node_idx int32 [P], score int64 [P],
+        refused uint32 [P], counts): counts a list of K arrays uint32 [G, n_domains_k] (None unless want_counts)."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        p = int(pods.n)
+        group = _c(group, np.int32).reshape(-1)
+        if group.shape[0] != p:
+            raise ValueError(f"group has {group.shape[0]} entries, pods {p}")
+        k = len(keys)
+        if not 1 <= k <= capi.KS_SPREAD_MAX_KEYS:
+            raise ValueError(f"{k} topology keys (1 to {capi.KS_SPREAD_MAX_KEYS})")
+        doms = [_c(d, np.int32).reshape(-1) for d, _ in keys]
+        nd = [int(n) for _, n in keys]
+        max_skew = _c(max_skew, np.uint32).reshape(-1, k)
+        g = max_skew.shape[0]
+        if min_domains is not None:
+            min_domains = _c(min_domains, np.uint32).reshape(-1)
+            if min_domains.shape[0] != g * k:
+                raise ValueError(f"min_domains has {min_domains.shape[0]} entries, groups x keys {g * k}")
+        s = sum(nd)
+        if existing is not None:
+            if len(existing) != k:
+                raise ValueError(f"existing has {len(existing)} blocks, keys {k}")
+            existing = _c(np.concatenate([np.asarray(e, np.uint32).reshape(g, n) for e, n in zip(existing, nd)],
+                                         axis=1), np.uint32).reshape(-1)
+        spread = capi.ks_spread_multi(k, (C.c_uint32 * capi.KS_SPREAD_MAX_KEYS)(*nd),
+                                      (C.c_void_p * capi.KS_SPREAD_MAX_KEYS)(*[_ptr(d) for d in doms]),
+                                      _ptr(max_skew), _ptr(min_domains), _ptr(existing))
+        idx = np.empty(p, np.int32)
+        score = np.empty(p, np.int64)
+        refused = np.empty(p, np.uint32)
+        counts = np.empty((g, s), np.uint32) if want_counts and 0 < g * s <= capi.KS_SPREAD_MAX_COUNTS else None
+        check(lib.ks_spread_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(spread), int(policy), _ptr(idx),
+                                 _ptr(score), _ptr(refused), _ptr(counts)), "ks_spread_bind")
+        if counts is not None:
+            counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
+        return idx, score, refused, counts
+
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
         """The reference's own policy (src/main.rs:49-71), seeded: (node_idx, attempts_used, draw_node, draw_code)."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
