@@ -127,6 +127,157 @@ def pod_slack(rc, rm, amax_c, amax_m, amin_c, amin_m):
     return dl - e
 
 
+# ---- the bit-parallel walk of both policies (bound_walk in ks_bitpar.cu, DESIGN.md 5i / 5j), restated ----
+I64_MAX = (1 << 63) - 1
+LB_UNBOUNDED = 1 << 62  # LEAST_BALANCED's stored bound above 200
+TILE, FIRST_WINDOW, WINDOW = 256, 8, 32
+
+
+def most_bound(fc, fm, ac, am):
+    """MOST_ALLOCATED's b(n) = term(f_c, A_c, 0) + term(f_m, A_m, 0), in [0, 200]."""
+    return term(int(fc), int(ac), 0) + term(int(fm), int(am), 0)
+
+
+def most_slack(rc, rm, amin_c, amin_m):
+    """MOST_ALLOCATED's D: every feasible cell of a pod with requests >= 0 scores <= (b(n) + D) // 2."""
+    return slack(rc, amin_c) + slack(rm, amin_m)
+
+
+def stored_bound(policy, fc, fm, ac, am):
+    """The bound the walk's order stores for a node: MOST_ALLOCATED's b(n); LEAST_BALANCED's b(n) as k_balanced_order
+    stores it, LB_UNBOUNDED above 200 and 0 below 0."""
+    if policy == MOST_ALLOCATED:
+        return most_bound(fc, fm, ac, am)
+    b = node_bound(int(fc), int(fm), int(ac), int(am))
+    return LB_UNBOUNDED if b > 200 else max(b, 0)
+
+
+def walk_limit(policy, top, d):
+    """The highest score a feasible cell in a slot of bound `top' can have: (top + D) / 2 or top - D (C division)."""
+    if policy == MOST_ALLOCATED:
+        x = top + d
+        return abs(x) // 2 * (1 if x >= 0 else -1)
+    return top - d
+
+
+def walk_packed(oracle, free_cpu, free_mem, alloc_cpu, alloc_mem, labels, req_cpu, req_mem, sel, policy, margin=0):
+    """k_most_alloc / k_least_balanced's control flow, not only its result: nodes in descending stored bound (ties to
+    the lower index), tiles of 256 slots in windows of 8 then 32 tiles, the exit test `best > limit(top) + margin' in
+    front of each window (from the second on) and in front of each tile with a feasible slot, no exit for a negative
+    request, an immediate -1 for a pod that fits nowhere by rank or selector.  margin shifts the exit limit (-1: an exit
+    one step too early) so that a test can show its cases would catch that.  Feasibility comes from the oracle's cell
+    codes.  Returns (node, score, scored, exit): per pod the tiles it scored and the tile in front of which it stopped
+    (-1: it walked to the end)."""
+    fc, fm = np.asarray(free_cpu, np.int64), np.asarray(free_mem, np.int64)
+    ac, am = np.asarray(alloc_cpu, np.int64), np.asarray(alloc_mem, np.int64)
+    rc, rm = np.asarray(req_cpu, np.int64), np.asarray(req_mem, np.int64)
+    N, P = fc.shape[0], rc.shape[0]
+    lab = np.ascontiguousarray(labels, np.uint64).reshape(N, -1)
+    sel = np.ascontiguousarray(sel, np.uint64).reshape(P, -1)
+    codes = oracle.orc.run_packed(fc, fm, ac, am, lab, rc, rm, sel, 0, want_mask=False, want_codes=True)[4]
+    bound = np.array([stored_bound(policy, *v) for v in zip(fc, fm, ac, am)], np.int64)
+    order = np.lexsort((np.arange(N), -bound))
+    top = bound[order]
+    n_tiles = (N + TILE - 1) // TILE
+    amax_c = I64_MAX if (ac <= 0).any() else int(ac.max())  # k_node_bound: a node with A <= 0 gives no slack
+    amax_m = I64_MAX if (am <= 0).any() else int(am.max())
+    amin_c = int(ac[ac > 0].min()) if (ac > 0).any() else I64_MAX
+    amin_m = int(am[am > 0].min()) if (am > 0).any() else I64_MAX
+    live = np.bitwise_or.reduce(lab, axis=0) if N else np.zeros(lab.shape[1], np.uint64)
+    score = SCORES[policy]
+    idx, sc = np.full(P, -1, np.int32), np.zeros(P, np.int64)
+    scored, exits = [], np.full(P, -1, np.int64)
+    for p in range(P):
+        q_c, q_m = int(rc[p]), int(rm[p])
+        seen = []
+        scored.append(seen)
+        if N == 0 or q_c > fc.max() or q_m > fm.max() or (sel[p] & ~live).any():
+            continue  # dead: k_pod_ranks' rank is N, or a required pair no node carries
+        bounded = q_c >= 0 and q_m >= 0
+        if not bounded:
+            d = 0
+        elif policy == MOST_ALLOCATED:
+            d = most_slack(q_c, q_m, amin_c, amin_m)
+        else:
+            d = pod_slack(q_c, q_m, amax_c, amax_m, amin_c, amin_m)
+        feas = codes[p][order] == 0
+        best, bidx = 0, -1
+
+        def stop(k):
+            return bounded and bidx >= 0 and best > walk_limit(policy, int(top[k * TILE]), d) + margin
+
+        k0, win = 0, FIRST_WINDOW
+        while exits[p] < 0 and k0 < n_tiles:
+            if k0 > 0 and stop(k0):
+                exits[p] = k0
+                break
+            for k in range(k0, min(k0 + win, n_tiles)):
+                f = np.nonzero(feas[k * TILE:(k + 1) * TILE])[0] + k * TILE
+                if not len(f):
+                    continue
+                if stop(k):
+                    exits[p] = k
+                    break
+                seen.append(k)
+                n = order[f]
+                s = score(fc[n], fm[n], ac[n], am[n], q_c, q_m)
+                j = np.lexsort((n, -s))[0]
+                if bidx < 0 or s[j] > best or (s[j] == best and n[j] < bidx):
+                    best, bidx = int(s[j]), int(n[j])
+            k0 += win
+            win = WINDOW
+        idx[p], sc[p] = bidx, best if bidx >= 0 else 0
+    return idx, sc, scored, exits
+
+
+# ---- clusters that put the winner exactly at an exit of the walk ----
+# Per policy, three node profiles as (share of cpu, share of memory) in percent, on allocatables of 100 and 100 MiB so
+# that every share is exact, for zero-request pods (D = 0, the bound is attained): X, Y with X one bound above Y and
+# the same score, and Y' one score below X.  MOST_ALLOCATED: b = 2k + 1 and 2k both score k.  LEAST_BALANCED: shares
+# 40 / 41 give b = 159 and score 158 (|P_c - P_m| = 1: bal = 100, balanced = trunc(99.5)); equal shares 42 score
+# their bound 158.  `before' nodes bound above X, `after' nodes below Y and Y'.
+EDGE_PROFILES = {
+    MOST_ALLOCATED: dict(x=(61, 60), y=(60, 60), y_low=(60, 59), before=(100, 100), after=(0, 0)),
+    LEAST_BALANCED: dict(x=(40, 41), y=(42, 42), y_low=(43, 43), before=(0, 0), after=(100, 100)),
+}
+EDGE_A_CPU, EDGE_A_MEM = 100, 100 << 20
+EDGE_BIT = 1 << 5  # the label every pod requires: X, Y and the nodes after them carry it, the nodes before do not
+# boundary -> (tile of X, tile of Y, number of tiles; Y sits at the first slot of its tile unless both share one).
+# "inside one tile" has no exit test between X and Y: the tie is the tile merge's; tiles 0/1 and 20/21 are exits inside
+# a window, 7/8 (also a column-block edge), 39/40 and 71/72 the exits in front of a window.
+EDGES = {"inside one tile": (3, 3, 6), "tile 0/1": (0, 1, 3), "tile 7/8": (7, 8, 10), "tile 20/21": (20, 21, 24),
+         "tile 39/40": (39, 40, 42), "tile 71/72": (71, 72, 74), "last tile": (76, 77, 78)}
+
+
+def exit_tie_cluster(policy, edge, mirror=False, seed=0):
+    """A packed cluster (fc, fm, ac, am, labels, rc, rm, sel) in which X lies in front of the boundary `edge' and Y
+    right after it in bound order, Y at a lower node index than X.  Tie (mirror False): Y scores as X and the limit of
+    its tile, so Y must win.  Mirror: Y scores one lower, the walk stops in front of Y's tile and X wins.  Two
+    zero-request pods require EDGE_BIT, the second also a pair on the second label word.  Returns the cluster and the
+    node indices of X and Y."""
+    tx, ty, n_tiles = EDGES[edge]
+    prof = EDGE_PROFILES[policy]
+    sx = ty * TILE - 1 if tx != ty else tx * TILE + 100  # slots in bound order
+    N = (n_tiles - 1) * TILE + 37  # the last tile is a partial one
+    rng = np.random.default_rng(seed)
+    shares = [prof["before"]] * sx + [prof["x"], prof["y_low"] if mirror else prof["y"]]
+    shares += [prof["after"]] * (N - len(shares))
+    perm = rng.permutation(N)  # slot -> node index, Y below X
+    if perm[sx + 1] > perm[sx]:
+        perm[sx], perm[sx + 1] = perm[sx + 1], perm[sx]
+    u = np.zeros((N, 2), np.int64)
+    u[perm] = np.array(shares, np.int64)
+    ac, am = np.full(N, EDGE_A_CPU, np.int64), np.full(N, EDGE_A_MEM, np.int64)
+    fc, fm = ac - u[:, 0], am - (u[:, 1] << 20)
+    lab = np.zeros((N, 2), np.uint64)
+    lab[:, 1] = rng.integers(0, 1 << 16, N).astype(np.uint64)
+    lab[perm[sx:], 0] = EDGE_BIT
+    lab[perm[sx:], 1] |= np.uint64(1)
+    sel = np.array([[EDGE_BIT, 0], [EDGE_BIT, 1]], np.uint64)
+    z = np.zeros(2, np.int64)
+    return (fc, fm, ac, am, lab, z, z.copy(), sel), int(perm[sx]), int(perm[sx + 1])
+
+
 class Oracle:
     """orc with policies 3 and 4 added to run_packed and stream_bind_packed."""
 
@@ -299,3 +450,46 @@ def hazard_cells(seed, n):
         (hit if distinct else calm).append((fc, fm, ac, am, q_c, 0))
     cells = hit[:n // 2] + calm[:n - n // 2]
     return tuple(np.array(c, np.int64) for c in zip(*cells)), len(hit[:n // 2])
+
+
+def walk_extreme_clusters(policy, seed=0):
+    """(name, cluster) at the walk's length extremes, ~20 000 nodes (79 tiles: every window) and 160 pods:
+      "last tiles only"    the selector of most pods is carried only by the 300 nodes of lowest bound: every window;
+      "free above alloc"   15 % of the nodes, scattered, hold free above allocatable (LEAST_BALANCED stores them 2^62);
+      "alloc <= 0"         10 % of the allocatables are 0 or negative (no LEAST_ALLOCATED slack: amax = INT64_MAX);
+      "one alloc of 1"     one node has allocatables of 1: D saturates and MOST_ALLOCATED's walks are exhaustive;
+      "equal allocatables" every node has the same allocatables, the tightest D."""
+    rng = np.random.default_rng(seed)
+    N, P = 79 * TILE - 40, 160
+
+    def base():
+        ac = rng.choice([4000, 8000, 16000, 32000, 96000], N).astype(np.int64)
+        am = rng.choice([4, 16, 64, 384], N).astype(np.int64) << 30
+        fc, fm = ac * rng.integers(0, 65, N) // 64, am * rng.integers(0, 65, N) // 64
+        lab = rng.integers(0, 1 << 8, (N, 1)).astype(np.uint64)
+        rc = rng.choice([0, 1, 100, 250, 1000, 4000], P).astype(np.int64)
+        rm = rng.choice([0, 1, 1 << 27, 1 << 30, 1 << 32], P).astype(np.int64)
+        sel = np.where(rng.random((P, 1)) < 0.3, np.uint64(1) << rng.integers(0, 8, (P, 1)).astype(np.uint64), 0)
+        return fc, fm, ac, am, lab, rc, rm, sel.astype(np.uint64)
+
+    fc, fm, ac, am, lab, rc, rm, sel = base()
+    low = np.argsort([-stored_bound(policy, *v) for v in zip(fc, fm, ac, am)], kind="stable")[-300:]
+    lab[low, 0] |= np.uint64(1 << 9)
+    sel[:P - 20, 0] = 1 << 9  # the last 20 pods keep a random selector: they stop early
+    yield "last tiles only", (fc, fm, ac, am, lab, rc, rm, sel)
+    fc, fm, ac, am, lab, rc, rm, sel = base()
+    over = rng.random(N) < 0.15
+    fc[over], fm[over] = ac[over] * rng.integers(2, 5, int(over.sum())), am[over] * 3 + 7
+    yield "free above alloc", (fc, fm, ac, am, lab, rc, rm, sel)
+    fc, fm, ac, am, lab, rc, rm, sel = base()
+    ac[rng.random(N) < 0.1] = 0
+    am[rng.random(N) < 0.05] = -(1 << 20)
+    yield "alloc <= 0", (fc, fm, ac, am, lab, rc, rm, sel)
+    fc, fm, ac, am, lab, rc, rm, sel = base()
+    n = int(rng.integers(0, N))
+    ac[n], am[n], fc[n], fm[n] = 1, 1, 1, 1
+    yield "one alloc of 1", (fc, fm, ac, am, lab, rc, rm, sel)
+    fc, fm, ac, am, lab, rc, rm, sel = base()
+    ac[:], am[:] = 16000, 64 << 30
+    fc, fm = ac * rng.integers(0, 1001, N) // 1000, am * rng.integers(0, 1001, N) // 1000
+    yield "equal allocatables", (fc, fm, ac, am, lab, rc, rm, sel)

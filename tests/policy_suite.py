@@ -1,9 +1,11 @@
 """The CPU tests of KS_SCORE_MOST_ALLOCATED (3) and KS_SCORE_LEAST_BALANCED (4) that hold for both policies, written
 once against the restatement of tests/policy_oracle.py: the restatement's select against the oracle's cell codes and
 its round loop against one pod at a time; the hand-derived GV-1 values of tests/golden/gv1_*.json; the policy constant
-in the header, ctypes and the Rust shim; and KS_ERR_NO_DEVICE from every object-level call that takes a policy on a
-packing-only context.  tests/test_most_allocated.py and tests/test_least_balanced.py collect these tests under their
-policy (a `policy` fixture) next to the tests of their own definition."""
+in the header, ctypes and the Rust shim; KS_ERR_NO_DEVICE from every object-level call that takes a policy on a
+packing-only context; and the model of the bit-parallel walk (walk_packed) against the oracle on random clusters, on
+clusters that sit exactly at its exits and at its length extremes.  tests/test_most_allocated.py and
+tests/test_least_balanced.py collect these tests under their policy (a `policy` fixture) next to the tests of their own
+definition."""
 import os
 import re
 
@@ -11,8 +13,9 @@ import numpy as np
 import pytest
 
 from helpers import load_golden
-from policy_oracle import (LEAST_BALANCED, MOST_ALLOCATED, PLAN, SCORE, Oracle, balanced, least, most_score,
-                           topk_packed)
+from policy_oracle import (EDGES, FIRST_WINDOW, LB_UNBOUNDED, LEAST_BALANCED, MOST_ALLOCATED, PLAN, SCORE, TILE,
+                           WINDOW, Oracle, balanced, exit_tie_cluster, least, most_score, stored_bound, topk_packed,
+                           walk_extreme_clusters, walk_packed)
 from replicas_oracle import sequential_packed
 
 __all__ = ["check_packing_only_context"]  # + every test_ function, below
@@ -116,6 +119,87 @@ def test_gv1_golden(ks, orc, policy):
     assert all(np.array_equal(a, b) for a, b in zip((rows, node, sc), seq))
     assert {f: int(rows[f][0]) for f in w["row"]} == w["row"]
     assert node.tolist() == w["node"] and sc.tolist() == w["score"]
+
+
+def _walk_clusters(rng):
+    """(name, cluster): random clusters from one to many windows, and test_least_alloc_float_model's value families
+    (negative requests, allocatables <= 0 and free above allocatable among them)."""
+    from test_least_alloc_float_model import _families
+    for N, P in ((37, 30), (1500, 60), (3000, 40), (12000, 25)):
+        yield f"random {N}", _cluster(rng, N, P, W=2)
+    for name, fc, fm, ac, am, rc, rm in _families(rng, 2600, 40):
+        fc, fm, ac, am = (np.asarray(a, np.int64) for a in (fc, fm, ac, am))
+        lab = rng.integers(0, 4, (len(fc), 1)).astype(np.uint64)
+        sel = np.where(rng.random((len(rc), 1)) < 0.3, 1, 0).astype(np.uint64)
+        yield name, (fc, fm, ac, am, lab, np.asarray(rc, np.int64), np.asarray(rm, np.int64), sel)
+
+
+def test_walk_model_equals_the_oracle(orc, policy):
+    """walk_packed, the restatement of the bit-parallel walk, returns the argmax of the definition on every pod, and
+    these clusters reach its early exit and its later windows."""
+    o = Oracle(orc)
+    rng = np.random.default_rng({MOST_ALLOCATED: 0xE3, LEAST_BALANCED: 0xE4}[policy])
+    exits = windows = 0
+    for name, cl in _walk_clusters(rng):
+        idx, sc, scored, ex = walk_packed(o, *cl, policy)
+        w = o.run_packed(*cl, policy, want_mask=False)
+        assert np.array_equal(idx, w[0]) and np.array_equal(sc, w[1]), name
+        exits += int((ex > 0).sum())
+        windows += sum(bool(s) and s[-1] >= FIRST_WINDOW for s in scored)
+    assert exits > 50 and windows > 10
+
+
+@pytest.mark.parametrize("edge", list(EDGES))
+def test_exit_edge_clusters_reach_their_boundary(orc, policy, edge):
+    """exit_tie_cluster puts X and Y on each side of the boundary.  Tie: the walk does not stop in front of Y's tile,
+    scores it, and Y - later in bound order, lower in index - wins.  Mirror: the walk stops exactly in front of Y's tile
+    and X wins.  An exit one step too early (margin -1) stops in front of Y's tile in the tie case too and loses Y: the
+    case catches that off-by-one wherever an exit test lies between X and Y."""
+    o = Oracle(orc)
+    tx, ty = EDGES[edge][:2]
+    for mirror in (False, True):
+        cl, x, y = exit_tie_cluster(policy, edge, mirror, seed=ty)
+        assert y < x
+        idx, sc, scored, ex = walk_packed(o, *cl, policy)
+        w = o.run_packed(*cl, policy, want_mask=False)
+        assert np.array_equal(idx, w[0]) and np.array_equal(sc, w[1]), (edge, mirror)
+        assert (w[0] == (x if mirror else y)).all(), (edge, mirror)
+        assert all(s[0] == tx for s in scored)  # nothing in front of X is feasible
+        if tx == ty:  # no exit test between them: the tie is the tile merge's
+            assert all(ty in s for s in scored) and (ex != ty).all()
+        elif mirror:
+            assert (ex == ty).all() and all(ty not in s for s in scored), edge
+        else:
+            assert all(ty in s for s in scored) and ((ex == -1) | (ex > ty)).all(), edge
+        early = walk_packed(o, *cl, policy, margin=-1)
+        if mirror or tx == ty:
+            assert np.array_equal(early[0], w[0]), (edge, mirror)
+        else:
+            assert (early[3] == ty).all() and (early[0] == x).all() and (early[1] == w[1]).all(), edge
+
+
+def test_walk_extreme_clusters_reach_their_extremes(orc, policy):
+    """The clusters of walk_extreme_clusters do what they are named for, by the walk model, which equals the oracle on
+    them: the selector pods of "last tiles only" score nothing before the last window; no walk stops while a node stored
+    at 2^62 is left; a saturated D leaves MOST_ALLOCATED no exit for a pod that requests something; equal allocatables
+    let most pods stop early."""
+    o = Oracle(orc)
+    for name, cl in walk_extreme_clusters(policy, seed=policy):
+        fc, fm, ac, am, lab, rc, rm, sel = cl
+        idx, sc, scored, ex = walk_packed(o, *cl, policy)
+        w = o.run_packed(*cl, policy, want_mask=False)
+        assert np.array_equal(idx, w[0]) and np.array_equal(sc, w[1]), name
+        if name == "last tiles only":
+            walked = [s for s, q in zip(scored, sel[:, 0]) if q == 1 << 9 and s]
+            assert len(walked) > 40 and all(s[0] >= FIRST_WINDOW + 2 * WINDOW for s in walked)
+        elif name == "free above alloc":
+            unbounded = sum(stored_bound(policy, *v) == LB_UNBOUNDED for v in zip(fc, fm, ac, am))
+            assert 2000 < unbounded < 4000 if policy == LEAST_BALANCED else unbounded == 0
+            assert (ex[ex >= 0] * TILE >= unbounded).all() and (ex > 0).any()
+        elif name == "one alloc of 1" and policy == MOST_ALLOCATED:  # D = 200 once both requests are positive
+            assert (ex[(rc > 0) & (rm > 0)] == -1).all() and (ex[(rc == 0) & (rm == 0)] > 0).any()
+        elif name == "equal allocatables":
+            assert (ex > 0).mean() > 0.5
 
 
 def test_policy_constant_mirrors(ks, policy):

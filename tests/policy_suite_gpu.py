@@ -2,7 +2,8 @@
 scoring), written once for both policies: every call that takes a policy, bit for bit against the CPU restatement of
 tests/policy_oracle.py: ks_select (per-cell kernel, the bit-parallel k_most_alloc / k_least_balanced, AUTO),
 ks_select_topk, ks_stream_bind on both loops, the ks_stream surface, ks_gang_bind with rollback, ks_drain_check,
-ks_place_replicas (prefix fill under 3, one copy at a time under 4) and the object-level host layer.
+ks_place_replicas (prefix fill under 3, one copy at a time under 4) and the object-level host layer; and the walk of
+k_most_alloc / k_least_balanced at its exits, at its length extremes and across graph replays and policy changes.
 
 tests/test_most_allocated_gpu.py and tests/test_least_balanced_gpu.py collect these tests under their policy (a
 `policy` fixture) and add the tests that hold for one policy only."""
@@ -12,7 +13,8 @@ import pytest
 from drain_oracle import bound_candidates, drain_packed
 from gang_oracle import gang_bind_packed, groups
 from gang_oracle import sequential_packed as one_at_a_time
-from policy_oracle import LEAST_BALANCED, MOST_ALLOCATED, PLAN, Oracle, topk_packed
+from policy_oracle import (EDGES, LEAST_BALANCED, MOST_ALLOCATED, PLAN, Oracle, exit_tie_cluster, topk_packed,
+                           walk_extreme_clusters)
 
 __all__ = ["pytestmark", "o", "cluster", "snapshot", "assert_refused"]  # + every test_ function, below
 pytestmark = pytest.mark.gpu
@@ -66,6 +68,8 @@ CASES = [  # (seed, N, P, W, family)
     (1, 1, 1, 1, "mixed"), (2, 1023, 1, 1, "mixed"), (3, 1025, 7, 2, "edges"), (4, 3000, 40, 4, "ties"),
     (5, 5001, 130, 8, "mixed"), (6, 777, 1500, 1, "edges"), (7, 20000, 3, 1, "ties"), (8, 4097, 600, 2, "mixed"),
     (9, 10000, 512, 1, "mixed"),  # C2's node count
+    (10, 150_000, 300, 1, "mixed"),  # more column blocks than SMs: every CTA walks several column blocks
+    (12, 12_000, 200, 8, "edges"),  # W = 8 over 6 column blocks of 8 tiles
 ]
 
 
@@ -99,6 +103,84 @@ def test_negative_requests_scan_every_tile(ks, o, policy):
         for flags in (ks.KS_SELECT_FORCE_BITPAR, ks.KS_SELECT_FORCE_DIRECT):
             r = s.select(rc, rm, sel, policy=policy, flags=flags)
             assert np.array_equal(r.node_idx, w[0]) and np.array_equal(r.score, w[1]) and np.array_equal(r.feasible_cnt, w[2])
+
+
+def _both_paths(ks, s, cl, want, policy, tag):
+    rc, rm, sel = cl[5:]
+    for flags in (ks.KS_SELECT_FORCE_BITPAR, ks.KS_SELECT_FORCE_DIRECT):
+        r = s.select(rc, rm, sel, policy=policy, flags=flags)
+        assert r.path == ("bitpar" if flags == ks.KS_SELECT_FORCE_BITPAR else "direct")
+        assert np.array_equal(r.node_idx, want[0]) and np.array_equal(r.score, want[1]), (tag, r.path)
+        assert np.array_equal(r.feasible_cnt, want[2]), (tag, r.path)
+
+
+@pytest.mark.parametrize("edge", list(EDGES))
+def test_exit_ties(ks, o, policy, edge):
+    """Ties exactly at the walk's early exit (exit_tie_cluster; tests/policy_suite.py shows with the walk model that each
+    cluster reaches its boundary): Y comes right after X in bound order, has the lower index, and scores as X and as the
+    limit of its tile, so the walk must not stop in front of Y's tile and Y wins.  Mirror: Y scores one lower, the walk
+    stops there and X wins."""
+    for mirror in (False, True):
+        cl, x, y = exit_tie_cluster(policy, edge, mirror, seed=EDGES[edge][1])
+        w = o.run_packed(*cl, policy, want_mask=False)
+        assert (w[0] == (x if mirror else y)).all()
+        with snapshot(ks, *cl[:5]) as s:
+            _both_paths(ks, s, cl, w, policy, (edge, mirror))
+
+
+def test_walk_length_extremes(ks, o, policy):
+    """walk_extreme_clusters: pods that walk every window, nodes stored at 2^62 scattered through the table, allocatables
+    <= 0, a saturated D (exhaustive walks) and the tightest D (all allocatables equal)."""
+    for name, cl in walk_extreme_clusters(policy, seed=policy):
+        w = o.run_packed(*cl, policy, want_mask=False)
+        assert (w[0] >= 0).sum() > 40, name
+        with snapshot(ks, *cl[:5]) as s:
+            _both_paths(ks, s, cl, w, policy, name)
+
+
+def test_graph_replay_and_alternating_policies(ks, o, policy):
+    """The bound orders of policies 3 and 4 are built outside the captured CUDA graph (bitpar_prepare_order).  A
+    replayed call sees a bind and new pod values in the same device buffers, and calls under policies 1, 3, 4, 3, 4 on
+    one snapshot, with binds between them, each see the current free[]: every result against the oracle."""
+    import torch
+    fc, fm, ac, am, lab, rc, rm, sel = cluster(90, 6000, 2000, 2)
+    P = len(rc)
+    dev = torch.device("cuda:0")
+    t = [torch.from_numpy(np.ascontiguousarray(a.view(np.int64))).to(dev) for a in (rc, rm, sel)]
+    idx = torch.empty(P, dtype=torch.int32, device=dev)
+    score = torch.empty(P, dtype=torch.int64, device=dev)
+    cnt = torch.empty(P, dtype=torch.int32, device=dev)
+    st = torch.cuda.Stream()
+    with snapshot(ks, fc, fm, ac, am, lab) as s:
+
+        def check(q, req_cpu, tag):
+            s.select_raw(P, t[0], t[1], t[2], ks.KS_MEM_DEVICE, idx, score, cnt, ks.KS_MEM_DEVICE, policy=q,
+                         flags=ks.KS_SELECT_FORCE_BITPAR, stream=st.cuda_stream)
+            st.synchronize()
+            assert s.last_path() == "bitpar"
+            f = s.free()
+            w = o.run_packed(f[0], f[1], ac, am, lab, req_cpu, rm, sel, q, want_mask=False)
+            got = idx.cpu().numpy(), score.cpu().numpy(), cnt.cpu().numpy().view(np.uint32)
+            assert all(np.array_equal(a, b) for a, b in zip(got, w[:3])), tag
+            return w[0]
+
+        first = None
+        for it in range(3):  # capture, replay, replay
+            first = check(policy, rc, ("replay", it))
+        s.apply_bind(int(first[first >= 0][0]), 10_000_000, 1 << 40)
+        assert not np.array_equal(check(policy, rc, "after a bind"), first)
+        rc2 = rc.copy()
+        rc2[::2] += 50
+        t[0].copy_(torch.from_numpy(rc2))
+        torch.cuda.synchronize()
+        check(policy, rc2, "new pod values")
+        t[0].copy_(torch.from_numpy(rc))
+        torch.cuda.synchronize()
+        for step, q in enumerate((ks.KS_SCORE_LEAST_ALLOCATED, MOST_ALLOCATED, LEAST_BALANCED, MOST_ALLOCATED,
+                                  LEAST_BALANCED)):
+            got = check(q, rc, ("alternating", step, q))
+            if step in (1, 2):  # a bind between the calls of 3 and 4, and of 4 and 3
+                s.apply_bind(int(got[got >= 0][step]), 4000 * step, 1 << 32)
 
 
 def test_index_follows_snapshot_changes(ks, o, policy):

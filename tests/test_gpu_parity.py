@@ -21,6 +21,15 @@ def _oracle(orc, cl, policy, want_codes=False):
     return orc.run_packed(fc, fm, ac, am, lab, rc, rm, sel, policy=policy, want_codes=want_codes)
 
 
+# The policies whose bit-parallel argmax walks a bound order with an early exit: k_least_alloc (1) and bound_walk's
+# k_most_alloc (3) and k_least_balanced (4).  LEAST_ALLOCATED's cases keep their ids.
+BOUND_ORDERED = {1: "", 3: "-most_allocated", 4: "-least_balanced"}
+
+
+def _with_policies(cases):
+    return [pytest.param(*c, q, id="-".join(map(str, c)) + sfx) for c in cases for q, sfx in BOUND_ORDERED.items()]
+
+
 def _snapshot(ks, cl):
     ac, am, lab, bn, bc, bm, rc, rm, sel = cl.packed()
     snap = ks.Snapshot(0)
@@ -120,11 +129,13 @@ def test_random_clusters_least_allocated(ks, orc, path, P, N, keys):
 
 
 @pytest.mark.parametrize("path", list(PATHS))
-@pytest.mark.parametrize("seed,P,N", [(11, 3000, 6000), (12, 700, 40_000)])
-def test_least_allocated_near_ties(ks, orc, path, seed, P, N):
+@pytest.mark.parametrize("seed,P,N,policy", _with_policies([(11, 3000, 6000), (12, 700, 40_000)]))
+def test_least_allocated_near_ties(ks, orc, path, seed, P, N, policy):
     """Homogeneous clusters: thousands of nodes whose LeastAllocated scores lie within a point or two of each other
     (and many exact ties), so the single-precision pre-filter of k_least_alloc keeps whole tiles of candidates and the
-    winner is decided by the exact integer score and then the lowest node index - vs the oracle, every pod."""
+    winner is decided by the exact integer score and then the lowest node index - vs the oracle, every pod.  Under
+    policies 3 and 4 the same near ties sit at bound_walk's early exit."""
+    from policy_oracle import Oracle
     rng = np.random.default_rng(seed)
     ac = rng.choice(np.array([64000, 64000, 64001, 63999, 32000], np.int64), N)
     am = rng.choice(np.array([1 << 38, (1 << 38) + 4096, 1 << 37], np.int64), N)
@@ -142,8 +153,8 @@ def test_least_allocated_near_ties(ks, orc, path, seed, P, N):
         snap.set_nodes(ac, am, lab)
         snap.set_bound(bn, bc, bm)
         ofc, ofm = orc.free_reduce(ac, am, bn, bc, bm)
-        r = snap.select(rc, rm, sel, policy=ks.KS_SCORE_LEAST_ALLOCATED, flags=PATHS[path], want_mask=False)
-        o = orc.run_packed(ofc, ofm, ac, am, lab, rc, rm, sel, policy=1, want_mask=False)
+        r = snap.select(rc, rm, sel, policy=policy, flags=PATHS[path], want_mask=False)
+        o = Oracle(orc).run_packed(ofc, ofm, ac, am, lab, rc, rm, sel, policy, want_mask=False)
         assert r.path == path
         assert np.array_equal(r.score, o[1]), f"near ties {path}: score"
         assert np.array_equal(r.node_idx, o[0]), f"near ties {path}: node_idx (tie-break by node index)"
@@ -151,11 +162,13 @@ def test_least_allocated_near_ties(ks, orc, path, seed, P, N):
         assert len(np.unique(r.score[r.node_idx >= 0])) <= 60  # the scores really are bunched
 
 
-@pytest.mark.parametrize("path", list(PATHS))
-def test_least_allocated_round_fills(ks, orc, path):
+@pytest.mark.parametrize("path,policy", _with_policies([(p,) for p in PATHS]))
+def test_least_allocated_round_fills(ks, orc, path, policy):
     """Nodes filled to exact quarters of round capacities and round requests: the memory quotient (free - request) * 100 /
     allocatable is often EXACTLY an integer, where k_least_alloc's single-precision estimate cannot know the floor and must
-    fall back to the 64-bit arithmetic of the evaluation row; every node is feasible for most pods and most scores tie."""
+    fall back to the 64-bit arithmetic of the evaluation row; every node is feasible for most pods and most scores tie.
+    Under policies 3 and 4 exact shares put many scores exactly on bound_walk's limits."""
+    from policy_oracle import Oracle
     rng = np.random.default_rng(5)
     N, P = 9000, 2500
     ac = rng.choice(np.array([4000, 8000, 16000], np.int64), N)
@@ -171,8 +184,8 @@ def test_least_allocated_round_fills(ks, orc, path):
         snap.set_nodes(ac, am, lab)
         snap.set_bound(bn, bc, bm)
         ofc, ofm = orc.free_reduce(ac, am, bn, bc, bm)
-        r = snap.select(rc, rm, sel, policy=ks.KS_SCORE_LEAST_ALLOCATED, flags=PATHS[path], want_mask=False)
-        o = orc.run_packed(ofc, ofm, ac, am, lab, rc, rm, sel, policy=1, want_mask=False)
+        r = snap.select(rc, rm, sel, policy=policy, flags=PATHS[path], want_mask=False)
+        o = Oracle(orc).run_packed(ofc, ofm, ac, am, lab, rc, rm, sel, policy, want_mask=False)
         assert r.path == path
         assert np.array_equal(r.score, o[1]), f"round fills {path}: score"
         assert np.array_equal(r.node_idx, o[0]), f"round fills {path}: node_idx"
@@ -557,11 +570,14 @@ def test_adversarial_values(ks, orc, path, seed, P, N, W):
         r = snap.select(rc, rm, sel, flags=PATHS[path], want_mask=True)
         o = orc.run_packed(ofc, ofm, ac, am, lab, rc, rm, sel)
         _assert_same(r, o, f"adversarial {path} seed {seed}")
-        # the non-separable score on the same path; negative requests void the early-exit bound of k_least_alloc
-        r1 = snap.select(rc, rm, sel, policy=ks.KS_SCORE_LEAST_ALLOCATED, flags=PATHS[path], want_mask=False)
-        o1 = orc.run_packed(ofc, ofm, ac, am, lab, rc, rm, sel, policy=1, want_mask=False)
-        assert r1.path == path and np.array_equal(r1.node_idx, o1[0]) and np.array_equal(r1.score, o1[1])
-        assert np.array_equal(r1.feasible_cnt, o1[2])
+        # the non-separable scores on the same path; negative requests void the early-exit bound of k_least_alloc and
+        # bound_walk, allocatables <= 0 give no slack, free above allocatable is stored at 2^62 under policy 4
+        from policy_oracle import Oracle
+        for q in BOUND_ORDERED:
+            r1 = snap.select(rc, rm, sel, policy=q, flags=PATHS[path], want_mask=False)
+            o1 = Oracle(orc).run_packed(ofc, ofm, ac, am, lab, rc, rm, sel, q, want_mask=False)
+            assert r1.path == path and np.array_equal(r1.node_idx, o1[0]) and np.array_equal(r1.score, o1[1]), q
+            assert np.array_equal(r1.feasible_cnt, o1[2]), q
 
 
 def _stream_states(ks, seed, P, first=0):

@@ -1,11 +1,11 @@
 """KS_SCORE_MOST_ALLOCATED (bin-packing), CPU part: the Python-integer definition against the numpy restatement on
-random and edge cells; the prefix-fill replica plan against one copy at a time on thousands of random small clusters;
-and, under policy 3, the tests of tests/policy_suite.py (select, round loop, GV-1, constant mirrors, packing-only
-context)."""
+random and edge cells; the early-exit bound of the bit-parallel walk on a million pairs per family; the prefix-fill
+replica plan against one copy at a time on thousands of random small clusters; and, under policy 3, the tests of
+tests/policy_suite.py (select, round loop, GV-1, constant mirrors, packing-only context, walk model)."""
 import numpy as np
 import pytest
 
-from policy_oracle import MOST_ALLOCATED, Oracle, prefix_fill_packed, term
+from policy_oracle import I64_MAX, MOST_ALLOCATED, Oracle, most_bound, most_slack, prefix_fill_packed, term
 from policy_oracle import most_score as score
 from policy_oracle import most_scores as scores
 from policy_suite import *  # noqa: F401,F403 - the shared tests, run under the policy fixture below
@@ -53,6 +53,56 @@ def test_numpy_restatement_equals_integers_on_edges_and_random_cells():
         if y > 0 and y % 100 == 0:
             k = (y - (x - z)) * 100 // y
             assert term(x, y, z) == min(max(k, 0), 100)
+
+
+@pytest.mark.parametrize("family", ["random", "adversarial", "exact percentages"])
+def test_walk_bound_holds_on_a_million_pairs(family):
+    """score(p, n) <= (b(n) + D(p)) // 2 on every feasible cell with requests >= 0 (k_most_alloc's early exit), and
+    with no request the bound is the score itself - which is what lets a tie sit exactly at the exit."""
+    rng = np.random.default_rng({"random": 0xB3, "adversarial": 0xB4, "exact percentages": 0xB5}[family])
+    N, P = 1000, 1000
+    if family == "random":
+        ac = rng.choice([1000, 4000, 16000, 96000], N).astype(np.int64)
+        am = rng.choice([1, 4, 64, 384], N).astype(np.int64) << 30
+        fc, fm = ac * rng.integers(0, 17, N) // 16, am * rng.integers(0, 17, N) // 16
+        rc = rng.choice([0, 1, 100, 500, 4000], P).astype(np.int64)
+        rm = rng.choice([0, 1, 1 << 27, 1 << 32], P).astype(np.int64)
+    elif family == "adversarial":  # tiny and huge allocatables, allocatable <= 0, free above allocatable, limits
+        ac = rng.choice([1, 2, 50, 4000, LIM_C], N).astype(np.int64)
+        am = rng.choice([1, 3, 50 << 20, 1 << 53, LIM_M], N).astype(np.int64)
+        ac[rng.random(N) < 0.05] = 0
+        am[rng.random(N) < 0.05] = -7
+        fc = ac // 50 * rng.integers(0, 51, N) + ac % 50
+        fm = am // 50 * rng.integers(0, 51, N) + am % 50
+        over = rng.random(N) < 0.05
+        fc[over] += 1000
+        fm[over] += 1 << 40
+        rc = rng.choice([0, 1, 2, 25, 1 << 20, LIM_C], P).astype(np.int64)
+        rm = rng.choice([0, 1, 7, 1 << 40, LIM_M], P).astype(np.int64)
+    else:  # A - (f - q) = k * A / 100 on every cell: each A / 100 divides 960 (512 MiB) and the requests are multiples
+        unit_c = rng.choice([48, 96, 320, 960], N).astype(np.int64)
+        unit_m = rng.choice([64, 128, 256, 512], N).astype(np.int64) << 20
+        ac, am = 100 * unit_c, 100 * unit_m
+        fc, fm = ac - unit_c * rng.integers(0, 101, N), am - unit_m * rng.integers(0, 101, N)
+        rc = 960 * rng.integers(0, 6, P).astype(np.int64)
+        rm = (512 << 20) * rng.integers(0, 13, P).astype(np.int64)
+        u = ac[None, :] - (fc[None, :] - rc[:, None])
+        assert (u % unit_c[None, :] == 0).all()
+    b = np.array([most_bound(*v) for v in zip(fc, fm, ac, am)], np.int64)
+    assert b.min() >= 0 and b.max() <= 200
+    amin_c = int(ac[ac > 0].min()) if (ac > 0).any() else I64_MAX
+    amin_m = int(am[am > 0].min()) if (am > 0).any() else I64_MAX
+    D = np.array([most_slack(int(x), int(y), amin_c, amin_m) for x, y in zip(rc, rm)], np.int64)
+    s = scores(fc[None, :], fm[None, :], ac[None, :], am[None, :], rc[:, None], rm[:, None])
+    feas = (rc[:, None] <= fc[None, :]) & (rm[:, None] <= fm[None, :])
+    lim = (b[None, :] + D[:, None]) // 2
+    assert feas.sum() > 100000
+    assert (s[feas] <= lim[feas]).all()
+    zero = (rc == 0) & (rm == 0)
+    assert zero.any() and (s[zero][feas[zero]] == lim[zero][feas[zero]]).all()  # attained without a request
+    assert np.median((lim - s)[feas]) <= 60  # and not vacuous with one
+    if family == "exact percentages":
+        assert ((lim - s)[feas] == 0).mean() > 0.05  # the limit is reached with requests too
 
 
 def test_prefix_fill_equals_one_copy_at_a_time(orc):
