@@ -32,6 +32,7 @@ pub const KSH_RECONCILE_NO_NODE_FOUND: c_int = 1; // ReconcileError::NoNodeFound
 pub const KSH_RECONCILE_BINDING_OBJECT_FAILED: c_int = 2; // ReconcileError::CreateBindingObjectFailed
 pub const KSH_RECONCILE_GANG_UNSATISFIED: c_int = 4; // ksh_reconcile_gangs: the pod's group rolled back
 pub const KSH_RECONCILE_SPREAD_UNSATISFIED: c_int = 5; // ksh_reconcile_spread: spread constraints refused every node
+pub const KSH_RECONCILE_AFFINITY_UNSATISFIED: c_int = 6; // ksh_reconcile_affinity: pod (anti-)affinity refused every node
 pub const KS_REFERENCE_ATTEMPTS: u32 = 5; // ATTEMPTS, src/main.rs:49
 pub const KS_MAX_PEERS: usize = 15;
 pub const KS_TOPK_MAX: u32 = 32; // largest k of ks_select_topk / ksh_rank_nodes
@@ -51,6 +52,12 @@ pub const KS_SPREAD_MAX_COUNTS: u64 = 1 << 26; // most specs x domains of existi
 pub const KS_SPREAD_MAX_KEYS: u32 = 4; // most topology keys of one ks_place_replicas_spread_multi call
 pub const KS_SPREAD_BIND_MAX_PODS: u32 = 65536; // most pods of one ks_spread_bind call
 pub const KS_SPREAD_BIND_MAX_GROUPS: u32 = 4096; // most groups of one ks_spread_bind call
+pub const KS_POD_AFFINITY: u8 = 0; // ks_pod_affinity term kinds
+pub const KS_POD_ANTI_AFFINITY: u8 = 1;
+pub const KS_AFFINITY_MAX_TERMS: u32 = 16384; // most terms of one ks_affinity_bind call
+pub const KS_AFFINITY_MAX_TARGETS: u64 = 1 << 22; // most target entries over all terms
+pub const KS_AFFINITY_MAX_EXISTING: u64 = 1 << 24; // most existing pods
+pub const KS_AFFINITY_MAX_UPDATES: u64 = 1 << 24; // most compiled update entries
 
 #[repr(C)]
 pub struct ks_kv {
@@ -205,6 +212,30 @@ pub struct ks_spread_multi {
     pub existing: *const u32,
 }
 #[repr(C)]
+pub struct ks_pod_affinity {
+    pub n_terms: u32,
+    pub owner: *const i32,
+    pub kind: *const u8,
+    pub key: *const u32,
+    pub target_offset: *const u64,
+    pub target: *const i32,
+    pub n_existing: u64,
+    pub existing_group: *const i32,
+    pub existing_node: *const i32,
+}
+#[repr(C)]
+pub struct ksh_pod_affinity {
+    pub n_terms: u32,
+    pub owner: *const i32,
+    pub kind: *const u8,
+    pub key: *const u32,
+    pub target_offset: *const u64,
+    pub target: *const i32,
+    pub n_existing: u64,
+    pub existing_group: *const i32,
+    pub existing_node_name: *const *const c_char,
+}
+#[repr(C)]
 #[derive(Clone, Copy, Default, Debug)]
 pub struct ks_spread_plan {
     pub placed: u32,
@@ -262,6 +293,9 @@ extern "C" {
     pub fn ks_spread_bind(s: *mut ks_snapshot, pods: *const ks_pods, group: *const i32, n_groups: u32,
                           spread: *const ks_spread_multi, policy: c_int, node_idx: *mut i32, score: *mut i64,
                           refused: *mut u32, domain_count: *mut u32) -> c_int;
+    pub fn ks_affinity_bind(s: *mut ks_snapshot, pods: *const ks_pods, group: *const i32, n_groups: u32,
+                            topo: *const ks_spread_multi, aff: *const ks_pod_affinity, policy: c_int,
+                            node_idx: *mut i32, score: *mut i64, refused: *mut u32, domain_count: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -329,6 +363,12 @@ extern "C" {
                                 min_domains: *const u32, existing_node_names: *const *const c_char,
                                 existing_offset: *const u64, policy: c_int, status: *mut i32, node_idx: *mut i32,
                                 json: *mut c_char, cap: usize, json_off: *mut i64) -> c_int;
+    pub fn ksh_reconcile_affinity(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group: *const i32,
+                                  n_groups: u32, topology_keys: *const *const c_char, n_keys: u32, max_skew: *const u32,
+                                  min_domains: *const u32, existing_node_names: *const *const c_char,
+                                  existing_offset: *const u64, aff: *const ksh_pod_affinity, policy: c_int,
+                                  status: *mut i32, node_idx: *mut i32, json: *mut c_char, cap: usize,
+                                  json_off: *mut i64) -> c_int;
     pub fn ksh_drain_nodes(ctx: *mut ksh_context, node_names: *const *const c_char, n: u64, pods: *const ks_pod_obj,
                            pod_offset: *const u64, policy: c_int, flags: u32, placed: *mut u32, node_idx: *mut i32) -> c_int;
     pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,

@@ -693,6 +693,73 @@ int ks_spread_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const i
                    int policy, int32_t* out_node_idx /* [P] */, int64_t* out_score /* [P] or NULL */,
                    uint32_t* out_refused /* [P] or NULL */, uint32_t* out_domain_count /* [G * S] or NULL */);
 
+/* ---- inter-pod affinity when binding: ks_spread_bind with required pod affinity and anti-affinity (upstream
+ * InterPodAffinity's Filter, requiredDuringSchedulingIgnoredDuringExecution; spec extension, DESIGN.md 5n) ----
+ * The arguments of ks_spread_bind, with topo->max_skew allowed NULL (= every max_skew 0, no spread constraint), and a
+ * term list aff.  Groups stand for label classes: the caller resolves each term's labelSelector and namespaces into the
+ * groups whose pods it matches, so group -1 is a pod that no term matches and that carries no term.  Term t belongs to
+ * the pods of group owner[t], is KS_POD_AFFINITY or KS_POD_ANTI_AFFINITY, has topology key key[t] (an index into topo's
+ * K keys) and matches the pods of the groups target[target_offset[t] .. target_offset[t + 1]).  The E existing pods are
+ * bound pods, pod e of group existing_group[e] on node existing_node[e]; they need to be listed only when some term
+ * matches them or they carry terms.  "Bound" below means the existing pods and every earlier pod of this call.  For pod
+ * p of group g >= 0 and node n, with d_k(n) = topo->node_domain[k][n]:
+ *   1. incoming anti-affinity: n is refused when, for some anti term of g on key k, d_k(n) >= 0 and a bound pod of a
+ *      target group sits on a node of domain d_k(n) (a node without key k passes that term);
+ *   2. existing anti-affinity (symmetry): n is refused when some bound pod, of group h, carries an anti term on key k
+ *      that targets g, d_k(n) >= 0 and that pod sits in domain d_k(n);
+ *   3. affinity: with M_g = the groups every affinity term of g targets, n is refused when it lacks the key of some
+ *      affinity term of g, or when for some affinity term on key k no bound pod of a group in M_g sits in domain d_k(n).
+ *      Upstream's first-pod rule: when no bound pod of M_g sits on a node that carries one of those keys and g is in
+ *      M_g, the terms hold on every node that carries their keys;
+ *   4. pods run as in ks_spread_bind, one at a time in array order: pod p's candidates are fit, selector and spread
+ *      (ks_spread_bind's rule 2, unchanged) and rules 1-3; it takes the best candidate under `policy`, ties to the lower
+ *      node index, free[] is charged and the pod is bound.  A pod with no candidate changes nothing;
+ *   5. out_refused[2p] = the nodes that passed fit and selector but failed spread (ks_spread_bind's out_refused[p]);
+ *      out_refused[2p + 1] = the nodes that passed fit, selector and spread but failed rules 1-3 (upstream's filter
+ *      order: PodTopologySpread before InterPodAffinity).  out_node_idx, out_score and out_domain_count as in
+ *      ks_spread_bind.
+ * Identities:
+ *   (I1) n_terms = 0: nodes, scores, out_refused[2p], counts and the final free[] are ks_spread_bind's, and every
+ *        out_refused[2p + 1] is 0;
+ *   (I2) n_terms = 0 and topo->max_skew NULL: the result is ks_gang_bind's with one singleton group per pod;
+ *   (I3) one group of R identical pods, one anti term of the group on itself on a key every node carries, no existing
+ *        pods: the nodes and scores are ks_place_replicas_spread's copy list (that key, max_skew 1) up to the first copy
+ *        whose domain already holds one; every later pod is unbound;
+ *   (I4) "g anti h on key k" and "h anti g on key k" give the same result: anti-affinity is symmetric in its owner.
+ * Checked on the host before any device work and before free[] changes: every check of ks_spread_bind (max_skew NULL
+ * allowed); KS_ERR_INVALID for an owner, target or existing group outside [0, G), an existing node outside [0, N), a
+ * kind other than 0 or 1, a key >= K, decreasing target_offset, or a NULL array that is needed; KS_ERR_RANGE for
+ * n_terms > KS_AFFINITY_MAX_TERMS, more than KS_AFFINITY_MAX_TARGETS targets, E > KS_AFFINITY_MAX_EXISTING, compiled
+ * counters above KS_SPREAD_MAX_COUNTS words, or update entries above KS_AFFINITY_MAX_UPDATES.  aff NULL = no term and
+ * no existing pod.
+ * The terms are compiled on the host into per-(group, key) counter arrays (B_{g,k} for rules 1 and 2, A_{g,k} for rule
+ * 3, D_k words each) and, per group h, the deduplicated (g, k, B|A) entries that a bind of a pod of h raises; one update
+ * entry per (g, k, kind).  Host-space arguments and outputs; one H2D copy; ks_spread_bind's setup kernel and one that
+ * applies the existing pods' entries; one cooperative launch that walks the pods (at most 2K counter loads per node);
+ * one D2H copy.  The bit-parallel index is marked stale. */
+#define KS_POD_AFFINITY 0
+#define KS_POD_ANTI_AFFINITY 1
+#define KS_AFFINITY_MAX_TERMS 16384u
+#define KS_AFFINITY_MAX_TARGETS (1ull << 22)
+#define KS_AFFINITY_MAX_EXISTING (1ull << 24)
+#define KS_AFFINITY_MAX_UPDATES (1ull << 24)
+typedef struct ks_pod_affinity {   /* host memory */
+    uint32_t n_terms;              /* T */
+    const int32_t* owner;          /* [T] group in [0, G) whose pods carry the term */
+    const uint8_t* kind;           /* [T] KS_POD_AFFINITY / KS_POD_ANTI_AFFINITY */
+    const uint32_t* key;           /* [T] topology key index in [0, K) of topo's keys */
+    const uint64_t* target_offset; /* [T + 1] */
+    const int32_t* target;         /* groups whose pods the term's labelSelector + namespaces match */
+    uint64_t n_existing;           /* E: bound pods that some term matches or that carry terms */
+    const int32_t* existing_group; /* [E] in [0, G) */
+    const int32_t* existing_node;  /* [E] in [0, N) */
+} ks_pod_affinity;
+int ks_affinity_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const int32_t* group /* [P] */,
+                     uint32_t n_groups, const ks_spread_multi* topo /* keys; max_skew may be NULL = no spread constraint */,
+                     const ks_pod_affinity* aff /* or NULL */, int policy, int32_t* out_node_idx /* [P] */,
+                     int64_t* out_score /* [P] or NULL */, uint32_t* out_refused /* [2P] or NULL */,
+                     uint32_t* out_domain_count /* [G * S] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -40,6 +40,9 @@ extern "C" {
 #define KSH_RECONCILE_SPREAD_UNSATISFIED 5   /* ksh_reconcile_spread: a node would take the pod but its spread constraints
                                                 refused every such node (upstream: "didn't match pod topology spread
                                                 constraints") */
+#define KSH_RECONCILE_AFFINITY_UNSATISFIED 6 /* ksh_reconcile_affinity: fit, selector and spread passed on some node but
+                                                the pod's inter-pod (anti-)affinity refused every such node (upstream:
+                                                "didn't match pod affinity/anti-affinity rules") */
 
 /* Kubernetes quantity strings, exact: cpu -> millicores, memory -> bytes.
  * KS_ERR_PARSE (malformed), KS_ERR_INEXACT (finer than 1m / 1 byte), KS_ERR_RANGE. */
@@ -278,6 +281,32 @@ int ksh_reconcile_spread(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_po
                          const uint32_t* min_domains, const char* const* existing_node_names,
                          const uint64_t* existing_offset, int policy, int32_t* out_status, int32_t* out_node_idx,
                          char* json, size_t cap, int64_t* out_json_off);
+
+/* reconcile() under topology spread and required inter-pod affinity (ks_affinity_bind, ksched.h): ksh_reconcile_spread
+ * with the terms of aff (or NULL: none), and max_skew may be NULL (no spread constraint).  Term t of group owner[t] is
+ * kind[t] (KS_POD_AFFINITY / KS_POD_ANTI_AFFINITY) on topology_keys[key[t]] and targets the groups
+ * target[target_offset[t] .. target_offset[t + 1]), resolved by the caller from the term's labelSelector and
+ * namespaces.  Existing pod e is of group existing_group[e] and bound to the node named existing_node_name[e]; a name
+ * not in the store is skipped.  An unbound pod gets KSH_RECONCILE_SPREAD_UNSATISFIED when its spread constraints refused
+ * some node that fit it, else KSH_RECONCILE_AFFINITY_UNSATISFIED when its affinity terms refused some node that passed
+ * fit, selector and spread, else KSH_RECONCILE_NO_NODE_FOUND.  Errors as ksh_reconcile_spread and ks_affinity_bind. */
+typedef struct ksh_pod_affinity {
+    uint32_t n_terms;
+    const int32_t* owner;              /* [T] */
+    const uint8_t* kind;               /* [T] */
+    const uint32_t* key;               /* [T] index into topology_keys */
+    const uint64_t* target_offset;     /* [T + 1] */
+    const int32_t* target;
+    uint64_t n_existing;               /* E */
+    const int32_t* existing_group;     /* [E] */
+    const char* const* existing_node_name; /* [E] */
+} ksh_pod_affinity;
+int ksh_reconcile_affinity(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, const int32_t* group,
+                           uint32_t n_groups, const char* const* topology_keys, uint32_t n_keys,
+                           const uint32_t* max_skew /* or NULL */, const uint32_t* min_domains,
+                           const char* const* existing_node_names, const uint64_t* existing_offset,
+                           const ksh_pod_affinity* aff, int policy, int32_t* out_status, int32_t* out_node_idx,
+                           char* json, size_t cap, int64_t* out_json_off);
 
 #ifdef __cplusplus
 }

@@ -221,6 +221,22 @@ _proto("ks_spread_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.
        C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
 KS_SPREAD_BIND_MAX_PODS = 65536
 KS_SPREAD_BIND_MAX_GROUPS = 4096
+
+
+class ks_pod_affinity(C.Structure):
+    _fields_ = [("n_terms", C.c_uint32), ("owner", C.c_void_p), ("kind", C.c_void_p), ("key", C.c_void_p),
+                ("target_offset", C.c_void_p), ("target", C.c_void_p), ("n_existing", C.c_uint64),
+                ("existing_group", C.c_void_p), ("existing_node", C.c_void_p)]
+
+
+_proto("ks_affinity_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_uint32,
+       C.POINTER(ks_spread_multi), C.POINTER(ks_pod_affinity), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+       C.c_void_p, optional=True)
+KS_POD_AFFINITY, KS_POD_ANTI_AFFINITY = 0, 1
+KS_AFFINITY_MAX_TERMS = 16384
+KS_AFFINITY_MAX_TARGETS = 1 << 22
+KS_AFFINITY_MAX_EXISTING = 1 << 24
+KS_AFFINITY_MAX_UPDATES = 1 << 24
 KS_PREEMPT_MAX_ABS_SUM = 1 << 62
 KS_ERR_INVALID, KS_ERR_RANGE = -1, -5
 KS_REFERENCE_ATTEMPTS = 5

@@ -34,6 +34,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 #pragma weak ks_place_replicas_spread
 #pragma weak ks_place_replicas_spread_multi
 #pragma weak ks_spread_bind
+#pragma weak ks_affinity_bind
 
 namespace {
 
@@ -1712,13 +1713,14 @@ KSH_CATCH
 
 // reconcile() under topology spread: ksh_reconcile_batch's filtering, then ks_spread_bind over the pods that go to the
 // device, each in its group.  Group g's existing pods under key k count when their node is in the store and carries key k
-// and every key g constrains.
-int ksh_reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
-                         const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
-                         const uint32_t* min_domains, const char* const* existing_node_names,
-                         const uint64_t* existing_offset, int policy, int32_t* out_status, int32_t* out_node_idx,
-                         char* json, size_t cap, int64_t* out_json_off) try {
-    if (!c || !topology_keys || (n && (!pods || !group || !out_status || !out_node_idx)) || (n_groups && !max_skew))
+// and every key g constrains.  With aff set (ksh_reconcile_affinity), ks_affinity_bind with its terms and the existing
+// pods whose node is in the store; max_skew may then be NULL.
+static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
+                            const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
+                            const uint32_t* min_domains, const char* const* existing_node_names,
+                            const uint64_t* existing_offset, const ksh_pod_affinity* aff, int policy, int32_t* out_status,
+                            int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off) {
+    if (!c || !topology_keys || (n && (!pods || !group || !out_status || !out_node_idx)) || (n_groups && !max_skew && !aff))
         return fail(KS_ERR_INVALID, "NULL argument");
     if (K == 0 || K > KS_SPREAD_MAX_KEYS)
         return fail(KS_ERR_RANGE, std::to_string(K) + " topology keys (1 to " + std::to_string(KS_SPREAD_MAX_KEYS) + ")");
@@ -1732,8 +1734,10 @@ int ksh_reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, con
     if (existing_offset)
         for (uint64_t i = 0; i < gk; i++)
             if (existing_offset[i + 1] < existing_offset[i]) return fail(KS_ERR_INVALID, "existing offsets decrease");
+    if (aff && aff->n_existing && (!aff->existing_group || !aff->existing_node_name))
+        return fail(KS_ERR_INVALID, "NULL existing_group or existing_node_name");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    int rc = device_ready(c, ks_spread_bind, "ks_spread_bind");
+    int rc = aff ? device_ready(c, ks_affinity_bind, "ks_affinity_bind") : device_ready(c, ks_spread_bind, "ks_spread_bind");
     if (rc) return rc;
     std::vector<uint64_t> todo;
     std::vector<ks_pod_obj> sub; // the pods that go to the device, in arrival order, and their groups
@@ -1773,7 +1777,7 @@ int ksh_reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, con
                     const int32_t idx = existing_node_names[i] ? node_index_of(c, existing_node_names[i]) : -1;
                     if (idx < 0) continue; // unknown: not counted
                     bool all = dom[k][idx] >= 0;
-                    for (uint32_t k2 = 0; k2 < K; k2++) all &= max_skew[g * K + k2] == 0 || dom[k2][idx] >= 0;
+                    for (uint32_t k2 = 0; k2 < K; k2++) all &= !max_skew || max_skew[g * K + k2] == 0 || dom[k2][idx] >= 0;
                     if (all) existing[g * S + P[k] + (uint32_t)dom[k][idx]]++;
                 }
     }
@@ -1782,9 +1786,27 @@ int ksh_reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, con
     sp.min_domains = min_domains;
     sp.existing = existing_offset ? existing.data() : nullptr;
     std::vector<int32_t> idx(sub.size(), -1);
-    std::vector<uint32_t> refused(sub.size(), 0);
-    rc = ks_spread_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, policy, idx.data(), nullptr, refused.data(),
-                        nullptr); // commits capacity on the device
+    const size_t R = aff ? 2 : 1; // refusal words per pod: spread, then affinity
+    std::vector<uint32_t> refused(sub.size() * R, 0);
+    if (aff) {
+        ks_pod_affinity pa{aff->n_terms, aff->owner, aff->kind, aff->key, aff->target_offset, aff->target, 0, nullptr,
+                           nullptr};
+        std::vector<int32_t> eg, en; // the existing pods whose node is in the store
+        for (uint64_t e = 0; e < aff->n_existing; e++) {
+            const int32_t at = aff->existing_node_name[e] ? node_index_of(c, aff->existing_node_name[e]) : -1;
+            if (at < 0) continue;
+            eg.push_back(aff->existing_group[e]);
+            en.push_back(at);
+        }
+        pa.n_existing = eg.size();
+        pa.existing_group = eg.data();
+        pa.existing_node = en.data();
+        rc = ks_affinity_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, policy, idx.data(), nullptr,
+                              refused.data(), nullptr);
+    } else {
+        rc = ks_spread_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, policy, idx.data(), nullptr, refused.data(),
+                            nullptr); // commits capacity on the device
+    }
     if (rc) {
         c->dirty = true; // the host list is the truth
         return rc;
@@ -1795,10 +1817,33 @@ int ksh_reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, con
         if (idx[k] >= 0)
             commit_bind(c, &pods[i], idx[k], kp.req_cpu[k], kp.req_mem[k], &out_status[i], &out_node_idx[i], bodies,
                         json && out_json_off ? &out_json_off[i] : nullptr);
-        else if (refused[k] > 0)
+        else if (refused[k * R] > 0)
             out_status[i] = KSH_RECONCILE_SPREAD_UNSATISFIED;
+        else if (aff && refused[k * R + 1] > 0)
+            out_status[i] = KSH_RECONCILE_AFFINITY_UNSATISFIED;
     }
     return KS_OK;
+}
+
+int ksh_reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
+                         const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
+                         const uint32_t* min_domains, const char* const* existing_node_names,
+                         const uint64_t* existing_offset, int policy, int32_t* out_status, int32_t* out_node_idx,
+                         char* json, size_t cap, int64_t* out_json_off) try {
+    return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
+                            existing_offset, nullptr, policy, out_status, out_node_idx, json, cap, out_json_off);
+}
+KSH_CATCH
+
+int ksh_reconcile_affinity(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
+                           const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
+                           const uint32_t* min_domains, const char* const* existing_node_names,
+                           const uint64_t* existing_offset, const ksh_pod_affinity* aff, int policy,
+                           int32_t* out_status, int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off) try {
+    const ksh_pod_affinity none{};
+    return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
+                            existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
+                            out_json_off);
 }
 KSH_CATCH
 

@@ -116,7 +116,7 @@ static int check_commit_requests(uint64_t n, const int64_t* req_cpu, const int64
 }
 
 // ---- host-staged calls: ks_stream_bind's device loop, ks_gang_bind, ks_drain_check, ks_scaleup_estimate,
-// ks_place_replicas, ks_place_replicas_spread (and _multi) and ks_spread_bind ----
+// ks_place_replicas, ks_place_replicas_spread (and _multi), ks_spread_bind and ks_affinity_bind ----
 // Such a call gathers its host inputs into the snapshot's pinned block, makes one H2D copy to d_in, launches, makes one
 // D2H copy from d_out and copies its results out before it returns.  Its HostStaged plan declares every array it stages
 // once, with its type and count: in() an input, gathered from src or, with src NULL, filled by the caller through
@@ -1791,16 +1791,128 @@ int ks_place_replicas_spread_multi(ks_snapshot* s, const ks_pods* specs, const u
                         out_domain_count);
 }
 
-int ks_spread_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
-                   const ks_spread_multi* spread, int policy, int32_t* out_node_idx, int64_t* out_score,
-                   uint32_t* out_refused, uint32_t* out_domain_count) {
+// ks_affinity_bind's terms compiled on the host (include/ksched.h, DESIGN.md 5n): the counter bases per (group, key),
+// the first-pod flag per group and each group's deduplicated update entries.
+struct AffinityPlan {
+    std::vector<uint32_t> abase;   // [G * K * 2]: B_{g,k}, A_{g,k} bases, AFF_NONE = none
+    std::vector<uint32_t> aflag;   // [G]
+    std::vector<uint32_t> upd_off; // [G + 1]
+    std::vector<uint32_t> upd;     // h | k << 16 | kind << 20
+    uint64_t words = 0;            // counter words, the G first-pod words included
+    uint32_t any_base = 0;
+};
+
+static int compile_affinity(const ks_pod_affinity* f, uint32_t G, uint32_t K, const uint32_t* Dk, uint32_t N,
+                            AffinityPlan* pl) {
+    const uint32_t T = f->n_terms;
+    const uint64_t E = f->n_existing;
+    if (T > KS_AFFINITY_MAX_TERMS) return fail(KS_ERR_RANGE, "%u affinity terms (at most %u)", T, KS_AFFINITY_MAX_TERMS);
+    if (E > KS_AFFINITY_MAX_EXISTING)
+        return fail(KS_ERR_RANGE, "%llu existing pods (at most 2^24)", (unsigned long long)E);
+    if (T && (!f->owner || !f->kind || !f->key || !f->target_offset))
+        return fail(KS_ERR_INVALID, "NULL owner, kind, key or target_offset");
+    if (E && (!f->existing_group || !f->existing_node)) return fail(KS_ERR_INVALID, "NULL existing_group or existing_node");
+    for (uint32_t t = 0; t < T; t++) {
+        if (f->owner[t] < 0 || f->owner[t] >= (int64_t)G)
+            return fail(KS_ERR_INVALID, "term %u: owner %d outside [0, %u)", t, f->owner[t], G);
+        if (f->kind[t] > KS_POD_ANTI_AFFINITY) return fail(KS_ERR_INVALID, "term %u: kind %u (0 or 1)", t, f->kind[t]);
+        if (f->key[t] >= K) return fail(KS_ERR_INVALID, "term %u: key %u (the call has %u)", t, f->key[t], K);
+        if (f->target_offset[t + 1] < f->target_offset[t]) return fail(KS_ERR_INVALID, "term %u: target offsets decrease", t);
+    }
+    const uint64_t t0 = T ? f->target_offset[0] : 0, nt = T ? f->target_offset[T] - t0 : 0;
+    if (nt > KS_AFFINITY_MAX_TARGETS) return fail(KS_ERR_RANGE, "%llu targets (at most 2^22)", (unsigned long long)nt);
+    if (nt && !f->target) return fail(KS_ERR_INVALID, "NULL target");
+    for (uint64_t i = t0; i < t0 + nt; i++)
+        if (f->target[i] < 0 || f->target[i] >= (int64_t)G)
+            return fail(KS_ERR_INVALID, "target %llu: group %d outside [0, %u)", (unsigned long long)i, f->target[i], G);
+    for (uint64_t e = 0; e < E; e++) {
+        if (f->existing_group[e] < 0 || f->existing_group[e] >= (int64_t)G)
+            return fail(KS_ERR_INVALID, "existing pod %llu: group %d outside [0, %u)", (unsigned long long)e,
+                        f->existing_group[e], G);
+        if (f->existing_node[e] < 0 || f->existing_node[e] >= (int64_t)N)
+            return fail(KS_ERR_INVALID, "existing pod %llu: node %d outside [0, %u)", (unsigned long long)e,
+                        f->existing_node[e], N);
+    }
+    // anti[g * K + k]: B_{g,k} exists (an anti relation of g on k, in either direction); akeys[g]: g's affinity keys;
+    // M[g]: the groups every affinity term of g targets, as a bitset of G bits
+    const uint64_t words = (G + 63) / 64;
+    std::vector<uint8_t> anti((size_t)G * K, 0), akeys(G, 0);
+    std::vector<uint64_t> M((size_t)G * words, 0), tmp(words);
+    std::vector<std::vector<uint32_t>> lists(G);
+    auto enc = [](uint32_t g, uint32_t k, uint32_t kind) { return g | k << 16 | kind << 20; };
+    for (uint32_t t = 0; t < T; t++) {
+        const uint32_t g = (uint32_t)f->owner[t], k = f->key[t];
+        if (f->kind[t] == KS_POD_ANTI_AFFINITY) {
+            anti[(size_t)g * K + k] = 1;
+            for (uint64_t i = f->target_offset[t]; i < f->target_offset[t + 1]; i++) {
+                const uint32_t h = (uint32_t)f->target[i];
+                anti[(size_t)h * K + k] = 1;
+                lists[h].push_back(enc(g, k, 0)); // rule 1: a pod of h raises g's count
+                lists[g].push_back(enc(h, k, 0)); // rule 2: a pod of g (carrying the term) raises h's count
+            }
+            continue;
+        }
+        std::fill(tmp.begin(), tmp.end(), 0);
+        for (uint64_t i = f->target_offset[t]; i < f->target_offset[t + 1]; i++)
+            tmp[f->target[i] >> 6] |= 1ull << (f->target[i] & 63);
+        uint64_t* m = M.data() + (size_t)g * words;
+        for (uint64_t w = 0; w < words; w++) m[w] = akeys[g] ? m[w] & tmp[w] : tmp[w];
+        akeys[g] |= (uint8_t)(1u << k);
+    }
+    // rule 3 adds |M_g| entries per affinity key of g, at most the targets of g's affinity terms: with rules 1 and 2's
+    // two per anti target, every list together stays below 3 * KS_AFFINITY_MAX_TARGETS entries before deduplication
+    pl->aflag.assign(G, 0);
+    for (uint32_t g = 0; g < G; g++) {
+        if (!akeys[g]) continue;
+        const uint64_t* m = M.data() + (size_t)g * words;
+        if (m[g >> 6] >> (g & 63) & 1) pl->aflag[g] = AFF_SELF;
+        for (uint32_t h = 0; h < G; h++)
+            if (m[h >> 6] >> (h & 63) & 1)
+                for (uint32_t k = 0; k < K; k++)
+                    if (akeys[g] >> k & 1) lists[h].push_back(enc(g, k, 1)); // rule 3: a pod of M_g raises A_{g,k}
+    }
+    pl->upd_off.assign(G + 1, 0);
+    for (uint32_t h = 0; h < G; h++) {
+        std::sort(lists[h].begin(), lists[h].end());
+        lists[h].erase(std::unique(lists[h].begin(), lists[h].end()), lists[h].end());
+        const uint64_t total = (uint64_t)pl->upd_off[h] + lists[h].size();
+        if (total > KS_AFFINITY_MAX_UPDATES)
+            return fail(KS_ERR_RANGE, "more than 2^24 update entries (%llu by group %u)", (unsigned long long)total, h);
+        pl->upd_off[h + 1] = (uint32_t)total;
+    }
+    pl->upd.reserve(pl->upd_off[G]);
+    for (uint32_t h = 0; h < G; h++) pl->upd.insert(pl->upd.end(), lists[h].begin(), lists[h].end());
+    pl->abase.assign((size_t)G * K * 2, AFF_NONE);
+    uint64_t word = 0;
+    for (uint32_t g = 0; g < G; g++)
+        for (uint32_t k = 0; k < K; k++) {
+            if (anti[(size_t)g * K + k]) {
+                pl->abase[((size_t)g * K + k) * 2] = (uint32_t)word;
+                word += Dk[k];
+            }
+            if (akeys[g] >> k & 1) {
+                pl->abase[((size_t)g * K + k) * 2 + 1] = (uint32_t)word;
+                word += Dk[k];
+            }
+        }
+    pl->any_base = (uint32_t)word;
+    pl->words = word + G;
+    if (pl->words > KS_SPREAD_MAX_COUNTS)
+        return fail(KS_ERR_RANGE, "%llu affinity counter words (at most 2^26)", (unsigned long long)pl->words);
+    return KS_OK;
+}
+
+// ks_spread_bind, and with aff set ks_affinity_bind (then max_skew may be NULL and out_refused holds 2P words)
+static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
+                       const ks_spread_multi* spread, const ks_pod_affinity* aff, int policy, int32_t* out_node_idx,
+                       int64_t* out_score, uint32_t* out_refused, uint32_t* out_domain_count) {
     int rc = check_pods(s, pods);
     if (rc) return rc;
-    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_spread_bind takes host-space pods");
+    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "%s takes host-space pods", call);
     if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
     const uint64_t P = pods->n, G = n_groups;
     if (P && (!group || !out_node_idx)) return fail(KS_ERR_INVALID, "NULL group or out_node_idx");
-    if (!spread || (G && !spread->max_skew)) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
+    if (!spread || (G && !spread->max_skew && !aff)) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
     if (P > KS_SPREAD_BIND_MAX_PODS)
         return fail(KS_ERR_RANGE, "%llu pods (at most %u)", (unsigned long long)P, KS_SPREAD_BIND_MAX_PODS);
     if (G > KS_SPREAD_BIND_MAX_GROUPS)
@@ -1823,7 +1935,7 @@ int ks_spread_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, ui
     try {
         first.assign(G, -1);
     } catch (...) {
-        return fail(KS_ERR_NOMEM, "out of host memory in ks_spread_bind");
+        return fail(KS_ERR_NOMEM, "out of host memory in %s", call);
     }
     for (uint64_t p = 0; p < P; p++) {
         const int32_t g = group[p];
@@ -1837,11 +1949,21 @@ int ks_spread_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, ui
     }
     rc = check_commit_requests(P, pods->req_cpu, pods->req_mem);
     if (rc) return rc;
+    AffinityPlan plan;
+    if (aff) {
+        try {
+            rc = compile_affinity(aff, (uint32_t)G, K, spread->n_domains, N, &plan);
+        } catch (...) {
+            return fail(KS_ERR_NOMEM, "out of host memory in %s", call);
+        }
+        if (rc) return rc;
+    }
+    const uint64_t R = aff ? 2 : 1; // refusal words per pod
     if (P == 0) return KS_OK;
     if (N == 0) { // no node: nothing is placed, every count is existing
         memset(out_node_idx, 0xff, P * 4);
         if (out_score) memset(out_score, 0, P * 8);
-        if (out_refused) memset(out_refused, 0, P * 4);
+        if (out_refused) memset(out_refused, 0, P * R * 4);
         if (out_domain_count) {
             if (spread->existing) memcpy(out_domain_count, spread->existing, GS * 4);
             else memset(out_domain_count, 0, GS * 4);
@@ -1858,15 +1980,24 @@ int ks_spread_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, ui
     const auto cpu = h.in(pods->req_cpu, P), mem = h.in(pods->req_mem, P);
     const auto sel = h.in(pods->sel, P * W);
     const auto grp = h.in(group, P);
-    const auto max_skew = h.in(spread->max_skew, G * K);
+    const auto max_skew = h.in(spread->max_skew, G * K); // NULL (affinity only): zeros, filled below
     const auto min_domains = h.in(spread->min_domains, spread->min_domains ? G * K : 0);
     const auto existing = h.in(spread->existing, spread->existing ? GS : 0);
     const auto dom = h.in<int32_t>(nullptr, (uint64_t)K * N);  // the K node_domain arrays, gathered below
     const auto gsel = h.in<uint64_t>(nullptr, G * W);          // each group's selector
     const auto score = h.out(out_score, P);
     const auto idx = h.out(out_node_idx, P);
-    const auto refused = h.out(out_refused, P);
+    const auto refused = h.out(out_refused, P * R);
     const auto count = h.out(out_domain_count, GS);           // the counts themselves: device state of the whole call
+    const uint64_t E = aff ? aff->n_existing : 0;
+    const auto abase = h.in<uint32_t>(nullptr, plan.abase.size()); // the compiled terms, copied from plan below
+    const auto aflag = h.in<uint32_t>(nullptr, plan.aflag.size());
+    const auto upd_off = h.in<uint32_t>(nullptr, plan.upd_off.size());
+    const auto upd = h.in<uint32_t>(nullptr, plan.upd.size());
+    const auto ex_group = h.in(aff ? aff->existing_group : nullptr, E);
+    const auto ex_node = h.in(aff ? aff->existing_node : nullptr, E);
+    const auto acnt = h.work<uint32_t>(plan.words, 16);
+    const auto paref = h.work<uint32_t>(aff ? a.grid : 0);
     const auto elig = h.work<uint8_t>(GS);
     const auto gk = h.work<uint32_t>(G * K * 4, 16);
     const auto pkey = h.work<int64_t>(a.grid);
@@ -1874,6 +2005,14 @@ int ks_spread_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, ui
     const auto pref = h.work<uint32_t>(a.grid);
     CU_TRY(h.reserve(s));
     for (uint32_t k = 0; k < K; k++) memcpy(h.host(dom) + (size_t)k * N, spread->node_domain[k], (size_t)N * 4);
+    if (!spread->max_skew) memset(h.host(max_skew), 0, G * K * 4);
+    auto put = [&](Staged<uint32_t> d, const std::vector<uint32_t>& v) {
+        if (!v.empty()) memcpy(h.host(d), v.data(), v.size() * 4);
+    };
+    put(abase, plan.abase);
+    put(aflag, plan.aflag);
+    put(upd_off, plan.upd_off);
+    put(upd, plan.upd);
     for (uint64_t g = 0; g < G; g++) {
         uint64_t* row = h.host(gsel) + g * W;
         if (first[g] >= 0) memcpy(row, pods->sel + first[g] * W, W * 8);
@@ -1915,13 +2054,42 @@ int ks_spread_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, ui
     a.out_idx = h.dev(idx);
     a.out_score = h.dev(score);
     a.out_refused = h.dev(refused);
+    if (aff) {
+        a.abase = h.dev(abase);
+        a.aflag = h.dev(aflag);
+        a.upd_off = h.dev(upd_off);
+        a.upd = h.dev(upd);
+        a.ex_group = h.dev(ex_group);
+        a.ex_node = h.dev(ex_node);
+        a.E = (uint32_t)E;
+        a.any_base = plan.any_base;
+        a.aff_grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((E + 7) / 8, 4ull * (uint64_t)s->sms));
+        a.acnt = h.dev(acnt);
+        a.paref = h.dev(paref);
+    }
     s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
     s->version++;
-    cudaError_t e = launch_spread_bind(a, W, st);
-    if (e != cudaSuccess) return fail(KS_ERR_CUDA, "spread bind launch failed: %s", cudaGetErrorString(e));
+    cudaError_t e = aff ? launch_affinity_bind(a, plan.words, W, st) : launch_spread_bind(a, W, st);
+    if (e != cudaSuccess)
+        return fail(KS_ERR_CUDA, "%s launch failed: %s", aff ? "affinity bind" : "spread bind", cudaGetErrorString(e));
     CU_TRY(h.finish(st));
-    s->last_path = "spread_bind";
+    s->last_path = aff ? "affinity_bind" : "spread_bind";
     return KS_OK;
+}
+
+int ks_spread_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
+                   const ks_spread_multi* spread, int policy, int32_t* out_node_idx, int64_t* out_score,
+                   uint32_t* out_refused, uint32_t* out_domain_count) {
+    return bind_spread(s, "ks_spread_bind", pods, group, n_groups, spread, nullptr, policy, out_node_idx, out_score,
+                       out_refused, out_domain_count);
+}
+
+int ks_affinity_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
+                     const ks_spread_multi* topo, const ks_pod_affinity* aff, int policy, int32_t* out_node_idx,
+                     int64_t* out_score, uint32_t* out_refused, uint32_t* out_domain_count) {
+    const ks_pod_affinity none{};
+    return bind_spread(s, "ks_affinity_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
+                       out_score, out_refused, out_domain_count);
 }
 
 // ---------------------------------------------------------------------------------------------- async streaming

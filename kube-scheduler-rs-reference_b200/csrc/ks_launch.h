@@ -254,9 +254,24 @@ struct SpreadBindArgs {
     uint32_t* pref;
     int32_t* out_idx;                 // [P]
     int64_t* out_score;               // [P]
-    uint32_t* out_refused;            // [P]
+    uint32_t* out_refused;            // [P]; [2P] under affinity: spread, then affinity refusals
     uint32_t grid, setup_grid;
+    // inter-pod affinity (ks_affinity_bind; read only by its kernels).  Counter arrays B_{g,k} / A_{g,k} of D_k words
+    // in acnt; one word per group at acnt[any_base + g] is set once a pod of M_g is bound on a node that carries one of
+    // g's affinity keys.  Update entry: h | k << 16 | kind << 20 (kind 0 = B, 1 = A) raises that array of group h.
+    const uint32_t* abase;            // [G * K * 2]: base of B_{g,k}, then of A_{g,k}, in acnt; AFF_NONE = no array
+    const uint32_t* aflag;            // [G]: AFF_SELF when g is in M_g
+    const uint32_t* upd_off;          // [G + 1]: group h's update entries
+    const uint32_t* upd;
+    const int32_t *ex_group, *ex_node; // [E] existing pods
+    uint32_t E, any_base, aff_grid;
+    uint32_t* acnt;                   // counters, zeroed by the launcher
+    uint32_t* paref;                  // [grid] per-CTA affinity refusals
 };
 uint32_t spread_bind_setup_grid(uint32_t G, int sms);
 cudaError_t launch_spread_bind(const SpreadBindArgs& a, uint32_t W, cudaStream_t st);
+constexpr uint32_t AFF_NONE = 0xffffffffu, AFF_SELF = 1u;
+// ks_affinity_bind (ks_spread_bind.cu): k_spread_bind_setup when G > 0, the counters zeroed, k_affinity_setup over the
+// existing pods (aff_grid CTAs, when E > 0), then one cooperative launch of grid CTAs, k_affinity_bind_seq
+cudaError_t launch_affinity_bind(const SpreadBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st);
 } // namespace ks

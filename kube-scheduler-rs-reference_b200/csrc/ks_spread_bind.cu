@@ -1,4 +1,5 @@
-// ks_spread_bind.cu — topology spread when binding (ks_spread_bind, include/ksched.h; DESIGN.md 5m).
+// ks_spread_bind.cu — topology spread when binding (ks_spread_bind, include/ksched.h; DESIGN.md 5m), and the same with
+// inter-pod affinity (ks_affinity_bind; DESIGN.md 5n).
 // A mixed pod queue is bound one pod at a time, each pod under its group's spread constraints against the counts and the
 // free[] every earlier pod left, as upstream kube-scheduler runs one scheduling cycle per pod.  Two kernels:
 //   k_spread_bind_setup  one CTA per group (grid-strided): the group's eligible domains per constrained key, its counts
@@ -7,6 +8,10 @@
 //                        owns one slice of the node table; per pod, phase A scans every slice and writes one partial per
 //                        CTA, phase B (CTA 0) merges the partials in CTA order, charges free[], writes the binding and
 //                        raises the counts; the two phases are separated by grid barriers.
+// ks_affinity_bind adds k_affinity_setup (the existing pods' update entries, one warp per pod) and runs
+// k_affinity_bind_seq, the same walk with the phase helpers' AFF instances: phase A also applies rules 1-3 of the header
+// through at most 2K counter loads per node, phase B also applies the bound pod's update entries across CTA 0.  The
+// AFF = false instances are the code k_spread_bind_seq always ran.
 #include "ks_internal.cuh"
 #include "ks_launch.h"
 
@@ -128,12 +133,26 @@ __global__ void __launch_bounds__(SBD_THREADS) k_spread_bind_setup(const SpreadB
     }
 }
 
+// Inter-pod affinity: one update entry of a pod bound at node n.  Entries of one list name distinct (group, key, kind)
+// arrays, so CTA 0's threads raise them without atomics; the existing pods' lists run concurrently and use atomics.
+template <bool ATOMIC>
+__device__ __forceinline__ void affinity_raise(const SpreadBindArgs& a, uint32_t entry, uint32_t n) {
+    const uint32_t h = entry & 0xffffu, k = entry >> 16 & 0xfu, kind = entry >> 20;
+    const int32_t d = __ldg(a.dom + (size_t)k * a.N + n);
+    if (d < 0) return; // the node lacks the key: no domain to count in
+    uint32_t* c = a.acnt + __ldg(a.abase + ((size_t)h * a.K + k) * 2 + kind) + (uint32_t)d;
+    if (ATOMIC) atomicAdd(c, 1u);
+    else *c = __ldcg(c) + 1;
+    if (kind) a.acnt[a.any_base + h] = 1; // a pod of M_h sits on a node that carries one of h's affinity keys
+}
+
 // Phase A of pod p in this CTA's slice [n0, n1): fit, selector and, for a constrained pod, cnt < m + max_skew on every
 // constrained key; the best candidate by the policy's key (ties to the lower node) and the refused count into the CTA's
-// partial
-template <int W>
+// partial.  AFF: then rules 1-3 of ks_affinity_bind against the pod's group's counter bases, formed once per pod; the
+// nodes they refuse into s_aref / paref.
+template <int W, bool AFF>
 __device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32_t p, uint32_t n0, uint32_t n1,
-                                                 int64_t* s_key, int32_t* s_idx, uint32_t* s_ref) {
+                                                 int64_t* s_key, int32_t* s_idx, uint32_t* s_ref, uint32_t* s_aref) {
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int32_t g = __ldg(a.group + p);
     const int64_t rc = __ldg(a.req_cpu + p), rm = __ldg(a.req_mem + p);
@@ -148,9 +167,20 @@ __device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32
                                       __ldg(a.max_skew + (size_t)g * a.K + k)
                                 : 0;
     const uint32_t* cnt = a.cnt + (size_t)(g < 0 ? 0 : g) * a.S;
+    uint32_t bB[KS_SPREAD_MAX_KEYS], bA[KS_SPREAD_MAX_KEYS]; // B_{g,k} / A_{g,k} bases, AFF_NONE = no such array
+    bool first = false;                                      // upstream's first-pod rule holds for g
+    if constexpr (AFF) {
+#pragma unroll
+        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) {
+            const bool on = g >= 0 && k < a.K;
+            bB[k] = on ? __ldg(a.abase + ((size_t)g * a.K + k) * 2) : AFF_NONE;
+            bA[k] = on ? __ldg(a.abase + ((size_t)g * a.K + k) * 2 + 1) : AFF_NONE;
+        }
+        first = g >= 0 && (__ldg(a.aflag + g) & AFF_SELF) && __ldcg(a.acnt + a.any_base + g) == 0;
+    }
     int64_t best = INT64_MIN;
     int32_t bidx = -1;
-    uint32_t refused = 0;
+    uint32_t refused = 0, arefused = 0;
     for (uint32_t n = n0 + tid; n < n1; n += SBD_THREADS) {
         const int64_t fc = __ldcg(a.free_cpu + n), fm = __ldcg(a.free_mem + n);
         uint64_t miss = 0;
@@ -168,6 +198,21 @@ __device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32
             refused++;
             continue;
         }
+        if constexpr (AFF) {
+            bool aok = true;
+#pragma unroll
+            for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
+                if ((bB[k] & bA[k]) != AFF_NONE) {
+                    const int32_t d = __ldg(a.dom + (size_t)k * a.N + n);
+                    const uint32_t dd = (uint32_t)max(d, 0);
+                    if (bB[k] != AFF_NONE) aok &= d < 0 || __ldcg(a.acnt + bB[k] + dd) == 0;        // rules 1 and 2
+                    if (bA[k] != AFF_NONE) aok &= d >= 0 && (first || __ldcg(a.acnt + bA[k] + dd) > 0); // rule 3
+                }
+            if (!aok) {
+                arefused++;
+                continue;
+            }
+        }
         const int64_t key = alloc_score_rt(a.policy, fc, fm, a.alloc_cpu, a.alloc_mem, n, rc, rm);
         if (key > best) { // ascending n per thread: strict '>' keeps the lowest index
             best = key;
@@ -176,10 +221,12 @@ __device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32
     }
     warp_argmax(best, bidx);
     refused = __reduce_add_sync(0xffffffffu, refused);
+    if constexpr (AFF) arefused = __reduce_add_sync(0xffffffffu, arefused);
     if (lane == 0) {
         s_key[warp] = best;
         s_idx[warp] = bidx;
         s_ref[warp] = refused;
+        if constexpr (AFF) s_aref[warp] = arefused;
     }
     __syncthreads();
     if (warp == 0) {
@@ -187,10 +234,12 @@ __device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32
         bidx = lane < SBD_WARPS ? s_idx[lane] : -1;
         warp_argmax(best, bidx);
         refused = __reduce_add_sync(0xffffffffu, lane < SBD_WARPS ? s_ref[lane] : 0u);
+        if constexpr (AFF) arefused = __reduce_add_sync(0xffffffffu, lane < SBD_WARPS ? s_aref[lane] : 0u);
         if (lane == 0) {
             a.pkey[blockIdx.x] = best;
             a.pidx[blockIdx.x] = bidx;
             a.pref[blockIdx.x] = refused;
+            if constexpr (AFF) a.paref[blockIdx.x] = arefused;
         }
     }
 }
@@ -198,25 +247,35 @@ __device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32
 // Phase B of pod p, CTA 0 only: merge the partials in CTA order, write the binding, charge free[] and raise the group's
 // counts.  When the last eligible domain at m takes the pod, m rises by exactly one and the domains at the new m are
 // counted over the group's domains of that key (the counts only rise, so at most final m - initial m such passes).
+// AFF: both refusals into out_refused[2p, 2p + 1], and the bound pod's update entries across the CTA (s_bidx).
+template <bool AFF>
 __device__ __forceinline__ void spread_bind_commit(const SpreadBindArgs& a, uint32_t p, uint32_t* s_rescan,
-                                                   uint32_t* s_red) {
+                                                   uint32_t* s_red, int32_t* s_bidx) {
     const uint32_t tid = threadIdx.x, lane = tid & 31;
     const int32_t g = __ldg(a.group + p);
     if (tid < 32) {
         int64_t best = INT64_MIN;
         int32_t bidx = -1;
-        uint32_t refused = 0;
+        uint32_t refused = 0, arefused = 0;
         for (uint32_t c = lane; c < gridDim.x; c += 32) { // ascending CTA = ascending node range
             merge_partial(best, bidx, __ldcg(a.pkey + c), __ldcg(a.pidx + c));
             refused += __ldcg(a.pref + c);
+            if constexpr (AFF) arefused += __ldcg(a.paref + c);
         }
         warp_argmax(best, bidx);
         refused = __reduce_add_sync(0xffffffffu, refused);
+        if constexpr (AFF) arefused = __reduce_add_sync(0xffffffffu, arefused);
         if (lane == 0) {
             uint32_t rescan = 0;
             a.out_idx[p] = bidx;
             a.out_score[p] = bidx >= 0 ? key_score_rt(a.policy, best, a.req_cpu, a.req_mem, p) : 0;
-            a.out_refused[p] = refused;
+            if constexpr (AFF) {
+                a.out_refused[2 * (size_t)p] = refused;
+                a.out_refused[2 * (size_t)p + 1] = arefused;
+                *s_bidx = bidx;
+            } else {
+                a.out_refused[p] = refused;
+            }
             if (bidx >= 0) {
                 a.free_cpu[bidx] = __ldcg(a.free_cpu + bidx) - __ldg(a.req_cpu + p);
                 a.free_mem[bidx] = __ldcg(a.free_mem + bidx) - __ldg(a.req_mem + p);
@@ -248,6 +307,12 @@ __device__ __forceinline__ void spread_bind_commit(const SpreadBindArgs& a, uint
         const uint32_t at = domains_at(a, (uint32_t)g, k, __ldcg(st + GK_M), s_red);
         if (tid == 0) st[GK_AT_M] = at;
     }
+    if constexpr (AFF) {
+        const int32_t b = *s_bidx;
+        if (b >= 0 && g >= 0)
+            for (uint32_t e = __ldg(a.upd_off + g) + tid, e1 = __ldg(a.upd_off + g + 1); e < e1; e += SBD_THREADS)
+                affinity_raise<false>(a, __ldg(a.upd + e), (uint32_t)b);
+    }
 }
 
 template <int W>
@@ -260,10 +325,41 @@ __global__ void __launch_bounds__(SBD_THREADS, 1) k_spread_bind_seq(const Spread
     const uint32_t G = gridDim.x;
     const uint32_t chunk = (a.N + G - 1) / G, n0 = min(a.N, blockIdx.x * chunk), n1 = min(a.N, n0 + chunk);
     for (uint32_t p = 0; p < a.P; p++) {
-        spread_bind_scan<W>(a, p, n0, n1, s_key, s_idx, s_ref);
+        spread_bind_scan<W, false>(a, p, n0, n1, s_key, s_idx, s_ref, nullptr);
         __threadfence();
         grid.sync();
-        if (blockIdx.x == 0) spread_bind_commit(a, p, &s_rescan, s_ref);
+        if (blockIdx.x == 0) spread_bind_commit<false>(a, p, &s_rescan, s_ref, nullptr);
+        __threadfence();
+        grid.sync();
+    }
+}
+
+// The existing pods' update entries into the zeroed counters, one warp per pod (grid-strided)
+__global__ void __launch_bounds__(SBD_THREADS) k_affinity_setup(const SpreadBindArgs a) {
+    const uint32_t lane = threadIdx.x & 31, warps = gridDim.x * SBD_WARPS;
+    for (uint32_t e = blockIdx.x * SBD_WARPS + (threadIdx.x >> 5); e < a.E; e += warps) {
+        const int32_t h = __ldg(a.ex_group + e), n = __ldg(a.ex_node + e);
+        for (uint32_t i = __ldg(a.upd_off + h) + lane, i1 = __ldg(a.upd_off + h + 1); i < i1; i += 32)
+            affinity_raise<true>(a, __ldg(a.upd + i), (uint32_t)n);
+    }
+}
+
+// k_spread_bind_seq with the AFF instances of both phases
+template <int W>
+__global__ void __launch_bounds__(SBD_THREADS, 1) k_affinity_bind_seq(const SpreadBindArgs a) {
+    cg::grid_group grid = cg::this_grid();
+    __shared__ int64_t s_key[SBD_WARPS];
+    __shared__ int32_t s_idx[SBD_WARPS];
+    __shared__ uint32_t s_ref[SBD_WARPS], s_aref[SBD_WARPS];
+    __shared__ uint32_t s_rescan;
+    __shared__ int32_t s_bidx;
+    const uint32_t G = gridDim.x;
+    const uint32_t chunk = (a.N + G - 1) / G, n0 = min(a.N, blockIdx.x * chunk), n1 = min(a.N, n0 + chunk);
+    for (uint32_t p = 0; p < a.P; p++) {
+        spread_bind_scan<W, true>(a, p, n0, n1, s_key, s_idx, s_ref, s_aref);
+        __threadfence();
+        grid.sync();
+        if (blockIdx.x == 0) spread_bind_commit<true>(a, p, &s_rescan, s_ref, &s_bidx);
         __threadfence();
         grid.sync();
     }
@@ -284,6 +380,32 @@ cudaError_t launch_spread_bind(const SpreadBindArgs& a, uint32_t W, cudaStream_t
         void* args[] = {&b};
         const cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(k_spread_bind_seq<LW>),
                                                           dim3(a.grid), dim3(SBD_THREADS), args, 0, st);
+        if (e == cudaSuccess) g_launches++;
+        return e;
+    });
+}
+
+cudaError_t launch_affinity_bind(const SpreadBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
+    return with_label_width(W, [&](auto w) {
+        constexpr int LW = decltype(w)::value;
+        if (a.G) {
+            k_spread_bind_setup<LW><<<a.setup_grid, SBD_THREADS, 0, st>>>(a);
+            g_launches++;
+            const cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess) return e;
+        }
+        cudaError_t e = cudaMemsetAsync(a.acnt, 0, acnt_words * 4, st);
+        if (e != cudaSuccess) return e;
+        if (a.E) {
+            k_affinity_setup<<<a.aff_grid, SBD_THREADS, 0, st>>>(a);
+            g_launches++;
+            e = cudaGetLastError();
+            if (e != cudaSuccess) return e;
+        }
+        SpreadBindArgs b = a;
+        void* args[] = {&b};
+        e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(k_affinity_bind_seq<LW>), dim3(a.grid),
+                                        dim3(SBD_THREADS), args, 0, st);
         if (e == cudaSuccess) g_launches++;
         return e;
     });

@@ -52,6 +52,8 @@ for _name, _res, _args in [
                                                   C.c_int, _vp, _vp, _vp, _vp]),
     ("ksh_reconcile_spread", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp, C.c_int,
                                        _vp, _vp, _vp, C.c_size_t, _vp]),
+    ("ksh_reconcile_affinity", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp,
+                                         C.c_int, _vp, _vp, _vp, C.c_size_t, _vp]),
 ]:
     _proto(_name, _res, *_args)
 
@@ -59,6 +61,13 @@ KSH_DEVICE_NONE = -1  # packing-only context: objects -> SoA arrays on the host,
 KSH_RECONCILE_OK, KSH_RECONCILE_NO_NODE_FOUND, KSH_RECONCILE_BINDING_OBJECT_FAILED = 0, 1, 2
 KSH_RECONCILE_GANG_UNSATISFIED = 4
 KSH_RECONCILE_SPREAD_UNSATISFIED = 5
+KSH_RECONCILE_AFFINITY_UNSATISFIED = 6
+
+
+class ksh_pod_affinity(C.Structure):
+    _fields_ = [("n_terms", C.c_uint32), ("owner", C.c_void_p), ("kind", C.c_void_p), ("key", C.c_void_p),
+                ("target_offset", C.c_void_p), ("target", C.c_void_p), ("n_existing", C.c_uint64),
+                ("existing_group", C.c_void_p), ("existing_node_name", C.c_void_p)]
 
 
 def _addr(arr, i=0):
@@ -432,6 +441,53 @@ class Context:
                                        None if names is None else C.cast(names, _vp),
                                        None if ex_off is None else ex_off.ctypes.data, int(policy), status.ctypes.data,
                                        node.ctypes.data, C.addressof(buf), cap, off.ctypes.data), "ksh_reconcile_spread")
+        return status, node, _string_list(buf, off)
+
+    def reconcile_affinity(self, pods, n, group, n_groups, topology_keys, terms=(), existing_pods=(), max_skew=None,
+                           min_domains=None, existing_nodes=None, policy=capi.KS_SCORE_LEFTOVER, json_cap=None):
+        """reconcile() under spread and required inter-pod affinity (ksh_reconcile_affinity): reconcile_spread with
+        max_skew optional (None: no spread constraint), terms a list of (owner group, kind KS_POD_AFFINITY /
+        KS_POD_ANTI_AFFINITY, index into topology_keys, target groups) and existing_pods a list of (group, node name) of
+        bound pods the terms see.  Returns (status[n], node_idx[n], bodies[n] (str | None))."""
+        k = len(topology_keys)
+        group = np.ascontiguousarray(group, np.int32).reshape(-1)
+        if group.shape[0] != n:
+            raise ValueError(f"group has {group.shape[0]} entries, pods {n}")
+        if max_skew is not None:
+            max_skew = np.ascontiguousarray(max_skew, np.uint32).reshape(-1)
+            if max_skew.shape[0] != n_groups * k:
+                raise ValueError(f"max_skew has {max_skew.shape[0]} entries, groups {n_groups}, keys {k}")
+        mind = None if min_domains is None else np.ascontiguousarray(min_domains, np.uint32).reshape(-1)
+        names, ex_off = None, None
+        if existing_nodes is not None:
+            lists = [lst for per_group in existing_nodes for lst in per_group]
+            flat = [s.encode() for lst in lists for s in lst]
+            names = (C.c_char_p * max(len(flat), 1))(*flat)
+            ex_off = np.zeros(n_groups * k + 1, np.uint64)
+            np.cumsum([len(lst) for lst in lists], out=ex_off[1:])
+        owner = np.ascontiguousarray([t[0] for t in terms], np.int32)
+        kind = np.ascontiguousarray([t[1] for t in terms], np.uint8)
+        tkey = np.ascontiguousarray([t[2] for t in terms], np.uint32)
+        toff = np.zeros(len(terms) + 1, np.uint64)
+        np.cumsum([len(t[3]) for t in terms], out=toff[1:])
+        target = np.ascontiguousarray([g for t in terms for g in t[3]], np.int32)
+        egroup = np.ascontiguousarray([e[0] for e in existing_pods], np.int32)
+        enames = (C.c_char_p * max(len(existing_pods), 1))(*[e[1].encode() for e in existing_pods])
+        aff = ksh_pod_affinity(len(terms), owner.ctypes.data, kind.ctypes.data, tkey.ctypes.data, toff.ctypes.data,
+                               target.ctypes.data, len(existing_pods), egroup.ctypes.data, C.cast(enames, _vp))
+        keys = (C.c_char_p * max(k, 1))(*[key.encode() for key in topology_keys])
+        status = np.empty(n, np.int32)
+        node = np.empty(n, np.int32)
+        off = np.empty(n, np.int64)
+        cap = int(json_cap if json_cap is not None else 512 * max(n, 1))
+        buf = C.create_string_buffer(max(cap, 1))
+        check(lib.ksh_reconcile_affinity(self._h, C.addressof(pods) if n else None, n, group.ctypes.data, int(n_groups),
+                                         C.cast(keys, _vp), k, None if max_skew is None else max_skew.ctypes.data,
+                                         None if mind is None else mind.ctypes.data,
+                                         None if names is None else C.cast(names, _vp),
+                                         None if ex_off is None else ex_off.ctypes.data, C.byref(aff), int(policy),
+                                         status.ctypes.data, node.ctypes.data, C.addressof(buf), cap, off.ctypes.data),
+              "ksh_reconcile_affinity")
         return status, node, _string_list(buf, off)
 
     def drain_nodes(self, node_names, pods, pod_offset, policy=capi.KS_SCORE_LEFTOVER, flags=0):

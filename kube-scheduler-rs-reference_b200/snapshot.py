@@ -395,6 +395,62 @@ class Snapshot:
             counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
         return idx, score, refused, counts
 
+    def affinity_bind(self, req_cpu, req_mem, sel, group, n_groups, keys, terms=(), existing_pods=None, max_skew=None,
+                      min_domains=None, existing=None, policy=capi.KS_SCORE_LEFTOVER, want_counts=True):
+        """spread_bind with required inter-pod affinity and anti-affinity (ks_affinity_bind): G = n_groups groups;
+        terms a list of (owner group, kind KS_POD_AFFINITY / KS_POD_ANTI_AFFINITY, key index, target groups);
+        existing_pods None or (groups, nodes) of the bound pods the terms see; max_skew [G, K] or None (no spread
+        constraint), min_domains and existing as in spread_bind.  Charges free[].  Returns (node_idx int32 [P], score
+        int64 [P], refused uint32 [P, 2] (spread, affinity), counts)."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        p, g = int(pods.n), int(n_groups)
+        group = _c(group, np.int32).reshape(-1)
+        if group.shape[0] != p:
+            raise ValueError(f"group has {group.shape[0]} entries, pods {p}")
+        k = len(keys)
+        if not 1 <= k <= capi.KS_SPREAD_MAX_KEYS:
+            raise ValueError(f"{k} topology keys (1 to {capi.KS_SPREAD_MAX_KEYS})")
+        doms = [_c(d, np.int32).reshape(-1) for d, _ in keys]
+        nd = [int(n) for _, n in keys]
+        if max_skew is not None:
+            max_skew = _c(max_skew, np.uint32).reshape(-1)
+            if max_skew.shape[0] != g * k:
+                raise ValueError(f"max_skew has {max_skew.shape[0]} entries, groups x keys {g * k}")
+        if min_domains is not None:
+            min_domains = _c(min_domains, np.uint32).reshape(-1)
+            if min_domains.shape[0] != g * k:
+                raise ValueError(f"min_domains has {min_domains.shape[0]} entries, groups x keys {g * k}")
+        s = sum(nd)
+        if existing is not None:
+            if len(existing) != k:
+                raise ValueError(f"existing has {len(existing)} blocks, keys {k}")
+            existing = _c(np.concatenate([np.asarray(e, np.uint32).reshape(g, n) for e, n in zip(existing, nd)],
+                                         axis=1), np.uint32).reshape(-1)
+        topo = capi.ks_spread_multi(k, (C.c_uint32 * capi.KS_SPREAD_MAX_KEYS)(*nd),
+                                    (C.c_void_p * capi.KS_SPREAD_MAX_KEYS)(*[_ptr(d) for d in doms]),
+                                    _ptr(max_skew), _ptr(min_domains), _ptr(existing))
+        owner = _c([t[0] for t in terms], np.int32)
+        kind = _c([t[1] for t in terms], np.uint8)
+        key = _c([t[2] for t in terms], np.uint32)
+        toff = np.zeros(len(terms) + 1, np.uint64)
+        np.cumsum([len(t[3]) for t in terms], out=toff[1:])
+        target = _c(np.concatenate([np.asarray(t[3], np.int64).reshape(-1) for t in terms]) if terms else [], np.int32)
+        eg, en = (np.zeros(0, np.int32),) * 2 if existing_pods is None else existing_pods
+        eg, en = _c(eg, np.int32).reshape(-1), _c(en, np.int32).reshape(-1)
+        if eg.shape[0] != en.shape[0]:
+            raise ValueError(f"existing pods: {eg.shape[0]} groups, {en.shape[0]} nodes")
+        aff = capi.ks_pod_affinity(len(terms), _ptr(owner), _ptr(kind), _ptr(key), _ptr(toff), _ptr(target),
+                                   eg.shape[0], _ptr(eg), _ptr(en))
+        idx = np.empty(p, np.int32)
+        score = np.empty(p, np.int64)
+        refused = np.empty((p, 2), np.uint32)
+        counts = np.empty((g, s), np.uint32) if want_counts and 0 < g * s <= capi.KS_SPREAD_MAX_COUNTS else None
+        check(lib.ks_affinity_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff), int(policy),
+                                   _ptr(idx), _ptr(score), _ptr(refused), _ptr(counts)), "ks_affinity_bind")
+        if counts is not None:
+            counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
+        return idx, score, refused, counts
+
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
         """The reference's own policy (src/main.rs:49-71), seeded: (node_idx, attempts_used, draw_node, draw_code)."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
