@@ -58,6 +58,8 @@ pub const KS_AFFINITY_MAX_TERMS: u32 = 16384; // most terms of one ks_affinity_b
 pub const KS_AFFINITY_MAX_TARGETS: u64 = 1 << 22; // most target entries over all terms
 pub const KS_AFFINITY_MAX_EXISTING: u64 = 1 << 24; // most existing pods
 pub const KS_AFFINITY_MAX_UPDATES: u64 = 1 << 24; // most compiled update entries
+pub const KS_POD_AFFINITY_PREFERRED: u8 = 2; // ks_profile_bind: preferred terms score only
+pub const KS_POD_ANTI_AFFINITY_PREFERRED: u8 = 3;
 
 #[repr(C)]
 pub struct ks_kv {
@@ -224,6 +226,15 @@ pub struct ks_pod_affinity {
     pub existing_node: *const i32,
 }
 #[repr(C)]
+pub struct ks_bind_scoring {
+    pub soft_skew: *const u32,
+    pub soft_all_keys: *const u8,
+    pub term_weight: *const u32,
+    pub hard_affinity_weight: u32,
+    pub weight_spread: u32,
+    pub weight_affinity: u32,
+}
+#[repr(C)]
 pub struct ksh_pod_affinity {
     pub n_terms: u32,
     pub owner: *const i32,
@@ -296,6 +307,10 @@ extern "C" {
     pub fn ks_affinity_bind(s: *mut ks_snapshot, pods: *const ks_pods, group: *const i32, n_groups: u32,
                             topo: *const ks_spread_multi, aff: *const ks_pod_affinity, policy: c_int,
                             node_idx: *mut i32, score: *mut i64, refused: *mut u32, domain_count: *mut u32) -> c_int;
+    pub fn ks_profile_bind(s: *mut ks_snapshot, pods: *const ks_pods, group: *const i32, n_groups: u32,
+                           topo: *const ks_spread_multi, aff: *const ks_pod_affinity, scoring: *const ks_bind_scoring,
+                           policy: c_int, node_idx: *mut i32, score: *mut i64, parts: *mut i64, refused: *mut u32,
+                           domain_count: *mut u32, soft_count: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -369,6 +384,12 @@ extern "C" {
                                   existing_offset: *const u64, aff: *const ksh_pod_affinity, policy: c_int,
                                   status: *mut i32, node_idx: *mut i32, json: *mut c_char, cap: usize,
                                   json_off: *mut i64) -> c_int;
+    pub fn ksh_reconcile_profile(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group: *const i32,
+                                 n_groups: u32, topology_keys: *const *const c_char, n_keys: u32, max_skew: *const u32,
+                                 min_domains: *const u32, existing_node_names: *const *const c_char,
+                                 existing_offset: *const u64, aff: *const ksh_pod_affinity,
+                                 scoring: *const ks_bind_scoring, policy: c_int, status: *mut i32, node_idx: *mut i32,
+                                 json: *mut c_char, cap: usize, json_off: *mut i64) -> c_int;
     pub fn ksh_drain_nodes(ctx: *mut ksh_context, node_names: *const *const c_char, n: u64, pods: *const ks_pod_obj,
                            pod_offset: *const u64, policy: c_int, flags: u32, placed: *mut u32, node_idx: *mut i32) -> c_int;
     pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,

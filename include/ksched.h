@@ -760,6 +760,81 @@ int ks_affinity_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const
                      int64_t* out_score /* [P] or NULL */, uint32_t* out_refused /* [2P] or NULL */,
                      uint32_t* out_domain_count /* [G * S] or NULL */);
 
+/* ---- soft constraints when binding: ks_affinity_bind scored as kube-scheduler's default profile scores, with
+ * PodTopologySpread's ScheduleAnyway constraints and InterPodAffinity's preferred terms (upstream scoring.go of both
+ * plugins, restated here; spec extension, DESIGN.md 5o) ----
+ * The arguments of ks_affinity_bind plus `scoring`.  The queue is bound exactly as ks_affinity_bind binds it - the same
+ * candidates (fit, selector, hard spread, rules 1-3), order, charge, refusals and hard counts - except for the score that
+ * picks among the candidates.  Term kinds 2 and 3 are preferred terms: they score and never filter.  term_weight[t] is
+ * the weight of term t, in [1, 100] for a preferred term and 0 for a required one (NULL = all 0).
+ * For pod p of group g at its turn: F = its candidates (ks_affinity_bind's rule 4); Sigma_g = the keys k with
+ * soft_skew[g * K + k] >= 1; sc_{g,k}[d] = a soft count per (group, key), starting at topo->existing (or 0).
+ * PodTopologySpread (soft).  Sigma_g empty (or g = -1): pts(n) = 0 for every n (upstream's Skip).  Otherwise:
+ *   - ignored: when soft_all_keys[g] = 1, a node of F that lacks some key of Sigma_g is ignored;
+ *   - size_k, k in Sigma_g: the number of distinct domains d_k(n) >= 0 over the non-ignored nodes of F, plus 1 when
+ *     soft_all_keys[g] = 0 and some node of F lacks k (upstream counts the empty label value as a domain);
+ *   - w_k = log((double)(size_k + 2)), by the C library's log, on the host, into a table indexed by size;
+ *   - raw(n), n not ignored: GoRound( sum over k in Sigma_g with d_k(n) >= 0, in ascending k, of
+ *     ((double)sc_{g,k}[d_k(n)] * w_k + (double)(soft_skew[g * K + k] - 1)) ), every IEEE operation rounded on its
+ *     own (no FMA contraction); GoRound rounds half away from zero;
+ *   - with min and max over the non-ignored nodes of F, max starting at 0: pts(n) = 0 for an ignored node, else 100
+ *     when max = 0, else 100 * (max + min - raw(n)) / max in int64;
+ *   - when the pod binds on n, sc_{g,k}[d_k(n)] rises by 1 for each k in Sigma_g with d_k(n) >= 0; when
+ *     soft_all_keys[g] = 1, only if n carries every key of Sigma_g.
+ * InterPodAffinity (preferred, and the existing pods' required affinity).  For each bound pod b of group h on node m and
+ * each key k with d_k(m) >= 0, every node of b's domain of key k gains:
+ *   - +w_t for each preferred affinity term of g on key k that targets h, -w_t for each preferred anti-affinity one;
+ *   - +hard_affinity_weight for each required affinity term of h on k that targets g, +w_t for each preferred affinity
+ *     term of h on k that targets g, -w_t for each preferred anti-affinity one.
+ *   Duplicate terms count twice; a term matches a pod once however often its target list names the pod's group.  A
+ *   self term (g targets g) counts twice against a bound pod of g: once as the incoming pod's term and once as the
+ *   bound pod's.  raw(n) = the sum over the keys n carries (int64, may be negative); with min and max over F,
+ *   ipa(n) = max > min ? (int64)(100.0 * ((double)(raw(n) - min) / (double)(max - min))) : 0.
+ * Total: score(n) = policy_score(n) + weight_spread * pts(n) + weight_affinity * ipa(n); the pod takes the highest
+ * total, ties to the lower node index.  Policies 1, 3 and 4 (upstream's 0-100 scales; 4 is the default profile's
+ * resource pair); LEFTOVER's scale would swamp every soft term.
+ * Outputs: out_node_idx, out_refused [2P], out_domain_count as ks_affinity_bind; out_score = the total;
+ * out_parts[3p .. 3p + 2] = the winner's policy score, pts and ipa (zeros for an unbound pod); out_soft_count = the
+ * final sc.  Each but out_node_idx may be NULL.
+ * Departures from upstream: ties go to the lowest index instead of at random; w_k comes from libm, not Go's math.Log;
+ * size_k is a distinct-domain count for every key, which is upstream's hostname special case whenever hostnames are
+ * unique; TaintToleration, NodeAffinity and ImageLocality are not modelled (constant for pods and nodes without taints
+ * or preferences, and the total omits those constants); nodeInclusionPolicies and matchLabelKeys are out of scope.
+ * Identities, policies 1, 3 and 4:
+ *   (J1) soft_skew NULL, no preferred term and hard_affinity_weight = 0 (or weight_spread = weight_affinity = 0): the
+ *        nodes, hard counts, free[] and both refusals are ks_affinity_bind's, out_score is its score and out_parts is
+ *        (score, 0, 0);
+ *   (J2) soft constraints and preferred terms only on keys where every node shares one domain: every node of F has
+ *        pts = 100 (0 if ignored) and ipa = 0; the nodes are ks_affinity_bind's, and each score is higher by exactly
+ *        100 * weight_spread when Sigma_g is non-empty;
+ *   (J3) for g != h, "g preferred-(anti-)affine to h on k, weight w" and "h preferred-(anti-)affine to g on k, weight
+ *        w" give the same result.
+ * Checked on the host before any device work and before free[] changes: every check of ks_affinity_bind, with kinds 0
+ * to 3; KS_ERR_INVALID for a NULL scoring, a preferred term whose weight is outside [1, 100], a required term with a
+ * non-zero weight, a plugin weight or hard_affinity_weight above 100, a soft_all_keys entry above 1, or a policy other
+ * than 1, 3 and 4; KS_ERR_RANGE for more than 2^26 IPA counter words or KS_AFFINITY_MAX_UPDATES IPA update entries.
+ * The terms compile into int64 counters I_{g,k} (D_k words) per (incoming group, key) with a non-zero coefficient, and
+ * per bound group h the entries (g, k, c) that a bind of a pod of h adds to I_{g,k}[d_k(n)], so a node's IPA raw is
+ * at most K counter loads.  Host-space arguments and outputs; one H2D copy; ks_affinity_bind's setup kernels and one
+ * that applies the existing pods' IPA entries; one cooperative launch with three or four grid barriers per pod; one
+ * D2H copy.  The bit-parallel index is marked stale. */
+#define KS_POD_AFFINITY_PREFERRED 2      /* scores only; never filters */
+#define KS_POD_ANTI_AFFINITY_PREFERRED 3
+typedef struct ks_bind_scoring {         /* host memory */
+    const uint32_t* soft_skew;           /* [G * K] or NULL: ScheduleAnyway maxSkew of group g on key k, 0 = none */
+    const uint8_t* soft_all_keys;        /* [G] or NULL (= all 1): 1 = explicit constraints, 0 = system-defaulted */
+    const uint32_t* term_weight;         /* [T] or NULL: weight in [1, 100] of each preferred term, 0 for required ones */
+    uint32_t hard_affinity_weight;       /* upstream hardPodAffinityWeight, [0, 100]; upstream default 1 */
+    uint32_t weight_spread;              /* PodTopologySpread plugin weight, [0, 100]; default profile 2 */
+    uint32_t weight_affinity;            /* InterPodAffinity plugin weight, [0, 100]; default profile 2 */
+} ks_bind_scoring;
+int ks_profile_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const int32_t* group /* [P] */,
+                    uint32_t n_groups, const ks_spread_multi* topo /* keys; max_skew may be NULL */,
+                    const ks_pod_affinity* aff /* or NULL */, const ks_bind_scoring* scoring, int policy,
+                    int32_t* out_node_idx /* [P] */, int64_t* out_score /* [P] or NULL */,
+                    int64_t* out_parts /* [3P] or NULL */, uint32_t* out_refused /* [2P] or NULL */,
+                    uint32_t* out_domain_count /* [G * S] or NULL */, uint32_t* out_soft_count /* [G * S] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -308,6 +308,19 @@ int ksh_reconcile_affinity(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_
                            const ksh_pod_affinity* aff, int policy, int32_t* out_status, int32_t* out_node_idx,
                            char* json, size_t cap, int64_t* out_json_off);
 
+/* reconcile() under topology spread, required inter-pod affinity and the default profile's soft scores
+ * (ks_profile_bind, ksched.h): ksh_reconcile_affinity with term kinds 0 to 3 (KS_POD_AFFINITY_PREFERRED /
+ * KS_POD_ANTI_AFFINITY_PREFERRED score only) and a scoring struct (required; its term_weight is indexed as aff's terms,
+ * its soft_skew and soft_all_keys by group and topology_keys).  The soft counts start from the same existing counts as
+ * the hard ones.  Soft terms never make a pod unschedulable, so the status mapping is ksh_reconcile_affinity's.  Errors
+ * as ksh_reconcile_affinity and ks_profile_bind; KS_ERR_INVALID for a NULL scoring. */
+int ksh_reconcile_profile(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, const int32_t* group,
+                          uint32_t n_groups, const char* const* topology_keys, uint32_t n_keys,
+                          const uint32_t* max_skew /* or NULL */, const uint32_t* min_domains,
+                          const char* const* existing_node_names, const uint64_t* existing_offset,
+                          const ksh_pod_affinity* aff /* or NULL */, const ks_bind_scoring* scoring, int policy,
+                          int32_t* out_status, int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off);
+
 #ifdef __cplusplus
 }
 #endif

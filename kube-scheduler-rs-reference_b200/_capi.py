@@ -233,6 +233,17 @@ _proto("ks_affinity_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, 
        C.POINTER(ks_spread_multi), C.POINTER(ks_pod_affinity), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
        C.c_void_p, optional=True)
 KS_POD_AFFINITY, KS_POD_ANTI_AFFINITY = 0, 1
+KS_POD_AFFINITY_PREFERRED, KS_POD_ANTI_AFFINITY_PREFERRED = 2, 3
+
+
+class ks_bind_scoring(C.Structure):
+    _fields_ = [("soft_skew", C.c_void_p), ("soft_all_keys", C.c_void_p), ("term_weight", C.c_void_p),
+                ("hard_affinity_weight", C.c_uint32), ("weight_spread", C.c_uint32), ("weight_affinity", C.c_uint32)]
+
+
+_proto("ks_profile_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_uint32,
+       C.POINTER(ks_spread_multi), C.POINTER(ks_pod_affinity), C.POINTER(ks_bind_scoring), C.c_int, C.c_void_p,
+       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
 KS_AFFINITY_MAX_TERMS = 16384
 KS_AFFINITY_MAX_TARGETS = 1 << 22
 KS_AFFINITY_MAX_EXISTING = 1 << 24

@@ -35,6 +35,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 #pragma weak ks_place_replicas_spread_multi
 #pragma weak ks_spread_bind
 #pragma weak ks_affinity_bind
+#pragma weak ks_profile_bind
 
 namespace {
 
@@ -1714,12 +1715,14 @@ KSH_CATCH
 // reconcile() under topology spread: ksh_reconcile_batch's filtering, then ks_spread_bind over the pods that go to the
 // device, each in its group.  Group g's existing pods under key k count when their node is in the store and carries key k
 // and every key g constrains.  With aff set (ksh_reconcile_affinity), ks_affinity_bind with its terms and the existing
-// pods whose node is in the store; max_skew may then be NULL.
+// pods whose node is in the store; max_skew may then be NULL.  With aff and sc set (ksh_reconcile_profile),
+// ks_profile_bind with the same terms and the soft terms of sc; the soft counts start from the same existing counts.
 static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
                             const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
                             const uint32_t* min_domains, const char* const* existing_node_names,
                             const uint64_t* existing_offset, const ksh_pod_affinity* aff, int policy, int32_t* out_status,
-                            int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off) {
+                            int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off,
+                            const ks_bind_scoring* sc = nullptr) {
     if (!c || !topology_keys || (n && (!pods || !group || !out_status || !out_node_idx)) || (n_groups && !max_skew && !aff))
         return fail(KS_ERR_INVALID, "NULL argument");
     if (K == 0 || K > KS_SPREAD_MAX_KEYS)
@@ -1737,7 +1740,9 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     if (aff && aff->n_existing && (!aff->existing_group || !aff->existing_node_name))
         return fail(KS_ERR_INVALID, "NULL existing_group or existing_node_name");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    int rc = aff ? device_ready(c, ks_affinity_bind, "ks_affinity_bind") : device_ready(c, ks_spread_bind, "ks_spread_bind");
+    int rc = sc    ? device_ready(c, ks_profile_bind, "ks_profile_bind")
+             : aff ? device_ready(c, ks_affinity_bind, "ks_affinity_bind")
+                   : device_ready(c, ks_spread_bind, "ks_spread_bind");
     if (rc) return rc;
     std::vector<uint64_t> todo;
     std::vector<ks_pod_obj> sub; // the pods that go to the device, in arrival order, and their groups
@@ -1801,8 +1806,10 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
         pa.n_existing = eg.size();
         pa.existing_group = eg.data();
         pa.existing_node = en.data();
-        rc = ks_affinity_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, policy, idx.data(), nullptr,
-                              refused.data(), nullptr);
+        rc = sc ? ks_profile_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, policy, idx.data(), nullptr,
+                                  nullptr, refused.data(), nullptr, nullptr)
+                : ks_affinity_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, policy, idx.data(), nullptr,
+                                   refused.data(), nullptr);
     } else {
         rc = ks_spread_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, policy, idx.data(), nullptr, refused.data(),
                             nullptr); // commits capacity on the device
@@ -1844,6 +1851,20 @@ int ksh_reconcile_affinity(ksh_context* c, const ks_pod_obj* pods, uint64_t n, c
     return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
                             existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
                             out_json_off);
+}
+KSH_CATCH
+
+int ksh_reconcile_profile(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
+                          const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
+                          const uint32_t* min_domains, const char* const* existing_node_names,
+                          const uint64_t* existing_offset, const ksh_pod_affinity* aff, const ks_bind_scoring* scoring,
+                          int policy, int32_t* out_status, int32_t* out_node_idx, char* json, size_t cap,
+                          int64_t* out_json_off) try {
+    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
+    const ksh_pod_affinity none{};
+    return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
+                            existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
+                            out_json_off, scoring);
 }
 KSH_CATCH
 

@@ -195,7 +195,7 @@ class HostStaged {
             if (c.block == OUT && block == OUT) memcpy(c.p, at<unsigned char>(host_[OUT], c.off), c.bytes);
         }
     }
-    static constexpr int MAX_COPIES = 16;
+    static constexpr int MAX_COPIES = 24;
     BlockLayout layout_[3];
     void* dev_[3] = {};
     void* host_[2] = {};
@@ -1792,7 +1792,8 @@ int ks_place_replicas_spread_multi(ks_snapshot* s, const ks_pods* specs, const u
 }
 
 // ks_affinity_bind's terms compiled on the host (include/ksched.h, DESIGN.md 5n): the counter bases per (group, key),
-// the first-pod flag per group and each group's deduplicated update entries.
+// the first-pod flag per group and each group's deduplicated update entries.  With ks_profile_bind's scoring (5o), also
+// the InterPodAffinity counters I_{g,k} and per bound group h the entries (g, k, c_{g,k}(h)) with c != 0.
 struct AffinityPlan {
     std::vector<uint32_t> abase;   // [G * K * 2]: B_{g,k}, A_{g,k} bases, AFF_NONE = none
     std::vector<uint32_t> aflag;   // [G]
@@ -1800,10 +1801,72 @@ struct AffinityPlan {
     std::vector<uint32_t> upd;     // h | k << 16 | kind << 20
     uint64_t words = 0;            // counter words, the G first-pod words included
     uint32_t any_base = 0;
+    std::vector<uint32_t> ibase;    // [G * K]: base of I_{g,k} (int64 words), AFF_NONE = none
+    std::vector<uint32_t> iupd_off; // [G + 1]
+    std::vector<uint32_t> iupd;     // g | k << 16
+    std::vector<int32_t> icoef;     // c_{g,k}(h)
+    uint64_t iwords = 0;
 };
 
+// c_{g,k}(h) of every (bound group h, incoming group g, key k), summed over the terms (include/ksched.h, 5o)
+static int compile_scoring(const ks_pod_affinity* f, const ks_bind_scoring* sc, uint32_t G, uint32_t K,
+                           const uint32_t* Dk, AffinityPlan* pl) {
+    std::vector<std::pair<uint64_t, int64_t>> c; // (h << 32 | g << 4 | k, coefficient)
+    std::vector<int32_t> tg;
+    auto add = [&](uint32_t h, uint32_t g, uint32_t k, int64_t v) { c.emplace_back((uint64_t)h << 32 | g << 4 | k, v); };
+    for (uint32_t t = 0; t < f->n_terms; t++) {
+        const uint32_t o = (uint32_t)f->owner[t], k = f->key[t], kind = f->kind[t];
+        const int64_t w = sc->term_weight ? sc->term_weight[t] : 0;
+        if (kind == KS_POD_ANTI_AFFINITY || (kind == KS_POD_AFFINITY && sc->hard_affinity_weight == 0)) continue;
+        tg.assign(f->target + f->target_offset[t], f->target + f->target_offset[t + 1]); // a term matches a pod once
+        std::sort(tg.begin(), tg.end());
+        tg.erase(std::unique(tg.begin(), tg.end()), tg.end());
+        for (const int32_t h : tg) {
+            if (kind == KS_POD_AFFINITY) { // an existing pod's required affinity term that matches the incoming pod
+                add(o, (uint32_t)h, k, sc->hard_affinity_weight);
+                continue;
+            }
+            const int64_t v = kind == KS_POD_AFFINITY_PREFERRED ? w : -w;
+            add((uint32_t)h, o, k, v); // the incoming pod's term, against a bound pod of h
+            add(o, (uint32_t)h, k, v); // the bound pod's term, against an incoming pod of h
+        }
+    }
+    std::sort(c.begin(), c.end());
+    std::vector<std::pair<uint64_t, int64_t>> m;
+    for (const auto& e : c) {
+        if (!m.empty() && m.back().first == e.first) m.back().second += e.second;
+        else m.push_back(e);
+    }
+    m.erase(std::remove_if(m.begin(), m.end(), [](const auto& e) { return e.second == 0; }), m.end());
+    if (m.size() > KS_AFFINITY_MAX_UPDATES)
+        return fail(KS_ERR_RANGE, "%llu scoring update entries (at most 2^24)", (unsigned long long)m.size());
+    pl->ibase.assign((size_t)G * K, AFF_NONE);
+    pl->iupd_off.assign(G + 1, 0);
+    pl->iupd.reserve(m.size());
+    pl->icoef.reserve(m.size());
+    for (const auto& e : m) {
+        const uint32_t h = (uint32_t)(e.first >> 32), g = (uint32_t)(e.first >> 4 & 0xfffffffu), k = e.first & 15u;
+        pl->iupd_off[h + 1]++;
+        pl->iupd.push_back(g | k << 16);
+        pl->icoef.push_back((int32_t)e.second); // |c| <= 2 * 100 * KS_AFFINITY_MAX_TERMS
+        pl->ibase[(size_t)g * K + k] = 0;
+    }
+    for (uint32_t h = 0; h < G; h++) pl->iupd_off[h + 1] += pl->iupd_off[h];
+    uint64_t word = 0;
+    for (uint32_t g = 0; g < G; g++)
+        for (uint32_t k = 0; k < K; k++)
+            if (pl->ibase[(size_t)g * K + k] != AFF_NONE) {
+                pl->ibase[(size_t)g * K + k] = (uint32_t)word;
+                word += Dk[k];
+                if (word > KS_SPREAD_MAX_COUNTS)
+                    return fail(KS_ERR_RANGE, "more than 2^26 scoring counter words (group %u, key %u)", g, k);
+            }
+    pl->iwords = word;
+    return KS_OK;
+}
+
 static int compile_affinity(const ks_pod_affinity* f, uint32_t G, uint32_t K, const uint32_t* Dk, uint32_t N,
-                            AffinityPlan* pl) {
+                            AffinityPlan* pl, const ks_bind_scoring* sc = nullptr) {
     const uint32_t T = f->n_terms;
     const uint64_t E = f->n_existing;
     if (T > KS_AFFINITY_MAX_TERMS) return fail(KS_ERR_RANGE, "%u affinity terms (at most %u)", T, KS_AFFINITY_MAX_TERMS);
@@ -1815,7 +1878,14 @@ static int compile_affinity(const ks_pod_affinity* f, uint32_t G, uint32_t K, co
     for (uint32_t t = 0; t < T; t++) {
         if (f->owner[t] < 0 || f->owner[t] >= (int64_t)G)
             return fail(KS_ERR_INVALID, "term %u: owner %d outside [0, %u)", t, f->owner[t], G);
-        if (f->kind[t] > KS_POD_ANTI_AFFINITY) return fail(KS_ERR_INVALID, "term %u: kind %u (0 or 1)", t, f->kind[t]);
+        if (!sc && f->kind[t] > KS_POD_ANTI_AFFINITY) return fail(KS_ERR_INVALID, "term %u: kind %u (0 or 1)", t, f->kind[t]);
+        if (sc && f->kind[t] > KS_POD_ANTI_AFFINITY_PREFERRED)
+            return fail(KS_ERR_INVALID, "term %u: kind %u (0 to 3)", t, f->kind[t]);
+        const uint32_t w = sc && sc->term_weight ? sc->term_weight[t] : 0;
+        if (sc && f->kind[t] >= KS_POD_AFFINITY_PREFERRED && (w < 1 || w > 100))
+            return fail(KS_ERR_INVALID, "term %u: preferred term weight %u (1 to 100)", t, w);
+        if (sc && f->kind[t] <= KS_POD_ANTI_AFFINITY && w)
+            return fail(KS_ERR_INVALID, "term %u: required term weight %u (0)", t, w);
         if (f->key[t] >= K) return fail(KS_ERR_INVALID, "term %u: key %u (the call has %u)", t, f->key[t], K);
         if (f->target_offset[t + 1] < f->target_offset[t]) return fail(KS_ERR_INVALID, "term %u: target offsets decrease", t);
     }
@@ -1842,6 +1912,7 @@ static int compile_affinity(const ks_pod_affinity* f, uint32_t G, uint32_t K, co
     auto enc = [](uint32_t g, uint32_t k, uint32_t kind) { return g | k << 16 | kind << 20; };
     for (uint32_t t = 0; t < T; t++) {
         const uint32_t g = (uint32_t)f->owner[t], k = f->key[t];
+        if (f->kind[t] > KS_POD_ANTI_AFFINITY) continue; // preferred terms score only
         if (f->kind[t] == KS_POD_ANTI_AFFINITY) {
             anti[(size_t)g * K + k] = 1;
             for (uint64_t i = f->target_offset[t]; i < f->target_offset[t + 1]; i++) {
@@ -1899,17 +1970,31 @@ static int compile_affinity(const ks_pod_affinity* f, uint32_t G, uint32_t K, co
     pl->words = word + G;
     if (pl->words > KS_SPREAD_MAX_COUNTS)
         return fail(KS_ERR_RANGE, "%llu affinity counter words (at most 2^26)", (unsigned long long)pl->words);
-    return KS_OK;
+    return sc ? compile_scoring(f, sc, G, K, Dk, pl) : KS_OK;
 }
 
-// ks_spread_bind, and with aff set ks_affinity_bind (then max_skew may be NULL and out_refused holds 2P words)
+// ks_spread_bind, and with aff set ks_affinity_bind (then max_skew may be NULL and out_refused holds 2P words), and with
+// aff and sc set ks_profile_bind (out_parts [3P] and out_soft_count [G * S] may be given)
 static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
                        const ks_spread_multi* spread, const ks_pod_affinity* aff, int policy, int32_t* out_node_idx,
-                       int64_t* out_score, uint32_t* out_refused, uint32_t* out_domain_count) {
+                       int64_t* out_score, uint32_t* out_refused, uint32_t* out_domain_count,
+                       const ks_bind_scoring* sc = nullptr, int64_t* out_parts = nullptr,
+                       uint32_t* out_soft_count = nullptr) {
     int rc = check_pods(s, pods);
     if (rc) return rc;
     if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "%s takes host-space pods", call);
     if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    if (sc) {
+        if (policy != KS_SCORE_LEAST_ALLOCATED && policy != KS_SCORE_MOST_ALLOCATED && policy != KS_SCORE_LEAST_BALANCED)
+            return fail(KS_ERR_INVALID, "%s takes policies 1, 3 and 4 (got %d)", call, policy);
+        if (sc->hard_affinity_weight > 100 || sc->weight_spread > 100 || sc->weight_affinity > 100)
+            return fail(KS_ERR_INVALID, "plugin weights %u, %u and hard affinity weight %u (at most 100)",
+                        sc->weight_spread, sc->weight_affinity, sc->hard_affinity_weight);
+        if (sc->soft_all_keys)
+            for (uint32_t g = 0; g < n_groups; g++)
+                if (sc->soft_all_keys[g] > 1)
+                    return fail(KS_ERR_INVALID, "group %u: soft_all_keys %u (0 or 1)", g, sc->soft_all_keys[g]);
+    }
     const uint64_t P = pods->n, G = n_groups;
     if (P && (!group || !out_node_idx)) return fail(KS_ERR_INVALID, "NULL group or out_node_idx");
     if (!spread || (G && !spread->max_skew && !aff)) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
@@ -1952,7 +2037,7 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     AffinityPlan plan;
     if (aff) {
         try {
-            rc = compile_affinity(aff, (uint32_t)G, K, spread->n_domains, N, &plan);
+            rc = compile_affinity(aff, (uint32_t)G, K, spread->n_domains, N, &plan, sc);
         } catch (...) {
             return fail(KS_ERR_NOMEM, "out of host memory in %s", call);
         }
@@ -1964,10 +2049,12 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         memset(out_node_idx, 0xff, P * 4);
         if (out_score) memset(out_score, 0, P * 8);
         if (out_refused) memset(out_refused, 0, P * R * 4);
-        if (out_domain_count) {
-            if (spread->existing) memcpy(out_domain_count, spread->existing, GS * 4);
-            else memset(out_domain_count, 0, GS * 4);
-        }
+        for (uint32_t* c : {out_domain_count, out_soft_count})
+            if (c) {
+                if (spread->existing) memcpy(c, spread->existing, GS * 4);
+                else memset(c, 0, GS * 4);
+            }
+        if (out_parts) memset(out_parts, 0, P * 24);
         return KS_OK;
     }
     std::lock_guard<std::mutex> lk(s->mu);
@@ -2003,12 +2090,58 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     const auto pkey = h.work<int64_t>(a.grid);
     const auto pidx = h.work<int32_t>(a.grid);
     const auto pref = h.work<uint32_t>(a.grid);
-    CU_TRY(h.reserve(s));
-    for (uint32_t k = 0; k < K; k++) memcpy(h.host(dom) + (size_t)k * N, spread->node_domain[k], (size_t)N * 4);
-    if (!spread->max_skew) memset(h.host(max_skew), 0, G * K * 4);
+    // ks_profile_bind: the soft terms, the log table and the compiled IPA entries; the domain bitmaps of the keys with
+    // more than one node in some domain, per parity
+    ProfileBindArgs q{};
+    const uint64_t Q = sc ? 1 : 0;
+    if (sc) {
+        std::vector<uint8_t> seen;
+        for (uint32_t k = 0; k < K; k++) {
+            try {
+                seen.assign(spread->n_domains[k], 0);
+            } catch (...) {
+                return fail(KS_ERR_NOMEM, "out of host memory in %s", call);
+            }
+            bool uniq = true;
+            for (uint32_t n = 0; n < N && uniq; n++) {
+                const int32_t d = spread->node_domain[k][n];
+                if (d >= 0) uniq = !seen[d]++;
+            }
+            q.bwo[k] = q.BW;
+            if (uniq) q.uniq |= 1u << k;
+            else q.BW += (spread->n_domains[k] + 31) / 32;
+        }
+    }
+    const auto soft_skew = h.in(sc ? sc->soft_skew : nullptr, Q * G * K); // NULL: zeros, filled below
+    const auto soft_all = h.in(sc ? sc->soft_all_keys : nullptr, Q * G);  // NULL: ones, filled below
+    const auto logw = h.in<double>(nullptr, Q * (N + 2ull));
+    const auto ibase = h.in<uint32_t>(nullptr, plan.ibase.size());
+    const auto iupd_off = h.in<uint32_t>(nullptr, plan.iupd_off.size());
+    const auto iupd = h.in<uint32_t>(nullptr, plan.iupd.size());
+    const auto icoef = h.in<int32_t>(nullptr, plan.icoef.size());
+    const auto parts = h.out(out_parts, Q * 3 * P);
+    const auto scnt = h.out(out_soft_count, Q * GS);
+    const auto icnt = h.work<int64_t>(plan.iwords, 16);
+    const auto bits = h.work<uint32_t>(2ull * q.BW, 16);
+    const auto iraw = h.work<int64_t>(Q * N), praw = h.work<int64_t>(Q * N);
+    const auto pdom = h.work<uint32_t>(Q * a.grid * KS_SPREAD_MAX_KEYS), plack = h.work<uint32_t>(Q * a.grid);
+    const auto pimin = h.work<int64_t>(Q * a.grid), pimax = h.work<int64_t>(Q * a.grid);
+    const auto ppmin = h.work<int64_t>(Q * a.grid), ppmax = h.work<int64_t>(Q * a.grid);
     auto put = [&](Staged<uint32_t> d, const std::vector<uint32_t>& v) {
         if (!v.empty()) memcpy(h.host(d), v.data(), v.size() * 4);
     };
+    CU_TRY(h.reserve(s));
+    if (sc) {
+        if (!sc->soft_skew) memset(h.host(soft_skew), 0, G * K * 4);
+        if (!sc->soft_all_keys) memset(h.host(soft_all), 1, G);
+        for (uint64_t i = 0; i < N + 2ull; i++) h.host(logw)[i] = log((double)(i + 2)); // the oracle's libm
+        put(ibase, plan.ibase);
+        put(iupd_off, plan.iupd_off);
+        put(iupd, plan.iupd);
+        if (!plan.icoef.empty()) memcpy(h.host(icoef), plan.icoef.data(), plan.icoef.size() * 4);
+    }
+    for (uint32_t k = 0; k < K; k++) memcpy(h.host(dom) + (size_t)k * N, spread->node_domain[k], (size_t)N * 4);
+    if (!spread->max_skew) memset(h.host(max_skew), 0, G * K * 4);
     put(abase, plan.abase);
     put(aflag, plan.aflag);
     put(upd_off, plan.upd_off);
@@ -2067,13 +2200,41 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         a.acnt = h.dev(acnt);
         a.paref = h.dev(paref);
     }
+    if (sc) {
+        q.b = a;
+        q.soft_skew = h.dev(soft_skew);
+        q.soft_all = h.dev(soft_all);
+        q.logw = h.dev(logw);
+        q.bits = h.dev(bits);
+        q.scnt = h.dev(scnt);
+        q.ibase = h.dev(ibase);
+        q.iupd_off = h.dev(iupd_off);
+        q.iupd = h.dev(iupd);
+        q.icoef = h.dev(icoef);
+        q.icnt = h.dev(icnt);
+        q.iwords = plan.iwords;
+        q.iraw = h.dev(iraw);
+        q.praw = h.dev(praw);
+        q.pdom = h.dev(pdom);
+        q.plack = h.dev(plack);
+        q.pimin = h.dev(pimin);
+        q.pimax = h.dev(pimax);
+        q.ppmin = h.dev(ppmin);
+        q.ppmax = h.dev(ppmax);
+        q.out_parts = h.dev(parts);
+        q.wspread = sc->weight_spread;
+        q.waff = sc->weight_affinity;
+    }
     s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
     s->version++;
-    cudaError_t e = aff ? launch_affinity_bind(a, plan.words, W, st) : launch_spread_bind(a, W, st);
+    cudaError_t e = sc    ? launch_profile_bind(q, plan.words, W, st)
+                    : aff ? launch_affinity_bind(a, plan.words, W, st)
+                          : launch_spread_bind(a, W, st);
     if (e != cudaSuccess)
-        return fail(KS_ERR_CUDA, "%s launch failed: %s", aff ? "affinity bind" : "spread bind", cudaGetErrorString(e));
+        return fail(KS_ERR_CUDA, "%s launch failed: %s", sc ? "profile bind" : aff ? "affinity bind" : "spread bind",
+                    cudaGetErrorString(e));
     CU_TRY(h.finish(st));
-    s->last_path = aff ? "affinity_bind" : "spread_bind";
+    s->last_path = sc ? "profile_bind" : aff ? "affinity_bind" : "spread_bind";
     return KS_OK;
 }
 
@@ -2090,6 +2251,16 @@ int ks_affinity_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, 
     const ks_pod_affinity none{};
     return bind_spread(s, "ks_affinity_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
                        out_score, out_refused, out_domain_count);
+}
+
+int ks_profile_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
+                    const ks_spread_multi* topo, const ks_pod_affinity* aff, const ks_bind_scoring* scoring, int policy,
+                    int32_t* out_node_idx, int64_t* out_score, int64_t* out_parts, uint32_t* out_refused,
+                    uint32_t* out_domain_count, uint32_t* out_soft_count) {
+    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
+    const ks_pod_affinity none{};
+    return bind_spread(s, "ks_profile_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
+                       out_score, out_refused, out_domain_count, scoring, out_parts, out_soft_count);
 }
 
 // ---------------------------------------------------------------------------------------------- async streaming

@@ -274,4 +274,36 @@ constexpr uint32_t AFF_NONE = 0xffffffffu, AFF_SELF = 1u;
 // ks_affinity_bind (ks_spread_bind.cu): k_spread_bind_setup when G > 0, the counters zeroed, k_affinity_setup over the
 // existing pods (aff_grid CTAs, when E > 0), then one cooperative launch of grid CTAs, k_affinity_bind_seq
 cudaError_t launch_affinity_bind(const SpreadBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st);
+
+// ks_profile_bind (ks_spread_bind.cu): ks_affinity_bind's state in b, plus the soft terms (DESIGN.md 5o).  The soft
+// counts scnt start at existing (or 0), the IPA counters I_{g,k} (int64, D_k words each at ibase[g * K + k] in icnt) at
+// 0 before the existing pods' entries.  Update entry of group h: g | k << 16 with coefficient icoef, added to
+// I_{g,k}[d_k(n)] when a pod of h binds on n.  Per node of the slice, pass 1 leaves iraw[n] = its IPA raw, or
+// PB_NOT_CAND when n is not a candidate, and pass 2 praw[n] = its PodTopologySpread raw, or -1 when it is ignored.
+constexpr uint32_t PB_SH_WORDS = 64; // domains below 64 * 32 of each key are marked in a per-CTA bitmap first
+struct ProfileBindArgs {
+    SpreadBindArgs b;
+    const uint32_t* soft_skew;        // [G * K], 0 = no soft constraint on the key
+    const uint8_t* soft_all;          // [G]
+    const double* logw;               // [N + 2]: log(size + 2)
+    uint32_t uniq;                    // bit k: key k has at most one node per domain (size_k counts nodes)
+    uint32_t bwo[KS_SPREAD_MAX_KEYS]; // word offset of key k in each parity's domain bitmap
+    uint32_t BW;                      // words per parity
+    uint32_t* bits;                   // [2 * BW], zeroed by the launcher; pod p marks parity p & 1
+    uint32_t* scnt;                   // [G * S] soft counts, final after the call
+    const uint32_t* ibase;            // [G * K], AFF_NONE = no IPA counters
+    const uint32_t* iupd_off;         // [G + 1]
+    const uint32_t* iupd;
+    const int32_t* icoef;
+    int64_t* icnt;                    // IPA counters, zeroed by the launcher
+    uint64_t iwords;
+    int64_t *iraw, *praw;             // [N]
+    uint32_t* pdom;                   // [grid * KS_SPREAD_MAX_KEYS] per-CTA partials: new domains per soft key
+    uint32_t* plack;                  // [grid]: soft keys some non-ignored candidate lacks
+    int64_t *pimin, *pimax, *ppmin, *ppmax; // [grid]: IPA raw and PodTopologySpread raw extremes
+    int64_t* out_parts;               // [3P]
+    uint32_t wspread, waff;
+};
+constexpr int64_t PB_NOT_CAND = INT64_MIN;
+cudaError_t launch_profile_bind(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st);
 } // namespace ks

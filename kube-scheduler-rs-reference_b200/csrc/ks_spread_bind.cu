@@ -12,6 +12,8 @@
 // k_affinity_bind_seq, the same walk with the phase helpers' AFF instances: phase A also applies rules 1-3 of the header
 // through at most 2K counter loads per node, phase B also applies the bound pod's update entries across CTA 0.  The
 // AFF = false instances are the code k_spread_bind_seq always ran.
+// ks_profile_bind (DESIGN.md 5o) runs k_profile_bind_seq: the same filter and commit, with soft PodTopologySpread and
+// InterPodAffinity scores that need grid-wide reductions over the candidates before any node's total exists.
 #include "ks_internal.cuh"
 #include "ks_launch.h"
 
@@ -146,6 +148,7 @@ __device__ __forceinline__ void affinity_raise(const SpreadBindArgs& a, uint32_t
     if (kind) a.acnt[a.any_base + h] = 1; // a pod of M_h sits on a node that carries one of h's affinity keys
 }
 
+// ProfileFilter (ks_profile_bind, below) repeats this filter rule for rule: a change here goes there too.
 // Phase A of pod p in this CTA's slice [n0, n1): fit, selector and, for a constrained pod, cnt < m + max_skew on every
 // constrained key; the best candidate by the policy's key (ties to the lower node) and the refused count into the CTA's
 // partial.  AFF: then rules 1-3 of ks_affinity_bind against the pod's group's counter bases, formed once per pod; the
@@ -405,6 +408,470 @@ cudaError_t launch_affinity_bind(const SpreadBindArgs& a, uint64_t acnt_words, u
         SpreadBindArgs b = a;
         void* args[] = {&b};
         e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(k_affinity_bind_seq<LW>), dim3(a.grid),
+                                        dim3(SBD_THREADS), args, 0, st);
+        if (e == cudaSuccess) g_launches++;
+        return e;
+    });
+}
+
+
+// ---- ks_profile_bind ----
+// Its candidate filter is spread_bind_scan's rule for rule, with the AFF rules; spread_bind_scan keeps its own copy so
+// that the code of k_spread_bind_seq and k_affinity_bind_seq stays as it was.
+template <int W>
+struct ProfileFilter {
+    int32_t g;
+    int64_t rc, rm;
+    uint64_t sw[W];
+    uint32_t ck;
+    uint64_t lim[KS_SPREAD_MAX_KEYS];
+    const uint32_t* cnt;
+    uint32_t bB[KS_SPREAD_MAX_KEYS], bA[KS_SPREAD_MAX_KEYS];
+    bool first;
+
+    __device__ __forceinline__ ProfileFilter(const SpreadBindArgs& a, uint32_t p) {
+        g = __ldg(a.group + p);
+        rc = __ldg(a.req_cpu + p);
+        rm = __ldg(a.req_mem + p);
+#pragma unroll
+        for (int w = 0; w < W; w++) sw[w] = __ldg(a.sel + (size_t)p * W + w);
+        ck = constrained_keys(a, g);
+#pragma unroll
+        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) {
+            lim[k] = (ck >> k & 1u) ? (uint64_t)__ldcg(a.gk + ((size_t)g * a.K + k) * GK_WORDS + GK_M) +
+                                          __ldg(a.max_skew + (size_t)g * a.K + k)
+                                    : 0;
+            const bool on = g >= 0 && k < a.K;
+            bB[k] = on ? __ldg(a.abase + ((size_t)g * a.K + k) * 2) : AFF_NONE;
+            bA[k] = on ? __ldg(a.abase + ((size_t)g * a.K + k) * 2 + 1) : AFF_NONE;
+        }
+        cnt = a.cnt + (size_t)(g < 0 ? 0 : g) * a.S;
+        first = g >= 0 && (__ldg(a.aflag + g) & AFF_SELF) && __ldcg(a.acnt + a.any_base + g) == 0;
+    }
+    // 0: unfit (fit or selector), 1: refused by spread, 2: refused by rules 1-3, 3: candidate
+    __device__ __forceinline__ int test(const SpreadBindArgs& a, uint32_t n, int64_t fc, int64_t fm) const {
+        uint64_t miss = 0;
+#pragma unroll
+        for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
+        if (!(rc <= fc && rm <= fm && miss == 0)) return 0;
+        bool ok = true;
+#pragma unroll
+        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
+            if (ck >> k & 1u) {
+                const int32_t d = __ldg(a.dom + (size_t)k * a.N + n);
+                ok &= d >= 0 && __ldcg(cnt + a.Pk[k] + (uint32_t)max(d, 0)) < lim[k];
+            }
+        if (!ok) return 1;
+        bool aok = true;
+#pragma unroll
+        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
+            if ((bB[k] & bA[k]) != AFF_NONE) {
+                const int32_t d = __ldg(a.dom + (size_t)k * a.N + n);
+                const uint32_t dd = (uint32_t)max(d, 0);
+                if (bB[k] != AFF_NONE) aok &= d < 0 || __ldcg(a.acnt + bB[k] + dd) == 0;
+                if (bA[k] != AFF_NONE) aok &= d >= 0 && (first || __ldcg(a.acnt + bA[k] + dd) > 0);
+            }
+        return aok ? 3 : 2;
+    }
+};
+
+// CTA-wide minimum and maximum of one int64 pair per thread; every thread gets the result.  s holds 2 * SBD_WARPS words.
+__device__ __forceinline__ void cta_minmax(int64_t& mn, int64_t& mx, int64_t* s) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        mn = min(mn, (int64_t)__shfl_xor_sync(0xffffffffu, (long long)mn, off));
+        mx = max(mx, (int64_t)__shfl_xor_sync(0xffffffffu, (long long)mx, off));
+    }
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) {
+        s[threadIdx.x >> 5] = mn;
+        s[SBD_WARPS + (threadIdx.x >> 5)] = mx;
+    }
+    __syncthreads();
+#pragma unroll
+    for (uint32_t w = 0; w < SBD_WARPS; w++) {
+        mn = min(mn, s[w]);
+        mx = max(mx, s[SBD_WARPS + w]);
+    }
+}
+
+// The pod's soft keys: bit k when soft_skew[g * K + k] >= 1
+__device__ __forceinline__ uint32_t soft_keys(const ProfileBindArgs& a, int32_t g) {
+    uint32_t sk = 0;
+    if (g >= 0)
+        for (uint32_t k = 0; k < a.b.K; k++)
+            if (__ldg(a.soft_skew + (size_t)g * a.b.K + k)) sk |= 1u << k;
+    return sk;
+}
+
+// ignored (header, PodTopologySpread): the group has explicit constraints and n lacks one of its soft keys
+__device__ __forceinline__ bool pts_ignored(const ProfileBindArgs& a, uint32_t sk, bool all, uint32_t n) {
+    if (!all) return false;
+    bool lacks = false;
+#pragma unroll
+    for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
+        if (sk >> k & 1u) lacks |= __ldg(a.b.dom + (size_t)k * a.b.N + n) < 0;
+    return lacks;
+}
+
+// The shared state of one CTA for one pod: the merged extremes, the soft weights and the domain marks
+struct ProfileShared {
+    int64_t key[SBD_WARPS];
+    int32_t idx[SBD_WARPS];
+    uint32_t ref[SBD_WARPS], aref[SBD_WARPS];
+    int64_t mm[2 * SBD_WARPS];
+    uint32_t bits[KS_SPREAD_MAX_KEYS * PB_SH_WORDS];
+    uint32_t dom[KS_SPREAD_MAX_KEYS], lack;
+    double w[KS_SPREAD_MAX_KEYS];
+    int64_t imin, imax, pmin, pmax;
+    uint32_t rescan;
+    int32_t bidx;
+};
+
+// Pass 1: the filter; per candidate its IPA raw into iraw[], and for a group with soft keys the domains of the
+// non-ignored candidates: a node-per-domain key counts its nodes, a domain below PB_SH_WORDS * 32 is marked in the CTA's
+// bitmap and merged into the parity's global bitmap once per CTA, a higher one is marked there directly.  Each new
+// bit counts one domain, so the partials add up to the distinct domains.  The other parity's bitmap is cleared.
+template <int W>
+__device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t p, uint32_t n0, uint32_t n1,
+                                              ProfileShared& sh) {
+    const SpreadBindArgs& b = a.b;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const ProfileFilter<W> f(b, p);
+    const uint32_t sk = soft_keys(a, f.g);
+    const bool all = f.g >= 0 && __ldg(a.soft_all + f.g);
+    uint32_t* bits = a.bits + (size_t)(p & 1u) * a.BW;
+    {
+        uint32_t* other = a.bits + (size_t)(~p & 1u) * a.BW;
+        for (uint32_t i = blockIdx.x * SBD_THREADS + tid; i < a.BW; i += gridDim.x * SBD_THREADS) other[i] = 0;
+    }
+    for (uint32_t i = tid; i < KS_SPREAD_MAX_KEYS * PB_SH_WORDS; i += SBD_THREADS) sh.bits[i] = 0;
+    if (tid < KS_SPREAD_MAX_KEYS) sh.dom[tid] = 0;
+    if (tid == 0) sh.lack = 0;
+    uint32_t ibase[KS_SPREAD_MAX_KEYS];
+#pragma unroll
+    for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
+        ibase[k] = f.g >= 0 && k < b.K ? __ldg(a.ibase + (size_t)f.g * b.K + k) : AFF_NONE;
+    __syncthreads();
+    uint32_t refused = 0, arefused = 0, lack = 0, ndom[KS_SPREAD_MAX_KEYS] = {0, 0, 0, 0};
+    int64_t imin = INT64_MAX, imax = INT64_MIN;
+    for (uint32_t n = n0 + tid; n < n1; n += SBD_THREADS) {
+        const int r = f.test(b, n, __ldcg(b.free_cpu + n), __ldcg(b.free_mem + n));
+        refused += r == 1;
+        arefused += r == 2;
+        if (r != 3) {
+            a.iraw[n] = PB_NOT_CAND;
+            continue;
+        }
+        int64_t raw = 0;
+#pragma unroll
+        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
+            if (ibase[k] != AFF_NONE) {
+                const int32_t d = __ldg(b.dom + (size_t)k * b.N + n);
+                if (d >= 0) raw += __ldcg(a.icnt + ibase[k] + (uint32_t)d);
+            }
+        a.iraw[n] = raw;
+        imin = min(imin, raw);
+        imax = max(imax, raw);
+        if (!sk || pts_ignored(a, sk, all, n)) continue;
+#pragma unroll
+        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) {
+            if (!(sk >> k & 1u)) continue;
+            const int32_t d = __ldg(b.dom + (size_t)k * b.N + n);
+            if (d < 0) {
+                lack |= 1u << k;
+            } else if (a.uniq >> k & 1u) {
+                ndom[k]++;
+            } else if ((uint32_t)d < PB_SH_WORDS * 32) {
+                atomicOr(sh.bits + k * PB_SH_WORDS + ((uint32_t)d >> 5), 1u << (d & 31));
+            } else {
+                uint32_t* wd = bits + a.bwo[k] + ((uint32_t)d >> 5);
+                const uint32_t bit = 1u << (d & 31);
+                if (!(__ldcg(wd) & bit) && !(atomicOr(wd, bit) & bit)) ndom[k]++;
+            }
+        }
+    }
+    refused = __reduce_add_sync(0xffffffffu, refused);
+    arefused = __reduce_add_sync(0xffffffffu, arefused);
+    lack = __reduce_or_sync(0xffffffffu, lack);
+    if (lane == 0) {
+        sh.ref[warp] = refused;
+        sh.aref[warp] = arefused;
+        if (lack) atomicOr(&sh.lack, lack);
+    }
+    if (sk) {
+#pragma unroll
+        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) {
+            const uint32_t c = __reduce_add_sync(0xffffffffu, ndom[k]);
+            if (lane == 0 && c) atomicAdd(sh.dom + k, c);
+        }
+    }
+    cta_minmax(imin, imax, sh.mm);
+    // sh.bits is complete (cta_minmax synchronises): its words into the parity's bitmap, the new bits counted
+    if (sk) {
+        for (uint32_t i = tid; i < KS_SPREAD_MAX_KEYS * PB_SH_WORDS; i += SBD_THREADS) {
+            const uint32_t k = i / PB_SH_WORDS, v = sh.bits[i];
+            if (!v) continue;
+            const uint32_t old = atomicOr(bits + a.bwo[k] + i % PB_SH_WORDS, v);
+            atomicAdd(sh.dom + k, (uint32_t)__popc(v & ~old));
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        uint32_t r = 0, ar = 0;
+#pragma unroll
+        for (uint32_t w = 0; w < SBD_WARPS; w++) {
+            r += sh.ref[w];
+            ar += sh.aref[w];
+        }
+        b.pref[blockIdx.x] = r;
+        b.paref[blockIdx.x] = ar;
+        a.pimin[blockIdx.x] = imin;
+        a.pimax[blockIdx.x] = imax;
+        a.plack[blockIdx.x] = sh.lack;
+#pragma unroll
+        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) a.pdom[(size_t)blockIdx.x * KS_SPREAD_MAX_KEYS + k] = sh.dom[k];
+    }
+}
+
+// Pass 2 (a pod whose group has soft keys): size_k over the grid's partials, w_k, the PodTopologySpread raw of the
+// slice's candidates into praw[] (-1 when ignored) and its extremes over the non-ignored ones, max from 0
+__device__ __forceinline__ void profile_pass2(const ProfileBindArgs& a, uint32_t p, uint32_t n0, uint32_t n1,
+                                              ProfileShared& sh) {
+    const SpreadBindArgs& b = a.b;
+    const uint32_t tid = threadIdx.x, lane = tid & 31;
+    const int32_t g = __ldg(b.group + p);
+    const uint32_t sk = soft_keys(a, g);
+    const bool all = __ldg(a.soft_all + g);
+    if (tid < 32) {
+        uint32_t lack = 0, c[KS_SPREAD_MAX_KEYS] = {0, 0, 0, 0};
+        for (uint32_t i = lane; i < gridDim.x; i += 32) {
+            lack |= __ldcg(a.plack + i);
+#pragma unroll
+            for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) c[k] += __ldcg(a.pdom + (size_t)i * KS_SPREAD_MAX_KEYS + k);
+        }
+        lack = __reduce_or_sync(0xffffffffu, lack);
+#pragma unroll
+        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) {
+            const uint32_t size = __reduce_add_sync(0xffffffffu, c[k]) + (!all && (lack >> k & 1u));
+            if (lane == 0) sh.w[k] = (sk >> k & 1u) ? __ldg(a.logw + size) : 0.0;
+        }
+    }
+    __syncthreads();
+    const uint32_t* sc = a.scnt + (size_t)g * b.S;
+    int64_t mn = INT64_MAX, mx = 0;
+    for (uint32_t n = n0 + tid; n < n1; n += SBD_THREADS) {
+        if (a.iraw[n] == PB_NOT_CAND) continue;
+        if (pts_ignored(a, sk, all, n)) {
+            a.praw[n] = -1;
+            continue;
+        }
+        double s = 0.0; // ascending k, every operation rounded on its own
+#pragma unroll
+        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) {
+            if (!(sk >> k & 1u)) continue;
+            const int32_t d = __ldg(b.dom + (size_t)k * b.N + n);
+            if (d < 0) continue;
+            const double t = __dadd_rn(__dmul_rn((double)__ldcg(sc + b.Pk[k] + (uint32_t)d), sh.w[k]),
+                                       (double)(__ldg(a.soft_skew + (size_t)g * b.K + k) - 1u));
+            s = __dadd_rn(s, t);
+        }
+        const int64_t raw = (int64_t)round(s); // half away from zero, as Go's math.Round
+        a.praw[n] = raw;
+        mn = min(mn, raw);
+        mx = max(mx, raw);
+    }
+    cta_minmax(mn, mx, sh.mm);
+    if (tid == 0) {
+        a.ppmin[blockIdx.x] = mn;
+        a.ppmax[blockIdx.x] = mx;
+    }
+}
+
+// The normalised scores of candidate n (pts 0 for a group without soft keys)
+__device__ __forceinline__ void profile_parts(const ProfileBindArgs& a, uint32_t sk, uint32_t n, const ProfileShared& sh,
+                                              int64_t& pts, int64_t& ipa) {
+    pts = 0;
+    if (sk) {
+        const int64_t r = __ldcg(a.praw + n);
+        pts = r < 0 ? 0 : sh.pmax == 0 ? 100 : 100 * (sh.pmax + sh.pmin - r) / sh.pmax;
+    }
+    ipa = 0;
+    if (sh.imax > sh.imin) {
+        const int64_t r = __ldcg(a.iraw + n);
+        ipa = (int64_t)__dmul_rn(100.0, __ddiv_rn((double)(r - sh.imin), (double)(sh.imax - sh.imin)));
+    }
+}
+
+// Pass 3: merge the extremes, the totals of the slice's candidates and the argmax partial
+__device__ __forceinline__ void profile_pass3(const ProfileBindArgs& a, uint32_t p, uint32_t n0, uint32_t n1,
+                                              ProfileShared& sh) {
+    const SpreadBindArgs& b = a.b;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int32_t g = __ldg(b.group + p);
+    const uint32_t sk = soft_keys(a, g);
+    if (tid < 32) {
+        int64_t imn = INT64_MAX, imx = INT64_MIN, pmn = INT64_MAX, pmx = 0;
+        for (uint32_t i = lane; i < gridDim.x; i += 32) {
+            imn = min(imn, __ldcg(a.pimin + i));
+            imx = max(imx, __ldcg(a.pimax + i));
+            if (sk) {
+                pmn = min(pmn, __ldcg(a.ppmin + i));
+                pmx = max(pmx, __ldcg(a.ppmax + i));
+            }
+        }
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) {
+            imn = min(imn, (int64_t)__shfl_xor_sync(0xffffffffu, (long long)imn, off));
+            imx = max(imx, (int64_t)__shfl_xor_sync(0xffffffffu, (long long)imx, off));
+            pmn = min(pmn, (int64_t)__shfl_xor_sync(0xffffffffu, (long long)pmn, off));
+            pmx = max(pmx, (int64_t)__shfl_xor_sync(0xffffffffu, (long long)pmx, off));
+        }
+        if (lane == 0) {
+            sh.imin = imn;
+            sh.imax = imx;
+            sh.pmin = pmn;
+            sh.pmax = pmx;
+        }
+    }
+    __syncthreads();
+    const int64_t rc = __ldg(b.req_cpu + p), rm = __ldg(b.req_mem + p);
+    int64_t best = INT64_MIN;
+    int32_t bidx = -1;
+    for (uint32_t n = n0 + tid; n < n1; n += SBD_THREADS) {
+        if (__ldcg(a.iraw + n) == PB_NOT_CAND) continue;
+        int64_t pts, ipa;
+        profile_parts(a, sk, n, sh, pts, ipa);
+        const int64_t key = alloc_score_rt(b.policy, __ldcg(b.free_cpu + n), __ldcg(b.free_mem + n), b.alloc_cpu,
+                                           b.alloc_mem, n, rc, rm) +
+                            (int64_t)a.wspread * pts + (int64_t)a.waff * ipa;
+        if (key > best) { // ascending n per thread: strict '>' keeps the lowest index
+            best = key;
+            bidx = (int32_t)n;
+        }
+    }
+    warp_argmax(best, bidx);
+    if (lane == 0) {
+        sh.key[warp] = best;
+        sh.idx[warp] = bidx;
+    }
+    __syncthreads();
+    if (warp == 0) {
+        best = lane < SBD_WARPS ? sh.key[lane] : INT64_MIN;
+        bidx = lane < SBD_WARPS ? sh.idx[lane] : -1;
+        warp_argmax(best, bidx);
+        if (lane == 0) {
+            b.pkey[blockIdx.x] = best;
+            b.pidx[blockIdx.x] = bidx;
+        }
+    }
+}
+
+// Phase B, CTA 0: spread_bind_commit's merge, binding, charge, hard counts and B/A entries (the merged key is the total,
+// which key_score_rt returns unchanged for every policy this call accepts); then the parts of the winner, the soft
+// counts and the bound pod's IPA entries.  The winner's parts are read from its raws and sh's extremes, which pass 3
+// left in this CTA, and its policy score is the total less the weighted parts.
+__device__ __forceinline__ void profile_commit(const ProfileBindArgs& a, uint32_t p, ProfileShared& sh) {
+    const SpreadBindArgs& b = a.b;
+    const uint32_t tid = threadIdx.x;
+    spread_bind_commit<true>(b, p, &sh.rescan, sh.ref, &sh.bidx);
+    const int32_t g = __ldg(b.group + p), n = sh.bidx;
+    const uint32_t sk = soft_keys(a, g);
+    if (tid == 0 && a.out_parts) {
+        int64_t pts = 0, ipa = 0, ps = 0;
+        if (n >= 0) {
+            profile_parts(a, sk, (uint32_t)n, sh, pts, ipa);
+            ps = __ldcg(b.out_score + p) - (int64_t)a.wspread * pts - (int64_t)a.waff * ipa;
+        }
+        a.out_parts[3 * (size_t)p] = ps;
+        a.out_parts[3 * (size_t)p + 1] = pts;
+        a.out_parts[3 * (size_t)p + 2] = ipa;
+    }
+    if (n < 0 || g < 0) return;
+    if (tid == 0 && sk && !pts_ignored(a, sk, __ldg(a.soft_all + g), (uint32_t)n)) {
+        uint32_t* sc = a.scnt + (size_t)g * b.S;
+        for (uint32_t k = 0; k < b.K; k++) {
+            if (!(sk >> k & 1u)) continue;
+            const int32_t d = __ldg(b.dom + (size_t)k * b.N + n);
+            if (d >= 0) sc[b.Pk[k] + (uint32_t)d] = __ldcg(sc + b.Pk[k] + (uint32_t)d) + 1;
+        }
+    }
+    // entries of one list name distinct (group, key) arrays: no atomics
+    for (uint32_t e = __ldg(a.iupd_off + g) + tid, e1 = __ldg(a.iupd_off + g + 1); e < e1; e += SBD_THREADS) {
+        const uint32_t en = __ldg(a.iupd + e), h = en & 0xffffu, k = en >> 16;
+        const int32_t d = __ldg(b.dom + (size_t)k * b.N + n);
+        if (d < 0) continue;
+        int64_t* c = a.icnt + __ldg(a.ibase + (size_t)h * b.K + k) + (uint32_t)d;
+        *c = __ldcg(c) + __ldg(a.icoef + e);
+    }
+}
+
+template <int W>
+__global__ void __launch_bounds__(SBD_THREADS, 1) k_profile_bind_seq(const ProfileBindArgs a) {
+    cg::grid_group grid = cg::this_grid();
+    __shared__ ProfileShared sh;
+    const uint32_t G = gridDim.x;
+    const uint32_t chunk = (a.b.N + G - 1) / G, n0 = min(a.b.N, blockIdx.x * chunk), n1 = min(a.b.N, n0 + chunk);
+    for (uint32_t p = 0; p < a.b.P; p++) {
+        profile_pass1<W>(a, p, n0, n1, sh);
+        __threadfence();
+        grid.sync();
+        if (soft_keys(a, __ldg(a.b.group + p))) { // uniform: every CTA knows the pod's group
+            profile_pass2(a, p, n0, n1, sh);
+            __threadfence();
+            grid.sync();
+        }
+        profile_pass3(a, p, n0, n1, sh);
+        __threadfence();
+        grid.sync();
+        if (blockIdx.x == 0) profile_commit(a, p, sh);
+        __threadfence();
+        grid.sync();
+    }
+}
+
+// The existing pods' IPA entries into the zeroed counters, one warp per pod (grid-strided)
+__global__ void __launch_bounds__(SBD_THREADS) k_profile_setup(const ProfileBindArgs a) {
+    const uint32_t lane = threadIdx.x & 31, warps = gridDim.x * SBD_WARPS;
+    for (uint32_t e = blockIdx.x * SBD_WARPS + (threadIdx.x >> 5); e < a.b.E; e += warps) {
+        const int32_t h = __ldg(a.b.ex_group + e), n = __ldg(a.b.ex_node + e);
+        for (uint32_t i = __ldg(a.iupd_off + h) + lane, i1 = __ldg(a.iupd_off + h + 1); i < i1; i += 32) {
+            const uint32_t en = __ldg(a.iupd + i), g = en & 0xffffu, k = en >> 16;
+            const int32_t d = __ldg(a.b.dom + (size_t)k * a.b.N + n);
+            if (d < 0) continue;
+            atomicAdd(reinterpret_cast<unsigned long long*>(a.icnt + __ldg(a.ibase + (size_t)g * a.b.K + k) + (uint32_t)d),
+                      (unsigned long long)(int64_t)__ldg(a.icoef + i));
+        }
+    }
+}
+
+cudaError_t launch_profile_bind(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
+    return with_label_width(W, [&](auto w) {
+        constexpr int LW = decltype(w)::value;
+        const SpreadBindArgs& b = a.b;
+        if (b.G) {
+            k_spread_bind_setup<LW><<<b.setup_grid, SBD_THREADS, 0, st>>>(b);
+            g_launches++;
+            const cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess) return e;
+        }
+        cudaError_t e = cudaMemsetAsync(b.acnt, 0, acnt_words * 4, st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(a.icnt, 0, a.iwords * 8, st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(a.bits, 0, (size_t)a.BW * 8, st);
+        if (e == cudaSuccess && (uint64_t)b.G * b.S)
+            e = b.existing ? cudaMemcpyAsync(a.scnt, b.existing, (size_t)b.G * b.S * 4, cudaMemcpyDeviceToDevice, st)
+                           : cudaMemsetAsync(a.scnt, 0, (size_t)b.G * b.S * 4, st);
+        if (e != cudaSuccess) return e;
+        if (b.E) {
+            k_affinity_setup<<<b.aff_grid, SBD_THREADS, 0, st>>>(b);
+            k_profile_setup<<<b.aff_grid, SBD_THREADS, 0, st>>>(a);
+            g_launches += 2;
+            e = cudaGetLastError();
+            if (e != cudaSuccess) return e;
+        }
+        ProfileBindArgs c = a;
+        void* args[] = {&c};
+        e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(k_profile_bind_seq<LW>), dim3(b.grid),
                                         dim3(SBD_THREADS), args, 0, st);
         if (e == cudaSuccess) g_launches++;
         return e;

@@ -54,6 +54,8 @@ for _name, _res, _args in [
                                        _vp, _vp, _vp, C.c_size_t, _vp]),
     ("ksh_reconcile_affinity", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp,
                                          C.c_int, _vp, _vp, _vp, C.c_size_t, _vp]),
+    ("ksh_reconcile_profile", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp,
+                                        _vp, C.c_int, _vp, _vp, _vp, C.c_size_t, _vp]),
 ]:
     _proto(_name, _res, *_args)
 
@@ -449,6 +451,37 @@ class Context:
         max_skew optional (None: no spread constraint), terms a list of (owner group, kind KS_POD_AFFINITY /
         KS_POD_ANTI_AFFINITY, index into topology_keys, target groups) and existing_pods a list of (group, node name) of
         bound pods the terms see.  Returns (status[n], node_idx[n], bodies[n] (str | None))."""
+        return self._reconcile_terms(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
+                                     min_domains, existing_nodes, policy, json_cap, None)
+
+    def reconcile_profile(self, pods, n, group, n_groups, topology_keys, terms=(), existing_pods=(), max_skew=None,
+                          min_domains=None, existing_nodes=None, policy=capi.KS_SCORE_LEAST_BALANCED, json_cap=None,
+                          soft_skew=None, soft_all_keys=None, term_weight=None, hard_affinity_weight=1, weight_spread=2,
+                          weight_affinity=2):
+        """reconcile_affinity scored as the default profile (ksh_reconcile_profile): terms may also be
+        KS_POD_AFFINITY_PREFERRED / KS_POD_ANTI_AFFINITY_PREFERRED with term_weight [T]; soft_skew [n_groups, K] or
+        None, soft_all_keys [n_groups] or None (all 1), and the three weights as Snapshot.profile_bind takes them.
+        Returns (status[n], node_idx[n], bodies[n] (str | None))."""
+        k = len(topology_keys)
+        soft = None if soft_skew is None else np.ascontiguousarray(soft_skew, np.uint32).reshape(-1)
+        if soft is not None and soft.shape[0] != n_groups * k:
+            raise ValueError(f"soft_skew has {soft.shape[0]} entries, groups {n_groups}, keys {k}")
+        sall = None if soft_all_keys is None else np.ascontiguousarray(soft_all_keys, np.uint8).reshape(-1)
+        if sall is not None and sall.shape[0] != n_groups:
+            raise ValueError(f"soft_all_keys has {sall.shape[0]} entries, groups {n_groups}")
+        tw = None if term_weight is None else np.ascontiguousarray(term_weight, np.uint32).reshape(-1)
+        if tw is not None and tw.shape[0] != len(terms):
+            raise ValueError(f"term_weight has {tw.shape[0]} entries, terms {len(terms)}")
+        scoring = capi.ks_bind_scoring(None if soft is None else soft.ctypes.data,
+                                       None if sall is None else sall.ctypes.data,
+                                       None if tw is None else tw.ctypes.data, int(hard_affinity_weight),
+                                       int(weight_spread), int(weight_affinity))
+        return self._reconcile_terms(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
+                                     min_domains, existing_nodes, policy, json_cap, scoring)
+
+    def _reconcile_terms(self, pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew, min_domains,
+                         existing_nodes, policy, json_cap, scoring):
+        # ksh_reconcile_affinity, or with scoring ksh_reconcile_profile
         k = len(topology_keys)
         group = np.ascontiguousarray(group, np.int32).reshape(-1)
         if group.shape[0] != n:
@@ -481,13 +514,15 @@ class Context:
         off = np.empty(n, np.int64)
         cap = int(json_cap if json_cap is not None else 512 * max(n, 1))
         buf = C.create_string_buffer(max(cap, 1))
-        check(lib.ksh_reconcile_affinity(self._h, C.addressof(pods) if n else None, n, group.ctypes.data, int(n_groups),
-                                         C.cast(keys, _vp), k, None if max_skew is None else max_skew.ctypes.data,
-                                         None if mind is None else mind.ctypes.data,
-                                         None if names is None else C.cast(names, _vp),
-                                         None if ex_off is None else ex_off.ctypes.data, C.byref(aff), int(policy),
-                                         status.ctypes.data, node.ctypes.data, C.addressof(buf), cap, off.ctypes.data),
-              "ksh_reconcile_affinity")
+        head = (self._h, C.addressof(pods) if n else None, n, group.ctypes.data, int(n_groups), C.cast(keys, _vp), k,
+                None if max_skew is None else max_skew.ctypes.data, None if mind is None else mind.ctypes.data,
+                None if names is None else C.cast(names, _vp), None if ex_off is None else ex_off.ctypes.data,
+                C.byref(aff))
+        tail = (int(policy), status.ctypes.data, node.ctypes.data, C.addressof(buf), cap, off.ctypes.data)
+        if scoring is None:
+            check(lib.ksh_reconcile_affinity(*head, *tail), "ksh_reconcile_affinity")
+        else:
+            check(lib.ksh_reconcile_profile(*head, C.byref(scoring), *tail), "ksh_reconcile_profile")
         return status, node, _string_list(buf, off)
 
     def drain_nodes(self, node_names, pods, pod_offset, policy=capi.KS_SCORE_LEFTOVER, flags=0):

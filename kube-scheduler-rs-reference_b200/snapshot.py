@@ -451,6 +451,79 @@ class Snapshot:
             counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
         return idx, score, refused, counts
 
+    def profile_bind(self, req_cpu, req_mem, sel, group, n_groups, keys, terms=(), existing_pods=None, max_skew=None,
+                     min_domains=None, existing=None, policy=capi.KS_SCORE_LEAST_BALANCED, soft_skew=None,
+                     soft_all_keys=None, term_weight=None, hard_affinity_weight=1, weight_spread=2, weight_affinity=2,
+                     want_counts=True):
+        """affinity_bind scored as the default profile (ks_profile_bind): terms may also be
+        KS_POD_AFFINITY_PREFERRED / KS_POD_ANTI_AFFINITY_PREFERRED, each with its term_weight [T] (0 for required
+        terms); soft_skew [G, K] or None (ScheduleAnyway maxSkew, 0 = none); soft_all_keys [G] or None (all 1).
+        Charges free[].  Returns (node_idx int32 [P], score int64 [P], parts int64 [P, 3] (policy, pts, ipa),
+        refused uint32 [P, 2], counts, soft_counts); both counts lists of K arrays [G, D_k], or None."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        p, g = int(pods.n), int(n_groups)
+        group = _c(group, np.int32).reshape(-1)
+        if group.shape[0] != p:
+            raise ValueError(f"group has {group.shape[0]} entries, pods {p}")
+        k = len(keys)
+        if not 1 <= k <= capi.KS_SPREAD_MAX_KEYS:
+            raise ValueError(f"{k} topology keys (1 to {capi.KS_SPREAD_MAX_KEYS})")
+        doms = [_c(d, np.int32).reshape(-1) for d, _ in keys]
+        nd = [int(n) for _, n in keys]
+
+        def per_group(a, dtype, width, name):
+            if a is None:
+                return None
+            a = _c(a, dtype).reshape(-1)
+            if a.shape[0] != g * width:
+                raise ValueError(f"{name} has {a.shape[0]} entries, expected {g * width}")
+            return a
+        max_skew = per_group(max_skew, np.uint32, k, "max_skew")
+        min_domains = per_group(min_domains, np.uint32, k, "min_domains")
+        soft_skew = per_group(soft_skew, np.uint32, k, "soft_skew")
+        soft_all_keys = per_group(soft_all_keys, np.uint8, 1, "soft_all_keys")
+        s = sum(nd)
+        if existing is not None:
+            if len(existing) != k:
+                raise ValueError(f"existing has {len(existing)} blocks, keys {k}")
+            existing = _c(np.concatenate([np.asarray(e, np.uint32).reshape(g, n) for e, n in zip(existing, nd)],
+                                         axis=1), np.uint32).reshape(-1)
+        topo = capi.ks_spread_multi(k, (C.c_uint32 * capi.KS_SPREAD_MAX_KEYS)(*nd),
+                                    (C.c_void_p * capi.KS_SPREAD_MAX_KEYS)(*[_ptr(d) for d in doms]),
+                                    _ptr(max_skew), _ptr(min_domains), _ptr(existing))
+        owner = _c([t[0] for t in terms], np.int32)
+        kind = _c([t[1] for t in terms], np.uint8)
+        key = _c([t[2] for t in terms], np.uint32)
+        toff = np.zeros(len(terms) + 1, np.uint64)
+        np.cumsum([len(t[3]) for t in terms], out=toff[1:])
+        target = _c(np.concatenate([np.asarray(t[3], np.int64).reshape(-1) for t in terms]) if terms else [], np.int32)
+        if term_weight is not None:
+            term_weight = _c(term_weight, np.uint32).reshape(-1)
+            if term_weight.shape[0] != len(terms):
+                raise ValueError(f"term_weight has {term_weight.shape[0]} entries, terms {len(terms)}")
+        eg, en = (np.zeros(0, np.int32),) * 2 if existing_pods is None else existing_pods
+        eg, en = _c(eg, np.int32).reshape(-1), _c(en, np.int32).reshape(-1)
+        if eg.shape[0] != en.shape[0]:
+            raise ValueError(f"existing pods: {eg.shape[0]} groups, {en.shape[0]} nodes")
+        aff = capi.ks_pod_affinity(len(terms), _ptr(owner), _ptr(kind), _ptr(key), _ptr(toff), _ptr(target),
+                                   eg.shape[0], _ptr(eg), _ptr(en))
+        scoring = capi.ks_bind_scoring(_ptr(soft_skew), _ptr(soft_all_keys), _ptr(term_weight),
+                                       int(hard_affinity_weight), int(weight_spread), int(weight_affinity))
+        idx = np.empty(p, np.int32)
+        score = np.empty(p, np.int64)
+        parts = np.empty((p, 3), np.int64)
+        refused = np.empty((p, 2), np.uint32)
+        want = want_counts and 0 < g * s <= capi.KS_SPREAD_MAX_COUNTS
+        counts = np.empty((g, s), np.uint32) if want else None
+        soft = np.empty((g, s), np.uint32) if want else None
+        check(lib.ks_profile_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
+                                  C.byref(scoring), int(policy), _ptr(idx), _ptr(score), _ptr(parts), _ptr(refused),
+                                  _ptr(counts), _ptr(soft)), "ks_profile_bind")
+        if want:
+            counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
+            soft = np.split(soft, np.cumsum(nd)[:-1], axis=1)
+        return idx, score, parts, refused, counts, soft
+
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
         """The reference's own policy (src/main.rs:49-71), seeded: (node_idx, attempts_used, draw_node, draw_code)."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
