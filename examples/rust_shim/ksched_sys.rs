@@ -33,6 +33,7 @@ pub const KSH_RECONCILE_BINDING_OBJECT_FAILED: c_int = 2; // ReconcileError::Cre
 pub const KSH_RECONCILE_GANG_UNSATISFIED: c_int = 4; // ksh_reconcile_gangs: the pod's group rolled back
 pub const KSH_RECONCILE_SPREAD_UNSATISFIED: c_int = 5; // ksh_reconcile_spread: spread constraints refused every node
 pub const KSH_RECONCILE_AFFINITY_UNSATISFIED: c_int = 6; // ksh_reconcile_affinity: pod (anti-)affinity refused every node
+pub const KSH_RECONCILE_NODE_RULES_UNSATISFIED: c_int = 7; // ksh_reconcile_nodes: taints or node affinity refused every node
 pub const KS_REFERENCE_ATTEMPTS: u32 = 5; // ATTEMPTS, src/main.rs:49
 pub const KS_MAX_PEERS: usize = 15;
 pub const KS_TOPK_MAX: u32 = 32; // largest k of ks_select_topk / ksh_rank_nodes
@@ -60,6 +61,10 @@ pub const KS_AFFINITY_MAX_EXISTING: u64 = 1 << 24; // most existing pods
 pub const KS_AFFINITY_MAX_UPDATES: u64 = 1 << 24; // most compiled update entries
 pub const KS_POD_AFFINITY_PREFERRED: u8 = 2; // ks_profile_bind: preferred terms score only
 pub const KS_POD_ANTI_AFFINITY_PREFERRED: u8 = 3;
+pub const KS_NODE_RULES_MAX_TAINTS: u32 = 64; // ks_node_bind
+pub const KS_NODE_RULES_MAX_KEYS: usize = 16;
+pub const KS_NODE_RULES_MAX_PREFERRED: u32 = 4096;
+pub const KS_NODE_RULES_MAX_WORDS: u64 = 1 << 26;
 
 #[repr(C)]
 pub struct ks_kv {
@@ -235,6 +240,59 @@ pub struct ks_bind_scoring {
     pub weight_affinity: u32,
 }
 #[repr(C)]
+pub struct ks_node_rules {
+    pub n_taints: u32,
+    pub node_taint_hard: *const u64,
+    pub node_taint_soft: *const u64,
+    pub tolerate_hard: *const u64,
+    pub tolerate_soft: *const u64,
+    pub n_keys: u32,
+    pub n_domains: [u32; KS_NODE_RULES_MAX_KEYS],
+    pub node_domain: [*const i32; KS_NODE_RULES_MAX_KEYS],
+    pub n_exprs: u32,
+    pub expr_key: *const u32,
+    pub expr_set_offset: *const u64,
+    pub expr_set: *const u64,
+    pub n_terms: u32,
+    pub term_owner: *const i32,
+    pub term_weight: *const u32,
+    pub term_expr_offset: *const u32,
+    pub weight_taint: u32,
+    pub weight_node_affinity: u32,
+}
+#[repr(C)]
+pub struct ksh_taint {
+    pub key: *const c_char,
+    pub value: *const c_char,
+    pub effect: *const c_char,
+}
+#[repr(C)]
+pub struct ksh_toleration {
+    pub key: *const c_char,
+    pub op: *const c_char,
+    pub value: *const c_char,
+    pub effect: *const c_char,
+}
+#[repr(C)]
+pub struct ksh_node_selector_requirement {
+    pub key: *const c_char,
+    pub op: *const c_char,
+    pub values: *const *const c_char,
+    pub n_values: u32,
+}
+#[repr(C)]
+pub struct ksh_node_rules {
+    pub toleration_offset: *const u64,
+    pub tolerations: *const ksh_toleration,
+    pub n_terms: u32,
+    pub term_owner: *const i32,
+    pub term_weight: *const u32,
+    pub term_req_offset: *const u64,
+    pub requirements: *const ksh_node_selector_requirement,
+    pub weight_taint: u32,
+    pub weight_node_affinity: u32,
+}
+#[repr(C)]
 pub struct ksh_pod_affinity {
     pub n_terms: u32,
     pub owner: *const i32,
@@ -311,6 +369,10 @@ extern "C" {
                            topo: *const ks_spread_multi, aff: *const ks_pod_affinity, scoring: *const ks_bind_scoring,
                            policy: c_int, node_idx: *mut i32, score: *mut i64, parts: *mut i64, refused: *mut u32,
                            domain_count: *mut u32, soft_count: *mut u32) -> c_int;
+    pub fn ks_node_bind(s: *mut ks_snapshot, pods: *const ks_pods, group: *const i32, n_groups: u32,
+                        topo: *const ks_spread_multi, aff: *const ks_pod_affinity, scoring: *const ks_bind_scoring,
+                        rules: *const ks_node_rules, policy: c_int, node_idx: *mut i32, score: *mut i64,
+                        parts: *mut i64, refused: *mut u32, domain_count: *mut u32, soft_count: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -384,6 +446,17 @@ extern "C" {
                                   existing_offset: *const u64, aff: *const ksh_pod_affinity, policy: c_int,
                                   status: *mut i32, node_idx: *mut i32, json: *mut c_char, cap: usize,
                                   json_off: *mut i64) -> c_int;
+    pub fn ksh_context_set_node_taints(ctx: *mut ksh_context, node_names: *const *const c_char, taint_offset: *const u64,
+                                       taints: *const ksh_taint, n: u64) -> c_int;
+    pub fn ksh_compile_node_rules(ctx: *mut ksh_context, n_groups: u32, rules: *const ksh_node_rules, hard: *mut u8,
+                                  affinity: *mut u8, soft: *mut u32, preferred: *mut u32) -> c_int;
+    pub fn ksh_reconcile_nodes(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group: *const i32, n_groups: u32,
+                               topology_keys: *const *const c_char, n_keys: u32, max_skew: *const u32,
+                               min_domains: *const u32, existing_node_names: *const *const c_char,
+                               existing_offset: *const u64, aff: *const ksh_pod_affinity,
+                               scoring: *const ks_bind_scoring, rules: *const ksh_node_rules, policy: c_int,
+                               status: *mut i32, node_idx: *mut i32, json: *mut c_char, cap: usize,
+                               json_off: *mut i64) -> c_int;
     pub fn ksh_reconcile_profile(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group: *const i32,
                                  n_groups: u32, topology_keys: *const *const c_char, n_keys: u32, max_skew: *const u32,
                                  min_domains: *const u32, existing_node_names: *const *const c_char,

@@ -798,7 +798,7 @@ int ks_affinity_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const
  * final sc.  Each but out_node_idx may be NULL.
  * Departures from upstream: ties go to the lowest index instead of at random; w_k comes from libm, not Go's math.Log;
  * size_k is a distinct-domain count for every key, which is upstream's hostname special case whenever hostnames are
- * unique; TaintToleration, NodeAffinity and ImageLocality are not modelled (constant for pods and nodes without taints
+ * unique; TaintToleration, NodeAffinity (see ks_node_bind) and ImageLocality are not modelled (constant for pods and nodes without taints
  * or preferences, and the total omits those constants); nodeInclusionPolicies and matchLabelKeys are out of scope.
  * Identities, policies 1, 3 and 4:
  *   (J1) soft_skew NULL, no preferred term and hard_affinity_weight = 0 (or weight_spread = weight_affinity = 0): the
@@ -834,6 +834,86 @@ int ks_profile_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const 
                     int32_t* out_node_idx /* [P] */, int64_t* out_score /* [P] or NULL */,
                     int64_t* out_parts /* [3P] or NULL */, uint32_t* out_refused /* [2P] or NULL */,
                     uint32_t* out_domain_count /* [G * S] or NULL */, uint32_t* out_soft_count /* [G * S] or NULL */);
+
+/* ---- taints and node affinity when binding: ks_profile_bind with upstream's TaintToleration and NodeAffinity
+ * plugins, Filter and Score (restated here; spec extension, DESIGN.md 5p) ----
+ * The arguments of ks_profile_bind plus `rules` (host memory).  All pods of one group share its tolerations and node
+ * affinity; group -1 tolerates nothing and has no node affinity, and is still filtered by taints.
+ * Taints: the caller numbers up to 64 distinct (key, value, effect) triples.  node_taint_hard[n] holds the bits of node
+ * n's NoSchedule and NoExecute taints, node_taint_soft[n] those of its PreferNoSchedule taints; tolerate_hard[g] and
+ * tolerate_soft[g] the bits group g tolerates (the soft mask from the tolerations whose effect is empty or
+ * PreferNoSchedule only, as upstream's getAllTolerationPreferNoSchedule).  Each of the four may be NULL (= all 0).
+ * Node affinity, resolved to domain sets: KN = n_keys rule keys, key k with D_k = n_domains[k] domains and
+ * node_domain[k][n] in [-1, D_k) (-1 = the node lacks the key), numbered as ksh_context_topology_domains numbers them.
+ * Expression x is (expr_key[x], a set over 0..D_k): words [expr_set_offset[x], expr_set_offset[x + 1]) of expr_set,
+ * exactly (D_k + 1 + 63) / 64 of them, bit i = domain i, bit D_k = "absent", no bit above D_k.  A node passes the
+ * expression iff bit (d >= 0 ? d : D_k) is set.  Term t of group term_owner[t] is the AND of its expressions
+ * [term_expr_offset[t], term_expr_offset[t + 1]); a term with no expression matches nothing.  term_weight[t] = 0 makes
+ * it a required term (the group's required terms are ORed; a group without one has no required affinity), a weight in
+ * [1, 100] a preferred one.  At most KS_NODE_RULES_MAX_PREFERRED preferred terms per group.
+ * For pod p of group g and node n, the filters run in this order: fit and selector; taints: refused when
+ * node_taint_hard[n] & ~tolerate_hard[g] != 0; required node affinity; hard spread; rules 1-3 of ks_affinity_bind.
+ * Spread eligibility (upstream's nodeAffinityPolicy Honor, nodeTaintsPolicy Ignore): a group's eligible domains come
+ * from the nodes that pass its selector, its required node affinity and carry its constrained keys; taints do not count.
+ * Scores over F, the pod's candidates after every filter:
+ *   - TaintToleration: raw(n) = popcount(node_taint_soft[n] & ~tolerate_soft[g]); with max over F, tt(n) = 100 when
+ *     max = 0, else 100 - 100 * raw(n) / max in int64 (upstream DefaultNormalizeScore(100, reverse = true));
+ *   - NodeAffinity: raw(n) = the sum of the weights of g's preferred terms n matches; na(n) = 0 when max = 0, else
+ *     100 * raw(n) / max (DefaultNormalizeScore(100, false)); 0 for a group without preferred terms (upstream's Skip);
+ *   - total = ks_profile_bind's total + weight_taint * tt(n) + weight_node_affinity * na(n), ties to the lower index.
+ * Outputs as ks_profile_bind's, except: out_parts[5p .. 5p + 4] = (policy, pts, ipa, tt, na) of the winner (zeros for
+ * an unbound pod); out_refused[4p .. 4p + 3] = the nodes that fit (fit and selector) but carry an untolerated hard
+ * taint, the nodes that fit and are tolerated but fail required node affinity, then ks_profile_bind's two words over
+ * the nodes that pass both.
+ * Identities, policies 1, 3 and 4:
+ *   (K1) rules NULL: every output is ks_profile_bind's, bit for bit, and out_parts words 3 and 4 are 0;
+ *   (K2) no node carries a taint and no group has a node-affinity term: the nodes, refusal words 2-3, both counts and
+ *        free[] are ks_profile_bind's, refusal words 0-1 are 0 and every score is higher by exactly 100 * weight_taint;
+ *   (K3) a required term `key In {v}` binds the same nodes as a nodeSelector key=v on the same groups;
+ *   (K4) a NoSchedule taint that every group tolerates changes nothing but the score constant.
+ * Checked on the host before any device work and before free[] changes: every check of ks_profile_bind; KS_ERR_INVALID
+ * for a taint bit at or above n_taints, a key at or above n_keys, a NULL node_domain or array that is needed, a node
+ * domain outside [-1, D_k), a set of the wrong width or with a bit above D_k, decreasing offsets, a term owner outside
+ * [0, G), a term weight above 100 or a plugin weight above 100; KS_ERR_RANGE for more than 64 taints, more than
+ * KS_NODE_RULES_MAX_KEYS keys, more than KS_NODE_RULES_MAX_PREFERRED preferred terms in a group, or more than
+ * KS_NODE_RULES_MAX_WORDS rule words.
+ * The groups are mapped to node-rule classes, their distinct (tolerations, terms) signatures; group -1 shares the class
+ * of the groups without rules.  k_node_rules_setup writes one 32-bit word per (class, node): the filter reason, the
+ * "passes required affinity" bit, the PreferNoSchedule count and the preferred-affinity raw, so the per-pod cycle reads
+ * one extra word per node however many expressions a group carries; rule words = classes x N.
+ * Out of scope: node rules in ks_select, ks_stream_bind, ks_gang_bind, the planners and ks_explain; matchFields;
+ * nodeTaintsPolicy Honor; NodeUnschedulable; ImageLocality; NoExecute eviction and tolerationSeconds; random ties. */
+#define KS_NODE_RULES_MAX_TAINTS 64u
+#define KS_NODE_RULES_MAX_KEYS 16u
+#define KS_NODE_RULES_MAX_PREFERRED 4096u     /* per group: the raw sum stays below 2^22 */
+#define KS_NODE_RULES_MAX_WORDS (1ull << 26)  /* classes x nodes */
+typedef struct ks_node_rules {                /* host memory */
+    uint32_t n_taints;                        /* [0, 64] */
+    const uint64_t* node_taint_hard;          /* [N] or NULL */
+    const uint64_t* node_taint_soft;          /* [N] or NULL */
+    const uint64_t* tolerate_hard;            /* [G] or NULL */
+    const uint64_t* tolerate_soft;            /* [G] or NULL */
+    uint32_t n_keys;                          /* KN, [0, KS_NODE_RULES_MAX_KEYS] */
+    uint32_t n_domains[KS_NODE_RULES_MAX_KEYS];
+    const int32_t* node_domain[KS_NODE_RULES_MAX_KEYS]; /* [N] each */
+    uint32_t n_exprs;
+    const uint32_t* expr_key;                 /* [X] */
+    const uint64_t* expr_set_offset;          /* [X + 1], in words of expr_set */
+    const uint64_t* expr_set;
+    uint32_t n_terms;
+    const int32_t* term_owner;                /* [T], in [0, G) */
+    const uint32_t* term_weight;              /* [T]: 0 = required, [1, 100] = preferred */
+    const uint32_t* term_expr_offset;         /* [T + 1] */
+    uint32_t weight_taint;                    /* TaintToleration plugin weight, [0, 100]; default profile 3 */
+    uint32_t weight_node_affinity;            /* NodeAffinity plugin weight, [0, 100]; default profile 2 */
+} ks_node_rules;
+int ks_node_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const int32_t* group /* [P] */,
+                 uint32_t n_groups, const ks_spread_multi* topo /* keys; max_skew may be NULL */,
+                 const ks_pod_affinity* aff /* or NULL */, const ks_bind_scoring* scoring,
+                 const ks_node_rules* rules /* or NULL */, int policy, int32_t* out_node_idx /* [P] */,
+                 int64_t* out_score /* [P] or NULL */, int64_t* out_parts /* [5P] or NULL */,
+                 uint32_t* out_refused /* [4P] or NULL */, uint32_t* out_domain_count /* [G * S] or NULL */,
+                 uint32_t* out_soft_count /* [G * S] or NULL */);
 
 #ifdef __cplusplus
 }

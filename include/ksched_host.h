@@ -43,6 +43,9 @@ extern "C" {
 #define KSH_RECONCILE_AFFINITY_UNSATISFIED 6 /* ksh_reconcile_affinity: fit, selector and spread passed on some node but
                                                 the pod's inter-pod (anti-)affinity refused every such node (upstream:
                                                 "didn't match pod affinity/anti-affinity rules") */
+#define KSH_RECONCILE_NODE_RULES_UNSATISFIED 7 /* ksh_reconcile_nodes: some node fit (resources and selector) but taints
+                                                  or required node affinity refused every such node (upstream:
+                                                  "untolerated taint" / "didn't match Pod's node affinity/selector") */
 
 /* Kubernetes quantity strings, exact: cpu -> millicores, memory -> bytes.
  * KS_ERR_PARSE (malformed), KS_ERR_INEXACT (finer than 1m / 1 byte), KS_ERR_RANGE. */
@@ -320,6 +323,69 @@ int ksh_reconcile_profile(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_p
                           const char* const* existing_node_names, const uint64_t* existing_offset,
                           const ksh_pod_affinity* aff /* or NULL */, const ks_bind_scoring* scoring, int policy,
                           int32_t* out_status, int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off);
+
+/* Taints and node affinity over objects (ks_node_bind, ksched.h; DESIGN.md 5p).
+ * ksh_context_set_node_taints records spec.taints of nodes in the store: node node_names[i] carries
+ * taints[taint_offset[i] .. taint_offset[i + 1]), replacing what it carried.  Names not in the store are ignored (KS_OK),
+ * as with the other events.  A node's taints are kept by name: they survive an upsert of that name, are dropped by
+ * ksh_context_remove_node and are cleared by ksh_context_set_nodes.  A taint needs a non-empty key and the effect
+ * NoSchedule, PreferNoSchedule or NoExecute (KS_ERR_INVALID otherwise, before anything changes); a NULL value is "".
+ * Pure host work: works on a packing-only context. */
+typedef struct ksh_taint { const char* key; const char* value; const char* effect; } ksh_taint;
+int ksh_context_set_node_taints(ksh_context* ctx, const char* const* node_names, const uint64_t* taint_offset,
+                                const ksh_taint* taints, uint64_t n);
+
+/* Per-group tolerations and node affinity (pods of one group share them, as they share selectors).
+ * Group g tolerates tolerations[toleration_offset[g] .. toleration_offset[g + 1]) (toleration_offset [G + 1] or NULL:
+ * none), matched against each taint as upstream's ToleratesTaint: an empty effect matches every effect, an empty key
+ * every key, operator Exists ignores the value, Equal or "" compares it.  Node-affinity term t of group term_owner[t] is
+ * the AND of requirements[term_req_offset[t] .. term_req_offset[t + 1]); term_weight[t] 0 = a required term (ORed),
+ * [1, 100] = a preferred one.  Requirement operators In, NotIn, Exists, DoesNotExist, Gt, Lt over the node store's label
+ * values; NotIn and DoesNotExist match nodes without the key; Gt and Lt parse the node's value as a base-10 int64, and a
+ * value that does not parse never matches.  KS_ERR_INVALID for what API validation rejects: an unknown toleration or
+ * requirement operator, Exists with a value, In/NotIn without values, Gt/Lt without exactly one integer value,
+ * Exists/DoesNotExist with values; KS_ERR_RANGE for more than 64 distinct taints in the store or more than
+ * KS_NODE_RULES_MAX_KEYS requirement keys. */
+typedef struct ksh_toleration { const char* key; const char* op; const char* value; const char* effect; } ksh_toleration;
+typedef struct ksh_node_selector_requirement {
+    const char* key;
+    const char* op;                      /* In, NotIn, Exists, DoesNotExist, Gt, Lt */
+    const char* const* values;
+    uint32_t n_values;
+} ksh_node_selector_requirement;
+typedef struct ksh_node_rules {
+    const uint64_t* toleration_offset;   /* [G + 1] or NULL */
+    const ksh_toleration* tolerations;
+    uint32_t n_terms;
+    const int32_t* term_owner;           /* [T] */
+    const uint32_t* term_weight;         /* [T] */
+    const uint64_t* term_req_offset;     /* [T + 1] */
+    const ksh_node_selector_requirement* requirements;
+    uint32_t weight_taint;               /* default profile 3 */
+    uint32_t weight_node_affinity;       /* default profile 2 */
+} ksh_node_rules;
+
+/* The compilation ksh_reconcile_nodes hands to ks_node_bind, evaluated per (group g, node n) at g * N + n from the
+ * compiled masks and domain sets: out_hard = 1 when n carries a NoSchedule/NoExecute taint g does not tolerate,
+ * out_affinity = 1 when n passes g's required node affinity, out_soft = n's PreferNoSchedule taints g does not tolerate
+ * (by the tolerations whose effect is empty or PreferNoSchedule), out_preferred = the summed weights of g's preferred
+ * terms n matches.  Each output may be NULL.  Errors as ksh_reconcile_nodes' compilation.  Pure host work: works on a
+ * packing-only context. */
+int ksh_compile_node_rules(ksh_context* ctx, uint32_t n_groups, const ksh_node_rules* rules, uint8_t* out_hard,
+                           uint8_t* out_affinity, uint32_t* out_soft, uint32_t* out_preferred);
+
+/* reconcile() under the default profile with taints and node affinity: ksh_reconcile_profile with the context's node
+ * taints and `rules' (NULL: no toleration and no term), bound by ks_node_bind.  An unbound pod gets
+ * KSH_RECONCILE_NODE_RULES_UNSATISFIED when some node fit it but taints or required node affinity refused every such
+ * node, else the statuses map as in ksh_reconcile_affinity over the nodes that pass both.  Errors as
+ * ksh_reconcile_profile, ks_node_bind and ksh_compile_node_rules. */
+int ksh_reconcile_nodes(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, const int32_t* group,
+                        uint32_t n_groups, const char* const* topology_keys, uint32_t n_keys,
+                        const uint32_t* max_skew /* or NULL */, const uint32_t* min_domains,
+                        const char* const* existing_node_names, const uint64_t* existing_offset,
+                        const ksh_pod_affinity* aff /* or NULL */, const ks_bind_scoring* scoring,
+                        const ksh_node_rules* rules /* or NULL */, int policy, int32_t* out_status,
+                        int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off);
 
 #ifdef __cplusplus
 }

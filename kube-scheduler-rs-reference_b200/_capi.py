@@ -244,6 +244,25 @@ class ks_bind_scoring(C.Structure):
 _proto("ks_profile_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_uint32,
        C.POINTER(ks_spread_multi), C.POINTER(ks_pod_affinity), C.POINTER(ks_bind_scoring), C.c_int, C.c_void_p,
        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
+KS_NODE_RULES_MAX_TAINTS = 64
+KS_NODE_RULES_MAX_KEYS = 16
+KS_NODE_RULES_MAX_PREFERRED = 4096
+KS_NODE_RULES_MAX_WORDS = 1 << 26
+
+
+class ks_node_rules(C.Structure):
+    _fields_ = [("n_taints", C.c_uint32), ("node_taint_hard", C.c_void_p), ("node_taint_soft", C.c_void_p),
+                ("tolerate_hard", C.c_void_p), ("tolerate_soft", C.c_void_p), ("n_keys", C.c_uint32),
+                ("n_domains", C.c_uint32 * KS_NODE_RULES_MAX_KEYS), ("node_domain", C.c_void_p * KS_NODE_RULES_MAX_KEYS),
+                ("n_exprs", C.c_uint32), ("expr_key", C.c_void_p), ("expr_set_offset", C.c_void_p),
+                ("expr_set", C.c_void_p), ("n_terms", C.c_uint32), ("term_owner", C.c_void_p),
+                ("term_weight", C.c_void_p), ("term_expr_offset", C.c_void_p), ("weight_taint", C.c_uint32),
+                ("weight_node_affinity", C.c_uint32)]
+
+
+_proto("ks_node_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_uint32,
+       C.POINTER(ks_spread_multi), C.POINTER(ks_pod_affinity), C.POINTER(ks_bind_scoring), C.POINTER(ks_node_rules),
+       C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
 KS_AFFINITY_MAX_TERMS = 16384
 KS_AFFINITY_MAX_TARGETS = 1 << 22
 KS_AFFINITY_MAX_EXISTING = 1 << 24

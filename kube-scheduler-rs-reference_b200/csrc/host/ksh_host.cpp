@@ -9,6 +9,7 @@
 #include <new>
 #include <string>
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <cstdlib>
 #include <mutex>
@@ -36,6 +37,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 #pragma weak ks_spread_bind
 #pragma weak ks_affinity_bind
 #pragma weak ks_profile_bind
+#pragma weak ks_node_bind
 
 namespace {
 
@@ -284,6 +286,8 @@ struct ksh_context {
     std::vector<int64_t> pk_cpu, pk_mem; // packed form of the last batch a device call packed (pack_batch)
     std::vector<uint64_t> pk_sel;
     bool dirty = true; // device snapshot must be re-uploaded
+    // spec.taints by node name (ksh_context_set_node_taints): key, value, effect
+    std::unordered_map<std::string, std::vector<std::array<std::string, 3>>> taints;
     // one lock per context: every ksh_* entry that takes a context holds it for the whole call (entries call each other)
     mutable std::recursive_mutex mu;
 };
@@ -1009,6 +1013,7 @@ int ksh_context_set_nodes(ksh_context* c, const ks_node_obj* nodes, uint32_t n) 
     }
     c->W = words_for_bits((uint32_t)c->bit2pair.size());
     bound_clear(c);
+    c->taints.clear();
     c->dirty = true;
     return KS_OK;
 }
@@ -1051,6 +1056,7 @@ int ksh_context_remove_node(ksh_context* c, const char* name) try {
     const int32_t found = node_index_of(c, name);
     if (found < 0) return KS_OK;
     const uint32_t idx = (uint32_t)found;
+    c->taints.erase(name);
     node_pairs_release(c, idx);
     c->nameid2idx[c->idx2nameid[idx]] = -1;
     c->idx2nameid.erase(c->idx2nameid.begin() + idx);
@@ -1712,6 +1718,190 @@ int ksh_place_replicas_spread_multi(ksh_context* c, const ks_pod_obj* pods, uint
 }
 KSH_CATCH
 
+// ---- taints and node affinity (ks_node_bind, DESIGN.md 5p) ----
+// The packed rules of one call over the node store, and the arrays its pointers reach
+struct CompiledNodeRules {
+    ks_node_rules r{};
+    std::vector<uint64_t> hard, soft, tol_h, tol_s, set_off, sets;
+    std::vector<std::vector<int32_t>> dom;
+    std::vector<uint32_t> expr_key, term_w, term_off;
+    std::vector<int32_t> owner;
+};
+
+// Go's strconv.ParseInt(s, 10, 64)
+static bool parse_int64(const char* s, int64_t* v) {
+    if (!s || !*s) return false;
+    size_t i = 0;
+    const bool neg = s[0] == '-';
+    if (s[0] == '+' || s[0] == '-') i = 1;
+    if (!s[i]) return false;
+    u128 m = 0;
+    for (; s[i]; i++) {
+        if (s[i] < '0' || s[i] > '9') return false;
+        m = m * 10 + (unsigned)(s[i] - '0');
+        if (m > ((u128)1 << 63)) return false;
+    }
+    if (!neg && m > (u128)INT64_MAX) return false;
+    *v = neg ? (int64_t)(0 - (uint64_t)m) : (int64_t)m;
+    return true;
+}
+
+static bool tolerates(const ksh_toleration& t, const std::array<std::string, 3>& taint) {
+    const std::string op = nz(t.op), eff = nz(t.effect), key = nz(t.key);
+    if (!eff.empty() && eff != taint[2]) return false;
+    if (!key.empty() && key != taint[0]) return false;
+    if (op == "Exists") return true;
+    return nz(t.value) == taint[1]; // "" or Equal
+}
+
+static int compile_node_rules(ksh_context* c, uint32_t G, const ksh_node_rules* in, CompiledNodeRules* out) {
+    const ksh_node_rules none{};
+    if (!in) in = &none;
+    const uint32_t N = c->N, T = in->n_terms;
+    if (in->toleration_offset && in->toleration_offset[G] && !in->tolerations) return fail(KS_ERR_INVALID, "NULL tolerations");
+    if (T && (!in->term_owner || !in->term_weight || !in->term_req_offset))
+        return fail(KS_ERR_INVALID, "NULL term_owner, term_weight or term_req_offset");
+    if (T && in->term_req_offset[T] && !in->requirements) return fail(KS_ERR_INVALID, "NULL requirements");
+    if (in->toleration_offset)
+        for (uint32_t g = 0; g < G; g++) {
+            if (in->toleration_offset[g + 1] < in->toleration_offset[g])
+                return fail(KS_ERR_INVALID, "toleration offsets decrease");
+            for (uint64_t i = in->toleration_offset[g]; i < in->toleration_offset[g + 1]; i++) {
+                const std::string op = nz(in->tolerations[i].op);
+                if (op != "" && op != "Equal" && op != "Exists")
+                    return fail(KS_ERR_INVALID, "group " + std::to_string(g) + ": toleration operator \"" + op + "\"");
+                if (op == "Exists" && *nz(in->tolerations[i].value))
+                    return fail(KS_ERR_INVALID, "group " + std::to_string(g) + ": Exists toleration with a value");
+            }
+        }
+    std::vector<std::string> keys; // requirement keys in order of first appearance
+    for (uint32_t t = 0; t < T; t++) {
+        if (in->term_owner[t] < 0 || in->term_owner[t] >= (int64_t)G)
+            return fail(KS_ERR_INVALID, "node-affinity term " + std::to_string(t) + ": owner outside [0, n_groups)");
+        if (in->term_weight[t] > 100) return fail(KS_ERR_INVALID, "node-affinity term " + std::to_string(t) + ": weight above 100");
+        if (in->term_req_offset[t + 1] < in->term_req_offset[t]) return fail(KS_ERR_INVALID, "requirement offsets decrease");
+        for (uint64_t i = in->term_req_offset[t]; i < in->term_req_offset[t + 1]; i++) {
+            const ksh_node_selector_requirement& q = in->requirements[i];
+            const std::string op = nz(q.op), where = "requirement " + std::to_string(i) + " (" + op + "): ";
+            if (!q.key || !*q.key) return fail(KS_ERR_INVALID, where + "empty key");
+            if (q.n_values && !q.values) return fail(KS_ERR_INVALID, where + "NULL values");
+            for (uint32_t v = 0; v < q.n_values; v++)
+                if (!q.values[v]) return fail(KS_ERR_INVALID, where + "NULL value");
+            int64_t x;
+            if (op == "In" || op == "NotIn") {
+                if (!q.n_values) return fail(KS_ERR_INVALID, where + "no values");
+            } else if (op == "Exists" || op == "DoesNotExist") {
+                if (q.n_values) return fail(KS_ERR_INVALID, where + "values given");
+            } else if (op == "Gt" || op == "Lt") {
+                if (q.n_values != 1 || !parse_int64(q.values[0], &x))
+                    return fail(KS_ERR_INVALID, where + "needs exactly one integer value");
+            } else {
+                return fail(KS_ERR_INVALID, where + "unknown operator");
+            }
+            if (std::find(keys.begin(), keys.end(), q.key) == keys.end()) keys.emplace_back(q.key);
+        }
+    }
+    if (keys.size() > KS_NODE_RULES_MAX_KEYS)
+        return fail(KS_ERR_RANGE, std::to_string(keys.size()) + " node-affinity keys (at most " +
+                                      std::to_string(KS_NODE_RULES_MAX_KEYS) + ")");
+    // taints: the distinct (key, value, effect) triples of the store's nodes, numbered in node order
+    std::vector<std::array<std::string, 3>> triples;
+    out->hard.assign(N, 0);
+    out->soft.assign(N, 0);
+    for (uint32_t n = 0; n < N; n++) {
+        const auto it = c->taints.find(c->names.str(c->idx2nameid[n]));
+        if (it == c->taints.end()) continue;
+        for (const auto& t : it->second) {
+            size_t b = std::find(triples.begin(), triples.end(), t) - triples.begin();
+            if (b == triples.size()) {
+                if (b == KS_NODE_RULES_MAX_TAINTS)
+                    return fail(KS_ERR_RANGE, "more than 64 distinct taints on the store's nodes");
+                triples.push_back(t);
+            }
+            (t[2] == "PreferNoSchedule" ? out->soft : out->hard)[n] |= 1ull << b;
+        }
+    }
+    out->tol_h.assign(G, 0);
+    out->tol_s.assign(G, 0);
+    for (uint32_t g = 0; g < G && in->toleration_offset; g++)
+        for (size_t b = 0; b < triples.size(); b++)
+            for (uint64_t i = in->toleration_offset[g]; i < in->toleration_offset[g + 1]; i++) {
+                const ksh_toleration& t = in->tolerations[i];
+                if (!tolerates(t, triples[b])) continue;
+                if (triples[b][2] != "PreferNoSchedule") out->tol_h[g] |= 1ull << b;
+                else if (!*nz(t.effect) || std::string(t.effect) == "PreferNoSchedule") out->tol_s[g] |= 1ull << b;
+            }
+    // node affinity: each key's domains over the store, each requirement a set over them plus the "absent" bit
+    std::vector<std::vector<std::string>> values(keys.size());
+    out->dom.assign(keys.size(), std::vector<int32_t>(N));
+    for (size_t k = 0; k < keys.size(); k++) {
+        std::vector<uint32_t> pids;
+        topology_domains(c, keys[k].c_str(), out->dom[k].data(), &pids);
+        for (const uint32_t pid : pids) {
+            const char* key = c->pairs.str(pid);
+            values[k].emplace_back(key + std::strlen(key) + 1);
+        }
+    }
+    out->set_off.push_back(0);
+    out->term_off.push_back(0);
+    for (uint32_t t = 0; t < T; t++) {
+        for (uint64_t i = in->term_req_offset[t]; i < in->term_req_offset[t + 1]; i++) {
+            const ksh_node_selector_requirement& q = in->requirements[i];
+            const uint32_t k = (uint32_t)(std::find(keys.begin(), keys.end(), q.key) - keys.begin());
+            const uint64_t D = values[k].size(), base = out->sets.size();
+            out->sets.resize(base + (D + 64) / 64, 0);
+            const std::string op = q.op;
+            int64_t lim = 0;
+            if (op == "Gt" || op == "Lt") parse_int64(q.values[0], &lim);
+            for (uint64_t d = 0; d <= D; d++) {
+                bool in_set;
+                if (d == D) { // the node lacks the key
+                    in_set = op == "NotIn" || op == "DoesNotExist";
+                } else {
+                    const std::string& v = values[k][d];
+                    bool listed = false;
+                    for (uint32_t j = 0; j < q.n_values; j++) listed |= v == q.values[j];
+                    int64_t x;
+                    in_set = op == "In"       ? listed
+                             : op == "NotIn"  ? !listed
+                             : op == "Exists" ? true
+                             : op == "Gt"     ? parse_int64(v.c_str(), &x) && x > lim
+                             : op == "Lt"     ? parse_int64(v.c_str(), &x) && x < lim
+                                              : false;
+                }
+                if (in_set) out->sets[base + d / 64] |= 1ull << (d % 64);
+            }
+            out->set_off.push_back(out->sets.size());
+            out->expr_key.push_back(k);
+        }
+        out->term_off.push_back((uint32_t)out->expr_key.size());
+        out->owner.push_back(in->term_owner[t]);
+        out->term_w.push_back(in->term_weight[t]);
+    }
+    ks_node_rules& r = out->r;
+    r.n_taints = (uint32_t)triples.size();
+    r.node_taint_hard = out->hard.data();
+    r.node_taint_soft = out->soft.data();
+    r.tolerate_hard = out->tol_h.data();
+    r.tolerate_soft = out->tol_s.data();
+    r.n_keys = (uint32_t)keys.size();
+    for (size_t k = 0; k < keys.size(); k++) {
+        r.n_domains[k] = (uint32_t)values[k].size();
+        r.node_domain[k] = out->dom[k].data();
+    }
+    r.n_exprs = (uint32_t)out->expr_key.size();
+    r.expr_key = out->expr_key.data();
+    r.expr_set_offset = out->set_off.data();
+    r.expr_set = out->sets.data();
+    r.n_terms = T;
+    r.term_owner = out->owner.data();
+    r.term_weight = out->term_w.data();
+    r.term_expr_offset = out->term_off.data();
+    r.weight_taint = in == &none ? 3 : in->weight_taint;
+    r.weight_node_affinity = in == &none ? 2 : in->weight_node_affinity;
+    return KS_OK;
+}
+
 // reconcile() under topology spread: ksh_reconcile_batch's filtering, then ks_spread_bind over the pods that go to the
 // device, each in its group.  Group g's existing pods under key k count when their node is in the store and carries key k
 // and every key g constrains.  With aff set (ksh_reconcile_affinity), ks_affinity_bind with its terms and the existing
@@ -1722,7 +1912,8 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
                             const uint32_t* min_domains, const char* const* existing_node_names,
                             const uint64_t* existing_offset, const ksh_pod_affinity* aff, int policy, int32_t* out_status,
                             int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off,
-                            const ks_bind_scoring* sc = nullptr) {
+                            const ks_bind_scoring* sc = nullptr, const ksh_node_rules* nr = nullptr,
+                            bool nodes = false) {
     if (!c || !topology_keys || (n && (!pods || !group || !out_status || !out_node_idx)) || (n_groups && !max_skew && !aff))
         return fail(KS_ERR_INVALID, "NULL argument");
     if (K == 0 || K > KS_SPREAD_MAX_KEYS)
@@ -1740,7 +1931,8 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     if (aff && aff->n_existing && (!aff->existing_group || !aff->existing_node_name))
         return fail(KS_ERR_INVALID, "NULL existing_group or existing_node_name");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    int rc = sc    ? device_ready(c, ks_profile_bind, "ks_profile_bind")
+    int rc = nodes ? device_ready(c, ks_node_bind, "ks_node_bind")
+             : sc  ? device_ready(c, ks_profile_bind, "ks_profile_bind")
              : aff ? device_ready(c, ks_affinity_bind, "ks_affinity_bind")
                    : device_ready(c, ks_spread_bind, "ks_spread_bind");
     if (rc) return rc;
@@ -1755,6 +1947,11 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
         todo.push_back(i);
         sub.push_back(pods[i]);
         sub_group.push_back(group[i]);
+    }
+    CompiledNodeRules cr;
+    if (nodes) { // compiled before anything is bound, so a bad rule fails the whole call
+        rc = compile_node_rules(c, n_groups, nr, &cr);
+        if (rc) return rc;
     }
     if (todo.empty()) return KS_OK;
     ks_pods kp;
@@ -1791,7 +1988,7 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     sp.min_domains = min_domains;
     sp.existing = existing_offset ? existing.data() : nullptr;
     std::vector<int32_t> idx(sub.size(), -1);
-    const size_t R = aff ? 2 : 1; // refusal words per pod: spread, then affinity
+    const size_t R = nodes ? 4 : aff ? 2 : 1; // refusal words per pod: [taint, node affinity,] spread, then affinity
     std::vector<uint32_t> refused(sub.size() * R, 0);
     if (aff) {
         ks_pod_affinity pa{aff->n_terms, aff->owner, aff->kind, aff->key, aff->target_offset, aff->target, 0, nullptr,
@@ -1806,7 +2003,9 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
         pa.n_existing = eg.size();
         pa.existing_group = eg.data();
         pa.existing_node = en.data();
-        rc = sc ? ks_profile_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, policy, idx.data(), nullptr,
+        rc = nodes ? ks_node_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, &cr.r, policy, idx.data(),
+                                  nullptr, nullptr, refused.data(), nullptr, nullptr)
+             : sc ? ks_profile_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, policy, idx.data(), nullptr,
                                   nullptr, refused.data(), nullptr, nullptr)
                 : ks_affinity_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, policy, idx.data(), nullptr,
                                    refused.data(), nullptr);
@@ -1819,14 +2018,17 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
         return rc;
     }
     StringList bodies{json, cap};
+    const size_t F = nodes ? 2 : 0; // the spread and affinity words follow the two node-rule words
     for (size_t k = 0; k < todo.size(); k++) {
         const uint64_t i = todo[k];
         if (idx[k] >= 0)
             commit_bind(c, &pods[i], idx[k], kp.req_cpu[k], kp.req_mem[k], &out_status[i], &out_node_idx[i], bodies,
                         json && out_json_off ? &out_json_off[i] : nullptr);
-        else if (refused[k * R] > 0)
+        else if (nodes && refused[k * R] + refused[k * R + 1] > 0 && refused[k * R + 2] == 0 && refused[k * R + 3] == 0)
+            out_status[i] = KSH_RECONCILE_NODE_RULES_UNSATISFIED;
+        else if (refused[k * R + F] > 0)
             out_status[i] = KSH_RECONCILE_SPREAD_UNSATISFIED;
-        else if (aff && refused[k * R + 1] > 0)
+        else if (aff && refused[k * R + F + 1] > 0)
             out_status[i] = KSH_RECONCILE_AFFINITY_UNSATISFIED;
     }
     return KS_OK;
@@ -1865,6 +2067,88 @@ int ksh_reconcile_profile(ksh_context* c, const ks_pod_obj* pods, uint64_t n, co
     return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
                             existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
                             out_json_off, scoring);
+}
+KSH_CATCH
+
+int ksh_context_set_node_taints(ksh_context* c, const char* const* node_names, const uint64_t* taint_offset,
+                                const ksh_taint* taints, uint64_t n) try {
+    if (!c || (n && (!node_names || !taint_offset)) || (n && taint_offset[n] && !taints))
+        return fail(KS_ERR_INVALID, "NULL argument");
+    for (uint64_t i = 0; i < n; i++) {
+        if (!node_names[i]) return fail(KS_ERR_INVALID, "NULL node name");
+        if (taint_offset[i + 1] < taint_offset[i]) return fail(KS_ERR_INVALID, "taint offsets decrease");
+        for (uint64_t t = taint_offset[i]; t < taint_offset[i + 1]; t++) {
+            const std::string e = nz(taints[t].effect);
+            if (!taints[t].key || !*taints[t].key || (e != "NoSchedule" && e != "PreferNoSchedule" && e != "NoExecute"))
+                return fail(KS_ERR_INVALID, "taint " + std::to_string(t) + ": empty key or effect \"" + e + "\"");
+        }
+    }
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    for (uint64_t i = 0; i < n; i++) {
+        if (node_index_of(c, node_names[i]) < 0) continue; // unknown: ignored
+        auto& list = c->taints[node_names[i]];
+        list.clear();
+        for (uint64_t t = taint_offset[i]; t < taint_offset[i + 1]; t++)
+            list.push_back({taints[t].key, nz(taints[t].value), taints[t].effect});
+    }
+    return KS_OK;
+}
+KSH_CATCH
+
+int ksh_compile_node_rules(ksh_context* c, uint32_t G, const ksh_node_rules* rules, uint8_t* out_hard,
+                           uint8_t* out_affinity, uint32_t* out_soft, uint32_t* out_preferred) try {
+    if (!c) return fail(KS_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    CompiledNodeRules cr;
+    const int rc = compile_node_rules(c, G, rules, &cr);
+    if (rc) return rc;
+    const ks_node_rules& r = cr.r;
+    const uint32_t N = c->N;
+    auto match = [&](uint32_t t, uint32_t n) {
+        if (r.term_expr_offset[t + 1] == r.term_expr_offset[t]) return false; // no expression: matches nothing
+        for (uint32_t x = r.term_expr_offset[t]; x < r.term_expr_offset[t + 1]; x++) {
+            const uint32_t k = r.expr_key[x];
+            const int32_t d = r.node_domain[k][n];
+            const uint64_t b = d < 0 ? r.n_domains[k] : (uint64_t)d;
+            if (!(r.expr_set[r.expr_set_offset[x] + b / 64] >> (b % 64) & 1)) return false;
+        }
+        return true;
+    };
+    for (uint32_t g = 0; g < G; g++)
+        for (uint32_t n = 0; n < N; n++) {
+            const uint64_t i = (uint64_t)g * N + n;
+            if (out_hard) out_hard[i] = (r.node_taint_hard[n] & ~r.tolerate_hard[g]) != 0;
+            if (out_soft) out_soft[i] = (uint32_t)__builtin_popcountll(r.node_taint_soft[n] & ~r.tolerate_soft[g]);
+            bool has_req = false, req_ok = false;
+            uint32_t pref = 0;
+            for (uint32_t t = 0; t < r.n_terms; t++) {
+                if (r.term_owner[t] != (int32_t)g) continue;
+                const bool ok = match(t, n);
+                if (r.term_weight[t] == 0) {
+                    has_req = true;
+                    req_ok |= ok;
+                } else if (ok) {
+                    pref += r.term_weight[t];
+                }
+            }
+            if (out_affinity) out_affinity[i] = !has_req || req_ok;
+            if (out_preferred) out_preferred[i] = pref;
+        }
+    return KS_OK;
+}
+KSH_CATCH
+
+int ksh_reconcile_nodes(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
+                        const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
+                        const uint32_t* min_domains, const char* const* existing_node_names,
+                        const uint64_t* existing_offset, const ksh_pod_affinity* aff, const ks_bind_scoring* scoring,
+                        const ksh_node_rules* rules, int policy, int32_t* out_status, int32_t* out_node_idx, char* json,
+                        size_t cap, int64_t* out_json_off) try {
+    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
+    const ksh_pod_affinity none{};
+    return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
+                            existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
+                            out_json_off, scoring, rules, true);
 }
 KSH_CATCH
 

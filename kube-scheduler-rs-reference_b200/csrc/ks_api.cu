@@ -12,6 +12,7 @@
 #include <mutex>
 #include <thread>
 #include <algorithm>
+#include <map>
 #include <vector>
 
 #include "ks_bitpar.h"
@@ -1973,13 +1974,125 @@ static int compile_affinity(const ks_pod_affinity* f, uint32_t G, uint32_t K, co
     return sc ? compile_scoring(f, sc, G, K, Dk, pl) : KS_OK;
 }
 
+// ks_node_bind's rules compiled on the host (include/ksched.h, DESIGN.md 5p): the class of each group (group -1 at 0),
+// and per class its tolerations and its terms with their expressions, which point into the caller's expr_set
+struct NodeRulesPlan {
+    std::vector<uint32_t> cls;               // [G + 1]
+    std::vector<uint64_t> ctol;              // [2C]: hard, soft
+    std::vector<uint32_t> cterm_off{0};      // [C + 1]
+    std::vector<uint32_t> cterm_w;           // [T']
+    std::vector<uint32_t> cexpr_off{0};      // [T' + 1]
+    std::vector<uint32_t> cexpr_key;         // [X']
+    std::vector<uint64_t> cexpr_set;         // [X']: word offset of the set in expr_set
+    uint64_t set_words = 0;                  // expr_set words the sets use
+    uint32_t C = 0;
+};
+
+static int compile_node_rules(const ks_node_rules* r, uint32_t G, uint32_t N, NodeRulesPlan* pl) {
+    if (r->weight_taint > 100 || r->weight_node_affinity > 100)
+        return fail(KS_ERR_INVALID, "plugin weights %u and %u (at most 100)", r->weight_taint, r->weight_node_affinity);
+    if (r->n_taints > KS_NODE_RULES_MAX_TAINTS) return fail(KS_ERR_RANGE, "%u taints (at most 64)", r->n_taints);
+    if (r->n_keys > KS_NODE_RULES_MAX_KEYS)
+        return fail(KS_ERR_RANGE, "%u node-affinity keys (at most %u)", r->n_keys, KS_NODE_RULES_MAX_KEYS);
+    const uint64_t valid = r->n_taints == 64 ? ~0ull : (1ull << r->n_taints) - 1;
+    const struct { const uint64_t* m; uint32_t n; const char* what; } masks[] = {
+        {r->node_taint_hard, N, "node_taint_hard"}, {r->node_taint_soft, N, "node_taint_soft"},
+        {r->tolerate_hard, G, "tolerate_hard"}, {r->tolerate_soft, G, "tolerate_soft"}};
+    for (const auto& m : masks)
+        if (m.m)
+            for (uint32_t i = 0; i < m.n; i++)
+                if (m.m[i] & ~valid) return fail(KS_ERR_INVALID, "%s[%u]: a taint bit at or above %u", m.what, i, r->n_taints);
+    for (uint32_t k = 0; k < r->n_keys; k++) {
+        if (N && !r->node_domain[k]) return fail(KS_ERR_INVALID, "NULL node_domain of node-affinity key %u", k);
+        for (uint32_t n = 0; n < N; n++)
+            if (r->node_domain[k][n] < -1 || r->node_domain[k][n] >= (int64_t)r->n_domains[k])
+                return fail(KS_ERR_INVALID, "node-affinity key %u, node %u: domain %d outside [-1, %u)", k, n,
+                            r->node_domain[k][n], r->n_domains[k]);
+    }
+    const uint32_t X = r->n_exprs, T = r->n_terms;
+    if (X && (!r->expr_key || !r->expr_set_offset || !r->expr_set))
+        return fail(KS_ERR_INVALID, "NULL expr_key, expr_set_offset or expr_set");
+    if (T && (!r->term_owner || !r->term_weight || !r->term_expr_offset))
+        return fail(KS_ERR_INVALID, "NULL term_owner, term_weight or term_expr_offset");
+    for (uint32_t x = 0; x < X; x++) {
+        const uint32_t k = r->expr_key[x];
+        if (k >= r->n_keys) return fail(KS_ERR_INVALID, "expression %u: key %u (the call has %u)", x, k, r->n_keys);
+        const uint64_t o = r->expr_set_offset[x], o1 = r->expr_set_offset[x + 1], D = r->n_domains[k];
+        if (o1 < o || o1 - o != (D + 64) / 64)
+            return fail(KS_ERR_INVALID, "expression %u: %llu set words (key %u needs %llu)", x,
+                        (unsigned long long)(o1 < o ? 0 : o1 - o), k, (unsigned long long)((D + 64) / 64));
+        if (o1 > KS_NODE_RULES_MAX_WORDS)
+            return fail(KS_ERR_RANGE, "expression %u: set words beyond 2^26", x);
+        const uint64_t top = r->expr_set[o1 - 1], used = (D + 1) % 64;
+        if (used && (top >> used)) return fail(KS_ERR_INVALID, "expression %u: a set bit above D_k = %llu", x,
+                                               (unsigned long long)D);
+        pl->set_words = std::max(pl->set_words, o1);
+    }
+    std::vector<std::vector<uint32_t>> own(G);
+    for (uint32_t t = 0; t < T; t++) {
+        if (r->term_owner[t] < 0 || r->term_owner[t] >= (int64_t)G)
+            return fail(KS_ERR_INVALID, "node-affinity term %u: owner %d outside [0, %u)", t, r->term_owner[t], G);
+        if (r->term_weight[t] > 100) return fail(KS_ERR_INVALID, "node-affinity term %u: weight %u (0 to 100)", t,
+                                                 r->term_weight[t]);
+        if (r->term_expr_offset[t + 1] < r->term_expr_offset[t] || r->term_expr_offset[t + 1] > X)
+            return fail(KS_ERR_INVALID, "node-affinity term %u: expression offsets decrease or pass %u", t, X);
+        own[r->term_owner[t]].push_back(t);
+    }
+    for (uint32_t g = 0; g < G; g++) {
+        uint32_t pref = 0;
+        for (const uint32_t t : own[g]) pref += r->term_weight[t] != 0;
+        if (pref > KS_NODE_RULES_MAX_PREFERRED)
+            return fail(KS_ERR_RANGE, "group %u: %u preferred node-affinity terms (at most %u)", g, pref,
+                        KS_NODE_RULES_MAX_PREFERRED);
+    }
+    // classes: the distinct signatures (tolerations, then each term's weight and expressions with their sets)
+    std::map<std::vector<uint64_t>, uint32_t> seen;
+    pl->cls.assign(G + 1, 0);
+    auto add_class = [&](int64_t g) {
+        std::vector<uint64_t> sig{g < 0 || !r->tolerate_hard ? 0 : r->tolerate_hard[g],
+                                  g < 0 || !r->tolerate_soft ? 0 : r->tolerate_soft[g]};
+        if (g >= 0)
+            for (const uint32_t t : own[g]) {
+                sig.push_back(r->term_weight[t]);
+                sig.push_back(r->term_expr_offset[t + 1] - r->term_expr_offset[t]);
+                for (uint32_t x = r->term_expr_offset[t]; x < r->term_expr_offset[t + 1]; x++) {
+                    sig.push_back(r->expr_key[x]);
+                    sig.insert(sig.end(), r->expr_set + r->expr_set_offset[x], r->expr_set + r->expr_set_offset[x + 1]);
+                }
+            }
+        const auto it = seen.find(sig);
+        if (it != seen.end()) return it->second;
+        const uint32_t c = pl->C++;
+        seen.emplace(std::move(sig), c);
+        pl->ctol.push_back(g < 0 || !r->tolerate_hard ? 0 : r->tolerate_hard[g]);
+        pl->ctol.push_back(g < 0 || !r->tolerate_soft ? 0 : r->tolerate_soft[g]);
+        if (g >= 0)
+            for (const uint32_t t : own[g]) {
+                pl->cterm_w.push_back(r->term_weight[t]);
+                for (uint32_t x = r->term_expr_offset[t]; x < r->term_expr_offset[t + 1]; x++) {
+                    pl->cexpr_key.push_back(r->expr_key[x]);
+                    pl->cexpr_set.push_back(r->expr_set_offset[x]);
+                }
+                pl->cexpr_off.push_back((uint32_t)pl->cexpr_key.size());
+            }
+        pl->cterm_off.push_back((uint32_t)pl->cterm_w.size());
+        return c;
+    };
+    pl->cls[0] = add_class(-1);
+    for (uint32_t g = 0; g < G; g++) pl->cls[g + 1] = add_class(g);
+    if ((uint64_t)pl->C * N > KS_NODE_RULES_MAX_WORDS)
+        return fail(KS_ERR_RANGE, "%u node-rule classes x %u nodes (at most 2^26 rule words)", pl->C, N);
+    return KS_OK;
+}
+
 // ks_spread_bind, and with aff set ks_affinity_bind (then max_skew may be NULL and out_refused holds 2P words), and with
-// aff and sc set ks_profile_bind (out_parts [3P] and out_soft_count [G * S] may be given)
+// aff and sc set ks_profile_bind (out_parts [3P] and out_soft_count [G * S] may be given), and with nr set as well
+// ks_node_bind (out_parts [5P], out_refused [4P])
 static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
                        const ks_spread_multi* spread, const ks_pod_affinity* aff, int policy, int32_t* out_node_idx,
                        int64_t* out_score, uint32_t* out_refused, uint32_t* out_domain_count,
                        const ks_bind_scoring* sc = nullptr, int64_t* out_parts = nullptr,
-                       uint32_t* out_soft_count = nullptr) {
+                       uint32_t* out_soft_count = nullptr, const ks_node_rules* nr = nullptr) {
     int rc = check_pods(s, pods);
     if (rc) return rc;
     if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "%s takes host-space pods", call);
@@ -2043,7 +2156,17 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         }
         if (rc) return rc;
     }
-    const uint64_t R = aff ? 2 : 1; // refusal words per pod
+    NodeRulesPlan nplan;
+    if (nr) {
+        try {
+            rc = compile_node_rules(nr, (uint32_t)G, N, &nplan);
+        } catch (...) {
+            return fail(KS_ERR_NOMEM, "out of host memory in %s", call);
+        }
+        if (rc) return rc;
+    }
+    const uint64_t R = nr ? 4 : aff ? 2 : 1; // refusal words per pod
+    const uint64_t PW = nr ? 5 : 3;          // parts per pod
     if (P == 0) return KS_OK;
     if (N == 0) { // no node: nothing is placed, every count is existing
         memset(out_node_idx, 0xff, P * 4);
@@ -2054,7 +2177,7 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
                 if (spread->existing) memcpy(c, spread->existing, GS * 4);
                 else memset(c, 0, GS * 4);
             }
-        if (out_parts) memset(out_parts, 0, P * 24);
+        if (out_parts) memset(out_parts, 0, P * PW * 8);
         return KS_OK;
     }
     std::lock_guard<std::mutex> lk(s->mu);
@@ -2119,7 +2242,7 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     const auto iupd_off = h.in<uint32_t>(nullptr, plan.iupd_off.size());
     const auto iupd = h.in<uint32_t>(nullptr, plan.iupd.size());
     const auto icoef = h.in<int32_t>(nullptr, plan.icoef.size());
-    const auto parts = h.out(out_parts, Q * 3 * P);
+    const auto parts = h.out(out_parts, Q * PW * P);
     const auto scnt = h.out(out_soft_count, Q * GS);
     const auto icnt = h.work<int64_t>(plan.iwords, 16);
     const auto bits = h.work<uint32_t>(2ull * q.BW, 16);
@@ -2127,10 +2250,40 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     const auto pdom = h.work<uint32_t>(Q * a.grid * KS_SPREAD_MAX_KEYS), plack = h.work<uint32_t>(Q * a.grid);
     const auto pimin = h.work<int64_t>(Q * a.grid), pimax = h.work<int64_t>(Q * a.grid);
     const auto ppmin = h.work<int64_t>(Q * a.grid), ppmax = h.work<int64_t>(Q * a.grid);
+    // ks_node_bind: the compiled classes, the rule keys' domains, the taints and the sets; one rule word per (class, node)
+    const uint64_t NR1 = nr ? 1 : 0;
+    const uint32_t KN = nr ? nr->n_keys : 0;
+    const auto ncls = h.in<uint32_t>(nullptr, nplan.cls.size());
+    const auto ctol = h.in<uint64_t>(nullptr, nplan.ctol.size());
+    const auto cterm_off = h.in<uint32_t>(nullptr, NR1 * nplan.cterm_off.size());
+    const auto cterm_w = h.in<uint32_t>(nullptr, nplan.cterm_w.size());
+    const auto cexpr_off = h.in<uint32_t>(nullptr, NR1 * nplan.cexpr_off.size());
+    const auto cexpr_key = h.in<uint32_t>(nullptr, nplan.cexpr_key.size());
+    const auto cexpr_set = h.in<uint64_t>(nullptr, nplan.cexpr_set.size());
+    const auto nset = h.in(nr ? nr->expr_set : nullptr, nplan.set_words);
+    const auto ndom = h.in<int32_t>(nullptr, (uint64_t)KN * N);
+    const auto taint_hard = h.in(nr ? nr->node_taint_hard : nullptr, NR1 * N); // NULL: zeros, filled below
+    const auto taint_soft = h.in(nr ? nr->node_taint_soft : nullptr, NR1 * N);
+    const auto nrules = h.work<uint32_t>((uint64_t)nplan.C * N);
+    const auto refused2 = h.work<uint32_t>(NR1 * 2 * P); // ks_profile_bind's two words, before the four are written
+    const auto ptref = h.work<uint32_t>(NR1 * a.grid), pnref = h.work<uint32_t>(NR1 * a.grid);
+    const auto ptmax = h.work<uint32_t>(NR1 * a.grid), pnmax = h.work<uint32_t>(NR1 * a.grid);
     auto put = [&](Staged<uint32_t> d, const std::vector<uint32_t>& v) {
         if (!v.empty()) memcpy(h.host(d), v.data(), v.size() * 4);
     };
     CU_TRY(h.reserve(s));
+    if (nr) {
+        put(ncls, nplan.cls);
+        memcpy(h.host(ctol), nplan.ctol.data(), nplan.ctol.size() * 8);
+        put(cterm_off, nplan.cterm_off);
+        put(cterm_w, nplan.cterm_w);
+        put(cexpr_off, nplan.cexpr_off);
+        put(cexpr_key, nplan.cexpr_key);
+        if (!nplan.cexpr_set.empty()) memcpy(h.host(cexpr_set), nplan.cexpr_set.data(), nplan.cexpr_set.size() * 8);
+        for (uint32_t k = 0; k < KN; k++) memcpy(h.host(ndom) + (size_t)k * N, nr->node_domain[k], (size_t)N * 4);
+        if (!nr->node_taint_hard) memset(h.host(taint_hard), 0, (size_t)N * 8);
+        if (!nr->node_taint_soft) memset(h.host(taint_soft), 0, (size_t)N * 8);
+    }
     if (sc) {
         if (!sc->soft_skew) memset(h.host(soft_skew), 0, G * K * 4);
         if (!sc->soft_all_keys) memset(h.host(soft_all), 1, G);
@@ -2225,16 +2378,44 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         q.wspread = sc->weight_spread;
         q.waff = sc->weight_affinity;
     }
+    if (nr) {
+        q.b.out_refused = h.dev(refused2);
+        q.out_refused4 = h.dev(refused);
+        q.ncls = h.dev(ncls);
+        q.nrules = h.dev(nrules);
+        q.C = nplan.C;
+        q.KN = KN;
+        for (uint32_t k = 0; k < KN; k++) q.NDk[k] = nr->n_domains[k];
+        q.ndom = h.dev(ndom);
+        q.taint_hard = h.dev(taint_hard);
+        q.taint_soft = h.dev(taint_soft);
+        q.ctol = h.dev(ctol);
+        q.cterm_off = h.dev(cterm_off);
+        q.cterm_w = h.dev(cterm_w);
+        q.cexpr_off = h.dev(cexpr_off);
+        q.cexpr_key = h.dev(cexpr_key);
+        q.cexpr_set = h.dev(cexpr_set);
+        q.nset = h.dev(nset);
+        q.ptref = h.dev(ptref);
+        q.pnref = h.dev(pnref);
+        q.ptmax = h.dev(ptmax);
+        q.pnmax = h.dev(pnmax);
+        q.wtaint = nr->weight_taint;
+        q.wnaff = nr->weight_node_affinity;
+        q.rules_grid = (uint32_t)std::max<uint64_t>(
+            1, std::min<uint64_t>(((uint64_t)nplan.C * N + 255) / 256, 4ull * (uint64_t)s->sms));
+    }
     s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
     s->version++;
-    cudaError_t e = sc    ? launch_profile_bind(q, plan.words, W, st)
+    cudaError_t e = nr    ? launch_node_bind(q, plan.words, W, st)
+                    : sc  ? launch_profile_bind(q, plan.words, W, st)
                     : aff ? launch_affinity_bind(a, plan.words, W, st)
                           : launch_spread_bind(a, W, st);
     if (e != cudaSuccess)
-        return fail(KS_ERR_CUDA, "%s launch failed: %s", sc ? "profile bind" : aff ? "affinity bind" : "spread bind",
-                    cudaGetErrorString(e));
+        return fail(KS_ERR_CUDA, "%s launch failed: %s",
+                    nr ? "node bind" : sc ? "profile bind" : aff ? "affinity bind" : "spread bind", cudaGetErrorString(e));
     CU_TRY(h.finish(st));
-    s->last_path = sc ? "profile_bind" : aff ? "affinity_bind" : "spread_bind";
+    s->last_path = nr ? "node_bind" : sc ? "profile_bind" : aff ? "affinity_bind" : "spread_bind";
     return KS_OK;
 }
 
@@ -2261,6 +2442,43 @@ int ks_profile_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, u
     const ks_pod_affinity none{};
     return bind_spread(s, "ks_profile_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
                        out_score, out_refused, out_domain_count, scoring, out_parts, out_soft_count);
+}
+
+int ks_node_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
+                 const ks_spread_multi* topo, const ks_pod_affinity* aff, const ks_bind_scoring* scoring,
+                 const ks_node_rules* rules, int policy, int32_t* out_node_idx, int64_t* out_score, int64_t* out_parts,
+                 uint32_t* out_refused, uint32_t* out_domain_count, uint32_t* out_soft_count) {
+    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
+    const ks_pod_affinity none{};
+    if (rules)
+        return bind_spread(s, "ks_node_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
+                           out_score, out_refused, out_domain_count, scoring, out_parts, out_soft_count, rules);
+    // K1: no rules is ks_profile_bind itself, its refusals and parts widened with zeros
+    const uint64_t P = pods ? pods->n : 0;
+    std::vector<uint32_t> ref;
+    std::vector<int64_t> parts;
+    try {
+        if (out_refused) ref.resize(2 * P);
+        if (out_parts) parts.resize(3 * P);
+    } catch (...) {
+        return fail(KS_ERR_NOMEM, "out of host memory in ks_node_bind");
+    }
+    const int rc = bind_spread(s, "ks_node_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
+                               out_score, out_refused ? ref.data() : nullptr, out_domain_count, scoring,
+                               out_parts ? parts.data() : nullptr, out_soft_count);
+    if (rc) return rc;
+    for (uint64_t p = 0; p < P; p++) {
+        if (out_refused) {
+            out_refused[4 * p] = out_refused[4 * p + 1] = 0;
+            out_refused[4 * p + 2] = ref[2 * p];
+            out_refused[4 * p + 3] = ref[2 * p + 1];
+        }
+        if (out_parts) {
+            for (int i = 0; i < 3; i++) out_parts[5 * p + i] = parts[3 * p + i];
+            out_parts[5 * p + 3] = out_parts[5 * p + 4] = 0;
+        }
+    }
+    return KS_OK;
 }
 
 // ---------------------------------------------------------------------------------------------- async streaming

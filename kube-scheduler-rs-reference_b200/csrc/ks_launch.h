@@ -301,9 +301,29 @@ struct ProfileBindArgs {
     uint32_t* pdom;                   // [grid * KS_SPREAD_MAX_KEYS] per-CTA partials: new domains per soft key
     uint32_t* plack;                  // [grid]: soft keys some non-ignored candidate lacks
     int64_t *pimin, *pimax, *ppmin, *ppmax; // [grid]: IPA raw and PodTopologySpread raw extremes
-    int64_t* out_parts;               // [3P]
+    int64_t* out_parts;               // [3P]; [5P] under ks_node_bind
     uint32_t wspread, waff;
+    // ks_node_bind (DESIGN.md 5p; read only by its kernels).  Rule word of (class c, node n) at nrules[c * N + n]:
+    // NR_REASON bits (0 pass, NR_TAINT, NR_AFFINITY), NR_AFF_OK, the PreferNoSchedule count at NR_TT_SHIFT and the
+    // preferred NodeAffinity raw at NR_NA_SHIFT.  Class c's terms [cterm_off[c], cterm_off[c + 1]): weight cterm_w (0 =
+    // required), expressions [cexpr_off[t], cexpr_off[t + 1]): key cexpr_key, set at word cexpr_set of nset.
+    const uint32_t* ncls;             // [G + 1]: the class of group g at g + 1, of group -1 at 0
+    uint32_t* nrules;                 // [C * N], written by k_node_rules_setup
+    uint32_t C, KN, NDk[KS_NODE_RULES_MAX_KEYS];
+    const int32_t* ndom;              // [KN * N]
+    const uint64_t *taint_hard, *taint_soft; // [N]
+    const uint64_t* ctol;             // [2C]: hard, soft tolerations
+    const uint32_t *cterm_off, *cterm_w, *cexpr_off, *cexpr_key;
+    const uint64_t *cexpr_set, *nset;
+    uint32_t *ptref, *pnref;          // [grid] per-CTA taint and node-affinity refusals
+    uint32_t *ptmax, *pnmax;          // [grid] per-CTA maxima of the two raws over the candidates
+    uint32_t* out_refused4;           // [4P]; out_refused of b is device scratch [2P]
+    uint32_t wtaint, wnaff, rules_grid;
 };
 constexpr int64_t PB_NOT_CAND = INT64_MIN;
 cudaError_t launch_profile_bind(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st);
+constexpr uint32_t NR_REASON = 3u, NR_TAINT = 1u, NR_AFFINITY = 2u, NR_AFF_OK = 4u, NR_TT_SHIFT = 3, NR_NA_SHIFT = 10;
+// ks_node_bind (ks_spread_bind.cu): k_node_rules_setup, then ks_profile_bind's launches with k_node_spread_setup and
+// k_node_bind_seq in place of k_spread_bind_setup and k_profile_bind_seq
+cudaError_t launch_node_bind(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st);
 } // namespace ks

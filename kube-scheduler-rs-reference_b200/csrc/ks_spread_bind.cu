@@ -14,6 +14,10 @@
 // AFF = false instances are the code k_spread_bind_seq always ran.
 // ks_profile_bind (DESIGN.md 5o) runs k_profile_bind_seq: the same filter and commit, with soft PodTopologySpread and
 // InterPodAffinity scores that need grid-wide reductions over the candidates before any node's total exists.
+// ks_node_bind (DESIGN.md 5p) first writes one rule word per (node-rule class, node) in k_node_rules_setup, then runs
+// k_node_spread_setup and k_node_bind_seq: the NR instances of the spread setup and of the profile passes, which read
+// that word per node for TaintToleration and NodeAffinity.  The NR = false instances are the code the existing kernels
+// always ran.
 #include "ks_internal.cuh"
 #include "ks_launch.h"
 
@@ -70,8 +74,10 @@ __device__ __forceinline__ uint32_t domains_at(const SpreadBindArgs& a, uint32_t
     return cta_sum(c, s);
 }
 
-template <int W>
-__global__ void __launch_bounds__(SBD_THREADS) k_spread_bind_setup(const SpreadBindArgs a) {
+// NR (ks_node_bind): a node is also eligible only when it passes the group's required node affinity (the NR_AFF_OK bit
+// of its rule word in the group's class row, nrules / ncls of ProfileBindArgs)
+template <int W, bool NR>
+__device__ __forceinline__ void spread_bind_setup(const SpreadBindArgs& a, const uint32_t* nrules, const uint32_t* ncls) {
     __shared__ uint32_t s_red[SBD_WARPS];
     const uint32_t tid = threadIdx.x;
     for (uint32_t g = blockIdx.x; g < a.G; g += gridDim.x) {
@@ -87,11 +93,13 @@ __global__ void __launch_bounds__(SBD_THREADS) k_spread_bind_setup(const SpreadB
             uint64_t sw[W];
 #pragma unroll
             for (int w = 0; w < W; w++) sw[w] = __ldg(a.gsel + (size_t)g * W + w);
+            const uint32_t* nrow = NR ? nrules + (size_t)__ldg(ncls + g + 1) * a.N : nullptr;
             for (uint32_t n = tid; n < a.N; n += SBD_THREADS) {
                 uint64_t miss = 0;
 #pragma unroll
                 for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
                 if (miss) continue;
+                if (NR && !(__ldg(nrow + n) & NR_AFF_OK)) continue;
                 int32_t d[KS_SPREAD_MAX_KEYS];
                 bool all = true;
 #pragma unroll
@@ -133,6 +141,11 @@ __global__ void __launch_bounds__(SBD_THREADS) k_spread_bind_setup(const SpreadB
         }
         __syncthreads(); // el and cnt of this group are final before the CTA's next group
     }
+}
+
+template <int W>
+__global__ void __launch_bounds__(SBD_THREADS) k_spread_bind_setup(const SpreadBindArgs a) {
+    spread_bind_setup<W, false>(a, nullptr, nullptr);
 }
 
 // Inter-pod affinity: one update entry of a pod bound at node n.  Entries of one list name distinct (group, key, kind)
@@ -448,12 +461,16 @@ struct ProfileFilter {
         cnt = a.cnt + (size_t)(g < 0 ? 0 : g) * a.S;
         first = g >= 0 && (__ldg(a.aflag + g) & AFF_SELF) && __ldcg(a.acnt + a.any_base + g) == 0;
     }
-    // 0: unfit (fit or selector), 1: refused by spread, 2: refused by rules 1-3, 3: candidate
-    __device__ __forceinline__ int test(const SpreadBindArgs& a, uint32_t n, int64_t fc, int64_t fm) const {
+    // 0: unfit (fit or selector), 1: refused by spread, 2: refused by rules 1-3, 3: candidate; NR (ks_node_bind) with
+    // the node's rule word rw: 4: refused by a taint, 5: refused by required node affinity, both before spread
+    template <bool NR = false>
+    __device__ __forceinline__ int test(const SpreadBindArgs& a, uint32_t n, int64_t fc, int64_t fm,
+                                        uint32_t rw = 0) const {
         uint64_t miss = 0;
 #pragma unroll
         for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
         if (!(rc <= fc && rm <= fm && miss == 0)) return 0;
+        if (NR && (rw & NR_REASON)) return 3 + (int)(rw & NR_REASON);
         bool ok = true;
 #pragma unroll
         for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
@@ -528,13 +545,33 @@ struct ProfileShared {
     int32_t bidx;
 };
 
+// ks_node_bind's share of one CTA's state for one pod: per-warp refusals and raw maxima, then the grid's maxima
+struct NodeShared {
+    uint32_t tref[SBD_WARPS], nref[SBD_WARPS], tmax[SBD_WARPS], nmax[SBD_WARPS];
+    uint32_t gtmax, gnmax;
+};
+
+// TaintToleration and NodeAffinity of a candidate from its rule word and the maxima over F (include/ksched.h, 5p)
+__device__ __forceinline__ void node_parts(uint32_t rw, const NodeShared& ns, int64_t& tt, int64_t& na) {
+    const int64_t t = rw >> NR_TT_SHIFT & 127u, v = rw >> NR_NA_SHIFT;
+    tt = ns.gtmax == 0 ? 100 : 100 - 100 * t / ns.gtmax;
+    na = ns.gnmax == 0 ? 0 : 100 * v / ns.gnmax;
+}
+
+// The row of rule words of the class of group g
+__device__ __forceinline__ const uint32_t* node_row(const ProfileBindArgs& a, int32_t g) {
+    return a.nrules + (size_t)__ldg(a.ncls + g + 1) * a.b.N;
+}
+
 // Pass 1: the filter; per candidate its IPA raw into iraw[], and for a group with soft keys the domains of the
 // non-ignored candidates: a node-per-domain key counts its nodes, a domain below PB_SH_WORDS * 32 is marked in the CTA's
 // bitmap and merged into the parity's global bitmap once per CTA, a higher one is marked there directly.  Each new
 // bit counts one domain, so the partials add up to the distinct domains.  The other parity's bitmap is cleared.
-template <int W>
+// NR (ks_node_bind): the node's rule word first; the taint and node-affinity refusals and, over the candidates, the
+// maxima of both raws into the CTA's partials.
+template <int W, bool NR = false>
 __device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t p, uint32_t n0, uint32_t n1,
-                                              ProfileShared& sh) {
+                                              ProfileShared& sh, NodeShared* ns = nullptr) {
     const SpreadBindArgs& b = a.b;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const ProfileFilter<W> f(b, p);
@@ -555,13 +592,24 @@ __device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t
     __syncthreads();
     uint32_t refused = 0, arefused = 0, lack = 0, ndom[KS_SPREAD_MAX_KEYS] = {0, 0, 0, 0};
     int64_t imin = INT64_MAX, imax = INT64_MIN;
+    const uint32_t* nrow = NR ? node_row(a, f.g) : nullptr;
+    uint32_t tref = 0, nref = 0, tmax = 0, nmax = 0;
     for (uint32_t n = n0 + tid; n < n1; n += SBD_THREADS) {
-        const int r = f.test(b, n, __ldcg(b.free_cpu + n), __ldcg(b.free_mem + n));
+        const uint32_t rw = NR ? __ldg(nrow + n) : 0u;
+        const int r = f.template test<NR>(b, n, __ldcg(b.free_cpu + n), __ldcg(b.free_mem + n), rw);
         refused += r == 1;
         arefused += r == 2;
+        if constexpr (NR) {
+            tref += r == 4;
+            nref += r == 5;
+        }
         if (r != 3) {
             a.iraw[n] = PB_NOT_CAND;
             continue;
+        }
+        if constexpr (NR) {
+            tmax = max(tmax, rw >> NR_TT_SHIFT & 127u);
+            nmax = max(nmax, rw >> NR_NA_SHIFT);
         }
         int64_t raw = 0;
 #pragma unroll
@@ -599,6 +647,18 @@ __device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t
         sh.aref[warp] = arefused;
         if (lack) atomicOr(&sh.lack, lack);
     }
+    if constexpr (NR) {
+        tref = __reduce_add_sync(0xffffffffu, tref);
+        nref = __reduce_add_sync(0xffffffffu, nref);
+        tmax = __reduce_max_sync(0xffffffffu, tmax);
+        nmax = __reduce_max_sync(0xffffffffu, nmax);
+        if (lane == 0) {
+            ns->tref[warp] = tref;
+            ns->nref[warp] = nref;
+            ns->tmax[warp] = tmax;
+            ns->nmax[warp] = nmax;
+        }
+    }
     if (sk) {
 #pragma unroll
         for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) {
@@ -631,6 +691,20 @@ __device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t
         a.plack[blockIdx.x] = sh.lack;
 #pragma unroll
         for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) a.pdom[(size_t)blockIdx.x * KS_SPREAD_MAX_KEYS + k] = sh.dom[k];
+        if constexpr (NR) {
+            uint32_t tr = 0, nr = 0, tm = 0, nm = 0;
+#pragma unroll
+            for (uint32_t w = 0; w < SBD_WARPS; w++) {
+                tr += ns->tref[w];
+                nr += ns->nref[w];
+                tm = max(tm, ns->tmax[w]);
+                nm = max(nm, ns->nmax[w]);
+            }
+            a.ptref[blockIdx.x] = tr;
+            a.pnref[blockIdx.x] = nr;
+            a.ptmax[blockIdx.x] = tm;
+            a.pnmax[blockIdx.x] = nm;
+        }
     }
 }
 
@@ -703,9 +777,11 @@ __device__ __forceinline__ void profile_parts(const ProfileBindArgs& a, uint32_t
     }
 }
 
-// Pass 3: merge the extremes, the totals of the slice's candidates and the argmax partial
+// Pass 3: merge the extremes, the totals of the slice's candidates and the argmax partial.  NR: also the maxima of the
+// two node-rule raws, and both weighted scores in the total.
+template <bool NR = false>
 __device__ __forceinline__ void profile_pass3(const ProfileBindArgs& a, uint32_t p, uint32_t n0, uint32_t n1,
-                                              ProfileShared& sh) {
+                                              ProfileShared& sh, NodeShared* ns = nullptr) {
     const SpreadBindArgs& b = a.b;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int32_t g = __ldg(b.group + p);
@@ -733,18 +809,37 @@ __device__ __forceinline__ void profile_pass3(const ProfileBindArgs& a, uint32_t
             sh.pmin = pmn;
             sh.pmax = pmx;
         }
+        if constexpr (NR) {
+            uint32_t tm = 0, nm = 0;
+            for (uint32_t i = lane; i < gridDim.x; i += 32) {
+                tm = max(tm, __ldcg(a.ptmax + i));
+                nm = max(nm, __ldcg(a.pnmax + i));
+            }
+            tm = __reduce_max_sync(0xffffffffu, tm);
+            nm = __reduce_max_sync(0xffffffffu, nm);
+            if (lane == 0) {
+                ns->gtmax = tm;
+                ns->gnmax = nm;
+            }
+        }
     }
     __syncthreads();
     const int64_t rc = __ldg(b.req_cpu + p), rm = __ldg(b.req_mem + p);
     int64_t best = INT64_MIN;
     int32_t bidx = -1;
+    const uint32_t* nrow = NR ? node_row(a, g) : nullptr;
     for (uint32_t n = n0 + tid; n < n1; n += SBD_THREADS) {
         if (__ldcg(a.iraw + n) == PB_NOT_CAND) continue;
         int64_t pts, ipa;
         profile_parts(a, sk, n, sh, pts, ipa);
-        const int64_t key = alloc_score_rt(b.policy, __ldcg(b.free_cpu + n), __ldcg(b.free_mem + n), b.alloc_cpu,
-                                           b.alloc_mem, n, rc, rm) +
-                            (int64_t)a.wspread * pts + (int64_t)a.waff * ipa;
+        int64_t key = alloc_score_rt(b.policy, __ldcg(b.free_cpu + n), __ldcg(b.free_mem + n), b.alloc_cpu,
+                                     b.alloc_mem, n, rc, rm) +
+                      (int64_t)a.wspread * pts + (int64_t)a.waff * ipa;
+        if constexpr (NR) {
+            int64_t tt, na;
+            node_parts(__ldg(nrow + n), *ns, tt, na);
+            key += (int64_t)a.wtaint * tt + (int64_t)a.wnaff * na;
+        }
         if (key > best) { // ascending n per thread: strict '>' keeps the lowest index
             best = key;
             bidx = (int32_t)n;
@@ -770,22 +865,51 @@ __device__ __forceinline__ void profile_pass3(const ProfileBindArgs& a, uint32_t
 // Phase B, CTA 0: spread_bind_commit's merge, binding, charge, hard counts and B/A entries (the merged key is the total,
 // which key_score_rt returns unchanged for every policy this call accepts); then the parts of the winner, the soft
 // counts and the bound pod's IPA entries.  The winner's parts are read from its raws and sh's extremes, which pass 3
-// left in this CTA, and its policy score is the total less the weighted parts.
-__device__ __forceinline__ void profile_commit(const ProfileBindArgs& a, uint32_t p, ProfileShared& sh) {
+// left in this CTA, and its policy score is the total less the weighted parts.  NR: five parts, and the four refusals
+// from the two that spread_bind_commit left in b.out_refused and the CTAs' taint and node-affinity partials.
+template <bool NR = false>
+__device__ __forceinline__ void profile_commit(const ProfileBindArgs& a, uint32_t p, ProfileShared& sh,
+                                               NodeShared* ns = nullptr) {
     const SpreadBindArgs& b = a.b;
     const uint32_t tid = threadIdx.x;
     spread_bind_commit<true>(b, p, &sh.rescan, sh.ref, &sh.bidx);
     const int32_t g = __ldg(b.group + p), n = sh.bidx;
     const uint32_t sk = soft_keys(a, g);
     if (tid == 0 && a.out_parts) {
-        int64_t pts = 0, ipa = 0, ps = 0;
+        int64_t pts = 0, ipa = 0, ps = 0, tt = 0, na = 0;
         if (n >= 0) {
             profile_parts(a, sk, (uint32_t)n, sh, pts, ipa);
             ps = __ldcg(b.out_score + p) - (int64_t)a.wspread * pts - (int64_t)a.waff * ipa;
+            if constexpr (NR) {
+                node_parts(__ldg(node_row(a, g) + n), *ns, tt, na);
+                ps -= (int64_t)a.wtaint * tt + (int64_t)a.wnaff * na;
+            }
         }
-        a.out_parts[3 * (size_t)p] = ps;
-        a.out_parts[3 * (size_t)p + 1] = pts;
-        a.out_parts[3 * (size_t)p + 2] = ipa;
+        constexpr size_t PW = NR ? 5 : 3;
+        a.out_parts[PW * p] = ps;
+        a.out_parts[PW * p + 1] = pts;
+        a.out_parts[PW * p + 2] = ipa;
+        if constexpr (NR) {
+            a.out_parts[PW * p + 3] = tt;
+            a.out_parts[PW * p + 4] = na;
+        }
+    }
+    if constexpr (NR) {
+        uint32_t tr = 0, nr = 0;
+        if (tid < 32) { // the CTAs' partials across the warp, as spread_bind_commit merges its own
+            for (uint32_t c = threadIdx.x; c < gridDim.x; c += 32) {
+                tr += __ldcg(a.ptref + c);
+                nr += __ldcg(a.pnref + c);
+            }
+            tr = __reduce_add_sync(0xffffffffu, tr);
+            nr = __reduce_add_sync(0xffffffffu, nr);
+        }
+        if (tid == 0) { // lane 0 wrote the two words of b.out_refused in spread_bind_commit
+            a.out_refused4[4 * (size_t)p] = tr;
+            a.out_refused4[4 * (size_t)p + 1] = nr;
+            a.out_refused4[4 * (size_t)p + 2] = __ldcg(b.out_refused + 2 * (size_t)p);
+            a.out_refused4[4 * (size_t)p + 3] = __ldcg(b.out_refused + 2 * (size_t)p + 1);
+        }
     }
     if (n < 0 || g < 0) return;
     if (tid == 0 && sk && !pts_ignored(a, sk, __ldg(a.soft_all + g), (uint32_t)n)) {
@@ -845,12 +969,84 @@ __global__ void __launch_bounds__(SBD_THREADS) k_profile_setup(const ProfileBind
     }
 }
 
-cudaError_t launch_profile_bind(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
+// ks_node_bind: one rule word per (class c, node n) over the grid-strided C x N pairs (include/ksched.h, 5p)
+__global__ void __launch_bounds__(SBD_THREADS) k_node_rules_setup(const ProfileBindArgs a) {
+    const uint64_t total = (uint64_t)a.C * a.b.N;
+    for (uint64_t i = (uint64_t)blockIdx.x * SBD_THREADS + threadIdx.x; i < total; i += (uint64_t)gridDim.x * SBD_THREADS) {
+        const uint32_t c = (uint32_t)(i / a.b.N), n = (uint32_t)(i % a.b.N);
+        const uint64_t hard = __ldg(a.taint_hard + n) & ~__ldg(a.ctol + 2 * c);
+        const uint32_t tt = __popcll(__ldg(a.taint_soft + n) & ~__ldg(a.ctol + 2 * c + 1));
+        bool has_req = false, req_ok = false;
+        uint32_t na = 0;
+        for (uint32_t t = __ldg(a.cterm_off + c), t1 = __ldg(a.cterm_off + c + 1); t < t1; t++) {
+            const uint32_t x0 = __ldg(a.cexpr_off + t), x1 = __ldg(a.cexpr_off + t + 1);
+            bool ok = x1 > x0; // a term with no expression matches nothing
+            for (uint32_t x = x0; x < x1 && ok; x++) {
+                const uint32_t k = __ldg(a.cexpr_key + x);
+                const int32_t d = __ldg(a.ndom + (size_t)k * a.b.N + n);
+                const uint32_t bit = d < 0 ? a.NDk[k] : (uint32_t)d;
+                ok = __ldg(a.nset + __ldg(a.cexpr_set + x) + bit / 64) >> (bit % 64) & 1u;
+            }
+            const uint32_t w = __ldg(a.cterm_w + t);
+            if (w == 0) {
+                has_req = true;
+                req_ok |= ok;
+            } else if (ok) {
+                na += w;
+            }
+        }
+        const bool aff_ok = !has_req || req_ok;
+        const uint32_t reason = hard ? NR_TAINT : aff_ok ? 0u : NR_AFFINITY;
+        a.nrules[i] = reason | (aff_ok ? NR_AFF_OK : 0u) | tt << NR_TT_SHIFT | na << NR_NA_SHIFT;
+    }
+}
+
+template <int W>
+__global__ void __launch_bounds__(SBD_THREADS) k_node_spread_setup(const ProfileBindArgs a) {
+    spread_bind_setup<W, true>(a.b, a.nrules, a.ncls);
+}
+
+// k_profile_bind_seq with the NR instances of its passes
+template <int W>
+__global__ void __launch_bounds__(SBD_THREADS, 1) k_node_bind_seq(const ProfileBindArgs a) {
+    cg::grid_group grid = cg::this_grid();
+    __shared__ ProfileShared sh;
+    __shared__ NodeShared ns;
+    const uint32_t G = gridDim.x;
+    const uint32_t chunk = (a.b.N + G - 1) / G, n0 = min(a.b.N, blockIdx.x * chunk), n1 = min(a.b.N, n0 + chunk);
+    for (uint32_t p = 0; p < a.b.P; p++) {
+        profile_pass1<W, true>(a, p, n0, n1, sh, &ns);
+        __threadfence();
+        grid.sync();
+        if (soft_keys(a, __ldg(a.b.group + p))) { // uniform: every CTA knows the pod's group
+            profile_pass2(a, p, n0, n1, sh);
+            __threadfence();
+            grid.sync();
+        }
+        profile_pass3<true>(a, p, n0, n1, sh, &ns);
+        __threadfence();
+        grid.sync();
+        if (blockIdx.x == 0) profile_commit<true>(a, p, sh, &ns);
+        __threadfence();
+        grid.sync();
+    }
+}
+
+// ks_profile_bind's launches; NR: k_node_rules_setup first, and the NR kernels in place of the spread setup and the walk
+template <bool NR>
+static cudaError_t launch_profile(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
     return with_label_width(W, [&](auto w) {
         constexpr int LW = decltype(w)::value;
         const SpreadBindArgs& b = a.b;
+        if (NR) {
+            k_node_rules_setup<<<a.rules_grid, SBD_THREADS, 0, st>>>(a);
+            g_launches++;
+            const cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess) return e;
+        }
         if (b.G) {
-            k_spread_bind_setup<LW><<<b.setup_grid, SBD_THREADS, 0, st>>>(b);
+            if (NR) k_node_spread_setup<LW><<<b.setup_grid, SBD_THREADS, 0, st>>>(a);
+            else k_spread_bind_setup<LW><<<b.setup_grid, SBD_THREADS, 0, st>>>(b);
             g_launches++;
             const cudaError_t e = cudaGetLastError();
             if (e != cudaSuccess) return e;
@@ -871,11 +1067,20 @@ cudaError_t launch_profile_bind(const ProfileBindArgs& a, uint64_t acnt_words, u
         }
         ProfileBindArgs c = a;
         void* args[] = {&c};
-        e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(k_profile_bind_seq<LW>), dim3(b.grid),
-                                        dim3(SBD_THREADS), args, 0, st);
+        e = cudaLaunchCooperativeKernel(NR ? reinterpret_cast<const void*>(k_node_bind_seq<LW>)
+                                           : reinterpret_cast<const void*>(k_profile_bind_seq<LW>),
+                                        dim3(b.grid), dim3(SBD_THREADS), args, 0, st);
         if (e == cudaSuccess) g_launches++;
         return e;
     });
+}
+
+cudaError_t launch_profile_bind(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
+    return launch_profile<false>(a, acnt_words, W, st);
+}
+
+cudaError_t launch_node_bind(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
+    return launch_profile<true>(a, acnt_words, W, st);
 }
 
 } // namespace ks

@@ -56,6 +56,10 @@ for _name, _res, _args in [
                                          C.c_int, _vp, _vp, _vp, C.c_size_t, _vp]),
     ("ksh_reconcile_profile", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp,
                                         _vp, C.c_int, _vp, _vp, _vp, C.c_size_t, _vp]),
+    ("ksh_context_set_node_taints", C.c_int, [_vp, _vp, _vp, _vp, C.c_uint64]),
+    ("ksh_compile_node_rules", C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp]),
+    ("ksh_reconcile_nodes", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp,
+                                      _vp, _vp, C.c_int, _vp, _vp, _vp, C.c_size_t, _vp]),
 ]:
     _proto(_name, _res, *_args)
 
@@ -64,6 +68,61 @@ KSH_RECONCILE_OK, KSH_RECONCILE_NO_NODE_FOUND, KSH_RECONCILE_BINDING_OBJECT_FAIL
 KSH_RECONCILE_GANG_UNSATISFIED = 4
 KSH_RECONCILE_SPREAD_UNSATISFIED = 5
 KSH_RECONCILE_AFFINITY_UNSATISFIED = 6
+KSH_RECONCILE_NODE_RULES_UNSATISFIED = 7
+
+
+class ksh_taint(C.Structure):
+    _fields_ = [("key", C.c_char_p), ("value", C.c_char_p), ("effect", C.c_char_p)]
+
+
+class ksh_toleration(C.Structure):
+    _fields_ = [("key", C.c_char_p), ("op", C.c_char_p), ("value", C.c_char_p), ("effect", C.c_char_p)]
+
+
+class ksh_node_selector_requirement(C.Structure):
+    _fields_ = [("key", C.c_char_p), ("op", C.c_char_p), ("values", C.c_void_p), ("n_values", C.c_uint32)]
+
+
+class ksh_node_rules(C.Structure):
+    _fields_ = [("toleration_offset", C.c_void_p), ("tolerations", C.c_void_p), ("n_terms", C.c_uint32),
+                ("term_owner", C.c_void_p), ("term_weight", C.c_void_p), ("term_req_offset", C.c_void_p),
+                ("requirements", C.c_void_p), ("weight_taint", C.c_uint32), ("weight_node_affinity", C.c_uint32)]
+
+
+def _b(s):
+    return None if s is None else s.encode()
+
+
+def node_rules(group_rules, weight_taint=3, weight_node_affinity=2):
+    """The ksh_node_rules of per-group rule dicts, and the objects its pointers reach (keep them alive).  group_rules[g]:
+    {"tolerations": [{"key", "operator", "value", "effect"}, ...], "required": [term, ...] or None,
+    "preferred": [(weight, term), ...]}, a term a list of {"key", "operator", "values"}."""
+    hold = []
+    tols = [t for r in group_rules for t in r.get("tolerations", ())]
+    toff = np.zeros(len(group_rules) + 1, np.uint64)
+    np.cumsum([len(r.get("tolerations", ())) for r in group_rules], out=toff[1:])
+    tarr = (ksh_toleration * max(len(tols), 1))(*[ksh_toleration(_b(t.get("key", "")), _b(t.get("operator", "")),
+                                                                 _b(t.get("value", "")), _b(t.get("effect", "")))
+                                                  for t in tols])
+    terms = []  # (owner, weight, requirements)
+    for g, r in enumerate(group_rules):
+        terms += [(g, 0, t) for t in (r.get("required") or [])]
+        terms += [(g, int(w), t) for w, t in r.get("preferred", ())]
+    reqs = [q for _, _, t in terms for q in t]
+    roff = np.zeros(len(terms) + 1, np.uint64)
+    np.cumsum([len(t) for _, _, t in terms], out=roff[1:])
+    rarr = (ksh_node_selector_requirement * max(len(reqs), 1))()
+    for i, q in enumerate(reqs):
+        vals = (C.c_char_p * max(len(q.get("values", ())), 1))(*[_b(v) for v in q.get("values", ())])
+        hold.append(vals)
+        rarr[i] = ksh_node_selector_requirement(_b(q["key"]), _b(q["operator"]), C.cast(vals, _vp),
+                                                len(q.get("values", ())))
+    owner = np.ascontiguousarray([t[0] for t in terms], np.int32)
+    weight = np.ascontiguousarray([t[1] for t in terms], np.uint32)
+    hold += [toff, tarr, rarr, roff, owner, weight]
+    nr = ksh_node_rules(toff.ctypes.data, C.addressof(tarr), len(terms), owner.ctypes.data, weight.ctypes.data,
+                        roff.ctypes.data, C.addressof(rarr), int(weight_taint), int(weight_node_affinity))
+    return nr, hold
 
 
 class ksh_pod_affinity(C.Structure):
@@ -479,9 +538,60 @@ class Context:
         return self._reconcile_terms(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
                                      min_domains, existing_nodes, policy, json_cap, scoring)
 
+    def set_node_taints(self, taints):
+        """spec.taints of nodes by name (ksh_context_set_node_taints): taints maps a node name to a list of
+        {"key", "value", "effect"}; it replaces what that node carried.  Unknown names are ignored."""
+        names = list(taints)
+        flat = [t for nm in names for t in taints[nm]]
+        off = np.zeros(len(names) + 1, np.uint64)
+        np.cumsum([len(taints[nm]) for nm in names], out=off[1:])
+        arr = (ksh_taint * max(len(flat), 1))(*[ksh_taint(_b(t["key"]), _b(t.get("value", "")), _b(t["effect"]))
+                                                 for t in flat])
+        cn = (C.c_char_p * max(len(names), 1))(*[nm.encode() for nm in names])
+        check(lib.ksh_context_set_node_taints(self._h, C.cast(cn, _vp), off.ctypes.data, C.addressof(arr), len(names)),
+              "ksh_context_set_node_taints")
+
+    def compile_node_rules(self, group_rules):
+        """The compiled rules evaluated per (group, node) (ksh_compile_node_rules): (hard uint8 [G, N], affinity uint8
+        [G, N], soft uint32 [G, N], preferred uint32 [G, N]); group_rules as node_rules takes them."""
+        G, N = len(group_rules), self.n_nodes
+        nr, hold = node_rules(group_rules)
+        out = (np.zeros((G, N), np.uint8), np.zeros((G, N), np.uint8), np.zeros((G, N), np.uint32),
+               np.zeros((G, N), np.uint32))
+        check(lib.ksh_compile_node_rules(self._h, G, C.byref(nr), *[o.ctypes.data for o in out]),
+              "ksh_compile_node_rules")
+        return out
+
+    def reconcile_nodes(self, pods, n, group, n_groups, topology_keys, terms=(), existing_pods=(), max_skew=None,
+                        min_domains=None, existing_nodes=None, policy=capi.KS_SCORE_LEAST_BALANCED, json_cap=None,
+                        soft_skew=None, soft_all_keys=None, term_weight=None, hard_affinity_weight=1, weight_spread=2,
+                        weight_affinity=2, group_rules=None, weight_taint=3, weight_node_affinity=2):
+        """reconcile_profile with the context's node taints and per-group rules (ksh_reconcile_nodes): group_rules
+        [n_groups] as node_rules takes them, or None (no toleration and no term).  Status 7
+        (KSH_RECONCILE_NODE_RULES_UNSATISFIED) for a pod that fit some node but taints or node affinity refused every
+        such node.  Returns (status[n], node_idx[n], bodies[n])."""
+        nr = None
+        if group_rules is not None:
+            if len(group_rules) != n_groups:
+                raise ValueError(f"group_rules has {len(group_rules)} entries, groups {n_groups}")
+            nr = node_rules(group_rules, weight_taint, weight_node_affinity)
+        k = len(topology_keys)
+        soft = None if soft_skew is None else np.ascontiguousarray(soft_skew, np.uint32).reshape(-1)
+        sall = None if soft_all_keys is None else np.ascontiguousarray(soft_all_keys, np.uint8).reshape(-1)
+        tw = None if term_weight is None else np.ascontiguousarray(term_weight, np.uint32).reshape(-1)
+        if soft is not None and soft.shape[0] != n_groups * k:
+            raise ValueError(f"soft_skew has {soft.shape[0]} entries, groups {n_groups}, keys {k}")
+        scoring = capi.ks_bind_scoring(None if soft is None else soft.ctypes.data,
+                                       None if sall is None else sall.ctypes.data,
+                                       None if tw is None else tw.ctypes.data, int(hard_affinity_weight),
+                                       int(weight_spread), int(weight_affinity))
+        return self._reconcile_terms(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
+                                     min_domains, existing_nodes, policy, json_cap, scoring, nodes=True,
+                                     rules=None if nr is None else nr[0])
+
     def _reconcile_terms(self, pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew, min_domains,
-                         existing_nodes, policy, json_cap, scoring):
-        # ksh_reconcile_affinity, or with scoring ksh_reconcile_profile
+                         existing_nodes, policy, json_cap, scoring, nodes=False, rules=None):
+        # ksh_reconcile_affinity, or with scoring ksh_reconcile_profile, or with nodes ksh_reconcile_nodes
         k = len(topology_keys)
         group = np.ascontiguousarray(group, np.int32).reshape(-1)
         if group.shape[0] != n:
@@ -519,7 +629,10 @@ class Context:
                 None if names is None else C.cast(names, _vp), None if ex_off is None else ex_off.ctypes.data,
                 C.byref(aff))
         tail = (int(policy), status.ctypes.data, node.ctypes.data, C.addressof(buf), cap, off.ctypes.data)
-        if scoring is None:
+        if nodes:
+            check(lib.ksh_reconcile_nodes(*head, C.byref(scoring), None if rules is None else C.byref(rules), *tail),
+                  "ksh_reconcile_nodes")
+        elif scoring is None:
             check(lib.ksh_reconcile_affinity(*head, *tail), "ksh_reconcile_affinity")
         else:
             check(lib.ksh_reconcile_profile(*head, C.byref(scoring), *tail), "ksh_reconcile_profile")

@@ -39,6 +39,47 @@ def replica_outputs(replicas, row_dtype, want_nodes):
     return offset, rows, np.empty(total, np.int32), np.empty(total, np.int64)
 
 
+def node_set(D, members):
+    """The set words of a node-affinity expression over a key of D domains (ks_node_rules): bit i for each domain i in
+    members, bit D (pass D itself) for "the node lacks the key"."""
+    words = np.zeros((D + 64) // 64, np.uint64)
+    for i in members:
+        words[i // 64] |= np.uint64(1 << (i % 64))
+    return words
+
+
+def node_rules(rules):
+    """The ks_node_rules struct of a Snapshot.node_bind rules dict, and the arrays it points into (keep them alive)."""
+    hold = []
+
+    def arr(a, dtype):
+        if a is None:
+            return None
+        a = _c(a, dtype).reshape(-1)
+        hold.append(a)
+        return _ptr(a)
+    keys = list(rules.get("rule_keys", ()))
+    if len(keys) > capi.KS_NODE_RULES_MAX_KEYS:
+        raise ValueError(f"{len(keys)} node-affinity keys (at most {capi.KS_NODE_RULES_MAX_KEYS})")
+    terms = list(rules.get("node_terms", ()))
+    exprs = [e for t in terms for e in t[2]]
+    toff = np.zeros(len(terms) + 1, np.uint32)
+    np.cumsum([len(t[2]) for t in terms], out=toff[1:])
+    soff = np.zeros(len(exprs) + 1, np.uint64)
+    np.cumsum([len(np.asarray(e[1]).reshape(-1)) for e in exprs], out=soff[1:])
+    sets = np.concatenate([np.asarray(e[1], np.uint64).reshape(-1) for e in exprs]) if exprs else np.zeros(0, np.uint64)
+    nd = [int(d) for _, d in keys] + [0] * (capi.KS_NODE_RULES_MAX_KEYS - len(keys))
+    doms = [arr(d, np.int32) for d, _ in keys] + [None] * (capi.KS_NODE_RULES_MAX_KEYS - len(keys))
+    nr = capi.ks_node_rules(
+        int(rules.get("n_taints", 0)), arr(rules.get("taint_hard"), np.uint64), arr(rules.get("taint_soft"), np.uint64),
+        arr(rules.get("tolerate_hard"), np.uint64), arr(rules.get("tolerate_soft"), np.uint64), len(keys),
+        (C.c_uint32 * capi.KS_NODE_RULES_MAX_KEYS)(*nd), (C.c_void_p * capi.KS_NODE_RULES_MAX_KEYS)(*doms),
+        len(exprs), arr([e[0] for e in exprs], np.uint32), arr(soff, np.uint64), arr(sets, np.uint64), len(terms),
+        arr([t[0] for t in terms], np.int32), arr([t[1] for t in terms], np.uint32), arr(toff, np.uint32),
+        int(rules.get("weight_taint", 3)), int(rules.get("weight_node_affinity", 2)))
+    return nr, hold
+
+
 @dataclass
 class SelectResult:
     node_idx: np.ndarray
@@ -460,6 +501,29 @@ class Snapshot:
         terms); soft_skew [G, K] or None (ScheduleAnyway maxSkew, 0 = none); soft_all_keys [G] or None (all 1).
         Charges free[].  Returns (node_idx int32 [P], score int64 [P], parts int64 [P, 3] (policy, pts, ipa),
         refused uint32 [P, 2], counts, soft_counts); both counts lists of K arrays [G, D_k], or None."""
+        return self._scored_bind(None, req_cpu, req_mem, sel, group, n_groups, keys, terms, existing_pods, max_skew,
+                                 min_domains, existing, policy, soft_skew, soft_all_keys, term_weight,
+                                 hard_affinity_weight, weight_spread, weight_affinity, want_counts)
+
+    def node_bind(self, req_cpu, req_mem, sel, group, n_groups, keys, terms=(), existing_pods=None, max_skew=None,
+                  min_domains=None, existing=None, policy=capi.KS_SCORE_LEAST_BALANCED, soft_skew=None,
+                  soft_all_keys=None, term_weight=None, hard_affinity_weight=1, weight_spread=2, weight_affinity=2,
+                  rules=None, want_counts=True):
+        """profile_bind with TaintToleration and NodeAffinity (ks_node_bind).  rules: None (the C call's NULL) or a
+        dict with any of n_taints, taint_hard [N], taint_soft [N], tolerate_hard [G], tolerate_soft [G] (uint64 taint
+        masks), rule_keys (a list of (node_domain [N], D_k)), node_terms (a list of (owner, weight, [(key, set words
+        uint64), ...]); weight 0 = required), weight_taint (default 3) and weight_node_affinity (default 2); see
+        node_set for the words.  Returns profile_bind's tuple with parts [P, 5] (policy, pts, ipa, tt, na) and refused
+        [P, 4] (taint, node affinity, spread, inter-pod affinity)."""
+        return self._scored_bind(rules if rules is not None else False, req_cpu, req_mem, sel, group, n_groups, keys,
+                                 terms, existing_pods, max_skew, min_domains, existing, policy, soft_skew,
+                                 soft_all_keys, term_weight, hard_affinity_weight, weight_spread, weight_affinity,
+                                 want_counts)
+
+    def _scored_bind(self, rules, req_cpu, req_mem, sel, group, n_groups, keys, terms, existing_pods, max_skew,
+                     min_domains, existing, policy, soft_skew, soft_all_keys, term_weight, hard_affinity_weight,
+                     weight_spread, weight_affinity, want_counts):
+        """ks_profile_bind when rules is None, else ks_node_bind (rules False = its NULL rules)."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
         p, g = int(pods.n), int(n_groups)
         group = _c(group, np.int32).reshape(-1)
@@ -511,14 +575,20 @@ class Snapshot:
                                        int(hard_affinity_weight), int(weight_spread), int(weight_affinity))
         idx = np.empty(p, np.int32)
         score = np.empty(p, np.int64)
-        parts = np.empty((p, 3), np.int64)
-        refused = np.empty((p, 2), np.uint32)
+        parts = np.empty((p, 3 if rules is None else 5), np.int64)
+        refused = np.empty((p, 2 if rules is None else 4), np.uint32)
         want = want_counts and 0 < g * s <= capi.KS_SPREAD_MAX_COUNTS
         counts = np.empty((g, s), np.uint32) if want else None
         soft = np.empty((g, s), np.uint32) if want else None
-        check(lib.ks_profile_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
-                                  C.byref(scoring), int(policy), _ptr(idx), _ptr(score), _ptr(parts), _ptr(refused),
-                                  _ptr(counts), _ptr(soft)), "ks_profile_bind")
+        if rules is None:
+            check(lib.ks_profile_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
+                                      C.byref(scoring), int(policy), _ptr(idx), _ptr(score), _ptr(parts),
+                                      _ptr(refused), _ptr(counts), _ptr(soft)), "ks_profile_bind")
+        else:
+            nr, hold = node_rules(rules) if rules is not False else (None, None)
+            check(lib.ks_node_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
+                                   C.byref(scoring), C.byref(nr) if nr is not None else None, int(policy), _ptr(idx),
+                                   _ptr(score), _ptr(parts), _ptr(refused), _ptr(counts), _ptr(soft)), "ks_node_bind")
         if want:
             counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
             soft = np.split(soft, np.cumsum(nd)[:-1], axis=1)
