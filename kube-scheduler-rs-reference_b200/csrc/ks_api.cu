@@ -2085,9 +2085,13 @@ static int compile_node_rules(const ks_node_rules* r, uint32_t G, uint32_t N, No
     return KS_OK;
 }
 
-// ks_spread_bind, and with aff set ks_affinity_bind (then max_skew may be NULL and out_refused holds 2P words), and with
-// aff and sc set ks_profile_bind (out_parts [3P] and out_soft_count [G * S] may be given), and with nr set as well
-// ks_node_bind (out_parts [5P], out_refused [4P])
+// last_path and the name in launch errors of each BindMode
+static const char* const BIND_PATH[] = {"spread_bind", "affinity_bind", "profile_bind", "node_bind"};
+static const char* const BIND_NAME[] = {"spread bind", "affinity bind", "profile bind", "node bind"};
+
+// ks_spread_bind, and with aff set ks_affinity_bind (then max_skew may be NULL), and with aff and sc set ks_profile_bind
+// (out_parts and out_soft_count [G * S] may be given), and with nr set as well ks_node_bind; out_refused and out_parts
+// hold the mode's words per pod (bind_refusal_words, bind_part_words)
 static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
                        const ks_spread_multi* spread, const ks_pod_affinity* aff, int policy, int32_t* out_node_idx,
                        int64_t* out_score, uint32_t* out_refused, uint32_t* out_domain_count,
@@ -2165,8 +2169,8 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         }
         if (rc) return rc;
     }
-    const uint64_t R = nr ? 4 : aff ? 2 : 1; // refusal words per pod
-    const uint64_t PW = nr ? 5 : 3;          // parts per pod
+    const BindMode mode = nr ? BIND_NODE : sc ? BIND_PROFILE : aff ? BIND_AFFINITY : BIND_SPREAD;
+    const uint64_t R = bind_refusal_words(mode), PW = bind_part_words(mode);
     if (P == 0) return KS_OK;
     if (N == 0) { // no node: nothing is placed, every count is existing
         memset(out_node_idx, 0xff, P * 4);
@@ -2183,9 +2187,10 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
     if (!s->coop) return fail(KS_ERR_CUDA, "device %d has no cooperative launch", s->device);
-    SpreadBindArgs a{};
+    ProfileBindArgs q{}; // the fields a mode does not read stay zero
+    SpreadBindArgs& a = q.b;
     a.grid = std::max(1u, std::min<uint32_t>((uint32_t)s->sms, (N + 127u) / 128u));
-    a.setup_grid = spread_bind_setup_grid((uint32_t)G, s->sms);
+    a.setup_grid = bind_setup_grid((uint32_t)G, s->sms);
     HostStaged h;
     const auto cpu = h.in(pods->req_cpu, P), mem = h.in(pods->req_mem, P);
     const auto sel = h.in(pods->sel, P * W);
@@ -2215,7 +2220,6 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     const auto pref = h.work<uint32_t>(a.grid);
     // ks_profile_bind: the soft terms, the log table and the compiled IPA entries; the domain bitmaps of the keys with
     // more than one node in some domain, per parity
-    ProfileBindArgs q{};
     const uint64_t Q = sc ? 1 : 0;
     if (sc) {
         std::vector<uint8_t> seen;
@@ -2265,7 +2269,6 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     const auto taint_hard = h.in(nr ? nr->node_taint_hard : nullptr, NR1 * N); // NULL: zeros, filled below
     const auto taint_soft = h.in(nr ? nr->node_taint_soft : nullptr, NR1 * N);
     const auto nrules = h.work<uint32_t>((uint64_t)nplan.C * N);
-    const auto refused2 = h.work<uint32_t>(NR1 * 2 * P); // ks_profile_bind's two words, before the four are written
     const auto ptref = h.work<uint32_t>(NR1 * a.grid), pnref = h.work<uint32_t>(NR1 * a.grid);
     const auto ptmax = h.work<uint32_t>(NR1 * a.grid), pnmax = h.work<uint32_t>(NR1 * a.grid);
     auto put = [&](Staged<uint32_t> d, const std::vector<uint32_t>& v) {
@@ -2354,7 +2357,6 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         a.paref = h.dev(paref);
     }
     if (sc) {
-        q.b = a;
         q.soft_skew = h.dev(soft_skew);
         q.soft_all = h.dev(soft_all);
         q.logw = h.dev(logw);
@@ -2379,8 +2381,6 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         q.waff = sc->weight_affinity;
     }
     if (nr) {
-        q.b.out_refused = h.dev(refused2);
-        q.out_refused4 = h.dev(refused);
         q.ncls = h.dev(ncls);
         q.nrules = h.dev(nrules);
         q.C = nplan.C;
@@ -2407,15 +2407,10 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     }
     s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
     s->version++;
-    cudaError_t e = nr    ? launch_node_bind(q, plan.words, W, st)
-                    : sc  ? launch_profile_bind(q, plan.words, W, st)
-                    : aff ? launch_affinity_bind(a, plan.words, W, st)
-                          : launch_spread_bind(a, W, st);
-    if (e != cudaSuccess)
-        return fail(KS_ERR_CUDA, "%s launch failed: %s",
-                    nr ? "node bind" : sc ? "profile bind" : aff ? "affinity bind" : "spread bind", cudaGetErrorString(e));
+    const cudaError_t e = launch_bind(mode, q, plan.words, W, st);
+    if (e != cudaSuccess) return fail(KS_ERR_CUDA, "%s launch failed: %s", BIND_NAME[mode], cudaGetErrorString(e));
     CU_TRY(h.finish(st));
-    s->last_path = nr ? "node_bind" : sc ? "profile_bind" : aff ? "affinity_bind" : "spread_bind";
+    s->last_path = BIND_PATH[mode];
     return KS_OK;
 }
 

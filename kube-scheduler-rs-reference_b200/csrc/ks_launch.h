@@ -228,9 +228,17 @@ struct GangArgs {
 };
 cudaError_t launch_gang_batch(const StreamBatchArgs& a, const GangArgs& g, uint32_t W, cudaStream_t st);
 
-// topology spread when binding (ks_spread_bind, ks_spread_bind.cu): k_spread_bind_setup (one CTA per group, grid-strided
-// over setup_grid CTAs; not launched when G = 0), then one cooperative launch of grid CTAs that walks the P pods.
-// Device memory.  Key k's domains are the counts [Pk[k], Pk[k] + Dk[k]) of each group's S.
+// The bind calls (ks_spread_bind.cu), one mode each: ks_spread_bind, ks_affinity_bind, ks_profile_bind and ks_node_bind
+// with rules.  Each mode filters as the one before it and adds rules; PROFILE and NODE also add scores.
+enum BindMode { BIND_SPREAD, BIND_AFFINITY, BIND_PROFILE, BIND_NODE };
+// Refusal words and score parts per pod in a mode's outputs (include/ksched.h)
+__host__ __device__ constexpr uint32_t bind_refusal_words(BindMode m) {
+    return m == BIND_NODE ? 4 : m == BIND_SPREAD ? 1 : 2;
+}
+__host__ __device__ constexpr uint32_t bind_part_words(BindMode m) { return m == BIND_NODE ? 5 : 3; }
+
+// topology spread when binding (ks_spread_bind), the state of every mode.  Device memory.  Key k's domains are the
+// counts [Pk[k], Pk[k] + Dk[k]) of each group's S.
 struct SpreadBindArgs {
     uint32_t N, Npad, P, G, K, S;
     uint32_t Dk[KS_SPREAD_MAX_KEYS], Pk[KS_SPREAD_MAX_KEYS];
@@ -254,9 +262,9 @@ struct SpreadBindArgs {
     uint32_t* pref;
     int32_t* out_idx;                 // [P]
     int64_t* out_score;               // [P]
-    uint32_t* out_refused;            // [P]; [2P] under affinity: spread, then affinity refusals
-    uint32_t grid, setup_grid;
-    // inter-pod affinity (ks_affinity_bind; read only by its kernels).  Counter arrays B_{g,k} / A_{g,k} of D_k words
+    uint32_t* out_refused;            // [bind_refusal_words(mode) * P]
+    uint32_t grid, setup_grid;        // the walk's CTAs; k_bind_setup's, one per group, grid-strided
+    // inter-pod affinity (read by every mode but SPREAD).  Counter arrays B_{g,k} / A_{g,k} of D_k words
     // in acnt; one word per group at acnt[any_base + g] is set once a pod of M_g is bound on a node that carries one of
     // g's affinity keys.  Update entry: h | k << 16 | kind << 20 (kind 0 = B, 1 = A) raises that array of group h.
     const uint32_t* abase;            // [G * K * 2]: base of B_{g,k}, then of A_{g,k}, in acnt; AFF_NONE = no array
@@ -268,18 +276,15 @@ struct SpreadBindArgs {
     uint32_t* acnt;                   // counters, zeroed by the launcher
     uint32_t* paref;                  // [grid] per-CTA affinity refusals
 };
-uint32_t spread_bind_setup_grid(uint32_t G, int sms);
-cudaError_t launch_spread_bind(const SpreadBindArgs& a, uint32_t W, cudaStream_t st);
+uint32_t bind_setup_grid(uint32_t G, int sms);
 constexpr uint32_t AFF_NONE = 0xffffffffu, AFF_SELF = 1u;
-// ks_affinity_bind (ks_spread_bind.cu): k_spread_bind_setup when G > 0, the counters zeroed, k_affinity_setup over the
-// existing pods (aff_grid CTAs, when E > 0), then one cooperative launch of grid CTAs, k_affinity_bind_seq
-cudaError_t launch_affinity_bind(const SpreadBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st);
 
-// ks_profile_bind (ks_spread_bind.cu): ks_affinity_bind's state in b, plus the soft terms (DESIGN.md 5o).  The soft
-// counts scnt start at existing (or 0), the IPA counters I_{g,k} (int64, D_k words each at ibase[g * K + k] in icnt) at
-// 0 before the existing pods' entries.  Update entry of group h: g | k << 16 with coefficient icoef, added to
-// I_{g,k}[d_k(n)] when a pod of h binds on n.  Per node of the slice, pass 1 leaves iraw[n] = its IPA raw, or
-// PB_NOT_CAND when n is not a candidate, and pass 2 praw[n] = its PodTopologySpread raw, or -1 when it is ignored.
+// Every bind kernel takes this: ks_affinity_bind's state in b, first, so that its fields keep their parameter offsets,
+// then the soft terms of ks_profile_bind (DESIGN.md 5o) and the node rules of ks_node_bind.  The soft counts scnt start
+// at existing (or 0), the IPA counters I_{g,k} (int64, D_k words each at ibase[g * K + k] in icnt) at 0 before the
+// existing pods' entries.  Update entry of group h: g | k << 16 with coefficient icoef, added to I_{g,k}[d_k(n)] when a
+// pod of h binds on n.  Per node of the slice, pass 1 leaves iraw[n] = its IPA raw, or PB_NOT_CAND when n is not a
+// candidate, and pass 2 praw[n] = its PodTopologySpread raw, or -1 when it is ignored.
 constexpr uint32_t PB_SH_WORDS = 64; // domains below 64 * 32 of each key are marked in a per-CTA bitmap first
 struct ProfileBindArgs {
     SpreadBindArgs b;
@@ -301,9 +306,9 @@ struct ProfileBindArgs {
     uint32_t* pdom;                   // [grid * KS_SPREAD_MAX_KEYS] per-CTA partials: new domains per soft key
     uint32_t* plack;                  // [grid]: soft keys some non-ignored candidate lacks
     int64_t *pimin, *pimax, *ppmin, *ppmax; // [grid]: IPA raw and PodTopologySpread raw extremes
-    int64_t* out_parts;               // [3P]; [5P] under ks_node_bind
+    int64_t* out_parts;               // [bind_part_words(mode) * P]
     uint32_t wspread, waff;
-    // ks_node_bind (DESIGN.md 5p; read only by its kernels).  Rule word of (class c, node n) at nrules[c * N + n]:
+    // ks_node_bind (DESIGN.md 5p; read by NODE only).  Rule word of (class c, node n) at nrules[c * N + n]:
     // NR_REASON bits (0 pass, NR_TAINT, NR_AFFINITY), NR_AFF_OK, the PreferNoSchedule count at NR_TT_SHIFT and the
     // preferred NodeAffinity raw at NR_NA_SHIFT.  Class c's terms [cterm_off[c], cterm_off[c + 1]): weight cterm_w (0 =
     // required), expressions [cexpr_off[t], cexpr_off[t + 1]): key cexpr_key, set at word cexpr_set of nset.
@@ -317,13 +322,13 @@ struct ProfileBindArgs {
     const uint64_t *cexpr_set, *nset;
     uint32_t *ptref, *pnref;          // [grid] per-CTA taint and node-affinity refusals
     uint32_t *ptmax, *pnmax;          // [grid] per-CTA maxima of the two raws over the candidates
-    uint32_t* out_refused4;           // [4P]; out_refused of b is device scratch [2P]
     uint32_t wtaint, wnaff, rules_grid;
 };
 constexpr int64_t PB_NOT_CAND = INT64_MIN;
-cudaError_t launch_profile_bind(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st);
 constexpr uint32_t NR_REASON = 3u, NR_TAINT = 1u, NR_AFFINITY = 2u, NR_AFF_OK = 4u, NR_TT_SHIFT = 3, NR_NA_SHIFT = 10;
-// ks_node_bind (ks_spread_bind.cu): k_node_rules_setup, then ks_profile_bind's launches with k_node_spread_setup and
-// k_node_bind_seq in place of k_spread_bind_setup and k_profile_bind_seq
-cudaError_t launch_node_bind(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st);
+// One bind call's launches, in order: (NODE) k_node_rules_setup; k_bind_setup when G > 0; (every mode but SPREAD) the
+// counters zeroed, (PROFILE, NODE) the IPA counters and the bitmaps zeroed and the soft counts set, then k_affinity_setup
+// and (PROFILE, NODE) k_profile_setup over the existing pods when E > 0; then the walk k_bind_seq, one cooperative launch
+// of grid CTAs.  The fields a mode does not read may be left zero.
+cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st);
 } // namespace ks

@@ -1,23 +1,23 @@
-// ks_spread_bind.cu — topology spread when binding (ks_spread_bind, include/ksched.h; DESIGN.md 5m), and the same with
-// inter-pod affinity (ks_affinity_bind; DESIGN.md 5n).
-// A mixed pod queue is bound one pod at a time, each pod under its group's spread constraints against the counts and the
-// free[] every earlier pod left, as upstream kube-scheduler runs one scheduling cycle per pod.  Two kernels:
-//   k_spread_bind_setup  one CTA per group (grid-strided): the group's eligible domains per constrained key, its counts
-//                        (existing, or 0), and per key |E|, m, the number of eligible domains at m and the minDomains flag
-//   k_spread_bind_seq    one cooperative launch that walks the pods, shaped like k_gang_batch (ks_stream.cu): every CTA
-//                        owns one slice of the node table; per pod, phase A scans every slice and writes one partial per
-//                        CTA, phase B (CTA 0) merges the partials in CTA order, charges free[], writes the binding and
-//                        raises the counts; the two phases are separated by grid barriers.
-// ks_affinity_bind adds k_affinity_setup (the existing pods' update entries, one warp per pod) and runs
-// k_affinity_bind_seq, the same walk with the phase helpers' AFF instances: phase A also applies rules 1-3 of the header
-// through at most 2K counter loads per node, phase B also applies the bound pod's update entries across CTA 0.  The
-// AFF = false instances are the code k_spread_bind_seq always ran.
-// ks_profile_bind (DESIGN.md 5o) runs k_profile_bind_seq: the same filter and commit, with soft PodTopologySpread and
-// InterPodAffinity scores that need grid-wide reductions over the candidates before any node's total exists.
-// ks_node_bind (DESIGN.md 5p) first writes one rule word per (node-rule class, node) in k_node_rules_setup, then runs
-// k_node_spread_setup and k_node_bind_seq: the NR instances of the spread setup and of the profile passes, which read
-// that word per node for TaintToleration and NodeAffinity.  The NR = false instances are the code the existing kernels
-// always ran.
+// ks_spread_bind.cu — the bind calls of include/ksched.h: ks_spread_bind (topology spread, DESIGN.md 5m),
+// ks_affinity_bind (and inter-pod affinity, 5n), ks_profile_bind (and the soft PodTopologySpread and InterPodAffinity
+// scores, 5o) and ks_node_bind (and TaintToleration and NodeAffinity, 5p).
+// Each binds a mixed pod queue one pod at a time, each pod against the counts and the free[] every earlier pod left, as
+// upstream kube-scheduler runs one scheduling cycle per pod.  The calls differ by one BindMode (ks_launch.h), SPREAD,
+// AFFINITY, PROFILE or NODE, and share:
+//   BindFilter          the candidate filter: fit and selector, (NODE) the node's rule word, hard spread and (AFF, every
+//                       mode but SPREAD) rules 1-3 of the header
+//   k_bind_setup        one CTA per group (grid-strided): the group's eligible domains per constrained key, its counts
+//                       (existing, or 0), and per key |E|, m, the number of eligible domains at m and the minDomains flag;
+//                       NR (NODE) also drops the nodes that fail the group's required node affinity
+//   k_bind_seq          one cooperative launch that walks the pods, shaped like k_gang_batch (ks_stream.cu): every CTA
+//                       owns one slice of the node table and grid barriers separate each pod's phases.  SPREAD and
+//                       AFFINITY: phase A scans every slice into one partial per CTA, phase B (CTA 0) merges the partials
+//                       in CTA order, charges free[], writes the binding and raises the counts.  PROFILE and NODE: three
+//                       passes, because the soft scores need grid-wide reductions over the candidates before any node's
+//                       total exists, then the same commit.
+//   launch_bind         one mode's launches, in order
+// Per call, k_affinity_setup and k_profile_setup apply the existing pods' update entries (every mode but SPREAD, and
+// PROFILE and NODE), and k_node_rules_setup writes one rule word per (node-rule class, node) (NODE).
 #include "ks_internal.cuh"
 #include "ks_launch.h"
 
@@ -143,9 +143,9 @@ __device__ __forceinline__ void spread_bind_setup(const SpreadBindArgs& a, const
     }
 }
 
-template <int W>
-__global__ void __launch_bounds__(SBD_THREADS) k_spread_bind_setup(const SpreadBindArgs a) {
-    spread_bind_setup<W, false>(a, nullptr, nullptr);
+template <int W, bool NR>
+__global__ void __launch_bounds__(SBD_THREADS) k_bind_setup(const ProfileBindArgs a) {
+    spread_bind_setup<W, NR>(a.b, a.nrules, a.ncls);
 }
 
 // Inter-pod affinity: one update entry of a pod bound at node n.  Entries of one list name distinct (group, key, kind)
@@ -161,48 +161,52 @@ __device__ __forceinline__ void affinity_raise(const SpreadBindArgs& a, uint32_t
     if (kind) a.acnt[a.any_base + h] = 1; // a pod of M_h sits on a node that carries one of h's affinity keys
 }
 
-// ProfileFilter (ks_profile_bind, below) repeats this filter rule for rule: a change here goes there too.
-// Phase A of pod p in this CTA's slice [n0, n1): fit, selector and, for a constrained pod, cnt < m + max_skew on every
-// constrained key; the best candidate by the policy's key (ties to the lower node) and the refused count into the CTA's
-// partial.  AFF: then rules 1-3 of ks_affinity_bind against the pod's group's counter bases, formed once per pod; the
-// nodes they refuse into s_aref / paref.
+// The candidate filter of every bind walk for pod p: fit, selector and, for a constrained pod, cnt < m + max_skew on
+// every constrained key (the bound formed once per pod); AFF: then rules 1-3 of ks_affinity_bind against the pod's
+// group's counter bases and first-pod flag, formed once per pod.  Without AFF (ks_spread_bind, whose abase, aflag and
+// acnt are NULL) none of them is read.
 template <int W, bool AFF>
-__device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32_t p, uint32_t n0, uint32_t n1,
-                                                 int64_t* s_key, int32_t* s_idx, uint32_t* s_ref, uint32_t* s_aref) {
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int32_t g = __ldg(a.group + p);
-    const int64_t rc = __ldg(a.req_cpu + p), rm = __ldg(a.req_mem + p);
+struct BindFilter {
+    int32_t g;
+    int64_t rc, rm;
     uint64_t sw[W];
+    uint32_t ck;
+    uint64_t lim[KS_SPREAD_MAX_KEYS];
+    const uint32_t* cnt;
+    uint32_t bB[KS_SPREAD_MAX_KEYS], bA[KS_SPREAD_MAX_KEYS]; // AFF: B_{g,k} / A_{g,k} bases, AFF_NONE = no such array
+    bool first;                                              // AFF: upstream's first-pod rule holds for g
+
+    __device__ __forceinline__ BindFilter(const SpreadBindArgs& a, uint32_t p) {
+        g = __ldg(a.group + p);
+        rc = __ldg(a.req_cpu + p);
+        rm = __ldg(a.req_mem + p);
 #pragma unroll
-    for (int w = 0; w < W; w++) sw[w] = __ldg(a.sel + (size_t)p * W + w);
-    const uint32_t ck = constrained_keys(a, g);
-    uint64_t lim[KS_SPREAD_MAX_KEYS]; // a domain admits while its count is below m + max_skew
-#pragma unroll
-    for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
-        lim[k] = (ck >> k & 1u) ? (uint64_t)__ldcg(a.gk + ((size_t)g * a.K + k) * GK_WORDS + GK_M) +
-                                      __ldg(a.max_skew + (size_t)g * a.K + k)
-                                : 0;
-    const uint32_t* cnt = a.cnt + (size_t)(g < 0 ? 0 : g) * a.S;
-    uint32_t bB[KS_SPREAD_MAX_KEYS], bA[KS_SPREAD_MAX_KEYS]; // B_{g,k} / A_{g,k} bases, AFF_NONE = no such array
-    bool first = false;                                      // upstream's first-pod rule holds for g
-    if constexpr (AFF) {
+        for (int w = 0; w < W; w++) sw[w] = __ldg(a.sel + (size_t)p * W + w);
+        ck = constrained_keys(a, g);
 #pragma unroll
         for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) {
-            const bool on = g >= 0 && k < a.K;
-            bB[k] = on ? __ldg(a.abase + ((size_t)g * a.K + k) * 2) : AFF_NONE;
-            bA[k] = on ? __ldg(a.abase + ((size_t)g * a.K + k) * 2 + 1) : AFF_NONE;
+            lim[k] = (ck >> k & 1u) ? (uint64_t)__ldcg(a.gk + ((size_t)g * a.K + k) * GK_WORDS + GK_M) +
+                                          __ldg(a.max_skew + (size_t)g * a.K + k)
+                                    : 0;
+            if constexpr (AFF) {
+                const bool on = g >= 0 && k < a.K;
+                bB[k] = on ? __ldg(a.abase + ((size_t)g * a.K + k) * 2) : AFF_NONE;
+                bA[k] = on ? __ldg(a.abase + ((size_t)g * a.K + k) * 2 + 1) : AFF_NONE;
+            }
         }
-        first = g >= 0 && (__ldg(a.aflag + g) & AFF_SELF) && __ldcg(a.acnt + a.any_base + g) == 0;
+        cnt = a.cnt + (size_t)(g < 0 ? 0 : g) * a.S;
+        if constexpr (AFF) first = g >= 0 && (__ldg(a.aflag + g) & AFF_SELF) && __ldcg(a.acnt + a.any_base + g) == 0;
     }
-    int64_t best = INT64_MIN;
-    int32_t bidx = -1;
-    uint32_t refused = 0, arefused = 0;
-    for (uint32_t n = n0 + tid; n < n1; n += SBD_THREADS) {
-        const int64_t fc = __ldcg(a.free_cpu + n), fm = __ldcg(a.free_mem + n);
+    // 0: unfit (fit or selector), 1: refused by spread, 2: refused by rules 1-3 (AFF), 3: candidate; NR (ks_node_bind)
+    // with the node's rule word rw: 4: refused by a taint, 5: refused by required node affinity, both before spread
+    template <bool NR = false>
+    __device__ __forceinline__ int test(const SpreadBindArgs& a, uint32_t n, int64_t fc, int64_t fm,
+                                        uint32_t rw = 0) const {
         uint64_t miss = 0;
 #pragma unroll
         for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
-        if (!(rc <= fc && rm <= fm && miss == 0)) continue;
+        if (!(rc <= fc && rm <= fm && miss == 0)) return 0;
+        if (NR && (rw & NR_REASON)) return 3 + (int)(rw & NR_REASON);
         bool ok = true;
 #pragma unroll
         for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
@@ -210,12 +214,9 @@ __device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32
                 const int32_t d = __ldg(a.dom + (size_t)k * a.N + n);
                 ok &= d >= 0 && __ldcg(cnt + a.Pk[k] + (uint32_t)max(d, 0)) < lim[k];
             }
-        if (!ok) {
-            refused++;
-            continue;
-        }
+        if (!ok) return 1;
+        bool aok = true;
         if constexpr (AFF) {
-            bool aok = true;
 #pragma unroll
             for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
                 if ((bB[k] & bA[k]) != AFF_NONE) {
@@ -224,12 +225,28 @@ __device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32
                     if (bB[k] != AFF_NONE) aok &= d < 0 || __ldcg(a.acnt + bB[k] + dd) == 0;        // rules 1 and 2
                     if (bA[k] != AFF_NONE) aok &= d >= 0 && (first || __ldcg(a.acnt + bA[k] + dd) > 0); // rule 3
                 }
-            if (!aok) {
-                arefused++;
-                continue;
-            }
         }
-        const int64_t key = alloc_score_rt(a.policy, fc, fm, a.alloc_cpu, a.alloc_mem, n, rc, rm);
+        return aok ? 3 : 2;
+    }
+};
+
+// Phase A of pod p in this CTA's slice [n0, n1): the filter; the best candidate by the policy's key (ties to the lower
+// node) and the spread refusals into the CTA's partial, AFF also the refusals of rules 1-3 (s_aref / paref).
+template <int W, bool AFF>
+__device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32_t p, uint32_t n0, uint32_t n1,
+                                                 int64_t* s_key, int32_t* s_idx, uint32_t* s_ref, uint32_t* s_aref) {
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const BindFilter<W, AFF> f(a, p);
+    int64_t best = INT64_MIN;
+    int32_t bidx = -1;
+    uint32_t refused = 0, arefused = 0;
+    for (uint32_t n = n0 + tid; n < n1; n += SBD_THREADS) {
+        const int64_t fc = __ldcg(a.free_cpu + n), fm = __ldcg(a.free_mem + n);
+        const int r = f.test(a, n, fc, fm);
+        refused += r == 1;
+        if constexpr (AFF) arefused += r == 2;
+        if (r != 3) continue;
+        const int64_t key = alloc_score_rt(a.policy, fc, fm, a.alloc_cpu, a.alloc_mem, n, f.rc, f.rm);
         if (key > best) { // ascending n per thread: strict '>' keeps the lowest index
             best = key;
             bidx = (int32_t)n;
@@ -263,10 +280,14 @@ __device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32
 // Phase B of pod p, CTA 0 only: merge the partials in CTA order, write the binding, charge free[] and raise the group's
 // counts.  When the last eligible domain at m takes the pod, m rises by exactly one and the domains at the new m are
 // counted over the group's domains of that key (the counts only rise, so at most final m - initial m such passes).
-// AFF: both refusals into out_refused[2p, 2p + 1], and the bound pod's update entries across the CTA (s_bidx).
-template <bool AFF>
+// The refusals go to out_refused[R * p + O] at the mode's stride R and offset O: 1 / 0 for SPREAD, 2 / 0 for AFFINITY
+// and PROFILE (spread, then affinity), 4 / 2 for NODE (after the taint and node-affinity words of profile_commit).
+// AFF: the bound pod's update entries across the CTA (s_bidx).
+template <BindMode M>
 __device__ __forceinline__ void spread_bind_commit(const SpreadBindArgs& a, uint32_t p, uint32_t* s_rescan,
                                                    uint32_t* s_red, int32_t* s_bidx) {
+    constexpr bool AFF = M != BIND_SPREAD;
+    constexpr size_t R = bind_refusal_words(M), O = M == BIND_NODE ? 2 : 0;
     const uint32_t tid = threadIdx.x, lane = tid & 31;
     const int32_t g = __ldg(a.group + p);
     if (tid < 32) {
@@ -285,12 +306,10 @@ __device__ __forceinline__ void spread_bind_commit(const SpreadBindArgs& a, uint
             uint32_t rescan = 0;
             a.out_idx[p] = bidx;
             a.out_score[p] = bidx >= 0 ? key_score_rt(a.policy, best, a.req_cpu, a.req_mem, p) : 0;
+            a.out_refused[R * p + O] = refused;
             if constexpr (AFF) {
-                a.out_refused[2 * (size_t)p] = refused;
-                a.out_refused[2 * (size_t)p + 1] = arefused;
+                a.out_refused[R * p + O + 1] = arefused;
                 *s_bidx = bidx;
-            } else {
-                a.out_refused[p] = refused;
             }
             if (bidx >= 0) {
                 a.free_cpu[bidx] = __ldcg(a.free_cpu + bidx) - __ldg(a.req_cpu + p);
@@ -331,27 +350,9 @@ __device__ __forceinline__ void spread_bind_commit(const SpreadBindArgs& a, uint
     }
 }
 
-template <int W>
-__global__ void __launch_bounds__(SBD_THREADS, 1) k_spread_bind_seq(const SpreadBindArgs a) {
-    cg::grid_group grid = cg::this_grid();
-    __shared__ int64_t s_key[SBD_WARPS];
-    __shared__ int32_t s_idx[SBD_WARPS];
-    __shared__ uint32_t s_ref[SBD_WARPS];
-    __shared__ uint32_t s_rescan;
-    const uint32_t G = gridDim.x;
-    const uint32_t chunk = (a.N + G - 1) / G, n0 = min(a.N, blockIdx.x * chunk), n1 = min(a.N, n0 + chunk);
-    for (uint32_t p = 0; p < a.P; p++) {
-        spread_bind_scan<W, false>(a, p, n0, n1, s_key, s_idx, s_ref, nullptr);
-        __threadfence();
-        grid.sync();
-        if (blockIdx.x == 0) spread_bind_commit<false>(a, p, &s_rescan, s_ref, nullptr);
-        __threadfence();
-        grid.sync();
-    }
-}
-
 // The existing pods' update entries into the zeroed counters, one warp per pod (grid-strided)
-__global__ void __launch_bounds__(SBD_THREADS) k_affinity_setup(const SpreadBindArgs a) {
+__global__ void __launch_bounds__(SBD_THREADS) k_affinity_setup(const ProfileBindArgs q) {
+    const SpreadBindArgs& a = q.b;
     const uint32_t lane = threadIdx.x & 31, warps = gridDim.x * SBD_WARPS;
     for (uint32_t e = blockIdx.x * SBD_WARPS + (threadIdx.x >> 5); e < a.E; e += warps) {
         const int32_t h = __ldg(a.ex_group + e), n = __ldg(a.ex_node + e);
@@ -360,137 +361,8 @@ __global__ void __launch_bounds__(SBD_THREADS) k_affinity_setup(const SpreadBind
     }
 }
 
-// k_spread_bind_seq with the AFF instances of both phases
-template <int W>
-__global__ void __launch_bounds__(SBD_THREADS, 1) k_affinity_bind_seq(const SpreadBindArgs a) {
-    cg::grid_group grid = cg::this_grid();
-    __shared__ int64_t s_key[SBD_WARPS];
-    __shared__ int32_t s_idx[SBD_WARPS];
-    __shared__ uint32_t s_ref[SBD_WARPS], s_aref[SBD_WARPS];
-    __shared__ uint32_t s_rescan;
-    __shared__ int32_t s_bidx;
-    const uint32_t G = gridDim.x;
-    const uint32_t chunk = (a.N + G - 1) / G, n0 = min(a.N, blockIdx.x * chunk), n1 = min(a.N, n0 + chunk);
-    for (uint32_t p = 0; p < a.P; p++) {
-        spread_bind_scan<W, true>(a, p, n0, n1, s_key, s_idx, s_ref, s_aref);
-        __threadfence();
-        grid.sync();
-        if (blockIdx.x == 0) spread_bind_commit<true>(a, p, &s_rescan, s_ref, &s_bidx);
-        __threadfence();
-        grid.sync();
-    }
-}
+// ---- ks_profile_bind and ks_node_bind: the soft scores ----
 
-uint32_t spread_bind_setup_grid(uint32_t G, int sms) { return std::max(1u, std::min<uint32_t>(G, 4u * (uint32_t)sms)); }
-
-cudaError_t launch_spread_bind(const SpreadBindArgs& a, uint32_t W, cudaStream_t st) {
-    return with_label_width(W, [&](auto w) {
-        constexpr int LW = decltype(w)::value;
-        if (a.G) {
-            k_spread_bind_setup<LW><<<a.setup_grid, SBD_THREADS, 0, st>>>(a);
-            g_launches++;
-            const cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) return e;
-        }
-        SpreadBindArgs b = a;
-        void* args[] = {&b};
-        const cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(k_spread_bind_seq<LW>),
-                                                          dim3(a.grid), dim3(SBD_THREADS), args, 0, st);
-        if (e == cudaSuccess) g_launches++;
-        return e;
-    });
-}
-
-cudaError_t launch_affinity_bind(const SpreadBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
-    return with_label_width(W, [&](auto w) {
-        constexpr int LW = decltype(w)::value;
-        if (a.G) {
-            k_spread_bind_setup<LW><<<a.setup_grid, SBD_THREADS, 0, st>>>(a);
-            g_launches++;
-            const cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) return e;
-        }
-        cudaError_t e = cudaMemsetAsync(a.acnt, 0, acnt_words * 4, st);
-        if (e != cudaSuccess) return e;
-        if (a.E) {
-            k_affinity_setup<<<a.aff_grid, SBD_THREADS, 0, st>>>(a);
-            g_launches++;
-            e = cudaGetLastError();
-            if (e != cudaSuccess) return e;
-        }
-        SpreadBindArgs b = a;
-        void* args[] = {&b};
-        e = cudaLaunchCooperativeKernel(reinterpret_cast<const void*>(k_affinity_bind_seq<LW>), dim3(a.grid),
-                                        dim3(SBD_THREADS), args, 0, st);
-        if (e == cudaSuccess) g_launches++;
-        return e;
-    });
-}
-
-
-// ---- ks_profile_bind ----
-// Its candidate filter is spread_bind_scan's rule for rule, with the AFF rules; spread_bind_scan keeps its own copy so
-// that the code of k_spread_bind_seq and k_affinity_bind_seq stays as it was.
-template <int W>
-struct ProfileFilter {
-    int32_t g;
-    int64_t rc, rm;
-    uint64_t sw[W];
-    uint32_t ck;
-    uint64_t lim[KS_SPREAD_MAX_KEYS];
-    const uint32_t* cnt;
-    uint32_t bB[KS_SPREAD_MAX_KEYS], bA[KS_SPREAD_MAX_KEYS];
-    bool first;
-
-    __device__ __forceinline__ ProfileFilter(const SpreadBindArgs& a, uint32_t p) {
-        g = __ldg(a.group + p);
-        rc = __ldg(a.req_cpu + p);
-        rm = __ldg(a.req_mem + p);
-#pragma unroll
-        for (int w = 0; w < W; w++) sw[w] = __ldg(a.sel + (size_t)p * W + w);
-        ck = constrained_keys(a, g);
-#pragma unroll
-        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) {
-            lim[k] = (ck >> k & 1u) ? (uint64_t)__ldcg(a.gk + ((size_t)g * a.K + k) * GK_WORDS + GK_M) +
-                                          __ldg(a.max_skew + (size_t)g * a.K + k)
-                                    : 0;
-            const bool on = g >= 0 && k < a.K;
-            bB[k] = on ? __ldg(a.abase + ((size_t)g * a.K + k) * 2) : AFF_NONE;
-            bA[k] = on ? __ldg(a.abase + ((size_t)g * a.K + k) * 2 + 1) : AFF_NONE;
-        }
-        cnt = a.cnt + (size_t)(g < 0 ? 0 : g) * a.S;
-        first = g >= 0 && (__ldg(a.aflag + g) & AFF_SELF) && __ldcg(a.acnt + a.any_base + g) == 0;
-    }
-    // 0: unfit (fit or selector), 1: refused by spread, 2: refused by rules 1-3, 3: candidate; NR (ks_node_bind) with
-    // the node's rule word rw: 4: refused by a taint, 5: refused by required node affinity, both before spread
-    template <bool NR = false>
-    __device__ __forceinline__ int test(const SpreadBindArgs& a, uint32_t n, int64_t fc, int64_t fm,
-                                        uint32_t rw = 0) const {
-        uint64_t miss = 0;
-#pragma unroll
-        for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
-        if (!(rc <= fc && rm <= fm && miss == 0)) return 0;
-        if (NR && (rw & NR_REASON)) return 3 + (int)(rw & NR_REASON);
-        bool ok = true;
-#pragma unroll
-        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
-            if (ck >> k & 1u) {
-                const int32_t d = __ldg(a.dom + (size_t)k * a.N + n);
-                ok &= d >= 0 && __ldcg(cnt + a.Pk[k] + (uint32_t)max(d, 0)) < lim[k];
-            }
-        if (!ok) return 1;
-        bool aok = true;
-#pragma unroll
-        for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++)
-            if ((bB[k] & bA[k]) != AFF_NONE) {
-                const int32_t d = __ldg(a.dom + (size_t)k * a.N + n);
-                const uint32_t dd = (uint32_t)max(d, 0);
-                if (bB[k] != AFF_NONE) aok &= d < 0 || __ldcg(a.acnt + bB[k] + dd) == 0;
-                if (bA[k] != AFF_NONE) aok &= d >= 0 && (first || __ldcg(a.acnt + bA[k] + dd) > 0);
-            }
-        return aok ? 3 : 2;
-    }
-};
 
 // CTA-wide minimum and maximum of one int64 pair per thread; every thread gets the result.  s holds 2 * SBD_WARPS words.
 __device__ __forceinline__ void cta_minmax(int64_t& mn, int64_t& mx, int64_t* s) {
@@ -574,7 +446,7 @@ __device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t
                                               ProfileShared& sh, NodeShared* ns = nullptr) {
     const SpreadBindArgs& b = a.b;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const ProfileFilter<W> f(b, p);
+    const BindFilter<W, true> f(b, p);
     const uint32_t sk = soft_keys(a, f.g);
     const bool all = f.g >= 0 && __ldg(a.soft_all + f.g);
     uint32_t* bits = a.bits + (size_t)(p & 1u) * a.BW;
@@ -865,14 +737,14 @@ __device__ __forceinline__ void profile_pass3(const ProfileBindArgs& a, uint32_t
 // Phase B, CTA 0: spread_bind_commit's merge, binding, charge, hard counts and B/A entries (the merged key is the total,
 // which key_score_rt returns unchanged for every policy this call accepts); then the parts of the winner, the soft
 // counts and the bound pod's IPA entries.  The winner's parts are read from its raws and sh's extremes, which pass 3
-// left in this CTA, and its policy score is the total less the weighted parts.  NR: five parts, and the four refusals
-// from the two that spread_bind_commit left in b.out_refused and the CTAs' taint and node-affinity partials.
+// left in this CTA, and its policy score is the total less the weighted parts.  NR: five parts, and the first two of the
+// four refusals, from the CTAs' taint and node-affinity partials.
 template <bool NR = false>
 __device__ __forceinline__ void profile_commit(const ProfileBindArgs& a, uint32_t p, ProfileShared& sh,
                                                NodeShared* ns = nullptr) {
     const SpreadBindArgs& b = a.b;
     const uint32_t tid = threadIdx.x;
-    spread_bind_commit<true>(b, p, &sh.rescan, sh.ref, &sh.bidx);
+    spread_bind_commit<NR ? BIND_NODE : BIND_PROFILE>(b, p, &sh.rescan, sh.ref, &sh.bidx);
     const int32_t g = __ldg(b.group + p), n = sh.bidx;
     const uint32_t sk = soft_keys(a, g);
     if (tid == 0 && a.out_parts) {
@@ -885,7 +757,7 @@ __device__ __forceinline__ void profile_commit(const ProfileBindArgs& a, uint32_
                 ps -= (int64_t)a.wtaint * tt + (int64_t)a.wnaff * na;
             }
         }
-        constexpr size_t PW = NR ? 5 : 3;
+        constexpr size_t PW = bind_part_words(NR ? BIND_NODE : BIND_PROFILE);
         a.out_parts[PW * p] = ps;
         a.out_parts[PW * p + 1] = pts;
         a.out_parts[PW * p + 2] = ipa;
@@ -904,11 +776,9 @@ __device__ __forceinline__ void profile_commit(const ProfileBindArgs& a, uint32_
             tr = __reduce_add_sync(0xffffffffu, tr);
             nr = __reduce_add_sync(0xffffffffu, nr);
         }
-        if (tid == 0) { // lane 0 wrote the two words of b.out_refused in spread_bind_commit
-            a.out_refused4[4 * (size_t)p] = tr;
-            a.out_refused4[4 * (size_t)p + 1] = nr;
-            a.out_refused4[4 * (size_t)p + 2] = __ldcg(b.out_refused + 2 * (size_t)p);
-            a.out_refused4[4 * (size_t)p + 3] = __ldcg(b.out_refused + 2 * (size_t)p + 1);
+        if (tid == 0) {
+            b.out_refused[4 * (size_t)p] = tr;
+            b.out_refused[4 * (size_t)p + 1] = nr;
         }
     }
     if (n < 0 || g < 0) return;
@@ -927,30 +797,6 @@ __device__ __forceinline__ void profile_commit(const ProfileBindArgs& a, uint32_
         if (d < 0) continue;
         int64_t* c = a.icnt + __ldg(a.ibase + (size_t)h * b.K + k) + (uint32_t)d;
         *c = __ldcg(c) + __ldg(a.icoef + e);
-    }
-}
-
-template <int W>
-__global__ void __launch_bounds__(SBD_THREADS, 1) k_profile_bind_seq(const ProfileBindArgs a) {
-    cg::grid_group grid = cg::this_grid();
-    __shared__ ProfileShared sh;
-    const uint32_t G = gridDim.x;
-    const uint32_t chunk = (a.b.N + G - 1) / G, n0 = min(a.b.N, blockIdx.x * chunk), n1 = min(a.b.N, n0 + chunk);
-    for (uint32_t p = 0; p < a.b.P; p++) {
-        profile_pass1<W>(a, p, n0, n1, sh);
-        __threadfence();
-        grid.sync();
-        if (soft_keys(a, __ldg(a.b.group + p))) { // uniform: every CTA knows the pod's group
-            profile_pass2(a, p, n0, n1, sh);
-            __threadfence();
-            grid.sync();
-        }
-        profile_pass3(a, p, n0, n1, sh);
-        __threadfence();
-        grid.sync();
-        if (blockIdx.x == 0) profile_commit(a, p, sh);
-        __threadfence();
-        grid.sync();
     }
 }
 
@@ -1001,86 +847,99 @@ __global__ void __launch_bounds__(SBD_THREADS) k_node_rules_setup(const ProfileB
     }
 }
 
-template <int W>
-__global__ void __launch_bounds__(SBD_THREADS) k_node_spread_setup(const ProfileBindArgs a) {
-    spread_bind_setup<W, true>(a.b, a.nrules, a.ncls);
-}
-
-// k_profile_bind_seq with the NR instances of its passes
-template <int W>
-__global__ void __launch_bounds__(SBD_THREADS, 1) k_node_bind_seq(const ProfileBindArgs a) {
+// The walk of every bind call: one cooperative launch, one node slice per CTA, the pods in queue order with grid
+// barriers between their phases.  SPREAD and AFFINITY run phase A and phase B; PROFILE and NODE run pass 1, pass 2 when
+// the pod's group has soft keys, pass 3 and the commit.  Each family declares only its own shared state.
+template <int W, BindMode M>
+__global__ void __launch_bounds__(SBD_THREADS, 1) k_bind_seq(const ProfileBindArgs a) {
+    constexpr bool AFF = M != BIND_SPREAD, NR = M == BIND_NODE;
     cg::grid_group grid = cg::this_grid();
-    __shared__ ProfileShared sh;
-    __shared__ NodeShared ns;
     const uint32_t G = gridDim.x;
     const uint32_t chunk = (a.b.N + G - 1) / G, n0 = min(a.b.N, blockIdx.x * chunk), n1 = min(a.b.N, n0 + chunk);
-    for (uint32_t p = 0; p < a.b.P; p++) {
-        profile_pass1<W, true>(a, p, n0, n1, sh, &ns);
-        __threadfence();
-        grid.sync();
-        if (soft_keys(a, __ldg(a.b.group + p))) { // uniform: every CTA knows the pod's group
-            profile_pass2(a, p, n0, n1, sh);
+    if constexpr (M == BIND_SPREAD || M == BIND_AFFINITY) {
+        __shared__ int64_t s_key[SBD_WARPS];
+        __shared__ int32_t s_idx[SBD_WARPS];
+        __shared__ uint32_t s_ref[SBD_WARPS], s_aref[SBD_WARPS]; // s_aref: AFF only
+        __shared__ uint32_t s_rescan;
+        __shared__ int32_t s_bidx; // AFF only
+        for (uint32_t p = 0; p < a.b.P; p++) {
+            spread_bind_scan<W, AFF>(a.b, p, n0, n1, s_key, s_idx, s_ref, s_aref);
+            __threadfence();
+            grid.sync();
+            if (blockIdx.x == 0) spread_bind_commit<M>(a.b, p, &s_rescan, s_ref, &s_bidx);
             __threadfence();
             grid.sync();
         }
-        profile_pass3<true>(a, p, n0, n1, sh, &ns);
-        __threadfence();
-        grid.sync();
-        if (blockIdx.x == 0) profile_commit<true>(a, p, sh, &ns);
-        __threadfence();
-        grid.sync();
+    } else {
+        __shared__ ProfileShared sh;
+        __shared__ NodeShared ns; // NR only
+        for (uint32_t p = 0; p < a.b.P; p++) {
+            profile_pass1<W, NR>(a, p, n0, n1, sh, &ns);
+            __threadfence();
+            grid.sync();
+            if (soft_keys(a, __ldg(a.b.group + p))) { // uniform: every CTA knows the pod's group
+                profile_pass2(a, p, n0, n1, sh);
+                __threadfence();
+            grid.sync();
+            }
+            profile_pass3<NR>(a, p, n0, n1, sh, &ns);
+            __threadfence();
+            grid.sync();
+            if (blockIdx.x == 0) profile_commit<NR>(a, p, sh, &ns);
+            __threadfence();
+            grid.sync();
+        }
     }
 }
 
-// ks_profile_bind's launches; NR: k_node_rules_setup first, and the NR kernels in place of the spread setup and the walk
-template <bool NR>
-static cudaError_t launch_profile(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
+uint32_t bind_setup_grid(uint32_t G, int sms) { return std::max(1u, std::min<uint32_t>(G, 4u * (uint32_t)sms)); }
+
+cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
     return with_label_width(W, [&](auto w) {
         constexpr int LW = decltype(w)::value;
         const SpreadBindArgs& b = a.b;
-        if (NR) {
+        const bool nr = mode == BIND_NODE, soft = mode == BIND_PROFILE || nr;
+        const auto launched = [](uint32_t n) {
+            g_launches += n;
+            return cudaGetLastError();
+        };
+        cudaError_t e;
+        if (nr) {
             k_node_rules_setup<<<a.rules_grid, SBD_THREADS, 0, st>>>(a);
-            g_launches++;
-            const cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) return e;
+            if ((e = launched(1)) != cudaSuccess) return e;
         }
         if (b.G) {
-            if (NR) k_node_spread_setup<LW><<<b.setup_grid, SBD_THREADS, 0, st>>>(a);
-            else k_spread_bind_setup<LW><<<b.setup_grid, SBD_THREADS, 0, st>>>(b);
-            g_launches++;
-            const cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) return e;
+            if (nr) k_bind_setup<LW, true><<<b.setup_grid, SBD_THREADS, 0, st>>>(a);
+            else k_bind_setup<LW, false><<<b.setup_grid, SBD_THREADS, 0, st>>>(a);
+            if ((e = launched(1)) != cudaSuccess) return e;
         }
-        cudaError_t e = cudaMemsetAsync(b.acnt, 0, acnt_words * 4, st);
-        if (e == cudaSuccess) e = cudaMemsetAsync(a.icnt, 0, a.iwords * 8, st);
-        if (e == cudaSuccess) e = cudaMemsetAsync(a.bits, 0, (size_t)a.BW * 8, st);
-        if (e == cudaSuccess && (uint64_t)b.G * b.S)
-            e = b.existing ? cudaMemcpyAsync(a.scnt, b.existing, (size_t)b.G * b.S * 4, cudaMemcpyDeviceToDevice, st)
-                           : cudaMemsetAsync(a.scnt, 0, (size_t)b.G * b.S * 4, st);
-        if (e != cudaSuccess) return e;
-        if (b.E) {
-            k_affinity_setup<<<b.aff_grid, SBD_THREADS, 0, st>>>(b);
-            k_profile_setup<<<b.aff_grid, SBD_THREADS, 0, st>>>(a);
-            g_launches += 2;
-            e = cudaGetLastError();
+        if (mode != BIND_SPREAD) {
+            e = cudaMemsetAsync(b.acnt, 0, acnt_words * 4, st);
+            if (soft) {
+                if (e == cudaSuccess) e = cudaMemsetAsync(a.icnt, 0, a.iwords * 8, st);
+                if (e == cudaSuccess) e = cudaMemsetAsync(a.bits, 0, (size_t)a.BW * 8, st);
+                if (e == cudaSuccess && b.G && b.S)
+                    e = b.existing
+                            ? cudaMemcpyAsync(a.scnt, b.existing, (size_t)b.G * b.S * 4, cudaMemcpyDeviceToDevice, st)
+                            : cudaMemsetAsync(a.scnt, 0, (size_t)b.G * b.S * 4, st);
+            }
             if (e != cudaSuccess) return e;
+            if (b.E) {
+                k_affinity_setup<<<b.aff_grid, SBD_THREADS, 0, st>>>(a);
+                if (soft) k_profile_setup<<<b.aff_grid, SBD_THREADS, 0, st>>>(a);
+                if ((e = launched(soft ? 2 : 1)) != cudaSuccess) return e;
+            }
         }
+        const void* walk = mode == BIND_SPREAD     ? reinterpret_cast<const void*>(k_bind_seq<LW, BIND_SPREAD>)
+                           : mode == BIND_AFFINITY ? reinterpret_cast<const void*>(k_bind_seq<LW, BIND_AFFINITY>)
+                           : mode == BIND_PROFILE  ? reinterpret_cast<const void*>(k_bind_seq<LW, BIND_PROFILE>)
+                                                   : reinterpret_cast<const void*>(k_bind_seq<LW, BIND_NODE>);
         ProfileBindArgs c = a;
         void* args[] = {&c};
-        e = cudaLaunchCooperativeKernel(NR ? reinterpret_cast<const void*>(k_node_bind_seq<LW>)
-                                           : reinterpret_cast<const void*>(k_profile_bind_seq<LW>),
-                                        dim3(b.grid), dim3(SBD_THREADS), args, 0, st);
+        e = cudaLaunchCooperativeKernel(walk, dim3(b.grid), dim3(SBD_THREADS), args, 0, st);
         if (e == cudaSuccess) g_launches++;
         return e;
     });
-}
-
-cudaError_t launch_profile_bind(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
-    return launch_profile<false>(a, acnt_words, W, st);
-}
-
-cudaError_t launch_node_bind(const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
-    return launch_profile<true>(a, acnt_words, W, st);
 }
 
 } // namespace ks
