@@ -34,6 +34,7 @@ pub const KSH_RECONCILE_GANG_UNSATISFIED: c_int = 4; // ksh_reconcile_gangs: the
 pub const KSH_RECONCILE_SPREAD_UNSATISFIED: c_int = 5; // ksh_reconcile_spread: spread constraints refused every node
 pub const KSH_RECONCILE_AFFINITY_UNSATISFIED: c_int = 6; // ksh_reconcile_affinity: pod (anti-)affinity refused every node
 pub const KSH_RECONCILE_NODE_RULES_UNSATISFIED: c_int = 7; // ksh_reconcile_nodes: taints or node affinity refused every node
+pub const KSH_RECONCILE_INSUFFICIENT_RESOURCES: c_int = 8; // ksh_reconcile_fit: every node that fit lacked a resource
 pub const KS_REFERENCE_ATTEMPTS: u32 = 5; // ATTEMPTS, src/main.rs:49
 pub const KS_MAX_PEERS: usize = 15;
 pub const KS_TOPK_MAX: u32 = 32; // largest k of ks_select_topk / ksh_rank_nodes
@@ -65,6 +66,7 @@ pub const KS_NODE_RULES_MAX_TAINTS: u32 = 64; // ks_node_bind
 pub const KS_NODE_RULES_MAX_KEYS: usize = 16;
 pub const KS_NODE_RULES_MAX_PREFERRED: u32 = 4096;
 pub const KS_NODE_RULES_MAX_WORDS: u64 = 1 << 26;
+pub const KS_BIND_MAX_RESOURCES: u32 = 8; // ks_fit_bind: most scalar resources of one call
 
 #[repr(C)]
 pub struct ks_kv {
@@ -261,6 +263,12 @@ pub struct ks_node_rules {
     pub weight_node_affinity: u32,
 }
 #[repr(C)]
+pub struct ks_bind_resources {
+    pub n_res: u32,
+    pub node_free: *const i64,
+    pub pod_req: *const i64,
+}
+#[repr(C)]
 pub struct ksh_taint {
     pub key: *const c_char,
     pub value: *const c_char,
@@ -373,6 +381,11 @@ extern "C" {
                         topo: *const ks_spread_multi, aff: *const ks_pod_affinity, scoring: *const ks_bind_scoring,
                         rules: *const ks_node_rules, policy: c_int, node_idx: *mut i32, score: *mut i64,
                         parts: *mut i64, refused: *mut u32, domain_count: *mut u32, soft_count: *mut u32) -> c_int;
+    pub fn ks_fit_bind(s: *mut ks_snapshot, pods: *const ks_pods, group: *const i32, n_groups: u32,
+                       topo: *const ks_spread_multi, aff: *const ks_pod_affinity, scoring: *const ks_bind_scoring,
+                       rules: *const ks_node_rules, res: *const ks_bind_resources, policy: c_int, node_idx: *mut i32,
+                       score: *mut i64, parts: *mut i64, refused: *mut u32, domain_count: *mut u32,
+                       soft_count: *mut u32, free: *mut i64) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -457,6 +470,15 @@ extern "C" {
                                scoring: *const ks_bind_scoring, rules: *const ksh_node_rules, policy: c_int,
                                status: *mut i32, node_idx: *mut i32, json: *mut c_char, cap: usize,
                                json_off: *mut i64) -> c_int;
+    pub fn ksh_compile_resources(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, names: *mut c_char, cap: usize,
+                                 node_free: *mut i64, pod_req: *mut i64) -> c_int;
+    pub fn ksh_reconcile_fit(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group: *const i32, n_groups: u32,
+                             topology_keys: *const *const c_char, n_keys: u32, max_skew: *const u32,
+                             min_domains: *const u32, existing_node_names: *const *const c_char,
+                             existing_offset: *const u64, aff: *const ksh_pod_affinity,
+                             scoring: *const ks_bind_scoring, rules: *const ksh_node_rules, policy: c_int,
+                             status: *mut i32, node_idx: *mut i32, json: *mut c_char, cap: usize,
+                             json_off: *mut i64) -> c_int;
     pub fn ksh_reconcile_profile(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group: *const i32,
                                  n_groups: u32, topology_keys: *const *const c_char, n_keys: u32, max_skew: *const u32,
                                  min_domains: *const u32, existing_node_names: *const *const c_char,

@@ -915,6 +915,58 @@ int ks_node_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const int
                  uint32_t* out_refused /* [4P] or NULL */, uint32_t* out_domain_count /* [G * S] or NULL */,
                  uint32_t* out_soft_count /* [G * S] or NULL */);
 
+/* ---- extended resources when binding: ks_node_bind with the rest of upstream's NodeResourcesFit filter, the pod
+ * count and every scalar resource a pod requests (restated here; spec extension, DESIGN.md 5r) ----
+ * The arguments of ks_node_bind plus `res` (host memory, may be NULL) and out_free.  R = res->n_res resources, each a
+ * row of node_free [R * N] (resource r of node n at r * N + n: allocatable minus what the pods already bound there
+ * request; any int64, negative included) and a column of pod_req [P * R] (pod p's request of r at p * R + r, >= 0).
+ * Resources are what the caller names them: upstream's pod count is a resource whose node_free is allocatable "pods"
+ * minus the pods bound there and whose request is 1 for every pod, group -1 included; nvidia.com/gpu, other extended
+ * resources, ephemeral-storage and hugepages-* are resources whose requests are the pods' requests.
+ * The fit rule (upstream fitsRequest): node n passes resource r for pod p iff pod_req[p * R + r] == 0 or
+ * pod_req[p * R + r] <= free_r[n], free_r[n] being r's free amount at p's turn; a zero request is skipped, so a node with
+ * negative free_r still takes a pod that does not request r.  The pod count's `len(pods) + 1 > allowed` is `1 > free`.
+ * cpu and memory keep ks_select's rule (no zero skip).
+ * For pod p of group g and node n, the filters run in this order: cpu, memory and selector; the R resources; taints;
+ * required node affinity; hard spread; rules 1-3 of ks_affinity_bind.  Spread eligibility is ks_node_bind's: resources
+ * play no part in it, as upstream.  When p binds on n, free_r[n] -= pod_req[p * R + r] for every r, alongside free[];
+ * the scores are ks_node_bind's (the default profile scores cpu and memory only).
+ * rules NULL: an empty rule set (no taint, no term) with both plugin weights 0, so the total is ks_profile_bind's; out_parts
+ * words 3 and 4 are then 0, as ks_node_bind's K1.
+ * Outputs as ks_node_bind's, except: out_refused[5p] = the nodes that pass cpu, memory and selector but fail some
+ * resource, and out_refused[5p + 1 .. 5p + 4] = ks_node_bind's four words over the nodes that pass every resource;
+ * out_free [R * N] (or NULL) = free_r after the call.
+ * Identities, policies 1, 3 and 4:
+ *   (L1) res NULL: every output is ks_node_bind's, bit for bit, and every out_refused[5p] is 0;
+ *   (L2) every request 0: the outputs are L1's, and out_free == node_free, negative entries included;
+ *   (L3) always: out_free[r * N + n] == node_free[r * N + n] - the sum of pod_req[p * R + r] over the pods bound on n;
+ *   (L4) every node_free at least the queue's total request of its resource: nodes, scores, parts, words 1-4, both counts
+ *        and free[] are ks_node_bind's;
+ *   (L5) a resource whose request is each pod's cpu request (all positive) and whose node_free is free_cpu changes
+ *        nothing.
+ * Checked on the host before any device work and before free[] changes: every check of ks_node_bind; KS_ERR_RANGE for
+ * R > KS_BIND_MAX_RESOURCES or a negative request; KS_ERR_INVALID for a NULL node_free (R > 0, N > 0) or pod_req
+ * (R > 0, P > 0).
+ * With rules given, the call makes ks_node_bind's launches; with rules NULL, one more than ks_node_bind (which then runs
+ * ks_profile_bind's walk, K1): k_node_rules_setup over the empty rule set.  Each pod's cycle loads one int64 per node
+ * for each resource the pod requests.
+ * Out of scope: resources in ks_select, ks_stream_bind, ks_gang_bind, the planners and ks_explain; scoring by them;
+ * initContainers and pod overhead; ignoredResources. */
+#define KS_BIND_MAX_RESOURCES 8u
+typedef struct ks_bind_resources {            /* host memory */
+    uint32_t n_res;                           /* R in [0, KS_BIND_MAX_RESOURCES] */
+    const int64_t* node_free;                 /* [R * N] */
+    const int64_t* pod_req;                   /* [P * R], each >= 0 */
+} ks_bind_resources;
+int ks_fit_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const int32_t* group /* [P] */,
+                uint32_t n_groups, const ks_spread_multi* topo /* keys; max_skew may be NULL */,
+                const ks_pod_affinity* aff /* or NULL */, const ks_bind_scoring* scoring,
+                const ks_node_rules* rules /* or NULL */, const ks_bind_resources* res /* or NULL */, int policy,
+                int32_t* out_node_idx /* [P] */, int64_t* out_score /* [P] or NULL */,
+                int64_t* out_parts /* [5P] or NULL */, uint32_t* out_refused /* [5P] or NULL */,
+                uint32_t* out_domain_count /* [G * S] or NULL */, uint32_t* out_soft_count /* [G * S] or NULL */,
+                int64_t* out_free /* [R * N] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

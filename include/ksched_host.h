@@ -46,6 +46,9 @@ extern "C" {
 #define KSH_RECONCILE_NODE_RULES_UNSATISFIED 7 /* ksh_reconcile_nodes: some node fit (resources and selector) but taints
                                                   or required node affinity refused every such node (upstream:
                                                   "untolerated taint" / "didn't match Pod's node affinity/selector") */
+#define KSH_RECONCILE_INSUFFICIENT_RESOURCES 8 /* ksh_reconcile_fit: some node passed cpu, memory and selector but every
+                                                  such node lacked a scalar resource the pod requests or was at its pod
+                                                  limit (upstream: "Insufficient nvidia.com/gpu" / "Too many pods") */
 
 /* Kubernetes quantity strings, exact: cpu -> millicores, memory -> bytes.
  * KS_ERR_PARSE (malformed), KS_ERR_INEXACT (finer than 1m / 1 byte), KS_ERR_RANGE. */
@@ -386,6 +389,38 @@ int ksh_reconcile_nodes(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pod
                         const ksh_pod_affinity* aff /* or NULL */, const ks_bind_scoring* scoring,
                         const ksh_node_rules* rules /* or NULL */, int policy, int32_t* out_status,
                         int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off);
+
+/* Extended resources (ks_fit_bind, DESIGN.md 5r).  The context keeps, per node, the allocatable quantity of every name
+ * other than cpu and memory (from ks_node_obj.allocatable), and per bound pod its non-zero requests of such names summed
+ * over spec.containers, as it keeps cpu and memory; every node and pod event keeps them in step.  Quantities parse as
+ * integers, as memory does.  A quantity that does not parse is recorded, not rejected, so no other call changes: the
+ * calls below report it, naming the node or pod, only when the batch requests that resource: KS_ERR_PARSE for a
+ * quantity that does not parse, KS_ERR_RANGE for a pod whose requests of one name sum past int64 over its containers.
+ * A batch's resources: "pods" first, then every name other than cpu and memory that some pod of the batch requests with
+ * a non-zero quantity, in order of first request; more than KS_BIND_MAX_RESOURCES is KS_ERR_RANGE (split the batch).
+ * node_free[r * N + n] = node n's allocatable of resource r minus the requests of the pods bound there ("pods": minus
+ * their number); a name missing from a node's allocatable counts as 0, as upstream, so a node without "pods" takes no
+ * pod (callers that build synthetic nodes must list it).  pod_req[p * R + r] = pod p's request (1 for "pods").
+ * ksh_compile_resources writes the names of the batch `pods` (taken whole, as the pods that go to the device) into
+ * names (each NUL-terminated; KS_ERR_RANGE when they do not fit in cap), node_free [R * N] and pod_req [n_pods * R]
+ * (either may be NULL; size them for R = KS_BIND_MAX_RESOURCES) and returns R.  Pure host work: works on a packing-only
+ * context. */
+int ksh_compile_resources(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, char* names, size_t cap,
+                          int64_t* out_node_free, int64_t* out_pod_req);
+
+/* reconcile() under the default profile with taints, node affinity and NodeResourcesFit's pod count and scalar
+ * resources: ksh_reconcile_nodes' arguments, bound by ks_fit_bind over the batch's resources (the pods that go to the
+ * device).  An unbound pod gets KSH_RECONCILE_INSUFFICIENT_RESOURCES when some node passed cpu, memory and selector but
+ * every such node failed a resource, else the statuses of ksh_reconcile_nodes over the nodes that pass every resource.
+ * Each bind is recorded with its extended requests, so the next call sees them.  Errors as ksh_reconcile_nodes,
+ * ks_fit_bind and ksh_compile_resources. */
+int ksh_reconcile_fit(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, const int32_t* group,
+                      uint32_t n_groups, const char* const* topology_keys, uint32_t n_keys,
+                      const uint32_t* max_skew /* or NULL */, const uint32_t* min_domains,
+                      const char* const* existing_node_names, const uint64_t* existing_offset,
+                      const ksh_pod_affinity* aff /* or NULL */, const ks_bind_scoring* scoring,
+                      const ksh_node_rules* rules /* or NULL */, int policy, int32_t* out_status,
+                      int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off);
 
 #ifdef __cplusplus
 }

@@ -263,12 +263,23 @@ class ks_node_rules(C.Structure):
 _proto("ks_node_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_uint32,
        C.POINTER(ks_spread_multi), C.POINTER(ks_pod_affinity), C.POINTER(ks_bind_scoring), C.POINTER(ks_node_rules),
        C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
+KS_BIND_MAX_RESOURCES = 8
+
+
+class ks_bind_resources(C.Structure):
+    _fields_ = [("n_res", C.c_uint32), ("node_free", C.c_void_p), ("pod_req", C.c_void_p)]
+
+
+_proto("ks_fit_bind", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_uint32,
+       C.POINTER(ks_spread_multi), C.POINTER(ks_pod_affinity), C.POINTER(ks_bind_scoring), C.POINTER(ks_node_rules),
+       C.POINTER(ks_bind_resources), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+       C.c_void_p, optional=True)
 KS_AFFINITY_MAX_TERMS = 16384
 KS_AFFINITY_MAX_TARGETS = 1 << 22
 KS_AFFINITY_MAX_EXISTING = 1 << 24
 KS_AFFINITY_MAX_UPDATES = 1 << 24
 KS_PREEMPT_MAX_ABS_SUM = 1 << 62
-KS_ERR_INVALID, KS_ERR_RANGE = -1, -5
+KS_ERR_INVALID, KS_ERR_PARSE, KS_ERR_RANGE = -1, -3, -5
 KS_REFERENCE_ATTEMPTS = 5
 _SAMPLING_MULT = 0xD1B54A32D192ED03
 

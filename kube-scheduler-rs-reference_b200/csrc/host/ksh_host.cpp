@@ -38,6 +38,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 #pragma weak ks_affinity_bind
 #pragma weak ks_profile_bind
 #pragma weak ks_node_bind
+#pragma weak ks_fit_bind
 
 namespace {
 
@@ -252,6 +253,16 @@ struct PosTable {
     }
 };
 
+// One quantity of a scalar resource (numbered by ksh_context::res_id).  A quantity that does not parse, or a pod's sum
+// over its containers that leaves int64, is kept with its error rather than rejected, so that every call that ignores
+// these resources behaves as before; a call that needs the resource reports it (ext_error).
+enum : uint8_t { EXT_OK = 0, EXT_PARSE = 1, EXT_OVERFLOW = 2 };
+struct ExtQty {
+    uint32_t res;
+    uint8_t err; // EXT_OK, EXT_PARSE or EXT_OVERFLOW; v is meaningful only with EXT_OK
+    int64_t v;
+};
+
 struct ksh_context {
     ks_snapshot* snap = nullptr;
     uint32_t N = 0;
@@ -288,6 +299,12 @@ struct ksh_context {
     bool dirty = true; // device snapshot must be re-uploaded
     // spec.taints by node name (ksh_context_set_node_taints): key, value, effect
     std::unordered_map<std::string, std::vector<std::array<std::string, 3>>> taints;
+    // scalar resources other than cpu and memory (ksh_reconcile_fit, DESIGN.md 5r): names numbered once; per node its
+    // allocatable quantities, per bound row its non-zero requests (empty for a pod without extended requests)
+    std::unordered_map<std::string, uint32_t> res_id;
+    std::vector<std::string> res_name;
+    std::vector<std::vector<ExtQty>> node_ext; // [N]
+    std::vector<std::vector<ExtQty>> bext;     // per bound row, in step with bnode
     // one lock per context: every ksh_* entry that takes a context holds it for the whole call (entries call each other)
     mutable std::recursive_mutex mu;
 };
@@ -597,6 +614,57 @@ static int64_t btab_slot_of_pos(const ksh_context* c, size_t pos) {
 
 static void bound_erase(ksh_context* c, size_t pos);
 
+static uint32_t res_id(ksh_context* c, const char* name) {
+    const auto it = c->res_id.find(name);
+    if (it != c->res_id.end()) return it->second;
+    const uint32_t id = (uint32_t)c->res_name.size();
+    c->res_name.emplace_back(name);
+    c->res_id.emplace(name, id);
+    return id;
+}
+
+static inline bool cpu_or_memory(const char* k) { return !std::strcmp(k, "cpu") || !std::strcmp(k, "memory"); }
+
+// The pod's requests of every resource but cpu and memory, summed over spec.containers as total_pod_resources sums cpu
+// and memory; zero sums dropped
+static std::vector<ExtQty> pod_ext(ksh_context* c, const ks_pod_obj* pod) {
+    std::vector<ExtQty> out;
+    if (!pod->has_spec) return out;
+    for (uint32_t i = 0; i < pod->n_containers; i++) {
+        const ks_container_obj& ct = pod->containers[i];
+        if (!ct.has_requests) continue;
+        for (uint32_t j = 0; j < ct.n_requests; j++) {
+            const ks_kv& kv = ct.requests[j];
+            if (!kv.key || cpu_or_memory(kv.key)) continue;
+            int64_t v = 0;
+            const uint8_t err = parse_quantity(kv.val, 0, &v) != KS_OK ? EXT_PARSE : EXT_OK;
+            const uint32_t r = res_id(c, kv.key);
+            auto it = std::find_if(out.begin(), out.end(), [r](const ExtQty& e) { return e.res == r; });
+            if (it == out.end()) out.push_back({r, err, err ? 0 : v});
+            else if (err) it->err = it->err ? it->err : err;
+            else if (!it->err && __builtin_add_overflow(it->v, v, &it->v)) it->err = EXT_OVERFLOW;
+        }
+    }
+    out.erase(std::remove_if(out.begin(), out.end(), [](const ExtQty& e) { return !e.err && e.v == 0; }), out.end());
+    return out;
+}
+
+// The node's allocatable quantities of every resource but cpu and memory ("pods" included), the first of a repeated key
+static std::vector<ExtQty> node_ext(ksh_context* c, const ks_node_obj& nd) {
+    std::vector<ExtQty> out;
+    if (!nd.has_allocatable) return out;
+    for (uint32_t j = 0; j < nd.n_allocatable; j++) {
+        const ks_kv& kv = nd.allocatable[j];
+        if (!kv.key || cpu_or_memory(kv.key)) continue;
+        const uint32_t r = res_id(c, kv.key);
+        if (std::any_of(out.begin(), out.end(), [r](const ExtQty& e) { return e.res == r; })) continue;
+        int64_t v = 0;
+        const uint8_t err = parse_quantity(kv.val, 0, &v) != KS_OK ? EXT_PARSE : EXT_OK;
+        out.push_back({r, err, err ? 0 : v});
+    }
+    return out;
+}
+
 // append a bound pod; a tracked key that is already present REPLACES its row (last one wins, as a map would): the old
 // row is removed so its requests are no longer charged, and the device copy is re-uploaded from the host truth
 static void bound_push(ksh_context* c, const ks_pod_obj* pod, uint64_t h, size_t lns, size_t lname, int32_t node, int64_t cpu,
@@ -613,6 +681,7 @@ static void bound_push(ksh_context* c, const ks_pod_obj* pod, uint64_t h, size_t
         }
     }
     const size_t pos = c->bnode.size();
+    c->bext.push_back(pod_ext(c, pod));
     c->bnode.push_back(node);
     c->bcpu.push_back(cpu);
     c->bmem.push_back(mem);
@@ -677,7 +746,9 @@ static void bound_erase(ksh_context* c, size_t pos) { // swap-remove
         c->boff[pos] = c->boff[last];
         c->blen[pos] = c->blen[last];
         c->bprio[pos] = c->bprio[last];
+        c->bext[pos] = std::move(c->bext[last]);
     }
+    c->bext.pop_back();
     c->bnode.pop_back();
     c->bcpu.pop_back();
     c->bmem.pop_back();
@@ -689,6 +760,7 @@ static void bound_erase(ksh_context* c, size_t pos) { // swap-remove
 }
 
 static void bound_clear(ksh_context* c) {
+    c->bext.clear();
     c->bnode.clear();
     c->bcpu.clear();
     c->bmem.clear();
@@ -993,6 +1065,7 @@ int ksh_context_set_nodes(ksh_context* c, const ks_node_obj* nodes, uint32_t n) 
     c->pair_bit.clear();
     c->bit2pair.clear();
     c->node_pids.assign(n, {});
+    c->node_ext.assign(n, {});
     c->N = n;
     c->alloc_cpu.swap(ac);
     c->alloc_mem.swap(am);
@@ -1001,6 +1074,7 @@ int ksh_context_set_nodes(ksh_context* c, const ks_node_obj* nodes, uint32_t n) 
         if (id == c->nameid2idx.size()) c->nameid2idx.push_back((int32_t)i); // first node of a name wins
         c->idx2nameid[i] = id;
         node_pairs_set(c, i, nodes[i]);
+        c->node_ext[i] = node_ext(c, nodes[i]);
     }
     for (const std::string& pk : named) {
         const char* k = pk.c_str();
@@ -1036,6 +1110,7 @@ int ksh_context_upsert_node(ksh_context* c, const ks_node_obj* node, uint32_t* o
         c->alloc_cpu.push_back(ac);
         c->alloc_mem.push_back(am);
         c->node_pids.emplace_back();
+        c->node_ext.emplace_back();
     } else {
         idx = (uint32_t)c->nameid2idx[id];
         c->alloc_cpu[idx] = ac;
@@ -1043,6 +1118,7 @@ int ksh_context_upsert_node(ksh_context* c, const ks_node_obj* node, uint32_t* o
         node_pairs_release(c, idx);
     }
     node_pairs_set(c, idx, *node);
+    c->node_ext[idx] = node_ext(c, *node);
     gc_pairs(c);
     c->dirty = true;
     if (out_idx) *out_idx = idx;
@@ -1063,6 +1139,7 @@ int ksh_context_remove_node(ksh_context* c, const char* name) try {
     c->alloc_cpu.erase(c->alloc_cpu.begin() + idx);
     c->alloc_mem.erase(c->alloc_mem.begin() + idx);
     c->node_pids.erase(c->node_pids.begin() + idx);
+    c->node_ext.erase(c->node_ext.begin() + idx);
     c->N--;
     // later nodes move down by one index; a name carried by several rows points to its first remaining row
     for (uint32_t i = c->N; i-- > idx;) c->nameid2idx[c->idx2nameid[i]] = (int32_t)i;
@@ -1170,6 +1247,7 @@ int ksh_context_set_cluster_pods(ksh_context* c, const ks_pod_obj* pods, uint64_
     c->boff.reserve(kept);
     c->blen.reserve(kept);
     c->bprio.reserve(kept);
+    c->bext.reserve(kept);
     c->bkeys.reserve(key_bytes);
     btab_rebuild(c, kept); // sized once for the whole list
     for (uint64_t p = 0; p < n; p++)
@@ -1902,6 +1980,76 @@ static int compile_node_rules(ksh_context* c, uint32_t G, const ksh_node_rules* 
     return KS_OK;
 }
 
+// ---- extended resources (ks_fit_bind, DESIGN.md 5r) ----
+// The scalar resources of a pending batch: "pods", then every other name some pod of the batch requests with a non-zero
+// quantity, in order of first request; node_free [R * N] = allocatable (0 when the node does not list the name) minus
+// the requests of the rows bound on the node (for "pods", the rows themselves); pod_req [P * R] (1 for "pods").
+struct CompiledResources {
+    std::vector<uint32_t> ids; // resource ids, ids[0] = "pods"
+    std::vector<int64_t> node_free, pod_req;
+};
+
+static std::string pod_key(const ks_pod_obj* pod) { return std::string(nz(pod->ns)) + "/" + nz(pod->name); }
+
+// The error of a recorded quantity e of `who` ("pod 'ns/name'", "node 'name'", ...): KS_ERR_PARSE for a quantity that
+// does not parse, KS_ERR_RANGE for a pod's requests that sum past int64
+static int ext_error(const ksh_context* c, const std::string& who, const char* what, const ExtQty& e) {
+    if (e.err == EXT_OVERFLOW)
+        return fail(KS_ERR_RANGE, who + ": its " + c->res_name[e.res] + " requests sum past int64");
+    return fail(KS_ERR_PARSE, who + ": cannot convert its " + what + c->res_name[e.res] + " to an integer");
+}
+
+static int compile_resources(ksh_context* c, const ks_pod_obj* pods, uint64_t n, CompiledResources* out) {
+    const uint32_t pods_id = res_id(c, "pods");
+    out->ids.assign(1, pods_id);
+    std::vector<std::vector<ExtQty>> req(n);
+    for (uint64_t p = 0; p < n; p++) {
+        req[p] = pod_ext(c, &pods[p]);
+        for (const ExtQty& e : req[p]) {
+            if (e.res == pods_id) continue; // the pod count is not requested: every pod counts 1
+            if (e.err) return ext_error(c, "pod '" + pod_key(&pods[p]) + "'", "request of ", e);
+            if (e.v < 0)
+                return fail(KS_ERR_RANGE, "pod '" + pod_key(&pods[p]) + "': negative " + c->res_name[e.res] + " request");
+            if (std::find(out->ids.begin(), out->ids.end(), e.res) == out->ids.end()) out->ids.push_back(e.res);
+        }
+    }
+    const size_t R = out->ids.size(), N = c->N;
+    if (R > KS_BIND_MAX_RESOURCES)
+        return fail(KS_ERR_RANGE, std::to_string(R) + " resources in one batch, \"pods\" included (at most " +
+                                      std::to_string(KS_BIND_MAX_RESOURCES) + "): split the batch");
+    std::vector<int32_t> col(c->res_name.size(), -1);
+    for (size_t r = 0; r < R; r++) col[out->ids[r]] = (int32_t)r;
+    out->node_free.assign(R * N, 0);
+    for (size_t i = 0; i < N; i++)
+        for (const ExtQty& e : c->node_ext[i]) {
+            if (col[e.res] < 0) continue;
+            if (e.err)
+                return ext_error(c, std::string("node '") + c->names.str(c->idx2nameid[i]) + "'", "allocatable ", e);
+            out->node_free[(size_t)col[e.res] * N + i] = e.v;
+        }
+    for (size_t b = 0; b < c->bnode.size(); b++) {
+        const size_t node = (size_t)c->bnode[b];
+        int64_t& pc = out->node_free[node];
+        bool over = __builtin_sub_overflow(pc, 1, &pc);
+        for (const ExtQty& e : c->bext[b]) {
+            if (e.res >= col.size() || col[e.res] <= 0) continue;
+            if (e.err)
+                return ext_error(c, "bound pod '" + std::string(c->bkeys.data() + c->boff[b], c->blen[b]) + "'",
+                                 "request of ", e);
+            int64_t& f = out->node_free[(size_t)col[e.res] * N + node];
+            over |= __builtin_sub_overflow(f, e.v, &f);
+        }
+        if (over) return fail(KS_ERR_RANGE, "free resources of a node overflow int64");
+    }
+    out->pod_req.assign(n * R, 0);
+    for (uint64_t p = 0; p < n; p++) {
+        out->pod_req[p * R] = 1;
+        for (const ExtQty& e : req[p])
+            if (col[e.res] > 0) out->pod_req[p * R + (size_t)col[e.res]] = e.v;
+    }
+    return KS_OK;
+}
+
 // reconcile() under topology spread: ksh_reconcile_batch's filtering, then ks_spread_bind over the pods that go to the
 // device, each in its group.  Group g's existing pods under key k count when their node is in the store and carries key k
 // and every key g constrains.  With aff set (ksh_reconcile_affinity), ks_affinity_bind with its terms and the existing
@@ -1913,7 +2061,7 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
                             const uint64_t* existing_offset, const ksh_pod_affinity* aff, int policy, int32_t* out_status,
                             int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off,
                             const ks_bind_scoring* sc = nullptr, const ksh_node_rules* nr = nullptr,
-                            bool nodes = false) {
+                            bool nodes = false, bool fit = false) {
     if (!c || !topology_keys || (n && (!pods || !group || !out_status || !out_node_idx)) || (n_groups && !max_skew && !aff))
         return fail(KS_ERR_INVALID, "NULL argument");
     if (K == 0 || K > KS_SPREAD_MAX_KEYS)
@@ -1931,7 +2079,8 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     if (aff && aff->n_existing && (!aff->existing_group || !aff->existing_node_name))
         return fail(KS_ERR_INVALID, "NULL existing_group or existing_node_name");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    int rc = nodes ? device_ready(c, ks_node_bind, "ks_node_bind")
+    int rc = fit     ? device_ready(c, ks_fit_bind, "ks_fit_bind")
+             : nodes ? device_ready(c, ks_node_bind, "ks_node_bind")
              : sc  ? device_ready(c, ks_profile_bind, "ks_profile_bind")
              : aff ? device_ready(c, ks_affinity_bind, "ks_affinity_bind")
                    : device_ready(c, ks_spread_bind, "ks_spread_bind");
@@ -1954,6 +2103,11 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
         if (rc) return rc;
     }
     if (todo.empty()) return KS_OK;
+    CompiledResources res;
+    if (fit) { // before the device, so a bad quantity fails the whole call
+        rc = compile_resources(c, sub.data(), sub.size(), &res);
+        if (rc) return rc;
+    }
     ks_pods kp;
     rc = pack_batch(c, sub.data(), sub.size(), &kp);
     if (rc) return rc;
@@ -1988,7 +2142,8 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     sp.min_domains = min_domains;
     sp.existing = existing_offset ? existing.data() : nullptr;
     std::vector<int32_t> idx(sub.size(), -1);
-    const size_t R = nodes ? 4 : aff ? 2 : 1; // refusal words per pod: [taint, node affinity,] spread, then affinity
+    // refusal words per pod: [resources,] [taint, node affinity,] spread, then affinity
+    const size_t R = fit ? 5 : nodes ? 4 : aff ? 2 : 1;
     std::vector<uint32_t> refused(sub.size() * R, 0);
     if (aff) {
         ks_pod_affinity pa{aff->n_terms, aff->owner, aff->kind, aff->key, aff->target_offset, aff->target, 0, nullptr,
@@ -2003,7 +2158,10 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
         pa.n_existing = eg.size();
         pa.existing_group = eg.data();
         pa.existing_node = en.data();
-        rc = nodes ? ks_node_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, &cr.r, policy, idx.data(),
+        const ks_bind_resources br{(uint32_t)res.ids.size(), res.node_free.data(), res.pod_req.data()};
+        rc = fit     ? ks_fit_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, &cr.r, &br, policy,
+                                   idx.data(), nullptr, nullptr, refused.data(), nullptr, nullptr, nullptr)
+             : nodes ? ks_node_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, &cr.r, policy, idx.data(),
                                   nullptr, nullptr, refused.data(), nullptr, nullptr)
              : sc ? ks_profile_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, policy, idx.data(), nullptr,
                                   nullptr, refused.data(), nullptr, nullptr)
@@ -2018,13 +2176,17 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
         return rc;
     }
     StringList bodies{json, cap};
-    const size_t F = nodes ? 2 : 0; // the spread and affinity words follow the two node-rule words
+    // the node-rule words follow the resource word, the spread and affinity words follow the two node-rule words
+    const size_t X = fit ? 1 : 0, F = nodes ? X + 2 : 0;
     for (size_t k = 0; k < todo.size(); k++) {
         const uint64_t i = todo[k];
+        const uint32_t* w = &refused[k * R];
         if (idx[k] >= 0)
             commit_bind(c, &pods[i], idx[k], kp.req_cpu[k], kp.req_mem[k], &out_status[i], &out_node_idx[i], bodies,
                         json && out_json_off ? &out_json_off[i] : nullptr);
-        else if (nodes && refused[k * R] + refused[k * R + 1] > 0 && refused[k * R + 2] == 0 && refused[k * R + 3] == 0)
+        else if (fit && w[0] > 0 && w[1] + w[2] + w[3] + w[4] == 0)
+            out_status[i] = KSH_RECONCILE_INSUFFICIENT_RESOURCES;
+        else if (nodes && w[X] + w[X + 1] > 0 && w[X + 2] == 0 && w[X + 3] == 0)
             out_status[i] = KSH_RECONCILE_NODE_RULES_UNSATISFIED;
         else if (refused[k * R + F] > 0)
             out_status[i] = KSH_RECONCILE_SPREAD_UNSATISFIED;
@@ -2149,6 +2311,37 @@ int ksh_reconcile_nodes(ksh_context* c, const ks_pod_obj* pods, uint64_t n, cons
     return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
                             existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
                             out_json_off, scoring, rules, true);
+}
+KSH_CATCH
+
+int ksh_compile_resources(ksh_context* c, const ks_pod_obj* pods, uint64_t n, char* names, size_t cap,
+                          int64_t* out_node_free, int64_t* out_pod_req) try {
+    if (!c || (n && !pods) || (cap && !names)) return fail(KS_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    CompiledResources res;
+    const int rc = compile_resources(c, pods, n, &res);
+    if (rc) return rc;
+    StringList list{names, cap};
+    for (const uint32_t id : res.ids)
+        if (list.append(c->res_name[id].c_str(), c->res_name[id].size() + 1) < 0)
+            return fail(KS_ERR_RANGE, "the resource names do not fit in cap bytes");
+    if (out_node_free) std::copy(res.node_free.begin(), res.node_free.end(), out_node_free);
+    if (out_pod_req) std::copy(res.pod_req.begin(), res.pod_req.end(), out_pod_req);
+    return (int)res.ids.size();
+}
+KSH_CATCH
+
+int ksh_reconcile_fit(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
+                      const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
+                      const uint32_t* min_domains, const char* const* existing_node_names,
+                      const uint64_t* existing_offset, const ksh_pod_affinity* aff, const ks_bind_scoring* scoring,
+                      const ksh_node_rules* rules, int policy, int32_t* out_status, int32_t* out_node_idx, char* json,
+                      size_t cap, int64_t* out_json_off) try {
+    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
+    const ksh_pod_affinity none{};
+    return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
+                            existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
+                            out_json_off, scoring, rules, true, true);
 }
 KSH_CATCH
 

@@ -2086,17 +2086,19 @@ static int compile_node_rules(const ks_node_rules* r, uint32_t G, uint32_t N, No
 }
 
 // last_path and the name in launch errors of each BindMode
-static const char* const BIND_PATH[] = {"spread_bind", "affinity_bind", "profile_bind", "node_bind"};
-static const char* const BIND_NAME[] = {"spread bind", "affinity bind", "profile bind", "node bind"};
+static const char* const BIND_PATH[] = {"spread_bind", "affinity_bind", "profile_bind", "node_bind", "fit_bind"};
+static const char* const BIND_NAME[] = {"spread bind", "affinity bind", "profile bind", "node bind", "fit bind"};
 
 // ks_spread_bind, and with aff set ks_affinity_bind (then max_skew may be NULL), and with aff and sc set ks_profile_bind
-// (out_parts and out_soft_count [G * S] may be given), and with nr set as well ks_node_bind; out_refused and out_parts
-// hold the mode's words per pod (bind_refusal_words, bind_part_words)
+// (out_parts and out_soft_count [G * S] may be given), and with nr set as well ks_node_bind, and with res set as well
+// ks_fit_bind (out_free [R * N] may be given); out_refused and out_parts hold the mode's words per pod
+// (bind_refusal_words, bind_part_words)
 static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
                        const ks_spread_multi* spread, const ks_pod_affinity* aff, int policy, int32_t* out_node_idx,
                        int64_t* out_score, uint32_t* out_refused, uint32_t* out_domain_count,
                        const ks_bind_scoring* sc = nullptr, int64_t* out_parts = nullptr,
-                       uint32_t* out_soft_count = nullptr, const ks_node_rules* nr = nullptr) {
+                       uint32_t* out_soft_count = nullptr, const ks_node_rules* nr = nullptr,
+                       const ks_bind_resources* res = nullptr, int64_t* out_free = nullptr) {
     int rc = check_pods(s, pods);
     if (rc) return rc;
     if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "%s takes host-space pods", call);
@@ -2151,6 +2153,14 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     }
     rc = check_commit_requests(P, pods->req_cpu, pods->req_mem);
     if (rc) return rc;
+    const uint64_t RS = res ? res->n_res : 0; // ks_fit_bind's scalar resources
+    if (RS > KS_BIND_MAX_RESOURCES)
+        return fail(KS_ERR_RANGE, "%llu resources (at most %u)", (unsigned long long)RS, KS_BIND_MAX_RESOURCES);
+    if (RS && ((N && !res->node_free) || (P && !res->pod_req))) return fail(KS_ERR_INVALID, "NULL node_free or pod_req");
+    for (uint64_t i = 0; i < P * RS; i++)
+        if (res->pod_req[i] < 0)
+            return fail(KS_ERR_RANGE, "pod %llu: request %lld of resource %llu (at least 0)", (unsigned long long)(i / RS),
+                        (long long)res->pod_req[i], (unsigned long long)(i % RS));
     AffinityPlan plan;
     if (aff) {
         try {
@@ -2169,8 +2179,9 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         }
         if (rc) return rc;
     }
-    const BindMode mode = nr ? BIND_NODE : sc ? BIND_PROFILE : aff ? BIND_AFFINITY : BIND_SPREAD;
+    const BindMode mode = res ? BIND_FIT : nr ? BIND_NODE : sc ? BIND_PROFILE : aff ? BIND_AFFINITY : BIND_SPREAD;
     const uint64_t R = bind_refusal_words(mode), PW = bind_part_words(mode);
+    if (out_free && RS && N && (P == 0)) memcpy(out_free, res->node_free, RS * N * 8); // nothing binds: L3
     if (P == 0) return KS_OK;
     if (N == 0) { // no node: nothing is placed, every count is existing
         memset(out_node_idx, 0xff, P * 4);
@@ -2271,6 +2282,11 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     const auto nrules = h.work<uint32_t>((uint64_t)nplan.C * N);
     const auto ptref = h.work<uint32_t>(NR1 * a.grid), pnref = h.work<uint32_t>(NR1 * a.grid);
     const auto ptmax = h.work<uint32_t>(NR1 * a.grid), pnmax = h.work<uint32_t>(NR1 * a.grid);
+    // ks_fit_bind: the requests, the caller's free amounts and the charged ones, one row per resource
+    const auto res_req = h.in(RS ? res->pod_req : nullptr, P * RS);
+    const auto res_node_free = h.in(RS ? res->node_free : nullptr, RS * N);
+    const auto res_free = h.out(out_free, RS * N);
+    const auto pfref = h.work<uint32_t>(res ? a.grid : 0);
     auto put = [&](Staged<uint32_t> d, const std::vector<uint32_t>& v) {
         if (!v.empty()) memcpy(h.host(d), v.data(), v.size() * 4);
     };
@@ -2405,6 +2421,13 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         q.rules_grid = (uint32_t)std::max<uint64_t>(
             1, std::min<uint64_t>(((uint64_t)nplan.C * N + 255) / 256, 4ull * (uint64_t)s->sms));
     }
+    if (res) {
+        q.R = (uint32_t)RS;
+        q.res_req = h.dev(res_req);
+        q.res_node_free = h.dev(res_node_free);
+        q.res_free = h.dev(res_free);
+        q.pfref = h.dev(pfref);
+    }
     s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
     s->version++;
     const cudaError_t e = launch_bind(mode, q, plan.words, W, st);
@@ -2473,6 +2496,23 @@ int ks_node_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint
             out_parts[5 * p + 3] = out_parts[5 * p + 4] = 0;
         }
     }
+    return KS_OK;
+}
+
+int ks_fit_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
+                const ks_spread_multi* topo, const ks_pod_affinity* aff, const ks_bind_scoring* scoring,
+                const ks_node_rules* rules, const ks_bind_resources* res, int policy, int32_t* out_node_idx,
+                int64_t* out_score, int64_t* out_parts, uint32_t* out_refused, uint32_t* out_domain_count,
+                uint32_t* out_soft_count, int64_t* out_free) {
+    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
+    const ks_pod_affinity none{};
+    const ks_node_rules no_rules{}; // no taint, no term, both plugin weights 0: the total is ks_profile_bind's
+    const ks_bind_resources no_res{};
+    const int rc = bind_spread(s, "ks_fit_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
+                               out_score, out_refused, out_domain_count, scoring, out_parts, out_soft_count,
+                               rules ? rules : &no_rules, res ? res : &no_res, out_free);
+    if (rc || rules || !out_parts) return rc;
+    for (uint64_t p = 0; p < pods->n; p++) out_parts[5 * p + 3] = out_parts[5 * p + 4] = 0; // as ks_node_bind's K1
     return KS_OK;
 }
 

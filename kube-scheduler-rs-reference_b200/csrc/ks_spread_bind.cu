@@ -1,11 +1,12 @@
 // ks_spread_bind.cu — the bind calls of include/ksched.h: ks_spread_bind (topology spread, DESIGN.md 5m),
 // ks_affinity_bind (and inter-pod affinity, 5n), ks_profile_bind (and the soft PodTopologySpread and InterPodAffinity
-// scores, 5o) and ks_node_bind (and TaintToleration and NodeAffinity, 5p).
+// scores, 5o), ks_node_bind (and TaintToleration and NodeAffinity, 5p) and ks_fit_bind (and the pod count and scalar
+// resources of NodeResourcesFit, 5r).
 // Each binds a mixed pod queue one pod at a time, each pod against the counts and the free[] every earlier pod left, as
 // upstream kube-scheduler runs one scheduling cycle per pod.  The calls differ by one BindMode (ks_launch.h), SPREAD,
-// AFFINITY, PROFILE or NODE, and share:
-//   BindFilter          the candidate filter: fit and selector, (NODE) the node's rule word, hard spread and (AFF, every
-//                       mode but SPREAD) rules 1-3 of the header
+// AFFINITY, PROFILE, NODE or FIT (NODE's launches and walk, with the resources), and share:
+//   BindFilter          the candidate filter: fit and selector, (FIT) the scalar resources, (NODE, FIT) the node's rule
+//                       word, hard spread and (AFF, every mode but SPREAD) rules 1-3 of the header
 //   k_bind_setup        one CTA per group (grid-strided): the group's eligible domains per constrained key, its counts
 //                       (existing, or 0), and per key |E|, m, the number of eligible domains at m and the minDomains flag;
 //                       NR (NODE) also drops the nodes that fail the group's required node affinity
@@ -17,7 +18,7 @@
 //                       total exists, then the same commit.
 //   launch_bind         one mode's launches, in order
 // Per call, k_affinity_setup and k_profile_setup apply the existing pods' update entries (every mode but SPREAD, and
-// PROFILE and NODE), and k_node_rules_setup writes one rule word per (node-rule class, node) (NODE).
+// PROFILE, NODE and FIT), and k_node_rules_setup writes one rule word per (node-rule class, node) (NODE, FIT).
 #include "ks_internal.cuh"
 #include "ks_launch.h"
 
@@ -164,8 +165,9 @@ __device__ __forceinline__ void affinity_raise(const SpreadBindArgs& a, uint32_t
 // The candidate filter of every bind walk for pod p: fit, selector and, for a constrained pod, cnt < m + max_skew on
 // every constrained key (the bound formed once per pod); AFF: then rules 1-3 of ks_affinity_bind against the pod's
 // group's counter bases and first-pod flag, formed once per pod.  Without AFF (ks_spread_bind, whose abase, aflag and
-// acnt are NULL) none of them is read.
-template <int W, bool AFF>
+// acnt are NULL) none of them is read.  FIT (ks_fit_bind): after fit and selector, the scalar resources the pod requests,
+// their mask and amounts formed once per pod; the other instances read none of it.
+template <int W, bool AFF, bool FIT = false>
 struct BindFilter {
     int32_t g;
     int64_t rc, rm;
@@ -175,6 +177,21 @@ struct BindFilter {
     const uint32_t* cnt;
     uint32_t bB[KS_SPREAD_MAX_KEYS], bA[KS_SPREAD_MAX_KEYS]; // AFF: B_{g,k} / A_{g,k} bases, AFF_NONE = no such array
     bool first;                                              // AFF: upstream's first-pod rule holds for g
+    uint32_t rmask;                                          // FIT: bit r = the pod requests resource r
+    int64_t rreq[KS_BIND_MAX_RESOURCES];                     // FIT: its requests
+    const int64_t* rfree;                                    // FIT: free_r[n] at r * N + n
+
+    __device__ __forceinline__ BindFilter(const ProfileBindArgs& q, uint32_t p) : BindFilter(q.b, p) {
+        if constexpr (FIT) {
+            rmask = 0;
+            rfree = q.res_free;
+#pragma unroll
+            for (uint32_t r = 0; r < KS_BIND_MAX_RESOURCES; r++) {
+                rreq[r] = r < q.R ? __ldg(q.res_req + (size_t)p * q.R + r) : 0;
+                if (rreq[r]) rmask |= 1u << r;
+            }
+        }
+    }
 
     __device__ __forceinline__ BindFilter(const SpreadBindArgs& a, uint32_t p) {
         g = __ldg(a.group + p);
@@ -198,7 +215,8 @@ struct BindFilter {
         if constexpr (AFF) first = g >= 0 && (__ldg(a.aflag + g) & AFF_SELF) && __ldcg(a.acnt + a.any_base + g) == 0;
     }
     // 0: unfit (fit or selector), 1: refused by spread, 2: refused by rules 1-3 (AFF), 3: candidate; NR (ks_node_bind)
-    // with the node's rule word rw: 4: refused by a taint, 5: refused by required node affinity, both before spread
+    // with the node's rule word rw: 4: refused by a taint, 5: refused by required node affinity, both before spread;
+    // FIT: 6: refused by a scalar resource, before the taints
     template <bool NR = false>
     __device__ __forceinline__ int test(const SpreadBindArgs& a, uint32_t n, int64_t fc, int64_t fm,
                                         uint32_t rw = 0) const {
@@ -206,6 +224,13 @@ struct BindFilter {
 #pragma unroll
         for (int w = 0; w < W; w++) miss |= sw[w] & ~__ldg(a.labels + (size_t)w * a.Npad + n);
         if (!(rc <= fc && rm <= fm && miss == 0)) return 0;
+        if constexpr (FIT) {
+            bool fits = true;
+#pragma unroll
+            for (uint32_t r = 0; r < KS_BIND_MAX_RESOURCES; r++)
+                if (rmask >> r & 1u) fits &= rreq[r] <= __ldcg(rfree + (size_t)r * a.N + n);
+            if (!fits) return 6;
+        }
         if (NR && (rw & NR_REASON)) return 3 + (int)(rw & NR_REASON);
         bool ok = true;
 #pragma unroll
@@ -281,13 +306,14 @@ __device__ __forceinline__ void spread_bind_scan(const SpreadBindArgs& a, uint32
 // counts.  When the last eligible domain at m takes the pod, m rises by exactly one and the domains at the new m are
 // counted over the group's domains of that key (the counts only rise, so at most final m - initial m such passes).
 // The refusals go to out_refused[R * p + O] at the mode's stride R and offset O: 1 / 0 for SPREAD, 2 / 0 for AFFINITY
-// and PROFILE (spread, then affinity), 4 / 2 for NODE (after the taint and node-affinity words of profile_commit).
-// AFF: the bound pod's update entries across the CTA (s_bidx).
+// and PROFILE (spread, then affinity), 4 / 2 for NODE (after the taint and node-affinity words of profile_commit), 5 / 3
+// for FIT (after the resource word and the two node-rule words).  AFF: the bound pod's update entries across the CTA
+// (s_bidx).
 template <BindMode M>
 __device__ __forceinline__ void spread_bind_commit(const SpreadBindArgs& a, uint32_t p, uint32_t* s_rescan,
                                                    uint32_t* s_red, int32_t* s_bidx) {
     constexpr bool AFF = M != BIND_SPREAD;
-    constexpr size_t R = bind_refusal_words(M), O = M == BIND_NODE ? 2 : 0;
+    constexpr size_t R = bind_refusal_words(M), O = M == BIND_FIT ? 3 : M == BIND_NODE ? 2 : 0;
     const uint32_t tid = threadIdx.x, lane = tid & 31;
     const int32_t g = __ldg(a.group + p);
     if (tid < 32) {
@@ -440,13 +466,15 @@ __device__ __forceinline__ const uint32_t* node_row(const ProfileBindArgs& a, in
 // bitmap and merged into the parity's global bitmap once per CTA, a higher one is marked there directly.  Each new
 // bit counts one domain, so the partials add up to the distinct domains.  The other parity's bitmap is cleared.
 // NR (ks_node_bind): the node's rule word first; the taint and node-affinity refusals and, over the candidates, the
-// maxima of both raws into the CTA's partials.
-template <int W, bool NR = false>
+// maxima of both raws into the CTA's partials.  FIT (ks_fit_bind, with NR): also the resource refusals, per warp in
+// s_fref, into the CTA's partial pfref.
+template <int W, bool NR = false, bool FIT = false>
 __device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t p, uint32_t n0, uint32_t n1,
                                               ProfileShared& sh, NodeShared* ns = nullptr) {
+    __shared__ uint32_t s_fref[SBD_WARPS]; // FIT only
     const SpreadBindArgs& b = a.b;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const BindFilter<W, true> f(b, p);
+    const BindFilter<W, true, FIT> f(a, p);
     const uint32_t sk = soft_keys(a, f.g);
     const bool all = f.g >= 0 && __ldg(a.soft_all + f.g);
     uint32_t* bits = a.bits + (size_t)(p & 1u) * a.BW;
@@ -466,6 +494,7 @@ __device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t
     int64_t imin = INT64_MAX, imax = INT64_MIN;
     const uint32_t* nrow = NR ? node_row(a, f.g) : nullptr;
     uint32_t tref = 0, nref = 0, tmax = 0, nmax = 0;
+    uint32_t fref = 0; // FIT only
     for (uint32_t n = n0 + tid; n < n1; n += SBD_THREADS) {
         const uint32_t rw = NR ? __ldg(nrow + n) : 0u;
         const int r = f.template test<NR>(b, n, __ldcg(b.free_cpu + n), __ldcg(b.free_mem + n), rw);
@@ -475,6 +504,7 @@ __device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t
             tref += r == 4;
             nref += r == 5;
         }
+        if constexpr (FIT) fref += r == 6;
         if (r != 3) {
             a.iraw[n] = PB_NOT_CAND;
             continue;
@@ -531,6 +561,10 @@ __device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t
             ns->nmax[warp] = nmax;
         }
     }
+    if constexpr (FIT) {
+        fref = __reduce_add_sync(0xffffffffu, fref);
+        if (lane == 0) s_fref[warp] = fref;
+    }
     if (sk) {
 #pragma unroll
         for (uint32_t k = 0; k < KS_SPREAD_MAX_KEYS; k++) {
@@ -576,6 +610,12 @@ __device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t
             a.pnref[blockIdx.x] = nr;
             a.ptmax[blockIdx.x] = tm;
             a.pnmax[blockIdx.x] = nm;
+        }
+        if constexpr (FIT) {
+            uint32_t fr = 0;
+#pragma unroll
+            for (uint32_t w = 0; w < SBD_WARPS; w++) fr += s_fref[w];
+            a.pfref[blockIdx.x] = fr;
         }
     }
 }
@@ -738,14 +778,26 @@ __device__ __forceinline__ void profile_pass3(const ProfileBindArgs& a, uint32_t
 // which key_score_rt returns unchanged for every policy this call accepts); then the parts of the winner, the soft
 // counts and the bound pod's IPA entries.  The winner's parts are read from its raws and sh's extremes, which pass 3
 // left in this CTA, and its policy score is the total less the weighted parts.  NR: five parts, and the first two of the
-// four refusals, from the CTAs' taint and node-affinity partials.
-template <bool NR = false>
+// four refusals, from the CTAs' taint and node-affinity partials.  FIT (with NR): the resource refusals in word 0 of
+// five, the node-rule words after it, and free_r of the winner charged.
+template <bool NR = false, bool FIT = false>
 __device__ __forceinline__ void profile_commit(const ProfileBindArgs& a, uint32_t p, ProfileShared& sh,
                                                NodeShared* ns = nullptr) {
     const SpreadBindArgs& b = a.b;
     const uint32_t tid = threadIdx.x;
-    spread_bind_commit<NR ? BIND_NODE : BIND_PROFILE>(b, p, &sh.rescan, sh.ref, &sh.bidx);
+    spread_bind_commit<FIT ? BIND_FIT : NR ? BIND_NODE : BIND_PROFILE>(b, p, &sh.rescan, sh.ref, &sh.bidx);
     const int32_t g = __ldg(b.group + p), n = sh.bidx;
+    if constexpr (FIT) {
+        uint32_t fr = 0;
+        if (tid < 32) {
+            for (uint32_t c = threadIdx.x; c < gridDim.x; c += 32) fr += __ldcg(a.pfref + c);
+            fr = __reduce_add_sync(0xffffffffu, fr);
+        }
+        if (tid == 0) b.out_refused[5 * (size_t)p] = fr;
+        if (n >= 0 && tid < a.R)
+            a.res_free[(size_t)tid * b.N + n] = __ldcg(a.res_free + (size_t)tid * b.N + n) -
+                                                __ldg(a.res_req + (size_t)p * a.R + tid);
+    }
     const uint32_t sk = soft_keys(a, g);
     if (tid == 0 && a.out_parts) {
         int64_t pts = 0, ipa = 0, ps = 0, tt = 0, na = 0;
@@ -757,7 +809,7 @@ __device__ __forceinline__ void profile_commit(const ProfileBindArgs& a, uint32_
                 ps -= (int64_t)a.wtaint * tt + (int64_t)a.wnaff * na;
             }
         }
-        constexpr size_t PW = bind_part_words(NR ? BIND_NODE : BIND_PROFILE);
+        constexpr size_t PW = bind_part_words(FIT ? BIND_FIT : NR ? BIND_NODE : BIND_PROFILE);
         a.out_parts[PW * p] = ps;
         a.out_parts[PW * p + 1] = pts;
         a.out_parts[PW * p + 2] = ipa;
@@ -777,8 +829,13 @@ __device__ __forceinline__ void profile_commit(const ProfileBindArgs& a, uint32_
             nr = __reduce_add_sync(0xffffffffu, nr);
         }
         if (tid == 0) {
-            b.out_refused[4 * (size_t)p] = tr;
-            b.out_refused[4 * (size_t)p + 1] = nr;
+            if constexpr (FIT) { // after the resource word
+                b.out_refused[5 * (size_t)p + 1] = tr;
+                b.out_refused[5 * (size_t)p + 2] = nr;
+            } else {
+                b.out_refused[4 * (size_t)p] = tr;
+                b.out_refused[4 * (size_t)p + 1] = nr;
+            }
         }
     }
     if (n < 0 || g < 0) return;
@@ -852,7 +909,7 @@ __global__ void __launch_bounds__(SBD_THREADS) k_node_rules_setup(const ProfileB
 // the pod's group has soft keys, pass 3 and the commit.  Each family declares only its own shared state.
 template <int W, BindMode M>
 __global__ void __launch_bounds__(SBD_THREADS, 1) k_bind_seq(const ProfileBindArgs a) {
-    constexpr bool AFF = M != BIND_SPREAD, NR = M == BIND_NODE;
+    constexpr bool AFF = M != BIND_SPREAD, NR = M == BIND_NODE || M == BIND_FIT, FIT = M == BIND_FIT;
     cg::grid_group grid = cg::this_grid();
     const uint32_t G = gridDim.x;
     const uint32_t chunk = (a.b.N + G - 1) / G, n0 = min(a.b.N, blockIdx.x * chunk), n1 = min(a.b.N, n0 + chunk);
@@ -874,7 +931,7 @@ __global__ void __launch_bounds__(SBD_THREADS, 1) k_bind_seq(const ProfileBindAr
         __shared__ ProfileShared sh;
         __shared__ NodeShared ns; // NR only
         for (uint32_t p = 0; p < a.b.P; p++) {
-            profile_pass1<W, NR>(a, p, n0, n1, sh, &ns);
+            profile_pass1<W, NR, FIT>(a, p, n0, n1, sh, &ns);
             __threadfence();
             grid.sync();
             if (soft_keys(a, __ldg(a.b.group + p))) { // uniform: every CTA knows the pod's group
@@ -885,7 +942,7 @@ __global__ void __launch_bounds__(SBD_THREADS, 1) k_bind_seq(const ProfileBindAr
             profile_pass3<NR>(a, p, n0, n1, sh, &ns);
             __threadfence();
             grid.sync();
-            if (blockIdx.x == 0) profile_commit<NR>(a, p, sh, &ns);
+            if (blockIdx.x == 0) profile_commit<NR, FIT>(a, p, sh, &ns);
             __threadfence();
             grid.sync();
         }
@@ -898,7 +955,7 @@ cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_w
     return with_label_width(W, [&](auto w) {
         constexpr int LW = decltype(w)::value;
         const SpreadBindArgs& b = a.b;
-        const bool nr = mode == BIND_NODE, soft = mode == BIND_PROFILE || nr;
+        const bool fit = mode == BIND_FIT, nr = mode == BIND_NODE || fit, soft = mode == BIND_PROFILE || nr;
         const auto launched = [](uint32_t n) {
             g_launches += n;
             return cudaGetLastError();
@@ -922,6 +979,8 @@ cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_w
                     e = b.existing
                             ? cudaMemcpyAsync(a.scnt, b.existing, (size_t)b.G * b.S * 4, cudaMemcpyDeviceToDevice, st)
                             : cudaMemsetAsync(a.scnt, 0, (size_t)b.G * b.S * 4, st);
+                if (e == cudaSuccess && fit && a.R)
+                    e = cudaMemcpyAsync(a.res_free, a.res_node_free, (size_t)a.R * b.N * 8, cudaMemcpyDeviceToDevice, st);
             }
             if (e != cudaSuccess) return e;
             if (b.E) {
@@ -933,7 +992,8 @@ cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_w
         const void* walk = mode == BIND_SPREAD     ? reinterpret_cast<const void*>(k_bind_seq<LW, BIND_SPREAD>)
                            : mode == BIND_AFFINITY ? reinterpret_cast<const void*>(k_bind_seq<LW, BIND_AFFINITY>)
                            : mode == BIND_PROFILE  ? reinterpret_cast<const void*>(k_bind_seq<LW, BIND_PROFILE>)
-                                                   : reinterpret_cast<const void*>(k_bind_seq<LW, BIND_NODE>);
+                           : mode == BIND_NODE     ? reinterpret_cast<const void*>(k_bind_seq<LW, BIND_NODE>)
+                                                   : reinterpret_cast<const void*>(k_bind_seq<LW, BIND_FIT>);
         ProfileBindArgs c = a;
         void* args[] = {&c};
         e = cudaLaunchCooperativeKernel(walk, dim3(b.grid), dim3(SBD_THREADS), args, 0, st);

@@ -60,6 +60,9 @@ for _name, _res, _args in [
     ("ksh_compile_node_rules", C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp]),
     ("ksh_reconcile_nodes", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp,
                                       _vp, _vp, C.c_int, _vp, _vp, _vp, C.c_size_t, _vp]),
+    ("ksh_compile_resources", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_size_t, _vp, _vp]),
+    ("ksh_reconcile_fit", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp,
+                                    _vp, _vp, C.c_int, _vp, _vp, _vp, C.c_size_t, _vp]),
 ]:
     _proto(_name, _res, *_args)
 
@@ -69,6 +72,7 @@ KSH_RECONCILE_GANG_UNSATISFIED = 4
 KSH_RECONCILE_SPREAD_UNSATISFIED = 5
 KSH_RECONCILE_AFFINITY_UNSATISFIED = 6
 KSH_RECONCILE_NODE_RULES_UNSATISFIED = 7
+KSH_RECONCILE_INSUFFICIENT_RESOURCES = 8
 
 
 class ksh_taint(C.Structure):
@@ -570,6 +574,42 @@ class Context:
         [n_groups] as node_rules takes them, or None (no toleration and no term).  Status 7
         (KSH_RECONCILE_NODE_RULES_UNSATISFIED) for a pod that fit some node but taints or node affinity refused every
         such node.  Returns (status[n], node_idx[n], bodies[n])."""
+        return self._reconcile_rules(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
+                                     min_domains, existing_nodes, policy, json_cap, soft_skew, soft_all_keys,
+                                     term_weight, hard_affinity_weight, weight_spread, weight_affinity, group_rules,
+                                     weight_taint, weight_node_affinity, False)
+
+    def compile_resources(self, pods, n):
+        """The scalar resources of the pending batch pods[0:n] (ksh_compile_resources): (names, node_free int64 [R, N],
+        pod_req int64 [n, R]); names[0] == "pods"."""
+        N, M = self.n_nodes, capi.KS_BIND_MAX_RESOURCES
+        free = np.zeros(M * N, np.int64)
+        req = np.zeros(M * n, np.int64)
+        cap = 64 * 1024
+        buf = C.create_string_buffer(cap)
+        r = lib.ksh_compile_resources(self._h, C.addressof(pods) if n else None, n, C.addressof(buf), cap,
+                                      free.ctypes.data, req.ctypes.data)
+        check(min(r, 0), "ksh_compile_resources")
+        names = [x.decode() for x in buf.raw.split(b"\0")[:r]]
+        return names, free[:r * N].reshape(r, N), req[:n * r].reshape(n, r)
+
+    def reconcile_fit(self, pods, n, group, n_groups, topology_keys, terms=(), existing_pods=(), max_skew=None,
+                      min_domains=None, existing_nodes=None, policy=capi.KS_SCORE_LEAST_BALANCED, json_cap=None,
+                      soft_skew=None, soft_all_keys=None, term_weight=None, hard_affinity_weight=1, weight_spread=2,
+                      weight_affinity=2, group_rules=None, weight_taint=3, weight_node_affinity=2):
+        """reconcile_nodes with the pod count and the scalar resources of NodeResourcesFit (ksh_reconcile_fit): the
+        batch's resources are compile_resources'.  Status 8 (KSH_RECONCILE_INSUFFICIENT_RESOURCES) for a pod that fit
+        some node by cpu, memory and selector but every such node lacked a resource or was at its pod limit.  Returns
+        (status[n], node_idx[n], bodies[n])."""
+        return self._reconcile_rules(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
+                                     min_domains, existing_nodes, policy, json_cap, soft_skew, soft_all_keys,
+                                     term_weight, hard_affinity_weight, weight_spread, weight_affinity, group_rules,
+                                     weight_taint, weight_node_affinity, True)
+
+    def _reconcile_rules(self, pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew, min_domains,
+                         existing_nodes, policy, json_cap, soft_skew, soft_all_keys, term_weight, hard_affinity_weight,
+                         weight_spread, weight_affinity, group_rules, weight_taint, weight_node_affinity, fit):
+        # ksh_reconcile_nodes, or with fit ksh_reconcile_fit
         nr = None
         if group_rules is not None:
             if len(group_rules) != n_groups:
@@ -587,11 +627,12 @@ class Context:
                                        int(weight_spread), int(weight_affinity))
         return self._reconcile_terms(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
                                      min_domains, existing_nodes, policy, json_cap, scoring, nodes=True,
-                                     rules=None if nr is None else nr[0])
+                                     rules=None if nr is None else nr[0], fit=fit)
 
     def _reconcile_terms(self, pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew, min_domains,
-                         existing_nodes, policy, json_cap, scoring, nodes=False, rules=None):
-        # ksh_reconcile_affinity, or with scoring ksh_reconcile_profile, or with nodes ksh_reconcile_nodes
+                         existing_nodes, policy, json_cap, scoring, nodes=False, rules=None, fit=False):
+        # ksh_reconcile_affinity, or with scoring ksh_reconcile_profile, or with nodes ksh_reconcile_nodes (with fit
+        # ksh_reconcile_fit)
         k = len(topology_keys)
         group = np.ascontiguousarray(group, np.int32).reshape(-1)
         if group.shape[0] != n:
@@ -629,7 +670,10 @@ class Context:
                 None if names is None else C.cast(names, _vp), None if ex_off is None else ex_off.ctypes.data,
                 C.byref(aff))
         tail = (int(policy), status.ctypes.data, node.ctypes.data, C.addressof(buf), cap, off.ctypes.data)
-        if nodes:
+        if fit:
+            check(lib.ksh_reconcile_fit(*head, C.byref(scoring), None if rules is None else C.byref(rules), *tail),
+                  "ksh_reconcile_fit")
+        elif nodes:
             check(lib.ksh_reconcile_nodes(*head, C.byref(scoring), None if rules is None else C.byref(rules), *tail),
                   "ksh_reconcile_nodes")
         elif scoring is None:

@@ -520,10 +520,37 @@ class Snapshot:
                                  soft_all_keys, term_weight, hard_affinity_weight, weight_spread, weight_affinity,
                                  want_counts)
 
+    def fit_bind(self, req_cpu, req_mem, sel, group, n_groups, keys, terms=(), existing_pods=None, max_skew=None,
+                 min_domains=None, existing=None, policy=capi.KS_SCORE_LEAST_BALANCED, soft_skew=None,
+                 soft_all_keys=None, term_weight=None, hard_affinity_weight=1, weight_spread=2, weight_affinity=2,
+                 rules=None, node_free=None, pod_req=None, want_counts=True):
+        """node_bind with the pod count and scalar resources of NodeResourcesFit (ks_fit_bind).  node_free [R, N] and
+        pod_req [P, R] (int64), or both None (the C call's NULL res); rules as node_bind takes them (None = NULL).
+        Returns node_bind's tuple with refused [P, 5] (resources, taint, node affinity, spread, inter-pod affinity),
+        then free_r int64 [R, N] after the call."""
+        if (node_free is None) != (pod_req is None):
+            raise ValueError("node_free and pod_req go together")
+        res = None
+        if node_free is not None:
+            node_free = _c(node_free, np.int64)
+            pod_req = _c(pod_req, np.int64)
+            p = int(np.asarray(req_cpu).reshape(-1).shape[0])
+            if node_free.ndim != 2 or node_free.shape[1] != self.n_nodes:
+                raise ValueError(f"node_free has shape {node_free.shape}, expected (R, {self.n_nodes})")
+            r = node_free.shape[0]
+            if pod_req.shape != (p, r):
+                raise ValueError(f"pod_req has shape {pod_req.shape}, expected ({p}, {r})")
+            res = (r, node_free.reshape(-1), pod_req.reshape(-1))
+        return self._scored_bind(rules if rules is not None else False, req_cpu, req_mem, sel, group, n_groups, keys,
+                                 terms, existing_pods, max_skew, min_domains, existing, policy, soft_skew,
+                                 soft_all_keys, term_weight, hard_affinity_weight, weight_spread, weight_affinity,
+                                 want_counts, res=res, fit=True)
+
     def _scored_bind(self, rules, req_cpu, req_mem, sel, group, n_groups, keys, terms, existing_pods, max_skew,
                      min_domains, existing, policy, soft_skew, soft_all_keys, term_weight, hard_affinity_weight,
-                     weight_spread, weight_affinity, want_counts):
-        """ks_profile_bind when rules is None, else ks_node_bind (rules False = its NULL rules)."""
+                     weight_spread, weight_affinity, want_counts, res=None, fit=False):
+        """ks_profile_bind when rules is None, else ks_node_bind (rules False = its NULL rules); with fit, ks_fit_bind
+        with res = (R, node_free, pod_req) or None."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
         p, g = int(pods.n), int(n_groups)
         group = _c(group, np.int32).reshape(-1)
@@ -576,11 +603,20 @@ class Snapshot:
         idx = np.empty(p, np.int32)
         score = np.empty(p, np.int64)
         parts = np.empty((p, 3 if rules is None else 5), np.int64)
-        refused = np.empty((p, 2 if rules is None else 4), np.uint32)
+        refused = np.empty((p, 5 if fit else 2 if rules is None else 4), np.uint32)
         want = want_counts and 0 < g * s <= capi.KS_SPREAD_MAX_COUNTS
         counts = np.empty((g, s), np.uint32) if want else None
         soft = np.empty((g, s), np.uint32) if want else None
-        if rules is None:
+        if fit:
+            nr, hold = node_rules(rules) if rules is not False else (None, None)
+            r = res[0] if res is not None else 0
+            br = capi.ks_bind_resources(r, _ptr(res[1]), _ptr(res[2])) if res is not None else None
+            free_r = np.empty((r, self.n_nodes), np.int64)
+            check(lib.ks_fit_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff), C.byref(scoring),
+                                  C.byref(nr) if nr is not None else None, C.byref(br) if br is not None else None,
+                                  int(policy), _ptr(idx), _ptr(score), _ptr(parts), _ptr(refused), _ptr(counts),
+                                  _ptr(soft), _ptr(free_r)), "ks_fit_bind")
+        elif rules is None:
             check(lib.ks_profile_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
                                       C.byref(scoring), int(policy), _ptr(idx), _ptr(score), _ptr(parts),
                                       _ptr(refused), _ptr(counts), _ptr(soft)), "ks_profile_bind")
@@ -592,6 +628,8 @@ class Snapshot:
         if want:
             counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
             soft = np.split(soft, np.cumsum(nd)[:-1], axis=1)
+        if fit:
+            return idx, score, parts, refused, counts, soft, free_r
         return idx, score, parts, refused, counts, soft
 
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
