@@ -386,6 +386,12 @@ extern "C" {
                        rules: *const ks_node_rules, res: *const ks_bind_resources, policy: c_int, node_idx: *mut i32,
                        score: *mut i64, parts: *mut i64, refused: *mut u32, domain_count: *mut u32,
                        soft_count: *mut u32, free: *mut i64) -> c_int;
+    // ks_fit_bind with gangs placed all or nothing (DESIGN.md 5s)
+    pub fn ks_gang_fit_bind(s: *mut ks_snapshot, pods: *const ks_pods, group: *const i32, n_groups: u32,
+                            topo: *const ks_spread_multi, aff: *const ks_pod_affinity, scoring: *const ks_bind_scoring,
+                            rules: *const ks_node_rules, res: *const ks_bind_resources, gangs: *const ks_gangs,
+                            policy: c_int, node_idx: *mut i32, score: *mut i64, parts: *mut i64, refused: *mut u32,
+                            domain_count: *mut u32, soft_count: *mut u32, free: *mut i64, placed: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -479,6 +485,14 @@ extern "C" {
                              scoring: *const ks_bind_scoring, rules: *const ksh_node_rules, policy: c_int,
                              status: *mut i32, node_idx: *mut i32, json: *mut c_char, cap: usize,
                              json_off: *mut i64) -> c_int;
+    pub fn ksh_reconcile_fit_gangs(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group: *const i32,
+                                   n_groups: u32, topology_keys: *const *const c_char, n_keys: u32,
+                                   max_skew: *const u32, min_domains: *const u32,
+                                   existing_node_names: *const *const c_char, existing_offset: *const u64,
+                                   aff: *const ksh_pod_affinity, scoring: *const ks_bind_scoring,
+                                   rules: *const ksh_node_rules, gang_offset: *const u64, n_gangs: u64,
+                                   min_member: *const u32, policy: c_int, status: *mut i32, node_idx: *mut i32,
+                                   placed: *mut u32, json: *mut c_char, cap: usize, json_off: *mut i64) -> c_int;
     pub fn ksh_reconcile_profile(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group: *const i32,
                                  n_groups: u32, topology_keys: *const *const c_char, n_keys: u32, max_skew: *const u32,
                                  min_domains: *const u32, existing_node_names: *const *const c_char,

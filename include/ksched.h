@@ -967,6 +967,52 @@ int ks_fit_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const int3
                 uint32_t* out_domain_count /* [G * S] or NULL */, uint32_t* out_soft_count /* [G * S] or NULL */,
                 int64_t* out_free /* [R * N] or NULL */);
 
+/* ---- gangs when binding: ks_fit_bind with pod groups placed all or nothing (upstream coscheduling's PodGroup
+ * minMember under the full filter; spec extension, DESIGN.md 5s) ----
+ * The arguments of ks_fit_bind plus `gangs` (ks_gang_bind's struct, host memory) and out_placed.  Gang j is the pods
+ * [offset[j], offset[j + 1]) of the queue: offset[0] = 0, offset[n] = P, every gang holds at least one pod and
+ * 0 <= min_member[j] <= its size.  A gang's pods may belong to different groups (a launcher and its workers, say); its
+ * size is bounded by the queue's KS_SPREAD_BIND_MAX_PODS only (KS_GANG_MAX_SIZE is ks_gang_bind's batch, not this call's).
+ *   1. the pods run in queue order with exactly ks_fit_bind's cycle: the same filters, scores, ties, charge and count
+ *      updates, each pod against the state every earlier pod left;
+ *   2. after a gang's last pod, placed[j] = the number of its pods that bound; when placed[j] >= min_member[j] the gang
+ *      commits and its pods keep their bindings;
+ *   3. otherwise it rolls back: every pod of the gang gets node -1, score 0 and zero parts, and every piece of state the
+ *      gang changed goes back bit for bit to its value before the gang - free[], free_r, the hard counts, the spread
+ *      minima, the inter-pod affinity counters and first-pod flags, the soft counts and the IPA counters - so the next
+ *      gang sees exactly what this one saw;
+ *   4. out_refused[5p .. 5p + 4] keep the words of pod p's own turn, also when its gang rolls back: they say why the
+ *      gang came up short;
+ *   5. there is no early exit: every pod of a gang runs its cycle, so every output is defined for every pod.
+ * out_domain_count, out_soft_count, out_free and free[] are the values after every rollback; out_placed[n] (or NULL) =
+ * placed[j] before any rollback.
+ * Identities, policies 1, 3 and 4:
+ *   (M1) every min_member 0: every output is ks_fit_bind's, bit for bit, and out_placed[j] counts the gang's bound pods;
+ *   (M2) singleton gangs with min_member 1: the same as M1;
+ *   (M3) with C the pods of the committed gangs in queue order: their nodes, scores, parts and refusal words are those
+ *        of ks_fit_bind run on C alone (the same groups and existing pods), and so are the final counts, soft counts,
+ *        free_r and free[];
+ *   (M4) every gang rolls back: free[], out_free, the counts and the soft counts are the call's inputs, and a ks_select
+ *        after the call, on either path, equals one before it.
+ * Checked on the host before any device work and before free[] changes: every check of ks_fit_bind; KS_ERR_INVALID for
+ * a NULL gangs, offset or min_member (n > 0), offset[0] != 0, decreasing offsets or offset[n] != P; KS_ERR_RANGE for an
+ * empty gang or a min_member above its gang's size.
+ * ks_fit_bind's launches, with its walk's own instance: the rollback runs in the commit of the gang's last pod, on one
+ * CTA, before that pod's last grid barrier, so a gang adds no barrier.  It subtracts what the gang's bound pods added and
+ * recomputes each touched group's spread minimum over that key's eligible domains (up to D_k loads per key) and each
+ * touched first-pod flag over the group's affinity counters.  The bit-parallel index is marked stale.
+ * Out of scope: a search over placements inside a gang (the walk is greedy, as upstream coscheduling and ks_gang_bind:
+ * a gang whose first pod takes a zone without room for the rest fails); permit timeouts; preemption for a gang. */
+int ks_gang_fit_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const int32_t* group /* [P] */,
+                     uint32_t n_groups, const ks_spread_multi* topo /* keys; max_skew may be NULL */,
+                     const ks_pod_affinity* aff /* or NULL */, const ks_bind_scoring* scoring,
+                     const ks_node_rules* rules /* or NULL */, const ks_bind_resources* res /* or NULL */,
+                     const ks_gangs* gangs, int policy, int32_t* out_node_idx /* [P] */,
+                     int64_t* out_score /* [P] or NULL */, int64_t* out_parts /* [5P] or NULL */,
+                     uint32_t* out_refused /* [5P] or NULL */, uint32_t* out_domain_count /* [G * S] or NULL */,
+                     uint32_t* out_soft_count /* [G * S] or NULL */, int64_t* out_free /* [R * N] or NULL */,
+                     uint32_t* out_placed /* [n] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

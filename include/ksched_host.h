@@ -422,6 +422,27 @@ int ksh_reconcile_fit(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods,
                       const ksh_node_rules* rules /* or NULL */, int policy, int32_t* out_status,
                       int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off);
 
+/* reconcile() for pod groups under the full bind filter (ks_gang_fit_bind, DESIGN.md 5s): ksh_reconcile_fit's arguments
+ * plus gangs cut as ksh_reconcile_gangs cuts its groups.  Gang j is pods [gang_offset[j], gang_offset[j + 1]), at least
+ * one pod, min_member[j] <= its size, and no other size limit than ks_gang_fit_bind's queue; its pods may belong to
+ * different groups.  Members are filtered as ksh_reconcile_gangs filters them: already bound members are skipped
+ * (KSH_RECONCILE_OK, node -1) and count toward min_member; nameless pods get KSH_RECONCILE_BINDING_OBJECT_FAILED and do
+ * not count; the rest of each gang goes to the device with max(0, min_member - bound members).  The batch's resources
+ * are built as ksh_compile_resources builds them over the pods that go to the device.  The pods of a gang that rolls
+ * back, or that has fewer schedulable members than it still needs, get KSH_RECONCILE_GANG_UNSATISFIED: no Binding body,
+ * and no charge or extended request is recorded for them.  The pods of a gang that commits get ksh_reconcile_fit's
+ * statuses.  out_placed[n_gangs] (may be NULL) = the gang's pods the device placed before any rollback.  Offsets and
+ * sizes are checked first: KS_ERR_INVALID (offsets) / KS_ERR_RANGE (an empty gang, min_member); otherwise errors as
+ * ksh_reconcile_fit and ks_gang_fit_bind. */
+int ksh_reconcile_fit_gangs(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, const int32_t* group,
+                            uint32_t n_groups, const char* const* topology_keys, uint32_t n_keys,
+                            const uint32_t* max_skew /* or NULL */, const uint32_t* min_domains,
+                            const char* const* existing_node_names, const uint64_t* existing_offset,
+                            const ksh_pod_affinity* aff /* or NULL */, const ks_bind_scoring* scoring,
+                            const ksh_node_rules* rules /* or NULL */, const uint64_t* gang_offset, uint64_t n_gangs,
+                            const uint32_t* min_member, int policy, int32_t* out_status, int32_t* out_node_idx,
+                            uint32_t* out_placed, char* json, size_t cap, int64_t* out_json_off);
+
 #ifdef __cplusplus
 }
 #endif

@@ -39,6 +39,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 #pragma weak ks_profile_bind
 #pragma weak ks_node_bind
 #pragma weak ks_fit_bind
+#pragma weak ks_gang_fit_bind
 
 namespace {
 
@@ -2055,15 +2056,29 @@ static int compile_resources(ksh_context* c, const ks_pod_obj* pods, uint64_t n,
 // and every key g constrains.  With aff set (ksh_reconcile_affinity), ks_affinity_bind with its terms and the existing
 // pods whose node is in the store; max_skew may then be NULL.  With aff and sc set (ksh_reconcile_profile),
 // ks_profile_bind with the same terms and the soft terms of sc; the soft counts start from the same existing counts.
+// With gang_offset set as well (ksh_reconcile_fit_gangs), ks_gang_fit_bind over the gangs' pods that go to the device,
+// one sub-gang per gang; already bound members count toward min_member, as in ksh_reconcile_gangs.
 static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
                             const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
                             const uint32_t* min_domains, const char* const* existing_node_names,
                             const uint64_t* existing_offset, const ksh_pod_affinity* aff, int policy, int32_t* out_status,
                             int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off,
                             const ks_bind_scoring* sc = nullptr, const ksh_node_rules* nr = nullptr,
-                            bool nodes = false, bool fit = false) {
+                            bool nodes = false, bool fit = false, const uint64_t* gang_offset = nullptr,
+                            uint64_t n_gangs = 0, const uint32_t* min_member = nullptr, uint32_t* out_placed = nullptr) {
     if (!c || !topology_keys || (n && (!pods || !group || !out_status || !out_node_idx)) || (n_groups && !max_skew && !aff))
         return fail(KS_ERR_INVALID, "NULL argument");
+    if (gang_offset) { // as ksh_reconcile_gangs checks them, without its size limit
+        if (n_gangs && !min_member) return fail(KS_ERR_INVALID, "NULL argument");
+        if (gang_offset[0] != 0) return fail(KS_ERR_INVALID, "gang_offset[0] must be 0");
+        for (uint64_t j = 0; j < n_gangs; j++) {
+            if (gang_offset[j + 1] < gang_offset[j]) return fail(KS_ERR_INVALID, "gang offsets decrease");
+            const uint64_t size = gang_offset[j + 1] - gang_offset[j];
+            if (size == 0) return fail(KS_ERR_RANGE, "a gang has no pod");
+            if (min_member[j] > size) return fail(KS_ERR_RANGE, "min_member above the gang's size");
+        }
+        if (gang_offset[n_gangs] != n) return fail(KS_ERR_INVALID, "gang_offset[n_gangs] must be n_pods");
+    }
     if (K == 0 || K > KS_SPREAD_MAX_KEYS)
         return fail(KS_ERR_RANGE, std::to_string(K) + " topology keys (1 to " + std::to_string(KS_SPREAD_MAX_KEYS) + ")");
     for (uint32_t k = 0; k < K; k++)
@@ -2079,7 +2094,8 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     if (aff && aff->n_existing && (!aff->existing_group || !aff->existing_node_name))
         return fail(KS_ERR_INVALID, "NULL existing_group or existing_node_name");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    int rc = fit     ? device_ready(c, ks_fit_bind, "ks_fit_bind")
+    int rc = gang_offset ? device_ready(c, ks_gang_fit_bind, "ks_gang_fit_bind")
+             : fit   ? device_ready(c, ks_fit_bind, "ks_fit_bind")
              : nodes ? device_ready(c, ks_node_bind, "ks_node_bind")
              : sc  ? device_ready(c, ks_profile_bind, "ks_profile_bind")
              : aff ? device_ready(c, ks_affinity_bind, "ks_affinity_bind")
@@ -2096,6 +2112,39 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
         todo.push_back(i);
         sub.push_back(pods[i]);
         sub_group.push_back(group[i]);
+    }
+    // ks_gang_fit_bind: sub-gang k is the device pods [sub_off[k], sub_off[k + 1]) of gang sub_gang[k], needing sub_min[k]
+    std::vector<uint64_t> sub_off{0}, sub_gang;
+    std::vector<uint32_t> sub_min;
+    if (out_placed)
+        for (uint64_t j = 0; j < n_gangs; j++) out_placed[j] = 0;
+    if (gang_offset) {
+        std::vector<uint64_t> keep;
+        std::vector<ks_pod_obj> keep_pods;
+        std::vector<int32_t> keep_group;
+        for (uint64_t j = 0, t = 0; j < n_gangs; j++) {
+            uint32_t bound = 0; // running members of the gang
+            for (uint64_t i = gang_offset[j]; i < gang_offset[j + 1]; i++) bound += out_status[i] == KSH_RECONCILE_OK;
+            const size_t first = t;
+            while (t < todo.size() && todo[t] < gang_offset[j + 1]) t++;
+            const uint32_t need = min_member[j] > bound ? min_member[j] - bound : 0;
+            if (t == first) continue;
+            if (need > t - first) { // too few schedulable members: the gang cannot commit, nothing is tried
+                for (size_t k = first; k < t; k++) out_status[todo[k]] = KSH_RECONCILE_GANG_UNSATISFIED;
+                continue;
+            }
+            for (size_t k = first; k < t; k++) {
+                keep.push_back(todo[k]);
+                keep_pods.push_back(sub[k]);
+                keep_group.push_back(sub_group[k]);
+            }
+            sub_off.push_back(keep.size());
+            sub_gang.push_back(j);
+            sub_min.push_back(need);
+        }
+        todo.swap(keep);
+        sub.swap(keep_pods);
+        sub_group.swap(keep_group);
     }
     CompiledNodeRules cr;
     if (nodes) { // compiled before anything is bound, so a bad rule fails the whole call
@@ -2145,6 +2194,7 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     // refusal words per pod: [resources,] [taint, node affinity,] spread, then affinity
     const size_t R = fit ? 5 : nodes ? 4 : aff ? 2 : 1;
     std::vector<uint32_t> refused(sub.size() * R, 0);
+    std::vector<uint32_t> placed(sub_gang.size());
     if (aff) {
         ks_pod_affinity pa{aff->n_terms, aff->owner, aff->kind, aff->key, aff->target_offset, aff->target, 0, nullptr,
                            nullptr};
@@ -2159,7 +2209,11 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
         pa.existing_group = eg.data();
         pa.existing_node = en.data();
         const ks_bind_resources br{(uint32_t)res.ids.size(), res.node_free.data(), res.pod_req.data()};
-        rc = fit     ? ks_fit_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, &cr.r, &br, policy,
+        const ks_gangs kg{sub_gang.size(), sub_off.data(), sub_min.data()};
+        rc = gang_offset ? ks_gang_fit_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, &cr.r, &br, &kg,
+                                            policy, idx.data(), nullptr, nullptr, refused.data(), nullptr, nullptr,
+                                            nullptr, placed.data())
+             : fit   ? ks_fit_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, &cr.r, &br, policy,
                                    idx.data(), nullptr, nullptr, refused.data(), nullptr, nullptr, nullptr)
              : nodes ? ks_node_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, &cr.r, policy, idx.data(),
                                   nullptr, nullptr, refused.data(), nullptr, nullptr)
@@ -2178,10 +2232,17 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     StringList bodies{json, cap};
     // the node-rule words follow the resource word, the spread and affinity words follow the two node-rule words
     const size_t X = fit ? 1 : 0, F = nodes ? X + 2 : 0;
+    std::vector<uint8_t> rolled(todo.size(), 0); // the pods of the sub-gangs that rolled back
+    for (size_t k = 0; k < sub_gang.size(); k++) {
+        if (out_placed) out_placed[sub_gang[k]] = placed[k];
+        if (placed[k] < sub_min[k]) std::fill(rolled.begin() + sub_off[k], rolled.begin() + sub_off[k + 1], 1);
+    }
     for (size_t k = 0; k < todo.size(); k++) {
         const uint64_t i = todo[k];
         const uint32_t* w = &refused[k * R];
-        if (idx[k] >= 0)
+        if (rolled[k])
+            out_status[i] = KSH_RECONCILE_GANG_UNSATISFIED;
+        else if (idx[k] >= 0)
             commit_bind(c, &pods[i], idx[k], kp.req_cpu[k], kp.req_mem[k], &out_status[i], &out_node_idx[i], bodies,
                         json && out_json_off ? &out_json_off[i] : nullptr);
         else if (fit && w[0] > 0 && w[1] + w[2] + w[3] + w[4] == 0)
@@ -2342,6 +2403,22 @@ int ksh_reconcile_fit(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const 
     return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
                             existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
                             out_json_off, scoring, rules, true, true);
+}
+KSH_CATCH
+
+int ksh_reconcile_fit_gangs(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
+                            const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
+                            const uint32_t* min_domains, const char* const* existing_node_names,
+                            const uint64_t* existing_offset, const ksh_pod_affinity* aff,
+                            const ks_bind_scoring* scoring, const ksh_node_rules* rules, const uint64_t* gang_offset,
+                            uint64_t n_gangs, const uint32_t* min_member, int policy, int32_t* out_status,
+                            int32_t* out_node_idx, uint32_t* out_placed, char* json, size_t cap,
+                            int64_t* out_json_off) try {
+    if (!scoring || !gang_offset) return fail(KS_ERR_INVALID, "NULL scoring or gang_offset");
+    const ksh_pod_affinity none{};
+    return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
+                            existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
+                            out_json_off, scoring, rules, true, true, gang_offset, n_gangs, min_member, out_placed);
 }
 KSH_CATCH
 

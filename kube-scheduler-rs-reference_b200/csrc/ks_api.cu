@@ -1243,6 +1243,25 @@ int ks_stream_bind(ks_snapshot* s, const ks_pods* pods, int policy, int32_t* out
     }
 }
 
+// The cut of P pods into gangs->n groups of 1 to max_size pods each, and each min_member within its group's size
+static int check_gangs(const ks_gangs* gangs, uint64_t P, uint64_t max_size) {
+    const uint64_t G = gangs->n;
+    const uint64_t* off = gangs->offset;
+    if (off[0] != 0) return fail(KS_ERR_INVALID, "offset[0] must be 0");
+    for (uint64_t g = 0; g < G; g++) {
+        if (off[g + 1] < off[g]) return fail(KS_ERR_INVALID, "offsets decrease at group %llu", (unsigned long long)g);
+        const uint64_t size = off[g + 1] - off[g];
+        if (size == 0 || size > max_size)
+            return fail(KS_ERR_RANGE, "group %llu has %llu pods (1..%llu)", (unsigned long long)g, (unsigned long long)size,
+                        (unsigned long long)max_size);
+        if (gangs->min_member[g] > size)
+            return fail(KS_ERR_RANGE, "group %llu: min_member %u above its %llu pods", (unsigned long long)g,
+                        gangs->min_member[g], (unsigned long long)size);
+    }
+    if (off[G] != P) return fail(KS_ERR_INVALID, "offset[n] must be pods->n");
+    return KS_OK;
+}
+
 int ks_gang_bind(ks_snapshot* s, const ks_pods* pods, const ks_gangs* gangs, int policy, int32_t* out_node_idx,
                  int64_t* out_score, uint32_t* out_placed, uint32_t* out_rounds) {
     int rc = check_pods(s, pods);
@@ -1253,18 +1272,8 @@ int ks_gang_bind(ks_snapshot* s, const ks_pods* pods, const ks_gangs* gangs, int
     if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
     const uint64_t P = pods->n, G = gangs->n;
     const uint64_t* off = gangs->offset;
-    if (off[0] != 0) return fail(KS_ERR_INVALID, "offset[0] must be 0");
-    for (uint64_t g = 0; g < G; g++) {
-        if (off[g + 1] < off[g]) return fail(KS_ERR_INVALID, "offsets decrease at group %llu", (unsigned long long)g);
-        const uint64_t size = off[g + 1] - off[g];
-        if (size == 0 || size > KS_GANG_MAX_SIZE)
-            return fail(KS_ERR_RANGE, "group %llu has %llu pods (1..%u)", (unsigned long long)g, (unsigned long long)size,
-                        KS_GANG_MAX_SIZE);
-        if (gangs->min_member[g] > size)
-            return fail(KS_ERR_RANGE, "group %llu: min_member %u above its %llu pods", (unsigned long long)g,
-                        gangs->min_member[g], (unsigned long long)size);
-    }
-    if (off[G] != P) return fail(KS_ERR_INVALID, "offset[n] must be pods->n");
+    rc = check_gangs(gangs, P, KS_GANG_MAX_SIZE);
+    if (rc) return rc;
     if (G == 0) return KS_OK;
     rc = check_commit_requests(P, pods->req_cpu, pods->req_mem);
     if (rc) return rc;
@@ -2086,19 +2095,22 @@ static int compile_node_rules(const ks_node_rules* r, uint32_t G, uint32_t N, No
 }
 
 // last_path and the name in launch errors of each BindMode
-static const char* const BIND_PATH[] = {"spread_bind", "affinity_bind", "profile_bind", "node_bind", "fit_bind"};
-static const char* const BIND_NAME[] = {"spread bind", "affinity bind", "profile bind", "node bind", "fit bind"};
+static const char* const BIND_PATH[] = {"spread_bind", "affinity_bind", "profile_bind", "node_bind", "fit_bind",
+                                        "gang_fit_bind"};
+static const char* const BIND_NAME[] = {"spread bind", "affinity bind", "profile bind", "node bind", "fit bind",
+                                        "gang fit bind"};
 
 // ks_spread_bind, and with aff set ks_affinity_bind (then max_skew may be NULL), and with aff and sc set ks_profile_bind
 // (out_parts and out_soft_count [G * S] may be given), and with nr set as well ks_node_bind, and with res set as well
-// ks_fit_bind (out_free [R * N] may be given); out_refused and out_parts hold the mode's words per pod
-// (bind_refusal_words, bind_part_words)
+// ks_fit_bind (out_free [R * N] may be given), and with gangs set as well ks_gang_fit_bind (out_placed [gangs->n] may
+// be given); out_refused and out_parts hold the mode's words per pod (bind_refusal_words, bind_part_words)
 static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
                        const ks_spread_multi* spread, const ks_pod_affinity* aff, int policy, int32_t* out_node_idx,
                        int64_t* out_score, uint32_t* out_refused, uint32_t* out_domain_count,
                        const ks_bind_scoring* sc = nullptr, int64_t* out_parts = nullptr,
                        uint32_t* out_soft_count = nullptr, const ks_node_rules* nr = nullptr,
-                       const ks_bind_resources* res = nullptr, int64_t* out_free = nullptr) {
+                       const ks_bind_resources* res = nullptr, int64_t* out_free = nullptr,
+                       const ks_gangs* gangs = nullptr, uint32_t* out_placed = nullptr) {
     int rc = check_pods(s, pods);
     if (rc) return rc;
     if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "%s takes host-space pods", call);
@@ -2161,6 +2173,12 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         if (res->pod_req[i] < 0)
             return fail(KS_ERR_RANGE, "pod %llu: request %lld of resource %llu (at least 0)", (unsigned long long)(i / RS),
                         (long long)res->pod_req[i], (unsigned long long)(i % RS));
+    const uint64_t NG = gangs ? gangs->n : 0; // ks_gang_fit_bind's gangs
+    if (gangs) {
+        if (!gangs->offset || (NG && !gangs->min_member)) return fail(KS_ERR_INVALID, "NULL gang array");
+        rc = check_gangs(gangs, P, KS_SPREAD_BIND_MAX_PODS);
+        if (rc) return rc;
+    }
     AffinityPlan plan;
     if (aff) {
         try {
@@ -2179,9 +2197,15 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         }
         if (rc) return rc;
     }
-    const BindMode mode = res ? BIND_FIT : nr ? BIND_NODE : sc ? BIND_PROFILE : aff ? BIND_AFFINITY : BIND_SPREAD;
+    const BindMode mode = gangs ? BIND_GANG_FIT
+                          : res ? BIND_FIT
+                          : nr  ? BIND_NODE
+                          : sc  ? BIND_PROFILE
+                          : aff ? BIND_AFFINITY
+                                : BIND_SPREAD;
     const uint64_t R = bind_refusal_words(mode), PW = bind_part_words(mode);
     if (out_free && RS && N && (P == 0)) memcpy(out_free, res->node_free, RS * N * 8); // nothing binds: L3
+    if (out_placed) memset(out_placed, 0, NG * 4); // rewritten by the walk when it runs
     if (P == 0) return KS_OK;
     if (N == 0) { // no node: nothing is placed, every count is existing
         memset(out_node_idx, 0xff, P * 4);
@@ -2287,6 +2311,11 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     const auto res_node_free = h.in(RS ? res->node_free : nullptr, RS * N);
     const auto res_free = h.out(out_free, RS * N);
     const auto pfref = h.work<uint32_t>(res ? a.grid : 0);
+    // ks_gang_fit_bind: the gangs' offsets (P < 2^32) and minimums, their counts, and the rollback's group marks and lists
+    const auto goff = h.in<uint32_t>(nullptr, gangs ? NG + 1 : 0);
+    const auto gmin = h.in(gangs ? gangs->min_member : nullptr, NG);
+    const auto gplaced = h.out(out_placed, NG);
+    const auto gmark = h.work<uint32_t>(gangs ? 2 * G : 0), glist = h.work<uint32_t>(gangs ? 2 * G : 0);
     auto put = [&](Staged<uint32_t> d, const std::vector<uint32_t>& v) {
         if (!v.empty()) memcpy(h.host(d), v.data(), v.size() * 4);
     };
@@ -2312,6 +2341,8 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         put(iupd, plan.iupd);
         if (!plan.icoef.empty()) memcpy(h.host(icoef), plan.icoef.data(), plan.icoef.size() * 4);
     }
+    if (gangs)
+        for (uint64_t j = 0; j <= NG; j++) h.host(goff)[j] = (uint32_t)gangs->offset[j];
     for (uint32_t k = 0; k < K; k++) memcpy(h.host(dom) + (size_t)k * N, spread->node_domain[k], (size_t)N * 4);
     if (!spread->max_skew) memset(h.host(max_skew), 0, G * K * 4);
     put(abase, plan.abase);
@@ -2428,6 +2459,14 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
         q.res_free = h.dev(res_free);
         q.pfref = h.dev(pfref);
     }
+    if (gangs) {
+        q.n_gangs = (uint32_t)NG;
+        q.goff = h.dev(goff);
+        q.gmin = h.dev(gmin);
+        q.gplaced = h.dev(gplaced);
+        q.gmark = h.dev(gmark);
+        q.glist = h.dev(glist);
+    }
     s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
     s->version++;
     const cudaError_t e = launch_bind(mode, q, plan.words, W, st);
@@ -2513,6 +2552,24 @@ int ks_fit_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint3
                                rules ? rules : &no_rules, res ? res : &no_res, out_free);
     if (rc || rules || !out_parts) return rc;
     for (uint64_t p = 0; p < pods->n; p++) out_parts[5 * p + 3] = out_parts[5 * p + 4] = 0; // as ks_node_bind's K1
+    return KS_OK;
+}
+
+int ks_gang_fit_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
+                     const ks_spread_multi* topo, const ks_pod_affinity* aff, const ks_bind_scoring* scoring,
+                     const ks_node_rules* rules, const ks_bind_resources* res, const ks_gangs* gangs, int policy,
+                     int32_t* out_node_idx, int64_t* out_score, int64_t* out_parts, uint32_t* out_refused,
+                     uint32_t* out_domain_count, uint32_t* out_soft_count, int64_t* out_free, uint32_t* out_placed) {
+    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
+    if (!gangs) return fail(KS_ERR_INVALID, "NULL gangs");
+    const ks_pod_affinity none{};
+    const ks_node_rules no_rules{}; // as ks_fit_bind's
+    const ks_bind_resources no_res{};
+    const int rc = bind_spread(s, "ks_gang_fit_bind", pods, group, n_groups, topo, aff ? aff : &none, policy,
+                               out_node_idx, out_score, out_refused, out_domain_count, scoring, out_parts, out_soft_count,
+                               rules ? rules : &no_rules, res ? res : &no_res, out_free, gangs, out_placed);
+    if (rc || rules || !out_parts) return rc;
+    for (uint64_t p = 0; p < pods->n; p++) out_parts[5 * p + 3] = out_parts[5 * p + 4] = 0; // M1: ks_fit_bind's
     return KS_OK;
 }
 

@@ -229,14 +229,17 @@ struct GangArgs {
 cudaError_t launch_gang_batch(const StreamBatchArgs& a, const GangArgs& g, uint32_t W, cudaStream_t st);
 
 // The bind calls (ks_spread_bind.cu), one mode each: ks_spread_bind, ks_affinity_bind, ks_profile_bind, ks_node_bind
-// with rules and ks_fit_bind.  Each mode filters as the one before it and adds rules; PROFILE and NODE also add scores;
-// FIT is NODE with the scalar resources after fit and selector.
-enum BindMode { BIND_SPREAD, BIND_AFFINITY, BIND_PROFILE, BIND_NODE, BIND_FIT };
+// with rules, ks_fit_bind and ks_gang_fit_bind.  Each mode filters as the one before it and adds rules; PROFILE and NODE
+// also add scores; FIT is NODE with the scalar resources after fit and selector; GANG_FIT is FIT with the pods cut into
+// gangs that commit or roll back whole.
+enum BindMode { BIND_SPREAD, BIND_AFFINITY, BIND_PROFILE, BIND_NODE, BIND_FIT, BIND_GANG_FIT };
 // Refusal words and score parts per pod in a mode's outputs (include/ksched.h)
 __host__ __device__ constexpr uint32_t bind_refusal_words(BindMode m) {
-    return m == BIND_FIT ? 5 : m == BIND_NODE ? 4 : m == BIND_SPREAD ? 1 : 2;
+    return m == BIND_FIT || m == BIND_GANG_FIT ? 5 : m == BIND_NODE ? 4 : m == BIND_SPREAD ? 1 : 2;
 }
-__host__ __device__ constexpr uint32_t bind_part_words(BindMode m) { return m == BIND_NODE || m == BIND_FIT ? 5 : 3; }
+__host__ __device__ constexpr uint32_t bind_part_words(BindMode m) {
+    return m == BIND_NODE || m == BIND_FIT || m == BIND_GANG_FIT ? 5 : 3;
+}
 
 // topology spread when binding (ks_spread_bind), the state of every mode.  Device memory.  Key k's domains are the
 // counts [Pk[k], Pk[k] + Dk[k]) of each group's S.
@@ -331,13 +334,23 @@ struct ProfileBindArgs {
     const int64_t* res_node_free;     // [R * N]: the caller's node_free, copied into res_free by the launcher
     int64_t* res_free;                // [R * N]: charged, final after the call
     uint32_t* pfref;                  // [grid] per-CTA resource refusals
+    // ks_gang_fit_bind (DESIGN.md 5s; read by GANG_FIT only), after every other field.  Gang j is the pods
+    // [goff[j], goff[j + 1]); after its last pod it commits when at least gmin[j] of them bound, else rolls back.  The
+    // rollback lists, once each, the groups whose gk words and the groups whose any-flag it recomputes: gmark[g] and
+    // gmark[G + h] hold the last gang (j + 1) that listed them, glist the lists.
+    uint32_t n_gangs;
+    const uint32_t* goff;             // [n_gangs + 1]
+    const uint32_t* gmin;             // [n_gangs]
+    uint32_t* gplaced;                // [n_gangs]: the pods of the gang that bound, before any rollback
+    uint32_t* gmark;                  // [2G], zeroed by the launcher
+    uint32_t* glist;                  // [2G]
 };
 constexpr int64_t PB_NOT_CAND = INT64_MIN;
 constexpr uint32_t NR_REASON = 3u, NR_TAINT = 1u, NR_AFFINITY = 2u, NR_AFF_OK = 4u, NR_TT_SHIFT = 3, NR_NA_SHIFT = 10;
 // One bind call's launches, in order: (NODE, FIT) k_node_rules_setup; k_bind_setup when G > 0; (every mode but SPREAD)
 // the counters zeroed, (PROFILE, NODE, FIT) the IPA counters and the bitmaps zeroed and the soft counts set, (FIT)
-// res_free set from res_node_free, then k_affinity_setup and (PROFILE, NODE, FIT) k_profile_setup over the existing pods
-// when E > 0; then the walk k_bind_seq, one cooperative launch of grid CTAs.  The fields a mode does not read may be left
-// zero.
+// res_free set from res_node_free, (GANG_FIT) gmark zeroed, then k_affinity_setup and (PROFILE, NODE, FIT)
+// k_profile_setup over the existing pods when E > 0; then the walk k_bind_seq, one cooperative launch of grid CTAs.  FIT
+// includes GANG_FIT here.  The fields a mode does not read may be left zero.
 cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st);
 } // namespace ks

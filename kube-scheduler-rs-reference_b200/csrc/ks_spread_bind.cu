@@ -1,10 +1,11 @@
 // ks_spread_bind.cu — the bind calls of include/ksched.h: ks_spread_bind (topology spread, DESIGN.md 5m),
 // ks_affinity_bind (and inter-pod affinity, 5n), ks_profile_bind (and the soft PodTopologySpread and InterPodAffinity
-// scores, 5o), ks_node_bind (and TaintToleration and NodeAffinity, 5p) and ks_fit_bind (and the pod count and scalar
-// resources of NodeResourcesFit, 5r).
+// scores, 5o), ks_node_bind (and TaintToleration and NodeAffinity, 5p), ks_fit_bind (and the pod count and scalar
+// resources of NodeResourcesFit, 5r) and ks_gang_fit_bind (ks_fit_bind with gangs that commit or roll back whole, 5s).
 // Each binds a mixed pod queue one pod at a time, each pod against the counts and the free[] every earlier pod left, as
 // upstream kube-scheduler runs one scheduling cycle per pod.  The calls differ by one BindMode (ks_launch.h), SPREAD,
-// AFFINITY, PROFILE, NODE or FIT (NODE's launches and walk, with the resources), and share:
+// AFFINITY, PROFILE, NODE, FIT (NODE's launches and walk, with the resources) or GANG_FIT (FIT's, with the gangs'
+// rollback), and share:
 //   BindFilter          the candidate filter: fit and selector, (FIT) the scalar resources, (NODE, FIT) the node's rule
 //                       word, hard spread and (AFF, every mode but SPREAD) rules 1-3 of the header
 //   k_bind_setup        one CTA per group (grid-strided): the group's eligible domains per constrained key, its counts
@@ -467,8 +468,9 @@ __device__ __forceinline__ const uint32_t* node_row(const ProfileBindArgs& a, in
 // bit counts one domain, so the partials add up to the distinct domains.  The other parity's bitmap is cleared.
 // NR (ks_node_bind): the node's rule word first; the taint and node-affinity refusals and, over the candidates, the
 // maxima of both raws into the CTA's partials.  FIT (ks_fit_bind, with NR): also the resource refusals, per warp in
-// s_fref, into the CTA's partial pfref.
-template <int W, bool NR = false, bool FIT = false>
+// s_fref, into the CTA's partial pfref.  GANG (ks_gang_fit_bind) changes no code here: it gives that walk its own
+// s_fref, since a function-local __shared__ array that two kernels share changes how the FIT walk addresses it.
+template <int W, bool NR = false, bool FIT = false, bool GANG = false>
 __device__ __forceinline__ void profile_pass1(const ProfileBindArgs& a, uint32_t p, uint32_t n0, uint32_t n1,
                                               ProfileShared& sh, NodeShared* ns = nullptr) {
     __shared__ uint32_t s_fref[SBD_WARPS]; // FIT only
@@ -872,6 +874,91 @@ __global__ void __launch_bounds__(SBD_THREADS) k_profile_setup(const ProfileBind
     }
 }
 
+// ---- ks_gang_fit_bind: the rollback of a gang (include/ksched.h, 5s) ----
+
+// CTA 0, after the commit of the gang's last pod: its pods [q0, q1) that bound are unbound and every piece of state their
+// commits changed goes back to its value before the gang.  The additive state is reversed by subtraction, per bound pod,
+// with the same node, update entries and soft-count condition that raised it; the sums wrap in two's complement, so the
+// order does not matter and atomics may run the pods in parallel.  Each group the gang charged (stamp = gang + 1 marks
+// it once) then gets its gk words from the restored counts, as k_bind_setup forms them: m = the minimum over the
+// eligible domains and the domains at m, except under minDomains (FORCED) or with no eligible domain, which no commit
+// changes.  Each group h whose any-flag a bound pod raised gets the flag from its restored A counters: the flag is 1
+// exactly when some pod of M_h counts in one of them.  Refusal words stay as the pods' turns wrote them.
+__device__ __forceinline__ void gang_rollback(const ProfileBindArgs& a, uint32_t q0, uint32_t q1, uint32_t stamp,
+                                           uint32_t* s_red) {
+    __shared__ uint32_t s_n[2]; // groups listed: for their gk words, for their any-flag
+    const SpreadBindArgs& b = a.b;
+    const uint32_t tid = threadIdx.x;
+    if (tid < 2) s_n[tid] = 0;
+    __syncthreads(); // also orders the commit's writes before the reads below
+    for (uint32_t q = q0 + tid; q < q1; q += SBD_THREADS) {
+        const int32_t n = __ldcg(b.out_idx + q);
+        if (n < 0) continue;
+        b.out_idx[q] = -1;
+        b.out_score[q] = 0;
+        if (a.out_parts)
+            for (uint32_t i = 0; i < 5; i++) a.out_parts[5 * (size_t)q + i] = 0;
+        atomicAdd(reinterpret_cast<unsigned long long*>(b.free_cpu + n), (unsigned long long)__ldg(b.req_cpu + q));
+        atomicAdd(reinterpret_cast<unsigned long long*>(b.free_mem + n), (unsigned long long)__ldg(b.req_mem + q));
+        for (uint32_t r = 0; r < a.R; r++)
+            atomicAdd(reinterpret_cast<unsigned long long*>(a.res_free + (size_t)r * b.N + n),
+                      (unsigned long long)__ldg(a.res_req + (size_t)q * a.R + r));
+        const int32_t g = __ldg(b.group + q);
+        if (g < 0) continue;
+        const uint32_t ck = constrained_keys(b, g), sk = soft_keys(a, g);
+        const bool soft = sk && !pts_ignored(a, sk, __ldg(a.soft_all + g), (uint32_t)n);
+        for (uint32_t k = 0; k < b.K; k++) {
+            const int32_t d = __ldg(b.dom + (size_t)k * b.N + n);
+            if (ck >> k & 1u) atomicSub(b.cnt + (size_t)g * b.S + b.Pk[k] + (uint32_t)d, 1u);
+            if (soft && (sk >> k & 1u) && d >= 0) atomicSub(a.scnt + (size_t)g * b.S + b.Pk[k] + (uint32_t)d, 1u);
+        }
+        if (ck && atomicExch(a.gmark + g, stamp) != stamp) a.glist[atomicAdd(s_n, 1u)] = (uint32_t)g;
+        for (uint32_t e = __ldg(b.upd_off + g), e1 = __ldg(b.upd_off + g + 1); e < e1; e++) {
+            const uint32_t en = __ldg(b.upd + e), h = en & 0xffffu, k = en >> 16 & 0xfu, kind = en >> 20;
+            const int32_t d = __ldg(b.dom + (size_t)k * b.N + n);
+            if (d < 0) continue;
+            atomicSub(b.acnt + __ldg(b.abase + ((size_t)h * b.K + k) * 2 + kind) + (uint32_t)d, 1u);
+            if (kind && atomicExch(a.gmark + b.G + h, stamp) != stamp) a.glist[b.G + atomicAdd(s_n + 1, 1u)] = h;
+        }
+        for (uint32_t e = __ldg(a.iupd_off + g), e1 = __ldg(a.iupd_off + g + 1); e < e1; e++) {
+            const uint32_t en = __ldg(a.iupd + e), h = en & 0xffffu, k = en >> 16;
+            const int32_t d = __ldg(b.dom + (size_t)k * b.N + n);
+            if (d < 0) continue;
+            atomicAdd(reinterpret_cast<unsigned long long*>(a.icnt + __ldg(a.ibase + (size_t)h * b.K + k) + (uint32_t)d),
+                      (unsigned long long)-(int64_t)__ldg(a.icoef + e));
+        }
+    }
+    __syncthreads();
+    for (uint32_t i = 0, n_gk = s_n[0]; i < n_gk; i++) {
+        const uint32_t g = __ldcg(a.glist + i), ck = constrained_keys(b, (int32_t)g);
+        for (uint32_t k = 0; k < b.K; k++) {
+            uint32_t* st = b.gk + ((size_t)g * b.K + k) * GK_WORDS;
+            if (!(ck >> k & 1u) || (__ldcg(st + GK_FLAGS) & GK_FORCED) || __ldcg(st + GK_NE) == 0) continue;
+            const size_t base = (size_t)g * b.S + b.Pk[k];
+            uint32_t mn = 0xffffffffu;
+            for (uint32_t d = tid; d < b.Dk[k]; d += SBD_THREADS)
+                if (b.elig[base + d]) mn = min(mn, __ldcg(b.cnt + base + d));
+            mn = cta_min(mn, s_red);
+            const uint32_t at = domains_at(b, g, k, mn, s_red);
+            if (tid == 0) {
+                st[GK_M] = mn;
+                st[GK_AT_M] = at;
+            }
+        }
+    }
+    for (uint32_t i = 0, n_any = s_n[1]; i < n_any; i++) {
+        const uint32_t h = __ldcg(a.glist + b.G + i);
+        uint32_t any = 0;
+        for (uint32_t k = 0; k < b.K; k++) {
+            const uint32_t base = __ldg(b.abase + ((size_t)h * b.K + k) * 2 + 1);
+            if (base == AFF_NONE) continue;
+            for (uint32_t d = tid; d < b.Dk[k]; d += SBD_THREADS) any |= __ldcg(b.acnt + base + d);
+        }
+        any = __syncthreads_or(any != 0);
+        if (tid == 0) b.acnt[b.any_base + h] = any ? 1u : 0u;
+    }
+}
+
 // ks_node_bind: one rule word per (class c, node n) over the grid-strided C x N pairs (include/ksched.h, 5p)
 __global__ void __launch_bounds__(SBD_THREADS) k_node_rules_setup(const ProfileBindArgs a) {
     const uint64_t total = (uint64_t)a.C * a.b.N;
@@ -906,10 +993,13 @@ __global__ void __launch_bounds__(SBD_THREADS) k_node_rules_setup(const ProfileB
 
 // The walk of every bind call: one cooperative launch, one node slice per CTA, the pods in queue order with grid
 // barriers between their phases.  SPREAD and AFFINITY run phase A and phase B; PROFILE and NODE run pass 1, pass 2 when
-// the pod's group has soft keys, pass 3 and the commit.  Each family declares only its own shared state.
+// the pod's group has soft keys, pass 3 and the commit.  GANG_FIT is FIT, and after the commit of a gang's last pod CTA 0
+// writes the gang's count and rolls it back when it is short, before that pod's last barrier.  Each family declares only
+// its own shared state.
 template <int W, BindMode M>
 __global__ void __launch_bounds__(SBD_THREADS, 1) k_bind_seq(const ProfileBindArgs a) {
-    constexpr bool AFF = M != BIND_SPREAD, NR = M == BIND_NODE || M == BIND_FIT, FIT = M == BIND_FIT;
+    constexpr bool AFF = M != BIND_SPREAD, GANG = M == BIND_GANG_FIT, FIT = M == BIND_FIT || GANG,
+                   NR = M == BIND_NODE || FIT;
     cg::grid_group grid = cg::this_grid();
     const uint32_t G = gridDim.x;
     const uint32_t chunk = (a.b.N + G - 1) / G, n0 = min(a.b.N, blockIdx.x * chunk), n1 = min(a.b.N, n0 + chunk);
@@ -930,8 +1020,9 @@ __global__ void __launch_bounds__(SBD_THREADS, 1) k_bind_seq(const ProfileBindAr
     } else {
         __shared__ ProfileShared sh;
         __shared__ NodeShared ns; // NR only
+        uint32_t j = 0, placed = 0; // GANG, CTA 0: the current gang and its pods bound so far
         for (uint32_t p = 0; p < a.b.P; p++) {
-            profile_pass1<W, NR, FIT>(a, p, n0, n1, sh, &ns);
+            profile_pass1<W, NR, FIT, GANG>(a, p, n0, n1, sh, &ns);
             __threadfence();
             grid.sync();
             if (soft_keys(a, __ldg(a.b.group + p))) { // uniform: every CTA knows the pod's group
@@ -942,7 +1033,18 @@ __global__ void __launch_bounds__(SBD_THREADS, 1) k_bind_seq(const ProfileBindAr
             profile_pass3<NR>(a, p, n0, n1, sh, &ns);
             __threadfence();
             grid.sync();
-            if (blockIdx.x == 0) profile_commit<NR, FIT>(a, p, sh, &ns);
+            if (blockIdx.x == 0) {
+                profile_commit<NR, FIT>(a, p, sh, &ns);
+                if constexpr (GANG) { // after the gang's last pod: its count, and the rollback before the barrier
+                    placed += sh.bidx >= 0;
+                    if (p + 1 == __ldg(a.goff + j + 1)) {
+                        if (threadIdx.x == 0) a.gplaced[j] = placed;
+                        if (placed < __ldg(a.gmin + j)) gang_rollback(a, __ldg(a.goff + j), p + 1, j + 1, sh.ref);
+                        j++;
+                        placed = 0;
+                    }
+                }
+            }
             __threadfence();
             grid.sync();
         }
@@ -955,7 +1057,8 @@ cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_w
     return with_label_width(W, [&](auto w) {
         constexpr int LW = decltype(w)::value;
         const SpreadBindArgs& b = a.b;
-        const bool fit = mode == BIND_FIT, nr = mode == BIND_NODE || fit, soft = mode == BIND_PROFILE || nr;
+        const bool gang = mode == BIND_GANG_FIT, fit = mode == BIND_FIT || gang, nr = mode == BIND_NODE || fit,
+                   soft = mode == BIND_PROFILE || nr;
         const auto launched = [](uint32_t n) {
             g_launches += n;
             return cudaGetLastError();
@@ -981,6 +1084,7 @@ cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_w
                             : cudaMemsetAsync(a.scnt, 0, (size_t)b.G * b.S * 4, st);
                 if (e == cudaSuccess && fit && a.R)
                     e = cudaMemcpyAsync(a.res_free, a.res_node_free, (size_t)a.R * b.N * 8, cudaMemcpyDeviceToDevice, st);
+                if (e == cudaSuccess && gang && b.G) e = cudaMemsetAsync(a.gmark, 0, (size_t)b.G * 8, st);
             }
             if (e != cudaSuccess) return e;
             if (b.E) {
@@ -993,7 +1097,8 @@ cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_w
                            : mode == BIND_AFFINITY ? reinterpret_cast<const void*>(k_bind_seq<LW, BIND_AFFINITY>)
                            : mode == BIND_PROFILE  ? reinterpret_cast<const void*>(k_bind_seq<LW, BIND_PROFILE>)
                            : mode == BIND_NODE     ? reinterpret_cast<const void*>(k_bind_seq<LW, BIND_NODE>)
-                                                   : reinterpret_cast<const void*>(k_bind_seq<LW, BIND_FIT>);
+                           : mode == BIND_FIT      ? reinterpret_cast<const void*>(k_bind_seq<LW, BIND_FIT>)
+                                                   : reinterpret_cast<const void*>(k_bind_seq<LW, BIND_GANG_FIT>);
         ProfileBindArgs c = a;
         void* args[] = {&c};
         e = cudaLaunchCooperativeKernel(walk, dim3(b.grid), dim3(SBD_THREADS), args, 0, st);

@@ -63,6 +63,9 @@ for _name, _res, _args in [
     ("ksh_compile_resources", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_size_t, _vp, _vp]),
     ("ksh_reconcile_fit", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp,
                                     _vp, _vp, C.c_int, _vp, _vp, _vp, C.c_size_t, _vp]),
+    ("ksh_reconcile_fit_gangs", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp,
+                                          _vp, _vp, _vp, _vp, C.c_uint64, _vp, C.c_int, _vp, _vp, _vp, _vp,
+                                          C.c_size_t, _vp]),
 ]:
     _proto(_name, _res, *_args)
 
@@ -606,9 +609,31 @@ class Context:
                                      term_weight, hard_affinity_weight, weight_spread, weight_affinity, group_rules,
                                      weight_taint, weight_node_affinity, True)
 
+    def reconcile_fit_gangs(self, pods, n, group, n_groups, topology_keys, offset, min_member, terms=(),
+                            existing_pods=(), max_skew=None, min_domains=None, existing_nodes=None,
+                            policy=capi.KS_SCORE_LEAST_BALANCED, json_cap=None, soft_skew=None, soft_all_keys=None,
+                            term_weight=None, hard_affinity_weight=1, weight_spread=2, weight_affinity=2,
+                            group_rules=None, weight_taint=3, weight_node_affinity=2):
+        """reconcile_fit over gangs placed all or nothing (ksh_reconcile_fit_gangs): gang j is pods
+        [offset[j], offset[j+1]), its running members count toward min_member[j], and the pods of a gang that cannot
+        commit get KSH_RECONCILE_GANG_UNSATISFIED.  Returns (status[n], node_idx[n], bodies[n], placed[n_gangs])."""
+        offset = np.ascontiguousarray(offset, np.uint64).reshape(-1)
+        min_member = np.ascontiguousarray(min_member, np.uint32).reshape(-1)
+        g = offset.shape[0] - 1
+        if g < 0 or min_member.shape[0] != g:
+            raise ValueError(f"need len(offset) >= 1 and len(min_member) == len(offset) - 1 "
+                             f"(got {offset.shape[0]} and {min_member.shape[0]})")
+        placed = np.empty(g, np.uint32)
+        return self._reconcile_rules(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
+                                     min_domains, existing_nodes, policy, json_cap, soft_skew, soft_all_keys,
+                                     term_weight, hard_affinity_weight, weight_spread, weight_affinity, group_rules,
+                                     weight_taint, weight_node_affinity, True,
+                                     gangs=(offset, g, min_member, placed)) + (placed,)
+
     def _reconcile_rules(self, pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew, min_domains,
                          existing_nodes, policy, json_cap, soft_skew, soft_all_keys, term_weight, hard_affinity_weight,
-                         weight_spread, weight_affinity, group_rules, weight_taint, weight_node_affinity, fit):
+                         weight_spread, weight_affinity, group_rules, weight_taint, weight_node_affinity, fit,
+                         gangs=None):
         # ksh_reconcile_nodes, or with fit ksh_reconcile_fit
         nr = None
         if group_rules is not None:
@@ -627,12 +652,12 @@ class Context:
                                        int(weight_spread), int(weight_affinity))
         return self._reconcile_terms(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
                                      min_domains, existing_nodes, policy, json_cap, scoring, nodes=True,
-                                     rules=None if nr is None else nr[0], fit=fit)
+                                     rules=None if nr is None else nr[0], fit=fit, gangs=gangs)
 
     def _reconcile_terms(self, pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew, min_domains,
-                         existing_nodes, policy, json_cap, scoring, nodes=False, rules=None, fit=False):
+                         existing_nodes, policy, json_cap, scoring, nodes=False, rules=None, fit=False, gangs=None):
         # ksh_reconcile_affinity, or with scoring ksh_reconcile_profile, or with nodes ksh_reconcile_nodes (with fit
-        # ksh_reconcile_fit)
+        # ksh_reconcile_fit, and with gangs = (offset, n_gangs, min_member, placed) ksh_reconcile_fit_gangs)
         k = len(topology_keys)
         group = np.ascontiguousarray(group, np.int32).reshape(-1)
         if group.shape[0] != n:
@@ -670,7 +695,13 @@ class Context:
                 None if names is None else C.cast(names, _vp), None if ex_off is None else ex_off.ctypes.data,
                 C.byref(aff))
         tail = (int(policy), status.ctypes.data, node.ctypes.data, C.addressof(buf), cap, off.ctypes.data)
-        if fit:
+        if gangs is not None:
+            offset, g, min_member, placed = gangs
+            check(lib.ksh_reconcile_fit_gangs(*head, C.byref(scoring), None if rules is None else C.byref(rules),
+                                              offset.ctypes.data, g, min_member.ctypes.data, int(policy),
+                                              status.ctypes.data, node.ctypes.data, placed.ctypes.data,
+                                              C.addressof(buf), cap, off.ctypes.data), "ksh_reconcile_fit_gangs")
+        elif fit:
             check(lib.ksh_reconcile_fit(*head, C.byref(scoring), None if rules is None else C.byref(rules), *tail),
                   "ksh_reconcile_fit")
         elif nodes:

@@ -523,7 +523,7 @@ class Snapshot:
     def fit_bind(self, req_cpu, req_mem, sel, group, n_groups, keys, terms=(), existing_pods=None, max_skew=None,
                  min_domains=None, existing=None, policy=capi.KS_SCORE_LEAST_BALANCED, soft_skew=None,
                  soft_all_keys=None, term_weight=None, hard_affinity_weight=1, weight_spread=2, weight_affinity=2,
-                 rules=None, node_free=None, pod_req=None, want_counts=True):
+                 rules=None, node_free=None, pod_req=None, want_counts=True, _gangs=None):
         """node_bind with the pod count and scalar resources of NodeResourcesFit (ks_fit_bind).  node_free [R, N] and
         pod_req [P, R] (int64), or both None (the C call's NULL res); rules as node_bind takes them (None = NULL).
         Returns node_bind's tuple with refused [P, 5] (resources, taint, node affinity, spread, inter-pod affinity),
@@ -544,13 +544,35 @@ class Snapshot:
         return self._scored_bind(rules if rules is not None else False, req_cpu, req_mem, sel, group, n_groups, keys,
                                  terms, existing_pods, max_skew, min_domains, existing, policy, soft_skew,
                                  soft_all_keys, term_weight, hard_affinity_weight, weight_spread, weight_affinity,
-                                 want_counts, res=res, fit=True)
+                                 want_counts, res=res, fit=True, gangs=_gangs)
+
+    def gang_fit_bind(self, req_cpu, req_mem, sel, group, n_groups, keys, offset, min_member, terms=(),
+                      existing_pods=None, max_skew=None, min_domains=None, existing=None,
+                      policy=capi.KS_SCORE_LEAST_BALANCED, soft_skew=None, soft_all_keys=None, term_weight=None,
+                      hard_affinity_weight=1, weight_spread=2, weight_affinity=2, rules=None, node_free=None,
+                      pod_req=None, want_counts=True):
+        """fit_bind with the queue cut into gangs placed all or nothing (ks_gang_fit_bind): gang j is the pods
+        [offset[j], offset[j+1]) and keeps its bindings only when at least min_member[j] of them bound; otherwise it
+        rolls back and the next gang sees exactly what it saw.  Returns fit_bind's tuple, then placed uint32 [n] (the
+        gang's pods that bound, before any rollback)."""
+        offset = _c(offset, np.uint64).reshape(-1)
+        min_member = _c(min_member, np.uint32).reshape(-1)
+        n = offset.shape[0] - 1
+        if n < 0 or min_member.shape[0] != n:
+            raise ValueError(f"need len(offset) >= 1 and len(min_member) == len(offset) - 1 "
+                             f"(got {offset.shape[0]} and {min_member.shape[0]})")
+        placed = np.empty(n, np.uint32)
+        gangs = capi.ks_gangs(n, _ptr(offset), _ptr(min_member))
+        return self.fit_bind(req_cpu, req_mem, sel, group, n_groups, keys, terms, existing_pods, max_skew, min_domains,
+                             existing, policy, soft_skew, soft_all_keys, term_weight, hard_affinity_weight,
+                             weight_spread, weight_affinity, rules, node_free, pod_req, want_counts,
+                             _gangs=(gangs, placed)) + (placed,)
 
     def _scored_bind(self, rules, req_cpu, req_mem, sel, group, n_groups, keys, terms, existing_pods, max_skew,
                      min_domains, existing, policy, soft_skew, soft_all_keys, term_weight, hard_affinity_weight,
-                     weight_spread, weight_affinity, want_counts, res=None, fit=False):
+                     weight_spread, weight_affinity, want_counts, res=None, fit=False, gangs=None):
         """ks_profile_bind when rules is None, else ks_node_bind (rules False = its NULL rules); with fit, ks_fit_bind
-        with res = (R, node_free, pod_req) or None."""
+        with res = (R, node_free, pod_req) or None, and with gangs = (ks_gangs, placed) ks_gang_fit_bind."""
         pods, keep = self._pods(req_cpu, req_mem, sel)
         p, g = int(pods.n), int(n_groups)
         group = _c(group, np.int32).reshape(-1)
@@ -612,10 +634,18 @@ class Snapshot:
             r = res[0] if res is not None else 0
             br = capi.ks_bind_resources(r, _ptr(res[1]), _ptr(res[2])) if res is not None else None
             free_r = np.empty((r, self.n_nodes), np.int64)
-            check(lib.ks_fit_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff), C.byref(scoring),
-                                  C.byref(nr) if nr is not None else None, C.byref(br) if br is not None else None,
-                                  int(policy), _ptr(idx), _ptr(score), _ptr(parts), _ptr(refused), _ptr(counts),
-                                  _ptr(soft), _ptr(free_r)), "ks_fit_bind")
+            if gangs is not None:
+                check(lib.ks_gang_fit_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
+                                           C.byref(scoring), C.byref(nr) if nr is not None else None,
+                                           C.byref(br) if br is not None else None, C.byref(gangs[0]), int(policy),
+                                           _ptr(idx), _ptr(score), _ptr(parts), _ptr(refused), _ptr(counts),
+                                           _ptr(soft), _ptr(free_r), _ptr(gangs[1])), "ks_gang_fit_bind")
+            else:
+                check(lib.ks_fit_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
+                                      C.byref(scoring), C.byref(nr) if nr is not None else None,
+                                      C.byref(br) if br is not None else None, int(policy), _ptr(idx), _ptr(score),
+                                      _ptr(parts), _ptr(refused), _ptr(counts), _ptr(soft), _ptr(free_r)),
+                      "ks_fit_bind")
         elif rules is None:
             check(lib.ks_profile_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
                                       C.byref(scoring), int(policy), _ptr(idx), _ptr(score), _ptr(parts),
