@@ -1452,6 +1452,24 @@ int ksh_reconcile_batch(ksh_context* c, const ks_pod_obj* pods, uint64_t n, int 
 }
 KSH_CATCH
 
+// A cut of n pods into n_cut groups or gangs (`what`) by offset: each of 1 to max_size pods (no limit at UINT64_MAX) and
+// its min_member within its size
+static int check_cut(const std::string& what, const uint64_t* offset, uint64_t n_cut, const uint32_t* min_member,
+                     uint64_t n, uint64_t max_size) {
+    if (offset[0] != 0) return fail(KS_ERR_INVALID, what + "_offset[0] must be 0");
+    for (uint64_t j = 0; j < n_cut; j++) {
+        if (offset[j + 1] < offset[j]) return fail(KS_ERR_INVALID, what + " offsets decrease");
+        const uint64_t size = offset[j + 1] - offset[j];
+        if (size == 0 || size > max_size)
+            return fail(KS_ERR_RANGE, max_size == UINT64_MAX ? "a " + what + " has no pod"
+                                                             : "a " + what + " has " + std::to_string(size) + " pods (1.." +
+                                                                   std::to_string(max_size) + ")");
+        if (min_member[j] > size) return fail(KS_ERR_RANGE, "min_member above the " + what + "'s size");
+    }
+    if (offset[n_cut] != n) return fail(KS_ERR_INVALID, what + "_offset[n_" + what + "s] must be n_pods");
+    return KS_OK;
+}
+
 // reconcile() for pod groups: ksh_reconcile_batch's filtering, then ks_gang_bind over the pods that go to the device,
 // one sub-group per group; already bound members count toward min_member
 int ksh_reconcile_gangs(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const uint64_t* group_offset, uint64_t n_groups,
@@ -1459,17 +1477,10 @@ int ksh_reconcile_gangs(ksh_context* c, const ks_pod_obj* pods, uint64_t n, cons
                         uint32_t* out_placed, char* json, size_t cap, int64_t* out_json_off) try {
     if (!c || !group_offset || (n && (!pods || !out_status || !out_node_idx)) || (n_groups && !min_member))
         return fail(KS_ERR_INVALID, "NULL argument");
-    if (group_offset[0] != 0) return fail(KS_ERR_INVALID, "group_offset[0] must be 0");
-    for (uint64_t g = 0; g < n_groups; g++) {
-        if (group_offset[g + 1] < group_offset[g]) return fail(KS_ERR_INVALID, "group offsets decrease");
-        const uint64_t size = group_offset[g + 1] - group_offset[g];
-        if (size == 0 || size > KS_GANG_MAX_SIZE)
-            return fail(KS_ERR_RANGE, "a group has " + std::to_string(size) + " pods (1.." + std::to_string(KS_GANG_MAX_SIZE) + ")");
-        if (min_member[g] > size) return fail(KS_ERR_RANGE, "min_member above the group's size");
-    }
-    if (group_offset[n_groups] != n) return fail(KS_ERR_INVALID, "group_offset[n_groups] must be n_pods");
+    int rc = check_cut("group", group_offset, n_groups, min_member, n, KS_GANG_MAX_SIZE);
+    if (rc) return rc;
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    int rc = device_ready(c, ks_gang_bind, "ks_gang_bind");
+    rc = device_ready(c, ks_gang_bind, "ks_gang_bind");
     if (rc) return rc;
     std::vector<uint64_t> todo, sub_off{0}, sub_group; // the pods that go to the device; sub-group k is group sub_group[k]
     std::vector<uint32_t> sub_min;
@@ -2051,33 +2062,109 @@ static int compile_resources(ksh_context* c, const ks_pod_obj* pods, uint64_t n,
     return KS_OK;
 }
 
-// reconcile() under topology spread: ksh_reconcile_batch's filtering, then ks_spread_bind over the pods that go to the
-// device, each in its group.  Group g's existing pods under key k count when their node is in the store and carries key k
-// and every key g constrains.  With aff set (ksh_reconcile_affinity), ks_affinity_bind with its terms and the existing
-// pods whose node is in the store; max_skew may then be NULL.  With aff and sc set (ksh_reconcile_profile),
-// ks_profile_bind with the same terms and the soft terms of sc; the soft counts start from the same existing counts.
-// With gang_offset set as well (ksh_reconcile_fit_gangs), ks_gang_fit_bind over the gangs' pods that go to the device,
-// one sub-gang per gang; already bound members count toward min_member, as in ksh_reconcile_gangs.
+// The bind call behind each reconcile mode (ks_spread_bind to ks_gang_fit_bind), and its refusal words per pod: the
+// word of each reason, -1 where the mode has none.  Node affinity follows taint.
+enum ReconcileMode { RM_SPREAD, RM_AFFINITY, RM_PROFILE, RM_NODES, RM_FIT, RM_FIT_GANGS };
+struct RefusalWords { size_t n; int res, taint, spread, aff; };
+static const RefusalWords REFUSAL_WORDS[] = {{1, -1, -1, 0, -1}, {2, -1, -1, 0, 1}, {2, -1, -1, 0, 1},
+                                             {4, -1, 0, 2, 3},   {5, 0, 1, 3, 4},    {5, 0, 1, 3, 4}};
+
+// What a reconcile mode adds to reconcile_spread's arguments: the soft terms (PROFILE on), the node rules (NODES on) and
+// the gangs (FIT_GANGS)
+struct ReconcileRequest {
+    ReconcileMode mode = RM_SPREAD;
+    const ks_bind_scoring* sc = nullptr;
+    const ksh_node_rules* nr = nullptr;
+    const uint64_t* gang_offset = nullptr;
+    uint64_t n_gangs = 0;
+    const uint32_t* min_member = nullptr;
+    uint32_t* out_placed = nullptr;
+};
+
+// The mode's device entry: with kp NULL, device_ready for it; else the call over the packed batch, which commits
+// capacity on the device
+static int bind_device(ksh_context* c, ReconcileMode m, const ks_pods* kp, const int32_t* group, uint32_t G,
+                       const ks_spread_multi* sp, const ks_pod_affinity* pa, const ks_bind_scoring* sc,
+                       const ks_node_rules* nr, const ks_bind_resources* br, const ks_gangs* kg, int policy,
+                       int32_t* idx, uint32_t* refused, uint32_t* placed) {
+    switch (m) {
+    case RM_SPREAD:
+        if (!kp) return device_ready(c, ks_spread_bind, "ks_spread_bind");
+        return ks_spread_bind(c->snap, kp, group, G, sp, policy, idx, nullptr, refused, nullptr);
+    case RM_AFFINITY:
+        if (!kp) return device_ready(c, ks_affinity_bind, "ks_affinity_bind");
+        return ks_affinity_bind(c->snap, kp, group, G, sp, pa, policy, idx, nullptr, refused, nullptr);
+    case RM_PROFILE:
+        if (!kp) return device_ready(c, ks_profile_bind, "ks_profile_bind");
+        return ks_profile_bind(c->snap, kp, group, G, sp, pa, sc, policy, idx, nullptr, nullptr, refused, nullptr,
+                               nullptr);
+    case RM_NODES:
+        if (!kp) return device_ready(c, ks_node_bind, "ks_node_bind");
+        return ks_node_bind(c->snap, kp, group, G, sp, pa, sc, nr, policy, idx, nullptr, nullptr, refused, nullptr,
+                            nullptr);
+    case RM_FIT:
+        if (!kp) return device_ready(c, ks_fit_bind, "ks_fit_bind");
+        return ks_fit_bind(c->snap, kp, group, G, sp, pa, sc, nr, br, policy, idx, nullptr, nullptr, refused, nullptr,
+                           nullptr, nullptr);
+    case RM_FIT_GANGS:
+        if (!kp) return device_ready(c, ks_gang_fit_bind, "ks_gang_fit_bind");
+        return ks_gang_fit_bind(c->snap, kp, group, G, sp, pa, sc, nr, br, kg, policy, idx, nullptr, nullptr, refused,
+                                nullptr, nullptr, nullptr, placed);
+    }
+    return fail(KS_ERR_INVALID, "bad reconcile mode");
+}
+
+// The gangs' part of a batch (ksh_reconcile_fit_gangs): keeps of todo, sub and sub_group the pods of the gangs that can
+// still commit, as sub-gang k = [sub_off[k], sub_off[k + 1]) of gang sub_gang[k] needing sub_min[k] more pods.  Running
+// members count toward min_member, as in ksh_reconcile_gangs; a gang with too few schedulable members is not tried.
+static void cut_gangs(const ReconcileRequest& m, int32_t* out_status, std::vector<uint64_t>& todo,
+                      std::vector<ks_pod_obj>& sub, std::vector<int32_t>& sub_group, std::vector<uint64_t>& sub_off,
+                      std::vector<uint64_t>& sub_gang, std::vector<uint32_t>& sub_min) {
+    std::vector<uint64_t> keep;
+    std::vector<ks_pod_obj> keep_pods;
+    std::vector<int32_t> keep_group;
+    for (uint64_t j = 0, t = 0; j < m.n_gangs; j++) {
+        uint32_t bound = 0; // running members of the gang
+        for (uint64_t i = m.gang_offset[j]; i < m.gang_offset[j + 1]; i++) bound += out_status[i] == KSH_RECONCILE_OK;
+        const size_t first = t;
+        while (t < todo.size() && todo[t] < m.gang_offset[j + 1]) t++;
+        const uint32_t need = m.min_member[j] > bound ? m.min_member[j] - bound : 0;
+        if (t == first) continue;
+        if (need > t - first) { // too few schedulable members: the gang cannot commit, nothing is tried
+            for (size_t k = first; k < t; k++) out_status[todo[k]] = KSH_RECONCILE_GANG_UNSATISFIED;
+            continue;
+        }
+        for (size_t k = first; k < t; k++) {
+            keep.push_back(todo[k]);
+            keep_pods.push_back(sub[k]);
+            keep_group.push_back(sub_group[k]);
+        }
+        sub_off.push_back(keep.size());
+        sub_gang.push_back(j);
+        sub_min.push_back(need);
+    }
+    todo.swap(keep);
+    sub.swap(keep_pods);
+    sub_group.swap(keep_group);
+}
+
+// reconcile() under topology spread: ksh_reconcile_batch's filtering, then the mode's bind call over the pods that go to
+// the device, each in its group.  Group g's existing pods under key k count when their node is in the store and carries
+// key k and every key g constrains.  AFFINITY on: the terms and the existing pods whose node is in the store; max_skew may
+// then be NULL.  PROFILE on: the soft terms of m.sc, whose counts start from the same existing counts.  NODES on: the
+// node rules.  FIT on: the batch's resources.  FIT_GANGS: one sub-gang per gang, as cut_gangs leaves them.
 static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
                             const char* const* topology_keys, uint32_t K, const uint32_t* max_skew,
                             const uint32_t* min_domains, const char* const* existing_node_names,
                             const uint64_t* existing_offset, const ksh_pod_affinity* aff, int policy, int32_t* out_status,
                             int32_t* out_node_idx, char* json, size_t cap, int64_t* out_json_off,
-                            const ks_bind_scoring* sc = nullptr, const ksh_node_rules* nr = nullptr,
-                            bool nodes = false, bool fit = false, const uint64_t* gang_offset = nullptr,
-                            uint64_t n_gangs = 0, const uint32_t* min_member = nullptr, uint32_t* out_placed = nullptr) {
+                            const ReconcileRequest& m) {
     if (!c || !topology_keys || (n && (!pods || !group || !out_status || !out_node_idx)) || (n_groups && !max_skew && !aff))
         return fail(KS_ERR_INVALID, "NULL argument");
-    if (gang_offset) { // as ksh_reconcile_gangs checks them, without its size limit
-        if (n_gangs && !min_member) return fail(KS_ERR_INVALID, "NULL argument");
-        if (gang_offset[0] != 0) return fail(KS_ERR_INVALID, "gang_offset[0] must be 0");
-        for (uint64_t j = 0; j < n_gangs; j++) {
-            if (gang_offset[j + 1] < gang_offset[j]) return fail(KS_ERR_INVALID, "gang offsets decrease");
-            const uint64_t size = gang_offset[j + 1] - gang_offset[j];
-            if (size == 0) return fail(KS_ERR_RANGE, "a gang has no pod");
-            if (min_member[j] > size) return fail(KS_ERR_RANGE, "min_member above the gang's size");
-        }
-        if (gang_offset[n_gangs] != n) return fail(KS_ERR_INVALID, "gang_offset[n_gangs] must be n_pods");
+    if (m.gang_offset) { // as ksh_reconcile_gangs checks them, without its size limit
+        if (m.n_gangs && !m.min_member) return fail(KS_ERR_INVALID, "NULL argument");
+        const int rc = check_cut("gang", m.gang_offset, m.n_gangs, m.min_member, n, UINT64_MAX);
+        if (rc) return rc;
     }
     if (K == 0 || K > KS_SPREAD_MAX_KEYS)
         return fail(KS_ERR_RANGE, std::to_string(K) + " topology keys (1 to " + std::to_string(KS_SPREAD_MAX_KEYS) + ")");
@@ -2094,12 +2181,8 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     if (aff && aff->n_existing && (!aff->existing_group || !aff->existing_node_name))
         return fail(KS_ERR_INVALID, "NULL existing_group or existing_node_name");
     std::lock_guard<std::recursive_mutex> lk(c->mu);
-    int rc = gang_offset ? device_ready(c, ks_gang_fit_bind, "ks_gang_fit_bind")
-             : fit   ? device_ready(c, ks_fit_bind, "ks_fit_bind")
-             : nodes ? device_ready(c, ks_node_bind, "ks_node_bind")
-             : sc  ? device_ready(c, ks_profile_bind, "ks_profile_bind")
-             : aff ? device_ready(c, ks_affinity_bind, "ks_affinity_bind")
-                   : device_ready(c, ks_spread_bind, "ks_spread_bind");
+    int rc = bind_device(c, m.mode, nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, nullptr,
+                         nullptr, nullptr);
     if (rc) return rc;
     std::vector<uint64_t> todo;
     std::vector<ks_pod_obj> sub; // the pods that go to the device, in arrival order, and their groups
@@ -2113,47 +2196,19 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
         sub.push_back(pods[i]);
         sub_group.push_back(group[i]);
     }
-    // ks_gang_fit_bind: sub-gang k is the device pods [sub_off[k], sub_off[k + 1]) of gang sub_gang[k], needing sub_min[k]
-    std::vector<uint64_t> sub_off{0}, sub_gang;
+    std::vector<uint64_t> sub_off{0}, sub_gang; // FIT_GANGS: the sub-gangs
     std::vector<uint32_t> sub_min;
-    if (out_placed)
-        for (uint64_t j = 0; j < n_gangs; j++) out_placed[j] = 0;
-    if (gang_offset) {
-        std::vector<uint64_t> keep;
-        std::vector<ks_pod_obj> keep_pods;
-        std::vector<int32_t> keep_group;
-        for (uint64_t j = 0, t = 0; j < n_gangs; j++) {
-            uint32_t bound = 0; // running members of the gang
-            for (uint64_t i = gang_offset[j]; i < gang_offset[j + 1]; i++) bound += out_status[i] == KSH_RECONCILE_OK;
-            const size_t first = t;
-            while (t < todo.size() && todo[t] < gang_offset[j + 1]) t++;
-            const uint32_t need = min_member[j] > bound ? min_member[j] - bound : 0;
-            if (t == first) continue;
-            if (need > t - first) { // too few schedulable members: the gang cannot commit, nothing is tried
-                for (size_t k = first; k < t; k++) out_status[todo[k]] = KSH_RECONCILE_GANG_UNSATISFIED;
-                continue;
-            }
-            for (size_t k = first; k < t; k++) {
-                keep.push_back(todo[k]);
-                keep_pods.push_back(sub[k]);
-                keep_group.push_back(sub_group[k]);
-            }
-            sub_off.push_back(keep.size());
-            sub_gang.push_back(j);
-            sub_min.push_back(need);
-        }
-        todo.swap(keep);
-        sub.swap(keep_pods);
-        sub_group.swap(keep_group);
-    }
+    if (m.out_placed)
+        for (uint64_t j = 0; j < m.n_gangs; j++) m.out_placed[j] = 0;
+    if (m.gang_offset) cut_gangs(m, out_status, todo, sub, sub_group, sub_off, sub_gang, sub_min);
     CompiledNodeRules cr;
-    if (nodes) { // compiled before anything is bound, so a bad rule fails the whole call
-        rc = compile_node_rules(c, n_groups, nr, &cr);
+    if (m.mode >= RM_NODES) { // compiled before anything is bound, so a bad rule fails the whole call
+        rc = compile_node_rules(c, n_groups, m.nr, &cr);
         if (rc) return rc;
     }
     if (todo.empty()) return KS_OK;
     CompiledResources res;
-    if (fit) { // before the device, so a bad quantity fails the whole call
+    if (m.mode >= RM_FIT) { // before the device, so a bad quantity fails the whole call
         rc = compile_resources(c, sub.data(), sub.size(), &res);
         if (rc) return rc;
     }
@@ -2190,15 +2245,10 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     sp.max_skew = max_skew;
     sp.min_domains = min_domains;
     sp.existing = existing_offset ? existing.data() : nullptr;
-    std::vector<int32_t> idx(sub.size(), -1);
-    // refusal words per pod: [resources,] [taint, node affinity,] spread, then affinity
-    const size_t R = fit ? 5 : nodes ? 4 : aff ? 2 : 1;
-    std::vector<uint32_t> refused(sub.size() * R, 0);
-    std::vector<uint32_t> placed(sub_gang.size());
+    ks_pod_affinity pa{};
+    std::vector<int32_t> eg, en; // the existing pods whose node is in the store
     if (aff) {
-        ks_pod_affinity pa{aff->n_terms, aff->owner, aff->kind, aff->key, aff->target_offset, aff->target, 0, nullptr,
-                           nullptr};
-        std::vector<int32_t> eg, en; // the existing pods whose node is in the store
+        pa = {aff->n_terms, aff->owner, aff->kind, aff->key, aff->target_offset, aff->target, 0, nullptr, nullptr};
         for (uint64_t e = 0; e < aff->n_existing; e++) {
             const int32_t at = aff->existing_node_name[e] ? node_index_of(c, aff->existing_node_name[e]) : -1;
             if (at < 0) continue;
@@ -2208,50 +2258,40 @@ static int reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
         pa.n_existing = eg.size();
         pa.existing_group = eg.data();
         pa.existing_node = en.data();
-        const ks_bind_resources br{(uint32_t)res.ids.size(), res.node_free.data(), res.pod_req.data()};
-        const ks_gangs kg{sub_gang.size(), sub_off.data(), sub_min.data()};
-        rc = gang_offset ? ks_gang_fit_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, &cr.r, &br, &kg,
-                                            policy, idx.data(), nullptr, nullptr, refused.data(), nullptr, nullptr,
-                                            nullptr, placed.data())
-             : fit   ? ks_fit_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, &cr.r, &br, policy,
-                                   idx.data(), nullptr, nullptr, refused.data(), nullptr, nullptr, nullptr)
-             : nodes ? ks_node_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, &cr.r, policy, idx.data(),
-                                  nullptr, nullptr, refused.data(), nullptr, nullptr)
-             : sc ? ks_profile_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, sc, policy, idx.data(), nullptr,
-                                  nullptr, refused.data(), nullptr, nullptr)
-                : ks_affinity_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, &pa, policy, idx.data(), nullptr,
-                                   refused.data(), nullptr);
-    } else {
-        rc = ks_spread_bind(c->snap, &kp, sub_group.data(), n_groups, &sp, policy, idx.data(), nullptr, refused.data(),
-                            nullptr); // commits capacity on the device
     }
+    const RefusalWords& L = REFUSAL_WORDS[m.mode];
+    std::vector<int32_t> idx(sub.size(), -1);
+    std::vector<uint32_t> refused(sub.size() * L.n, 0);
+    std::vector<uint32_t> placed(sub_gang.size());
+    const ks_bind_resources br{(uint32_t)res.ids.size(), res.node_free.data(), res.pod_req.data()};
+    const ks_gangs kg{sub_gang.size(), sub_off.data(), sub_min.data()};
+    rc = bind_device(c, m.mode, &kp, sub_group.data(), n_groups, &sp, &pa, m.sc, &cr.r, &br, &kg, policy, idx.data(),
+                     refused.data(), placed.data());
     if (rc) {
         c->dirty = true; // the host list is the truth
         return rc;
     }
     StringList bodies{json, cap};
-    // the node-rule words follow the resource word, the spread and affinity words follow the two node-rule words
-    const size_t X = fit ? 1 : 0, F = nodes ? X + 2 : 0;
     std::vector<uint8_t> rolled(todo.size(), 0); // the pods of the sub-gangs that rolled back
     for (size_t k = 0; k < sub_gang.size(); k++) {
-        if (out_placed) out_placed[sub_gang[k]] = placed[k];
+        if (m.out_placed) m.out_placed[sub_gang[k]] = placed[k];
         if (placed[k] < sub_min[k]) std::fill(rolled.begin() + sub_off[k], rolled.begin() + sub_off[k + 1], 1);
     }
     for (size_t k = 0; k < todo.size(); k++) {
         const uint64_t i = todo[k];
-        const uint32_t* w = &refused[k * R];
+        const uint32_t* w = &refused[k * L.n];
         if (rolled[k])
             out_status[i] = KSH_RECONCILE_GANG_UNSATISFIED;
         else if (idx[k] >= 0)
             commit_bind(c, &pods[i], idx[k], kp.req_cpu[k], kp.req_mem[k], &out_status[i], &out_node_idx[i], bodies,
                         json && out_json_off ? &out_json_off[i] : nullptr);
-        else if (fit && w[0] > 0 && w[1] + w[2] + w[3] + w[4] == 0)
+        else if (L.res >= 0 && w[L.res] > 0 && w[L.taint] + w[L.taint + 1] + w[L.spread] + w[L.aff] == 0)
             out_status[i] = KSH_RECONCILE_INSUFFICIENT_RESOURCES;
-        else if (nodes && w[X] + w[X + 1] > 0 && w[X + 2] == 0 && w[X + 3] == 0)
+        else if (L.taint >= 0 && w[L.taint] + w[L.taint + 1] > 0 && w[L.spread] == 0 && w[L.aff] == 0)
             out_status[i] = KSH_RECONCILE_NODE_RULES_UNSATISFIED;
-        else if (refused[k * R + F] > 0)
+        else if (w[L.spread] > 0)
             out_status[i] = KSH_RECONCILE_SPREAD_UNSATISFIED;
-        else if (aff && refused[k * R + F + 1] > 0)
+        else if (L.aff >= 0 && w[L.aff] > 0)
             out_status[i] = KSH_RECONCILE_AFFINITY_UNSATISFIED;
     }
     return KS_OK;
@@ -2263,7 +2303,8 @@ int ksh_reconcile_spread(ksh_context* c, const ks_pod_obj* pods, uint64_t n, con
                          const uint64_t* existing_offset, int policy, int32_t* out_status, int32_t* out_node_idx,
                          char* json, size_t cap, int64_t* out_json_off) try {
     return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
-                            existing_offset, nullptr, policy, out_status, out_node_idx, json, cap, out_json_off);
+                            existing_offset, nullptr, policy, out_status, out_node_idx, json, cap, out_json_off,
+                            {RM_SPREAD});
 }
 KSH_CATCH
 
@@ -2275,7 +2316,7 @@ int ksh_reconcile_affinity(ksh_context* c, const ks_pod_obj* pods, uint64_t n, c
     const ksh_pod_affinity none{};
     return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
                             existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
-                            out_json_off);
+                            out_json_off, {RM_AFFINITY});
 }
 KSH_CATCH
 
@@ -2289,7 +2330,7 @@ int ksh_reconcile_profile(ksh_context* c, const ks_pod_obj* pods, uint64_t n, co
     const ksh_pod_affinity none{};
     return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
                             existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
-                            out_json_off, scoring);
+                            out_json_off, {RM_PROFILE, scoring});
 }
 KSH_CATCH
 
@@ -2371,7 +2412,7 @@ int ksh_reconcile_nodes(ksh_context* c, const ks_pod_obj* pods, uint64_t n, cons
     const ksh_pod_affinity none{};
     return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
                             existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
-                            out_json_off, scoring, rules, true);
+                            out_json_off, {RM_NODES, scoring, rules});
 }
 KSH_CATCH
 
@@ -2402,7 +2443,7 @@ int ksh_reconcile_fit(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const 
     const ksh_pod_affinity none{};
     return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
                             existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
-                            out_json_off, scoring, rules, true, true);
+                            out_json_off, {RM_FIT, scoring, rules});
 }
 KSH_CATCH
 
@@ -2418,7 +2459,7 @@ int ksh_reconcile_fit_gangs(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     const ksh_pod_affinity none{};
     return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
                             existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
-                            out_json_off, scoring, rules, true, true, gang_offset, n_gangs, min_member, out_placed);
+                            out_json_off, {RM_FIT_GANGS, scoring, rules, gang_offset, n_gangs, min_member, out_placed});
 }
 KSH_CATCH
 

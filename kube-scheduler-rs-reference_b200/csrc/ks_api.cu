@@ -117,7 +117,8 @@ static int check_commit_requests(uint64_t n, const int64_t* req_cpu, const int64
 }
 
 // ---- host-staged calls: ks_stream_bind's device loop, ks_gang_bind, ks_drain_check, ks_scaleup_estimate,
-// ks_place_replicas, ks_place_replicas_spread (and _multi), ks_spread_bind and ks_affinity_bind ----
+// ks_place_replicas, ks_place_replicas_spread (and _multi), and the bind walk's ks_spread_bind, ks_affinity_bind,
+// ks_profile_bind, ks_node_bind, ks_fit_bind and ks_gang_fit_bind ----
 // Such a call gathers its host inputs into the snapshot's pinned block, makes one H2D copy to d_in, launches, makes one
 // D2H copy from d_out and copies its results out before it returns.  Its HostStaged plan declares every array it stages
 // once, with its type and count: in() an input, gathered from src or, with src NULL, filled by the caller through
@@ -140,14 +141,17 @@ class HostStaged {
     Staged<T> work(uint64_t n, size_t align = alignof(T)) { return add<T>(WORK, nullptr, n, align); }
     // With the snapshot locked and every array declared: ensures h_stage, d_in, d_out and d_work once, for the whole plan
     // and at least min_in / min_out bytes of inputs / results, then gathers the inputs that have a source.  A growing
-    // ensure frees what the buffer held, so no pointer is handed out before this.
-    cudaError_t reserve(ks_snapshot* s, size_t min_in = 0, size_t min_out = 0) {
+    // ensure frees what the buffer held, so no pointer is handed out before this.  KS_OK or a KS_ERR_* with its message.
+    int reserve(ks_snapshot* s, size_t min_in = 0, size_t min_out = 0) {
+        if (overflow_)
+            return fail(KS_ERR_RANGE, "a staging plan of more than %d gathered and scattered arrays", MAX_COPIES);
         const size_t in = std::max(layout_[IN].size, min_in), out = std::max(layout_[OUT].size, min_out);
         cudaError_t e = s->h_stage.ensure((in + 15) / 16 * 16 + out);
         if (e == cudaSuccess) e = s->d_in.ensure(in);
         if (e == cudaSuccess) e = s->d_out.ensure(out);
         if (e == cudaSuccess) e = s->d_work.ensure(layout_[WORK].size);
-        if (e != cudaSuccess) return e;
+        if (e != cudaSuccess)
+            return fail(KS_ERR_CUDA, "h.reserve(s) failed: %s (%s:%d)", cudaGetErrorString(e), __FILE__, __LINE__);
         dev_[IN] = s->d_in.p;
         dev_[OUT] = s->d_out.p;
         dev_[WORK] = s->d_work.p;
@@ -184,8 +188,8 @@ class HostStaged {
     Staged<T> add(int block, T* p, uint64_t n, size_t align) {
         const size_t off = layout_[block].take<T>(n, align);
         if (p && n) {
-            assert(n_copies_ < MAX_COPIES);
-            copies_[n_copies_++] = Copy{block, off, p, n * sizeof(T)};
+            if (n_copies_ < MAX_COPIES) copies_[n_copies_++] = Copy{block, off, p, n * sizeof(T)};
+            else overflow_ = true; // reported by reserve(), before any device work
         }
         return Staged<T>{block, off, n};
     }
@@ -196,12 +200,14 @@ class HostStaged {
             if (c.block == OUT && block == OUT) memcpy(c.p, at<unsigned char>(host_[OUT], c.off), c.bytes);
         }
     }
-    static constexpr int MAX_COPIES = 24;
+    // The largest plan: ks_gang_fit_bind with every optional array given, 32 inputs and 8 results (bind_spread)
+    static constexpr int MAX_COPIES = 40;
     BlockLayout layout_[3];
     void* dev_[3] = {};
     void* host_[2] = {};
     Copy copies_[MAX_COPIES];
     int n_copies_ = 0;
+    bool overflow_ = false;
     bool reserved_ = false;
 };
 
@@ -1170,7 +1176,9 @@ int ks_stream_bind(ks_snapshot* s, const ks_pods* pods, int policy, int32_t* out
         const auto ctl = h.out<uint32_t>(nullptr, 2);
         const StreamBatchScratch w = stream_batch_scratch(h, s->sms);
         // sized for STREAM_BATCH_MAX pods on first use, so a stream of growing micro-batches never reallocates
-        CU_TRY(h.reserve(s, (size_t)STREAM_BATCH_MAX * (16 + 8 * KS_MAX_LABEL_WORDS), (size_t)STREAM_BATCH_MAX * 12 + 8));
+        if (const int rc = h.reserve(s, (size_t)STREAM_BATCH_MAX * (16 + 8 * KS_MAX_LABEL_WORDS),
+                                     (size_t)STREAM_BATCH_MAX * 12 + 8))
+            return rc;
         cudaStream_t st = s->stream;
         CU_TRY(h.upload(st));
         StreamBatchArgs a = stream_batch_args(s, policy, h, w);
@@ -1291,7 +1299,7 @@ int ks_gang_bind(ks_snapshot* s, const ks_pods* pods, const ks_gangs* gangs, int
     const auto ctl = h.out<uint32_t>(nullptr, 2 * G);
     const auto placed = h.out(out_placed, G);
     const StreamBatchScratch w = stream_batch_scratch(h, s->sms);
-    CU_TRY(h.reserve(s));
+    if (const int rc = h.reserve(s)) return rc;
     for (uint64_t g = 0; g <= G; g++) h.host(offset)[g] = (uint32_t)off[g];
     cudaStream_t st = s->stream;
     CU_TRY(h.upload(st));
@@ -1385,7 +1393,7 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidate
     const auto ov_fc = h.work<int64_t>(P), ov_fm = h.work<int64_t>(P), part_key = h.work<int64_t>(part_rows);
     const auto ov_node = h.work<int32_t>(P), part_idx = h.work<int32_t>(part_rows);
     const auto ov_cnt = h.work<uint32_t>(2 * D); // ov_cnt D, failed D: one array, zeroed together
-    CU_TRY(h.reserve(s));
+    if (const int rc = h.reserve(s)) return rc;
     int64_t *h_rc = h.host(cpu), *h_rm = h.host(mem);
     uint64_t* h_sel = h.host(sel);
     int32_t* h_node = h.host(cand_node);
@@ -1486,7 +1494,7 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const ks_node_templ
     const auto node = h.out(out_node, out_node ? T * P : 0);
     const uint32_t slots = scaleup_slots((uint32_t)T, s->sms);
     const auto scratch = h.work<uint32_t>((uint64_t)slots * 2 * P);
-    CU_TRY(h.reserve(s));
+    if (const int rc = h.reserve(s)) return rc;
     cudaStream_t st = s->stream;
     CU_TRY(h.upload(st));
     if (out_node) CU_TRY(cudaMemsetAsync(h.dev(node), 0xff, T * P * 4, st));
@@ -1587,7 +1595,7 @@ int ks_place_replicas(ks_snapshot* s, const ks_pods* specs, const uint32_t* repl
     // KS_SCORE_LEAST_BALANCED: [scores | copies placed] per node and k_rep_seq CTA
     const auto seq_score = h.work<int64_t>((uint64_t)seq_ctas * s->N);
     const auto seq_placed = h.work<uint32_t>((uint64_t)seq_ctas * s->N);
-    CU_TRY(h.reserve(s));
+    if (const int rc = h.reserve(s)) return rc;
     for (uint64_t t = 0, o = 0; t < T; o += replicas[t], t++) h.host(offset)[t] = o;
     cudaStream_t st = s->stream;
     CU_TRY(h.upload(st));
@@ -1721,7 +1729,7 @@ static int place_spread(ks_snapshot* s, const char* call, const ks_pods* specs, 
         dstart[i] = h.work<uint32_t>((uint64_t)Dk[i] + 1);
     }
     const auto seq = h.work<unsigned char>(seq_bytes, 16); // k_spread_seq's scratch
-    CU_TRY(h.reserve(s));
+    if (const int rc = h.reserve(s)) return rc;
     for (uint64_t t = 0, o = 0; t < T; o += replicas[t], t++) h.host(offset)[t] = o;
     cudaStream_t st = s->stream;
     CU_TRY(h.upload(st));
@@ -2094,50 +2102,98 @@ static int compile_node_rules(const ks_node_rules* r, uint32_t G, uint32_t N, No
     return KS_OK;
 }
 
+// ks_fit_bind's scalar resources (5r): at most KS_BIND_MAX_RESOURCES rows, every request at least 0
+static int check_bind_resources(const ks_bind_resources* res, uint64_t P, uint32_t N) {
+    const uint64_t RS = res->n_res;
+    if (RS > KS_BIND_MAX_RESOURCES)
+        return fail(KS_ERR_RANGE, "%llu resources (at most %u)", (unsigned long long)RS, KS_BIND_MAX_RESOURCES);
+    if (RS && ((N && !res->node_free) || (P && !res->pod_req))) return fail(KS_ERR_INVALID, "NULL node_free or pod_req");
+    for (uint64_t i = 0; i < P * RS; i++)
+        if (res->pod_req[i] < 0)
+            return fail(KS_ERR_RANGE, "pod %llu: request %lld of resource %llu (at least 0)", (unsigned long long)(i / RS),
+                        (long long)res->pod_req[i], (unsigned long long)(i % RS));
+    return KS_OK;
+}
+
 // last_path and the name in launch errors of each BindMode
 static const char* const BIND_PATH[] = {"spread_bind", "affinity_bind", "profile_bind", "node_bind", "fit_bind",
                                         "gang_fit_bind"};
 static const char* const BIND_NAME[] = {"spread bind", "affinity bind", "profile bind", "node bind", "fit bind",
                                         "gang fit bind"};
 
-// ks_spread_bind, and with aff set ks_affinity_bind (then max_skew may be NULL), and with aff and sc set ks_profile_bind
-// (out_parts and out_soft_count [G * S] may be given), and with nr set as well ks_node_bind, and with res set as well
-// ks_fit_bind (out_free [R * N] may be given), and with gangs set as well ks_gang_fit_bind (out_placed [gangs->n] may
-// be given); out_refused and out_parts hold the mode's words per pod (bind_refusal_words, bind_part_words)
-static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
-                       const ks_spread_multi* spread, const ks_pod_affinity* aff, int policy, int32_t* out_node_idx,
-                       int64_t* out_score, uint32_t* out_refused, uint32_t* out_domain_count,
-                       const ks_bind_scoring* sc = nullptr, int64_t* out_parts = nullptr,
-                       uint32_t* out_soft_count = nullptr, const ks_node_rules* nr = nullptr,
-                       const ks_bind_resources* res = nullptr, int64_t* out_free = nullptr,
-                       const ks_gangs* gangs = nullptr, uint32_t* out_placed = nullptr) {
-    int rc = check_pods(s, pods);
+// One call of the bind walk, as its public entry (include/ksched.h) passes it.  Each mode reads what the mode before it
+// reads and adds one part: AFFINITY aff (topo->max_skew may then be NULL), PROFILE scoring, NODE rules, FIT res and
+// GANG_FIT gangs.  bind_spread reads a NULL aff, rules or res of the mode as empty; scoring and gangs are required.
+struct BindOutputs {
+    int32_t* node_idx = nullptr;      // [P], required
+    int64_t* score = nullptr;         // [P]
+    uint32_t* refused = nullptr;      // [P * bind_refusal_words(mode)]
+    uint32_t* domain_count = nullptr; // [G * S]
+    int64_t* parts = nullptr;         // [P * bind_part_words(mode)]
+    uint32_t* soft_count = nullptr;   // [G * S]
+    int64_t* free_r = nullptr;        // [R * N]
+    uint32_t* placed = nullptr;       // [gangs->n]
+};
+struct BindRequest {
+    const char* call = nullptr; // the public entry, in error messages
+    BindMode mode = BIND_SPREAD;
+    const ks_pods* pods = nullptr;
+    const int32_t* group = nullptr;
+    uint32_t n_groups = 0;
+    const ks_spread_multi* topo = nullptr;
+    int policy = 0;
+    BindOutputs out{};
+    const ks_pod_affinity* aff = nullptr;
+    const ks_bind_scoring* scoring = nullptr;
+    const ks_node_rules* rules = nullptr;
+    const ks_bind_resources* res = nullptr;
+    const ks_gangs* gangs = nullptr;
+};
+
+// What plan_bind derives from a request: the counts per group S, the walk's CTAs, first[g] = the first pod of group g or
+// -1, the compiled terms and rules; and, filled by bind_spread once a walk runs, with scoring the domain bitmaps of the keys with more than one node in some
+// domain (bit k of uniq: key k has none; bwo[k]: key k's word offset in each parity, BW words per parity).
+struct BindPlan {
+    uint64_t S = 0;
+    uint32_t grid = 0;
+    std::vector<int64_t> first;
+    AffinityPlan aff;
+    NodeRulesPlan rules;
+    uint32_t uniq = 0, bwo[KS_SPREAD_MAX_KEYS] = {}, BW = 0;
+};
+
+// Every check of a bind call, in the order callers see them, then its plan; nothing has changed when it fails
+static int plan_bind(const ks_snapshot* s, const BindRequest& r, BindPlan* pl) {
+    const char* call = r.call;
+    const ks_bind_scoring* sc = r.scoring;
+    int rc = check_pods(s, r.pods);
     if (rc) return rc;
-    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "%s takes host-space pods", call);
-    if (!policy_valid(policy)) return fail(KS_ERR_INVALID, "bad policy");
+    if (r.pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "%s takes host-space pods", call);
+    if (!policy_valid(r.policy)) return fail(KS_ERR_INVALID, "bad policy");
     if (sc) {
-        if (policy != KS_SCORE_LEAST_ALLOCATED && policy != KS_SCORE_MOST_ALLOCATED && policy != KS_SCORE_LEAST_BALANCED)
-            return fail(KS_ERR_INVALID, "%s takes policies 1, 3 and 4 (got %d)", call, policy);
+        if (r.policy != KS_SCORE_LEAST_ALLOCATED && r.policy != KS_SCORE_MOST_ALLOCATED &&
+            r.policy != KS_SCORE_LEAST_BALANCED)
+            return fail(KS_ERR_INVALID, "%s takes policies 1, 3 and 4 (got %d)", call, r.policy);
         if (sc->hard_affinity_weight > 100 || sc->weight_spread > 100 || sc->weight_affinity > 100)
             return fail(KS_ERR_INVALID, "plugin weights %u, %u and hard affinity weight %u (at most 100)",
                         sc->weight_spread, sc->weight_affinity, sc->hard_affinity_weight);
         if (sc->soft_all_keys)
-            for (uint32_t g = 0; g < n_groups; g++)
+            for (uint32_t g = 0; g < r.n_groups; g++)
                 if (sc->soft_all_keys[g] > 1)
                     return fail(KS_ERR_INVALID, "group %u: soft_all_keys %u (0 or 1)", g, sc->soft_all_keys[g]);
     }
-    const uint64_t P = pods->n, G = n_groups;
-    if (P && (!group || !out_node_idx)) return fail(KS_ERR_INVALID, "NULL group or out_node_idx");
-    if (!spread || (G && !spread->max_skew && !aff)) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
+    const ks_spread_multi* spread = r.topo;
+    const uint64_t P = r.pods->n, G = r.n_groups;
+    if (P && (!r.group || !r.out.node_idx)) return fail(KS_ERR_INVALID, "NULL group or out_node_idx");
+    if (!spread || (G && !spread->max_skew && !r.aff)) return fail(KS_ERR_INVALID, "NULL spread, node_domain or max_skew");
     if (P > KS_SPREAD_BIND_MAX_PODS)
         return fail(KS_ERR_RANGE, "%llu pods (at most %u)", (unsigned long long)P, KS_SPREAD_BIND_MAX_PODS);
     if (G > KS_SPREAD_BIND_MAX_GROUPS)
         return fail(KS_ERR_RANGE, "%llu groups (at most %u)", (unsigned long long)G, KS_SPREAD_BIND_MAX_GROUPS);
-    uint64_t S;
-    rc = check_spread_keys(s, spread, &S);
+    rc = check_spread_keys(s, spread, &pl->S);
     if (rc) return rc;
     const uint32_t K = spread->n_keys, W = s->W, N = s->N;
-    const uint64_t GS = G * S;
+    const uint64_t S = pl->S, GS = G * S;
     if (GS > KS_SPREAD_MAX_COUNTS)
         return fail(KS_ERR_RANGE, "%llu groups x %llu domains of counts (at most 2^26)", (unsigned long long)G,
                     (unsigned long long)S);
@@ -2146,224 +2202,300 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
             if (spread->existing[i] > KS_SPREAD_MAX_EXISTING)
                 return fail(KS_ERR_RANGE, "group %llu, count %llu: %u existing pods (at most 2^24)",
                             (unsigned long long)(i / S), (unsigned long long)(i % S), spread->existing[i]);
-    // every pod of a group carries the group's selector: first[g] = the first pod of group g, or -1
-    std::vector<int64_t> first;
+    // every pod of a group carries the group's selector
+    std::vector<int64_t>& first = pl->first;
     try {
         first.assign(G, -1);
     } catch (...) {
         return fail(KS_ERR_NOMEM, "out of host memory in %s", call);
     }
     for (uint64_t p = 0; p < P; p++) {
-        const int32_t g = group[p];
+        const int32_t g = r.group[p];
         if (g < -1 || g >= (int64_t)G)
-            return fail(KS_ERR_INVALID, "pod %llu: group %d outside [-1, %u)", (unsigned long long)p, g, n_groups);
+            return fail(KS_ERR_INVALID, "pod %llu: group %d outside [-1, %u)", (unsigned long long)p, g, r.n_groups);
         if (g < 0) continue;
         if (first[g] < 0) first[g] = (int64_t)p;
-        else if (memcmp(pods->sel + p * W, pods->sel + first[g] * W, W * 8) != 0)
+        else if (memcmp(r.pods->sel + p * W, r.pods->sel + first[g] * W, W * 8) != 0)
             return fail(KS_ERR_INVALID, "pod %llu: selector differs from pod %lld of group %d", (unsigned long long)p,
                         (long long)first[g], g);
     }
-    rc = check_commit_requests(P, pods->req_cpu, pods->req_mem);
+    rc = check_commit_requests(P, r.pods->req_cpu, r.pods->req_mem);
+    if (!rc && r.res) rc = check_bind_resources(r.res, P, N);
+    if (!rc && r.gangs && (!r.gangs->offset || (r.gangs->n && !r.gangs->min_member)))
+        return fail(KS_ERR_INVALID, "NULL gang array");
+    if (!rc && r.gangs) rc = check_gangs(r.gangs, P, KS_SPREAD_BIND_MAX_PODS); // a gang as large as the queue may be
+    try {
+        if (!rc && r.aff) rc = compile_affinity(r.aff, (uint32_t)G, K, spread->n_domains, N, &pl->aff, sc);
+        if (!rc && r.rules) rc = compile_node_rules(r.rules, (uint32_t)G, N, &pl->rules);
+    } catch (...) {
+        return fail(KS_ERR_NOMEM, "out of host memory in %s", call);
+    }
+    pl->grid = std::max(1u, std::min<uint32_t>((uint32_t)s->sms, (N + 127u) / 128u));
+    return rc;
+}
+
+// The staging of a bind call (ProfileBindArgs, ks_launch.h).  Building it declares every array on h in member order,
+// feature by feature, with no element for a feature the mode does not read; after HostStaged::reserve(), place() fills
+// the arrays converted or defaulted in place and points the kernel's fields at the staged arrays, in the same order.
+// The compiled plans and the caller's host arrays are gathered from where they are.
+struct BindStage {
+    HostStaged& h;
+    const ks_snapshot* s;
+    const BindRequest& r;
+    const BindPlan& pl;
+    const uint64_t P = r.pods->n, G = r.n_groups, K = r.topo->n_keys, GS = G * pl.S, N = s->N, W = s->W;
+    const uint64_t E = r.aff ? r.aff->n_existing : 0, Q = r.scoring ? 1 : 0, NR = r.rules ? 1 : 0;
+    const uint64_t RS = r.res ? r.res->n_res : 0, NG = r.gangs ? r.gangs->n + 1 : 0, CTA = pl.grid;
+    // every mode: the queue, the topology and the outputs
+    Staged<int64_t> cpu = h.in(r.pods->req_cpu, P), mem = h.in(r.pods->req_mem, P);
+    Staged<uint64_t> sel = h.in(r.pods->sel, P * W);
+    Staged<int32_t> grp = h.in(r.group, P);
+    Staged<uint32_t> max_skew = h.in(r.topo->max_skew, G * K);
+    Staged<uint32_t> min_domains = h.in(r.topo->min_domains, r.topo->min_domains ? G * K : 0);
+    Staged<uint32_t> existing = h.in(r.topo->existing, r.topo->existing ? GS : 0);
+    Staged<int32_t> dom = h.in<int32_t>(nullptr, K * N);
+    Staged<uint64_t> gsel = h.in<uint64_t>(nullptr, G * W);
+    Staged<int64_t> score = h.out(r.out.score, P);
+    Staged<int32_t> idx = h.out(r.out.node_idx, P);
+    Staged<uint32_t> refused = h.out(r.out.refused, P * bind_refusal_words(r.mode));
+    Staged<uint32_t> count = h.out(r.out.domain_count, GS); // the counts themselves: device state of the whole call
+    Staged<uint8_t> elig = h.work<uint8_t>(GS);
+    Staged<uint32_t> gk = h.work<uint32_t>(G * K * 4, 16);
+    Staged<int64_t> pkey = h.work<int64_t>(CTA);
+    Staged<int32_t> pidx = h.work<int32_t>(CTA);
+    Staged<uint32_t> pref = h.work<uint32_t>(CTA);
+    // AFFINITY on: the compiled terms, the existing pods and the counters
+    Staged<uint32_t> abase = h.in(pl.aff.abase.data(), pl.aff.abase.size());
+    Staged<uint32_t> aflag = h.in(pl.aff.aflag.data(), pl.aff.aflag.size());
+    Staged<uint32_t> upd_off = h.in(pl.aff.upd_off.data(), pl.aff.upd_off.size());
+    Staged<uint32_t> upd = h.in(pl.aff.upd.data(), pl.aff.upd.size());
+    Staged<int32_t> ex_group = h.in(r.aff ? r.aff->existing_group : nullptr, E);
+    Staged<int32_t> ex_node = h.in(r.aff ? r.aff->existing_node : nullptr, E);
+    Staged<uint32_t> acnt = h.work<uint32_t>(pl.aff.words, 16);
+    Staged<uint32_t> paref = h.work<uint32_t>(r.aff ? CTA : 0);
+    // PROFILE on: the soft terms, the log table, the compiled IPA entries, the IPA counters and the domain bitmaps
+    Staged<uint32_t> soft_skew = h.in(r.scoring ? r.scoring->soft_skew : nullptr, Q * G * K);
+    Staged<uint8_t> soft_all = h.in(r.scoring ? r.scoring->soft_all_keys : nullptr, Q * G);
+    Staged<double> logw = h.in<double>(nullptr, Q * (N + 2));
+    Staged<uint32_t> ibase = h.in(pl.aff.ibase.data(), pl.aff.ibase.size());
+    Staged<uint32_t> iupd_off = h.in(pl.aff.iupd_off.data(), pl.aff.iupd_off.size());
+    Staged<uint32_t> iupd = h.in(pl.aff.iupd.data(), pl.aff.iupd.size());
+    Staged<int32_t> icoef = h.in(pl.aff.icoef.data(), pl.aff.icoef.size());
+    Staged<int64_t> parts = h.out(r.out.parts, Q * P * bind_part_words(r.mode));
+    Staged<uint32_t> scnt = h.out(r.out.soft_count, Q * GS);
+    Staged<int64_t> icnt = h.work<int64_t>(pl.aff.iwords, 16);
+    Staged<uint32_t> bits = h.work<uint32_t>(2ull * pl.BW, 16);
+    Staged<int64_t> iraw = h.work<int64_t>(Q * N), praw = h.work<int64_t>(Q * N);
+    Staged<uint32_t> pdom = h.work<uint32_t>(Q * CTA * KS_SPREAD_MAX_KEYS), plack = h.work<uint32_t>(Q * CTA);
+    Staged<int64_t> pimin = h.work<int64_t>(Q * CTA), pimax = h.work<int64_t>(Q * CTA);
+    Staged<int64_t> ppmin = h.work<int64_t>(Q * CTA), ppmax = h.work<int64_t>(Q * CTA);
+    // NODE on: the compiled classes, the rule keys' domains, the taints and the sets; one rule word per (class, node)
+    Staged<uint32_t> ncls = h.in(pl.rules.cls.data(), pl.rules.cls.size());
+    Staged<uint64_t> ctol = h.in(pl.rules.ctol.data(), pl.rules.ctol.size());
+    Staged<uint32_t> cterm_off = h.in(pl.rules.cterm_off.data(), NR * pl.rules.cterm_off.size());
+    Staged<uint32_t> cterm_w = h.in(pl.rules.cterm_w.data(), pl.rules.cterm_w.size());
+    Staged<uint32_t> cexpr_off = h.in(pl.rules.cexpr_off.data(), NR * pl.rules.cexpr_off.size());
+    Staged<uint32_t> cexpr_key = h.in(pl.rules.cexpr_key.data(), pl.rules.cexpr_key.size());
+    Staged<uint64_t> cexpr_set = h.in(pl.rules.cexpr_set.data(), pl.rules.cexpr_set.size());
+    Staged<uint64_t> nset = h.in(r.rules ? r.rules->expr_set : nullptr, pl.rules.set_words);
+    Staged<int32_t> ndom = h.in<int32_t>(nullptr, (r.rules ? r.rules->n_keys : 0) * N);
+    Staged<uint64_t> taint_hard = h.in(r.rules ? r.rules->node_taint_hard : nullptr, NR * N);
+    Staged<uint64_t> taint_soft = h.in(r.rules ? r.rules->node_taint_soft : nullptr, NR * N);
+    Staged<uint32_t> nrules = h.work<uint32_t>(pl.rules.C * N);
+    Staged<uint32_t> ptref = h.work<uint32_t>(NR * CTA), pnref = h.work<uint32_t>(NR * CTA);
+    Staged<uint32_t> ptmax = h.work<uint32_t>(NR * CTA), pnmax = h.work<uint32_t>(NR * CTA);
+    // FIT on: the requests, the caller's free amounts and the charged ones, one row per resource
+    Staged<int64_t> res_req = h.in(RS ? r.res->pod_req : nullptr, P * RS);
+    Staged<int64_t> res_node_free = h.in(RS ? r.res->node_free : nullptr, RS * N);
+    Staged<int64_t> res_free = h.out(r.out.free_r, RS * N);
+    Staged<uint32_t> pfref = h.work<uint32_t>(r.res ? CTA : 0);
+    // GANG_FIT: the gangs' offsets (NG of them) and minimums, their counts, and the rollback's group marks and lists
+    Staged<uint32_t> goff = h.in<uint32_t>(nullptr, NG);
+    Staged<uint32_t> gmin = h.in(r.gangs ? r.gangs->min_member : nullptr, r.gangs ? r.gangs->n : 0);
+    Staged<uint32_t> gplaced = h.out(r.out.placed, r.gangs ? r.gangs->n : 0);
+    Staged<uint32_t> gmark = h.work<uint32_t>(r.gangs ? 2 * G : 0), glist = h.work<uint32_t>(r.gangs ? 2 * G : 0);
+
+    void place(ProfileBindArgs& q) const {
+        const ks_spread_multi* t = r.topo;
+        SpreadBindArgs& a = q.b;
+        for (uint32_t k = 0; k < K; k++) memcpy(h.host(dom) + (size_t)k * N, t->node_domain[k], (size_t)N * 4);
+        if (!t->max_skew) memset(h.host(max_skew), 0, G * K * 4); // AFFINITY on: zeros
+        for (uint64_t g = 0; g < G; g++) {
+            uint64_t* row = h.host(gsel) + g * W;
+            if (pl.first[g] >= 0) memcpy(row, r.pods->sel + pl.first[g] * W, W * 8);
+            else memset(row, 0, W * 8);
+        }
+        a.req_cpu = h.dev(cpu);
+        a.req_mem = h.dev(mem);
+        a.sel = h.dev(sel);
+        a.group = h.dev(grp);
+        a.gsel = h.dev(gsel);
+        a.dom = h.dev(dom);
+        a.max_skew = h.dev(max_skew);
+        a.min_domains = t->min_domains ? h.dev(min_domains) : nullptr;
+        a.existing = t->existing ? h.dev(existing) : nullptr;
+        a.elig = h.dev(elig);
+        a.gk = h.dev(gk);
+        a.cnt = h.dev(count);
+        a.pkey = h.dev(pkey);
+        a.pidx = h.dev(pidx);
+        a.pref = h.dev(pref);
+        a.out_idx = h.dev(idx);
+        a.out_score = h.dev(score);
+        a.out_refused = h.dev(refused);
+        if (r.aff) {
+            a.abase = h.dev(abase);
+            a.aflag = h.dev(aflag);
+            a.upd_off = h.dev(upd_off);
+            a.upd = h.dev(upd);
+            a.ex_group = h.dev(ex_group);
+            a.ex_node = h.dev(ex_node);
+            a.E = (uint32_t)E;
+            a.any_base = pl.aff.any_base;
+            a.aff_grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((a.E + 7) / 8, 4ull * (uint64_t)s->sms));
+            a.acnt = h.dev(acnt);
+            a.paref = h.dev(paref);
+        }
+        if (const ks_bind_scoring* sc = r.scoring) {
+            if (!sc->soft_skew) memset(h.host(soft_skew), 0, G * K * 4);
+            if (!sc->soft_all_keys) memset(h.host(soft_all), 1, G);
+            for (uint64_t i = 0; i < N + 2ull; i++) h.host(logw)[i] = log((double)(i + 2)); // the oracle's libm
+            q.soft_skew = h.dev(soft_skew);
+            q.soft_all = h.dev(soft_all);
+            q.logw = h.dev(logw);
+            q.uniq = pl.uniq;
+            std::copy(pl.bwo, pl.bwo + K, q.bwo);
+            q.BW = pl.BW;
+            q.bits = h.dev(bits);
+            q.scnt = h.dev(scnt);
+            q.ibase = h.dev(ibase);
+            q.iupd_off = h.dev(iupd_off);
+            q.iupd = h.dev(iupd);
+            q.icoef = h.dev(icoef);
+            q.icnt = h.dev(icnt);
+            q.iwords = pl.aff.iwords;
+            q.iraw = h.dev(iraw);
+            q.praw = h.dev(praw);
+            q.pdom = h.dev(pdom);
+            q.plack = h.dev(plack);
+            q.pimin = h.dev(pimin);
+            q.pimax = h.dev(pimax);
+            q.ppmin = h.dev(ppmin);
+            q.ppmax = h.dev(ppmax);
+            q.out_parts = h.dev(parts);
+            q.wspread = sc->weight_spread;
+            q.waff = sc->weight_affinity;
+        }
+        if (const ks_node_rules* nr = r.rules) {
+            const uint32_t KN = nr->n_keys;
+            for (uint32_t k = 0; k < KN; k++) memcpy(h.host(ndom) + (size_t)k * N, nr->node_domain[k], (size_t)N * 4);
+            if (!nr->node_taint_hard) memset(h.host(taint_hard), 0, (size_t)N * 8);
+            if (!nr->node_taint_soft) memset(h.host(taint_soft), 0, (size_t)N * 8);
+            q.ncls = h.dev(ncls);
+            q.nrules = h.dev(nrules);
+            q.C = pl.rules.C;
+            q.KN = KN;
+            for (uint32_t k = 0; k < KN; k++) q.NDk[k] = nr->n_domains[k];
+            q.ndom = h.dev(ndom);
+            q.taint_hard = h.dev(taint_hard);
+            q.taint_soft = h.dev(taint_soft);
+            q.ctol = h.dev(ctol);
+            q.cterm_off = h.dev(cterm_off);
+            q.cterm_w = h.dev(cterm_w);
+            q.cexpr_off = h.dev(cexpr_off);
+            q.cexpr_key = h.dev(cexpr_key);
+            q.cexpr_set = h.dev(cexpr_set);
+            q.nset = h.dev(nset);
+            q.ptref = h.dev(ptref);
+            q.pnref = h.dev(pnref);
+            q.ptmax = h.dev(ptmax);
+            q.pnmax = h.dev(pnmax);
+            q.wtaint = nr->weight_taint;
+            q.wnaff = nr->weight_node_affinity;
+            q.rules_grid = (uint32_t)std::max<uint64_t>(
+                1, std::min<uint64_t>(((uint64_t)q.C * N + 255) / 256, 4ull * (uint64_t)s->sms));
+        }
+        if (r.res) {
+            q.R = (uint32_t)RS;
+            q.res_req = h.dev(res_req);
+            q.res_node_free = h.dev(res_node_free);
+            q.res_free = h.dev(res_free);
+            q.pfref = h.dev(pfref);
+        }
+        if (const ks_gangs* gangs = r.gangs) {
+            for (uint64_t j = 0; j <= gangs->n; j++) h.host(goff)[j] = (uint32_t)gangs->offset[j]; // P < 2^32
+            q.n_gangs = (uint32_t)gangs->n;
+            q.goff = h.dev(goff);
+            q.gmin = h.dev(gmin);
+            q.gplaced = h.dev(gplaced);
+            q.gmark = h.dev(gmark);
+            q.glist = h.dev(glist);
+        }
+    }
+};
+
+// The six bind entries' one call: plan_bind, the staging, one H2D copy, launch_bind and one D2H copy
+static int bind_spread(ks_snapshot* s, const BindRequest& req) {
+    static const ks_pod_affinity no_aff{};
+    static const ks_node_rules no_rules{}; // no taint, no term, both plugin weights 0: the total is ks_profile_bind's
+    static const ks_bind_resources no_res{};
+    if (req.mode >= BIND_PROFILE && !req.scoring) return fail(KS_ERR_INVALID, "NULL scoring");
+    if (req.mode == BIND_GANG_FIT && !req.gangs) return fail(KS_ERR_INVALID, "NULL gangs");
+    BindRequest r = req;
+    if (r.mode >= BIND_AFFINITY && !r.aff) r.aff = &no_aff;
+    if (r.mode >= BIND_NODE && !r.rules) r.rules = &no_rules;
+    if (r.mode >= BIND_FIT && !r.res) r.res = &no_res;
+    BindPlan pl;
+    const int rc = plan_bind(s, r, &pl);
     if (rc) return rc;
-    const uint64_t RS = res ? res->n_res : 0; // ks_fit_bind's scalar resources
-    if (RS > KS_BIND_MAX_RESOURCES)
-        return fail(KS_ERR_RANGE, "%llu resources (at most %u)", (unsigned long long)RS, KS_BIND_MAX_RESOURCES);
-    if (RS && ((N && !res->node_free) || (P && !res->pod_req))) return fail(KS_ERR_INVALID, "NULL node_free or pod_req");
-    for (uint64_t i = 0; i < P * RS; i++)
-        if (res->pod_req[i] < 0)
-            return fail(KS_ERR_RANGE, "pod %llu: request %lld of resource %llu (at least 0)", (unsigned long long)(i / RS),
-                        (long long)res->pod_req[i], (unsigned long long)(i % RS));
-    const uint64_t NG = gangs ? gangs->n : 0; // ks_gang_fit_bind's gangs
-    if (gangs) {
-        if (!gangs->offset || (NG && !gangs->min_member)) return fail(KS_ERR_INVALID, "NULL gang array");
-        rc = check_gangs(gangs, P, KS_SPREAD_BIND_MAX_PODS);
-        if (rc) return rc;
-    }
-    AffinityPlan plan;
-    if (aff) {
-        try {
-            rc = compile_affinity(aff, (uint32_t)G, K, spread->n_domains, N, &plan, sc);
-        } catch (...) {
-            return fail(KS_ERR_NOMEM, "out of host memory in %s", call);
-        }
-        if (rc) return rc;
-    }
-    NodeRulesPlan nplan;
-    if (nr) {
-        try {
-            rc = compile_node_rules(nr, (uint32_t)G, N, &nplan);
-        } catch (...) {
-            return fail(KS_ERR_NOMEM, "out of host memory in %s", call);
-        }
-        if (rc) return rc;
-    }
-    const BindMode mode = gangs ? BIND_GANG_FIT
-                          : res ? BIND_FIT
-                          : nr  ? BIND_NODE
-                          : sc  ? BIND_PROFILE
-                          : aff ? BIND_AFFINITY
-                                : BIND_SPREAD;
-    const uint64_t R = bind_refusal_words(mode), PW = bind_part_words(mode);
-    if (out_free && RS && N && (P == 0)) memcpy(out_free, res->node_free, RS * N * 8); // nothing binds: L3
-    if (out_placed) memset(out_placed, 0, NG * 4); // rewritten by the walk when it runs
+    const BindOutputs& o = r.out;
+    const uint64_t P = r.pods->n, GS = (uint64_t)r.n_groups * pl.S, RS = r.res ? r.res->n_res : 0;
+    const uint32_t N = s->N;
+    if (o.free_r && RS && N && (P == 0)) memcpy(o.free_r, r.res->node_free, RS * N * 8); // nothing binds: L3
+    if (o.placed) memset(o.placed, 0, r.gangs->n * 4); // rewritten by the walk when it runs
     if (P == 0) return KS_OK;
     if (N == 0) { // no node: nothing is placed, every count is existing
-        memset(out_node_idx, 0xff, P * 4);
-        if (out_score) memset(out_score, 0, P * 8);
-        if (out_refused) memset(out_refused, 0, P * R * 4);
-        for (uint32_t* c : {out_domain_count, out_soft_count})
+        memset(o.node_idx, 0xff, P * 4);
+        if (o.score) memset(o.score, 0, P * 8);
+        if (o.refused) memset(o.refused, 0, P * bind_refusal_words(r.mode) * 4);
+        for (uint32_t* c : {o.domain_count, o.soft_count})
             if (c) {
-                if (spread->existing) memcpy(c, spread->existing, GS * 4);
+                if (r.topo->existing) memcpy(c, r.topo->existing, GS * 4);
                 else memset(c, 0, GS * 4);
             }
-        if (out_parts) memset(out_parts, 0, P * PW * 8);
+        if (o.parts) memset(o.parts, 0, P * bind_part_words(r.mode) * 8);
         return KS_OK;
+    }
+    for (uint32_t k = 0; r.scoring && k < r.topo->n_keys; k++) { // the domain bitmaps, once a walk runs
+        const uint32_t D = r.topo->n_domains[k];
+        std::vector<uint8_t> seen;
+        try {
+            seen.assign(D, 0);
+        } catch (...) {
+            return fail(KS_ERR_NOMEM, "out of host memory in %s", r.call);
+        }
+        bool uniq = true;
+        for (uint32_t n = 0; n < N && uniq; n++) {
+            const int32_t d = r.topo->node_domain[k][n];
+            if (d >= 0) uniq = !seen[d]++;
+        }
+        pl.bwo[k] = pl.BW;
+        if (uniq) pl.uniq |= 1u << k;
+        else pl.BW += (D + 31) / 32;
     }
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
     if (!s->coop) return fail(KS_ERR_CUDA, "device %d has no cooperative launch", s->device);
     ProfileBindArgs q{}; // the fields a mode does not read stay zero
     SpreadBindArgs& a = q.b;
-    a.grid = std::max(1u, std::min<uint32_t>((uint32_t)s->sms, (N + 127u) / 128u));
-    a.setup_grid = bind_setup_grid((uint32_t)G, s->sms);
-    HostStaged h;
-    const auto cpu = h.in(pods->req_cpu, P), mem = h.in(pods->req_mem, P);
-    const auto sel = h.in(pods->sel, P * W);
-    const auto grp = h.in(group, P);
-    const auto max_skew = h.in(spread->max_skew, G * K); // NULL (affinity only): zeros, filled below
-    const auto min_domains = h.in(spread->min_domains, spread->min_domains ? G * K : 0);
-    const auto existing = h.in(spread->existing, spread->existing ? GS : 0);
-    const auto dom = h.in<int32_t>(nullptr, (uint64_t)K * N);  // the K node_domain arrays, gathered below
-    const auto gsel = h.in<uint64_t>(nullptr, G * W);          // each group's selector
-    const auto score = h.out(out_score, P);
-    const auto idx = h.out(out_node_idx, P);
-    const auto refused = h.out(out_refused, P * R);
-    const auto count = h.out(out_domain_count, GS);           // the counts themselves: device state of the whole call
-    const uint64_t E = aff ? aff->n_existing : 0;
-    const auto abase = h.in<uint32_t>(nullptr, plan.abase.size()); // the compiled terms, copied from plan below
-    const auto aflag = h.in<uint32_t>(nullptr, plan.aflag.size());
-    const auto upd_off = h.in<uint32_t>(nullptr, plan.upd_off.size());
-    const auto upd = h.in<uint32_t>(nullptr, plan.upd.size());
-    const auto ex_group = h.in(aff ? aff->existing_group : nullptr, E);
-    const auto ex_node = h.in(aff ? aff->existing_node : nullptr, E);
-    const auto acnt = h.work<uint32_t>(plan.words, 16);
-    const auto paref = h.work<uint32_t>(aff ? a.grid : 0);
-    const auto elig = h.work<uint8_t>(GS);
-    const auto gk = h.work<uint32_t>(G * K * 4, 16);
-    const auto pkey = h.work<int64_t>(a.grid);
-    const auto pidx = h.work<int32_t>(a.grid);
-    const auto pref = h.work<uint32_t>(a.grid);
-    // ks_profile_bind: the soft terms, the log table and the compiled IPA entries; the domain bitmaps of the keys with
-    // more than one node in some domain, per parity
-    const uint64_t Q = sc ? 1 : 0;
-    if (sc) {
-        std::vector<uint8_t> seen;
-        for (uint32_t k = 0; k < K; k++) {
-            try {
-                seen.assign(spread->n_domains[k], 0);
-            } catch (...) {
-                return fail(KS_ERR_NOMEM, "out of host memory in %s", call);
-            }
-            bool uniq = true;
-            for (uint32_t n = 0; n < N && uniq; n++) {
-                const int32_t d = spread->node_domain[k][n];
-                if (d >= 0) uniq = !seen[d]++;
-            }
-            q.bwo[k] = q.BW;
-            if (uniq) q.uniq |= 1u << k;
-            else q.BW += (spread->n_domains[k] + 31) / 32;
-        }
-    }
-    const auto soft_skew = h.in(sc ? sc->soft_skew : nullptr, Q * G * K); // NULL: zeros, filled below
-    const auto soft_all = h.in(sc ? sc->soft_all_keys : nullptr, Q * G);  // NULL: ones, filled below
-    const auto logw = h.in<double>(nullptr, Q * (N + 2ull));
-    const auto ibase = h.in<uint32_t>(nullptr, plan.ibase.size());
-    const auto iupd_off = h.in<uint32_t>(nullptr, plan.iupd_off.size());
-    const auto iupd = h.in<uint32_t>(nullptr, plan.iupd.size());
-    const auto icoef = h.in<int32_t>(nullptr, plan.icoef.size());
-    const auto parts = h.out(out_parts, Q * PW * P);
-    const auto scnt = h.out(out_soft_count, Q * GS);
-    const auto icnt = h.work<int64_t>(plan.iwords, 16);
-    const auto bits = h.work<uint32_t>(2ull * q.BW, 16);
-    const auto iraw = h.work<int64_t>(Q * N), praw = h.work<int64_t>(Q * N);
-    const auto pdom = h.work<uint32_t>(Q * a.grid * KS_SPREAD_MAX_KEYS), plack = h.work<uint32_t>(Q * a.grid);
-    const auto pimin = h.work<int64_t>(Q * a.grid), pimax = h.work<int64_t>(Q * a.grid);
-    const auto ppmin = h.work<int64_t>(Q * a.grid), ppmax = h.work<int64_t>(Q * a.grid);
-    // ks_node_bind: the compiled classes, the rule keys' domains, the taints and the sets; one rule word per (class, node)
-    const uint64_t NR1 = nr ? 1 : 0;
-    const uint32_t KN = nr ? nr->n_keys : 0;
-    const auto ncls = h.in<uint32_t>(nullptr, nplan.cls.size());
-    const auto ctol = h.in<uint64_t>(nullptr, nplan.ctol.size());
-    const auto cterm_off = h.in<uint32_t>(nullptr, NR1 * nplan.cterm_off.size());
-    const auto cterm_w = h.in<uint32_t>(nullptr, nplan.cterm_w.size());
-    const auto cexpr_off = h.in<uint32_t>(nullptr, NR1 * nplan.cexpr_off.size());
-    const auto cexpr_key = h.in<uint32_t>(nullptr, nplan.cexpr_key.size());
-    const auto cexpr_set = h.in<uint64_t>(nullptr, nplan.cexpr_set.size());
-    const auto nset = h.in(nr ? nr->expr_set : nullptr, nplan.set_words);
-    const auto ndom = h.in<int32_t>(nullptr, (uint64_t)KN * N);
-    const auto taint_hard = h.in(nr ? nr->node_taint_hard : nullptr, NR1 * N); // NULL: zeros, filled below
-    const auto taint_soft = h.in(nr ? nr->node_taint_soft : nullptr, NR1 * N);
-    const auto nrules = h.work<uint32_t>((uint64_t)nplan.C * N);
-    const auto ptref = h.work<uint32_t>(NR1 * a.grid), pnref = h.work<uint32_t>(NR1 * a.grid);
-    const auto ptmax = h.work<uint32_t>(NR1 * a.grid), pnmax = h.work<uint32_t>(NR1 * a.grid);
-    // ks_fit_bind: the requests, the caller's free amounts and the charged ones, one row per resource
-    const auto res_req = h.in(RS ? res->pod_req : nullptr, P * RS);
-    const auto res_node_free = h.in(RS ? res->node_free : nullptr, RS * N);
-    const auto res_free = h.out(out_free, RS * N);
-    const auto pfref = h.work<uint32_t>(res ? a.grid : 0);
-    // ks_gang_fit_bind: the gangs' offsets (P < 2^32) and minimums, their counts, and the rollback's group marks and lists
-    const auto goff = h.in<uint32_t>(nullptr, gangs ? NG + 1 : 0);
-    const auto gmin = h.in(gangs ? gangs->min_member : nullptr, NG);
-    const auto gplaced = h.out(out_placed, NG);
-    const auto gmark = h.work<uint32_t>(gangs ? 2 * G : 0), glist = h.work<uint32_t>(gangs ? 2 * G : 0);
-    auto put = [&](Staged<uint32_t> d, const std::vector<uint32_t>& v) {
-        if (!v.empty()) memcpy(h.host(d), v.data(), v.size() * 4);
-    };
-    CU_TRY(h.reserve(s));
-    if (nr) {
-        put(ncls, nplan.cls);
-        memcpy(h.host(ctol), nplan.ctol.data(), nplan.ctol.size() * 8);
-        put(cterm_off, nplan.cterm_off);
-        put(cterm_w, nplan.cterm_w);
-        put(cexpr_off, nplan.cexpr_off);
-        put(cexpr_key, nplan.cexpr_key);
-        if (!nplan.cexpr_set.empty()) memcpy(h.host(cexpr_set), nplan.cexpr_set.data(), nplan.cexpr_set.size() * 8);
-        for (uint32_t k = 0; k < KN; k++) memcpy(h.host(ndom) + (size_t)k * N, nr->node_domain[k], (size_t)N * 4);
-        if (!nr->node_taint_hard) memset(h.host(taint_hard), 0, (size_t)N * 8);
-        if (!nr->node_taint_soft) memset(h.host(taint_soft), 0, (size_t)N * 8);
-    }
-    if (sc) {
-        if (!sc->soft_skew) memset(h.host(soft_skew), 0, G * K * 4);
-        if (!sc->soft_all_keys) memset(h.host(soft_all), 1, G);
-        for (uint64_t i = 0; i < N + 2ull; i++) h.host(logw)[i] = log((double)(i + 2)); // the oracle's libm
-        put(ibase, plan.ibase);
-        put(iupd_off, plan.iupd_off);
-        put(iupd, plan.iupd);
-        if (!plan.icoef.empty()) memcpy(h.host(icoef), plan.icoef.data(), plan.icoef.size() * 4);
-    }
-    if (gangs)
-        for (uint64_t j = 0; j <= NG; j++) h.host(goff)[j] = (uint32_t)gangs->offset[j];
-    for (uint32_t k = 0; k < K; k++) memcpy(h.host(dom) + (size_t)k * N, spread->node_domain[k], (size_t)N * 4);
-    if (!spread->max_skew) memset(h.host(max_skew), 0, G * K * 4);
-    put(abase, plan.abase);
-    put(aflag, plan.aflag);
-    put(upd_off, plan.upd_off);
-    put(upd, plan.upd);
-    for (uint64_t g = 0; g < G; g++) {
-        uint64_t* row = h.host(gsel) + g * W;
-        if (first[g] >= 0) memcpy(row, pods->sel + first[g] * W, W * 8);
-        else memset(row, 0, W * 8);
-    }
-    cudaStream_t st = s->stream;
-    CU_TRY(h.upload(st));
     a.N = N;
     a.Npad = s->Npad;
     a.P = (uint32_t)P;
-    a.G = (uint32_t)G;
-    a.K = K;
-    a.S = (uint32_t)S;
-    for (uint32_t k = 0, o = 0; k < K; o += spread->n_domains[k], k++) {
-        a.Dk[k] = spread->n_domains[k];
+    a.G = r.n_groups;
+    a.K = r.topo->n_keys;
+    a.S = (uint32_t)pl.S;
+    for (uint32_t k = 0, o = 0; k < a.K; o += r.topo->n_domains[k], k++) {
+        a.Dk[k] = r.topo->n_domains[k];
         a.Pk[k] = o;
     }
     a.alloc_cpu = s->alloc_cpu.as<int64_t>();
@@ -2371,146 +2503,65 @@ static int bind_spread(ks_snapshot* s, const char* call, const ks_pods* pods, co
     a.labels = s->labels.as<uint64_t>();
     a.free_cpu = s->free_cpu.as<int64_t>();
     a.free_mem = s->free_mem.as<int64_t>();
-    a.policy = policy;
-    a.req_cpu = h.dev(cpu);
-    a.req_mem = h.dev(mem);
-    a.sel = h.dev(sel);
-    a.group = h.dev(grp);
-    a.gsel = h.dev(gsel);
-    a.dom = h.dev(dom);
-    a.max_skew = h.dev(max_skew);
-    a.min_domains = spread->min_domains ? h.dev(min_domains) : nullptr;
-    a.existing = spread->existing ? h.dev(existing) : nullptr;
-    a.elig = h.dev(elig);
-    a.gk = h.dev(gk);
-    a.cnt = h.dev(count);
-    a.pkey = h.dev(pkey);
-    a.pidx = h.dev(pidx);
-    a.pref = h.dev(pref);
-    a.out_idx = h.dev(idx);
-    a.out_score = h.dev(score);
-    a.out_refused = h.dev(refused);
-    if (aff) {
-        a.abase = h.dev(abase);
-        a.aflag = h.dev(aflag);
-        a.upd_off = h.dev(upd_off);
-        a.upd = h.dev(upd);
-        a.ex_group = h.dev(ex_group);
-        a.ex_node = h.dev(ex_node);
-        a.E = (uint32_t)E;
-        a.any_base = plan.any_base;
-        a.aff_grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((E + 7) / 8, 4ull * (uint64_t)s->sms));
-        a.acnt = h.dev(acnt);
-        a.paref = h.dev(paref);
-    }
-    if (sc) {
-        q.soft_skew = h.dev(soft_skew);
-        q.soft_all = h.dev(soft_all);
-        q.logw = h.dev(logw);
-        q.bits = h.dev(bits);
-        q.scnt = h.dev(scnt);
-        q.ibase = h.dev(ibase);
-        q.iupd_off = h.dev(iupd_off);
-        q.iupd = h.dev(iupd);
-        q.icoef = h.dev(icoef);
-        q.icnt = h.dev(icnt);
-        q.iwords = plan.iwords;
-        q.iraw = h.dev(iraw);
-        q.praw = h.dev(praw);
-        q.pdom = h.dev(pdom);
-        q.plack = h.dev(plack);
-        q.pimin = h.dev(pimin);
-        q.pimax = h.dev(pimax);
-        q.ppmin = h.dev(ppmin);
-        q.ppmax = h.dev(ppmax);
-        q.out_parts = h.dev(parts);
-        q.wspread = sc->weight_spread;
-        q.waff = sc->weight_affinity;
-    }
-    if (nr) {
-        q.ncls = h.dev(ncls);
-        q.nrules = h.dev(nrules);
-        q.C = nplan.C;
-        q.KN = KN;
-        for (uint32_t k = 0; k < KN; k++) q.NDk[k] = nr->n_domains[k];
-        q.ndom = h.dev(ndom);
-        q.taint_hard = h.dev(taint_hard);
-        q.taint_soft = h.dev(taint_soft);
-        q.ctol = h.dev(ctol);
-        q.cterm_off = h.dev(cterm_off);
-        q.cterm_w = h.dev(cterm_w);
-        q.cexpr_off = h.dev(cexpr_off);
-        q.cexpr_key = h.dev(cexpr_key);
-        q.cexpr_set = h.dev(cexpr_set);
-        q.nset = h.dev(nset);
-        q.ptref = h.dev(ptref);
-        q.pnref = h.dev(pnref);
-        q.ptmax = h.dev(ptmax);
-        q.pnmax = h.dev(pnmax);
-        q.wtaint = nr->weight_taint;
-        q.wnaff = nr->weight_node_affinity;
-        q.rules_grid = (uint32_t)std::max<uint64_t>(
-            1, std::min<uint64_t>(((uint64_t)nplan.C * N + 255) / 256, 4ull * (uint64_t)s->sms));
-    }
-    if (res) {
-        q.R = (uint32_t)RS;
-        q.res_req = h.dev(res_req);
-        q.res_node_free = h.dev(res_node_free);
-        q.res_free = h.dev(res_free);
-        q.pfref = h.dev(pfref);
-    }
-    if (gangs) {
-        q.n_gangs = (uint32_t)NG;
-        q.goff = h.dev(goff);
-        q.gmin = h.dev(gmin);
-        q.gplaced = h.dev(gplaced);
-        q.gmark = h.dev(gmark);
-        q.glist = h.dev(glist);
-    }
+    a.policy = r.policy;
+    a.grid = pl.grid;
+    a.setup_grid = bind_setup_grid(r.n_groups, s->sms);
+    HostStaged h;
+    const BindStage stage{h, s, r, pl};
+    if (const int e = h.reserve(s)) return e;
+    stage.place(q);
+    cudaStream_t st = s->stream;
+    CU_TRY(h.upload(st));
     s->derived_dirty = true; // free[] changes: the bit-parallel index is stale
     s->version++;
-    const cudaError_t e = launch_bind(mode, q, plan.words, W, st);
-    if (e != cudaSuccess) return fail(KS_ERR_CUDA, "%s launch failed: %s", BIND_NAME[mode], cudaGetErrorString(e));
+    const cudaError_t e = launch_bind(r.mode, q, pl.aff.words, s->W, st);
+    if (e != cudaSuccess) return fail(KS_ERR_CUDA, "%s launch failed: %s", BIND_NAME[r.mode], cudaGetErrorString(e));
     CU_TRY(h.finish(st));
-    s->last_path = BIND_PATH[mode];
+    s->last_path = BIND_PATH[r.mode];
+    return KS_OK;
+}
+
+// ks_fit_bind and ks_gang_fit_bind: with rules NULL, parts words 3-4 read 0, as ks_node_bind's K1 gives them (M1)
+static int bind_fit(ks_snapshot* s, const BindRequest& r) {
+    const int rc = bind_spread(s, r);
+    if (rc || r.rules || !r.out.parts) return rc;
+    for (uint64_t p = 0; p < r.pods->n; p++) r.out.parts[5 * p + 3] = r.out.parts[5 * p + 4] = 0;
     return KS_OK;
 }
 
 int ks_spread_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
                    const ks_spread_multi* spread, int policy, int32_t* out_node_idx, int64_t* out_score,
                    uint32_t* out_refused, uint32_t* out_domain_count) {
-    return bind_spread(s, "ks_spread_bind", pods, group, n_groups, spread, nullptr, policy, out_node_idx, out_score,
-                       out_refused, out_domain_count);
+    return bind_spread(s, {"ks_spread_bind", BIND_SPREAD, pods, group, n_groups, spread, policy,
+                           {out_node_idx, out_score, out_refused, out_domain_count}});
 }
 
 int ks_affinity_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
                      const ks_spread_multi* topo, const ks_pod_affinity* aff, int policy, int32_t* out_node_idx,
                      int64_t* out_score, uint32_t* out_refused, uint32_t* out_domain_count) {
-    const ks_pod_affinity none{};
-    return bind_spread(s, "ks_affinity_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
-                       out_score, out_refused, out_domain_count);
+    return bind_spread(s, {"ks_affinity_bind", BIND_AFFINITY, pods, group, n_groups, topo, policy,
+                           {out_node_idx, out_score, out_refused, out_domain_count}, aff});
 }
 
 int ks_profile_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
                     const ks_spread_multi* topo, const ks_pod_affinity* aff, const ks_bind_scoring* scoring, int policy,
                     int32_t* out_node_idx, int64_t* out_score, int64_t* out_parts, uint32_t* out_refused,
                     uint32_t* out_domain_count, uint32_t* out_soft_count) {
-    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
-    const ks_pod_affinity none{};
-    return bind_spread(s, "ks_profile_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
-                       out_score, out_refused, out_domain_count, scoring, out_parts, out_soft_count);
+    return bind_spread(s, {"ks_profile_bind", BIND_PROFILE, pods, group, n_groups, topo, policy,
+                           {out_node_idx, out_score, out_refused, out_domain_count, out_parts, out_soft_count}, aff,
+                           scoring});
 }
 
 int ks_node_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
                  const ks_spread_multi* topo, const ks_pod_affinity* aff, const ks_bind_scoring* scoring,
                  const ks_node_rules* rules, int policy, int32_t* out_node_idx, int64_t* out_score, int64_t* out_parts,
                  uint32_t* out_refused, uint32_t* out_domain_count, uint32_t* out_soft_count) {
-    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
-    const ks_pod_affinity none{};
-    if (rules)
-        return bind_spread(s, "ks_node_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
-                           out_score, out_refused, out_domain_count, scoring, out_parts, out_soft_count, rules);
+    BindRequest r{"ks_node_bind", BIND_NODE, pods, group, n_groups, topo, policy,
+                  {out_node_idx, out_score, out_refused, out_domain_count, out_parts, out_soft_count}, aff, scoring,
+                  rules};
+    if (rules) return bind_spread(s, r);
     // K1: no rules is ks_profile_bind itself, its refusals and parts widened with zeros
+    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
     const uint64_t P = pods ? pods->n : 0;
     std::vector<uint32_t> ref;
     std::vector<int64_t> parts;
@@ -2520,9 +2571,10 @@ int ks_node_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint
     } catch (...) {
         return fail(KS_ERR_NOMEM, "out of host memory in ks_node_bind");
     }
-    const int rc = bind_spread(s, "ks_node_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
-                               out_score, out_refused ? ref.data() : nullptr, out_domain_count, scoring,
-                               out_parts ? parts.data() : nullptr, out_soft_count);
+    r.mode = BIND_PROFILE;
+    r.out.refused = out_refused ? ref.data() : nullptr;
+    r.out.parts = out_parts ? parts.data() : nullptr;
+    const int rc = bind_spread(s, r);
     if (rc) return rc;
     for (uint64_t p = 0; p < P; p++) {
         if (out_refused) {
@@ -2543,16 +2595,9 @@ int ks_fit_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint3
                 const ks_node_rules* rules, const ks_bind_resources* res, int policy, int32_t* out_node_idx,
                 int64_t* out_score, int64_t* out_parts, uint32_t* out_refused, uint32_t* out_domain_count,
                 uint32_t* out_soft_count, int64_t* out_free) {
-    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
-    const ks_pod_affinity none{};
-    const ks_node_rules no_rules{}; // no taint, no term, both plugin weights 0: the total is ks_profile_bind's
-    const ks_bind_resources no_res{};
-    const int rc = bind_spread(s, "ks_fit_bind", pods, group, n_groups, topo, aff ? aff : &none, policy, out_node_idx,
-                               out_score, out_refused, out_domain_count, scoring, out_parts, out_soft_count,
-                               rules ? rules : &no_rules, res ? res : &no_res, out_free);
-    if (rc || rules || !out_parts) return rc;
-    for (uint64_t p = 0; p < pods->n; p++) out_parts[5 * p + 3] = out_parts[5 * p + 4] = 0; // as ks_node_bind's K1
-    return KS_OK;
+    return bind_fit(s, {"ks_fit_bind", BIND_FIT, pods, group, n_groups, topo, policy,
+                        {out_node_idx, out_score, out_refused, out_domain_count, out_parts, out_soft_count, out_free},
+                        aff, scoring, rules, res});
 }
 
 int ks_gang_fit_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
@@ -2560,17 +2605,10 @@ int ks_gang_fit_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, 
                      const ks_node_rules* rules, const ks_bind_resources* res, const ks_gangs* gangs, int policy,
                      int32_t* out_node_idx, int64_t* out_score, int64_t* out_parts, uint32_t* out_refused,
                      uint32_t* out_domain_count, uint32_t* out_soft_count, int64_t* out_free, uint32_t* out_placed) {
-    if (!scoring) return fail(KS_ERR_INVALID, "NULL scoring");
-    if (!gangs) return fail(KS_ERR_INVALID, "NULL gangs");
-    const ks_pod_affinity none{};
-    const ks_node_rules no_rules{}; // as ks_fit_bind's
-    const ks_bind_resources no_res{};
-    const int rc = bind_spread(s, "ks_gang_fit_bind", pods, group, n_groups, topo, aff ? aff : &none, policy,
-                               out_node_idx, out_score, out_refused, out_domain_count, scoring, out_parts, out_soft_count,
-                               rules ? rules : &no_rules, res ? res : &no_res, out_free, gangs, out_placed);
-    if (rc || rules || !out_parts) return rc;
-    for (uint64_t p = 0; p < pods->n; p++) out_parts[5 * p + 3] = out_parts[5 * p + 4] = 0; // M1: ks_fit_bind's
-    return KS_OK;
+    return bind_fit(s, {"ks_gang_fit_bind", BIND_GANG_FIT, pods, group, n_groups, topo, policy,
+                        {out_node_idx, out_score, out_refused, out_domain_count, out_parts, out_soft_count, out_free,
+                         out_placed},
+                        aff, scoring, rules, res, gangs});
 }
 
 // ---------------------------------------------------------------------------------------------- async streaming

@@ -132,6 +132,24 @@ def node_rules(group_rules, weight_taint=3, weight_node_affinity=2):
     return nr, hold
 
 
+def _scoring(n_groups, k, n_terms, soft_skew, soft_all_keys, term_weight, hard_affinity_weight, weight_spread,
+             weight_affinity):
+    """The ks_bind_scoring of the reconcile calls that score, and the arrays it points into (keep them alive):
+    soft_skew [n_groups, K], soft_all_keys [n_groups] and term_weight [n_terms], each None or of exactly that length."""
+    def arr(a, dtype, n, name):
+        if a is None:
+            return None
+        a = np.ascontiguousarray(a, dtype).reshape(-1)
+        if a.shape[0] != n:
+            raise ValueError(f"{name} has {a.shape[0]} entries, expected {n}")
+        return a
+    hold = (arr(soft_skew, np.uint32, n_groups * k, "soft_skew"),
+            arr(soft_all_keys, np.uint8, n_groups, "soft_all_keys"), arr(term_weight, np.uint32, n_terms, "term_weight"))
+    scoring = capi.ks_bind_scoring(*[None if a is None else a.ctypes.data for a in hold], int(hard_affinity_weight),
+                                   int(weight_spread), int(weight_affinity))
+    return scoring, hold
+
+
 class ksh_pod_affinity(C.Structure):
     _fields_ = [("n_terms", C.c_uint32), ("owner", C.c_void_p), ("kind", C.c_void_p), ("key", C.c_void_p),
                 ("target_offset", C.c_void_p), ("target", C.c_void_p), ("n_existing", C.c_uint64),
@@ -483,33 +501,8 @@ class Context:
         group with max_skew and min_domains [n_groups, K] over topology_keys (max_skew 0 = the key is not constrained);
         existing_nodes[g][k] lists the node names of group g's bound pods for key k (None: none).  Pods are bound one at
         a time in arrival order.  Returns (status[n], node_idx[n], bodies[n] (str | None))."""
-        k = len(topology_keys)
-        group = np.ascontiguousarray(group, np.int32).reshape(-1)
-        max_skew = np.ascontiguousarray(max_skew, np.uint32).reshape(-1)
-        if group.shape[0] != n or max_skew.shape[0] != n_groups * k:
-            raise ValueError(f"group / max_skew have {group.shape[0]} / {max_skew.shape[0]} entries, pods {n}, groups "
-                             f"{n_groups}, keys {k}")
-        mind = None if min_domains is None else np.ascontiguousarray(min_domains, np.uint32).reshape(-1)
-        names, ex_off = None, None
-        if existing_nodes is not None:
-            lists = [lst for per_group in existing_nodes for lst in per_group]
-            flat = [s.encode() for lst in lists for s in lst]
-            names = (C.c_char_p * max(len(flat), 1))(*flat)
-            ex_off = np.zeros(n_groups * k + 1, np.uint64)
-            np.cumsum([len(lst) for lst in lists], out=ex_off[1:])
-        keys = (C.c_char_p * max(k, 1))(*[key.encode() for key in topology_keys])
-        status = np.empty(n, np.int32)
-        node = np.empty(n, np.int32)
-        off = np.empty(n, np.int64)
-        cap = int(json_cap if json_cap is not None else 512 * max(n, 1))
-        buf = C.create_string_buffer(max(cap, 1))
-        check(lib.ksh_reconcile_spread(self._h, C.addressof(pods) if n else None, n, group.ctypes.data, int(n_groups),
-                                       C.cast(keys, _vp), k, max_skew.ctypes.data,
-                                       None if mind is None else mind.ctypes.data,
-                                       None if names is None else C.cast(names, _vp),
-                                       None if ex_off is None else ex_off.ctypes.data, int(policy), status.ctypes.data,
-                                       node.ctypes.data, C.addressof(buf), cap, off.ctypes.data), "ksh_reconcile_spread")
-        return status, node, _string_list(buf, off)
+        return self._reconcile_terms("ksh_reconcile_spread", pods, n, group, n_groups, topology_keys, None, (),
+                                     max_skew, min_domains, existing_nodes, policy, json_cap)
 
     def reconcile_affinity(self, pods, n, group, n_groups, topology_keys, terms=(), existing_pods=(), max_skew=None,
                            min_domains=None, existing_nodes=None, policy=capi.KS_SCORE_LEFTOVER, json_cap=None):
@@ -517,8 +510,8 @@ class Context:
         max_skew optional (None: no spread constraint), terms a list of (owner group, kind KS_POD_AFFINITY /
         KS_POD_ANTI_AFFINITY, index into topology_keys, target groups) and existing_pods a list of (group, node name) of
         bound pods the terms see.  Returns (status[n], node_idx[n], bodies[n] (str | None))."""
-        return self._reconcile_terms(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
-                                     min_domains, existing_nodes, policy, json_cap, None)
+        return self._reconcile_terms("ksh_reconcile_affinity", pods, n, group, n_groups, topology_keys, terms,
+                                     existing_pods, max_skew, min_domains, existing_nodes, policy, json_cap)
 
     def reconcile_profile(self, pods, n, group, n_groups, topology_keys, terms=(), existing_pods=(), max_skew=None,
                           min_domains=None, existing_nodes=None, policy=capi.KS_SCORE_LEAST_BALANCED, json_cap=None,
@@ -528,22 +521,11 @@ class Context:
         KS_POD_AFFINITY_PREFERRED / KS_POD_ANTI_AFFINITY_PREFERRED with term_weight [T]; soft_skew [n_groups, K] or
         None, soft_all_keys [n_groups] or None (all 1), and the three weights as Snapshot.profile_bind takes them.
         Returns (status[n], node_idx[n], bodies[n] (str | None))."""
-        k = len(topology_keys)
-        soft = None if soft_skew is None else np.ascontiguousarray(soft_skew, np.uint32).reshape(-1)
-        if soft is not None and soft.shape[0] != n_groups * k:
-            raise ValueError(f"soft_skew has {soft.shape[0]} entries, groups {n_groups}, keys {k}")
-        sall = None if soft_all_keys is None else np.ascontiguousarray(soft_all_keys, np.uint8).reshape(-1)
-        if sall is not None and sall.shape[0] != n_groups:
-            raise ValueError(f"soft_all_keys has {sall.shape[0]} entries, groups {n_groups}")
-        tw = None if term_weight is None else np.ascontiguousarray(term_weight, np.uint32).reshape(-1)
-        if tw is not None and tw.shape[0] != len(terms):
-            raise ValueError(f"term_weight has {tw.shape[0]} entries, terms {len(terms)}")
-        scoring = capi.ks_bind_scoring(None if soft is None else soft.ctypes.data,
-                                       None if sall is None else sall.ctypes.data,
-                                       None if tw is None else tw.ctypes.data, int(hard_affinity_weight),
-                                       int(weight_spread), int(weight_affinity))
-        return self._reconcile_terms(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
-                                     min_domains, existing_nodes, policy, json_cap, scoring)
+        scoring, hold = _scoring(n_groups, len(topology_keys), len(terms), soft_skew, soft_all_keys, term_weight,
+                                 hard_affinity_weight, weight_spread, weight_affinity)
+        return self._reconcile_terms("ksh_reconcile_profile", pods, n, group, n_groups, topology_keys, terms,
+                                     existing_pods, max_skew, min_domains, existing_nodes, policy, json_cap,
+                                     (C.byref(scoring),))
 
     def set_node_taints(self, taints):
         """spec.taints of nodes by name (ksh_context_set_node_taints): taints maps a node name to a list of
@@ -580,7 +562,7 @@ class Context:
         return self._reconcile_rules(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
                                      min_domains, existing_nodes, policy, json_cap, soft_skew, soft_all_keys,
                                      term_weight, hard_affinity_weight, weight_spread, weight_affinity, group_rules,
-                                     weight_taint, weight_node_affinity, False)
+                                     weight_taint, weight_node_affinity, "ksh_reconcile_nodes")
 
     def compile_resources(self, pods, n):
         """The scalar resources of the pending batch pods[0:n] (ksh_compile_resources): (names, node_free int64 [R, N],
@@ -607,7 +589,7 @@ class Context:
         return self._reconcile_rules(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
                                      min_domains, existing_nodes, policy, json_cap, soft_skew, soft_all_keys,
                                      term_weight, hard_affinity_weight, weight_spread, weight_affinity, group_rules,
-                                     weight_taint, weight_node_affinity, True)
+                                     weight_taint, weight_node_affinity, "ksh_reconcile_fit")
 
     def reconcile_fit_gangs(self, pods, n, group, n_groups, topology_keys, offset, min_member, terms=(),
                             existing_pods=(), max_skew=None, min_domains=None, existing_nodes=None,
@@ -627,37 +609,29 @@ class Context:
         return self._reconcile_rules(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
                                      min_domains, existing_nodes, policy, json_cap, soft_skew, soft_all_keys,
                                      term_weight, hard_affinity_weight, weight_spread, weight_affinity, group_rules,
-                                     weight_taint, weight_node_affinity, True,
-                                     gangs=(offset, g, min_member, placed)) + (placed,)
+                                     weight_taint, weight_node_affinity, "ksh_reconcile_fit_gangs",
+                                     (offset.ctypes.data, g, min_member.ctypes.data), placed) + (placed,)
 
     def _reconcile_rules(self, pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew, min_domains,
                          existing_nodes, policy, json_cap, soft_skew, soft_all_keys, term_weight, hard_affinity_weight,
-                         weight_spread, weight_affinity, group_rules, weight_taint, weight_node_affinity, fit,
-                         gangs=None):
-        # ksh_reconcile_nodes, or with fit ksh_reconcile_fit
+                         weight_spread, weight_affinity, group_rules, weight_taint, weight_node_affinity, entry,
+                         gangs=(), placed=None):
+        # ksh_reconcile_nodes, ksh_reconcile_fit, or ksh_reconcile_fit_gangs with gangs (offset, n_gangs, min_member)
         nr = None
         if group_rules is not None:
             if len(group_rules) != n_groups:
                 raise ValueError(f"group_rules has {len(group_rules)} entries, groups {n_groups}")
             nr = node_rules(group_rules, weight_taint, weight_node_affinity)
-        k = len(topology_keys)
-        soft = None if soft_skew is None else np.ascontiguousarray(soft_skew, np.uint32).reshape(-1)
-        sall = None if soft_all_keys is None else np.ascontiguousarray(soft_all_keys, np.uint8).reshape(-1)
-        tw = None if term_weight is None else np.ascontiguousarray(term_weight, np.uint32).reshape(-1)
-        if soft is not None and soft.shape[0] != n_groups * k:
-            raise ValueError(f"soft_skew has {soft.shape[0]} entries, groups {n_groups}, keys {k}")
-        scoring = capi.ks_bind_scoring(None if soft is None else soft.ctypes.data,
-                                       None if sall is None else sall.ctypes.data,
-                                       None if tw is None else tw.ctypes.data, int(hard_affinity_weight),
-                                       int(weight_spread), int(weight_affinity))
-        return self._reconcile_terms(pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
-                                     min_domains, existing_nodes, policy, json_cap, scoring, nodes=True,
-                                     rules=None if nr is None else nr[0], fit=fit, gangs=gangs)
+        scoring, hold = _scoring(n_groups, len(topology_keys), len(terms), soft_skew, soft_all_keys, term_weight,
+                                 hard_affinity_weight, weight_spread, weight_affinity)
+        return self._reconcile_terms(entry, pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
+                                     min_domains, existing_nodes, policy, json_cap,
+                                     (C.byref(scoring), None if nr is None else C.byref(nr[0]), *gangs), placed)
 
-    def _reconcile_terms(self, pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew, min_domains,
-                         existing_nodes, policy, json_cap, scoring, nodes=False, rules=None, fit=False, gangs=None):
-        # ksh_reconcile_affinity, or with scoring ksh_reconcile_profile, or with nodes ksh_reconcile_nodes (with fit
-        # ksh_reconcile_fit, and with gangs = (offset, n_gangs, min_member, placed) ksh_reconcile_fit_gangs)
+    def _reconcile_terms(self, entry, pods, n, group, n_groups, topology_keys, terms, existing_pods, max_skew,
+                         min_domains, existing_nodes, policy, json_cap, mid=(), placed=None):
+        # the host-layer call `entry`: its queue and topology, then (terms not None) the terms and existing pods, then
+        # mid (scoring, rules, gangs), the policy and the outputs, with placed before the bodies when given
         k = len(topology_keys)
         group = np.ascontiguousarray(group, np.int32).reshape(-1)
         if group.shape[0] != n:
@@ -674,43 +648,31 @@ class Context:
             names = (C.c_char_p * max(len(flat), 1))(*flat)
             ex_off = np.zeros(n_groups * k + 1, np.uint64)
             np.cumsum([len(lst) for lst in lists], out=ex_off[1:])
-        owner = np.ascontiguousarray([t[0] for t in terms], np.int32)
-        kind = np.ascontiguousarray([t[1] for t in terms], np.uint8)
-        tkey = np.ascontiguousarray([t[2] for t in terms], np.uint32)
-        toff = np.zeros(len(terms) + 1, np.uint64)
-        np.cumsum([len(t[3]) for t in terms], out=toff[1:])
-        target = np.ascontiguousarray([g for t in terms for g in t[3]], np.int32)
-        egroup = np.ascontiguousarray([e[0] for e in existing_pods], np.int32)
-        enames = (C.c_char_p * max(len(existing_pods), 1))(*[e[1].encode() for e in existing_pods])
-        aff = ksh_pod_affinity(len(terms), owner.ctypes.data, kind.ctypes.data, tkey.ctypes.data, toff.ctypes.data,
-                               target.ctypes.data, len(existing_pods), egroup.ctypes.data, C.cast(enames, _vp))
         keys = (C.c_char_p * max(k, 1))(*[key.encode() for key in topology_keys])
+        args = [self._h, C.addressof(pods) if n else None, n, group.ctypes.data, int(n_groups), C.cast(keys, _vp), k,
+                None if max_skew is None else max_skew.ctypes.data, None if mind is None else mind.ctypes.data,
+                None if names is None else C.cast(names, _vp), None if ex_off is None else ex_off.ctypes.data]
+        if terms is not None:
+            owner = np.ascontiguousarray([t[0] for t in terms], np.int32)
+            kind = np.ascontiguousarray([t[1] for t in terms], np.uint8)
+            tkey = np.ascontiguousarray([t[2] for t in terms], np.uint32)
+            toff = np.zeros(len(terms) + 1, np.uint64)
+            np.cumsum([len(t[3]) for t in terms], out=toff[1:])
+            target = np.ascontiguousarray([g for t in terms for g in t[3]], np.int32)
+            egroup = np.ascontiguousarray([e[0] for e in existing_pods], np.int32)
+            enames = (C.c_char_p * max(len(existing_pods), 1))(*[e[1].encode() for e in existing_pods])
+            aff = ksh_pod_affinity(len(terms), owner.ctypes.data, kind.ctypes.data, tkey.ctypes.data,
+                                   toff.ctypes.data, target.ctypes.data, len(existing_pods), egroup.ctypes.data,
+                                   C.cast(enames, _vp))
+            args.append(C.byref(aff))
         status = np.empty(n, np.int32)
         node = np.empty(n, np.int32)
         off = np.empty(n, np.int64)
         cap = int(json_cap if json_cap is not None else 512 * max(n, 1))
         buf = C.create_string_buffer(max(cap, 1))
-        head = (self._h, C.addressof(pods) if n else None, n, group.ctypes.data, int(n_groups), C.cast(keys, _vp), k,
-                None if max_skew is None else max_skew.ctypes.data, None if mind is None else mind.ctypes.data,
-                None if names is None else C.cast(names, _vp), None if ex_off is None else ex_off.ctypes.data,
-                C.byref(aff))
-        tail = (int(policy), status.ctypes.data, node.ctypes.data, C.addressof(buf), cap, off.ctypes.data)
-        if gangs is not None:
-            offset, g, min_member, placed = gangs
-            check(lib.ksh_reconcile_fit_gangs(*head, C.byref(scoring), None if rules is None else C.byref(rules),
-                                              offset.ctypes.data, g, min_member.ctypes.data, int(policy),
-                                              status.ctypes.data, node.ctypes.data, placed.ctypes.data,
-                                              C.addressof(buf), cap, off.ctypes.data), "ksh_reconcile_fit_gangs")
-        elif fit:
-            check(lib.ksh_reconcile_fit(*head, C.byref(scoring), None if rules is None else C.byref(rules), *tail),
-                  "ksh_reconcile_fit")
-        elif nodes:
-            check(lib.ksh_reconcile_nodes(*head, C.byref(scoring), None if rules is None else C.byref(rules), *tail),
-                  "ksh_reconcile_nodes")
-        elif scoring is None:
-            check(lib.ksh_reconcile_affinity(*head, *tail), "ksh_reconcile_affinity")
-        else:
-            check(lib.ksh_reconcile_profile(*head, C.byref(scoring), *tail), "ksh_reconcile_profile")
+        args += [*mid, int(policy), status.ctypes.data, node.ctypes.data]
+        args += ([] if placed is None else [placed.ctypes.data]) + [C.addressof(buf), cap, off.ctypes.data]
+        check(getattr(lib, entry)(*args), entry)
         return status, node, _string_list(buf, off)
 
     def drain_nodes(self, node_names, pods, pod_offset, policy=capi.KS_SCORE_LEFTOVER, flags=0):

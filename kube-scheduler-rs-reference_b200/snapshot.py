@@ -80,6 +80,71 @@ def node_rules(rules):
     return nr, hold
 
 
+def _topology(keys, rows, max_skew, min_domains, existing, what):
+    """The ks_spread_multi of keys (a list of K (node_domain, n_domains) pairs) for `rows` specs or groups (`what`):
+    max_skew and min_domains [rows, K] or None, existing None or a list of K arrays [rows, n_domains_k].  Returns the
+    struct, the arrays it points into (keep them alive) and the K domain counts."""
+    k = len(keys)
+    if not 1 <= k <= capi.KS_SPREAD_MAX_KEYS:
+        raise ValueError(f"{k} topology keys (1 to {capi.KS_SPREAD_MAX_KEYS})")
+    doms = [_c(d, np.int32).reshape(-1) for d, _ in keys]
+    nd = [int(n) for _, n in keys]
+
+    def per_row(a, name):
+        if a is None:
+            return None
+        a = _c(a, np.uint32).reshape(-1)
+        if a.shape[0] != rows * k:
+            raise ValueError(f"{name} has {a.shape[0]} entries, {what} x keys {rows * k}")
+        return a
+    max_skew, min_domains = per_row(max_skew, "max_skew"), per_row(min_domains, "min_domains")
+    if existing is not None:
+        if len(existing) != k:
+            raise ValueError(f"existing has {len(existing)} blocks, keys {k}")
+        existing = _c(np.concatenate([np.asarray(e, np.uint32).reshape(rows, n) for e, n in zip(existing, nd)],
+                                     axis=1), np.uint32).reshape(-1)
+    spread = capi.ks_spread_multi(k, (C.c_uint32 * capi.KS_SPREAD_MAX_KEYS)(*nd),
+                                  (C.c_void_p * capi.KS_SPREAD_MAX_KEYS)(*[_ptr(d) for d in doms]),
+                                  _ptr(max_skew), _ptr(min_domains), _ptr(existing))
+    return spread, (doms, max_skew, min_domains, existing), nd
+
+
+def _counts(rows, nd, want):
+    """The output of per-domain counts [rows, sum(nd)], or None unless want and within KS_SPREAD_MAX_COUNTS"""
+    return np.empty((rows, sum(nd)), np.uint32) if want and 0 < rows * sum(nd) <= capi.KS_SPREAD_MAX_COUNTS else None
+
+
+def _split(counts, nd):
+    """counts [rows, sum(nd)] as a list of K arrays [rows, nd[k]], or None"""
+    return None if counts is None else np.split(counts, np.cumsum(nd)[:-1], axis=1)
+
+
+def _pod_affinity(terms, existing_pods):
+    """The ks_pod_affinity of terms (a list of (owner group, kind, key index, target groups)) and existing_pods (None
+    or (groups, nodes)), and the arrays it points into (keep them alive)."""
+    owner = _c([t[0] for t in terms], np.int32)
+    kind = _c([t[1] for t in terms], np.uint8)
+    key = _c([t[2] for t in terms], np.uint32)
+    toff = np.zeros(len(terms) + 1, np.uint64)
+    np.cumsum([len(t[3]) for t in terms], out=toff[1:])
+    target = _c(np.concatenate([np.asarray(t[3], np.int64).reshape(-1) for t in terms]) if terms else [], np.int32)
+    eg, en = (np.zeros(0, np.int32),) * 2 if existing_pods is None else existing_pods
+    eg, en = _c(eg, np.int32).reshape(-1), _c(en, np.int32).reshape(-1)
+    if eg.shape[0] != en.shape[0]:
+        raise ValueError(f"existing pods: {eg.shape[0]} groups, {en.shape[0]} nodes")
+    aff = capi.ks_pod_affinity(len(terms), _ptr(owner), _ptr(kind), _ptr(key), _ptr(toff), _ptr(target),
+                               eg.shape[0], _ptr(eg), _ptr(en))
+    return aff, (owner, kind, key, toff, target, eg, en)
+
+
+def _rules_arg(rules):
+    """The ks_node_rules argument of a rules dict (node_rules) or None (NULL), and what it points into"""
+    if rules is None:
+        return None, None
+    nr, hold = node_rules(rules)
+    return C.byref(nr), (nr, hold)
+
+
 @dataclass
 class SelectResult:
     node_idx: np.ndarray
@@ -363,36 +428,14 @@ class Snapshot:
         if t and (replicas.min() < 0 or replicas.max() > 0xFFFFFFFF):
             raise ValueError("replicas must lie in [0, 2^32)")
         replicas = _c(replicas, np.uint32)
-        k = len(keys)
-        if not 1 <= k <= capi.KS_SPREAD_MAX_KEYS:
-            raise ValueError(f"{k} topology keys (1 to {capi.KS_SPREAD_MAX_KEYS})")
-        doms = [_c(d, np.int32).reshape(-1) for d, _ in keys]
-        nd = [int(n) for _, n in keys]
-        max_skew = _c(max_skew, np.uint32).reshape(-1)
-        if max_skew.shape[0] != t * k:
-            raise ValueError(f"max_skew has {max_skew.shape[0]} entries, specs x keys {t * k}")
-        if min_domains is not None:
-            min_domains = _c(min_domains, np.uint32).reshape(-1)
-            if min_domains.shape[0] != t * k:
-                raise ValueError(f"min_domains has {min_domains.shape[0]} entries, specs x keys {t * k}")
-        s = sum(nd)
-        if existing is not None:
-            if len(existing) != k:
-                raise ValueError(f"existing has {len(existing)} blocks, keys {k}")
-            existing = _c(np.concatenate([np.asarray(e, np.uint32).reshape(t, n) for e, n in zip(existing, nd)],
-                                         axis=1), np.uint32).reshape(-1)
-        spread = capi.ks_spread_multi(k, (C.c_uint32 * capi.KS_SPREAD_MAX_KEYS)(*nd),
-                                      (C.c_void_p * capi.KS_SPREAD_MAX_KEYS)(*[_ptr(d) for d in doms]),
-                                      _ptr(max_skew), _ptr(min_domains), _ptr(existing))
+        spread, hold, nd = _topology(keys, t, max_skew, min_domains, existing, "specs")
         offset, _, node, score = replica_outputs(replicas, capi.SPREAD_PLAN_DTYPE, want_nodes)
-        rows = np.zeros((t, k), capi.SPREAD_PLAN_DTYPE)
-        counts = np.empty((t, s), np.uint32) if want_counts and 0 < t * s <= capi.KS_SPREAD_MAX_COUNTS else None
+        rows = np.zeros((t, len(keys)), capi.SPREAD_PLAN_DTYPE)
+        counts = _counts(t, nd, want_counts)
         check(lib.ks_place_replicas_spread_multi(self._h, C.byref(pods), _ptr(replicas), C.byref(spread), int(policy),
                                                  _ptr(rows), _ptr(node), _ptr(score), _ptr(counts)),
               "ks_place_replicas_spread_multi")
-        if counts is not None:
-            counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
-        return rows, node, score, offset, counts
+        return rows, node, score, offset, _split(counts, nd)
 
     def spread_bind(self, req_cpu, req_mem, sel, group, keys, max_skew, min_domains=None, existing=None,
                     policy=capi.KS_SCORE_LEFTOVER, want_counts=True):
@@ -406,35 +449,15 @@ class Snapshot:
         group = _c(group, np.int32).reshape(-1)
         if group.shape[0] != p:
             raise ValueError(f"group has {group.shape[0]} entries, pods {p}")
-        k = len(keys)
-        if not 1 <= k <= capi.KS_SPREAD_MAX_KEYS:
-            raise ValueError(f"{k} topology keys (1 to {capi.KS_SPREAD_MAX_KEYS})")
-        doms = [_c(d, np.int32).reshape(-1) for d, _ in keys]
-        nd = [int(n) for _, n in keys]
-        max_skew = _c(max_skew, np.uint32).reshape(-1, k)
-        g = max_skew.shape[0]
-        if min_domains is not None:
-            min_domains = _c(min_domains, np.uint32).reshape(-1)
-            if min_domains.shape[0] != g * k:
-                raise ValueError(f"min_domains has {min_domains.shape[0]} entries, groups x keys {g * k}")
-        s = sum(nd)
-        if existing is not None:
-            if len(existing) != k:
-                raise ValueError(f"existing has {len(existing)} blocks, keys {k}")
-            existing = _c(np.concatenate([np.asarray(e, np.uint32).reshape(g, n) for e, n in zip(existing, nd)],
-                                         axis=1), np.uint32).reshape(-1)
-        spread = capi.ks_spread_multi(k, (C.c_uint32 * capi.KS_SPREAD_MAX_KEYS)(*nd),
-                                      (C.c_void_p * capi.KS_SPREAD_MAX_KEYS)(*[_ptr(d) for d in doms]),
-                                      _ptr(max_skew), _ptr(min_domains), _ptr(existing))
+        g = _c(max_skew, np.uint32).reshape(-1, max(len(keys), 1)).shape[0]
+        spread, hold, nd = _topology(keys, g, max_skew, min_domains, existing, "groups")
         idx = np.empty(p, np.int32)
         score = np.empty(p, np.int64)
         refused = np.empty(p, np.uint32)
-        counts = np.empty((g, s), np.uint32) if want_counts and 0 < g * s <= capi.KS_SPREAD_MAX_COUNTS else None
+        counts = _counts(g, nd, want_counts)
         check(lib.ks_spread_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(spread), int(policy), _ptr(idx),
                                  _ptr(score), _ptr(refused), _ptr(counts)), "ks_spread_bind")
-        if counts is not None:
-            counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
-        return idx, score, refused, counts
+        return idx, score, refused, _split(counts, nd)
 
     def affinity_bind(self, req_cpu, req_mem, sel, group, n_groups, keys, terms=(), existing_pods=None, max_skew=None,
                       min_domains=None, existing=None, policy=capi.KS_SCORE_LEFTOVER, want_counts=True):
@@ -448,49 +471,15 @@ class Snapshot:
         group = _c(group, np.int32).reshape(-1)
         if group.shape[0] != p:
             raise ValueError(f"group has {group.shape[0]} entries, pods {p}")
-        k = len(keys)
-        if not 1 <= k <= capi.KS_SPREAD_MAX_KEYS:
-            raise ValueError(f"{k} topology keys (1 to {capi.KS_SPREAD_MAX_KEYS})")
-        doms = [_c(d, np.int32).reshape(-1) for d, _ in keys]
-        nd = [int(n) for _, n in keys]
-        if max_skew is not None:
-            max_skew = _c(max_skew, np.uint32).reshape(-1)
-            if max_skew.shape[0] != g * k:
-                raise ValueError(f"max_skew has {max_skew.shape[0]} entries, groups x keys {g * k}")
-        if min_domains is not None:
-            min_domains = _c(min_domains, np.uint32).reshape(-1)
-            if min_domains.shape[0] != g * k:
-                raise ValueError(f"min_domains has {min_domains.shape[0]} entries, groups x keys {g * k}")
-        s = sum(nd)
-        if existing is not None:
-            if len(existing) != k:
-                raise ValueError(f"existing has {len(existing)} blocks, keys {k}")
-            existing = _c(np.concatenate([np.asarray(e, np.uint32).reshape(g, n) for e, n in zip(existing, nd)],
-                                         axis=1), np.uint32).reshape(-1)
-        topo = capi.ks_spread_multi(k, (C.c_uint32 * capi.KS_SPREAD_MAX_KEYS)(*nd),
-                                    (C.c_void_p * capi.KS_SPREAD_MAX_KEYS)(*[_ptr(d) for d in doms]),
-                                    _ptr(max_skew), _ptr(min_domains), _ptr(existing))
-        owner = _c([t[0] for t in terms], np.int32)
-        kind = _c([t[1] for t in terms], np.uint8)
-        key = _c([t[2] for t in terms], np.uint32)
-        toff = np.zeros(len(terms) + 1, np.uint64)
-        np.cumsum([len(t[3]) for t in terms], out=toff[1:])
-        target = _c(np.concatenate([np.asarray(t[3], np.int64).reshape(-1) for t in terms]) if terms else [], np.int32)
-        eg, en = (np.zeros(0, np.int32),) * 2 if existing_pods is None else existing_pods
-        eg, en = _c(eg, np.int32).reshape(-1), _c(en, np.int32).reshape(-1)
-        if eg.shape[0] != en.shape[0]:
-            raise ValueError(f"existing pods: {eg.shape[0]} groups, {en.shape[0]} nodes")
-        aff = capi.ks_pod_affinity(len(terms), _ptr(owner), _ptr(kind), _ptr(key), _ptr(toff), _ptr(target),
-                                   eg.shape[0], _ptr(eg), _ptr(en))
+        topo, hold, nd = _topology(keys, g, max_skew, min_domains, existing, "groups")
+        aff, hold_aff = _pod_affinity(terms, existing_pods)
         idx = np.empty(p, np.int32)
         score = np.empty(p, np.int64)
         refused = np.empty((p, 2), np.uint32)
-        counts = np.empty((g, s), np.uint32) if want_counts and 0 < g * s <= capi.KS_SPREAD_MAX_COUNTS else None
+        counts = _counts(g, nd, want_counts)
         check(lib.ks_affinity_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff), int(policy),
                                    _ptr(idx), _ptr(score), _ptr(refused), _ptr(counts)), "ks_affinity_bind")
-        if counts is not None:
-            counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
-        return idx, score, refused, counts
+        return idx, score, refused, _split(counts, nd)
 
     def profile_bind(self, req_cpu, req_mem, sel, group, n_groups, keys, terms=(), existing_pods=None, max_skew=None,
                      min_domains=None, existing=None, policy=capi.KS_SCORE_LEAST_BALANCED, soft_skew=None,
@@ -501,9 +490,10 @@ class Snapshot:
         terms); soft_skew [G, K] or None (ScheduleAnyway maxSkew, 0 = none); soft_all_keys [G] or None (all 1).
         Charges free[].  Returns (node_idx int32 [P], score int64 [P], parts int64 [P, 3] (policy, pts, ipa),
         refused uint32 [P, 2], counts, soft_counts); both counts lists of K arrays [G, D_k], or None."""
-        return self._scored_bind(None, req_cpu, req_mem, sel, group, n_groups, keys, terms, existing_pods, max_skew,
-                                 min_domains, existing, policy, soft_skew, soft_all_keys, term_weight,
-                                 hard_affinity_weight, weight_spread, weight_affinity, want_counts)
+        return self._scored_bind("ks_profile_bind", (), (), (3, 2), req_cpu, req_mem, sel, group, n_groups, keys,
+                                 terms, existing_pods, max_skew, min_domains, existing, policy, soft_skew,
+                                 soft_all_keys, term_weight, hard_affinity_weight, weight_spread, weight_affinity,
+                                 want_counts)
 
     def node_bind(self, req_cpu, req_mem, sel, group, n_groups, keys, terms=(), existing_pods=None, max_skew=None,
                   min_domains=None, existing=None, policy=capi.KS_SCORE_LEAST_BALANCED, soft_skew=None,
@@ -515,10 +505,10 @@ class Snapshot:
         uint64), ...]); weight 0 = required), weight_taint (default 3) and weight_node_affinity (default 2); see
         node_set for the words.  Returns profile_bind's tuple with parts [P, 5] (policy, pts, ipa, tt, na) and refused
         [P, 4] (taint, node affinity, spread, inter-pod affinity)."""
-        return self._scored_bind(rules if rules is not None else False, req_cpu, req_mem, sel, group, n_groups, keys,
-                                 terms, existing_pods, max_skew, min_domains, existing, policy, soft_skew,
-                                 soft_all_keys, term_weight, hard_affinity_weight, weight_spread, weight_affinity,
-                                 want_counts)
+        nr, hold = _rules_arg(rules)
+        return self._scored_bind("ks_node_bind", (nr,), (), (5, 4), req_cpu, req_mem, sel, group, n_groups, keys, terms,
+                                 existing_pods, max_skew, min_domains, existing, policy, soft_skew, soft_all_keys,
+                                 term_weight, hard_affinity_weight, weight_spread, weight_affinity, want_counts)
 
     def fit_bind(self, req_cpu, req_mem, sel, group, n_groups, keys, terms=(), existing_pods=None, max_skew=None,
                  min_domains=None, existing=None, policy=capi.KS_SCORE_LEAST_BALANCED, soft_skew=None,
@@ -530,7 +520,7 @@ class Snapshot:
         then free_r int64 [R, N] after the call."""
         if (node_free is None) != (pod_req is None):
             raise ValueError("node_free and pod_req go together")
-        res = None
+        r, br = 0, None
         if node_free is not None:
             node_free = _c(node_free, np.int64)
             pod_req = _c(pod_req, np.int64)
@@ -540,11 +530,16 @@ class Snapshot:
             r = node_free.shape[0]
             if pod_req.shape != (p, r):
                 raise ValueError(f"pod_req has shape {pod_req.shape}, expected ({p}, {r})")
-            res = (r, node_free.reshape(-1), pod_req.reshape(-1))
-        return self._scored_bind(rules if rules is not None else False, req_cpu, req_mem, sel, group, n_groups, keys,
-                                 terms, existing_pods, max_skew, min_domains, existing, policy, soft_skew,
-                                 soft_all_keys, term_weight, hard_affinity_weight, weight_spread, weight_affinity,
-                                 want_counts, res=res, fit=True, gangs=_gangs)
+            br = capi.ks_bind_resources(r, _ptr(node_free), _ptr(pod_req))
+        nr, hold = _rules_arg(rules)
+        free_r = np.empty((r, self.n_nodes), np.int64)
+        entry, mid, outs = "ks_fit_bind", (nr, None if br is None else C.byref(br)), (_ptr(free_r),)
+        if _gangs is not None:  # gang_fit_bind's (ks_gangs, placed)
+            entry, mid, outs = "ks_gang_fit_bind", mid + (C.byref(_gangs[0]),), outs + (_ptr(_gangs[1]),)
+        return self._scored_bind(entry, mid, outs, (5, 5), req_cpu, req_mem, sel, group, n_groups, keys, terms,
+                                 existing_pods, max_skew, min_domains, existing, policy, soft_skew, soft_all_keys,
+                                 term_weight, hard_affinity_weight, weight_spread, weight_affinity,
+                                 want_counts) + (free_r,)
 
     def gang_fit_bind(self, req_cpu, req_mem, sel, group, n_groups, keys, offset, min_member, terms=(),
                       existing_pods=None, max_skew=None, min_domains=None, existing=None,
@@ -568,21 +563,18 @@ class Snapshot:
                              weight_spread, weight_affinity, rules, node_free, pod_req, want_counts,
                              _gangs=(gangs, placed)) + (placed,)
 
-    def _scored_bind(self, rules, req_cpu, req_mem, sel, group, n_groups, keys, terms, existing_pods, max_skew,
-                     min_domains, existing, policy, soft_skew, soft_all_keys, term_weight, hard_affinity_weight,
-                     weight_spread, weight_affinity, want_counts, res=None, fit=False, gangs=None):
-        """ks_profile_bind when rules is None, else ks_node_bind (rules False = its NULL rules); with fit, ks_fit_bind
-        with res = (R, node_free, pod_req) or None, and with gangs = (ks_gangs, placed) ks_gang_fit_bind."""
+    def _scored_bind(self, entry, mid, outs, widths, req_cpu, req_mem, sel, group, n_groups, keys, terms,
+                     existing_pods, max_skew, min_domains, existing, policy, soft_skew, soft_all_keys, term_weight,
+                     hard_affinity_weight, weight_spread, weight_affinity, want_counts):
+        """The C call `entry` with its scoring, then mid (rules, resources, gangs), the policy, the six outputs every
+        scored bind returns (parts and refused of widths words per pod) and outs"""
         pods, keep = self._pods(req_cpu, req_mem, sel)
         p, g = int(pods.n), int(n_groups)
         group = _c(group, np.int32).reshape(-1)
         if group.shape[0] != p:
             raise ValueError(f"group has {group.shape[0]} entries, pods {p}")
-        k = len(keys)
-        if not 1 <= k <= capi.KS_SPREAD_MAX_KEYS:
-            raise ValueError(f"{k} topology keys (1 to {capi.KS_SPREAD_MAX_KEYS})")
-        doms = [_c(d, np.int32).reshape(-1) for d, _ in keys]
-        nd = [int(n) for _, n in keys]
+        topo, hold, nd = _topology(keys, g, max_skew, min_domains, existing, "groups")
+        aff, hold_aff = _pod_affinity(terms, existing_pods)
 
         def per_group(a, dtype, width, name):
             if a is None:
@@ -591,76 +583,23 @@ class Snapshot:
             if a.shape[0] != g * width:
                 raise ValueError(f"{name} has {a.shape[0]} entries, expected {g * width}")
             return a
-        max_skew = per_group(max_skew, np.uint32, k, "max_skew")
-        min_domains = per_group(min_domains, np.uint32, k, "min_domains")
-        soft_skew = per_group(soft_skew, np.uint32, k, "soft_skew")
+        soft_skew = per_group(soft_skew, np.uint32, len(keys), "soft_skew")
         soft_all_keys = per_group(soft_all_keys, np.uint8, 1, "soft_all_keys")
-        s = sum(nd)
-        if existing is not None:
-            if len(existing) != k:
-                raise ValueError(f"existing has {len(existing)} blocks, keys {k}")
-            existing = _c(np.concatenate([np.asarray(e, np.uint32).reshape(g, n) for e, n in zip(existing, nd)],
-                                         axis=1), np.uint32).reshape(-1)
-        topo = capi.ks_spread_multi(k, (C.c_uint32 * capi.KS_SPREAD_MAX_KEYS)(*nd),
-                                    (C.c_void_p * capi.KS_SPREAD_MAX_KEYS)(*[_ptr(d) for d in doms]),
-                                    _ptr(max_skew), _ptr(min_domains), _ptr(existing))
-        owner = _c([t[0] for t in terms], np.int32)
-        kind = _c([t[1] for t in terms], np.uint8)
-        key = _c([t[2] for t in terms], np.uint32)
-        toff = np.zeros(len(terms) + 1, np.uint64)
-        np.cumsum([len(t[3]) for t in terms], out=toff[1:])
-        target = _c(np.concatenate([np.asarray(t[3], np.int64).reshape(-1) for t in terms]) if terms else [], np.int32)
         if term_weight is not None:
             term_weight = _c(term_weight, np.uint32).reshape(-1)
             if term_weight.shape[0] != len(terms):
                 raise ValueError(f"term_weight has {term_weight.shape[0]} entries, terms {len(terms)}")
-        eg, en = (np.zeros(0, np.int32),) * 2 if existing_pods is None else existing_pods
-        eg, en = _c(eg, np.int32).reshape(-1), _c(en, np.int32).reshape(-1)
-        if eg.shape[0] != en.shape[0]:
-            raise ValueError(f"existing pods: {eg.shape[0]} groups, {en.shape[0]} nodes")
-        aff = capi.ks_pod_affinity(len(terms), _ptr(owner), _ptr(kind), _ptr(key), _ptr(toff), _ptr(target),
-                                   eg.shape[0], _ptr(eg), _ptr(en))
         scoring = capi.ks_bind_scoring(_ptr(soft_skew), _ptr(soft_all_keys), _ptr(term_weight),
                                        int(hard_affinity_weight), int(weight_spread), int(weight_affinity))
         idx = np.empty(p, np.int32)
         score = np.empty(p, np.int64)
-        parts = np.empty((p, 3 if rules is None else 5), np.int64)
-        refused = np.empty((p, 5 if fit else 2 if rules is None else 4), np.uint32)
-        want = want_counts and 0 < g * s <= capi.KS_SPREAD_MAX_COUNTS
-        counts = np.empty((g, s), np.uint32) if want else None
-        soft = np.empty((g, s), np.uint32) if want else None
-        if fit:
-            nr, hold = node_rules(rules) if rules is not False else (None, None)
-            r = res[0] if res is not None else 0
-            br = capi.ks_bind_resources(r, _ptr(res[1]), _ptr(res[2])) if res is not None else None
-            free_r = np.empty((r, self.n_nodes), np.int64)
-            if gangs is not None:
-                check(lib.ks_gang_fit_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
-                                           C.byref(scoring), C.byref(nr) if nr is not None else None,
-                                           C.byref(br) if br is not None else None, C.byref(gangs[0]), int(policy),
-                                           _ptr(idx), _ptr(score), _ptr(parts), _ptr(refused), _ptr(counts),
-                                           _ptr(soft), _ptr(free_r), _ptr(gangs[1])), "ks_gang_fit_bind")
-            else:
-                check(lib.ks_fit_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
-                                      C.byref(scoring), C.byref(nr) if nr is not None else None,
-                                      C.byref(br) if br is not None else None, int(policy), _ptr(idx), _ptr(score),
-                                      _ptr(parts), _ptr(refused), _ptr(counts), _ptr(soft), _ptr(free_r)),
-                      "ks_fit_bind")
-        elif rules is None:
-            check(lib.ks_profile_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
-                                      C.byref(scoring), int(policy), _ptr(idx), _ptr(score), _ptr(parts),
-                                      _ptr(refused), _ptr(counts), _ptr(soft)), "ks_profile_bind")
-        else:
-            nr, hold = node_rules(rules) if rules is not False else (None, None)
-            check(lib.ks_node_bind(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
-                                   C.byref(scoring), C.byref(nr) if nr is not None else None, int(policy), _ptr(idx),
-                                   _ptr(score), _ptr(parts), _ptr(refused), _ptr(counts), _ptr(soft)), "ks_node_bind")
-        if want:
-            counts = np.split(counts, np.cumsum(nd)[:-1], axis=1)
-            soft = np.split(soft, np.cumsum(nd)[:-1], axis=1)
-        if fit:
-            return idx, score, parts, refused, counts, soft, free_r
-        return idx, score, parts, refused, counts, soft
+        parts = np.empty((p, widths[0]), np.int64)
+        refused = np.empty((p, widths[1]), np.uint32)
+        counts, soft = _counts(g, nd, want_counts), _counts(g, nd, want_counts)
+        check(getattr(lib, entry)(self._h, C.byref(pods), _ptr(group), g, C.byref(topo), C.byref(aff),
+                                  C.byref(scoring), *mid, int(policy), _ptr(idx), _ptr(score), _ptr(parts),
+                                  _ptr(refused), _ptr(counts), _ptr(soft), *outs), entry)
+        return idx, score, parts, refused, _split(counts, nd), _split(soft, nd)
 
     def select_sampling(self, req_cpu, req_mem, sel, attempts=capi.KS_REFERENCE_ATTEMPTS, seed=0, first_pod_index=0):
         """The reference's own policy (src/main.rs:49-71), seeded: (node_idx, attempts_used, draw_node, draw_code)."""

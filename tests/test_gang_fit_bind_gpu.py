@@ -70,13 +70,15 @@ def run_fit(ks, snap, nodes, queue, kw, pods=None):
 
 
 # ------------------------------------------------------------------------------------------- 1. against the restatement
-CASES = [(1, 1, (1,), 3, 24), (2, 129, (3, "host"), 4, 60), (4, 2100, (3, "host"), 5, 60), (8, 16897, (3,), 4, 30)]
+# the last flag adds existing pods and soft_all_keys, so that the call stages every array it can take
+CASES = [(1, 1, (1,), 3, 24, False), (2, 129, (3, "host"), 4, 60, False), (4, 2100, (3, "host"), 5, 60, True),
+         (8, 16897, (3,), 4, 30, False)]
 
 
 @pytest.mark.parametrize("policy", POLICIES)
 @pytest.mark.parametrize("case", CASES, ids=[f"W{c[0]}-N{c[1]}" for c in CASES])
 def test_against_the_oracle(ks, case, policy):
-    W, N, modes, G, P = case
+    W, N, modes, G, P, every_array = case
     rng = np.random.default_rng([W, N, policy, 0x6A6F])
     fc, fm, ac, am, lab = _nodes(rng, N, W)
     keys = key_set(rng, N, modes)
@@ -92,16 +94,22 @@ def test_against_the_oracle(ks, case, policy):
     rc = rc.copy()
     rc[int(offset[1]) - 1] = 1 << 36  # gang 0's last pod fits no node and gang 0 needs every pod: it rolls back
     mm[0] = int(offset[1])
+    existing_pods = soft_all = None
+    if every_array:
+        existing_pods = (rng.integers(0, G, 40).astype(np.int32), rng.integers(0, N, 40).astype(np.int32))
+        soft_all = rng.integers(0, 2, G).astype(np.uint8)
+    rules = compile_rules(nl, nt, gr)
     with ks.Snapshot(0) as snap:
         load(ks, snap, fc, fm, ac, am, lab)
-        got = snap.gang_fit_bind(rc, rm, sel, group, G, keys, offset, mm, terms, None, skew, mind, ex, policy,
-                                 soft_skew=soft, term_weight=[0, 0, 40], rules=compile_rules(nl, nt, gr),
+        got = snap.gang_fit_bind(rc, rm, sel, group, G, keys, offset, mm, terms, existing_pods, skew, mind, ex, policy,
+                                 soft_skew=soft, soft_all_keys=soft_all, term_weight=[0, 0, 40], rules=rules,
                                  node_free=free0, pod_req=req)
         gfc, gfm = snap.free()
     ofc, ofm = fc.copy(), fm.copy()
     want = gang_fit_bind_packed(ofc, ofm, ac, am, lab, rc, rm, sel, group, G, keys, nl, nt, gr, alloc, bound, pod_res,
-                                offset, mm, terms=terms, max_skew=skew, min_domains=mind, existing=ex, policy=policy,
-                                soft_skew=soft, term_weight=[0, 0, 40])
+                                offset, mm, terms=terms, existing_pods=existing_pods, max_skew=skew, min_domains=mind,
+                                existing=ex, policy=policy, soft_skew=soft, soft_all_keys=soft_all,
+                                term_weight=[0, 0, 40])
     for i in range(4):
         assert np.array_equal(got[i], want[i]), i
     for i in (4, 5):
@@ -110,6 +118,8 @@ def test_against_the_oracle(ks, case, policy):
     assert np.array_equal(gfc, ofc) and np.array_equal(gfm, ofm)
     if N > 100:
         assert (want[7] < mm).any() and (want[7] >= mm).any() and (got[0] >= 0).any()
+    if every_array:  # both taint masks and a node-affinity expression as well
+        assert rules["taint_hard"].any() and rules["taint_soft"].any() and any(t[2] for t in rules["node_terms"])
 
 
 @pytest.mark.parametrize("case", GOLDEN, ids=[c["name"] for c in GOLDEN])
