@@ -392,6 +392,11 @@ extern "C" {
                             rules: *const ks_node_rules, res: *const ks_bind_resources, gangs: *const ks_gangs,
                             policy: c_int, node_idx: *mut i32, score: *mut i64, parts: *mut i64, refused: *mut u32,
                             domain_count: *mut u32, soft_count: *mut u32, free: *mut i64, placed: *mut u32) -> c_int;
+    // ks_preempt under the full filter: pod count, scalar resources, taints and required node affinity (DESIGN.md 5t)
+    pub fn ks_fit_preempt(s: *mut ks_snapshot, pods: *const ks_pods, group: *const i32, n_groups: u32,
+                          rules: *const ks_node_rules, res: *const ks_bind_resources, pod_priority: *const i32,
+                          bound: *const ks_bound_pods, bound_req: *const i64, max_victims: u32,
+                          out: *mut ks_preemption, out_victims: *mut i32, out_unresolvable: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -493,6 +498,11 @@ extern "C" {
                                    rules: *const ksh_node_rules, gang_offset: *const u64, n_gangs: u64,
                                    min_member: *const u32, policy: c_int, status: *mut i32, node_idx: *mut i32,
                                    placed: *mut u32, json: *mut c_char, cap: usize, json_off: *mut i64) -> c_int;
+    // ksh_preempt_pods under the full filter: taints, node affinity, extended resources and the pod limit (DESIGN.md 5t)
+    pub fn ksh_preempt_fit_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group: *const i32,
+                                n_groups: u32, rules: *const ksh_node_rules, pod_priority: *const i32,
+                                max_victims: u32, out: *mut ks_preemption, victims: *mut c_char, cap: usize,
+                                out_victim_off: *mut i64) -> c_int;
     pub fn ksh_reconcile_profile(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, group: *const i32,
                                  n_groups: u32, topology_keys: *const *const c_char, n_keys: u32, max_skew: *const u32,
                                  min_domains: *const u32, existing_node_names: *const *const c_char,

@@ -377,6 +377,59 @@ typedef struct ks_preemption { /* 32 bytes per pod */
 int ks_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* pod_priority, const ks_bound_pods* bound,
                uint32_t max_victims, ks_preemption* out, int32_t* out_victims, int32_t out_space, void* cuda_stream);
 
+/* ---- preemption under the full filter: ks_preempt with the pod count, scalar resources, taints and required node
+ * affinity (upstream DefaultPreemption re-running NodeResourcesFit, TaintToleration and NodeAffinity with the victims
+ * removed; spec extension, DESIGN.md 5t) ----
+ * `group`, `rules` and `res` mean what they mean for ks_fit_bind (below): pod p belongs to group[p] in [-1, n_groups),
+ * group -1 tolerates nothing and has no node affinity; res->node_free[r * N + n] is allocatable minus the bound pods'
+ * bound_req, res->pod_req[p * R + r] >= 0.  bound_req[b * R + r] (host memory) is bound pod b's request of resource r,
+ * >= 0 (1 for the pod-count resource).  The caller keeps these consistent, as ks_preempt requires of free[]: `bound` is
+ * the list that produced free[] and node_free is allocatable minus the bound pods' bound_req.  "p fits n" is ks_fit_bind's
+ * resource rule: cpu and memory without a zero skip, each r with upstream's (pod_req 0 always fits).  For pod p, real
+ * node n:
+ *   1. unresolvable: n fails p's selector, carries a hard taint p's group does not tolerate, or fails the group's
+ *      required node affinity; no eviction helps and n is never eligible.  out_unresolvable[p] counts these nodes;
+ *   2. eligible: n is resolvable and p does not fit n;
+ *   3. L = the pods on n with priority strictly below pi_p; empty L: not a candidate.  For every dimension x (cpu,
+ *      memory, each r) avail_x = free_x[n] + sum of req_b,x over L; unless p fits avail: not a candidate;
+ *   4. reprieve: L in ks_preempt's order (priority descending, ties to the lower bound index); b is reprieved when p
+ *      still fits avail - req_b in every dimension (then avail -= req_b), else it is a victim.  Evicting a victim frees
+ *      its pod-count 1 like any other request;
+ *   5. steps 5-7 of ks_preempt unchanged: more than max_victims victims is no candidate, the 128-bit node order picks the
+ *      plan's node, and feasible_cnt - the resolvable nodes p fits with no eviction - above 0 gives no plan.
+ * Rows as ks_preemption; out_victims[p * max_victims ..] bound indices in visit order, -1 past n_victims.  Nothing is
+ * charged and the snapshot does not change.  rules->weight_* and preferred terms are checked as ks_node_bind checks them
+ * and play no part: preemption does not score.
+ * Identities:
+ *   (Q1) rules NULL and res NULL: out and out_victims are ks_preempt's, bit for bit, and out_unresolvable[p] is the
+ *        number of nodes whose labels miss p's selector;
+ *   (Q2) an extra resource that copies cpu (pod_req each pod's positive cpu request, node_free free_cpu, bound_req the
+ *        bound cpu) changes nothing;
+ *   (Q3) feasible_cnt[p] = ks_select's feasible count minus ks_fit_bind's refusal words 0-2 for p bound alone with no
+ *        spread or affinity;
+ *   (Q4) evict then bind: with a plan's victims removed (node_free raised by their bound_req, free[] by their requests)
+ *        the pod passes the full filter on the planned node, and a second call reports feasible_cnt > 0 for it;
+ *   (Q5) returning any single victim makes the pod fail the planned node again.
+ * Checked on the host before any device work: every check of ks_preempt on `bound` and max_victims (including the
+ * 2^62 rule); ks_fit_bind's checks on group (KS_ERR_INVALID for a NULL group with P > 0 or one outside [-1, G),
+ * KS_ERR_RANGE for G > KS_SPREAD_BIND_MAX_GROUPS), rules and res; KS_ERR_INVALID for device-space pods, a NULL
+ * pod_priority or out (P > 0), or a NULL bound_req with R > 0 and B > 0; KS_ERR_RANGE for a negative bound_req, or for
+ * a (r, n) with |node_free[r * N + n]| + the sum of bound_req over n's bound pods above 2^62 (this keeps every sum of
+ * the walk inside int64).  pods->n = 0 does nothing; an empty snapshot gives every pod no plan and 0 unresolvable nodes.
+ * One H2D copy of the host arrays, the bound list and bound_req copied into the victim index's scratch, then
+ * k_node_rules_setup (ks_node_bind's rule words), the victim index with R request columns, the scan over node tiles,
+ * the emit, and one D2H copy; the call returns after completion.
+ * Out of scope: PodTopologySpread and InterPodAffinity with the victims removed (upstream re-runs them; they are not
+ * inputs here); PodDisruptionBudgets, pod start time, preemptionPolicy, nominatedNodeName; preemption for a gang. */
+struct ks_node_rules;     /* defined with ks_node_bind below */
+struct ks_bind_resources; /* defined with ks_fit_bind below */
+int ks_fit_preempt(ks_snapshot* s, const ks_pods* pods /* host space */, const int32_t* group /* [P] */,
+                   uint32_t n_groups, const struct ks_node_rules* rules /* or NULL */,
+                   const struct ks_bind_resources* res /* or NULL */, const int32_t* pod_priority /* [P] */,
+                   const ks_bound_pods* bound, const int64_t* bound_req /* [B * R], NULL when R = 0 */,
+                   uint32_t max_victims, ks_preemption* out /* [P] */, int32_t* out_victims /* [P * max_victims] or NULL */,
+                   uint32_t* out_unresolvable /* [P] or NULL */);
+
 /* ---- drain simulation: if a node were removed, where would its pods go (cluster-autoscaler's scale-down simulation,
  * Karpenter consolidation, the descheduler; spec extension, DESIGN.md 5f) ----
  * Candidate d is node node_idx[d] (duplicates allowed) and owns pods [offset[d], offset[d+1]) of `pods`, in the caller's

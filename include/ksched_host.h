@@ -443,6 +443,19 @@ int ksh_reconcile_fit_gangs(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n
                             const uint32_t* min_member, int policy, int32_t* out_status, int32_t* out_node_idx,
                             uint32_t* out_placed, char* json, size_t cap, int64_t* out_json_off);
 
+/* Priority preemption under the full filter over objects (ks_fit_preempt, DESIGN.md 5t): ksh_preempt_pods' arguments
+ * plus group[n_pods] in [-1, n_groups) and rules (NULL allowed), as ksh_reconcile_nodes takes them.  The context's node
+ * taints and the rules' tolerations and node-affinity terms are compiled as ksh_reconcile_nodes compiles them; the
+ * batch's resources are built as ksh_compile_resources builds them over `pods`, and each bound pod's bound_req from its
+ * recorded extended requests, 1 for "pods".  Bound pods without namespace and name are passed at priority INT32_MAX and
+ * are never victims; victim keys are written as ksh_preempt_pods writes them.  A malformed quantity of a requested
+ * resource is reported as ksh_reconcile_fit reports it (KS_ERR_PARSE or KS_ERR_RANGE, naming the node or pod).  Nothing
+ * is charged.  KS_ERR_RANGE for max_victims outside [1, KS_PREEMPT_MAX_VICTIMS]; KS_ERR_NO_DEVICE on a packing-only
+ * context. */
+int ksh_preempt_fit_pods(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_pods, const int32_t* group,
+                         uint32_t n_groups, const ksh_node_rules* rules /* or NULL */, const int32_t* pod_priority,
+                         uint32_t max_victims, ks_preemption* out, char* victims, size_t cap, int64_t* out_victim_off);
+
 #ifdef __cplusplus
 }
 #endif

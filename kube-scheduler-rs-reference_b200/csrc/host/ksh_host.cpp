@@ -40,6 +40,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 #pragma weak ks_node_bind
 #pragma weak ks_fit_bind
 #pragma weak ks_gang_fit_bind
+#pragma weak ks_fit_preempt
 
 namespace {
 
@@ -2460,6 +2461,62 @@ int ksh_reconcile_fit_gangs(ksh_context* c, const ks_pod_obj* pods, uint64_t n, 
     return reconcile_spread(c, pods, n, group, n_groups, topology_keys, K, max_skew, min_domains, existing_node_names,
                             existing_offset, aff ? aff : &none, policy, out_status, out_node_idx, json, cap,
                             out_json_off, {RM_FIT_GANGS, scoring, rules, gang_offset, n_gangs, min_member, out_placed});
+}
+KSH_CATCH
+
+int ksh_preempt_fit_pods(ksh_context* c, const ks_pod_obj* pods, uint64_t n, const int32_t* group, uint32_t n_groups,
+                         const ksh_node_rules* rules, const int32_t* pod_priority, uint32_t max_victims,
+                         ks_preemption* out, char* victims, size_t cap, int64_t* out_victim_off) try {
+    if (!c || (n && (!pods || !group || !pod_priority || !out))) return fail(KS_ERR_INVALID, "NULL argument");
+    if (max_victims == 0 || max_victims > KS_PREEMPT_MAX_VICTIMS)
+        return fail(KS_ERR_RANGE, "max_victims must be in [1, " + std::to_string(KS_PREEMPT_MAX_VICTIMS) + "]");
+    for (uint64_t i = 0; i < n; i++)
+        if (group[i] < -1 || group[i] >= (int64_t)n_groups)
+            return fail(KS_ERR_INVALID, "pod " + std::to_string(i) + ": group outside [-1, n_groups)");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    int rc = device_ready(c, ks_fit_preempt, "ks_fit_preempt");
+    if (rc) return rc;
+    if (out_victim_off)
+        for (uint64_t i = 0; i < n; i++) out_victim_off[i] = -1;
+    CompiledNodeRules cr;
+    rc = compile_node_rules(c, n_groups, rules, &cr);
+    if (rc || n == 0) return rc;
+    CompiledResources res;
+    rc = compile_resources(c, pods, n, &res);
+    if (rc) return rc;
+    ks_pods kp;
+    rc = pack_batch(c, pods, n, &kp); // after this the device's free[] comes from the bound rows below
+    if (rc) return rc;
+    const size_t B = c->bnode.size(), R = res.ids.size();
+    std::vector<int32_t> col(c->res_name.size(), -1);
+    for (size_t r = 0; r < R; r++) col[res.ids[r]] = (int32_t)r;
+    std::vector<int32_t> prio(B);
+    std::vector<int64_t> breq(B * R, 0);
+    for (size_t b = 0; b < B; b++) {
+        prio[b] = c->blen[b] ? c->bprio[b] : INT32_MAX; // anonymous: cannot be evicted
+        breq[b * R] = 1;
+        for (const ExtQty& e : c->bext[b]) // malformed requested quantities were reported by compile_resources
+            if (e.res < col.size() && col[e.res] > 0) breq[b * R + (size_t)col[e.res]] = e.v;
+    }
+    std::vector<int32_t> vic((size_t)n * max_victims);
+    const ks_bound_pods kb{B, c->bnode.data(), c->bcpu.data(), c->bmem.data(), prio.data()};
+    const ks_bind_resources br{(uint32_t)R, res.node_free.data(), res.pod_req.data()};
+    rc = ks_fit_preempt(c->snap, &kp, group, n_groups, &cr.r, &br, pod_priority, &kb, breq.data(), max_victims, out,
+                        vic.data(), nullptr);
+    if (rc || !victims || !out_victim_off) return rc;
+    StringList list{victims, cap};
+    std::string keys;
+    for (uint64_t i = 0; i < n; i++) {
+        if (out[i].node_idx < 0) continue;
+        keys.clear();
+        for (uint32_t j = 0; j < out[i].n_victims; j++) { // "namespace/name", NUL-terminated, in visit order
+            const size_t b = (size_t)vic[(size_t)i * max_victims + j];
+            keys.append(c->bkeys.data() + c->boff[b], c->blen[b]);
+            keys.push_back('\0');
+        }
+        out_victim_off[i] = list.append(keys.data(), keys.size());
+    }
+    return KS_OK;
 }
 KSH_CATCH
 

@@ -2234,6 +2234,54 @@ static int plan_bind(const ks_snapshot* s, const BindRequest& r, BindPlan* pl) {
     return rc;
 }
 
+// The staging of compiled node rules (NodeRulesPlan) for k_node_rules_setup, on a caller's HostStaged plan: the classes,
+// the rule keys' domains, the taints and the sets, and one rule word per (class, node) in d_work.  With rules NULL every
+// array is empty.  place() fills the arrays converted or defaulted in place and sets the NODE fields of ProfileBindArgs
+// that k_node_rules_setup reads, and rules_grid; the caller sets q.b.N.
+struct NodeRulesStage {
+    HostStaged& h;
+    const ks_node_rules* rules;
+    const NodeRulesPlan& pl;
+    const uint32_t N;
+    const uint64_t NR = rules ? 1 : 0;
+    Staged<uint32_t> ncls = h.in(pl.cls.data(), pl.cls.size());
+    Staged<uint64_t> ctol = h.in(pl.ctol.data(), pl.ctol.size());
+    Staged<uint32_t> cterm_off = h.in(pl.cterm_off.data(), NR * pl.cterm_off.size());
+    Staged<uint32_t> cterm_w = h.in(pl.cterm_w.data(), pl.cterm_w.size());
+    Staged<uint32_t> cexpr_off = h.in(pl.cexpr_off.data(), NR * pl.cexpr_off.size());
+    Staged<uint32_t> cexpr_key = h.in(pl.cexpr_key.data(), pl.cexpr_key.size());
+    Staged<uint64_t> cexpr_set = h.in(pl.cexpr_set.data(), pl.cexpr_set.size());
+    Staged<uint64_t> nset = h.in(rules ? rules->expr_set : nullptr, pl.set_words);
+    Staged<int32_t> ndom = h.in<int32_t>(nullptr, (uint64_t)(rules ? rules->n_keys : 0) * N);
+    Staged<uint64_t> taint_hard = h.in(rules ? rules->node_taint_hard : nullptr, NR * N);
+    Staged<uint64_t> taint_soft = h.in(rules ? rules->node_taint_soft : nullptr, NR * N);
+    Staged<uint32_t> nrules = h.work<uint32_t>((uint64_t)pl.C * N);
+
+    void place(ProfileBindArgs& q, int sms) const {
+        const uint32_t KN = rules->n_keys;
+        for (uint32_t k = 0; k < KN; k++) memcpy(h.host(ndom) + (size_t)k * N, rules->node_domain[k], (size_t)N * 4);
+        if (!rules->node_taint_hard) memset(h.host(taint_hard), 0, (size_t)N * 8);
+        if (!rules->node_taint_soft) memset(h.host(taint_soft), 0, (size_t)N * 8);
+        q.ncls = h.dev(ncls);
+        q.nrules = h.dev(nrules);
+        q.C = pl.C;
+        q.KN = KN;
+        for (uint32_t k = 0; k < KN; k++) q.NDk[k] = rules->n_domains[k];
+        q.ndom = h.dev(ndom);
+        q.taint_hard = h.dev(taint_hard);
+        q.taint_soft = h.dev(taint_soft);
+        q.ctol = h.dev(ctol);
+        q.cterm_off = h.dev(cterm_off);
+        q.cterm_w = h.dev(cterm_w);
+        q.cexpr_off = h.dev(cexpr_off);
+        q.cexpr_key = h.dev(cexpr_key);
+        q.cexpr_set = h.dev(cexpr_set);
+        q.nset = h.dev(nset);
+        q.rules_grid =
+            (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)q.C * N + 255) / 256, 4ull * (uint64_t)sms));
+    }
+};
+
 // The staging of a bind call (ProfileBindArgs, ks_launch.h).  Building it declares every array on h in member order,
 // feature by feature, with no element for a feature the mode does not read; after HostStaged::reserve(), place() fills
 // the arrays converted or defaulted in place and points the kernel's fields at the staged arrays, in the same order.
@@ -2289,19 +2337,8 @@ struct BindStage {
     Staged<uint32_t> pdom = h.work<uint32_t>(Q * CTA * KS_SPREAD_MAX_KEYS), plack = h.work<uint32_t>(Q * CTA);
     Staged<int64_t> pimin = h.work<int64_t>(Q * CTA), pimax = h.work<int64_t>(Q * CTA);
     Staged<int64_t> ppmin = h.work<int64_t>(Q * CTA), ppmax = h.work<int64_t>(Q * CTA);
-    // NODE on: the compiled classes, the rule keys' domains, the taints and the sets; one rule word per (class, node)
-    Staged<uint32_t> ncls = h.in(pl.rules.cls.data(), pl.rules.cls.size());
-    Staged<uint64_t> ctol = h.in(pl.rules.ctol.data(), pl.rules.ctol.size());
-    Staged<uint32_t> cterm_off = h.in(pl.rules.cterm_off.data(), NR * pl.rules.cterm_off.size());
-    Staged<uint32_t> cterm_w = h.in(pl.rules.cterm_w.data(), pl.rules.cterm_w.size());
-    Staged<uint32_t> cexpr_off = h.in(pl.rules.cexpr_off.data(), NR * pl.rules.cexpr_off.size());
-    Staged<uint32_t> cexpr_key = h.in(pl.rules.cexpr_key.data(), pl.rules.cexpr_key.size());
-    Staged<uint64_t> cexpr_set = h.in(pl.rules.cexpr_set.data(), pl.rules.cexpr_set.size());
-    Staged<uint64_t> nset = h.in(r.rules ? r.rules->expr_set : nullptr, pl.rules.set_words);
-    Staged<int32_t> ndom = h.in<int32_t>(nullptr, (r.rules ? r.rules->n_keys : 0) * N);
-    Staged<uint64_t> taint_hard = h.in(r.rules ? r.rules->node_taint_hard : nullptr, NR * N);
-    Staged<uint64_t> taint_soft = h.in(r.rules ? r.rules->node_taint_soft : nullptr, NR * N);
-    Staged<uint32_t> nrules = h.work<uint32_t>(pl.rules.C * N);
+    // NODE on: the compiled classes and their rule words
+    NodeRulesStage rs{h, r.rules, pl.rules, (uint32_t)N};
     Staged<uint32_t> ptref = h.work<uint32_t>(NR * CTA), pnref = h.work<uint32_t>(NR * CTA);
     Staged<uint32_t> ptmax = h.work<uint32_t>(NR * CTA), pnmax = h.work<uint32_t>(NR * CTA);
     // FIT on: the requests, the caller's free amounts and the charged ones, one row per resource
@@ -2387,33 +2424,13 @@ struct BindStage {
             q.waff = sc->weight_affinity;
         }
         if (const ks_node_rules* nr = r.rules) {
-            const uint32_t KN = nr->n_keys;
-            for (uint32_t k = 0; k < KN; k++) memcpy(h.host(ndom) + (size_t)k * N, nr->node_domain[k], (size_t)N * 4);
-            if (!nr->node_taint_hard) memset(h.host(taint_hard), 0, (size_t)N * 8);
-            if (!nr->node_taint_soft) memset(h.host(taint_soft), 0, (size_t)N * 8);
-            q.ncls = h.dev(ncls);
-            q.nrules = h.dev(nrules);
-            q.C = pl.rules.C;
-            q.KN = KN;
-            for (uint32_t k = 0; k < KN; k++) q.NDk[k] = nr->n_domains[k];
-            q.ndom = h.dev(ndom);
-            q.taint_hard = h.dev(taint_hard);
-            q.taint_soft = h.dev(taint_soft);
-            q.ctol = h.dev(ctol);
-            q.cterm_off = h.dev(cterm_off);
-            q.cterm_w = h.dev(cterm_w);
-            q.cexpr_off = h.dev(cexpr_off);
-            q.cexpr_key = h.dev(cexpr_key);
-            q.cexpr_set = h.dev(cexpr_set);
-            q.nset = h.dev(nset);
+            rs.place(q, s->sms);
             q.ptref = h.dev(ptref);
             q.pnref = h.dev(pnref);
             q.ptmax = h.dev(ptmax);
             q.pnmax = h.dev(pnmax);
             q.wtaint = nr->weight_taint;
             q.wnaff = nr->weight_node_affinity;
-            q.rules_grid = (uint32_t)std::max<uint64_t>(
-                1, std::min<uint64_t>(((uint64_t)q.C * N + 255) / 256, 4ull * (uint64_t)s->sms));
         }
         if (r.res) {
             q.R = (uint32_t)RS;
@@ -2609,6 +2626,135 @@ int ks_gang_fit_bind(ks_snapshot* s, const ks_pods* pods, const int32_t* group, 
                         {out_node_idx, out_score, out_refused, out_domain_count, out_parts, out_soft_count, out_free,
                          out_placed},
                         aff, scoring, rules, res, gangs});
+}
+
+// ks_fit_preempt's bound requests against node_free (include/ksched.h): each >= 0, and per (r, n) |node_free| plus the
+// sum over n's bound pods at most 2^62
+static int check_fit_preempt_bound(const ks_snapshot* s, const ks_bound_pods* bound, const int64_t* bound_req,
+                                   const ks_bind_resources* res) {
+    const uint64_t B = bound->n, R = res->n_res, N = s->N;
+    std::vector<uint64_t> sum;
+    try {
+        sum.assign(R * N, 0);
+    } catch (...) {
+        return fail(KS_ERR_NOMEM, "out of host memory checking %llu bound pods", (unsigned long long)B);
+    }
+    const uint64_t LIMIT = (uint64_t)KS_PREEMPT_MAX_ABS_SUM;
+    for (uint64_t i = 0; i < R * N; i++) {
+        const int64_t f = res->node_free[i];
+        sum[i] = f < 0 ? 0 - (uint64_t)f : (uint64_t)f;
+        if (sum[i] > LIMIT)
+            return fail(KS_ERR_RANGE, "resource %llu, node %llu: |node_free| above 2^62", (unsigned long long)(i / N),
+                        (unsigned long long)(i % N));
+    }
+    for (uint64_t b = 0; b < B; b++)
+        for (uint64_t r = 0; r < R; r++) {
+            const int64_t q = bound_req[b * R + r];
+            if (q < 0)
+                return fail(KS_ERR_RANGE, "bound pod %llu: request %lld of resource %llu (at least 0)",
+                            (unsigned long long)b, (long long)q, (unsigned long long)r);
+            uint64_t& a = sum[r * N + (uint32_t)bound->node_idx[b]]; // node range checked by check_preempt_bound
+            if ((uint64_t)q > LIMIT - a)
+                return fail(KS_ERR_RANGE, "resource %llu, node %d: |node_free| and the bound requests sum above 2^62",
+                            (unsigned long long)r, bound->node_idx[b]);
+            a += (uint64_t)q;
+        }
+    return KS_OK;
+}
+
+int ks_fit_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
+                   const ks_node_rules* rules, const ks_bind_resources* res, const int32_t* pod_priority,
+                   const ks_bound_pods* bound, const int64_t* bound_req, uint32_t max_victims, ks_preemption* out,
+                   int32_t* out_victims, uint32_t* out_unresolvable) {
+    static const ks_node_rules no_rules{};
+    static const ks_bind_resources no_res{};
+    int rc = check_pods(s, pods);
+    if (rc) return rc;
+    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_fit_preempt takes host-space pods");
+    if (max_victims == 0 || max_victims > KS_PREEMPT_MAX_VICTIMS)
+        return fail(KS_ERR_RANGE, "max_victims must be in [1, %u] (got %u)", KS_PREEMPT_MAX_VICTIMS, max_victims);
+    const uint64_t P = pods->n, G = n_groups;
+    if (P && (!pod_priority || !out)) return fail(KS_ERR_INVALID, "pod_priority or out is NULL");
+    if (!bound) return fail(KS_ERR_INVALID, "bound is NULL");
+    const uint64_t B = bound->n;
+    if (B && (!bound->node_idx || !bound->req_cpu || !bound->req_mem || !bound->priority))
+        return fail(KS_ERR_INVALID, "NULL bound array");
+    if (B > 0xffffffffull) return fail(KS_ERR_RANGE, "too many bound pods in one call");
+    if (P && !group) return fail(KS_ERR_INVALID, "NULL group");
+    if (G > KS_SPREAD_BIND_MAX_GROUPS)
+        return fail(KS_ERR_RANGE, "%llu groups (at most %u)", (unsigned long long)G, KS_SPREAD_BIND_MAX_GROUPS);
+    for (uint64_t p = 0; p < P; p++)
+        if (group[p] < -1 || group[p] >= (int64_t)G)
+            return fail(KS_ERR_INVALID, "pod %llu: group %d outside [-1, %u)", (unsigned long long)p, group[p], n_groups);
+    const ks_node_rules* nr = rules ? rules : &no_rules;
+    if (!res) res = &no_res;
+    const uint32_t N = s->N, R = res->n_res;
+    rc = check_bind_resources(res, P, N);
+    if (rc) return rc;
+    if (R && B && !bound_req) return fail(KS_ERR_INVALID, "NULL bound_req");
+    NodeRulesPlan rp;
+    try {
+        rc = compile_node_rules(nr, (uint32_t)G, N, &rp);
+    } catch (...) {
+        return fail(KS_ERR_NOMEM, "out of host memory in ks_fit_preempt");
+    }
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lk(s->mu);
+    rc = check_preempt_bound(s, bound);
+    if (!rc) rc = check_fit_preempt_bound(s, bound, bound_req, res);
+    if (rc || P == 0) return rc;
+    CU_TRY(cudaSetDevice(s->device));
+    const cudaStream_t st = s->stream;
+    const DirectGrid g = N ? fit_preempt_grid((uint32_t)P, s->Npad, s->sms) : DirectGrid{};
+    const uint64_t part_rows = (uint64_t)g.n_chunks * P;
+    const size_t vx_bytes = N ? victim_index_bytes(B, N) : 0;
+    HostStaged h;
+    const Staged<int64_t> cpu = h.in(pods->req_cpu, P), mem = h.in(pods->req_mem, P);
+    const Staged<uint64_t> sel = h.in(pods->sel, P * s->W);
+    const Staged<int32_t> prio = h.in(pod_priority, P), grp = h.in(group, P);
+    const Staged<int64_t> req = h.in(R ? res->pod_req : nullptr, P * R);
+    const Staged<int64_t> node_free = h.in(R ? res->node_free : nullptr, (uint64_t)R * N);
+    const NodeRulesStage rs{h, nr, rp, N};
+    const Staged<ks_preemption> rows = h.out(out, P);
+    const Staged<int32_t> vic = h.out(out_victims, out_victims ? P * max_victims : 0);
+    const Staged<uint32_t> unres = h.out(out_unresolvable, out_unresolvable ? P : 0);
+    const Staged<uint64_t> hi = h.work<uint64_t>(part_rows), lo = h.work<uint64_t>(part_rows);
+    const Staged<uint32_t> cand = h.work<uint32_t>(part_rows), cnt = h.work<uint32_t>(part_rows);
+    const Staged<uint32_t> unres_part = h.work<uint32_t>(part_rows);
+    // the victim index's scratch: build_victim_index's block (the bound list uploaded at its start), then bound_req and
+    // the R sorted request columns with their prefix sums
+    const Staged<unsigned char> vx_scratch = h.work<unsigned char>(vx_bytes, 256);
+    const Staged<int64_t> breq = h.work<int64_t>(N ? B * R : 0, 256);
+    const Staged<int64_t> vres = h.work<int64_t>(N ? (uint64_t)R * B : 0, 256);
+    const Staged<int64_t> vpre = h.work<int64_t>(N ? (uint64_t)R * B : 0, 256);
+    if (const int e = h.reserve(s)) return e;
+    ProfileBindArgs q{}; // k_node_rules_setup reads the NODE fields and b.N only
+    q.b.N = N;
+    rs.place(q, s->sms);
+    CU_TRY(h.upload(st));
+    VictimIndex vx{};
+    FitPreemptArgs fa{R, (uint32_t)B, h.dev(req), h.dev(node_free), h.dev(grp), h.dev(rs.ncls), h.dev(rs.nrules),
+                      h.dev(vres), h.dev(vpre), h.dev(unres_part)};
+    if (N) {
+        void* scratch = h.dev(vx_scratch);
+        if (B) {
+            const BoundUpload up = victim_index_inputs(scratch, B, N);
+            CU_TRY(cudaMemcpyAsync(up.node, bound->node_idx, B * 4, cudaMemcpyHostToDevice, st));
+            CU_TRY(cudaMemcpyAsync(up.cpu, bound->req_cpu, B * 8, cudaMemcpyHostToDevice, st));
+            CU_TRY(cudaMemcpyAsync(up.mem, bound->req_mem, B * 8, cudaMemcpyHostToDevice, st));
+            CU_TRY(cudaMemcpyAsync(up.prio, bound->priority, B * 4, cudaMemcpyHostToDevice, st));
+            if (R) CU_TRY(cudaMemcpyAsync(h.dev(breq), bound_req, B * R * 8, cudaMemcpyHostToDevice, st));
+        }
+        CU_TRY(launch_node_rules(q, st));
+        CU_TRY(build_victim_index(scratch, B, N, &vx, st));
+        CU_TRY(build_fit_victim_index(vx, h.dev(breq), fa, N, st));
+    }
+    const PodView pv{h.dev(cpu), h.dev(mem), h.dev(sel), (uint32_t)P};
+    const PreemptPartials part{h.dev(hi), h.dev(lo), h.dev(cand), h.dev(cnt)};
+    CU_TRY(launch_fit_preempt(node_table(s), pv, h.dev(prio), vx, fa, max_victims, part, g, h.dev(rows),
+                              out_victims ? h.dev(vic) : nullptr, out_unresolvable ? h.dev(unres) : nullptr, st));
+    CU_TRY(h.finish(st));
+    return KS_OK;
 }
 
 // ---------------------------------------------------------------------------------------------- async streaming

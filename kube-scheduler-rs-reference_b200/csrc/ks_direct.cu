@@ -7,7 +7,9 @@
 //   K2k k_select_topk          per-pod ranked list of the k best feasible nodes (ks_select_topk), held across the warp
 //   K2p k_preempt_scan         per-pod best preemption candidate (ks_preempt) over a per-call victim index;
 //       k_preempt_emit         chunk merge, victim list and ks_preemption row
-// K2d, K2e, K2k and K2p share one node-tile scan (scan_node_tiles): tiles staged through shared memory by TMA bulk
+//   K2q k_fit_preempt_scan     the same under the full filter (ks_fit_preempt): rule words, scalar resources, pod count;
+//       k_fit_preempt_emit     its merge, victim list, row and unresolvable count
+// K2d, K2e, K2k, K2p and K2q share one node-tile scan (scan_node_tiles): tiles staged through shared memory by TMA bulk
 // copies (cp.async.bulk + mbarrier), one lane per node, several pods per warp in registers.
 // The per-cell kernel is the generic path (any score policy, any P); ks_bitpar.cu holds the bit-parallel
 // fast path that the headline configuration uses.
@@ -745,6 +747,213 @@ __global__ void __launch_bounds__(256)
     out[p] = r;
 }
 
+// ------------------------------------------------------------------------------------------------ K2q (ks_fit_preempt)
+// preempt_walk with the R request columns (include/ksched.h, ks_fit_preempt steps 3-4): besides cpu and memory, every
+// resource in rmask (the pod's non-zero requests req[r]; a zero request always fits) keeps its own avail, free_r[n] plus
+// the lower set's prefix sum, and a bound pod is reprieved only when the pod still fits in every one of them.  The
+// requested resources are listed once, 4 bits each in rlist, so each step of the walk costs one test per requested
+// resource and one more; a pod that requests none walks as preempt_walk does.  The range rule of ks_fit_preempt keeps
+// every sum inside int64.
+__device__ __forceinline__ bool fit_preempt_walk(const VictimIndex& vx, const FitPreemptArgs& fa, uint32_t N,
+                                                 uint32_t node, int32_t pi, int64_t rc, int64_t rm, int64_t fc,
+                                                 int64_t fm, const int64_t* req, uint32_t rmask, uint32_t max_victims,
+                                                 int32_t& vmax, int64_t& vsum, uint32_t& vcnt, int32_t* out) {
+    const uint32_t s0 = __ldg(vx.off + node), s1 = __ldg(vx.off + node + 1);
+    uint32_t lo = s0, hi = s1;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (__ldg(vx.prio + mid) < pi) lo = mid + 1;
+        else hi = mid;
+    }
+    if (lo == s0) return false; // no pod of lower priority
+    int64_t ac = fc + __ldg(vx.pre_cpu + lo - 1), am = fm + __ldg(vx.pre_mem + lo - 1);
+    bool room = rc <= ac && rm <= am;
+    const uint32_t nreq = __popc(rmask);
+    uint32_t rlist = 0;
+    for (uint32_t m = rmask, k = 0; m; m &= m - 1, k++) rlist |= (uint32_t)(__ffs(m) - 1) << (4 * k);
+    int64_t ar[KS_BIND_MAX_RESOURCES];
+#pragma unroll
+    for (uint32_t k = 0; k < KS_BIND_MAX_RESOURCES; k++) {
+        if (k == nreq) break;
+        const uint32_t r = rlist >> (4 * k) & 15u;
+        ar[k] = __ldg(fa.node_free + (size_t)r * N + node) + __ldg(fa.vpre + (size_t)r * fa.B + lo - 1);
+        room &= req[r] <= ar[k];
+    }
+    if (!room) return false; // evicting the whole lower set is not enough
+    vmax = INT32_MIN;
+    vsum = 0;
+    vcnt = 0;
+    for (uint32_t j = lo; j-- > s0;) {
+        const int64_t bc = __ldg(vx.cpu + j), bm = __ldg(vx.mem + j);
+        bool keep = rc <= ac - bc && rm <= am - bm;
+#pragma unroll
+        for (uint32_t k = 0; k < KS_BIND_MAX_RESOURCES; k++) {
+            if (k == nreq) break;
+            const uint32_t r = rlist >> (4 * k) & 15u;
+            keep &= req[r] <= ar[k] - __ldg(fa.vres + (size_t)r * fa.B + j);
+        }
+        if (keep) { // still fits without evicting b: reprieved
+            ac -= bc;
+            am -= bm;
+#pragma unroll
+            for (uint32_t k = 0; k < KS_BIND_MAX_RESOURCES; k++) {
+                if (k == nreq) break;
+                ar[k] -= __ldg(fa.vres + (size_t)(rlist >> (4 * k) & 15u) * fa.B + j);
+            }
+            continue;
+        }
+        if (vcnt == max_victims) return false;
+        const int32_t bp = __ldg(vx.prio + j);
+        if (vcnt == 0) vmax = bp; // visited in descending priority: the first victim has the highest
+        if (out) out[vcnt] = (int32_t)__ldg(vx.idx + j);
+        vsum += (int64_t)bp + 2147483648ll;
+        vcnt++;
+    }
+    return true; // at least one victim: with none, the pod would fit every dimension and the node would not be eligible
+}
+
+// Candidate scan (ks_fit_preempt): per pod the full-filter feasible count, the unresolvable count, the number of
+// candidate nodes and the best candidate's key.  Each cell reads the class's rule word (one coalesced load per node) and,
+// where cpu and memory fit on a resolvable node, the free amounts of the pod's requested resources (coalesced as well);
+// only eligible cells below min_prio go to fit_preempt_walk.  A warp's pods keep their requests in shared memory and a
+// mask of the non-zero ones in registers.  Results go to partials [blockIdx.y][P], merged by k_fit_preempt_emit.
+// One pod per warp (FIT_PREEMPT_PODS_PER_WARP): the walks, latency-bound dependent loads, set the time, and with K2p's
+// 2-8 pods per warp the walk's R avails took the scan to 210-250 registers, one CTA per SM.  The cell work a warp no
+// longer shares across pods is a few shared-memory loads per node.
+template <int W>
+__global__ void __launch_bounds__(DIRECT_THREADS)
+    k_fit_preempt_scan(NodeTable nt, PodView pv, const int32_t* __restrict__ pod_prio, VictimIndex vx, FitPreemptArgs fa,
+                       uint32_t max_victims, PreemptPartials part, uint32_t tiles_per_chunk) {
+    constexpr int PW = FIT_PREEMPT_PODS_PER_WARP;
+    __shared__ int64_t s_req[DIRECT_THREADS / 32][PW][KS_BIND_MAX_RESOURCES];
+    int64_t rc[PW], rm[PW];
+    uint64_t sel[PW][W];
+    uint32_t p0;
+    int32_t pi[PW];
+    uint32_t rmask[PW], rrow[PW]; // non-zero requests; the class's first rule word
+    uint64_t bhi[PW], blo[PW];
+    uint32_t cnt[PW], ncand[PW], nunres[PW];
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t q0 = warp_first_pod<PW>(); // the p0 scan_node_tiles sets
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        const uint32_t p = min(q0 + i, pv.P - 1);
+        pi[i] = __ldg(pod_prio + p);
+        rrow[i] = __ldg(fa.ncls + __ldg(fa.group + p) + 1) * nt.N;
+        const int64_t q = lane < fa.R ? __ldg(fa.req + (size_t)p * fa.R + lane) : 0;
+        if (lane < KS_BIND_MAX_RESOURCES) s_req[warp][i][lane] = q;
+        rmask[i] = __ballot_sync(0xffffffffu, q != 0) & ((1u << KS_BIND_MAX_RESOURCES) - 1u);
+        bhi[i] = blo[i] = PREEMPT_NONE;
+        cnt[i] = ncand[i] = nunres[i] = 0;
+    }
+    __syncwarp();
+
+    scan_node_tiles<W, false>(
+        nt, tiles_per_chunk, pv, p0, rc, rm, sel,
+        [&](uint32_t, uint32_t node, bool real, int64_t fc, int64_t fm, const uint64_t(&lab)[W], int64_t, int64_t) {
+            const int32_t mp = real ? __ldg(vx.min_prio + node) : INT32_MAX; // padding: never a candidate
+#pragma unroll
+            for (int i = 0; i < PW; i++) {
+                uint64_t miss = 0;
+#pragma unroll
+                for (int w = 0; w < W; w++) miss |= sel[i][w] & ~lab[w];
+                const uint32_t word = real ? __ldg(fa.nrules + rrow[i] + node) : 0u;
+                const bool resolvable = real && miss == 0 && (word & NR_REASON) == 0;
+                bool fit = (rc[i] <= fc) & (rm[i] <= fm);
+                if (resolvable && fit) {
+#pragma unroll
+                    for (uint32_t r = 0; r < KS_BIND_MAX_RESOURCES; r++)
+                        if (rmask[i] >> r & 1u) fit &= s_req[warp][i][r] <= __ldg(fa.node_free + (size_t)r * nt.N + node);
+                }
+                cnt[i] += __popc(__ballot_sync(0xffffffffu, resolvable && fit));
+                nunres[i] += __popc(__ballot_sync(0xffffffffu, real && !resolvable));
+                if (resolvable && !fit && mp < pi[i]) {
+                    int32_t vmax;
+                    int64_t vsum;
+                    uint32_t vcnt;
+                    if (fit_preempt_walk(vx, fa, nt.N, node, pi[i], rc[i], rm[i], fc, fm, s_req[warp][i], rmask[i],
+                                         max_victims, vmax, vsum, vcnt, nullptr)) {
+                        uint64_t h, l;
+                        preempt_key(vmax, vsum, vcnt, node, h, l);
+                        ncand[i]++;
+                        if (preempt_less(h, l, bhi[i], blo[i])) {
+                            bhi[i] = h;
+                            blo[i] = l;
+                        }
+                    }
+                }
+            }
+        },
+        [](uint32_t) {});
+
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        uint64_t h = bhi[i], l = blo[i];
+        warp_preempt_min(h, l);
+        const uint32_t c = __reduce_add_sync(0xffffffffu, ncand[i]);
+        const uint32_t p = p0 + i;
+        if (lane == 0 && p < pv.P) {
+            const uint64_t o = (uint64_t)blockIdx.y * pv.P + p;
+            part.hi[o] = h;
+            part.lo[o] = l;
+            part.cand[o] = c;
+            part.cnt[o] = cnt[i];
+            fa.unres[o] = nunres[i];
+        }
+    }
+}
+
+// One thread per pod: k_preempt_emit's merge, "already fits => no plan" and row, with fit_preempt_walk for the victims,
+// and the unresolvable count.  n_chunks = 0 (no node) gives every pod no plan and 0 unresolvable nodes.
+__global__ void __launch_bounds__(256)
+    k_fit_preempt_emit(NodeTable nt, PodView pv, const int32_t* __restrict__ pod_prio, VictimIndex vx, FitPreemptArgs fa,
+                       uint32_t max_victims, PreemptPartials part, uint32_t n_chunks, ks_preemption* __restrict__ out,
+                       int32_t* __restrict__ victims, uint32_t* __restrict__ unres) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= pv.P) return;
+    uint64_t hi = PREEMPT_NONE, lo = PREEMPT_NONE;
+    uint32_t cand = 0, cnt = 0, nu = 0;
+    for (uint32_t ch = 0; ch < n_chunks; ch++) {
+        const uint64_t o = (uint64_t)ch * pv.P + p;
+        cnt += part.cnt[o];
+        cand += part.cand[o];
+        nu += fa.unres[o];
+        if (preempt_less(part.hi[o], part.lo[o], hi, lo)) {
+            hi = part.hi[o];
+            lo = part.lo[o];
+        }
+    }
+    ks_preemption r;
+    r.node_idx = -1;
+    r.n_victims = 0;
+    r.candidates = cnt ? 0u : cand;
+    r.feasible_cnt = cnt;
+    r.max_victim_priority = INT32_MIN;
+    r.reserved = 0;
+    r.victim_priority_sum = 0;
+    int32_t* v = victims ? victims + (uint64_t)p * max_victims : nullptr;
+    if (cnt == 0 && hi != PREEMPT_NONE) {
+        const uint32_t node = (uint32_t)(lo & 0xffffffffffffull);
+        const int64_t* req = fa.req + (size_t)p * fa.R;
+        uint32_t rmask = 0;
+        for (uint32_t k = 0; k < fa.R; k++) rmask |= (req[k] != 0 ? 1u : 0u) << k;
+        int32_t vmax;
+        int64_t vsum;
+        uint32_t vcnt;
+        if (fit_preempt_walk(vx, fa, nt.N, node, pod_prio[p], pv.req_cpu[p], pv.req_mem[p], nt.free_cpu[node],
+                             nt.free_mem[node], req, rmask, max_victims, vmax, vsum, vcnt, v)) {
+            r.node_idx = (int32_t)node;
+            r.n_victims = vcnt;
+            r.max_victim_priority = vmax;
+            r.victim_priority_sum = vsum;
+        }
+    }
+    if (v)
+        for (uint32_t j = r.n_victims; j < max_victims; j++) v[j] = -1;
+    out[p] = r;
+    if (unres) unres[p] = nu;
+}
+
 // ------------------------------------------------------------------------------------------------ K2r (ks_drain_check)
 // Round r places pod r of every candidate still running (DrainArgs, ks_launch.h).  A candidate's private free f differs
 // from free[] only on its overlay nodes, and its own node (plus, with KS_DRAIN_EXCLUDE_CANDIDATES, every candidate's node)
@@ -1084,6 +1293,42 @@ __global__ void __launch_bounds__(256)
     if (lane == 0) min_prio[n] = s1 > s0 ? prio[s0] : INT32_MAX;
 }
 
+// ks_fit_preempt's request columns: vres[r * B + j] = breq[idx[j] * R + r], gathered through the sorted bound indices
+__global__ void __launch_bounds__(256)
+    k_victim_gather_res(const uint32_t* __restrict__ idx, const int64_t* __restrict__ breq, int64_t* __restrict__ vres,
+                        uint32_t B, uint32_t R) {
+    const uint64_t total = (uint64_t)B * R;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t r = (uint32_t)(i / B), j = (uint32_t)(i % B);
+        vres[i] = breq[(uint64_t)idx[j] * R + r];
+    }
+}
+
+// one warp per (node, column blockIdx.y): inclusive prefix sums of the column within the node's segment, as
+// k_victim_prefix sums cpu and memory
+__global__ void __launch_bounds__(256)
+    k_victim_prefix_res(const uint32_t* __restrict__ off, const int64_t* __restrict__ vres, int64_t* __restrict__ vpre,
+                        uint32_t N, uint32_t B) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (n >= N) return; // warp-uniform
+    const int64_t* col = vres + (size_t)blockIdx.y * B;
+    int64_t* pre = vpre + (size_t)blockIdx.y * B;
+    const uint32_t s0 = off[n], s1 = off[n + 1];
+    int64_t carry = 0;
+    for (uint32_t j0 = s0; j0 < s1; j0 += 32) {
+        const uint32_t j = j0 + lane;
+        int64_t c = j < s1 ? col[j] : 0;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const int64_t u = __shfl_up_sync(0xffffffffu, c, d);
+            if (lane >= (uint32_t)d) c += u;
+        }
+        if (j < s1) pre[j] = carry + c;
+        carry += __shfl_sync(0xffffffffu, c, 31);
+    }
+}
+
 // scratch layout: the upload, two key/value buffers of the sort, the digit counts, then the index itself
 struct VictimLayout {
     size_t node, cpu, mem, prio, key[2], val[2], hist, s_prio, s_cpu, s_mem, pre_cpu, pre_mem, off, min_prio, total;
@@ -1172,9 +1417,21 @@ cudaError_t build_victim_index(void* scratch, uint64_t B, uint32_t N, VictimInde
     return cudaSuccess;
 }
 
+cudaError_t build_fit_victim_index(const VictimIndex& vx, const int64_t* breq, const FitPreemptArgs& fa, uint32_t N,
+                                   cudaStream_t st) {
+    if (fa.R == 0 || fa.B == 0 || N == 0) return cudaSuccess;
+    const uint64_t total = (uint64_t)fa.B * fa.R;
+    const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(4096, (total + 255) / 256));
+    k_victim_gather_res<<<grid, 256, 0, st>>>(vx.idx, breq, const_cast<int64_t*>(fa.vres), fa.B, fa.R);
+    k_victim_prefix_res<<<dim3((N + 7) / 8, fa.R), 256, 0, st>>>(vx.off, fa.vres, const_cast<int64_t*>(fa.vpre), N,
+                                                                 fa.B);
+    g_launches += 2;
+    return cudaGetLastError();
+}
+
 // node chunks across gridDim.y when the pods alone give fewer than two CTAs per SM
-DirectGrid direct_grid(uint32_t W, uint32_t P, uint32_t Npad, int sms) {
-    const uint32_t pods_per_cta = (DIRECT_THREADS / 32) * pods_per_warp(W);
+static DirectGrid direct_grid_ppw(uint32_t ppw, uint32_t P, uint32_t Npad, int sms) {
+    const uint32_t pods_per_cta = (DIRECT_THREADS / 32) * ppw;
     const uint32_t n_tiles = Npad / TILE_N;
     const uint32_t want_ctas = 2u * (uint32_t)sms;
     DirectGrid g;
@@ -1184,6 +1441,12 @@ DirectGrid direct_grid(uint32_t W, uint32_t P, uint32_t Npad, int sms) {
     g.tiles_per_chunk = (n_tiles + g.n_chunks - 1) / g.n_chunks;
     g.n_chunks = (n_tiles + g.tiles_per_chunk - 1) / g.tiles_per_chunk;
     return g;
+}
+
+DirectGrid direct_grid(uint32_t W, uint32_t P, uint32_t Npad, int sms) { return direct_grid_ppw(pods_per_warp(W), P, Npad, sms); }
+
+DirectGrid fit_preempt_grid(uint32_t P, uint32_t Npad, int sms) {
+    return direct_grid_ppw(FIT_PREEMPT_PODS_PER_WARP, P, Npad, sms);
 }
 
 // opt-in shared memory sizes of every K2d / K2e kernel on the current device (must not run inside a stream capture)
@@ -1197,6 +1460,7 @@ cudaError_t prepare_direct() {
             constexpr int W_ = decltype(w)::value;
             opt_in(k_explain_counts<W_>, tile_smem_bytes<W_, false>());
             opt_in(k_preempt_scan<W_>, tile_smem_bytes<W_, false>());
+            opt_in(k_fit_preempt_scan<W_>, tile_smem_bytes<W_, false>());
             for (int policy : {KS_SCORE_LEFTOVER, KS_SCORE_LEAST_ALLOCATED, KS_SCORE_MOST_ALLOCATED, KS_SCORE_LEAST_BALANCED})
                 with_policy(policy, [&](auto pol) {
                     constexpr int POL = decltype(pol)::value;
@@ -1292,6 +1556,29 @@ cudaError_t launch_preempt(const NodeTable& nt, const PodView& pv, const int32_t
         n_chunks = g.n_chunks;
     }
     k_preempt_emit<<<(pv.P + 255) / 256, 256, 0, st>>>(nt, pv, pod_prio, vx, max_victims, part, n_chunks, out, victims);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_fit_preempt(const NodeTable& nt, const PodView& pv, const int32_t* pod_prio, const VictimIndex& vx,
+                               const FitPreemptArgs& fa, uint32_t max_victims, const PreemptPartials& part,
+                               const DirectGrid& g, ks_preemption* out, int32_t* victims, uint32_t* unres,
+                               cudaStream_t st) {
+    if (pv.P == 0) return cudaSuccess;
+    uint32_t n_chunks = 0;
+    if (nt.N > 0) {
+        const cudaError_t e = with_label_width(nt.W, [&](auto w) {
+            constexpr int W = decltype(w)::value;
+            k_fit_preempt_scan<W><<<dim3(g.pod_ctas, g.n_chunks), DIRECT_THREADS, tile_smem_bytes<W, false>(), st>>>(
+                nt, pv, pod_prio, vx, fa, max_victims, part, g.tiles_per_chunk);
+            g_launches++;
+            return cudaGetLastError();
+        });
+        if (e != cudaSuccess) return e;
+        n_chunks = g.n_chunks;
+    }
+    k_fit_preempt_emit<<<(pv.P + 255) / 256, 256, 0, st>>>(nt, pv, pod_prio, vx, fa, max_victims, part, n_chunks, out,
+                                                           victims, unres);
     g_launches++;
     return cudaGetLastError();
 }

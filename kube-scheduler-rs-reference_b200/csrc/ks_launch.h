@@ -66,6 +66,35 @@ cudaError_t launch_preempt(const NodeTable& nt, const PodView& pv, const int32_t
                            uint32_t max_victims, const PreemptPartials& part, const DirectGrid& g, ks_preemption* out,
                            int32_t* victims, cudaStream_t st);
 
+// preemption under the full filter (ks_fit_preempt).  The victim index of build_victim_index plus R request columns in
+// its sorted order and their per-segment inclusive prefix sums, and what the scan reads beyond ks_preempt's inputs: each
+// pod's requests and node-rule class, the free amounts and the rule words of ks_node_bind.  Device memory.
+struct FitPreemptArgs {
+    uint32_t R;                // [0, KS_BIND_MAX_RESOURCES]
+    uint32_t B;                // bound pods
+    const int64_t* req;        // [P * R]: pod p's request of r at p * R + r
+    const int64_t* node_free;  // [R * N]
+    const int32_t* group;      // [P], each in [-1, G)
+    const uint32_t* ncls;      // [G + 1]: the class of group g at g + 1, of group -1 at 0
+    const uint32_t* nrules;    // [C * N], written by k_node_rules_setup
+    const int64_t* vres;       // [R * B]: bound requests in the victim index's order, column r at r * B
+    const int64_t* vpre;       // [R * B]: their inclusive prefix sums within each node's segment
+    uint32_t* unres;           // [n_chunks * P]: partial unresolvable counts of the scan
+};
+// k_fit_preempt_scan's pods per warp, and its launch geometry (direct_grid's rule)
+constexpr uint32_t FIT_PREEMPT_PODS_PER_WARP = 1;
+DirectGrid fit_preempt_grid(uint32_t P, uint32_t Npad, int sms);
+// the R request columns after build_victim_index: breq [B * R] (bound pod b's request of r at b * R + r) gathered
+// through vx.idx into fa.vres, then scanned per segment into fa.vpre
+cudaError_t build_fit_victim_index(const VictimIndex& vx, const int64_t* breq, const FitPreemptArgs& fa, uint32_t N,
+                                   cudaStream_t st);
+// out[P], victims[P * max_victims] (may be null) and unres[P] (may be null), device memory.  With nt.N == 0 only the rows
+// and counts are written (no plan).
+cudaError_t launch_fit_preempt(const NodeTable& nt, const PodView& pv, const int32_t* pod_prio, const VictimIndex& vx,
+                               const FitPreemptArgs& fa, uint32_t max_victims, const PreemptPartials& part,
+                               const DirectGrid& g, ks_preemption* out, int32_t* victims, uint32_t* unres,
+                               cudaStream_t st);
+
 // drain simulation (ks_drain_check).  Candidates are in the host's round order (pod count descending), so the pods of
 // round r - pod r of every candidate that has one - are the first R_r candidates; slot j of every round is candidate j.
 // Each candidate's moves are an overlay sorted by node, (node, f_cpu, f_mem) with f its private free, kept in
@@ -353,4 +382,7 @@ constexpr uint32_t NR_REASON = 3u, NR_TAINT = 1u, NR_AFFINITY = 2u, NR_AFF_OK = 
 // k_profile_setup over the existing pods when E > 0; then the walk k_bind_seq, one cooperative launch of grid CTAs.  FIT
 // includes GANG_FIT here.  The fields a mode does not read may be left zero.
 cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st);
+// k_node_rules_setup alone: the rule words nrules [C * N] from the NODE fields of a and a.b.N (launch_bind's first
+// launch in NODE and FIT; ks_fit_preempt's rule words)
+cudaError_t launch_node_rules(const ProfileBindArgs& a, cudaStream_t st);
 } // namespace ks

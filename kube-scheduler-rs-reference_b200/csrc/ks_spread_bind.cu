@@ -1051,6 +1051,12 @@ __global__ void __launch_bounds__(SBD_THREADS, 1) k_bind_seq(const ProfileBindAr
     }
 }
 
+cudaError_t launch_node_rules(const ProfileBindArgs& a, cudaStream_t st) {
+    k_node_rules_setup<<<a.rules_grid, SBD_THREADS, 0, st>>>(a);
+    g_launches++;
+    return cudaGetLastError();
+}
+
 uint32_t bind_setup_grid(uint32_t G, int sms) { return std::max(1u, std::min<uint32_t>(G, 4u * (uint32_t)sms)); }
 
 cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_words, uint32_t W, cudaStream_t st) {
@@ -1064,10 +1070,7 @@ cudaError_t launch_bind(BindMode mode, const ProfileBindArgs& a, uint64_t acnt_w
             return cudaGetLastError();
         };
         cudaError_t e;
-        if (nr) {
-            k_node_rules_setup<<<a.rules_grid, SBD_THREADS, 0, st>>>(a);
-            if ((e = launched(1)) != cudaSuccess) return e;
-        }
+        if (nr && (e = launch_node_rules(a, st)) != cudaSuccess) return e;
         if (b.G) {
             if (nr) k_bind_setup<LW, true><<<b.setup_grid, SBD_THREADS, 0, st>>>(a);
             else k_bind_setup<LW, false><<<b.setup_grid, SBD_THREADS, 0, st>>>(a);

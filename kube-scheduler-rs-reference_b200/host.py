@@ -66,6 +66,8 @@ for _name, _res, _args in [
     ("ksh_reconcile_fit_gangs", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, _vp, _vp,
                                           _vp, _vp, _vp, _vp, C.c_uint64, _vp, C.c_int, _vp, _vp, _vp, _vp,
                                           C.c_size_t, _vp]),
+    ("ksh_preempt_fit_pods", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, _vp, C.c_uint32, _vp, _vp,
+                                       C.c_size_t, _vp]),
 ]:
     _proto(_name, _res, *_args)
 
@@ -452,6 +454,30 @@ class Context:
         buf = C.create_string_buffer(max(cap, 1))
         check(lib.ksh_preempt_pods(self._h, _addr(pods, first), n, priority.ctypes.data, int(max_victims),
                                    rows.ctypes.data, C.addressof(buf), cap, off.ctypes.data), "ksh_preempt_pods")
+        return rows, _string_list(buf, off, rows["n_victims"])
+
+    def preempt_fit_pods(self, pods, n, group, n_groups, priority, max_victims, group_rules=None, first=0,
+                         victims_cap=None):
+        """Priority preemption under the full filter (ksh_preempt_fit_pods): preempt_pods with group [n] and
+        group_rules [n_groups] as reconcile_nodes takes them (None: no toleration and no term); the context's taints,
+        the batch's extended resources and the pod limit apply.  Returns (rows, victims) as preempt_pods."""
+        priority = np.ascontiguousarray(priority, np.int32).reshape(-1)
+        group = np.ascontiguousarray(group, np.int32).reshape(-1)
+        if priority.shape[0] != n or group.shape[0] != n:
+            raise ValueError(f"priority has {priority.shape[0]} and group {group.shape[0]} entries, pods {n}")
+        nr = None
+        if group_rules is not None:
+            if len(group_rules) != n_groups:
+                raise ValueError(f"group_rules has {len(group_rules)} entries, groups {n_groups}")
+            nr = node_rules(group_rules)
+        rows = np.empty(n, capi.PREEMPTION_DTYPE)
+        off = np.empty(n, np.int64)
+        cap = int(victims_cap if victims_cap is not None else 64 * int(max_victims) * max(n, 1))
+        buf = C.create_string_buffer(max(cap, 1))
+        check(lib.ksh_preempt_fit_pods(self._h, _addr(pods, first), n, group.ctypes.data, int(n_groups),
+                                       None if nr is None else C.addressof(nr[0]), priority.ctypes.data,
+                                       int(max_victims), rows.ctypes.data, C.addressof(buf), cap, off.ctypes.data),
+              "ksh_preempt_fit_pods")
         return rows, _string_list(buf, off, rows["n_victims"])
 
     def reconcile(self, pods, i, policy=capi.KS_SCORE_LEFTOVER):

@@ -678,6 +678,41 @@ class Snapshot:
         check(lib.ks_preempt(self._h, C.byref(pods), _ptr(priority), C.byref(b), int(max_victims), _ptr(out),
                              _ptr(victims), int(out_space), C.c_void_p(stream) if stream else None), "ks_preempt")
 
+    def fit_preempt(self, req_cpu, req_mem, sel, priority, group, n_groups, bound_node, bound_cpu, bound_mem,
+                    bound_priority, max_victims, rules=None, node_free=None, pod_req=None, bound_req=None):
+        """preempt under the full filter (ks_fit_preempt): group [P] and rules as fit_bind takes them (rules None =
+        NULL); node_free [R, N], pod_req [P, R] and bound_req [B, R] (int64), or all three None (the C call's NULL res).
+        Returns preempt's (rows, victims), then unresolvable uint32 [P]: the nodes no eviction can open to the pod."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        p = int(pods.n)
+        priority = _c(priority, np.int32).reshape(-1)
+        group = _c(group, np.int32).reshape(-1)
+        if priority.shape[0] != p or group.shape[0] != p:
+            raise ValueError(f"priority has {priority.shape[0]} and group {group.shape[0]} entries, pods {p}")
+        bound, keep_b = self._bound(bound_node, bound_cpu, bound_mem, bound_priority)
+        if (node_free is None) != (pod_req is None) or (node_free is None) != (bound_req is None):
+            raise ValueError("node_free, pod_req and bound_req go together")
+        br, r = None, 0
+        if node_free is not None:
+            node_free, pod_req, bound_req = _c(node_free, np.int64), _c(pod_req, np.int64), _c(bound_req, np.int64)
+            if node_free.ndim != 2 or node_free.shape[1] != self.n_nodes:
+                raise ValueError(f"node_free has shape {node_free.shape}, expected (R, {self.n_nodes})")
+            r = node_free.shape[0]
+            if pod_req.shape != (p, r):
+                raise ValueError(f"pod_req has shape {pod_req.shape}, expected ({p}, {r})")
+            if bound_req.shape != (int(bound.n), r):
+                raise ValueError(f"bound_req has shape {bound_req.shape}, expected ({int(bound.n)}, {r})")
+            br = capi.ks_bind_resources(r, _ptr(node_free), _ptr(pod_req))
+        nr, hold = _rules_arg(rules)
+        rows = np.empty(p, capi.PREEMPTION_DTYPE)
+        victims = np.empty((p, int(max_victims)), np.int32)
+        unres = np.empty(p, np.uint32)
+        check(lib.ks_fit_preempt(self._h, C.byref(pods), _ptr(group), int(n_groups), nr,
+                                 None if br is None else C.byref(br), _ptr(priority), C.byref(bound),
+                                 _ptr(bound_req), int(max_victims), _ptr(rows), _ptr(victims), _ptr(unres)),
+              "ks_fit_preempt")
+        return rows, victims, unres
+
     def last_timings(self):
         ms = (C.c_float * 3)()
         check(lib.ks_last_timings(self._h, ms), "ks_last_timings")
