@@ -397,6 +397,11 @@ extern "C" {
                           rules: *const ks_node_rules, res: *const ks_bind_resources, pod_priority: *const i32,
                           bound: *const ks_bound_pods, bound_req: *const i64, max_victims: u32,
                           out: *mut ks_preemption, out_victims: *mut i32, out_unresolvable: *mut u32) -> c_int;
+    // ks_drain_check under the full filter: pod count, scalar resources, taints and required node affinity (DESIGN.md 5u)
+    pub fn ks_fit_drain_check(s: *mut ks_snapshot, pods: *const ks_pods, group: *const i32, n_groups: u32,
+                              rules: *const ks_node_rules, res: *const ks_bind_resources,
+                              cand: *const ks_drain_candidates, policy: c_int, flags: u32, out_placed: *mut u32,
+                              out_node_idx: *mut i32, out_score: *mut i64, out_refused: *mut u32) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -511,6 +516,11 @@ extern "C" {
                                  json: *mut c_char, cap: usize, json_off: *mut i64) -> c_int;
     pub fn ksh_drain_nodes(ctx: *mut ksh_context, node_names: *const *const c_char, n: u64, pods: *const ks_pod_obj,
                            pod_offset: *const u64, policy: c_int, flags: u32, placed: *mut u32, node_idx: *mut i32) -> c_int;
+    // ksh_drain_nodes under the full filter: taints, node affinity, extended resources and the pod limit (DESIGN.md 5u)
+    pub fn ksh_drain_fit_nodes(ctx: *mut ksh_context, node_names: *const *const c_char, n: u64, pods: *const ks_pod_obj,
+                               pod_offset: *const u64, group: *const i32, n_groups: u32, rules: *const ksh_node_rules,
+                               policy: c_int, flags: u32, placed: *mut u32, node_idx: *mut i32,
+                               refused: *mut u32) -> c_int;
     pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,
                             messages: *mut c_char, cap: usize, msg_off: *mut i64) -> c_int;
     pub fn ksh_format_unschedulable(n_nodes: u32, r: *const ks_pod_reasons, buf: *mut c_char, cap: usize) -> c_int;

@@ -1066,6 +1066,62 @@ int ks_gang_fit_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const
                      uint32_t* out_soft_count /* [G * S] or NULL */, int64_t* out_free /* [R * N] or NULL */,
                      uint32_t* out_placed /* [n] or NULL */);
 
+/* ---- drain simulation under the full filter: ks_drain_check with the pod count, scalar resources, taints and required
+ * node affinity (cluster-autoscaler's removal simulation and Karpenter's consolidation running the scheduler's filters;
+ * spec extension, DESIGN.md 5u) ----
+ * ks_drain_check's steps 1-4 (above), changed only where written here.  `group`, `rules` and `res` mean what they mean
+ * for ks_fit_bind: pod p belongs to group[p] in [-1, n_groups), group -1 tolerates nothing, has no node affinity and is
+ * still filtered by taints; res->node_free[r * N + n] is allocatable minus what the bound pods request there (any
+ * int64), res->pod_req[p * R + r] >= 0 what pod p, one of the pods being drained, requests; the pod count is a resource
+ * whose request is 1.
+ *   1. destinations: ks_drain_check's - every real node but the candidate's own, and with KS_DRAIN_EXCLUDE_CANDIDATES no
+ *      candidate's node at all;
+ *   2. placement: each candidate starts from private copies f of free[] and f_r of node_free, and visits its pods in
+ *      array order.  Pod p may go to destination n when it passes ks_fit_bind's filter there at that point: cpu and
+ *      memory against f (no zero skip), the selector, each resource against f_r (upstream's zero skip: a zero request
+ *      always fits), no untolerated hard taint, and the group's required node affinity.  Among those it takes the argmax
+ *      of `policy`'s score over f, ties to the lower node index, and its requests are subtracted from f and from every
+ *      f_r at that node, so later pods of the candidate see the move.  A requested resource fits before it is
+ *      subtracted, so f_r never drops below 0 by a move and never overflows;
+ *   3. stop, placed and drainable as ks_drain_check: the first pod with no destination stops the candidate, it and every
+ *      later pod get node -1 and score 0, out_placed[d] counts the pods placed before it, and the candidate is
+ *      drainable iff that is its pod count;
+ *   4. nothing is charged: free[], the bit-parallel index and the snapshot are unchanged.
+ * out_refused[4d .. 4d + 3] (or NULL) says why a stopped candidate stopped.  The words count the destinations of its
+ * stopping pod p = offset[d] + out_placed[d], at p's turn (against f and f_r after the earlier moves): word 0 the nodes
+ * that fail cpu, memory or the selector; word 1 those that pass them but fail a resource; word 2 those that pass all of
+ * that but carry a hard taint the group does not tolerate; word 3 those that pass all of that but fail required node
+ * affinity.  Words 1-3 are ks_fit_bind's refusal words 0-2 in its filter order, and the four sum to the candidate's
+ * destination count.  They are all 0 for a drainable candidate.
+ * Scores are the resource policy's, as in ks_drain_check; TaintToleration and NodeAffinity do not score here.  This is
+ * deliberate: drainability depends only on the filter and on the order of the moves, and (D1) stays exact.
+ * rules->weight_* and preferred terms are checked as ks_node_bind checks them and play no part.
+ * Identities:
+ *   (D1) rules and res NULL (any group): out_placed, out_node_idx and out_score are ks_drain_check's, bit for bit, at
+ *        every policy, with and without KS_DRAIN_EXCLUDE_CANDIDATES;
+ *   (D2) an extra resource that copies cpu (pod_req each pod's positive cpu request, node_free free_cpu) changes nothing;
+ *   (D3) no node carries a taint, no group has a node-affinity term and every node_free is at least the total request of
+ *        its resource over every candidate: the outputs are D1's;
+ *   (D4) a drainable candidate's moves, replayed one at a time on a copy of the cluster (free[] reduced by the requests,
+ *        node_free by pod_req), pass the full filter at every step;
+ *   (D5) a stopped candidate's four words sum to its destination count.
+ * Checked on the host before any device work: every check of ks_drain_check; ks_fit_bind's checks on group
+ * (KS_ERR_INVALID for a NULL group with pods->n > 0 or one outside [-1, G), KS_ERR_RANGE for G >
+ * KS_SPREAD_BIND_MAX_GROUPS), rules and res.  n = 0 does nothing.
+ * One H2D copy (the pods in round order with their groups and pod_req, the candidates, the excluded column and
+ * node_free, and the rules), k_node_rules_setup (ks_node_bind's rule words), one scan and one commit per round enqueued
+ * back to back, with out_refused one counting scan after the last round, and one D2H copy; the call returns after
+ * completion.
+ * Out of scope: PodTopologySpread and InterPodAffinity with the moved pods (upstream re-runs them; they are not inputs
+ * here, as in ks_fit_preempt); PodDisruptionBudgets and pod filtering, the caller's job as in ks_drain_check; scoring by
+ * TaintToleration and NodeAffinity; NodeUnschedulable other than through its taint; the scale-up estimator and
+ * ks_explain under the full filter. */
+int ks_fit_drain_check(ks_snapshot* s, const ks_pods* pods /* host space */, const int32_t* group /* [P] */,
+                       uint32_t n_groups, const struct ks_node_rules* rules /* or NULL */,
+                       const struct ks_bind_resources* res /* or NULL */, const ks_drain_candidates* cand, int policy,
+                       uint32_t flags, uint32_t* out_placed /* [n] */, int32_t* out_node_idx /* [P] */,
+                       int64_t* out_score /* [P] or NULL */, uint32_t* out_refused /* [4n] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

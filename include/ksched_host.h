@@ -456,6 +456,22 @@ int ksh_preempt_fit_pods(ksh_context* ctx, const ks_pod_obj* pods, uint64_t n_po
                          uint32_t n_groups, const ksh_node_rules* rules /* or NULL */, const int32_t* pod_priority,
                          uint32_t max_victims, ks_preemption* out, char* victims, size_t cap, int64_t* out_victim_off);
 
+/* Node drain under the full filter over objects (ks_fit_drain_check, DESIGN.md 5u): ksh_drain_nodes' arguments and
+ * checks plus group[pod_offset[n]] in [-1, n_groups) and rules (NULL allowed), as ksh_preempt_fit_pods takes them.  The
+ * context's node taints and the rules' tolerations and node-affinity terms are compiled as ksh_preempt_fit_pods compiles
+ * them; the batch's resources are built as ksh_compile_resources builds them over the drained pods, so the pod count is
+ * always among them and a destination at its allocatable "pods" takes no more ("Too many pods").  The drained pods are
+ * bound to their candidate, which is never a destination, so the context's node_free is used as it is.
+ * Cordoned and draining nodes: mark them with the taint node.kubernetes.io/unschedulable:NoSchedule through
+ * ksh_context_set_node_taints, as the node lifecycle controller does; a group that does not tolerate it then sends
+ * nothing there.  out_refused[4n] (or NULL) as ks_fit_drain_check gives it.  A malformed quantity of a requested
+ * resource is reported as ksh_reconcile_fit reports it (KS_ERR_PARSE or KS_ERR_RANGE, naming the node or pod).  Nothing
+ * is charged.  KS_ERR_NO_DEVICE on a packing-only context. */
+int ksh_drain_fit_nodes(ksh_context* ctx, const char* const* node_names, uint64_t n, const ks_pod_obj* pods,
+                        const uint64_t* pod_offset, const int32_t* group, uint32_t n_groups,
+                        const ksh_node_rules* rules /* or NULL */, int policy, uint32_t flags, uint32_t* out_placed,
+                        int32_t* out_node_idx, uint32_t* out_refused /* [4n] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -41,6 +41,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 #pragma weak ks_fit_bind
 #pragma weak ks_gang_fit_bind
 #pragma weak ks_fit_preempt
+#pragma weak ks_fit_drain_check
 
 namespace {
 
@@ -2517,6 +2518,54 @@ int ksh_preempt_fit_pods(ksh_context* c, const ks_pod_obj* pods, uint64_t n, con
         out_victim_off[i] = list.append(keys.data(), keys.size());
     }
     return KS_OK;
+}
+KSH_CATCH
+
+// ksh_drain_nodes' candidates under the full filter: the context's taints and the groups' rules compiled as
+// ksh_preempt_fit_pods compiles them, and the batch's resources (the pod count always among them) from the drained
+// pods.  Those pods are bound to their candidate, which is never a destination, so the context's node_free is used as
+// it is.
+int ksh_drain_fit_nodes(ksh_context* c, const char* const* node_names, uint64_t n, const ks_pod_obj* pods,
+                        const uint64_t* pod_offset, const int32_t* group, uint32_t n_groups, const ksh_node_rules* rules,
+                        int policy, uint32_t flags, uint32_t* out_placed, int32_t* out_node_idx,
+                        uint32_t* out_refused) try {
+    if (!c || !pod_offset || (n && (!node_names || !out_placed))) return fail(KS_ERR_INVALID, "NULL argument");
+    if (pod_offset[0] != 0) return fail(KS_ERR_INVALID, "pod_offset[0] must be 0");
+    for (uint64_t d = 0; d < n; d++)
+        if (pod_offset[d + 1] < pod_offset[d]) return fail(KS_ERR_INVALID, "pod offsets decrease");
+    const uint64_t P = pod_offset[n];
+    if (P && (!pods || !out_node_idx || !group)) return fail(KS_ERR_INVALID, "NULL argument");
+    for (uint64_t i = 0; i < P; i++)
+        if (group[i] < -1 || group[i] >= (int64_t)n_groups)
+            return fail(KS_ERR_INVALID, "pod " + std::to_string(i) + ": group outside [-1, n_groups)");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    std::vector<int32_t> node(n);
+    for (uint64_t d = 0; d < n; d++) { // mis-grouped input is refused before anything is packed
+        const char* name = node_names[d];
+        if (!name) return fail(KS_ERR_INVALID, "candidate " + std::to_string(d) + ": node name is NULL");
+        node[d] = node_index_of(c, name);
+        if (node[d] < 0) return fail(KS_ERR_INVALID, "candidate " + std::to_string(d) + ": node \"" + name + "\" is not in the store");
+        for (uint64_t i = pod_offset[d]; i < pod_offset[d + 1]; i++)
+            if (!ksh_is_pod_bound(&pods[i]) || std::strcmp(pods[i].node_name, name) != 0)
+                return fail(KS_ERR_INVALID, "pod " + std::to_string(i) + " (" + nz(pods[i].ns) + "/" + nz(pods[i].name) +
+                                                ") has spec.nodeName \"" + (ksh_is_pod_bound(&pods[i]) ? pods[i].node_name : "") +
+                                                "\", not its candidate's node \"" + name + "\"");
+    }
+    int rc = device_ready(c, ks_fit_drain_check, "ks_fit_drain_check");
+    if (rc) return rc;
+    CompiledNodeRules cr;
+    rc = compile_node_rules(c, n_groups, rules, &cr);
+    if (rc) return rc;
+    CompiledResources res;
+    rc = compile_resources(c, pods, P, &res);
+    if (rc) return rc;
+    ks_pods kp;
+    rc = pack_batch(c, pods, P, &kp);
+    if (rc) return rc;
+    const ks_drain_candidates kc{n, node.data(), pod_offset};
+    const ks_bind_resources br{(uint32_t)res.ids.size(), res.node_free.data(), res.pod_req.data()};
+    return ks_fit_drain_check(c->snap, &kp, group, n_groups, &cr.r, &br, &kc, policy, flags, out_placed, out_node_idx,
+                              nullptr, out_refused);
 }
 KSH_CATCH
 

@@ -1329,11 +1329,20 @@ int ks_gang_bind(ks_snapshot* s, const ks_pods* pods, const ks_gangs* gangs, int
     return KS_OK;
 }
 
-int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidates* cand, int policy, uint32_t flags,
-                   uint32_t* out_placed, int32_t* out_node_idx, int64_t* out_score) {
+// ks_drain_check's and ks_fit_drain_check's candidates: every check of ks_drain_check (include/ksched.h), in the order
+// callers see them, then the round order - candidates by pod count descending, stable - and the candidates still
+// running in each round.  Host code only; nothing is read from the device.
+struct DrainPlan {
+    uint64_t P = 0, D = 0;
+    uint32_t rounds = 0;
+    std::vector<uint32_t> order, per_round;
+};
+
+static int plan_drain(const ks_snapshot* s, const char* call, const ks_pods* pods, const ks_drain_candidates* cand,
+                      int policy, uint32_t flags, const uint32_t* out_placed, const int32_t* out_node_idx, DrainPlan* pl) {
     int rc = check_pods(s, pods);
     if (rc) return rc;
-    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_drain_check takes host-space pods");
+    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "%s takes host-space pods", call);
     if (!cand || !cand->offset || (cand->n && (!cand->node_idx || !out_placed)))
         return fail(KS_ERR_INVALID, "NULL candidate array or out_placed");
     if (pods->n && !out_node_idx) return fail(KS_ERR_INVALID, "out_node_idx is NULL");
@@ -1356,11 +1365,13 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidate
         rounds = std::max(rounds, (uint32_t)size);
     }
     if (off[D] != P) return fail(KS_ERR_INVALID, "offset[n] must be pods->n");
-    if (D == 0) return KS_OK;
-    rc = check_commit_requests(P, pods->req_cpu, pods->req_mem);
+    rc = check_commit_requests(P, pods->req_cpu, pods->req_mem); // P = 0 when D = 0
     if (rc) return rc;
-    const uint32_t W = s->W;
-    std::vector<uint32_t> order, per_round; // candidates by pod count descending; candidates still running in round r
+    pl->P = P;
+    pl->D = D;
+    pl->rounds = rounds;
+    std::vector<uint32_t>& order = pl->order; // candidates by pod count descending
+    std::vector<uint32_t>& per_round = pl->per_round; // candidates still running in round r
     try {
         order.resize(D);
         per_round.assign(rounds, 0);
@@ -1373,6 +1384,19 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidate
     });
     for (uint64_t d = 0; d < D; d++)
         for (uint64_t r = 0; r < off[d + 1] - off[d]; r++) per_round[r]++;
+    return KS_OK;
+}
+
+int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidates* cand, int policy, uint32_t flags,
+                   uint32_t* out_placed, int32_t* out_node_idx, int64_t* out_score) {
+    DrainPlan dp;
+    const int rc = plan_drain(s, "ks_drain_check", pods, cand, policy, flags, out_placed, out_node_idx, &dp);
+    if (rc || dp.D == 0) return rc;
+    const uint64_t P = dp.P, D = dp.D;
+    const uint64_t* off = cand->offset;
+    const uint32_t rounds = dp.rounds;
+    const std::vector<uint32_t>&order = dp.order, &per_round = dp.per_round;
+    const uint32_t W = s->W;
     std::lock_guard<std::mutex> lk(s->mu);
     CU_TRY(cudaSetDevice(s->device));
     // pods in round order, then the candidates in round order
@@ -2754,6 +2778,155 @@ int ks_fit_preempt(ks_snapshot* s, const ks_pods* pods, const int32_t* group, ui
     CU_TRY(launch_fit_preempt(node_table(s), pv, h.dev(prio), vx, fa, max_victims, part, g, h.dev(rows),
                               out_victims ? h.dev(vic) : nullptr, out_unresolvable ? h.dev(unres) : nullptr, st));
     CU_TRY(h.finish(st));
+    return KS_OK;
+}
+
+int ks_fit_drain_check(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
+                       const ks_node_rules* rules, const ks_bind_resources* res, const ks_drain_candidates* cand,
+                       int policy, uint32_t flags, uint32_t* out_placed, int32_t* out_node_idx, int64_t* out_score,
+                       uint32_t* out_refused) {
+    static const ks_node_rules no_rules{};
+    static const ks_bind_resources no_res{};
+    DrainPlan dp;
+    int rc = plan_drain(s, "ks_fit_drain_check", pods, cand, policy, flags, out_placed, out_node_idx, &dp);
+    if (rc) return rc;
+    const uint64_t P = dp.P, D = dp.D, G = n_groups;
+    if (P && !group) return fail(KS_ERR_INVALID, "NULL group");
+    if (G > KS_SPREAD_BIND_MAX_GROUPS)
+        return fail(KS_ERR_RANGE, "%llu groups (at most %u)", (unsigned long long)G, KS_SPREAD_BIND_MAX_GROUPS);
+    for (uint64_t p = 0; p < P; p++)
+        if (group[p] < -1 || group[p] >= (int64_t)G)
+            return fail(KS_ERR_INVALID, "pod %llu: group %d outside [-1, %u)", (unsigned long long)p, group[p], n_groups);
+    const ks_node_rules* nr = rules ? rules : &no_rules;
+    if (!res) res = &no_res;
+    const uint32_t N = s->N, R = res->n_res, W = s->W;
+    rc = check_bind_resources(res, P, N);
+    if (rc) return rc;
+    NodeRulesPlan rp;
+    try {
+        rc = compile_node_rules(nr, (uint32_t)G, N, &rp);
+    } catch (...) {
+        return fail(KS_ERR_NOMEM, "out of host memory in ks_fit_drain_check");
+    }
+    if (rc || D == 0) return rc;
+    const uint64_t* off = cand->offset;
+    const std::vector<uint32_t>&order = dp.order, &per_round = dp.per_round;
+    std::lock_guard<std::mutex> lk(s->mu);
+    CU_TRY(cudaSetDevice(s->device));
+    // pods in round order with their groups and requests, the candidates in round order, the excluded column, node_free
+    // and the node rules
+    const bool excl = flags & KS_DRAIN_EXCLUDE_CANDIDATES, refusals = out_refused != nullptr;
+    HostStaged h;
+    const auto cpu = h.in<int64_t>(nullptr, P), mem = h.in<int64_t>(nullptr, P);
+    const auto sel = h.in<uint64_t>(nullptr, P * W);
+    const auto grp = h.in<int32_t>(nullptr, P);
+    const auto cand_node = h.in<int32_t>(nullptr, D);
+    const auto pod_base = h.in<uint32_t>(nullptr, D), cand_id = h.in<uint32_t>(nullptr, D);
+    const auto excluded = h.in<uint32_t>(nullptr, excl ? s->Npad / 32 : 0); // bits of the candidates' nodes
+    const auto req = h.in<int64_t>(nullptr, P * R);
+    const auto node_free = h.in(R ? res->node_free : nullptr, (uint64_t)R * N);
+    const NodeRulesStage rs{h, nr, rp, N};
+    const auto score = h.out(out_score, P);
+    const auto idx = h.out(out_node_idx, P);
+    const auto placed = h.out(out_placed, D);
+    const auto refused = h.out(out_refused, refusals ? 4 * D : 0);
+    uint64_t part_rows = 0; // node-chunk partials: the largest round needs the most
+    for (uint32_t r = 0; r < dp.rounds; r++)
+        part_rows = std::max<uint64_t>(part_rows, (uint64_t)fit_drain_grid(per_round[r], s->Npad, s->sms).n_chunks * per_round[r]);
+    const auto ov_fc = h.work<int64_t>(P), ov_fm = h.work<int64_t>(P), part_key = h.work<int64_t>(part_rows);
+    const auto ov_fr = h.work<int64_t>(P * R);
+    const auto ov_node = h.work<int32_t>(P), part_idx = h.work<int32_t>(part_rows);
+    const auto ov_cnt = h.work<uint32_t>(3 * D); // ov_cnt D, failed D, D zeros for the refusal pass: zeroed together
+    const uint64_t DS = refusals ? D : 0;         // the stop arrays
+    const auto stop_cpu = h.work<int64_t>(DS), stop_mem = h.work<int64_t>(DS), stop_req = h.work<int64_t>(DS * R);
+    const auto stop_sel = h.work<uint64_t>(DS * W);
+    const auto stop_grp = h.work<int32_t>(DS);
+    if (const int e = h.reserve(s)) return e;
+    ProfileBindArgs q{}; // k_node_rules_setup reads the NODE fields and b.N only
+    q.b.N = N;
+    rs.place(q, s->sms);
+    int64_t *h_rc = h.host(cpu), *h_rm = h.host(mem), *h_req = h.host(req);
+    uint64_t* h_sel = h.host(sel);
+    int32_t *h_node = h.host(cand_node), *h_grp = h.host(grp);
+    uint32_t *h_base = h.host(pod_base), *h_id = h.host(cand_id);
+    for (uint64_t j = 0; j < D; j++) {
+        h_node[j] = cand->node_idx[order[j]];
+        h_base[j] = (uint32_t)off[order[j]];
+        h_id[j] = order[j];
+    }
+    for (uint64_t r = 0, r0 = 0; r < dp.rounds; r0 += per_round[r], r++) // round r: pod r of the first per_round[r] candidates
+        for (uint64_t j = 0; j < per_round[r]; j++) {
+            const uint64_t p = off[order[j]] + r;
+            h_rc[r0 + j] = pods->req_cpu[p];
+            h_rm[r0 + j] = pods->req_mem[p];
+            h_grp[r0 + j] = group[p];
+            memcpy(h_sel + (r0 + j) * W, pods->sel + p * W, 8 * W);
+            if (R) memcpy(h_req + (r0 + j) * R, res->pod_req + p * R, 8 * R);
+        }
+    if (excl) {
+        uint32_t* h_excl = h.host(excluded);
+        memset(h_excl, 0, excluded.n * 4);
+        for (uint64_t d = 0; d < D; d++) h_excl[cand->node_idx[d] >> 5] |= 1u << (cand->node_idx[d] & 31);
+    }
+    cudaStream_t st = s->stream;
+    CU_TRY(h.upload(st));
+    CU_TRY(cudaMemsetAsync(h.dev(score), 0, P * 8, st));
+    CU_TRY(cudaMemsetAsync(h.dev(idx), 0xff, P * 4, st));
+    CU_TRY(cudaMemsetAsync(h.dev(placed), 0, D * 4, st));
+    CU_TRY(cudaMemsetAsync(h.dev(ov_cnt), 0, D * 12, st));
+    if (refusals) CU_TRY(cudaMemsetAsync(h.dev(refused), 0, D * 16, st));
+    CU_TRY(launch_node_rules(q, st));
+    DrainArgs da;
+    da.cand_node = h.dev(cand_node);
+    da.pod_base = h.dev(pod_base);
+    da.cand_id = h.dev(cand_id);
+    da.excl = excl ? h.dev(excluded) : nullptr;
+    da.ov_cnt = h.dev(ov_cnt);
+    da.failed = da.ov_cnt + D;
+    da.ov_node = h.dev(ov_node);
+    da.ov_fc = h.dev(ov_fc);
+    da.ov_fm = h.dev(ov_fm);
+    da.out_idx = h.dev(idx);
+    da.out_score = h.dev(score);
+    da.placed = h.dev(placed);
+    FitDrainArgs fa{};
+    fa.R = R;
+    fa.P = (uint32_t)P;
+    fa.node_free = h.dev(node_free);
+    fa.ncls = h.dev(rs.ncls);
+    fa.nrules = h.dev(rs.nrules);
+    fa.ov_fr = h.dev(ov_fr);
+    if (refusals) {
+        fa.stop_cpu = h.dev(stop_cpu);
+        fa.stop_mem = h.dev(stop_mem);
+        fa.stop_sel = h.dev(stop_sel);
+        fa.stop_req = h.dev(stop_req);
+        fa.stop_grp = h.dev(stop_grp);
+    }
+    const PartialView part{h.dev(part_key), h.dev(part_idx), nullptr};
+    const NodeTable nt = node_table(s);
+    for (uint64_t r = 0, r0 = 0; r < dp.rounds; r0 += per_round[r], r++) {
+        const PodView pv{h.dev(cpu) + r0, h.dev(mem) + r0, h.dev(sel) + r0 * W, per_round[r]};
+        fa.req = h.dev(req) + r0 * R;
+        fa.group = h.dev(grp) + r0;
+        const DirectGrid g = fit_drain_grid(per_round[r], s->Npad, s->sms);
+        const cudaError_t e = launch_fit_drain_round(nt, pv, da, fa, policy, (uint32_t)r, part, g, st);
+        if (e != cudaSuccess)
+            return fail(KS_ERR_CUDA, "fit drain round %llu launch failed: %s", (unsigned long long)r, cudaGetErrorString(e));
+    }
+    if (refusals) { // the stopped candidates' stopping pods, against their frozen overlays
+        const PodView pv{fa.stop_cpu, fa.stop_mem, fa.stop_sel, (uint32_t)D};
+        fa.req = fa.stop_req;
+        fa.group = fa.stop_grp;
+        fa.stopped = da.failed;
+        fa.refused = h.dev(refused);
+        DrainArgs dz = da;
+        dz.failed = da.ov_cnt + 2 * D; // zeros: every slot's skip word is its destinations'
+        const cudaError_t e = launch_fit_drain_refusals(nt, pv, dz, fa, fit_drain_grid((uint32_t)D, s->Npad, s->sms), st);
+        if (e != cudaSuccess) return fail(KS_ERR_CUDA, "fit drain refusal pass launch failed: %s", cudaGetErrorString(e));
+    }
+    CU_TRY(h.finish(st));
+    s->last_path = "fit_drain";
     return KS_OK;
 }
 

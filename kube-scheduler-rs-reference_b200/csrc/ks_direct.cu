@@ -9,6 +9,8 @@
 //       k_preempt_emit         chunk merge, victim list and ks_preemption row
 //   K2q k_fit_preempt_scan     the same under the full filter (ks_fit_preempt): rule words, scalar resources, pod count;
 //       k_fit_preempt_emit     its merge, victim list, row and unresolvable count
+//   K2u k_fit_drain_scan       ks_drain_check's scan under the full filter (ks_fit_drain_check), and its refusal pass;
+//       k_fit_drain_commit     its commit, with the overlay's resource columns
 // K2d, K2e, K2k, K2p and K2q share one node-tile scan (scan_node_tiles): tiles staged through shared memory by TMA bulk
 // copies (cp.async.bulk + mbarrier), one lane per node, several pods per warp in registers.
 // The per-cell kernel is the generic path (any score policy, any P); ks_bitpar.cu holds the bit-parallel
@@ -1141,6 +1143,256 @@ __global__ void __launch_bounds__(256)
     }
 }
 
+// ------------------------------------------------------------------------------------------------ K2u (ks_fit_drain_check)
+// K2r under the full filter (include/ksched.h, ks_fit_drain_check).  A destination that passes cpu, memory and the
+// selector also needs its class's rule word (one coalesced load per node) and, for each resource the pod requests, its
+// free amount: node_free in the scan, the overlay's ov_fr column in the commit.  Scores stay the policy's over f.
+// COUNT: the refusal pass after the last round, over the stopping pods of the stopped candidates (fa.stopped), whose
+// overlays are frozen since their stop.  Each destination lands in one of four words by the first filter it fails; the
+// scan counts the nodes off the overlay, the warp of node chunk 0 then the overlay nodes, so the words sum to the
+// destination count.  One pod per warp (FIT_DRAIN_PODS_PER_WARP): with K2d's 2-8 the scan took 236-255 registers at
+// W = 1 and 2, spilled in the refusal pass, and the c3 sweep ran 31% slower (DESIGN.md 5u).
+template <int W, int POLICY, bool COUNT>
+__global__ void __launch_bounds__(DIRECT_THREADS, 1)
+    k_fit_drain_scan(NodeTable nt, PodView pv, DrainArgs da, FitDrainArgs fa, PartialView part, uint32_t tiles_per_chunk) {
+    constexpr int PW = FIT_DRAIN_PODS_PER_WARP;
+    constexpr bool ALLOC = !COUNT && POLICY != KS_SCORE_LEFTOVER; // scored from the allocatables
+    __shared__ int64_t s_req[DIRECT_THREADS / 32][PW][KS_BIND_MAX_RESOURCES];
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t q0 = warp_first_pod<PW>(); // the p0 scan_node_tiles sets
+    bool dead = true; // every pod of this warp is done (or there is none)
+#pragma unroll
+    for (int i = 0; i < PW; i++)
+        if (q0 + i < pv.P && (COUNT ? fa.stopped[q0 + i] != 0 : !da.failed[q0 + i])) dead = false;
+    if (__syncthreads_and(dead)) return; // the whole CTA: nothing to scan
+    int64_t rc[PW], rm[PW];
+    uint64_t sel[PW][W];
+    uint32_t p0;
+    int64_t best[PW];
+    int32_t bidx[PW];
+    uint32_t skip[PW], cur[PW];
+    uint32_t rmask[PW], rrow[PW]; // non-zero requests; the class's first rule word
+    uint32_t nref[PW][4];         // COUNT: the four words
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        const uint32_t p = min(q0 + i, pv.P - 1);
+        // COUNT: the commit wrote a slot's stop record only if its candidate stopped; any other slot reads as group -1
+        // with no request, so that its leftover bytes index nothing (its counts are never written)
+        const bool live = !COUNT || fa.stopped[p] != 0;
+        rrow[i] = __ldg(fa.ncls + (live ? __ldg(fa.group + p) : -1) + 1) * nt.N;
+        const int64_t q = live && lane < fa.R ? __ldg(fa.req + (size_t)p * fa.R + lane) : 0;
+        if (lane < KS_BIND_MAX_RESOURCES) s_req[warp][i][lane] = q;
+        rmask[i] = __ballot_sync(0xffffffffu, q != 0) & ((1u << KS_BIND_MAX_RESOURCES) - 1u);
+        best[i] = INT64_MIN;
+        bidx[i] = -1;
+        skip[i] = 0;
+        cur[i] = 0;
+        nref[i][0] = nref[i][1] = nref[i][2] = nref[i][3] = 0;
+    }
+    __syncwarp();
+
+    scan_node_tiles<W, ALLOC>(
+        nt, tiles_per_chunk, pv, p0, rc, rm, sel,
+        [&](uint32_t g, uint32_t node, bool real, int64_t fc, int64_t fm, const uint64_t(&lab)[W], int64_t ac, int64_t am) {
+            if (g == 0) { // first group of a tile: this tile's skip words
+                const uint32_t tb = node - lane;
+                const uint32_t xw = da.excl ? __ldg(da.excl + tb / 32 + lane) : 0u;
+#pragma unroll
+                for (int i = 0; i < PW; i++) skip[i] = drain_skip_word(da, min(p0 + i, pv.P - 1), tb, xw, cur[i]);
+            }
+#pragma unroll
+            for (int i = 0; i < PW; i++) {
+                uint64_t miss = 0;
+#pragma unroll
+                for (int w = 0; w < W; w++) miss |= sel[i][w] & ~lab[w];
+                const bool off = (__shfl_sync(0xffffffffu, skip[i], g) >> lane) & 1u;
+                const bool dest = real && !off;
+                const bool pass = dest && (rc[i] <= fc) && (rm[i] <= fm) && miss == 0;
+                uint32_t word = 0;
+                bool fit_r = true;
+                if (pass) {
+                    word = __ldg(fa.nrules + rrow[i] + node) & NR_REASON;
+#pragma unroll
+                    for (uint32_t r = 0; r < KS_BIND_MAX_RESOURCES; r++)
+                        if (rmask[i] >> r & 1u) fit_r &= s_req[warp][i][r] <= __ldg(fa.node_free + (size_t)r * nt.N + node);
+                }
+                if (COUNT) {
+                    nref[i][0] += __popc(__ballot_sync(0xffffffffu, dest && !pass));
+                    nref[i][1] += __popc(__ballot_sync(0xffffffffu, pass && !fit_r));
+                    nref[i][2] += __popc(__ballot_sync(0xffffffffu, pass && fit_r && word == NR_TAINT));
+                    nref[i][3] += __popc(__ballot_sync(0xffffffffu, pass && fit_r && word == NR_AFFINITY));
+                } else if (pass && fit_r && word == 0) {
+                    const int64_t key = ALLOC ? alloc_score<POLICY>(fc, fm, ac, am, rc[i], rm[i]) : leftover_key(fc, fm);
+                    if (key > best[i]) {
+                        best[i] = key;
+                        bidx[i] = (int32_t)node;
+                    }
+                }
+            }
+        },
+        [](uint32_t) {});
+
+#pragma unroll
+    for (int i = 0; i < PW; i++) {
+        const uint32_t p = p0 + i;
+        if (!COUNT) {
+            int64_t k = best[i];
+            int32_t ix = bidx[i];
+            warp_argmax(k, ix);
+            if (lane == 0 && p < pv.P) {
+                const uint64_t o = (uint64_t)blockIdx.y * pv.P + p;
+                part.key[o] = k;
+                part.idx[o] = ix;
+            }
+            continue;
+        }
+        if (p >= pv.P || !fa.stopped[p]) continue; // warp-uniform
+        if (blockIdx.y == 0) { // the overlay nodes, against f and f_r
+            const uint32_t n = da.ov_cnt[p], base = da.pod_base[p];
+            for (uint32_t k0 = 0; k0 < n; k0 += 32) {
+                const uint32_t k = k0 + lane;
+                const bool v = k < n;
+                const int32_t node = v ? da.ov_node[base + k] : 0;
+                uint64_t miss = 0;
+#pragma unroll
+                for (int w = 0; w < W; w++) miss |= sel[i][w] & ~nt.labels[(uint64_t)w * nt.Npad + node];
+                const bool pass = v && rc[i] <= da.ov_fc[base + k] && rm[i] <= da.ov_fm[base + k] && miss == 0;
+                uint32_t word = 0;
+                bool fit_r = true;
+                if (pass) {
+                    word = fa.nrules[rrow[i] + node] & NR_REASON;
+                    for (uint32_t r = 0; r < fa.R; r++)
+                        if (rmask[i] >> r & 1u) fit_r &= s_req[warp][i][r] <= fa.ov_fr[(size_t)r * fa.P + base + k];
+                }
+                nref[i][0] += __popc(__ballot_sync(0xffffffffu, v && !pass));
+                nref[i][1] += __popc(__ballot_sync(0xffffffffu, pass && !fit_r));
+                nref[i][2] += __popc(__ballot_sync(0xffffffffu, pass && fit_r && word == NR_TAINT));
+                nref[i][3] += __popc(__ballot_sync(0xffffffffu, pass && fit_r && word == NR_AFFINITY));
+            }
+        }
+        const uint32_t c = lane == 0 ? nref[i][0] : lane == 1 ? nref[i][1] : lane == 2 ? nref[i][2] : nref[i][3];
+        if (lane < 4 && c) atomicAdd(fa.refused + 4 * (size_t)da.cand_id[p] + lane, c); // integer adds: any order
+    }
+}
+
+// k_drain_commit with the full filter: an overlay node also needs the class's rule word to pass and each requested
+// resource to fit its ov_fr column; the move charges f_r along with f, and an insert shifts the R columns with the
+// rest.  A candidate that stops leaves its stopping pod in the stop arrays when fa.stop_cpu is set.
+template <int W, int POLICY>
+__global__ void __launch_bounds__(256, 1)
+    k_fit_drain_commit(NodeTable nt, PodView pv, DrainArgs da, FitDrainArgs fa, PartialView part, uint32_t n_chunks,
+                       uint32_t r) {
+    constexpr bool ALLOC = POLICY != KS_SCORE_LEFTOVER; // scored from the allocatables
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (p >= pv.P || da.failed[p]) return; // warp-uniform
+    const int64_t rc = pv.req_cpu[p], rm = pv.req_mem[p];
+    const uint64_t* sel = pv.sel + (uint64_t)p * W; // read where it is used: nothing but the loop state lives across
+    const uint32_t R = fa.R;                        // alloc_score's int64 divisions
+    const int64_t* req = fa.req + (size_t)p * R;
+    const uint32_t rmask = __ballot_sync(0xffffffffu, lane < R && req[lane] != 0); // the requested resources
+    const uint32_t rrow = fa.ncls[fa.group[p] + 1] * nt.N;
+    int64_t key = INT64_MIN;
+    int32_t idx = -1;
+    for (uint32_t ch = lane; ch < n_chunks; ch += 32) { // each lane's chunks in ascending order
+        const uint64_t o = (uint64_t)ch * pv.P + p;
+        merge_partial(key, idx, part.key[o], part.idx[o]);
+    }
+    const uint32_t n = da.ov_cnt[p], base = da.pod_base[p];
+#pragma unroll 1
+    for (uint32_t k0 = 0; k0 < n; k0 += 32) {
+        const uint32_t k = k0 + lane;
+        const int32_t node = k < n ? da.ov_node[base + k] : 0;
+        const int64_t fc = k < n ? da.ov_fc[base + k] : 0, fm = k < n ? da.ov_fm[base + k] : 0;
+        uint64_t miss = 0;
+#pragma unroll
+        for (int w = 0; w < W; w++) miss |= sel[w] & ~nt.labels[(uint64_t)w * nt.Npad + node];
+        bool ok = k < n && rc <= fc && rm <= fm && miss == 0 && (fa.nrules[rrow + node] & NR_REASON) == 0;
+        for (uint32_t m = rmask; m; m &= m - 1) { // a zero request always fits
+            const uint32_t j = __ffs(m) - 1;
+            if (ok) ok = req[j] <= fa.ov_fr[(size_t)j * fa.P + base + k];
+        }
+        if (ok) {
+            const int64_t kk = ALLOC ? alloc_score<POLICY>(fc, fm, nt.alloc_cpu[node], nt.alloc_mem[node], rc, rm) : leftover_key(fc, fm);
+            if (topk_beats(kk, node, key, idx)) {
+                key = kk;
+                idx = node;
+            }
+        }
+    }
+    warp_argmax(key, idx);
+    const int64_t rq = lane < R ? req[lane] : 0; // lane j: the request of resource j
+    if (idx < 0) {
+        if (fa.stop_cpu) { // the stopping pod, for the refusal pass
+            if (lane == 0) {
+                fa.stop_cpu[p] = rc;
+                fa.stop_mem[p] = rm;
+                fa.stop_grp[p] = fa.group[p];
+            }
+            if (lane < W) fa.stop_sel[(uint64_t)p * W + lane] = pv.sel[(uint64_t)p * W + lane];
+            if (lane < R) fa.stop_req[(size_t)p * R + lane] = rq;
+        }
+        if (lane == 0) da.failed[p] = 1;
+        return;
+    }
+    const uint32_t pod = da.pod_base[p] + r;
+    if (lane == 0) {
+        da.out_idx[pod] = idx;
+        da.out_score[pod] = ALLOC ? key : leftover_score(key, rc, rm);
+        da.placed[da.cand_id[p]] = r + 1;
+    }
+    uint32_t pos = 0; // entries below idx
+    bool found = false;
+    for (uint32_t k0 = 0; k0 < n; k0 += 32) {
+        const uint32_t k = k0 + lane;
+        const int32_t v = k < n ? da.ov_node[base + k] : INT32_MAX;
+        pos += __popc(__ballot_sync(0xffffffffu, v < idx));
+        found |= __any_sync(0xffffffffu, v == idx);
+    }
+    if (found) {
+        if (lane == 0) {
+            da.ov_fc[base + pos] -= rc;
+            da.ov_fm[base + pos] -= rm;
+        }
+        if (lane < R) fa.ov_fr[(size_t)lane * fa.P + base + pos] -= rq;
+        return;
+    }
+    for (uint32_t top = n; top > pos; top = top > pos + 32 ? top - 32 : pos) { // shift [pos, n) up one, top chunk first
+        const int64_t k = (int64_t)top - 1 - lane;
+        const bool mv = k >= (int64_t)pos;
+        int32_t vn = 0;
+        int64_t vc = 0, vm = 0;
+        if (mv) {
+            vn = da.ov_node[base + k];
+            vc = da.ov_fc[base + k];
+            vm = da.ov_fm[base + k];
+        }
+        __syncwarp();
+        if (mv) {
+            da.ov_node[base + k + 1] = vn;
+            da.ov_fc[base + k + 1] = vc;
+            da.ov_fm[base + k + 1] = vm;
+        }
+        __syncwarp();
+#pragma unroll 1
+        for (uint32_t j = 0; j < R; j++) { // the R columns, one at a time
+            int64_t* col = fa.ov_fr + (size_t)j * fa.P + base;
+            const int64_t v = mv ? col[k] : 0;
+            __syncwarp();
+            if (mv) col[k + 1] = v;
+            __syncwarp();
+        }
+    }
+    if (lane == 0) {
+        da.ov_node[base + pos] = idx;
+        da.ov_fc[base + pos] = nt.free_cpu[idx] - rc;
+        da.ov_fm[base + pos] = nt.free_mem[idx] - rm;
+        da.ov_cnt[p] = n + 1;
+    }
+    if (lane < R)
+        fa.ov_fr[(size_t)lane * fa.P + base + pos] = fa.node_free[(size_t)lane * nt.N + idx] - rq;
+}
+
 // ---- the victim index, built per call: a stable LSD radix sort of (node << 32 | priority + 2^31) keys over the bound
 // list fed in descending bound index, then segment offsets, prefix sums and per-node minimum priorities.
 constexpr uint32_t RADIX_TILE = 2048; // keys per CTA of a radix pass (256 threads x 8 rounds)
@@ -1449,6 +1701,8 @@ DirectGrid fit_preempt_grid(uint32_t P, uint32_t Npad, int sms) {
     return direct_grid_ppw(FIT_PREEMPT_PODS_PER_WARP, P, Npad, sms);
 }
 
+DirectGrid fit_drain_grid(uint32_t P, uint32_t Npad, int sms) { return direct_grid_ppw(FIT_DRAIN_PODS_PER_WARP, P, Npad, sms); }
+
 // opt-in shared memory sizes of every K2d / K2e kernel on the current device (must not run inside a stream capture)
 cudaError_t prepare_direct() {
     cudaError_t e = cudaSuccess;
@@ -1461,6 +1715,7 @@ cudaError_t prepare_direct() {
             opt_in(k_explain_counts<W_>, tile_smem_bytes<W_, false>());
             opt_in(k_preempt_scan<W_>, tile_smem_bytes<W_, false>());
             opt_in(k_fit_preempt_scan<W_>, tile_smem_bytes<W_, false>());
+            opt_in(k_fit_drain_scan<W_, KS_SCORE_LEFTOVER, true>, tile_smem_bytes<W_, false>());
             for (int policy : {KS_SCORE_LEFTOVER, KS_SCORE_LEAST_ALLOCATED, KS_SCORE_MOST_ALLOCATED, KS_SCORE_LEAST_BALANCED})
                 with_policy(policy, [&](auto pol) {
                     constexpr int POL = decltype(pol)::value;
@@ -1469,6 +1724,7 @@ cudaError_t prepare_direct() {
                     opt_in(k_select_direct<W_, POL, false>, SMEM);
                     opt_in(k_select_topk<W_, POL>, SMEM);
                     opt_in(k_drain_scan<W_, POL>, SMEM);
+                    opt_in(k_fit_drain_scan<W_, POL, false>, SMEM);
                     return e;
                 });
             return e;
@@ -1601,6 +1857,41 @@ cudaError_t launch_drain_round(const NodeTable& nt, const PodView& pv, const Dra
         return with_policy(policy, [&](auto pol) {
             return launch_drain_t<W, decltype(pol)::value>(nt, pv, da, r, part, g, st);
         });
+    });
+}
+
+template <int W, int POLICY>
+static cudaError_t launch_fit_drain_t(const NodeTable& nt, const PodView& pv, const DrainArgs& da, const FitDrainArgs& fa,
+                                      uint32_t r, const PartialView& part, const DirectGrid& g, cudaStream_t st) {
+    constexpr uint32_t SMEM = tile_smem_bytes<W, POLICY != KS_SCORE_LEFTOVER>();
+    k_fit_drain_scan<W, POLICY, false><<<dim3(g.pod_ctas, g.n_chunks), DIRECT_THREADS, SMEM, st>>>(nt, pv, da, fa, part,
+                                                                                                   g.tiles_per_chunk);
+    k_fit_drain_commit<W, POLICY><<<(pv.P + 7) / 8, 256, 0, st>>>(nt, pv, da, fa, part, g.n_chunks, r);
+    g_launches += 2;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_fit_drain_round(const NodeTable& nt, const PodView& pv, const DrainArgs& da, const FitDrainArgs& fa,
+                                   int policy, uint32_t r, const PartialView& part, const DirectGrid& g, cudaStream_t st) {
+    if (pv.P == 0) return cudaSuccess;
+    return with_label_width(nt.W, [&](auto w) {
+        constexpr int W = decltype(w)::value;
+        return with_policy(policy, [&](auto pol) {
+            return launch_fit_drain_t<W, decltype(pol)::value>(nt, pv, da, fa, r, part, g, st);
+        });
+    });
+}
+
+cudaError_t launch_fit_drain_refusals(const NodeTable& nt, const PodView& pv, const DrainArgs& da,
+                                      const FitDrainArgs& fa, const DirectGrid& g, cudaStream_t st) {
+    if (pv.P == 0) return cudaSuccess;
+    return with_label_width(nt.W, [&](auto w) {
+        constexpr int W = decltype(w)::value;
+        k_fit_drain_scan<W, KS_SCORE_LEFTOVER, true><<<dim3(g.pod_ctas, g.n_chunks), DIRECT_THREADS,
+                                                       tile_smem_bytes<W, false>(), st>>>(nt, pv, da, fa, PartialView{},
+                                                                                          g.tiles_per_chunk);
+        g_launches++;
+        return cudaGetLastError();
     });
 }
 

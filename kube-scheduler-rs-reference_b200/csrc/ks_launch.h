@@ -118,6 +118,38 @@ struct DrainArgs {
 cudaError_t launch_drain_round(const NodeTable& nt, const PodView& pv, const DrainArgs& da, int policy, uint32_t r,
                                const PartialView& part, const DirectGrid& g, cudaStream_t st);
 
+// drain simulation under the full filter (ks_fit_drain_check).  DrainArgs for the candidates and the overlay, plus what
+// the scan and the commit read beyond ks_drain_check's inputs: the round's pod requests and groups, the free amounts and
+// the rule words of ks_node_bind, and R more overlay columns.  With refusal words, the commit that stops a candidate
+// copies its stopping pod to the candidate's slot of the stop arrays, and one counting scan over those slots follows the
+// last round.  Device memory.
+struct FitDrainArgs {
+    uint32_t R;                // [0, KS_BIND_MAX_RESOURCES]
+    uint32_t P;                // pods of the call: the stride of ov_fr's columns
+    const int64_t* req;        // [P_r * R]: the round's pod j's request of r at j * R + r (the count pass: stop_req)
+    const int32_t* group;      // [P_r]: the round's pods' groups, each in [-1, G) (the count pass: stop_grp)
+    const int64_t* node_free;  // [R * N]
+    const uint32_t* ncls;      // [G + 1]: the class of group g at g + 1, of group -1 at 0
+    const uint32_t* nrules;    // [C * N], written by k_node_rules_setup
+    int64_t* ov_fr;            // [R * P]: f_r of overlay entry k of candidate j at r * P + pod_base[j] + k
+    int64_t *stop_cpu, *stop_mem; // [D] the stopping pod of candidate slot j; all five null without refusal words
+    uint64_t* stop_sel;        // [D * W]
+    int64_t* stop_req;         // [D * R]
+    int32_t* stop_grp;         // [D]
+    const uint32_t* stopped;   // [D] the count pass: the rounds' failed flags (its own DrainArgs::failed reads 0)
+    uint32_t* refused;         // [4 * D] caller's order, zeroed before the count pass
+};
+// k_fit_drain_scan's pods per warp, and its launch geometry (direct_grid's rule)
+constexpr uint32_t FIT_DRAIN_PODS_PER_WARP = 1;
+DirectGrid fit_drain_grid(uint32_t P, uint32_t Npad, int sms);
+// one round of ks_fit_drain_check: the scan for pod r of the pv.P running candidates, then their commit.  part holds
+// g.n_chunks * pv.P keys and indices.
+cudaError_t launch_fit_drain_round(const NodeTable& nt, const PodView& pv, const DrainArgs& da, const FitDrainArgs& fa,
+                                   int policy, uint32_t r, const PartialView& part, const DirectGrid& g, cudaStream_t st);
+// the refusal words after the last round: the counting scan over the D candidate slots, pv = the stop arrays
+cudaError_t launch_fit_drain_refusals(const NodeTable& nt, const PodView& pv, const DrainArgs& da,
+                                      const FitDrainArgs& fa, const DirectGrid& g, cudaStream_t st);
+
 // scale-up estimate (ks_scaleup_estimate, ks_scaleup.cu).  T templates, each packed on its own by one CTA of
 // k_scaleup_pack; the grid holds `slots` CTAs, CTA b takes templates b, b + slots, ... and sorts in its own scratch
 // slot of 2 * pv.P entries.  Device memory.

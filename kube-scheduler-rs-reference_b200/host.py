@@ -68,6 +68,8 @@ for _name, _res, _args in [
                                           C.c_size_t, _vp]),
     ("ksh_preempt_fit_pods", C.c_int, [_vp, _vp, C.c_uint64, _vp, C.c_uint32, _vp, _vp, C.c_uint32, _vp, _vp,
                                        C.c_size_t, _vp]),
+    ("ksh_drain_fit_nodes", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, _vp, C.c_uint32, _vp, C.c_int, C.c_uint32, _vp,
+                                      _vp, _vp]),
 ]:
     _proto(_name, _res, *_args)
 
@@ -716,6 +718,35 @@ class Context:
                                   pod_offset.ctypes.data, int(policy), int(flags), placed.ctypes.data,
                                   node.ctypes.data), "ksh_drain_nodes")
         return placed, node
+
+    def drain_fit_nodes(self, node_names, pods, pod_offset, group, n_groups, group_rules=None,
+                        policy=capi.KS_SCORE_LEFTOVER, flags=0, want_refused=True):
+        """Drain simulation under the full filter (ksh_drain_fit_nodes): drain_nodes with group [P] and group_rules
+        [n_groups] as preempt_fit_pods takes them (None: no toleration and no term); the context's taints, the drained
+        pods' extended resources and the pod limit apply.  Returns (placed[D], node_idx[P], refused[D, 4] or None)."""
+        pod_offset = np.ascontiguousarray(pod_offset, np.uint64).reshape(-1)
+        d = len(node_names)
+        if pod_offset.shape[0] != d + 1:
+            raise ValueError(f"need len(pod_offset) == len(node_names) + 1 (got {pod_offset.shape[0]} and {d})")
+        p = int(pod_offset[-1])
+        group = np.ascontiguousarray(group, np.int32).reshape(-1)
+        if group.shape[0] != p:
+            raise ValueError(f"group has {group.shape[0]} entries, pods {p}")
+        nr = None
+        if group_rules is not None:
+            if len(group_rules) != n_groups:
+                raise ValueError(f"group_rules has {len(group_rules)} entries, groups {n_groups}")
+            nr = node_rules(group_rules)
+        names = (C.c_char_p * max(d, 1))(*[n.encode() if isinstance(n, str) else n for n in node_names])
+        placed = np.empty(d, np.uint32)
+        node = np.empty(p, np.int32)
+        refused = np.empty((d, 4), np.uint32) if want_refused else None
+        check(lib.ksh_drain_fit_nodes(self._h, C.addressof(names), d, C.addressof(pods) if pods is not None else None,
+                                      pod_offset.ctypes.data, group.ctypes.data, int(n_groups),
+                                      None if nr is None else C.addressof(nr[0]), int(policy), int(flags),
+                                      placed.ctypes.data, node.ctypes.data,
+                                      None if refused is None else refused.ctypes.data), "ksh_drain_fit_nodes")
+        return placed, node, refused
 
     def scaleup_estimate(self, templates, n_templates, max_nodes, pods, n_pods, overhead_pods=None, n_overhead=0,
                          want_nodes=True, want_reasons=True):

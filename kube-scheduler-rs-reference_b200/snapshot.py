@@ -713,6 +713,44 @@ class Snapshot:
               "ks_fit_preempt")
         return rows, victims, unres
 
+    def fit_drain_check(self, req_cpu, req_mem, sel, group, n_groups, node_idx, offset, policy=capi.KS_SCORE_LEFTOVER,
+                        flags=0, rules=None, node_free=None, pod_req=None, want_refused=True):
+        """drain_check under the full filter (ks_fit_drain_check): group [P] and rules as fit_bind takes them (rules
+        None = NULL); node_free [R, N] and pod_req [P, R] (int64), or both None (the C call's NULL res).  Returns
+        drain_check's (placed[D], node_idx[P], score[P]), then refused uint32 [D, 4] (None unless want_refused): why
+        each stopped candidate's stopping pod found no destination."""
+        pods, keep = self._pods(req_cpu, req_mem, sel)
+        p = int(pods.n)
+        group = _c(group, np.int32).reshape(-1)
+        if group.shape[0] != p:
+            raise ValueError(f"group has {group.shape[0]} entries, pods {p}")
+        node_idx = _c(node_idx, np.int32).reshape(-1)
+        offset = _c(offset, np.uint64).reshape(-1)
+        d = node_idx.shape[0]
+        if offset.shape[0] != d + 1:
+            raise ValueError(f"need len(offset) == len(node_idx) + 1 (got {offset.shape[0]} and {d})")
+        if (node_free is None) != (pod_req is None):
+            raise ValueError("node_free and pod_req go together")
+        br = None
+        if node_free is not None:
+            node_free, pod_req = _c(node_free, np.int64), _c(pod_req, np.int64)
+            if node_free.ndim != 2 or node_free.shape[1] != self.n_nodes:
+                raise ValueError(f"node_free has shape {node_free.shape}, expected (R, {self.n_nodes})")
+            r = node_free.shape[0]
+            if pod_req.shape != (p, r):
+                raise ValueError(f"pod_req has shape {pod_req.shape}, expected ({p}, {r})")
+            br = capi.ks_bind_resources(r, _ptr(node_free), _ptr(pod_req))
+        nr, hold = _rules_arg(rules)
+        cand = capi.ks_drain_candidates(d, _ptr(node_idx), _ptr(offset))
+        placed = np.empty(d, np.uint32)
+        idx = np.empty(p, np.int32)
+        score = np.empty(p, np.int64)
+        refused = np.empty((d, 4), np.uint32) if want_refused else None
+        check(lib.ks_fit_drain_check(self._h, C.byref(pods), _ptr(group), int(n_groups), nr,
+                                     None if br is None else C.byref(br), C.byref(cand), int(policy), int(flags),
+                                     _ptr(placed), _ptr(idx), _ptr(score), _ptr(refused)), "ks_fit_drain_check")
+        return placed, idx, score, refused
+
     def last_timings(self):
         ms = (C.c_float * 3)()
         check(lib.ks_last_timings(self._h, ms), "ks_last_timings")
