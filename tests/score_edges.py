@@ -12,13 +12,10 @@ the total tie.  Mutants are source patches of the oracle functions, live only in
 mutants it kills, and test_score_edges.py checks each claim on the CPU.
 
 Regenerate the search fixture (about a minute) with `python tests/score_edges.py --regenerate`."""
-import contextlib
-import inspect
 import json
 import math
 import os
 import sys
-import textwrap
 from dataclasses import dataclass, field
 from fractions import Fraction
 
@@ -26,6 +23,7 @@ import numpy as np
 
 import fit_bind_oracle
 import node_bind_oracle
+import oracle_mutants
 import profile_bind_oracle
 from affinity_bind_oracle import AFFINITY
 from bind_edges import bind_slices, resource_maps
@@ -93,43 +91,9 @@ NEUTRAL = {
 }
 
 
-def _replace(fn, new):
-    """Bind `new` wherever a loaded module holds `fn` (the oracles import each other's functions by name)"""
-    undo = []
-    for m in list(sys.modules.values()):
-        d = getattr(m, "__dict__", None)
-        if not d:
-            continue
-        for k, v in list(d.items()):
-            if v is fn:
-                undo.append((d, k, v))
-                d[k] = new
-    return undo
-
-
-@contextlib.contextmanager
 def mutant(name):
     """The oracle with one mutant's patches applied; restored on exit"""
-    _, funcs, edits = {**MUTANTS, **NEUTRAL}[name]
-    undo = []
-    try:
-        for modname, fname in funcs:
-            mod = sys.modules[modname]
-            fn = getattr(mod, fname)
-            src = textwrap.dedent(inspect.getsource(fn))
-            hit = False
-            for old, new in edits:
-                if old in src:
-                    assert src.count(old) == 1, (name, fname, old)
-                    src, hit = src.replace(old, new), True
-            assert hit, f"mutant {name}: no edit applies to {modname}.{fname}"
-            ns = dict(vars(mod), Fraction=Fraction, np=np, SHARED_BITMAP=SHARED_BITMAP)
-            exec(compile(src, f"<mutant {name} of {modname}.{fname}>", "exec"), ns)
-            undo += _replace(fn, ns[fname])
-        yield
-    finally:
-        for d, k, v in reversed(undo):
-            d[k] = v
+    return oracle_mutants.mutant({**MUTANTS, **NEUTRAL}, name, Fraction=Fraction, np=np, SHARED_BITMAP=SHARED_BITMAP)
 
 
 # ----------------------------------------------------------------------------------------------------------- searches
