@@ -402,6 +402,11 @@ extern "C" {
                               rules: *const ks_node_rules, res: *const ks_bind_resources,
                               cand: *const ks_drain_candidates, policy: c_int, flags: u32, out_placed: *mut u32,
                               out_node_idx: *mut i32, out_score: *mut i64, out_refused: *mut u32) -> c_int;
+    // ks_scaleup_estimate under the full filter, with the templates as the nodes of rules and res (DESIGN.md 5v)
+    pub fn ks_fit_scaleup_estimate(s: *mut ks_snapshot, pods: *const ks_pods, group: *const i32, n_groups: u32,
+                                   rules: *const ks_node_rules, res: *const ks_bind_resources,
+                                   t: *const ks_node_templates, out: *mut ks_scaleup_option, best: *mut i32,
+                                   node: *mut i32, out_refused: *mut u32, out_used: *mut i64) -> c_int;
     // asynchronous streaming surface = the Controller's work queue (src/main.rs:73,141-148)
     pub fn ks_stream_open(s: *mut ks_snapshot, policy: c_int, max_batch: u32, out: *mut *mut ks_stream) -> c_int;
     pub fn ks_stream_submit(q: *mut ks_stream, n: u64, cpu: *const i64, mem: *const i64, sel: *const u64, tickets: *const u64) -> c_int;
@@ -521,6 +526,12 @@ extern "C" {
                                pod_offset: *const u64, group: *const i32, n_groups: u32, rules: *const ksh_node_rules,
                                policy: c_int, flags: u32, placed: *mut u32, node_idx: *mut i32,
                                refused: *mut u32) -> c_int;
+    pub fn ksh_scaleup_fit_estimate(ctx: *mut ksh_context, templates: *const ks_node_obj, n_templates: u64,
+                                    max_nodes: *const u32, template_taint_offset: *const u64,
+                                    template_taints: *const ksh_taint, overhead_pods: *const ks_pod_obj,
+                                    n_overhead: u64, pods: *const ks_pod_obj, n_pods: u64, group: *const i32,
+                                    n_groups: u32, rules: *const ksh_node_rules, out: *mut ks_scaleup_option,
+                                    best: *mut i32, node: *mut i32, refused: *mut u32) -> c_int;
     pub fn ksh_explain_pods(ctx: *mut ksh_context, pods: *const ks_pod_obj, n: u64, out: *mut ks_pod_reasons,
                             messages: *mut c_char, cap: usize, msg_off: *mut i64) -> c_int;
     pub fn ksh_format_unschedulable(n_nodes: u32, r: *const ks_pod_reasons, buf: *mut c_char, cap: usize) -> c_int;

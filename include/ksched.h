@@ -1114,13 +1114,65 @@ int ks_gang_fit_bind(ks_snapshot* s, const ks_pods* pods /* host space */, const
  * completion.
  * Out of scope: PodTopologySpread and InterPodAffinity with the moved pods (upstream re-runs them; they are not inputs
  * here, as in ks_fit_preempt); PodDisruptionBudgets and pod filtering, the caller's job as in ks_drain_check; scoring by
- * TaintToleration and NodeAffinity; NodeUnschedulable other than through its taint; the scale-up estimator and
- * ks_explain under the full filter. */
+ * TaintToleration and NodeAffinity; NodeUnschedulable other than through its taint; ks_explain under the full filter
+ * (the scale-up estimator under it is ks_fit_scaleup_estimate below). */
 int ks_fit_drain_check(ks_snapshot* s, const ks_pods* pods /* host space */, const int32_t* group /* [P] */,
                        uint32_t n_groups, const struct ks_node_rules* rules /* or NULL */,
                        const struct ks_bind_resources* res /* or NULL */, const ks_drain_candidates* cand, int policy,
                        uint32_t flags, uint32_t* out_placed /* [n] */, int32_t* out_node_idx /* [P] */,
                        int64_t* out_score /* [P] or NULL */, uint32_t* out_refused /* [4n] or NULL */);
+
+/* ---- scale-up estimate under the full filter: ks_scaleup_estimate with the pod count, scalar resources, taints and
+ * required node affinity on the new nodes (cluster-autoscaler's binpacking estimator and Karpenter's instance-type
+ * sizing running the scheduler's filters against a template node; spec extension, DESIGN.md 5v) ----
+ * ks_scaleup_estimate's steps 1-7 (above), changed only where written here.  The templates play the part of the nodes
+ * in `group`, `rules` and `res`, which mean what they mean for ks_fit_bind with N = T: rules->node_taint_hard/soft[t]
+ * and rules->node_domain[k][t] are template t's; group -1 tolerates nothing and has no node affinity;
+ * res->node_free[r * T + t] is the amount of resource r on one empty node of template t (its allocatable minus its
+ * DaemonSet pods' requests; for the pod count, minus their number; any value in [-2^52, 2^52]) and
+ * res->pod_req[p * R + r] >= 0 pod p's request.
+ *   1. eligible: pod p is eligible for t iff it passes ks_fit_bind's filter on an empty node of t: cpu and memory <= F
+ *      (no zero skip) and the selector; each resource with upstream's zero skip (pod_req == 0 or pod_req <= node_free);
+ *      no hard taint of t that p's group does not tolerate; the group's required node affinity;
+ *   2. order: unchanged (the cpu/memory key; cluster-autoscaler's decreasing-size orderer scores cpu and memory only);
+ *   3. first fit: each open node keeps a remaining amount of every resource, starting from node_free[r * T + t]; a pod
+ *      fits an open node when cpu, memory and every resource it requests (zero skip) fit the node's remaining amounts,
+ *      and placing it subtracts all its requests.  Opening a node, max_nodes and skipping a pod that fits nowhere are
+ *      unchanged;
+ *   4. out[t] and *out_best as ks_scaleup_estimate's (utilization over cpu and memory); out_used[t * R + r] (may be
+ *      NULL) = the sum of resource r over t's placed pods, so a caller can weigh GPU waste between groups;
+ *   5. out_refused[4p .. 4p + 3] (may be NULL) count the templates by the first filter each fails, in ks_fit_bind's
+ *      order: word 0 cpu, memory or the selector; word 1 a resource; word 2 an untolerated hard taint; word 3 required
+ *      node affinity.  With the templates p is eligible for they sum to T (ks_fit_drain_check's word layout);
+ *   6. nothing is charged: free[], the bit-parallel index and the snapshot are unchanged.  rules->weight_* and preferred
+ *      terms are checked as ks_node_bind checks them and play no part.
+ * Identities:
+ *   (E1) rules and res NULL (any groups): out, *out_best and out_node are ks_scaleup_estimate's, bit for bit; out_refused
+ *        word 0 is its not_enough_resources + node_selector_mismatch and words 1-3 are 0;
+ *   (E2) an extra resource that copies cpu (pod_req each pod's positive cpu request, node_free the template's cpu
+ *        capacity F) changes nothing;
+ *   (E3) no template carries a taint, no group has a node-affinity term and every node_free is at least the queue's
+ *        total request of its resource: rows, best and nodes are E1's;
+ *   (E4) replaying each template's out_node, every opened node's summed requests fit F and every node_free in every
+ *        dimension (zero skip), and every placed pod is eligible;
+ *   (E5) for every pod, the four refusal words plus its eligible-template count equal T;
+ *   (E6) splitting the templates over calls gives the same rows, as for ks_scaleup_estimate.
+ * Checked on the host before any device work: every check of ks_scaleup_estimate; ks_fit_bind's checks on group
+ * (KS_ERR_INVALID for a NULL group with pods->n > 0 or one outside [-1, G), KS_ERR_RANGE for G >
+ * KS_SPREAD_BIND_MAX_GROUPS), rules (with N = T) and res; KS_ERR_RANGE for a node_free outside [-2^52, 2^52], which with
+ * at most KS_SCALEUP_MAX_NODES nodes per template keeps every per-node remainder and every out_used sum inside int64.
+ * n = 0 or pods->n = 0 needs no device work: rows, words and sums are zero and *out_best = -1.
+ * One H2D copy (pods, groups, pod_req, templates, node_free, rules), k_node_rules_setup over the templates, one packing
+ * kernel, with out_refused one reasons kernel, and one D2H copy; the best template is picked on the host.
+ * Out of scope: PodTopologySpread and InterPodAffinity on the new nodes; startup and ignored taints (the caller passes
+ * the taints it wants counted); cluster-autoscaler's "last node first" fit heuristic and other expanders; existing
+ * nodes (run a bind call first, as in 5g, and pass the pods it leaves unplaced). */
+int ks_fit_scaleup_estimate(ks_snapshot* s, const ks_pods* pods /* host space */, const int32_t* group /* [P] */,
+                            uint32_t n_groups, const struct ks_node_rules* rules /* node arrays over templates, or NULL */,
+                            const struct ks_bind_resources* res /* node_free [R * T], or NULL */,
+                            const ks_node_templates* t, ks_scaleup_option* out /* [T] */, int32_t* out_best,
+                            int32_t* out_node /* [T * P] or NULL */, uint32_t* out_refused /* [4P] or NULL */,
+                            int64_t* out_used /* [T * R] or NULL */);
 
 #ifdef __cplusplus
 }

@@ -472,6 +472,26 @@ int ksh_drain_fit_nodes(ksh_context* ctx, const char* const* node_names, uint64_
                         const ksh_node_rules* rules /* or NULL */, int policy, uint32_t flags, uint32_t* out_placed,
                         int32_t* out_node_idx, uint32_t* out_refused /* [4n] or NULL */);
 
+/* Node-group scale-up estimate under the full filter over objects (ks_fit_scaleup_estimate, DESIGN.md 5v):
+ * ksh_scaleup_estimate's arguments, checks and packing (templates, overhead pods, the call-local label dictionary) plus
+ * group[n_pods] in [-1, n_groups) and rules (NULL allowed), as ksh_drain_fit_nodes takes them, and each template's
+ * spec.taints: template t carries template_taints[template_taint_offset[t] .. template_taint_offset[t + 1])
+ * (template_taint_offset [n_templates + 1] or NULL: none), checked as ksh_context_set_node_taints checks a node's.
+ * Templates are not in the context's node store, so the rules are compiled over the templates: the taint bits from
+ * their taints, and each node-affinity key's domains from their labels, numbered by first appearance in template order.
+ * The resources are the batch's, as ksh_compile_resources builds them over `pods` ("pods" first), and a template's
+ * node_free is its allocatable of each name (0 when missing, so a template without "pods" takes no pod, as upstream)
+ * minus its overhead pods' requests and, for "pods", their number.  A malformed quantity of a requested resource is
+ * reported as ksh_reconcile_fit reports it, naming the template or overhead pod.  The context's node store, bound list
+ * and snapshot are not changed.  Outputs as ks_fit_scaleup_estimate gives them (out_used is not returned here).
+ * KS_ERR_NO_DEVICE on a packing-only context, after every check. */
+int ksh_scaleup_fit_estimate(ksh_context* ctx, const ks_node_obj* templates, uint64_t n_templates,
+                             const uint32_t* max_nodes, const uint64_t* template_taint_offset /* [T + 1] or NULL */,
+                             const ksh_taint* template_taints, const ks_pod_obj* overhead_pods, uint64_t n_overhead,
+                             const ks_pod_obj* pods, uint64_t n_pods, const int32_t* group, uint32_t n_groups,
+                             const ksh_node_rules* rules /* or NULL */, ks_scaleup_option* out, int32_t* out_best,
+                             int32_t* out_node /* [T * n_pods] or NULL */, uint32_t* out_refused /* [4 n_pods] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -284,6 +284,9 @@ _proto("ks_fit_preempt", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.
 _proto("ks_fit_drain_check", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_uint32, C.POINTER(ks_node_rules),
        C.POINTER(ks_bind_resources), C.POINTER(ks_drain_candidates), C.c_int, C.c_uint32, C.c_void_p, C.c_void_p,
        C.c_void_p, C.c_void_p, optional=True)
+_proto("ks_fit_scaleup_estimate", C.c_int, C.c_void_p, C.POINTER(ks_pods), C.c_void_p, C.c_uint32,
+       C.POINTER(ks_node_rules), C.POINTER(ks_bind_resources), C.POINTER(ks_node_templates), C.c_void_p, C.c_void_p,
+       C.c_void_p, C.c_void_p, C.c_void_p, optional=True)
 KS_AFFINITY_MAX_TERMS = 16384
 KS_AFFINITY_MAX_TARGETS = 1 << 22
 KS_AFFINITY_MAX_EXISTING = 1 << 24

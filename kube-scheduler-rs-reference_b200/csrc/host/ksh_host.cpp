@@ -12,6 +12,7 @@
 #include <array>
 #include <atomic>
 #include <cstdlib>
+#include <functional>
 #include <mutex>
 #include <thread>
 #include <unordered_map>
@@ -31,6 +32,7 @@ extern "C" void ks__set_error(const char* msg); // defined in ks_api.cu (not par
 #pragma weak ks_gang_bind
 #pragma weak ks_drain_check
 #pragma weak ks_scaleup_estimate
+#pragma weak ks_fit_scaleup_estimate
 #pragma weak ks_place_replicas
 #pragma weak ks_place_replicas_spread
 #pragma weak ks_place_replicas_spread_multi
@@ -1846,10 +1848,40 @@ static bool tolerates(const ksh_toleration& t, const std::array<std::string, 3>&
     return nz(t.value) == taint[1]; // "" or Equal
 }
 
-static int compile_node_rules(ksh_context* c, uint32_t G, const ksh_node_rules* in, CompiledNodeRules* out) {
+// The node side of a rule compilation: the store's nodes (store_nodes) or a call's node templates.  taints_of(n) is node
+// n's spec.taints (NULL: none); domains(key, dom, values) numbers the key's values over the nodes as topology_domains
+// does, dom[n] = -1 for a node without the key, values[d] = domain d's value.
+using Taint = std::array<std::string, 3>; // key, value, effect
+struct RuleNodes {
+    uint32_t N = 0;
+    const char* what = ""; // in the too-many-taints message
+    std::function<const std::vector<Taint>*(uint32_t)> taints_of;
+    std::function<void(const std::string&, int32_t*, std::vector<std::string>*)> domains;
+};
+
+static RuleNodes store_nodes(const ksh_context* c) {
+    RuleNodes nodes;
+    nodes.N = c->N;
+    nodes.what = "the store's nodes";
+    nodes.taints_of = [c](uint32_t n) -> const std::vector<Taint>* {
+        const auto it = c->taints.find(c->names.str(c->idx2nameid[n]));
+        return it == c->taints.end() ? nullptr : &it->second;
+    };
+    nodes.domains = [c](const std::string& key, int32_t* dom, std::vector<std::string>* values) {
+        std::vector<uint32_t> pids;
+        topology_domains(c, key.c_str(), dom, &pids);
+        for (const uint32_t pid : pids) {
+            const char* k = c->pairs.str(pid);
+            values->emplace_back(k + std::strlen(k) + 1);
+        }
+    };
+    return nodes;
+}
+
+static int compile_rules_over(const RuleNodes& nodes, uint32_t G, const ksh_node_rules* in, CompiledNodeRules* out) {
     const ksh_node_rules none{};
     if (!in) in = &none;
-    const uint32_t N = c->N, T = in->n_terms;
+    const uint32_t N = nodes.N, T = in->n_terms;
     if (in->toleration_offset && in->toleration_offset[G] && !in->tolerations) return fail(KS_ERR_INVALID, "NULL tolerations");
     if (T && (!in->term_owner || !in->term_weight || !in->term_req_offset))
         return fail(KS_ERR_INVALID, "NULL term_owner, term_weight or term_req_offset");
@@ -1896,18 +1928,18 @@ static int compile_node_rules(ksh_context* c, uint32_t G, const ksh_node_rules* 
     if (keys.size() > KS_NODE_RULES_MAX_KEYS)
         return fail(KS_ERR_RANGE, std::to_string(keys.size()) + " node-affinity keys (at most " +
                                       std::to_string(KS_NODE_RULES_MAX_KEYS) + ")");
-    // taints: the distinct (key, value, effect) triples of the store's nodes, numbered in node order
-    std::vector<std::array<std::string, 3>> triples;
+    // taints: the distinct (key, value, effect) triples of the nodes, numbered in node order
+    std::vector<Taint> triples;
     out->hard.assign(N, 0);
     out->soft.assign(N, 0);
     for (uint32_t n = 0; n < N; n++) {
-        const auto it = c->taints.find(c->names.str(c->idx2nameid[n]));
-        if (it == c->taints.end()) continue;
-        for (const auto& t : it->second) {
+        const std::vector<Taint>* ts = nodes.taints_of(n);
+        if (!ts) continue;
+        for (const auto& t : *ts) {
             size_t b = std::find(triples.begin(), triples.end(), t) - triples.begin();
             if (b == triples.size()) {
                 if (b == KS_NODE_RULES_MAX_TAINTS)
-                    return fail(KS_ERR_RANGE, "more than 64 distinct taints on the store's nodes");
+                    return fail(KS_ERR_RANGE, std::string("more than 64 distinct taints on ") + nodes.what);
                 triples.push_back(t);
             }
             (t[2] == "PreferNoSchedule" ? out->soft : out->hard)[n] |= 1ull << b;
@@ -1923,17 +1955,10 @@ static int compile_node_rules(ksh_context* c, uint32_t G, const ksh_node_rules* 
                 if (triples[b][2] != "PreferNoSchedule") out->tol_h[g] |= 1ull << b;
                 else if (!*nz(t.effect) || std::string(t.effect) == "PreferNoSchedule") out->tol_s[g] |= 1ull << b;
             }
-    // node affinity: each key's domains over the store, each requirement a set over them plus the "absent" bit
+    // node affinity: each key's domains over the nodes, each requirement a set over them plus the "absent" bit
     std::vector<std::vector<std::string>> values(keys.size());
     out->dom.assign(keys.size(), std::vector<int32_t>(N));
-    for (size_t k = 0; k < keys.size(); k++) {
-        std::vector<uint32_t> pids;
-        topology_domains(c, keys[k].c_str(), out->dom[k].data(), &pids);
-        for (const uint32_t pid : pids) {
-            const char* key = c->pairs.str(pid);
-            values[k].emplace_back(key + std::strlen(key) + 1);
-        }
-    }
+    for (size_t k = 0; k < keys.size(); k++) nodes.domains(keys[k], out->dom[k].data(), &values[k]);
     out->set_off.push_back(0);
     out->term_off.push_back(0);
     for (uint32_t t = 0; t < T; t++) {
@@ -1994,6 +2019,11 @@ static int compile_node_rules(ksh_context* c, uint32_t G, const ksh_node_rules* 
     return KS_OK;
 }
 
+// over the store's nodes and their recorded taints
+static int compile_node_rules(ksh_context* c, uint32_t G, const ksh_node_rules* in, CompiledNodeRules* out) {
+    return compile_rules_over(store_nodes(c), G, in, out);
+}
+
 // ---- extended resources (ks_fit_bind, DESIGN.md 5r) ----
 // The scalar resources of a pending batch: "pods", then every other name some pod of the batch requests with a non-zero
 // quantity, in order of first request; node_free [R * N] = allocatable (0 when the node does not list the name) minus
@@ -2013,7 +2043,8 @@ static int ext_error(const ksh_context* c, const std::string& who, const char* w
     return fail(KS_ERR_PARSE, who + ": cannot convert its " + what + c->res_name[e.res] + " to an integer");
 }
 
-static int compile_resources(ksh_context* c, const ks_pod_obj* pods, uint64_t n, CompiledResources* out) {
+// The batch side of compile_resources: ids, and pod_req [n * R]
+static int batch_resources(ksh_context* c, const ks_pod_obj* pods, uint64_t n, CompiledResources* out) {
     const uint32_t pods_id = res_id(c, "pods");
     out->ids.assign(1, pods_id);
     std::vector<std::vector<ExtQty>> req(n);
@@ -2027,10 +2058,25 @@ static int compile_resources(ksh_context* c, const ks_pod_obj* pods, uint64_t n,
             if (std::find(out->ids.begin(), out->ids.end(), e.res) == out->ids.end()) out->ids.push_back(e.res);
         }
     }
-    const size_t R = out->ids.size(), N = c->N;
+    const size_t R = out->ids.size();
     if (R > KS_BIND_MAX_RESOURCES)
         return fail(KS_ERR_RANGE, std::to_string(R) + " resources in one batch, \"pods\" included (at most " +
                                       std::to_string(KS_BIND_MAX_RESOURCES) + "): split the batch");
+    std::vector<int32_t> col(c->res_name.size(), -1);
+    for (size_t r = 0; r < R; r++) col[out->ids[r]] = (int32_t)r;
+    out->pod_req.assign(n * R, 0);
+    for (uint64_t p = 0; p < n; p++) {
+        out->pod_req[p * R] = 1;
+        for (const ExtQty& e : req[p])
+            if (col[e.res] > 0) out->pod_req[p * R + (size_t)col[e.res]] = e.v;
+    }
+    return KS_OK;
+}
+
+static int compile_resources(ksh_context* c, const ks_pod_obj* pods, uint64_t n, CompiledResources* out) {
+    const int rc = batch_resources(c, pods, n, out);
+    if (rc) return rc;
+    const size_t R = out->ids.size(), N = c->N;
     std::vector<int32_t> col(c->res_name.size(), -1);
     for (size_t r = 0; r < R; r++) col[out->ids[r]] = (int32_t)r;
     out->node_free.assign(R * N, 0);
@@ -2054,12 +2100,6 @@ static int compile_resources(ksh_context* c, const ks_pod_obj* pods, uint64_t n,
             over |= __builtin_sub_overflow(f, e.v, &f);
         }
         if (over) return fail(KS_ERR_RANGE, "free resources of a node overflow int64");
-    }
-    out->pod_req.assign(n * R, 0);
-    for (uint64_t p = 0; p < n; p++) {
-        out->pod_req[p * R] = 1;
-        for (const ExtQty& e : req[p])
-            if (col[e.res] > 0) out->pod_req[p * R + (size_t)col[e.res]] = e.v;
     }
     return KS_OK;
 }
@@ -2569,51 +2609,55 @@ int ksh_drain_fit_nodes(ksh_context* c, const char* const* node_names, uint64_t 
 }
 KSH_CATCH
 
-int ksh_scaleup_estimate(ksh_context* c, const ks_node_obj* templates, uint64_t n_templates, const uint32_t* max_nodes,
-                         const ks_pod_obj* overhead_pods, uint64_t n_overhead, const ks_pod_obj* pods, uint64_t n_pods,
-                         ks_scaleup_option* out, int32_t* out_best, int32_t* out_node, ks_pod_reasons* out_reasons) try {
-    if (!c || !out_best || (n_templates && (!templates || !max_nodes || !out)) || (n_overhead && !overhead_pods) ||
-        (n_pods && !pods))
-        return fail(KS_ERR_INVALID, "NULL argument");
-    if (n_pods > KS_SCALEUP_MAX_PODS || n_templates > KS_SCALEUP_MAX_TEMPLATES)
-        return fail(KS_ERR_RANGE, "more than " + std::to_string(KS_SCALEUP_MAX_PODS) + " pods or " +
-                                      std::to_string(KS_SCALEUP_MAX_TEMPLATES) + " templates");
-    std::lock_guard<std::recursive_mutex> lk(c->mu);
-    // templates: names, allocatable as ksh_context_set_nodes parses it; capacity = allocatable minus the overhead pods
-    std::unordered_map<std::string, uint32_t> index;
-    std::vector<int64_t> ac(n_templates), am(n_templates), fc(n_templates), fm(n_templates);
+// ksh_scaleup_estimate's objects, packed for ks_scaleup_estimate: the templates (names, allocatable as
+// ksh_context_set_nodes parses it, capacity = allocatable minus the overhead pods), the pending pods' requests, and the
+// call-local label dictionary.  ksh_scaleup_fit_estimate packs its objects the same way.
+struct ScaleupObjects {
+    std::unordered_map<std::string, uint32_t> index; // template name -> template
+    std::vector<int64_t> ac, am, fc, fm, rc, rm;
+    std::vector<uint64_t> lab, sel;
+    uint32_t W = 1;
+};
+
+static int scaleup_objects(const ks_node_obj* templates, uint64_t n_templates, const ks_pod_obj* overhead_pods,
+                           uint64_t n_overhead, const ks_pod_obj* pods, uint64_t n_pods, ScaleupObjects* o) {
+    o->ac.resize(n_templates);
+    o->am.resize(n_templates);
+    o->fc.resize(n_templates);
+    o->fm.resize(n_templates);
     for (uint64_t t = 0; t < n_templates; t++) {
         if (!templates[t].name) return fail(KS_ERR_INVALID, "template " + std::to_string(t) + ": name is NULL");
-        if (!index.emplace(templates[t].name, (uint32_t)t).second)
+        if (!o->index.emplace(templates[t].name, (uint32_t)t).second)
             return fail(KS_ERR_INVALID, "template " + std::to_string(t) + ": duplicate name \"" + templates[t].name + "\"");
         std::string err;
-        const int rc = parse_node_allocatable(templates[t], &ac[t], &am[t], &err);
+        const int rc = parse_node_allocatable(templates[t], &o->ac[t], &o->am[t], &err);
         if (rc) return fail(rc, "template " + std::to_string(t) + ": " + err);
-        fc[t] = ac[t];
-        fm[t] = am[t];
+        o->fc[t] = o->ac[t];
+        o->fm[t] = o->am[t];
     }
     for (uint64_t i = 0; i < n_overhead; i++) { // DaemonSet pods, charged to the template spec.nodeName names
         const ks_pod_obj& pod = overhead_pods[i];
         const std::string who = "overhead pod " + std::to_string(i) + " (" + nz(pod.ns) + "/" + nz(pod.name) + ")";
         if (!ksh_is_pod_bound(&pod)) return fail(KS_ERR_INVALID, who + " has no spec.nodeName naming its template");
-        const auto it = index.find(pod.node_name);
-        if (it == index.end()) return fail(KS_ERR_INVALID, who + " names unknown template \"" + pod.node_name + "\"");
+        const auto it = o->index.find(pod.node_name);
+        if (it == o->index.end()) return fail(KS_ERR_INVALID, who + " names unknown template \"" + pod.node_name + "\"");
         int64_t cpu, mem;
         std::string err;
         const int rc = total_pod_resources(&pod, &cpu, &mem, &err);
         if (rc) return fail(rc, who + ": " + err);
-        if (__builtin_sub_overflow(fc[it->second], cpu, &fc[it->second]) ||
-            __builtin_sub_overflow(fm[it->second], mem, &fm[it->second]))
+        if (__builtin_sub_overflow(o->fc[it->second], cpu, &o->fc[it->second]) ||
+            __builtin_sub_overflow(o->fm[it->second], mem, &o->fm[it->second]))
             return fail(KS_ERR_RANGE, who + ": capacity of its template overflows");
     }
     // pending pods: unbound, requests as ksh_select_nodes packs them
-    std::vector<int64_t> rc_(n_pods), rm_(n_pods);
+    o->rc.resize(n_pods);
+    o->rm.resize(n_pods);
     for (uint64_t p = 0; p < n_pods; p++) {
         const std::string who = "pod " + std::to_string(p) + " (" + nz(pods[p].ns) + "/" + nz(pods[p].name) + ")";
         if (ksh_is_pod_bound(&pods[p]))
             return fail(KS_ERR_INVALID, who + " has spec.nodeName \"" + pods[p].node_name + "\": not a pending pod");
         std::string err;
-        const int rc = total_pod_resources(&pods[p], &rc_[p], &rm_[p], &err);
+        const int rc = total_pod_resources(&pods[p], &o->rc[p], &o->rm[p], &err);
         if (rc) return fail(rc, who + ": " + err);
     }
     // call-local dictionary: a bit for every pair that some pending pod names and some template carries, in the order
@@ -2634,26 +2678,135 @@ int ksh_scaleup_estimate(ksh_context* c, const ks_node_obj* templates, uint64_t 
     if (bits > 64 * KS_MAX_LABEL_WORDS - 1)
         return fail(KS_ERR_RANGE, "more than 511 distinct (key,value) pairs named by pending pods and carried by templates");
     const uint32_t W = words_for_bits(bits), never = 64 * W - 1;
-    std::vector<uint64_t> lab(n_templates * W, 0), sel(n_pods * W, 0);
+    o->W = W;
+    o->lab.assign(n_templates * W, 0);
+    o->sel.assign(n_pods * W, 0);
     for (uint64_t t = 0; t < n_templates; t++)
         if (templates[t].has_labels)
             for (uint32_t i = 0; i < templates[t].n_labels; i++) {
                 const int32_t b = carried[std::string(nz(templates[t].labels[i].key)) + '\0' + nz(templates[t].labels[i].val)];
-                if (b >= 0) lab[t * W + b / 64] |= 1ull << (b % 64);
+                if (b >= 0) o->lab[t * W + b / 64] |= 1ull << (b % 64);
             }
     for (uint64_t p = 0; p < n_pods; p++) {
         if (!(pods[p].has_spec && pods[p].has_node_selector)) continue;
         for (uint32_t i = 0; i < pods[p].n_selector; i++) {
             const auto it = carried.find(std::string(nz(pods[p].selector[i].key)) + '\0' + nz(pods[p].selector[i].val));
             const uint32_t b = it != carried.end() ? (uint32_t)it->second : never;
-            sel[p * W + b / 64] |= 1ull << (b % 64);
+            o->sel[p * W + b / 64] |= 1ull << (b % 64);
         }
     }
-    const int rc = device_ready(c, ks_scaleup_estimate, "ks_scaleup_estimate");
+    return KS_OK;
+}
+
+int ksh_scaleup_estimate(ksh_context* c, const ks_node_obj* templates, uint64_t n_templates, const uint32_t* max_nodes,
+                         const ks_pod_obj* overhead_pods, uint64_t n_overhead, const ks_pod_obj* pods, uint64_t n_pods,
+                         ks_scaleup_option* out, int32_t* out_best, int32_t* out_node, ks_pod_reasons* out_reasons) try {
+    if (!c || !out_best || (n_templates && (!templates || !max_nodes || !out)) || (n_overhead && !overhead_pods) ||
+        (n_pods && !pods))
+        return fail(KS_ERR_INVALID, "NULL argument");
+    if (n_pods > KS_SCALEUP_MAX_PODS || n_templates > KS_SCALEUP_MAX_TEMPLATES)
+        return fail(KS_ERR_RANGE, "more than " + std::to_string(KS_SCALEUP_MAX_PODS) + " pods or " +
+                                      std::to_string(KS_SCALEUP_MAX_TEMPLATES) + " templates");
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    ScaleupObjects o;
+    int rc = scaleup_objects(templates, n_templates, overhead_pods, n_overhead, pods, n_pods, &o);
     if (rc) return rc;
-    ks_pods kp{n_pods, rc_.data(), rm_.data(), sel.data(), KS_MEM_HOST};
-    ks_node_templates kt{n_templates, W, ac.data(), am.data(), fc.data(), fm.data(), lab.data(), max_nodes};
+    rc = device_ready(c, ks_scaleup_estimate, "ks_scaleup_estimate");
+    if (rc) return rc;
+    ks_pods kp{n_pods, o.rc.data(), o.rm.data(), o.sel.data(), KS_MEM_HOST};
+    ks_node_templates kt{n_templates, o.W, o.ac.data(), o.am.data(), o.fc.data(), o.fm.data(), o.lab.data(), max_nodes};
     return ks_scaleup_estimate(c->snap, &kp, &kt, out, out_best, out_node, out_reasons);
+}
+KSH_CATCH
+
+// ksh_scaleup_estimate's objects under the full filter: the templates' taints and label values as the node side of the
+// rule compilation, and the batch's resources with each template's node_free from its allocatable and overhead pods
+int ksh_scaleup_fit_estimate(ksh_context* c, const ks_node_obj* templates, uint64_t n_templates, const uint32_t* max_nodes,
+                             const uint64_t* template_taint_offset, const ksh_taint* template_taints,
+                             const ks_pod_obj* overhead_pods, uint64_t n_overhead, const ks_pod_obj* pods,
+                             uint64_t n_pods, const int32_t* group, uint32_t n_groups, const ksh_node_rules* rules,
+                             ks_scaleup_option* out, int32_t* out_best, int32_t* out_node, uint32_t* out_refused) try {
+    if (!c || !out_best || (n_templates && (!templates || !max_nodes || !out)) || (n_overhead && !overhead_pods) ||
+        (n_pods && (!pods || !group)))
+        return fail(KS_ERR_INVALID, "NULL argument");
+    if (n_pods > KS_SCALEUP_MAX_PODS || n_templates > KS_SCALEUP_MAX_TEMPLATES)
+        return fail(KS_ERR_RANGE, "more than " + std::to_string(KS_SCALEUP_MAX_PODS) + " pods or " +
+                                      std::to_string(KS_SCALEUP_MAX_TEMPLATES) + " templates");
+    for (uint64_t i = 0; i < n_pods; i++)
+        if (group[i] < -1 || group[i] >= (int64_t)n_groups)
+            return fail(KS_ERR_INVALID, "pod " + std::to_string(i) + ": group outside [-1, n_groups)");
+    const uint64_t* toff = template_taint_offset;
+    if (toff && toff[n_templates] && !template_taints) return fail(KS_ERR_INVALID, "NULL template_taints");
+    // the templates' taints, checked as ksh_context_set_node_taints checks a node's
+    std::vector<std::vector<Taint>> taints(n_templates);
+    for (uint64_t t = 0; toff && t < n_templates; t++) {
+        if (toff[t + 1] < toff[t]) return fail(KS_ERR_INVALID, "template taint offsets decrease");
+        for (uint64_t i = toff[t]; i < toff[t + 1]; i++) {
+            const std::string e = nz(template_taints[i].effect);
+            if (!template_taints[i].key || !*template_taints[i].key ||
+                (e != "NoSchedule" && e != "PreferNoSchedule" && e != "NoExecute"))
+                return fail(KS_ERR_INVALID, "template taint " + std::to_string(i) + ": empty key or effect \"" + e + "\"");
+            taints[t].push_back({template_taints[i].key, nz(template_taints[i].value), e});
+        }
+    }
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
+    ScaleupObjects o;
+    int rc = scaleup_objects(templates, n_templates, overhead_pods, n_overhead, pods, n_pods, &o);
+    if (rc) return rc;
+    // the rules over the templates: their taints, and each rule key's values numbered in template order
+    RuleNodes nodes;
+    nodes.N = (uint32_t)n_templates;
+    nodes.what = "the templates";
+    nodes.taints_of = [&](uint32_t t) { return &taints[t]; };
+    nodes.domains = [&](const std::string& key, int32_t* dom, std::vector<std::string>* values) {
+        std::unordered_map<std::string, int32_t> of_value;
+        for (uint64_t t = 0; t < n_templates; t++) {
+            dom[t] = -1;
+            for (uint32_t i = 0; templates[t].has_labels && i < templates[t].n_labels; i++) {
+                if (key != nz(templates[t].labels[i].key)) continue;
+                const auto it = of_value.emplace(nz(templates[t].labels[i].val), (int32_t)values->size()).first;
+                if (it->second == (int32_t)values->size()) values->push_back(it->first);
+                dom[t] = it->second;
+                break; // the first of a repeated key, as the store keeps it
+            }
+        }
+    };
+    CompiledNodeRules cr;
+    rc = compile_rules_over(nodes, n_groups, rules, &cr);
+    if (rc) return rc;
+    // resources: the batch's names; node_free = a template's allocatable of each (0 when missing) minus its overhead
+    // pods' requests, and for "pods" minus their number
+    CompiledResources res;
+    rc = batch_resources(c, pods, n_pods, &res);
+    if (rc) return rc;
+    const size_t R = res.ids.size(), T = n_templates;
+    std::vector<int32_t> col(c->res_name.size(), -1);
+    for (size_t r = 0; r < R; r++) col[res.ids[r]] = (int32_t)r;
+    res.node_free.assign(R * T, 0);
+    for (size_t t = 0; t < T; t++)
+        for (const ExtQty& e : node_ext(c, templates[t])) {
+            if (e.res >= col.size() || col[e.res] < 0) continue;
+            if (e.err) return ext_error(c, "template '" + std::string(templates[t].name) + "'", "allocatable ", e);
+            res.node_free[(size_t)col[e.res] * T + t] = e.v;
+        }
+    for (uint64_t i = 0; i < n_overhead; i++) {
+        const size_t t = o.index[overhead_pods[i].node_name]; // checked by scaleup_objects
+        bool over = __builtin_sub_overflow(res.node_free[t], 1, &res.node_free[t]);
+        for (const ExtQty& e : pod_ext(c, &overhead_pods[i])) {
+            if (e.res >= col.size() || col[e.res] <= 0) continue;
+            if (e.err) return ext_error(c, "overhead pod '" + pod_key(&overhead_pods[i]) + "'", "request of ", e);
+            int64_t& f = res.node_free[(size_t)col[e.res] * T + t];
+            over |= __builtin_sub_overflow(f, e.v, &f);
+        }
+        if (over) return fail(KS_ERR_RANGE, "free resources of a template overflow int64");
+    }
+    rc = device_ready(c, ks_fit_scaleup_estimate, "ks_fit_scaleup_estimate");
+    if (rc) return rc;
+    ks_pods kp{n_pods, o.rc.data(), o.rm.data(), o.sel.data(), KS_MEM_HOST};
+    ks_node_templates kt{n_templates, o.W, o.ac.data(), o.am.data(), o.fc.data(), o.fm.data(), o.lab.data(), max_nodes};
+    const ks_bind_resources br{(uint32_t)R, res.node_free.data(), res.pod_req.data()};
+    return ks_fit_scaleup_estimate(c->snap, &kp, group, n_groups, &cr.r, &br, &kt, out, out_best, out_node, out_refused,
+                                   nullptr);
 }
 KSH_CATCH
 

@@ -1471,11 +1471,13 @@ int ks_drain_check(ks_snapshot* s, const ks_pods* pods, const ks_drain_candidate
     return KS_OK;
 }
 
-int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const ks_node_templates* t, ks_scaleup_option* out,
-                        int32_t* out_best, int32_t* out_node, ks_pod_reasons* out_reasons) {
+// Every check of ks_scaleup_estimate (include/ksched.h), in the order callers see them; ks_fit_scaleup_estimate runs
+// them first
+static int check_scaleup(ks_snapshot* s, const char* call, const ks_pods* pods, const ks_node_templates* t,
+                         const ks_scaleup_option* out, const int32_t* out_best) {
     int rc = check_pods(s, pods);
     if (rc) return rc;
-    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "ks_scaleup_estimate takes host-space pods");
+    if (pods->mem_space != KS_MEM_HOST) return fail(KS_ERR_INVALID, "%s takes host-space pods", call);
     if (!t || !out_best) return fail(KS_ERR_INVALID, "NULL templates or out_best");
     const uint64_t P = pods->n, T = t->n;
     const uint32_t W = t->label_words;
@@ -1498,8 +1500,34 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const ks_node_templ
             return fail(KS_ERR_RANGE, "template %llu: max_nodes %u (at most %u)", (unsigned long long)i, t->max_nodes[i],
                         KS_SCALEUP_MAX_NODES);
     }
-    rc = check_commit_requests(P, pods->req_cpu, pods->req_mem);
+    return check_commit_requests(P, pods->req_cpu, pods->req_mem);
+}
+
+// The best template of the rows: most pods placed, then the highest utilization, then the fewest nodes, then the lowest
+// index; -1 when none places a pod
+static int32_t best_template(const ks_scaleup_option* out, uint64_t T) {
+    int32_t best = -1;
+    for (uint32_t i = 0; i < T; i++) {
+        const ks_scaleup_option& r = out[i];
+        if (r.placed == 0) continue;
+        if (best < 0) {
+            best = (int32_t)i;
+            continue;
+        }
+        const ks_scaleup_option& b = out[best];
+        if (r.placed > b.placed || (r.placed == b.placed && (r.utilization > b.utilization ||
+                                                            (r.utilization == b.utilization && r.nodes < b.nodes))))
+            best = (int32_t)i;
+    }
+    return best;
+}
+
+int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const ks_node_templates* t, ks_scaleup_option* out,
+                        int32_t* out_best, int32_t* out_node, ks_pod_reasons* out_reasons) {
+    const int rc = check_scaleup(s, "ks_scaleup_estimate", pods, t, out, out_best);
     if (rc) return rc;
+    const uint64_t P = pods->n, T = t->n;
+    const uint32_t W = t->label_words;
     *out_best = -1;
     if (T == 0 || P == 0) { // nothing to pack: every row and reason count is zero
         if (T) memset(out, 0, T * sizeof(ks_scaleup_option));
@@ -1539,21 +1567,7 @@ int ks_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const ks_node_templ
     cudaError_t e = launch_scaleup(pv, W, a, st);
     if (e != cudaSuccess) return fail(KS_ERR_CUDA, "scale-up launch failed: %s", cudaGetErrorString(e));
     CU_TRY(h.finish(st));
-    // the best template: most pods placed, then the highest utilization, then the fewest nodes, then the lowest index
-    int32_t best = -1;
-    for (uint32_t i = 0; i < T; i++) {
-        const ks_scaleup_option& r = out[i];
-        if (r.placed == 0) continue;
-        if (best < 0) {
-            best = (int32_t)i;
-            continue;
-        }
-        const ks_scaleup_option& b = out[best];
-        if (r.placed > b.placed || (r.placed == b.placed && (r.utilization > b.utilization ||
-                                                            (r.utilization == b.utilization && r.nodes < b.nodes))))
-            best = (int32_t)i;
-    }
-    *out_best = best;
+    *out_best = best_template(out, T);
     s->last_path = "scaleup";
     return KS_OK;
 }
@@ -2927,6 +2941,101 @@ int ks_fit_drain_check(ks_snapshot* s, const ks_pods* pods, const int32_t* group
     }
     CU_TRY(h.finish(st));
     s->last_path = "fit_drain";
+    return KS_OK;
+}
+
+int ks_fit_scaleup_estimate(ks_snapshot* s, const ks_pods* pods, const int32_t* group, uint32_t n_groups,
+                            const ks_node_rules* rules, const ks_bind_resources* res, const ks_node_templates* t,
+                            ks_scaleup_option* out, int32_t* out_best, int32_t* out_node, uint32_t* out_refused,
+                            int64_t* out_used) {
+    static const ks_node_rules no_rules{};
+    static const ks_bind_resources no_res{};
+    int rc = check_scaleup(s, "ks_fit_scaleup_estimate", pods, t, out, out_best);
+    if (rc) return rc;
+    const uint64_t P = pods->n, T = t->n, G = n_groups;
+    const uint32_t W = t->label_words;
+    if (P && !group) return fail(KS_ERR_INVALID, "NULL group");
+    if (G > KS_SPREAD_BIND_MAX_GROUPS)
+        return fail(KS_ERR_RANGE, "%llu groups (at most %u)", (unsigned long long)G, KS_SPREAD_BIND_MAX_GROUPS);
+    for (uint64_t p = 0; p < P; p++)
+        if (group[p] < -1 || group[p] >= (int64_t)G)
+            return fail(KS_ERR_INVALID, "pod %llu: group %d outside [-1, %u)", (unsigned long long)p, group[p], n_groups);
+    const ks_node_rules* nr = rules ? rules : &no_rules;
+    if (!res) res = &no_res;
+    const uint32_t R = res->n_res;
+    rc = check_bind_resources(res, P, (uint32_t)T);
+    if (rc) return rc;
+    // |node_free| <= 2^52: with at most 1024 nodes per template every remainder and every out_used sum stays in int64
+    for (uint64_t i = 0; i < (uint64_t)R * T; i++)
+        if (res->node_free[i] < -(1ll << 52) || res->node_free[i] > (1ll << 52))
+            return fail(KS_ERR_RANGE, "resource %llu, template %llu: node_free %lld outside [-2^52, 2^52]",
+                        (unsigned long long)(i / T), (unsigned long long)(i % T), (long long)res->node_free[i]);
+    NodeRulesPlan rp;
+    try {
+        rc = compile_node_rules(nr, (uint32_t)G, (uint32_t)T, &rp);
+    } catch (...) {
+        return fail(KS_ERR_NOMEM, "out of host memory in ks_fit_scaleup_estimate");
+    }
+    if (rc) return rc;
+    *out_best = -1;
+    if (T == 0 || P == 0) { // nothing to pack: every row, refusal word and sum is zero
+        if (T) memset(out, 0, T * sizeof(ks_scaleup_option));
+        if (out_refused && P) memset(out_refused, 0, P * 16);
+        if (out_used && T * R) memset(out_used, 0, T * R * 8);
+        return KS_OK;
+    }
+    std::lock_guard<std::mutex> lk(s->mu);
+    CU_TRY(cudaSetDevice(s->device));
+    HostStaged h;
+    const auto cpu = h.in(pods->req_cpu, P), mem = h.in(pods->req_mem, P), alloc_cpu = h.in(t->alloc_cpu, T),
+               alloc_mem = h.in(t->alloc_mem, T), free_cpu = h.in(t->free_cpu, T), free_mem = h.in(t->free_mem, T);
+    const auto sel = h.in(pods->sel, P * W), labels = h.in(t->labels, T * W);
+    const auto max_nodes = h.in(t->max_nodes, T);
+    const auto grp = h.in(group, P);
+    const auto req = h.in(R ? res->pod_req : nullptr, P * R);
+    const auto node_free = h.in(R ? res->node_free : nullptr, (uint64_t)R * T);
+    const NodeRulesStage rs{h, nr, rp, (uint32_t)T};
+    const auto rows = h.out(out, T);
+    const auto refused = h.out(out_refused, out_refused ? 4 * P : 0, 16); // k_fit_scaleup_reasons stores uint4
+    const auto node = h.out(out_node, out_node ? T * P : 0);
+    const auto used = h.out(out_used, out_used ? T * R : 0);
+    const uint32_t slots = scaleup_slots((uint32_t)T, s->sms);
+    const auto scratch = h.work<uint32_t>((uint64_t)slots * 2 * P);
+    if (const int e = h.reserve(s)) return e;
+    ProfileBindArgs q{}; // k_node_rules_setup reads the NODE fields and b.N only
+    q.b.N = (uint32_t)T;
+    rs.place(q, s->sms);
+    cudaStream_t st = s->stream;
+    CU_TRY(h.upload(st));
+    if (out_node) CU_TRY(cudaMemsetAsync(h.dev(node), 0xff, T * P * 4, st));
+    CU_TRY(launch_node_rules(q, st));
+    const PodView pv{h.dev(cpu), h.dev(mem), h.dev(sel), (uint32_t)P};
+    ScaleupArgs a{};
+    a.T = (uint32_t)T;
+    a.alloc_cpu = h.dev(alloc_cpu);
+    a.alloc_mem = h.dev(alloc_mem);
+    a.free_cpu = h.dev(free_cpu);
+    a.free_mem = h.dev(free_mem);
+    a.labels = h.dev(labels);
+    a.max_nodes = h.dev(max_nodes);
+    a.rows = h.dev(rows);
+    a.out_node = out_node ? h.dev(node) : nullptr;
+    a.scratch = h.dev(scratch);
+    a.slots = slots;
+    FitScaleupArgs f{};
+    f.R = R;
+    f.req = h.dev(req);
+    f.group = h.dev(grp);
+    f.node_free = h.dev(node_free);
+    f.ncls = h.dev(rs.ncls);
+    f.nrules = h.dev(rs.nrules);
+    f.used = out_used && R ? h.dev(used) : nullptr;
+    f.refused = out_refused ? h.dev(refused) : nullptr;
+    const cudaError_t e = launch_fit_scaleup(pv, W, a, f, st);
+    if (e != cudaSuccess) return fail(KS_ERR_CUDA, "fit scale-up launch failed: %s", cudaGetErrorString(e));
+    CU_TRY(h.finish(st));
+    *out_best = best_template(out, T);
+    s->last_path = "fit_scaleup";
     return KS_OK;
 }
 

@@ -167,6 +167,22 @@ struct ScaleupArgs {
 uint32_t scaleup_slots(uint32_t T, int sms);
 cudaError_t launch_scaleup(const PodView& pv, uint32_t W, const ScaleupArgs& a, cudaStream_t st);
 
+// scale-up estimate under the full filter (ks_fit_scaleup_estimate, ks_scaleup.cu): ScaleupArgs (its `reasons` unused)
+// plus ks_fit_bind's resources and rule words with the templates as the nodes.  Device memory.
+struct FitScaleupArgs {
+    uint32_t R;               // [0, KS_BIND_MAX_RESOURCES]
+    const int64_t* req;       // [P * R]: pod p's request of r at p * R + r
+    const int32_t* group;     // [P], each in [-1, G)
+    const int64_t* node_free; // [R * T]: one empty node of template t, resource r at r * T + t
+    const uint32_t* ncls;     // [G + 1]: the class of group g at g + 1, of group -1 at 0
+    const uint32_t* nrules;   // [C * T], written by k_node_rules_setup over the templates
+    int64_t* used;            // [T * R] the placed pods' requests per template, or null
+    uint32_t* refused;        // [P][4] the refusal words, or null
+};
+// k_fit_scaleup_pack, then with f.refused k_fit_scaleup_reasons
+cudaError_t launch_fit_scaleup(const PodView& pv, uint32_t W, const ScaleupArgs& a, const FitScaleupArgs& f,
+                               cudaStream_t st);
+
 // replica placement (ks_place_replicas, ks_replicas.cu).  T specs, each evaluated on its own over the node table by a
 // grid of (node chunk, spec) CTAs: a scan, a fixed number of threshold-search passes, the tie split and, with the copy
 // list, one CTA per spec that sorts its copies.  Device memory.

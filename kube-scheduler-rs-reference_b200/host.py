@@ -70,6 +70,8 @@ for _name, _res, _args in [
                                        C.c_size_t, _vp]),
     ("ksh_drain_fit_nodes", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, _vp, C.c_uint32, _vp, C.c_int, C.c_uint32, _vp,
                                       _vp, _vp]),
+    ("ksh_scaleup_fit_estimate", C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, _vp, _vp, C.c_uint64, _vp, C.c_uint64, _vp,
+                                           C.c_uint32, _vp, _vp, _vp, _vp, _vp]),
 ]:
     _proto(_name, _res, *_args)
 
@@ -770,3 +772,47 @@ class Context:
                                        n_overhead, obj(pods), n_pods, ptr(rows), C.addressof(best), ptr(node),
                                        ptr(why)), "ksh_scaleup_estimate")
         return rows, best.value, node, why
+
+    def scaleup_fit_estimate(self, templates, n_templates, max_nodes, pods, n_pods, group, n_groups, group_rules=None,
+                             template_taints=None, overhead_pods=None, n_overhead=0, want_nodes=True,
+                             want_refused=True):
+        """Scale-up estimate under the full filter over objects (ksh_scaleup_fit_estimate): scaleup_estimate with group
+        [n_pods] and group_rules [n_groups] as drain_fit_nodes takes them, and template_taints, a list of n_templates
+        lists of {"key", "value", "effect"} (None: no taint).  The pending pods' extended resources, the templates' pod
+        limit, taints and required node affinity apply.  Returns (rows, best, node [T, P] or None, refused [P, 4] or
+        None)."""
+        max_nodes = np.ascontiguousarray(max_nodes, np.uint32).reshape(-1)
+        if max_nodes.shape[0] != n_templates:
+            raise ValueError(f"need {n_templates} max_nodes entries (got {max_nodes.shape[0]})")
+        group = np.ascontiguousarray(group, np.int32).reshape(-1)
+        if group.shape[0] != n_pods:
+            raise ValueError(f"group has {group.shape[0]} entries, pods {n_pods}")
+        nr = None
+        if group_rules is not None:
+            if len(group_rules) != n_groups:
+                raise ValueError(f"group_rules has {len(group_rules)} entries, groups {n_groups}")
+            nr = node_rules(group_rules)
+        toff, taints = None, None
+        if template_taints is not None:
+            if len(template_taints) != n_templates:
+                raise ValueError(f"template_taints has {len(template_taints)} entries, templates {n_templates}")
+            flat = [t for ts in template_taints for t in ts]
+            toff = np.zeros(n_templates + 1, np.uint64)
+            np.cumsum([len(ts) for ts in template_taints], out=toff[1:])
+            taints = (ksh_taint * max(len(flat), 1))(*[ksh_taint(_b(t["key"]), _b(t.get("value", "")),
+                                                                 _b(t["effect"])) for t in flat])
+        rows = np.zeros(n_templates, capi.SCALEUP_OPTION_DTYPE)
+        best = C.c_int32(-1)
+        node = np.empty((n_templates, n_pods), np.int32) if want_nodes else None
+        refused = np.empty((n_pods, 4), np.uint32) if want_refused else None
+
+        def ptr(a):
+            return None if a is None else a.ctypes.data
+
+        def obj(a):
+            return C.addressof(a) if a is not None else None
+        check(lib.ksh_scaleup_fit_estimate(self._h, obj(templates), n_templates, ptr(max_nodes), ptr(toff), obj(taints),
+                                           obj(overhead_pods), n_overhead, obj(pods), n_pods, ptr(group), int(n_groups),
+                                           None if nr is None else C.addressof(nr[0]), ptr(rows), C.addressof(best),
+                                           ptr(node), ptr(refused)), "ksh_scaleup_fit_estimate")
+        return rows, best.value, node, refused

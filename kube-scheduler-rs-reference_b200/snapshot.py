@@ -356,6 +356,58 @@ class Snapshot:
                                       _ptr(why)), "ks_scaleup_estimate")
         return rows, best.value, node, why
 
+    def fit_scaleup_estimate(self, req_cpu, req_mem, sel, alloc_cpu, alloc_mem, free_cpu, free_mem, labels, max_nodes,
+                             group, n_groups, rules=None, node_free=None, pod_req=None, want_nodes=True,
+                             want_refused=True, want_used=True):
+        """scaleup_estimate under the full filter (ks_fit_scaleup_estimate): group [P] and rules as fit_bind takes them
+        with the templates as the nodes (rules None = NULL: taint_hard / taint_soft and rule_keys' domains are [T]);
+        node_free [R, T] (one empty node of each template) and pod_req [P, R] (int64), or both None (the C call's NULL
+        res).  Returns scaleup_estimate's (rows, best, node), then refused uint32 [P, 4] (None unless want_refused)
+        and used int64 [T, R] (None unless want_used): the placed pods' requests of each resource."""
+        req_cpu, req_mem = _c(req_cpu, np.int64).reshape(-1), _c(req_mem, np.int64).reshape(-1)
+        alloc_cpu, alloc_mem = _c(alloc_cpu, np.int64).reshape(-1), _c(alloc_mem, np.int64).reshape(-1)
+        free_cpu, free_mem = _c(free_cpu, np.int64).reshape(-1), _c(free_mem, np.int64).reshape(-1)
+        max_nodes = _c(max_nodes, np.uint32).reshape(-1)
+        t, p = alloc_cpu.shape[0], req_cpu.shape[0]
+        labels = _c(labels, np.uint64).reshape(t, -1) if t else None
+        sel = _c(sel, np.uint64).reshape(p, -1) if p else None
+        w = labels.shape[1] if t else sel.shape[1] if p else 1
+        if p and sel.shape[1] != w:
+            raise ValueError(f"sel has {sel.shape[1]} words per pod, labels {w}")
+        for name, a in (("alloc_mem", alloc_mem), ("free_cpu", free_cpu), ("free_mem", free_mem), ("max_nodes", max_nodes)):
+            if a.shape[0] != t:
+                raise ValueError(f"{name} has {a.shape[0]} entries, alloc_cpu {t}")
+        if req_mem.shape[0] != p:
+            raise ValueError(f"req_mem has {req_mem.shape[0]} entries, req_cpu {p}")
+        group = _c(group, np.int32).reshape(-1)
+        if group.shape[0] != p:
+            raise ValueError(f"group has {group.shape[0]} entries, pods {p}")
+        if (node_free is None) != (pod_req is None):
+            raise ValueError("node_free and pod_req go together")
+        br, r = None, 0
+        if node_free is not None:
+            node_free, pod_req = _c(node_free, np.int64), _c(pod_req, np.int64)
+            if node_free.ndim != 2 or node_free.shape[1] != t:
+                raise ValueError(f"node_free has shape {node_free.shape}, expected (R, {t})")
+            r = node_free.shape[0]
+            if pod_req.shape != (p, r):
+                raise ValueError(f"pod_req has shape {pod_req.shape}, expected ({p}, {r})")
+            br = capi.ks_bind_resources(r, _ptr(node_free), _ptr(pod_req))
+        nr, hold = _rules_arg(rules)
+        pods = ks_pods(p, _ptr(req_cpu), _ptr(req_mem), _ptr(sel), capi.KS_MEM_HOST)
+        tmpl = capi.ks_node_templates(t, w, _ptr(alloc_cpu), _ptr(alloc_mem), _ptr(free_cpu), _ptr(free_mem),
+                                      _ptr(labels), _ptr(max_nodes))
+        rows = np.zeros(t, capi.SCALEUP_OPTION_DTYPE)
+        best = C.c_int32(-1)
+        node = np.empty((t, p), np.int32) if want_nodes else None
+        refused = np.empty((p, 4), np.uint32) if want_refused else None
+        used = np.empty((t, r), np.int64) if want_used else None
+        check(lib.ks_fit_scaleup_estimate(self._h, C.byref(pods), _ptr(group), int(n_groups), nr,
+                                          None if br is None else C.byref(br), C.byref(tmpl), _ptr(rows),
+                                          C.addressof(best), _ptr(node), _ptr(refused), _ptr(used)),
+              "ks_fit_scaleup_estimate")
+        return rows, best.value, node, refused, used
+
     def place_replicas(self, req_cpu, req_mem, sel, replicas, policy=capi.KS_SCORE_LEFTOVER, want_nodes=True):
         """Replica placement (ks_place_replicas): spec t (a row of req_cpu / req_mem / sel) asks for replicas[t] copies,
         placed one at a time by ks_select's argmax with the earlier copies bound.  Nothing is charged.  Returns (rows,
